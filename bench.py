@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- image-text pairs/sec through the ViLBERT forward on B200, BASELINE.json's metric.
+"""bench.py -- image-text pairs/sec through the ViLBERT forward on H100, BASELINE.json's metric.
 
     python bench.py --gpus N --steps K --warmup W                       # configs[1]: batch 64 / GPU, VQA head, 36 x 30
     python bench.py --impl reference --gpus N --steps K --warmup W      # the reference's CPU PyTorch path (oracle port)
@@ -12,11 +12,15 @@ blocks on the compute stream -> strong scaling).  Rank 0 prints ONE JSON line.
 
 value      : whole-job pairs/s with inputs resident in HBM (device-pointer C-ABI call, CUDA-event timed, max over ranks)
 e2e        : the same through the host-buffer C-ABI call (pinned host inputs -> H2D -> forward -> D2H logits)
-roofline   : tensor-pipe roofline of the dominant kernel family (the tcgen05 GEMMs, 97 % of the FLOPs)
+roofline   : tensor-pipe roofline of the dominant kernel family (the wgmma GEMMs, 97 % of the FLOPs)
 alt        : the other 16-bit operand format measured in the same run (configs[1] names bf16; the engine's default is fp16 --
-             same tcgen05 kind::f16 rate, 3 more significand bits), each with its measured max-abs-error vs the fp32 oracle
+             same wgmma rate, 3 more significand bits), each with its measured max-abs-error vs the fp32 oracle
 cpu_baseline: the fp32 PyTorch oracle (port of the reference's eager forward, all heads as the reference runs them) timed on
              this box's host cores, rank 0 at N=1 only, bounded sample
+
+--dump-outputs DIR writes what the timed path returned in its last timed step as DIR/<name>.npy (float32; a fixed row sample when
+the arrays would exceed 64 MB).  Inputs are generated from fixed seeds, so two builds run with the same arguments can be compared
+output for output.
 """
 import argparse
 import json
@@ -61,7 +65,42 @@ def parse():
     p.add_argument("--captions", type=int, default=1000, help="retrieval: captions (rows of the score matrix)")
     p.add_argument("--images", type=int, default=1000, help="retrieval: images (columns)")
     p.add_argument("--no-reuse", action="store_true", help="retrieval: full forward per pair instead of cached prefixes")
+    p.add_argument("--dump-outputs", default="", metavar="DIR",
+                   help="write the outputs of the last timed step to DIR/<name>.npy (float32, at most 64 MB in all)")
     return p.parse_args()
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+NPY_HEADER_BYTES = 128                       # what np.save puts in front of the data of a float array of at most a few dimensions
+
+
+def dump_outputs(outdir, arrays):
+    """arrays: name -> tensor.  Written as float32 .npy; if the files would exceed DUMP_LIMIT_BYTES, the same fraction of each array's
+    leading-dimension rows is kept, chosen by a fixed seed (the row indices go to <name>_rows.npy as float64 and count in the limit)."""
+    import numpy as np
+    import torch
+    os.makedirs(outdir, exist_ok=True)
+    total = sum(t.numel() * 4 + NPY_HEADER_BYTES for t in arrays.values())
+    # sampled: a kept row costs its data plus its 8-byte index; every array then has two files with a header each
+    budget = DUMP_LIMIT_BYTES - 2 * NPY_HEADER_BYTES * len(arrays)
+    full_cost = sum(t.numel() * 4 + 8 * t.shape[0] for t in arrays.values() if t.dim() > 0)
+    for name, t in arrays.items():
+        t = t.detach().float()
+        if total > DUMP_LIMIT_BYTES and t.dim() > 0:
+            keep = max(1, int(t.shape[0] * budget // full_cost))
+            rows = torch.randperm(t.shape[0], generator=torch.Generator().manual_seed(0))[:keep].sort().values
+            t = t[rows.to(t.device)]
+            np.save(os.path.join(outdir, name + "_rows.npy"), rows.numpy().astype(np.float64))
+        np.save(os.path.join(outdir, name + ".npy"), t.cpu().numpy())
+
+
+def named_outputs(out):
+    """The tensors of the engine's result tuple (worker.py:286-289 order), keyed by output name."""
+    import torch
+    from vilbert_b200 import _lib as L
+    return {L.OUTPUT_FIELDS[i]: t for i, t in enumerate(out[:9]) if torch.is_tensor(t)}
 
 
 def env_rank():
@@ -75,7 +114,8 @@ def peaks():
         return {"bf16_burst": d["bf16_tflops"], "bf16_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                 "hbm": d["hbm_gbs"], "src": "measured"}
     except Exception:
-        return {"bf16_burst": 1590.0, "bf16_sustained": 1400.0, "hbm": 6650.0, "src": "fallback"}
+        # NVIDIA's H100 SXM data sheet (dense BF16, HBM3, 700 W): a ceiling to compare against, not a measured rate
+        return {"bf16_burst": 989.0, "bf16_sustained": 989.0, "hbm": 3350.0, "src": "H100 SXM data sheet"}
 
 
 class ClockSampler(threading.Thread):
@@ -127,17 +167,19 @@ CPU_THREADS = min(16, os.cpu_count() or 1)   # measured on the 128-vCPU GPU box:
 
 
 def time_oracle(model, req, steps, warmup, all_heads=True):
+    """-> (seconds per timed step, the outputs of the last step)."""
     import torch
     torch.set_num_threads(CPU_THREADS)
     times = []
+    out = None
     with torch.no_grad():
         for i in range(warmup + steps):
             t0 = time.perf_counter()
-            model(*req, output_all_attention_masks=True, compute_pretraining_heads=all_heads)   # as the reference runs it
+            out = model(*req, output_all_attention_masks=True, compute_pretraining_heads=all_heads)   # as the reference runs it
             dt = time.perf_counter() - t0
             if i >= warmup:
                 times.append(dt)
-    return times
+    return times, out
 
 
 def run_reference(args):
@@ -154,7 +196,9 @@ def run_reference(args):
     ref_batch = max(4, min(args.batch, 2400 // max(1, args.steps)))
     req = S.synthetic_request(ref_batch, args.n_tokens, args.n_regions, seed=1234)
     steps = args.steps
-    times = time_oracle(model, req, steps, max(1, min(args.warmup, 2)))
+    times, out = time_oracle(model, req, steps, max(1, min(args.warmup, 2)))
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, named_outputs(out))
     total = sum(times)
     value = ref_batch * len(times) / total
     cores = CPU_THREADS
@@ -173,7 +217,7 @@ def run_reference(args):
     print(json.dumps(line), flush=True)
 
 
-# ------------------------------------------------------------------------------------------------ B200 arm: shared pieces
+# ------------------------------------------------------------------------------------------------ CUDA engine arm: shared pieces
 def make_engine(args, sd, cfg, dtype, local_rank):
     import vilbert_b200 as vb
     return vb.VILBertForVLTasks.from_pretrained(sd, config=cfg, num_labels=3129, use_cuda_graph=not args.no_graph,
@@ -322,7 +366,8 @@ def measure_vqa(args, model, reqs, dev, world, rank, local_rank, select, with_pr
     assert torch.allclose(chk, hout["vil_prediction"], atol=1e-5), "host/device C-ABI paths disagree"
 
     res = dict(value=value, ms=ms, per_rank_ms=per_rank, e2e_value=e2e_value, e2e_s=e2e_s, in_bytes=in_bytes, out_bytes=out_bytes,
-               n_launch=int(n_launch), flops=flops, nfl=nfl, enfl=enfl, clocks=sampler.result(), timed_region_s=ms * 1e-3)
+               n_launch=int(n_launch), flops=flops, nfl=nfl, enfl=enfl, clocks=sampler.result(), timed_region_s=ms * 1e-3,
+               last_out=out)
     if with_profile:
         # ---- per-kernel times, live: every kernel of the step replayed from its own CUDA graph between two CUDA events
         ops = model.profile_ops(B, Tin, V, select, iters=5)
@@ -345,7 +390,6 @@ def measure_vqa(args, model, reqs, dev, world, rank, local_rank, select, with_pr
         res["fam"] = fam
         res["top"] = max((o for o in ops if o["kind"] == "gemm"), key=lambda o: o["flops"])
         # the same GEMM launches with every resident CTA slot as their grid: what a launch does with the GPU to itself
-        # (production starts 2/3 of the slots, which is slower alone and faster in the step -- profiles/r2_grid_size.md)
         full = [o for o in model.profile_ops(B, Tin, V, select, iters=5, grid_pct=100) if o["kind"] == "gemm"]
         res["gemm_full_grid_tflops"] = sum(o["flops"] for o in full) / (sum(o["ms"] for o in full) * 1e-3) / 1e12
     return res
@@ -364,7 +408,7 @@ def run_vqa(args):
     cfg = vb.BertConfig(task_specific_tokens=True, visualization=True)       # worker.py:509-522
     sd = S.synthetic_state_dict(cfg, seed=42)
     select = L.OUT_TASK_HEADS if args.all_heads else L.OUT_VIL_PREDICTION
-    # resident inputs: `rotate` distinct batches (8 x 19 MB > 126 MB L2 together with 466 MB of weights)
+    # resident inputs: `rotate` distinct batches (together with 466 MB of weights far more than the 50 MB L2)
     reqs = [S.synthetic_request(B, Tin, V, seed=1234 + rank * 1000 + i) for i in range(args.rotate)]
     head = "bf16" if args.dtype == "both" else args.dtype      # BASELINE.json configs[1] names bf16
     alts = ["fp16"] if args.dtype == "both" else []
@@ -373,6 +417,8 @@ def run_vqa(args):
 
     model = make_engine(args, sd, cfg, head, local_rank)
     m = measure_vqa(args, model, reqs, dev, world, rank, local_rank, select, with_profile=True)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, named_outputs(m["last_out"]))
     par = parity_rows(model, oracle, reqs[0], rows) if rank == 0 else None
     weight_mb = model._dims["weight_bytes"] / 1e6
     model.close()
@@ -391,28 +437,20 @@ def run_vqa(args):
     g = fam["gemm"]
     gemm_tflops = g["flops"] / (g["ms"] * 1e-3) / 1e12
     serial_ms = sum(f["ms"] for f in fam.values())
-    traffic = None
-    for name in ("r2_traffic.json", "r1_traffic.json"):
-        try:
-            with open(os.path.join(ROOT, "profiles", name)) as f:
-                traffic = json.load(f).get("gemm_dram_bytes_per_launch")
-            break
-        except Exception:
-            pass
     # the whole step is compared with the peak that matches the length of its timed region: a sub-second burst runs at boost
-    # clock (burst cuBLAS peak), a seconds-long run sits under the 1000 W cap (sustained peak)
+    # clock (burst peak), a seconds-long run sits under the power cap (sustained peak)
     step_peak = pk["bf16_burst"] if m["timed_region_s"] < 1.0 else pk["bf16_sustained"]
     in_bytes = m["in_bytes"]
     line = {"metric": METRIC, "value": m["value"], "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3),
             "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
             "dtype": head, "data": "synthetic",
             "config": {"workload": f"batch={B} per GPU, VQA head, {V} regions x {Tin} tokens (BASELINE.json configs[1]), "
-                                   f"{head} tensor-core operands / fp32 accumulate (tcgen05 kind::f16); "
+                                   f"{head} tensor-core operands / fp32 accumulate (wgmma); "
                                    f"random-init 268M-param ViLBERT (seed 42)",
                        "global_batch": B * world, "per_gpu_batch": B, "n_tokens": Tin, "n_regions": V,
                        "parallelism": f"dp{world} (batch sharding, no collective)",
                        "l2": f"inputs rotate over {args.rotate} resident batches ({args.rotate * in_bytes / 1e6:.0f} MB) "
-                             f"+ {weight_mb:.0f} MB of weights > 126 MB L2",
+                             f"+ {weight_mb:.0f} MB of weights > 50 MB L2",
                        "batches_in_flight": m["nfl"],
                        "cuda_graph": not args.no_graph, "pdl": "every kernel" if args.pdl != "off" else "off", "layernorm": "fused" if args.fused_ln else "split",
                        "heads": "task heads" if args.all_heads else "vil_prediction"},
@@ -425,14 +463,14 @@ def run_vqa(args):
             "alt": alt,
             "per_rank_ms_per_step": [x / args.steps for x in m["per_rank_ms"]],
             "roofline": {"bound": "tensor", "achieved": gemm_tflops, "peak": pk["bf16_burst"], "unit": "TFLOP/s",
-                         "frac": gemm_tflops / pk["bf16_burst"], "traffic": traffic,
-                         "kernel": "gemm_persistent_kernel (tcgen05): all %d GEMM launches of one step, algorithmic 2MNK FLOPs / "
+                         "frac": gemm_tflops / pk["bf16_burst"],
+                         "kernel": "gemm_persistent_kernel (wgmma): all %d GEMM launches of one step, algorithmic 2MNK FLOPs / "
                                    "CUDA-event time per launch" % g["launches"],
                          "avg_launch_us": 1e3 * g["ms"] / g["launches"],
                          "largest_gemm": {"M": top["dims"][0], "N": top["dims"][1], "K": top["dims"][2], "us": 1e3 * top["ms"],
                                           "tflops": top["flops"] / (top["ms"] * 1e-3) / 1e12},
                          "achieved_full_grid": m["gemm_full_grid_tflops"], "frac_full_grid": m["gemm_full_grid_tflops"] / pk["bf16_burst"],
-                         "grid_note": "achieved/frac: the launches as the step issues them (persistent grid = 2/3 of the 296 CTA slots); "
+                         "grid_note": "achieved/frac: the launches as the step issues them; "
                                       "*_full_grid: the same launches with all slots, i.e. each kernel alone on the GPU",
                          "share_of_step": g["ms"] / serial_ms,
                          "families_ms": {k: round(v["ms"], 4) for k, v in fam.items()},
@@ -440,13 +478,13 @@ def run_vqa(args):
                          "whole_step_peak": step_peak, "whole_step_frac_vs_burst": tflops / pk["bf16_burst"],
                          "whole_step_frac_vs_sustained": tflops / pk["bf16_sustained"],
                          "flops_per_step": flops,
-                         "peak_source": pk["src"] + ": burst cuBLAS bf16 for the kernels timed alone (peak); the whole step against the "
+                         "peak_source": pk["src"] + ": bf16 peak for the kernels timed alone; the whole step against the "
                                         "burst peak when its timed region is < 1 s, else the sustained one (%.0f)" % pk["bf16_sustained"]},
             "clocks": m["clocks"]}
 
     if rank == 0 and world == 1 and not args.no_cpu_baseline:
         nb = 3
-        times = time_oracle(oracle, reqs[0], nb, 1)
+        times, _ = time_oracle(oracle, reqs[0], nb, 1)
         v = B * len(times) / sum(times)
         line["cpu_baseline"] = {"value": v, "unit": UNIT, "cores": CPU_THREADS, "kind": "port",
                                 "sample": f"{nb} forwards of batch {B} after 1 warm-up (torch fp32 oracle, "
@@ -494,6 +532,8 @@ def run_multitask(args):
     ms_local, out, _ = timed_loop(step, args.steps, args.warmup, streams, dev, world, sampler)
     ms, per_rank = all_rank_ms(ms_local, world, dev)
     sampler.join(timeout=1.0)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, named_outputs(out))
     n_launch, flops = model.plan_info(hi - lo, Tin, V, select)
     # parity on this rank's slice: rows re-run alone must give the same bits (shard independence), rank 0 also checks the oracle
     o_all = model(*dreqs[0], select=select)
@@ -590,6 +630,8 @@ def run_retrieval(args):
     ms, per_rank = all_rank_ms(e0.elapsed_time(e1), world, dev)
     sampler.join(timeout=1.0)
     assert full.shape == (n_cap, n_img) and torch.isfinite(full).all()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"vil_logit_scores": full})
     # ---- checks on EVERY rank: (a) the gathered matrix is the same on all ranks, (b) sampled entries, recomputed here with the
     # plain full forward of that pair (no sharding, no reuse), match the matrix bit for bit; rank 0: (c) two entries vs the oracle
     csum = full.double().sum().reshape(1)

@@ -1,7 +1,7 @@
-/* vilbert_b200 -- C ABI of the B200-native ViLBERT multi-task forward.
+/* vilbert_b200 -- C ABI of the H100-native (sm_90a) ViLBERT multi-task forward.
  *
  * The reference has no FFI for this path: its boundary is the Python object protocol that
- * /root/reference/worker.py fixes (SURVEY.md section 8b):
+ * the reference worker.py fixes (SURVEY.md section 8b):
  *     config = BertConfig.from_json_file(...)                          worker.py:495, 506-522
  *     model  = VILBertForVLTasks.from_pretrained(ckpt, config=config,
  *                                                num_labels=3129, ...) worker.py:530-532
@@ -40,7 +40,7 @@ typedef enum {
     VB200_ERR_CONFIG = -2,       /* config JSON could not be parsed or is unsupported */
     VB200_ERR_CHECKPOINT = -3,   /* missing / unexpected / mis-shaped state_dict entry */
     VB200_ERR_CUDA = -4,         /* CUDA runtime or driver error (message has the detail) */
-    VB200_ERR_NO_DEVICE = -5     /* no sm_100 device: there is deliberately no CPU fallback */
+    VB200_ERR_NO_DEVICE = -5     /* no sm_90 device: there is deliberately no CPU fallback */
 } vb200_status;
 
 typedef enum { VB200_F32 = 0, VB200_F16 = 1, VB200_BF16 = 2 } vb200_dtype;
@@ -116,17 +116,17 @@ typedef struct {
     int32_t use_cuda_graph;        /* default on: each (B,Tin,V,select) plan is captured once and replayed */
     int32_t use_pdl;               /* programmatic dependent launch: 0 default (= every kernel), > 0 every kernel, < 0 none */
     int32_t strict;                /* default on: unexpected checkpoint keys are an error */
-    int32_t act_fp16;              /* 16-bit format of the tensor-core operands (weights AND activations; tcgen05 kind::f16
-                                      needs matching A/B formats).  default on: IEEE fp16 (11-bit significand; activations
+    int32_t act_fp16;              /* 16-bit format of the tensor-core operands (weights AND activations; wgmma needs
+                                      matching A/B formats).  default on: IEEE fp16 (11-bit significand; activations
                                       are LayerNorm-bounded, converts saturate); -1: bf16.  Accumulation, residual stream,
                                       LayerNorm, softmax and logits are fp32 either way. */
     int32_t fused_layernorm;       /* default off: LayerNorm(dense(x) + residual) runs as GEMM (fp32 out) + an L2-resident row
                                       kernel; 1: cluster-LayerNorm GEMM epilogue (N tiles of a row-panel form a thread-block
                                       cluster and exchange (mean, M2) through distributed shared memory).  Both are
-                                      parity-tested; the split form measured faster on B200 at every batch tried. */
+                                      parity-tested. */
     int32_t split_fp32;            /* 1: fp32-parity mode ("fp32x").  Every GEMM operand travels as TWO fp16 numbers (hi = fp16(x),
                                       lo = fp16(x - hi), 22 significand bits); operand buffers hold hi | lo | hi (weights hi | hi |
-                                      lo) per 64 columns, so an ordinary tcgen05 GEMM over K' = 3K adds hi.hi + lo.hi + hi.lo in its
+                                      lo) per 64 columns, so an ordinary wgmma GEMM over K' = 3K adds hi.hi + lo.hi + hi.lo in its
                                       fp32 accumulator; attention runs in fp32 on CUDA cores; GELU uses the 1.5e-7 erf.  3x the
                                       tensor work of the default mode -- for logit parity with the reference's fp32 forward
                                       (<= 1e-3 per logit, BASELINE.json north_star), not for throughput.  Implies act_fp16. */
@@ -134,9 +134,8 @@ typedef struct {
                                       u = dense(x) + residual writes u (fp32 + 16-bit) and per-row (mean, M2) statistics instead of
                                       LayerNorm(u); the next GEMM runs on u with weights pre-scaled by gamma and finishes with
                                       rstd * (acc - mean * s) + c; residual readers rebuild LayerNorm(u) on the fly.  Same math,
-                                      57 of a forward's 62 LayerNorm launches gone -- but measured SLOWER on B200 at batch 64
-                                      (the extra epilogue work exceeds the row kernels it replaces, profiles/r2_ln_fold.md), so
-                                      it is an option, parity-tested, not the default.  Ignored in split_fp32 / fused_layernorm. */
+                                      57 of a forward's 62 LayerNorm launches gone, at the cost of heavier GEMM epilogues; an
+                                      option, parity-tested, not the default.  Ignored in split_fp32 / fused_layernorm. */
     int32_t max_plans;             /* plan-cache bound: plans (workspace + CUDA graph per (batch, tokens, regions, select, slot))
                                       beyond this are evicted least-recently-used; 0 -> 24 */
 } vb200_options;
@@ -182,13 +181,13 @@ int vb200_plan_info(vb200_handle h, int32_t batch, int32_t n_tokens, int32_t n_r
                     int64_t* n_launches, double* flops);
 int vb200_model_dim(vb200_handle h, const char* key, int64_t* value);
 /* Run-time knobs: "max_plans" (plan-cache bound); "profile_grid_pct" (0 or 10..100): the NEXT vb200_profile_ops call launches every
- * GEMM with this percentage of the resident CTA slots as its persistent grid (production: two thirds, profiles/r2_grid_size.md) --
+ * GEMM with this percentage of the resident CTA slots as its persistent grid --
  * for reporting what a launch does when it has the GPU to itself; forwards are never affected.  "chain_ffn" (0/1): issue every
  * FFN-in -> FFN-out pair as ONE chained persistent launch (csrc/gemm_chain.cu: dynamic tile list + per-row-panel dependency counters;
- * same bits, measured slower at batch 64, profiles/r2_chain.md -> off by default); changing it drains the device and drops cached plans. */
+ * same bits; off by default); changing it drains the device and drops cached plans. */
 int vb200_set_option(vb200_handle h, const char* key, int64_t value);
-/* Profiling: after vb200_set_option(h, "timeline", 1) every tcgen05 GEMM launch of a forward records 16 stamps per CTA (0: clock64 at
- * entry, 1: setup done, 2: first k-block landed [-DVB200_STAMPS builds], 8 / 9: %globaltimer ns at entry / exit, 10: last MMA committed,
+/* Profiling: after vb200_set_option(h, "timeline", 1) every persistent GEMM launch of a forward records 16 stamps per CTA (0: clock64 at
+ * entry, 1: setup done, 2: first k-block landed [-DVB200_STAMPS builds], 8 / 9: %globaltimer ns at entry / exit, 10: last tile accumulated,
  * 11: tiles walked, 12: SM id).  Copies the stamps of the LAST forward run on (shape, select, slot): stamps[n_ops][304][16],
  * dims[n_ops][4] = M, N, K, graph branch.  Synchronises the device.  scripts/step_timeline.py turns two slots' worth into per-SM
  * occupancy figures. */
@@ -252,10 +251,10 @@ int vb200_forward_cached(vb200_handle h, int32_t batch, int32_t n_tokens, int32_
 /* y = epilogue(x[M,K] (16-bit) . w[N,K]^T (16-bit)); act: 0 none, 1 GELU(erf), 2 ReLU; LayerNorm applied when gamma != NULL.
  * act_fp16 != 0: x, w and the 16-bit output y are fp16, else bf16 (parameter names keep the historical _bf16 suffix).
  * act 3 = GELU with the 1.5e-7 erf (fp32-parity mode).  variant 0: persistent kernel (gemm_persistent.cuh, what the engine
- * uses); 2: CTA-pair kernel (gemm_pair.cu, cta_group::2); 3: persistent kernel with three CTAs per SM (128-wide tile, PCfg MODE 6);
- * 4: persistent kernel with one CTA per SM and a 6-stage ring (128- or 64-wide tile, PCfg MODE 7 -- what the engine uses for forwards
- * of <= 320 rows).  Variants 0, 3 and 4 produce the same bits.
- * timing: NULL, or a device buffer of 16 int64 per CTA that receives clock64() / %globaltimer stamps (profiling aid, variants 0, 3, 4). */
+ * uses); 2: CTA pair (PCfg MODE 8: a cluster of two CTAs shares each weight tile through TMA multicast; plain epilogue, 128-wide
+ * tile, N % 128 == 0); 3 and 4 (names of Blackwell occupancy configurations) select the persistent kernel.  Plain (non-LayerNorm)
+ * tiles are 64, 128 or 192 columns wide; block_n 256 runs as 128-wide tiles.  Variants 0, 3, 4 and every width give the same bits.
+ * timing: NULL, or a device buffer of 16 int64 per CTA that receives clock64() / %globaltimer stamps (profiling aid). */
 int vb200_linear(const void* x_bf16, int64_t ld_x, const void* w_bf16, int64_t ld_w, const float* bias,
                  const float* residual, int64_t ld_res, const float* gamma, const float* beta, float eps, int32_t act,
                  void* y_bf16, int64_t ld_y_bf16, float* y_f32, int64_t ld_y_f32, int64_t M, int64_t N, int64_t K,

@@ -3,7 +3,7 @@
 Plain-PyTorch fp32 restatement of the hot path the reference worker calls once per
 request: ``model(question, features, spatials, segment_ids, input_mask, image_mask,
 co_attention_mask, task_tokens, output_all_attention_masks=True)``
-(/root/reference/worker.py:286-289) on the object built at worker.py:530-536
+(worker.py:286-289) on the object built at worker.py:530-536
 (``VILBertForVLTasks.from_pretrained(..., config=config, num_labels=3129)``).
 
 The arithmetic itself lives in the third-party package ``vilbert`` (upstream
@@ -12,7 +12,7 @@ It is un-vendored, un-pinned (absent from requirements.txt:1-69, ``.SUBMODULES.j
 submodules) and not installed here, and the reference holds no test, golden vector or checkpoint
 for this path (demo/tests.py:1-3 is an empty stub).  This file therefore restates the *published*
 algorithm (arXiv:1908.02265 section 3, arXiv:1912.02315) constrained by every in-tree call site;
-there is nothing in /root/reference to pin it against numerically  ==>  "parity unpinned".
+there is nothing in the reference tree to pin it against numerically  ==>  "parity unpinned".
 The one number the tree does pin -- "270 million" parameters (README.md:4) -- is checked by
 ``count_parameters`` (268.0 M unique parameters, the tied LM decoder counted once).  Three pieces are additionally
 cross-checked against independent implementations (tests/test_oracle.py): the text ``BertLayer`` and ``BertEmbeddings`` against

@@ -48,7 +48,7 @@ def main():
     ap.add_argument("--batch", type=int, default=64)
     ap.add_argument("--act", default="fp16")
     ap.add_argument("--sets", type=int, default=4, help="operand sets cycled through per kernel")
-    ap.add_argument("--variant", type=int, default=0, help="0 persistent kernel, 2 CTA-pair kernel, 3 persistent with three CTAs per SM (PCfg MODE 6, 128-wide tile)")
+    ap.add_argument("--variant", type=int, default=0, help="vb200_linear variant: 0 persistent kernel, 2 CTA pair (128-wide tile, N %% 128 == 0)")
     ap.add_argument("--stamps", action="store_true", help="print clock64 phase stamps of the persistent kernel")
     ap.add_argument("--bn", type=int, default=0, help="override block_n of every plain GEMM")
     ap.add_argument("--debug", default="0", help="VB200_DEBUG timing decomposition (comma list, each timed in turn): "
@@ -81,11 +81,9 @@ def main():
             continue
         if a.variant == 2 and (ln or N % 128 or M < 256):
             continue
-        if a.variant == 3 and ln:
-            continue
         if a.bn and not ln:
             bn = a.bn
-        if a.variant == 3:
+        if a.variant == 2:
             bn = 128
         sets = []
         for _ in range(a.sets):

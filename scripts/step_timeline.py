@@ -1,14 +1,14 @@
-"""Where the SMs spend a step: per-SM occupancy by tcgen05 GEMM CTAs while `--inflight` batches run concurrently.
+"""Where the SMs spend a step: per-SM occupancy by persistent GEMM CTAs while `--inflight` batches run concurrently.
 
 Needs a -DVB200_STAMPS build for the "first k-block landed" stamp (`make -C vilbert-multi-task_b200/csrc EXTRA=-DVB200_STAMPS`).
 Every GEMM CTA of the LAST forward of each workspace slot leaves (SM id, %globaltimer at entry / exit, clock64 at entry, first
-operand tile landed, last MMA committed, exit) -- include/vilbert_b200.h vb200_timeline.  Inside the window in which all slots'
+operand tile landed, last tile accumulated, exit) -- include/vilbert_b200.h vb200_timeline.  Inside the window in which all slots'
 last forwards overlap, for every SM:
 
   resident k   fraction of the window with exactly k GEMM CTAs resident (k = 0: the SM runs LayerNorm / attention CTAs or nothing)
-  mma k        fraction with exactly k resident CTAs between "first k-block landed" and "last MMA committed" (their main loop)
+  mma k        fraction with exactly k resident CTAs between "first k-block landed" and "last tile accumulated" (their main loop)
 
-and per launch family the mean CTA lifetime split into prologue (entry -> first k-block), main loop, tail (last MMA -> exit).
+and per launch family the mean CTA lifetime split into prologue (entry -> first k-block), main loop, tail (last tile accumulated -> exit).
 Prints one JSON object; `--out` also saves it.
 """
 import argparse
@@ -94,7 +94,7 @@ def main():
 
     def occupancy(key_lo, key_hi):
         """Fractions of the window with exactly k intervals [lo, hi) open, averaged over the SMs."""
-        n_sm = 148
+        n_sm = torch.cuda.get_device_properties(0).multi_processor_count
         frac = np.zeros(4)
         for sm in range(n_sm):
             ev = []
@@ -129,7 +129,7 @@ def main():
             b[0] += 1
             for i, (lo, hi) in enumerate([(0, 1), (1, 6), (6, 2), (2, 10), (10, 4), (4, 14), (14, 15), (15, 5), (5, 13)]):
                 b[1 + i] += float(x[hi] - x[lo])
-    names = ["setup", "setup_to_pdl_wait_done", "pdl_to_first_kblock", "main_loop", "mma_drain", "first_tmem_load", "first_chunk_store",
+    names = ["setup", "setup_to_pdl_wait_done", "pdl_to_first_kblock", "main_loop", "mma_drain", "first_acc_read", "first_chunk_store",
              "other_chunks_and_tma_store", "teardown"]
     out["one_tile_cta_cycles"] = [dict(M=k[0], N=k[1], K=k[2], ctas=v[0], **{n: round(v[1 + i] / v[0]) for i, n in enumerate(names)})
                                   for k, v in sorted(br.items(), key=lambda kv: -kv[1][0])]
@@ -155,12 +155,12 @@ def main():
 
     out["gemm_launches_resident_hist"] = launches_active(3, 6)      # index = number of GEMM launches with a resident CTA (7 = 7 or more)
     out["gemm_launches_in_main_loop_hist"] = launches_active(4, 5)
-    # CTAs resident GPU-wide (of 296 slots), time-weighted mean and the share of them that are still waiting for their producer kernel
+    # CTAs resident GPU-wide (of one slot per SM), time-weighted mean and the share of them that are still waiting for their producer kernel
     res_ns = sum(min(r[6], w1) - max(r[3], w0) for r in iv if min(r[6], w1) > max(r[3], w0))
     out["mean_gemm_ctas_resident"] = round(res_ns / (w1 - w0), 1)
     tot = sum(r[6] - r[3] for r in iv if r[3] >= w0 and r[6] <= w1)
     out["gemm_cta_ns_in_window"] = tot
-    out["slot_capacity_ns"] = 296 * (w1 - w0)
+    out["slot_capacity_ns"] = torch.cuda.get_device_properties(0).multi_processor_count * (w1 - w0)
     print(json.dumps(out))
     if args.out:
         with open(args.out, "w") as f:

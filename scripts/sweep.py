@@ -1,7 +1,7 @@
 """BASELINE.json configs[4]: sequence-length sweep at batch 256 -- text 16..128 tokens x regions 10..100 --
 pairs/s, TFLOP/s and fraction of the tensor roofline per point (CUDA-event timed, CUDA-graph replay).
 
-    python scripts/sweep.py [--batch 256] > profiles/r1_sweep.jsonl
+    python scripts/sweep.py [--batch 256] > sweep.jsonl
 """
 import argparse
 import json

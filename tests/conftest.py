@@ -10,7 +10,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with `-m gpu` under gpurun)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (run with `-m gpu`)")
 
 
 def _has_gpu():

@@ -4,7 +4,7 @@
                                                      [--config config/bert_base_6layer_6conect.json]
 
 Status today: "parity unpinned".  The hot path's arithmetic lives in the third-party package `vilbert`
-(facebookresearch/vilbert-multi-task, imported at /root/reference/worker.py:44-46, un-vendored and unpinned); neither it nor its
+(facebookresearch/vilbert-multi-task, imported at worker.py:44-46, un-vendored and unpinned); neither it nor its
 dependencies (pytorch_transformers, easydict) nor the checkpoint `pytorch_model_9.bin` (worker.py:470) exist on the build box, so
 tests/golden/full_*.npz hold the outputs of oracle/vilbert_ref.py -- our restatement -- not of the reference.
 

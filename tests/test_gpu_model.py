@@ -1,10 +1,10 @@
-"""End-to-end parity of the CUDA engine (worker-facing Python protocol -> C ABI -> sm_100a kernels) against the
+"""End-to-end parity of the CUDA engine (worker-facing Python protocol -> C ABI -> sm_90a kernels) against the
 fp32 CPU oracle on identical seeded inputs.  `-m gpu` only.
 
 Tolerances (BASELINE.json north_star: "within 1e-3 fp32 / 1e-2 bf16 per logit"):
 
 * TOL = 1e-2 per logit against the fp32 oracle -- met by the DEFAULT engine mode (fp16 tensor-core operands,
-  fp32 accumulation / residual stream / LayerNorm / softmax; same tcgen05 kind::f16 rate as bf16).
+  fp32 accumulation / residual stream / LayerNorm / softmax; same tensor-core rate as bf16).
 * The bf16-operand mode (compute_dtype="bf16") cannot meet 1e-2 against fp32: rounding the ~150 GEMM operands of
   this network to an 8-bit significand moves the VQA logits (std 0.91) by up to ~1.9e-2 in *exact* arithmetic --
   the oracle itself shows it when its activations are rounded to bf16 at the same points

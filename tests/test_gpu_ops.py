@@ -18,7 +18,7 @@ def _ptr(t):
     return C.c_void_p(t.data_ptr()) if t is not None else None
 
 
-VARIANT = 0     # 0 = persistent kernel, 2 = CTA-pair kernel (cta_group::2); set by the fixture
+VARIANT = 0     # 0 = persistent kernel, 2 = CTA pair (cluster of two, TMA multicast of W); set by the fixture
 
 
 @pytest.fixture(params=[0, 2], ids=["persistent", "pair"])
@@ -31,7 +31,7 @@ def variant(request):
 
 def run_linear(x, w, bias=None, res=None, gamma=None, beta=None, act=0, block_n=0, want_bf16=True, want_f32=True,
                ld_f32=None, pdl=0):
-    """x, w: both fp16 or both bf16 (tcgen05 kind::f16 needs matching operand formats); same format for the 16-bit output."""
+    """x, w: both fp16 or both bf16 (wgmma needs matching operand formats); same format for the 16-bit output."""
     L, lib = _lib()
     M, K = x.shape
     N = w.shape[0]
@@ -84,8 +84,8 @@ def _mk(M, N, K, seed=0, act=torch.bfloat16):
     (200, 384, 768, 128),       # ragged M
     (1984, 2304, 768, 128),     # text QKV at B=64
     (2304, 3072, 1024, 128),    # co-attention image QKV at B=64
-    (1984, 3072, 768, 256),     # wide tile
-    (1984, 3072, 768, 192),     # 128x192 tiles (round 2): the N = 3072 GEMMs at batch 64 in one wave
+    (1984, 3072, 768, 256),     # block_n 256: runs as 128-wide tiles
+    (1984, 3072, 768, 192),     # 128x192 tiles: the N = 3072 GEMMs at batch 64 in 16 column tiles
     (2304, 3072, 1024, 192),
     (300, 384, 512, 192),       # ragged M, two N tiles
     (77, 64, 128, 64),          # narrow tile
@@ -125,7 +125,7 @@ def test_linear_act(act, act_dt, variant, parity_log):
     (1984, 768, 768, 0),        # text attention-output at B=64: cluster of 6 (or 96 x 8)
     (1984, 768, 3072, 0),       # text FFN-out
     (2304, 1024, 2112, 0),      # image embedding: cluster of 8, K with zero tail
-    (64, 2048, 1024, 1),        # SimpleClassifier: GELU then LayerNorm over 2048 = 256 x 8
+    (64, 2048, 1024, 1),        # SimpleClassifier: GELU then LayerNorm over 2048 = 128 x 16
     (5000, 1024, 512, 0),       # 40 M tiles: persistent clusters loop (accumulator + partial double-buffering)
     (16000, 768, 256, 1),       # 125 M tiles over <= 24 clusters of 6
 ])
@@ -504,17 +504,17 @@ def test_gemm_chain(M, K1, N1, N2, act, act_dt, parity_log):
     (128, 128, 64, 0),          # one tile, one k-block
     (256, 256, 1024, 0),        # the 2-stage ring wraps eight times
     (200, 384, 768, 1),         # ragged M, GELU
-    (1984, 3072, 768, 1),       # text FFN-in at batch 64: 384 tiles on 3 x 148 slots
+    (1984, 3072, 768, 1),       # text FFN-in at batch 64: 384 tiles, about three per persistent CTA
     (2304, 3072, 1024, 0),      # image QKV: 432 tiles
     (64, 3129, 2048, 0),        # ragged N (per-lane remainder path)
-    (15872, 768, 768, 2),       # 744 tiles: CTAs walk several tiles on ONE accumulator (tmem_empty hand-shake)
+    (15872, 768, 768, 2),       # 744 tiles: CTAs walk several tiles through one deposit area
 ])
 @pytest.mark.parametrize("act_dt", ACT)
 @pytest.mark.parametrize("kernel_variant", [3, 4], ids=["three_ctas_per_sm", "lone_cta_6_stages"])
 def test_linear_three_ctas_per_sm(M, N, K, act, act_dt, kernel_variant, parity_log):
-    """PCfg MODE 6 (variant 3: three CTAs per SM, 2-stage ring, one accumulator, four software-pipelined epilogue warps) and MODE 7
-    (variant 4: one CTA per SM, 6-stage ring -- the small-batch latency configuration): same tiles and k order as the default kernel
-    -> the same bits in the fp32 and in the 16-bit output."""
+    """vb200_linear variants 3 and 4 (ABI names of Blackwell occupancy configurations; on sm_90a they select the persistent
+    kernel) must give variant 0's bits, and the TMA-store epilogue (16-bit output only, yb3b) the same bits as the register-store
+    one (fp32 + 16-bit outputs)."""
     global VARIANT
     x, w, b, _ = _mk(M, N, K, seed=5, act=act_dt)
     ld = (N + 3) // 4 * 4
@@ -538,8 +538,8 @@ def test_linear_three_ctas_per_sm(M, N, K, act, act_dt, kernel_variant, parity_l
 @pytest.mark.parametrize("M,N,K,act", [(31, 768, 768, 0), (36, 3072, 1024, 1), (248, 768, 3072, 0), (288, 1024, 1024, 2), (64, 3129, 2048, 0)])
 @pytest.mark.parametrize("act_dt", ACT)
 def test_linear_lone_cta_64_wide(M, N, K, act, act_dt, parity_log):
-    """What a small forward (batch <= 8) runs: PCfg MODE 7 with 64-wide tiles (variant 4, block_n 64).  Neither the ring depth nor the
-    tile width changes an element's accumulation order: the same bits as the default 128-wide kernel."""
+    """What a small forward (batch <= 8) runs: 64-wide tiles (variant 4 selects the persistent kernel).  The tile width does not
+    change an element's accumulation order: the same bits as the default 128-wide kernel."""
     global VARIANT
     x, w, b, _ = _mk(M, N, K, seed=6, act=act_dt)
     ld = (N + 3) // 4 * 4

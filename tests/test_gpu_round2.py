@@ -419,7 +419,7 @@ def test_chained_ffn_launch_is_bit_identical(full_oracle, parity_log):
 
 # ----------------------------------------------------------------------------------------------- step timeline (profiling hook)
 def test_timeline_records_every_gemm_cta(tiny_oracle):
-    """set_option("timeline", 1): every plain tcgen05 GEMM launch of a forward leaves per-CTA stamps (entry / exit %globaltimer, SM id);
+    """set_option("timeline", 1): every plain persistent GEMM launch of a forward leaves per-CTA stamps (entry / exit %globaltimer, SM id);
     the logits are the same bits as without the hook."""
     import ctypes as C
     import numpy as np
@@ -438,15 +438,16 @@ def test_timeline_records_every_gemm_cta(tiny_oracle):
     dims = (C.c_int32 * (4 * cap))()
     st = np.zeros((cap, ctas, 16), dtype=np.int64)
     L.check(L.load().vb200_timeline(eng._handle, 4, 30, 36, sel, 0, cap, C.byref(n), dims, st.ctypes.data_as(C.POINTER(C.c_int64))), eng._handle)
-    assert 100 <= n.value <= cap                                   # 125 GEMM launches minus whatever runs on the LN / pair variants
+    assert 100 <= n.value <= cap                                   # 125 GEMM launches minus whatever runs on the LN variant
+    n_sms = torch.cuda.get_device_properties(0).multi_processor_count
     for o in range(n.value):
         M, N, K = dims[4 * o], dims[4 * o + 1], dims[4 * o + 2]
         live = st[o][:, 9] > 0
         tiles = ((M + 127) // 128) * ((N + 63) // 64)                              # 64-wide tiles at most
-        assert 1 <= live.sum() <= min(tiles, 296), (o, M, N, K, int(live.sum()))
+        assert 1 <= live.sum() <= min(tiles, n_sms), (o, M, N, K, int(live.sum()))        # one CTA per SM
         s = st[o][live]
         assert (s[:, 9] >= s[:, 8]).all() and (s[:, 13] > s[:, 0]).all()          # exit after entry (globaltimer and clock64)
-        assert (s[:, 12] >= 0).all() and (s[:, 12] < 148).all()                      # SM id
+        assert (s[:, 12] >= 0).all() and (s[:, 12] < n_sms).all()                    # SM id
     eng.set_option("timeline", 0)
     assert torch.equal(eng(*dev, select=sel)[0], plain)
     eng.close()

@@ -172,12 +172,14 @@ class RowModel:
                  output_all_attention_masks=False, select=None):
         B, V = features.shape[0], features.shape[1]
         self.calls.append(dict(B=B, select=select))
+        dev = features.device                      # MicroBatchWorker places its inputs on the GPU when one is visible
+        w = {k: v.to(dev) for k, v in self.w.items()}
         x = torch.cat([features.float().mean(1), (question * input_mask).sum(1, keepdim=True).float() * 1e-3 +
                        task_tokens.float()], dim=1)
-        vl = (torch.cat([features.float(), spatials.float()], dim=2) @ self.wv).unsqueeze(-1) + x[:, -1].view(B, 1, 1)
-        pair = (x.view(B // 2, 2, -1).sum(1) @ self.w["bin"]) if B % 2 == 0 else x @ self.w["bin"]
-        return (x @ self.w["vqa"], x @ self.w["gqa"], x @ self.w["logit"], pair, x @ self.w["tri"], None, vl, None,
-                torch.zeros(B, question.shape[1] + 1, 1), [])
+        vl = (torch.cat([features.float(), spatials.float()], dim=2) @ self.wv.to(dev)).unsqueeze(-1) + x[:, -1].view(B, 1, 1)
+        pair = (x.view(B // 2, 2, -1).sum(1) @ w["bin"]) if B % 2 == 0 else x @ w["bin"]
+        return (x @ w["vqa"], x @ w["gqa"], x @ w["logit"], pair, x @ w["tri"], None, vl, None,
+                torch.zeros(B, question.shape[1] + 1, 1, device=dev), [])
 
 
 def _rand_req(task_id, n_img, V, seed, T=37):

@@ -1,4 +1,4 @@
-"""vilbert_b200: B200-native ViLBERT multi-task forward behind the reference worker's object protocol.
+"""vilbert_b200: H100-native (sm_90a) ViLBERT multi-task forward behind the reference worker's object protocol.
 
 Import as ``vilbert_b200`` (the directory name ``vilbert-multi-task_b200`` is not a Python identifier; the
 top-level ``vilbert_b200.py`` maps the name onto this package).

@@ -1,7 +1,7 @@
 """ctypes binding of libvilbert_b200.so (the C ABI declared in include/vilbert_b200.h).
 
 The shared library is built in-tree by ``__graft_entry__.build()`` / ``csrc/Makefile``.  There is
-deliberately NO fallback: if the library is missing, or no sm_100 GPU is visible when an engine is
+deliberately NO fallback: if the library is missing, or no sm_90 GPU is visible when an engine is
 created, the call raises -- the reference-facing API never silently runs on CPU or through PyTorch ops.
 """
 from __future__ import annotations

@@ -2,10 +2,10 @@
 //
 // Replaces, per layer, the reference's 2 batched SGEMMs + scale + mask-add + softmax kernels of
 // BertSelfAttention / BertImageSelfAttention, and the 4 bmm + 2 softmax of BertBiAttention
-// ([UPSTREAM] vilbert/vilbert.py; anchor /root/reference/worker.py:286-289).
+// ([UPSTREAM] vilbert/vilbert.py; anchor worker.py:286-289).
 //
 // Sequences are tiny (T <= 129, V <= 101) and attention is < 1 % of the FLOPs, so the goals are fusion, launch
-// count and instruction count -- not tcgen05 throughput (a 128-row UMMA tile would be 75 % padding at T = 31).
+// count and instruction count -- not tensor-core tile throughput (a 64-row wgmma tile would be half padding at T = 31).
 // One CTA owns one (sample, head): Q/K/V head slices are staged once in shared memory (16-bit, rows padded by
 // 16 B so ldmatrix is conflict-free); each warp owns 16 query rows and runs a register-resident flash-attention
 // pass over the keys in blocks of 64: S = Q K^T on warp-level tensor-core MMAs (mma.sync m16n8k16, fp32
@@ -72,8 +72,7 @@ __device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], 
 
 // One warp: 16 query rows [r0, r0+16) of Qs against nk keys (Ks/Vs zero-padded to a multiple of 16 rows), output columns
 // [oc0, oc0 + OW) of the head.  D = 128 is split into two 64-column work items (S is recomputed by both): 32 instead of 64
-// accumulator registers per thread keep the kernel under 128 registers, i.e. five CTAs per SM and one wave at batch 64
-// (at 170 registers: two CTAs per SM, 1.7 waves -- profiles/r1_attention_ncu.txt).
+// accumulator registers per thread keep the kernel under 128 registers, so several CTAs share an SM.
 // mask_l2[j] = additive key mask * log2(e).  out: 16-bit global, already offset to this head's first column.
 template <int D, int OW, bool F16>
 __device__ __forceinline__ void attend_tile(const uint16_t* Qs, const uint16_t* Ks, const uint16_t* Vs, int r0, int nq,
@@ -373,8 +372,8 @@ static cudaError_t launch_self(const __nv_bfloat16* qkv, int ld_qkv, int hidden,
     cudaError_t e = set_smem(self_attention_kernel<D, F16>, smem);
     if (e != cudaSuccess) return e;
     static const int split_warps = [] { const char* e = getenv("VB200_ATTN_SPLIT_WARPS"); return e ? atoi(e) : 0; }();
-    // one warp per 16-row tile, walking its D / 64 column slices in turn (measured better than one warp per slice: 3-warp CTAs
-    // of the 128-wide heads fit five per SM -> one wave; VB200_ATTN_SPLIT_WARPS=1 for the other layout)
+    // one warp per 16-row tile, walking its D / 64 column slices in turn (small CTAs: many per SM); VB200_ATTN_SPLIT_WARPS=1 for
+    // one warp per slice
     const int nwarps = min(8, (Lp / 16) * (split_warps ? D / 64 : 1));
     const float scale_l2 = kLog2e / sqrtf(static_cast<float>(D));
     return launch_ex(self_attention_kernel<D, F16>, dim3(heads, B), dim3(32 * nwarps), smem, pdl, st,

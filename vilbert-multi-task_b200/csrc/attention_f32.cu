@@ -4,7 +4,7 @@
 // attention.cu):
 //   * the fp32-parity mode (compute_dtype = "fp32x"): Q/K/V arrive as fp32 from the split-operand QKV GEMM and the context
 //     leaves as the fp16 hi | lo | hi operand of the next GEMM (common.cuh split_col);
-//   * `attn_data_list`, element 9 of the reference's 10-tuple (/root/reference/worker.py:287-288, returned because the worker
+//   * `attn_data_list`, element 9 of the reference's 10-tuple (worker.py:287-288, returned because the worker
 //     sets config.visualization, worker.py:522): the attention probabilities [B, heads, Lq, Lk] in fp32, written by this
 //     kernel from the same 16-bit Q/K the tensor-core kernel consumed (context output off).
 //

@@ -1,5 +1,5 @@
-// sm_100a device primitives shared by the vilbert_b200 kernels: mbarrier, TMA, tcgen05/TMEM,
-// cluster/DSMEM helpers and small math.  Raw PTX only (no CUTLASS dependency).
+// sm_90a device primitives shared by the vilbert_b200 kernels: mbarrier, TMA, cluster/DSMEM helpers and small math
+// (the warpgroup MMA wrappers are in wgmma.cuh).  Raw PTX only (no CUTLASS dependency).
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -41,7 +41,7 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
 }
 __device__ __forceinline__ void mbar_fence_init() {
-    // make mbarrier.init visible to the async proxy (TMA / tcgen05.commit) and to the cluster
+    // make mbarrier.init visible to the async proxy (TMA) and to the cluster
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t tx_bytes) {
@@ -72,6 +72,15 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
                    parity);
             __trap();
         }
+    }
+}
+
+// The same wait without the diagnostic printf, for code that waits while a wgmma group is in flight: a function call (vprintf)
+// inside that window makes ptxas serialise every wgmma of the kernel (C7510).
+__device__ __forceinline__ void mbar_wait_nocall(uint64_t* bar, uint32_t parity) {
+    uint32_t spins = 0;
+    while (!mbar_try_wait(bar, parity)) {
+        if (++spins > VB_SPIN_LIMIT) __trap();
     }
 }
 
@@ -109,94 +118,6 @@ __device__ __forceinline__ void tma_store_commit_and_wait_read() {
 }
 // generic-proxy writes to shared memory -> visible to the async proxy (TMA) that is about to read them
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-
-// ------------------------------------------------------------------ tcgen05 / TMEM
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst) {  // whole warp
-    static_assert(kCols >= 32 && kCols <= 512 && (kCols & (kCols - 1)) == 0, "TMEM columns: power of two in [32,512]");
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-                 "r"(kCols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {  // whole warp (the allocating one)
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(kCols) : "memory");
-}
-
-// Shared-memory matrix descriptor, K-major operand, 128-byte swizzle, rows of exactly 128 bytes
-// (64 bf16): 8-row groups are 1024 B apart (SBO); LBO is unused for swizzled K-major layouts.
-// Bit layout: [0,14) addr>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [46,48) version=1 | [61,64) layout (2 = SWIZZLE_128B)
-__device__ __forceinline__ uint64_t umma_desc_kmajor_sw128(const void* smem_ptr) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((smem_u32(smem_ptr) & 0x3FFFFu) >> 4);
-    d |= static_cast<uint64_t>(1) << 16;             // LBO (ignored)
-    d |= static_cast<uint64_t>(1024 >> 4) << 32;     // SBO
-    d |= static_cast<uint64_t>(1) << 46;             // descriptor version (Blackwell)
-    d |= static_cast<uint64_t>(2) << 61;             // SWIZZLE_128B
-    return d;
-}
-
-// Instruction descriptor for kind::f16: F16 x F16 or BF16 x BF16 -> FP32, both operands K-major.
-// (Mixing F16 activations with BF16 weights is encodable but traps as an illegal instruction on sm_100a -- measured.)
-// [4,6) D fmt (1=F32) | [7,10) A fmt (0=F16, 1=BF16) | [10,13) B fmt | 15/16 A/B major (0=K) | [17,23) N>>3 | [24,29) M>>4
-__host__ __device__ constexpr uint32_t umma_idesc_f32acc(uint32_t m, uint32_t n, bool is_f16) {
-    return (1u << 4) | ((is_f16 ? 0u : 1u) << 7) | ((is_f16 ? 0u : 1u) << 10) | ((n >> 3) << 17) | ((m >> 4) << 24);
-}
-
-// D[tmem] (+)= A[smem] * B[smem]^T ; issued by ONE thread.
-__device__ __forceinline__ void umma_bf16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// mbarrier arrive when all previously issued tcgen05.mma of this thread have completed
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-
-// TMEM -> registers: this warp's 32 lanes x 32 consecutive fp32 columns (thread i <- lane base+i).
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-    uint32_t* r = reinterpret_cast<uint32_t*>(v);
-    __syncwarp();   // .sync.aligned below: reconverge after any divergent epilogue code
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-// registers -> TMEM, same shape.
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const float (&v)[32]) {
-    const uint32_t* r = reinterpret_cast<const uint32_t*>(v);
-    __syncwarp();
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-        ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-        "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]),
-        "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]),
-        "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-        : "memory");
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
 
 // ------------------------------------------------------------------ cluster / DSMEM
 __device__ __forceinline__ uint32_t cluster_ctarank() {
@@ -251,10 +172,9 @@ __device__ __forceinline__ float gelu_erf_as(float x) { return x * 0.5f * (1.0f 
 // Same function, 11 issue slots and no MUFU: gelu(x) = x * Phi(x) with Phi(x) ~ sat(0.5 + x * Q(x^2)), Q of degree 8 in x^2 fitted on
 // |x| <= 4.25 with weight |x| (scripts/fit_gelu.py), sat = the FFMA's free saturation to [0, 1].  Q's leading coefficient is positive, so
 // beyond the fitted range x * Q(x^2) runs monotonically to +-inf and the saturation returns Phi = 1 / 0 EXACTLY: a strongly negative
-// pre-activation gives -0 and a strongly positive one x itself, with no range clamp (round 1 clamped z and returned -1.1e-5 * x there;
-// the first round-2 form needed min(z^2, 9) and a two-sided clamp: 16 slots).  |gelu error| <= 4.3e-5 over the whole fp32 range, < 5 % of
-// half an fp16 ulp at the magnitude where it occurs; the A&S form above is 30x more accurate but costs ~27 slots incl. 2 MUFU, and the
-// FFN-in epilogue is FP32-pipe bound (16 K evaluations per 128x128 tile; FFMA2 halves the issue slots, not the pipe time -- measured).
+// pre-activation gives -0 and a strongly positive one x itself, with no range clamp.  |gelu error| <= 4.3e-5 over the whole fp32 range,
+// < 5 % of half an fp16 ulp at the magnitude where it occurs; the A&S form above is 30x more accurate but costs ~27 slots incl. 2 MUFU,
+// and the FFN-in epilogue evaluates it 16 K times per 128x128 tile.
 __device__ __forceinline__ float gelu_erf(float x) {
     const float u = x * x;
     float q = 4.547042257e-11f;

@@ -3,7 +3,7 @@
 //
 // Replaces BertEmbeddings (3 gathers + cat + LayerNorm), the input side of BertImageEmbeddings and the
 // 1-/3-wide nn.Linear heads (vil_logit, vil_tri_prediction, vision_logit, linguisic_logit, the last layer of
-// vil_binary_prediction) of [UPSTREAM] vilbert/vilbert.py; anchors /root/reference/worker.py:286-289, 416-419, 452-455.
+// vil_binary_prediction) of [UPSTREAM] vilbert/vilbert.py; anchors worker.py:286-289, 416-419, 452-455.
 #include "kernels.h"
 
 namespace vb {

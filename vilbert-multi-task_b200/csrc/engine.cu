@@ -1,7 +1,7 @@
 // Host side of the vilbert_b200 engine: BertConfig JSON, state_dict audit + weight repack, per-shape plans
 // (workspace, TMA descriptors, launch list, CUDA graph) and the C ABI of include/vilbert_b200.h.
 //
-// Mirrors what the reference does at /root/reference/worker.py:495-536 (config + from_pretrained + cuda)
+// Mirrors what the reference does at worker.py:495-536 (config + from_pretrained + cuda)
 // and worker.py:286-289 (the forward call); the layer schedule and module wiring follow the [UPSTREAM]
 // vilbert/vilbert.py restated in SURVEY.md section 3C / 8a.
 #include "../../include/vilbert_b200.h"
@@ -359,7 +359,7 @@ struct Op {
     GemmEpilogue ep;
     int block_n = 128;
     bool ln = false;
-    bool pair = false;             // CTA-pair kernel (cta_group::2); tb then has box rows block_n / 2
+    bool pair = false;             // CTA pair (gemm_persistent.cuh PCfg MODE 8); tb then has box rows block_n / 2
     // chained GEMM (gemm_chain.cu): this GEMM's 16-bit output is the A operand of a second one issued from the same launch
     CUtensorMap ta2, tb2;
     GemmEpilogue ep2;
@@ -439,26 +439,16 @@ struct vb200_engine {
     int num_labels = 0, gqa_labels = 0;
     bool dry = false;          // audit pass: check names / shapes / dtypes only, touch no device
     bool ln_fold = false;      // LayerNorm folded into the neighbouring GEMMs (row_stats in gemm_persistent.cuh); opt-in
-                               // (vb200_options::ln_fold = 1 / VB200_LNFOLD=1): 57 fewer launches per forward, but the heavier
-                               // GEMM epilogues cost more than the row kernels they replace (measured: 36.9 k vs 40.8 k pairs/s
-                               // at batch 64, profiles/r2_ln_fold.md) -- default stays GEMM (fp32 out) + row LayerNorm kernel
+                               // (vb200_options::ln_fold = 1 / VB200_LNFOLD=1): 57 fewer launches per forward, paid for with
+                               // heavier GEMM epilogues -- default stays GEMM (fp32 out) + row LayerNorm kernel
     std::set<std::string> fold_out_t, fold_out_v;   // stages ("T3", "C0", "E", ...) whose OUTPUT LayerNorm stays pending
     bool chain_ffn = false;    // VB200_CHAIN=1 / vb200_set_option("chain_ffn", 1): FFN-in and FFN-out as ONE chained launch (gemm_chain.cu);
-                               // bit-identical, measured slower at batch 64 (profiles/r2_chain.md) -> opt-in
-    bool wide192 = false;      // VB200_BN192=1: 128x192 tiles for GEMMs that need more than one wave of 128-wide ones.  Faster per
-                               // launch (FFN-in 18.5 -> 16.2 us, image QKV 16.9 -> 14.9 us, 973 TFLOP/s) but the STEP is 3 % slower
-                               // with them (38.8 k vs 40.1 k pairs/s, profiles/r2_tile192.md) -- opt-in
-    int tri_min_tiles = 0;     // VB200_TRI=<tiles> (0 = off): plain 128-wide GEMMs with at least this many tiles run THREE CTAs per SM
-                               // (PCfg MODE 6: 2-stage ring, one accumulator, four epilogue warps)
+                               // bit-identical to two launches; opt-in
     int lone_rows = 320;       // VB200_LONE_ROWS (0 = off): forwards with at most this many rows in either stream (batch <= 8 at the default
-                               // shapes) run their plain 128-wide GEMMs one CTA per SM with a 6-stage ring (PCfg MODE 7): nothing else is
-                               // there to share the SM, and a lone CTA's k loop is 1.5x faster with six stages in flight
+                               // shapes) run their plain GEMMs with 64-wide tiles while those still fit one CTA per SM
     bool x3 = false;           // fp32-parity mode (vb200_options::split_fp32): fp16 hi/lo split operands, K' = 3K GEMMs, fp32 attention
     // Programmatic dependent launch.  Default: every kernel ("full": each kernel triggers its dependents once its main work is
-    // issued; a dependent GEMM's producer puts its first weight tiles in flight before griddepcontrol.wait).  Measured with two
-    // batches in flight, per step: off 1.597-1.604 ms | full 1.567 | "mediumplus" (everything except edges across a fork / join)
-    // 1.571-1.581 | "medium" (into LayerNorm / attention and into the GEMM that follows one) 1.557-1.566 on another box whose
-    // off was 1.601; with ONE batch in flight 1.83 (full) vs 1.96 ms (off).
+    // issued; a dependent GEMM's producer puts its first weight tiles in flight before griddepcontrol.wait).
     // VB200_PDL=off|light|medium|mediumplus|full; use_pdl < 0 = off, > 0 = full.
     bool pdl_light = true;
     bool pdl_medium = true;
@@ -466,14 +456,12 @@ struct vb200_engine {
     bool early_w = true;            // VB200_EARLYW=0: no weight loads ahead of griddepcontrol.wait
     bool pdl_gemm_gemm = false;     // VB200_PDL=mediumplus: also GEMM -> GEMM edges of one graph branch (FFN-in -> FFN-out)
     int light_pdl() const { return (pdl_light || opt.use_pdl) ? 1 : 0; }
-    // CTA-pair GEMM (cta_group::2, gemm_pair.cu).  -1 = auto: 256-wide pair tiles where a GEMM has >= 4 waves of them (large
-    // batches: +6 % at batch 512); below that the single-CTA kernel wins -- one or two tiles per CTA, where the pair's extra
-    // cluster syncs and coarser tiles cost more than the halved W traffic saves (profiles/README.md).  VB200_PAIR=0|128|256
-    // forces it off / on for every plain GEMM with >= 256 rows.
-    int pair_bn = -1;
-    int pair_min_waves = 0;    // automatic CTA-pair selection: at least this many waves of 256 x 256 pair tiles.  0 = measured rule
-                               // (profiles/r2_b512.md): 2 waves when the GEMM has >= 20 row panels of 256 (batch >= ~160: 512: +5.7 %,
-                               // 384: +2 %, 192: +1 %, 256: =), else 4 (batch 128 loses 4.5 % with 2).  VB200_PAIR_MIN_WAVES overrides.
+    // CTA pair (launch_gemm_pair: two CTAs of a cluster share each weight tile through TMA multicast).  Off by default: on an H100
+    // it measured 0.59x (batch 512) and 0.66x (batch 64) the step throughput of the single-CTA kernel (DESIGN.md section 5).
+    // VB200_PAIR=1 forces it on for every plain GEMM with >= 256 rows and N % 128 == 0; VB200_PAIR=auto picks it for GEMMs with at
+    // least PAIR_MIN_WAVES waves of 256 x 128 pair tiles over the SM pairs.
+    int pair_mode = 0;
+    int pair_min_waves = 2;        // VB200_PAIR_MIN_WAVES
     bool fused_ln = false;     // VB200_FUSED_LN=1: cluster-LayerNorm GEMM epilogue instead of GEMM(fp32) + row LayerNorm kernel
     Arena weights;
     std::string last_error;
@@ -857,7 +845,7 @@ struct vb200_engine {
     // One nn.Linear (+ activation, + residual LayerNorm) -> one or two launch-list entries on `stream`.
     //   fused_ln:  a single cluster-LayerNorm GEMM (epilogue normalises across the N tiles of a cluster)
     //   default :  GEMM (+bias, +activation) writing fp32 to the stream's scratch, then the row LayerNorm kernel
-    //              (adds the residual) -- measured faster at every batch size tried (profiles/).
+    //              (adds the residual).
     // All sizes are LOGICAL (elements of the mathematical matrices).  In fp32-parity mode (x3) every 16-bit operand buffer is
     // physically 3x as wide (fp16 hi | lo | hi per 64 columns), so operand strides, the contraction length and the 16-bit
     // output stride are multiplied by S = 3 here and nowhere else.
@@ -889,40 +877,20 @@ struct vb200_engine {
         op.ln = ln != nullptr && !split_ln && !keep_pending;      // cluster-LayerNorm epilogue (fused_layernorm option)
         op.block_n = vb::gemm_p_pick_block_n(W.N, op.ln);
         if (op.block_n == 0) fail(VB200_ERR_INVALID, "no LayerNorm-fused GEMM tiling for N=%d", W.N);
-        if (!x3 && !op.ln && !keep_pending && !fold_in && a_rows >= 256) {
-            if (pair_bn > 0) op.pair = W.N % pair_bn == 0;
-            else if (pair_bn < 0) {
-                const long long panels = (a_rows + 255) / 256;
-                const int waves = pair_min_waves > 0 ? pair_min_waves : (panels >= 20 ? 2 : 4);
-                op.pair = W.N % 256 == 0 && panels * (W.N / 256) >= static_cast<long long>(waves) * (vb::num_sms_host() / 2);
-            }
-            if (op.pair) op.block_n = pair_bn > 0 ? pair_bn : 256;
+        if (pair_mode != 0 && !x3 && !op.ln && !keep_pending && !fold_in && a_rows >= 256 && W.N % 128 == 0) {
+            const long long pair_tiles = ((a_rows + 255) / 256) * (W.N / 128);
+            op.pair = pair_mode > 0 || pair_tiles >= static_cast<long long>(pair_min_waves) * (vb::num_sms_host() / 2);
+            if (op.pair) op.block_n = 128;
         }
-        if (wide192 && !x3 && !op.ln && !op.pair && !keep_pending && !fold_in && W.N % 192 == 0 && op.block_n == 128) {
-            // 128x192 tiles when 128-wide ones need more than one wave of the 2-per-SM CTA slots and 192-wide ones fit in one
-            // (the N = 3072 GEMMs at batch 64).  The tile width never changes an element's accumulation order: results are the same bits.
-            const long long slots = 2LL * vb::num_sms_host(), mt = (a_rows + 127) / 128;
-            if (mt * ((W.N + 127) / 128) > slots && mt * (W.N / 192) <= slots) op.block_n = 192;
-        }
-        // Small forwards (<= lone_rows rows in either stream, batch <= 8): one CTA per SM with a 6-stage ring (PCfg MODE 7), and 64-wide
-        // tiles while they still fit one per SM -- twice the CTAs, half the epilogue each (batch 1: 0.932 -> 0.869 ms per forward,
-        // profiles/r2_small_batch_latency.md).  Neither changes an element's accumulation order.
-        bool lone = false;
-        if (lone_rows > 0 && tri_min_tiles == 0 && !x3 && !op.ln && !op.pair && !keep_pending && !fold_in && (op.block_n == 128 || op.block_n == 64) &&
-            std::max(pl.B * pl.T, pl.B * pl.V) <= lone_rows) {
-            const long long mt = (a_rows + 127) / 128;
-            if (mt * ((W.N + 127) / 128) <= vb::num_sms_host()) {
-                lone = true;
-                if (W.N % 64 == 0 && mt * (W.N / 64) <= vb::num_sms_host()) op.block_n = 64;
-            }
-        }
+        // Small forwards (<= lone_rows rows in either stream, batch <= 8): 64-wide tiles while they still fit one CTA per SM -- twice
+        // the CTAs, half the epilogue each.  The tile width never changes an element's accumulation order.
+        if (lone_rows > 0 && !x3 && !op.ln && !op.pair && !keep_pending && !fold_in && op.block_n == 128 && W.N % 64 == 0 &&
+            std::max(pl.B * pl.T, pl.B * pl.V) <= lone_rows && ((a_rows + 127) / 128) * (W.N / 64) <= vb::num_sms_host())
+            op.block_n = 64;
         op.ta = make_tmap(A, a_rows, static_cast<int64_t>(W.ldw) * S, lda * S, 128, opt.act_fp16 != 0);
         op.tb = make_tmap(W.w, W.N, static_cast<int64_t>(W.ldw) * S, static_cast<int64_t>(W.ldw) * S, op.pair ? op.block_n / 2 : op.block_n,
                           opt.act_fp16 != 0);
         GemmEpilogue& e = op.ep;
-        if (tri_min_tiles > 0 && !x3 && !op.ln && !op.pair && !keep_pending && !fold_in && op.block_n == 128 &&
-            ((a_rows + 127) / 128) * ((W.N + 127) / 128) >= tri_min_tiles) e.tri = 1;
-        if (lone) e.lone = 1;
         e.M = static_cast<int>(a_rows); e.N = W.N; e.K = W.ldw * S;
         e.bias = W.bias; e.mul = mul; e.ld_mul = ld_mul; e.eps = cfg.ln_eps; e.act = act; e.pdl = pdl_light ? 2 : (opt.use_pdl ? (early_w ? 5 : 1) : 0);
         e.a_f16 = opt.act_fp16; e.out_f16 = opt.act_fp16;
@@ -1238,12 +1206,12 @@ struct vb200_engine {
     static constexpr int kTimelineCtas = 304;
     void attach_timeline(Plan& pl) {
         size_t n = 0;
-        for (const Op& op : pl.ops) if (op.kind == Op::GEMM && !op.pair && !op.ln && !op.chain_sync) ++n;
+        for (const Op& op : pl.ops) if (op.kind == Op::GEMM && !op.ln && !op.chain_sync) ++n;
         if (n == 0) return;
         pl.timeline = pl.mem.alloc_n<long long>(n * kTimelineCtas * 16);
         CUDA_CHECK(cudaMemset(pl.timeline, 0, n * kTimelineCtas * 16 * sizeof(long long)));
         size_t i = 0;
-        for (Op& op : pl.ops) if (op.kind == Op::GEMM && !op.pair && !op.ln && !op.chain_sync) op.ep.timing = pl.timeline + (i++) * kTimelineCtas * 16;
+        for (Op& op : pl.ops) if (op.kind == Op::GEMM && !op.ln && !op.chain_sync) op.ep.timing = pl.timeline + (i++) * kTimelineCtas * 16;
     }
 
     // Plan cache bound (a MicroBatchWorker produces many (batch, length, regions) combinations): beyond max_plans the least
@@ -1335,8 +1303,9 @@ struct vb200_engine {
                     if (le != cudaSuccess)
                         fail(VB200_ERR_CUDA, "chained GEMM launch failed: %s (layer %s, M=%d N1=%d K1=%d N2=%d)", cudaGetErrorString(le),
                              op.tag ? op.tag : "?", op.ep.M, op.ep.N, op.ep.K, op.ep2.N);
-                } else if (op.pair) CUDA_CHECK(vb::launch_gemm_pair(op.ta, op.tb, op.ep, op.block_n, st));
-                else {
+                } else if (op.pair) {
+                    CUDA_CHECK(vb::launch_gemm_pair(op.ta, op.tb, op.ep, op.block_n, st));
+                } else {
                     GemmEpilogue e = op.ep;
                     e.tmap_c_host = e.tma_store ? &op.tc : nullptr;       // Op objects move when the list grows: bind here
                     e.grid_pct = profile_grid_pct;                        // 0 outside vb200_profile_ops
@@ -1481,7 +1450,7 @@ struct vb200_engine {
 
     // PDL "medium" (default): additionally launch a GEMM programmatically when the kernel before it on its graph branch is a light one
     // (LayerNorm / attention trigger their dependents right after loading their inputs, so the GEMM's prologue -- barrier init,
-    // TMEM allocation, descriptor prefetch -- overlaps the light kernel's math instead of following it).
+    // descriptor prefetch, first weight tiles -- overlaps the light kernel's math instead of following it).
     void link_pdl(Plan& pl) {
         if (!pdl_medium) return;
         int prev_kind[2] = {-1, -1};
@@ -1641,7 +1610,7 @@ void require_device(int device) {
     if (device < 0 || device >= n) fail(VB200_ERR_INVALID, "device ordinal %d out of range (0..%d)", device, n - 1);
     cudaDeviceProp p;
     CUDA_CHECK(cudaGetDeviceProperties(&p, device));
-    if (p.major != 10) fail(VB200_ERR_NO_DEVICE, "device %d is sm_%d%d; the kernels are built for sm_100a only", device, p.major, p.minor);
+    if (p.major != 9 || p.minor != 0) fail(VB200_ERR_NO_DEVICE, "device %d is sm_%d%d; the kernels are built for sm_90a only", device, p.major, p.minor);
     CUDA_CHECK(cudaSetDevice(device));
 }
 }  // namespace
@@ -1681,9 +1650,9 @@ int vb200_create(const char* config_json, int64_t n_tensors, const vb200_tensor*
         eng->x3 = o.split_fp32 != 0;
         eng->fused_ln = o.fused_layernorm != 0;
         if (const char* v = getenv("VB200_FUSED_LN")) eng->fused_ln = (strcmp(v, "1") == 0) && !eng->x3;
-        if (const char* v = getenv("VB200_BN192")) eng->wide192 = (strcmp(v, "0") != 0);
-        if (const char* v = getenv("VB200_TRI")) eng->tri_min_tiles = std::max(0, atoi(v));
         if (const char* v = getenv("VB200_LONE_ROWS")) eng->lone_rows = std::max(0, atoi(v));
+        if (const char* v = getenv("VB200_PAIR")) eng->pair_mode = strcmp(v, "auto") == 0 ? -1 : (atoi(v) != 0 ? 1 : 0);
+        if (const char* v = getenv("VB200_PAIR_MIN_WAVES")) eng->pair_min_waves = std::max(1, atoi(v));
         if (const char* v = getenv("VB200_CHAIN")) eng->chain_ffn = (strcmp(v, "0") != 0);
         eng->ln_fold = o.ln_fold > 0;
         if (const char* v = getenv("VB200_LNFOLD")) eng->ln_fold = (strcmp(v, "0") != 0);
@@ -1701,8 +1670,6 @@ int vb200_create(const char* config_json, int64_t n_tensors, const vb200_tensor*
         }
         if (const char* v = getenv("VB200_TMASTORE")) eng->tma_store_enabled = (strcmp(v, "0") != 0);
         if (const char* v = getenv("VB200_EARLYW")) eng->early_w = (strcmp(v, "0") != 0);
-        if (const char* v = getenv("VB200_PAIR_MIN_WAVES")) eng->pair_min_waves = std::max(0, atoi(v));
-        if (const char* v = getenv("VB200_PAIR")) { const int b = atoi(v); eng->pair_bn = (b == 128 || b == 256) ? b : (strcmp(v, "auto") == 0 ? -1 : 0); }
         CUDA_CHECK(cudaStreamCreateWithFlags(&eng->side_stream, cudaStreamNonBlocking));
         CUDA_CHECK(cudaEventCreateWithFlags(&eng->ev_fork, cudaEventDisableTiming));
         CUDA_CHECK(cudaEventCreateWithFlags(&eng->ev_join, cudaEventDisableTiming));
@@ -1985,11 +1952,21 @@ int vb200_linear(const void* x_bf16, int64_t ld_x, const void* w_bf16, int64_t l
                  int32_t block_n, int32_t use_pdl, int32_t act_fp16, int32_t variant, long long* timing, void* cuda_stream) {
     return op_guard([&] {
         const bool ln = gamma != nullptr;
-        const bool pair = variant == 2;                                    // CTA-pair kernel: block_n 128 (default) or 256
+        // variant 2: CTA pair (128-wide tiles, N % 128 == 0).  Variants 3 and 4 named Blackwell occupancy configurations of the
+        // persistent kernel (three CTAs per SM; one CTA with a 6-stage ring); ABI version 2 keeps accepting them, and on sm_90a they
+        // select the persistent kernel itself.  block_n 256 (the Blackwell 256-wide tile, plain or pair) runs as 128-wide tiles,
+        // which give the same bits: the tile width never changes an element's accumulation order.
+        const bool pair = variant == 2;
         if (variant != 0 && variant != 2 && variant != 3 && variant != 4)
-            fail(VB200_ERR_INVALID, "vb200_linear: variant %d does not exist (0 persistent, 2 CTA pair, 3 three CTAs per SM, 4 one CTA per SM with a 6-stage ring)", variant);
+            fail(VB200_ERR_INVALID, "vb200_linear: variant %d does not exist (0 persistent, 2 CTA pair, 3 / 4 = 0)", variant);
         int bn = block_n > 0 ? block_n : (pair ? 128 : vb::gemm_p_pick_block_n(static_cast<int>(N), ln));
         if (bn == 0) fail(VB200_ERR_INVALID, "no tiling for N=%lld with LayerNorm", (long long)N);
+        if (!ln && bn == 256) bn = 128;
+        if (!ln && bn != 64 && bn != 128 && bn != 192)
+            fail(VB200_ERR_INVALID, "vb200_linear: block_n %d (plain tiles are 64, 128, 192 or 256 wide)", bn);
+        if (pair && (ln || bn != 128)) fail(VB200_ERR_INVALID, "vb200_linear: the CTA pair is the plain 128- or 256-wide tile");
+        if ((variant == 3 || variant == 4) && (ln || (bn != 128 && !(variant == 4 && bn == 64))))
+            fail(VB200_ERR_INVALID, "vb200_linear: variant 3 is the plain 128-wide tile, variant 4 the 128- or 64-wide one");
         CUtensorMap ta = make_tmap(x_bf16, M, K, ld_x, 128, act_fp16 != 0);
         CUtensorMap tb = make_tmap(w_bf16, N, K, ld_w, pair ? bn / 2 : bn, act_fp16 != 0);
         GemmEpilogue e{};
@@ -2000,11 +1977,7 @@ int vb200_linear(const void* x_bf16, int64_t ld_x, const void* w_bf16, int64_t l
         if (const char* dbg = getenv("VB200_DEBUG")) e.debug = atoi(dbg);          // timing decomposition (kernels.h), op entry only
         CUtensorMap tc;
         const char* ts = getenv("VB200_TMASTORE");
-        if (variant == 3 || variant == 4) {
-            if (ln || (bn != 128 && !(variant == 4 && bn == 64))) fail(VB200_ERR_INVALID, "vb200_linear: variant 3 is the plain 128-wide tile, variant 4 the 128- or 64-wide one");
-            if (variant == 3) e.tri = 1; else e.lone = 1;
-        }
-        if (variant != 2 && !ln && !(ts && strcmp(ts, "0") == 0)) { setup_tma_store(&tc, e); e.tmap_c_host = e.tma_store ? &tc : nullptr; }
+        if (!pair && !ln && !(ts && strcmp(ts, "0") == 0)) { setup_tma_store(&tc, e); e.tmap_c_host = e.tma_store ? &tc : nullptr; }
         if (pair) CUDA_CHECK(vb::launch_gemm_pair(ta, tb, e, bn, static_cast<cudaStream_t>(cuda_stream)));
         else CUDA_CHECK(vb::launch_gemm_persistent(ta, tb, e, bn, ln, static_cast<cudaStream_t>(cuda_stream)));
     });

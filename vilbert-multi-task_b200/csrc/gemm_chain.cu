@@ -1,11 +1,11 @@
 // Two dependent GEMMs in ONE persistent launch (VERDICT r1 item 2(ii)): the FFN of a BertLayer / BertImageLayer / connection layer,
 //     H = act(X W1^T + b1)   (16-bit, [M, N1])          Y = H W2^T + b2   ([M, N2], fp32 for the LayerNorm that follows)
-// ([UPSTREAM] BertIntermediate + BertOutput.dense, vilbert/vilbert.py; anchor /root/reference/worker.py:286-289).
+// ([UPSTREAM] BertIntermediate + BertOutput.dense, vilbert/vilbert.py; anchor worker.py:286-289).
 //
-// Why: at batch 64 a GEMM launch is dominated by per-CTA fixed cost and every CTA owns one tile (profiles/r2_gemm_decomposition.md).
+// Why: at batch 64 a GEMM launch is dominated by per-CTA fixed cost and every CTA owns one or two tiles.
 // Here the CTAs of one grid pull tiles of BOTH GEMMs from one ordered list (chain_decode) -- the second GEMM's tiles of a row panel
 // become available right after the first GEMM's tiles of the NEXT panel -- so there is no launch gap and no second prologue, the
-// double-buffered TMEM accumulator hides each epilogue under the next tile's MMAs, and the long-K second GEMM (96 tiles at batch
+// producer fills the ring for the next tile while the consumers run an epilogue, and the long-K second GEMM (96 tiles at batch
 // 64) no longer leaves a third of the SMs idle.
 //
 // Dependency: tile (m, n) of GEMM 2 reads rows [128 m, 128 m + 128) of H, i.e. ALL N1 / 128 tiles of panel m of GEMM 1.  Every GEMM-1
@@ -54,11 +54,15 @@ __device__ __forceinline__ ChainTile chain_decode(int pos, int P, int n0, int n1
     return t;
 }
 
+// the plain kernel's layout plus two tile_done barriers
+constexpr int kChainSmemBytes = PCfg<128, false, 0>::kSmemBytes + 16;
+static_assert(kChainSmemBytes <= 232448, "shared memory budget");
+
 template <bool F16>
-__global__ void __launch_bounds__(PCfg<128, false, true, 0>::kThreads, 2)
+__global__ void __launch_bounds__(PCfg<128, false, 0>::kThreads, 1)
 gemm_chain_kernel(const __grid_constant__ CUtensorMap ta0, const __grid_constant__ CUtensorMap tb0,
                   const __grid_constant__ CUtensorMap ta1, const __grid_constant__ CUtensorMap tb1, const ChainParams cp) {
-    using Cfg = PCfg<128, false, true, 0>;
+    using Cfg = PCfg<128, false, 0>;
     constexpr int BLOCK_N = 128;
     constexpr int kStages = Cfg::kStages;
     constexpr int kNC = Cfg::kNumChunks;
@@ -67,15 +71,14 @@ gemm_chain_kernel(const __grid_constant__ CUtensorMap ta0, const __grid_constant
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     if ((smem_u32(smem_raw) & 1023u) != 0u) __trap();
     uint8_t* ring = smem_raw;
-    float* s_bias = reinterpret_cast<float*>(ring + kStages * Cfg::kStageBytes);
+    float* s_acc = reinterpret_cast<float*>(ring + kStages * Cfg::kStageBytes);
+    float* s_bias = s_acc + kBlockM * Cfg::kAccLd;
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(s_bias + Cfg::kBiasFloats);
     uint64_t* empty_bar = full_bar + kStages;
-    uint64_t* tmem_full_bar = empty_bar + kStages;
-    uint64_t* tmem_empty_bar = tmem_full_bar + 2;
-    uint64_t* sched_full = tmem_empty_bar + 2;                        // the two barrier slots the cluster-LayerNorm variant uses
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(sched_full + 2);      // [0] TMEM base, [2], [3]: the scheduler's tile slots
-    uint8_t* s_xpose = reinterpret_cast<uint8_t*>(tmem_ptr_smem + 4);
-    volatile int* s_tile = reinterpret_cast<volatile int*>(tmem_ptr_smem + 2);
+    uint64_t* sched_full = empty_bar + kStages;                       // [2] position published in s_tile[i & 1]
+    uint64_t* tile_done = sched_full + 2;                             // [2] the consumers have finished the tile of slot i & 1
+    volatile int* s_tile = reinterpret_cast<volatile int*>(tile_done + 2);
+    uint8_t* s_xpose = reinterpret_cast<uint8_t*>(tile_done + 2) + 16;   // kChainSmemBytes: 16 bytes more than the plain kernel
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int P = cp.m_tiles, n0t = cp.n_tiles[0], n1t = cp.n_tiles[1];
@@ -85,36 +88,26 @@ gemm_chain_kernel(const __grid_constant__ CUtensorMap ta0, const __grid_constant
     int* next_pos = cp.sync + P;
     int* fin = cp.sync + P + 1;
 
-    if (warp == 0 && lane == 0) {
+    if (warp == Cfg::kProducerWarp && lane == 0) {
         tma_prefetch_desc(&ta0); tma_prefetch_desc(&tb0); tma_prefetch_desc(&ta1); tma_prefetch_desc(&tb1);
-        for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(&tmem_full_bar[a], 1);
-            mbar_init(&tmem_empty_bar[a], kEpiThreads);
-            mbar_init(&sched_full[a], 1);
-        }
+        for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], Cfg::kConsumerWarps); }
+        for (int a = 0; a < 2; ++a) { mbar_init(&sched_full[a], 1); mbar_init(&tile_done[a], 1); }
         mbar_fence_init();
-    } else if (warp == 1) {
-        tmem_alloc<Cfg::kTmemCols>(tmem_ptr_smem);
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_smem;
     if (pdl) pdl_wait();
 
     // Dynamic tile scheduler.  The producer thread fetches list positions (atomicAdd) and publishes position i of this CTA in
-    // s_tile[i & 1] / sched_full[i & 1].  A slot is rewritten for position i + 2 only after the epilogue has finished position i
-    // (the producer waits for tmem_empty of accumulator i & 1, whose phase the epilogue completes after reading tile i) -- and the MMA
-    // thread has read slot i long before (it issued tile i's MMAs).  So no extra "slot free" barrier is needed.
-    if (warp == 0) {
+    // s_tile[i & 1] / sched_full[i & 1]; it rewrites a slot for position i + 2 only after the consumers have finished tile i
+    // (tile_done[i & 1]).
+    if (warp == Cfg::kProducerWarp) {
         // ============================================================ TMA producer + scheduler
         if (lane == 0) {
             int s = 0;
             uint32_t phase = 0, it = 0;
             while (true) {
                 const int pos = atomicAdd(next_pos, 1);
-                if (it >= 2) mbar_wait(&tmem_empty_bar[it & 1u], ((it >> 1) & 1u) ^ 1u);   // tile it - 2 fully drained: slot reusable
+                if (it >= 2) mbar_wait_nocall(&tile_done[it & 1u], ((it >> 1) & 1u) ^ 1u);   // tile it - 2 finished: slot reusable
                 s_tile[it & 1u] = pos;
                 mbar_arrive(&sched_full[it & 1u]);                     // release: the consumers' try_wait acquires
                 if (pos >= total) break;
@@ -126,13 +119,13 @@ gemm_chain_kernel(const __grid_constant__ CUtensorMap ta0, const __grid_constant
                     // rows of H this tile reads come from the N1 / 128 GEMM-1 tiles of panel m_t, written by other CTAs
                     uint32_t spins = 0;
                     while (ld_acquire_gpu(panel_done + t.m_t) < n0t) {
-                        if (++spins > VB_SPIN_LIMIT) { printf("vb: chain dependency timeout block %d panel %d\n", blockIdx.x, t.m_t); __trap(); }
+                        if (++spins > VB_SPIN_LIMIT) __trap();          // no printf: a call here would serialise the wgmma (C7510)
                     }
                     fence_proxy_async_all();           // generic-proxy observation -> the async-proxy (TMA) reads that follow
                 }
                 for (int kb = 0; kb < num_kb; ++kb) {
                     uint8_t* sa = ring + s * Cfg::kStageBytes;
-                    mbar_wait(&empty_bar[s], phase ^ 1u);
+                    mbar_wait_nocall(&empty_bar[s], phase ^ 1u);
                     mbar_arrive_expect_tx(&full_bar[s], Cfg::kStageBytes);
                     tma_load_2d(sa, ta, &full_bar[s], kb * kBlockK, t.m_t * kBlockM);
                     tma_load_2d(sa + Cfg::kStageBytesA, tb, &full_bar[s], kb * kBlockK, t.n_t * BLOCK_N);
@@ -142,61 +135,44 @@ gemm_chain_kernel(const __grid_constant__ CUtensorMap ta0, const __grid_constant
             }
         }
         __syncwarp();
-    } else if (warp == 1) {
-        // ============================================================ MMA issuer
-        if (lane == 0) {
-            constexpr uint32_t idesc = umma_idesc_f32acc(kBlockM, BLOCK_N, F16);
-            constexpr uint64_t kDescStage = static_cast<uint64_t>(Cfg::kStageBytes >> 4);
-            const uint64_t da0 = umma_desc_kmajor_sw128(ring);
-            const uint64_t db0 = umma_desc_kmajor_sw128(ring + Cfg::kStageBytesA);
-            int s = 0;
-            uint32_t phase = 0;
-            for (uint32_t it = 0;; ++it) {
-                mbar_wait(&sched_full[it & 1u], (it >> 1) & 1u);
-                const int pos = s_tile[it & 1u];
-                if (pos >= total) break;
-                const int g = chain_decode(pos, P, n0t, n1t).g;
-                const int num_kb = (cp.p[g].K + kBlockK - 1) / kBlockK;
-                const uint32_t acc = it & 1u, acc_phase = (it >> 1) & 1u;
-                mbar_wait(&tmem_empty_bar[acc], acc_phase ^ 1u);
-                tc_fence_after();
-                const uint32_t tmem_d = tmem_base + acc * BLOCK_N;
-                uint32_t accumulate = 0u;
-                for (int kb = 0; kb < num_kb; ++kb) {
-                    mbar_wait(&full_bar[s], phase);
-                    tc_fence_after();
-                    const uint64_t da = da0 + kDescStage * static_cast<uint64_t>(s);
-                    const uint64_t db = db0 + kDescStage * static_cast<uint64_t>(s);
-#pragma unroll
-                    for (int k = 0; k < kBlockK / kUmmaK; ++k) {
-                        umma_bf16_ss(tmem_d, da + 2u * k, db + 2u * k, idesc, accumulate);
-                        accumulate = 1u;
-                    }
-                    umma_commit(&empty_bar[s]);
-                    if (++s == kStages) { s = 0; phase ^= 1u; }
-                }
-                umma_commit(&tmem_full_bar[acc]);
-            }
-            if (pdl) pdl_launch_dependents();
-        }
-        __syncwarp();
     } else {
-        // ============================================================ epilogue warps
-        const int ew = warp - 2, q = warp & 3, et = threadIdx.x - 64;
+        // ============================================================ consumer warpgroups: MMA, then epilogue
+        constexpr uint64_t kDescStage = static_cast<uint64_t>(Cfg::kStageBytes >> 4);
+        const int wg = warp >> 2;
+        const uint64_t da0 = gmma_desc_kmajor_sw128(smem_u32(ring + wg * 64 * 128));
+        const uint64_t db0 = gmma_desc_kmajor_sw128(smem_u32(ring + Cfg::kStageBytesA));
+        const int ew = warp, q = warp & 3, et = threadIdx.x;
+        const int row = q * 32 + lane;
+        const float* acc_row = s_acc + row * Cfg::kAccLd;
+        int ks = 0;
+        uint32_t kphase = 0;
         for (uint32_t it = 0;; ++it) {
-            mbar_wait(&sched_full[it & 1u], (it >> 1) & 1u);
+            mbar_wait_nocall(&sched_full[it & 1u], (it >> 1) & 1u);
             const int pos = s_tile[it & 1u];
             if (pos >= total) break;
             const ChainTile t = chain_decode(pos, P, n0t, n1t);
             const GemmEpilogue& p = cp.p[t.g];
-            const uint32_t acc = it & 1u, acc_phase = (it >> 1) & 1u;
+            const int num_kb = (p.K + kBlockK - 1) / kBlockK;
             const int m0 = t.m_t * kBlockM, n0 = t.n_t * BLOCK_N;
-            const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * BLOCK_N;
-            if (it > 0) epi_bar_sync<kEpiThreads>();                   // the previous tile's bias slice has been read by everybody
             for (int i = et; i < BLOCK_N; i += kEpiThreads) s_bias[i] = (p.bias && n0 + i < p.N) ? p.bias[n0 + i] : 0.0f;
-            epi_bar_sync<kEpiThreads>();
-            mbar_wait(&tmem_full_bar[acc], acc_phase);
-            tc_fence_after();
+            {
+                float d[BLOCK_N / 2];
+                int prev = -1;
+                for (int kb = 0; kb < num_kb; ++kb) {
+                    mbar_wait_nocall(&full_bar[ks], kphase);
+                    mma_kblock<BLOCK_N, F16>(d, da0 + kDescStage * static_cast<uint64_t>(ks), db0 + kDescStage * static_cast<uint64_t>(ks), kb == 0);
+                    if (prev >= 0) {
+                        wgmma_wait<1>();
+                        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+                    }
+                    prev = ks;
+                    if (++ks == kStages) { ks = 0; kphase ^= 1u; }
+                }
+                wgmma_wait<0>();
+                if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+                acc_deposit<BLOCK_N>(s_acc, d, threadIdx.x);
+            }
+            epi_bar_sync<kEpiThreads>();                               // tile deposited, bias slice written
             constexpr int kCPG = kNC / 2;
             const int cg = ew >> 2;
 #pragma unroll
@@ -204,8 +180,7 @@ gemm_chain_kernel(const __grid_constant__ CUtensorMap ta0, const __grid_constant
                 const int c = cg * kCPG + ci;
                 const int nc = n0 + c * 32;
                 float v[32];
-                tmem_ld32_issue(taddr + c * 32, v);
-                tmem_ld_wait();
+                acc_ld32(acc_row + c * 32, v);
                 const float* bs = s_bias + c * 32;
                 if (p.act == kActGelu) bias_act32<kActGelu>(v, bs);
                 else if (p.act == kActRelu) bias_act32<kActRelu>(v, bs);
@@ -216,25 +191,19 @@ gemm_chain_kernel(const __grid_constant__ CUtensorMap ta0, const __grid_constant
                     if (p.out_bf16 != nullptr) store16_sw<F16>(xb, p.out_bf16, p.ld_bf16, m0 + q * 32, p.M, nc, v, lane);
                 }
             }
-            if (t.g == 0) {
-                // this tile of H is complete once every epilogue thread's stores are visible device-wide
-                __threadfence();
-                epi_bar_sync<kEpiThreads>();
-                if (et == 0) red_release_gpu_add(panel_done + t.m_t, 1);
+            // this tile of H is complete once every consumer thread's stores are visible device-wide; the barrier also frees
+            // s_acc and the bias slice for the next tile
+            if (t.g == 0) __threadfence();
+            epi_bar_sync<kEpiThreads>();
+            if (et == 0) {
+                if (t.g == 0) red_release_gpu_add(panel_done + t.m_t, 1);
+                mbar_arrive(&tile_done[it & 1u]);
             }
-            // accumulator (and with it the scheduler slot of this parity) back to the MMA thread / the producer -- AFTER the tile is
-            // completely finished, because the producer reuses slot it & 1 for position it + 2 on this barrier
-            tc_fence_before();
-            mbar_arrive(&tmem_empty_bar[acc]);
         }
+        if (pdl && threadIdx.x == 0) pdl_launch_dependents();
     }
 
-    tc_fence_before();
     __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc<Cfg::kTmemCols>(tmem_base);
-    }
     // the last CTA to leave zeroes the counters: the launch can be replayed (CUDA graph) without a memset node
     if (threadIdx.x == 0) {
         __threadfence();
@@ -251,7 +220,7 @@ gemm_chain_kernel(const __grid_constant__ CUtensorMap ta0, const __grid_constant
 cudaError_t launch_gemm_chain(const CUtensorMap& ta0, const CUtensorMap& tb0, const GemmEpilogue& ep0, const CUtensorMap& ta1,
                               const CUtensorMap& tb1, const GemmEpilogue& ep1, int* sync, cudaStream_t st) {
     using namespace pgemm;
-    using Cfg = PCfg<128, false, true, 0>;
+    using Cfg = PCfg<128, false, 0>;
     if (ep0.M != ep1.M || ep0.M < 1 || ep0.N < 1 || ep1.N < 1 || ep0.K < 1 || ep1.K < 1 || sync == nullptr) return cudaErrorInvalidValue;
     if (ep0.a_f16 != ep1.a_f16 || ep0.a_f16 != ep0.out_f16 || ep1.a_f16 != ep1.out_f16) return cudaErrorInvalidValue;
     for (const GemmEpilogue* e : {&ep0, &ep1}) {
@@ -261,7 +230,7 @@ cudaError_t launch_gemm_chain(const CUtensorMap& ta0, const CUtensorMap& tb0, co
     }
     if (ep0.out_bf16 == nullptr) return cudaErrorInvalidValue;                            // H is GEMM 2's A operand
     auto kern = ep0.a_f16 ? gemm_chain_kernel<true> : gemm_chain_kernel<false>;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kChainSmemBytes);
     if (e != cudaSuccess) return e;
     ChainParams cp{};
     cp.p[0] = ep0; cp.p[1] = ep1;
@@ -270,11 +239,12 @@ cudaError_t launch_gemm_chain(const CUtensorMap& ta0, const CUtensorMap& tb0, co
     cp.n_tiles[0] = (ep0.N + 127) / 128; cp.n_tiles[1] = (ep1.N + 127) / 128;
     cp.sync = sync;
     const int tiles = cp.m_tiles * (cp.n_tiles[0] + cp.n_tiles[1]);
-    static const int env_pct = [] { const char* v = getenv("VB200_CHAIN_GRID_PCT"); const int x = v ? atoi(v) : 67; return (x >= 10 && x <= 100) ? x : 67; }();
-    const int slots = std::max(1, num_sms() * 2 * env_pct / 100);
+    static const int env_pct = [] { const char* v = getenv("VB200_CHAIN_GRID_PCT"); const int x = v ? atoi(v) : 100; return (x >= 10 && x <= 100) ? x : 100; }();
+    const int slots = std::max(1, num_sms() * Cfg::kMinBlocks * env_pct / 100);
     cudaLaunchConfig_t cfg;
     cudaLaunchAttribute attrs[2];
     fill_cfg<Cfg, false>(cfg, attrs, dim3(std::min(tiles, slots), 1, 1), 1, ep0.pdl == 1 || ep0.pdl == 5, st);
+    cfg.dynamicSmemBytes = kChainSmemBytes;
     return cudaLaunchKernelEx(&cfg, kern, ta0, tb0, ta1, tb1, cp);
 }
 

@@ -1,27 +1,26 @@
-// Persistent, warp-specialised tcgen05 GEMM (v2 of K3/K6/K7/K8): same math and epilogues as gemm_tcgen05.cu, but
-//   * each CTA (each CLUSTER for the LayerNorm variant) loops over output tiles, so barrier init, TMEM allocation,
-//     descriptor prefetch and the TMA/L2 latency of the first k-block are paid once per kernel, not once per tile;
-//   * the TMA producer runs ahead across tile boundaries (the shared-memory ring never drains);
-//   * the fp32 accumulator is double-buffered in TMEM (2 x BLOCK_N columns): the epilogue of tile i overlaps the MMAs
-//     of tile i+1, and the accumulator is handed back as soon as it has been read into registers;
-//   * epilogue code is specialised OUTSIDE the per-element loops (activation, 16-bit format) -- measured: per-element
-//     run-time branches made a bias-only epilogue cost 11 k cycles per 128x128 tile, 4x the MMA time;
-//   * eight epilogue warps (two per SM sub-partition), every staging access a true LDS/STS, outputs transposed through a
-//     swizzled 2 KB per-warp buffer so that a store instruction writes 8 rows x 64 bytes, GELU through a 15-slot polynomial
-//     erf -- together 10 % of the whole step (profiles/r1_mma_issue_rate.txt, section 8);
+// Persistent, warp-specialised wgmma GEMM (sm_90a):
+//   * each CTA (each CLUSTER for the LayerNorm variant) loops over output tiles, so barrier init, descriptor prefetch and the
+//     TMA/L2 latency of the first k-block are paid once per kernel, not once per tile;
+//   * one TMA producer warp runs ahead across tile boundaries (the shared-memory ring never drains);
+//   * two consumer warpgroups accumulate the 128 x BLOCK_N tile in registers (64 rows each, one k-block of wgmma in flight while
+//     the previous stage is handed back), deposit it in a padded fp32 shared-memory tile and then, as eight epilogue warps, read
+//     it back one row per thread in 32-column chunks -- meanwhile the producer already fills the ring for the next tile;
+//   * epilogue code is specialised OUTSIDE the per-element loops (activation, 16-bit format); outputs are transposed through a
+//     swizzled 2 KB per-warp buffer so that a store instruction writes 8 rows x 64 bytes; GELU through a polynomial erf;
 //   * launched programmatically (GemmEpilogue::pdl) the producer issues the weight tiles of the first ring pass before
-//     griddepcontrol.wait; every kernel triggers its dependents once its last MMA is issued;
+//     griddepcontrol.wait; every kernel triggers its dependents once its last tile is accumulated;
 //   * LN variant: the fp32 residual of the next 32-column chunk is prefetched while the current chunk is processed, and the
 //     first chunk's residual is requested before the accumulator is even ready;
-//   * LayerNorm (8 epilogue warps, x kept in registers, TMEM read once) exchanges ONE (mean, M2) pair per row, column
-//     half and CTA through distributed shared memory (Chan's parallel variance), synchronised by cluster-scope
-//     mbarriers that only the epilogue warps touch -- producer and MMA warps are never stalled by the normalisation.
+//   * LayerNorm (8 epilogue warps, x kept in registers) exchanges ONE (mean, M2) pair per row, column half and CTA through
+//     distributed shared memory (Chan's parallel variance), synchronised by cluster-scope mbarriers that only the epilogue warps
+//     touch -- the producer is never stalled by the normalisation.
 //
 //   D[M,N] = epilogue( A[M,K] (16-bit, row-major)  x  W[N,K]^T (16-bit, nn.Linear layout = K-major) ), fp32 accumulate.
 #pragma once
 #include <algorithm>
 #include <cstdlib>
 #include "kernels.h"
+#include "wgmma.cuh"
 
 namespace vb {
 
@@ -29,78 +28,60 @@ namespace pgemm {
 
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;
-constexpr int kUmmaK = 16;
+constexpr int kMmaK = 16;
 
-// EPI8: eight epilogue warps (two column groups per TMEM lane quarter) -- every instantiation uses it now (KCfg); with four,
-// each SM sub-partition ran ONE epilogue warp and every dependent instruction paid its full latency.
 // MODE 0: default.  MODE 3: the same kernel with the fp32-parity mode's hi | lo | hi 16-bit output (a compile-time variant so the
-// default kernel's 96-register budget is untouched).  MODE 4 / 5: the LayerNorm fold (see row_stats below) -- 4 ("FOLD") consumes an
-// activation whose LayerNorm is still pending, 5 ("LNOUT") produces one.  MODE 2 ("WIDE2", BLOCK_N = 192 or 256):
-// 128x192 (opt-in, VB200_BN192=1) gives the N = 3072 GEMMs at batch 64 256 / 288 tiles = ONE wave of the 296 CTA slots where
-// 128-wide tiles give 384 / 432 (1.3 - 1.5 waves), and a 192-wide MMA takes 96 cycles, so two co-resident issuers (~530 cycles per
-// k-block each, profiles/r2_gemm_decomposition.md) keep the tensor pipe ~90 % busy instead of ~78 %.  The 256-wide form:
-// 128x256 tiles at TWO CTAs per SM -- a 256-wide MMA takes 128 cycles, so the one-issuer limit (134 cycles per MMA) does not
-// bite, and two CTAs keep both the tensor pipe and the ~98 B/clk operand ingest busy; paid for with a 2-stage 48 KB ring, a
-// single-buffered 256-column accumulator and the bias read through L1 instead of shared memory (the budget is 96 bytes short).
-template <int BLOCK_N, bool LN, bool EPI8 = LN, int MODE = 0>
+// default kernel's register budget is untouched).  MODE 4 / 5: the LayerNorm fold (see row_stats below) -- 4 ("FOLD") consumes an
+// activation whose LayerNorm is still pending, 5 ("LNOUT") produces one.  MODE 8 ("PAIR", plain epilogue): the CTA pair -- two CTAs
+// of a cluster take the vertically adjacent 128 x BLOCK_N tiles of one 256-row panel; each loads its own A rows and HALF of the
+// weight tile, which the TMA multicasts into both CTAs, so every weight byte crosses L2 -> SM once per 256 output rows.
+// MODE 0 also comes 192 wide (96 accumulators per consumer thread, a 2-stage ring): 128 x 192 tiles cover an N = 3072 GEMM in
+// 16 column tiles instead of 24.
+// One CTA per SM: each consumer thread holds BLOCK_N / 2 fp32 accumulators, and the deposited tile plus a ring deep enough to
+// cover the L2 latency take most of the 227 KB of shared memory.
+template <int BLOCK_N, bool LN, int MODE = 0>
 struct PCfg {
-    static constexpr bool WIDE2 = MODE == 2;
-    static_assert(!WIDE2 || ((BLOCK_N == 256 || BLOCK_N == 192) && !LN), "WIDE2 is the 192- / 256-wide plain tile");
-    // MODE 6 ("TRI"): THREE CTAs per SM for the GEMMs with more tiles than 2 x 148 -- 128x128 tiles, 2-stage ring (64 KB), one 128-column
-    // accumulator, four epilogue warps (192 threads x 112 registers x 3 fit the register file; 3 x 75 KB the shared memory; 3 x 128 columns
-    // TMEM).  The same six stages per SM are in flight as with 2 x 3, but three CTAs are in three different phases: while one sits in its
-    // prologue or drains its accumulator the other two feed the tensor pipe (profiles/r2_step_timeline.md: a one-tile CTA spends only half
-    // of its life in the main loop, and with two slots an SM has NO main loop running 45 % of the time).
-    static constexpr bool TRI = MODE == 6;
-    static_assert(!TRI || (BLOCK_N == 128 && !LN), "TRI is the 128-wide plain tile");
-    // MODE 7 ("LONE"): ONE CTA per SM with a 6-stage ring (192 KB) -- for the small-batch forwards (batch <= ~8) whose GEMMs have far
-    // fewer tiles than the GPU has SMs, so that no second CTA is there to supply the other three stages the tensor pipe needs: a lone
-    // CTA runs 613 cycles per k-block with 3 stages and 389 with 6 (profiles/r1_mma_issue_rate.txt section 6); the launch chain of a
-    // batch-1 forward is 213 such kernels.  Never used when other kernels could share the SM (batch 64: the step got slower, ibid. 5).
-    static constexpr bool LONE = MODE == 7;
-    static_assert(!LONE || ((BLOCK_N == 128 || BLOCK_N == 64) && !LN), "LONE is the 128- or 64-wide plain tile");
+    static_assert(BLOCK_N == 64 || BLOCK_N == 128 || (LN && BLOCK_N == 96) || (!LN && MODE == 0 && BLOCK_N == 192),
+                  "tile widths: 64 / 128 (LayerNorm also 96, the default plain kernel also 192)");
+    static constexpr bool PAIR = MODE == 8;
+    static_assert(!PAIR || (BLOCK_N == 128 && !LN), "the CTA pair is the plain 128-wide tile");
     static constexpr int kStageBytesA = kBlockM * kBlockK * 2;
     static constexpr int kStageBytesB = BLOCK_N * kBlockK * 2;
     static constexpr int kStageBytes = kStageBytesA + kStageBytesB;
     static constexpr int kNumChunks = BLOCK_N / 32;
-    // Ring depth.  Measured L2->smem latency under load is ~1600 cycles and one 128x128x64 k-block is 256 MMA cycles, so
-    // an SM needs ~6 stages in flight to be MMA-bound.  Plain tiles: 3 stages x 2 CTAs per SM (the second CTA also lets a
-    // kernel of the other ViLBERT stream share the SM).  LayerNorm tiles run one CTA per SM (clusters, 8 epilogue warps
-    // with the row slice in registers) and take the whole ring themselves.
-    static constexpr int kEpiWarps = (LN || (EPI8 && !TRI)) ? 8 : 4;
+    // warps 0-7: two consumer warpgroups (wgmma wants whole, aligned warpgroups; each owns 64 rows of the tile and then works as
+    // four of the eight epilogue warps), warp 8: TMA producer.  Nine warps leave up to 168 registers per thread.
+    static constexpr int kConsumerWarps = 8;
+    static constexpr int kProducerWarp = 8;
+    static constexpr int kEpiWarps = 8;
     static constexpr int kEpiThreads = 32 * kEpiWarps;
-    // warp 0 TMA, warp 1 MMA (+TMEM alloc), then the epilogue warps
-    static constexpr int kThreads = 64 + kEpiThreads;
-    static constexpr int kMinBlocks = TRI ? 3 : (WIDE2 ? 2 : ((LN || LONE || BLOCK_N >= 192) ? 1 : 2));
-    // Per-epilogue-warp transpose buffer so global stores are row-contiguous (a TMEM row lives in ONE lane; writing 16 B per
-    // lane to 32 different rows costs 32 transactions per instruction -- measured ~370 cycles per store instruction).
+    static constexpr int kThreads = 32 * (kConsumerWarps + 1);
+    static constexpr int kMinBlocks = 1;
+    // Deposited accumulator tile: [128][BLOCK_N + 4] fp32.  The pad makes both the row-per-thread float4 reads of the epilogue
+    // and the fragment-layout float2 writes of the consumer warpgroups (at most) two-way bank conflicted.
+    static constexpr int kAccLd = BLOCK_N + 4;
+    static constexpr int kAccBytes = kBlockM * kAccLd * 4;
+    // Per-epilogue-warp transpose buffer so global stores are row-contiguous.
     //   plain: 32 rows x 64 bytes, XOR-swizzled (store16_sw / store_f32_sw);  LN: 32 rows x 33 fp32
-    static constexpr int kXposeBytesPerWarp = LN ? 32 * 33 * 4 : 2048;      // plain: 32 rows x 64 B, swizzled (store16_sw)
+    static constexpr int kXposeBytesPerWarp = LN ? 32 * 33 * 4 : 2048;
     static constexpr int kXposeBytes = kEpiWarps * kXposeBytesPerWarp;
-    static constexpr int kFit = (200 * 1024 - kXposeBytes) / kStageBytes;
-    static constexpr int kStages = (WIDE2 || TRI) ? 2 : (LONE ? 6 : (kMinBlocks == 2 ? 3 : (kFit > 8 ? 8 : kFit)));
-    // Accumulator layout in TMEM: two buffers of BLOCK_N columns (epilogue of tile i overlaps the MMAs of tile i+1); WIDE2: one.
-    // (A lone CTA runs at ~536 cycles per k-block whatever BLOCK_N -- profiles/r1_mma_issue_rate.txt; the round-1 "DEEP" variant
-    // with a second MMA-issuing warp was faster alone and slower in the step, and was removed in round 2.)
-    static constexpr int kAccBufs = (WIDE2 || TRI) ? 1 : 2;
-    static constexpr int kAccCols = kAccBufs * BLOCK_N;
-    static_assert(kAccCols <= 512, "TMEM has 512 columns");
-    static constexpr uint32_t kTmemCols = kAccCols <= 32 ? 32 : (kAccCols <= 64 ? 64 : (kAccCols <= 128 ? 128 : (kAccCols <= 256 ? 256 : 512)));
-    // LN: chunks per epilogue thread (two column halves per TMEM lane quarter)
+    // LN: chunks per epilogue thread (two column halves per row quarter)
     static constexpr int kCPT = (kNumChunks + 1) / 2;
-    // ring | bias (LN: + gamma beta) | LN: part[2 bufs][2 halves][128] float2 | barriers | tmem ptr | transpose buffers
-    static constexpr int kNumBars = 2 * kStages + 4 + 2;
-    // LN-only pieces (gamma, beta, cluster partials) cost nothing in the plain kernel, whose budget is 233472 / 2 - 1024
+    // LN-only pieces: gamma, beta, cluster partials [2 bufs][2 halves][128] float2
     static constexpr int kLnAux = LN ? 2 * BLOCK_N * 4 + 4 * kBlockM * 8 : 0;
     // plain: ONE bias slice (the tile-end barrier of the epilogue warps protects it); LN keeps bias | gamma | beta resident
-    static constexpr bool kBiasInSmem = !WIDE2 || BLOCK_N == 192;     // the 192-wide ring leaves room for the bias slice
-    static constexpr int kBiasFloats = LN ? 2 * BLOCK_N : (kBiasInSmem ? BLOCK_N : 0);
+    static constexpr int kBiasFloats = LN ? 2 * BLOCK_N : BLOCK_N;
+    static constexpr int kBarBytes = (2 * 8 + 2) * 8 + 16;
+    static constexpr int kFit = (232448 - kAccBytes - kXposeBytes - kBiasFloats * 4 - kLnAux - kBarBytes) / kStageBytes;
+    static constexpr int kStages = kFit > 8 ? 8 : kFit;
+    static constexpr int kNumBars = 2 * kStages + 2;
     static constexpr int kSmemAux = kBiasFloats * 4 + kLnAux + kNumBars * 8 + 16 + kXposeBytes;
-    // no alignment slack: the dynamic shared-memory window starts 1024-aligned (checked at kernel entry).  An SM has 233472
-    // bytes and every CTA costs its dynamic size + 1024 reserved.
-    static constexpr int kSmemBytes = kStages * kStageBytes + kSmemAux;
-    static_assert(kMinBlocks == 1 ? kSmemBytes <= 232448 : kMinBlocks * (kSmemBytes + 1024) <= 233472, "shared memory budget");
+    // no alignment slack: the dynamic shared-memory window starts 1024-aligned (checked at kernel entry)
+    static constexpr int kSmemBytes = kStages * kStageBytes + kAccBytes + kSmemAux;
+    static_assert(kStages >= 2 && kSmemBytes <= 232448, "shared memory budget (227 KB per block)");
 };
+// Largest LayerNorm cluster: a row of up to 16 tiles (non-portable cluster size on H100).
+constexpr int kMaxCluster = 16;
 
 // ---- cluster-scope mbarrier helpers (LayerNorm exchange)
 __device__ __forceinline__ uint32_t mapa_u32(const void* local_smem_ptr, uint32_t rank) {
@@ -125,8 +106,7 @@ __device__ __forceinline__ void mbar_wait_acquire_cluster(uint64_t* bar, uint32_
             : "memory");
         if (ok) break;
         if (++spins > VB_SPIN_LIMIT) {
-            printf("vb: cluster mbarrier timeout block(%d,%d) thread %d\n", blockIdx.x, blockIdx.y, threadIdx.x);
-            __trap();
+            __trap();                    // no printf: a call in a kernel that issues wgmma serialises it (C7510)
         }
     }
 }
@@ -138,42 +118,35 @@ __device__ __forceinline__ float2 dsmem_ld_f32x2(uint32_t cluster_addr) {
 template <int kThreadsInBar>
 __device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kThreadsInBar) : "memory"); }
 
-// ---- TMEM load split into issue / wait so a chunk's load overlaps the previous chunk's math and stores
-__device__ __forceinline__ void tmem_ld32_issue(uint32_t taddr, float (&v)[32]) {
-    uint32_t* r = reinterpret_cast<uint32_t*>(v);
-    __syncwarp();
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
+// ---- one row's 32 consecutive accumulator columns from the deposited tile
+__device__ __forceinline__ void acc_ld32(const float* src, float (&v)[32]) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        const float4 f = reinterpret_cast<const float4*>(src)[j];
+        v[4 * j] = f.x; v[4 * j + 1] = f.y; v[4 * j + 2] = f.z; v[4 * j + 3] = f.w;
+    }
 }
-__device__ __forceinline__ void tmem_ld16_issue(uint32_t taddr, float (&v)[16]) {
-    uint32_t* r = reinterpret_cast<uint32_t*>(v);
-    __syncwarp();
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
+
+// ---- consumer warpgroup wg: rows [64 wg, 64 wg + 64) of the 128 x BLOCK_N accumulator, one k-block (four k steps)
+template <int BLOCK_N, bool F16>
+__device__ __forceinline__ void mma_kblock(float (&d)[BLOCK_N / 2], uint64_t da, uint64_t db, bool first) {
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < kBlockK / kMmaK; ++k) Wgmma<BLOCK_N, F16>::mma(d, da + 2u * k, db + 2u * k, (first && k == 0) ? 0u : 1u);
+    wgmma_commit();
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// The same wait, tied to the registers of a load that was issued EARLIER than the code just above this call (software-pipelined
-// epilogue): the "+f" operands make every later use of v depend on the wait, so nothing that reads v can be scheduled ahead of it.
-__device__ __forceinline__ void tmem_ld_wait_for(float (&v)[32]) {
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+f"(v[0]), "+f"(v[1]), "+f"(v[2]), "+f"(v[3]), "+f"(v[4]), "+f"(v[5]), "+f"(v[6]), "+f"(v[7]), "+f"(v[8]), "+f"(v[9]),
-                   "+f"(v[10]), "+f"(v[11]), "+f"(v[12]), "+f"(v[13]), "+f"(v[14]), "+f"(v[15]), "+f"(v[16]), "+f"(v[17]), "+f"(v[18]),
-                   "+f"(v[19]), "+f"(v[20]), "+f"(v[21]), "+f"(v[22]), "+f"(v[23]), "+f"(v[24]), "+f"(v[25]), "+f"(v[26]), "+f"(v[27]),
-                   "+f"(v[28]), "+f"(v[29]), "+f"(v[30]), "+f"(v[31])
-                 :: "memory");
+// Fragment layout of m64nNk16 (thread t of the consumer threads, t / 128 = warpgroup): d[4j + {0,1}] -> row 16 (t / 32) + (t % 32) / 4,
+// columns 8j + 2 (t % 4) + {0,1}; d[4j + {2,3}] -> the same columns 8 rows further down.
+template <int BLOCK_N>
+__device__ __forceinline__ void acc_deposit(float* s_acc, const float (&d)[BLOCK_N / 2], int t) {
+    constexpr int ld = BLOCK_N + 4;
+    const int r0 = 16 * (t >> 5) + ((t & 31) >> 2), c0 = 2 * (t & 3);
+#pragma unroll
+    for (int j = 0; j < BLOCK_N / 8; ++j) {
+        float* o = s_acc + r0 * ld + 8 * j + c0;
+        *reinterpret_cast<float2*>(o) = make_float2(d[4 * j], d[4 * j + 1]);
+        *reinterpret_cast<float2*>(o + 8 * ld) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+    }
 }
 
 // ---- straight-line per-chunk epilogue pieces (all flags resolved outside the element loops)
@@ -411,17 +384,12 @@ __device__ __forceinline__ void row_stats(const float2* __restrict__ stats, int 
     rstd = 1.0f / sqrtf(m2 / n_cols + eps);
 }
 
-template <int BLOCK_N, bool LN, int ACT, int MODE = 0>
-struct KCfg { using type = PCfg<BLOCK_N, LN, true, MODE>; };   // 8 epilogue warps everywhere: with 4, each SM sub-partition
-                                                                 // runs ONE epilogue warp -- every dependent instruction pays
-                                                                 // its full latency (~4 k cycles per 128x128 tile, measured)
-
 template <int BLOCK_N, bool LN, int ACT, bool F16, int MODE = 0>
-__global__ void __launch_bounds__(KCfg<BLOCK_N, LN, ACT, MODE>::type::kThreads, KCfg<BLOCK_N, LN, ACT, MODE>::type::kMinBlocks)
+__global__ void __launch_bounds__(PCfg<BLOCK_N, LN, MODE>::kThreads, PCfg<BLOCK_N, LN, MODE>::kMinBlocks)
 gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                        const __grid_constant__ CUtensorMap tmap_c, const GemmEpilogue p, const int num_m_tiles,
                        const int num_n_tiles) {
-    using Cfg = typename KCfg<BLOCK_N, LN, ACT, MODE>::type;
+    using Cfg = PCfg<BLOCK_N, LN, MODE>;
     constexpr int kStages = Cfg::kStages;
     constexpr int kNC = Cfg::kNumChunks;
     constexpr int kEpiThreads = Cfg::kEpiThreads;
@@ -435,23 +403,21 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
         __trap();
     }
     uint8_t* ring = smem_raw;
-    float* s_bias = reinterpret_cast<float*>(ring + kStages * Cfg::kStageBytes);   // [BLOCK_N] (LN: [2][BLOCK_N], 2nd half unused)
+    float* s_acc = reinterpret_cast<float*>(ring + kStages * Cfg::kStageBytes);    // [128][kAccLd] deposited accumulator
+    float* s_bias = s_acc + kBlockM * Cfg::kAccLd;                                  // [BLOCK_N] (LN: [2][BLOCK_N], 2nd half unused)
     float* s_gamma = s_bias + Cfg::kBiasFloats;                                     // LN only (zero-sized otherwise)
     float* s_beta = s_gamma + (LN ? BLOCK_N : 0);
     float2* s_part = reinterpret_cast<float2*>(s_beta + (LN ? BLOCK_N : 0));        // [2 bufs][2 halves][128] (mean, M2)
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(s_part + (LN ? 4 * kBlockM : 0));
     uint64_t* empty_bar = full_bar + kStages;
-    uint64_t* tmem_full_bar = empty_bar + kStages;     // [2]
-    uint64_t* tmem_empty_bar = tmem_full_bar + 2;      // [2]
-    uint64_t* ln_bar = tmem_empty_bar + 2;             // [2] cluster exchange, alternating per tile so that arrivals
+    uint64_t* ln_bar = empty_bar + kStages;             // [2] cluster exchange, alternating per tile so that arrivals
                                                        //     for tile i+1 can never be counted into tile i's phase
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(ln_bar + 2);
-    uint8_t* s_xpose = reinterpret_cast<uint8_t*>(tmem_ptr_smem + 4);               // [kEpiWarps][kXposeBytesPerWarp]
+    uint8_t* s_xpose = reinterpret_cast<uint8_t*>(ln_bar + 2) + 16;               // [kEpiWarps][kXposeBytesPerWarp]
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
     const int num_kb = (p.K + kBlockK - 1) / kBlockK;
-    // profiling stamps (first tile of each CTA): 0 entry, 1 setup done, 2 first k-block landed, 3 last MMA issued,
+    // profiling stamps (first tile of each CTA): 0 entry, 1 setup done, 2 first k-block landed, 3 last k-block accumulated,
     // 4 accumulator ready, 5 accumulator read + local statistics done, 6 LayerNorm exchange done, 7 epilogue done
     long long* stamps = p.timing ? p.timing + 16 * (static_cast<size_t>(blockIdx.y) * gridDim.x + blockIdx.x) : nullptr;
     if (stamps && threadIdx.x == 0) {
@@ -467,11 +433,19 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
     // ---- tile assignment.  Non-LN: CTA b takes tiles b, b+grid, ... with the N index fastest (CTAs that run together
     // share an A row-panel in L2).  LN: gridDim.x = cluster size = num_n_tiles, blockIdx.y = cluster id; cluster c takes
     // M tiles c, c + gridDim.y, ... and the CTA's rank in the cluster is its (fixed) N tile.
-    const int total_tiles = LN ? num_m_tiles : num_m_tiles * num_n_tiles;
-    const int first_tile = LN ? static_cast<int>(blockIdx.y) : static_cast<int>(blockIdx.x);
-    const int tile_stride = LN ? static_cast<int>(gridDim.y) : static_cast<int>(gridDim.x);
-    const uint32_t cluster_size = LN ? cluster_nctarank() : 1u;
-    const uint32_t my_rank = LN ? cluster_ctarank() : 0u;
+    // PAIR: cluster c = blockIdx.x / 2 walks pair tiles c, c + grid / 2, ... (256-row panel, N index fastest); rank r of the
+    // cluster takes the 128 rows 256 * panel + 128 r (a last odd panel leaves rank 1 all rows >= M: it still loads and
+    // multicasts its half of W, and its zero-filled rows are never stored).
+    constexpr bool PAIR = Cfg::PAIR;
+    const int total_tiles = LN ? num_m_tiles : (PAIR ? (num_m_tiles + 1) / 2 : num_m_tiles) * num_n_tiles;
+    const int first_tile = LN ? static_cast<int>(blockIdx.y) : static_cast<int>(PAIR ? blockIdx.x >> 1 : blockIdx.x);
+    const int tile_stride = LN ? static_cast<int>(gridDim.y) : static_cast<int>(PAIR ? gridDim.x >> 1 : gridDim.x);
+    const uint32_t cluster_size = (LN || PAIR) ? cluster_nctarank() : 1u;
+    const uint32_t my_rank = (LN || PAIR) ? cluster_ctarank() : 0u;
+    auto tile_m0 = [&](int tile) {
+        return (LN ? tile : (PAIR ? 2 * (tile / num_n_tiles) + static_cast<int>(my_rank) : tile / num_n_tiles)) * kBlockM;
+    };
+    auto tile_n0 = [&](int tile) { return (LN ? static_cast<int>(my_rank) : tile % num_n_tiles) * BLOCK_N; };
 
     // ---------------------------------------------------------------- one-time setup
     // The producer thread does not wait for the CTA-wide setup barrier: as soon as ITS barriers exist it puts the first ring
@@ -480,17 +454,15 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
     // activation tiles then follow after griddepcontrol.wait.
     int early = 0;                 // k-blocks of the first tile already (partly) in flight     } producer thread only
     bool early_a = false;          // ... including their activation tiles                       }
-    if (warp == 0 && lane == 0) {
+    if (warp == Cfg::kProducerWarp && lane == 0) {
         tma_prefetch_desc(&tmap_a);
         tma_prefetch_desc(&tmap_b);
         if (!LN && p.tma_store) tma_prefetch_desc(&tmap_c);
         for (int s = 0; s < kStages; ++s) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], 1);
+            mbar_init(&empty_bar[s], (PAIR ? 2 : 1) * Cfg::kConsumerWarps);   // one arrival per consumer warp (PAIR: of both CTAs)
         }
         for (int a = 0; a < 2; ++a) {
-            mbar_init(&tmem_full_bar[a], 1);
-            mbar_init(&tmem_empty_bar[a], kEpiThreads);
             mbar_init(&ln_bar[a], LN ? cluster_size : 1u);                   // one arrival per CTA of the cluster
         }
         mbar_fence_init();
@@ -499,7 +471,7 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
 #else
         constexpr bool early_ok = true;
 #endif
-        if (!LN && first_tile < total_tiles && p.pdl != 1 && early_ok) {
+        if (!LN && !PAIR && first_tile < total_tiles && p.pdl != 1 && early_ok) {
             early_a = p.pdl != 5;
             const int m0 = (first_tile / num_n_tiles) * kBlockM, n0 = (first_tile % num_n_tiles) * BLOCK_N;
             early = min(kStages, num_kb);
@@ -510,27 +482,23 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
                 tma_load_2d(sa + Cfg::kStageBytesA, &tmap_b, &full_bar[i], i * kBlockK, n0);
             }
         }
-    } else if (warp == 1) {
-        tmem_alloc<Cfg::kTmemCols>(tmem_ptr_smem);
-    } else if (LN && warp >= 2) {
+    } else if (LN && warp < Cfg::kConsumerWarps) {
         const int n0 = static_cast<int>(my_rank) * BLOCK_N;
-        for (int i = threadIdx.x - 64; i < BLOCK_N; i += kEpiThreads) {
+        for (int i = threadIdx.x; i < BLOCK_N; i += kEpiThreads) {
             s_bias[i] = p.bias ? p.bias[n0 + i] : 0.0f;
             s_gamma[i] = p.gamma[n0 + i];
             s_beta[i] = p.beta[n0 + i];
         }
     }
-    tc_fence_before();
-    if (LN) cluster_sync_all(); else __syncthreads();   // LN: peers' barriers must be initialised before remote arrives
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_smem;
+    if (LN || PAIR) cluster_sync_all(); else __syncthreads();   // peers' barriers must be initialised before remote arrives / multicasts
     if (stamps && threadIdx.x == 0) stamps[1] = clock64();
 
     // Programmatic dependent launch: everything above overlapped the previous kernel's tail; its outputs are visible after the
     // wait.  (The producer thread of a pdl == 5 kernel waits inside its own branch, right before the first activation tile.)
-    if (p.pdl && !(p.pdl == 5 && !LN && threadIdx.x == 0)) pdl_wait();
+    const bool producer_thread = warp == Cfg::kProducerWarp && lane == 0;
+    if (p.pdl && !(p.pdl == 5 && !LN && producer_thread)) pdl_wait();
 
-    if (warp == 0) {
+    if (warp == Cfg::kProducerWarp) {
         // ============================================================ TMA producer
         if (lane == 0) {
             int s = 0;
@@ -540,8 +508,7 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
             if (stamps && !LN) stamps[6] = clock64();                  // producer past griddepcontrol.wait (non-LN kernels: slot 6 is free)
 #endif
             for (int tile = first_tile; tile < total_tiles; tile += tile_stride) {
-                const int m0 = (LN ? tile : tile / num_n_tiles) * kBlockM;
-                const int n0 = (LN ? static_cast<int>(my_rank) : tile % num_n_tiles) * BLOCK_N;
+                const int m0 = tile_m0(tile), n0 = tile_n0(tile);
                 for (int kb = 0; kb < num_kb; ++kb) {
                     uint8_t* sa = ring + s * Cfg::kStageBytes;
                     uint8_t* sb = sa + Cfg::kStageBytesA;
@@ -549,7 +516,7 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
                         --early;
                         if (!early_a) tma_load_2d(sa, &tmap_a, &full_bar[s], kb * kBlockK, m0);
                     } else {
-                        mbar_wait(&empty_bar[s], phase ^ 1u);
+                        mbar_wait_nocall(&empty_bar[s], phase ^ 1u);
 #ifdef VB200_DECOMPOSE
                         if (p.debug & 4) {
                             mbar_arrive(&full_bar[s]);                 // timing decomposition: MMAs on stale shared memory
@@ -558,100 +525,93 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
                         {
                             mbar_arrive_expect_tx(&full_bar[s], Cfg::kStageBytes);
                             tma_load_2d(sa, &tmap_a, &full_bar[s], kb * kBlockK, m0);
-                            tma_load_2d(sb, &tmap_b, &full_bar[s], kb * kBlockK, n0);
+                            if constexpr (PAIR) {      // my half of the weight rows, into the same offset of both CTAs
+                                constexpr int kHalf = BLOCK_N / 2;
+                                tma_load_2d_mcast(sb + my_rank * kHalf * 128, &tmap_b, &full_bar[s], kb * kBlockK,
+                                                  n0 + static_cast<int>(my_rank) * kHalf, 0x3);
+                            } else {
+                                tma_load_2d(sb, &tmap_b, &full_bar[s], kb * kBlockK, n0);
+                            }
                         }
                     }
                     if (++s == kStages) { s = 0; phase ^= 1u; }
                 }
             }
-        }
-        __syncwarp();
-    } else if (warp == 1) {
-        // ============================================================ MMA issuer
-        // This thread's serial loop (wait -> fence -> 4 x tcgen05.mma -> commit) is what paces a lone CTA: ~335 cycles per k-block
-        // with neither loads nor MMAs in it, ~530 with (profiles/r2_gemm_decomposition.md) -- every instruction here is on the
-        // critical path, so descriptors advance by adds and nothing optional lives inside the k loop.  (A converged warp with
-        // one elected issuing lane instead of lane 0 in a divergent branch measured 1-3 % -- not worth the extra syncs.)
-        if (lane == 0) {
-            constexpr uint32_t idesc = umma_idesc_f32acc(kBlockM, BLOCK_N, F16);
-            constexpr uint64_t kDescStage = static_cast<uint64_t>(Cfg::kStageBytes >> 4);       // descriptor address units (16 B)
-            const uint64_t da0 = umma_desc_kmajor_sw128(ring);
-            const uint64_t db0 = umma_desc_kmajor_sw128(ring + Cfg::kStageBytesA);
-            int s = 0;
-            uint32_t phase = 0;
-            uint32_t it = 0;
-            for (int tile = first_tile; tile < total_tiles; tile += tile_stride, ++it) {
-                const uint32_t acc = Cfg::kAccBufs == 2 ? (it & 1u) : 0u;
-                const uint32_t acc_phase = Cfg::kAccBufs == 2 ? ((it >> 1) & 1u) : (it & 1u);
-                mbar_wait(&tmem_empty_bar[acc], acc_phase ^ 1u);      // epilogue has drained this accumulator
-                tc_fence_after();
-                const uint32_t tmem_d = tmem_base + acc * BLOCK_N;
-                uint32_t accumulate = 0u;
-                for (int kb = 0; kb < num_kb; ++kb) {
-                    mbar_wait(&full_bar[s], phase);
-                    tc_fence_after();
-#ifdef VB200_STAMPS
-                    if (stamps && it == 0 && kb == 0) stamps[2] = clock64();
-#endif
-                    const uint64_t da = da0 + kDescStage * static_cast<uint64_t>(s);
-                    const uint64_t db = db0 + kDescStage * static_cast<uint64_t>(s);
-#ifdef VB200_DECOMPOSE
-                    if (!(p.debug & 1))
-#endif
-                    {
-#pragma unroll
-                        for (int k = 0; k < kBlockK / kUmmaK; ++k) {
-                            umma_bf16_ss(tmem_d, da + 2u * k, db + 2u * k, idesc, accumulate);
-                            accumulate = 1u;
-                        }
-                    }
-                    umma_commit(&empty_bar[s]);
-                    if (++s == kStages) { s = 0; phase ^= 1u; }
-                }
-                umma_commit(&tmem_full_bar[acc]);
-#ifdef VB200_STAMPS
-                if (stamps && it == 0) stamps[3] = clock64();
-#endif
-            }
-#ifdef VB200_STAMPS
-            if (stamps) { stamps[10] = clock64(); stamps[11] = it; }     // steady state: (s10 - s2) / (tiles * k-blocks)
-#endif
-            // This CTA's tensor work is issued: let the next kernel's CTAs come up while the epilogue drains (their
-            // griddepcontrol.wait still holds them until this whole grid has finished).  Triggering at kernel entry instead made
-            // the dependents sit on the second CTA slot of every SM for the whole main loop (measured: step 6 % slower).
-            if (p.pdl) pdl_launch_dependents();
         }
         __syncwarp();
     } else {
-        // ============================================================ epilogue warps
-        const int ew = warp - 2;                      // 0..kEpiWarps-1
-        const int q = warp & 3;                       // TMEM lane quarter this warp may read
+        // ============================================================ consumer warpgroups: MMA, then epilogue
+        // One k-block's wgmma group stays in flight while the stage of the previous one is handed back to the producer.
+        constexpr uint64_t kDescStage = static_cast<uint64_t>(Cfg::kStageBytes >> 4);       // descriptor address units (16 B)
+        const int wg = warp >> 2;
+        const uint64_t da0 = gmma_desc_kmajor_sw128(smem_u32(ring + wg * 64 * 128));         // this warpgroup's 64 rows of A
+        const uint64_t db0 = gmma_desc_kmajor_sw128(smem_u32(ring + Cfg::kStageBytesA));
+        int ks = 0;
+        uint32_t kphase = 0;
+        // a stage is free once this warp's wgmma have read it; PAIR: the peer's producer writes half of it too, so both CTAs' barriers
+        auto release = [&](int st) __attribute__((always_inline)) {
+            if (lane != 0) return;
+            if constexpr (PAIR) {
+                mbar_arrive_remote_release(mapa_u32(&empty_bar[st], 0));
+                mbar_arrive_remote_release(mapa_u32(&empty_bar[st], 1));
+            } else {
+                mbar_arrive(&empty_bar[st]);
+            }
+        };
+        // accumulate tile `tile` and deposit it in s_acc; returns once all 128 rows are there
+        auto mma_tile = [&](int tile, uint32_t it) __attribute__((always_inline)) {
+            float d[BLOCK_N / 2];
+            int prev = -1;
+            for (int kb = 0; kb < num_kb; ++kb) {
+                mbar_wait_nocall(&full_bar[ks], kphase);
+#ifdef VB200_STAMPS
+                if (stamps && threadIdx.x == 0 && it == 0 && kb == 0) stamps[2] = clock64();
+#endif
+                const uint64_t da = da0 + kDescStage * static_cast<uint64_t>(ks);
+                const uint64_t db = db0 + kDescStage * static_cast<uint64_t>(ks);
+#ifdef VB200_DECOMPOSE
+                if (!(p.debug & 1))
+#endif
+                    mma_kblock<BLOCK_N, F16>(d, da, db, kb == 0);
+                if (prev >= 0) {
+                    wgmma_wait<1>();                                     // k-block kb - 1 has read its stage
+                    release(prev);
+                }
+                prev = ks;
+                if (++ks == kStages) { ks = 0; kphase ^= 1u; }
+            }
+            wgmma_wait<0>();
+            if (prev >= 0) release(prev);
+#ifdef VB200_STAMPS
+            if (stamps && threadIdx.x == 0 && it == 0) stamps[3] = clock64();
+#endif
+            // This CTA's tensor work is done: let the next kernel's CTAs come up while the epilogue drains (their
+            // griddepcontrol.wait still holds them until this whole grid has finished).
+            if (p.pdl && threadIdx.x == 0 && tile + tile_stride >= total_tiles) pdl_launch_dependents();
+            acc_deposit<BLOCK_N>(s_acc, d, threadIdx.x);
+            epi_bar_sync<kEpiThreads>();                                 // the whole tile is deposited
+        };
+        const int ew = warp;                          // 0..kEpiWarps-1
+        const int q = ew & 3;                         // row quarter of the tile this warp owns
         const int half = LN ? (ew >> 2) : 0;          // LN: column half of the tile
         const int row = q * 32 + lane;
-        const int et = threadIdx.x - 64;
+        const int et = threadIdx.x;
         const bool st_fast = (p.out_bf16 == nullptr || (p.ld_bf16 & 7) == 0) && (p.out_f32 == nullptr || (p.ld_f32 & 3) == 0);
         uint32_t it = 0;
         for (int tile = first_tile; tile < total_tiles; tile += tile_stride, ++it) {
-            const uint32_t acc = Cfg::kAccBufs == 2 ? (it & 1u) : 0u;
-            const uint32_t acc_phase = Cfg::kAccBufs == 2 ? ((it >> 1) & 1u) : (it & 1u);
-            const int m0 = (LN ? tile : tile / num_n_tiles) * kBlockM;
-            const int n0 = (LN ? static_cast<int>(my_rank) : tile % num_n_tiles) * BLOCK_N;
+            const int m0 = tile_m0(tile), n0 = tile_n0(tile);
             const int m = m0 + row;
             const bool m_ok = m < p.M;
-            const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * BLOCK_N;
+            const float* acc_row = s_acc + row * Cfg::kAccLd;
             const bool stamp = stamps && it == 0 && et == 0;
 
             if constexpr (!LN) {
-                // ------------------------------------------------ plain epilogue: 4 warps, chunk-pipelined
+                // ------------------------------------------------ plain epilogue: 8 warps, one 32-column chunk at a time
                 const float* bias_t = s_bias;
-                if constexpr (Cfg::kBiasInSmem) {
-                    // per-tile bias slice; the barrier below orders it before the reads, the one at the end of the tile orders
-                    // the reads before the next tile's writes
-                    for (int i = et; i < BLOCK_N; i += kEpiThreads) s_bias[i] = (p.bias && n0 + i < p.N) ? p.bias[n0 + i] : 0.0f;
-                    epi_bar_sync<kEpiThreads>();
-                } else {
-                    bias_t = p.bias + n0;                  // WIDE2 / 256: straight from global / L1 (host guarantees bias != null, N % 256 == 0)
-                }
+                // per-tile bias slice; the barrier below orders it before the reads, the one at the end of the tile orders
+                // the reads before the next tile's writes
+                for (int i = et; i < BLOCK_N; i += kEpiThreads) s_bias[i] = (p.bias && n0 + i < p.N) ? p.bias[n0 + i] : 0.0f;
+                epi_bar_sync<kEpiThreads>();
                 // LayerNorm fold: this row's statistics, computed while the main loop runs (the epilogue warps are idle until the
                 // accumulator is ready).  a_*: pending LayerNorm of the A operand (MODE 4); r_*: of the residual (MODE 5).
                 float a_mean = 0.0f, a_rstd = 1.0f, r_mean = 0.0f, r_rstd = 1.0f;
@@ -662,12 +622,11 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
                     if (m_ok && p.res_stats != nullptr)
                         row_stats(p.res_stats, p.res_parts, p.stats_ld, m, static_cast<float>(p.res_parts * 32), p.eps, r_mean, r_rstd);
                 }
-                mbar_wait(&tmem_full_bar[acc], acc_phase);
-                tc_fence_after();
+                mma_tile(tile, it);
                 if (stamp) stamps[4] = clock64();
                 float* const out_f32 = p.out_f32;
                 // TMA-store path (CTA-uniform): this is the CTA's last tile, so no operand load is or will be in flight and
-                // every MMA that read the ring has completed (tmem_full above)
+                // every MMA that read the ring has completed (mma_tile above)
                 constexpr bool kF32SlabsFit = (BLOCK_N / 32) * (kBlockM * 128) <= kStages * Cfg::kStageBytes;
                 const bool use_tma = p.tma_store != 0 && st_fast && tile + tile_stride >= total_tiles &&
                                      (p.tma_store == 1 || kF32SlabsFit) &&
@@ -785,44 +744,16 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
                         store_chunk<F16>(ps, m, nc, false, v);
                     }
                 };
-                if constexpr (Cfg::TRI) {
-                    // four warps, one per TMEM lane quarter, all kNC chunks each; software-pipelined: the load of chunk c + 1 is in
-                    // flight while chunk c is finished (two chunks in registers -- the 112-register budget of this mode allows it)
-                    static_assert(kNC % 2 == 0, "pipelined in pairs");
-                    float va[32], vb[32];
-                    tmem_ld32_issue(taddr, va);
-#pragma unroll
-                    for (int c = 0; c < kNC; c += 2) {
-                        tmem_ld_wait_for(va);
-                        tmem_ld32_issue(taddr + (c + 1) * 32, vb);
-                        if (stamp && c == 0) stamps[14] = clock64();
-                        finish_chunk(va, n0 + c * 32);
-                        if (stamp && c == 0) stamps[15] = clock64();
-                        tmem_ld_wait_for(vb);
-                        if (c + 2 < kNC) {
-                            tmem_ld32_issue(taddr + (c + 2) * 32, va);
-                        } else {
-                            tc_fence_before();
-                            mbar_arrive(&tmem_empty_bar[acc]);         // the accumulator is in registers: the next tile's MMAs may start
-                        }
-                        finish_chunk(vb, n0 + (c + 1) * 32);
-                    }
-                } else {
-                    // eight warps: column group g = ew / 4 takes chunks [g * kNC/2, (g+1) * kNC/2); thread-level parallelism
-                    // hides the TMEM latency, one chunk in registers at a time keeps two CTAs per SM within 102 registers
+                {
+                    // eight warps: column group g = ew / 4 takes chunks [g * kNC/2, (g+1) * kNC/2)
                     constexpr int kCPG = kNC / 2;
                     const int g = ew >> 2;
 #pragma unroll
                     for (int ci = 0; ci < kCPG; ++ci) {
                         const int c = g * kCPG + ci;
                         float v[32];
-                        tmem_ld32_issue(taddr + c * 32, v);
-                        tmem_ld_wait();
+                        acc_ld32(acc_row + c * 32, v);
                         if (stamp && ci == 0) stamps[14] = clock64();         // first chunk in registers
-                        if (ci + 1 == kCPG) {
-                            tc_fence_before();
-                            mbar_arrive(&tmem_empty_bar[acc]);
-                        }
                         finish_chunk(v, n0 + c * 32);
                         if (stamp && ci == 0) stamps[15] = clock64();         // first chunk stored
                     }
@@ -842,7 +773,7 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
                     }
                 }
                 if (stamp) { stamps[5] = clock64(); stamps[7] = clock64(); }
-                if (Cfg::kBiasInSmem && tile + tile_stride < total_tiles) epi_bar_sync<kEpiThreads>();   // bias slice free for the next tile
+                if (tile + tile_stride < total_tiles) epi_bar_sync<kEpiThreads>();   // bias slice and s_acc free for the next tile
             } else {
                 // ------------------------------------------------ LayerNorm epilogue: 8 warps, row slice in registers
                 constexpr int kCPT = Cfg::kCPT;
@@ -853,15 +784,11 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
                 float x[kCPT][32];
                 float4 rcur[8];
                 if (has_res) res_load(p, m, n0 + c_begin * 32, true, rcur);       // in flight while the MMAs run
-                mbar_wait(&tmem_full_bar[acc], acc_phase);
-                tc_fence_after();
+                mma_tile(tile, it);
                 if (stamp) stamps[4] = clock64();
 #pragma unroll
                 for (int i = 0; i < kCPT; ++i)
-                    if (c_begin + i < c_end) tmem_ld32_issue(taddr + (c_begin + i) * 32, x[i]);
-                tmem_ld_wait();
-                tc_fence_before();
-                mbar_arrive(&tmem_empty_bar[acc]);                                // TMEM read once; hand the accumulator back
+                    if (c_begin + i < c_end) acc_ld32(acc_row + (c_begin + i) * 32, x[i]);   // the partials barrier below frees s_acc
                 float lsum = 0.0f;
 #pragma unroll
                 for (int i = 0; i < kCPT; ++i) {
@@ -897,25 +824,26 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
                 mbar_wait_acquire_cluster(lb, (it >> 1) & 1u);                    // every CTA's partials for this tile are visible
                 constexpr float kColsH0 = static_cast<float>(kCPT * 32);          // columns of half 0
                 constexpr float kColsH1 = static_cast<float>(BLOCK_N - kCPT * 32);  // columns of half 1
-                float2 pr0[8], pr1[8];
-#pragma unroll
-                for (uint32_t rk = 0; rk < 8; ++rk) {
-                    if (rk < cluster_size) {
-                        pr0[rk] = dsmem_ld_f32x2(mapa_u32(&part[row], rk));
-                        pr1[rk] = dsmem_ld_f32x2(mapa_u32(&part[kBlockM + row], rk));
-                    }
-                }
+                // two passes over the peers' partials (the second re-reads them) keep the register budget independent of the
+                // cluster size; the summation order is fixed, so the result does not depend on timing
                 float tot = 0.0f;
 #pragma unroll
-                for (uint32_t rk = 0; rk < 8; ++rk)
-                    if (rk < cluster_size) tot += pr0[rk].x * kColsH0 + pr1[rk].x * kColsH1;
+                for (uint32_t rk = 0; rk < kMaxCluster; ++rk) {
+                    if (rk < cluster_size) {
+                        const float2 a0 = dsmem_ld_f32x2(mapa_u32(&part[row], rk));
+                        const float2 a1 = dsmem_ld_f32x2(mapa_u32(&part[kBlockM + row], rk));
+                        tot += a0.x * kColsH0 + a1.x * kColsH1;
+                    }
+                }
                 const float mean = tot / static_cast<float>(p.N);
                 float M2 = 0.0f;
 #pragma unroll
-                for (uint32_t rk = 0; rk < 8; ++rk) {
+                for (uint32_t rk = 0; rk < kMaxCluster; ++rk) {
                     if (rk < cluster_size) {
-                        const float d0 = pr0[rk].x - mean, d1 = pr1[rk].x - mean;
-                        M2 += pr0[rk].y + kColsH0 * d0 * d0 + pr1[rk].y + kColsH1 * d1 * d1;
+                        const float2 a0 = dsmem_ld_f32x2(mapa_u32(&part[row], rk));
+                        const float2 a1 = dsmem_ld_f32x2(mapa_u32(&part[kBlockM + row], rk));
+                        const float d0 = a0.x - mean, d1 = a1.x - mean;
+                        M2 += a0.y + kColsH0 * d0 * d0 + a1.y + kColsH1 * d1 * d1;
                     }
                 }
                 const float rstd = 1.0f / sqrtf(M2 / static_cast<float>(p.N) + p.eps);
@@ -943,12 +871,8 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
     }
 
     // ---------------------------------------------------------------- teardown
-    tc_fence_before();
-    if (LN) cluster_sync_all(); else __syncthreads();     // LN: nobody exits while a peer may still read its partials
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc<Cfg::kTmemCols>(tmem_base);
-    }
+    // nobody exits while a peer may still read its partials (LN) or multicast into / arrive on its shared memory (PAIR)
+    if (LN || PAIR) cluster_sync_all(); else __syncthreads();
     if (stamps && threadIdx.x == 0) {
         unsigned long long gt;
         asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt));
@@ -965,7 +889,7 @@ inline int num_sms() {
         int dev = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        if (n <= 0) n = 148;
+        if (n <= 0) n = 132;
     }
     return n;
 }
@@ -978,7 +902,7 @@ void fill_cfg(cudaLaunchConfig_t& cfg, cudaLaunchAttribute* attrs, dim3 grid, in
     cfg.dynamicSmemBytes = Cfg::kSmemBytes;
     cfg.stream = st;
     unsigned na = 0;
-    if (LN) {
+    if (LN || cluster > 1) {
         attrs[na].id = cudaLaunchAttributeClusterDimension;
         attrs[na].val.clusterDim.x = cluster;
         attrs[na].val.clusterDim.y = 1;
@@ -997,9 +921,10 @@ void fill_cfg(cudaLaunchConfig_t& cfg, cudaLaunchAttribute* attrs, dim3 grid, in
 // resident: LN only -- how many clusters of this size can be co-resident (grid.y is capped to it)
 template <int BLOCK_N, bool LN, int ACT, bool F16, int MODE = 0>
 cudaError_t launch_p(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilogue& ep, int resident, cudaStream_t st) {
-    using Cfg = typename KCfg<BLOCK_N, LN, ACT, MODE>::type;
+    using Cfg = PCfg<BLOCK_N, LN, MODE>;
     auto kern = gemm_persistent_kernel<BLOCK_N, LN, ACT, F16, MODE>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
+    if (e == cudaSuccess && LN) e = cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
     if (e != cudaSuccess) return e;
     const int n_tiles = (ep.N + BLOCK_N - 1) / BLOCK_N;
     const int m_tiles = (ep.M + kBlockM - 1) / kBlockM;
@@ -1010,32 +935,26 @@ cudaError_t launch_p(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpi
         if (resident <= 0) return cudaErrorInvalidConfiguration;
         grid = dim3(cluster, std::min(m_tiles, resident), 1);
     } else {
-        // Persistent grid: two thirds of the resident CTA slots (197 of 296), not all of them.  A GEMM with more tiles than that
-        // (QKV, FFN-in at batch 64) then has CTAs that walk two tiles -- epilogue of tile i under the MMAs of tile i+1 -- and leaves
-        // slots to whichever kernel of the other ViLBERT stream / the other in-flight batch is runnable, which de-synchronises the two
-        // CTAs of an SM (two CTAs of ONE kernel run in lock-step: same prologue, same epilogue, tensor pipe idle in both).
-        // Measured, two batches in flight, 200-step runs: 100 % 40.5-40.9 k pairs/s | 85 % 40.9-41.0 | 75 % 41.5-41.8 | 67 % 41.7-41.9 |
-        // 60 % 41.3 | 50 % 41.6-41.8; timed alone a launch is ~8 % slower (profiles/r2_grid_size.md).  VB200_GRID_PCT overrides.
-        static const int env_pct = [] { const char* e = getenv("VB200_GRID_PCT"); const int v = e ? atoi(e) : 67; return (v >= 10 && v <= 100) ? v : 67; }();
-        static const bool env_set = getenv("VB200_GRID_PCT") != nullptr;
-        const int tiles = m_tiles * n_tiles;
-        // From two full waves up (batch >= ~256) every CTA owns several tiles anyway and the full grid wins: batch 512, 45.3 k pairs/s
-        // at 67 %, 45.9 k at 100 % (profiles/r2_b512.md).
-        const int auto_pct = (!env_set && tiles >= 2 * num_sms() * Cfg::kMinBlocks) ? 100 : env_pct;
-        const int pct = (ep.grid_pct >= 10 && ep.grid_pct <= 100) ? ep.grid_pct : auto_pct;     // per-launch override (profiling: timed alone)
-        const int slots = std::max(1, num_sms() * Cfg::kMinBlocks * pct / 100);
-        // balanced walk: every CTA gets the same number of tiles (+-1): tiles = 288, cap 197 -> 144 CTAs x 2 instead of 91 x 2 + 106 x 1
+        // Persistent grid: every SM (one CTA each) by default.  VB200_GRID_PCT caps it at that percentage of the SMs, leaving room
+        // for kernels of the other ViLBERT stream / the other in-flight batch.
+        static const int env_pct = [] { const char* e = getenv("VB200_GRID_PCT"); const int v = e ? atoi(e) : 100; return (v >= 10 && v <= 100) ? v : 100; }();
+        // PAIR: counted in clusters of two CTAs and pair tiles of 256 rows
+        if (Cfg::PAIR) cluster = 2;
+        const int tiles = (Cfg::PAIR ? (m_tiles + 1) / 2 : m_tiles) * n_tiles;
+        const int pct = (ep.grid_pct >= 10 && ep.grid_pct <= 100) ? ep.grid_pct : env_pct;     // per-launch override (profiling: timed alone)
+        const int slots = std::max(1, num_sms() * Cfg::kMinBlocks * pct / 100 / cluster);
+        // balanced walk: every CTA gets the same number of tiles (+-1): tiles = 288, cap 132 -> 96 CTAs x 3 instead of 24 x 3 + 108 x 2
         static const bool balance = [] { const char* e = getenv("VB200_GRID_BALANCE"); return e == nullptr || atoi(e) != 0; }();
         int g = std::min(tiles, slots);
         if (balance && tiles > slots) { const int per = (tiles + slots - 1) / slots; g = (tiles + per - 1) / per; }
-        grid = dim3(g, 1, 1);
+        grid = dim3(g * cluster, 1, 1);
     }
     cudaLaunchConfig_t cfg;
     cudaLaunchAttribute attrs[2];
     fill_cfg<Cfg, LN>(cfg, attrs, grid, cluster, ep.pdl == 1 || ep.pdl == 5, st);
     GemmEpilogue e2 = ep;
     const CUtensorMap* tc = static_cast<const CUtensorMap*>(ep.tmap_c_host);
-    if (tc == nullptr || LN) { e2.tma_store = 0; tc = &ta; }          // &ta: any valid map for the unused slot
+    if (tc == nullptr || LN || Cfg::PAIR) { e2.tma_store = 0; tc = &ta; }          // &ta: any valid map for the unused slot
     return cudaLaunchKernelEx(&cfg, kern, ta, tb, *tc, e2, m_tiles, n_tiles);
 }
 

@@ -1,4 +1,4 @@
-// LayerNorm-fused (cluster) instantiations of the persistent tcgen05 GEMM; see gemm_persistent.cuh.
+// LayerNorm-fused (cluster) instantiations of the persistent wgmma GEMM; see gemm_persistent.cuh.
 #include <cstdlib>
 #include "gemm_persistent.cuh"
 
@@ -9,12 +9,13 @@ using namespace pgemm;
 template <int BLOCK_N>
 static int max_clusters(int cluster) {
     using Cfg = PCfg<BLOCK_N, true>;
-    static int cache[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};   // 0 unknown, -1 unsupported
-    if (cluster < 1 || cluster > 8) return 0;
+    static int cache[kMaxCluster + 1] = {};   // 0 unknown, -1 unsupported
+    if (cluster < 1 || cluster > kMaxCluster) return 0;
     if (cache[cluster] != 0) return cache[cluster] < 0 ? 0 : cache[cluster];
     auto kern = gemm_persistent_kernel<BLOCK_N, true, kActNone, true>;
     int n = 0;
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes) == cudaSuccess) {
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes) == cudaSuccess &&
+        cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess) {
         cudaLaunchConfig_t cfg;
         cudaLaunchAttribute attrs[2];
         fill_cfg<Cfg, true>(cfg, attrs, dim3(cluster, 1, 1), cluster, 0, nullptr);
@@ -25,13 +26,13 @@ static int max_clusters(int cluster) {
     return n > 0 ? n : 0;
 }
 
+int num_sms_host() { return pgemm::num_sms(); }
+
 int gemm_p_max_clusters(int block_n, int cluster) {
     switch (block_n) {
         case 64: return max_clusters<64>(cluster);
         case 96: return max_clusters<96>(cluster);
         case 128: return max_clusters<128>(cluster);
-        case 192: return max_clusters<192>(cluster);
-        case 256: return max_clusters<256>(cluster);
     }
     return 0;
 }
@@ -39,15 +40,15 @@ int gemm_p_max_clusters(int block_n, int cluster) {
 int gemm_p_pick_block_n(int N, bool ln) {
     if (!ln) {
         static const int forced = [] { const char* e = getenv("VB200_BN"); return e ? atoi(e) : 0; }();   // A/B switch
-        if ((forced == 64 || forced == 128 || forced == 256) && N % forced == 0) return forced;
+        if ((forced == 64 || forced == 128) && N % forced == 0) return forced;
         return N <= 64 ? 64 : 128;
     }
     static const int first = [] { const char* e = getenv("VB200_LN_BN"); return e ? atoi(e) : 128; }();   // A/B: preferred width
-    const int cands[6] = {first, 128, 96, 192, 256, 64};
-    for (int ci = 0; ci < 6; ++ci) {
+    const int cands[4] = {first, 128, 96, 64};
+    for (int ci = 0; ci < 4; ++ci) {
         const int bn = cands[ci];
-        if (bn != 64 && bn != 96 && bn != 128 && bn != 192 && bn != 256) continue;
-        if (N % bn != 0 || N / bn > 8) continue;
+        if (bn != 64 && bn != 96 && bn != 128) continue;
+        if (N % bn != 0 || N / bn > kMaxCluster) continue;
         if (gemm_p_max_clusters(bn, N / bn) > 0) return bn;
     }
     return 0;
@@ -68,7 +69,7 @@ cudaError_t launch_gemm_persistent(const CUtensorMap& ta, const CUtensorMap& tb,
                                    bool ln, cudaStream_t st) {
     if (ep.M < 1 || ep.N < 1 || ep.K < 1) return cudaErrorInvalidValue;
     if (!ln) return launch_gemm_persistent_plain(ta, tb, ep, block_n, st);
-    if (ep.N % block_n != 0 || ep.N / block_n > 8 || ep.gamma == nullptr || ep.beta == nullptr ||
+    if (ep.N % block_n != 0 || ep.N / block_n > kMaxCluster || ep.gamma == nullptr || ep.beta == nullptr ||
         (ep.out_bf16 && (ep.ld_bf16 & 7)) || (ep.out_f32 && (ep.ld_f32 & 3)) || (ep.res && (ep.ld_res & 3)) ||
         ep.mul != nullptr || ep.a_f16 != ep.out_f16)
         return cudaErrorInvalidValue;
@@ -76,8 +77,6 @@ cudaError_t launch_gemm_persistent(const CUtensorMap& ta, const CUtensorMap& tb,
         case 64: return dispatch_ln<64>(ta, tb, ep, st);
         case 96: return dispatch_ln<96>(ta, tb, ep, st);
         case 128: return dispatch_ln<128>(ta, tb, ep, st);
-        case 192: return dispatch_ln<192>(ta, tb, ep, st);
-        case 256: return dispatch_ln<256>(ta, tb, ep, st);
     }
     return cudaErrorInvalidValue;
 }

@@ -1,4 +1,4 @@
-// Plain (bias / GELU / ReLU / pooled-product) instantiations of the persistent tcgen05 GEMM; see gemm_persistent.cuh.
+// Plain (bias / GELU / ReLU / pooled-product) instantiations of the persistent wgmma GEMM; see gemm_persistent.cuh.
 #include <cstdlib>
 #include "gemm_persistent.cuh"
 
@@ -43,14 +43,12 @@ static cudaError_t dispatch_fold(const CUtensorMap& ta, const CUtensorMap& tb, c
     return cudaErrorInvalidValue;
 }
 
-template <int BN>
-static cudaError_t dispatch_plain(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilogue& ep, cudaStream_t st) {
-    if constexpr (BN == 256) {
-        // 128x256 tiles at two CTAs per SM (PCfg MODE 2); experiment: VB200_WIDE2=1 (with VB200_BN=256 to select the tile width)
-        static const bool wide2 = getenv("VB200_WIDE2") != nullptr && atoi(getenv("VB200_WIDE2")) != 0;
-        if (wide2 && ep.N % 256 == 0 && ep.bias != nullptr) return dispatch_act<256, 2>(ta, tb, ep, st);
-    }
-    return dispatch_act<BN, 0>(ta, tb, ep, st);
+// CTA pair (PCfg MODE 8): 256 x 128 tiles per cluster of two, tmap_b box rows = 64 (each CTA loads and multicasts half of W)
+cudaError_t launch_gemm_pair(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilogue& ep, int block_n, cudaStream_t st) {
+    if (block_n != 128 || ep.M < 1 || ep.K < 1 || ep.N < 128 || (ep.N % 128) || ep.res != nullptr || ep.gamma != nullptr ||
+        ep.ln_mode != 0 || ep.split16 || ep.act == kActGeluExact || ep.a_f16 != ep.out_f16)
+        return cudaErrorInvalidValue;
+    return dispatch_act<128, 8>(ta, tb, ep, st);
 }
 
 cudaError_t launch_gemm_persistent_plain(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilogue& ep, int block_n,
@@ -73,17 +71,11 @@ cudaError_t launch_gemm_persistent_plain(const CUtensorMap& ta, const CUtensorMa
         return dispatch_fold<128>(ta, tb, ep, st);
     }
     switch (block_n) {
-        case 64:
-            if (ep.lone) return dispatch_act<64, 7>(ta, tb, ep, st);
-            return dispatch_plain<64>(ta, tb, ep, st);
-        case 128:
-            if (ep.tri) return dispatch_act<128, 6>(ta, tb, ep, st);        // three CTAs per SM (PCfg MODE 6)
-            if (ep.lone) return dispatch_act<128, 7>(ta, tb, ep, st);       // one CTA per SM, 6-stage ring (PCfg MODE 7)
-            return dispatch_plain<128>(ta, tb, ep, st);
-        case 192:                                    // 128x192 tiles, two CTAs per SM, 2-stage ring, one accumulator (PCfg MODE 2)
+        case 64: return dispatch_act<64, 0>(ta, tb, ep, st);
+        case 128: return dispatch_act<128, 0>(ta, tb, ep, st);
+        case 192:                                    // 128x192 tiles, 2-stage ring
             if (ep.N % 192 != 0) return cudaErrorInvalidValue;
-            return dispatch_act<192, 2>(ta, tb, ep, st);
-        case 256: return dispatch_plain<256>(ta, tb, ep, st);
+            return dispatch_act<192, 0>(ta, tb, ep, st);
     }
     return cudaErrorInvalidValue;
 }

@@ -1,4 +1,4 @@
-// Internal launch interface of the vilbert_b200 sm_100a kernels (not part of the C ABI; see include/vilbert_b200.h).
+// Internal launch interface of the vilbert_b200 sm_90a kernels (not part of the C ABI; see include/vilbert_b200.h).
 #pragma once
 #include "common.cuh"
 
@@ -6,7 +6,7 @@ namespace vb {
 
 enum Act : int { kActNone = 0, kActGelu = 1, kActRelu = 2, kActGeluExact = 3 };   // 3: erf to 1.5e-7 (fp32-parity mode)
 
-// Epilogue of the tcgen05 GEMM:  x = act(acc + bias + res) * mul ; LN variant: y = LayerNorm(x) * gamma + beta.
+// Epilogue of the wgmma GEMM:  x = act(acc + bias + res) * mul ; LN variant: y = LayerNorm(x) * gamma + beta.
 struct GemmEpilogue {
     int M, N, K;
     const float* bias;            // [N] or null
@@ -47,19 +47,18 @@ struct GemmEpilogue {
     int stats_ld;                 // row capacity of every stats array of this launch (>= M)
     int grid_pct;                 // 0: default persistent grid (2/3 of the CTA slots, launch_p); 10..100: this percentage of them
     int ln_mode;                  // 0 none, 4 fold-in (consumer), 5 pre-LayerNorm output + statistics (producer)
-    int tri;                      // plain 128-wide tile only: three CTAs per SM (gemm_persistent.cuh PCfg MODE 6)
-    int lone;                     // plain 128-wide tile only: one CTA per SM, 6-stage ring (PCfg MODE 7; small-batch latency)
     int debug;                    // timing decomposition only (VB200_DEBUG through vb200_linear): 1 = issue no MMA, 2 = no epilogue
                                   // stores, 4 = no operand loads (the ring is "filled" by plain arrives); results are garbage
-};                                //   every GEMM starts on HBM misses (weights never survive in the 126 MB L2 until the next step)
+};
 
-// v2: persistent CTAs / clusters, TMEM double-buffered accumulators, single-exchange LayerNorm (gemm_persistent.cu)
+// persistent CTAs / clusters, wgmma consumer warpgroups, single-exchange LayerNorm (gemm_persistent.cuh)
 int gemm_p_pick_block_n(int N, bool ln);
 int gemm_p_max_clusters(int block_n, int cluster);
 cudaError_t launch_gemm_persistent(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b, const GemmEpilogue& ep,
                                    int block_n, bool ln, cudaStream_t st);
-int num_sms_host();          // SM count of the current device (148 on B200)
-// CTA-pair kernel (gemm_pair.cu, tcgen05 cta_group::2, 256 x block_n tile per pair); tmap_b box rows = block_n / 2
+int num_sms_host();          // SM count of the current device (132 on H100 SXM)
+// CTA pair (gemm_persistent.cuh PCfg MODE 8: a cluster of two CTAs shares each weight tile through TMA multicast, 256 x 128 tile
+// per pair; plain epilogue, N % 128 == 0); tmap_b box rows = block_n / 2
 cudaError_t launch_gemm_pair(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b, const GemmEpilogue& ep, int block_n,
                              cudaStream_t stream);
 // Two dependent GEMMs (FFN-in -> FFN-out) in one persistent launch with a dynamic tile list (gemm_chain.cu); sync: (M tiles + 2) zeroed ints

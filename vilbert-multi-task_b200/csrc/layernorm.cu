@@ -1,12 +1,11 @@
 // Residual-add + LayerNorm row kernel: x = y + res; out = (x - mean) / sqrt(var + eps) * gamma + beta, written as the
 // fp32 residual stream AND the 16-bit operand of the next GEMM.
 //
-// This is the un-fused alternative to the cluster-LayerNorm GEMM epilogue (gemm_persistent_ln.cu).  Measured on B200 at
-// the batch-64 shapes (profiles/): the fused epilogue needs a cluster-wide exchange plus ~2000 dependent instructions per
-// thread on 8 warps (~17 k cycles per 128x128 tile), while a plain tcgen05 GEMM that writes fp32 followed by this
-// L2-resident row kernel (one warp per row, 16-byte coalesced accesses, two-pass fp32 statistics in registers) is
-// faster end to end.  Replaces BertSelfOutput / BertOutput / BertBiOutput `LayerNorm(dense(x) + residual)` and the
-// LayerNorm inside SimpleClassifier ([UPSTREAM] vilbert/vilbert.py; anchor /root/reference/worker.py:286-289).
+// This is the un-fused alternative to the cluster-LayerNorm GEMM epilogue (gemm_persistent_ln.cu): the fused epilogue needs a
+// cluster-wide exchange plus ~2000 dependent instructions per thread, while a plain GEMM that writes fp32 followed by this
+// L2-resident row kernel (one warp per row, 16-byte coalesced accesses, two-pass fp32 statistics in registers) keeps the GEMM
+// epilogue light.  Replaces BertSelfOutput / BertOutput / BertBiOutput `LayerNorm(dense(x) + residual)` and the
+// LayerNorm inside SimpleClassifier ([UPSTREAM] vilbert/vilbert.py; anchor worker.py:286-289).
 #include <cstdlib>
 #include "kernels.h"
 
@@ -112,7 +111,7 @@ cudaError_t launch_ln_residual(const float* y, int ld_y, const float* res, int l
     if (N % 128 != 0 || N / 128 > kLnMaxVec || (ld_y & 3) || (res && (ld_res & 3)) || (out_f32 && (ld_f32 & 3)) ||
         (out16 && (ld16 & 3)) || M < 1 || (split16 && !f16))
         return cudaErrorInvalidValue;
-    // one warp per row; 2 rows per CTA: 992 CTAs for 1984 rows spread 7:6 over the 148 SMs (8 rows per CTA: 248 CTAs, 2:1)
+    // one warp per row; 2 rows per CTA by default (VB200_LN_ROWS: 1..8)
     static const int rows_per_cta = [] { const char* e = getenv("VB200_LN_ROWS"); const int v = e ? atoi(e) : 2; return (v >= 1 && v <= 8) ? v : 2; }();
     const dim3 grid((M + rows_per_cta - 1) / rows_per_cta), block(32 * rows_per_cta);
     uint16_t* o16 = reinterpret_cast<uint16_t*>(out16);

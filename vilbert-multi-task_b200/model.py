@@ -7,9 +7,9 @@
     out10  = model(question, features, spatials, segment_ids, input_mask, image_mask,
                    co_attention_mask, task_tokens, output_all_attention_masks=True)  worker.py:286-289
 
-Everything between the input tensors and the ten outputs runs in libvilbert_b200.so (hand-written sm_100a
+Everything between the input tensors and the ten outputs runs in libvilbert_b200.so (hand-written sm_90a
 kernels).  torch is used only as the tensor container and for the CUDA stream.  No CPU path exists: calling
-the model without a B200 raises.
+the model without an H100 raises.
 """
 from __future__ import annotations
 
@@ -102,7 +102,7 @@ class VILBertForVLTasks(object):
     def to(self, device):
         device = torch.device(device)
         if device.type != "cuda":
-            raise L.VilbertB200Error("vilbert_b200 runs on sm_100 GPUs only; there is no CPU path")
+            raise L.VilbertB200Error("vilbert_b200 runs on sm_90 GPUs only; there is no CPU path")
         return self.cuda(device.index or 0)
 
     def half(self):            # tensor-core operands are 16-bit already (compute_dtype); accepted for call-site compatibility

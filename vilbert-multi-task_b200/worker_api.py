@@ -1,14 +1,14 @@
 """Task / prediction API of the reference worker, minus Django, RabbitMQ and the detector.
 
 Same call signatures, same validation, same per-task output dictionaries as
-/root/reference/worker.py:
+worker.py:
 
     custom_prediction(query, task, features, infos, task_id)                      worker.py:388-458
     prediction(question, features, spatials, segment_ids, input_mask, image_mask,
                co_attention_mask, task_tokens, task_id, infos)                    worker.py:248-386
     shape_result(task_id, answer, image_path)   (the `result` dicts of callback)  worker.py:564-645
 
-Differences that do not change results: the model call goes to the sm_100a engine; only the heads a task
+Differences that do not change results: the model call goes to the sm_90a engine; only the heads a task
 reads are computed (the reference computes all ten outputs and drops nine); top-N uses `topk` instead of a
 full sort + per-element `.item()`; label maps are loaded once instead of per request (worker.py:299-300,
 311-315); `eval(task_id)` (worker.py:562) is `int(task_id)`.
