@@ -11,6 +11,9 @@
  *                                                                      worker.py:286-289
  * The entry points below are exactly what a binding for that protocol needs, and nothing else:
  * vb200_create <- from_pretrained + cuda(i); vb200_forward <- __call__; vb200_destroy <- del.
+ * Beyond the protocol: packed variable-length batches (vb200_packed_inputs: samples with their own text lengths and region counts
+ * in one forward, plans keyed on capacity buckets, GEMM tiles past the call's row totals skipped), detector output in
+ * (vb200_region_inputs), caption-image retrieval with reuse, and kernel-level entry points for the tests.
  * The Python shim in vilbert-multi-task_b200/ (ctypes) implements the protocol on top of them; see
  * INTEGRATION.md for the stub a maintainer of the reference would add.
  *
@@ -230,6 +233,34 @@ typedef struct {
 int vb200_forward_regions(vb200_handle h, const vb200_region_inputs* in, const vb200_outputs* out, uint32_t select, int32_t slot,
                           void* cuda_stream);
 
+/* ---- Packed variable-length batches: one forward for samples with different text lengths and region counts.  Sample i's
+ * Tin_i tokens and V_i regions are stored back to back with no padding and no masks: every row is a real token or region.  The
+ * result is the forward of the same samples padded to a common shape with input_mask / image_mask = 1 on the real rows,
+ * restricted to the real rows -- and bit-identical to a forward of each sample alone at its own (Tin_i, V_i).
+ * Per-sample outputs keep their shapes ([B, num_labels], [B/2, 2], pooled_output, ...); per-row outputs are packed: vision_logit
+ * [sum V_i, 1], vision_prediction [sum V_i, v_target], linguisic_logit [sum T_i, 1], linguisic_prediction [sum T_i, vocab] and the
+ * sequence_output_t / _v taps, with T_i = Tin_i + 1 (task token).
+ * Plans are keyed on (B, round16(max_tokens + 1), round16(max_regions), select, slot): a capacity costs workspace only (GEMM tiles
+ * past the call's row totals are skipped, attention runs each sample at its own length), so a server that passes fixed capacities
+ * keeps one plan and one CUDA graph per batch size whatever the lengths.  The lengths are host arrays (the plan is chosen on the
+ * host); the per-sample offsets and row totals are copied to the plan's workspace on cuda_stream through a pinned staging buffer.
+ * VB200_ERR_INVALID for VB200_OUT_ATTENTION, split_fp32 engines, a length < 1 or above a non-zero capacity, T_i or V_i > 256 and
+ * Tin_i > max_position_embeddings. */
+typedef struct {
+    int32_t batch;                  /* B */
+    int32_t max_tokens;             /* plan capacity: 0 -> max Tin_i of this call; else >= every Tin_i */
+    int32_t max_regions;            /* plan capacity: 0 -> max V_i of this call;   else >= every V_i */
+    const int32_t* n_tokens;        /* HOST [B]: Tin_i >= 1 (T_i = Tin_i + 1 with task tokens) */
+    const int32_t* n_regions;       /* HOST [B]: V_i >= 1 */
+    const int64_t* question;        /* DEVICE [sum Tin_i]      sample i's tokens back to back, no padding */
+    const int64_t* segment_ids;     /* DEVICE [sum Tin_i] */
+    const float*   features;        /* DEVICE [sum V_i, v_feature_size] */
+    const float*   spatials;        /* DEVICE [sum V_i, 5] */
+    const int64_t* task_tokens;     /* DEVICE [B, 1] */
+} vb200_packed_inputs;
+int vb200_forward_packed(vb200_handle h, const vb200_packed_inputs* in, const vb200_outputs* out, uint32_t select,
+                         int32_t slot, void* cuda_stream);
+
 /* ---- Caption-image retrieval with reuse (SURVEY.md section 8e; reference semantics worker.py:278-284, 359).  Everything ahead of
  * the first connection layer depends on the caption alone or on the image alone: encode each caption / image ONCE, then score
  * pairs from the cached states.  Same kernels on the same rows as the full forward: scores are bit-identical to vb200_forward.
@@ -259,6 +290,11 @@ int vb200_linear(const void* x_bf16, int64_t ld_x, const void* w_bf16, int64_t l
                  const float* residual, int64_t ld_res, const float* gamma, const float* beta, float eps, int32_t act,
                  void* y_bf16, int64_t ld_y_bf16, float* y_f32, int64_t ld_y_f32, int64_t M, int64_t N, int64_t K,
                  int32_t block_n, int32_t use_pdl, int32_t act_fp16, int32_t variant, long long* timing, void* cuda_stream);
+/* The plain GEMM (variant 0, no residual / LayerNorm) with a device row count: rows >= min(*m_rows, M) are neither loaded nor
+ * computed -- the 128-row tiles that start at or past it are skipped, what packed plans rely on (m_rows: device int32). */
+int vb200_linear_rows(const void* x16, int64_t ld_x, const void* w16, int64_t ld_w, const float* bias, int32_t act, void* y16,
+                      int64_t ld_y16, float* y_f32, int64_t ld_y_f32, int64_t M, int64_t N, int64_t K, int32_t block_n, int32_t act_fp16,
+                      const int32_t* m_rows, void* cuda_stream);
 /* The same GEMM on fp32-parity-mode operands (fp16 only): x16 holds hi | lo | hi and w16 hi | hi | lo per 64 logical columns, K3 is
  * the PHYSICAL contraction length (3x the logical one), y16 (optional) is written in the activation split layout (stride ld_y16 of
  * the 3x wider buffer), y_f32 (optional) as usual. */

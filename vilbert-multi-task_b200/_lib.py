@@ -54,6 +54,13 @@ class RegionInputs(C.Structure):
                 ("image_wh", C.c_void_p), ("num_boxes", C.c_void_p), ("spatials_out", C.c_void_p)]
 
 
+class PackedInputs(C.Structure):
+    """vb200_packed_inputs: a packed variable-length batch (n_tokens / n_regions are HOST int32 arrays, the rest device memory)."""
+    _fields_ = [("batch", C.c_int32), ("max_tokens", C.c_int32), ("max_regions", C.c_int32),
+                ("n_tokens", C.c_void_p), ("n_regions", C.c_void_p), ("question", C.c_void_p), ("segment_ids", C.c_void_p),
+                ("features", C.c_void_p), ("spatials", C.c_void_p), ("task_tokens", C.c_void_p)]
+
+
 class Outputs(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in OUTPUT_FIELDS]
 
@@ -67,8 +74,8 @@ class Options(C.Structure):
 # every symbol include/vilbert_b200.h declares (tests/test_cabi.py checks the list against the header)
 EXPORTS = ["vb200_abi_version", "vb200_create", "vb200_destroy", "vb200_last_error", "vb200_forward", "vb200_forward_slot",
            "vb200_forward_host", "vb200_forward_host_slot", "vb200_plan_info", "vb200_model_dim", "vb200_set_option", "vb200_timeline", "vb200_profile_ops",
-           "vb200_attention_layout", "vb200_forward_regions", "vb200_encode_text", "vb200_encode_image", "vb200_forward_cached",
-           "vb200_linear", "vb200_linear_split", "vb200_linear_ln", "vb200_linear_chain", "vb200_layernorm", "vb200_layernorm_split", "vb200_attention_f32",
+           "vb200_attention_layout", "vb200_forward_regions", "vb200_forward_packed", "vb200_encode_text", "vb200_encode_image", "vb200_forward_cached",
+           "vb200_linear", "vb200_linear_rows", "vb200_linear_split", "vb200_linear_ln", "vb200_linear_chain", "vb200_layernorm", "vb200_layernorm_split", "vb200_attention_f32",
            "vb200_self_attention", "vb200_co_attention"]
 
 _lib = None
@@ -109,6 +116,8 @@ def load():
                                       C.POINTER(C.c_double), C.POINTER(i32)]
     lib.vb200_attention_layout.argtypes = [vp, i32, i32, i32, i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(i64), C.POINTER(i64)]
     lib.vb200_forward_regions.argtypes = [vp, C.POINTER(RegionInputs), C.POINTER(Outputs), u32, i32, vp]
+    lib.vb200_forward_packed.argtypes = [vp, C.POINTER(PackedInputs), C.POINTER(Outputs), u32, i32, vp]
+    lib.vb200_linear_rows.argtypes = [vp, i64, vp, i64, vp, i32, vp, i64, vp, i64, i64, i64, i64, i32, i32, vp, vp]
     lib.vb200_encode_text.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp]
     lib.vb200_encode_image.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp, vp, vp]
     lib.vb200_forward_cached.argtypes = [vp, i32, i32, i32, vp, i32, vp, vp, vp, vp, i32, vp, vp, vp, C.POINTER(Outputs), u32, i32, vp]

@@ -272,10 +272,14 @@ __device__ __forceinline__ void attend_tile_short(const uint16_t* Qs, const uint
 template <int D, bool F16>
 __global__ void __launch_bounds__(256, 2)     // <= 128 registers: 5 CTAs of 3-4 warps per SM -> one wave at batch 64
 self_attention_kernel(const uint16_t* __restrict__ qkv, int ld_qkv, int hidden, const float* __restrict__ key_mask_add,
-                      uint16_t* __restrict__ ctx, int ld_ctx, int L, float scale_l2, int pdl) {
+                      uint16_t* __restrict__ ctx, int ld_ctx, int L_cap, float scale_l2, int pdl, const int* __restrict__ offs) {
     extern __shared__ __align__(16) uint8_t smem_attn[];
     constexpr int kStride = AttnTile<D>::kStride;
     const int h = blockIdx.x, b = blockIdx.y;
+    // sample b: rows [r0, r0 + L).  Packed batches (offs) give every sample its own length; everything below -- tile sizes,
+    // loop bounds, the short-key path -- depends on that length only, so a sample computes what a batch of it alone computes.
+    const int r0 = offs ? offs[b] : b * L_cap;
+    const int L = offs ? offs[b + 1] - r0 : L_cap;
     const int Lp = pad16(L);
     uint16_t* Qs = reinterpret_cast<uint16_t*>(smem_attn);
     uint16_t* Ks = Qs + Lp * kStride;
@@ -285,15 +289,15 @@ self_attention_kernel(const uint16_t* __restrict__ qkv, int ld_qkv, int hidden, 
 
     if (pdl) pdl_wait();
 
-    const uint16_t* base = qkv + static_cast<size_t>(b) * L * ld_qkv + h * D;
+    const uint16_t* base = qkv + static_cast<size_t>(r0) * ld_qkv + h * D;
     load_tile<D>(Qs, base, L, Lp, ld_qkv);
     load_tile<D>(Ks, base + hidden, L, Lp, ld_qkv);
     load_tile<D>(Vs, base + 2 * hidden, L, Lp, ld_qkv);
-    for (int j = threadIdx.x; j < L; j += blockDim.x) mask_s[j] = key_mask_add[b * L + j] * kLog2e;
+    for (int j = threadIdx.x; j < L; j += blockDim.x) mask_s[j] = key_mask_add[r0 + j] * kLog2e;
     cp_async_wait_all();
     __syncthreads();
     if (pdl) pdl_launch_dependents();       // tiles are staged: the next kernel's prologue may overlap the math
-    uint16_t* outp = ctx + static_cast<size_t>(b) * L * ld_ctx + h * D;
+    uint16_t* outp = ctx + static_cast<size_t>(r0) * ld_ctx + h * D;
     constexpr int kSplit = D / 64, kOW = D / kSplit;             // work item = (16-row tile, 64-column slice of the head)
     if (L <= kKeyBlock) {                                        // one key block: S and the softmax once per row tile
         for (int t = warp; t * 16 < L; t += nwarps)
@@ -308,8 +312,8 @@ template <int D, bool F16>
 __global__ void __launch_bounds__(256, 2)
 co_attention_kernel(const uint16_t* __restrict__ qkv_img, int ld_img, const uint16_t* __restrict__ qkv_txt, int ld_txt,
                     int hidden, const float* __restrict__ img_mask_add, const float* __restrict__ txt_mask_add,
-                    uint16_t* __restrict__ ctx_txt, int ld_ctx_txt, uint16_t* __restrict__ ctx_img, int ld_ctx_img, int T,
-                    int V, float scale_l2, int pdl) {
+                    uint16_t* __restrict__ ctx_txt, int ld_ctx_txt, uint16_t* __restrict__ ctx_img, int ld_ctx_img, int T_cap,
+                    int V_cap, float scale_l2, int pdl, const int* __restrict__ offs_t, const int* __restrict__ offs_v) {
     // Two phases over ONE set of Q/K/V buffers sized for the longer sequence (39 KB at T=31/V=36 instead of 65 KB for all
     // six tiles: 5 CTAs per SM, so the 512 (sample, head) CTAs of a batch-64 layer are resident in a single wave).
     //   phase 1: text queries (Q2) over image keys/values (K1, V1) -> context for the text stream
@@ -317,6 +321,9 @@ co_attention_kernel(const uint16_t* __restrict__ qkv_img, int ld_img, const uint
     extern __shared__ __align__(16) uint8_t smem_attn[];
     constexpr int kStride = AttnTile<D>::kStride;
     const int h = blockIdx.x, b = blockIdx.y;
+    // sample b: text rows [t0, t0 + T), image rows [v0, v0 + V) -- per-sample lengths in packed batches (see self_attention_kernel)
+    const int t0 = offs_t ? offs_t[b] : b * T_cap, T = offs_t ? offs_t[b + 1] - t0 : T_cap;
+    const int v0 = offs_v ? offs_v[b] : b * V_cap, V = offs_v ? offs_v[b + 1] - v0 : V_cap;
     const int Tp = pad16(T), Vp = pad16(V);
     const int Lp = Tp > Vp ? Tp : Vp;
     uint16_t* Qs = reinterpret_cast<uint16_t*>(smem_attn);
@@ -328,16 +335,16 @@ co_attention_kernel(const uint16_t* __restrict__ qkv_img, int ld_img, const uint
 
     if (pdl) pdl_wait();
 
-    const uint16_t* bi = qkv_img + static_cast<size_t>(b) * V * ld_img + h * D;
-    const uint16_t* bt = qkv_txt + static_cast<size_t>(b) * T * ld_txt + h * D;
+    const uint16_t* bi = qkv_img + static_cast<size_t>(v0) * ld_img + h * D;
+    const uint16_t* bt = qkv_txt + static_cast<size_t>(t0) * ld_txt + h * D;
     load_tile<D>(Qs, bt, T, Tp, ld_txt);                         // Q2
     load_tile<D>(Ks, bi + hidden, V, Vp, ld_img);                // K1
     load_tile<D>(Vs, bi + 2 * hidden, V, Vp, ld_img);            // V1
-    for (int j = threadIdx.x; j < V; j += blockDim.x) mask_img[j] = img_mask_add[b * V + j] * kLog2e;
-    for (int j = threadIdx.x; j < T; j += blockDim.x) mask_txt[j] = txt_mask_add[b * T + j] * kLog2e;
+    for (int j = threadIdx.x; j < V; j += blockDim.x) mask_img[j] = img_mask_add[v0 + j] * kLog2e;
+    for (int j = threadIdx.x; j < T; j += blockDim.x) mask_txt[j] = txt_mask_add[t0 + j] * kLog2e;
     cp_async_wait_all();
     __syncthreads();
-    uint16_t* out_t = ctx_txt + static_cast<size_t>(b) * T * ld_ctx_txt + h * D;
+    uint16_t* out_t = ctx_txt + static_cast<size_t>(t0) * ld_ctx_txt + h * D;
     constexpr int kSplit = D / 64, kOW = D / kSplit;
     if (V <= kKeyBlock) {
         for (int t = warp; t * 16 < T; t += nwarps)
@@ -353,7 +360,7 @@ co_attention_kernel(const uint16_t* __restrict__ qkv_img, int ld_img, const uint
     cp_async_wait_all();
     __syncthreads();
     if (pdl) pdl_launch_dependents();
-    uint16_t* out_v = ctx_img + static_cast<size_t>(b) * V * ld_ctx_img + h * D;
+    uint16_t* out_v = ctx_img + static_cast<size_t>(v0) * ld_ctx_img + h * D;
     if (T <= kKeyBlock) {
         for (int t = warp; t * 16 < V; t += nwarps)
             attend_tile_short<D, F16>(Qs, Ks, Vs, t * 16, V, T, mask_txt, scale_l2, out_v, ld_ctx_img, lane);
@@ -365,7 +372,8 @@ co_attention_kernel(const uint16_t* __restrict__ qkv_img, int ld_img, const uint
 
 template <int D, bool F16>
 static cudaError_t launch_self(const __nv_bfloat16* qkv, int ld_qkv, int hidden, const float* key_mask_add,
-                               __nv_bfloat16* ctx, int ld_ctx, int B, int L, int heads, int pdl, cudaStream_t st) {
+                               __nv_bfloat16* ctx, int ld_ctx, int B, int L, int heads, int pdl, cudaStream_t st,
+                               const int* offs) {
     const int Lp = pad16(L);
     const size_t smem = 3 * AttnTile<D>::bytes(Lp) + sizeof(float) * L;
     if (smem > 227 * 1024) return cudaErrorInvalidValue;
@@ -378,26 +386,26 @@ static cudaError_t launch_self(const __nv_bfloat16* qkv, int ld_qkv, int hidden,
     const float scale_l2 = kLog2e / sqrtf(static_cast<float>(D));
     return launch_ex(self_attention_kernel<D, F16>, dim3(heads, B), dim3(32 * nwarps), smem, pdl, st,
                      reinterpret_cast<const uint16_t*>(qkv), ld_qkv, hidden, key_mask_add, reinterpret_cast<uint16_t*>(ctx),
-                     ld_ctx, L, scale_l2, pdl);
+                     ld_ctx, L, scale_l2, pdl, offs);
 }
 
 cudaError_t launch_self_attention(const __nv_bfloat16* qkv, int ld_qkv, int hidden, const float* key_mask_add,
                                   __nv_bfloat16* ctx, int ld_ctx, int B, int L, int heads, int head_dim, int pdl,
-                                  int f16, cudaStream_t st) {
+                                  int f16, cudaStream_t st, const int* offs) {
     if (L < 1 || (head_dim != 64 && head_dim != 128) || (ld_qkv & 7) || (ld_ctx & 1) || (hidden & 7))
         return cudaErrorInvalidValue;
     if (head_dim == 64)
-        return f16 ? launch_self<64, true>(qkv, ld_qkv, hidden, key_mask_add, ctx, ld_ctx, B, L, heads, pdl, st)
-                   : launch_self<64, false>(qkv, ld_qkv, hidden, key_mask_add, ctx, ld_ctx, B, L, heads, pdl, st);
-    return f16 ? launch_self<128, true>(qkv, ld_qkv, hidden, key_mask_add, ctx, ld_ctx, B, L, heads, pdl, st)
-               : launch_self<128, false>(qkv, ld_qkv, hidden, key_mask_add, ctx, ld_ctx, B, L, heads, pdl, st);
+        return f16 ? launch_self<64, true>(qkv, ld_qkv, hidden, key_mask_add, ctx, ld_ctx, B, L, heads, pdl, st, offs)
+                   : launch_self<64, false>(qkv, ld_qkv, hidden, key_mask_add, ctx, ld_ctx, B, L, heads, pdl, st, offs);
+    return f16 ? launch_self<128, true>(qkv, ld_qkv, hidden, key_mask_add, ctx, ld_ctx, B, L, heads, pdl, st, offs)
+               : launch_self<128, false>(qkv, ld_qkv, hidden, key_mask_add, ctx, ld_ctx, B, L, heads, pdl, st, offs);
 }
 
 template <int D, bool F16>
 static cudaError_t launch_co(const __nv_bfloat16* qkv_img, int ld_img, const __nv_bfloat16* qkv_txt, int ld_txt, int hidden,
                              const float* img_mask_add, const float* txt_mask_add, __nv_bfloat16* ctx_txt, int ld_ctx_txt,
                              __nv_bfloat16* ctx_img, int ld_ctx_img, int B, int T, int V, int heads, int pdl,
-                             cudaStream_t st) {
+                             cudaStream_t st, const int* offs_t, const int* offs_v) {
     const int Tp = pad16(T), Vp = pad16(V);
     const int Lp = Tp > Vp ? Tp : Vp;
     const size_t smem = 3 * AttnTile<D>::bytes(Lp) + sizeof(float) * (T + V);
@@ -410,18 +418,19 @@ static cudaError_t launch_co(const __nv_bfloat16* qkv_img, int ld_img, const __n
     return launch_ex(co_attention_kernel<D, F16>, dim3(heads, B), dim3(32 * nwarps), smem, pdl, st,
                      reinterpret_cast<const uint16_t*>(qkv_img), ld_img, reinterpret_cast<const uint16_t*>(qkv_txt), ld_txt,
                      hidden, img_mask_add, txt_mask_add, reinterpret_cast<uint16_t*>(ctx_txt), ld_ctx_txt,
-                     reinterpret_cast<uint16_t*>(ctx_img), ld_ctx_img, T, V, scale_l2, pdl);
+                     reinterpret_cast<uint16_t*>(ctx_img), ld_ctx_img, T, V, scale_l2, pdl, offs_t, offs_v);
 }
 
 cudaError_t launch_co_attention(const __nv_bfloat16* qkv_img, int ld_img, const __nv_bfloat16* qkv_txt, int ld_txt,
                                 int hidden, const float* img_mask_add, const float* txt_mask_add,
                                 __nv_bfloat16* ctx_txt, int ld_ctx_txt, __nv_bfloat16* ctx_img, int ld_ctx_img, int B,
-                                int T, int V, int heads, int head_dim, int pdl, int f16, cudaStream_t st) {
+                                int T, int V, int heads, int head_dim, int pdl, int f16, cudaStream_t st,
+                                const int* offs_t, const int* offs_v) {
     if (T < 1 || V < 1 || (head_dim != 64 && head_dim != 128) || (ld_img & 7) || (ld_txt & 7) || (hidden & 7) ||
         (ld_ctx_txt & 1) || (ld_ctx_img & 1))
         return cudaErrorInvalidValue;
 #define VB_CO(D, F) launch_co<D, F>(qkv_img, ld_img, qkv_txt, ld_txt, hidden, img_mask_add, txt_mask_add, ctx_txt, ld_ctx_txt, \
-                                    ctx_img, ld_ctx_img, B, T, V, heads, pdl, st)
+                                    ctx_img, ld_ctx_img, B, T, V, heads, pdl, st, offs_t, offs_v)
     if (head_dim == 64) return f16 ? VB_CO(64, true) : VB_CO(64, false);
     return f16 ? VB_CO(128, true) : VB_CO(128, false);
 #undef VB_CO

@@ -17,12 +17,19 @@ text_embed_kernel(const int64_t* __restrict__ ids, const int64_t* __restrict__ s
                   const float* __restrict__ task_tab, const float* __restrict__ gamma, const float* __restrict__ beta,
                   float eps, float* __restrict__ out_f32, __nv_bfloat16* __restrict__ out_bf16,
                   float* __restrict__ mask_add, int B, int Tin, int H, int vocab, int max_pos, int n_type, int n_task,
-                  int task_tokens, int f16, int split16) {
-    const int T = Tin + (task_tokens ? 1 : 0);
+                  int task_tokens, int f16, int split16, const int* __restrict__ offs, int rows) {
     const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
-    if (row >= B * T) return;
-    const int b = row / T, t = row % T;
+    if (row >= rows) return;
+    int b, t, in0;                                                // sample, position in it, first input token of the sample
+    if (offs == nullptr) {
+        const int T = Tin + (task_tokens ? 1 : 0);
+        b = row / T; t = row % T; in0 = b * Tin;
+    } else {                                                      // packed batch: the sample whose rows [offs[b], offs[b+1]) hold `row`
+        int lo = 0, hi = B - 1;
+        while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (offs[mid] <= row) lo = mid; else hi = mid - 1; }
+        b = lo; t = row - offs[b]; in0 = offs[b] - (task_tokens ? b : 0);
+    }
     const int nvec = H / 128;
 
     // which source token does output position t carry?  [CLS], <task>, tok1, tok2, ...
@@ -36,8 +43,8 @@ text_embed_kernel(const int64_t* __restrict__ ids, const int64_t* __restrict__ s
 #pragma unroll
         for (int k = 0; k < kMaxVec; ++k) if (k < nvec) x[k] = tp[lane + 32 * k];
     } else {
-        long long id = ids[b * Tin + src];
-        long long sg = seg[b * Tin + src];
+        long long id = ids[in0 + src];
+        long long sg = seg[in0 + src];
         id = id < 0 ? 0 : (id >= vocab ? vocab - 1 : id);
         sg = sg < 0 ? 0 : (sg >= n_type ? n_type - 1 : sg);
         const int ps = src < max_pos ? src : max_pos - 1;
@@ -94,8 +101,10 @@ text_embed_kernel(const int64_t* __restrict__ ids, const int64_t* __restrict__ s
         // [UPSTREAM] BertModel.forward prepends a 1 to the mask when task tokens are on:
         //   ext_mask[0] = 1, ext_mask[t] = input_mask[t - 1] for t >= 1
         // (position 1, the task row, therefore carries input_mask[0], the [CLS] flag).
-        const float m = task_tokens ? (t == 0 ? 1.0f : static_cast<float>(input_mask[b * Tin + (t - 1)]))
-                                    : static_cast<float>(input_mask[b * Tin + t]);
+        // packed batches have no padding: every row's flag is 1
+        const float m = offs != nullptr ? 1.0f
+                                        : task_tokens ? (t == 0 ? 1.0f : static_cast<float>(input_mask[in0 + (t - 1)]))
+                                                      : static_cast<float>(input_mask[in0 + t]);
         mask_add[row] = (1.0f - m) * -10000.0f;
     }
 }
@@ -133,7 +142,7 @@ image_pack_kernel(const float* __restrict__ feats, const float* __restrict__ loc
             put(nvec + threadIdx.x, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f);
         }
     }
-    if (threadIdx.x == 0) mask_add[row] = (1.0f - static_cast<float>(image_mask[row])) * -10000.0f;
+    if (threadIdx.x == 0) mask_add[row] = (1.0f - (image_mask ? static_cast<float>(image_mask[row]) : 1.0f)) * -10000.0f;
 }
 
 // custom_prediction()'s input builder on the device (worker.py:422-455): per image, the detector's n box features [n, F] become the
@@ -216,23 +225,27 @@ gather_state_kernel(const int32_t* __restrict__ idx, int n_src, const float* __r
     const int b = blockIdx.x;
     int s = idx[b];
     s = s < 0 ? 0 : (s >= n_src ? n_src - 1 : s);
-    const uint4* a = reinterpret_cast<const uint4*>(src_f32) + static_cast<size_t>(s) * n32;
-    uint4* d = reinterpret_cast<uint4*>(dst_f32) + static_cast<size_t>(b) * n32;
-    for (int i = threadIdx.x; i < n32; i += blockDim.x) d[i] = a[i];
+    if (src_f32 != nullptr) {
+        const uint4* a = reinterpret_cast<const uint4*>(src_f32) + static_cast<size_t>(s) * n32;
+        uint4* d = reinterpret_cast<uint4*>(dst_f32) + static_cast<size_t>(b) * n32;
+        for (int i = threadIdx.x; i < n32; i += blockDim.x) d[i] = a[i];
+    }
     const uint4* a2 = reinterpret_cast<const uint4*>(src_16) + static_cast<size_t>(s) * n16;
     uint4* d2 = reinterpret_cast<uint4*>(dst_16) + static_cast<size_t>(b) * n16;
     for (int i = threadIdx.x; i < n16; i += blockDim.x) d2[i] = a2[i];
-    for (int i = threadIdx.x; i < L; i += blockDim.x) dst_mask[static_cast<size_t>(b) * L + i] = src_mask[static_cast<size_t>(s) * L + i];
+    if (src_mask != nullptr)
+        for (int i = threadIdx.x; i < L; i += blockDim.x) dst_mask[static_cast<size_t>(b) * L + i] = src_mask[static_cast<size_t>(s) * L + i];
 }
 
 // one warp per row; n_out <= 4
 __global__ void __launch_bounds__(128)
 rowdot_kernel(const float* __restrict__ x, int ld_x, const float* __restrict__ W, const float* __restrict__ bias,
-              const float* __restrict__ add, float* __restrict__ out, int ld_out, int M, int K, int n_out, int pdl) {
+              const float* __restrict__ add, float* __restrict__ out, int ld_out, int M, int K, int n_out, int pdl,
+              const int* __restrict__ m_rows) {
     if (pdl) { pdl_wait(); pdl_launch_dependents(); }
     const int m = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
-    if (m >= M) return;
+    if (m >= M || (m_rows != nullptr && m >= *m_rows)) return;       // packed batches: rows past the device row count
     float acc[4] = {0.0f, 0.0f, 0.0f, 0.0f};
     const float4* xp = reinterpret_cast<const float4*>(x + static_cast<size_t>(m) * ld_x);
     for (int k = lane; k < K / 4; k += 32) {
@@ -257,13 +270,13 @@ cudaError_t launch_text_embed(const int64_t* ids, const int64_t* seg, const int6
                               const float* word, const float* pos, const float* type, const float* task_tab,
                               const float* gamma, const float* beta, float eps, float* out_f32,
                               __nv_bfloat16* out_bf16, float* mask_add, int B, int Tin, int H, int vocab, int max_pos,
-                              int n_type, int n_task, int task_tokens, int f16, int split16, cudaStream_t st) {
-    if (H % 128 != 0 || H / 128 > kMaxVec || (split16 && !f16)) return cudaErrorInvalidValue;
-    const int T = Tin + (task_tokens ? 1 : 0);
-    const int rows = B * T;
+                              int n_type, int n_task, int task_tokens, int f16, int split16, cudaStream_t st,
+                              const int* offs, int rows) {
+    if (H % 128 != 0 || H / 128 > kMaxVec || (split16 && !f16) || (offs != nullptr && (B < 1 || rows < 1))) return cudaErrorInvalidValue;
+    if (offs == nullptr) rows = B * (Tin + (task_tokens ? 1 : 0));
     text_embed_kernel<<<(rows + 3) / 4, 128, 0, st>>>(ids, seg, input_mask, task, word, pos, type, task_tab, gamma, beta,
                                                       eps, out_f32, out_bf16, mask_add, B, Tin, H, vocab, max_pos,
-                                                      n_type, n_task, task_tokens, f16, split16);
+                                                      n_type, n_task, task_tokens, f16, split16, offs, rows);
     return cudaGetLastError();
 }
 
@@ -292,10 +305,10 @@ cudaError_t launch_gather_state(const int32_t* idx, int n_src, const float* src_
 }
 
 cudaError_t launch_rowdot(const float* x, int ld_x, const float* W, const float* b, const float* add, float* out,
-                          int ld_out, int M, int K, int n_out, int pdl, cudaStream_t st) {
+                          int ld_out, int M, int K, int n_out, int pdl, cudaStream_t st, const int* m_rows) {
     if (n_out < 1 || n_out > 4 || K % 4 != 0 || ld_x % 4 != 0) return cudaErrorInvalidValue;
     return launch_ex(rowdot_kernel, dim3((M + 3) / 4), dim3(128), 0, pdl, st, x, ld_x, W, b, add, out, ld_out, M, K,
-                     n_out, pdl);
+                     n_out, pdl, m_rows);
 }
 
 }  // namespace vb

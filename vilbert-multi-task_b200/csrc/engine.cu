@@ -352,7 +352,7 @@ void setup_tma_store(CUtensorMap* tc, GemmEpilogue& e) {
 
 // ------------------------------------------------------------------------------------------ launch list
 struct Op {
-    enum Kind { GEMM, SELF_ATTN, CO_ATTN, ROWDOT, LAYERNORM, ATTN_F32 } kind;
+    enum Kind { GEMM, SELF_ATTN, CO_ATTN, ROWDOT, LAYERNORM, ATTN_F32, GATHER } kind;
     int stream = 0;                // 0 main, 1 side (image branch) inside the captured graph
     // GEMM
     CUtensorMap ta, tb, tc;        // operands, and the output (TMA-store epilogue, ep.tma_store != 0)
@@ -388,6 +388,11 @@ struct Op {
     const float *x = nullptr, *W = nullptr, *bias = nullptr, *add = nullptr;
     float* out = nullptr;
     int ld_x = 0, ld_out = 0, M = 0, K = 0, n_out = 0;
+    // packed plans: device row count of the GEMM / LayerNorm / rowdot rows (ep.m_rows for GEMMs), per-sample row offsets of
+    // the attention operands (offs_a: La stream, offs_b: Lb stream); GATHER: row offs_a[b] of qkv_a (16-bit, ld_a wide) -> row b
+    // of ctx_a, b < B, clamped to M rows
+    const int* m_rows = nullptr;
+    const int *offs_a = nullptr, *offs_b = nullptr;
     // fork/join markers for the two-stream graph
     enum Sync { NONE, FORK, JOIN } sync = NONE;
     double flops = 0;
@@ -424,9 +429,21 @@ struct Plan {
     float *d_feat = nullptr, *d_loc = nullptr;
     uint8_t* d_imask = nullptr;
     float* d_out[12] = {nullptr};
+    // packed plans (vb200_forward_packed): d_meta = text row offsets [B + 1] | image row offsets [B + 1] | text rows | image rows,
+    // filled per call from the pinned h_meta; meta_copied marks when the last copy out of h_meta has been made
+    bool packed = false;
+    int* d_meta = nullptr;
+    int* h_meta = nullptr;
+    cudaEvent_t meta_copied = nullptr;
+    const int* offs_t() const { return d_meta; }
+    const int* offs_v() const { return d_meta + B + 1; }
+    const int* rows_t() const { return d_meta + 2 * (B + 1); }
+    const int* rows_v() const { return d_meta + 2 * (B + 1) + 1; }
     ~Plan() {
         if (exec) cudaGraphExecDestroy(exec);
         if (graph) cudaGraphDestroy(graph);
+        if (meta_copied) { cudaEventSynchronize(meta_copied); cudaEventDestroy(meta_copied); }
+        if (h_meta) cudaFreeHost(h_meta);
     }
 };
 
@@ -861,7 +878,7 @@ struct vb200_engine {
     };
     void add_linear(Plan& pl, const bf16* A, int64_t a_rows, int64_t lda, const LinearW& W, int act, const float* res, int ld_res,
                     const LNW* ln, bf16* out_b, int ld_b, float* out_f, int ld_f, int stream = 0, Op::Sync sync = Op::NONE,
-                    const float* mul = nullptr, int ld_mul = 0, const FoldArgs* fa = nullptr) {
+                    const float* mul = nullptr, int ld_mul = 0, const FoldArgs* fa = nullptr, const int* m_rows = nullptr) {
         const int S = x3 ? 3 : 1;
         const bool keep_pending = ln != nullptr && fa != nullptr && fa->out_stats != nullptr;
         const bool fold_in = fa != nullptr && fa->a_stats != nullptr;
@@ -894,6 +911,7 @@ struct vb200_engine {
         e.M = static_cast<int>(a_rows); e.N = W.N; e.K = W.ldw * S;
         e.bias = W.bias; e.mul = mul; e.ld_mul = ld_mul; e.eps = cfg.ln_eps; e.act = act; e.pdl = pdl_light ? 2 : (opt.use_pdl ? (early_w ? 5 : 1) : 0);
         e.a_f16 = opt.act_fp16; e.out_f16 = opt.act_fp16;
+        e.m_rows = m_rows;
         if (fold_in) {
             e.ln_mode = 4; e.a_stats = fa->a_stats; e.a_parts = fa->a_parts; e.fold_s = W.fold_s; e.stats_ld = fa->stats_ld;
         }
@@ -926,6 +944,7 @@ struct vb200_engine {
             l.ln_g = ln->g; l.ln_b = ln->b; l.ln_out_f = out_f; l.ln_out_h = out_b; l.ln_ld = W.N;
             l.ld_out = out_f ? ld_f : 0; l.ld_a = out_b ? ld_b * S : 0;
             l.ln_M = static_cast<int>(a_rows); l.ln_N = W.N;
+            l.m_rows = m_rows;
             if (fa != nullptr && fa->res_stats != nullptr)
                 l.ln_pend = vb::LnPending{fa->res_stats, fa->res_parts, fa->stats_ld, fa->res_ln->g, fa->res_ln->b};
             pl.ops.push_back(l);
@@ -950,8 +969,9 @@ struct vb200_engine {
         if (x3) { a.flops = 4.0 * pl.B * heads * Lq * Lk * (hid / heads); pl.flops += a.flops; }
         pl.ops.push_back(a);
     }
-    Op rowdot_op(const float* x, int ld_x, const RowW& w, const float* add, float* out, int ld_out, int M) {
+    Op rowdot_op(const float* x, int ld_x, const RowW& w, const float* add, float* out, int ld_out, int M, const int* m_rows = nullptr) {
         Op op{};
+        op.m_rows = m_rows;
         op.kind = Op::ROWDOT;
         op.x = x; op.ld_x = ld_x; op.W = w.w; op.bias = w.b; op.add = add; op.out = out; op.ld_out = ld_out;
         op.M = M; op.K = w.K; op.n_out = w.n_out;
@@ -969,7 +989,10 @@ struct vb200_engine {
     // the text layers scheduled ahead of C0) or on the image alone (image embedding + any image layer ahead of C0), so a
     // 1000 x 1000 score matrix computes those once per caption / per image and runs only the SUFFIX per pair -- the same kernels on
     // the same rows, hence bit-identical scores.
-    enum PlanMode { FULL = 0, TEXT_PREFIX = 1, IMAGE_PREFIX = 2, SUFFIX = 3 };
+    // PACKED runs FULL's schedule on a packed variable-length batch (vb200_forward_packed): Tin + task tokens and V are the plan's
+    // per-sample capacities (multiples of 16), every buffer holds B x capacity rows, and the kernels take the call's row offsets and
+    // row totals from the plan's d_meta -- GEMMs skip the tiles past the totals, attention runs each sample at its own length.
+    enum PlanMode { FULL = 0, TEXT_PREFIX = 1, IMAGE_PREFIX = 2, SUFFIX = 3, PACKED = 4 };
 
     Plan* get_plan(int B, int Tin, int V, uint32_t select, int slot = 0, int mode = FULL, bool want_attn = false) {
         if (slot < 0 || slot > 15) fail(VB200_ERR_INVALID, "slot %d out of range (0..15)", slot);
@@ -984,12 +1007,26 @@ struct vb200_engine {
         const int T = Tin + (c.task_tokens ? 1 : 0);
         if (B < 1 || Tin < 1 || V < 1) fail(VB200_ERR_INVALID, "batch, n_tokens and n_regions must be positive");
         if (T > 256 || V > 256) fail(VB200_ERR_INVALID, "sequence too long for the small-sequence attention kernels (T=%d, V=%d, max 256)", T, V);
-        if (Tin > c.max_pos) fail(VB200_ERR_INVALID, "n_tokens %d exceeds max_position_embeddings %d", Tin, c.max_pos);
+        if (Tin > c.max_pos && mode != PACKED) fail(VB200_ERR_INVALID, "n_tokens %d exceeds max_position_embeddings %d", Tin, c.max_pos);
         pl.B = B; pl.Tin = Tin; pl.T = T; pl.V = V; pl.select = select;
+        if (mode == PACKED) {
+            // zero offsets and totals until the first call: the validation pass and the capture below then touch no row
+            pl.packed = true;
+            const size_t n_meta = 2 * (static_cast<size_t>(B) + 1) + 2;
+            pl.d_meta = pl.mem.alloc_n<int>(n_meta);
+            CUDA_CHECK(cudaMemset(pl.d_meta, 0, n_meta * sizeof(int)));
+            CUDA_CHECK(cudaMallocHost(&pl.h_meta, n_meta * sizeof(int)));
+            CUDA_CHECK(cudaEventCreateWithFlags(&pl.meta_copied, cudaEventDisableTiming));
+        }
+        const int* rows_t = pl.packed ? pl.rows_t() : nullptr;
+        const int* rows_v = pl.packed ? pl.rows_v() : nullptr;
+        const int* offs_t = pl.packed ? pl.offs_t() : nullptr;
+        const int* offs_v = pl.packed ? pl.offs_v() : nullptr;
         const int Mt = B * T, Mv = B * V, H = c.hidden, Hv = c.v_hidden, Hb = c.bi_hidden;
         const size_t S = x3 ? 3 : 1;                 // physical width factor of the 16-bit operand buffers (fp32-parity mode)
-        const bool do_t = mode == FULL || mode == TEXT_PREFIX, do_v = mode == FULL || mode == IMAGE_PREFIX;
-        const bool do_s = mode == FULL || mode == SUFFIX;
+        const bool full = mode == FULL || mode == PACKED;
+        const bool do_t = full || mode == TEXT_PREFIX, do_v = full || mode == IMAGE_PREFIX;
+        const bool do_s = full || mode == SUFFIX;
         pl.kp = img_emb.ldw;
         pl.img_a = pl.mem.alloc_n<bf16>(static_cast<size_t>(Mv) * pl.kp * S);
         pl.mask_t = pl.mem.alloc_n<float>(Mt);
@@ -1026,6 +1063,7 @@ struct vb200_engine {
         struct StreamSt {
             float** f32; bf16** b16; float2** stats; int cur; const LNW* pend; int hid, rows, stats_ld, stream; const float* mask; int seq;
             uint8_t* qkv; bf16* ctx; bf16* inter;
+            const int* m_rows; const int* offs;     // packed plans: device row count and per-sample row offsets of the stream
         };
         if (ln_fold) {
             pl.stats_ld_t = (Mt + 31) & ~31; pl.stats_ld_v = (Mv + 31) & ~31;
@@ -1034,8 +1072,8 @@ struct vb200_engine {
                 pl.v_stats[i] = static_cast<float2*>(pl.mem.alloc(static_cast<size_t>(Hv / 32) * pl.stats_ld_v * sizeof(float2)));
             }
         }
-        StreamSt ts{pl.t_f32, pl.t_b16, pl.t_stats, 0, nullptr, H, Mt, pl.stats_ld_t, 0, pl.mask_t, T, qkv_t, ctx_t, inter_t};
-        StreamSt vs{pl.v_f32, pl.v_b16, pl.v_stats, 0, nullptr, Hv, Mv, pl.stats_ld_v, 1, pl.mask_v, V, qkv_v, ctx_v, inter_v};
+        StreamSt ts{pl.t_f32, pl.t_b16, pl.t_stats, 0, nullptr, H, Mt, pl.stats_ld_t, 0, pl.mask_t, T, qkv_t, ctx_t, inter_t, rows_t, offs_t};
+        StreamSt vs{pl.v_f32, pl.v_b16, pl.v_stats, 0, nullptr, Hv, Mv, pl.stats_ld_v, 1, pl.mask_v, V, qkv_v, ctx_v, inter_v, rows_v, offs_v};
         auto fold_in_args = [&](const StreamSt& st, int which) {          // consume buffers[which] of a stream as a GEMM's A operand
             FoldArgs fa;
             fa.a_stats = st.stats[which]; fa.a_parts = st.hid / 32; fa.stats_ld = st.stats_ld;
@@ -1050,7 +1088,7 @@ struct vb200_engine {
             if (res_pend != nullptr) { fa.res_stats = st.stats[rwhich]; fa.res_parts = st.hid / 32; fa.res_ln = res_pend; }
             if (keep) fa.out_stats = st.stats[owhich];
             add_linear(pl, A, st.rows, lda, W, vb::kActNone, st.f32[rwhich], st.hid, &ln, st.b16[owhich], st.hid, st.f32[owhich], st.hid,
-                       st.stream, sync, nullptr, 0, (res_pend != nullptr || keep) ? &fa : nullptr);
+                       st.stream, sync, nullptr, 0, (res_pend != nullptr || keep) ? &fa : nullptr, st.m_rows);
         };
 
         // ---- image embedding: LayerNorm(feat.W_img^T + loc.W_loc^T + b) as ONE GEMM over K = v_feat + 64
@@ -1060,7 +1098,7 @@ struct vb200_engine {
             fa.stats_ld = vs.stats_ld;
             if (keep) fa.out_stats = vs.stats[0];
             add_linear(pl, pl.img_a, Mv, pl.kp, img_emb, vb::kActNone, nullptr, 0, &vemb_ln, pl.v_b16[0], Hv, pl.v_f32[0], Hv,
-                       1, Op::NONE, nullptr, 0, keep ? &fa : nullptr);   // side stream: overlaps the text layers ahead of the first co-attention
+                       1, Op::NONE, nullptr, 0, keep ? &fa : nullptr, vs.m_rows);   // side stream: overlaps the text layers ahead of the first co-attention
         }
         if (do_v && ln_fold && fold_out_v.count("E") != 0) vs.pend = &vemb_ln;
 
@@ -1072,14 +1110,14 @@ struct vb200_engine {
             {
                 FoldArgs fa = fold_in_args(st, cur);
                 add_linear(pl, st.b16[cur], M, hid, L.qkv, vb::kActNone, nullptr, 0, nullptr, qb, 3 * hid, qf, 3 * hid, stream, Op::NONE,
-                           nullptr, 0, st.pend ? &fa : nullptr);
+                           nullptr, 0, st.pend ? &fa : nullptr, st.m_rows);
             }
             if (!x3) {
                 Op a{};
                 a.kind = Op::SELF_ATTN;
                 a.stream = stream;
                 a.qkv_a = qb; a.ld_a = 3 * hid; a.hidden = hid; a.mask_a = st.mask; a.ctx_a = st.ctx; a.ld_ctx_a = hid;
-                a.B = B; a.La = st.seq; a.heads = heads; a.head_dim = hid / heads;
+                a.B = B; a.La = st.seq; a.heads = heads; a.head_dim = hid / heads; a.offs_a = st.offs;
                 a.flops = 4.0 * B * heads * st.seq * st.seq * (hid / heads);
                 pl.flops += a.flops;
                 ops.push_back(a);
@@ -1092,7 +1130,7 @@ struct vb200_engine {
             {
                 FoldArgs fa = fold_in_args(st, 1 - cur);
                 add_linear(pl, st.b16[1 - cur], M, hid, L.inter, vb::kActGelu, nullptr, 0, nullptr, st.inter, inter, nullptr, 0, stream,
-                           Op::NONE, nullptr, 0, ln_fold ? &fa : nullptr);
+                           Op::NONE, nullptr, 0, ln_fold ? &fa : nullptr, st.m_rows);
             }
             // FFN output + LayerNorm2 (residual: LayerNorm1's output) -> buffers [cur]
             ln_linear(st, st.inter, inter, L.out, L.ln2, 1 - cur, ln_fold ? &L.ln1 : nullptr, cur, keep_out, Op::NONE);
@@ -1123,9 +1161,9 @@ struct vb200_engine {
                 {
                     FoldArgs fv = fold_in_args(vs, vcur), ft = fold_in_args(ts, tcur);
                     add_linear(pl, pl.v_b16[vcur], Mv, Hv, W.qkv_img, vb::kActNone, nullptr, 0, nullptr, qvb, 3 * Hb, qvf, 3 * Hb, 1, Op::NONE,
-                               nullptr, 0, vs.pend ? &fv : nullptr);
+                               nullptr, 0, vs.pend ? &fv : nullptr, vs.m_rows);
                     add_linear(pl, pl.t_b16[tcur], Mt, H, W.qkv_txt, vb::kActNone, nullptr, 0, nullptr, qtb, 3 * Hb, qtf, 3 * Hb, 0, Op::NONE,
-                               nullptr, 0, ts.pend ? &ft : nullptr);
+                               nullptr, 0, ts.pend ? &ft : nullptr, ts.m_rows);
                 }
                 const size_t first_co = ops.size();
                 if (!x3) {
@@ -1133,7 +1171,7 @@ struct vb200_engine {
                     a.kind = Op::CO_ATTN;
                     a.qkv_a = qvb; a.ld_a = 3 * Hb; a.qkv_b = qtb; a.ld_b = 3 * Hb; a.hidden = Hb;
                     a.mask_a = pl.mask_v; a.mask_b = pl.mask_t; a.ctx_a = ctx_t; a.ld_ctx_a = Hb; a.ctx_b = ctx_v; a.ld_ctx_b = Hb;
-                    a.B = B; a.La = T; a.Lb = V; a.heads = c.bi_heads; a.head_dim = Hb / c.bi_heads;
+                    a.B = B; a.La = T; a.Lb = V; a.heads = c.bi_heads; a.head_dim = Hb / c.bi_heads; a.offs_a = offs_t; a.offs_b = offs_v;
                     a.flops = 8.0 * B * c.bi_heads * T * V * (Hb / c.bi_heads);
                     pl.flops += a.flops;
                     ops.push_back(a);
@@ -1152,7 +1190,7 @@ struct vb200_engine {
                 {
                     FoldArgs fa = fold_in_args(vs, 1 - vcur);
                     add_linear(pl, pl.v_b16[1 - vcur], Mv, Hv, W.v_inter, vb::kActGelu, nullptr, 0, nullptr, inter_v, c.v_inter, nullptr, 0, 1,
-                               Op::NONE, nullptr, 0, ln_fold ? &fa : nullptr);
+                               Op::NONE, nullptr, 0, ln_fold ? &fa : nullptr, vs.m_rows);
                 }
                 ln_linear(vs, inter_v, c.v_inter, W.v_out, W.v_ln, 1 - vcur, ln_fold ? &W.ln1 : nullptr, vcur, keep_v, Op::NONE);
                 vs.pend = keep_v ? &W.v_ln : nullptr;
@@ -1161,7 +1199,7 @@ struct vb200_engine {
                 {
                     FoldArgs fa = fold_in_args(ts, 1 - tcur);
                     add_linear(pl, pl.t_b16[1 - tcur], Mt, H, W.t_inter, vb::kActGelu, nullptr, 0, nullptr, inter_t, c.inter, nullptr, 0, 0,
-                               Op::NONE, nullptr, 0, ln_fold ? &fa : nullptr);
+                               Op::NONE, nullptr, 0, ln_fold ? &fa : nullptr, ts.m_rows);
                 }
                 ln_linear(ts, inter_t, c.inter, W.t_out, W.t_ln, 1 - tcur, ln_fold ? &W.ln2 : nullptr, tcur, keep_t, Op::NONE);
                 ts.pend = keep_t ? &W.t_ln : nullptr;
@@ -1238,10 +1276,26 @@ struct vb200_engine {
         float* pooled_t = pl.mem.alloc_n<float>(static_cast<size_t>(B) * Hb);
         float* pooled = pl.mem.alloc_n<float>(static_cast<size_t>(B) * Hb);
         bf16* pooled_b = pl.mem.alloc_n<bf16>(static_cast<size_t>(B) * Hb * S);
-        {
+        if (pl.packed) {
+            // a sample's first row sits at a per-call offset, not at a fixed stride: gather the B first rows of each stream into
+            // compact [B, hidden] operands for the poolers
+            bf16* first_t = pl.mem.alloc_n<bf16>(static_cast<size_t>(B) * H * S);
+            bf16* first_v = pl.mem.alloc_n<bf16>(static_cast<size_t>(B) * Hv * S);
+            Op g{};
+            g.kind = Op::GATHER; g.sync = Op::JOIN; g.B = B;
+            g.qkv_a = pl.t_b16[tc]; g.ctx_a = first_t; g.ld_a = static_cast<int>(H * S); g.offs_a = pl.offs_t(); g.M = Mt;
+            ops.push_back(g);
+            g.sync = Op::NONE;
+            g.qkv_a = pl.v_b16[vc]; g.ctx_a = first_v; g.ld_a = static_cast<int>(Hv * S); g.offs_a = pl.offs_v(); g.M = Mv;
+            ops.push_back(g);
+            add_linear(pl, first_t, B, H, t_pool, vb::kActRelu, nullptr, 0, nullptr, nullptr, 0, pooled_t, Hb, 0, Op::NONE);
+            add_linear(pl, first_v, B, Hv, v_pool, vb::kActRelu, nullptr, 0, nullptr, pooled_b, Hb, pooled, Hb, 0, Op::NONE, pooled_t, Hb);
+        } else {
             add_linear(pl, pl.t_b16[tc], B, static_cast<int64_t>(T) * H, t_pool, vb::kActRelu, nullptr, 0, nullptr, nullptr, 0, pooled_t, Hb, 0, Op::JOIN);
             add_linear(pl, pl.v_b16[vc], B, static_cast<int64_t>(V) * Hv, v_pool, vb::kActRelu, nullptr, 0, nullptr, pooled_b, Hb, pooled, Hb, 0, Op::NONE, pooled_t, Hb);
         }
+        const int* rows_t = pl.packed ? pl.rows_t() : nullptr;
+        const int* rows_v = pl.packed ? pl.rows_v() : nullptr;
         pl.outs[11] = OutBuf{pooled, B, Hb, Hb};
         auto cls_head = [&](const ClsW& w, int n_out, int slot) {
             bf16* hid = pl.mem.alloc_n<bf16>(static_cast<size_t>(B) * 2 * Hb * S);
@@ -1274,23 +1328,27 @@ struct vb200_engine {
         }
         if (select & VB200_OUT_VISION_PREDICTION) {
             bf16* hid = pl.mem.alloc_n<bf16>(static_cast<size_t>(Mv) * Hv * S);
-            add_linear(pl, pl.v_b16[vc], Mv, Hv, img_transform, vb::kActGelu, nullptr, 0, &img_ln, hid, Hv, nullptr, 0);
+            add_linear(pl, pl.v_b16[vc], Mv, Hv, img_transform, vb::kActGelu, nullptr, 0, &img_ln, hid, Hv, nullptr, 0, 0, Op::NONE,
+                       nullptr, 0, nullptr, rows_v);
             pl.outs[5] = make_out(pl, Mv, c.v_target);
-            add_linear(pl, hid, Mv, Hv, img_decoder, vb::kActNone, nullptr, 0, nullptr, nullptr, 0, pl.outs[5].p, pl.outs[5].ld);
+            add_linear(pl, hid, Mv, Hv, img_decoder, vb::kActNone, nullptr, 0, nullptr, nullptr, 0, pl.outs[5].p, pl.outs[5].ld, 0, Op::NONE,
+                       nullptr, 0, nullptr, rows_v);
         }
         if (select & VB200_OUT_VISION_LOGIT) {
             pl.outs[6] = make_out(pl, Mv, 1);
-            ops.push_back(rowdot_op(pl.v_f32[vc], Hv, vision_logit, pl.mask_v, pl.outs[6].p, pl.outs[6].ld, Mv));
+            ops.push_back(rowdot_op(pl.v_f32[vc], Hv, vision_logit, pl.mask_v, pl.outs[6].p, pl.outs[6].ld, Mv, rows_v));
         }
         if (select & VB200_OUT_LINGUISIC_PREDICTION) {
             bf16* hid = pl.mem.alloc_n<bf16>(static_cast<size_t>(Mt) * H * S);
-            add_linear(pl, pl.t_b16[tc], Mt, H, lm_transform, vb::kActGelu, nullptr, 0, &lm_ln, hid, H, nullptr, 0);
+            add_linear(pl, pl.t_b16[tc], Mt, H, lm_transform, vb::kActGelu, nullptr, 0, &lm_ln, hid, H, nullptr, 0, 0, Op::NONE,
+                       nullptr, 0, nullptr, rows_t);
             pl.outs[7] = make_out(pl, Mt, c.vocab);
-            add_linear(pl, hid, Mt, H, lm_decoder, vb::kActNone, nullptr, 0, nullptr, nullptr, 0, pl.outs[7].p, pl.outs[7].ld);
+            add_linear(pl, hid, Mt, H, lm_decoder, vb::kActNone, nullptr, 0, nullptr, nullptr, 0, pl.outs[7].p, pl.outs[7].ld, 0, Op::NONE,
+                       nullptr, 0, nullptr, rows_t);
         }
         if (select & VB200_OUT_LINGUISIC_LOGIT) {
             pl.outs[8] = make_out(pl, Mt, 1);
-            ops.push_back(rowdot_op(pl.t_f32[tc], H, ling_logit, nullptr, pl.outs[8].p, pl.outs[8].ld, Mt));
+            ops.push_back(rowdot_op(pl.t_f32[tc], H, ling_logit, nullptr, pl.outs[8].p, pl.outs[8].ld, Mt, rows_t));
         }
     }
 
@@ -1317,17 +1375,17 @@ struct vb200_engine {
                 break;
             case Op::SELF_ATTN:
                 CUDA_CHECK(vb::launch_self_attention(op.qkv_a, op.ld_a, op.hidden, op.mask_a, op.ctx_a, op.ld_ctx_a, op.B, op.La,
-                                                     op.heads, op.head_dim, light_pdl(), opt.act_fp16, st));
+                                                     op.heads, op.head_dim, light_pdl(), opt.act_fp16, st, op.offs_a));
                 break;
             case Op::CO_ATTN:
                 CUDA_CHECK(vb::launch_co_attention(op.qkv_a, op.ld_a, op.qkv_b, op.ld_b, op.hidden, op.mask_a, op.mask_b, op.ctx_a,
                                                    op.ld_ctx_a, op.ctx_b, op.ld_ctx_b, op.B, op.La, op.Lb, op.heads, op.head_dim,
-                                                   light_pdl(), opt.act_fp16, st));
+                                                   light_pdl(), opt.act_fp16, st, op.offs_a, op.offs_b));
                 break;
             case Op::LAYERNORM:
                 CUDA_CHECK(vb::launch_ln_residual(op.ln_y, op.ln_ld, op.ln_res, op.ld_x, op.ln_g, op.ln_b, cfg.ln_eps, op.ln_out_f,
                                                   op.ld_out, op.ln_out_h, op.ld_a, op.ln_M, op.ln_N, opt.act_fp16, x3 ? 1 : 0,
-                                                  light_pdl(), st, op.ln_pend.stats ? &op.ln_pend : nullptr));
+                                                  light_pdl(), st, op.ln_pend.stats ? &op.ln_pend : nullptr, op.m_rows));
                 break;
             case Op::ATTN_F32:
                 CUDA_CHECK(vb::launch_attention_f32(op.f_q, op.f_ld_q, op.f_k, op.f_v, op.f_ld_kv, op.f_in, op.f_mask, op.B, op.f_Lq,
@@ -1335,7 +1393,12 @@ struct vb200_engine {
                                                     light_pdl(), st));
                 break;
             case Op::ROWDOT:
-                CUDA_CHECK(vb::launch_rowdot(op.x, op.ld_x, op.W, op.bias, op.add, op.out, op.ld_out, op.M, op.K, op.n_out, opt.use_pdl, st));
+                CUDA_CHECK(vb::launch_rowdot(op.x, op.ld_x, op.W, op.bias, op.add, op.out, op.ld_out, op.M, op.K, op.n_out, opt.use_pdl, st,
+                                             op.m_rows));
+                break;
+            case Op::GATHER:
+                CUDA_CHECK(vb::launch_gather_state(op.offs_a, op.M, nullptr, op.qkv_a, nullptr, nullptr, op.ctx_a, nullptr, op.B, 1,
+                                                   op.ld_a, op.ld_a, st));
                 break;
         }
     }
@@ -1518,6 +1581,28 @@ struct vb200_engine {
                                           pl.B, pl.V - 1, c.v_feat, pl.kp, opt.act_fp16, x3 ? 1 : 0, st));
         run_plan(pl, st);
     }
+    // Packed batch (PlanMode PACKED): offsets and row totals go to the plan's d_meta through its pinned staging buffer, ahead of the
+    // graph on the same stream; the pack kernels then run on the real rows only and zero the operand rows up to the next 128-row
+    // boundary (the rest of the last GEMM tile that holds a real row, the only rows past the totals a GEMM loads).
+    void forward_packed(Plan& pl, const vb200_packed_inputs& in, const std::vector<int>& meta, cudaStream_t st) {
+        const Config& c = cfg;
+        const int B = pl.B, rows_t = meta[2 * (B + 1)], rows_v = meta[2 * (B + 1) + 1];
+        CUDA_CHECK(cudaEventSynchronize(pl.meta_copied));           // the previous call's copy has left the staging buffer
+        memcpy(pl.h_meta, meta.data(), meta.size() * sizeof(int));
+        CUDA_CHECK(cudaMemcpyAsync(pl.d_meta, pl.h_meta, meta.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+        CUDA_CHECK(cudaEventRecord(pl.meta_copied, st));
+        auto zero_tail = [&](bf16* buf, int rows, int cap, size_t width) {
+            const int end = std::min(cap, (rows + 127) / 128 * 128);
+            if (end > rows) CUDA_CHECK(cudaMemsetAsync(buf + static_cast<size_t>(rows) * width, 0, static_cast<size_t>(end - rows) * width * 2, st));
+        };
+        CUDA_CHECK(vb::launch_text_embed(in.question, in.segment_ids, nullptr, in.task_tokens, word, pos, type, task, emb_ln.g, emb_ln.b,
+                                         c.ln_eps, pl.t_f32[0], pl.t_b16[0], pl.mask_t, B, 0, c.hidden, c.vocab, c.max_pos, c.type_vocab,
+                                         c.n_task, c.task_tokens, opt.act_fp16, 0, st, pl.offs_t(), rows_t));
+        zero_tail(pl.t_b16[0], rows_t, B * pl.T, c.hidden);
+        CUDA_CHECK(vb::launch_image_pack(in.features, in.spatials, nullptr, pl.img_a, pl.mask_v, rows_v, c.v_feat, pl.kp, opt.act_fp16, 0, st));
+        zero_tail(pl.img_a, rows_v, B * pl.V, pl.kp);
+        run_plan(pl, st);
+    }
     // ---- retrieval reuse (PlanMode): per-caption / per-image prefixes and the pair suffix
     void encode_text(int n, int Tin, const int64_t* q, const int64_t* seg, const int64_t* im, const int64_t* tk, float* st_f32,
                      void* st_16, float* st_mask, cudaStream_t st) {
@@ -1565,14 +1650,18 @@ struct vb200_engine {
         }
         return nullptr;
     }
-    void copy_outputs(Plan& pl, const vb200_outputs& out, cudaStream_t st, cudaMemcpyKind kind) {
+    // rows_t / rows_v (packed plans): the call's row totals -- the per-row outputs hold that many packed rows
+    void copy_outputs(Plan& pl, const vb200_outputs& out, cudaStream_t st, cudaMemcpyKind kind, int rows_t = 0, int rows_v = 0) {
         for (int s = 0; s < 12; ++s) {
             float* dst = out_ptr(out, s);
             const OutBuf& o = pl.outs[s];
             if (dst == nullptr) continue;
             if (o.p == nullptr) fail(VB200_ERR_INVALID, "output slot %d requested but not selected in the `select` mask", s);
+            int rows = o.rows;
+            if (pl.packed && (s == 5 || s == 6 || s == 10)) rows = rows_v;
+            if (pl.packed && (s == 7 || s == 8 || s == 9)) rows = rows_t;
             CUDA_CHECK(cudaMemcpy2DAsync(dst, static_cast<size_t>(o.cols) * 4, o.p, static_cast<size_t>(o.ld) * 4,
-                                         static_cast<size_t>(o.cols) * 4, o.rows, kind, st));
+                                         static_cast<size_t>(o.cols) * 4, rows, kind, st));
         }
         if (out.attention_probs != nullptr) {
             if (pl.attn.empty()) fail(VB200_ERR_INVALID, "attention_probs requested but VB200_OUT_ATTENTION is not set in `select`");
@@ -1706,6 +1795,49 @@ int vb200_forward_slot(vb200_handle h, const vb200_inputs* in, const vb200_outpu
         cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
         h->forward_device(*pl, *in, st);
         h->copy_outputs(*pl, *out, st, cudaMemcpyDeviceToDevice);
+    });
+}
+
+int vb200_forward_packed(vb200_handle h, const vb200_packed_inputs* in, const vb200_outputs* out, uint32_t select, int32_t slot,
+                         void* cuda_stream) {
+    if (h == nullptr) return VB200_ERR_INVALID;
+    return guard(h, [&] {
+        if (in == nullptr || out == nullptr) fail(VB200_ERR_INVALID, "inputs/outputs struct is NULL");
+        if (select & VB200_OUT_ATTENTION) fail(VB200_ERR_INVALID, "packed batches: the attention-probability output (VB200_OUT_ATTENTION) is not supported");
+        if (h->x3) fail(VB200_ERR_INVALID, "packed batches are not supported in split_fp32 (fp32x) mode");
+        const Config& c = h->cfg;
+        const int B = in->batch, task = c.task_tokens ? 1 : 0;
+        if (B < 1) fail(VB200_ERR_INVALID, "packed batches: batch must be positive");
+        if (in->max_tokens < 0 || in->max_regions < 0) fail(VB200_ERR_INVALID, "packed batches: negative capacity");
+        if (!in->n_tokens || !in->n_regions || !in->question || !in->segment_ids || !in->features || !in->spatials || (task && !in->task_tokens))
+            fail(VB200_ERR_INVALID, "vb200_packed_inputs has a NULL required pointer");
+        // meta = text row offsets [B + 1] | image row offsets [B + 1] | text rows | image rows (the plan's d_meta layout)
+        std::vector<int> meta(2 * (static_cast<size_t>(B) + 1) + 2, 0);
+        int max_tin = 0, max_v = 0;
+        for (int b = 0; b < B; ++b) {
+            const int tin = in->n_tokens[b], v = in->n_regions[b];
+            if (tin < 1 || v < 1) fail(VB200_ERR_INVALID, "packed batches: sample %d has n_tokens %d, n_regions %d (both must be >= 1)", b, tin, v);
+            if ((in->max_tokens > 0 && tin > in->max_tokens) || (in->max_regions > 0 && v > in->max_regions))
+                fail(VB200_ERR_INVALID, "packed batches: sample %d (n_tokens %d, n_regions %d) exceeds the capacity (max_tokens %d, max_regions %d)",
+                     b, tin, v, in->max_tokens, in->max_regions);
+            if (tin + task > 256 || v > 256)
+                fail(VB200_ERR_INVALID, "packed batches: sample %d too long for the small-sequence attention kernels (T=%d, V=%d, max 256)", b, tin + task, v);
+            if (tin > c.max_pos) fail(VB200_ERR_INVALID, "packed batches: sample %d has n_tokens %d > max_position_embeddings %d", b, tin, c.max_pos);
+            meta[b + 1] = meta[b] + tin + task;
+            meta[B + 1 + b + 1] = meta[B + 1 + b] + v;
+            max_tin = std::max(max_tin, tin);
+            max_v = std::max(max_v, v);
+        }
+        meta[2 * (B + 1)] = meta[B];
+        meta[2 * (B + 1) + 1] = meta[2 * B + 1];
+        const int t_cap = (in->max_tokens > 0 ? in->max_tokens : max_tin) + task, v_cap = in->max_regions > 0 ? in->max_regions : max_v;
+        if (t_cap > 256 || v_cap > 256) fail(VB200_ERR_INVALID, "packed batches: capacity above 256 rows per sample (T=%d, V=%d)", t_cap, v_cap);
+        const int t16 = (t_cap + 15) / 16 * 16, v16 = (v_cap + 15) / 16 * 16;     // the attention kernels' pad16 buckets
+        CUDA_CHECK(cudaSetDevice(h->opt.device));
+        Plan* pl = h->get_plan(B, t16 - task, v16, select & VB200_OUT_ALL, slot, vb200_engine::PACKED, false);
+        cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+        h->forward_packed(*pl, *in, meta, st);
+        h->copy_outputs(*pl, *out, st, cudaMemcpyDeviceToDevice, meta[2 * (B + 1)], meta[2 * (B + 1) + 1]);
     });
 }
 
@@ -1980,6 +2112,25 @@ int vb200_linear(const void* x_bf16, int64_t ld_x, const void* w_bf16, int64_t l
         if (!pair && !ln && !(ts && strcmp(ts, "0") == 0)) { setup_tma_store(&tc, e); e.tmap_c_host = e.tma_store ? &tc : nullptr; }
         if (pair) CUDA_CHECK(vb::launch_gemm_pair(ta, tb, e, bn, static_cast<cudaStream_t>(cuda_stream)));
         else CUDA_CHECK(vb::launch_gemm_persistent(ta, tb, e, bn, ln, static_cast<cudaStream_t>(cuda_stream)));
+    });
+}
+
+int vb200_linear_rows(const void* x16, int64_t ld_x, const void* w16, int64_t ld_w, const float* bias, int32_t act, void* y16,
+                      int64_t ld_y16, float* y_f32, int64_t ld_y_f32, int64_t M, int64_t N, int64_t K, int32_t block_n, int32_t act_fp16,
+                      const int32_t* m_rows, void* cuda_stream) {
+    return op_guard([&] {
+        if (m_rows == nullptr) fail(VB200_ERR_INVALID, "vb200_linear_rows: m_rows is NULL");
+        const int bn = block_n > 0 ? block_n : vb::gemm_p_pick_block_n(static_cast<int>(N), false);
+        if (bn != 64 && bn != 128 && bn != 192) fail(VB200_ERR_INVALID, "vb200_linear_rows: block_n %d (plain tiles are 64, 128 or 192 wide)", bn);
+        CUtensorMap ta = make_tmap(x16, M, K, ld_x, 128, act_fp16 != 0);
+        CUtensorMap tb = make_tmap(w16, N, K, ld_w, bn, act_fp16 != 0);
+        GemmEpilogue e{};
+        e.M = (int)M; e.N = (int)N; e.K = (int)K; e.bias = bias; e.act = act; e.a_f16 = act_fp16 ? 1 : 0; e.out_f16 = e.a_f16;
+        e.out_bf16 = static_cast<bf16*>(y16); e.ld_bf16 = (int)ld_y16; e.out_f32 = y_f32; e.ld_f32 = (int)ld_y_f32; e.m_rows = m_rows;
+        CUtensorMap tc;
+        setup_tma_store(&tc, e);
+        e.tmap_c_host = e.tma_store ? &tc : nullptr;
+        CUDA_CHECK(vb::launch_gemm_persistent(ta, tb, e, bn, false, static_cast<cudaStream_t>(cuda_stream)));
     });
 }
 

@@ -35,13 +35,15 @@ constexpr int kMmaK = 16;
 // activation whose LayerNorm is still pending, 5 ("LNOUT") produces one.  MODE 8 ("PAIR", plain epilogue): the CTA pair -- two CTAs
 // of a cluster take the vertically adjacent 128 x BLOCK_N tiles of one 256-row panel; each loads its own A rows and HALF of the
 // weight tile, which the TMA multicasts into both CTAs, so every weight byte crosses L2 -> SM once per 256 output rows.
-// MODE 0 also comes 192 wide (96 accumulators per consumer thread, a 2-stage ring): 128 x 192 tiles cover an N = 3072 GEMM in
+// MODE 6 ("ROWS"): MODE 0 whose tile list ends at a device row count (GemmEpilogue::m_rows, packed batches) -- a variant of its
+// own so that MODE 0 keeps its register allocation.
+// MODE 0 and 6 also come 192 wide (96 accumulators per consumer thread, a 2-stage ring): 128 x 192 tiles cover an N = 3072 GEMM in
 // 16 column tiles instead of 24.
 // One CTA per SM: each consumer thread holds BLOCK_N / 2 fp32 accumulators, and the deposited tile plus a ring deep enough to
 // cover the L2 latency take most of the 227 KB of shared memory.
 template <int BLOCK_N, bool LN, int MODE = 0>
 struct PCfg {
-    static_assert(BLOCK_N == 64 || BLOCK_N == 128 || (LN && BLOCK_N == 96) || (!LN && MODE == 0 && BLOCK_N == 192),
+    static_assert(BLOCK_N == 64 || BLOCK_N == 128 || (LN && BLOCK_N == 96) || (!LN && (MODE == 0 || MODE == 6) && BLOCK_N == 192),
                   "tile widths: 64 / 128 (LayerNorm also 96, the default plain kernel also 192)");
     static constexpr bool PAIR = MODE == 8;
     static_assert(!PAIR || (BLOCK_N == 128 && !LN), "the CTA pair is the plain 128-wide tile");
@@ -437,7 +439,15 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
     // cluster takes the 128 rows 256 * panel + 128 r (a last odd panel leaves rank 1 all rows >= M: it still loads and
     // multicasts its half of W, and its zero-filled rows are never stored).
     constexpr bool PAIR = Cfg::PAIR;
-    const int total_tiles = LN ? num_m_tiles : (PAIR ? (num_m_tiles + 1) / 2 : num_m_tiles) * num_n_tiles;
+    // Packed batches (p.m_rows): the producer and the consumers derive the same, shorter tile list from the device row count --
+    // M tiles whose first row is at or past it do not exist for this launch.  The count is written before the graph starts.  A CTA
+    // left without a tile triggers its dependents by exiting.
+    int run_m_tiles = num_m_tiles;
+    if constexpr (MODE == 6) {
+        const int mr = max(0, min(*p.m_rows, p.M));
+        run_m_tiles = min(num_m_tiles, (mr + kBlockM - 1) / kBlockM);
+    }
+    const int total_tiles = LN ? num_m_tiles : (PAIR ? (num_m_tiles + 1) / 2 : run_m_tiles) * num_n_tiles;
     const int first_tile = LN ? static_cast<int>(blockIdx.y) : static_cast<int>(PAIR ? blockIdx.x >> 1 : blockIdx.x);
     const int tile_stride = LN ? static_cast<int>(gridDim.y) : static_cast<int>(PAIR ? gridDim.x >> 1 : gridDim.x);
     const uint32_t cluster_size = (LN || PAIR) ? cluster_nctarank() : 1u;

@@ -70,12 +70,13 @@ cudaError_t launch_gemm_persistent_plain(const CUtensorMap& ta, const CUtensorMa
             return cudaErrorInvalidValue;
         return dispatch_fold<128>(ta, tb, ep, st);
     }
+    const bool rows = ep.m_rows != nullptr;          // MODE 6: the tile list ends at a device row count (packed batches)
     switch (block_n) {
-        case 64: return dispatch_act<64, 0>(ta, tb, ep, st);
-        case 128: return dispatch_act<128, 0>(ta, tb, ep, st);
+        case 64: return rows ? dispatch_act<64, 6>(ta, tb, ep, st) : dispatch_act<64, 0>(ta, tb, ep, st);
+        case 128: return rows ? dispatch_act<128, 6>(ta, tb, ep, st) : dispatch_act<128, 0>(ta, tb, ep, st);
         case 192:                                    // 128x192 tiles, 2-stage ring
             if (ep.N % 192 != 0) return cudaErrorInvalidValue;
-            return dispatch_act<192, 0>(ta, tb, ep, st);
+            return rows ? dispatch_act<192, 6>(ta, tb, ep, st) : dispatch_act<192, 0>(ta, tb, ep, st);
     }
     return cudaErrorInvalidValue;
 }

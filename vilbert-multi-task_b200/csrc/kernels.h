@@ -49,6 +49,11 @@ struct GemmEpilogue {
     int ln_mode;                  // 0 none, 4 fold-in (consumer), 5 pre-LayerNorm output + statistics (producer)
     int debug;                    // timing decomposition only (VB200_DEBUG through vb200_linear): 1 = issue no MMA, 2 = no epilogue
                                   // stores, 4 = no operand loads (the ring is "filled" by plain arrives); results are garbage
+    const int* m_rows;            // optional device row count (packed batches): rows >= min(*m_rows, M) are neither loaded nor
+                                  // computed -- the tile list ends at the last 128-row tile holding a row below it.  Written
+                                  // before the launch's graph starts, so it is read ahead of griddepcontrol.wait.  Honoured by
+                                  // the plain persistent kernel (PCfg MODE 6 in place of MODE 0); the fp32-parity, LayerNorm
+                                  // fold, cluster-LayerNorm, pair and chain kernels compute every row.
 };
 
 // persistent CTAs / clusters, wgmma consumer warpgroups, single-exchange LayerNorm (gemm_persistent.cuh)
@@ -71,13 +76,16 @@ cudaError_t launch_gemm_persistent_plain(const CUtensorMap& tmap_a, const CUtens
 // K4: softmax(Q K^T / sqrt(d) + mask) V per (sample, head); qkv row = [Q | K | V], each `hidden` wide.
 cudaError_t launch_self_attention(const __nv_bfloat16* qkv, int ld_qkv, int hidden, const float* key_mask_add,
                                   __nv_bfloat16* ctx, int ld_ctx, int B, int L, int heads, int head_dim, int pdl,
-                                  int f16, cudaStream_t st);
+                                  int f16, cudaStream_t st, const int* offs = nullptr);
+// offs (packed batches, optional): device [B + 1] row offsets; sample b is rows [offs[b], offs[b+1]) of qkv / mask / ctx, and
+// L is the shared-memory capacity (>= every sample's length).  nullptr: sample b is rows [b L, b L + L).
 // K5: both co-attention directions in one kernel.  qkv_img rows = [Q1|K1|V1], qkv_txt rows = [Q2|K2|V2].
 //   ctx_txt[b,t] = softmax(Q2 K1^T / sqrt(d) + img_mask) V1      ctx_img[b,v] = softmax(Q1 K2^T / sqrt(d) + txt_mask) V2
 cudaError_t launch_co_attention(const __nv_bfloat16* qkv_img, int ld_img, const __nv_bfloat16* qkv_txt, int ld_txt,
                                 int hidden, const float* img_mask_add, const float* txt_mask_add,
                                 __nv_bfloat16* ctx_txt, int ld_ctx_txt, __nv_bfloat16* ctx_img, int ld_ctx_img, int B,
-                                int T, int V, int heads, int head_dim, int pdl, int f16, cudaStream_t st);
+                                int T, int V, int heads, int head_dim, int pdl, int f16, cudaStream_t st,
+                                const int* offs_t = nullptr, const int* offs_v = nullptr);   // as launch_self_attention, per stream
 
 // un-fused LayerNorm(y + res): fp32 stream out + 16-bit operand out (layernorm.cu); split16: hi | lo | hi operand (fp32-parity mode)
 struct LnPending {                // a residual whose own LayerNorm is still pending (LayerNorm fold): statistics + parameters
@@ -87,14 +95,20 @@ struct LnPending {                // a residual whose own LayerNorm is still pen
 };
 cudaError_t launch_ln_residual(const float* y, int ld_y, const float* res, int ld_res, const float* gamma, const float* beta,
                                float eps, float* out_f32, int ld_f32, __nv_bfloat16* out16, int ld16, int M, int N, int f16,
-                               int split16, int pdl, cudaStream_t st, const LnPending* res_pending = nullptr);
+                               int split16, int pdl, cudaStream_t st, const LnPending* res_pending = nullptr,
+                               const int* m_rows = nullptr);   // optional device row count: rows >= *m_rows are skipped
 // K2: word + position + token-type gather, task-token row at index 1, LayerNorm; also builds the additive text mask.
 cudaError_t launch_text_embed(const int64_t* ids, const int64_t* seg, const int64_t* input_mask, const int64_t* task,
                               const float* word, const float* pos, const float* type, const float* task_tab,
                               const float* gamma, const float* beta, float eps, float* out_f32,
                               __nv_bfloat16* out_bf16, float* mask_add, int B, int Tin, int H, int vocab, int max_pos,
-                              int n_type, int n_task, int task_tokens, int f16, int split16, cudaStream_t st);
-// K1 (input half): fp32 region features + 5-d boxes -> bf16 GEMM operand [B*V, Kp] = [feat | loc | 0], additive image mask.
+                              int n_type, int n_task, int task_tokens, int f16, int split16, cudaStream_t st,
+                              const int* offs = nullptr, int rows = 0);
+// Packed batches (offs != nullptr): offs = device [B + 1] OUTPUT row offsets (T_b = Tin_b + task_tokens rows per sample), ids / seg
+// hold sample b's Tin_b tokens at offs[b] - b * task_tokens, positions restart at 0 per sample, input_mask is unused (every row is
+// real), `rows` = offs[B] and Tin is ignored.
+// K1 (input half): fp32 region features + 5-d boxes -> bf16 GEMM operand [B*V, Kp] = [feat | loc | 0], additive image mask
+// (image_mask nullptr: every row is real -- packed batches).
 cudaError_t launch_image_pack(const float* feats, const float* loc, const uint8_t* image_mask, __nv_bfloat16* a_out,
                               float* mask_add, int rows, int F, int Kp, int f16, int split16, cudaStream_t st);
 // custom_prediction()'s tensor construction on the device (worker.py:422-455): box features [B, n, F] + pixel boxes [B, n, 4] +
@@ -102,7 +116,8 @@ cudaError_t launch_image_pack(const float* feats, const float* loc, const uint8_
 cudaError_t launch_region_pack(const float* box_feats, const float* boxes, const float* image_wh, const int32_t* num_boxes,
                                __nv_bfloat16* a_out, float* mask_add, float* spatials_out, int B, int n, int F, int Kp, int f16,
                                int split16, cudaStream_t st);
-// retrieval reuse: cached encoder state rows idx[b] -> sample b of a pair plan (fp32 stream [L, H], 16-bit operand [L, H16], mask [L])
+// retrieval reuse: cached encoder state rows idx[b] -> sample b of a pair plan (fp32 stream [L, H], 16-bit operand [L, H16], mask [L]);
+// the fp32 and mask copies are skipped when their pointers are null (packed poolers: the first 16-bit row of every sample)
 cudaError_t launch_gather_state(const int32_t* idx, int n_src, const float* src_f32, const void* src_16, const float* src_mask,
                                 float* dst_f32, void* dst_16, float* dst_mask, int B, int L, int H, int H16, cudaStream_t st);
 // fp32 CUDA-core attention (attention_f32.cu): in_kind 0 fp32 / 1 fp16 / 2 bf16 Q, K, V; ctx_mode 0 none / 1 fp16 / 2 bf16 /
@@ -112,7 +127,7 @@ cudaError_t launch_attention_f32(const void* q, int ld_q, const void* k, const v
                                  int ctx_mode, float* probs, int pdl, cudaStream_t st);
 // K8 (narrow heads): out[m, j] = dot(x[m, :K], W[j, :K]) + b[j] + (add ? add[m] : 0), j < n_out <= 4.
 cudaError_t launch_rowdot(const float* x, int ld_x, const float* W, const float* b, const float* add, float* out,
-                          int ld_out, int M, int K, int n_out, int pdl, cudaStream_t st);
+                          int ld_out, int M, int K, int n_out, int pdl, cudaStream_t st, const int* m_rows = nullptr);
 
 // ---- shared host-side launch helpers
 template <typename K>

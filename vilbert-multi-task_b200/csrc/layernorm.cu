@@ -22,11 +22,12 @@ ln_residual_kernel(const float* __restrict__ y, int ld_y, const float* __restric
                    const float2* __restrict__ res_stats, int res_parts, int stats_ld, const float* __restrict__ res_gamma,
                    const float* __restrict__ res_beta,
                    const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
-                   float* __restrict__ out_f32, int ld_f32, uint16_t* __restrict__ out16, int ld16, int M, int N, int pdl) {
+                   float* __restrict__ out_f32, int ld_f32, uint16_t* __restrict__ out16, int ld16, int M, int N, int pdl,
+                   const int* __restrict__ m_rows) {
     if (pdl) pdl_wait();
     const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
-    if (row >= M) return;
+    if (row >= M || (m_rows != nullptr && row >= *m_rows)) return;      // packed batches: rows past the device row count
     const int nvec = NV < kLnMaxVec ? NV : (N >> 7);
     const float4* yp = reinterpret_cast<const float4*>(y + static_cast<size_t>(row) * ld_y);
     const float4* rp = res ? reinterpret_cast<const float4*>(res + static_cast<size_t>(row) * ld_res) : nullptr;
@@ -102,7 +103,7 @@ ln_residual_kernel(const float* __restrict__ y, int ld_y, const float* __restric
 
 cudaError_t launch_ln_residual(const float* y, int ld_y, const float* res, int ld_res, const float* gamma, const float* beta,
                                float eps, float* out_f32, int ld_f32, __nv_bfloat16* out16, int ld16, int M, int N, int f16,
-                               int split16, int pdl, cudaStream_t st, const LnPending* rp) {
+                               int split16, int pdl, cudaStream_t st, const LnPending* rp, const int* m_rows) {
     const float2* res_stats = rp ? rp->stats : nullptr;
     const int res_parts = rp ? rp->parts : 0, stats_ld = rp ? rp->ld : 0;
     const float *res_gamma = rp ? rp->gamma : nullptr, *res_beta = rp ? rp->beta : nullptr;
@@ -117,7 +118,7 @@ cudaError_t launch_ln_residual(const float* y, int ld_y, const float* res, int l
     uint16_t* o16 = reinterpret_cast<uint16_t*>(out16);
 #define VB_LN(F, S, V) launch_ex(ln_residual_kernel<F, S, V>, grid, block, 0, pdl, st, y, ld_y, res, ld_res, res_stats, res_parts, \
                                stats_ld, res_gamma, res_beta, gamma, beta, eps,                                                  \
-                               out_f32, ld_f32, o16, ld16, M, N, pdl)
+                               out_f32, ld_f32, o16, ld16, M, N, pdl, m_rows)
     if (split16) return VB_LN(true, true, kLnMaxVec);
     if (N == 768) return f16 ? VB_LN(true, false, 6) : VB_LN(false, false, 6);
     if (N == 1024) return f16 ? VB_LN(true, false, 8) : VB_LN(false, false, 8);

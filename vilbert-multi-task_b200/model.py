@@ -369,6 +369,61 @@ class VILBertForVLTasks(object):
             L.check(lib.vb200_forward_regions(self._handle, C.byref(inp), C.byref(o), select, slot, C.c_void_p(stream)), self._handle)
         return self._result(outs, B, Tin, n + 1, False), sp
 
+    # ------------------------------------------------------------------ packed variable-length batches
+    @torch.no_grad()
+    def forward_packed(self, question, features, spatials, segment_ids, task_tokens, n_tokens, n_regions,
+                       select: int = L.OUT_TASK_HEADS, slot: int = 0, debug_taps: bool = False, max_tokens: int = 0,
+                       max_regions: int = 0):
+        """One forward of B samples with their own text lengths and region counts, stored back to back without padding:
+        ``question`` / ``segment_ids`` ``[sum Tin_i]``, ``features`` ``[sum V_i, F]``, ``spatials`` ``[sum V_i, 5]``,
+        ``task_tokens`` ``[B, 1]``; ``n_tokens`` / ``n_regions`` (lists or CPU int tensors) give Tin_i and V_i.  Every row is real
+        (no masks).  Returns the 10-tuple: per-sample outputs as in ``forward``, per-row outputs packed (``vision_logit``
+        ``[sum V_i, 1]``, ``linguisic_logit`` ``[sum T_i, 1]`` with T_i = Tin_i + 1, ...), element 9 ``[]``.  ``max_tokens`` /
+        ``max_regions`` (0: this call's maxima) are the plan's capacities: calls with the same batch size and capacities share one
+        plan and CUDA graph whatever their lengths."""
+        if self._handle is None:
+            raise L.VilbertB200Error("call model.cuda(i) first (worker.py:536); there is no CPU path")
+        lib = L.load()
+        device = torch.device("cuda", self._device)
+        nt = [int(x) for x in (n_tokens.tolist() if torch.is_tensor(n_tokens) else n_tokens)]
+        nr = [int(x) for x in (n_regions.tolist() if torch.is_tensor(n_regions) else n_regions)]
+        B = len(nt)
+        if len(nr) != B or B < 1:
+            raise ValueError("forward_packed: n_tokens and n_regions must have the same, positive length")
+
+        def dev(t, dtype):
+            return torch.as_tensor(t).to(device=device, dtype=dtype, non_blocking=True).contiguous()
+        F = self._dims["v_feature_size"]
+        q = dev(question, torch.int64).reshape(-1)
+        seg = dev(segment_ids if segment_ids is not None else torch.zeros_like(q), torch.int64).reshape(-1)
+        f = dev(features, torch.float32).reshape(-1, F)
+        s = dev(spatials, torch.float32).reshape(-1, 5)
+        tk = dev(task_tokens if task_tokens is not None else torch.zeros(B, 1, dtype=torch.int64), torch.int64).reshape(B, -1)[:, :1]
+        tk = tk.contiguous()
+        sum_tin, sum_v = sum(nt), sum(nr)
+        if q.numel() != sum_tin or seg.numel() != sum_tin or f.shape[0] != sum_v or s.shape[0] != sum_v:
+            raise ValueError("forward_packed: question / segment_ids need sum(n_tokens) rows, features / spatials sum(n_regions)")
+        rows_t = sum_tin + (B if self._dims["task_specific_tokens"] else 0)
+        d = self._dims
+        packed = {"vision_prediction": (sum_v, d["v_target_size"]), "vision_logit": (sum_v, 1),
+                  "linguisic_prediction": (rows_t, d["vocab_size"]), "linguisic_logit": (rows_t, 1)}
+        outs = {k: torch.empty(packed.get(k, shape), dtype=torch.float32, device=device)
+                for k, shape in self._out_shapes(B, 1, 1, select).items()}
+        if debug_taps:
+            outs["sequence_output_t"] = torch.empty(rows_t, d["hidden_size"], dtype=torch.float32, device=device)
+            outs["sequence_output_v"] = torch.empty(sum_v, d["v_hidden_size"], dtype=torch.float32, device=device)
+            outs["pooled_output"] = torch.empty(B, d["bi_hidden_size"], dtype=torch.float32, device=device)
+        o = L.Outputs()
+        for k, t in outs.items():
+            setattr(o, k, t.data_ptr())
+        nt_c, nr_c = (C.c_int32 * B)(*nt), (C.c_int32 * B)(*nr)
+        inp = L.PackedInputs(B, int(max_tokens), int(max_regions), C.cast(nt_c, C.c_void_p), C.cast(nr_c, C.c_void_p), q.data_ptr(),
+                             seg.data_ptr(), f.data_ptr(), s.data_ptr(), tk.data_ptr())
+        with torch.cuda.device(device):
+            stream = torch.cuda.current_stream(device).cuda_stream
+            L.check(lib.vb200_forward_packed(self._handle, C.byref(inp), C.byref(o), select, slot, C.c_void_p(stream)), self._handle)
+        return self._result(outs, B, 0, 0, debug_taps)
+
     # ------------------------------------------------------------------ retrieval reuse (SURVEY.md section 8e)
     @torch.no_grad()
     def encode_text(self, question, segment_ids, input_mask, task_tokens):

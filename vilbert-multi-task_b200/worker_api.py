@@ -210,6 +210,80 @@ def prediction_batch(requests, bucket: int = 8, select: Optional[int] = None):
     return answers
 
 
+def _prefix_len(mask_row):
+    """Length of a 0/1 text mask that is a run of ones followed by zeros (>= 1), else None."""
+    m = [int(x) for x in mask_row.tolist()]
+    k = sum(1 for x in m if x != 0)
+    return k if k >= 1 and all(x == 1 for x in m[:k]) and all(x == 0 for x in m[k:]) else None
+
+
+def prediction_packed(requests, bucket: int = 8, select: Optional[int] = None):
+    """`prediction_batch` in ONE model call whatever the requests' shapes: a packed variable-length batch
+    (`model.forward_packed`).  Padded text tokens are dropped (the `input_mask` must be a prefix of ones), region rows are kept
+    as given (the `image_mask` must be all ones); a request that breaks either rule, or fails validation, gets a `ValueError` /
+    its exception as its answer.  NLVR2 pairs go on even rows and the batch is padded to a multiple of `bucket`, both with
+    filler rows of one token and one region.  The plan capacities are the widest padded text and the most regions among the
+    requests (37 tokens from the worker's tokenizer), so a long-running worker sees one plan per batch bucket."""
+    if bucket < 1:
+        raise ValueError("bucket must be >= 1")
+    fixed_select = L.OUT_TASK_HEADS if select is None else int(select)
+    answers = [None] * len(requests)
+    samples, spans, need = [], {}, 0            # samples: (tokens [Tin], segments [Tin], task [1], features [V, F], spatials [V, 5])
+    max_tin, max_v, F, dev = 1, 1, None, None
+    for i, r in enumerate(requests):
+        (question, features, spatials, segment_ids, input_mask, image_mask, co_mask, task_tokens, task_id, infos) = r
+        try:
+            _validate(task_id, infos)
+            if image_mask is not None and not bool((image_mask != 0).all()):
+                raise ValueError("prediction_packed: image_mask must be all ones (packed rows are all real)")
+            q, im, seg, tk = _expand_text(task_id, features.size(0), question, input_mask, segment_ids, task_tokens)
+            lens = [_prefix_len(im[j]) for j in range(features.size(0))]
+            if any(k is None for k in lens):
+                raise ValueError("prediction_packed: input_mask must be a prefix of ones")
+        except (AssertionError, ValueError) as e:
+            answers[i] = e
+            continue
+        F, dev = features.size(2), features.device
+        if task_id == "12" and len(samples) % 2 == 1:
+            samples.append(None)                    # filler: the pair starts on an even row
+        spans[i] = (len(samples), len(samples) + features.size(0))
+        for j, k in enumerate(lens):
+            samples.append((q[j, :k], seg[j, :k], tk[j].reshape(1), features[j], spatials[j]))
+        max_tin, max_v = max(max_tin, q.size(1)), max(max_v, features.size(1))
+        need |= TASK_OUTPUT[task_id]
+    if not spans:
+        return answers
+    sel = fixed_select | need
+    target = -(-len(samples) // bucket) * bucket
+    if target % 2 == 1 and (sel & L.OUT_VIL_BINARY_PREDICTION):
+        target += 1                                  # the binary head needs an even number of rows
+    samples += [None] * (target - len(samples))
+    filler = (torch.zeros(1, dtype=torch.long, device=dev), torch.zeros(1, dtype=torch.long, device=dev),
+              torch.zeros(1, dtype=torch.long, device=dev), torch.zeros(1, F, device=dev), torch.zeros(1, 5, device=dev))
+    samples = [filler if smp is None else smp for smp in samples]
+    cat = [torch.cat([smp[k] for smp in samples], dim=0) for k in range(5)]
+    n_tokens = [int(smp[0].numel()) for smp in samples]
+    n_regions = [int(smp[3].shape[0]) for smp in samples]
+    with model_lock:
+        out = model.forward_packed(cat[0], cat[3], cat[4], cat[1], cat[2].view(-1, 1), n_tokens, n_regions, select=sel,
+                                   max_tokens=max_tin, max_regions=max_v)
+    t_off = np.concatenate([[0], np.cumsum([n + 1 for n in n_tokens])])   # packed text rows (task token included)
+    v_off = np.concatenate([[0], np.cumsum(n_regions)])
+    for i, (lo, hi) in spans.items():
+        task_id, infos, spatials = requests[i][8], requests[i][9], requests[i][2]
+        sl = [None if o is None or isinstance(o, list) else o[lo:hi] for o in out[:9]] + [[]]
+        if out[3] is not None:
+            sl[3] = out[3][lo // 2:hi // 2] if task_id == "12" else out[3][0:0]
+        for k in (5, 6):                             # per-region rows: [images, V, ...] (the request's images share V)
+            if out[k] is not None:
+                sl[k] = out[k][int(v_off[lo]):int(v_off[hi])].reshape(hi - lo, -1, out[k].shape[-1])
+        for k in (7, 8):                             # per-token rows
+            if out[k] is not None:
+                sl[k] = out[k][int(t_off[lo]):int(t_off[hi])].reshape(hi - lo, -1, out[k].shape[-1])
+        answers[i] = _decode(task_id, tuple(sl), spatials, infos)
+    return answers
+
+
 def build_inputs(query, task, features, infos, device, tok=None):
     """The tensor construction half of custom_prediction (worker.py:402-455), returned instead of consumed."""
     tokens, input_mask, segment_ids = tokenize_query(query, tok)
