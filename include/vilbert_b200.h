@@ -133,12 +133,8 @@ typedef struct {
                                       fp32 accumulator; attention runs in fp32 on CUDA cores; GELU uses the 1.5e-7 erf.  3x the
                                       tensor work of the default mode -- for logit parity with the reference's fp32 forward
                                       (<= 1e-3 per logit, BASELINE.json north_star), not for throughput.  Implies act_fp16. */
-    int32_t ln_fold;               /* 1: LayerNorm folded into the GEMMs around it (default off).  The GEMM that produces
-                                      u = dense(x) + residual writes u (fp32 + 16-bit) and per-row (mean, M2) statistics instead of
-                                      LayerNorm(u); the next GEMM runs on u with weights pre-scaled by gamma and finishes with
-                                      rstd * (acc - mean * s) + c; residual readers rebuild LayerNorm(u) on the fly.  Same math,
-                                      57 of a forward's 62 LayerNorm launches gone, at the cost of heavier GEMM epilogues; an
-                                      option, parity-tested, not the default.  Ignored in split_fp32 / fused_layernorm. */
+    int32_t ln_fold;               /* reserved, must be 0 (was the LayerNorm fold, which is removed; vb200_create returns
+                                      VB200_ERR_INVALID for any other value) */
     int32_t max_plans;             /* plan-cache bound: plans (workspace + CUDA graph per (batch, tokens, regions, select, slot))
                                       beyond this are evicted least-recently-used; 0 -> 24 */
 } vb200_options;
@@ -185,9 +181,7 @@ int vb200_plan_info(vb200_handle h, int32_t batch, int32_t n_tokens, int32_t n_r
 int vb200_model_dim(vb200_handle h, const char* key, int64_t* value);
 /* Run-time knobs: "max_plans" (plan-cache bound); "profile_grid_pct" (0 or 10..100): the NEXT vb200_profile_ops call launches every
  * GEMM with this percentage of the resident CTA slots as its persistent grid --
- * for reporting what a launch does when it has the GPU to itself; forwards are never affected.  "chain_ffn" (0/1): issue every
- * FFN-in -> FFN-out pair as ONE chained persistent launch (csrc/gemm_chain.cu: dynamic tile list + per-row-panel dependency counters;
- * same bits; off by default); changing it drains the device and drops cached plans. */
+ * for reporting what a launch does when it has the GPU to itself; forwards are never affected. */
 int vb200_set_option(vb200_handle h, const char* key, int64_t value);
 /* Profiling: after vb200_set_option(h, "timeline", 1) every persistent GEMM launch of a forward records 16 stamps per CTA (0: clock64 at
  * entry, 1: setup done, 2: first k-block landed [-DVB200_STAMPS builds], 8 / 9: %globaltimer ns at entry / exit, 10: last tile accumulated,
@@ -282,9 +276,9 @@ int vb200_forward_cached(vb200_handle h, int32_t batch, int32_t n_tokens, int32_
 /* y = epilogue(x[M,K] (16-bit) . w[N,K]^T (16-bit)); act: 0 none, 1 GELU(erf), 2 ReLU; LayerNorm applied when gamma != NULL.
  * act_fp16 != 0: x, w and the 16-bit output y are fp16, else bf16 (parameter names keep the historical _bf16 suffix).
  * act 3 = GELU with the 1.5e-7 erf (fp32-parity mode).  variant 0: persistent kernel (gemm_persistent.cuh, what the engine
- * uses); 2: CTA pair (PCfg MODE 8: a cluster of two CTAs shares each weight tile through TMA multicast; plain epilogue, 128-wide
- * tile, N % 128 == 0); 3 and 4 (names of Blackwell occupancy configurations) select the persistent kernel.  Plain (non-LayerNorm)
- * tiles are 64, 128 or 192 columns wide; block_n 256 runs as 128-wide tiles.  Variants 0, 3, 4 and every width give the same bits.
+ * uses); 2, 3 and 4 (names of Blackwell kernel configurations) select the persistent kernel: 2 and 3 with the plain 128-wide tile,
+ * 4 with the plain 128- or 64-wide one.  Plain (non-LayerNorm) tiles are 64, 128 or 192 columns wide; block_n 256 runs as
+ * 128-wide tiles.  Every variant and every width gives the same bits.
  * timing: NULL, or a device buffer of 16 int64 per CTA that receives clock64() / %globaltimer stamps (profiling aid). */
 int vb200_linear(const void* x_bf16, int64_t ld_x, const void* w_bf16, int64_t ld_w, const float* bias,
                  const float* residual, int64_t ld_res, const float* gamma, const float* beta, float eps, int32_t act,
@@ -305,22 +299,6 @@ int vb200_linear_split(const void* x16, int64_t ld_x, const void* w16, int64_t l
 int vb200_layernorm(const float* y, int64_t ld_y, const float* residual, int64_t ld_res, const float* gamma, const float* beta,
                     float eps, float* out_f32, int64_t ld_f32, void* out_16, int64_t ld_16, int64_t M, int64_t N,
                     int32_t act_fp16, void* cuda_stream);
-/* Two dependent GEMMs in one launch (vilbert-multi-task_b200/csrc/gemm_chain.cu): h = act(x w1^T + b1) (16-bit, [M, N1]) and
- * y = h w2^T + b2 ([M, N2], 16-bit and/or fp32).  sync_ints: device memory, M / 128 (rounded up) + 2 ints, zero before the first
- * call (the kernel leaves it zeroed).  Results are bit-identical to two vb200_linear calls. */
-int vb200_linear_chain(const void* x16, int64_t ld_x, const void* w1, int64_t ld_w1, const float* b1, int32_t act, void* h16, int64_t ld_h,
-                       const void* w2, int64_t ld_w2, const float* b2, void* y16, int64_t ld_y16, float* y_f32, int64_t ld_y_f32, int64_t M,
-                       int64_t N1, int64_t K1, int64_t N2, int32_t act_fp16, void* sync_ints, void* cuda_stream);
-/* The GEMM with the LayerNorm fold epilogues (vilbert-multi-task_b200/csrc/gemm_persistent.cuh, row_stats).  Statistics arrays are
- * float2 (mean, M2 = sum (x - mean)^2) per row and 32-column chunk, laid out [N_src / 32][stats_ld].
- * mode 5 (producer): u = x w^T + bias + residual, where the residual is res, or LayerNorm_{res_gamma,res_beta}(res) rebuilt from
- *         res_stats when that is non-NULL; writes u to y_f32 AND y16, and its statistics to out_stats.
- * mode 4 (consumer): x holds such a u, w = gamma o W (16-bit), fold_s[n] = sum_k w[n,k], bias = c;
- *         y = act(rstd * (x w^T - mean * s) + c), mean / rstd from a_stats (a_parts = K_logical / 32). */
-int vb200_linear_ln(const void* x16, int64_t ld_x, const void* w16, int64_t ld_w, const float* bias, int32_t mode, const void* a_stats,
-                    int32_t a_parts, const float* fold_s, const float* res, int64_t ld_res, const void* res_stats, int32_t res_parts,
-                    const float* res_gamma, const float* res_beta, void* out_stats, int32_t stats_ld, float eps, int32_t act, void* y16,
-                    int64_t ld_y16, float* y_f32, int64_t ld_y_f32, int64_t M, int64_t N, int64_t K, int32_t act_fp16, void* cuda_stream);
 /* split16 != 0: out_16 is the fp16 hi | lo | hi operand (stride ld_16 of the 3x wider buffer). */
 int vb200_layernorm_split(const float* y, int64_t ld_y, const float* residual, int64_t ld_res, const float* gamma, const float* beta,
                           float eps, float* out_f32, int64_t ld_f32, void* out_16, int64_t ld_16, int64_t M, int64_t N, void* cuda_stream);

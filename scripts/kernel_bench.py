@@ -48,7 +48,6 @@ def main():
     ap.add_argument("--batch", type=int, default=64)
     ap.add_argument("--act", default="fp16")
     ap.add_argument("--sets", type=int, default=4, help="operand sets cycled through per kernel")
-    ap.add_argument("--variant", type=int, default=0, help="vb200_linear variant: 0 persistent kernel, 2 CTA pair (128-wide tile, N %% 128 == 0)")
     ap.add_argument("--stamps", action="store_true", help="print clock64 phase stamps of the persistent kernel")
     ap.add_argument("--bn", type=int, default=0, help="override block_n of every plain GEMM")
     ap.add_argument("--debug", default="0", help="VB200_DEBUG timing decomposition (comma list, each timed in turn): "
@@ -79,12 +78,8 @@ def main():
     for name, M, N, K, actf, ln, bn in gemms:
         if only and not any(o == name or (o.endswith("*") and o[:-1] in name) for o in only):
             continue
-        if a.variant == 2 and (ln or N % 128 or M < 256):
-            continue
         if a.bn and not ln:
             bn = a.bn
-        if a.variant == 2:
-            bn = 128
         sets = []
         for _ in range(a.sets):
             x = torch.randn(M, K, generator=g, device="cuda").to(act)
@@ -101,7 +96,7 @@ def main():
         def run(i):
             x, w, b, r, ga, be, yb, yf, ldf = sets[i % a.sets]
             rc = lib.vb200_linear(ptr(x), K, ptr(w), K, ptr(b), ptr(r), N if ln else 0, ptr(ga), ptr(be), 1e-12, actf,
-                                  ptr(yb), N, ptr(yf), ldf, M, N, K, bn, 0, f16, a.variant, None, C.c_void_p(cur()))
+                                  ptr(yb), N, ptr(yf), ldf, M, N, K, bn, 0, f16, 0, None, C.c_void_p(cur()))
             L.check(rc, None)
         for dbg in debug_modes:
             os.environ["VB200_DEBUG"] = str(dbg)
@@ -109,11 +104,11 @@ def main():
             fl = 2.0 * M * N * K
             res.append(dict(kernel=name, M=M, N=N, K=K, debug=dbg, us=round(us, 2), tflops=round(fl / us / 1e6, 1)))
             print(json.dumps(res[-1]), flush=True)
-            if a.stamps and a.variant in (0, 2):
+            if a.stamps:
                 tb = torch.zeros(16 * 4096, dtype=torch.int64, device="cuda")
                 x, w, b, r, ga, be, yb, yf, ldf = sets[0]
                 rc = lib.vb200_linear(ptr(x), K, ptr(w), K, ptr(b), ptr(r), N if ln else 0, ptr(ga), ptr(be), 1e-12, actf,
-                                      ptr(yb), N, ptr(yf), ldf, M, N, K, bn, 0, f16, a.variant, ptr(tb), C.c_void_p(cur()))
+                                      ptr(yb), N, ptr(yf), ldf, M, N, K, bn, 0, f16, 0, ptr(tb), C.c_void_p(cur()))
                 L.check(rc, None)
                 torch.cuda.synchronize()
                 t = tb.view(-1, 16).cpu()

@@ -42,7 +42,7 @@ def test_ctypes_structs_match_header_layout():
     assert C.sizeof(L.RegionInputs) == 16 + 9 * 8
 
 
-def _create(cfg, sd, **opt):
+def _create(cfg, sd, ln_fold=0, **opt):
     m = vb.VILBertForVLTasks.from_pretrained(sd, config=cfg, num_labels=opt.pop("num_labels", 40), **opt)
     lib = L.load()
     names = [k.encode() for k in m._sd]
@@ -54,6 +54,7 @@ def _create(cfg, sd, **opt):
     o = L.Options()
     o.num_labels = m.num_labels
     o.strict = 1 if m._opts["strict"] else -1
+    o.ln_fold = ln_fold
     h = C.c_void_p()
     rc = lib.vb200_create(m._config_json(), len(m._sd), arr, C.byref(o), C.byref(h))
     msg = lib.vb200_last_error(None).decode()
@@ -106,6 +107,15 @@ def test_checkpoint_audit_num_labels_mismatch():
     sd = S.synthetic_state_dict(cfg, num_labels=40, gqa_labels=24, seed=1)
     rc, msg = _create(cfg, sd, num_labels=3129)
     assert rc == -3 and "num_labels" in msg
+
+
+def test_reserved_ln_fold_option_rejected():
+    """vb200_options::ln_fold is reserved since the LayerNorm fold was removed: a non-zero value is refused before the checkpoint
+    audit, so with or without a device."""
+    cfg = _tiny_cfg()
+    sd = S.synthetic_state_dict(cfg, num_labels=40, gqa_labels=24, seed=1)
+    rc, msg = _create(cfg, sd, ln_fold=1)
+    assert rc == -1 and "LayerNorm fold was removed" in msg, (rc, msg)
 
 
 def test_checkpoint_legacy_names_accepted():

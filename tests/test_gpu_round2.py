@@ -362,61 +362,6 @@ def test_micro_batch_worker_on_engine(full_oracle, full_h):
             assert r["result"]["confidence_list"] == pytest.approx(w["confidence_list"], abs=0.3)
 
 
-# ----------------------------------------------------------------------------------------------- LayerNorm fold
-def test_layernorm_fold_vs_unfolded_and_oracle(tiny_oracle, full_oracle, parity_log):
-    """ln_fold=True (57 LayerNorms folded into the GEMMs around them) vs the default form (every LayerNorm as GEMM + row kernel):
-    both within the fp16 tolerance of the fp32 oracle, and the launch count of a forward drops accordingly."""
-    from oracle import vilbert_ref as R
-    from vilbert_b200 import _lib as L
-    for tag, oracle, inp in (("tiny", tiny_oracle, _tiny_inputs(tiny_oracle, 3, 30, 36, 91, pad=2)),
-                             ("full", full_oracle, list(R.make_inputs(3, 30, 36, seed=92, pad_regions=2)))):
-        ref = oracle(*inp, compute_pretraining_heads=True)
-        dev = [t.cuda() for t in inp]
-        fold, plain = _engine(oracle, ln_fold=True), _engine(oracle)
-        a = fold(*dev, compute_pretraining_heads=True)
-        b = plain(*dev, compute_pretraining_heads=True)
-        torch.cuda.synchronize()
-        ea, eb = _max_err(ref, a), _max_err(ref, b)
-        for name in ea:
-            parity_log(test="ln_fold_" + tag, output=name, err_fold_vs_fp32=ea[name][0], err_unfolded_vs_fp32=eb[name][0], ref_std=ea[name][1])
-            assert ea[name][0] < 1e-2, (tag, name, ea[name][0])
-        n_fold, _ = fold.plan_info(64, 30, 36, L.OUT_VIL_PREDICTION)
-        n_plain, _ = plain.plan_info(64, 30, 36, L.OUT_VIL_PREDICTION)
-        parity_log(test="ln_fold_launches_" + tag, launches_fold=n_fold, launches_unfolded=n_plain)
-        assert n_plain - n_fold == 57 and n_fold <= 160
-        # a pair's logits still do not depend on its batch neighbours
-        one = fold(*[t[1:2] for t in dev])
-        assert torch.equal(one[0], a[0][1:2])
-        fold.close()
-        plain.close()
-
-
-# ----------------------------------------------------------------------------------------------- chained FFN launch
-def test_chained_ffn_launch_is_bit_identical(full_oracle, parity_log):
-    """set_option("chain_ffn", 1): every FFN-in -> FFN-out pair becomes one persistent launch with a dynamic tile list and per-row-panel
-    dependency counters (csrc/gemm_chain.cu).  Same tiles, same accumulation order: every output keeps its bits; 30 launches fewer."""
-    from oracle import vilbert_ref as R
-    from vilbert_b200 import _lib as L
-    inp = list(R.make_inputs(16, 30, 36, seed=93, pad_regions=2))      # 16 x 31 rows >= 256: the engine chains from M = 256 up
-    dev = [t.cuda() for t in inp]
-    eng = _engine(full_oracle)
-    plain = [t.clone() for t in eng(*dev)[:9] if t is not None]
-    n_plain, _ = eng.plan_info(16, 30, 36, L.OUT_TASK_HEADS)
-    eng.set_option("chain_ffn", 1)
-    n_chain, _ = eng.plan_info(16, 30, 36, L.OUT_TASK_HEADS)
-    for rep in range(3):                                                # the dependency counters reset themselves between launches
-        chained = [t for t in eng(*dev)[:9] if t is not None]
-        torch.cuda.synchronize()
-        assert len(chained) == len(plain) >= 7
-        for a, b in zip(plain, chained):
-            assert torch.equal(a, b)
-    parity_log(test="chain_ffn_launches", launches_chained=n_chain, launches_plain=n_plain)
-    assert n_plain - n_chain == 30
-    eng.set_option("chain_ffn", 0)
-    assert eng.plan_info(16, 30, 36, L.OUT_TASK_HEADS)[0] == n_plain
-    eng.close()
-
-
 # ----------------------------------------------------------------------------------------------- step timeline (profiling hook)
 def test_timeline_records_every_gemm_cta(tiny_oracle):
     """set_option("timeline", 1): every plain persistent GEMM launch of a forward leaves per-CTA stamps (entry / exit %globaltimer, SM id);

@@ -75,7 +75,7 @@ class Options(C.Structure):
 EXPORTS = ["vb200_abi_version", "vb200_create", "vb200_destroy", "vb200_last_error", "vb200_forward", "vb200_forward_slot",
            "vb200_forward_host", "vb200_forward_host_slot", "vb200_plan_info", "vb200_model_dim", "vb200_set_option", "vb200_timeline", "vb200_profile_ops",
            "vb200_attention_layout", "vb200_forward_regions", "vb200_forward_packed", "vb200_encode_text", "vb200_encode_image", "vb200_forward_cached",
-           "vb200_linear", "vb200_linear_rows", "vb200_linear_split", "vb200_linear_ln", "vb200_linear_chain", "vb200_layernorm", "vb200_layernorm_split", "vb200_attention_f32",
+           "vb200_linear", "vb200_linear_rows", "vb200_linear_split", "vb200_layernorm", "vb200_layernorm_split", "vb200_attention_f32",
            "vb200_self_attention", "vb200_co_attention"]
 
 _lib = None
@@ -122,9 +122,6 @@ def load():
     lib.vb200_encode_image.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp, vp, vp]
     lib.vb200_forward_cached.argtypes = [vp, i32, i32, i32, vp, i32, vp, vp, vp, vp, i32, vp, vp, vp, C.POINTER(Outputs), u32, i32, vp]
     lib.vb200_linear_split.argtypes = [vp, i64, vp, i64, vp, i32, vp, i64, vp, i64, i64, i64, i64, vp]
-    lib.vb200_linear_ln.argtypes = [vp, i64, vp, i64, vp, i32, vp, i32, vp, vp, i64, vp, i32, vp, vp, vp, i32, f32, i32, vp, i64, vp, i64,
-                                    i64, i64, i64, i32, vp]
-    lib.vb200_linear_chain.argtypes = [vp, i64, vp, i64, vp, i32, vp, i64, vp, i64, vp, vp, i64, vp, i64, i64, i64, i64, i64, i32, vp, vp]
     lib.vb200_layernorm_split.argtypes = [vp, i64, vp, i64, vp, vp, f32, vp, i64, vp, i64, i64, i64, vp]
     lib.vb200_attention_f32.argtypes = [vp, i64, vp, vp, i64, i32, vp, i32, i32, i32, i32, i32, vp, i64, i32, vp, vp]
     lib.vb200_linear.argtypes = [vp, i64, vp, i64, vp, vp, i64, vp, vp, f32, i32, vp, i64, vp, i64,

@@ -95,16 +95,6 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const void* desc, ui
         ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(desc)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
         : "memory");
 }
-// Same, multicast to every CTA of the cluster whose bit is set in cta_mask (same smem offset + barrier offset in each).
-__device__ __forceinline__ void tma_load_2d_mcast(void* smem_dst, const void* desc, uint64_t* bar, int32_t c0,
-                                                  int32_t c1, uint16_t cta_mask) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-        " [%0], [%1, {%3, %4}], [%2], %5;"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(desc)), "r"(smem_u32(bar)), "r"(c0), "r"(c1),
-        "h"(cta_mask)
-        : "memory");
-}
 
 // 2-D tiled store shared (this CTA) -> global through the TMA; completion tracked with bulk groups.
 __device__ __forceinline__ void tma_store_2d(const void* desc, const void* smem_src, int32_t c0, int32_t c1) {

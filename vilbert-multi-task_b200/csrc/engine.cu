@@ -15,7 +15,6 @@
 #include <functional>
 #include <map>
 #include <memory>
-#include <set>
 #include <stdexcept>
 #include <string>
 #include <vector>
@@ -280,12 +279,8 @@ struct LinearW {            // nn.Linear [N, K] -> bf16 [N, ldw] (K zero-padded 
     bf16* w = nullptr;
     float* bias = nullptr;
     int N = 0, K = 0, ldw = 0;
-    // LayerNorm fold (gemm_persistent.cuh row_stats): this Linear's input is LayerNorm_{g,b}(u) of a pending LayerNorm; then
-    // w = g o W (16-bit), bias = c = sum_k b_k W[n,k] + bias_n, fold_s = s = sum_k w[n,k]; fold_g identifies that LayerNorm
-    float* fold_s = nullptr;
-    const float* fold_g = nullptr;
 };
-struct LNW { float* g = nullptr; float* b = nullptr; int n = 0; std::vector<float> hg, hb; };   // hg / hb: host copies (fold)
+struct LNW { float* g = nullptr; float* b = nullptr; int n = 0; };
 struct RowW { float* w = nullptr; float* b = nullptr; int n_out = 0, K = 0; };   // narrow fp32 heads
 struct LayerW { LinearW qkv, attn_out, inter, out; LNW ln1, ln2; };
 struct ConnW { LinearW qkv_img, qkv_txt, dense1, dense2, v_inter, v_out, t_inter, t_out; LNW ln1, ln2, v_ln, t_ln; };
@@ -359,14 +354,7 @@ struct Op {
     GemmEpilogue ep;
     int block_n = 128;
     bool ln = false;
-    bool pair = false;             // CTA pair (gemm_persistent.cuh PCfg MODE 8); tb then has box rows block_n / 2
-    // chained GEMM (gemm_chain.cu): this GEMM's 16-bit output is the A operand of a second one issued from the same launch
-    CUtensorMap ta2, tb2;
-    GemmEpilogue ep2;
-    int* chain_sync = nullptr;
-    double flops2 = 0;
     // fp32 attention (attention_f32.cu): fp32-parity mode and the attention-probability output
-    const void* a_ptr = nullptr;   // GEMM: the A operand (chain detection)
     const void *f_q = nullptr, *f_k = nullptr, *f_v = nullptr;
     int f_ld_q = 0, f_ld_kv = 0, f_in = 0, f_Lq = 0, f_Lk = 0, f_ctx_mode = 0, f_ld_ctx = 0;
     const float* f_mask = nullptr;
@@ -383,7 +371,6 @@ struct Op {
     float* ln_out_f = nullptr;
     bf16* ln_out_h = nullptr;
     int ln_ld = 0, ln_M = 0, ln_N = 0;
-    vb::LnPending ln_pend{nullptr, 0, 0, nullptr, nullptr};   // residual whose own LayerNorm is still pending (LayerNorm fold)
     // rowdot
     const float *x = nullptr, *W = nullptr, *bias = nullptr, *add = nullptr;
     float* out = nullptr;
@@ -411,9 +398,6 @@ struct Plan {
     float* t_f32[2]; bf16* t_b16[2];
     float* v_f32[2]; bf16* v_b16[2];
     float* y_scratch[2] = {nullptr, nullptr};   // per-stream fp32 GEMM output feeding the un-fused LayerNorm kernel
-    float2* t_stats[2] = {nullptr, nullptr};    // LayerNorm fold: per-row (mean, M2) per 32 columns of t_f32[i] / v_f32[i],
-    float2* v_stats[2] = {nullptr, nullptr};    //   [hidden / 32][stats_ld] (gemm_persistent.cuh row_stats)
-    int stats_ld_t = 0, stats_ld_v = 0;
     int t_cur = 0, v_cur = 0;
     std::vector<Op> ops;
     OutBuf outs[12];
@@ -455,30 +439,14 @@ struct vb200_engine {
     vb200_options opt{};
     int num_labels = 0, gqa_labels = 0;
     bool dry = false;          // audit pass: check names / shapes / dtypes only, touch no device
-    bool ln_fold = false;      // LayerNorm folded into the neighbouring GEMMs (row_stats in gemm_persistent.cuh); opt-in
-                               // (vb200_options::ln_fold = 1 / VB200_LNFOLD=1): 57 fewer launches per forward, paid for with
-                               // heavier GEMM epilogues -- default stays GEMM (fp32 out) + row LayerNorm kernel
-    std::set<std::string> fold_out_t, fold_out_v;   // stages ("T3", "C0", "E", ...) whose OUTPUT LayerNorm stays pending
-    bool chain_ffn = false;    // VB200_CHAIN=1 / vb200_set_option("chain_ffn", 1): FFN-in and FFN-out as ONE chained launch (gemm_chain.cu);
-                               // bit-identical to two launches; opt-in
     int lone_rows = 320;       // VB200_LONE_ROWS (0 = off): forwards with at most this many rows in either stream (batch <= 8 at the default
                                // shapes) run their plain GEMMs with 64-wide tiles while those still fit one CTA per SM
     bool x3 = false;           // fp32-parity mode (vb200_options::split_fp32): fp16 hi/lo split operands, K' = 3K GEMMs, fp32 attention
-    // Programmatic dependent launch.  Default: every kernel ("full": each kernel triggers its dependents once its main work is
-    // issued; a dependent GEMM's producer puts its first weight tiles in flight before griddepcontrol.wait).
-    // VB200_PDL=off|light|medium|mediumplus|full; use_pdl < 0 = off, > 0 = full.
-    bool pdl_light = true;
-    bool pdl_medium = true;
+    // Programmatic dependent launch (opt.use_pdl): every kernel triggers its dependents once its main work is issued, and a
+    // dependent GEMM's producer puts its first weight tiles in flight before griddepcontrol.wait.  On by default;
+    // VB200_PDL=off|full, use_pdl < 0 = off.
     bool tma_store_enabled = true;  // VB200_TMASTORE=0: every tile leaves through the register / LSU epilogue
     bool early_w = true;            // VB200_EARLYW=0: no weight loads ahead of griddepcontrol.wait
-    bool pdl_gemm_gemm = false;     // VB200_PDL=mediumplus: also GEMM -> GEMM edges of one graph branch (FFN-in -> FFN-out)
-    int light_pdl() const { return (pdl_light || opt.use_pdl) ? 1 : 0; }
-    // CTA pair (launch_gemm_pair: two CTAs of a cluster share each weight tile through TMA multicast).  Off by default: on an H100
-    // it measured 0.59x (batch 512) and 0.66x (batch 64) the step throughput of the single-CTA kernel (DESIGN.md section 5).
-    // VB200_PAIR=1 forces it on for every plain GEMM with >= 256 rows and N % 128 == 0; VB200_PAIR=auto picks it for GEMMs with at
-    // least PAIR_MIN_WAVES waves of 256 x 128 pair tiles over the SM pairs.
-    int pair_mode = 0;
-    int pair_min_waves = 2;        // VB200_PAIR_MIN_WAVES
     bool fused_ln = false;     // VB200_FUSED_LN=1: cluster-LayerNorm GEMM epilogue instead of GEMM(fp32) + row LayerNorm kernel
     Arena weights;
     std::string last_error;
@@ -545,25 +513,15 @@ struct vb200_engine {
         else for (int64_t i = 0; i < r * c; ++i) h[i] = t.at(i);
         return upload_f32(h);
     }
-    std::map<std::string, LNW> ln_cache;        // every LayerNorm is loaded once (a fold source is needed before its own layer)
     LNW load_ln(const std::string& prefix, int n) {
-        auto it = ln_cache.find(prefix);
-        if (it != ln_cache.end()) return it->second;
         LNW l; l.n = n;
-        HostTensor& tg = need(prefix + ".weight", 1, n);
-        HostTensor& tb = need(prefix + ".bias", 1, n);
-        if (!dry) {
-            l.hg.resize(n); l.hb.resize(n);
-            for (int i = 0; i < n; ++i) { l.hg[i] = tg.at(i); l.hb[i] = tb.at(i); }
-            l.g = upload_f32(l.hg);
-            l.b = upload_f32(l.hb);
-        }
-        ln_cache[prefix] = l;
+        l.g = load_vec(prefix + ".weight", n);
+        l.b = load_vec(prefix + ".bias", n);
         return l;
     }
     // one or several nn.Linear stacked along N (fused QKV), optional extra K columns from a second weight
     LinearW load_linear(const std::vector<std::string>& prefixes, int64_t n_each, int64_t k,
-                        const std::string& extra_k_prefix = "", int64_t extra_k = 0, const LNW* fold = nullptr) {
+                        const std::string& extra_k_prefix = "", int64_t extra_k = 0) {
         LinearW L;
         L.N = static_cast<int>(n_each * prefixes.size());
         L.K = static_cast<int>(k + (extra_k ? 64 : 0));
@@ -577,34 +535,6 @@ struct vb200_engine {
         if (x3) { load_linear_split(L, prefixes, n_each, k, extra_k_prefix, extra_k); return L; }
         std::vector<uint16_t> h(static_cast<size_t>(L.N) * L.ldw, 0);
         std::vector<float> hb(L.N, 0.0f);
-        if (fold != nullptr) {
-            // LayerNorm fold: W' = g o W in 16 bits, s_n = sum of the ROUNDED W'[n,:] (so the mean term cancels exactly against
-            // what the tensor cores multiply), c_n = sum_k b_k W[n,k] + bias_n
-            if (extra_k || static_cast<int64_t>(fold->hg.size()) != k) fail(VB200_ERR_INVALID, "LayerNorm fold: width mismatch");
-            std::vector<float> hs(L.N, 0.0f);
-            for (size_t pi = 0; pi < prefixes.size(); ++pi) {
-                HostTensor& w = need(prefixes[pi] + ".weight", 2, n_each, k);
-                HostTensor& b = need(prefixes[pi] + ".bias", 1, n_each);
-                for (int64_t n = 0; n < n_each; ++n) {
-                    uint16_t* dst = &h[(pi * n_each + n) * L.ldw];
-                    double sn = 0.0, cn = 0.0;
-                    for (int64_t j = 0; j < k; ++j) {
-                        const float wv = w.at(n * k + j);
-                        dst[j] = cvt16(wv * fold->hg[j]);
-                        sn += static_cast<double>(f16 ? half_bits_to_f32(dst[j]) : bf16_bits_to_f32(dst[j]));
-                        cn += static_cast<double>(fold->hb[j]) * static_cast<double>(wv);
-                    }
-                    hs[pi * n_each + n] = static_cast<float>(sn);
-                    hb[pi * n_each + n] = static_cast<float>(cn + static_cast<double>(b.at(n)));
-                }
-            }
-            L.w = weights.alloc_n<bf16>(h.size());
-            CUDA_CHECK(cudaMemcpy(L.w, h.data(), h.size() * 2, cudaMemcpyHostToDevice));
-            L.bias = upload_f32(hb);
-            L.fold_s = upload_f32(hs);
-            L.fold_g = fold->g;
-            return L;
-        }
         for (size_t pi = 0; pi < prefixes.size(); ++pi) {
             HostTensor& w = need(prefixes[pi] + ".weight", 2, n_each, k);
             HostTensor& b = need(prefixes[pi] + ".bias", 1, n_each);
@@ -667,23 +597,20 @@ struct vb200_engine {
         CUDA_CHECK(cudaMemcpy(L.w, h.data(), h.size() * 2, cudaMemcpyHostToDevice));
         L.bias = upload_f32(hb);
     }
-    LinearW load_linear1(const std::string& prefix, int64_t n, int64_t k, const LNW* fold = nullptr) {
-        return load_linear({prefix}, n, k, "", 0, fold);
-    }
+    LinearW load_linear1(const std::string& prefix, int64_t n, int64_t k) { return load_linear({prefix}, n, k); }
     RowW load_row(const std::string& prefix, int n_out, int k) {
         RowW r; r.n_out = n_out; r.K = k;
         r.w = load_mat_f32(prefix + ".weight", n_out, k);
         r.b = load_vec(prefix + ".bias", n_out);
         return r;
     }
-    // src: the pending LayerNorm of this layer's input (previous stage of the stream) when that one is folded, else null
-    LayerW load_layer(const std::string& p, int hid, int inter, const LNW* src) {
+    LayerW load_layer(const std::string& p, int hid, int inter) {
         LayerW L;
         L.ln1 = load_ln(p + ".attention.output.LayerNorm", hid);
         L.ln2 = load_ln(p + ".output.LayerNorm", hid);
-        L.qkv = load_linear({p + ".attention.self.query", p + ".attention.self.key", p + ".attention.self.value"}, hid, hid, "", 0, src);
+        L.qkv = load_linear({p + ".attention.self.query", p + ".attention.self.key", p + ".attention.self.value"}, hid, hid);
         L.attn_out = load_linear1(p + ".attention.output.dense", hid, hid);
-        L.inter = load_linear1(p + ".intermediate.dense", inter, hid, ln_fold ? &L.ln1 : nullptr);
+        L.inter = load_linear1(p + ".intermediate.dense", inter, hid);
         L.out = load_linear1(p + ".output.dense", hid, inter);
         return L;
     }
@@ -745,66 +672,24 @@ struct vb200_engine {
             for (int k = v_start; k < c.v_layers; ++k) schedule.push_back("V" + std::to_string(k));
             for (int k = t_start; k < c.layers; ++k) schedule.push_back("T" + std::to_string(k));
         }
-        // LayerNorm fold map (gemm_persistent.cuh row_stats).  Each stream is a chain of stages (text: T layers and the text half of
-        // the connection layers; image: the embedding, V layers, the image half of the connection layers).  A stage's OUTPUT
-        // LayerNorm stays pending -- folded into the next stage's first GEMM and rebuilt in its residual -- unless the stage is the
-        // stream's last one (poolers, heads and the output taps read real values) or the last one ahead of the first connection
-        // layer (that is where the retrieval path caches per-caption / per-image states, and every plan mode must compute the same
-        // bits).  The LayerNorm INSIDE a stage (after the attention / co-attention output projection) always folds.
-        std::vector<std::string> t_st, v_st{"E"};
-        for (const std::string& st : schedule) {
-            if (st[0] == 'T' || st[0] == 'C') t_st.push_back(st);
-            if (st[0] == 'V' || st[0] == 'C') v_st.push_back(st);
-        }
-        auto stage_ln = [&](const std::string& st, bool text) -> std::pair<std::string, int> {
-            const std::string i = st.substr(st[0] == 'E' ? 0 : 1);
-            if (st[0] == 'E') return {"bert.v_embeddings.LayerNorm", c.v_hidden};
-            if (st[0] == 'T') return {"bert.encoder.layer." + i + ".output.LayerNorm", c.hidden};
-            if (st[0] == 'V') return {"bert.encoder.v_layer." + i + ".output.LayerNorm", c.v_hidden};
-            return text ? std::make_pair("bert.encoder.c_layer." + i + ".t_output.LayerNorm", c.hidden)
-                        : std::make_pair("bert.encoder.c_layer." + i + ".v_output.LayerNorm", c.v_hidden);
-        };
-        // src_of[stage] = the previous stage's output LayerNorm if it folds, else nothing; fold_out[stage] as above
-        std::map<std::string, LNW> src_t, src_v;
-        auto walk = [&](const std::vector<std::string>& stages, bool text, std::map<std::string, LNW>& src, std::set<std::string>& folds) {
-            int first_c = -1;
-            for (size_t i = 0; i < stages.size(); ++i) if (stages[i][0] == 'C') { first_c = static_cast<int>(i); break; }
-            for (size_t i = 0; i < stages.size(); ++i) {
-                const bool fo = ln_fold && i + 1 < stages.size() && static_cast<int>(i) != first_c - 1;
-                if (fo) {
-                    folds.insert(stages[i]);
-                    auto nm = stage_ln(stages[i], text);
-                    src[stages[i + 1]] = load_ln(nm.first, nm.second);
-                }
-            }
-        };
-        walk(t_st, true, src_t, fold_out_t);
-        walk(v_st, false, src_v, fold_out_v);
-        auto src_ptr = [](std::map<std::string, LNW>& m, const std::string& st) -> const LNW* {
-            auto it = m.find(st);
-            return it == m.end() ? nullptr : &it->second;
-        };
         for (int i = 0; i < c.layers; ++i)
-            t_layers.push_back(load_layer("bert.encoder.layer." + std::to_string(i), c.hidden, c.inter, src_ptr(src_t, "T" + std::to_string(i))));
+            t_layers.push_back(load_layer("bert.encoder.layer." + std::to_string(i), c.hidden, c.inter));
         for (int i = 0; i < c.v_layers; ++i)
-            v_layers.push_back(load_layer("bert.encoder.v_layer." + std::to_string(i), c.v_hidden, c.v_inter, src_ptr(src_v, "V" + std::to_string(i))));
+            v_layers.push_back(load_layer("bert.encoder.v_layer." + std::to_string(i), c.v_hidden, c.v_inter));
         for (size_t i = 0; i < c.v_bi_id.size(); ++i) {
             const std::string p = "bert.encoder.c_layer." + std::to_string(i);
-            const std::string cs = "C" + std::to_string(i);
             ConnW w;
             w.ln1 = load_ln(p + ".biOutput.LayerNorm1", c.v_hidden);
             w.ln2 = load_ln(p + ".biOutput.LayerNorm2", c.hidden);
             w.v_ln = load_ln(p + ".v_output.LayerNorm", c.v_hidden);
             w.t_ln = load_ln(p + ".t_output.LayerNorm", c.hidden);
-            w.qkv_img = load_linear({p + ".biattention.query1", p + ".biattention.key1", p + ".biattention.value1"}, c.bi_hidden, c.v_hidden,
-                                    "", 0, src_ptr(src_v, cs));
-            w.qkv_txt = load_linear({p + ".biattention.query2", p + ".biattention.key2", p + ".biattention.value2"}, c.bi_hidden, c.hidden,
-                                    "", 0, src_ptr(src_t, cs));
+            w.qkv_img = load_linear({p + ".biattention.query1", p + ".biattention.key1", p + ".biattention.value1"}, c.bi_hidden, c.v_hidden);
+            w.qkv_txt = load_linear({p + ".biattention.query2", p + ".biattention.key2", p + ".biattention.value2"}, c.bi_hidden, c.hidden);
             w.dense1 = load_linear1(p + ".biOutput.dense1", c.v_hidden, c.bi_hidden);
             w.dense2 = load_linear1(p + ".biOutput.dense2", c.hidden, c.bi_hidden);
-            w.v_inter = load_linear1(p + ".v_intermediate.dense", c.v_inter, c.v_hidden, ln_fold ? &w.ln1 : nullptr);
+            w.v_inter = load_linear1(p + ".v_intermediate.dense", c.v_inter, c.v_hidden);
             w.v_out = load_linear1(p + ".v_output.dense", c.v_hidden, c.v_inter);
-            w.t_inter = load_linear1(p + ".t_intermediate.dense", c.inter, c.hidden, ln_fold ? &w.ln2 : nullptr);
+            w.t_inter = load_linear1(p + ".t_intermediate.dense", c.inter, c.hidden);
             w.t_out = load_linear1(p + ".t_output.dense", c.hidden, c.inter);
             c_layers.push_back(w);
             // [UPSTREAM] present in the checkpoint, never applied in forward
@@ -855,7 +740,6 @@ struct vb200_engine {
             if (n) fail(VB200_ERR_CHECKPOINT, "checkpoint has %d unexpected key(s):%s%s", n, extra.c_str(), n > 8 ? " ..." : "");
         }
         sd.clear();   // host pointers are the caller's; do not keep them
-        ln_cache.clear();
     }
 
     // ---------------------------------------------------------------- plan construction
@@ -866,64 +750,33 @@ struct vb200_engine {
     // All sizes are LOGICAL (elements of the mathematical matrices).  In fp32-parity mode (x3) every 16-bit operand buffer is
     // physically 3x as wide (fp16 hi | lo | hi per 64 columns), so operand strides, the contraction length and the 16-bit
     // output stride are multiplied by S = 3 here and nowhere else.
-    // LayerNorm fold (row_stats in gemm_persistent.cuh): what add_linear needs to know beyond the plain call
-    struct FoldArgs {
-        const float2* a_stats = nullptr;   // the A operand's LayerNorm is pending: its row statistics (W must be a folded Linear)
-        int a_parts = 0;
-        const float2* res_stats = nullptr; // the residual's LayerNorm is pending: its statistics and parameters
-        int res_parts = 0;
-        const LNW* res_ln = nullptr;
-        float2* out_stats = nullptr;       // keep THIS Linear's LayerNorm pending: write u (fp32 + 16-bit) and its statistics here
-        int stats_ld = 0;
-    };
     void add_linear(Plan& pl, const bf16* A, int64_t a_rows, int64_t lda, const LinearW& W, int act, const float* res, int ld_res,
                     const LNW* ln, bf16* out_b, int ld_b, float* out_f, int ld_f, int stream = 0, Op::Sync sync = Op::NONE,
-                    const float* mul = nullptr, int ld_mul = 0, const FoldArgs* fa = nullptr, const int* m_rows = nullptr) {
+                    const float* mul = nullptr, int ld_mul = 0, const int* m_rows = nullptr) {
         const int S = x3 ? 3 : 1;
-        const bool keep_pending = ln != nullptr && fa != nullptr && fa->out_stats != nullptr;
-        const bool fold_in = fa != nullptr && fa->a_stats != nullptr;
-        if ((W.fold_s != nullptr) != fold_in)
-            fail(VB200_ERR_INVALID, "LayerNorm fold: Linear N=%d K=%d was %s with a pending LayerNorm but its input is %s", W.N, W.K,
-                 W.fold_s ? "folded" : "not folded", fold_in ? "pending" : "final");
-        const bool split_ln = ln != nullptr && !fused_ln && !keep_pending;
+        const bool split_ln = ln != nullptr && !fused_ln;
         if (x3 && act == vb::kActGelu) act = vb::kActGeluExact;
         Op op{};
         op.kind = Op::GEMM;
         op.stream = stream;
         op.sync = sync;
-        op.ln = ln != nullptr && !split_ln && !keep_pending;      // cluster-LayerNorm epilogue (fused_layernorm option)
+        op.ln = ln != nullptr && !split_ln;      // cluster-LayerNorm epilogue (fused_layernorm option)
         op.block_n = vb::gemm_p_pick_block_n(W.N, op.ln);
         if (op.block_n == 0) fail(VB200_ERR_INVALID, "no LayerNorm-fused GEMM tiling for N=%d", W.N);
-        if (pair_mode != 0 && !x3 && !op.ln && !keep_pending && !fold_in && a_rows >= 256 && W.N % 128 == 0) {
-            const long long pair_tiles = ((a_rows + 255) / 256) * (W.N / 128);
-            op.pair = pair_mode > 0 || pair_tiles >= static_cast<long long>(pair_min_waves) * (vb::num_sms_host() / 2);
-            if (op.pair) op.block_n = 128;
-        }
         // Small forwards (<= lone_rows rows in either stream, batch <= 8): 64-wide tiles while they still fit one CTA per SM -- twice
         // the CTAs, half the epilogue each.  The tile width never changes an element's accumulation order.
-        if (lone_rows > 0 && !x3 && !op.ln && !op.pair && !keep_pending && !fold_in && op.block_n == 128 && W.N % 64 == 0 &&
+        if (lone_rows > 0 && !x3 && !op.ln && op.block_n == 128 && W.N % 64 == 0 &&
             std::max(pl.B * pl.T, pl.B * pl.V) <= lone_rows && ((a_rows + 127) / 128) * (W.N / 64) <= vb::num_sms_host())
             op.block_n = 64;
         op.ta = make_tmap(A, a_rows, static_cast<int64_t>(W.ldw) * S, lda * S, 128, opt.act_fp16 != 0);
-        op.tb = make_tmap(W.w, W.N, static_cast<int64_t>(W.ldw) * S, static_cast<int64_t>(W.ldw) * S, op.pair ? op.block_n / 2 : op.block_n,
-                          opt.act_fp16 != 0);
+        op.tb = make_tmap(W.w, W.N, static_cast<int64_t>(W.ldw) * S, static_cast<int64_t>(W.ldw) * S, op.block_n, opt.act_fp16 != 0);
         GemmEpilogue& e = op.ep;
         e.M = static_cast<int>(a_rows); e.N = W.N; e.K = W.ldw * S;
-        e.bias = W.bias; e.mul = mul; e.ld_mul = ld_mul; e.eps = cfg.ln_eps; e.act = act; e.pdl = pdl_light ? 2 : (opt.use_pdl ? (early_w ? 5 : 1) : 0);
+        e.bias = W.bias; e.mul = mul; e.ld_mul = ld_mul; e.eps = cfg.ln_eps; e.act = act; e.pdl = opt.use_pdl ? (early_w ? 5 : 1) : 0;
         e.a_f16 = opt.act_fp16; e.out_f16 = opt.act_fp16;
         e.m_rows = m_rows;
-        if (fold_in) {
-            e.ln_mode = 4; e.a_stats = fa->a_stats; e.a_parts = fa->a_parts; e.fold_s = W.fold_s; e.stats_ld = fa->stats_ld;
-        }
         if (split_ln) {
             e.out_f32 = pl.y_scratch[stream]; e.ld_f32 = W.N;
-        } else if (keep_pending) {
-            // producer of a pending LayerNorm: u = acc + bias + residual in fp32 and 16 bits, plus the row statistics
-            e.ln_mode = 5; e.res = res; e.ld_res = ld_res;
-            e.res_stats = fa->res_stats; e.res_parts = fa->res_parts;
-            e.res_gamma = fa->res_ln ? fa->res_ln->g : nullptr; e.res_beta = fa->res_ln ? fa->res_ln->b : nullptr;
-            e.out_stats = fa->out_stats; e.stats_ld = fa->stats_ld;
-            e.out_bf16 = out_b; e.ld_bf16 = ld_b; e.out_f32 = out_f; e.ld_f32 = ld_f;
         } else {
             e.res = res; e.ld_res = ld_res;
             e.gamma = ln ? ln->g : nullptr; e.beta = ln ? ln->b : nullptr;
@@ -931,9 +784,8 @@ struct vb200_engine {
             e.split16 = (x3 && out_b != nullptr) ? 1 : 0;
             if (e.split16 && (W.N & 63)) fail(VB200_ERR_INVALID, "fp32-parity mode: 16-bit GEMM output of width %d is not a multiple of 64", W.N);
         }
-        if (tma_store_enabled && !op.pair && !op.ln) setup_tma_store(&op.tc, e);
+        if (tma_store_enabled && !op.ln) setup_tma_store(&op.tc, e);
         op.flops = 2.0 * a_rows * W.N * W.K;
-        op.a_ptr = A;
         pl.flops += op.flops;
         pl.ops.push_back(op);
         if (split_ln) {
@@ -945,8 +797,6 @@ struct vb200_engine {
             l.ld_out = out_f ? ld_f : 0; l.ld_a = out_b ? ld_b * S : 0;
             l.ln_M = static_cast<int>(a_rows); l.ln_N = W.N;
             l.m_rows = m_rows;
-            if (fa != nullptr && fa->res_stats != nullptr)
-                l.ln_pend = vb::LnPending{fa->res_stats, fa->res_parts, fa->stats_ld, fa->res_ln->g, fa->res_ln->b};
             pl.ops.push_back(l);
         }
     }
@@ -1058,60 +908,33 @@ struct vb200_engine {
         };
         auto qkv_at = [&](const uint8_t* q, int col) -> const void* { return q + static_cast<size_t>(col) * qe; };
 
-        // ---- LayerNorm fold state of the two streams: `pend` = the LayerNorm still to be applied to buffers [cur] (null: the
-        // buffers hold final values), its row statistics live in stats[cur]
+        // ---- the two streams: activations ping-pong between buffers [cur] and [1 - cur]
         struct StreamSt {
-            float** f32; bf16** b16; float2** stats; int cur; const LNW* pend; int hid, rows, stats_ld, stream; const float* mask; int seq;
+            float** f32; bf16** b16; int cur; int hid, rows, stream; const float* mask; int seq;
             uint8_t* qkv; bf16* ctx; bf16* inter;
             const int* m_rows; const int* offs;     // packed plans: device row count and per-sample row offsets of the stream
         };
-        if (ln_fold) {
-            pl.stats_ld_t = (Mt + 31) & ~31; pl.stats_ld_v = (Mv + 31) & ~31;
-            for (int i = 0; i < 2; ++i) {
-                pl.t_stats[i] = static_cast<float2*>(pl.mem.alloc(static_cast<size_t>(H / 32) * pl.stats_ld_t * sizeof(float2)));
-                pl.v_stats[i] = static_cast<float2*>(pl.mem.alloc(static_cast<size_t>(Hv / 32) * pl.stats_ld_v * sizeof(float2)));
-            }
-        }
-        StreamSt ts{pl.t_f32, pl.t_b16, pl.t_stats, 0, nullptr, H, Mt, pl.stats_ld_t, 0, pl.mask_t, T, qkv_t, ctx_t, inter_t, rows_t, offs_t};
-        StreamSt vs{pl.v_f32, pl.v_b16, pl.v_stats, 0, nullptr, Hv, Mv, pl.stats_ld_v, 1, pl.mask_v, V, qkv_v, ctx_v, inter_v, rows_v, offs_v};
-        auto fold_in_args = [&](const StreamSt& st, int which) {          // consume buffers[which] of a stream as a GEMM's A operand
-            FoldArgs fa;
-            fa.a_stats = st.stats[which]; fa.a_parts = st.hid / 32; fa.stats_ld = st.stats_ld;
-            return fa;
-        };
-        // GEMM + LayerNorm whose residual is buffers[rwhich] of stream st (its own LayerNorm possibly pending: res_pend);
-        // the result lands in buffers[owhich]; keep == true leaves THIS LayerNorm pending (statistics in stats[owhich])
-        auto ln_linear = [&](StreamSt& st, const bf16* A, int64_t lda, const LinearW& W, const LNW& ln, int rwhich, const LNW* res_pend,
-                             int owhich, bool keep, Op::Sync sync) {
-            FoldArgs fa;
-            fa.stats_ld = st.stats_ld;
-            if (res_pend != nullptr) { fa.res_stats = st.stats[rwhich]; fa.res_parts = st.hid / 32; fa.res_ln = res_pend; }
-            if (keep) fa.out_stats = st.stats[owhich];
+        StreamSt ts{pl.t_f32, pl.t_b16, 0, H, Mt, 0, pl.mask_t, T, qkv_t, ctx_t, inter_t, rows_t, offs_t};
+        StreamSt vs{pl.v_f32, pl.v_b16, 0, Hv, Mv, 1, pl.mask_v, V, qkv_v, ctx_v, inter_v, rows_v, offs_v};
+        // GEMM + LayerNorm whose residual is buffers[rwhich] of stream st; the result lands in buffers[owhich]
+        auto ln_linear = [&](StreamSt& st, const bf16* A, int64_t lda, const LinearW& W, const LNW& ln, int rwhich, int owhich,
+                             Op::Sync sync) {
             add_linear(pl, A, st.rows, lda, W, vb::kActNone, st.f32[rwhich], st.hid, &ln, st.b16[owhich], st.hid, st.f32[owhich], st.hid,
-                       st.stream, sync, nullptr, 0, (res_pend != nullptr || keep) ? &fa : nullptr, st.m_rows);
+                       st.stream, sync, nullptr, 0, st.m_rows);
         };
 
         // ---- image embedding: LayerNorm(feat.W_img^T + loc.W_loc^T + b) as ONE GEMM over K = v_feat + 64
-        if (do_v) {
-            const bool keep = ln_fold && fold_out_v.count("E") != 0;
-            FoldArgs fa;
-            fa.stats_ld = vs.stats_ld;
-            if (keep) fa.out_stats = vs.stats[0];
+        if (do_v)
             add_linear(pl, pl.img_a, Mv, pl.kp, img_emb, vb::kActNone, nullptr, 0, &vemb_ln, pl.v_b16[0], Hv, pl.v_f32[0], Hv,
-                       1, Op::NONE, nullptr, 0, keep ? &fa : nullptr, vs.m_rows);   // side stream: overlaps the text layers ahead of the first co-attention
-        }
-        if (do_v && ln_fold && fold_out_v.count("E") != 0) vs.pend = &vemb_ln;
+                       1, Op::NONE, nullptr, 0, vs.m_rows);   // side stream: overlaps the text layers ahead of the first co-attention
 
-        // one BertLayer / BertImageLayer.  keep_out: this stage's output LayerNorm stays pending (LayerNorm fold map, ingest())
-        auto single_layer = [&](const LayerW& L, StreamSt& st, int inter, int heads, bool keep_out) {
+        // one BertLayer / BertImageLayer
+        auto single_layer = [&](const LayerW& L, StreamSt& st, int inter, int heads) {
             const int hid = st.hid, cur = st.cur, M = st.rows, stream = st.stream;
             bf16* qb; float* qf;
             qkv_out(st.qkv, qb, qf);
-            {
-                FoldArgs fa = fold_in_args(st, cur);
-                add_linear(pl, st.b16[cur], M, hid, L.qkv, vb::kActNone, nullptr, 0, nullptr, qb, 3 * hid, qf, 3 * hid, stream, Op::NONE,
-                           nullptr, 0, st.pend ? &fa : nullptr, st.m_rows);
-            }
+            add_linear(pl, st.b16[cur], M, hid, L.qkv, vb::kActNone, nullptr, 0, nullptr, qb, 3 * hid, qf, 3 * hid, stream, Op::NONE,
+                       nullptr, 0, st.m_rows);
             if (!x3) {
                 Op a{};
                 a.kind = Op::SELF_ATTN;
@@ -1126,15 +949,11 @@ struct vb200_engine {
                 add_attn_f32(pl, qkv_at(st.qkv, 0), 3 * hid, qkv_at(st.qkv, hid), qkv_at(st.qkv, 2 * hid), 3 * hid, st.mask, st.seq, st.seq,
                              heads, hid, st.ctx, want_attn, stream);
             // attention output + LayerNorm1 (residual: the layer input) -> buffers [1 - cur]
-            ln_linear(st, st.ctx, hid, L.attn_out, L.ln1, cur, st.pend, 1 - cur, ln_fold, Op::NONE);
-            {
-                FoldArgs fa = fold_in_args(st, 1 - cur);
-                add_linear(pl, st.b16[1 - cur], M, hid, L.inter, vb::kActGelu, nullptr, 0, nullptr, st.inter, inter, nullptr, 0, stream,
-                           Op::NONE, nullptr, 0, ln_fold ? &fa : nullptr, st.m_rows);
-            }
+            ln_linear(st, st.ctx, hid, L.attn_out, L.ln1, cur, 1 - cur, Op::NONE);
+            add_linear(pl, st.b16[1 - cur], M, hid, L.inter, vb::kActGelu, nullptr, 0, nullptr, st.inter, inter, nullptr, 0, stream,
+                       Op::NONE, nullptr, 0, st.m_rows);
             // FFN output + LayerNorm2 (residual: LayerNorm1's output) -> buffers [cur]
-            ln_linear(st, st.inter, inter, L.out, L.ln2, 1 - cur, ln_fold ? &L.ln1 : nullptr, cur, keep_out, Op::NONE);
-            st.pend = keep_out ? &L.ln2 : nullptr;
+            ln_linear(st, st.inter, inter, L.out, L.ln2, 1 - cur, cur, Op::NONE);
         };
 
         for (Op& op : ops) op.tag = "embed";
@@ -1149,22 +968,19 @@ struct vb200_engine {
                 ~Tagger() { for (size_t i = from; i < ops.size(); ++i) ops[i].tag = name; }
             } tagger{ops, ops.size(), step.c_str()};
             if (step[0] == 'T') {
-                if (in_suffix ? do_s : do_t) single_layer(t_layers[idx], ts, c.inter, c.heads, ln_fold && fold_out_t.count(step) != 0);
+                if (in_suffix ? do_s : do_t) single_layer(t_layers[idx], ts, c.inter, c.heads);
             } else if (step[0] == 'V') {
-                if (in_suffix ? do_s : do_v) single_layer(v_layers[idx], vs, c.v_inter, c.v_heads, ln_fold && fold_out_v.count(step) != 0);
+                if (in_suffix ? do_s : do_v) single_layer(v_layers[idx], vs, c.v_inter, c.v_heads);
             } else if (do_s) {
                 const ConnW& W = c_layers[idx];
                 const int tcur = ts.cur, vcur = vs.cur;
                 bf16 *qvb, *qtb; float *qvf, *qtf;
                 qkv_out(qkv_v, qvb, qvf);
                 qkv_out(qkv_t, qtb, qtf);
-                {
-                    FoldArgs fv = fold_in_args(vs, vcur), ft = fold_in_args(ts, tcur);
-                    add_linear(pl, pl.v_b16[vcur], Mv, Hv, W.qkv_img, vb::kActNone, nullptr, 0, nullptr, qvb, 3 * Hb, qvf, 3 * Hb, 1, Op::NONE,
-                               nullptr, 0, vs.pend ? &fv : nullptr, vs.m_rows);
-                    add_linear(pl, pl.t_b16[tcur], Mt, H, W.qkv_txt, vb::kActNone, nullptr, 0, nullptr, qtb, 3 * Hb, qtf, 3 * Hb, 0, Op::NONE,
-                               nullptr, 0, ts.pend ? &ft : nullptr, ts.m_rows);
-                }
+                add_linear(pl, pl.v_b16[vcur], Mv, Hv, W.qkv_img, vb::kActNone, nullptr, 0, nullptr, qvb, 3 * Hb, qvf, 3 * Hb, 1, Op::NONE,
+                           nullptr, 0, vs.m_rows);
+                add_linear(pl, pl.t_b16[tcur], Mt, H, W.qkv_txt, vb::kActNone, nullptr, 0, nullptr, qtb, 3 * Hb, qtf, 3 * Hb, 0, Op::NONE,
+                           nullptr, 0, ts.m_rows);
                 const size_t first_co = ops.size();
                 if (!x3) {
                     Op a{};
@@ -1184,29 +1000,18 @@ struct vb200_engine {
                                  c.bi_heads, Hb, ctx_v, want_attn, 0);
                 }
                 ops[first_co].sync = Op::JOIN;              // needs both projections
-                const bool keep_v = ln_fold && fold_out_v.count(step) != 0, keep_t = ln_fold && fold_out_t.count(step) != 0;
                 // image branch (side stream; forks from the co-attention): biOutput.dense1 + LayerNorm1, v_intermediate, v_output + LayerNorm
-                ln_linear(vs, ctx_v, Hb, W.dense1, W.ln1, vcur, vs.pend, 1 - vcur, ln_fold, Op::FORK);
-                {
-                    FoldArgs fa = fold_in_args(vs, 1 - vcur);
-                    add_linear(pl, pl.v_b16[1 - vcur], Mv, Hv, W.v_inter, vb::kActGelu, nullptr, 0, nullptr, inter_v, c.v_inter, nullptr, 0, 1,
-                               Op::NONE, nullptr, 0, ln_fold ? &fa : nullptr, vs.m_rows);
-                }
-                ln_linear(vs, inter_v, c.v_inter, W.v_out, W.v_ln, 1 - vcur, ln_fold ? &W.ln1 : nullptr, vcur, keep_v, Op::NONE);
-                vs.pend = keep_v ? &W.v_ln : nullptr;
+                ln_linear(vs, ctx_v, Hb, W.dense1, W.ln1, vcur, 1 - vcur, Op::FORK);
+                add_linear(pl, pl.v_b16[1 - vcur], Mv, Hv, W.v_inter, vb::kActGelu, nullptr, 0, nullptr, inter_v, c.v_inter, nullptr, 0, 1,
+                           Op::NONE, nullptr, 0, vs.m_rows);
+                ln_linear(vs, inter_v, c.v_inter, W.v_out, W.v_ln, 1 - vcur, vcur, Op::NONE);
                 // text branch (main stream)
-                ln_linear(ts, ctx_t, Hb, W.dense2, W.ln2, tcur, ts.pend, 1 - tcur, ln_fold, Op::NONE);
-                {
-                    FoldArgs fa = fold_in_args(ts, 1 - tcur);
-                    add_linear(pl, pl.t_b16[1 - tcur], Mt, H, W.t_inter, vb::kActGelu, nullptr, 0, nullptr, inter_t, c.inter, nullptr, 0, 0,
-                               Op::NONE, nullptr, 0, ln_fold ? &fa : nullptr, ts.m_rows);
-                }
-                ln_linear(ts, inter_t, c.inter, W.t_out, W.t_ln, 1 - tcur, ln_fold ? &W.ln2 : nullptr, tcur, keep_t, Op::NONE);
-                ts.pend = keep_t ? &W.t_ln : nullptr;
+                ln_linear(ts, ctx_t, Hb, W.dense2, W.ln2, tcur, 1 - tcur, Op::NONE);
+                add_linear(pl, pl.t_b16[1 - tcur], Mt, H, W.t_inter, vb::kActGelu, nullptr, 0, nullptr, inter_t, c.inter, nullptr, 0, 0,
+                           Op::NONE, nullptr, 0, ts.m_rows);
+                ln_linear(ts, inter_t, c.inter, W.t_out, W.t_ln, 1 - tcur, tcur, Op::NONE);
             }
         }
-        if ((do_s || do_t) && ts.pend != nullptr) fail(VB200_ERR_INVALID, "LayerNorm fold: the text stream ends with a pending LayerNorm");
-        if ((do_s || do_v) && vs.pend != nullptr) fail(VB200_ERR_INVALID, "LayerNorm fold: the image stream ends with a pending LayerNorm");
         const int tc = ts.cur, vc = vs.cur;
         pl.t_cur = tc; pl.v_cur = vc;
         pl.outs[9] = OutBuf{pl.t_f32[tc], Mt, H, H};
@@ -1217,8 +1022,6 @@ struct vb200_engine {
         for (size_t i = n_before_heads; i < ops.size(); ++i) ops[i].tag = "heads";
         for (Op& op : ops) if (op.kind == Op::ROWDOT) pl.flops += op.flops;
 
-        link_chains(pl);
-        link_pdl(pl);
         if (timeline) attach_timeline(pl);
         // One eager pass first: opts kernels into their shared-memory sizes and surfaces launch-configuration
         // errors with a real message (errors inside a capture only invalidate the capture).
@@ -1244,12 +1047,12 @@ struct vb200_engine {
     static constexpr int kTimelineCtas = 304;
     void attach_timeline(Plan& pl) {
         size_t n = 0;
-        for (const Op& op : pl.ops) if (op.kind == Op::GEMM && !op.ln && !op.chain_sync) ++n;
+        for (const Op& op : pl.ops) if (op.kind == Op::GEMM && !op.ln) ++n;
         if (n == 0) return;
         pl.timeline = pl.mem.alloc_n<long long>(n * kTimelineCtas * 16);
         CUDA_CHECK(cudaMemset(pl.timeline, 0, n * kTimelineCtas * 16 * sizeof(long long)));
         size_t i = 0;
-        for (Op& op : pl.ops) if (op.kind == Op::GEMM && !op.ln && !op.chain_sync) op.ep.timing = pl.timeline + (i++) * kTimelineCtas * 16;
+        for (Op& op : pl.ops) if (op.kind == Op::GEMM && !op.ln) op.ep.timing = pl.timeline + (i++) * kTimelineCtas * 16;
     }
 
     // Plan cache bound (a MicroBatchWorker produces many (batch, length, regions) combinations): beyond max_plans the least
@@ -1329,10 +1132,10 @@ struct vb200_engine {
         if (select & VB200_OUT_VISION_PREDICTION) {
             bf16* hid = pl.mem.alloc_n<bf16>(static_cast<size_t>(Mv) * Hv * S);
             add_linear(pl, pl.v_b16[vc], Mv, Hv, img_transform, vb::kActGelu, nullptr, 0, &img_ln, hid, Hv, nullptr, 0, 0, Op::NONE,
-                       nullptr, 0, nullptr, rows_v);
+                       nullptr, 0, rows_v);
             pl.outs[5] = make_out(pl, Mv, c.v_target);
             add_linear(pl, hid, Mv, Hv, img_decoder, vb::kActNone, nullptr, 0, nullptr, nullptr, 0, pl.outs[5].p, pl.outs[5].ld, 0, Op::NONE,
-                       nullptr, 0, nullptr, rows_v);
+                       nullptr, 0, rows_v);
         }
         if (select & VB200_OUT_VISION_LOGIT) {
             pl.outs[6] = make_out(pl, Mv, 1);
@@ -1341,10 +1144,10 @@ struct vb200_engine {
         if (select & VB200_OUT_LINGUISIC_PREDICTION) {
             bf16* hid = pl.mem.alloc_n<bf16>(static_cast<size_t>(Mt) * H * S);
             add_linear(pl, pl.t_b16[tc], Mt, H, lm_transform, vb::kActGelu, nullptr, 0, &lm_ln, hid, H, nullptr, 0, 0, Op::NONE,
-                       nullptr, 0, nullptr, rows_t);
+                       nullptr, 0, rows_t);
             pl.outs[7] = make_out(pl, Mt, c.vocab);
             add_linear(pl, hid, Mt, H, lm_decoder, vb::kActNone, nullptr, 0, nullptr, nullptr, 0, pl.outs[7].p, pl.outs[7].ld, 0, Op::NONE,
-                       nullptr, 0, nullptr, rows_t);
+                       nullptr, 0, rows_t);
         }
         if (select & VB200_OUT_LINGUISIC_LOGIT) {
             pl.outs[8] = make_out(pl, Mt, 1);
@@ -1355,42 +1158,34 @@ struct vb200_engine {
     // ---------------------------------------------------------------- execution
     void launch_op(const Op& op, cudaStream_t st) {
         switch (op.kind) {
-            case Op::GEMM:
-                if (op.chain_sync != nullptr) {
-                    const cudaError_t le = vb::launch_gemm_chain(op.ta, op.tb, op.ep, op.ta2, op.tb2, op.ep2, op.chain_sync, st);
-                    if (le != cudaSuccess)
-                        fail(VB200_ERR_CUDA, "chained GEMM launch failed: %s (layer %s, M=%d N1=%d K1=%d N2=%d)", cudaGetErrorString(le),
-                             op.tag ? op.tag : "?", op.ep.M, op.ep.N, op.ep.K, op.ep2.N);
-                } else if (op.pair) {
-                    CUDA_CHECK(vb::launch_gemm_pair(op.ta, op.tb, op.ep, op.block_n, st));
-                } else {
-                    GemmEpilogue e = op.ep;
-                    e.tmap_c_host = e.tma_store ? &op.tc : nullptr;       // Op objects move when the list grows: bind here
-                    e.grid_pct = profile_grid_pct;                        // 0 outside vb200_profile_ops
-                    const cudaError_t le = vb::launch_gemm_persistent(op.ta, op.tb, e, op.block_n, op.ln, st);
-                    if (le != cudaSuccess)
-                        fail(VB200_ERR_CUDA, "GEMM launch failed: %s (layer %s, M=%d N=%d K=%d act=%d block_n=%d cluster_ln=%d ln_mode=%d split16=%d tma_store=%d)",
-                             cudaGetErrorString(le), op.tag ? op.tag : "?", e.M, e.N, e.K, e.act, op.block_n, (int)op.ln, e.ln_mode, e.split16, e.tma_store);
-                }
+            case Op::GEMM: {
+                GemmEpilogue e = op.ep;
+                e.tmap_c_host = e.tma_store ? &op.tc : nullptr;       // Op objects move when the list grows: bind here
+                e.grid_pct = profile_grid_pct;                        // 0 outside vb200_profile_ops
+                const cudaError_t le = vb::launch_gemm_persistent(op.ta, op.tb, e, op.block_n, op.ln, st);
+                if (le != cudaSuccess)
+                    fail(VB200_ERR_CUDA, "GEMM launch failed: %s (layer %s, M=%d N=%d K=%d act=%d block_n=%d cluster_ln=%d split16=%d tma_store=%d)",
+                         cudaGetErrorString(le), op.tag ? op.tag : "?", e.M, e.N, e.K, e.act, op.block_n, (int)op.ln, e.split16, e.tma_store);
                 break;
+            }
             case Op::SELF_ATTN:
                 CUDA_CHECK(vb::launch_self_attention(op.qkv_a, op.ld_a, op.hidden, op.mask_a, op.ctx_a, op.ld_ctx_a, op.B, op.La,
-                                                     op.heads, op.head_dim, light_pdl(), opt.act_fp16, st, op.offs_a));
+                                                     op.heads, op.head_dim, opt.use_pdl, opt.act_fp16, st, op.offs_a));
                 break;
             case Op::CO_ATTN:
                 CUDA_CHECK(vb::launch_co_attention(op.qkv_a, op.ld_a, op.qkv_b, op.ld_b, op.hidden, op.mask_a, op.mask_b, op.ctx_a,
                                                    op.ld_ctx_a, op.ctx_b, op.ld_ctx_b, op.B, op.La, op.Lb, op.heads, op.head_dim,
-                                                   light_pdl(), opt.act_fp16, st, op.offs_a, op.offs_b));
+                                                   opt.use_pdl, opt.act_fp16, st, op.offs_a, op.offs_b));
                 break;
             case Op::LAYERNORM:
                 CUDA_CHECK(vb::launch_ln_residual(op.ln_y, op.ln_ld, op.ln_res, op.ld_x, op.ln_g, op.ln_b, cfg.ln_eps, op.ln_out_f,
                                                   op.ld_out, op.ln_out_h, op.ld_a, op.ln_M, op.ln_N, opt.act_fp16, x3 ? 1 : 0,
-                                                  light_pdl(), st, op.ln_pend.stats ? &op.ln_pend : nullptr, op.m_rows));
+                                                  opt.use_pdl, st, op.m_rows));
                 break;
             case Op::ATTN_F32:
                 CUDA_CHECK(vb::launch_attention_f32(op.f_q, op.f_ld_q, op.f_k, op.f_v, op.f_ld_kv, op.f_in, op.f_mask, op.B, op.f_Lq,
                                                     op.f_Lk, op.heads, op.head_dim, op.f_ctx, op.f_ld_ctx, op.f_ctx_mode, op.f_probs,
-                                                    light_pdl(), st));
+                                                    opt.use_pdl, st));
                 break;
             case Op::ROWDOT:
                 CUDA_CHECK(vb::launch_rowdot(op.x, op.ld_x, op.W, op.bias, op.add, op.out, op.ld_out, op.M, op.K, op.n_out, opt.use_pdl, st,
@@ -1477,56 +1272,6 @@ struct vb200_engine {
             throw;
         }
         cudaEventDestroy(e0); cudaEventDestroy(e1); cudaStreamDestroy(st);
-    }
-    // FFN-in -> FFN-out (and every other producer / consumer pair of plain 128-wide GEMMs that sit next to each other on one graph
-    // branch, the first writing only the 16-bit operand the second reads) become ONE chained launch (gemm_chain.cu).
-    void link_chains(Plan& pl) {
-        if (!chain_ffn || x3) return;
-        std::vector<Op> out;
-        out.reserve(pl.ops.size());
-        for (size_t i = 0; i < pl.ops.size(); ++i) {
-            Op a = pl.ops[i];
-            if (i + 1 < pl.ops.size() && a.kind == Op::GEMM && !a.chain_sync) {
-                const Op& b = pl.ops[i + 1];
-                auto plain = [](const Op& o) {
-                    const GemmEpilogue& e = o.ep;
-                    return o.kind == Op::GEMM && !o.pair && !o.ln && o.block_n == 128 && e.ln_mode == 0 && !e.split16 && e.res == nullptr &&
-                           e.mul == nullptr && e.gamma == nullptr && (e.N & 31) == 0 && e.act != vb::kActGeluExact;
-                };
-                if (plain(a) && plain(b) && a.stream == b.stream && b.sync == Op::NONE && a.ep.M == b.ep.M && a.ep.M >= 256 &&
-                    a.ep.out_bf16 != nullptr && a.ep.out_f32 == nullptr && (a.ep.ld_bf16 & 7) == 0 && b.a_ptr == a.ep.out_bf16 &&
-                    b.ep.K == a.ep.N && (b.ep.out_bf16 == nullptr || (b.ep.ld_bf16 & 7) == 0) && (b.ep.out_f32 == nullptr || (b.ep.ld_f32 & 3) == 0)) {
-                    a.ta2 = b.ta; a.tb2 = b.tb; a.ep2 = b.ep; a.flops2 = b.flops;
-                    const int m_tiles = (a.ep.M + 127) / 128;
-                    a.chain_sync = pl.mem.alloc_n<int>(m_tiles + 2);
-                    CUDA_CHECK(cudaMemset(a.chain_sync, 0, sizeof(int) * (m_tiles + 2)));
-                    a.ep.tma_store = 0; a.ep2.tma_store = 0;
-                    out.push_back(a);
-                    ++i;                       // b is issued by the same launch
-                    continue;
-                }
-            }
-            out.push_back(a);
-        }
-        pl.ops.swap(out);
-    }
-
-    // PDL "medium" (default): additionally launch a GEMM programmatically when the kernel before it on its graph branch is a light one
-    // (LayerNorm / attention trigger their dependents right after loading their inputs, so the GEMM's prologue -- barrier init,
-    // descriptor prefetch, first weight tiles -- overlaps the light kernel's math instead of following it).
-    void link_pdl(Plan& pl) {
-        if (!pdl_medium) return;
-        int prev_kind[2] = {-1, -1};
-        for (Op& op : pl.ops) {
-            const int st = op.stream & 1;
-            if (op.kind == Op::GEMM && op.ep.pdl == 2 &&
-                (prev_kind[st] == Op::LAYERNORM || prev_kind[st] == Op::SELF_ATTN || prev_kind[st] == Op::CO_ATTN ||
-                 prev_kind[st] == Op::ATTN_F32 ||
-                 (pdl_gemm_gemm && prev_kind[st] == Op::GEMM)))
-                op.ep.pdl = early_w ? 5 : 1;
-            prev_kind[st] = op.kind;
-            if (op.sync != Op::NONE) prev_kind[0] = prev_kind[1] = -1;      // fork / join: the predecessor set is not one kernel
-        }
     }
 
     void capture(Plan& pl) {
@@ -1718,6 +1463,7 @@ int vb200_create(const char* config_json, int64_t n_tensors, const vb200_tensor*
         if (tensors == nullptr || n_tensors <= 0) fail(VB200_ERR_CHECKPOINT, "empty state_dict");
         vb200_options o{};
         if (opt) o = *opt;
+        if (o.ln_fold != 0) fail(VB200_ERR_INVALID, "vb200_options: the LayerNorm fold was removed (its reserved field must be 0)");
         // tri-state flags: 0 = default, 1 = on, -1 = off
         o.use_cuda_graph = o.use_cuda_graph >= 0 ? 1 : 0;
         o.strict = o.strict >= 0 ? 1 : 0;
@@ -1729,7 +1475,7 @@ int vb200_create(const char* config_json, int64_t n_tensors, const vb200_tensor*
         Config c = parse_config(config_json);
         {   // audit the state_dict (names, shapes, dtypes, strictness) before touching any device
             vb200_engine audit;
-            audit.cfg = c; audit.opt = o; audit.dry = true; audit.x3 = o.split_fp32 != 0; audit.ln_fold = false;
+            audit.cfg = c; audit.opt = o; audit.dry = true; audit.x3 = o.split_fp32 != 0;
             audit.ingest(n_tensors, tensors);
         }
         require_device(o.device);
@@ -1740,20 +1486,10 @@ int vb200_create(const char* config_json, int64_t n_tensors, const vb200_tensor*
         eng->fused_ln = o.fused_layernorm != 0;
         if (const char* v = getenv("VB200_FUSED_LN")) eng->fused_ln = (strcmp(v, "1") == 0) && !eng->x3;
         if (const char* v = getenv("VB200_LONE_ROWS")) eng->lone_rows = std::max(0, atoi(v));
-        if (const char* v = getenv("VB200_PAIR")) eng->pair_mode = strcmp(v, "auto") == 0 ? -1 : (atoi(v) != 0 ? 1 : 0);
-        if (const char* v = getenv("VB200_PAIR_MIN_WAVES")) eng->pair_min_waves = std::max(1, atoi(v));
-        if (const char* v = getenv("VB200_CHAIN")) eng->chain_ffn = (strcmp(v, "0") != 0);
-        eng->ln_fold = o.ln_fold > 0;
-        if (const char* v = getenv("VB200_LNFOLD")) eng->ln_fold = (strcmp(v, "0") != 0);
-        if (eng->x3 || eng->fused_ln) eng->ln_fold = false;      // those modes keep every LayerNorm as its own step
         eng->max_plans = o.max_plans > 0 ? static_cast<size_t>(o.max_plans) : 24;
         if (const char* v = getenv("VB200_MAX_PLANS")) { const int n = atoi(v); if (n > 0) eng->max_plans = static_cast<size_t>(n); }
-        eng->pdl_light = eng->pdl_medium = false;
         if (pdl_req == 0) eng->opt.use_pdl = 1;               // default: full
         if (const char* v = getenv("VB200_PDL")) {
-            eng->pdl_gemm_gemm = strcmp(v, "mediumplus") == 0;
-            eng->pdl_light = strcmp(v, "light") == 0 || strcmp(v, "medium") == 0 || eng->pdl_gemm_gemm;
-            eng->pdl_medium = strcmp(v, "medium") == 0 || eng->pdl_gemm_gemm;
             if (strcmp(v, "full") == 0) eng->opt.use_pdl = 1;
             if (strcmp(v, "off") == 0) eng->opt.use_pdl = 0;
         }
@@ -1989,14 +1725,12 @@ int vb200_profile_ops(vb200_handle h, int32_t batch, int32_t n_tokens, int32_t n
             const Op& op = pl->ops[i];
             if (kinds) kinds[i] = static_cast<int>(op.kind);
             if (ms) ms[i] = t[i];
-            if (flops) flops[i] = op.flops + op.flops2;
+            if (flops) flops[i] = op.flops;
             if (dims) {
                 dims[4 * i + 0] = op.kind == Op::GEMM ? op.ep.M : (op.kind == Op::LAYERNORM ? op.ln_M : op.B);
                 dims[4 * i + 1] = op.kind == Op::GEMM ? op.ep.N : (op.kind == Op::LAYERNORM ? op.ln_N : op.La);
                 dims[4 * i + 2] = op.kind == Op::GEMM ? op.ep.K : op.Lb;
-                dims[4 * i + 3] = op.kind == Op::GEMM ? (op.ep.act | (op.ln ? 16 : 0) | (op.ep.ln_mode == 4 ? 32 : 0) | (op.ep.ln_mode == 5 ? 64 : 0) |
-                                                         (op.chain_sync ? 128 : 0))
-                                                      : op.heads;
+                dims[4 * i + 3] = op.kind == Op::GEMM ? (op.ep.act | (op.ln ? 16 : 0)) : op.heads;
             }
         }
     });
@@ -2017,13 +1751,6 @@ int vb200_set_option(vb200_handle h, const char* key, int64_t value) {
                 CUDA_CHECK(cudaDeviceSynchronize());
                 h->plans.clear();
                 h->timeline = value != 0;
-            }
-        } else if (k == "chain_ffn") {
-            // changes how plans are built: drop the cached ones (the device is drained first, a plan may still be executing)
-            if ((value != 0) != h->chain_ffn) {
-                CUDA_CHECK(cudaDeviceSynchronize());
-                h->plans.clear();
-                h->chain_ffn = value != 0;
             }
         } else fail(VB200_ERR_INVALID, "unknown option \"%s\"", key);
     });
@@ -2063,7 +1790,6 @@ int vb200_model_dim(vb200_handle h, const char* key, int64_t* value) {
         else if (k == "task_specific_tokens") *value = c.task_tokens;
         else if (k == "weight_bytes") *value = static_cast<int64_t>(h->weights.total);
         else if (k == "operand_width_factor") *value = h->x3 ? 3 : 1;
-        else if (k == "ln_fold") *value = h->ln_fold ? 1 : 0;
         else if (k == "n_plans") *value = static_cast<int64_t>(h->plans.size());
         else if (k == "n_layers_scheduled") *value = static_cast<int64_t>(h->schedule.size());
         else fail(VB200_ERR_INVALID, "unknown model dimension \"%s\"", key);
@@ -2084,23 +1810,21 @@ int vb200_linear(const void* x_bf16, int64_t ld_x, const void* w_bf16, int64_t l
                  int32_t block_n, int32_t use_pdl, int32_t act_fp16, int32_t variant, long long* timing, void* cuda_stream) {
     return op_guard([&] {
         const bool ln = gamma != nullptr;
-        // variant 2: CTA pair (128-wide tiles, N % 128 == 0).  Variants 3 and 4 named Blackwell occupancy configurations of the
-        // persistent kernel (three CTAs per SM; one CTA with a 6-stage ring); ABI version 2 keeps accepting them, and on sm_90a they
-        // select the persistent kernel itself.  block_n 256 (the Blackwell 256-wide tile, plain or pair) runs as 128-wide tiles,
-        // which give the same bits: the tile width never changes an element's accumulation order.
-        const bool pair = variant == 2;
-        if (variant != 0 && variant != 2 && variant != 3 && variant != 4)
-            fail(VB200_ERR_INVALID, "vb200_linear: variant %d does not exist (0 persistent, 2 CTA pair, 3 / 4 = 0)", variant);
-        int bn = block_n > 0 ? block_n : (pair ? 128 : vb::gemm_p_pick_block_n(static_cast<int>(N), ln));
+        // Variant 2 named the Blackwell CTA-pair kernel, variants 3 and 4 Blackwell occupancy configurations of the persistent kernel
+        // (three CTAs per SM; one CTA with a 6-stage ring); ABI version 2 keeps accepting them, and on sm_90a they select the
+        // persistent kernel itself.  block_n 256 (the Blackwell 256-wide tile) runs as 128-wide tiles, which give the same bits: the
+        // tile width never changes an element's accumulation order.
+        if (variant < 0 || variant == 1 || variant > 4)
+            fail(VB200_ERR_INVALID, "vb200_linear: variant %d does not exist (0 persistent, 2 / 3 / 4 = 0)", variant);
+        int bn = block_n > 0 ? block_n : vb::gemm_p_pick_block_n(static_cast<int>(N), ln);
         if (bn == 0) fail(VB200_ERR_INVALID, "no tiling for N=%lld with LayerNorm", (long long)N);
         if (!ln && bn == 256) bn = 128;
         if (!ln && bn != 64 && bn != 128 && bn != 192)
             fail(VB200_ERR_INVALID, "vb200_linear: block_n %d (plain tiles are 64, 128, 192 or 256 wide)", bn);
-        if (pair && (ln || bn != 128)) fail(VB200_ERR_INVALID, "vb200_linear: the CTA pair is the plain 128- or 256-wide tile");
-        if ((variant == 3 || variant == 4) && (ln || (bn != 128 && !(variant == 4 && bn == 64))))
-            fail(VB200_ERR_INVALID, "vb200_linear: variant 3 is the plain 128-wide tile, variant 4 the 128- or 64-wide one");
+        if (variant >= 2 && (ln || (bn != 128 && !(variant == 4 && bn == 64))))
+            fail(VB200_ERR_INVALID, "vb200_linear: variants 2 and 3 are the plain 128-wide tile, variant 4 the 128- or 64-wide one");
         CUtensorMap ta = make_tmap(x_bf16, M, K, ld_x, 128, act_fp16 != 0);
-        CUtensorMap tb = make_tmap(w_bf16, N, K, ld_w, pair ? bn / 2 : bn, act_fp16 != 0);
+        CUtensorMap tb = make_tmap(w_bf16, N, K, ld_w, bn, act_fp16 != 0);
         GemmEpilogue e{};
         e.M = (int)M; e.N = (int)N; e.K = (int)K; e.bias = bias; e.res = residual; e.ld_res = (int)ld_res;
         e.gamma = gamma; e.beta = beta; e.eps = eps; e.out_bf16 = static_cast<bf16*>(y_bf16); e.ld_bf16 = (int)ld_y_bf16;
@@ -2109,9 +1833,8 @@ int vb200_linear(const void* x_bf16, int64_t ld_x, const void* w_bf16, int64_t l
         if (const char* dbg = getenv("VB200_DEBUG")) e.debug = atoi(dbg);          // timing decomposition (kernels.h), op entry only
         CUtensorMap tc;
         const char* ts = getenv("VB200_TMASTORE");
-        if (!pair && !ln && !(ts && strcmp(ts, "0") == 0)) { setup_tma_store(&tc, e); e.tmap_c_host = e.tma_store ? &tc : nullptr; }
-        if (pair) CUDA_CHECK(vb::launch_gemm_pair(ta, tb, e, bn, static_cast<cudaStream_t>(cuda_stream)));
-        else CUDA_CHECK(vb::launch_gemm_persistent(ta, tb, e, bn, ln, static_cast<cudaStream_t>(cuda_stream)));
+        if (!ln && !(ts && strcmp(ts, "0") == 0)) { setup_tma_store(&tc, e); e.tmap_c_host = e.tma_store ? &tc : nullptr; }
+        CUDA_CHECK(vb::launch_gemm_persistent(ta, tb, e, bn, ln, static_cast<cudaStream_t>(cuda_stream)));
     });
 }
 
@@ -2165,40 +1888,6 @@ int vb200_linear_split(const void* x16, int64_t ld_x, const void* w16, int64_t l
         e.ld_bf16 = (int)ld_y16; e.out_f32 = y_f32; e.ld_f32 = (int)ld_y_f32; e.act = act; e.a_f16 = 1; e.out_f16 = 1;
         e.split16 = y16 != nullptr ? 1 : 0;
         CUDA_CHECK(vb::launch_gemm_persistent(ta, tb, e, bn, false, static_cast<cudaStream_t>(cuda_stream)));
-    });
-}
-
-int vb200_linear_ln(const void* x16, int64_t ld_x, const void* w16, int64_t ld_w, const float* bias, int32_t mode, const void* a_stats,
-                    int32_t a_parts, const float* fold_s, const float* res, int64_t ld_res, const void* res_stats, int32_t res_parts,
-                    const float* res_gamma, const float* res_beta, void* out_stats, int32_t stats_ld, float eps, int32_t act, void* y16,
-                    int64_t ld_y16, float* y_f32, int64_t ld_y_f32, int64_t M, int64_t N, int64_t K, int32_t act_fp16, void* cuda_stream) {
-    return op_guard([&] {
-        if (mode != 4 && mode != 5) fail(VB200_ERR_INVALID, "vb200_linear_ln: mode must be 4 (fold-in) or 5 (pre-LayerNorm output)");
-        CUtensorMap ta = make_tmap(x16, M, K, ld_x, 128, act_fp16 != 0);
-        CUtensorMap tb = make_tmap(w16, N, K, ld_w, 128, act_fp16 != 0);
-        GemmEpilogue e{};
-        e.M = (int)M; e.N = (int)N; e.K = (int)K; e.bias = bias; e.eps = eps; e.act = act; e.a_f16 = act_fp16 ? 1 : 0; e.out_f16 = e.a_f16;
-        e.out_bf16 = static_cast<bf16*>(y16); e.ld_bf16 = (int)ld_y16; e.out_f32 = y_f32; e.ld_f32 = (int)ld_y_f32;
-        e.ln_mode = mode; e.stats_ld = stats_ld;
-        e.a_stats = static_cast<const float2*>(a_stats); e.a_parts = a_parts; e.fold_s = fold_s;
-        e.res = res; e.ld_res = (int)ld_res; e.res_stats = static_cast<const float2*>(res_stats); e.res_parts = res_parts;
-        e.res_gamma = res_gamma; e.res_beta = res_beta; e.out_stats = static_cast<float2*>(out_stats);
-        CUDA_CHECK(vb::launch_gemm_persistent(ta, tb, e, 128, false, static_cast<cudaStream_t>(cuda_stream)));
-    });
-}
-
-int vb200_linear_chain(const void* x16, int64_t ld_x, const void* w1, int64_t ld_w1, const float* b1, int32_t act, void* h16, int64_t ld_h,
-                       const void* w2, int64_t ld_w2, const float* b2, void* y16, int64_t ld_y16, float* y_f32, int64_t ld_y_f32, int64_t M,
-                       int64_t N1, int64_t K1, int64_t N2, int32_t act_fp16, void* sync_ints, void* cuda_stream) {
-    return op_guard([&] {
-        CUtensorMap ta0 = make_tmap(x16, M, K1, ld_x, 128, act_fp16 != 0), tb0 = make_tmap(w1, N1, K1, ld_w1, 128, act_fp16 != 0);
-        CUtensorMap ta1 = make_tmap(h16, M, N1, ld_h, 128, act_fp16 != 0), tb1 = make_tmap(w2, N2, N1, ld_w2, 128, act_fp16 != 0);
-        GemmEpilogue e0{}, e1{};
-        e0.M = e1.M = (int)M; e0.N = (int)N1; e0.K = (int)K1; e1.N = (int)N2; e1.K = (int)N1;
-        e0.bias = b1; e1.bias = b2; e0.act = act; e0.a_f16 = e0.out_f16 = e1.a_f16 = e1.out_f16 = act_fp16 ? 1 : 0;
-        e0.out_bf16 = static_cast<bf16*>(h16); e0.ld_bf16 = (int)ld_h;
-        e1.out_bf16 = static_cast<bf16*>(y16); e1.ld_bf16 = (int)ld_y16; e1.out_f32 = y_f32; e1.ld_f32 = (int)ld_y_f32;
-        CUDA_CHECK(vb::launch_gemm_chain(ta0, tb0, e0, ta1, tb1, e1, static_cast<int*>(sync_ints), static_cast<cudaStream_t>(cuda_stream)));
     });
 }
 

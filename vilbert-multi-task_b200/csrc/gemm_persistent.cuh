@@ -31,12 +31,8 @@ constexpr int kBlockK = 64;
 constexpr int kMmaK = 16;
 
 // MODE 0: default.  MODE 3: the same kernel with the fp32-parity mode's hi | lo | hi 16-bit output (a compile-time variant so the
-// default kernel's register budget is untouched).  MODE 4 / 5: the LayerNorm fold (see row_stats below) -- 4 ("FOLD") consumes an
-// activation whose LayerNorm is still pending, 5 ("LNOUT") produces one.  MODE 8 ("PAIR", plain epilogue): the CTA pair -- two CTAs
-// of a cluster take the vertically adjacent 128 x BLOCK_N tiles of one 256-row panel; each loads its own A rows and HALF of the
-// weight tile, which the TMA multicasts into both CTAs, so every weight byte crosses L2 -> SM once per 256 output rows.
-// MODE 6 ("ROWS"): MODE 0 whose tile list ends at a device row count (GemmEpilogue::m_rows, packed batches) -- a variant of its
-// own so that MODE 0 keeps its register allocation.
+// default kernel's register budget is untouched).  MODE 6 ("ROWS"): MODE 0 whose tile list ends at a device row count
+// (GemmEpilogue::m_rows, packed batches) -- a variant of its own so that MODE 0 keeps its register allocation.
 // MODE 0 and 6 also come 192 wide (96 accumulators per consumer thread, a 2-stage ring): 128 x 192 tiles cover an N = 3072 GEMM in
 // 16 column tiles instead of 24.
 // One CTA per SM: each consumer thread holds BLOCK_N / 2 fp32 accumulators, and the deposited tile plus a ring deep enough to
@@ -45,8 +41,6 @@ template <int BLOCK_N, bool LN, int MODE = 0>
 struct PCfg {
     static_assert(BLOCK_N == 64 || BLOCK_N == 128 || (LN && BLOCK_N == 96) || (!LN && (MODE == 0 || MODE == 6) && BLOCK_N == 192),
                   "tile widths: 64 / 128 (LayerNorm also 96, the default plain kernel also 192)");
-    static constexpr bool PAIR = MODE == 8;
-    static_assert(!PAIR || (BLOCK_N == 128 && !LN), "the CTA pair is the plain 128-wide tile");
     static constexpr int kStageBytesA = kBlockM * kBlockK * 2;
     static constexpr int kStageBytesB = BLOCK_N * kBlockK * 2;
     static constexpr int kStageBytes = kStageBytesA + kStageBytesB;
@@ -288,31 +282,6 @@ __device__ __forceinline__ void store_f32_sw(uint4* st, float* out, int ld, int 
     }
 }
 
-// The reverse of store_f32_sw: 32 rows x 32 fp32 columns of a row-major matrix -> one row per lane.  Every global load instruction
-// reads 8 rows x 64 contiguous bytes (a row-per-lane load would touch 32 lines per instruction); 16 columns per pass through the
-// same swizzled 2 KB buffer.  Rows >= M read as zero.
-__device__ __forceinline__ void load_f32_sw(uint4* st, const float* src, int ld, int m_warp, int M, int ncol, float (&r)[32], int lane) {
-    const int j = lane & 3;
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-#pragma unroll
-        for (int it = 0; it < 4; ++it) {
-            const int row = it * 8 + (lane >> 2);
-            uint4 u = make_uint4(0u, 0u, 0u, 0u);
-            if (m_warp + row < M) u = *reinterpret_cast<const uint4*>(src + static_cast<size_t>(m_warp + row) * ld + ncol + 16 * h + 4 * j);
-            st[sw_unit(row, j)] = u;
-        }
-        __syncwarp();
-#pragma unroll
-        for (int jj = 0; jj < 4; ++jj) {
-            const uint4 u = st[sw_unit(lane, jj)];
-            const float4 f = *reinterpret_cast<const float4*>(&u);
-            r[16 * h + 4 * jj] = f.x; r[16 * h + 4 * jj + 1] = f.y; r[16 * h + 4 * jj + 2] = f.z; r[16 * h + 4 * jj + 3] = f.w;
-        }
-        __syncwarp();
-    }
-}
-
 // LayerNorm outputs (fp32 stream copy and 16-bit GEMM operand) of one chunk from an fp32 [32][33] transpose buffer.
 template <bool F16>
 __device__ __forceinline__ void store_ln_coalesced(float* st, const GemmEpilogue& p, int m_warp, int ncol, const float (&v)[32],
@@ -347,43 +316,6 @@ __device__ __forceinline__ void store_ln_coalesced(float* st, const GemmEpilogue
         }
     }
     __syncwarp();
-}
-
-// ---- LayerNorm folded into the GEMMs around it (round 2; replaces 57 of the 62 row-LayerNorm launches of a forward)
-// A residual block ends in  a = LayerNorm_{g,b}(u),  u = dense(x) + residual.  Instead of materialising `a`, the producing GEMM
-// (MODE 5) writes u -- fp32 for the residual stream, 16-bit as the next GEMM's operand -- plus, per row and 32-column chunk, the
-// pair (mean, M2 = sum (x - mean)^2).  Whoever needs `a` later rebuilds it from exact per-row statistics:
-//   * a GEMM that consumes `a` as its A operand (MODE 4) runs on u with column-scaled weights W' = g o W and finishes with
-//         y[m, n] = rstd_m * (acc[m, n] - mean_m * s_n) + c_n,     s_n = sum_k W'[n, k],  c_n = sum_k b_k W[n, k] + bias_n
-//     (algebraically LayerNorm(u) W^T + bias; s is summed over the ROUNDED 16-bit W' the tensor cores see, so the mean term
-//     cancels exactly);
-//   * a GEMM (MODE 5) or the row-LayerNorm kernel that needs `a` as its residual computes (u - mean) rstd g + b on the fly.
-// The chunk statistics are combined with Chan's parallel formula (equal counts), deterministically and per row only, so a
-// pair's result still does not depend on its batch neighbours (bit-exact sharding).  stats layout: [N / 32][ld] float2, part-major
-// (a warp's 32 rows are 256 contiguous bytes).
-__device__ __forceinline__ void row_stats(const float2* __restrict__ stats, int parts, int ld, int m, float n_cols, float eps,
-                                          float& mean, float& rstd) {
-    // eight independent loads in flight per step (a rolled loop would pay one L2 round trip per chunk); the second pass re-reads
-    // the same lines from L1.  The summation order is fixed (q ascending), so results do not depend on anything but the row.
-    const float2* sp = stats + m;
-    float sm = 0.0f;
-    for (int q0 = 0; q0 < parts; q0 += 8) {
-        float t[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) t[j] = (q0 + j < parts) ? sp[static_cast<size_t>(q0 + j) * ld].x : 0.0f;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) sm += t[j];
-    }
-    mean = sm / static_cast<float>(parts);
-    float m2 = 0.0f;
-    for (int q0 = 0; q0 < parts; q0 += 8) {
-        float2 t[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) t[j] = (q0 + j < parts) ? sp[static_cast<size_t>(q0 + j) * ld] : make_float2(mean, 0.0f);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) { const float d = t[j].x - mean; m2 += t[j].y + 32.0f * d * d; }
-    }
-    rstd = 1.0f / sqrtf(m2 / n_cols + eps);
 }
 
 template <int BLOCK_N, bool LN, int ACT, bool F16, int MODE = 0>
@@ -435,10 +367,6 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
     // ---- tile assignment.  Non-LN: CTA b takes tiles b, b+grid, ... with the N index fastest (CTAs that run together
     // share an A row-panel in L2).  LN: gridDim.x = cluster size = num_n_tiles, blockIdx.y = cluster id; cluster c takes
     // M tiles c, c + gridDim.y, ... and the CTA's rank in the cluster is its (fixed) N tile.
-    // PAIR: cluster c = blockIdx.x / 2 walks pair tiles c, c + grid / 2, ... (256-row panel, N index fastest); rank r of the
-    // cluster takes the 128 rows 256 * panel + 128 r (a last odd panel leaves rank 1 all rows >= M: it still loads and
-    // multicasts its half of W, and its zero-filled rows are never stored).
-    constexpr bool PAIR = Cfg::PAIR;
     // Packed batches (p.m_rows): the producer and the consumers derive the same, shorter tile list from the device row count --
     // M tiles whose first row is at or past it do not exist for this launch.  The count is written before the graph starts.  A CTA
     // left without a tile triggers its dependents by exiting.
@@ -447,19 +375,17 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
         const int mr = max(0, min(*p.m_rows, p.M));
         run_m_tiles = min(num_m_tiles, (mr + kBlockM - 1) / kBlockM);
     }
-    const int total_tiles = LN ? num_m_tiles : (PAIR ? (num_m_tiles + 1) / 2 : run_m_tiles) * num_n_tiles;
-    const int first_tile = LN ? static_cast<int>(blockIdx.y) : static_cast<int>(PAIR ? blockIdx.x >> 1 : blockIdx.x);
-    const int tile_stride = LN ? static_cast<int>(gridDim.y) : static_cast<int>(PAIR ? gridDim.x >> 1 : gridDim.x);
-    const uint32_t cluster_size = (LN || PAIR) ? cluster_nctarank() : 1u;
-    const uint32_t my_rank = (LN || PAIR) ? cluster_ctarank() : 0u;
-    auto tile_m0 = [&](int tile) {
-        return (LN ? tile : (PAIR ? 2 * (tile / num_n_tiles) + static_cast<int>(my_rank) : tile / num_n_tiles)) * kBlockM;
-    };
+    const int total_tiles = LN ? num_m_tiles : run_m_tiles * num_n_tiles;
+    const int first_tile = LN ? static_cast<int>(blockIdx.y) : static_cast<int>(blockIdx.x);
+    const int tile_stride = LN ? static_cast<int>(gridDim.y) : static_cast<int>(gridDim.x);
+    const uint32_t cluster_size = LN ? cluster_nctarank() : 1u;
+    const uint32_t my_rank = LN ? cluster_ctarank() : 0u;
+    auto tile_m0 = [&](int tile) { return (LN ? tile : tile / num_n_tiles) * kBlockM; };
     auto tile_n0 = [&](int tile) { return (LN ? static_cast<int>(my_rank) : tile % num_n_tiles) * BLOCK_N; };
 
     // ---------------------------------------------------------------- one-time setup
     // The producer thread does not wait for the CTA-wide setup barrier: as soon as ITS barriers exist it puts the first ring
-    // pass of the first tile in flight -- activations and weights when the kernel has no programmatic dependency (pdl 0 / 2),
+    // pass of the first tile in flight -- activations and weights when the kernel has no programmatic dependency (pdl 0),
     // only the weights (they do not depend on the previous kernel) when it was launched programmatically with pdl == 5; the
     // activation tiles then follow after griddepcontrol.wait.
     int early = 0;                 // k-blocks of the first tile already (partly) in flight     } producer thread only
@@ -470,7 +396,7 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
         if (!LN && p.tma_store) tma_prefetch_desc(&tmap_c);
         for (int s = 0; s < kStages; ++s) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], (PAIR ? 2 : 1) * Cfg::kConsumerWarps);   // one arrival per consumer warp (PAIR: of both CTAs)
+            mbar_init(&empty_bar[s], Cfg::kConsumerWarps);                   // one arrival per consumer warp
         }
         for (int a = 0; a < 2; ++a) {
             mbar_init(&ln_bar[a], LN ? cluster_size : 1u);                   // one arrival per CTA of the cluster
@@ -481,7 +407,7 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
 #else
         constexpr bool early_ok = true;
 #endif
-        if (!LN && !PAIR && first_tile < total_tiles && p.pdl != 1 && early_ok) {
+        if (!LN && first_tile < total_tiles && p.pdl != 1 && early_ok) {
             early_a = p.pdl != 5;
             const int m0 = (first_tile / num_n_tiles) * kBlockM, n0 = (first_tile % num_n_tiles) * BLOCK_N;
             early = min(kStages, num_kb);
@@ -500,7 +426,7 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
             s_beta[i] = p.beta[n0 + i];
         }
     }
-    if (LN || PAIR) cluster_sync_all(); else __syncthreads();   // peers' barriers must be initialised before remote arrives / multicasts
+    if (LN) cluster_sync_all(); else __syncthreads();           // peers' barriers must be initialised before remote arrives
     if (stamps && threadIdx.x == 0) stamps[1] = clock64();
 
     // Programmatic dependent launch: everything above overlapped the previous kernel's tail; its outputs are visible after the
@@ -535,13 +461,7 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
                         {
                             mbar_arrive_expect_tx(&full_bar[s], Cfg::kStageBytes);
                             tma_load_2d(sa, &tmap_a, &full_bar[s], kb * kBlockK, m0);
-                            if constexpr (PAIR) {      // my half of the weight rows, into the same offset of both CTAs
-                                constexpr int kHalf = BLOCK_N / 2;
-                                tma_load_2d_mcast(sb + my_rank * kHalf * 128, &tmap_b, &full_bar[s], kb * kBlockK,
-                                                  n0 + static_cast<int>(my_rank) * kHalf, 0x3);
-                            } else {
-                                tma_load_2d(sb, &tmap_b, &full_bar[s], kb * kBlockK, n0);
-                            }
+                            tma_load_2d(sb, &tmap_b, &full_bar[s], kb * kBlockK, n0);
                         }
                     }
                     if (++s == kStages) { s = 0; phase ^= 1u; }
@@ -558,15 +478,9 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
         const uint64_t db0 = gmma_desc_kmajor_sw128(smem_u32(ring + Cfg::kStageBytesA));
         int ks = 0;
         uint32_t kphase = 0;
-        // a stage is free once this warp's wgmma have read it; PAIR: the peer's producer writes half of it too, so both CTAs' barriers
+        // a stage is free once this warp's wgmma have read it
         auto release = [&](int st) __attribute__((always_inline)) {
-            if (lane != 0) return;
-            if constexpr (PAIR) {
-                mbar_arrive_remote_release(mapa_u32(&empty_bar[st], 0));
-                mbar_arrive_remote_release(mapa_u32(&empty_bar[st], 1));
-            } else {
-                mbar_arrive(&empty_bar[st]);
-            }
+            if (lane == 0) mbar_arrive(&empty_bar[st]);
         };
         // accumulate tile `tile` and deposit it in s_acc; returns once all 128 rows are there
         auto mma_tile = [&](int tile, uint32_t it) __attribute__((always_inline)) {
@@ -622,16 +536,6 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
                 // the reads before the next tile's writes
                 for (int i = et; i < BLOCK_N; i += kEpiThreads) s_bias[i] = (p.bias && n0 + i < p.N) ? p.bias[n0 + i] : 0.0f;
                 epi_bar_sync<kEpiThreads>();
-                // LayerNorm fold: this row's statistics, computed while the main loop runs (the epilogue warps are idle until the
-                // accumulator is ready).  a_*: pending LayerNorm of the A operand (MODE 4); r_*: of the residual (MODE 5).
-                float a_mean = 0.0f, a_rstd = 1.0f, r_mean = 0.0f, r_rstd = 1.0f;
-                if constexpr (MODE == 4) {
-                    if (m_ok) row_stats(p.a_stats, p.a_parts, p.stats_ld, m, static_cast<float>(p.a_parts * 32), p.eps, a_mean, a_rstd);
-                }
-                if constexpr (MODE == 5) {
-                    if (m_ok && p.res_stats != nullptr)
-                        row_stats(p.res_stats, p.res_parts, p.stats_ld, m, static_cast<float>(p.res_parts * 32), p.eps, r_mean, r_rstd);
-                }
                 mma_tile(tile, it);
                 if (stamp) stamps[4] = clock64();
                 float* const out_f32 = p.out_f32;
@@ -643,48 +547,7 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
                                      (p.tma_store == 1 ? (p.out_bf16 != nullptr && p.out_f32 == nullptr)
                                                        : (p.out_f32 != nullptr && p.out_bf16 == nullptr));
                 auto finish_chunk = [&](float (&v)[32], int nc) __attribute__((always_inline)) {
-                    if constexpr (MODE == 4) {                       // y = rstd * (acc - mean * s) + c; c arrives as the bias below
-                        const float4* s4 = reinterpret_cast<const float4*>(p.fold_s + nc);
-                        const float ms = -a_mean * a_rstd;
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            const float4 sv = (nc + 4 * j < p.N) ? __ldg(s4 + j) : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-                            v[4 * j] = fmaf(v[4 * j], a_rstd, ms * sv.x); v[4 * j + 1] = fmaf(v[4 * j + 1], a_rstd, ms * sv.y);
-                            v[4 * j + 2] = fmaf(v[4 * j + 2], a_rstd, ms * sv.z); v[4 * j + 3] = fmaf(v[4 * j + 3], a_rstd, ms * sv.w);
-                        }
-                    }
                     bias_act32<ACT>(v, bias_t + (nc - n0));
-                    if constexpr (MODE == 5) {
-                        // u = acc + bias + residual (the residual's own LayerNorm applied on the fly when it is still pending),
-                        // then this chunk's (mean, M2) for whoever consumes LayerNorm(u)
-                        if (p.res != nullptr) {                         // warp-uniform
-                            float r[32];
-                            load_f32_sw(reinterpret_cast<uint4*>(s_xpose + ew * Cfg::kXposeBytesPerWarp), p.res, p.ld_res, m0 + q * 32, p.M,
-                                        nc, r, lane);
-                            if (p.res_stats != nullptr) {
-                                const float4* g4 = reinterpret_cast<const float4*>(p.res_gamma + nc);
-                                const float4* b4 = reinterpret_cast<const float4*>(p.res_beta + nc);
-                                const float rs = r_rstd, rm = -r_mean * r_rstd;
-#pragma unroll
-                                for (int j = 0; j < 8; ++j) {
-                                    const float4 g = __ldg(g4 + j), b = __ldg(b4 + j);
-                                    v[4 * j] += fmaf(fmaf(r[4 * j], rs, rm), g.x, b.x); v[4 * j + 1] += fmaf(fmaf(r[4 * j + 1], rs, rm), g.y, b.y);
-                                    v[4 * j + 2] += fmaf(fmaf(r[4 * j + 2], rs, rm), g.z, b.z); v[4 * j + 3] += fmaf(fmaf(r[4 * j + 3], rs, rm), g.w, b.w);
-                                }
-                            } else {
-#pragma unroll
-                                for (int j = 0; j < 32; ++j) v[j] += r[j];
-                            }
-                        }
-                        float cs = 0.0f;
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) cs += v[j];
-                        const float cm = cs * (1.0f / 32.0f);
-                        float m2 = 0.0f;
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) { const float d = v[j] - cm; m2 = fmaf(d, d, m2); }
-                        if (m_ok) p.out_stats[static_cast<size_t>(nc >> 5) * p.stats_ld + m] = make_float2(cm, m2);
-                    }
 #ifdef VB200_DECOMPOSE
                     if ((p.debug & 2) && __float_as_uint(v[0]) != 0x7fc12345u) return;     // timing decomposition: no stores
 #endif
@@ -881,8 +744,8 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
     }
 
     // ---------------------------------------------------------------- teardown
-    // nobody exits while a peer may still read its partials (LN) or multicast into / arrive on its shared memory (PAIR)
-    if (LN || PAIR) cluster_sync_all(); else __syncthreads();
+    // nobody exits while a peer may still read its partials (LN)
+    if (LN) cluster_sync_all(); else __syncthreads();
     if (stamps && threadIdx.x == 0) {
         unsigned long long gt;
         asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt));
@@ -948,23 +811,21 @@ cudaError_t launch_p(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpi
         // Persistent grid: every SM (one CTA each) by default.  VB200_GRID_PCT caps it at that percentage of the SMs, leaving room
         // for kernels of the other ViLBERT stream / the other in-flight batch.
         static const int env_pct = [] { const char* e = getenv("VB200_GRID_PCT"); const int v = e ? atoi(e) : 100; return (v >= 10 && v <= 100) ? v : 100; }();
-        // PAIR: counted in clusters of two CTAs and pair tiles of 256 rows
-        if (Cfg::PAIR) cluster = 2;
-        const int tiles = (Cfg::PAIR ? (m_tiles + 1) / 2 : m_tiles) * n_tiles;
+        const int tiles = m_tiles * n_tiles;
         const int pct = (ep.grid_pct >= 10 && ep.grid_pct <= 100) ? ep.grid_pct : env_pct;     // per-launch override (profiling: timed alone)
-        const int slots = std::max(1, num_sms() * Cfg::kMinBlocks * pct / 100 / cluster);
+        const int slots = std::max(1, num_sms() * Cfg::kMinBlocks * pct / 100);
         // balanced walk: every CTA gets the same number of tiles (+-1): tiles = 288, cap 132 -> 96 CTAs x 3 instead of 24 x 3 + 108 x 2
         static const bool balance = [] { const char* e = getenv("VB200_GRID_BALANCE"); return e == nullptr || atoi(e) != 0; }();
         int g = std::min(tiles, slots);
         if (balance && tiles > slots) { const int per = (tiles + slots - 1) / slots; g = (tiles + per - 1) / per; }
-        grid = dim3(g * cluster, 1, 1);
+        grid = dim3(g, 1, 1);
     }
     cudaLaunchConfig_t cfg;
     cudaLaunchAttribute attrs[2];
     fill_cfg<Cfg, LN>(cfg, attrs, grid, cluster, ep.pdl == 1 || ep.pdl == 5, st);
     GemmEpilogue e2 = ep;
     const CUtensorMap* tc = static_cast<const CUtensorMap*>(ep.tmap_c_host);
-    if (tc == nullptr || LN || Cfg::PAIR) { e2.tma_store = 0; tc = &ta; }          // &ta: any valid map for the unused slot
+    if (tc == nullptr || LN) { e2.tma_store = 0; tc = &ta; }                       // &ta: any valid map for the unused slot
     return cudaLaunchKernelEx(&cfg, kern, ta, tb, *tc, e2, m_tiles, n_tiles);
 }
 

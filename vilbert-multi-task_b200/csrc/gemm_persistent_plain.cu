@@ -28,47 +28,14 @@ static cudaError_t dispatch_split(const CUtensorMap& ta, const CUtensorMap& tb, 
     return cudaErrorInvalidValue;
 }
 
-// LayerNorm fold (PCfg MODE 4 / 5, see row_stats in gemm_persistent.cuh)
-template <int BN>
-static cudaError_t dispatch_fold(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilogue& ep, cudaStream_t st) {
-    const bool f16 = ep.a_f16 != 0;
-    if (ep.ln_mode == 5) {
-        if (ep.act != kActNone) return cudaErrorInvalidValue;
-        return f16 ? launch_p<BN, false, kActNone, true, 5>(ta, tb, ep, 0, st) : launch_p<BN, false, kActNone, false, 5>(ta, tb, ep, 0, st);
-    }
-    switch (ep.act) {
-        case kActNone: return f16 ? launch_p<BN, false, kActNone, true, 4>(ta, tb, ep, 0, st) : launch_p<BN, false, kActNone, false, 4>(ta, tb, ep, 0, st);
-        case kActGelu: return f16 ? launch_p<BN, false, kActGelu, true, 4>(ta, tb, ep, 0, st) : launch_p<BN, false, kActGelu, false, 4>(ta, tb, ep, 0, st);
-    }
-    return cudaErrorInvalidValue;
-}
-
-// CTA pair (PCfg MODE 8): 256 x 128 tiles per cluster of two, tmap_b box rows = 64 (each CTA loads and multicasts half of W)
-cudaError_t launch_gemm_pair(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilogue& ep, int block_n, cudaStream_t st) {
-    if (block_n != 128 || ep.M < 1 || ep.K < 1 || ep.N < 128 || (ep.N % 128) || ep.res != nullptr || ep.gamma != nullptr ||
-        ep.ln_mode != 0 || ep.split16 || ep.act == kActGeluExact || ep.a_f16 != ep.out_f16)
-        return cudaErrorInvalidValue;
-    return dispatch_act<128, 8>(ta, tb, ep, st);
-}
-
 cudaError_t launch_gemm_persistent_plain(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilogue& ep, int block_n,
                                          cudaStream_t st) {
-    if ((ep.res != nullptr && ep.ln_mode != 5) || ep.a_f16 != ep.out_f16) return cudaErrorInvalidValue;   // residual only with LayerNorm
+    if (ep.res != nullptr || ep.a_f16 != ep.out_f16) return cudaErrorInvalidValue;   // residual only with LayerNorm
     if (ep.split16 || ep.act == kActGeluExact) {
         // hi | lo | hi output: fp16, whole 64-column groups, no TMA store; narrow tiles only (the mode is for parity, not speed)
         if (!ep.a_f16 || (ep.split16 && (ep.out_bf16 == nullptr || (ep.N & 63) || (ep.ld_bf16 & 7))) || ep.tma_store == 1)
             return cudaErrorInvalidValue;
         return block_n == 64 ? dispatch_split<64>(ta, tb, ep, st) : dispatch_split<128>(ta, tb, ep, st);
-    }
-    if (ep.ln_mode == 4 || ep.ln_mode == 5) {
-        // fold-in: statistics + s of a LayerNorm over whole 32-column chunks; producer: fp32 + 16-bit u and its statistics
-        if (block_n != 128 || (ep.N & 31) || ep.mul != nullptr || ep.stats_ld < ep.M) return cudaErrorInvalidValue;
-        if (ep.ln_mode == 4 && (ep.a_stats == nullptr || ep.fold_s == nullptr || ep.a_parts < 1 || ep.bias == nullptr)) return cudaErrorInvalidValue;
-        if (ep.ln_mode == 5 && (ep.out_stats == nullptr || ep.out_f32 == nullptr || ep.out_bf16 == nullptr || (ep.ld_f32 & 3) || (ep.ld_bf16 & 7) ||
-                                (ep.res != nullptr && (ep.ld_res & 3)) ||
-                                (ep.res_stats != nullptr && (ep.res == nullptr || ep.res_gamma == nullptr || ep.res_beta == nullptr || ep.res_parts * 32 != ep.N))))
-            return cudaErrorInvalidValue;
-        return dispatch_fold<128>(ta, tb, ep, st);
     }
     const bool rows = ep.m_rows != nullptr;          // MODE 6: the tile list ends at a device row count (packed batches)
     switch (block_n) {

@@ -22,11 +22,10 @@ struct GemmEpilogue {
     float* out_f32;               // optional
     int ld_f32;
     int act;
-    int pdl;                      // in-kernel griddepcontrol.wait / launch_dependents; 1 = also LAUNCHED with programmatic stream
-                                  // serialization, 2 = trigger only (this GEMM waits for its predecessor the normal way, but
-                                  // lets a light dependent -- LayerNorm, attention -- start under its epilogue),
-                                  // 5 = as 1, and the producer puts the first ring pass of WEIGHT tiles in flight before
-                                  // griddepcontrol.wait (weights do not depend on the previous kernel)
+    int pdl;                      // 0 = no programmatic dependent launch; 1 = LAUNCHED with programmatic stream serialization
+                                  // (in-kernel griddepcontrol.wait / launch_dependents); 5 = as 1, and the producer puts the
+                                  // first ring pass of WEIGHT tiles in flight before griddepcontrol.wait (weights do not depend
+                                  // on the previous kernel)
     int a_f16;                    // both GEMM operands (activations A, weights W) are fp16 instead of bf16
     int out_f16;                  // 16-bit output is fp16 instead of bf16
     int split16;                  // fp32-parity mode: the 16-bit output is written as fp16 hi | lo | hi per 64 columns
@@ -35,25 +34,14 @@ struct GemmEpilogue {
     const void* tmap_c_host;      // host pointer to the CUtensorMap of the output (launchers copy it into a kernel parameter)
     int tma_store;                // 0: register/LSU stores only; 1: 16-bit output, 2: fp32 output may leave through a TMA store
                                   // (plain persistent kernel: the LAST tile of every CTA is staged in the idle operand ring)
-    // LayerNorm fold (gemm_persistent.cuh, PCfg MODE 4 / 5).  stats arrays: [N_src / 32][stats_ld] float2 (mean, M2) per 32 columns
-    const float2* a_stats;        // MODE 4: statistics of the A operand's rows (its LayerNorm is pending); bias then holds c
-    int a_parts;                  //         N_src / 32
-    const float* fold_s;          //         s_n = sum_k W'[n, k]   [N]
-    const float2* res_stats;      // MODE 5: statistics of the residual's rows, or null when the residual holds final values
-    int res_parts;
-    const float* res_gamma;       //         the residual's pending LayerNorm parameters [N]
-    const float* res_beta;
-    float2* out_stats;            // MODE 5: this GEMM's own row statistics, [N / 32][stats_ld]
-    int stats_ld;                 // row capacity of every stats array of this launch (>= M)
     int grid_pct;                 // 0: default persistent grid (2/3 of the CTA slots, launch_p); 10..100: this percentage of them
-    int ln_mode;                  // 0 none, 4 fold-in (consumer), 5 pre-LayerNorm output + statistics (producer)
     int debug;                    // timing decomposition only (VB200_DEBUG through vb200_linear): 1 = issue no MMA, 2 = no epilogue
                                   // stores, 4 = no operand loads (the ring is "filled" by plain arrives); results are garbage
     const int* m_rows;            // optional device row count (packed batches): rows >= min(*m_rows, M) are neither loaded nor
                                   // computed -- the tile list ends at the last 128-row tile holding a row below it.  Written
                                   // before the launch's graph starts, so it is read ahead of griddepcontrol.wait.  Honoured by
-                                  // the plain persistent kernel (PCfg MODE 6 in place of MODE 0); the fp32-parity, LayerNorm
-                                  // fold, cluster-LayerNorm, pair and chain kernels compute every row.
+                                  // the plain persistent kernel (PCfg MODE 6 in place of MODE 0); the fp32-parity and
+                                  // cluster-LayerNorm kernels compute every row.
 };
 
 // persistent CTAs / clusters, wgmma consumer warpgroups, single-exchange LayerNorm (gemm_persistent.cuh)
@@ -62,13 +50,6 @@ int gemm_p_max_clusters(int block_n, int cluster);
 cudaError_t launch_gemm_persistent(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b, const GemmEpilogue& ep,
                                    int block_n, bool ln, cudaStream_t st);
 int num_sms_host();          // SM count of the current device (132 on H100 SXM)
-// CTA pair (gemm_persistent.cuh PCfg MODE 8: a cluster of two CTAs shares each weight tile through TMA multicast, 256 x 128 tile
-// per pair; plain epilogue, N % 128 == 0); tmap_b box rows = block_n / 2
-cudaError_t launch_gemm_pair(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b, const GemmEpilogue& ep, int block_n,
-                             cudaStream_t stream);
-// Two dependent GEMMs (FFN-in -> FFN-out) in one persistent launch with a dynamic tile list (gemm_chain.cu); sync: (M tiles + 2) zeroed ints
-cudaError_t launch_gemm_chain(const CUtensorMap& ta0, const CUtensorMap& tb0, const GemmEpilogue& ep0, const CUtensorMap& ta1,
-                              const CUtensorMap& tb1, const GemmEpilogue& ep1, int* sync, cudaStream_t st);
 cudaError_t launch_gemm_persistent_plain(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b, const GemmEpilogue& ep,
                                          int block_n, cudaStream_t st);
 
@@ -88,14 +69,9 @@ cudaError_t launch_co_attention(const __nv_bfloat16* qkv_img, int ld_img, const 
                                 const int* offs_t = nullptr, const int* offs_v = nullptr);   // as launch_self_attention, per stream
 
 // un-fused LayerNorm(y + res): fp32 stream out + 16-bit operand out (layernorm.cu); split16: hi | lo | hi operand (fp32-parity mode)
-struct LnPending {                // a residual whose own LayerNorm is still pending (LayerNorm fold): statistics + parameters
-    const float2* stats;          // [parts][ld] (mean, M2) per 32 columns
-    int parts, ld;
-    const float *gamma, *beta;
-};
 cudaError_t launch_ln_residual(const float* y, int ld_y, const float* res, int ld_res, const float* gamma, const float* beta,
                                float eps, float* out_f32, int ld_f32, __nv_bfloat16* out16, int ld16, int M, int N, int f16,
-                               int split16, int pdl, cudaStream_t st, const LnPending* res_pending = nullptr,
+                               int split16, int pdl, cudaStream_t st,
                                const int* m_rows = nullptr);   // optional device row count: rows >= *m_rows are skipped
 // K2: word + position + token-type gather, task-token row at index 1, LayerNorm; also builds the additive text mask.
 cudaError_t launch_text_embed(const int64_t* ids, const int64_t* seg, const int64_t* input_mask, const int64_t* task,

@@ -19,8 +19,6 @@ constexpr int kLnMaxVec = 16;   // N <= 2048: float4 per lane per 128 columns
 template <bool F16, bool SPLIT, int NV>
 __global__ void __launch_bounds__(256)
 ln_residual_kernel(const float* __restrict__ y, int ld_y, const float* __restrict__ res, int ld_res,
-                   const float2* __restrict__ res_stats, int res_parts, int stats_ld, const float* __restrict__ res_gamma,
-                   const float* __restrict__ res_beta,
                    const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
                    float* __restrict__ out_f32, int ld_f32, uint16_t* __restrict__ out16, int ld16, int M, int N, int pdl,
                    const int* __restrict__ m_rows) {
@@ -31,15 +29,6 @@ ln_residual_kernel(const float* __restrict__ y, int ld_y, const float* __restric
     const int nvec = NV < kLnMaxVec ? NV : (N >> 7);
     const float4* yp = reinterpret_cast<const float4*>(y + static_cast<size_t>(row) * ld_y);
     const float4* rp = res ? reinterpret_cast<const float4*>(res + static_cast<size_t>(row) * ld_res) : nullptr;
-    // residual whose own LayerNorm is still pending (LayerNorm fold, gemm_persistent.cuh row_stats): rebuild it on the fly
-    float r_mean = 0.0f, r_rstd = 1.0f;
-    if (res_stats != nullptr) {
-        const float2 t = lane < res_parts ? res_stats[static_cast<size_t>(lane) * stats_ld + row] : make_float2(0.0f, 0.0f);
-        r_mean = warp_sum(t.x) / static_cast<float>(res_parts);
-        const float d = t.x - r_mean;
-        const float m2 = warp_sum(lane < res_parts ? t.y + 32.0f * d * d : 0.0f);
-        r_rstd = 1.0f / sqrtf(m2 / static_cast<float>(res_parts * 32) + eps);
-    }
     float4 x[NV];
     float s = 0.0f;
 #pragma unroll
@@ -47,13 +36,7 @@ ln_residual_kernel(const float* __restrict__ y, int ld_y, const float* __restric
         if (k < nvec) {
             float4 a = yp[lane + 32 * k];
             if (rp) {
-                float4 r = rp[lane + 32 * k];
-                if (res_stats != nullptr) {
-                    const float4 g = reinterpret_cast<const float4*>(res_gamma)[lane + 32 * k];
-                    const float4 b = reinterpret_cast<const float4*>(res_beta)[lane + 32 * k];
-                    r.x = fmaf((r.x - r_mean) * r_rstd, g.x, b.x); r.y = fmaf((r.y - r_mean) * r_rstd, g.y, b.y);
-                    r.z = fmaf((r.z - r_mean) * r_rstd, g.z, b.z); r.w = fmaf((r.w - r_mean) * r_rstd, g.w, b.w);
-                }
+                const float4 r = rp[lane + 32 * k];
                 a.x += r.x; a.y += r.y; a.z += r.z; a.w += r.w;
             }
             x[k] = a;
@@ -103,12 +86,7 @@ ln_residual_kernel(const float* __restrict__ y, int ld_y, const float* __restric
 
 cudaError_t launch_ln_residual(const float* y, int ld_y, const float* res, int ld_res, const float* gamma, const float* beta,
                                float eps, float* out_f32, int ld_f32, __nv_bfloat16* out16, int ld16, int M, int N, int f16,
-                               int split16, int pdl, cudaStream_t st, const LnPending* rp, const int* m_rows) {
-    const float2* res_stats = rp ? rp->stats : nullptr;
-    const int res_parts = rp ? rp->parts : 0, stats_ld = rp ? rp->ld : 0;
-    const float *res_gamma = rp ? rp->gamma : nullptr, *res_beta = rp ? rp->beta : nullptr;
-    if (res_stats != nullptr && (res == nullptr || res_parts < 1 || res_parts > 32 || res_parts * 32 != N || stats_ld < M || !res_gamma || !res_beta))
-        return cudaErrorInvalidValue;
+                               int split16, int pdl, cudaStream_t st, const int* m_rows) {
     if (N % 128 != 0 || N / 128 > kLnMaxVec || (ld_y & 3) || (res && (ld_res & 3)) || (out_f32 && (ld_f32 & 3)) ||
         (out16 && (ld16 & 3)) || M < 1 || (split16 && !f16))
         return cudaErrorInvalidValue;
@@ -116,8 +94,7 @@ cudaError_t launch_ln_residual(const float* y, int ld_y, const float* res, int l
     static const int rows_per_cta = [] { const char* e = getenv("VB200_LN_ROWS"); const int v = e ? atoi(e) : 2; return (v >= 1 && v <= 8) ? v : 2; }();
     const dim3 grid((M + rows_per_cta - 1) / rows_per_cta), block(32 * rows_per_cta);
     uint16_t* o16 = reinterpret_cast<uint16_t*>(out16);
-#define VB_LN(F, S, V) launch_ex(ln_residual_kernel<F, S, V>, grid, block, 0, pdl, st, y, ld_y, res, ld_res, res_stats, res_parts, \
-                               stats_ld, res_gamma, res_beta, gamma, beta, eps,                                                  \
+#define VB_LN(F, S, V) launch_ex(ln_residual_kernel<F, S, V>, grid, block, 0, pdl, st, y, ld_y, res, ld_res, gamma, beta, eps, \
                                out_f32, ld_f32, o16, ld16, M, N, pdl, m_rows)
     if (split16) return VB_LN(true, true, kLnMaxVec);
     if (N == 768) return f16 ? VB_LN(true, false, 6) : VB_LN(false, false, 6);

@@ -47,7 +47,7 @@ class VILBertForVLTasks(object):
 
     def __init__(self, config: BertConfig, num_labels: int = 3129, state_dict=None, default_gpu: bool = True,
                  use_cuda_graph: bool = True, use_pdl: Optional[bool] = None, strict: bool = True, compute_dtype: str = "fp16",
-                 fused_layernorm: bool = False, return_attention: bool = False, max_plans: int = 0, ln_fold: bool = False):
+                 fused_layernorm: bool = False, return_attention: bool = False, max_plans: int = 0):
         self.config = config
         self.num_labels = num_labels
         self._sd = _normalise_state_dict(state_dict) if state_dict is not None else None
@@ -60,7 +60,7 @@ class VILBertForVLTasks(object):
         # the reference's fp32 forward, 3x the tensor work).  Accumulation, residual stream, LayerNorm, softmax and logits are
         # fp32 in every mode.
         self._opts = dict(use_cuda_graph=use_cuda_graph, use_pdl=use_pdl, strict=strict, compute_dtype=compute_dtype,
-                          fused_layernorm=fused_layernorm, max_plans=int(max_plans), ln_fold=bool(ln_fold))
+                          fused_layernorm=fused_layernorm, max_plans=int(max_plans))
         # attn_data_list (element 9 of the tuple): the reference returns the 24 layers' attention probabilities when called with
         # output_all_attention_masks=True (worker.py:287-288) and never reads them; here they are computed only when this flag
         # is set as well (model.return_attention = True), otherwise element 9 is [].
@@ -150,7 +150,6 @@ class VILBertForVLTasks(object):
         opt.fused_layernorm = 1 if self._opts["fused_layernorm"] else 0
         opt.split_fp32 = 1 if self._opts["compute_dtype"] == "fp32x" else 0
         opt.max_plans = self._opts["max_plans"]
-        opt.ln_fold = 1 if self._opts["ln_fold"] else 0
         h = C.c_void_p()
         with torch.cuda.device(device):
             rc = lib.vb200_create(self._config_json(), len(self._sd), arr, C.byref(opt), C.byref(h))
@@ -197,7 +196,7 @@ class VILBertForVLTasks(object):
         return n.value, f.value
 
     def set_option(self, key, value):
-        """Run-time knobs of the engine (include/vilbert_b200.h, vb200_set_option): "max_plans", "chain_ffn", "profile_grid_pct"."""
+        """Run-time knobs of the engine (include/vilbert_b200.h, vb200_set_option): "max_plans", "timeline", "profile_grid_pct"."""
         L.check(L.load().vb200_set_option(self._handle, key.encode(), int(value)), self._handle)
 
     def profile_ops(self, batch, n_tokens, n_regions, select=L.OUT_TASK_HEADS, iters=5, grid_pct=0):
