@@ -13,7 +13,8 @@
  * vb200_create <- from_pretrained + cuda(i); vb200_forward <- __call__; vb200_destroy <- del.
  * Beyond the protocol: packed variable-length batches (vb200_packed_inputs: samples with their own text lengths and region counts
  * in one forward, plans keyed on capacity buckets, GEMM tiles past the call's row totals skipped), detector output in
- * (vb200_region_inputs), caption-image retrieval with reuse, and kernel-level entry points for the tests.
+ * (vb200_region_inputs), caption-image retrieval with reuse, dense or packed (vb200_packed_pairs: captions and images encoded once
+ * at their own lengths, pairs scored without padding), and kernel-level entry points for the tests.
  * The Python shim in vilbert-multi-task_b200/ (ctypes) implements the protocol on top of them; see
  * INTEGRATION.md for the stub a maintainer of the reference would add.
  *
@@ -271,6 +272,39 @@ int vb200_forward_cached(vb200_handle h, int32_t batch, int32_t n_tokens, int32_
                          int32_t n_text, const float* text_f32, const void* text_16, const float* text_mask,
                          const int32_t* image_index, int32_t n_image, const float* image_f32, const void* image_16,
                          const float* image_mask, const vb200_outputs* out, uint32_t select, int32_t slot, void* cuda_stream);
+
+/* ---- Packed caption-image retrieval: the reuse above with every caption and image at its own length, stored back to back as in
+ * vb200_packed_inputs, with no padding and no masks: every row is real.  Caption c's state is rows [sum_{c' < c} T_c', ... + T_c) with
+ * T_c = Tin_c + 1 (task token); image i's state is rows [sum_{i' < i} V_i', ... + V_i).  State buffers are caller-allocated device
+ * memory: fp32 [sum rows, hidden] and 16-bit [sum rows, hidden] (2 bytes per element).  Each caption's / image's rows are bit-identical
+ * to vb200_encode_text / vb200_encode_image of that item alone at its own length.  Capacities follow vb200_forward_packed: 0 means
+ * this call's maximum, and plans are keyed on round16 of the capacity.  VB200_ERR_INVALID for split_fp32 engines, NULL pointers, a
+ * length < 1 or above a non-zero capacity, T or V > 256 and Tin > max_position_embeddings. */
+int vb200_encode_text_packed(vb200_handle h, int32_t n, int32_t max_tokens, const int32_t* n_tokens /* HOST [n] Tin_c */,
+                             const int64_t* question /* DEVICE [sum Tin_c] */, const int64_t* segment_ids /* DEVICE [sum Tin_c] */,
+                             const int64_t* task_tokens /* DEVICE [n, 1] */, float* state_f32, void* state_16, void* cuda_stream);
+int vb200_encode_image_packed(vb200_handle h, int32_t n, int32_t max_regions, const int32_t* n_regions /* HOST [n] V_i */,
+                              const float* features /* DEVICE [sum V_i, v_feature_size] */, const float* spatials /* DEVICE [sum V_i, 5] */,
+                              float* state_f32, void* state_16, void* cuda_stream);
+/* Pair b = (caption text_index[b], image image_index[b]) from packed states.  The index arrays and state offsets are HOST arrays (the
+ * engine validates them and builds the plan's offsets on the host); the per-call offsets reach the plan's workspace on cuda_stream
+ * through a pinned staging buffer, and one kernel gathers every pair's rows from the states.  Outputs follow vb200_forward_packed:
+ * per-pair outputs keep their shapes, per-row outputs come back packed.  Scores are bit-identical to vb200_forward_packed of the same
+ * pairs, which is bit-identical to a dense forward of each pair alone at its own (Tin_c, V_i).  VB200_ERR_INVALID for
+ * VB200_OUT_ATTENTION, split_fp32 engines, NULL pointers, an index outside [0, n_text) / [0, n_image), offsets that do not increase
+ * (a state of 0 rows included), a length above a non-zero capacity, T or V > 256 and Tin > max_position_embeddings. */
+typedef struct {
+    int32_t batch;                  /* B pairs */
+    int32_t max_tokens, max_regions;   /* plan capacities (Tin and V units, as vb200_packed_inputs); 0 -> this call's maxima */
+    const int32_t* text_index;      /* HOST [B] caption of pair b */
+    const int32_t* image_index;     /* HOST [B] image of pair b */
+    int32_t n_text;  const int32_t* text_offsets;   /* HOST [n_text + 1] state row offsets (rows T_c = Tin_c + 1) */
+    const float* text_f32;  const void* text_16;    /* DEVICE packed text states from vb200_encode_text_packed */
+    int32_t n_image; const int32_t* image_offsets;  /* HOST [n_image + 1] */
+    const float* image_f32; const void* image_16;   /* DEVICE packed image states from vb200_encode_image_packed */
+} vb200_packed_pairs;
+int vb200_forward_cached_packed(vb200_handle h, const vb200_packed_pairs* in, const vb200_outputs* out, uint32_t select,
+                                int32_t slot, void* cuda_stream);
 
 /* ---- Kernel-level entry points (device pointers), used by the parity tests and the roofline bench.  ---- */
 /* y = epilogue(x[M,K] (16-bit) . w[N,K]^T (16-bit)); act: 0 none, 1 GELU(erf), 2 ReLU; LayerNorm applied when gamma != NULL.

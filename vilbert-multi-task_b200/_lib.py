@@ -61,6 +61,14 @@ class PackedInputs(C.Structure):
                 ("features", C.c_void_p), ("spatials", C.c_void_p), ("task_tokens", C.c_void_p)]
 
 
+class PackedPairs(C.Structure):
+    """vb200_packed_pairs: pairs scored from packed caption / image states (index and offset arrays HOST int32, states device)."""
+    _fields_ = [("batch", C.c_int32), ("max_tokens", C.c_int32), ("max_regions", C.c_int32),
+                ("text_index", C.c_void_p), ("image_index", C.c_void_p),
+                ("n_text", C.c_int32), ("text_offsets", C.c_void_p), ("text_f32", C.c_void_p), ("text_16", C.c_void_p),
+                ("n_image", C.c_int32), ("image_offsets", C.c_void_p), ("image_f32", C.c_void_p), ("image_16", C.c_void_p)]
+
+
 class Outputs(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in OUTPUT_FIELDS]
 
@@ -75,7 +83,7 @@ class Options(C.Structure):
 EXPORTS = ["vb200_abi_version", "vb200_create", "vb200_destroy", "vb200_last_error", "vb200_forward", "vb200_forward_slot",
            "vb200_forward_host", "vb200_forward_host_slot", "vb200_plan_info", "vb200_model_dim", "vb200_set_option", "vb200_timeline", "vb200_profile_ops",
            "vb200_attention_layout", "vb200_forward_regions", "vb200_forward_packed", "vb200_encode_text", "vb200_encode_image", "vb200_forward_cached",
-           "vb200_linear", "vb200_linear_rows", "vb200_linear_split", "vb200_layernorm", "vb200_layernorm_split", "vb200_attention_f32",
+           "vb200_encode_text_packed", "vb200_encode_image_packed", "vb200_forward_cached_packed", "vb200_linear", "vb200_linear_rows", "vb200_linear_split", "vb200_layernorm", "vb200_layernorm_split", "vb200_attention_f32",
            "vb200_self_attention", "vb200_co_attention"]
 
 _lib = None
@@ -121,6 +129,9 @@ def load():
     lib.vb200_encode_text.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp]
     lib.vb200_encode_image.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp, vp, vp]
     lib.vb200_forward_cached.argtypes = [vp, i32, i32, i32, vp, i32, vp, vp, vp, vp, i32, vp, vp, vp, C.POINTER(Outputs), u32, i32, vp]
+    lib.vb200_encode_text_packed.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp, vp, vp]
+    lib.vb200_encode_image_packed.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp, vp]
+    lib.vb200_forward_cached_packed.argtypes = [vp, C.POINTER(PackedPairs), C.POINTER(Outputs), u32, i32, vp]
     lib.vb200_linear_split.argtypes = [vp, i64, vp, i64, vp, i32, vp, i64, vp, i64, i64, i64, i64, vp]
     lib.vb200_layernorm_split.argtypes = [vp, i64, vp, i64, vp, vp, f32, vp, i64, vp, i64, i64, i64, vp]
     lib.vb200_attention_f32.argtypes = [vp, i64, vp, vp, i64, i32, vp, i32, i32, i32, i32, i32, vp, i64, i32, vp, vp]

@@ -237,6 +237,25 @@ gather_state_kernel(const int32_t* __restrict__ idx, int n_src, const float* __r
         for (int i = threadIdx.x; i < L; i += blockDim.x) dst_mask[static_cast<size_t>(b) * L + i] = src_mask[static_cast<size_t>(s) * L + i];
 }
 
+// Packed retrieval: pair b's cached rows [src[b], src[b] + dst[b+1] - dst[b]) of a packed caption / image state -> rows
+// [dst[b], dst[b+1]) of the pair plan's buffers (fp32 residual stream and 16-bit GEMM operand).  grid (B, 2): y = 0 text, 1 image;
+// one contiguous range per CTA, 16-byte copies.
+__device__ __forceinline__ void copy_packed_rows(const PackedStateCopy& c, int b) {
+    const int d0 = c.dst_offs[b], rows = c.dst_offs[b + 1] - d0, s0 = c.src_offs[b];
+    const size_t n32 = static_cast<size_t>(rows) * c.n32, n16 = static_cast<size_t>(rows) * c.n16;
+    const uint4* a = reinterpret_cast<const uint4*>(c.src_f32) + static_cast<size_t>(s0) * c.n32;
+    uint4* d = reinterpret_cast<uint4*>(c.dst_f32) + static_cast<size_t>(d0) * c.n32;
+    for (size_t i = threadIdx.x; i < n32; i += blockDim.x) d[i] = a[i];
+    const uint4* a2 = static_cast<const uint4*>(c.src_16) + static_cast<size_t>(s0) * c.n16;
+    uint4* d2 = static_cast<uint4*>(c.dst_16) + static_cast<size_t>(d0) * c.n16;
+    for (size_t i = threadIdx.x; i < n16; i += blockDim.x) d2[i] = a2[i];
+}
+__global__ void __launch_bounds__(256)
+gather_packed_state_kernel(PackedStateCopy text, PackedStateCopy image) {
+    if (blockIdx.y == 0) copy_packed_rows(text, blockIdx.x);
+    else copy_packed_rows(image, blockIdx.x);
+}
+
 // one warp per row; n_out <= 4
 __global__ void __launch_bounds__(128)
 rowdot_kernel(const float* __restrict__ x, int ld_x, const float* __restrict__ W, const float* __restrict__ bias,
@@ -301,6 +320,16 @@ cudaError_t launch_gather_state(const int32_t* idx, int n_src, const float* src_
     if (B < 1 || n_src < 1 || (static_cast<long long>(L) * H) % 4 != 0 || (static_cast<long long>(L) * H16) % 8 != 0) return cudaErrorInvalidValue;
     gather_state_kernel<<<B, 256, 0, st>>>(idx, n_src, src_f32, static_cast<const uint16_t*>(src_16), src_mask, dst_f32,
                                            static_cast<uint16_t*>(dst_16), dst_mask, L, L * H / 4, L * H16 / 8);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_gather_packed_state(const PackedStateCopy& text, const PackedStateCopy& image, int B, cudaStream_t st) {
+    if (B < 1) return cudaErrorInvalidValue;
+    for (const PackedStateCopy* c : {&text, &image})
+        if (c->n32 < 1 || c->n16 < 1 || (reinterpret_cast<uintptr_t>(c->src_f32) | reinterpret_cast<uintptr_t>(c->src_16) |
+                                         reinterpret_cast<uintptr_t>(c->dst_f32) | reinterpret_cast<uintptr_t>(c->dst_16)) & 15)
+            return cudaErrorInvalidValue;
+    gather_packed_state_kernel<<<dim3(B, 2), 256, 0, st>>>(text, image);
     return cudaGetLastError();
 }
 

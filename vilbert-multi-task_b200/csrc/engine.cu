@@ -413,8 +413,9 @@ struct Plan {
     float *d_feat = nullptr, *d_loc = nullptr;
     uint8_t* d_imask = nullptr;
     float* d_out[12] = {nullptr};
-    // packed plans (vb200_forward_packed): d_meta = text row offsets [B + 1] | image row offsets [B + 1] | text rows | image rows,
-    // filled per call from the pinned h_meta; meta_copied marks when the last copy out of h_meta has been made
+    // packed plans (vb200_forward_packed and the packed retrieval calls): d_meta = text row offsets [B + 1] | image row offsets
+    // [B + 1] | text rows | image rows, and for a packed pair suffix also the pairs' source rows in the cached text states [B] |
+    // image states [B]; filled per call from the pinned h_meta; meta_copied marks when the last copy out of h_meta has been made
     bool packed = false;
     int* d_meta = nullptr;
     int* h_meta = nullptr;
@@ -423,6 +424,8 @@ struct Plan {
     const int* offs_v() const { return d_meta + B + 1; }
     const int* rows_t() const { return d_meta + 2 * (B + 1); }
     const int* rows_v() const { return d_meta + 2 * (B + 1) + 1; }
+    const int* src_t() const { return d_meta + 2 * (B + 1) + 2; }
+    const int* src_v() const { return d_meta + 2 * (B + 1) + 2 + B; }
     ~Plan() {
         if (exec) cudaGraphExecDestroy(exec);
         if (graph) cudaGraphDestroy(graph);
@@ -842,12 +845,17 @@ struct vb200_engine {
     // PACKED runs FULL's schedule on a packed variable-length batch (vb200_forward_packed): Tin + task tokens and V are the plan's
     // per-sample capacities (multiples of 16), every buffer holds B x capacity rows, and the kernels take the call's row offsets and
     // row totals from the plan's d_meta -- GEMMs skip the tiles past the totals, attention runs each sample at its own length.
-    enum PlanMode { FULL = 0, TEXT_PREFIX = 1, IMAGE_PREFIX = 2, SUFFIX = 3, PACKED = 4 };
+    // PACKED_TEXT_PREFIX, PACKED_IMAGE_PREFIX and PACKED_SUFFIX are the retrieval split of PACKED: captions, images and pairs
+    // stored back to back at their own lengths (mode = PACKED + the dense mode).
+    enum PlanMode { FULL = 0, TEXT_PREFIX = 1, IMAGE_PREFIX = 2, SUFFIX = 3, PACKED = 4,
+                    PACKED_TEXT_PREFIX = 5, PACKED_IMAGE_PREFIX = 6, PACKED_SUFFIX = 7 };
 
     Plan* get_plan(int B, int Tin, int V, uint32_t select, int slot = 0, int mode = FULL, bool want_attn = false) {
         if (slot < 0 || slot > 15) fail(VB200_ERR_INVALID, "slot %d out of range (0..15)", slot);
         if (slot > 0 && !opt.use_cuda_graph) fail(VB200_ERR_INVALID, "concurrent slots need CUDA-graph plans (use_cuda_graph)");
-        if (mode == TEXT_PREFIX || mode == IMAGE_PREFIX) { select = 0; want_attn = false; }
+        const bool packed = mode >= PACKED;
+        const int schedule_mode = packed ? mode - PACKED : mode;     // which part of the schedule: FULL, a prefix or the suffix
+        if (schedule_mode == TEXT_PREFIX || schedule_mode == IMAGE_PREFIX) { select = 0; want_attn = false; }
         std::vector<int64_t> key{B, Tin, V, static_cast<int64_t>(select), slot, mode, want_attn ? 1 : 0};
         auto it = plans.find(key);
         if (it != plans.end()) { it->second->last_use = ++use_clock; return it->second.get(); }
@@ -857,12 +865,12 @@ struct vb200_engine {
         const int T = Tin + (c.task_tokens ? 1 : 0);
         if (B < 1 || Tin < 1 || V < 1) fail(VB200_ERR_INVALID, "batch, n_tokens and n_regions must be positive");
         if (T > 256 || V > 256) fail(VB200_ERR_INVALID, "sequence too long for the small-sequence attention kernels (T=%d, V=%d, max 256)", T, V);
-        if (Tin > c.max_pos && mode != PACKED) fail(VB200_ERR_INVALID, "n_tokens %d exceeds max_position_embeddings %d", Tin, c.max_pos);
+        if (Tin > c.max_pos && !packed) fail(VB200_ERR_INVALID, "n_tokens %d exceeds max_position_embeddings %d", Tin, c.max_pos);
         pl.B = B; pl.Tin = Tin; pl.T = T; pl.V = V; pl.select = select;
-        if (mode == PACKED) {
+        if (packed) {
             // zero offsets and totals until the first call: the validation pass and the capture below then touch no row
             pl.packed = true;
-            const size_t n_meta = 2 * (static_cast<size_t>(B) + 1) + 2;
+            const size_t n_meta = 2 * (static_cast<size_t>(B) + 1) + 2 + (mode == PACKED_SUFFIX ? 2 * static_cast<size_t>(B) : 0);
             pl.d_meta = pl.mem.alloc_n<int>(n_meta);
             CUDA_CHECK(cudaMemset(pl.d_meta, 0, n_meta * sizeof(int)));
             CUDA_CHECK(cudaMallocHost(&pl.h_meta, n_meta * sizeof(int)));
@@ -874,13 +882,19 @@ struct vb200_engine {
         const int* offs_v = pl.packed ? pl.offs_v() : nullptr;
         const int Mt = B * T, Mv = B * V, H = c.hidden, Hv = c.v_hidden, Hb = c.bi_hidden;
         const size_t S = x3 ? 3 : 1;                 // physical width factor of the 16-bit operand buffers (fp32-parity mode)
-        const bool full = mode == FULL || mode == PACKED;
-        const bool do_t = full || mode == TEXT_PREFIX, do_v = full || mode == IMAGE_PREFIX;
-        const bool do_s = full || mode == SUFFIX;
+        const bool full = schedule_mode == FULL;
+        const bool do_t = full || schedule_mode == TEXT_PREFIX, do_v = full || schedule_mode == IMAGE_PREFIX;
+        const bool do_s = full || schedule_mode == SUFFIX;
         pl.kp = img_emb.ldw;
         pl.img_a = pl.mem.alloc_n<bf16>(static_cast<size_t>(Mv) * pl.kp * S);
         pl.mask_t = pl.mem.alloc_n<float>(Mt);
         pl.mask_v = pl.mem.alloc_n<float>(Mv);
+        if (mode == PACKED_SUFFIX) {
+            // the attention kernels read the additive key masks in packed plans too, and every packed row is real: all zero, for good
+            // (no embedding kernel of a packed suffix writes them)
+            CUDA_CHECK(cudaMemset(pl.mask_t, 0, static_cast<size_t>(Mt) * sizeof(float)));
+            CUDA_CHECK(cudaMemset(pl.mask_v, 0, static_cast<size_t>(Mv) * sizeof(float)));
+        }
         for (int i = 0; i < 2; ++i) {
             pl.t_f32[i] = pl.mem.alloc_n<float>(static_cast<size_t>(Mt) * H);
             pl.t_b16[i] = pl.mem.alloc_n<bf16>(static_cast<size_t>(Mt) * H * S);
@@ -1330,22 +1344,65 @@ struct vb200_engine {
     // graph on the same stream; the pack kernels then run on the real rows only and zero the operand rows up to the next 128-row
     // boundary (the rest of the last GEMM tile that holds a real row, the only rows past the totals a GEMM loads).
     void forward_packed(Plan& pl, const vb200_packed_inputs& in, const std::vector<int>& meta, cudaStream_t st) {
-        const Config& c = cfg;
-        const int B = pl.B, rows_t = meta[2 * (B + 1)], rows_v = meta[2 * (B + 1) + 1];
+        stage_meta(pl, meta, st);
+        embed_text_packed(pl, in.question, in.segment_ids, in.task_tokens, meta[2 * (pl.B + 1)], st);
+        pack_image_packed(pl, in.features, in.spatials, meta[2 * (pl.B + 1) + 1], st);
+        run_plan(pl, st);
+    }
+    // meta (host, the plan's d_meta layout) -> d_meta, in stream order ahead of the plan's kernels
+    void stage_meta(Plan& pl, const std::vector<int>& meta, cudaStream_t st) {
         CUDA_CHECK(cudaEventSynchronize(pl.meta_copied));           // the previous call's copy has left the staging buffer
         memcpy(pl.h_meta, meta.data(), meta.size() * sizeof(int));
         CUDA_CHECK(cudaMemcpyAsync(pl.d_meta, pl.h_meta, meta.size() * sizeof(int), cudaMemcpyHostToDevice, st));
         CUDA_CHECK(cudaEventRecord(pl.meta_copied, st));
-        auto zero_tail = [&](bf16* buf, int rows, int cap, size_t width) {
-            const int end = std::min(cap, (rows + 127) / 128 * 128);
-            if (end > rows) CUDA_CHECK(cudaMemsetAsync(buf + static_cast<size_t>(rows) * width, 0, static_cast<size_t>(end - rows) * width * 2, st));
-        };
-        CUDA_CHECK(vb::launch_text_embed(in.question, in.segment_ids, nullptr, in.task_tokens, word, pos, type, task, emb_ln.g, emb_ln.b,
-                                         c.ln_eps, pl.t_f32[0], pl.t_b16[0], pl.mask_t, B, 0, c.hidden, c.vocab, c.max_pos, c.type_vocab,
-                                         c.n_task, c.task_tokens, opt.act_fp16, 0, st, pl.offs_t(), rows_t));
-        zero_tail(pl.t_b16[0], rows_t, B * pl.T, c.hidden);
-        CUDA_CHECK(vb::launch_image_pack(in.features, in.spatials, nullptr, pl.img_a, pl.mask_v, rows_v, c.v_feat, pl.kp, opt.act_fp16, 0, st));
-        zero_tail(pl.img_a, rows_v, B * pl.V, pl.kp);
+    }
+    // zero the 16-bit operand rows [rows, next 128-row boundary) of a buffer with `cap` rows
+    static void zero_tail(bf16* buf, int rows, int cap, size_t width, cudaStream_t st) {
+        const int end = std::min(cap, (rows + 127) / 128 * 128);
+        if (end > rows) CUDA_CHECK(cudaMemsetAsync(buf + static_cast<size_t>(rows) * width, 0, static_cast<size_t>(end - rows) * width * 2, st));
+    }
+    void embed_text_packed(Plan& pl, const int64_t* q, const int64_t* seg, const int64_t* tk, int rows_t, cudaStream_t st) {
+        const Config& c = cfg;
+        CUDA_CHECK(vb::launch_text_embed(q, seg, nullptr, tk, word, pos, type, task, emb_ln.g, emb_ln.b, c.ln_eps, pl.t_f32[0], pl.t_b16[0],
+                                         pl.mask_t, pl.B, 0, c.hidden, c.vocab, c.max_pos, c.type_vocab, c.n_task, c.task_tokens,
+                                         opt.act_fp16, 0, st, pl.offs_t(), rows_t));
+        zero_tail(pl.t_b16[0], rows_t, pl.B * pl.T, c.hidden, st);
+    }
+    void pack_image_packed(Plan& pl, const float* feats, const float* loc, int rows_v, cudaStream_t st) {
+        const Config& c = cfg;
+        CUDA_CHECK(vb::launch_image_pack(feats, loc, nullptr, pl.img_a, pl.mask_v, rows_v, c.v_feat, pl.kp, opt.act_fp16, 0, st));
+        zero_tail(pl.img_a, rows_v, pl.B * pl.V, pl.kp, st);
+    }
+    // ---- packed retrieval (PACKED_TEXT_PREFIX / PACKED_IMAGE_PREFIX / PACKED_SUFFIX): the prefixes write each caption's / image's
+    // rows back to back into the caller's state; the suffix gathers every pair's rows from those states into its packed buffers
+    void encode_text_packed(Plan& pl, const std::vector<int>& meta, const int64_t* q, const int64_t* seg, const int64_t* tk, float* st_f32,
+                            void* st_16, cudaStream_t st) {
+        const int rows = meta[2 * (pl.B + 1)];
+        stage_meta(pl, meta, st);
+        embed_text_packed(pl, q, seg, tk, rows, st);
+        run_plan(pl, st);
+        CUDA_CHECK(cudaMemcpyAsync(st_f32, pl.t_f32[pl.t_cur], static_cast<size_t>(rows) * cfg.hidden * 4, cudaMemcpyDeviceToDevice, st));
+        CUDA_CHECK(cudaMemcpyAsync(st_16, pl.t_b16[pl.t_cur], static_cast<size_t>(rows) * cfg.hidden * 2, cudaMemcpyDeviceToDevice, st));
+    }
+    void encode_image_packed(Plan& pl, const std::vector<int>& meta, const float* feats, const float* loc, float* st_f32, void* st_16,
+                             cudaStream_t st) {
+        const int rows = meta[2 * (pl.B + 1) + 1];
+        stage_meta(pl, meta, st);
+        pack_image_packed(pl, feats, loc, rows, st);
+        run_plan(pl, st);
+        CUDA_CHECK(cudaMemcpyAsync(st_f32, pl.v_f32[pl.v_cur], static_cast<size_t>(rows) * cfg.v_hidden * 4, cudaMemcpyDeviceToDevice, st));
+        CUDA_CHECK(cudaMemcpyAsync(st_16, pl.v_b16[pl.v_cur], static_cast<size_t>(rows) * cfg.v_hidden * 2, cudaMemcpyDeviceToDevice, st));
+    }
+    void forward_cached_packed(Plan& pl, const vb200_packed_pairs& in, const std::vector<int>& meta, cudaStream_t st) {
+        const Config& c = cfg;
+        const int B = pl.B;
+        stage_meta(pl, meta, st);
+        const vb::PackedStateCopy text{pl.offs_t(), pl.src_t(), in.text_f32, in.text_16, pl.t_f32[0], pl.t_b16[0], c.hidden / 4, c.hidden / 8};
+        const vb::PackedStateCopy image{pl.offs_v(), pl.src_v(), in.image_f32, in.image_16, pl.v_f32[0], pl.v_b16[0], c.v_hidden / 4,
+                                        c.v_hidden / 8};
+        CUDA_CHECK(vb::launch_gather_packed_state(text, image, B, st));
+        zero_tail(pl.t_b16[0], meta[2 * (B + 1)], B * pl.T, c.hidden, st);
+        zero_tail(pl.v_b16[0], meta[2 * (B + 1) + 1], B * pl.V, c.v_hidden, st);
         run_plan(pl, st);
     }
     // ---- retrieval reuse (PlanMode): per-caption / per-image prefixes and the pair suffix
@@ -1446,6 +1503,34 @@ void require_device(int device) {
     CUDA_CHECK(cudaGetDeviceProperties(&p, device));
     if (p.major != 9 || p.minor != 0) fail(VB200_ERR_NO_DEVICE, "device %d is sm_%d%d; the kernels are built for sm_90a only", device, p.major, p.minor);
     CUDA_CHECK(cudaSetDevice(device));
+}
+
+// Row offsets of one stream of a packed call from HOST lengths (text: Tin_i, rows T_i = Tin_i + task token; image: V_i rows):
+// offs[i + 1] = offs[i] + rows_i.  Rejects a length < 1 or above a non-zero capacity `cap`, more than 256 rows (the small-sequence
+// attention kernels) and Tin_i > max_position_embeddings.  Returns the longest length.
+int pack_lengths(const char* api, const char* item, bool text, const Config& c, const int32_t* len, int n, int cap, int* offs) {
+    const char* name = text ? "n_tokens" : "n_regions";
+    const int extra = text && c.task_tokens ? 1 : 0;
+    int longest = 0;
+    offs[0] = 0;
+    for (int i = 0; i < n; ++i) {
+        const int l = len[i];
+        if (l < 1) fail(VB200_ERR_INVALID, "%s: %s %d has %s %d (must be >= 1)", api, item, i, name, l);
+        if (cap > 0 && l > cap) fail(VB200_ERR_INVALID, "%s: %s %d has %s %d, above the capacity %d", api, item, i, name, l, cap);
+        if (l + extra > 256)
+            fail(VB200_ERR_INVALID, "%s: %s %d too long for the small-sequence attention kernels (%s=%d, max 256)", api, item, i,
+                 text ? "T" : "V", l + extra);
+        if (text && l > c.max_pos) fail(VB200_ERR_INVALID, "%s: %s %d has n_tokens %d > max_position_embeddings %d", api, item, i, l, c.max_pos);
+        offs[i + 1] = offs[i] + l + extra;
+        longest = std::max(longest, l);
+    }
+    return longest;
+}
+// Plan capacity in rows per item, rounded up to the attention kernels' 16-row buckets: `cap` (0: the call's longest) + extra rows.
+int capacity16(const char* api, int cap, int longest, int extra, const char* rows_name) {
+    const int rows = (cap > 0 ? cap : longest) + extra;
+    if (rows > 256) fail(VB200_ERR_INVALID, "%s: capacity above 256 rows per sample (%s=%d)", api, rows_name, rows);
+    return (rows + 15) / 16 * 16;
 }
 }  // namespace
 
@@ -1549,26 +1634,12 @@ int vb200_forward_packed(vb200_handle h, const vb200_packed_inputs* in, const vb
             fail(VB200_ERR_INVALID, "vb200_packed_inputs has a NULL required pointer");
         // meta = text row offsets [B + 1] | image row offsets [B + 1] | text rows | image rows (the plan's d_meta layout)
         std::vector<int> meta(2 * (static_cast<size_t>(B) + 1) + 2, 0);
-        int max_tin = 0, max_v = 0;
-        for (int b = 0; b < B; ++b) {
-            const int tin = in->n_tokens[b], v = in->n_regions[b];
-            if (tin < 1 || v < 1) fail(VB200_ERR_INVALID, "packed batches: sample %d has n_tokens %d, n_regions %d (both must be >= 1)", b, tin, v);
-            if ((in->max_tokens > 0 && tin > in->max_tokens) || (in->max_regions > 0 && v > in->max_regions))
-                fail(VB200_ERR_INVALID, "packed batches: sample %d (n_tokens %d, n_regions %d) exceeds the capacity (max_tokens %d, max_regions %d)",
-                     b, tin, v, in->max_tokens, in->max_regions);
-            if (tin + task > 256 || v > 256)
-                fail(VB200_ERR_INVALID, "packed batches: sample %d too long for the small-sequence attention kernels (T=%d, V=%d, max 256)", b, tin + task, v);
-            if (tin > c.max_pos) fail(VB200_ERR_INVALID, "packed batches: sample %d has n_tokens %d > max_position_embeddings %d", b, tin, c.max_pos);
-            meta[b + 1] = meta[b] + tin + task;
-            meta[B + 1 + b + 1] = meta[B + 1 + b] + v;
-            max_tin = std::max(max_tin, tin);
-            max_v = std::max(max_v, v);
-        }
+        const int max_tin = pack_lengths("packed batches", "sample", true, c, in->n_tokens, B, in->max_tokens, meta.data());
+        const int max_v = pack_lengths("packed batches", "sample", false, c, in->n_regions, B, in->max_regions, meta.data() + B + 1);
         meta[2 * (B + 1)] = meta[B];
         meta[2 * (B + 1) + 1] = meta[2 * B + 1];
-        const int t_cap = (in->max_tokens > 0 ? in->max_tokens : max_tin) + task, v_cap = in->max_regions > 0 ? in->max_regions : max_v;
-        if (t_cap > 256 || v_cap > 256) fail(VB200_ERR_INVALID, "packed batches: capacity above 256 rows per sample (T=%d, V=%d)", t_cap, v_cap);
-        const int t16 = (t_cap + 15) / 16 * 16, v16 = (v_cap + 15) / 16 * 16;     // the attention kernels' pad16 buckets
+        const int t16 = capacity16("packed batches", in->max_tokens, max_tin, task, "T");
+        const int v16 = capacity16("packed batches", in->max_regions, max_v, 0, "V");
         CUDA_CHECK(cudaSetDevice(h->opt.device));
         Plan* pl = h->get_plan(B, t16 - task, v16, select & VB200_OUT_ALL, slot, vb200_engine::PACKED, false);
         cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
@@ -1628,6 +1699,99 @@ int vb200_forward_cached(vb200_handle h, int32_t batch, int32_t n_tokens, int32_
         h->forward_cached(*pl, text_index, n_text, text_f32, text_16, text_mask, image_index, n_image, image_f32, image_16,
                           image_mask, st);
         h->copy_outputs(*pl, *out, st, cudaMemcpyDeviceToDevice);
+    });
+}
+
+int vb200_encode_text_packed(vb200_handle h, int32_t n, int32_t max_tokens, const int32_t* n_tokens, const int64_t* question,
+                             const int64_t* segment_ids, const int64_t* task_tokens, float* state_f32, void* state_16, void* cuda_stream) {
+    if (h == nullptr) return VB200_ERR_INVALID;
+    return guard(h, [&] {
+        const char* api = "vb200_encode_text_packed";
+        const Config& c = h->cfg;
+        const int task = c.task_tokens ? 1 : 0;
+        if (h->x3) fail(VB200_ERR_INVALID, "%s: packed retrieval is not supported in split_fp32 (fp32x) mode", api);
+        if (n < 1) fail(VB200_ERR_INVALID, "%s: n must be positive", api);
+        if (max_tokens < 0) fail(VB200_ERR_INVALID, "%s: negative capacity", api);
+        if (!n_tokens || !question || !segment_ids || (task && !task_tokens) || !state_f32 || !state_16)
+            fail(VB200_ERR_INVALID, "%s: NULL pointer", api);
+        std::vector<int> meta(2 * (static_cast<size_t>(n) + 1) + 2, 0);
+        const int max_tin = pack_lengths(api, "caption", true, c, n_tokens, n, max_tokens, meta.data());
+        meta[2 * (n + 1)] = meta[n];
+        const int t16 = capacity16(api, max_tokens, max_tin, task, "T");
+        CUDA_CHECK(cudaSetDevice(h->opt.device));
+        Plan* pl = h->get_plan(n, t16 - task, 1, 0, 0, vb200_engine::PACKED_TEXT_PREFIX);
+        h->encode_text_packed(*pl, meta, question, segment_ids, task_tokens, state_f32, state_16, static_cast<cudaStream_t>(cuda_stream));
+    });
+}
+
+int vb200_encode_image_packed(vb200_handle h, int32_t n, int32_t max_regions, const int32_t* n_regions, const float* features,
+                              const float* spatials, float* state_f32, void* state_16, void* cuda_stream) {
+    if (h == nullptr) return VB200_ERR_INVALID;
+    return guard(h, [&] {
+        const char* api = "vb200_encode_image_packed";
+        if (h->x3) fail(VB200_ERR_INVALID, "%s: packed retrieval is not supported in split_fp32 (fp32x) mode", api);
+        if (n < 1) fail(VB200_ERR_INVALID, "%s: n must be positive", api);
+        if (max_regions < 0) fail(VB200_ERR_INVALID, "%s: negative capacity", api);
+        if (!n_regions || !features || !spatials || !state_f32 || !state_16) fail(VB200_ERR_INVALID, "%s: NULL pointer", api);
+        std::vector<int> meta(2 * (static_cast<size_t>(n) + 1) + 2, 0);
+        const int max_v = pack_lengths(api, "image", false, h->cfg, n_regions, n, max_regions, meta.data() + n + 1);
+        meta[2 * (n + 1) + 1] = meta[2 * n + 1];
+        const int v16 = capacity16(api, max_regions, max_v, 0, "V");
+        CUDA_CHECK(cudaSetDevice(h->opt.device));
+        Plan* pl = h->get_plan(n, 1, v16, 0, 0, vb200_engine::PACKED_IMAGE_PREFIX);
+        h->encode_image_packed(*pl, meta, features, spatials, state_f32, state_16, static_cast<cudaStream_t>(cuda_stream));
+    });
+}
+
+int vb200_forward_cached_packed(vb200_handle h, const vb200_packed_pairs* in, const vb200_outputs* out, uint32_t select, int32_t slot,
+                                void* cuda_stream) {
+    if (h == nullptr) return VB200_ERR_INVALID;
+    return guard(h, [&] {
+        const char* api = "vb200_forward_cached_packed";
+        if (in == nullptr || out == nullptr) fail(VB200_ERR_INVALID, "inputs/outputs struct is NULL");
+        if (select & VB200_OUT_ATTENTION) fail(VB200_ERR_INVALID, "%s: the attention-probability output (VB200_OUT_ATTENTION) is not supported", api);
+        if (h->x3) fail(VB200_ERR_INVALID, "%s: packed retrieval is not supported in split_fp32 (fp32x) mode", api);
+        const Config& c = h->cfg;
+        const int B = in->batch, task = c.task_tokens ? 1 : 0;
+        if (B < 1) fail(VB200_ERR_INVALID, "%s: batch must be positive", api);
+        if (in->max_tokens < 0 || in->max_regions < 0) fail(VB200_ERR_INVALID, "%s: negative capacity", api);
+        if (in->n_text < 1 || in->n_image < 1) fail(VB200_ERR_INVALID, "%s: n_text and n_image must be positive", api);
+        if (!in->text_index || !in->image_index || !in->text_offsets || !in->image_offsets || !in->text_f32 || !in->text_16 ||
+            !in->image_f32 || !in->image_16)
+            fail(VB200_ERR_INVALID, "%s: vb200_packed_pairs has a NULL required pointer", api);
+        auto check_offsets = [&](const int32_t* offs, int n, const char* what) {
+            if (offs[0] < 0) fail(VB200_ERR_INVALID, "%s: %s_offsets[0] = %d is negative", api, what, offs[0]);
+            for (int i = 0; i < n; ++i)
+                if (offs[i + 1] <= offs[i])
+                    fail(VB200_ERR_INVALID, "%s: %s state %d has %d rows (the offsets must increase)", api, what, i, offs[i + 1] - offs[i]);
+        };
+        check_offsets(in->text_offsets, in->n_text, "text");
+        check_offsets(in->image_offsets, in->n_image, "image");
+        // meta = pair text row offsets [B + 1] | pair image row offsets [B + 1] | text rows | image rows | source text rows [B] |
+        // source image rows [B] (the plan's d_meta layout)
+        std::vector<int> meta(2 * (static_cast<size_t>(B) + 1) + 2 + 2 * static_cast<size_t>(B), 0);
+        int* src_t = meta.data() + 2 * (B + 1) + 2;
+        int* src_v = src_t + B;
+        std::vector<int32_t> tin(B), nv(B);
+        for (int b = 0; b < B; ++b) {
+            const int ti = in->text_index[b], vi = in->image_index[b];
+            if (ti < 0 || ti >= in->n_text) fail(VB200_ERR_INVALID, "%s: pair %d: text_index %d outside [0, %d)", api, b, ti, in->n_text);
+            if (vi < 0 || vi >= in->n_image) fail(VB200_ERR_INVALID, "%s: pair %d: image_index %d outside [0, %d)", api, b, vi, in->n_image);
+            tin[b] = in->text_offsets[ti + 1] - in->text_offsets[ti] - task;
+            nv[b] = in->image_offsets[vi + 1] - in->image_offsets[vi];
+            src_t[b] = in->text_offsets[ti];
+            src_v[b] = in->image_offsets[vi];
+        }
+        const int max_tin = pack_lengths(api, "pair", true, c, tin.data(), B, in->max_tokens, meta.data());
+        const int max_v = pack_lengths(api, "pair", false, c, nv.data(), B, in->max_regions, meta.data() + B + 1);
+        meta[2 * (B + 1)] = meta[B];
+        meta[2 * (B + 1) + 1] = meta[2 * B + 1];
+        const int t16 = capacity16(api, in->max_tokens, max_tin, task, "T"), v16 = capacity16(api, in->max_regions, max_v, 0, "V");
+        CUDA_CHECK(cudaSetDevice(h->opt.device));
+        Plan* pl = h->get_plan(B, t16 - task, v16, select & VB200_OUT_ALL, slot, vb200_engine::PACKED_SUFFIX, false);
+        cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+        h->forward_cached_packed(*pl, *in, meta, st);
+        h->copy_outputs(*pl, *out, st, cudaMemcpyDeviceToDevice, meta[2 * (B + 1)], meta[2 * (B + 1) + 1]);
     });
 }
 

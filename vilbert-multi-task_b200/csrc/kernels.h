@@ -96,6 +96,19 @@ cudaError_t launch_region_pack(const float* box_feats, const float* boxes, const
 // the fp32 and mask copies are skipped when their pointers are null (packed poolers: the first 16-bit row of every sample)
 cudaError_t launch_gather_state(const int32_t* idx, int n_src, const float* src_f32, const void* src_16, const float* src_mask,
                                 float* dst_f32, void* dst_16, float* dst_mask, int B, int L, int H, int H16, cudaStream_t st);
+// packed retrieval: one stream's copy from a packed caption / image state into a packed pair plan.  Pair b's rows
+// [dst_offs[b], dst_offs[b+1]) come from rows starting at src_offs[b] (both device int32, [B + 1] and [B]); n32 / n16 = 16-byte
+// vectors per row of the fp32 / 16-bit buffer.  Every pointer 16-byte aligned.
+struct PackedStateCopy {
+    const int* dst_offs;
+    const int* src_offs;
+    const float* src_f32;
+    const void* src_16;
+    float* dst_f32;
+    void* dst_16;
+    int n32, n16;
+};
+cudaError_t launch_gather_packed_state(const PackedStateCopy& text, const PackedStateCopy& image, int B, cudaStream_t st);
 // fp32 CUDA-core attention (attention_f32.cu): in_kind 0 fp32 / 1 fp16 / 2 bf16 Q, K, V; ctx_mode 0 none / 1 fp16 / 2 bf16 /
 // 3 fp16 hi | lo | hi; probs: optional [B, heads, Lq, Lk] fp32 attention probabilities.
 cudaError_t launch_attention_f32(const void* q, int ld_q, const void* k, const void* v, int ld_kv, int in_kind,

@@ -42,6 +42,19 @@ def _normalise_state_dict(sd) -> Dict[str, torch.Tensor]:
     return out
 
 
+def _host_ints(x):
+    return [int(v) for v in (x.tolist() if torch.is_tensor(x) else x)]
+
+
+def packed_offsets(lengths, extra: int = 0):
+    """Row offsets [n + 1] of n items stored back to back with lengths[i] + extra rows each (extra = 1: the task-token row of
+    a caption state)."""
+    offs = [0]
+    for n in lengths:
+        offs.append(offs[-1] + int(n) + extra)
+    return offs
+
+
 class VILBertForVLTasks(object):
     """Drop-in for ``vilbert.vilbert.VILBertForVLTasks`` on the inference path the worker uses."""
 
@@ -384,8 +397,7 @@ class VILBertForVLTasks(object):
             raise L.VilbertB200Error("call model.cuda(i) first (worker.py:536); there is no CPU path")
         lib = L.load()
         device = torch.device("cuda", self._device)
-        nt = [int(x) for x in (n_tokens.tolist() if torch.is_tensor(n_tokens) else n_tokens)]
-        nr = [int(x) for x in (n_regions.tolist() if torch.is_tensor(n_regions) else n_regions)]
+        nt, nr = _host_ints(n_tokens), _host_ints(n_regions)
         B = len(nt)
         if len(nr) != B or B < 1:
             raise ValueError("forward_packed: n_tokens and n_regions must have the same, positive length")
@@ -403,18 +415,7 @@ class VILBertForVLTasks(object):
         if q.numel() != sum_tin or seg.numel() != sum_tin or f.shape[0] != sum_v or s.shape[0] != sum_v:
             raise ValueError("forward_packed: question / segment_ids need sum(n_tokens) rows, features / spatials sum(n_regions)")
         rows_t = sum_tin + (B if self._dims["task_specific_tokens"] else 0)
-        d = self._dims
-        packed = {"vision_prediction": (sum_v, d["v_target_size"]), "vision_logit": (sum_v, 1),
-                  "linguisic_prediction": (rows_t, d["vocab_size"]), "linguisic_logit": (rows_t, 1)}
-        outs = {k: torch.empty(packed.get(k, shape), dtype=torch.float32, device=device)
-                for k, shape in self._out_shapes(B, 1, 1, select).items()}
-        if debug_taps:
-            outs["sequence_output_t"] = torch.empty(rows_t, d["hidden_size"], dtype=torch.float32, device=device)
-            outs["sequence_output_v"] = torch.empty(sum_v, d["v_hidden_size"], dtype=torch.float32, device=device)
-            outs["pooled_output"] = torch.empty(B, d["bi_hidden_size"], dtype=torch.float32, device=device)
-        o = L.Outputs()
-        for k, t in outs.items():
-            setattr(o, k, t.data_ptr())
+        outs, o = self._alloc_packed_outputs(B, rows_t, sum_v, select, debug_taps, device)
         nt_c, nr_c = (C.c_int32 * B)(*nt), (C.c_int32 * B)(*nr)
         inp = L.PackedInputs(B, int(max_tokens), int(max_regions), C.cast(nt_c, C.c_void_p), C.cast(nr_c, C.c_void_p), q.data_ptr(),
                              seg.data_ptr(), f.data_ptr(), s.data_ptr(), tk.data_ptr())
@@ -422,6 +423,22 @@ class VILBertForVLTasks(object):
             stream = torch.cuda.current_stream(device).cuda_stream
             L.check(lib.vb200_forward_packed(self._handle, C.byref(inp), C.byref(o), select, slot, C.c_void_p(stream)), self._handle)
         return self._result(outs, B, 0, 0, debug_taps)
+
+    def _alloc_packed_outputs(self, B, rows_t, rows_v, select, debug_taps, device):
+        """Outputs of a packed call: per-sample outputs [B, ...], per-row outputs and taps [rows_t or rows_v, ...]."""
+        d = self._dims
+        packed = {"vision_prediction": (rows_v, d["v_target_size"]), "vision_logit": (rows_v, 1),
+                  "linguisic_prediction": (rows_t, d["vocab_size"]), "linguisic_logit": (rows_t, 1)}
+        outs = {k: torch.empty(packed.get(k, shape), dtype=torch.float32, device=device)
+                for k, shape in self._out_shapes(B, 1, 1, select).items()}
+        if debug_taps:
+            outs["sequence_output_t"] = torch.empty(rows_t, d["hidden_size"], dtype=torch.float32, device=device)
+            outs["sequence_output_v"] = torch.empty(rows_v, d["v_hidden_size"], dtype=torch.float32, device=device)
+            outs["pooled_output"] = torch.empty(B, d["bi_hidden_size"], dtype=torch.float32, device=device)
+        o = L.Outputs()
+        for k, t in outs.items():
+            setattr(o, k, t.data_ptr())
+        return outs, o
 
     # ------------------------------------------------------------------ retrieval reuse (SURVEY.md section 8e)
     @torch.no_grad()
@@ -487,6 +504,93 @@ class VILBertForVLTasks(object):
                                              image_state["mask"].data_ptr(), C.byref(o), select, slot, C.c_void_p(stream)),
                     self._handle)
         return self._result(outs, B, Tin, V, False)
+
+    # ------------------------------------------------------------------ packed retrieval: every caption / image at its own length
+    @torch.no_grad()
+    def encode_text_packed(self, question, segment_ids, task_tokens, n_tokens, max_tokens: int = 0):
+        """``encode_text`` of n captions stored back to back without padding: ``question`` / ``segment_ids`` ``[sum Tin_c]``,
+        ``task_tokens`` ``[n, 1]``, ``n_tokens`` (list or CPU tensor) the Tin_c.  Returns an opaque state for
+        ``forward_cached_packed``: caption c's rows sit at ``offsets[c]`` (T_c = Tin_c + 1 rows with the task token) and equal
+        ``encode_text`` of that caption alone.  ``max_tokens`` (0: this call's maximum) is the plan capacity."""
+        lib = L.load()
+        device = torch.device("cuda", self._device)
+        nt = _host_ints(n_tokens)
+        n = len(nt)
+        q = torch.as_tensor(question).to(device=device, dtype=torch.int64).reshape(-1).contiguous()
+        seg = torch.as_tensor(segment_ids).to(device=device, dtype=torch.int64).reshape(-1).contiguous()
+        tk = torch.as_tensor(task_tokens).to(device=device, dtype=torch.int64).reshape(n, -1)[:, :1].contiguous()
+        if n < 1 or q.numel() != sum(nt) or seg.numel() != sum(nt):
+            raise ValueError("encode_text_packed: question / segment_ids need sum(n_tokens) entries for n >= 1 captions")
+        offs = packed_offsets(nt, 1 if self._dims["task_specific_tokens"] else 0)
+        H = self._dims["hidden_size"]
+        st = dict(kind="text", n=n, offsets=torch.tensor(offs, dtype=torch.int32), max_len=max(nt),
+                  f32=torch.empty(offs[-1], H, dtype=torch.float32, device=device),
+                  h16=torch.empty(offs[-1], H, dtype=torch.int16, device=device))
+        nt_c = (C.c_int32 * n)(*nt)
+        with torch.cuda.device(device):
+            stream = torch.cuda.current_stream(device).cuda_stream
+            L.check(lib.vb200_encode_text_packed(self._handle, n, int(max_tokens), C.cast(nt_c, C.c_void_p), q.data_ptr(), seg.data_ptr(),
+                                                 tk.data_ptr(), st["f32"].data_ptr(), st["h16"].data_ptr(), C.c_void_p(stream)),
+                    self._handle)
+        return st
+
+    @torch.no_grad()
+    def encode_image_packed(self, features, spatials, n_regions, max_regions: int = 0):
+        """``encode_image`` of n images stored back to back without padding: ``features`` ``[sum V_i, F]``, ``spatials``
+        ``[sum V_i, 5]``, ``n_regions`` the V_i.  Image i's state rows sit at ``offsets[i]`` and equal ``encode_image`` of that
+        image alone."""
+        lib = L.load()
+        device = torch.device("cuda", self._device)
+        nr = _host_ints(n_regions)
+        n = len(nr)
+        f = torch.as_tensor(features).to(device=device, dtype=torch.float32).reshape(-1, self._dims["v_feature_size"]).contiguous()
+        s = torch.as_tensor(spatials).to(device=device, dtype=torch.float32).reshape(-1, 5).contiguous()
+        if n < 1 or f.shape[0] != sum(nr) or s.shape[0] != sum(nr):
+            raise ValueError("encode_image_packed: features / spatials need sum(n_regions) rows for n >= 1 images")
+        offs = packed_offsets(nr)
+        Hv = self._dims["v_hidden_size"]
+        st = dict(kind="image", n=n, offsets=torch.tensor(offs, dtype=torch.int32), max_len=max(nr),
+                  f32=torch.empty(offs[-1], Hv, dtype=torch.float32, device=device),
+                  h16=torch.empty(offs[-1], Hv, dtype=torch.int16, device=device))
+        nr_c = (C.c_int32 * n)(*nr)
+        with torch.cuda.device(device):
+            stream = torch.cuda.current_stream(device).cuda_stream
+            L.check(lib.vb200_encode_image_packed(self._handle, n, int(max_regions), C.cast(nr_c, C.c_void_p), f.data_ptr(), s.data_ptr(),
+                                                  st["f32"].data_ptr(), st["h16"].data_ptr(), C.c_void_p(stream)), self._handle)
+        return st
+
+    @torch.no_grad()
+    def forward_cached_packed(self, text_state, text_index, image_state, image_index, select: int = L.OUT_VIL_LOGIT, slot: int = 0,
+                              max_tokens: Optional[int] = None, max_regions: Optional[int] = None, debug_taps: bool = False):
+        """Pair b = (caption text_index[b], image image_index[b]) from packed states, every pair at its own lengths.  Index tensors may
+        be on the CPU or the GPU (they are read on the host).  Returns the 10-tuple as ``forward_packed`` does (per-row outputs packed,
+        pair after pair), bit-identical to ``forward_packed`` of the same pairs.  Capacities default to the states' longest caption /
+        largest image, so every call on the same states and batch size shares one plan."""
+        if text_state.get("kind") != "text" or image_state.get("kind") != "image" or "offsets" not in text_state \
+                or "offsets" not in image_state:
+            raise ValueError("forward_cached_packed: pass the states of encode_text_packed and encode_image_packed")
+        lib = L.load()
+        device = torch.device("cuda", self._device)
+        ti = torch.as_tensor(text_index).to(device="cpu", dtype=torch.int32).reshape(-1).contiguous()
+        vi = torch.as_tensor(image_index).to(device="cpu", dtype=torch.int32).reshape(-1).contiguous()
+        B = ti.numel()
+        if vi.numel() != B:
+            raise ValueError("text_index and image_index must have the same length")
+        toffs, voffs = text_state["offsets"], image_state["offsets"]
+        mt = text_state["max_len"] if max_tokens is None else int(max_tokens)
+        mr = image_state["max_len"] if max_regions is None else int(max_regions)
+        # row totals for the per-row outputs (indices clamped here; the engine rejects out-of-range ones)
+        rows_t = int((toffs[1:] - toffs[:-1])[ti.long().clamp(0, text_state["n"] - 1)].sum())
+        rows_v = int((voffs[1:] - voffs[:-1])[vi.long().clamp(0, image_state["n"] - 1)].sum())
+        outs, o = self._alloc_packed_outputs(B, rows_t, rows_v, select, debug_taps, device)
+        pairs = L.PackedPairs(B, mt, mr, ti.data_ptr(), vi.data_ptr(), text_state["n"], toffs.data_ptr(), text_state["f32"].data_ptr(),
+                              text_state["h16"].data_ptr(), image_state["n"], voffs.data_ptr(), image_state["f32"].data_ptr(),
+                              image_state["h16"].data_ptr())
+        with torch.cuda.device(device):
+            stream = torch.cuda.current_stream(device).cuda_stream
+            L.check(lib.vb200_forward_cached_packed(self._handle, C.byref(pairs), C.byref(o), select, slot, C.c_void_p(stream)),
+                    self._handle)
+        return self._result(outs, B, 0, 0, debug_taps)
 
     # ------------------------------------------------------------------ host-buffer entry (bench e2e, serving)
     def forward_host(self, question, features, spatials, segment_ids, input_mask, image_mask, task_tokens,

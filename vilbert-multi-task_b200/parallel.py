@@ -17,6 +17,8 @@ from typing import Callable, List, Sequence, Tuple
 import torch
 import torch.distributed as dist
 
+from .worker_api import _prefix_len
+
 
 def shard_range(n: int, rank: int, world: int, pair_aligned: bool = False) -> Tuple[int, int]:
     """Contiguous slice [lo, hi) of `n` samples for `rank`; sizes differ by at most one unit
@@ -136,6 +138,73 @@ def retrieval_scores_cached(model, captions, images, task_id: int = 7, pair_batc
     scores = torch.empty(padded, dtype=torch.float32, device=dev)
     for s0 in range(0, padded, pair_batch):
         out = model.forward_cached(ts, ci[s0:s0 + pair_batch], vs, ii[s0:s0 + pair_batch], select=L.OUT_VIL_LOGIT)
+        scores[s0:s0 + pair_batch] = out[2].view(-1)
+    local = scores[:total].view(hi - lo, n_img)
+    if ev:
+        ev[2].record()
+    full = all_gather_rows(local, n_cap, group, comm)
+    if ev:
+        ev[3].record()
+        torch.cuda.synchronize(dev)
+        timings.update(encode_ms=ev[0].elapsed_time(ev[1]), pairs_ms=ev[1].elapsed_time(ev[2]), gather_ms=ev[2].elapsed_time(ev[3]),
+                       local_captions=hi - lo, pairs=total)
+    return full
+
+
+def strip_padding(mask: torch.Tensor, name: str = "mask") -> List[int]:
+    """Real length of every row of a padded batch: each row of `mask` must be a run of ones followed by zeros, with at least one
+    one; anything else raises ValueError (packed rows are all real, so a hole in the mask cannot be represented)."""
+    lens = [_prefix_len(row) for row in mask.detach().cpu()]
+    bad = [i for i, k in enumerate(lens) if k is None]
+    if bad:
+        raise ValueError(f"{name} row {bad[0]} is not a prefix of ones")
+    return lens
+
+
+def pack_rows(x: torch.Tensor, lens: Sequence[int]) -> torch.Tensor:
+    """The first lens[i] rows of every item of a padded [n, L, ...] tensor, back to back: [sum(lens), ...]."""
+    keep = torch.arange(x.shape[1], device=x.device)[None, :] < torch.as_tensor(list(lens), device=x.device)[:, None]
+    return x[keep]
+
+
+def retrieval_pairs(n_captions: int, n_images: int, pair_batch: int):
+    """Caption and image index (CPU int32) of every pair of an n_captions x n_images block, caption-major, padded with pair 0 to a
+    multiple of `pair_batch` (one plan for every chunk; the padded pairs' scores are dropped), and the number of real pairs."""
+    total = n_captions * n_images
+    flat = torch.arange(-(-total // pair_batch) * pair_batch, dtype=torch.int64)
+    flat = torch.where(flat < total, flat, torch.zeros_like(flat))
+    return (flat // n_images).to(torch.int32), (flat % n_images).to(torch.int32), total
+
+
+def retrieval_scores_packed(model, captions, images, task_id: int = 7, pair_batch: int = 256, group=None, comm=None,
+                            timings=None) -> torch.Tensor:
+    """`retrieval_scores_cached` without padding: the same padded inputs, but every caption and image runs at its own length.
+    `input_mask` and `image_mask` must have every row a prefix of ones (ValueError otherwise).  The real rows are packed, this rank's
+    captions and all images are encoded once (`model.encode_text_packed` / `encode_image_packed`), and pairs are scored in chunks of
+    `pair_batch` from the packed states (`model.forward_cached_packed`, one plan per chunk size).  Each score equals the
+    unpadded forward of its pair; with uniform lengths and no padding it is bit-identical to `retrieval_scores_cached`.  One
+    all-gather at the end.  `timings` (dict) receives CUDA-event milliseconds: encode / pairs / gather."""
+    from . import _lib as L
+    world = dist.get_world_size(group) if dist.is_initialized() else 1
+    rank = dist.get_rank(group) if dist.is_initialized() else 0
+    q, seg, im = captions
+    f, s, vm = images
+    n_cap, n_img = q.shape[0], f.shape[0]
+    lo, hi = shard_range(n_cap, rank, world)
+    dev = f.device
+    t_lens, v_lens = strip_padding(im[lo:hi], "input_mask"), strip_padding(vm, "image_mask")
+    ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)] if timings is not None else None
+    if ev:
+        ev[0].record()
+    task = torch.full((hi - lo, 1), task_id, dtype=torch.long, device=dev)
+    vs = model.encode_image_packed(pack_rows(f, v_lens), pack_rows(s, v_lens), v_lens)
+    ts = model.encode_text_packed(pack_rows(q[lo:hi], t_lens), pack_rows(seg[lo:hi], t_lens), task, t_lens)
+    if ev:
+        ev[1].record()
+    ci, ii, total = retrieval_pairs(hi - lo, n_img, pair_batch)
+    scores = torch.empty(ci.numel(), dtype=torch.float32, device=dev)
+    for s0 in range(0, ci.numel(), pair_batch):
+        out = model.forward_cached_packed(ts, ci[s0:s0 + pair_batch], vs, ii[s0:s0 + pair_batch], select=L.OUT_VIL_LOGIT)
         scores[s0:s0 + pair_batch] = out[2].view(-1)
     local = scores[:total].view(hi - lo, n_img)
     if ev:
