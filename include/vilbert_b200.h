@@ -182,7 +182,9 @@ int vb200_plan_info(vb200_handle h, int32_t batch, int32_t n_tokens, int32_t n_r
 int vb200_model_dim(vb200_handle h, const char* key, int64_t* value);
 /* Run-time knobs: "max_plans" (plan-cache bound); "profile_grid_pct" (0 or 10..100): the NEXT vb200_profile_ops call launches every
  * GEMM with this percentage of the resident CTA slots as its persistent grid --
- * for reporting what a launch does when it has the GPU to itself; forwards are never affected. */
+ * for reporting what a launch does when it has the GPU to itself; forwards are never affected.  "gemm_kernel": 1 (default, or 0
+ * under VB200_GEMM=coop) runs the plain GEMMs the ping-pong kernel supports on it, 0 runs every GEMM on the cooperative persistent
+ * kernel; a change drops the cached plans.  Both give the same bits. */
 int vb200_set_option(vb200_handle h, const char* key, int64_t value);
 /* Profiling: after vb200_set_option(h, "timeline", 1) every persistent GEMM launch of a forward records 16 stamps per CTA (0: clock64 at
  * entry, 1: setup done, 2: first k-block landed [-DVB200_STAMPS builds], 8 / 9: %globaltimer ns at entry / exit, 10: last tile accumulated,
@@ -311,15 +313,18 @@ int vb200_forward_cached_packed(vb200_handle h, const vb200_packed_pairs* in, co
  * act_fp16 != 0: x, w and the 16-bit output y are fp16, else bf16 (parameter names keep the historical _bf16 suffix).
  * act 3 = GELU with the 1.5e-7 erf (fp32-parity mode).  variant 0: persistent kernel (gemm_persistent.cuh, what the engine
  * uses); 2, 3 and 4 (names of Blackwell kernel configurations) select the persistent kernel: 2 and 3 with the plain 128-wide tile,
- * 4 with the plain 128- or 64-wide one.  Plain (non-LayerNorm) tiles are 64, 128 or 192 columns wide; block_n 256 runs as
- * 128-wide tiles.  Every variant and every width gives the same bits.
+ * 4 with the plain 128- or 64-wide one.  variant 5: the ping-pong kernel (gemm_pingpong.cuh, what the engine uses for the plain
+ * GEMMs it supports): no residual / LayerNorm, act 0-2, N a multiple of block_n 64 or 128, outputs the TMA can store (16-byte aligned
+ * base and row stride); VB200_ERR_INVALID otherwise.  Plain (non-LayerNorm) tiles are 64, 128 or 192 columns wide; block_n 256 runs
+ * as 128-wide tiles.  Every variant and every width gives the same bits.
  * timing: NULL, or a device buffer of 16 int64 per CTA that receives clock64() / %globaltimer stamps (profiling aid). */
 int vb200_linear(const void* x_bf16, int64_t ld_x, const void* w_bf16, int64_t ld_w, const float* bias,
                  const float* residual, int64_t ld_res, const float* gamma, const float* beta, float eps, int32_t act,
                  void* y_bf16, int64_t ld_y_bf16, float* y_f32, int64_t ld_y_f32, int64_t M, int64_t N, int64_t K,
                  int32_t block_n, int32_t use_pdl, int32_t act_fp16, int32_t variant, long long* timing, void* cuda_stream);
-/* The plain GEMM (variant 0, no residual / LayerNorm) with a device row count: rows >= min(*m_rows, M) are neither loaded nor
- * computed -- the 128-row tiles that start at or past it are skipped, what packed plans rely on (m_rows: device int32). */
+/* The plain GEMM (no residual / LayerNorm) with a device row count: rows >= min(*m_rows, M) are neither loaded nor computed -- the
+ * 128-row tiles that start at or past it are skipped, what packed plans rely on (m_rows: device int32).  Runs on the kernel the
+ * engine would pick: ping-pong (variant 5) where it applies unless VB200_GEMM=coop, else variant 0. */
 int vb200_linear_rows(const void* x16, int64_t ld_x, const void* w16, int64_t ld_w, const float* bias, int32_t act, void* y16,
                       int64_t ld_y16, float* y_f32, int64_t ld_y_f32, int64_t M, int64_t N, int64_t K, int32_t block_n, int32_t act_fp16,
                       const int32_t* m_rows, void* cuda_stream);

@@ -1,7 +1,7 @@
 """Per-kernel timing through the C ABI (CUDA events on the launching stream, after warm-up), at the shapes one
 B=64 forward launches.  Used to pick optimisation targets and, under `ncu --set full`, to read stall reasons.
 
-    python scripts/kernel_bench.py [--only NAME] [--reps 50] [--batch 64]
+    python scripts/kernel_bench.py [--only NAME] [--reps 50] [--batch 64] [--variant 0,5] [--bn 64]
 """
 import argparse
 import ctypes as C
@@ -50,10 +50,13 @@ def main():
     ap.add_argument("--sets", type=int, default=4, help="operand sets cycled through per kernel")
     ap.add_argument("--stamps", action="store_true", help="print clock64 phase stamps of the persistent kernel")
     ap.add_argument("--bn", type=int, default=0, help="override block_n of every plain GEMM")
+    ap.add_argument("--variant", default="0", help="vb200_linear variant of the plain GEMMs (comma list, each timed in turn): "
+                                                   "0 cooperative persistent kernel, 5 ping-pong")
     ap.add_argument("--debug", default="0", help="VB200_DEBUG timing decomposition (comma list, each timed in turn): "
                                                  "1 no MMA, 2 no stores, 4 no operand loads")
     a = ap.parse_args()
     debug_modes = [int(x) for x in str(a.debug).split(",")]
+    variants = [int(x) for x in str(a.variant).split(",")]
     only = [x for x in a.only.split(",") if x]
     lib = L.load()
     B, T, V = a.batch, 31, 36
@@ -96,19 +99,20 @@ def main():
         def run(i):
             x, w, b, r, ga, be, yb, yf, ldf = sets[i % a.sets]
             rc = lib.vb200_linear(ptr(x), K, ptr(w), K, ptr(b), ptr(r), N if ln else 0, ptr(ga), ptr(be), 1e-12, actf,
-                                  ptr(yb), N, ptr(yf), ldf, M, N, K, bn, 0, f16, 0, None, C.c_void_p(cur()))
+                                  ptr(yb), N, ptr(yf), ldf, M, N, K, bn, 0, f16, variant, None, C.c_void_p(cur()))
             L.check(rc, None)
-        for dbg in debug_modes:
+        plain_pp = not ln and N % (bn if bn in (64, 128) else 128) == 0 and bn != 256
+        for variant, dbg in [(v, d) for v in variants for d in debug_modes if v == 0 or plain_pp]:
             os.environ["VB200_DEBUG"] = str(dbg)
             us = time_graph(run, a.reps)
             fl = 2.0 * M * N * K
-            res.append(dict(kernel=name, M=M, N=N, K=K, debug=dbg, us=round(us, 2), tflops=round(fl / us / 1e6, 1)))
+            res.append(dict(kernel=name, M=M, N=N, K=K, bn=bn, variant=variant, debug=dbg, us=round(us, 2), tflops=round(fl / us / 1e6, 1)))
             print(json.dumps(res[-1]), flush=True)
             if a.stamps:
                 tb = torch.zeros(16 * 4096, dtype=torch.int64, device="cuda")
                 x, w, b, r, ga, be, yb, yf, ldf = sets[0]
                 rc = lib.vb200_linear(ptr(x), K, ptr(w), K, ptr(b), ptr(r), N if ln else 0, ptr(ga), ptr(be), 1e-12, actf,
-                                      ptr(yb), N, ptr(yf), ldf, M, N, K, bn, 0, f16, 0, ptr(tb), C.c_void_p(cur()))
+                                      ptr(yb), N, ptr(yf), ldf, M, N, K, bn, 0, f16, variant, ptr(tb), C.c_void_p(cur()))
                 L.check(rc, None)
                 torch.cuda.synchronize()
                 t = tb.view(-1, 16).cpu()

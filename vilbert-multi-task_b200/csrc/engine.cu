@@ -344,16 +344,30 @@ void setup_tma_store(CUtensorMap* tc, GemmEpilogue& e) {
         if (make_tmap_out(tc, e.out_f32, e.M, e.N, e.ld_f32, true, false)) e.tma_store = 2;
     }
 }
+// Output maps of the ping-pong kernel (every output leaves through the TMA); false when an output does not meet the TMA's rules.
+bool setup_pingpong_store(CUtensorMap* c16, CUtensorMap* c32, const GemmEpilogue& e) {
+    if (e.out_bf16 != nullptr && !make_tmap_out(c16, e.out_bf16, e.M, e.N, e.ld_bf16, false, e.out_f16 != 0)) return false;
+    if (e.out_f32 != nullptr && !make_tmap_out(c32, e.out_f32, e.M, e.N, e.ld_f32, true, false)) return false;
+    return true;
+}
+// Which kernel takes the plain GEMMs it supports: 1 ping-pong (default), 0 the cooperative gemm_persistent_kernel.
+// VB200_GEMM=coop|pingpong is the A/B switch; vb200_set_option("gemm_kernel") changes it per engine.
+int default_gemm_kernel() {
+    static const int v = [] { const char* e = getenv("VB200_GEMM"); return (e && strcmp(e, "coop") == 0) ? 0 : 1; }();
+    return v;
+}
 
 // ------------------------------------------------------------------------------------------ launch list
 struct Op {
     enum Kind { GEMM, SELF_ATTN, CO_ATTN, ROWDOT, LAYERNORM, ATTN_F32, GATHER } kind;
     int stream = 0;                // 0 main, 1 side (image branch) inside the captured graph
     // GEMM
-    CUtensorMap ta, tb, tc;        // operands, and the output (TMA-store epilogue, ep.tma_store != 0)
+    CUtensorMap ta, tb, tc;        // operands, and the output (TMA-store epilogue, ep.tma_store != 0; ping-pong: the 16-bit output)
+    CUtensorMap tc32;              // ping-pong: the fp32 output
     GemmEpilogue ep;
     int block_n = 128;
     bool ln = false;
+    bool pingpong = false;         // launched as the ping-pong kernel (gemm_pingpong.cuh)
     // fp32 attention (attention_f32.cu): fp32-parity mode and the attention-probability output
     const void *f_q = nullptr, *f_k = nullptr, *f_v = nullptr;
     int f_ld_q = 0, f_ld_kv = 0, f_in = 0, f_Lq = 0, f_Lk = 0, f_ctx_mode = 0, f_ld_ctx = 0;
@@ -451,6 +465,7 @@ struct vb200_engine {
     bool tma_store_enabled = true;  // VB200_TMASTORE=0: every tile leaves through the register / LSU epilogue
     bool early_w = true;            // VB200_EARLYW=0: no weight loads ahead of griddepcontrol.wait
     bool fused_ln = false;     // VB200_FUSED_LN=1: cluster-LayerNorm GEMM epilogue instead of GEMM(fp32) + row LayerNorm kernel
+    int gemm_kernel = 1;       // default_gemm_kernel(): 1 = plain GEMMs the ping-pong kernel supports run on it, 0 = all on the cooperative one
     Arena weights;
     std::string last_error;
     // embeddings
@@ -787,7 +802,14 @@ struct vb200_engine {
             e.split16 = (x3 && out_b != nullptr) ? 1 : 0;
             if (e.split16 && (W.N & 63)) fail(VB200_ERR_INVALID, "fp32-parity mode: 16-bit GEMM output of width %d is not a multiple of 64", W.N);
         }
-        if (tma_store_enabled && !op.ln) setup_tma_store(&op.tc, e);
+        // Ping-pong kernel: each consumer warpgroup's epilogue runs under the other's mainloop.  It takes every plain GEMM it
+        // supports (not the cluster LayerNorm, fp32-parity, pooled-product or ragged-N ones) whose outputs the TMA can store.
+        // It takes the tile width chosen above, 128 even where that leaves one tile per CTA: 64-wide ping-pong tiles measured slower on H100 SXM
+        // (700 W, bf16, 16-bit output, scripts/kernel_bench.py) at 1984x768x768 (9.74 vs 8.20 us), 1984x768x3072 (29.19 vs 20.32) and
+        // 2304x1024x1024 (16.71 vs 15.88), and only 4 % faster with GELU at 2304x1024x1024 (18.04 vs 18.81).
+        op.pingpong = gemm_kernel == 1 && tma_store_enabled && !op.ln && !x3 && vb::gemm_pingpong_supports(e, op.block_n) &&
+                      setup_pingpong_store(&op.tc, &op.tc32, e);
+        if (tma_store_enabled && !op.ln && !op.pingpong) setup_tma_store(&op.tc, e);
         op.flops = 2.0 * a_rows * W.N * W.K;
         pl.flops += op.flops;
         pl.ops.push_back(op);
@@ -1176,7 +1198,9 @@ struct vb200_engine {
                 GemmEpilogue e = op.ep;
                 e.tmap_c_host = e.tma_store ? &op.tc : nullptr;       // Op objects move when the list grows: bind here
                 e.grid_pct = profile_grid_pct;                        // 0 outside vb200_profile_ops
-                const cudaError_t le = vb::launch_gemm_persistent(op.ta, op.tb, e, op.block_n, op.ln, st);
+                const cudaError_t le = op.pingpong
+                    ? vb::launch_gemm_pingpong(op.ta, op.tb, &op.tc, &op.tc32, e, op.block_n, st)
+                    : vb::launch_gemm_persistent(op.ta, op.tb, e, op.block_n, op.ln, st);
                 if (le != cudaSuccess)
                     fail(VB200_ERR_CUDA, "GEMM launch failed: %s (layer %s, M=%d N=%d K=%d act=%d block_n=%d cluster_ln=%d split16=%d tma_store=%d)",
                          cudaGetErrorString(le), op.tag ? op.tag : "?", e.M, e.N, e.K, e.act, op.block_n, (int)op.ln, e.split16, e.tma_store);
@@ -1580,6 +1604,7 @@ int vb200_create(const char* config_json, int64_t n_tensors, const vb200_tensor*
         }
         if (const char* v = getenv("VB200_TMASTORE")) eng->tma_store_enabled = (strcmp(v, "0") != 0);
         if (const char* v = getenv("VB200_EARLYW")) eng->early_w = (strcmp(v, "0") != 0);
+        eng->gemm_kernel = default_gemm_kernel();
         CUDA_CHECK(cudaStreamCreateWithFlags(&eng->side_stream, cudaStreamNonBlocking));
         CUDA_CHECK(cudaEventCreateWithFlags(&eng->ev_fork, cudaEventDisableTiming));
         CUDA_CHECK(cudaEventCreateWithFlags(&eng->ev_join, cudaEventDisableTiming));
@@ -1916,6 +1941,13 @@ int vb200_set_option(vb200_handle h, const char* key, int64_t value) {
                 h->plans.clear();
                 h->timeline = value != 0;
             }
+        } else if (k == "gemm_kernel") {
+            if (value != 0 && value != 1) fail(VB200_ERR_INVALID, "gemm_kernel must be 0 (cooperative) or 1 (ping-pong)");
+            if (value != h->gemm_kernel) {              // the kernel is chosen when a plan is built
+                CUDA_CHECK(cudaDeviceSynchronize());
+                h->plans.clear();
+                h->gemm_kernel = static_cast<int>(value);
+            }
         } else fail(VB200_ERR_INVALID, "unknown option \"%s\"", key);
     });
 }
@@ -1978,8 +2010,23 @@ int vb200_linear(const void* x_bf16, int64_t ld_x, const void* w_bf16, int64_t l
         // (three CTAs per SM; one CTA with a 6-stage ring); ABI version 2 keeps accepting them, and on sm_90a they select the
         // persistent kernel itself.  block_n 256 (the Blackwell 256-wide tile) runs as 128-wide tiles, which give the same bits: the
         // tile width never changes an element's accumulation order.
-        if (variant < 0 || variant == 1 || variant > 4)
-            fail(VB200_ERR_INVALID, "vb200_linear: variant %d does not exist (0 persistent, 2 / 3 / 4 = 0)", variant);
+        if (variant < 0 || variant == 1 || variant > 5)
+            fail(VB200_ERR_INVALID, "vb200_linear: variant %d does not exist (0 persistent, 2 / 3 / 4 = 0, 5 ping-pong)", variant);
+        if (variant == 5) {
+            const int bn = block_n > 0 ? block_n : vb::gemm_p_pick_block_n(static_cast<int>(N), false);
+            CUtensorMap ta = make_tmap(x_bf16, M, K, ld_x, 128, act_fp16 != 0);
+            CUtensorMap tb = make_tmap(w_bf16, N, K, ld_w, bn, act_fp16 != 0);
+            GemmEpilogue e{};
+            e.M = (int)M; e.N = (int)N; e.K = (int)K; e.bias = bias; e.res = residual; e.gamma = gamma; e.act = act; e.pdl = use_pdl;
+            e.out_bf16 = static_cast<bf16*>(y_bf16); e.ld_bf16 = (int)ld_y_bf16; e.out_f32 = y_f32; e.ld_f32 = (int)ld_y_f32;
+            e.a_f16 = act_fp16 ? 1 : 0; e.out_f16 = e.a_f16; e.timing = timing;
+            CUtensorMap c16, c32;
+            if (!vb::gemm_pingpong_supports(e, bn) || !setup_pingpong_store(&c16, &c32, e))
+                fail(VB200_ERR_INVALID, "vb200_linear: variant 5 (ping-pong) takes plain GEMMs with N a multiple of block_n 64 / 128 and "
+                                        "TMA-storable outputs (N=%lld block_n=%d)", (long long)N, bn);
+            CUDA_CHECK(vb::launch_gemm_pingpong(ta, tb, &c16, &c32, e, bn, static_cast<cudaStream_t>(cuda_stream)));
+            return;
+        }
         int bn = block_n > 0 ? block_n : vb::gemm_p_pick_block_n(static_cast<int>(N), ln);
         if (bn == 0) fail(VB200_ERR_INVALID, "no tiling for N=%lld with LayerNorm", (long long)N);
         if (!ln && bn == 256) bn = 128;
@@ -2014,7 +2061,11 @@ int vb200_linear_rows(const void* x16, int64_t ld_x, const void* w16, int64_t ld
         GemmEpilogue e{};
         e.M = (int)M; e.N = (int)N; e.K = (int)K; e.bias = bias; e.act = act; e.a_f16 = act_fp16 ? 1 : 0; e.out_f16 = e.a_f16;
         e.out_bf16 = static_cast<bf16*>(y16); e.ld_bf16 = (int)ld_y16; e.out_f32 = y_f32; e.ld_f32 = (int)ld_y_f32; e.m_rows = m_rows;
-        CUtensorMap tc;
+        CUtensorMap tc, tc32;
+        if (default_gemm_kernel() == 1 && vb::gemm_pingpong_supports(e, bn) && setup_pingpong_store(&tc, &tc32, e)) {   // as the engine
+            CUDA_CHECK(vb::launch_gemm_pingpong(ta, tb, &tc, &tc32, e, bn, static_cast<cudaStream_t>(cuda_stream)));
+            return;
+        }
         setup_tma_store(&tc, e);
         e.tmap_c_host = e.tma_store ? &tc : nullptr;
         CUDA_CHECK(vb::launch_gemm_persistent(ta, tb, e, bn, false, static_cast<cudaStream_t>(cuda_stream)));

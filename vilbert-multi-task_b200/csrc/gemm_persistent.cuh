@@ -791,6 +791,20 @@ void fill_cfg(cudaLaunchConfig_t& cfg, cudaLaunchAttribute* attrs, dim3 grid, in
     cfg.numAttrs = na;
 }
 
+// Persistent grid of a plain kernel with one CTA per SM: every SM by default.  VB200_GRID_PCT caps it at that percentage of the
+// SMs, leaving room for kernels of the other ViLBERT stream / the other in-flight batch; grid_pct (10..100) overrides it per launch
+// (profiling: timed alone).
+inline int persistent_grid(int tiles, int grid_pct) {
+    static const int env_pct = [] { const char* e = getenv("VB200_GRID_PCT"); const int v = e ? atoi(e) : 100; return (v >= 10 && v <= 100) ? v : 100; }();
+    const int pct = (grid_pct >= 10 && grid_pct <= 100) ? grid_pct : env_pct;
+    const int slots = std::max(1, num_sms() * pct / 100);
+    // balanced walk: every CTA gets the same number of tiles (+-1): tiles = 288, cap 132 -> 96 CTAs x 3 instead of 24 x 3 + 108 x 2
+    static const bool balance = [] { const char* e = getenv("VB200_GRID_BALANCE"); return e == nullptr || atoi(e) != 0; }();
+    int g = std::min(tiles, slots);
+    if (balance && tiles > slots) { const int per = (tiles + slots - 1) / slots; g = (tiles + per - 1) / per; }
+    return g;
+}
+
 // resident: LN only -- how many clusters of this size can be co-resident (grid.y is capped to it)
 template <int BLOCK_N, bool LN, int ACT, bool F16, int MODE = 0>
 cudaError_t launch_p(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilogue& ep, int resident, cudaStream_t st) {
@@ -808,17 +822,8 @@ cudaError_t launch_p(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpi
         if (resident <= 0) return cudaErrorInvalidConfiguration;
         grid = dim3(cluster, std::min(m_tiles, resident), 1);
     } else {
-        // Persistent grid: every SM (one CTA each) by default.  VB200_GRID_PCT caps it at that percentage of the SMs, leaving room
-        // for kernels of the other ViLBERT stream / the other in-flight batch.
-        static const int env_pct = [] { const char* e = getenv("VB200_GRID_PCT"); const int v = e ? atoi(e) : 100; return (v >= 10 && v <= 100) ? v : 100; }();
-        const int tiles = m_tiles * n_tiles;
-        const int pct = (ep.grid_pct >= 10 && ep.grid_pct <= 100) ? ep.grid_pct : env_pct;     // per-launch override (profiling: timed alone)
-        const int slots = std::max(1, num_sms() * Cfg::kMinBlocks * pct / 100);
-        // balanced walk: every CTA gets the same number of tiles (+-1): tiles = 288, cap 132 -> 96 CTAs x 3 instead of 24 x 3 + 108 x 2
-        static const bool balance = [] { const char* e = getenv("VB200_GRID_BALANCE"); return e == nullptr || atoi(e) != 0; }();
-        int g = std::min(tiles, slots);
-        if (balance && tiles > slots) { const int per = (tiles + slots - 1) / slots; g = (tiles + per - 1) / per; }
-        grid = dim3(g, 1, 1);
+        static_assert(Cfg::kMinBlocks == 1, "persistent_grid assumes one CTA per SM");
+        grid = dim3(persistent_grid(m_tiles * n_tiles, ep.grid_pct), 1, 1);
     }
     cudaLaunchConfig_t cfg;
     cudaLaunchAttribute attrs[2];

@@ -52,6 +52,12 @@ cudaError_t launch_gemm_persistent(const CUtensorMap& tmap_a, const CUtensorMap&
 int num_sms_host();          // SM count of the current device (132 on H100 SXM)
 cudaError_t launch_gemm_persistent_plain(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b, const GemmEpilogue& ep,
                                          int block_n, cudaStream_t st);
+// ping-pong consumer warpgroups (gemm_pingpong.cuh): plain bias / activation GEMMs with N a multiple of block_n (64 or 128), no
+// residual, LayerNorm, pooled product or fp32-parity output; every output leaves through its TMA map (tmap_c16 for out_bf16,
+// tmap_c32 for out_f32, SWIZZLE_128B boxes of 128 rows x 128 bytes).  Same bits as launch_gemm_persistent.
+bool gemm_pingpong_supports(const GemmEpilogue& ep, int block_n);
+cudaError_t launch_gemm_pingpong(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b, const CUtensorMap* tmap_c16,
+                                 const CUtensorMap* tmap_c32, const GemmEpilogue& ep, int block_n, cudaStream_t st);
 
 // 16-bit activation buffers are typed __nv_bfloat16* throughout; `f16` says the bits are IEEE fp16 instead.
 // K4: softmax(Q K^T / sqrt(d) + mask) V per (sample, head); qkv row = [Q | K | V], each `hidden` wide.
