@@ -12,8 +12,8 @@
  * The entry points below are exactly what a binding for that protocol needs, and nothing else:
  * vb200_create <- from_pretrained + cuda(i); vb200_forward <- __call__; vb200_destroy <- del.
  * Beyond the protocol: packed variable-length batches (vb200_packed_inputs: samples with their own text lengths and region counts
- * in one forward, plans keyed on capacity buckets, GEMM tiles past the call's row totals skipped), detector output in
- * (vb200_region_inputs), caption-image retrieval with reuse, dense or packed (vb200_packed_pairs: captions and images encoded once
+ * in one forward, plans keyed on capacity buckets, GEMM tiles past the call's row totals skipped), detector output in, dense or
+ * packed (vb200_region_inputs, vb200_packed_region_inputs: every image at its own box count), caption-image retrieval with reuse, dense or packed (vb200_packed_pairs: captions and images encoded once
  * at their own lengths, pairs scored without padding), and kernel-level entry points for the tests.
  * The Python shim in vilbert-multi-task_b200/ (ctypes) implements the protocol on top of them; see
  * INTEGRATION.md for the stub a maintainer of the reference would add.
@@ -257,6 +257,31 @@ typedef struct {
 } vb200_packed_inputs;
 int vb200_forward_packed(vb200_handle h, const vb200_packed_inputs* in, const vb200_outputs* out, uint32_t select,
                          int32_t slot, void* cuda_stream);
+
+/* ---- Packed detector output: vb200_forward_regions with every image at its own box count and every text at its own length, stored
+ * back to back as in vb200_packed_inputs, with no padding and no masks.  Image i has V_i = n_boxes_i + 1 regions (its global mean row
+ * first); one kernel writes each image's operand rows at its packed offset.  Each image's outputs, taps and spatials_out rows are
+ * bit-identical to vb200_forward_regions of that image alone (batch 1, n_boxes = n_boxes_i, n_tokens = Tin_i).  Plans are the
+ * PACKED plans of vb200_forward_packed, keyed on (B, round16(max_tokens + 1), round16(max_boxes + 1), select, slot): the same plan and
+ * CUDA graph serve both calls at equal capacities.  Outputs follow vb200_forward_packed (per-image outputs [B, ...], per-row outputs
+ * packed over sum V_i / sum T_i rows).  VB200_ERR_INVALID for VB200_OUT_ATTENTION, split_fp32 engines, NULL required pointers,
+ * n_boxes_i < 1 or above a non-zero max_boxes, V_i > 256, T_i > 256, Tin_i > max_position_embeddings and negative capacities. */
+typedef struct {
+    int32_t batch;                  /* B images (rows of the forward); text already repeated per image as for vb200_region_inputs */
+    int32_t max_tokens;             /* plan capacity in Tin units: 0 -> this call's maximum */
+    int32_t max_boxes;              /* plan capacity in detector boxes (regions = boxes + 1): 0 -> this call's maximum */
+    const int32_t* n_tokens;        /* HOST [B] Tin_i >= 1 */
+    const int32_t* n_boxes;         /* HOST [B] boxes of image i >= 1; V_i = n_boxes_i + 1 */
+    const int64_t* question;        /* DEVICE [sum Tin_i] */
+    const int64_t* segment_ids;     /* DEVICE [sum Tin_i] */
+    const int64_t* task_tokens;     /* DEVICE [B, 1] */
+    const float*   box_features;    /* DEVICE [sum n_boxes_i, v_feature_size] */
+    const float*   boxes;           /* DEVICE [sum n_boxes_i, 4] pixel x1, y1, x2, y2 */
+    const float*   image_wh;        /* DEVICE [B, 2] */
+    float*         spatials_out;    /* optional DEVICE [sum V_i, 5] */
+} vb200_packed_region_inputs;
+int vb200_forward_regions_packed(vb200_handle h, const vb200_packed_region_inputs* in, const vb200_outputs* out,
+                                 uint32_t select, int32_t slot, void* cuda_stream);
 
 /* ---- Caption-image retrieval with reuse (SURVEY.md section 8e; reference semantics worker.py:278-284, 359).  Everything ahead of
  * the first connection layer depends on the caption alone or on the image alone: encode each caption / image ONCE, then score

@@ -61,6 +61,14 @@ class PackedInputs(C.Structure):
                 ("features", C.c_void_p), ("spatials", C.c_void_p), ("task_tokens", C.c_void_p)]
 
 
+class PackedRegionInputs(C.Structure):
+    """vb200_packed_region_inputs: packed detector output (n_tokens / n_boxes HOST int32 arrays, the rest device memory)."""
+    _fields_ = [("batch", C.c_int32), ("max_tokens", C.c_int32), ("max_boxes", C.c_int32),
+                ("n_tokens", C.c_void_p), ("n_boxes", C.c_void_p), ("question", C.c_void_p), ("segment_ids", C.c_void_p),
+                ("task_tokens", C.c_void_p), ("box_features", C.c_void_p), ("boxes", C.c_void_p), ("image_wh", C.c_void_p),
+                ("spatials_out", C.c_void_p)]
+
+
 class PackedPairs(C.Structure):
     """vb200_packed_pairs: pairs scored from packed caption / image states (index and offset arrays HOST int32, states device)."""
     _fields_ = [("batch", C.c_int32), ("max_tokens", C.c_int32), ("max_regions", C.c_int32),
@@ -82,7 +90,7 @@ class Options(C.Structure):
 # every symbol include/vilbert_b200.h declares (tests/test_cabi.py checks the list against the header)
 EXPORTS = ["vb200_abi_version", "vb200_create", "vb200_destroy", "vb200_last_error", "vb200_forward", "vb200_forward_slot",
            "vb200_forward_host", "vb200_forward_host_slot", "vb200_plan_info", "vb200_model_dim", "vb200_set_option", "vb200_timeline", "vb200_profile_ops",
-           "vb200_attention_layout", "vb200_forward_regions", "vb200_forward_packed", "vb200_encode_text", "vb200_encode_image", "vb200_forward_cached",
+           "vb200_attention_layout", "vb200_forward_regions", "vb200_forward_packed", "vb200_forward_regions_packed", "vb200_encode_text", "vb200_encode_image", "vb200_forward_cached",
            "vb200_encode_text_packed", "vb200_encode_image_packed", "vb200_forward_cached_packed", "vb200_linear", "vb200_linear_rows", "vb200_linear_split", "vb200_layernorm", "vb200_layernorm_split", "vb200_attention_f32",
            "vb200_self_attention", "vb200_co_attention"]
 
@@ -125,6 +133,7 @@ def load():
     lib.vb200_attention_layout.argtypes = [vp, i32, i32, i32, i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(i64), C.POINTER(i64)]
     lib.vb200_forward_regions.argtypes = [vp, C.POINTER(RegionInputs), C.POINTER(Outputs), u32, i32, vp]
     lib.vb200_forward_packed.argtypes = [vp, C.POINTER(PackedInputs), C.POINTER(Outputs), u32, i32, vp]
+    lib.vb200_forward_regions_packed.argtypes = [vp, C.POINTER(PackedRegionInputs), C.POINTER(Outputs), u32, i32, vp]
     lib.vb200_linear_rows.argtypes = [vp, i64, vp, i64, vp, i32, vp, i64, vp, i64, i64, i64, i64, i32, i32, vp, vp]
     lib.vb200_encode_text.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp]
     lib.vb200_encode_image.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp, vp, vp]

@@ -151,13 +151,24 @@ image_pack_kernel(const float* __restrict__ feats, const float* __restrict__ loc
 // (x1/w, y1/h, x2/w, y2/h, area/(w h); global row 0,0,1,1,1), masks are set.  num_boxes (optional) marks padded boxes per image:
 // they are excluded from the mean, written as zeros and masked.
 // grid (B, ceil(F / 1024) + 1): the last grid row writes the location columns, the masks and the optional spatials copy.
+// Packed batch (offs = the plan's image row offsets [B + 1]): image b owns regions [offs[b], offs[b+1]) -- its mean row, then its
+// offs[b+1] - offs[b] - 1 boxes, which start at detector row offs[b] - b (one global row per image) -- every row is real, and
+// spatials_out is packed [sum V_i, 5].
 __global__ void __launch_bounds__(128)
 region_pack_kernel(const float* __restrict__ box_feats, const float* __restrict__ boxes, const float* __restrict__ image_wh,
                    const int32_t* __restrict__ num_boxes, __nv_bfloat16* __restrict__ a_out, float* __restrict__ mask_add,
-                   float* __restrict__ spatials_out, int n, int F, int Kp, int f16, int split16) {
-    const int b = blockIdx.x, V = n + 1;
-    int nb = num_boxes ? num_boxes[b] : n;
-    nb = nb < 0 ? 0 : (nb > n ? n : nb);
+                   float* __restrict__ spatials_out, int n, int F, int Kp, int f16, int split16, const int* __restrict__ offs) {
+    const int b = blockIdx.x;
+    int row0, box0, nb;                                              // first operand row, first detector row, valid boxes
+    if (offs == nullptr) {
+        row0 = b * (n + 1); box0 = b * n;
+        nb = num_boxes ? num_boxes[b] : n;
+        nb = nb < 0 ? 0 : (nb > n ? n : nb);
+    } else {
+        row0 = offs[b]; box0 = row0 - b;
+        n = nb = offs[b + 1] - row0 - 1;
+    }
+    const int V = n + 1;
     const size_t ld = static_cast<size_t>(split16 ? 3 * Kp : Kp);
     auto put = [&](int row, int i, const float (&x)[8]) {           // 8 columns [8i, 8i+8) of operand row `row`
         uint4* dst = reinterpret_cast<uint4*>(a_out + static_cast<size_t>(row) * ld);
@@ -175,7 +186,7 @@ region_pack_kernel(const float* __restrict__ box_feats, const float* __restrict_
         const int i = blockIdx.y * blockDim.x + threadIdx.x;           // 8-column group
         if (i * 8 >= F) return;
         float sum[8] = {0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f};
-        const float* src = box_feats + static_cast<size_t>(b) * n * F + i * 8;
+        const float* src = box_feats + static_cast<size_t>(box0) * F + i * 8;
         for (int r = 0; r < n; ++r) {
             float x[8] = {0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f};
             if (r < nb) {
@@ -185,12 +196,12 @@ region_pack_kernel(const float* __restrict__ box_feats, const float* __restrict_
 #pragma unroll
                 for (int j = 0; j < 8; ++j) sum[j] += x[j];
             }
-            put(b * V + r + 1, i, x);
+            put(row0 + r + 1, i, x);
         }
         const float cnt = static_cast<float>(nb > 0 ? nb : 1);
 #pragma unroll
         for (int j = 0; j < 8; ++j) sum[j] = sum[j] / cnt;              // torch.sum(feature, dim=0) / num_boxes (worker.py:432)
-        put(b * V, i, sum);
+        put(row0, i, sum);
         return;
     }
     const float w = image_wh[2 * b], h = image_wh[2 * b + 1];
@@ -201,18 +212,18 @@ region_pack_kernel(const float* __restrict__ box_feats, const float* __restrict_
         const bool real = r == 0 || r - 1 < nb;
         if (r == 0) { loc[2] = loc[3] = loc[4] = 1.0f; }               // g_location = [0, 0, 1, 1, 1] (worker.py:443)
         else if (real) {
-            const float* bx = boxes + (static_cast<size_t>(b) * n + (r - 1)) * 4;
+            const float* bx = boxes + (static_cast<size_t>(box0) + (r - 1)) * 4;
             const float x1 = bx[0], y1 = bx[1], x2 = bx[2], y2 = bx[3];
             loc[4] = (y2 - y1) * (x2 - x1) / wh;                       // computed before the coordinates are normalised (worker.py:438)
             loc[0] = x1 / w; loc[1] = y1 / h; loc[2] = x2 / w; loc[3] = y2 / h;
         }
         const float zero[8] = {0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f};
         for (int g = 0; g < tail_groups; ++g) {
-            if (g == 0) put(b * V + r, F / 8, loc); else put(b * V + r, F / 8 + g, zero);
+            if (g == 0) put(row0 + r, F / 8, loc); else put(row0 + r, F / 8 + g, zero);
         }
-        mask_add[b * V + r] = real ? 0.0f : -10000.0f;
+        mask_add[row0 + r] = real ? 0.0f : -10000.0f;
         if (spatials_out)
-            for (int j = 0; j < 5; ++j) spatials_out[(static_cast<size_t>(b) * V + r) * 5 + j] = loc[j];
+            for (int j = 0; j < 5; ++j) spatials_out[(static_cast<size_t>(row0) + r) * 5 + j] = loc[j];
     }
 }
 
@@ -308,10 +319,13 @@ cudaError_t launch_image_pack(const float* feats, const float* loc, const uint8_
 
 cudaError_t launch_region_pack(const float* box_feats, const float* boxes, const float* image_wh, const int32_t* num_boxes,
                                __nv_bfloat16* a_out, float* mask_add, float* spatials_out, int B, int n, int F, int Kp, int f16,
-                               int split16, cudaStream_t st) {
-    if (B < 1 || n < 1 || F % 8 != 0 || Kp % 8 != 0 || Kp < F + 8 || (split16 && (!f16 || (Kp & 63)))) return cudaErrorInvalidValue;
+                               int split16, cudaStream_t st, const int* offs) {
+    if (B < 1 || (offs == nullptr && n < 1) || F % 8 != 0 || Kp % 8 != 0 || Kp < F + 8 || (split16 && (!f16 || (Kp & 63))) ||
+        (offs != nullptr && (num_boxes != nullptr || split16)))
+        return cudaErrorInvalidValue;
     const dim3 grid(B, (F / 8 + 127) / 128 + 1);
-    region_pack_kernel<<<grid, 128, 0, st>>>(box_feats, boxes, image_wh, num_boxes, a_out, mask_add, spatials_out, n, F, Kp, f16, split16);
+    region_pack_kernel<<<grid, 128, 0, st>>>(box_feats, boxes, image_wh, num_boxes, a_out, mask_add, spatials_out, n, F, Kp, f16, split16,
+                                             offs);
     return cudaGetLastError();
 }
 

@@ -1373,6 +1373,18 @@ struct vb200_engine {
         pack_image_packed(pl, in.features, in.spatials, meta[2 * (pl.B + 1) + 1], st);
         run_plan(pl, st);
     }
+    // Packed detector output on a PACKED plan: the region-pack kernel writes every image's mean row and boxes at the plan's image
+    // offsets (the same rows forward_regions writes for that image alone), then the packed forward runs as above
+    void forward_regions_packed(Plan& pl, const vb200_packed_region_inputs& in, const std::vector<int>& meta, cudaStream_t st) {
+        const Config& c = cfg;
+        const int rows_v = meta[2 * (pl.B + 1) + 1];
+        stage_meta(pl, meta, st);
+        embed_text_packed(pl, in.question, in.segment_ids, in.task_tokens, meta[2 * (pl.B + 1)], st);
+        CUDA_CHECK(vb::launch_region_pack(in.box_features, in.boxes, in.image_wh, nullptr, pl.img_a, pl.mask_v, in.spatials_out, pl.B, 0,
+                                          c.v_feat, pl.kp, opt.act_fp16, 0, st, pl.offs_v()));
+        zero_tail(pl.img_a, rows_v, pl.B * pl.V, pl.kp, st);
+        run_plan(pl, st);
+    }
     // meta (host, the plan's d_meta layout) -> d_meta, in stream order ahead of the plan's kernels
     void stage_meta(Plan& pl, const std::vector<int>& meta, cudaStream_t st) {
         CUDA_CHECK(cudaEventSynchronize(pl.meta_copied));           // the previous call's copy has left the staging buffer
@@ -1669,6 +1681,51 @@ int vb200_forward_packed(vb200_handle h, const vb200_packed_inputs* in, const vb
         Plan* pl = h->get_plan(B, t16 - task, v16, select & VB200_OUT_ALL, slot, vb200_engine::PACKED, false);
         cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
         h->forward_packed(*pl, *in, meta, st);
+        h->copy_outputs(*pl, *out, st, cudaMemcpyDeviceToDevice, meta[2 * (B + 1)], meta[2 * (B + 1) + 1]);
+    });
+}
+
+int vb200_forward_regions_packed(vb200_handle h, const vb200_packed_region_inputs* in, const vb200_outputs* out, uint32_t select,
+                                 int32_t slot, void* cuda_stream) {
+    if (h == nullptr) return VB200_ERR_INVALID;
+    return guard(h, [&] {
+        const char* api = "vb200_forward_regions_packed";
+        if (in == nullptr || out == nullptr) fail(VB200_ERR_INVALID, "inputs/outputs struct is NULL");
+        if (select & VB200_OUT_ATTENTION) fail(VB200_ERR_INVALID, "%s: the attention-probability output (VB200_OUT_ATTENTION) is not supported", api);
+        if (h->x3) fail(VB200_ERR_INVALID, "%s: packed batches are not supported in split_fp32 (fp32x) mode", api);
+        const Config& c = h->cfg;
+        const int B = in->batch, task = c.task_tokens ? 1 : 0;
+        if (B < 1) fail(VB200_ERR_INVALID, "%s: batch must be positive", api);
+        if (in->max_tokens < 0) fail(VB200_ERR_INVALID, "%s: negative capacity max_tokens %d", api, in->max_tokens);
+        if (in->max_boxes < 0) fail(VB200_ERR_INVALID, "%s: negative capacity max_boxes %d", api, in->max_boxes);
+        if (!in->n_tokens || !in->n_boxes || !in->question || !in->segment_ids || !in->box_features || !in->boxes || !in->image_wh ||
+            (task && !in->task_tokens))
+            fail(VB200_ERR_INVALID, "vb200_packed_region_inputs has a NULL required pointer");
+        if (in->max_boxes > 255) fail(VB200_ERR_INVALID, "%s: capacity max_boxes %d above 255 (V = boxes + 1 <= 256)", api, in->max_boxes);
+        // regions per image = boxes + the global mean row; these checks name the caller's fields before pack_lengths sees V_i / T_i
+        std::vector<int32_t> nv(B);
+        for (int i = 0; i < B; ++i) {
+            const int n = in->n_boxes[i], t = in->n_tokens[i];
+            if (n < 1) fail(VB200_ERR_INVALID, "%s: image %d has n_boxes %d (must be >= 1)", api, i, n);
+            if (in->max_boxes > 0 && n > in->max_boxes)
+                fail(VB200_ERR_INVALID, "%s: image %d has n_boxes %d, above the capacity max_boxes %d", api, i, n, in->max_boxes);
+            if (n + 1 > 256) fail(VB200_ERR_INVALID, "%s: image %d has n_boxes %d (V = n_boxes + 1 must be <= 256)", api, i, n);
+            if (t + task > 256) fail(VB200_ERR_INVALID, "%s: image %d has n_tokens %d (T = n_tokens + 1 must be <= 256)", api, i, t);
+            nv[i] = n + 1;
+        }
+        const int cap_v = in->max_boxes > 0 ? in->max_boxes + 1 : 0;
+        // meta = text row offsets [B + 1] | image row offsets [B + 1] | text rows | image rows (the plan's d_meta layout)
+        std::vector<int> meta(2 * (static_cast<size_t>(B) + 1) + 2, 0);
+        const int max_tin = pack_lengths(api, "image", true, c, in->n_tokens, B, in->max_tokens, meta.data());
+        const int max_v = pack_lengths(api, "image", false, c, nv.data(), B, cap_v, meta.data() + B + 1);
+        meta[2 * (B + 1)] = meta[B];
+        meta[2 * (B + 1) + 1] = meta[2 * B + 1];
+        const int t16 = capacity16(api, in->max_tokens, max_tin, task, "T");
+        const int v16 = capacity16(api, cap_v, max_v, 0, "V");
+        CUDA_CHECK(cudaSetDevice(h->opt.device));
+        Plan* pl = h->get_plan(B, t16 - task, v16, select & VB200_OUT_ALL, slot, vb200_engine::PACKED, false);
+        cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+        h->forward_regions_packed(*pl, *in, meta, st);
         h->copy_outputs(*pl, *out, st, cudaMemcpyDeviceToDevice, meta[2 * (B + 1)], meta[2 * (B + 1) + 1]);
     });
 }

@@ -95,9 +95,12 @@ cudaError_t launch_image_pack(const float* feats, const float* loc, const uint8_
                               float* mask_add, int rows, int F, int Kp, int f16, int split16, cudaStream_t st);
 // custom_prediction()'s tensor construction on the device (worker.py:422-455): box features [B, n, F] + pixel boxes [B, n, 4] +
 // image sizes [B, 2] (+ optional valid-box counts) -> operand rows [B * (n + 1), Kp] with the global mean row first, masks, spatials.
+// Packed batches (offs != nullptr): offs = device [B + 1] image row offsets (V_b = boxes_b + 1 regions per image), box_features /
+// boxes hold image b's V_b - 1 boxes from detector row offs[b] - b, every row is real, n and num_boxes are unused (num_boxes must be
+// null, and split16 0), spatials_out is [offs[B], 5].
 cudaError_t launch_region_pack(const float* box_feats, const float* boxes, const float* image_wh, const int32_t* num_boxes,
                                __nv_bfloat16* a_out, float* mask_add, float* spatials_out, int B, int n, int F, int Kp, int f16,
-                               int split16, cudaStream_t st);
+                               int split16, cudaStream_t st, const int* offs = nullptr);
 // retrieval reuse: cached encoder state rows idx[b] -> sample b of a pair plan (fp32 stream [L, H], 16-bit operand [L, H16], mask [L]);
 // the fp32 and mask copies are skipped when their pointers are null (packed poolers: the first 16-bit row of every sample)
 cudaError_t launch_gather_state(const int32_t* idx, int n_src, const float* src_f32, const void* src_16, const float* src_mask,

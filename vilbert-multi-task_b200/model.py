@@ -425,6 +425,54 @@ class VILBertForVLTasks(object):
             L.check(lib.vb200_forward_packed(self._handle, C.byref(inp), C.byref(o), select, slot, C.c_void_p(stream)), self._handle)
         return self._result(outs, B, 0, 0, debug_taps)
 
+    @torch.no_grad()
+    def forward_regions_packed(self, question, segment_ids, task_tokens, box_features, boxes, image_wh, n_tokens, n_boxes,
+                               select: int = L.OUT_TASK_HEADS, slot: int = 0, max_tokens: int = 0, max_boxes: int = 0,
+                               debug_taps: bool = False, return_spatials: bool = True):
+        """``forward_regions`` with every image at its own box count and every text at its own length, stored back to back without
+        padding: ``question`` / ``segment_ids`` ``[sum Tin_i]`` (text already repeated per image), ``task_tokens`` ``[B, 1]``,
+        ``box_features`` ``[sum n_boxes_i, F]`` and pixel ``boxes`` ``[sum n_boxes_i, 4]`` as the detector returned them,
+        ``image_wh`` ``[B, 2]``; ``n_tokens`` / ``n_boxes`` (lists or CPU int tensors) give Tin_i and the box counts.  Image i has
+        V_i = n_boxes_i + 1 regions (its global mean row first).  Returns ``(10-tuple, spatials)``: the tuple as ``forward_packed``
+        returns it (per-image outputs ``[B, ...]``, per-row outputs packed over sum V_i / sum T_i rows), ``spatials`` the packed
+        ``[sum V_i, 5]`` locations the reference would have built (None with ``return_spatials=False``).  Each image's rows are
+        bit-identical to ``forward_regions`` of that image alone.  ``max_tokens`` / ``max_boxes`` (0: this call's maxima) are the
+        plan's capacities; the plan is the one ``forward_packed`` uses at ``max_regions = max_boxes + 1``."""
+        if self._handle is None:
+            raise L.VilbertB200Error("call model.cuda(i) first (worker.py:536); there is no CPU path")
+        lib = L.load()
+        device = torch.device("cuda", self._device)
+        nt, nb = _host_ints(n_tokens), _host_ints(n_boxes)
+        B = len(nt)
+        if len(nb) != B or B < 1:
+            raise ValueError("forward_regions_packed: n_tokens and n_boxes must have the same, positive length")
+
+        def dev(t, dtype):
+            return torch.as_tensor(t).to(device=device, dtype=dtype, non_blocking=True).contiguous()
+        F = self._dims["v_feature_size"]
+        q = dev(question, torch.int64).reshape(-1)
+        seg = dev(segment_ids if segment_ids is not None else torch.zeros_like(q), torch.int64).reshape(-1)
+        tk = dev(task_tokens if task_tokens is not None else torch.zeros(B, 1, dtype=torch.int64), torch.int64).reshape(B, -1)[:, :1]
+        tk = tk.contiguous()
+        bf, bx, wh = dev(box_features, torch.float32).reshape(-1, F), dev(boxes, torch.float32).reshape(-1, 4), dev(image_wh, torch.float32)
+        sum_tin, sum_n = sum(nt), sum(nb)
+        if q.numel() != sum_tin or seg.numel() != sum_tin or bf.shape[0] != sum_n or bx.shape[0] != sum_n or tuple(wh.shape) != (B, 2):
+            raise ValueError("forward_regions_packed: question / segment_ids need sum(n_tokens) entries, box_features / boxes "
+                             "sum(n_boxes) rows, image_wh [B, 2]")
+        rows_t = sum_tin + (B if self._dims["task_specific_tokens"] else 0)
+        rows_v = sum_n + B
+        sp = torch.empty(rows_v, 5, dtype=torch.float32, device=device) if return_spatials else None
+        outs, o = self._alloc_packed_outputs(B, rows_t, rows_v, select, debug_taps, device)
+        nt_c, nb_c = (C.c_int32 * B)(*nt), (C.c_int32 * B)(*nb)
+        inp = L.PackedRegionInputs(B, int(max_tokens), int(max_boxes), C.cast(nt_c, C.c_void_p), C.cast(nb_c, C.c_void_p),
+                                   q.data_ptr(), seg.data_ptr(), tk.data_ptr(), bf.data_ptr(), bx.data_ptr(), wh.data_ptr(),
+                                   sp.data_ptr() if sp is not None else None)
+        with torch.cuda.device(device):
+            stream = torch.cuda.current_stream(device).cuda_stream
+            L.check(lib.vb200_forward_regions_packed(self._handle, C.byref(inp), C.byref(o), select, slot, C.c_void_p(stream)),
+                    self._handle)
+        return self._result(outs, B, 0, 0, debug_taps), sp
+
     def _alloc_packed_outputs(self, B, rows_t, rows_v, select, debug_taps, device):
         """Outputs of a packed call: per-sample outputs [B, ...], per-row outputs and taps [rows_t or rows_v, ...]."""
         d = self._dims

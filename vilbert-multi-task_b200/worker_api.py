@@ -360,6 +360,120 @@ def custom_prediction(query, task, features, infos, task_id):
     return _decode(task_id, out, spatials, infos)
 
 
+def real_tokens(query, tok=None):
+    """tokenize_query without the padding: the input_mask prefix of (tokens, segment_ids)."""
+    tokens, input_mask, segment_ids = tokenize_query(query, tok)
+    k = sum(1 for m in input_mask if m)
+    return tokens[:k], segment_ids[:k]
+
+
+def pack_region_requests(requests, bucket: int = 8, select: Optional[int] = None, max_boxes: int = 100, tok=None):
+    """The host half of `custom_prediction_packed`: `custom_prediction` argument tuples `(query, task, features, infos, task_id)` ->
+    the inputs of ONE `forward_regions_packed` call, as CPU tensors.
+
+    Every text keeps its real tokens only and is repeated per image for NLVR2 / retrieval; every image keeps its own box count.
+    NLVR2 pairs start on even rows and the batch is padded to a multiple of `bucket` (even when the pair head is computed), both with
+    filler rows of one token and one zero box in a 1 x 1 image.  The capacities are max(MAX_LENGTH, longest query) tokens and
+    max(`max_boxes`, most boxes): with the defaults a long-running worker keeps one plan per batch size.  A request that fails
+    validation gets its exception in `answers` and takes no row.  Returns a dict: answers, spans {request: (first row, end row)},
+    n_tokens, n_boxes, question, segment_ids, task_tokens [B, 1], box_features, boxes, image_wh, select, max_tokens, max_boxes."""
+    if bucket < 1:
+        raise ValueError("bucket must be >= 1")
+    fixed_select = L.OUT_TASK_HEADS if select is None else int(select)
+    answers = [None] * len(requests)
+    rows, spans, need, F = [], {}, 0, None        # rows: (tokens, segments, task, box features [n, F], boxes [n, 4], (w, h))
+    for i, (query, task, features, infos, task_id) in enumerate(requests):
+        try:
+            _validate(task_id, infos)
+            if len(features) != len(infos):
+                raise ValueError(f"{len(features)} feature arrays for {len(infos)} images")
+            tokens, segs = real_tokens(query, tok)
+            if len(tokens) + 1 > 256:
+                raise ValueError(f"query of {len(tokens)} tokens: packed rows hold at most 255")
+            imgs = []
+            for f, info in zip(features, infos):
+                f = torch.as_tensor(f, dtype=torch.float32)
+                n = int(f.shape[0]) if f.dim() == 2 else 0
+                if n < 1 or n + 1 > 256 or (F is not None and f.shape[1] != F):
+                    raise ValueError(f"box features of shape {tuple(f.shape)}: need [n, F] with 1 <= n <= 255"
+                                     + (f" and F = {F}" if F is not None else ""))
+                bx = torch.as_tensor(np.asarray(info["bbox"], dtype=np.float32))
+                if bx.dim() != 2 or bx.shape[0] < n or bx.shape[1] < 4:
+                    raise ValueError(f"bbox of shape {tuple(bx.shape)} for {n} boxes")
+                imgs.append((f, bx[:n, :4], (float(info["image_width"]), float(info["image_height"]))))
+            t = int(np.array(task).reshape(-1)[0])
+        except Exception as e:                      # noqa: BLE001 -- the request's answer, as callback()'s catch-all (worker.py:653-655)
+            answers[i] = e
+            continue
+        F = int(imgs[0][0].shape[1])
+        if task_id in PAIR_TASKS and len(rows) % 2 == 1:
+            rows.append(None)                       # filler: the pair starts on an even row
+        rep = task_id in PAIR_TASKS + RETRIEVAL_TASKS
+        spans[i] = (len(rows), len(rows) + (len(imgs) if rep else 1))
+        for f, bx, wh in (imgs if rep else imgs[:1]):
+            rows.append((tokens, segs, t, f, bx, wh))
+        need |= TASK_OUTPUT[task_id]
+    sel = fixed_select | need
+    target = -(-len(rows) // bucket) * bucket
+    if target % 2 == 1 and (sel & L.OUT_VIL_BINARY_PREDICTION):
+        target += 1                                 # the binary head needs an even number of rows
+    rows += [None] * (target - len(rows))
+    filler = ([0], [0], 0, torch.zeros(1, F or 1), torch.zeros(1, 4), (1.0, 1.0))
+    rows = [filler if r is None else r for r in rows]
+    n_tokens = [len(r[0]) for r in rows]
+    n_boxes = [int(r[3].shape[0]) for r in rows]
+    return dict(answers=answers, spans=spans, n_tokens=n_tokens, n_boxes=n_boxes,
+                question=torch.tensor([x for r in rows for x in r[0]], dtype=torch.long),
+                segment_ids=torch.tensor([x for r in rows for x in r[1]], dtype=torch.long),
+                task_tokens=torch.tensor([[r[2]] for r in rows], dtype=torch.long),
+                box_features=torch.cat([r[3] for r in rows], dim=0) if rows else torch.zeros(0, 1),
+                boxes=torch.cat([r[4] for r in rows], dim=0) if rows else torch.zeros(0, 4),
+                image_wh=torch.tensor([list(r[5]) for r in rows], dtype=torch.float32).reshape(-1, 2),
+                select=sel, max_tokens=max([MAX_LENGTH] + n_tokens), max_boxes=max([int(max_boxes)] + n_boxes))
+
+
+def split_region_outputs(out, spatials, n_tokens, n_boxes, lo, hi, task_id):
+    """Rows [lo, hi) of a `forward_regions_packed` result -> the 10-tuple and spatials `_decode` reads for one request.  Per-image
+    outputs are sliced; the pair head keeps the request's pair; per-row outputs (and spatials) keep the request's packed rows, shaped
+    [1, V, ...] for a single-image request (the grounding decode reads its own vision_logit and spatials rows)."""
+    t_off = np.concatenate([[0], np.cumsum([n + 1 for n in n_tokens])])   # packed text rows (task token included)
+    v_off = np.concatenate([[0], np.cumsum([n + 1 for n in n_boxes])])    # packed regions: the global row, then the boxes
+    sl = [None if o is None or isinstance(o, list) else o[lo:hi] for o in out[:9]] + [[]]
+    if out[3] is not None:
+        sl[3] = out[3][lo // 2:hi // 2] if task_id == "12" else out[3][0:0]
+    one = hi - lo == 1
+    for k, offs in ((5, v_off), (6, v_off), (7, t_off), (8, t_off)):
+        if out[k] is not None:
+            r = out[k][int(offs[lo]):int(offs[hi])]
+            sl[k] = r.reshape(1, -1, r.shape[-1]) if one else r
+    sp = None
+    if spatials is not None:
+        sp = spatials[int(v_off[lo]):int(v_off[hi])]
+        sp = sp.reshape(1, -1, 5) if one else sp
+    return tuple(sl), sp
+
+
+def custom_prediction_packed(requests, bucket: int = 8, select: Optional[int] = None, max_boxes: int = 100):
+    """`custom_prediction` for many requests in ONE model call (`model.forward_regions_packed`): every question at its own length,
+    every image at its own box count, no padding and no masks.  `requests` are argument tuples of `custom_prediction`:
+    `(query, task, features, infos, task_id)`; the answers come back in the same order, a request that fails validation gets its
+    exception.  The host packing is `pack_region_requests`.  Answers agree with `custom_prediction` within tolerance; they are not
+    guaranteed bit for bit, because dropping the text padding may change the accumulation."""
+    p = pack_region_requests(requests, bucket, select, max_boxes)
+    answers = p["answers"]
+    if not p["spans"]:
+        return answers
+    with model_lock:
+        out, spatials = model.forward_regions_packed(p["question"], p["segment_ids"], p["task_tokens"], p["box_features"], p["boxes"],
+                                                     p["image_wh"], p["n_tokens"], p["n_boxes"], select=p["select"],
+                                                     max_tokens=p["max_tokens"], max_boxes=p["max_boxes"])
+    for i, (lo, hi) in p["spans"].items():
+        task_id, infos = requests[i][4], requests[i][3]
+        sl, sp = split_region_outputs(out, spatials, p["n_tokens"], p["n_boxes"], lo, hi, task_id)
+        answers[i] = _decode(task_id, sl, sp, infos)
+    return answers
+
+
 def shape_result(task_id: str, answer, image_path: Sequence[str], image_names: Optional[List[str]] = None):
     """The JSON-able `result` dict callback() pushes to the WebSocket, per task family (worker.py:564-645).
     Box drawing / file writing (cv2, worker.py:596-600) is left to the caller; pass the names it chose."""
@@ -400,12 +514,19 @@ class MicroBatchWorker(object):
     `concurrent.futures.Future` whose result is `{"socket_id": ..., "result": <the dict callback() pushes to the WebSocket,
     worker.py:564-649>}`.  A background thread drains the queue: it waits at most `max_wait_ms` after the first pending message
     for up to `max_rows` image rows, runs them through `prediction_batch` (one model call per shape group) and resolves the
-    futures; a failing request resolves to its exception, like the try/except of callback (worker.py:653-655)."""
+    futures; a failing request resolves to its exception, like the try/except of callback (worker.py:653-655).
 
-    def __init__(self, max_rows: int = 64, max_wait_ms: float = 2.0, bucket: int = 8):
+    `packed=True` hands the raw detector output of the pending messages to `custom_prediction_packed` instead: ONE model call
+    whatever their text lengths and box counts (images of one message may have different box counts too), with no host-side
+    feature construction.  Answers agree with the dense path within tolerance; they are not guaranteed bit for bit, because dropping
+    the text padding may change the accumulation.  The default stays dense; making packed the default and deleting the dense
+    branch is a follow-up, to be decided on the A/B of scripts/regions_packed_bench.py."""
+
+    def __init__(self, max_rows: int = 64, max_wait_ms: float = 2.0, bucket: int = 8, packed: bool = False):
         import queue
         import threading
         self.max_rows, self.max_wait, self.bucket = int(max_rows), float(max_wait_ms) * 1e-3, int(bucket)
+        self.packed = bool(packed)
         self._q = queue.Queue()
         self._stop = False
         self.batches = []                      # rows per model call group, for tests / monitoring
@@ -462,6 +583,8 @@ class MicroBatchWorker(object):
             self._run(pending)
 
     def _run(self, pending):
+        if self.packed:
+            return self._run_packed(pending)
         device = torch.device("cuda", model._device) if torch.cuda.is_available() else torch.device("cpu")
         reqs, live = [], []
         for body, features, infos, fut in pending:
@@ -480,6 +603,29 @@ class MicroBatchWorker(object):
                 fut.set_exception(e)
             return
         self.batches.append(sum(r[1].shape[0] for r in reqs))
+        self._resolve(live, answers)
+
+    def _run_packed(self, pending):
+        reqs, live = [], []
+        for body, features, infos, fut in pending:
+            try:
+                task_id = str(body["task_id"])
+                reqs.append((body["question"], [int(task_id)], features, infos, task_id))
+                live.append((body, fut, task_id))
+            except Exception as e:             # noqa: BLE001
+                fut.set_exception(e)
+        if not reqs:
+            return
+        try:
+            answers = custom_prediction_packed(reqs, bucket=self.bucket)
+        except Exception as e:                 # noqa: BLE001
+            for _, fut, _ in live:
+                fut.set_exception(e)
+            return
+        self.batches.append(sum(len(r[3]) for r, a in zip(reqs, answers) if not isinstance(a, Exception)))
+        self._resolve(live, answers)
+
+    def _resolve(self, live, answers):
         for (body, fut, task_id), ans in zip(live, answers):
             if isinstance(ans, Exception):
                 fut.set_exception(ans)
