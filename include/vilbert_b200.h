@@ -71,10 +71,13 @@ enum {
     VB200_OUT_LINGUISIC_LOGIT = 1 << 8,        /* [B, T, 1]        never read by the worker */
     VB200_OUT_TASK_HEADS = 0x15F,              /* the seven task heads (everything but the two pre-training heads) */
     VB200_OUT_ALL = 0x1FF,
-    VB200_OUT_ATTENTION = 1 << 9               /* element 9 of the tuple, attn_data_list: the attention probabilities of all 24 layers
+    VB200_OUT_ATTENTION = 1 << 9,              /* element 9 of the tuple, attn_data_list: the attention probabilities of all 24 layers
                                                   (worker.py:287-288; the reference returns them because config.visualization is set,
                                                   worker.py:522, and never reads them).  Off unless requested: see
                                                   vb200_attention_layout and vb200_outputs.attention_probs. */
+    VB200_OUT_ATTENTION_PACKED = 1 << 10       /* the same probabilities for a packed batch, every sample at its own lengths: accepted by
+                                                  vb200_forward_packed and vb200_forward_regions_packed only (see there and
+                                                  vb200_attention_layout_packed); VB200_ERR_INVALID on every other forward */
 };
 
 /* Inputs of one forward, in the dtypes the worker builds them (worker.py:416-419, 452-455).
@@ -110,7 +113,8 @@ typedef struct {
     float* pooled_output;          /* optional debug tap: pooled_t * pooled_v [B, bi_hidden] */
     float* attention_probs;        /* VB200_OUT_ATTENTION: one flat fp32 buffer holding every layer's softmax probabilities
                                       [B, heads, Lq, Lk] back to back in execution order (vb200_attention_layout gives the
-                                      offsets); NULL skips the copy */
+                                      offsets); NULL skips the copy.  VB200_OUT_ATTENTION_PACKED: required, device memory of
+                                      vb200_attention_layout_packed's total_floats, written in place by the forward's kernels */
 } vb200_outputs;
 
 /* Engine options (all optional; zero-initialise for defaults).  Flags are tri-state: 0 default, 1 on, -1 off. */
@@ -241,6 +245,7 @@ int vb200_forward_regions(vb200_handle h, const vb200_region_inputs* in, const v
  * past the call's row totals are skipped, attention runs each sample at its own length), so a server that passes fixed capacities
  * keeps one plan and one CUDA graph per batch size whatever the lengths.  The lengths are host arrays (the plan is chosen on the
  * host); the per-sample offsets and row totals are copied to the plan's workspace on cuda_stream through a pinned staging buffer.
+ * Attention maps: VB200_OUT_ATTENTION_PACKED, see vb200_attention_layout_packed.
  * VB200_ERR_INVALID for VB200_OUT_ATTENTION, split_fp32 engines, a length < 1 or above a non-zero capacity, T_i or V_i > 256 and
  * Tin_i > max_position_embeddings. */
 typedef struct {
@@ -264,7 +269,8 @@ int vb200_forward_packed(vb200_handle h, const vb200_packed_inputs* in, const vb
  * bit-identical to vb200_forward_regions of that image alone (batch 1, n_boxes = n_boxes_i, n_tokens = Tin_i).  Plans are the
  * PACKED plans of vb200_forward_packed, keyed on (B, round16(max_tokens + 1), round16(max_boxes + 1), select, slot): the same plan and
  * CUDA graph serve both calls at equal capacities.  Outputs follow vb200_forward_packed (per-image outputs [B, ...], per-row outputs
- * packed over sum V_i / sum T_i rows).  VB200_ERR_INVALID for VB200_OUT_ATTENTION, split_fp32 engines, NULL required pointers,
+ * packed over sum V_i / sum T_i rows).  Attention maps: VB200_OUT_ATTENTION_PACKED, see vb200_attention_layout_packed (V_i = n_boxes_i + 1).
+ * VB200_ERR_INVALID for VB200_OUT_ATTENTION, split_fp32 engines, NULL required pointers,
  * n_boxes_i < 1 or above a non-zero max_boxes, V_i > 256, T_i > 256, Tin_i > max_position_embeddings and negative capacities. */
 typedef struct {
     int32_t batch;                  /* B images (rows of the forward); text already repeated per image as for vb200_region_inputs */
@@ -282,6 +288,25 @@ typedef struct {
 } vb200_packed_region_inputs;
 int vb200_forward_regions_packed(vb200_handle h, const vb200_packed_region_inputs* in, const vb200_outputs* out,
                                  uint32_t select, int32_t slot, void* cuda_stream);
+
+/* ---- Attention maps of a packed batch (VB200_OUT_ATTENTION_PACKED, both packed forwards above).  VB200_OUT_ATTENTION keeps
+ * meaning the dense [B, heads, Lq, Lk] layout and stays VB200_ERR_INVALID on packed calls; the packed bit selects this layout instead:
+ * entry e (execution order, the kinds of vb200_attention_layout: 30 entries for the 12/6/6 configuration) starts at float
+ * offsets[e] and holds, for sample b in batch order, a contiguous [heads, Lq_b, Lk_b] block at heads * sum_{b' < b} Lq_b' * Lk_b'
+ * inside the entry, with (Lq_b, Lk_b) = (T_b, T_b), (V_b, V_b), (T_b, V_b) or (V_b, T_b) for kinds 0-3 and T_b = Tin_b + 1 (task token).
+ * dims[2e] = heads, dims[2e + 1] = kind; total_floats is the buffer size (every float of it is written); arrays may be NULL to query
+ * the count only.  Builds no plan and never blocks.  n_tokens / n_regions are HOST arrays of Tin_b and V_b, validated as the
+ * packed forwards validate them (a length < 1, T_b or V_b > 256, Tin_b > max_position_embeddings: VB200_ERR_INVALID); for
+ * vb200_forward_regions_packed pass V_b = n_boxes_b + 1.
+ * A forward with the bit needs vb200_outputs.attention_probs (VB200_ERR_INVALID if NULL): the probability kernels write into it
+ * directly, each sample bit-identical to the probabilities of a dense forward of that sample alone, and every other output is
+ * bit-identical to the same call without the bit.  The destination pointer is staged with the call's offsets, so a call returns as
+ * soon as its work is enqueued, as without maps, and back-to-back calls may pass different buffers.  A packed plan with maps is a
+ * plan of its own (built, with its blocking first call, once per batch size and capacities), shared by every call at those
+ * capacities whatever the lengths. */
+int vb200_attention_layout_packed(vb200_handle h, int32_t batch, const int32_t* n_tokens /* HOST [batch] Tin_b */,
+                                  const int32_t* n_regions /* HOST [batch] V_b */, int32_t max_entries, int32_t* n_entries,
+                                  int32_t* dims, int64_t* offsets, int64_t* total_floats);
 
 /* ---- Caption-image retrieval with reuse (SURVEY.md section 8e; reference semantics worker.py:278-284, 359).  Everything ahead of
  * the first connection layer depends on the caption alone or on the image alone: encode each caption / image ONCE, then score

@@ -11,6 +11,12 @@
 // One CTA = (head, sample, 8 query rows), one warp per query row.  Keys are staged 32 at a time in shared memory with an odd
 // row stride, lane j owns key j of the chunk (no shuffle reductions); P V reads V rows straight from global memory (32
 // consecutive columns per warp instruction; the rows stay in L1/L2 for the other seven warps).
+//
+// Packed batches (VB200_OUT_ATTENTION_PACKED, kernels.h PackedProbs): the same kernel with PACKED = true.  Each CTA takes its
+// sample's query / key row offsets from the plan's d_meta, runs every loop, the key chunking and the softmax at the sample's own
+// Lq_b / Lk_b (the grid and shared memory are sized for the capacities; CTAs past Lq_b exit at once) and writes its probability
+// rows straight into the caller's buffer.  The arithmetic is this one code path, so each sample's probabilities are bit-identical
+// to a dense forward of that sample alone.  No context output: the tensor-core kernel writes it.
 #include "kernels.h"
 
 namespace vb {
@@ -34,24 +40,32 @@ __device__ __forceinline__ float ld_as_f32(const typename InT<IN>::type* p) {
 
 // q / k / v point at column 0 of head 0 of sample 0; row (b, i) of Q is q + (b * Lq + i) * ld_q, K/V rows use ld_kv.
 // ctx_mode: 0 no context output, 1 fp16, 2 bf16, 3 fp16 hi | lo | hi (ld_ctx is then the 3x wider physical stride).
-template <int IN>
+// PACKED: Lq / Lk are the capacities; sample b's rows and lengths come from pk (probs and ctx are unused).
+template <int IN, bool PACKED>
 __global__ void __launch_bounds__(32 * kQRows)
 attention_f32_kernel(const typename InT<IN>::type* __restrict__ q, int ld_q, const typename InT<IN>::type* __restrict__ k,
                      const typename InT<IN>::type* __restrict__ v, int ld_kv, const float* __restrict__ key_mask_add, int Lq,
                      int Lk, int D, float scale, uint16_t* __restrict__ ctx, int ld_ctx, int ctx_mode, float* __restrict__ probs,
-                     int pdl) {
+                     int pdl, PackedProbs pk) {
     extern __shared__ __align__(16) float smem_f32[];
     const int h = blockIdx.x, b = blockIdx.y, i0 = blockIdx.z * kQRows;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int Lkp = (Lk + 31) & ~31;
+    const int Lkp = (Lk + 31) & ~31;                   // PACKED: the capacity's, an upper bound of every sample's
     float* qs = smem_f32;                              // [kQRows][D]
     float* ks = qs + kQRows * D;                       // [kKeyChunk][D + 1]
     float* ps = ks + kKeyChunk * (D + 1);              // [kQRows][Lkp]
     if (pdl) pdl_wait();
+    // sample b: query rows [q0, q0 + Lq), key rows [k0, k0 + Lk)
+    int q0 = b * Lq, k0 = b * Lk;
+    if constexpr (PACKED) {
+        q0 = pk.offs_q[b]; Lq = pk.offs_q[b + 1] - q0;
+        k0 = pk.offs_k[b]; Lk = pk.offs_k[b + 1] - k0;
+        if (i0 >= Lq) return;                          // the whole CTA is past this sample's rows (no barrier reached yet)
+    }
     const int i = i0 + warp;                           // this warp's query row
     const bool row_ok = i < Lq;
     if (row_ok) {
-        const auto* qp = q + static_cast<size_t>(b * Lq + i) * ld_q + h * D;
+        const auto* qp = q + static_cast<size_t>(q0 + i) * ld_q + h * D;
         for (int d = lane; d < D; d += 32) qs[warp * D + d] = ld_as_f32<IN>(qp + d);
     }
     // ---- scores
@@ -59,7 +73,7 @@ attention_f32_kernel(const typename InT<IN>::type* __restrict__ q, int ld_q, con
         __syncthreads();                               // previous chunk consumed (and qs written, first pass)
         for (int e = threadIdx.x; e < kKeyChunk * D; e += blockDim.x) {
             const int j = e / D, d = e - j * D;
-            ks[j * (D + 1) + d] = (j0 + j < Lk) ? ld_as_f32<IN>(k + static_cast<size_t>(b * Lk + j0 + j) * ld_kv + h * D + d) : 0.0f;
+            ks[j * (D + 1) + d] = (j0 + j < Lk) ? ld_as_f32<IN>(k + static_cast<size_t>(k0 + j0 + j) * ld_kv + h * D + d) : 0.0f;
         }
         __syncthreads();
         if (row_ok) {
@@ -69,7 +83,7 @@ attention_f32_kernel(const typename InT<IN>::type* __restrict__ q, int ld_q, con
 #pragma unroll 8
             for (int d = 0; d < D; ++d) acc = fmaf(qr[d], kr[d], acc);
             const int j = j0 + lane;
-            ps[warp * Lkp + j] = j < Lk ? acc * scale + key_mask_add[b * Lk + j] : -INFINITY;
+            ps[warp * Lkp + j] = j < Lk ? acc * scale + key_mask_add[k0 + j] : -INFINITY;
         }
     }
     if (pdl) pdl_launch_dependents();
@@ -84,14 +98,22 @@ attention_f32_kernel(const typename InT<IN>::type* __restrict__ q, int ld_q, con
     for (int j = lane; j < Lk; j += 32) { const float e = expf(pr[j] - m); pr[j] = e; sum += e; }
     sum = warp_sum(sum);
     const float inv = 1.0f / sum;
-    float* gp = probs ? probs + ((static_cast<size_t>(b) * gridDim.x + h) * Lq + i) * Lk : nullptr;
+    float* gp = nullptr;
+    if constexpr (PACKED) {
+        // entry offset + heads * sum_{b' < b} Lq_b' Lk_b' + (h, i) inside the sample's [heads, Lq, Lk] block, in int64: one call's
+        // entries hold more than 2^31 floats at large batches
+        float* dst = reinterpret_cast<float*>(pk.dst[0]);
+        if (dst) gp = dst + pk.entry[0] + static_cast<int64_t>(gridDim.x) * pk.prefix[b] + (static_cast<int64_t>(h) * Lq + i) * Lk;
+    } else {
+        gp = probs ? probs + ((static_cast<size_t>(b) * gridDim.x + h) * Lq + i) * Lk : nullptr;
+    }
     for (int j = lane; j < Lk; j += 32) {
         const float pj = pr[j] * inv;
         pr[j] = pj;
         if (gp) gp[j] = pj;
     }
     __syncwarp();
-    if (ctx_mode == 0) return;
+    if (PACKED || ctx_mode == 0) return;
     // ---- context row: lane owns columns lane, lane + 32, ...
     float acc[4] = {0.0f, 0.0f, 0.0f, 0.0f};           // D <= 128
     const auto* vb = v + static_cast<size_t>(b) * Lk * ld_kv + h * D;
@@ -102,7 +124,7 @@ attention_f32_kernel(const typename InT<IN>::type* __restrict__ q, int ld_q, con
         for (int t = 0; t < 4; ++t)
             if (lane + 32 * t < D) acc[t] = fmaf(pj, ld_as_f32<IN>(vr + lane + 32 * t), acc[t]);
     }
-    uint16_t* orow = ctx + static_cast<size_t>(b * Lq + i) * ld_ctx;
+    uint16_t* orow = ctx + static_cast<size_t>(q0 + i) * ld_ctx;
 #pragma unroll
     for (int t = 0; t < 4; ++t) {
         const int c = h * D + lane + 32 * t;
@@ -124,27 +146,35 @@ attention_f32_kernel(const typename InT<IN>::type* __restrict__ q, int ld_q, con
 
 cudaError_t launch_attention_f32(const void* q, int ld_q, const void* k, const void* v, int ld_kv, int in_kind,
                                  const float* key_mask_add, int B, int Lq, int Lk, int heads, int D, __nv_bfloat16* ctx, int ld_ctx,
-                                 int ctx_mode, float* probs, int pdl, cudaStream_t st) {
+                                 int ctx_mode, float* probs, int pdl, cudaStream_t st, const PackedProbs* packed) {
     if (B < 1 || Lq < 1 || Lk < 1 || heads < 1 || D < 32 || D > 128 || (D & 31) || in_kind < 0 || in_kind > 2 || ctx_mode < 0 ||
-        ctx_mode > 3 || (ctx_mode != 0 && ctx == nullptr) || (ctx_mode == 0 && probs == nullptr))
+        ctx_mode > 3 || (ctx_mode != 0 && ctx == nullptr) || (ctx_mode == 0 && probs == nullptr && packed == nullptr))
         return cudaErrorInvalidValue;
+    if (packed && (ctx_mode != 0 || probs != nullptr || in_kind == 0 || !packed->offs_q || !packed->offs_k || !packed->dst ||
+                   !packed->entry || !packed->prefix))
+        return cudaErrorInvalidValue;
+    const PackedProbs pk = packed ? *packed : PackedProbs{};
     const int Lkp = (Lk + 31) & ~31;
     const size_t smem = sizeof(float) * (static_cast<size_t>(kQRows) * D + kKeyChunk * (D + 1) + static_cast<size_t>(kQRows) * Lkp);
     const dim3 grid(heads, B, (Lq + kQRows - 1) / kQRows), block(32 * kQRows);
     const float scale = 1.0f / sqrtf(static_cast<float>(D));
     uint16_t* c16 = reinterpret_cast<uint16_t*>(ctx);
-#define VB_AF(IN)                                                                                                        \
+#define VB_AF(IN, P)                                                                                                     \
     do {                                                                                                                 \
-        cudaError_t e = set_smem(attention_f32_kernel<IN>, smem);                                                        \
+        cudaError_t e = set_smem(attention_f32_kernel<IN, P>, smem);                                                     \
         if (e != cudaSuccess) return e;                                                                                  \
         using T = typename InT<IN>::type;                                                                                \
-        return launch_ex(attention_f32_kernel<IN>, grid, block, smem, pdl, st, static_cast<const T*>(q), ld_q,           \
+        return launch_ex(attention_f32_kernel<IN, P>, grid, block, smem, pdl, st, static_cast<const T*>(q), ld_q,        \
                          static_cast<const T*>(k), static_cast<const T*>(v), ld_kv, key_mask_add, Lq, Lk, D, scale, c16, \
-                         ld_ctx, ctx_mode, probs, pdl);                                                                  \
+                         ld_ctx, ctx_mode, probs, pdl, pk);                                                              \
     } while (0)
-    if (in_kind == 0) VB_AF(0);
-    if (in_kind == 1) VB_AF(1);
-    VB_AF(2);
+    if (packed) {
+        if (in_kind == 1) VB_AF(1, true);
+        VB_AF(2, true);
+    }
+    if (in_kind == 0) VB_AF(0, false);
+    if (in_kind == 1) VB_AF(1, false);
+    VB_AF(2, false);
 #undef VB_AF
 }
 

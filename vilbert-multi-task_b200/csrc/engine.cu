@@ -374,6 +374,8 @@ struct Op {
     const float* f_mask = nullptr;
     bf16* f_ctx = nullptr;
     float* f_probs = nullptr;
+    bool f_packed = false;         // packed plan with VB200_OUT_ATTENTION_PACKED: per-sample rows and destination from f_pk
+    vb::PackedProbs f_pk{};
     // attention
     const bf16 *qkv_a = nullptr, *qkv_b = nullptr;
     int ld_a = 0, ld_b = 0, hidden = 0;
@@ -440,6 +442,13 @@ struct Plan {
     const int* rows_v() const { return d_meta + 2 * (B + 1) + 1; }
     const int* src_t() const { return d_meta + 2 * (B + 1) + 2; }
     const int* src_v() const { return d_meta + 2 * (B + 1) + 2 + B; }
+    // packed plans with the packed attention-probability output (VB200_OUT_ATTENTION_PACKED): d_meta continues, 8-byte aligned at
+    // int probs_base(B), with int64 destination pointer | entry float offsets [n_probs] | per-sample prefix sums [3][B + 1]
+    // (sum T_b'^2, sum V_b'^2, sum T_b' V_b' over b' < b), staged per call with the rest of the meta
+    int n_probs = 0;
+    static size_t probs_base(int B) { return (2 * (static_cast<size_t>(B) + 1) + 2 + 1) & ~static_cast<size_t>(1); }
+    static size_t probs_meta_len(int B, int n_entries) { return 1 + static_cast<size_t>(n_entries) + 3 * (static_cast<size_t>(B) + 1); }
+    const int64_t* probs_meta() const { return reinterpret_cast<const int64_t*>(d_meta + probs_base(B)); }
     ~Plan() {
         if (exec) cudaGraphExecDestroy(exec);
         if (graph) cudaGraphDestroy(graph);
@@ -827,9 +836,12 @@ struct vb200_engine {
     }
     // softmax(Q K^T / sqrt(d) + mask) V of one stream (self) or one direction of a connection layer.  Default: the tensor-core
     // kernel writes the context (callers push that op themselves); this adds the fp32 kernel -- as THE attention in fp32-parity
-    // mode (context out as hi | lo | hi), and/or as the producer of the attention-probability output.
+    // mode (context out as hi | lo | hi), and/or as the producer of the attention-probability output.  Packed plans: the
+    // probabilities of every sample at its own lengths (query rows offs_q, key rows offs_k) straight into the caller's buffer, at
+    // the entry's offset and the sample's prefix sum `prefix` (0 T^2, 1 V^2, 2 T V) of the plan's probability meta.
     void add_attn_f32(Plan& pl, const void* q, int ld_q, const void* k, const void* v, int ld_kv, const float* mask, int Lq, int Lk,
-                      int heads, int hid, bf16* ctx, bool want_probs, int stream) {
+                      int heads, int hid, bf16* ctx, bool want_probs, int stream, const int* offs_q = nullptr,
+                      const int* offs_k = nullptr, int prefix = 0) {
         Op a{};
         a.kind = Op::ATTN_F32;
         a.stream = stream;
@@ -837,7 +849,13 @@ struct vb200_engine {
         a.f_in = x3 ? 0 : (opt.act_fp16 ? 1 : 2);
         a.B = pl.B; a.heads = heads; a.head_dim = hid / heads;
         a.f_ctx = x3 ? ctx : nullptr; a.f_ctx_mode = x3 ? 3 : 0; a.f_ld_ctx = x3 ? 3 * hid : 0;
-        if (want_probs) {
+        if (want_probs && pl.packed) {
+            const int n_entries = attention_entries();
+            const int64_t* pm = pl.probs_meta();
+            a.f_packed = true;
+            a.f_pk = vb::PackedProbs{offs_q, offs_k, pm, pm + 1 + pl.n_probs, pm + 1 + n_entries + static_cast<size_t>(prefix) * (pl.B + 1)};
+            ++pl.n_probs;
+        } else if (want_probs) {
             a.f_probs = pl.mem.alloc_n<float>(static_cast<size_t>(pl.B) * heads * Lq * Lk);
             pl.attn.push_back(Plan::AttnOut{a.f_probs, heads, Lq, Lk});
         }
@@ -852,6 +870,12 @@ struct vb200_engine {
         op.M = M; op.K = w.K; op.n_out = w.n_out;
         op.flops = 2.0 * M * w.K * w.n_out;
         return op;
+    }
+    // attention-probability entries of one forward: one per text / image layer, two per connection layer
+    int attention_entries() const {
+        int n = 0;
+        for (const std::string& step : schedule) n += step[0] == 'C' ? 2 : 1;
+        return n;
     }
     OutBuf make_out(Plan& pl, int rows, int cols) {
         OutBuf o; o.rows = rows; o.cols = cols; o.ld = (cols + 3) / 4 * 4;
@@ -892,7 +916,8 @@ struct vb200_engine {
         if (packed) {
             // zero offsets and totals until the first call: the validation pass and the capture below then touch no row
             pl.packed = true;
-            const size_t n_meta = 2 * (static_cast<size_t>(B) + 1) + 2 + (mode == PACKED_SUFFIX ? 2 * static_cast<size_t>(B) : 0);
+            size_t n_meta = 2 * (static_cast<size_t>(B) + 1) + 2 + (mode == PACKED_SUFFIX ? 2 * static_cast<size_t>(B) : 0);
+            if (want_attn) n_meta = Plan::probs_base(B) + 2 * Plan::probs_meta_len(B, attention_entries());
             pl.d_meta = pl.mem.alloc_n<int>(n_meta);
             CUDA_CHECK(cudaMemset(pl.d_meta, 0, n_meta * sizeof(int)));
             CUDA_CHECK(cudaMallocHost(&pl.h_meta, n_meta * sizeof(int)));
@@ -983,7 +1008,7 @@ struct vb200_engine {
             }
             if (x3 || want_attn)
                 add_attn_f32(pl, qkv_at(st.qkv, 0), 3 * hid, qkv_at(st.qkv, hid), qkv_at(st.qkv, 2 * hid), 3 * hid, st.mask, st.seq, st.seq,
-                             heads, hid, st.ctx, want_attn, stream);
+                             heads, hid, st.ctx, want_attn, stream, st.offs, st.offs, stream);   // prefix: stream 0 T^2, 1 V^2
             // attention output + LayerNorm1 (residual: the layer input) -> buffers [1 - cur]
             ln_linear(st, st.ctx, hid, L.attn_out, L.ln1, cur, 1 - cur, Op::NONE);
             add_linear(pl, st.b16[1 - cur], M, hid, L.inter, vb::kActGelu, nullptr, 0, nullptr, st.inter, inter, nullptr, 0, stream,
@@ -1031,9 +1056,9 @@ struct vb200_engine {
                 if (x3 || want_attn) {
                     // text queries (Q2) over image keys / values (K1, V1) -> text context; then image queries (Q1) over K2, V2
                     add_attn_f32(pl, qkv_at(qkv_t, 0), 3 * Hb, qkv_at(qkv_v, Hb), qkv_at(qkv_v, 2 * Hb), 3 * Hb, pl.mask_v, T, V,
-                                 c.bi_heads, Hb, ctx_t, want_attn, 0);
+                                 c.bi_heads, Hb, ctx_t, want_attn, 0, offs_t, offs_v, 2);
                     add_attn_f32(pl, qkv_at(qkv_v, 0), 3 * Hb, qkv_at(qkv_t, Hb), qkv_at(qkv_t, 2 * Hb), 3 * Hb, pl.mask_t, V, T,
-                                 c.bi_heads, Hb, ctx_v, want_attn, 0);
+                                 c.bi_heads, Hb, ctx_v, want_attn, 0, offs_v, offs_t, 2);
                 }
                 ops[first_co].sync = Op::JOIN;              // needs both projections
                 // image branch (side stream; forks from the co-attention): biOutput.dense1 + LayerNorm1, v_intermediate, v_output + LayerNorm
@@ -1223,7 +1248,7 @@ struct vb200_engine {
             case Op::ATTN_F32:
                 CUDA_CHECK(vb::launch_attention_f32(op.f_q, op.f_ld_q, op.f_k, op.f_v, op.f_ld_kv, op.f_in, op.f_mask, op.B, op.f_Lq,
                                                     op.f_Lk, op.heads, op.head_dim, op.f_ctx, op.f_ld_ctx, op.f_ctx_mode, op.f_probs,
-                                                    opt.use_pdl, st));
+                                                    opt.use_pdl, st, op.f_packed ? &op.f_pk : nullptr));
                 break;
             case Op::ROWDOT:
                 CUDA_CHECK(vb::launch_rowdot(op.x, op.ld_x, op.W, op.bias, op.add, op.out, op.ld_out, op.M, op.K, op.n_out, opt.use_pdl, st,
@@ -1501,7 +1526,8 @@ struct vb200_engine {
             CUDA_CHECK(cudaMemcpy2DAsync(dst, static_cast<size_t>(o.cols) * 4, o.p, static_cast<size_t>(o.ld) * 4,
                                          static_cast<size_t>(o.cols) * 4, rows, kind, st));
         }
-        if (out.attention_probs != nullptr) {
+        // packed probabilities (pl.n_probs > 0) were written into out.attention_probs by the plan's kernels: nothing to copy
+        if (out.attention_probs != nullptr && pl.n_probs == 0) {
             if (pl.attn.empty()) fail(VB200_ERR_INVALID, "attention_probs requested but VB200_OUT_ATTENTION is not set in `select`");
             float* dst = out.attention_probs;
             for (const Plan::AttnOut& a : pl.attn) {
@@ -1561,6 +1587,56 @@ int pack_lengths(const char* api, const char* item, bool text, const Config& c, 
         longest = std::max(longest, l);
     }
     return longest;
+}
+// Layout of the packed attention probabilities (VB200_OUT_ATTENTION_PACKED) from the two streams' row offsets [B + 1]: entries in
+// execution order (the order get_plan adds the probability ops in), each holding sample b's [heads, Lq_b, Lk_b] block at
+// heads * prefix[b]; prefix = sum over b' < b of T_b'^2 (text layers), V_b'^2 (image layers) or T_b' V_b' (both directions of a
+// connection layer).  int64 throughout: at batch 512 with 256 rows per sample one call holds more than 2^31 floats.
+struct PackedAttnLayout {
+    std::vector<int32_t> heads, kind;
+    std::vector<int64_t> offset;
+    std::vector<int64_t> prefix;       // [3][B + 1]
+    int64_t total = 0;
+};
+PackedAttnLayout packed_attn_layout(const Config& c, const std::vector<std::string>& schedule, int B, const int* offs_t, const int* offs_v) {
+    PackedAttnLayout l;
+    const size_t n = static_cast<size_t>(B) + 1;
+    l.prefix.assign(3 * n, 0);
+    for (int b = 0; b < B; ++b) {
+        const int64_t T = offs_t[b + 1] - offs_t[b], V = offs_v[b + 1] - offs_v[b];
+        l.prefix[b + 1] = l.prefix[b] + T * T;
+        l.prefix[n + b + 1] = l.prefix[n + b] + V * V;
+        l.prefix[2 * n + b + 1] = l.prefix[2 * n + b] + T * V;
+    }
+    auto put = [&](int heads, int kind) {
+        l.heads.push_back(heads);
+        l.kind.push_back(kind);
+        l.offset.push_back(l.total);
+        l.total += heads * l.prefix[(kind < 2 ? kind : 2) * n + B];
+    };
+    for (const std::string& step : schedule) {
+        if (step[0] == 'T') put(c.heads, 0);
+        else if (step[0] == 'V') put(c.v_heads, 1);
+        else { put(c.bi_heads, 2); put(c.bi_heads, 3); }
+    }
+    return l;
+}
+// Appends the plan's probability meta (Plan::probs_meta: destination | entry offsets | prefix sums) to a packed call's meta.
+void put_probs_meta(std::vector<int>& meta, int B, float* dst, const PackedAttnLayout& l) {
+    std::vector<int64_t> ext;
+    ext.reserve(1 + l.offset.size() + l.prefix.size());
+    ext.push_back(static_cast<int64_t>(reinterpret_cast<uintptr_t>(dst)));
+    ext.insert(ext.end(), l.offset.begin(), l.offset.end());
+    ext.insert(ext.end(), l.prefix.begin(), l.prefix.end());
+    const size_t base = Plan::probs_base(B);
+    meta.resize(base + 2 * ext.size(), 0);
+    memcpy(meta.data() + base, ext.data(), ext.size() * sizeof(int64_t));
+}
+// The packed probability layout exists for the two packed forwards only; every other forward rejects its select bit.
+void reject_packed_attention(uint32_t select, const char* api) {
+    if (select & VB200_OUT_ATTENTION_PACKED)
+        fail(VB200_ERR_INVALID, "%s: VB200_OUT_ATTENTION_PACKED is only supported by vb200_forward_packed and vb200_forward_regions_packed",
+             api);
 }
 // Plan capacity in rows per item, rounded up to the attention kernels' 16-row buckets: `cap` (0: the call's longest) + extra rows.
 int capacity16(const char* api, int cap, int longest, int extra, const char* rows_name) {
@@ -1647,6 +1723,7 @@ int vb200_forward_slot(vb200_handle h, const vb200_inputs* in, const vb200_outpu
     if (h == nullptr) return VB200_ERR_INVALID;
     return guard(h, [&] {
         if (in == nullptr || out == nullptr) fail(VB200_ERR_INVALID, "inputs/outputs struct is NULL");
+        reject_packed_attention(select, "vb200_forward");
         CUDA_CHECK(cudaSetDevice(h->opt.device));
         Plan* pl = h->get_plan(in->batch, in->n_tokens, in->n_regions, select & VB200_OUT_ALL, slot, vb200_engine::FULL,
                                (select & VB200_OUT_ATTENTION) != 0);
@@ -1663,6 +1740,9 @@ int vb200_forward_packed(vb200_handle h, const vb200_packed_inputs* in, const vb
         if (in == nullptr || out == nullptr) fail(VB200_ERR_INVALID, "inputs/outputs struct is NULL");
         if (select & VB200_OUT_ATTENTION) fail(VB200_ERR_INVALID, "packed batches: the attention-probability output (VB200_OUT_ATTENTION) is not supported");
         if (h->x3) fail(VB200_ERR_INVALID, "packed batches are not supported in split_fp32 (fp32x) mode");
+        const bool maps = (select & VB200_OUT_ATTENTION_PACKED) != 0;
+        if (maps && out->attention_probs == nullptr)
+            fail(VB200_ERR_INVALID, "packed batches: VB200_OUT_ATTENTION_PACKED needs vb200_outputs.attention_probs (NULL)");
         const Config& c = h->cfg;
         const int B = in->batch, task = c.task_tokens ? 1 : 0;
         if (B < 1) fail(VB200_ERR_INVALID, "packed batches: batch must be positive");
@@ -1677,8 +1757,9 @@ int vb200_forward_packed(vb200_handle h, const vb200_packed_inputs* in, const vb
         meta[2 * (B + 1) + 1] = meta[2 * B + 1];
         const int t16 = capacity16("packed batches", in->max_tokens, max_tin, task, "T");
         const int v16 = capacity16("packed batches", in->max_regions, max_v, 0, "V");
+        if (maps) put_probs_meta(meta, B, out->attention_probs, packed_attn_layout(c, h->schedule, B, meta.data(), meta.data() + B + 1));
         CUDA_CHECK(cudaSetDevice(h->opt.device));
-        Plan* pl = h->get_plan(B, t16 - task, v16, select & VB200_OUT_ALL, slot, vb200_engine::PACKED, false);
+        Plan* pl = h->get_plan(B, t16 - task, v16, select & VB200_OUT_ALL, slot, vb200_engine::PACKED, maps);
         cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
         h->forward_packed(*pl, *in, meta, st);
         h->copy_outputs(*pl, *out, st, cudaMemcpyDeviceToDevice, meta[2 * (B + 1)], meta[2 * (B + 1) + 1]);
@@ -1693,6 +1774,9 @@ int vb200_forward_regions_packed(vb200_handle h, const vb200_packed_region_input
         if (in == nullptr || out == nullptr) fail(VB200_ERR_INVALID, "inputs/outputs struct is NULL");
         if (select & VB200_OUT_ATTENTION) fail(VB200_ERR_INVALID, "%s: the attention-probability output (VB200_OUT_ATTENTION) is not supported", api);
         if (h->x3) fail(VB200_ERR_INVALID, "%s: packed batches are not supported in split_fp32 (fp32x) mode", api);
+        const bool maps = (select & VB200_OUT_ATTENTION_PACKED) != 0;
+        if (maps && out->attention_probs == nullptr)
+            fail(VB200_ERR_INVALID, "%s: VB200_OUT_ATTENTION_PACKED needs vb200_outputs.attention_probs (NULL)", api);
         const Config& c = h->cfg;
         const int B = in->batch, task = c.task_tokens ? 1 : 0;
         if (B < 1) fail(VB200_ERR_INVALID, "%s: batch must be positive", api);
@@ -1722,8 +1806,9 @@ int vb200_forward_regions_packed(vb200_handle h, const vb200_packed_region_input
         meta[2 * (B + 1) + 1] = meta[2 * B + 1];
         const int t16 = capacity16(api, in->max_tokens, max_tin, task, "T");
         const int v16 = capacity16(api, cap_v, max_v, 0, "V");
+        if (maps) put_probs_meta(meta, B, out->attention_probs, packed_attn_layout(c, h->schedule, B, meta.data(), meta.data() + B + 1));
         CUDA_CHECK(cudaSetDevice(h->opt.device));
-        Plan* pl = h->get_plan(B, t16 - task, v16, select & VB200_OUT_ALL, slot, vb200_engine::PACKED, false);
+        Plan* pl = h->get_plan(B, t16 - task, v16, select & VB200_OUT_ALL, slot, vb200_engine::PACKED, maps);
         cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
         h->forward_regions_packed(*pl, *in, meta, st);
         h->copy_outputs(*pl, *out, st, cudaMemcpyDeviceToDevice, meta[2 * (B + 1)], meta[2 * (B + 1) + 1]);
@@ -1736,6 +1821,7 @@ int vb200_forward_regions(vb200_handle h, const vb200_region_inputs* in, const v
     return guard(h, [&] {
         if (in == nullptr || out == nullptr) fail(VB200_ERR_INVALID, "inputs/outputs struct is NULL");
         if (in->n_boxes < 1) fail(VB200_ERR_INVALID, "n_boxes must be positive");
+        reject_packed_attention(select, "vb200_forward_regions");
         CUDA_CHECK(cudaSetDevice(h->opt.device));
         Plan* pl = h->get_plan(in->batch, in->n_tokens, in->n_boxes + 1, select & VB200_OUT_ALL, slot, vb200_engine::FULL,
                                (select & VB200_OUT_ATTENTION) != 0);
@@ -1774,6 +1860,7 @@ int vb200_forward_cached(vb200_handle h, int32_t batch, int32_t n_tokens, int32_
     return guard(h, [&] {
         if (out == nullptr) fail(VB200_ERR_INVALID, "outputs struct is NULL");
         if (n_text < 1 || n_image < 1) fail(VB200_ERR_INVALID, "cached state counts must be positive");
+        reject_packed_attention(select, "vb200_forward_cached");
         CUDA_CHECK(cudaSetDevice(h->opt.device));
         Plan* pl = h->get_plan(batch, n_tokens, n_regions, select & VB200_OUT_ALL, slot, vb200_engine::SUFFIX,
                                (select & VB200_OUT_ATTENTION) != 0);
@@ -1832,6 +1919,7 @@ int vb200_forward_cached_packed(vb200_handle h, const vb200_packed_pairs* in, co
         const char* api = "vb200_forward_cached_packed";
         if (in == nullptr || out == nullptr) fail(VB200_ERR_INVALID, "inputs/outputs struct is NULL");
         if (select & VB200_OUT_ATTENTION) fail(VB200_ERR_INVALID, "%s: the attention-probability output (VB200_OUT_ATTENTION) is not supported", api);
+        reject_packed_attention(select, api);
         if (h->x3) fail(VB200_ERR_INVALID, "%s: packed retrieval is not supported in split_fp32 (fp32x) mode", api);
         const Config& c = h->cfg;
         const int B = in->batch, task = c.task_tokens ? 1 : 0;
@@ -1904,6 +1992,28 @@ int vb200_attention_layout(vb200_handle h, int32_t batch, int32_t n_tokens, int3
     });
 }
 
+int vb200_attention_layout_packed(vb200_handle h, int32_t batch, const int32_t* n_tokens, const int32_t* n_regions, int32_t max_entries,
+                                  int32_t* n_entries, int32_t* dims, int64_t* offsets, int64_t* total_floats) {
+    if (h == nullptr || n_entries == nullptr) return VB200_ERR_INVALID;
+    return guard(h, [&] {
+        // from the lengths and the layer schedule alone (no plan is built), validated as the packed forwards validate them
+        const char* api = "vb200_attention_layout_packed";
+        if (batch < 1) fail(VB200_ERR_INVALID, "%s: batch must be positive", api);
+        if (!n_tokens || !n_regions) fail(VB200_ERR_INVALID, "%s: NULL length array", api);
+        std::vector<int> offs(2 * (static_cast<size_t>(batch) + 1), 0);
+        pack_lengths(api, "sample", true, h->cfg, n_tokens, batch, 0, offs.data());
+        pack_lengths(api, "sample", false, h->cfg, n_regions, batch, 0, offs.data() + batch + 1);
+        const PackedAttnLayout l = packed_attn_layout(h->cfg, h->schedule, batch, offs.data(), offs.data() + batch + 1);
+        const int n = static_cast<int>(l.heads.size());
+        for (int e = 0; e < n && e < max_entries; ++e) {
+            if (dims) { dims[2 * e] = l.heads[e]; dims[2 * e + 1] = l.kind[e]; }
+            if (offsets) offsets[e] = l.offset[e];
+        }
+        *n_entries = n;
+        if (total_floats) *total_floats = l.total;
+    });
+}
+
 int vb200_forward_host(vb200_handle h, const vb200_inputs* in, const vb200_outputs* out, uint32_t select, void* cuda_stream) {
     return vb200_forward_host_slot(h, in, out, select, 0, 1, cuda_stream);
 }
@@ -1913,6 +2023,7 @@ int vb200_forward_host_slot(vb200_handle h, const vb200_inputs* in, const vb200_
     if (h == nullptr) return VB200_ERR_INVALID;
     return guard(h, [&] {
         if (in == nullptr || out == nullptr) fail(VB200_ERR_INVALID, "inputs/outputs struct is NULL");
+        reject_packed_attention(select, "vb200_forward_host");
         CUDA_CHECK(cudaSetDevice(h->opt.device));
         Plan* pl = h->get_plan(in->batch, in->n_tokens, in->n_regions, select & VB200_OUT_ALL, slot, vb200_engine::FULL,
                                (select & VB200_OUT_ATTENTION) != 0);

@@ -118,11 +118,23 @@ struct PackedStateCopy {
     int n32, n16;
 };
 cudaError_t launch_gather_packed_state(const PackedStateCopy& text, const PackedStateCopy& image, int B, cudaStream_t st);
+// Packed probabilities of the fp32 attention kernel (VB200_OUT_ATTENTION_PACKED).  Sample b's query rows are [offs_q[b],
+// offs_q[b + 1]) of Q, its key rows [offs_k[b], offs_k[b + 1]) of K and of the key mask; its [heads, Lq_b, Lk_b] block goes to
+// float dst[0] + entry[0] + heads * prefix[b], where dst[0] is the destination pointer (0: no write), entry[0] the entry's float
+// offset and prefix[b] = sum over b' < b of Lq_b' * Lk_b'.  All of it lives in the plan's d_meta, filled per call.
+struct PackedProbs {
+    const int* offs_q;
+    const int* offs_k;
+    const int64_t* dst;
+    const int64_t* entry;
+    const int64_t* prefix;
+};
 // fp32 CUDA-core attention (attention_f32.cu): in_kind 0 fp32 / 1 fp16 / 2 bf16 Q, K, V; ctx_mode 0 none / 1 fp16 / 2 bf16 /
-// 3 fp16 hi | lo | hi; probs: optional [B, heads, Lq, Lk] fp32 attention probabilities.
+// 3 fp16 hi | lo | hi; probs: optional [B, heads, Lq, Lk] fp32 attention probabilities.  packed (optional): a packed batch --
+// Lq / Lk are then the per-sample capacities, the probabilities go where *packed says (probs must be null, ctx_mode 0, in_kind 1 or 2).
 cudaError_t launch_attention_f32(const void* q, int ld_q, const void* k, const void* v, int ld_kv, int in_kind,
                                  const float* key_mask_add, int B, int Lq, int Lk, int heads, int D, __nv_bfloat16* ctx, int ld_ctx,
-                                 int ctx_mode, float* probs, int pdl, cudaStream_t st);
+                                 int ctx_mode, float* probs, int pdl, cudaStream_t st, const PackedProbs* packed = nullptr);
 // K8 (narrow heads): out[m, j] = dot(x[m, :K], W[j, :K]) + b[j] + (add ? add[m] : 0), j < n_out <= 4.
 cudaError_t launch_rowdot(const float* x, int ld_x, const float* W, const float* b, const float* add, float* out,
                           int ld_out, int M, int K, int n_out, int pdl, cudaStream_t st, const int* m_rows = nullptr);

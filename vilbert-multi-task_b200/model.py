@@ -55,6 +55,27 @@ def packed_offsets(lengths, extra: int = 0):
     return offs
 
 
+def split_packed_attention(flat, layout, t_rows, v_rows):
+    """The packed attention buffer (VB200_OUT_ATTENTION_PACKED) as the reference's attn_data_list: ``layout`` is
+    ``[(heads, kind, float_offset)]`` of ``attention_layout_packed``, ``t_rows`` / ``v_rows`` the samples' T_b / V_b.  A text or image
+    layer (kinds 0 / 1) gives a list of B views ``[heads, L_b, L_b]``; a connection layer (kinds 2 and 3, adjacent) a tuple of two
+    such lists, ``[heads, T_b, V_b]`` and ``[heads, V_b, T_b]``.  Inside an entry sample b's block follows sample b - 1's."""
+    dims = {0: (t_rows, t_rows), 1: (v_rows, v_rows), 2: (t_rows, v_rows), 3: (v_rows, t_rows)}
+    attn, pending = [], None
+    for heads, kind, off in layout:
+        shapes = [(heads, lq, lk) for lq, lk in zip(*dims[kind])]
+        sizes = [h * lq * lk for h, lq, lk in shapes]
+        parts = torch.split(flat[int(off):int(off) + sum(sizes)], sizes)
+        per = [p.view(s) for p, s in zip(parts, shapes)]
+        if kind == 2:
+            pending = per
+        elif kind == 3:
+            attn.append((pending, per))
+        else:
+            attn.append(per)
+    return attn
+
+
 class VILBertForVLTasks(object):
     """Drop-in for ``vilbert.vilbert.VILBertForVLTasks`` on the inference path the worker uses."""
 
@@ -307,6 +328,38 @@ class VILBertForVLTasks(object):
         L.check(lib.vb200_attention_layout(self._handle, B, Tin, V, n.value, C.byref(n), dims, offs, C.byref(total)), self._handle)
         return [(dims[4 * i], dims[4 * i + 1], dims[4 * i + 2], dims[4 * i + 3], offs[i]) for i in range(n.value)], total.value
 
+    def attention_layout_packed(self, n_tokens, n_regions):
+        """[(heads, kind, float_offset)] of the packed attention buffer of a batch with these Tin_b / V_b (for
+        ``forward_regions_packed``, V_b = n_boxes_b + 1) + its size in floats (vb200_attention_layout_packed)."""
+        lib = L.load()
+        nt, nr = _host_ints(n_tokens), _host_ints(n_regions)
+        if len(nt) != len(nr):
+            raise ValueError("attention_layout_packed: n_tokens and n_regions must have the same length")
+        B = len(nt)
+        nt_c, nr_c = (C.c_int32 * max(B, 1))(*nt), (C.c_int32 * max(B, 1))(*nr)
+        args = (self._handle, B, C.cast(nt_c, C.c_void_p), C.cast(nr_c, C.c_void_p))
+        n, total = C.c_int32(), C.c_int64()
+        L.check(lib.vb200_attention_layout_packed(*args, 0, C.byref(n), None, None, C.byref(total)), self._handle)
+        dims = (C.c_int32 * (2 * n.value))()
+        offs = (C.c_int64 * n.value)()
+        L.check(lib.vb200_attention_layout_packed(*args, n.value, C.byref(n), dims, offs, C.byref(total)), self._handle)
+        return [(dims[2 * i], dims[2 * i + 1], offs[i]) for i in range(n.value)], total.value
+
+    def _packed_attention(self, nt, nv, select, o, device):
+        """Flat buffer of the packed attention maps for Tin_b = nt, V_b = nv, bound to ``o.attention_probs``: (select, flat, split)."""
+        layout, total = self.attention_layout_packed(nt, nv)
+        flat = torch.empty(total, dtype=torch.float32, device=device)
+        o.attention_probs = flat.data_ptr()
+        task = 1 if self._dims["task_specific_tokens"] else 0
+        return select | L.OUT_ATTENTION_PACKED, lambda: split_packed_attention(flat, layout, [t + task for t in nt], nv)
+
+    @staticmethod
+    def _with_attention(result, attn, debug_taps):
+        """``_result``'s tuple with element 9 replaced by ``attn``."""
+        if debug_taps:
+            return result[0][:9] + (attn,), result[1]
+        return result[:9] + (attn,)
+
     def _alloc_outputs(self, B, Tin, V, select, debug_taps, want_attn, device):
         T = Tin + (1 if self._dims["task_specific_tokens"] else 0)
         outs = {k: torch.empty(shape, dtype=torch.float32, device=device)
@@ -386,14 +439,16 @@ class VILBertForVLTasks(object):
     @torch.no_grad()
     def forward_packed(self, question, features, spatials, segment_ids, task_tokens, n_tokens, n_regions,
                        select: int = L.OUT_TASK_HEADS, slot: int = 0, debug_taps: bool = False, max_tokens: int = 0,
-                       max_regions: int = 0):
+                       max_regions: int = 0, output_all_attention_masks: bool = False):
         """One forward of B samples with their own text lengths and region counts, stored back to back without padding:
         ``question`` / ``segment_ids`` ``[sum Tin_i]``, ``features`` ``[sum V_i, F]``, ``spatials`` ``[sum V_i, 5]``,
         ``task_tokens`` ``[B, 1]``; ``n_tokens`` / ``n_regions`` (lists or CPU int tensors) give Tin_i and V_i.  Every row is real
         (no masks).  Returns the 10-tuple: per-sample outputs as in ``forward``, per-row outputs packed (``vision_logit``
-        ``[sum V_i, 1]``, ``linguisic_logit`` ``[sum T_i, 1]`` with T_i = Tin_i + 1, ...), element 9 ``[]``.  ``max_tokens`` /
-        ``max_regions`` (0: this call's maxima) are the plan's capacities: calls with the same batch size and capacities share one
-        plan and CUDA graph whatever their lengths."""
+        ``[sum V_i, 1]``, ``linguisic_logit`` ``[sum T_i, 1]`` with T_i = Tin_i + 1, ...).  Element 9 is ``[]``, or with
+        ``output_all_attention_masks`` AND ``self.return_attention`` the 24 layers' attention probabilities at each sample's own
+        lengths (``split_packed_attention``: per layer a list of B ``[heads, L_i, L_i]`` tensors, a connection layer a tuple of two
+        such lists), views of one flat buffer.  ``max_tokens`` / ``max_regions`` (0: this call's maxima) are the plan's capacities:
+        calls with the same batch size and capacities share one plan and CUDA graph whatever their lengths."""
         if self._handle is None:
             raise L.VilbertB200Error("call model.cuda(i) first (worker.py:536); there is no CPU path")
         lib = L.load()
@@ -417,18 +472,22 @@ class VILBertForVLTasks(object):
             raise ValueError("forward_packed: question / segment_ids need sum(n_tokens) rows, features / spatials sum(n_regions)")
         rows_t = sum_tin + (B if self._dims["task_specific_tokens"] else 0)
         outs, o = self._alloc_packed_outputs(B, rows_t, sum_v, select, debug_taps, device)
+        want_attn = bool(output_all_attention_masks and self.return_attention)
+        if want_attn:
+            select, maps = self._packed_attention(nt, nr, select, o, device)
         nt_c, nr_c = (C.c_int32 * B)(*nt), (C.c_int32 * B)(*nr)
         inp = L.PackedInputs(B, int(max_tokens), int(max_regions), C.cast(nt_c, C.c_void_p), C.cast(nr_c, C.c_void_p), q.data_ptr(),
                              seg.data_ptr(), f.data_ptr(), s.data_ptr(), tk.data_ptr())
         with torch.cuda.device(device):
             stream = torch.cuda.current_stream(device).cuda_stream
             L.check(lib.vb200_forward_packed(self._handle, C.byref(inp), C.byref(o), select, slot, C.c_void_p(stream)), self._handle)
-        return self._result(outs, B, 0, 0, debug_taps)
+        result = self._result(outs, B, 0, 0, debug_taps)
+        return self._with_attention(result, maps(), debug_taps) if want_attn else result
 
     @torch.no_grad()
     def forward_regions_packed(self, question, segment_ids, task_tokens, box_features, boxes, image_wh, n_tokens, n_boxes,
                                select: int = L.OUT_TASK_HEADS, slot: int = 0, max_tokens: int = 0, max_boxes: int = 0,
-                               debug_taps: bool = False, return_spatials: bool = True):
+                               debug_taps: bool = False, return_spatials: bool = True, output_all_attention_masks: bool = False):
         """``forward_regions`` with every image at its own box count and every text at its own length, stored back to back without
         padding: ``question`` / ``segment_ids`` ``[sum Tin_i]`` (text already repeated per image), ``task_tokens`` ``[B, 1]``,
         ``box_features`` ``[sum n_boxes_i, F]`` and pixel ``boxes`` ``[sum n_boxes_i, 4]`` as the detector returned them,
@@ -437,7 +496,9 @@ class VILBertForVLTasks(object):
         returns it (per-image outputs ``[B, ...]``, per-row outputs packed over sum V_i / sum T_i rows), ``spatials`` the packed
         ``[sum V_i, 5]`` locations the reference would have built (None with ``return_spatials=False``).  Each image's rows are
         bit-identical to ``forward_regions`` of that image alone.  ``max_tokens`` / ``max_boxes`` (0: this call's maxima) are the
-        plan's capacities; the plan is the one ``forward_packed`` uses at ``max_regions = max_boxes + 1``."""
+        plan's capacities; the plan is the one ``forward_packed`` uses at ``max_regions = max_boxes + 1``.  Element 9 follows
+        ``forward_packed``: the attention maps at each image's own T_i / V_i with ``output_all_attention_masks`` and
+        ``self.return_attention``, else ``[]``."""
         if self._handle is None:
             raise L.VilbertB200Error("call model.cuda(i) first (worker.py:536); there is no CPU path")
         lib = L.load()
@@ -463,6 +524,9 @@ class VILBertForVLTasks(object):
         rows_v = sum_n + B
         sp = torch.empty(rows_v, 5, dtype=torch.float32, device=device) if return_spatials else None
         outs, o = self._alloc_packed_outputs(B, rows_t, rows_v, select, debug_taps, device)
+        want_attn = bool(output_all_attention_masks and self.return_attention)
+        if want_attn:
+            select, maps = self._packed_attention(nt, [n + 1 for n in nb], select, o, device)
         nt_c, nb_c = (C.c_int32 * B)(*nt), (C.c_int32 * B)(*nb)
         inp = L.PackedRegionInputs(B, int(max_tokens), int(max_boxes), C.cast(nt_c, C.c_void_p), C.cast(nb_c, C.c_void_p),
                                    q.data_ptr(), seg.data_ptr(), tk.data_ptr(), bf.data_ptr(), bx.data_ptr(), wh.data_ptr(),
@@ -471,7 +535,8 @@ class VILBertForVLTasks(object):
             stream = torch.cuda.current_stream(device).cuda_stream
             L.check(lib.vb200_forward_regions_packed(self._handle, C.byref(inp), C.byref(o), select, slot, C.c_void_p(stream)),
                     self._handle)
-        return self._result(outs, B, 0, 0, debug_taps), sp
+        result = self._result(outs, B, 0, 0, debug_taps)
+        return (self._with_attention(result, maps(), debug_taps) if want_attn else result), sp
 
     def _alloc_packed_outputs(self, B, rows_t, rows_v, select, debug_taps, device):
         """Outputs of a packed call: per-sample outputs [B, ...], per-row outputs and taps [rows_t or rows_v, ...]."""
