@@ -404,6 +404,50 @@ int vb200_co_attention(const void* qkv_img_bf16, int64_t ld_img, const void* qkv
                        int32_t hidden, const float* img_mask_add, const float* txt_mask_add, void* ctx_txt_bf16,
                        int64_t ld_ctx_txt, void* ctx_img_bf16, int64_t ld_ctx_img, int32_t B, int32_t T, int32_t V,
                        int32_t heads, int32_t head_dim, int32_t act_fp16, void* cuda_stream);
+/* Packed self-attention: sample b is rows [offs[b], offs[b+1]) of qkv / mask_add / ctx (offs: device int32 [B + 1]); L_cap >= every
+ * sample's length.  Each sample's rows are bit-identical to vb200_self_attention of that sample alone. */
+int vb200_self_attention_packed(const void* qkv16, int64_t ld_qkv, int32_t hidden, const float* mask_add, void* ctx16, int64_t ld_ctx,
+                                int32_t B, int32_t L_cap, int32_t heads, int32_t head_dim, int32_t act_fp16, const int32_t* offs,
+                                void* cuda_stream);
+/* Packed co-attention: per stream as vb200_self_attention_packed (offs_t text rows, offs_v image rows; T_cap / V_cap capacities). */
+int vb200_co_attention_packed(const void* qkv_img16, int64_t ld_img, const void* qkv_txt16, int64_t ld_txt, int32_t hidden,
+                              const float* img_mask_add, const float* txt_mask_add, void* ctx_txt16, int64_t ld_ctx_txt, void* ctx_img16,
+                              int64_t ld_ctx_img, int32_t B, int32_t T_cap, int32_t V_cap, int32_t heads, int32_t head_dim,
+                              int32_t act_fp16, const int32_t* offs_t, const int32_t* offs_v, void* cuda_stream);
+/* Pooled-product GEMM: y = act(x . w^T + bias) * mul (mul fp32 [M, ld_mul]) on the cooperative persistent kernel, as the engine's
+ * pooler builds it; act 0-2, 16-bit and / or fp32 outputs. */
+int vb200_linear_product(const void* x16, int64_t ld_x, const void* w16, int64_t ld_w, const float* bias, int32_t act, const float* mul,
+                         int64_t ld_mul, void* y16, int64_t ld_y16, float* y_f32, int64_t ld_y_f32, int64_t M, int64_t N, int64_t K,
+                         int32_t block_n, int32_t act_fp16, void* cuda_stream);
+/* Text embeddings: LayerNorm(word[id] + position + token_type[seg]), the task row at index 1 when task_tokens != 0, the additive text
+ * mask; ids / segments / task ids are clamped into their tables and positions to max_pos - 1.  offs NULL: dense [B, Tin] inputs;
+ * else packed (device int32 [B + 1] output row offsets, `rows` = offs[B], every row real).  split16: fp16 hi | lo | hi output. */
+int vb200_text_embed(const int64_t* ids, const int64_t* seg, const int64_t* input_mask, const int64_t* task, const float* word,
+                     const float* pos, const float* type, const float* task_tab, const float* gamma, const float* beta, float eps,
+                     float* out_f32, void* out16, float* mask_add, int32_t B, int32_t Tin, int32_t H, int32_t vocab, int32_t max_pos,
+                     int32_t n_type, int32_t n_task, int32_t task_tokens, int32_t act_fp16, int32_t split16, const int32_t* offs,
+                     int32_t rows, void* cuda_stream);
+/* Image operand: rows of [feats (F) | loc (5) | 0 ...] (Kp wide) in 16 bits, additive mask from image_mask (NULL: every row real). */
+int vb200_image_pack(const float* feats, const float* loc, const uint8_t* image_mask, void* a_out, float* mask_add, int32_t rows,
+                     int32_t F, int32_t Kp, int32_t act_fp16, int32_t split16, void* cuda_stream);
+/* Detector output -> image operand rows [mean row | box rows], masks and optional spatials (vb200_forward_regions' input builder);
+ * offs NULL: dense [B, n] boxes with optional num_boxes, else packed (device int32 [B + 1] image row offsets). */
+int vb200_region_pack(const float* box_feats, const float* boxes, const float* image_wh, const int32_t* num_boxes, void* a_out,
+                      float* mask_add, float* spatials_out, int32_t B, int32_t n, int32_t F, int32_t Kp, int32_t act_fp16, int32_t split16,
+                      const int32_t* offs, void* cuda_stream);
+/* Narrow heads: out[m, j] = x[m] . w[j] + bias[j] + add[m] for j < n_out <= 4 (bias, add optional); rows >= *m_rows skipped if given. */
+int vb200_rowdot(const float* x, int64_t ld_x, const float* w, const float* bias, const float* add, float* out, int64_t ld_out,
+                 int64_t M, int64_t K, int32_t n_out, const int32_t* m_rows, void* cuda_stream);
+/* Row-block gather: sample b of dst = block clamp(idx[b], 0, n_src - 1) of src (fp32 [L, H], 16-bit [L, H16], mask [L]; the fp32 and
+ * mask copies are skipped when NULL). */
+int vb200_gather_state(const int32_t* idx, int32_t n_src, const float* src_f32, const void* src16, const float* src_mask, float* dst_f32,
+                       void* dst16, float* dst_mask, int32_t B, int32_t L, int32_t H, int32_t H16, void* cuda_stream);
+/* Packed row-range gather, text (t_) and image (i_) streams in one launch: pair b's rows [dst_offs[b], dst_offs[b+1]) come from rows
+ * starting at src_offs[b]; n32 / n16 = 16-byte vectors per row of the fp32 / 16-bit buffers; every pointer 16-byte aligned. */
+int vb200_gather_packed_state(int32_t B, const int32_t* t_dst_offs, const int32_t* t_src_offs, const float* t_src_f32, const void* t_src16,
+                              float* t_dst_f32, void* t_dst16, int32_t t_n32, int32_t t_n16, const int32_t* i_dst_offs,
+                              const int32_t* i_src_offs, const float* i_src_f32, const void* i_src16, float* i_dst_f32, void* i_dst16,
+                              int32_t i_n32, int32_t i_n16, void* cuda_stream);
 
 #ifdef __cplusplus
 }

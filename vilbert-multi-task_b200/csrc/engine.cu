@@ -2307,4 +2307,105 @@ int vb200_co_attention(const void* qkv_img_bf16, int64_t ld_img, const void* qkv
     });
 }
 
+int vb200_self_attention_packed(const void* qkv16, int64_t ld_qkv, int32_t hidden, const float* mask_add, void* ctx16, int64_t ld_ctx,
+                                int32_t B, int32_t L_cap, int32_t heads, int32_t head_dim, int32_t act_fp16, const int32_t* offs,
+                                void* cuda_stream) {
+    return op_guard([&] {
+        if (offs == nullptr) fail(VB200_ERR_INVALID, "vb200_self_attention_packed: offs is NULL");
+        CUDA_CHECK(vb::launch_self_attention(static_cast<const bf16*>(qkv16), (int)ld_qkv, hidden, mask_add, static_cast<bf16*>(ctx16),
+                                             (int)ld_ctx, B, L_cap, heads, head_dim, 0, act_fp16 ? 1 : 0,
+                                             static_cast<cudaStream_t>(cuda_stream), offs));
+    });
+}
+
+int vb200_co_attention_packed(const void* qkv_img16, int64_t ld_img, const void* qkv_txt16, int64_t ld_txt, int32_t hidden,
+                              const float* img_mask_add, const float* txt_mask_add, void* ctx_txt16, int64_t ld_ctx_txt, void* ctx_img16,
+                              int64_t ld_ctx_img, int32_t B, int32_t T_cap, int32_t V_cap, int32_t heads, int32_t head_dim,
+                              int32_t act_fp16, const int32_t* offs_t, const int32_t* offs_v, void* cuda_stream) {
+    return op_guard([&] {
+        if (offs_t == nullptr || offs_v == nullptr) fail(VB200_ERR_INVALID, "vb200_co_attention_packed: offs_t / offs_v is NULL");
+        CUDA_CHECK(vb::launch_co_attention(static_cast<const bf16*>(qkv_img16), (int)ld_img, static_cast<const bf16*>(qkv_txt16),
+                                           (int)ld_txt, hidden, img_mask_add, txt_mask_add, static_cast<bf16*>(ctx_txt16),
+                                           (int)ld_ctx_txt, static_cast<bf16*>(ctx_img16), (int)ld_ctx_img, B, T_cap, V_cap, heads,
+                                           head_dim, 0, act_fp16 ? 1 : 0, static_cast<cudaStream_t>(cuda_stream), offs_t, offs_v));
+    });
+}
+
+int vb200_linear_product(const void* x16, int64_t ld_x, const void* w16, int64_t ld_w, const float* bias, int32_t act, const float* mul,
+                         int64_t ld_mul, void* y16, int64_t ld_y16, float* y_f32, int64_t ld_y_f32, int64_t M, int64_t N, int64_t K,
+                         int32_t block_n, int32_t act_fp16, void* cuda_stream) {
+    return op_guard([&] {
+        if (mul == nullptr) fail(VB200_ERR_INVALID, "vb200_linear_product: mul is NULL");
+        // as add_linear builds the pooled product: the cooperative kernel (ping-pong takes no product), its tile width, its TMA store
+        const int bn = block_n > 0 ? block_n : vb::gemm_p_pick_block_n(static_cast<int>(N), false);
+        if (bn != 64 && bn != 128 && bn != 192) fail(VB200_ERR_INVALID, "vb200_linear_product: block_n %d (plain tiles are 64, 128 or 192 wide)", bn);
+        CUtensorMap ta = make_tmap(x16, M, K, ld_x, 128, act_fp16 != 0);
+        CUtensorMap tb = make_tmap(w16, N, K, ld_w, bn, act_fp16 != 0);
+        GemmEpilogue e{};
+        e.M = (int)M; e.N = (int)N; e.K = (int)K; e.bias = bias; e.act = act; e.mul = mul; e.ld_mul = (int)ld_mul;
+        e.a_f16 = act_fp16 ? 1 : 0; e.out_f16 = e.a_f16;
+        e.out_bf16 = static_cast<bf16*>(y16); e.ld_bf16 = (int)ld_y16; e.out_f32 = y_f32; e.ld_f32 = (int)ld_y_f32;
+        CUtensorMap tc;
+        setup_tma_store(&tc, e);
+        e.tmap_c_host = e.tma_store ? &tc : nullptr;
+        CUDA_CHECK(vb::launch_gemm_persistent(ta, tb, e, bn, false, static_cast<cudaStream_t>(cuda_stream)));
+    });
+}
+
+int vb200_text_embed(const int64_t* ids, const int64_t* seg, const int64_t* input_mask, const int64_t* task, const float* word,
+                     const float* pos, const float* type, const float* task_tab, const float* gamma, const float* beta, float eps,
+                     float* out_f32, void* out16, float* mask_add, int32_t B, int32_t Tin, int32_t H, int32_t vocab, int32_t max_pos,
+                     int32_t n_type, int32_t n_task, int32_t task_tokens, int32_t act_fp16, int32_t split16, const int32_t* offs,
+                     int32_t rows, void* cuda_stream) {
+    return op_guard([&] {
+        CUDA_CHECK(vb::launch_text_embed(ids, seg, input_mask, task, word, pos, type, task_tab, gamma, beta, eps, out_f32,
+                                         static_cast<bf16*>(out16), mask_add, B, Tin, H, vocab, max_pos, n_type, n_task, task_tokens,
+                                         act_fp16 ? 1 : 0, split16 ? 1 : 0, static_cast<cudaStream_t>(cuda_stream), offs, rows));
+    });
+}
+
+int vb200_image_pack(const float* feats, const float* loc, const uint8_t* image_mask, void* a_out, float* mask_add, int32_t rows,
+                     int32_t F, int32_t Kp, int32_t act_fp16, int32_t split16, void* cuda_stream) {
+    return op_guard([&] {
+        CUDA_CHECK(vb::launch_image_pack(feats, loc, image_mask, static_cast<bf16*>(a_out), mask_add, rows, F, Kp, act_fp16 ? 1 : 0,
+                                         split16 ? 1 : 0, static_cast<cudaStream_t>(cuda_stream)));
+    });
+}
+
+int vb200_region_pack(const float* box_feats, const float* boxes, const float* image_wh, const int32_t* num_boxes, void* a_out,
+                      float* mask_add, float* spatials_out, int32_t B, int32_t n, int32_t F, int32_t Kp, int32_t act_fp16, int32_t split16,
+                      const int32_t* offs, void* cuda_stream) {
+    return op_guard([&] {
+        CUDA_CHECK(vb::launch_region_pack(box_feats, boxes, image_wh, num_boxes, static_cast<bf16*>(a_out), mask_add, spatials_out, B, n,
+                                          F, Kp, act_fp16 ? 1 : 0, split16 ? 1 : 0, static_cast<cudaStream_t>(cuda_stream), offs));
+    });
+}
+
+int vb200_rowdot(const float* x, int64_t ld_x, const float* w, const float* bias, const float* add, float* out, int64_t ld_out,
+                 int64_t M, int64_t K, int32_t n_out, const int32_t* m_rows, void* cuda_stream) {
+    return op_guard([&] {
+        CUDA_CHECK(vb::launch_rowdot(x, (int)ld_x, w, bias, add, out, (int)ld_out, (int)M, (int)K, n_out, 0,
+                                     static_cast<cudaStream_t>(cuda_stream), m_rows));
+    });
+}
+
+int vb200_gather_state(const int32_t* idx, int32_t n_src, const float* src_f32, const void* src16, const float* src_mask, float* dst_f32,
+                       void* dst16, float* dst_mask, int32_t B, int32_t L, int32_t H, int32_t H16, void* cuda_stream) {
+    return op_guard([&] {
+        CUDA_CHECK(vb::launch_gather_state(idx, n_src, src_f32, src16, src_mask, dst_f32, dst16, dst_mask, B, L, H, H16,
+                                           static_cast<cudaStream_t>(cuda_stream)));
+    });
+}
+
+int vb200_gather_packed_state(int32_t B, const int32_t* t_dst_offs, const int32_t* t_src_offs, const float* t_src_f32, const void* t_src16,
+                              float* t_dst_f32, void* t_dst16, int32_t t_n32, int32_t t_n16, const int32_t* i_dst_offs,
+                              const int32_t* i_src_offs, const float* i_src_f32, const void* i_src16, float* i_dst_f32, void* i_dst16,
+                              int32_t i_n32, int32_t i_n16, void* cuda_stream) {
+    return op_guard([&] {
+        const vb::PackedStateCopy text{t_dst_offs, t_src_offs, t_src_f32, t_src16, t_dst_f32, t_dst16, t_n32, t_n16};
+        const vb::PackedStateCopy image{i_dst_offs, i_src_offs, i_src_f32, i_src16, i_dst_f32, i_dst16, i_n32, i_n16};
+        CUDA_CHECK(vb::launch_gather_packed_state(text, image, B, static_cast<cudaStream_t>(cuda_stream)));
+    });
+}
+
 }  // extern "C"
