@@ -14,7 +14,9 @@
  * Beyond the protocol: packed variable-length batches (vb200_packed_inputs: samples with their own text lengths and region counts
  * in one forward, plans keyed on capacity buckets, GEMM tiles past the call's row totals skipped), detector output in, dense or
  * packed (vb200_region_inputs, vb200_packed_region_inputs: every image at its own box count), caption-image retrieval with reuse, dense or packed (vb200_packed_pairs: captions and images encoded once
- * at their own lengths, pairs scored without padding), and kernel-level entry points for the tests.
+ * at their own lengths, pairs scored without padding), the answer decode of every message of a batch in one kernel (vb200_decode_answers:
+ * softmax, top N and grounding boxes, so a C host answers a message without re-implementing prediction()'s decode), and kernel-level
+ * entry points for the tests.
  * The Python shim in vilbert-multi-task_b200/ (ctypes) implements the protocol on top of them; see
  * INTEGRATION.md for the stub a maintainer of the reference would add.
  *
@@ -357,6 +359,67 @@ typedef struct {
 } vb200_packed_pairs;
 int vb200_forward_cached_packed(vb200_handle h, const vb200_packed_pairs* in, const vb200_outputs* out, uint32_t select,
                                 int32_t slot, void* cuda_stream);
+
+/* ---- Answer decode: the step of prediction() that turns logits into answers (worker.py:295-386), for every message of a batch in
+ * one kernel (one CTA per message).  Message i's segment is rows [first, first + count) of its family's source, flattened; the kernel
+ * computes the softmax over the segment in fp32 as torch.softmax(x.view(-1), 0) does (max, expf(x - max), sum, division by the sum)
+ * and writes the top_n probabilities and their indices in the segment.  Ties: equal probabilities rank the lower index first.
+ *
+ *   family                    source (vb200_outputs)   rows of the source                          segment width  reference
+ *   VB200_DECODE_VQA          vil_prediction           batch                                       num_labels     worker.py:296
+ *   VB200_DECODE_GQA          vil_prediction_gqa       batch                                       gqa_labels     worker.py:313
+ *   VB200_DECODE_NLVR2        vil_binary_prediction    batch / 2 (batch even), else batch (pairs)  2              worker.py:329
+ *   VB200_DECODE_SNLI_VE      vil_tri_prediction       batch                                       3              worker.py:345
+ *   VB200_DECODE_RETRIEVAL    vil_logit                batch                                       1              worker.py:359
+ *   VB200_DECODE_GROUNDING    vision_logit + spatials  vision_rows                                 1              worker.py:374-385
+ *
+ * The per-image families take one row (count 1) in the reference's decode, retrieval the request's count images (top_n = count), an
+ * NLVR2 pair its pair row (image row lo of the pair -> pair row lo / 2).  Grounding reads vision_logit and spatials as flat [rows, 1]
+ * and [rows, 5], which serves dense outputs (image b is rows b * V ... b * V + V - 1) and packed ones (image b is its packed rows)
+ * alike; the segment is the image's rows, the global box included.  For each of the top_n rows the kernel writes box = x1, y1, x2, y2:
+ * spatials columns 0-3 converted to double, times the double image_w / image_h, truncated toward zero -- the reference's
+ * int(b[1] * image_h) on Python floats (worker.py:381-384).  Labels (worker.py:299-300, 311-315) and the confidence * 100 /
+ * round(..., 2) of callback() (worker.py:571, 599, 617, 637) stay with the caller. */
+#define VB200_DECODE_MAX_TOP 10
+typedef enum {
+    VB200_DECODE_VQA = 1,          /* task ids 1, 2 */
+    VB200_DECODE_GQA = 2,          /* task id 15 */
+    VB200_DECODE_NLVR2 = 3,        /* task id 12 */
+    VB200_DECODE_SNLI_VE = 4,      /* task id 13 */
+    VB200_DECODE_RETRIEVAL = 5,    /* task id 7 */
+    VB200_DECODE_GROUNDING = 6     /* task ids 4, 16, 11 */
+} vb200_decode_family;
+
+typedef struct {
+    int32_t family;                /* vb200_decode_family */
+    int32_t first;                 /* first row of the source */
+    int32_t count;                 /* rows of the segment (>= 1) */
+    int32_t top_n;                 /* 1 .. min(VB200_DECODE_MAX_TOP, count * segment width) */
+    double image_w, image_h;       /* grounding only: the image size in pixels */
+} vb200_decode_msg;
+
+typedef struct vb200_answer {
+    int32_t n;                                  /* top_n */
+    int32_t index[VB200_DECODE_MAX_TOP];        /* position in the flattened segment, best first; -1 past n */
+    float prob[VB200_DECODE_MAX_TOP];           /* softmax probability; 0 past n */
+    int32_t box[VB200_DECODE_MAX_TOP][4];       /* grounding: pixel x1, y1, x2, y2 of row `index`; 0 otherwise */
+} vb200_answer;
+
+/* Decodes n messages of one forward's outputs: `out` holds the device pointers that forward wrote (only the sources of the families
+ * used are read), `batch` its per-sample row count, `vision_rows` the rows of vision_logit and of `spatials` (DEVICE fp32 [vision_rows, 5],
+ * required for grounding).  Every descriptor is checked on the host before anything is enqueued: VB200_ERR_INVALID, with a message
+ * naming the message index, for n < 1, an unknown family, count < 1, a row range outside its source, top_n < 1, above
+ * VB200_DECODE_MAX_TOP or above the segment length, and a NULL source for a family that is used.  The descriptors reach the device
+ * through a pinned staging buffer, asynchronously on cuda_stream: the call blocks only while the previous call's copy out of that
+ * buffer is still in flight (and when a batch larger than any before grows that buffer), so back-to-back calls need no synchronisation
+ * in between.  `answers` is DEVICE memory [n], complete once cuda_stream reaches the point of the call. */
+int vb200_decode_answers(vb200_handle h, const vb200_decode_msg* msgs /* HOST [n] */, int32_t n, const vb200_outputs* out, int32_t batch,
+                         int32_t vision_rows, const float* spatials, vb200_answer* answers /* DEVICE [n] */, void* cuda_stream);
+/* The same with `answers` in HOST memory: the answers are copied back and cuda_stream is synchronised before the call returns.  The
+ * form a C worker uses: forward, then this call, then the label lookup. */
+int vb200_decode_answers_host(vb200_handle h, const vb200_decode_msg* msgs /* HOST [n] */, int32_t n, const vb200_outputs* out,
+                              int32_t batch, int32_t vision_rows, const float* spatials, vb200_answer* answers /* HOST [n] */,
+                              void* cuda_stream);
 
 /* ---- Kernel-level entry points (device pointers), used by the parity tests and the roofline bench.  ---- */
 /* y = epilogue(x[M,K] (16-bit) . w[N,K]^T (16-bit)); act: 0 none, 1 GELU(erf), 2 ReLU; LayerNorm applied when gamma != NULL.

@@ -82,6 +82,26 @@ class Outputs(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in OUTPUT_FIELDS]
 
 
+# vb200_decode_family: which output a decode message reads (include/vilbert_b200.h, vb200_decode_answers)
+DECODE_VQA, DECODE_GQA, DECODE_NLVR2, DECODE_SNLI_VE, DECODE_RETRIEVAL, DECODE_GROUNDING = 1, 2, 3, 4, 5, 6
+DECODE_MAX_TOP = 10
+# the worker's task ids -> decode family (worker.py:295-374)
+TASK_DECODE_FAMILY = {"1": DECODE_VQA, "2": DECODE_VQA, "15": DECODE_GQA, "12": DECODE_NLVR2, "13": DECODE_SNLI_VE,
+                      "7": DECODE_RETRIEVAL, "4": DECODE_GROUNDING, "16": DECODE_GROUNDING, "11": DECODE_GROUNDING}
+
+
+class DecodeMsg(C.Structure):
+    """vb200_decode_msg: one message's segment (rows [first, first + count) of its family's source) and top_n."""
+    _fields_ = [("family", C.c_int32), ("first", C.c_int32), ("count", C.c_int32), ("top_n", C.c_int32),
+                ("image_w", C.c_double), ("image_h", C.c_double)]
+
+
+class Answer(C.Structure):
+    """vb200_answer: top_n indices (best first) and probabilities, and grounding boxes x1, y1, x2, y2 in pixels."""
+    _fields_ = [("n", C.c_int32), ("index", C.c_int32 * DECODE_MAX_TOP), ("prob", C.c_float * DECODE_MAX_TOP),
+                ("box", (C.c_int32 * 4) * DECODE_MAX_TOP)]
+
+
 class Options(C.Structure):
     _fields_ = [("device", C.c_int32), ("num_labels", C.c_int32), ("use_cuda_graph", C.c_int32),
                 ("use_pdl", C.c_int32), ("strict", C.c_int32), ("act_fp16", C.c_int32),
@@ -95,7 +115,7 @@ EXPORTS = ["vb200_abi_version", "vb200_create", "vb200_destroy", "vb200_last_err
            "vb200_encode_text_packed", "vb200_encode_image_packed", "vb200_forward_cached_packed", "vb200_linear", "vb200_linear_rows", "vb200_linear_split", "vb200_layernorm", "vb200_layernorm_split", "vb200_attention_f32",
            "vb200_self_attention", "vb200_co_attention", "vb200_self_attention_packed", "vb200_co_attention_packed",
            "vb200_linear_product", "vb200_text_embed", "vb200_image_pack", "vb200_region_pack", "vb200_rowdot", "vb200_gather_state",
-           "vb200_gather_packed_state"]
+           "vb200_gather_packed_state", "vb200_decode_answers", "vb200_decode_answers_host"]
 
 _lib = None
 
@@ -163,6 +183,8 @@ def load():
     lib.vb200_rowdot.argtypes = [vp, i64, vp, vp, vp, vp, i64, i64, i64, i32, vp, vp]
     lib.vb200_gather_state.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, vp]
     lib.vb200_gather_packed_state.argtypes = [i32, vp, vp, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp, i32, i32, vp]
+    lib.vb200_decode_answers.argtypes = [vp, C.POINTER(DecodeMsg), i32, C.POINTER(Outputs), i32, i32, vp, vp, vp]
+    lib.vb200_decode_answers_host.argtypes = [vp, C.POINTER(DecodeMsg), i32, C.POINTER(Outputs), i32, i32, vp, C.POINTER(Answer), vp]
     for name in EXPORTS:
         if name not in ("vb200_last_error",):
             getattr(lib, name).restype = C.c_int

@@ -1,0 +1,96 @@
+// Answer decode: logits of a forward -> each message's top-N probabilities, indices and (grounding) pixel boxes, one CTA per
+// message.  Replaces prediction()'s per-message decode (worker.py:295-386): torch.softmax over the message's flattened logits,
+// topk, and for grounding spatials[0][idx] scaled back to pixels (worker.py:374-385).
+//
+// Softmax as torch.softmax(x.view(-1), 0) computes it, in fp32: max, expf(x - max) (the accurate expf, not __expf), block sum,
+// then a division by the sum.  Only the summation order differs from torch, so probabilities agree to rounding of the sum.
+// Ranking is by probability, descending; equal probabilities rank the lower index first (torch.topk leaves that order open).
+// Boxes: int((double)spatial * (double)image_size), truncated toward zero, as the reference's int(b[1] * image_h) on Python
+// floats -- an fp32 product rounds some values across an integer boundary.
+#include "kernels.h"
+
+namespace vb {
+
+constexpr int kDecodeThreads = 256;
+constexpr int kDecodeWarps = kDecodeThreads / 32;
+
+__device__ __forceinline__ unsigned long long warp_max_u64(unsigned long long v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const unsigned long long w = __shfl_xor_sync(0xffffffffu, v, o);
+        v = w > v ? w : v;
+    }
+    return v;
+}
+
+// Ranking key of element i with probability p >= 0: the bits of a non-negative float order as the float does, and the low word
+// 0xffffffff - i puts the lower index first among equal probabilities.  Every element has its own key.
+__device__ __forceinline__ unsigned long long rank_key(float p, int i) {
+    return (static_cast<unsigned long long>(__float_as_uint(p)) << 32) | (0xffffffffu - static_cast<unsigned>(i));
+}
+
+__global__ void __launch_bounds__(kDecodeThreads)
+answer_decode_kernel(const DecodeDesc* __restrict__ descs, vb200_answer* __restrict__ answers) {
+    __shared__ float s_f[kDecodeWarps];
+    __shared__ unsigned long long s_k[kDecodeWarps];
+    __shared__ unsigned long long s_pick[VB200_DECODE_MAX_TOP];
+    const DecodeDesc d = descs[blockIdx.x];
+    const float* __restrict__ x = d.src;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+
+    float m = -INFINITY;
+    for (int i = tid; i < d.len; i += kDecodeThreads) m = fmaxf(m, x[i]);
+    m = warp_max(m);
+    if (lane == 0) s_f[warp] = m;
+    __syncthreads();
+    m = warp_max(lane < kDecodeWarps ? s_f[lane] : -INFINITY);
+    __syncthreads();
+
+    float s = 0.f;
+    for (int i = tid; i < d.len; i += kDecodeThreads) s += expf(x[i] - m);
+    s = warp_sum(s);
+    if (lane == 0) s_f[warp] = s;
+    __syncthreads();
+    s = warp_sum(lane < kDecodeWarps ? s_f[lane] : 0.f);
+
+    // pick k is the largest key below pick k - 1's: N passes over the segment, each recomputing the same probabilities
+    unsigned long long prev = ~0ull;
+    for (int k = 0; k < d.top_n; ++k) {
+        unsigned long long best = 0;
+        for (int i = tid; i < d.len; i += kDecodeThreads) {
+            const unsigned long long key = rank_key(expf(x[i] - m) / s, i);
+            if (key < prev && key > best) best = key;
+        }
+        best = warp_max_u64(best);
+        if (lane == 0) s_k[warp] = best;
+        __syncthreads();
+        best = warp_max_u64(lane < kDecodeWarps ? s_k[lane] : 0ull);
+        if (tid == 0) s_pick[k] = best;
+        __syncthreads();
+        prev = best;
+    }
+
+    vb200_answer* a = answers + blockIdx.x;
+    if (tid == 0) a->n = d.top_n;
+    if (tid < VB200_DECODE_MAX_TOP) {
+        const bool on = tid < d.top_n;
+        a->index[tid] = on ? static_cast<int32_t>(0xffffffffu - static_cast<unsigned>(s_pick[tid] & 0xffffffffu)) : -1;
+        a->prob[tid] = on ? __uint_as_float(static_cast<unsigned>(s_pick[tid] >> 32)) : 0.f;
+    }
+    if (tid < 4 * VB200_DECODE_MAX_TOP) {
+        const int k = tid >> 2, c = tid & 3;       // box k, coordinate c of x1, y1, x2, y2 (spatials columns 0-3)
+        int v = 0;
+        if (d.spatials != nullptr && k < d.top_n) {
+            const int row = static_cast<int>(0xffffffffu - static_cast<unsigned>(s_pick[k] & 0xffffffffu));
+            const double size = (c & 1) ? d.image_h : d.image_w;
+            v = __double2int_rz(static_cast<double>(d.spatials[static_cast<size_t>(row) * 5 + c]) * size);
+        }
+        a->box[k][c] = v;
+    }
+}
+
+cudaError_t launch_answer_decode(const DecodeDesc* descs, int n, vb200_answer* answers, cudaStream_t st) {
+    return launch_ex(answer_decode_kernel, dim3(n), dim3(kDecodeThreads), 0, 0, st, descs, answers);
+}
+
+}  // namespace vb

@@ -500,8 +500,20 @@ struct vb200_engine {
     cudaStream_t side_stream = nullptr;
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
     std::vector<std::string> schedule;
+    // answer decode (vb200_decode_answers): descriptors go to dec_d through the pinned dec_h, dec_copied marks when the last copy out
+    // of dec_h has been made; ans_d holds vb200_decode_answers_host's device answers.  All three grow on demand.
+    vb::DecodeDesc* dec_h = nullptr;
+    vb::DecodeDesc* dec_d = nullptr;
+    size_t dec_cap = 0;
+    cudaEvent_t dec_copied = nullptr;
+    vb200_answer* ans_d = nullptr;
+    size_t ans_cap = 0;
 
     ~vb200_engine() {
+        if (dec_copied) { cudaEventSynchronize(dec_copied); cudaEventDestroy(dec_copied); }
+        if (dec_h) cudaFreeHost(dec_h);
+        if (dec_d) cudaFree(dec_d);
+        if (ans_d) cudaFree(ans_d);
         plans.clear();
         if (side_stream) cudaStreamDestroy(side_stream);
         if (ev_fork) cudaEventDestroy(ev_fork);
@@ -1504,6 +1516,79 @@ struct vb200_engine {
                                            c.v_hidden, c.v_hidden * S, st));
         run_plan(pl, st);
     }
+    // ---- answer decode: every descriptor is resolved and bounds-checked before anything is enqueued
+    std::vector<vb::DecodeDesc> decode_descs(const char* api, const vb200_decode_msg* msgs, int n, const vb200_outputs* out, int batch,
+                                             int vision_rows, const float* spatials) const {
+        if (n < 1) fail(VB200_ERR_INVALID, "%s: n must be positive (n = %d)", api, n);
+        if (msgs == nullptr || out == nullptr) fail(VB200_ERR_INVALID, "%s: msgs / out is NULL", api);
+        if (batch < 0 || vision_rows < 0) fail(VB200_ERR_INVALID, "%s: negative batch %d or vision_rows %d", api, batch, vision_rows);
+        std::vector<vb::DecodeDesc> d(n);
+        for (int i = 0; i < n; ++i) {
+            const vb200_decode_msg& m = msgs[i];
+            const char* field = nullptr;
+            const float* src = nullptr;
+            int64_t rows = batch, width = 1;
+            switch (m.family) {
+                case VB200_DECODE_VQA: field = "vil_prediction"; src = out->vil_prediction; width = num_labels; break;
+                case VB200_DECODE_GQA: field = "vil_prediction_gqa"; src = out->vil_prediction_gqa; width = gqa_labels; break;
+                case VB200_DECODE_NLVR2:
+                    field = "vil_binary_prediction"; src = out->vil_binary_prediction; width = 2; rows = batch % 2 == 0 ? batch / 2 : batch;
+                    break;
+                case VB200_DECODE_SNLI_VE: field = "vil_tri_prediction"; src = out->vil_tri_prediction; width = 3; break;
+                case VB200_DECODE_RETRIEVAL: field = "vil_logit"; src = out->vil_logit; break;
+                case VB200_DECODE_GROUNDING: field = "vision_logit"; src = out->vision_logit; rows = vision_rows; break;
+                default: fail(VB200_ERR_INVALID, "%s: message %d has unknown family %d", api, i, m.family);
+            }
+            if (src == nullptr) fail(VB200_ERR_INVALID, "%s: message %d (family %d) reads vb200_outputs.%s, which is NULL", api, i, m.family, field);
+            const bool grounding = m.family == VB200_DECODE_GROUNDING;
+            if (grounding && spatials == nullptr) fail(VB200_ERR_INVALID, "%s: message %d is a grounding message and spatials is NULL", api, i);
+            if (m.count < 1 || m.first < 0 || static_cast<int64_t>(m.first) + m.count > rows)
+                fail(VB200_ERR_INVALID, "%s: message %d has rows [%d, %lld) outside %s's %lld rows", api, i, m.first,
+                     static_cast<long long>(static_cast<int64_t>(m.first) + m.count), field, static_cast<long long>(rows));
+            const int64_t len = static_cast<int64_t>(m.count) * width;
+            if (len > INT32_MAX) fail(VB200_ERR_INVALID, "%s: message %d has a segment of %lld logits", api, i, static_cast<long long>(len));
+            if (m.top_n < 1 || m.top_n > VB200_DECODE_MAX_TOP || m.top_n > len)
+                fail(VB200_ERR_INVALID, "%s: message %d has top_n %d outside [1, %lld] (segment of %lld logits, at most %d)", api, i, m.top_n,
+                     static_cast<long long>(std::min<int64_t>(len, VB200_DECODE_MAX_TOP)), static_cast<long long>(len), VB200_DECODE_MAX_TOP);
+            d[i].src = src + static_cast<size_t>(m.first) * width;
+            d[i].spatials = grounding ? spatials + static_cast<size_t>(m.first) * 5 : nullptr;
+            d[i].image_w = m.image_w;
+            d[i].image_h = m.image_h;
+            d[i].len = static_cast<int>(len);
+            d[i].top_n = m.top_n;
+        }
+        return d;
+    }
+    // descriptors -> dec_d through the pinned dec_h (in stream order), then the decode kernel writes answers [n]
+    void decode_answers(const std::vector<vb::DecodeDesc>& d, vb200_answer* answers, cudaStream_t st) {
+        const size_t n = d.size();
+        if (dec_copied == nullptr) CUDA_CHECK(cudaEventCreateWithFlags(&dec_copied, cudaEventDisableTiming));
+        CUDA_CHECK(cudaEventSynchronize(dec_copied));                // the previous call's copy has left the staging buffer
+        if (n > dec_cap) {
+            const size_t cap = std::max<size_t>({n, 2 * dec_cap, 256});
+            if (dec_h) CUDA_CHECK(cudaFreeHost(dec_h));
+            dec_h = nullptr;
+            CUDA_CHECK(cudaMallocHost(&dec_h, cap * sizeof(vb::DecodeDesc)));
+            if (dec_d) CUDA_CHECK(cudaFreeAsync(dec_d, st));          // after the kernels already enqueued on st have read it
+            dec_d = nullptr;
+            CUDA_CHECK(cudaMallocAsync(&dec_d, cap * sizeof(vb::DecodeDesc), st));
+            dec_cap = cap;
+        }
+        memcpy(dec_h, d.data(), n * sizeof(vb::DecodeDesc));
+        CUDA_CHECK(cudaMemcpyAsync(dec_d, dec_h, n * sizeof(vb::DecodeDesc), cudaMemcpyHostToDevice, st));
+        CUDA_CHECK(cudaEventRecord(dec_copied, st));
+        CUDA_CHECK(vb::launch_answer_decode(dec_d, static_cast<int>(n), answers, st));
+    }
+    vb200_answer* answer_scratch(size_t n, cudaStream_t st) {
+        if (n > ans_cap) {
+            const size_t cap = std::max<size_t>({n, 2 * ans_cap, 256});
+            if (ans_d) CUDA_CHECK(cudaFreeAsync(ans_d, st));
+            ans_d = nullptr;
+            CUDA_CHECK(cudaMallocAsync(&ans_d, cap * sizeof(vb200_answer), st));
+            ans_cap = cap;
+        }
+        return ans_d;
+    }
     static float* out_ptr(const vb200_outputs& o, int slot) {
         switch (slot) {
             case 0: return o.vil_prediction; case 1: return o.vil_prediction_gqa; case 2: return o.vil_logit;
@@ -1962,6 +2047,34 @@ int vb200_forward_cached_packed(vb200_handle h, const vb200_packed_pairs* in, co
         cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
         h->forward_cached_packed(*pl, *in, meta, st);
         h->copy_outputs(*pl, *out, st, cudaMemcpyDeviceToDevice, meta[2 * (B + 1)], meta[2 * (B + 1) + 1]);
+    });
+}
+
+int vb200_decode_answers(vb200_handle h, const vb200_decode_msg* msgs, int32_t n, const vb200_outputs* out, int32_t batch,
+                         int32_t vision_rows, const float* spatials, vb200_answer* answers, void* cuda_stream) {
+    if (h == nullptr) return VB200_ERR_INVALID;
+    return guard(h, [&] {
+        const char* api = "vb200_decode_answers";
+        const std::vector<vb::DecodeDesc> d = h->decode_descs(api, msgs, n, out, batch, vision_rows, spatials);
+        if (answers == nullptr) fail(VB200_ERR_INVALID, "%s: answers is NULL", api);
+        CUDA_CHECK(cudaSetDevice(h->opt.device));
+        h->decode_answers(d, answers, static_cast<cudaStream_t>(cuda_stream));
+    });
+}
+
+int vb200_decode_answers_host(vb200_handle h, const vb200_decode_msg* msgs, int32_t n, const vb200_outputs* out, int32_t batch,
+                              int32_t vision_rows, const float* spatials, vb200_answer* answers, void* cuda_stream) {
+    if (h == nullptr) return VB200_ERR_INVALID;
+    return guard(h, [&] {
+        const char* api = "vb200_decode_answers_host";
+        const std::vector<vb::DecodeDesc> d = h->decode_descs(api, msgs, n, out, batch, vision_rows, spatials);
+        if (answers == nullptr) fail(VB200_ERR_INVALID, "%s: answers is NULL", api);
+        CUDA_CHECK(cudaSetDevice(h->opt.device));
+        cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+        vb200_answer* dev = h->answer_scratch(d.size(), st);
+        h->decode_answers(d, dev, st);
+        CUDA_CHECK(cudaMemcpyAsync(answers, dev, d.size() * sizeof(vb200_answer), cudaMemcpyDeviceToHost, st));
+        CUDA_CHECK(cudaStreamSynchronize(st));
     });
 }
 

@@ -1,6 +1,7 @@
 // Internal launch interface of the vilbert_b200 sm_90a kernels (not part of the C ABI; see include/vilbert_b200.h).
 #pragma once
 #include "common.cuh"
+#include "../../include/vilbert_b200.h"
 
 namespace vb {
 
@@ -138,6 +139,16 @@ cudaError_t launch_attention_f32(const void* q, int ld_q, const void* k, const v
 // K8 (narrow heads): out[m, j] = dot(x[m, :K], W[j, :K]) + b[j] + (add ? add[m] : 0), j < n_out <= 4.
 cudaError_t launch_rowdot(const float* x, int ld_x, const float* W, const float* b, const float* add, float* out,
                           int ld_out, int M, int K, int n_out, int pdl, cudaStream_t st, const int* m_rows = nullptr);
+// Answer decode (decode.cu, vb200_decode_answers): message b's softmax over the `len` logits at src, its top_n (<= 10)
+// probabilities and indices, and for grounding (spatials != null: the segment's first [len, 5] spatials row) the pixel boxes of
+// the picked rows.  One CTA per message; the descriptors are resolved and bounds-checked on the host.
+struct DecodeDesc {
+    const float* src;
+    const float* spatials;
+    double image_w, image_h;
+    int len, top_n;
+};
+cudaError_t launch_answer_decode(const DecodeDesc* descs, int n, vb200_answer* answers, cudaStream_t st);
 
 // ---- shared host-side launch helpers
 template <typename K>

@@ -554,6 +554,67 @@ class VILBertForVLTasks(object):
             setattr(o, k, t.data_ptr())
         return outs, o
 
+    # ------------------------------------------------------------------ answer decode (worker.py:295-386)
+    def decode_answers(self, out, messages, spatials=None):
+        """prediction()'s decode for many messages in one kernel and one device-to-host copy (vb200_decode_answers_host).
+
+        ``out`` is the 10-tuple a forward returned, dense or packed.  ``messages`` is a list of ``(family or task_id, first, count,
+        top_n, image_wh)``: a str is a worker task id ("1", "15", "12", ...), an int a family (``_lib.DECODE_*``); the message's
+        segment is rows [first, first + count) of its family's output, flattened (an NLVR2 pair row is image row // 2; grounding
+        rows are rows of ``vision_logit`` flattened to [rows, 1]); ``image_wh`` is the (width, height) of a grounding message's
+        image, else ignored.  ``spatials`` (grounding): the locations the forward read or wrote, dense [B, V, 5] or packed [rows, 5].
+        Returns one ``(indices, probs, boxes)`` per message: top_n indices in the segment, best first (equal probabilities: lower
+        index first), the fp32 softmax probabilities as Python floats, and for grounding top_n ``[x1, y1, x2, y2]`` pixel boxes
+        (``int(spatial * size)``, worker.py:381-384), else None."""
+        if self._handle is None:
+            raise L.VilbertB200Error("call model.cuda(i) first (worker.py:536); there is no CPU path")
+        args, families = self._decode_args(out, messages, spatials)
+        n = len(messages)
+        answers = (L.Answer * max(n, 1))()
+        device = torch.device("cuda", self._device)
+        with torch.cuda.device(device):
+            stream = torch.cuda.current_stream(device).cuda_stream
+            L.check(L.load().vb200_decode_answers_host(self._handle, *args, answers, C.c_void_p(stream)), self._handle)
+        res = []
+        for a, fam in zip(answers[:n], families):
+            k = a.n
+            boxes = [list(a.box[j]) for j in range(k)] if fam == L.DECODE_GROUNDING else None
+            res.append((list(a.index[:k]), list(a.prob[:k]), boxes))
+        return res
+
+    def _decode_args(self, out, messages, spatials):
+        """(msgs, n, outputs, batch, vision_rows, spatials) of vb200_decode_answers[_host] for a forward's 10-tuple, and the
+        messages' families."""
+        n = len(messages)
+        msgs = (L.DecodeMsg * max(n, 1))()
+        families = []
+        for i, (fam, first, count, top_n, wh) in enumerate(messages):
+            f = L.TASK_DECODE_FAMILY.get(fam, 0) if isinstance(fam, str) else int(fam)
+            w, h = (float(wh[0]), float(wh[1])) if wh is not None else (0.0, 0.0)
+            msgs[i] = L.DecodeMsg(f, int(first), int(count), int(top_n), w, h)
+            families.append(f)
+        o = L.Outputs()
+        for k, name in ((0, "vil_prediction"), (1, "vil_prediction_gqa"), (2, "vil_logit"), (3, "vil_binary_prediction"),
+                        (4, "vil_tri_prediction"), (6, "vision_logit")):
+            t = out[k]
+            if t is None:
+                continue
+            if t.dtype != torch.float32 or not t.is_cuda or not t.is_contiguous():
+                raise ValueError(f"decode_answers: {name} must be a contiguous fp32 device tensor")
+            setattr(o, name, t.data_ptr())
+        # the per-sample row count: the pair head alone has B / 2 rows for an even B and B rows for an odd one, so 2 R is consistent
+        batch = next((int(out[k].shape[0]) for k in (0, 1, 2, 4) if out[k] is not None),
+                     2 * int(out[3].shape[0]) if out[3] is not None else 0)
+        vision_rows = int(out[6].numel()) if out[6] is not None else 0
+        sp = None
+        if spatials is not None:
+            if spatials.dtype != torch.float32 or not spatials.is_cuda or not spatials.is_contiguous() or spatials.shape[-1] != 5:
+                raise ValueError("decode_answers: spatials must be a contiguous fp32 device tensor [..., 5]")
+            if out[6] is not None and spatials.numel() // 5 != vision_rows:
+                raise ValueError(f"decode_answers: spatials has {spatials.numel() // 5} rows, vision_logit {vision_rows}")
+            sp = spatials.data_ptr()
+        return (msgs, n, C.byref(o), batch, vision_rows, sp), families
+
     # ------------------------------------------------------------------ retrieval reuse (SURVEY.md section 8e)
     @torch.no_grad()
     def encode_text(self, question, segment_ids, input_mask, task_tokens):

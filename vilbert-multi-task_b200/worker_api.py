@@ -136,6 +136,63 @@ def _decode(task_id, out, spatials, infos):
              "confidence": c * 100} for b, c in zip(boxes, conf)]
 
 
+def _check_decode(decode):
+    if decode not in ("host", "device"):
+        raise ValueError(f"decode must be 'host' or 'device', not {decode!r}")
+
+
+def decode_messages(tasks, spans, v_off):
+    """The descriptors of `model.decode_answers` for the requests of one forward, with `_decode`'s N and segments.
+
+    `tasks` maps a request to its `(task_id, infos)`, `spans` a request to the batch rows `(lo, hi)` it took, and `v_off` gives
+    the first `vision_logit` row of every batch row (B + 1 entries: multiples of V for a dense forward, prefix sums of the rows per
+    image for a packed one).  An NLVR2 pair (even lo) reads pair row lo // 2, retrieval its hi - lo rows with N = len(infos), grounding
+    the image's vision rows [v_off[lo], v_off[hi]), the global box included, with the image size of infos[0].
+    Returns `[(request, (task_id, first, count, top_n, image_wh))]` in the order of `spans`."""
+    msgs = []
+    for i, (lo, hi) in spans.items():
+        task_id, infos = tasks[i]
+        wh = None
+        if task_id in GROUNDING_TASKS:
+            first, count, top = int(v_off[lo]), int(v_off[hi]) - int(v_off[lo]), 3
+            wh = (infos[0]["image_width"], infos[0]["image_height"])
+        elif task_id == "12":
+            first, count, top = lo // 2, hi // 2 - lo // 2, 2
+        else:
+            first, count, top = lo, hi - lo, (len(infos) if task_id == "7" else 3)
+        msgs.append((i, (task_id, first, count, top, wh)))
+    return msgs
+
+
+def _answer(task_id, idx, conf, boxes):
+    """`_decode`'s answer for one request from a device decode's indices, probabilities and boxes."""
+    if task_id in ("1", "2"):
+        return {"top3_answer": [_label("vqa", i) for i in idx], "top3_confidence": conf}
+    if task_id == "15":
+        return {"top3_answer": [_label("gqa", i) for i in idx], "top3_confidence": conf}
+    if task_id == "12":
+        names = {0: "False", 1: "True"}
+        return {"top3_answer": [names[i] for i in idx], "top3_confidence": conf}
+    if task_id == "13":
+        names = {0: "contradiction (false)", 1: "neutral", 2: "entailment (true)"}
+        return {"top3_answer": [names[i] for i in idx], "top3_confidence": conf}
+    if task_id == "7":
+        return {"top3_answer": idx, "top3_confidence": conf}
+    return [{"y1": b[1], "y2": b[3], "x1": b[0], "x2": b[2], "confidence": c * 100} for b, c in zip(boxes, conf)]
+
+
+def _decode_device(out, spatials, tasks, spans, v_off):
+    """Every request of one forward decoded by one `model.decode_answers` call -> {request: `_decode`'s answer}."""
+    msgs = decode_messages(tasks, spans, v_off)
+    if not msgs:
+        return {}
+    if spatials is not None:
+        spatials = spatials.to(device=torch.device("cuda", model._device), dtype=torch.float32).contiguous()
+    with model_lock:
+        res = model.decode_answers(out, [m for _, m in msgs], spatials)
+    return {i: _answer(m[0], *r) for (i, m), r in zip(msgs, res)}
+
+
 def prediction(question, features, spatials, segment_ids, input_mask, image_mask, co_attention_mask, task_tokens,
                task_id, infos):
     """Validate, expand the text for pair / retrieval tasks, run the model once, decode.  worker.py:248-386."""
@@ -148,7 +205,7 @@ def prediction(question, features, spatials, segment_ids, input_mask, image_mask
     return _decode(task_id, out, spatials, infos)
 
 
-def prediction_batch(requests, bucket: int = 8, select: Optional[int] = None):
+def prediction_batch(requests, bucket: int = 8, select: Optional[int] = None, *, decode: str = "host"):
     """Micro-batching across requests (SURVEY.md section 8f-4; the reference handles one message at a time, worker.py:664-673).
 
     `requests` is a list of argument tuples of `prediction()`.  Requests whose tensors have the same text length, region count
@@ -159,9 +216,13 @@ def prediction_batch(requests, bucket: int = 8, select: Optional[int] = None):
 
     The engine keeps one plan (workspace + CUDA graph) per (batch, text length, regions, select): so that a long-running worker
     sees a small, fixed set of plans, the batch is padded with filler rows to a multiple of `bucket` (even, so the binary
-    head always has whole pairs) and `select` defaults to the seven task heads whatever tasks happen to be pending."""
+    head always has whole pairs) and `select` defaults to the seven task heads whatever tasks happen to be pending.
+
+    `decode="device"` answers every request of a model call with one decode kernel and one device-to-host copy
+    (`model.decode_answers`) instead of `_decode` per request; the answers have `_decode`'s structure."""
     if bucket < 1:
         raise ValueError("bucket must be >= 1")
+    _check_decode(decode)
     fixed_select = L.OUT_TASK_HEADS if select is None else int(select)
     answers = [None] * len(requests)
     groups = {}
@@ -200,6 +261,14 @@ def prediction_batch(requests, bucket: int = 8, select: Optional[int] = None):
         cat = [torch.cat([r[k] for r in rows], dim=0) for k in range(8)]
         with model_lock:
             out = model(*cat, output_all_attention_masks=True, select=sel)
+        if decode == "device":
+            V = cat[1].shape[1]
+            ground = any(requests[i][8] in GROUNDING_TASKS for i in idxs)
+            dec = _decode_device(out, cat[2] if ground else None, {i: (requests[i][8], requests[i][9]) for i in idxs}, spans,
+                                 [k * V for k in range(n + 1)])
+            for i in idxs:
+                answers[i] = dec[i]
+            continue
         for i in idxs:
             lo, hi = spans[i]
             task_id, infos, spatials = requests[i][8], requests[i][9], requests[i][2]
@@ -217,15 +286,17 @@ def _prefix_len(mask_row):
     return k if k >= 1 and all(x == 1 for x in m[:k]) and all(x == 0 for x in m[k:]) else None
 
 
-def prediction_packed(requests, bucket: int = 8, select: Optional[int] = None):
+def prediction_packed(requests, bucket: int = 8, select: Optional[int] = None, *, decode: str = "host"):
     """`prediction_batch` in ONE model call whatever the requests' shapes: a packed variable-length batch
     (`model.forward_packed`).  Padded text tokens are dropped (the `input_mask` must be a prefix of ones), region rows are kept
     as given (the `image_mask` must be all ones); a request that breaks either rule, or fails validation, gets a `ValueError` /
     its exception as its answer.  NLVR2 pairs go on even rows and the batch is padded to a multiple of `bucket`, both with
     filler rows of one token and one region.  The plan capacities are the widest padded text and the most regions among the
-    requests (37 tokens from the worker's tokenizer), so a long-running worker sees one plan per batch bucket."""
+    requests (37 tokens from the worker's tokenizer), so a long-running worker sees one plan per batch bucket.  `decode` as for
+    `prediction_batch`."""
     if bucket < 1:
         raise ValueError("bucket must be >= 1")
+    _check_decode(decode)
     fixed_select = L.OUT_TASK_HEADS if select is None else int(select)
     answers = [None] * len(requests)
     samples, spans, need = [], {}, 0            # samples: (tokens [Tin], segments [Tin], task [1], features [V, F], spatials [V, 5])
@@ -269,6 +340,12 @@ def prediction_packed(requests, bucket: int = 8, select: Optional[int] = None):
                                    max_tokens=max_tin, max_regions=max_v)
     t_off = np.concatenate([[0], np.cumsum([n + 1 for n in n_tokens])])   # packed text rows (task token included)
     v_off = np.concatenate([[0], np.cumsum(n_regions)])
+    if decode == "device":
+        ground = any(requests[i][8] in GROUNDING_TASKS for i in spans)
+        dec = _decode_device(out, cat[4] if ground else None, {i: (requests[i][8], requests[i][9]) for i in spans}, spans, v_off)
+        for i in spans:
+            answers[i] = dec[i]
+        return answers
     for i, (lo, hi) in spans.items():
         task_id, infos, spatials = requests[i][8], requests[i][9], requests[i][2]
         sl = [None if o is None or isinstance(o, list) else o[lo:hi] for o in out[:9]] + [[]]
@@ -453,12 +530,13 @@ def split_region_outputs(out, spatials, n_tokens, n_boxes, lo, hi, task_id):
     return tuple(sl), sp
 
 
-def custom_prediction_packed(requests, bucket: int = 8, select: Optional[int] = None, max_boxes: int = 100):
+def custom_prediction_packed(requests, bucket: int = 8, select: Optional[int] = None, max_boxes: int = 100, *, decode: str = "host"):
     """`custom_prediction` for many requests in ONE model call (`model.forward_regions_packed`): every question at its own length,
     every image at its own box count, no padding and no masks.  `requests` are argument tuples of `custom_prediction`:
     `(query, task, features, infos, task_id)`; the answers come back in the same order, a request that fails validation gets its
     exception.  The host packing is `pack_region_requests`.  Answers agree with `custom_prediction` within tolerance; they are not
-    guaranteed bit for bit, because dropping the text padding may change the accumulation."""
+    guaranteed bit for bit, because dropping the text padding may change the accumulation.  `decode` as for `prediction_batch`."""
+    _check_decode(decode)
     p = pack_region_requests(requests, bucket, select, max_boxes)
     answers = p["answers"]
     if not p["spans"]:
@@ -467,6 +545,12 @@ def custom_prediction_packed(requests, bucket: int = 8, select: Optional[int] = 
         out, spatials = model.forward_regions_packed(p["question"], p["segment_ids"], p["task_tokens"], p["box_features"], p["boxes"],
                                                      p["image_wh"], p["n_tokens"], p["n_boxes"], select=p["select"],
                                                      max_tokens=p["max_tokens"], max_boxes=p["max_boxes"])
+    if decode == "device":
+        v_off = np.concatenate([[0], np.cumsum([n + 1 for n in p["n_boxes"]])])   # packed regions: the global row, then the boxes
+        dec = _decode_device(out, spatials, {i: (requests[i][4], requests[i][3]) for i in p["spans"]}, p["spans"], v_off)
+        for i in p["spans"]:
+            answers[i] = dec[i]
+        return answers
     for i, (lo, hi) in p["spans"].items():
         task_id, infos = requests[i][4], requests[i][3]
         sl, sp = split_region_outputs(out, spatials, p["n_tokens"], p["n_boxes"], lo, hi, task_id)
@@ -520,13 +604,18 @@ class MicroBatchWorker(object):
     whatever their text lengths and box counts (images of one message may have different box counts too), with no host-side
     feature construction.  Answers agree with the dense path within tolerance; they are not guaranteed bit for bit, because dropping
     the text padding may change the accumulation.  The default stays dense; making packed the default and deleting the dense
-    branch is a follow-up, to be decided on the A/B of scripts/regions_packed_bench.py."""
+    branch is a follow-up, to be decided on the A/B of scripts/regions_packed_bench.py.
 
-    def __init__(self, max_rows: int = 64, max_wait_ms: float = 2.0, bucket: int = 8, packed: bool = False):
+    `decode="device"` decodes every answer of a model call in one kernel (`model.decode_answers`) instead of one softmax, top-N
+    and host synchronisation per message; the default stays on the host."""
+
+    def __init__(self, max_rows: int = 64, max_wait_ms: float = 2.0, bucket: int = 8, packed: bool = False, *, decode: str = "host"):
         import queue
         import threading
+        _check_decode(decode)
         self.max_rows, self.max_wait, self.bucket = int(max_rows), float(max_wait_ms) * 1e-3, int(bucket)
         self.packed = bool(packed)
+        self.decode = decode
         self._q = queue.Queue()
         self._stop = False
         self.batches = []                      # rows per model call group, for tests / monitoring
@@ -597,7 +686,7 @@ class MicroBatchWorker(object):
         if not reqs:
             return
         try:
-            answers = prediction_batch(reqs, bucket=self.bucket)
+            answers = prediction_batch(reqs, bucket=self.bucket, decode=self.decode)
         except Exception as e:                 # noqa: BLE001
             for _, fut, _ in live:
                 fut.set_exception(e)
@@ -617,7 +706,7 @@ class MicroBatchWorker(object):
         if not reqs:
             return
         try:
-            answers = custom_prediction_packed(reqs, bucket=self.bucket)
+            answers = custom_prediction_packed(reqs, bucket=self.bucket, decode=self.decode)
         except Exception as e:                 # noqa: BLE001
             for _, fut, _ in live:
                 fut.set_exception(e)
