@@ -404,6 +404,139 @@ struct Op {
 
 struct OutBuf { float* p = nullptr; int rows = 0, cols = 0, ld = 0; };
 
+// ------------------------------------------------------------------------------------------ packed batches
+// The d_meta format of a packed plan, in ints: text row offsets [B + 1] | image row offsets [B + 1]; with `src` (a packed pair suffix)
+// then the pairs' first rows in the cached text states [B] | image states [B]; with n_entries > 0 (the packed attention
+// probabilities, VB200_OUT_ATTENTION_PACKED) then, 8-byte aligned, the int64 destination pointer | entry float offsets [n_entries] |
+// per-sample prefix sums [3][B + 1] (sum T_b'^2, sum V_b'^2, sum T_b' V_b' over b' < b).  A stream's row total, which bounds its GEMM,
+// LayerNorm and rowdot rows, is its last offset.
+struct MetaLayout {
+    size_t B = 0, n_entries = 0;
+    bool src = false;
+    size_t offs_t() const { return 0; }
+    size_t offs_v() const { return B + 1; }
+    size_t rows_t() const { return offs_t() + B; }
+    size_t rows_v() const { return offs_v() + B; }
+    size_t src_t() const { return 2 * (B + 1); }
+    size_t src_v() const { return src_t() + B; }
+    size_t rows_end() const { return src ? src_v() + B : src_t(); }
+    size_t probs_dst() const { return (rows_end() + 1) & ~static_cast<size_t>(1); }
+    size_t probs_entry(size_t e) const { return probs_dst() + 2 * (1 + e); }
+    size_t probs_prefix(int k) const { return probs_entry(n_entries) + 2 * static_cast<size_t>(k) * (B + 1); }
+    size_t size() const { return n_entries ? probs_prefix(3) : rows_end(); }
+};
+
+// Layout of the packed attention probabilities (VB200_OUT_ATTENTION_PACKED) from the two streams' row offsets [B + 1]: entries in
+// execution order (the order get_plan adds the probability ops in), each holding sample b's [heads, Lq_b, Lk_b] block at
+// heads * prefix[b]; prefix = sum over b' < b of T_b'^2 (text layers), V_b'^2 (image layers) or T_b' V_b' (both directions of a
+// connection layer).  int64 throughout: at batch 512 with 256 rows per sample one call holds more than 2^31 floats.
+struct PackedAttnLayout {
+    std::vector<int32_t> heads, kind;
+    std::vector<int64_t> offset;
+    std::vector<int64_t> prefix;       // [3][B + 1]
+    int64_t total = 0;
+};
+PackedAttnLayout packed_attn_layout(const Config& c, const std::vector<std::string>& schedule, int B, const int* offs_t, const int* offs_v) {
+    PackedAttnLayout l;
+    const size_t n = static_cast<size_t>(B) + 1;
+    l.prefix.assign(3 * n, 0);
+    for (int b = 0; b < B; ++b) {
+        const int64_t T = offs_t[b + 1] - offs_t[b], V = offs_v[b + 1] - offs_v[b];
+        l.prefix[b + 1] = l.prefix[b] + T * T;
+        l.prefix[n + b + 1] = l.prefix[n + b] + V * V;
+        l.prefix[2 * n + b + 1] = l.prefix[2 * n + b] + T * V;
+    }
+    auto put = [&](int heads, int kind) {
+        l.heads.push_back(heads);
+        l.kind.push_back(kind);
+        l.offset.push_back(l.total);
+        l.total += heads * l.prefix[(kind < 2 ? kind : 2) * n + B];
+    };
+    for (const std::string& step : schedule) {
+        if (step[0] == 'T') put(c.heads, 0);
+        else if (step[0] == 'V') put(c.v_heads, 1);
+        else { put(c.bi_heads, 2); put(c.bi_heads, 3); }
+    }
+    return l;
+}
+// The packed probability layout exists for the two packed forwards only; every other forward rejects its select bit.
+void reject_packed_attention(uint32_t select, const char* api) {
+    if (select & VB200_OUT_ATTENTION_PACKED)
+        fail(VB200_ERR_INVALID, "%s: VB200_OUT_ATTENTION_PACKED is only supported by vb200_forward_packed and vb200_forward_regions_packed",
+             api);
+}
+
+// Host lengths of one packed call.  Text lengths count tokens without the task token; a capacity (rows per item, 0: the call's
+// longest) only sizes the plan.  A stream without lengths (the retrieval prefixes) is not part of the call: its offsets stay zero.
+struct PackedLengths {
+    const char* item;                                   // what one entry of the batch is called in messages
+    int B;
+    const int32_t* n_tokens; int max_tokens;
+    const int32_t* n_regions; int max_regions;
+    const int32_t* src_t = nullptr;                     // packed pair suffix: each pair's first row in the cached text states
+    const int32_t* src_v = nullptr;                     //   and in the cached image states
+};
+// One packed call's rows: the plan's per-sample capacities and the d_meta contents (in `layout`) its kernels read.
+struct PackedBatch {
+    int Tin = 1, V = 1;              // plan capacities: T = Tin + task token and V rounded up to 16 rows; 1 for a stream not in the call
+    MetaLayout layout;
+    std::vector<int> meta;
+    const int* offs_t() const { return meta.data() + layout.offs_t(); }
+    const int* offs_v() const { return meta.data() + layout.offs_v(); }
+    int rows_t() const { return meta[layout.rows_t()]; }
+    int rows_v() const { return meta[layout.rows_v()]; }
+};
+// Validates a packed call's lengths and lays out its rows: offs[i + 1] = offs[i] + rows_i per stream (text: T_i = Tin_i + task
+// token).  Rejects a batch < 1, a negative capacity, a length < 1 or above a non-zero capacity, more than 256 rows (the
+// small-sequence attention kernels) and Tin_i > max_position_embeddings.  maps (non-null): where the plan's kernels write the packed
+// attention probabilities, whose layout then joins the meta.
+PackedBatch pack_batch(const char* api, const Config& c, const std::vector<std::string>& schedule, const PackedLengths& in, float* maps) {
+    if (in.B < 1) fail(VB200_ERR_INVALID, "%s: batch must be positive", api);
+    if (in.max_tokens < 0) fail(VB200_ERR_INVALID, "%s: negative capacity max_tokens %d", api, in.max_tokens);
+    if (in.max_regions < 0) fail(VB200_ERR_INVALID, "%s: negative capacity max_regions %d", api, in.max_regions);
+    const int task = c.task_tokens ? 1 : 0;
+    PackedBatch b;
+    b.layout = MetaLayout{static_cast<size_t>(in.B), 0, in.src_t != nullptr};
+    b.meta.assign(b.layout.size(), 0);
+    auto pack = [&](bool text, const int32_t* len, int cap, size_t at) {      // one stream's offsets; returns its plan capacity
+        const char* name = text ? "n_tokens" : "n_regions";
+        const int extra = text ? task : 0;
+        int* offs = b.meta.data() + at;
+        int longest = 0;
+        for (int i = 0; i < in.B; ++i) {
+            const int l = len[i];
+            if (l < 1) fail(VB200_ERR_INVALID, "%s: %s %d has %s %d (must be >= 1)", api, in.item, i, name, l);
+            if (cap > 0 && l > cap) fail(VB200_ERR_INVALID, "%s: %s %d has %s %d, above the capacity %d", api, in.item, i, name, l, cap);
+            if (l + extra > 256)
+                fail(VB200_ERR_INVALID, "%s: %s %d too long for the small-sequence attention kernels (%s=%d, max 256)", api, in.item, i,
+                     text ? "T" : "V", l + extra);
+            if (text && l > c.max_pos)
+                fail(VB200_ERR_INVALID, "%s: %s %d has n_tokens %d > max_position_embeddings %d", api, in.item, i, l, c.max_pos);
+            offs[i + 1] = offs[i] + l + extra;
+            longest = std::max(longest, l);
+        }
+        const int rows = (cap > 0 ? cap : longest) + extra;                     // rounded up to the attention kernels' 16-row buckets
+        if (rows > 256) fail(VB200_ERR_INVALID, "%s: capacity above 256 rows per sample (%s=%d)", api, text ? "T" : "V", rows);
+        return (rows + 15) / 16 * 16;
+    };
+    if (in.n_tokens) b.Tin = pack(true, in.n_tokens, in.max_tokens, b.layout.offs_t()) - task;
+    if (in.n_regions) b.V = pack(false, in.n_regions, in.max_regions, b.layout.offs_v());
+    if (b.layout.src) {
+        std::copy(in.src_t, in.src_t + in.B, b.meta.begin() + b.layout.src_t());
+        std::copy(in.src_v, in.src_v + in.B, b.meta.begin() + b.layout.src_v());
+    }
+    if (maps) {
+        const PackedAttnLayout l = packed_attn_layout(c, schedule, in.B, b.offs_t(), b.offs_v());
+        const int64_t dst = static_cast<int64_t>(reinterpret_cast<uintptr_t>(maps));
+        b.layout.n_entries = l.offset.size();
+        b.meta.resize(b.layout.size(), 0);
+        memcpy(b.meta.data() + b.layout.probs_dst(), &dst, sizeof(dst));
+        memcpy(b.meta.data() + b.layout.probs_entry(0), l.offset.data(), l.offset.size() * sizeof(int64_t));
+        memcpy(b.meta.data() + b.layout.probs_prefix(0), l.prefix.data(), l.prefix.size() * sizeof(int64_t));
+    }
+    return b;
+}
+
 struct Plan {
     int B = 0, Tin = 0, T = 0, V = 0;
     uint32_t select = 0;
@@ -429,26 +562,21 @@ struct Plan {
     float *d_feat = nullptr, *d_loc = nullptr;
     uint8_t* d_imask = nullptr;
     float* d_out[12] = {nullptr};
-    // packed plans (vb200_forward_packed and the packed retrieval calls): d_meta = text row offsets [B + 1] | image row offsets
-    // [B + 1] | text rows | image rows, and for a packed pair suffix also the pairs' source rows in the cached text states [B] |
-    // image states [B]; filled per call from the pinned h_meta; meta_copied marks when the last copy out of h_meta has been made
+    // packed plans (the packed forwards and retrieval calls): d_meta in the format `layout` describes, filled per call from the
+    // pinned h_meta (stage_meta); meta_copied marks when the last copy out of h_meta has been made
     bool packed = false;
+    MetaLayout layout;
     int* d_meta = nullptr;
     int* h_meta = nullptr;
     cudaEvent_t meta_copied = nullptr;
-    const int* offs_t() const { return d_meta; }
-    const int* offs_v() const { return d_meta + B + 1; }
-    const int* rows_t() const { return d_meta + 2 * (B + 1); }
-    const int* rows_v() const { return d_meta + 2 * (B + 1) + 1; }
-    const int* src_t() const { return d_meta + 2 * (B + 1) + 2; }
-    const int* src_v() const { return d_meta + 2 * (B + 1) + 2 + B; }
-    // packed plans with the packed attention-probability output (VB200_OUT_ATTENTION_PACKED): d_meta continues, 8-byte aligned at
-    // int probs_base(B), with int64 destination pointer | entry float offsets [n_probs] | per-sample prefix sums [3][B + 1]
-    // (sum T_b'^2, sum V_b'^2, sum T_b' V_b' over b' < b), staged per call with the rest of the meta
-    int n_probs = 0;
-    static size_t probs_base(int B) { return (2 * (static_cast<size_t>(B) + 1) + 2 + 1) & ~static_cast<size_t>(1); }
-    static size_t probs_meta_len(int B, int n_entries) { return 1 + static_cast<size_t>(n_entries) + 3 * (static_cast<size_t>(B) + 1); }
-    const int64_t* probs_meta() const { return reinterpret_cast<const int64_t*>(d_meta + probs_base(B)); }
+    int n_probs = 0;                                   // packed attention-probability ops added so far (their entry index)
+    const int* offs_t() const { return d_meta + layout.offs_t(); }
+    const int* offs_v() const { return d_meta + layout.offs_v(); }
+    const int* rows_t() const { return d_meta + layout.rows_t(); }
+    const int* rows_v() const { return d_meta + layout.rows_v(); }
+    const int* src_t() const { return d_meta + layout.src_t(); }
+    const int* src_v() const { return d_meta + layout.src_v(); }
+    const int64_t* meta64(size_t at) const { return reinterpret_cast<const int64_t*>(d_meta + at); }
     ~Plan() {
         if (exec) cudaGraphExecDestroy(exec);
         if (graph) cudaGraphDestroy(graph);
@@ -862,10 +990,10 @@ struct vb200_engine {
         a.B = pl.B; a.heads = heads; a.head_dim = hid / heads;
         a.f_ctx = x3 ? ctx : nullptr; a.f_ctx_mode = x3 ? 3 : 0; a.f_ld_ctx = x3 ? 3 * hid : 0;
         if (want_probs && pl.packed) {
-            const int n_entries = attention_entries();
-            const int64_t* pm = pl.probs_meta();
+            const MetaLayout& m = pl.layout;
             a.f_packed = true;
-            a.f_pk = vb::PackedProbs{offs_q, offs_k, pm, pm + 1 + pl.n_probs, pm + 1 + n_entries + static_cast<size_t>(prefix) * (pl.B + 1)};
+            a.f_pk = vb::PackedProbs{offs_q, offs_k, pl.meta64(m.probs_dst()), pl.meta64(m.probs_entry(pl.n_probs)),
+                                     pl.meta64(m.probs_prefix(prefix))};
             ++pl.n_probs;
         } else if (want_probs) {
             a.f_probs = pl.mem.alloc_n<float>(static_cast<size_t>(pl.B) * heads * Lq * Lk);
@@ -926,10 +1054,10 @@ struct vb200_engine {
         if (Tin > c.max_pos && !packed) fail(VB200_ERR_INVALID, "n_tokens %d exceeds max_position_embeddings %d", Tin, c.max_pos);
         pl.B = B; pl.Tin = Tin; pl.T = T; pl.V = V; pl.select = select;
         if (packed) {
-            // zero offsets and totals until the first call: the validation pass and the capture below then touch no row
+            // zero offsets until the first call: the validation pass and the capture below then touch no row
             pl.packed = true;
-            size_t n_meta = 2 * (static_cast<size_t>(B) + 1) + 2 + (mode == PACKED_SUFFIX ? 2 * static_cast<size_t>(B) : 0);
-            if (want_attn) n_meta = Plan::probs_base(B) + 2 * Plan::probs_meta_len(B, attention_entries());
+            pl.layout = MetaLayout{static_cast<size_t>(B), want_attn ? static_cast<size_t>(attention_entries()) : 0, mode == PACKED_SUFFIX};
+            const size_t n_meta = pl.layout.size();
             pl.d_meta = pl.mem.alloc_n<int>(n_meta);
             CUDA_CHECK(cudaMemset(pl.d_meta, 0, n_meta * sizeof(int)));
             CUDA_CHECK(cudaMallocHost(&pl.h_meta, n_meta * sizeof(int)));
@@ -1374,12 +1502,28 @@ struct vb200_engine {
         if (!in.question || !in.features || !in.spatials || !in.segment_ids || !in.input_mask || !in.image_mask ||
             (c.task_tokens && !in.task_tokens))
             fail(VB200_ERR_INVALID, "vb200_inputs has a NULL required pointer");
-        CUDA_CHECK(vb::launch_text_embed(in.question, in.segment_ids, in.input_mask, in.task_tokens, word, pos, type, task,
-                                         emb_ln.g, emb_ln.b, c.ln_eps, pl.t_f32[0], pl.t_b16[0], pl.mask_t, pl.B, pl.Tin,
-                                         c.hidden, c.vocab, c.max_pos, c.type_vocab, c.n_task, c.task_tokens, opt.act_fp16, x3 ? 1 : 0, st));
-        CUDA_CHECK(vb::launch_image_pack(in.features, in.spatials, in.image_mask, pl.img_a, pl.mask_v, pl.B * pl.V, c.v_feat, pl.kp,
-                                         opt.act_fp16, x3 ? 1 : 0, st));
+        embed_text(pl, in.question, in.segment_ids, in.input_mask, in.task_tokens, pl.B * pl.T, st);
+        pack_image(pl, in.features, in.spatials, in.image_mask, pl.B * pl.V, st);
         run_plan(pl, st);
+    }
+    // The input kernels of every plan.  `rows`: the text / image rows of the call -- B x T / B x V on dense plans (padding from the
+    // masks), the call's row totals on packed plans (no masks: every row is real; the rows up to the next 128-row GEMM tile are
+    // zeroed, the only rows past the totals a GEMM loads).
+    void embed_text(Plan& pl, const int64_t* q, const int64_t* seg, const int64_t* input_mask, const int64_t* tk, int rows, cudaStream_t st) {
+        const Config& c = cfg;
+        CUDA_CHECK(vb::launch_text_embed(q, seg, input_mask, tk, word, pos, type, task, emb_ln.g, emb_ln.b, c.ln_eps, pl.t_f32[0], pl.t_b16[0],
+                                         pl.mask_t, pl.B, pl.Tin, c.hidden, c.vocab, c.max_pos, c.type_vocab, c.n_task, c.task_tokens,
+                                         opt.act_fp16, x3 ? 1 : 0, st, pl.packed ? pl.offs_t() : nullptr, rows));
+        if (pl.packed) zero_tail(pl.t_b16[0], rows, pl.B * pl.T, c.hidden, st);
+    }
+    void pack_image(Plan& pl, const float* feats, const float* loc, const uint8_t* image_mask, int rows, cudaStream_t st) {
+        CUDA_CHECK(vb::launch_image_pack(feats, loc, image_mask, pl.img_a, pl.mask_v, rows, cfg.v_feat, pl.kp, opt.act_fp16, x3 ? 1 : 0, st));
+        if (pl.packed) zero_tail(pl.img_a, rows, pl.B * pl.V, pl.kp, st);
+    }
+    // zero the 16-bit operand rows [rows, next 128-row boundary) of a buffer with `cap` rows
+    static void zero_tail(bf16* buf, int rows, int cap, size_t width, cudaStream_t st) {
+        const int end = std::min(cap, (rows + 127) / 128 * 128);
+        if (end > rows) CUDA_CHECK(cudaMemsetAsync(buf + static_cast<size_t>(rows) * width, 0, static_cast<size_t>(end - rows) * width * 2, st));
     }
     void run_plan(Plan& pl, cudaStream_t st) {
         if (pl.ops.empty()) return;
@@ -1394,116 +1538,85 @@ struct vb200_engine {
         if (!in.question || !in.segment_ids || !in.input_mask || (c.task_tokens && !in.task_tokens) || !in.box_features || !in.boxes ||
             !in.image_wh)
             fail(VB200_ERR_INVALID, "vb200_region_inputs has a NULL required pointer");
-        CUDA_CHECK(vb::launch_text_embed(in.question, in.segment_ids, in.input_mask, in.task_tokens, word, pos, type, task,
-                                         emb_ln.g, emb_ln.b, c.ln_eps, pl.t_f32[0], pl.t_b16[0], pl.mask_t, pl.B, pl.Tin,
-                                         c.hidden, c.vocab, c.max_pos, c.type_vocab, c.n_task, c.task_tokens, opt.act_fp16, x3 ? 1 : 0, st));
+        embed_text(pl, in.question, in.segment_ids, in.input_mask, in.task_tokens, pl.B * pl.T, st);
         CUDA_CHECK(vb::launch_region_pack(in.box_features, in.boxes, in.image_wh, in.num_boxes, pl.img_a, pl.mask_v, in.spatials_out,
                                           pl.B, pl.V - 1, c.v_feat, pl.kp, opt.act_fp16, x3 ? 1 : 0, st));
         run_plan(pl, st);
     }
-    // Packed batch (PlanMode PACKED): offsets and row totals go to the plan's d_meta through its pinned staging buffer, ahead of the
-    // graph on the same stream; the pack kernels then run on the real rows only and zero the operand rows up to the next 128-row
-    // boundary (the rest of the last GEMM tile that holds a real row, the only rows past the totals a GEMM loads).
-    void forward_packed(Plan& pl, const vb200_packed_inputs& in, const std::vector<int>& meta, cudaStream_t st) {
-        stage_meta(pl, meta, st);
-        embed_text_packed(pl, in.question, in.segment_ids, in.task_tokens, meta[2 * (pl.B + 1)], st);
-        pack_image_packed(pl, in.features, in.spatials, meta[2 * (pl.B + 1) + 1], st);
+    // ---- packed batches (run_packed has staged the call's d_meta ahead of these, in stream order)
+    void forward_packed(Plan& pl, const vb200_packed_inputs& in, const PackedBatch& b, cudaStream_t st) {
+        embed_text(pl, in.question, in.segment_ids, nullptr, in.task_tokens, b.rows_t(), st);
+        pack_image(pl, in.features, in.spatials, nullptr, b.rows_v(), st);
         run_plan(pl, st);
     }
     // Packed detector output on a PACKED plan: the region-pack kernel writes every image's mean row and boxes at the plan's image
     // offsets (the same rows forward_regions writes for that image alone), then the packed forward runs as above
-    void forward_regions_packed(Plan& pl, const vb200_packed_region_inputs& in, const std::vector<int>& meta, cudaStream_t st) {
-        const Config& c = cfg;
-        const int rows_v = meta[2 * (pl.B + 1) + 1];
-        stage_meta(pl, meta, st);
-        embed_text_packed(pl, in.question, in.segment_ids, in.task_tokens, meta[2 * (pl.B + 1)], st);
+    void forward_regions_packed(Plan& pl, const vb200_packed_region_inputs& in, const PackedBatch& b, cudaStream_t st) {
+        embed_text(pl, in.question, in.segment_ids, nullptr, in.task_tokens, b.rows_t(), st);
         CUDA_CHECK(vb::launch_region_pack(in.box_features, in.boxes, in.image_wh, nullptr, pl.img_a, pl.mask_v, in.spatials_out, pl.B, 0,
-                                          c.v_feat, pl.kp, opt.act_fp16, 0, st, pl.offs_v()));
-        zero_tail(pl.img_a, rows_v, pl.B * pl.V, pl.kp, st);
+                                          cfg.v_feat, pl.kp, opt.act_fp16, 0, st, pl.offs_v()));
+        zero_tail(pl.img_a, b.rows_v(), pl.B * pl.V, pl.kp, st);
         run_plan(pl, st);
     }
-    // meta (host, the plan's d_meta layout) -> d_meta, in stream order ahead of the plan's kernels
+    // packed pair suffix: every pair's rows are gathered from the packed caption / image states into the plan's packed buffers
+    void forward_cached_packed(Plan& pl, const vb200_packed_pairs& in, const PackedBatch& b, cudaStream_t st) {
+        const Config& c = cfg;
+        const vb::PackedStateCopy text{pl.offs_t(), pl.src_t(), in.text_f32, in.text_16, pl.t_f32[0], pl.t_b16[0], c.hidden / 4, c.hidden / 8};
+        const vb::PackedStateCopy image{pl.offs_v(), pl.src_v(), in.image_f32, in.image_16, pl.v_f32[0], pl.v_b16[0], c.v_hidden / 4,
+                                        c.v_hidden / 8};
+        CUDA_CHECK(vb::launch_gather_packed_state(text, image, pl.B, st));
+        zero_tail(pl.t_b16[0], b.rows_t(), pl.B * pl.T, c.hidden, st);
+        zero_tail(pl.v_b16[0], b.rows_v(), pl.B * pl.V, c.v_hidden, st);
+        run_plan(pl, st);
+    }
+    // What every packed entry point shares once it has checked its own inputs: the engine-wide rejections, the call's rows
+    // (pack_batch), its plan, the d_meta staged ahead of `run` (the call's input kernels and the plan) and, for the forwards
+    // (out != null), the outputs at the call's row totals.
+    void run_packed(const char* api, int mode, const PackedLengths& len, uint32_t select, int slot, const vb200_outputs* out,
+                    void* cuda_stream, const std::function<void(Plan&, const PackedBatch&, cudaStream_t)>& run) {
+        if (select & VB200_OUT_ATTENTION)
+            fail(VB200_ERR_INVALID, "%s: the attention-probability output (VB200_OUT_ATTENTION) is not supported", api);
+        if (mode != PACKED) reject_packed_attention(select, api);
+        const bool maps = (select & VB200_OUT_ATTENTION_PACKED) != 0;
+        if (maps && out->attention_probs == nullptr)
+            fail(VB200_ERR_INVALID, "%s: VB200_OUT_ATTENTION_PACKED needs vb200_outputs.attention_probs (NULL)", api);
+        if (x3) fail(VB200_ERR_INVALID, "%s: packed batches are not supported in split_fp32 (fp32x) mode", api);
+        const PackedBatch b = pack_batch(api, cfg, schedule, len, maps ? out->attention_probs : nullptr);
+        CUDA_CHECK(cudaSetDevice(opt.device));
+        Plan& pl = *get_plan(len.B, b.Tin, b.V, select & VB200_OUT_ALL, slot, mode, maps);
+        const cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+        stage_meta(pl, b.meta, st);
+        run(pl, b, st);
+        if (out != nullptr) copy_outputs(pl, *out, st, cudaMemcpyDeviceToDevice, b.rows_t(), b.rows_v());
+    }
+    // meta (host, in the plan's d_meta layout) -> d_meta, in stream order ahead of the plan's kernels
     void stage_meta(Plan& pl, const std::vector<int>& meta, cudaStream_t st) {
         CUDA_CHECK(cudaEventSynchronize(pl.meta_copied));           // the previous call's copy has left the staging buffer
         memcpy(pl.h_meta, meta.data(), meta.size() * sizeof(int));
         CUDA_CHECK(cudaMemcpyAsync(pl.d_meta, pl.h_meta, meta.size() * sizeof(int), cudaMemcpyHostToDevice, st));
         CUDA_CHECK(cudaEventRecord(pl.meta_copied, st));
     }
-    // zero the 16-bit operand rows [rows, next 128-row boundary) of a buffer with `cap` rows
-    static void zero_tail(bf16* buf, int rows, int cap, size_t width, cudaStream_t st) {
-        const int end = std::min(cap, (rows + 127) / 128 * 128);
-        if (end > rows) CUDA_CHECK(cudaMemsetAsync(buf + static_cast<size_t>(rows) * width, 0, static_cast<size_t>(end - rows) * width * 2, st));
-    }
-    void embed_text_packed(Plan& pl, const int64_t* q, const int64_t* seg, const int64_t* tk, int rows_t, cudaStream_t st) {
-        const Config& c = cfg;
-        CUDA_CHECK(vb::launch_text_embed(q, seg, nullptr, tk, word, pos, type, task, emb_ln.g, emb_ln.b, c.ln_eps, pl.t_f32[0], pl.t_b16[0],
-                                         pl.mask_t, pl.B, 0, c.hidden, c.vocab, c.max_pos, c.type_vocab, c.n_task, c.task_tokens,
-                                         opt.act_fp16, 0, st, pl.offs_t(), rows_t));
-        zero_tail(pl.t_b16[0], rows_t, pl.B * pl.T, c.hidden, st);
-    }
-    void pack_image_packed(Plan& pl, const float* feats, const float* loc, int rows_v, cudaStream_t st) {
-        const Config& c = cfg;
-        CUDA_CHECK(vb::launch_image_pack(feats, loc, nullptr, pl.img_a, pl.mask_v, rows_v, c.v_feat, pl.kp, opt.act_fp16, 0, st));
-        zero_tail(pl.img_a, rows_v, pl.B * pl.V, pl.kp, st);
-    }
-    // ---- packed retrieval (PACKED_TEXT_PREFIX / PACKED_IMAGE_PREFIX / PACKED_SUFFIX): the prefixes write each caption's / image's
-    // rows back to back into the caller's state; the suffix gathers every pair's rows from those states into its packed buffers
-    void encode_text_packed(Plan& pl, const std::vector<int>& meta, const int64_t* q, const int64_t* seg, const int64_t* tk, float* st_f32,
-                            void* st_16, cudaStream_t st) {
-        const int rows = meta[2 * (pl.B + 1)];
-        stage_meta(pl, meta, st);
-        embed_text_packed(pl, q, seg, tk, rows, st);
-        run_plan(pl, st);
-        CUDA_CHECK(cudaMemcpyAsync(st_f32, pl.t_f32[pl.t_cur], static_cast<size_t>(rows) * cfg.hidden * 4, cudaMemcpyDeviceToDevice, st));
-        CUDA_CHECK(cudaMemcpyAsync(st_16, pl.t_b16[pl.t_cur], static_cast<size_t>(rows) * cfg.hidden * 2, cudaMemcpyDeviceToDevice, st));
-    }
-    void encode_image_packed(Plan& pl, const std::vector<int>& meta, const float* feats, const float* loc, float* st_f32, void* st_16,
-                             cudaStream_t st) {
-        const int rows = meta[2 * (pl.B + 1) + 1];
-        stage_meta(pl, meta, st);
-        pack_image_packed(pl, feats, loc, rows, st);
-        run_plan(pl, st);
-        CUDA_CHECK(cudaMemcpyAsync(st_f32, pl.v_f32[pl.v_cur], static_cast<size_t>(rows) * cfg.v_hidden * 4, cudaMemcpyDeviceToDevice, st));
-        CUDA_CHECK(cudaMemcpyAsync(st_16, pl.v_b16[pl.v_cur], static_cast<size_t>(rows) * cfg.v_hidden * 2, cudaMemcpyDeviceToDevice, st));
-    }
-    void forward_cached_packed(Plan& pl, const vb200_packed_pairs& in, const std::vector<int>& meta, cudaStream_t st) {
-        const Config& c = cfg;
-        const int B = pl.B;
-        stage_meta(pl, meta, st);
-        const vb::PackedStateCopy text{pl.offs_t(), pl.src_t(), in.text_f32, in.text_16, pl.t_f32[0], pl.t_b16[0], c.hidden / 4, c.hidden / 8};
-        const vb::PackedStateCopy image{pl.offs_v(), pl.src_v(), in.image_f32, in.image_16, pl.v_f32[0], pl.v_b16[0], c.v_hidden / 4,
-                                        c.v_hidden / 8};
-        CUDA_CHECK(vb::launch_gather_packed_state(text, image, B, st));
-        zero_tail(pl.t_b16[0], meta[2 * (B + 1)], B * pl.T, c.hidden, st);
-        zero_tail(pl.v_b16[0], meta[2 * (B + 1) + 1], B * pl.V, c.v_hidden, st);
-        run_plan(pl, st);
-    }
-    // ---- retrieval reuse (PlanMode): per-caption / per-image prefixes and the pair suffix
-    void encode_text(int n, int Tin, const int64_t* q, const int64_t* seg, const int64_t* im, const int64_t* tk, float* st_f32,
+    // ---- retrieval reuse (PlanMode): per-caption / per-image prefixes and the pair suffix.  A prefix leaves its stream's state after
+    // the layers ahead of the first connection layer in the caller's buffers: `rows` rows, B x T / B x V with the mask on dense
+    // plans, the call's rows back to back and no mask (st_mask null) on packed plans
+    void encode_text(Plan& pl, const int64_t* q, const int64_t* seg, const int64_t* im, const int64_t* tk, int rows, float* st_f32,
                      void* st_16, float* st_mask, cudaStream_t st) {
-        const Config& c = cfg;
-        if (!q || !seg || !im || (c.task_tokens && !tk) || !st_f32 || !st_16 || !st_mask) fail(VB200_ERR_INVALID, "vb200_encode_text: NULL pointer");
-        Plan& pl = *get_plan(n, Tin, 1, 0, 0, TEXT_PREFIX);
-        CUDA_CHECK(vb::launch_text_embed(q, seg, im, tk, word, pos, type, task, emb_ln.g, emb_ln.b, c.ln_eps, pl.t_f32[0], pl.t_b16[0],
-                                         pl.mask_t, pl.B, pl.Tin, c.hidden, c.vocab, c.max_pos, c.type_vocab, c.n_task, c.task_tokens,
-                                         opt.act_fp16, x3 ? 1 : 0, st));
+        embed_text(pl, q, seg, im, tk, rows, st);
         run_plan(pl, st);
-        const size_t rows = static_cast<size_t>(pl.B) * pl.T, S = x3 ? 3 : 1;
-        CUDA_CHECK(cudaMemcpyAsync(st_f32, pl.t_f32[pl.t_cur], rows * c.hidden * 4, cudaMemcpyDeviceToDevice, st));
-        CUDA_CHECK(cudaMemcpyAsync(st_16, pl.t_b16[pl.t_cur], rows * c.hidden * S * 2, cudaMemcpyDeviceToDevice, st));
-        CUDA_CHECK(cudaMemcpyAsync(st_mask, pl.mask_t, rows * 4, cudaMemcpyDeviceToDevice, st));
+        copy_state(pl.t_f32[pl.t_cur], pl.t_b16[pl.t_cur], pl.mask_t, rows, cfg.hidden, st_f32, st_16, st_mask, st);
     }
-    void encode_image(int n, int V, const float* feats, const float* loc, const uint8_t* vmask, float* st_f32, void* st_16,
+    void encode_image(Plan& pl, const float* feats, const float* loc, const uint8_t* vmask, int rows, float* st_f32, void* st_16,
                       float* st_mask, cudaStream_t st) {
-        const Config& c = cfg;
-        if (!feats || !loc || !vmask || !st_f32 || !st_16 || !st_mask) fail(VB200_ERR_INVALID, "vb200_encode_image: NULL pointer");
-        Plan& pl = *get_plan(n, 1, V, 0, 0, IMAGE_PREFIX);
-        CUDA_CHECK(vb::launch_image_pack(feats, loc, vmask, pl.img_a, pl.mask_v, pl.B * pl.V, c.v_feat, pl.kp, opt.act_fp16, x3 ? 1 : 0, st));
+        pack_image(pl, feats, loc, vmask, rows, st);
         run_plan(pl, st);
-        const size_t rows = static_cast<size_t>(pl.B) * pl.V, S = x3 ? 3 : 1;
-        CUDA_CHECK(cudaMemcpyAsync(st_f32, pl.v_f32[pl.v_cur], rows * c.v_hidden * 4, cudaMemcpyDeviceToDevice, st));
-        CUDA_CHECK(cudaMemcpyAsync(st_16, pl.v_b16[pl.v_cur], rows * c.v_hidden * S * 2, cudaMemcpyDeviceToDevice, st));
-        CUDA_CHECK(cudaMemcpyAsync(st_mask, pl.mask_v, rows * 4, cudaMemcpyDeviceToDevice, st));
+        copy_state(pl.v_f32[pl.v_cur], pl.v_b16[pl.v_cur], pl.mask_v, rows, cfg.v_hidden, st_f32, st_16, st_mask, st);
+    }
+    void copy_state(const float* f32, const bf16* b16, const float* mask, size_t rows, size_t H, float* st_f32, void* st_16,
+                    float* st_mask, cudaStream_t st) {
+        const size_t S = x3 ? 3 : 1;
+        CUDA_CHECK(cudaMemcpyAsync(st_f32, f32, rows * H * 4, cudaMemcpyDeviceToDevice, st));
+        CUDA_CHECK(cudaMemcpyAsync(st_16, b16, rows * H * S * 2, cudaMemcpyDeviceToDevice, st));
+        if (st_mask != nullptr) CUDA_CHECK(cudaMemcpyAsync(st_mask, mask, rows * 4, cudaMemcpyDeviceToDevice, st));
     }
     void forward_cached(Plan& pl, const int32_t* t_idx, int n_text, const float* t_f32, const void* t_16, const float* t_mask,
                         const int32_t* v_idx, int n_img, const float* v_f32, const void* v_16, const float* v_mask, cudaStream_t st) {
@@ -1652,83 +1765,6 @@ void require_device(int device) {
     CUDA_CHECK(cudaSetDevice(device));
 }
 
-// Row offsets of one stream of a packed call from HOST lengths (text: Tin_i, rows T_i = Tin_i + task token; image: V_i rows):
-// offs[i + 1] = offs[i] + rows_i.  Rejects a length < 1 or above a non-zero capacity `cap`, more than 256 rows (the small-sequence
-// attention kernels) and Tin_i > max_position_embeddings.  Returns the longest length.
-int pack_lengths(const char* api, const char* item, bool text, const Config& c, const int32_t* len, int n, int cap, int* offs) {
-    const char* name = text ? "n_tokens" : "n_regions";
-    const int extra = text && c.task_tokens ? 1 : 0;
-    int longest = 0;
-    offs[0] = 0;
-    for (int i = 0; i < n; ++i) {
-        const int l = len[i];
-        if (l < 1) fail(VB200_ERR_INVALID, "%s: %s %d has %s %d (must be >= 1)", api, item, i, name, l);
-        if (cap > 0 && l > cap) fail(VB200_ERR_INVALID, "%s: %s %d has %s %d, above the capacity %d", api, item, i, name, l, cap);
-        if (l + extra > 256)
-            fail(VB200_ERR_INVALID, "%s: %s %d too long for the small-sequence attention kernels (%s=%d, max 256)", api, item, i,
-                 text ? "T" : "V", l + extra);
-        if (text && l > c.max_pos) fail(VB200_ERR_INVALID, "%s: %s %d has n_tokens %d > max_position_embeddings %d", api, item, i, l, c.max_pos);
-        offs[i + 1] = offs[i] + l + extra;
-        longest = std::max(longest, l);
-    }
-    return longest;
-}
-// Layout of the packed attention probabilities (VB200_OUT_ATTENTION_PACKED) from the two streams' row offsets [B + 1]: entries in
-// execution order (the order get_plan adds the probability ops in), each holding sample b's [heads, Lq_b, Lk_b] block at
-// heads * prefix[b]; prefix = sum over b' < b of T_b'^2 (text layers), V_b'^2 (image layers) or T_b' V_b' (both directions of a
-// connection layer).  int64 throughout: at batch 512 with 256 rows per sample one call holds more than 2^31 floats.
-struct PackedAttnLayout {
-    std::vector<int32_t> heads, kind;
-    std::vector<int64_t> offset;
-    std::vector<int64_t> prefix;       // [3][B + 1]
-    int64_t total = 0;
-};
-PackedAttnLayout packed_attn_layout(const Config& c, const std::vector<std::string>& schedule, int B, const int* offs_t, const int* offs_v) {
-    PackedAttnLayout l;
-    const size_t n = static_cast<size_t>(B) + 1;
-    l.prefix.assign(3 * n, 0);
-    for (int b = 0; b < B; ++b) {
-        const int64_t T = offs_t[b + 1] - offs_t[b], V = offs_v[b + 1] - offs_v[b];
-        l.prefix[b + 1] = l.prefix[b] + T * T;
-        l.prefix[n + b + 1] = l.prefix[n + b] + V * V;
-        l.prefix[2 * n + b + 1] = l.prefix[2 * n + b] + T * V;
-    }
-    auto put = [&](int heads, int kind) {
-        l.heads.push_back(heads);
-        l.kind.push_back(kind);
-        l.offset.push_back(l.total);
-        l.total += heads * l.prefix[(kind < 2 ? kind : 2) * n + B];
-    };
-    for (const std::string& step : schedule) {
-        if (step[0] == 'T') put(c.heads, 0);
-        else if (step[0] == 'V') put(c.v_heads, 1);
-        else { put(c.bi_heads, 2); put(c.bi_heads, 3); }
-    }
-    return l;
-}
-// Appends the plan's probability meta (Plan::probs_meta: destination | entry offsets | prefix sums) to a packed call's meta.
-void put_probs_meta(std::vector<int>& meta, int B, float* dst, const PackedAttnLayout& l) {
-    std::vector<int64_t> ext;
-    ext.reserve(1 + l.offset.size() + l.prefix.size());
-    ext.push_back(static_cast<int64_t>(reinterpret_cast<uintptr_t>(dst)));
-    ext.insert(ext.end(), l.offset.begin(), l.offset.end());
-    ext.insert(ext.end(), l.prefix.begin(), l.prefix.end());
-    const size_t base = Plan::probs_base(B);
-    meta.resize(base + 2 * ext.size(), 0);
-    memcpy(meta.data() + base, ext.data(), ext.size() * sizeof(int64_t));
-}
-// The packed probability layout exists for the two packed forwards only; every other forward rejects its select bit.
-void reject_packed_attention(uint32_t select, const char* api) {
-    if (select & VB200_OUT_ATTENTION_PACKED)
-        fail(VB200_ERR_INVALID, "%s: VB200_OUT_ATTENTION_PACKED is only supported by vb200_forward_packed and vb200_forward_regions_packed",
-             api);
-}
-// Plan capacity in rows per item, rounded up to the attention kernels' 16-row buckets: `cap` (0: the call's longest) + extra rows.
-int capacity16(const char* api, int cap, int longest, int extra, const char* rows_name) {
-    const int rows = (cap > 0 ? cap : longest) + extra;
-    if (rows > 256) fail(VB200_ERR_INVALID, "%s: capacity above 256 rows per sample (%s=%d)", api, rows_name, rows);
-    return (rows + 15) / 16 * 16;
-}
 }  // namespace
 
 // =========================================================================================== C ABI
@@ -1823,31 +1859,12 @@ int vb200_forward_packed(vb200_handle h, const vb200_packed_inputs* in, const vb
     if (h == nullptr) return VB200_ERR_INVALID;
     return guard(h, [&] {
         if (in == nullptr || out == nullptr) fail(VB200_ERR_INVALID, "inputs/outputs struct is NULL");
-        if (select & VB200_OUT_ATTENTION) fail(VB200_ERR_INVALID, "packed batches: the attention-probability output (VB200_OUT_ATTENTION) is not supported");
-        if (h->x3) fail(VB200_ERR_INVALID, "packed batches are not supported in split_fp32 (fp32x) mode");
-        const bool maps = (select & VB200_OUT_ATTENTION_PACKED) != 0;
-        if (maps && out->attention_probs == nullptr)
-            fail(VB200_ERR_INVALID, "packed batches: VB200_OUT_ATTENTION_PACKED needs vb200_outputs.attention_probs (NULL)");
-        const Config& c = h->cfg;
-        const int B = in->batch, task = c.task_tokens ? 1 : 0;
-        if (B < 1) fail(VB200_ERR_INVALID, "packed batches: batch must be positive");
-        if (in->max_tokens < 0 || in->max_regions < 0) fail(VB200_ERR_INVALID, "packed batches: negative capacity");
-        if (!in->n_tokens || !in->n_regions || !in->question || !in->segment_ids || !in->features || !in->spatials || (task && !in->task_tokens))
+        if (!in->n_tokens || !in->n_regions || !in->question || !in->segment_ids || !in->features || !in->spatials ||
+            (h->cfg.task_tokens && !in->task_tokens))
             fail(VB200_ERR_INVALID, "vb200_packed_inputs has a NULL required pointer");
-        // meta = text row offsets [B + 1] | image row offsets [B + 1] | text rows | image rows (the plan's d_meta layout)
-        std::vector<int> meta(2 * (static_cast<size_t>(B) + 1) + 2, 0);
-        const int max_tin = pack_lengths("packed batches", "sample", true, c, in->n_tokens, B, in->max_tokens, meta.data());
-        const int max_v = pack_lengths("packed batches", "sample", false, c, in->n_regions, B, in->max_regions, meta.data() + B + 1);
-        meta[2 * (B + 1)] = meta[B];
-        meta[2 * (B + 1) + 1] = meta[2 * B + 1];
-        const int t16 = capacity16("packed batches", in->max_tokens, max_tin, task, "T");
-        const int v16 = capacity16("packed batches", in->max_regions, max_v, 0, "V");
-        if (maps) put_probs_meta(meta, B, out->attention_probs, packed_attn_layout(c, h->schedule, B, meta.data(), meta.data() + B + 1));
-        CUDA_CHECK(cudaSetDevice(h->opt.device));
-        Plan* pl = h->get_plan(B, t16 - task, v16, select & VB200_OUT_ALL, slot, vb200_engine::PACKED, maps);
-        cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-        h->forward_packed(*pl, *in, meta, st);
-        h->copy_outputs(*pl, *out, st, cudaMemcpyDeviceToDevice, meta[2 * (B + 1)], meta[2 * (B + 1) + 1]);
+        h->run_packed("vb200_forward_packed", vb200_engine::PACKED,
+                      {"sample", in->batch, in->n_tokens, in->max_tokens, in->n_regions, in->max_regions}, select, slot, out, cuda_stream,
+                      [&](Plan& pl, const PackedBatch& b, cudaStream_t st) { h->forward_packed(pl, *in, b, st); });
     });
 }
 
@@ -1857,46 +1874,26 @@ int vb200_forward_regions_packed(vb200_handle h, const vb200_packed_region_input
     return guard(h, [&] {
         const char* api = "vb200_forward_regions_packed";
         if (in == nullptr || out == nullptr) fail(VB200_ERR_INVALID, "inputs/outputs struct is NULL");
-        if (select & VB200_OUT_ATTENTION) fail(VB200_ERR_INVALID, "%s: the attention-probability output (VB200_OUT_ATTENTION) is not supported", api);
-        if (h->x3) fail(VB200_ERR_INVALID, "%s: packed batches are not supported in split_fp32 (fp32x) mode", api);
-        const bool maps = (select & VB200_OUT_ATTENTION_PACKED) != 0;
-        if (maps && out->attention_probs == nullptr)
-            fail(VB200_ERR_INVALID, "%s: VB200_OUT_ATTENTION_PACKED needs vb200_outputs.attention_probs (NULL)", api);
-        const Config& c = h->cfg;
-        const int B = in->batch, task = c.task_tokens ? 1 : 0;
-        if (B < 1) fail(VB200_ERR_INVALID, "%s: batch must be positive", api);
-        if (in->max_tokens < 0) fail(VB200_ERR_INVALID, "%s: negative capacity max_tokens %d", api, in->max_tokens);
-        if (in->max_boxes < 0) fail(VB200_ERR_INVALID, "%s: negative capacity max_boxes %d", api, in->max_boxes);
+        const int task = h->cfg.task_tokens ? 1 : 0;
         if (!in->n_tokens || !in->n_boxes || !in->question || !in->segment_ids || !in->box_features || !in->boxes || !in->image_wh ||
             (task && !in->task_tokens))
             fail(VB200_ERR_INVALID, "vb200_packed_region_inputs has a NULL required pointer");
+        if (in->max_boxes < 0) fail(VB200_ERR_INVALID, "%s: negative capacity max_boxes %d", api, in->max_boxes);
         if (in->max_boxes > 255) fail(VB200_ERR_INVALID, "%s: capacity max_boxes %d above 255 (V = boxes + 1 <= 256)", api, in->max_boxes);
-        // regions per image = boxes + the global mean row; these checks name the caller's fields before pack_lengths sees V_i / T_i
-        std::vector<int32_t> nv(B);
-        for (int i = 0; i < B; ++i) {
+        // regions per image = boxes + the global mean row; these checks name the caller's fields before pack_batch sees V_i / T_i
+        std::vector<int32_t> nv;
+        for (int i = 0; i < in->batch; ++i) {
             const int n = in->n_boxes[i], t = in->n_tokens[i];
             if (n < 1) fail(VB200_ERR_INVALID, "%s: image %d has n_boxes %d (must be >= 1)", api, i, n);
             if (in->max_boxes > 0 && n > in->max_boxes)
                 fail(VB200_ERR_INVALID, "%s: image %d has n_boxes %d, above the capacity max_boxes %d", api, i, n, in->max_boxes);
             if (n + 1 > 256) fail(VB200_ERR_INVALID, "%s: image %d has n_boxes %d (V = n_boxes + 1 must be <= 256)", api, i, n);
             if (t + task > 256) fail(VB200_ERR_INVALID, "%s: image %d has n_tokens %d (T = n_tokens + 1 must be <= 256)", api, i, t);
-            nv[i] = n + 1;
+            nv.push_back(n + 1);
         }
-        const int cap_v = in->max_boxes > 0 ? in->max_boxes + 1 : 0;
-        // meta = text row offsets [B + 1] | image row offsets [B + 1] | text rows | image rows (the plan's d_meta layout)
-        std::vector<int> meta(2 * (static_cast<size_t>(B) + 1) + 2, 0);
-        const int max_tin = pack_lengths(api, "image", true, c, in->n_tokens, B, in->max_tokens, meta.data());
-        const int max_v = pack_lengths(api, "image", false, c, nv.data(), B, cap_v, meta.data() + B + 1);
-        meta[2 * (B + 1)] = meta[B];
-        meta[2 * (B + 1) + 1] = meta[2 * B + 1];
-        const int t16 = capacity16(api, in->max_tokens, max_tin, task, "T");
-        const int v16 = capacity16(api, cap_v, max_v, 0, "V");
-        if (maps) put_probs_meta(meta, B, out->attention_probs, packed_attn_layout(c, h->schedule, B, meta.data(), meta.data() + B + 1));
-        CUDA_CHECK(cudaSetDevice(h->opt.device));
-        Plan* pl = h->get_plan(B, t16 - task, v16, select & VB200_OUT_ALL, slot, vb200_engine::PACKED, maps);
-        cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-        h->forward_regions_packed(*pl, *in, meta, st);
-        h->copy_outputs(*pl, *out, st, cudaMemcpyDeviceToDevice, meta[2 * (B + 1)], meta[2 * (B + 1) + 1]);
+        h->run_packed(api, vb200_engine::PACKED,
+                      {"image", in->batch, in->n_tokens, in->max_tokens, nv.data(), in->max_boxes > 0 ? in->max_boxes + 1 : 0}, select, slot,
+                      out, cuda_stream, [&](Plan& pl, const PackedBatch& b, cudaStream_t st) { h->forward_regions_packed(pl, *in, b, st); });
     });
 }
 
@@ -1922,7 +1919,10 @@ int vb200_encode_text(vb200_handle h, int32_t n, int32_t n_tokens, const int64_t
     if (h == nullptr) return VB200_ERR_INVALID;
     return guard(h, [&] {
         CUDA_CHECK(cudaSetDevice(h->opt.device));
-        h->encode_text(n, n_tokens, question, segment_ids, input_mask, task_tokens, state_f32, state_16, state_mask,
+        if (!question || !segment_ids || !input_mask || (h->cfg.task_tokens && !task_tokens) || !state_f32 || !state_16 || !state_mask)
+            fail(VB200_ERR_INVALID, "vb200_encode_text: NULL pointer");
+        Plan& pl = *h->get_plan(n, n_tokens, 1, 0, 0, vb200_engine::TEXT_PREFIX);
+        h->encode_text(pl, question, segment_ids, input_mask, task_tokens, pl.B * pl.T, state_f32, state_16, state_mask,
                        static_cast<cudaStream_t>(cuda_stream));
     });
 }
@@ -1932,7 +1932,10 @@ int vb200_encode_image(vb200_handle h, int32_t n, int32_t n_regions, const float
     if (h == nullptr) return VB200_ERR_INVALID;
     return guard(h, [&] {
         CUDA_CHECK(cudaSetDevice(h->opt.device));
-        h->encode_image(n, n_regions, features, spatials, image_mask, state_f32, state_16, state_mask,
+        if (!features || !spatials || !image_mask || !state_f32 || !state_16 || !state_mask)
+            fail(VB200_ERR_INVALID, "vb200_encode_image: NULL pointer");
+        Plan& pl = *h->get_plan(n, 1, n_regions, 0, 0, vb200_engine::IMAGE_PREFIX);
+        h->encode_image(pl, features, spatials, image_mask, pl.B * pl.V, state_f32, state_16, state_mask,
                         static_cast<cudaStream_t>(cuda_stream));
     });
 }
@@ -1961,20 +1964,12 @@ int vb200_encode_text_packed(vb200_handle h, int32_t n, int32_t max_tokens, cons
     if (h == nullptr) return VB200_ERR_INVALID;
     return guard(h, [&] {
         const char* api = "vb200_encode_text_packed";
-        const Config& c = h->cfg;
-        const int task = c.task_tokens ? 1 : 0;
-        if (h->x3) fail(VB200_ERR_INVALID, "%s: packed retrieval is not supported in split_fp32 (fp32x) mode", api);
-        if (n < 1) fail(VB200_ERR_INVALID, "%s: n must be positive", api);
-        if (max_tokens < 0) fail(VB200_ERR_INVALID, "%s: negative capacity", api);
-        if (!n_tokens || !question || !segment_ids || (task && !task_tokens) || !state_f32 || !state_16)
+        if (!n_tokens || !question || !segment_ids || (h->cfg.task_tokens && !task_tokens) || !state_f32 || !state_16)
             fail(VB200_ERR_INVALID, "%s: NULL pointer", api);
-        std::vector<int> meta(2 * (static_cast<size_t>(n) + 1) + 2, 0);
-        const int max_tin = pack_lengths(api, "caption", true, c, n_tokens, n, max_tokens, meta.data());
-        meta[2 * (n + 1)] = meta[n];
-        const int t16 = capacity16(api, max_tokens, max_tin, task, "T");
-        CUDA_CHECK(cudaSetDevice(h->opt.device));
-        Plan* pl = h->get_plan(n, t16 - task, 1, 0, 0, vb200_engine::PACKED_TEXT_PREFIX);
-        h->encode_text_packed(*pl, meta, question, segment_ids, task_tokens, state_f32, state_16, static_cast<cudaStream_t>(cuda_stream));
+        h->run_packed(api, vb200_engine::PACKED_TEXT_PREFIX, {"caption", n, n_tokens, max_tokens, nullptr, 0}, 0, 0, nullptr, cuda_stream,
+                      [&](Plan& pl, const PackedBatch& b, cudaStream_t st) {
+                          h->encode_text(pl, question, segment_ids, nullptr, task_tokens, b.rows_t(), state_f32, state_16, nullptr, st);
+                      });
     });
 }
 
@@ -1983,17 +1978,11 @@ int vb200_encode_image_packed(vb200_handle h, int32_t n, int32_t max_regions, co
     if (h == nullptr) return VB200_ERR_INVALID;
     return guard(h, [&] {
         const char* api = "vb200_encode_image_packed";
-        if (h->x3) fail(VB200_ERR_INVALID, "%s: packed retrieval is not supported in split_fp32 (fp32x) mode", api);
-        if (n < 1) fail(VB200_ERR_INVALID, "%s: n must be positive", api);
-        if (max_regions < 0) fail(VB200_ERR_INVALID, "%s: negative capacity", api);
         if (!n_regions || !features || !spatials || !state_f32 || !state_16) fail(VB200_ERR_INVALID, "%s: NULL pointer", api);
-        std::vector<int> meta(2 * (static_cast<size_t>(n) + 1) + 2, 0);
-        const int max_v = pack_lengths(api, "image", false, h->cfg, n_regions, n, max_regions, meta.data() + n + 1);
-        meta[2 * (n + 1) + 1] = meta[2 * n + 1];
-        const int v16 = capacity16(api, max_regions, max_v, 0, "V");
-        CUDA_CHECK(cudaSetDevice(h->opt.device));
-        Plan* pl = h->get_plan(n, 1, v16, 0, 0, vb200_engine::PACKED_IMAGE_PREFIX);
-        h->encode_image_packed(*pl, meta, features, spatials, state_f32, state_16, static_cast<cudaStream_t>(cuda_stream));
+        h->run_packed(api, vb200_engine::PACKED_IMAGE_PREFIX, {"image", n, nullptr, 0, n_regions, max_regions}, 0, 0, nullptr, cuda_stream,
+                      [&](Plan& pl, const PackedBatch& b, cudaStream_t st) {
+                          h->encode_image(pl, features, spatials, nullptr, b.rows_v(), state_f32, state_16, nullptr, st);
+                      });
     });
 }
 
@@ -2003,13 +1992,6 @@ int vb200_forward_cached_packed(vb200_handle h, const vb200_packed_pairs* in, co
     return guard(h, [&] {
         const char* api = "vb200_forward_cached_packed";
         if (in == nullptr || out == nullptr) fail(VB200_ERR_INVALID, "inputs/outputs struct is NULL");
-        if (select & VB200_OUT_ATTENTION) fail(VB200_ERR_INVALID, "%s: the attention-probability output (VB200_OUT_ATTENTION) is not supported", api);
-        reject_packed_attention(select, api);
-        if (h->x3) fail(VB200_ERR_INVALID, "%s: packed retrieval is not supported in split_fp32 (fp32x) mode", api);
-        const Config& c = h->cfg;
-        const int B = in->batch, task = c.task_tokens ? 1 : 0;
-        if (B < 1) fail(VB200_ERR_INVALID, "%s: batch must be positive", api);
-        if (in->max_tokens < 0 || in->max_regions < 0) fail(VB200_ERR_INVALID, "%s: negative capacity", api);
         if (in->n_text < 1 || in->n_image < 1) fail(VB200_ERR_INVALID, "%s: n_text and n_image must be positive", api);
         if (!in->text_index || !in->image_index || !in->text_offsets || !in->image_offsets || !in->text_f32 || !in->text_16 ||
             !in->image_f32 || !in->image_16)
@@ -2022,31 +2004,21 @@ int vb200_forward_cached_packed(vb200_handle h, const vb200_packed_pairs* in, co
         };
         check_offsets(in->text_offsets, in->n_text, "text");
         check_offsets(in->image_offsets, in->n_image, "image");
-        // meta = pair text row offsets [B + 1] | pair image row offsets [B + 1] | text rows | image rows | source text rows [B] |
-        // source image rows [B] (the plan's d_meta layout)
-        std::vector<int> meta(2 * (static_cast<size_t>(B) + 1) + 2 + 2 * static_cast<size_t>(B), 0);
-        int* src_t = meta.data() + 2 * (B + 1) + 2;
-        int* src_v = src_t + B;
-        std::vector<int32_t> tin(B), nv(B);
-        for (int b = 0; b < B; ++b) {
+        // each pair's lengths and first rows in the cached states
+        const int task = h->cfg.task_tokens ? 1 : 0;
+        std::vector<int32_t> tin, nv, src_t, src_v;
+        for (int b = 0; b < in->batch; ++b) {
             const int ti = in->text_index[b], vi = in->image_index[b];
             if (ti < 0 || ti >= in->n_text) fail(VB200_ERR_INVALID, "%s: pair %d: text_index %d outside [0, %d)", api, b, ti, in->n_text);
             if (vi < 0 || vi >= in->n_image) fail(VB200_ERR_INVALID, "%s: pair %d: image_index %d outside [0, %d)", api, b, vi, in->n_image);
-            tin[b] = in->text_offsets[ti + 1] - in->text_offsets[ti] - task;
-            nv[b] = in->image_offsets[vi + 1] - in->image_offsets[vi];
-            src_t[b] = in->text_offsets[ti];
-            src_v[b] = in->image_offsets[vi];
+            tin.push_back(in->text_offsets[ti + 1] - in->text_offsets[ti] - task);
+            nv.push_back(in->image_offsets[vi + 1] - in->image_offsets[vi]);
+            src_t.push_back(in->text_offsets[ti]);
+            src_v.push_back(in->image_offsets[vi]);
         }
-        const int max_tin = pack_lengths(api, "pair", true, c, tin.data(), B, in->max_tokens, meta.data());
-        const int max_v = pack_lengths(api, "pair", false, c, nv.data(), B, in->max_regions, meta.data() + B + 1);
-        meta[2 * (B + 1)] = meta[B];
-        meta[2 * (B + 1) + 1] = meta[2 * B + 1];
-        const int t16 = capacity16(api, in->max_tokens, max_tin, task, "T"), v16 = capacity16(api, in->max_regions, max_v, 0, "V");
-        CUDA_CHECK(cudaSetDevice(h->opt.device));
-        Plan* pl = h->get_plan(B, t16 - task, v16, select & VB200_OUT_ALL, slot, vb200_engine::PACKED_SUFFIX, false);
-        cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-        h->forward_cached_packed(*pl, *in, meta, st);
-        h->copy_outputs(*pl, *out, st, cudaMemcpyDeviceToDevice, meta[2 * (B + 1)], meta[2 * (B + 1) + 1]);
+        h->run_packed(api, vb200_engine::PACKED_SUFFIX,
+                      {"pair", in->batch, tin.data(), in->max_tokens, nv.data(), in->max_regions, src_t.data(), src_v.data()}, select, slot,
+                      out, cuda_stream, [&](Plan& pl, const PackedBatch& b, cudaStream_t st) { h->forward_cached_packed(pl, *in, b, st); });
     });
 }
 
@@ -2111,12 +2083,9 @@ int vb200_attention_layout_packed(vb200_handle h, int32_t batch, const int32_t* 
     return guard(h, [&] {
         // from the lengths and the layer schedule alone (no plan is built), validated as the packed forwards validate them
         const char* api = "vb200_attention_layout_packed";
-        if (batch < 1) fail(VB200_ERR_INVALID, "%s: batch must be positive", api);
         if (!n_tokens || !n_regions) fail(VB200_ERR_INVALID, "%s: NULL length array", api);
-        std::vector<int> offs(2 * (static_cast<size_t>(batch) + 1), 0);
-        pack_lengths(api, "sample", true, h->cfg, n_tokens, batch, 0, offs.data());
-        pack_lengths(api, "sample", false, h->cfg, n_regions, batch, 0, offs.data() + batch + 1);
-        const PackedAttnLayout l = packed_attn_layout(h->cfg, h->schedule, batch, offs.data(), offs.data() + batch + 1);
+        const PackedBatch b = pack_batch(api, h->cfg, h->schedule, {"sample", batch, n_tokens, 0, n_regions, 0}, nullptr);
+        const PackedAttnLayout l = packed_attn_layout(h->cfg, h->schedule, batch, b.offs_t(), b.offs_v());
         const int n = static_cast<int>(l.heads.size());
         for (int e = 0; e < n && e < max_entries; ++e) {
             if (dims) { dims[2 * e] = l.heads[e]; dims[2 * e + 1] = l.kind[e]; }
