@@ -130,10 +130,9 @@ typedef struct {
                                       matching A/B formats).  default on: IEEE fp16 (11-bit significand; activations
                                       are LayerNorm-bounded, converts saturate); -1: bf16.  Accumulation, residual stream,
                                       LayerNorm, softmax and logits are fp32 either way. */
-    int32_t fused_layernorm;       /* default off: LayerNorm(dense(x) + residual) runs as GEMM (fp32 out) + an L2-resident row
-                                      kernel; 1: cluster-LayerNorm GEMM epilogue (N tiles of a row-panel form a thread-block
-                                      cluster and exchange (mean, M2) through distributed shared memory).  Both are
-                                      parity-tested. */
+    int32_t fused_layernorm;       /* reserved, must be 0 or negative (was the cluster-LayerNorm GEMM epilogue, which is removed;
+                                      vb200_create returns VB200_ERR_INVALID for a positive value).  LayerNorm(dense(x) +
+                                      residual) always runs as GEMM (fp32 out) + an L2-resident row kernel. */
     int32_t split_fp32;            /* 1: fp32-parity mode ("fp32x").  Every GEMM operand travels as TWO fp16 numbers (hi = fp16(x),
                                       lo = fp16(x - hi), 22 significand bits); operand buffers hold hi | lo | hi (weights hi | hi |
                                       lo) per 64 columns, so an ordinary wgmma GEMM over K' = 3K adds hi.hi + lo.hi + hi.lo in its
@@ -201,7 +200,7 @@ int vb200_timeline(vb200_handle h, int32_t batch, int32_t n_tokens, int32_t n_re
                    int32_t* n_ops, int32_t* dims, int64_t* stamps);
 /* Per-launch device time of one forward of this shape (after at least one vb200_forward of it): every kernel of the plan is
  * captured 8x into its own CUDA graph and replayed `iters` times between two CUDA events (no host launch gaps).  kinds: 0 GEMM, 1 self-attention,
- * 2 co-attention, 3 narrow head, 4 LayerNorm; dims[4*i..] = {M, N, K, act|16*fusedLN} for GEMMs.  Profiling aid for bench.py. */
+ * 2 co-attention, 3 narrow head, 4 LayerNorm; dims[4*i..] = {M, N, K, act} for GEMMs.  Profiling aid for bench.py. */
 int vb200_profile_ops(vb200_handle h, int32_t batch, int32_t n_tokens, int32_t n_regions, uint32_t select, int32_t iters,
                       int32_t max_ops, int32_t* n_ops, int32_t* kinds, double* ms, double* flops, int32_t* dims);
 
@@ -422,20 +421,21 @@ int vb200_decode_answers_host(vb200_handle h, const vb200_decode_msg* msgs /* HO
                               void* cuda_stream);
 
 /* ---- Kernel-level entry points (device pointers), used by the parity tests and the roofline bench.  ---- */
-/* y = epilogue(x[M,K] (16-bit) . w[N,K]^T (16-bit)); act: 0 none, 1 GELU(erf), 2 ReLU; LayerNorm applied when gamma != NULL.
+/* y = act(x[M,K] (16-bit) . w[N,K]^T (16-bit) + bias); act: 0 none, 1 GELU(erf), 2 ReLU.  residual, gamma and beta are reserved
+ * and must be NULL (VB200_ERR_INVALID otherwise; LayerNorm is vb200_layernorm on the fp32 output); ld_res and eps are ignored.
  * act_fp16 != 0: x, w and the 16-bit output y are fp16, else bf16 (parameter names keep the historical _bf16 suffix).
  * act 3 = GELU with the 1.5e-7 erf (fp32-parity mode).  variant 0: persistent kernel (gemm_persistent.cuh, what the engine
  * uses); 2, 3 and 4 (names of Blackwell kernel configurations) select the persistent kernel: 2 and 3 with the plain 128-wide tile,
  * 4 with the plain 128- or 64-wide one.  variant 5: the ping-pong kernel (gemm_pingpong.cuh, what the engine uses for the plain
- * GEMMs it supports): no residual / LayerNorm, act 0-2, N a multiple of block_n 64 or 128, outputs the TMA can store (16-byte aligned
- * base and row stride); VB200_ERR_INVALID otherwise.  Plain (non-LayerNorm) tiles are 64, 128 or 192 columns wide; block_n 256 runs
+ * GEMMs it supports): act 0-2, N a multiple of block_n 64 or 128, outputs the TMA can store (16-byte aligned
+ * base and row stride); VB200_ERR_INVALID otherwise.  Tiles are 64, 128 or 192 columns wide; block_n 256 runs
  * as 128-wide tiles.  Every variant and every width gives the same bits.
  * timing: NULL, or a device buffer of 16 int64 per CTA that receives clock64() / %globaltimer stamps (profiling aid). */
 int vb200_linear(const void* x_bf16, int64_t ld_x, const void* w_bf16, int64_t ld_w, const float* bias,
                  const float* residual, int64_t ld_res, const float* gamma, const float* beta, float eps, int32_t act,
                  void* y_bf16, int64_t ld_y_bf16, float* y_f32, int64_t ld_y_f32, int64_t M, int64_t N, int64_t K,
                  int32_t block_n, int32_t use_pdl, int32_t act_fp16, int32_t variant, long long* timing, void* cuda_stream);
-/* The plain GEMM (no residual / LayerNorm) with a device row count: rows >= min(*m_rows, M) are neither loaded nor computed -- the
+/* The GEMM of vb200_linear with a device row count: rows >= min(*m_rows, M) are neither loaded nor computed -- the
  * 128-row tiles that start at or past it are skipped, what packed plans rely on (m_rows: device int32).  Runs on the kernel the
  * engine would pick: ping-pong (variant 5) where it applies unless VB200_GEMM=coop, else variant 0. */
 int vb200_linear_rows(const void* x16, int64_t ld_x, const void* w16, int64_t ld_w, const float* bias, int32_t act, void* y16,

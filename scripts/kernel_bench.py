@@ -65,43 +65,40 @@ def main():
     f16 = 1 if a.act == "fp16" else 0
     cur = lambda: torch.cuda.current_stream().cuda_stream      # the capture stream while a graph is being recorded
     g = torch.Generator(device="cuda").manual_seed(0)
-    # name, M, N, K, act, residual+LN, block_n
+    # name, M, N, K, act, fp32 output only (the GEMMs a row LayerNorm follows), block_n
     gemms = [
-        ("text_qkv", Mt, 2304, 768, 0, False, 0), ("text_attn_out_ln", Mt, 768, 768, 0, True, 0),
-        ("text_ffn_in_gelu", Mt, 3072, 768, 1, False, 0), ("text_ffn_out_ln", Mt, 768, 3072, 0, True, 0),
-        ("img_qkv", Mv, 3072, 1024, 0, False, 0), ("img_attn_out_ln", Mv, 1024, 1024, 0, True, 0),
-        ("img_ffn_in_gelu", Mv, 1024, 1024, 1, False, 0), ("img_embed_ln", Mv, 1024, 2112, 0, True, 0),
-        ("co_txt_qkv", Mt, 3072, 768, 0, False, 0), ("co_dense2_ln", Mt, 768, 1024, 0, True, 0),
+        ("text_qkv", Mt, 2304, 768, 0, False, 0), ("text_attn_out_f32", Mt, 768, 768, 0, True, 0),
+        ("text_ffn_in_gelu", Mt, 3072, 768, 1, False, 0), ("text_ffn_out_f32", Mt, 768, 3072, 0, True, 0),
+        ("img_qkv", Mv, 3072, 1024, 0, False, 0), ("img_attn_out_f32", Mv, 1024, 1024, 0, True, 0),
+        ("img_ffn_in_gelu", Mv, 1024, 1024, 1, False, 0), ("img_embed_f32", Mv, 1024, 2112, 0, True, 0),
+        ("co_txt_qkv", Mt, 3072, 768, 0, False, 0), ("co_dense2_f32", Mt, 768, 1024, 0, True, 0),
         ("text_ffn_in_gelu_bn256", Mt, 3072, 768, 1, False, 256), ("pool_t", B, 1024, 768, 2, False, 0),
-        ("vqa_fc0_gelu_ln", B, 2048, 1024, 1, True, 0), ("vqa_fc3", B, 3129, 2048, 0, False, 0),
+        ("vqa_fc0_gelu_f32", B, 2048, 1024, 1, True, 0), ("vqa_fc3", B, 3129, 2048, 0, False, 0),
         ("plain_text_ffn_out", Mt, 768, 3072, 0, False, 0), ("plain_img_out", Mv, 1024, 1024, 0, False, 0),
         ("plain_text_attn_out", Mt, 768, 768, 0, False, 0),
     ]
     res = []
-    for name, M, N, K, actf, ln, bn in gemms:
+    for name, M, N, K, actf, f32, bn in gemms:
         if only and not any(o == name or (o.endswith("*") and o[:-1] in name) for o in only):
             continue
-        if a.bn and not ln:
+        if a.bn:
             bn = a.bn
         sets = []
         for _ in range(a.sets):
             x = torch.randn(M, K, generator=g, device="cuda").to(act)
             w = (torch.randn(N, K, generator=g, device="cuda") / math.sqrt(K)).to(act)
             b = torch.randn(N, generator=g, device="cuda")
-            r = torch.randn(M, N, generator=g, device="cuda") if ln else None
-            ga = torch.ones(N, device="cuda") if ln else None
-            be = torch.zeros(N, device="cuda") if ln else None
             ldf = (N + 3) // 4 * 4
-            yb = torch.empty(M, N, dtype=act, device="cuda") if N % 8 == 0 else None
-            yf = torch.empty(M, ldf, device="cuda") if (ln or N % 8) else None
-            sets.append((x, w, b, r, ga, be, yb, yf, ldf))
+            yb = torch.empty(M, N, dtype=act, device="cuda") if N % 8 == 0 and not f32 else None
+            yf = torch.empty(M, ldf, device="cuda") if (f32 or N % 8) else None
+            sets.append((x, w, b, yb, yf, ldf))
 
         def run(i):
-            x, w, b, r, ga, be, yb, yf, ldf = sets[i % a.sets]
-            rc = lib.vb200_linear(ptr(x), K, ptr(w), K, ptr(b), ptr(r), N if ln else 0, ptr(ga), ptr(be), 1e-12, actf,
+            x, w, b, yb, yf, ldf = sets[i % a.sets]
+            rc = lib.vb200_linear(ptr(x), K, ptr(w), K, ptr(b), None, 0, None, None, 1e-12, actf,
                                   ptr(yb), N, ptr(yf), ldf, M, N, K, bn, 0, f16, variant, None, C.c_void_p(cur()))
             L.check(rc, None)
-        plain_pp = not ln and N % (bn if bn in (64, 128) else 128) == 0 and bn != 256
+        plain_pp = N % (bn if bn in (64, 128) else 128) == 0 and bn != 256
         for variant, dbg in [(v, d) for v in variants for d in debug_modes if v == 0 or plain_pp]:
             os.environ["VB200_DEBUG"] = str(dbg)
             us = time_graph(run, a.reps)
@@ -110,15 +107,15 @@ def main():
             print(json.dumps(res[-1]), flush=True)
             if a.stamps:
                 tb = torch.zeros(16 * 4096, dtype=torch.int64, device="cuda")
-                x, w, b, r, ga, be, yb, yf, ldf = sets[0]
-                rc = lib.vb200_linear(ptr(x), K, ptr(w), K, ptr(b), ptr(r), N if ln else 0, ptr(ga), ptr(be), 1e-12, actf,
+                x, w, b, yb, yf, ldf = sets[0]
+                rc = lib.vb200_linear(ptr(x), K, ptr(w), K, ptr(b), None, 0, None, None, 1e-12, actf,
                                       ptr(yb), N, ptr(yf), ldf, M, N, K, bn, 0, f16, variant, ptr(tb), C.c_void_p(cur()))
                 L.check(rc, None)
                 torch.cuda.synchronize()
                 t = tb.view(-1, 16).cpu()
                 t = t[t[:, 0] != 0]
                 d = (t - t[:, :1]).double()
-                names = ["entry", "setup", "first_kblock", "mma_issued", "acc_ready", "epi_pass1", "ln_exchange", "epi_done",
+                names = ["entry", "setup", "first_kblock", "mma_issued", "acc_ready", "epi_pass1", "producer_waited", "epi_done",
                          "c0_ld", "c0_res", "c0_math", "c0_store", "c1_ld", "c1_res", "c1_math", "c1_store"]
                 print("   stamps (SM cycles since CTA entry, median over %d CTAs): " % len(t) +
                       ", ".join(f"{n}={int(d[:, i].median())}" for i, n in enumerate(names[:8]) if (t[:, i] != 0).any()), flush=True)

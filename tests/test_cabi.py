@@ -42,7 +42,7 @@ def test_ctypes_structs_match_header_layout():
     assert C.sizeof(L.RegionInputs) == 16 + 9 * 8
 
 
-def _create(cfg, sd, ln_fold=0, **opt):
+def _create(cfg, sd, ln_fold=0, fused_layernorm=0, split_fp32=0, **opt):
     m = vb.VILBertForVLTasks.from_pretrained(sd, config=cfg, num_labels=opt.pop("num_labels", 40), **opt)
     lib = L.load()
     names = [k.encode() for k in m._sd]
@@ -55,6 +55,8 @@ def _create(cfg, sd, ln_fold=0, **opt):
     o.num_labels = m.num_labels
     o.strict = 1 if m._opts["strict"] else -1
     o.ln_fold = ln_fold
+    o.fused_layernorm = fused_layernorm
+    o.split_fp32 = split_fp32
     h = C.c_void_p()
     rc = lib.vb200_create(m._config_json(), len(m._sd), arr, C.byref(o), C.byref(h))
     msg = lib.vb200_last_error(None).decode()
@@ -116,6 +118,48 @@ def test_reserved_ln_fold_option_rejected():
     sd = S.synthetic_state_dict(cfg, num_labels=40, gqa_labels=24, seed=1)
     rc, msg = _create(cfg, sd, ln_fold=1)
     assert rc == -1 and "LayerNorm fold was removed" in msg, (rc, msg)
+
+
+@pytest.mark.parametrize("split_fp32", [0, 1])
+def test_reserved_fused_layernorm_option_rejected(split_fp32):
+    """vb200_options::fused_layernorm is reserved since the cluster-LayerNorm GEMM epilogue was removed: a positive value is
+    refused before the checkpoint audit, so with or without a device, and in fp32-parity mode too."""
+    cfg = _tiny_cfg()
+    sd = S.synthetic_state_dict(cfg, num_labels=40, gqa_labels=24, seed=1)
+    rc, msg = _create(cfg, sd, fused_layernorm=1, split_fp32=split_fp32)
+    assert rc == -1 and "cluster-LayerNorm GEMM epilogue was removed" in msg, (rc, msg)
+
+
+@pytest.mark.parametrize("value", [0, -1])
+def test_fused_layernorm_off_values_accepted(value):
+    """0 and negative fused_layernorm values ("off" in the tri-state convention) get past the option check: the checkpoint
+    audit, which needs no device, then reports the missing key."""
+    cfg = _tiny_cfg()
+    sd = S.synthetic_state_dict(cfg, num_labels=40, gqa_labels=24, seed=1)
+    del sd["bert.encoder.c_layer.3.biattention.query2.weight"]
+    rc, msg = _create(cfg, sd, fused_layernorm=value)
+    assert rc == -3 and "c_layer.3.biattention.query2.weight" in msg, (rc, msg)
+
+
+@pytest.mark.parametrize("arg", ["residual", "gamma", "beta"])
+def test_linear_rejects_layernorm_arguments(arg):
+    """vb200_linear has no LayerNorm epilogue: a non-null residual, gamma or beta is an invalid argument, refused before any
+    CUDA call (so also without a device)."""
+    lib = L.load()
+    buf = torch.zeros(64)
+    p = C.c_void_p(buf.data_ptr())
+    ptrs = {k: (p if k == arg else None) for k in ("residual", "gamma", "beta")}
+    rc = lib.vb200_linear(p, 64, p, 64, None, ptrs["residual"], 64, ptrs["gamma"], ptrs["beta"], 1e-12, 0,
+                          None, 0, p, 64, 1, 8, 64, 0, 0, 0, 0, None, None)
+    assert rc == -1
+    assert "residual, gamma and beta must be NULL" in lib.vb200_last_error(None).decode()
+
+
+def test_model_rejects_fused_layernorm():
+    cfg = _tiny_cfg()
+    sd = S.synthetic_state_dict(cfg, num_labels=40, gqa_labels=24, seed=1)
+    with pytest.raises(ValueError, match="cluster-LayerNorm GEMM epilogue was removed"):
+        vb.VILBertForVLTasks.from_pretrained(sd, config=cfg, num_labels=40, fused_layernorm=True)
 
 
 def test_checkpoint_legacy_names_accepted():

@@ -144,36 +144,6 @@ def test_tiny_model_pdl(tiny_oracle, tiny_engines):
         other.close()
 
 
-def test_tiny_model_fused_layernorm(tiny_oracle, tiny_engines, parity_log):
-    """The cluster-LayerNorm GEMM epilogue (fused_layernorm=True) and the default GEMM + row-LayerNorm split agree to
-    fp32 round-off of the statistics (different summation orders, same 16-bit rounding afterwards)."""
-    dev = [t.cuda() for t in _tiny_inputs(tiny_oracle, 3, 20, 12, 9, pad=2)]
-    fused = _engine(tiny_oracle, fused_layernorm=True)
-    a = tiny_engines["fp16"](*dev, compute_pretraining_heads=True)
-    b = fused(*dev, compute_pretraining_heads=True)
-    torch.cuda.synchronize()
-    for name, x, y in zip(NAMES, a[:9], b[:9]):
-        small = x.abs() < 1000
-        d = float((x - y).abs()[small].max())
-        parity_log(test="fused_vs_split_layernorm", output=name, max_abs_diff=d)
-        assert d < 5e-3, (name, d)
-    fused.close()
-
-
-def test_full_model_fused_layernorm(full_oracle, parity_log):
-    from oracle import vilbert_ref as R
-    inp = R.make_inputs(2, 30, 36, seed=1236)
-    ref = full_oracle(*inp, compute_pretraining_heads=False)
-    fused = _engine(full_oracle, fused_layernorm=True)
-    out = fused(*[t.cuda() for t in inp])
-    torch.cuda.synchronize()
-    e = _errs(ref, out)
-    for name, (err, std) in e.items():
-        parity_log(test="full_fused_layernorm", output=name, err_vs_fp32=err, ref_std=std)
-        assert err < TOL, (name, err)
-    fused.close()
-
-
 def test_tiny_model_host_api(tiny_oracle, tiny_engines):
     """vb200_forward_host (pinned host buffers in/out) == vb200_forward (device pointers)."""
     from vilbert_b200 import _lib as L

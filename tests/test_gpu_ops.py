@@ -29,8 +29,7 @@ def variant(request):
     VARIANT = 0
 
 
-def run_linear(x, w, bias=None, res=None, gamma=None, beta=None, act=0, block_n=0, want_bf16=True, want_f32=True,
-               ld_f32=None, pdl=0):
+def run_linear(x, w, bias=None, act=0, block_n=0, want_bf16=True, want_f32=True, ld_f32=None, pdl=0):
     """x, w: both fp16 or both bf16 (wgmma needs matching operand formats); same format for the 16-bit output."""
     L, lib = _lib()
     M, K = x.shape
@@ -41,28 +40,21 @@ def run_linear(x, w, bias=None, res=None, gamma=None, beta=None, act=0, block_n=
     ldf = ld_f32 or N
     yf = torch.full((M, ldf), float("nan"), dtype=torch.float32, device=dev) if want_f32 else None
     stream = torch.cuda.current_stream().cuda_stream
-    rc = lib.vb200_linear(_ptr(x), x.stride(0), _ptr(w), w.stride(0), _ptr(bias), _ptr(res),
-                          res.stride(0) if res is not None else 0, _ptr(gamma), _ptr(beta), 1e-12, act,
+    rc = lib.vb200_linear(_ptr(x), x.stride(0), _ptr(w), w.stride(0), _ptr(bias), None, 0, None, None, 1e-12, act,
                           _ptr(yb), N, _ptr(yf), ldf, M, N, K, block_n, pdl, f16, VARIANT, None, C.c_void_p(stream))
     L.check(rc, None)
     torch.cuda.synchronize()
     return yb, (yf[:, :N] if yf is not None else None)
 
 
-def ref_linear(x, w, bias=None, res=None, gamma=None, beta=None, act=0):
+def ref_linear(x, w, bias=None, act=0):
     y = x.double() @ w.double().t()
     if bias is not None:
         y = y + bias.double()
-    if res is not None:
-        y = y + res.double()
     if act == 1:
         y = y * 0.5 * (1.0 + torch.erf(y / math.sqrt(2.0)))
     elif act == 2:
         y = torch.relu(y)
-    if gamma is not None:
-        u = y.mean(-1, keepdim=True)
-        s = (y - u).pow(2).mean(-1, keepdim=True)
-        y = (y - u) / torch.sqrt(s + 1e-12) * gamma.double() + beta.double()
     return y.float()
 
 
@@ -117,50 +109,6 @@ def test_linear_act(act, act_dt, variant, parity_log):
     err = (yf - ref).abs().max().item()
     parity_log(test="linear_act", act=act, max_abs_err=err)
     assert err < 2e-3
-
-
-@pytest.mark.parametrize("M,N,K,act", [
-    (128, 128, 128, 0),         # cluster of 1
-    (300, 256, 256, 0),         # cluster of 2 (tiny config)
-    (1984, 768, 768, 0),        # text attention-output at B=64: cluster of 6 (or 96 x 8)
-    (1984, 768, 3072, 0),       # text FFN-out
-    (2304, 1024, 2112, 0),      # image embedding: cluster of 8, K with zero tail
-    (64, 2048, 1024, 1),        # SimpleClassifier: GELU then LayerNorm over 2048 = 128 x 16
-    (5000, 1024, 512, 0),       # 40 M tiles: persistent clusters loop (accumulator + partial double-buffering)
-    (16000, 768, 256, 1),       # 125 M tiles over <= 24 clusters of 6
-])
-@pytest.mark.parametrize("act_dt", ACT)
-def test_linear_residual_layernorm(M, N, K, act, act_dt, variant, parity_log):
-    if variant == 2:
-        pytest.skip("variant 2 is the plain 128-wide tile, without the LayerNorm epilogue")
-    x, w, b, g = _mk(M, N, K, seed=2, act=act_dt)
-    res = torch.randn(M, N, generator=g, device="cuda")
-    gamma = 1.0 + 0.1 * torch.randn(N, generator=g, device="cuda")
-    beta = 0.1 * torch.randn(N, generator=g, device="cuda")
-    yb, yf = run_linear(x, w, b, res=res, gamma=gamma, beta=beta, act=act)
-    ref = ref_linear(x, w, b, res=res, gamma=gamma, beta=beta, act=act)
-    err = (yf - ref).abs().max().item()
-    parity_log(test="linear_res_ln", M=M, N=N, K=K, max_abs_err=err)
-    assert err < 2e-3
-    assert (yb.float() - ref).abs().max().item() < 5e-2
-
-
-def test_linear_inplace_residual():
-    """LN epilogue may write its fp32 output over the residual it read (the engine's ping-pong never needs it,
-    but the kernel contract allows it)."""
-    L, lib = _lib()
-    M, N, K = 256, 256, 128
-    x, w, b, g = _mk(M, N, K, seed=3)
-    res = torch.randn(M, N, generator=g, device="cuda")
-    gamma = torch.ones(N, device="cuda")
-    beta = torch.zeros(N, device="cuda")
-    ref = ref_linear(x, w, b, res=res, gamma=gamma, beta=beta)
-    buf = res.clone()
-    rc = lib.vb200_linear(_ptr(x), K, _ptr(w), K, _ptr(b), _ptr(buf), N, _ptr(gamma), _ptr(beta), 1e-12, 0,
-                          None, 0, _ptr(buf), N, M, N, K, 0, 0, 0, 0, None, C.c_void_p(torch.cuda.current_stream().cuda_stream))
-    L.check(rc, None)
-    torch.cuda.synchronize()
-    assert (buf - ref).abs().max().item() < 2e-3
 
 
 def test_linear_pdl_chain():
@@ -238,7 +186,7 @@ def test_co_attention(B, T, V, heads, d, act_dt, parity_log):
 @pytest.mark.parametrize("act_dt", ACT)
 @pytest.mark.parametrize("M,N,with_res", [(1984, 768, True), (2304, 1024, True), (64, 2048, False), (37, 128, True), (5, 256, False)])
 def test_layernorm_row_kernel(M, N, with_res, act_dt, parity_log):
-    """vb200_layernorm: LayerNorm(y + residual) with fp32 and 16-bit outputs (the un-fused LayerNorm path)."""
+    """vb200_layernorm: LayerNorm(y + residual) with fp32 and 16-bit outputs (the LayerNorm after every residual GEMM)."""
     L, lib = _lib()
     g = torch.Generator(device="cuda").manual_seed(9)
     y = torch.randn(M, N, generator=g, device="cuda") * 3 + 0.5

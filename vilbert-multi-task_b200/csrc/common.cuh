@@ -1,4 +1,4 @@
-// sm_90a device primitives shared by the vilbert_b200 kernels: mbarrier, TMA, cluster/DSMEM helpers and small math
+// sm_90a device primitives shared by the vilbert_b200 kernels: mbarrier, TMA, programmatic dependent launch and small math
 // (the warpgroup MMA wrappers are in wgmma.cuh).  Raw PTX only (no CUTLASS dependency).
 #pragma once
 #include <cuda.h>
@@ -108,32 +108,6 @@ __device__ __forceinline__ void tma_store_commit_and_wait_read() {
 }
 // generic-proxy writes to shared memory -> visible to the async proxy (TMA) that is about to read them
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-
-// ------------------------------------------------------------------ cluster / DSMEM
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ uint32_t cluster_nctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {  // every thread of every CTA in the cluster
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// Read a float from the same shared-memory offset in CTA `rank` of this cluster.
-__device__ __forceinline__ float dsmem_ld_f32(const float* local_smem_ptr, uint32_t rank) {
-    uint32_t remote;
-    float v;
-    asm("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(local_smem_ptr)), "r"(rank));
-    // volatile (not hoisted above the cluster barrier, which clobbers memory) but no memory clobber of its own, so the
-    // loads from all peers are issued back to back instead of one round trip at a time
-    asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(remote));
-    return v;
-}
 
 // ------------------------------------------------------------------ programmatic dependent launch
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }

@@ -209,7 +209,7 @@ Config parse_config(const char* json) {
     for (int d : {c.hidden, c.v_hidden, c.bi_hidden, c.inter, c.v_inter})
         if (d % 128 != 0) fail(VB200_ERR_CONFIG, "hidden/intermediate sizes must be multiples of 128 (got %d)", d);
     if (c.hidden > 1024 || c.v_hidden > 1024 || c.bi_hidden > 1024)
-        fail(VB200_ERR_CONFIG, "hidden sizes above 1024 need a wider LayerNorm cluster than 8 CTAs");
+        fail(VB200_ERR_CONFIG, "hidden sizes above 1024 are not supported");
     if (c.v_feat % 8 != 0) fail(VB200_ERR_CONFIG, "v_feature_size must be a multiple of 8");
     return c;
 }
@@ -337,7 +337,7 @@ bool make_tmap_out(CUtensorMap* m, const void* base, int64_t rows, int64_t cols,
 // Decide whether a plain GEMM may use the TMA-store epilogue and build its output map (exactly one output, aligned).
 void setup_tma_store(CUtensorMap* tc, GemmEpilogue& e) {
     e.tma_store = 0;
-    if (e.split16 || e.gamma != nullptr) return;
+    if (e.split16) return;
     if (e.out_bf16 != nullptr && e.out_f32 == nullptr) {
         if (make_tmap_out(tc, e.out_bf16, e.M, e.N, e.ld_bf16, false, e.out_f16 != 0)) e.tma_store = 1;
     } else if (e.out_f32 != nullptr && e.out_bf16 == nullptr) {
@@ -366,7 +366,6 @@ struct Op {
     CUtensorMap tc32;              // ping-pong: the fp32 output
     GemmEpilogue ep;
     int block_n = 128;
-    bool ln = false;
     bool pingpong = false;         // launched as the ping-pong kernel (gemm_pingpong.cuh)
     // fp32 attention (attention_f32.cu): fp32-parity mode and the attention-probability output
     const void *f_q = nullptr, *f_k = nullptr, *f_v = nullptr;
@@ -382,7 +381,7 @@ struct Op {
     const float *mask_a = nullptr, *mask_b = nullptr;
     bf16 *ctx_a = nullptr, *ctx_b = nullptr;
     int ld_ctx_a = 0, ld_ctx_b = 0, B = 0, La = 0, Lb = 0, heads = 0, head_dim = 0;
-    // layernorm (un-fused): out = LN(ln_y + ln_res)
+    // layernorm: out = LN(ln_y + ln_res)
     const float *ln_y = nullptr, *ln_res = nullptr, *ln_g = nullptr, *ln_b = nullptr;
     float* ln_out_f = nullptr;
     bf16* ln_out_h = nullptr;
@@ -546,7 +545,7 @@ struct Plan {
     float *mask_t = nullptr, *mask_v = nullptr;
     float* t_f32[2]; bf16* t_b16[2];
     float* v_f32[2]; bf16* v_b16[2];
-    float* y_scratch[2] = {nullptr, nullptr};   // per-stream fp32 GEMM output feeding the un-fused LayerNorm kernel
+    float* y_scratch[2] = {nullptr, nullptr};   // per-stream fp32 GEMM output feeding the row LayerNorm kernel
     int t_cur = 0, v_cur = 0;
     std::vector<Op> ops;
     OutBuf outs[12];
@@ -601,7 +600,6 @@ struct vb200_engine {
     // VB200_PDL=off|full, use_pdl < 0 = off.
     bool tma_store_enabled = true;  // VB200_TMASTORE=0: every tile leaves through the register / LSU epilogue
     bool early_w = true;            // VB200_EARLYW=0: no weight loads ahead of griddepcontrol.wait
-    bool fused_ln = false;     // VB200_FUSED_LN=1: cluster-LayerNorm GEMM epilogue instead of GEMM(fp32) + row LayerNorm kernel
     int gemm_kernel = 1;       // default_gemm_kernel(): 1 = plain GEMMs the ping-pong kernel supports run on it, 0 = all on the cooperative one
     Arena weights;
     std::string last_error;
@@ -910,10 +908,8 @@ struct vb200_engine {
     }
 
     // ---------------------------------------------------------------- plan construction
-    // One nn.Linear (+ activation, + residual LayerNorm) -> one or two launch-list entries on `stream`.
-    //   fused_ln:  a single cluster-LayerNorm GEMM (epilogue normalises across the N tiles of a cluster)
-    //   default :  GEMM (+bias, +activation) writing fp32 to the stream's scratch, then the row LayerNorm kernel
-    //              (adds the residual).
+    // One nn.Linear (+ activation, + residual LayerNorm) -> one or two launch-list entries on `stream`: the GEMM (+bias,
+    // +activation), and with `ln` it writes fp32 to the stream's scratch and the row LayerNorm kernel (adds the residual) follows.
     // All sizes are LOGICAL (elements of the mathematical matrices).  In fp32-parity mode (x3) every 16-bit operand buffer is
     // physically 3x as wide (fp16 hi | lo | hi per 64 columns), so operand strides, the contraction length and the 16-bit
     // output stride are multiplied by S = 3 here and nowhere else.
@@ -921,48 +917,43 @@ struct vb200_engine {
                     const LNW* ln, bf16* out_b, int ld_b, float* out_f, int ld_f, int stream = 0, Op::Sync sync = Op::NONE,
                     const float* mul = nullptr, int ld_mul = 0, const int* m_rows = nullptr) {
         const int S = x3 ? 3 : 1;
-        const bool split_ln = ln != nullptr && !fused_ln;
         if (x3 && act == vb::kActGelu) act = vb::kActGeluExact;
         Op op{};
         op.kind = Op::GEMM;
         op.stream = stream;
         op.sync = sync;
-        op.ln = ln != nullptr && !split_ln;      // cluster-LayerNorm epilogue (fused_layernorm option)
-        op.block_n = vb::gemm_p_pick_block_n(W.N, op.ln);
-        if (op.block_n == 0) fail(VB200_ERR_INVALID, "no LayerNorm-fused GEMM tiling for N=%d", W.N);
+        op.block_n = vb::gemm_p_pick_block_n(W.N);
         // Small forwards (<= lone_rows rows in either stream, batch <= 8): 64-wide tiles while they still fit one CTA per SM -- twice
         // the CTAs, half the epilogue each.  The tile width never changes an element's accumulation order.
-        if (lone_rows > 0 && !x3 && !op.ln && op.block_n == 128 && W.N % 64 == 0 &&
+        if (lone_rows > 0 && !x3 && op.block_n == 128 && W.N % 64 == 0 &&
             std::max(pl.B * pl.T, pl.B * pl.V) <= lone_rows && ((a_rows + 127) / 128) * (W.N / 64) <= vb::num_sms_host())
             op.block_n = 64;
         op.ta = make_tmap(A, a_rows, static_cast<int64_t>(W.ldw) * S, lda * S, 128, opt.act_fp16 != 0);
         op.tb = make_tmap(W.w, W.N, static_cast<int64_t>(W.ldw) * S, static_cast<int64_t>(W.ldw) * S, op.block_n, opt.act_fp16 != 0);
         GemmEpilogue& e = op.ep;
         e.M = static_cast<int>(a_rows); e.N = W.N; e.K = W.ldw * S;
-        e.bias = W.bias; e.mul = mul; e.ld_mul = ld_mul; e.eps = cfg.ln_eps; e.act = act; e.pdl = opt.use_pdl ? (early_w ? 5 : 1) : 0;
+        e.bias = W.bias; e.mul = mul; e.ld_mul = ld_mul; e.act = act; e.pdl = opt.use_pdl ? (early_w ? 5 : 1) : 0;
         e.a_f16 = opt.act_fp16; e.out_f16 = opt.act_fp16;
         e.m_rows = m_rows;
-        if (split_ln) {
+        if (ln) {
             e.out_f32 = pl.y_scratch[stream]; e.ld_f32 = W.N;
         } else {
-            e.res = res; e.ld_res = ld_res;
-            e.gamma = ln ? ln->g : nullptr; e.beta = ln ? ln->b : nullptr;
             e.out_bf16 = out_b; e.ld_bf16 = ld_b * S; e.out_f32 = out_f; e.ld_f32 = ld_f;
             e.split16 = (x3 && out_b != nullptr) ? 1 : 0;
             if (e.split16 && (W.N & 63)) fail(VB200_ERR_INVALID, "fp32-parity mode: 16-bit GEMM output of width %d is not a multiple of 64", W.N);
         }
         // Ping-pong kernel: each consumer warpgroup's epilogue runs under the other's mainloop.  It takes every plain GEMM it
-        // supports (not the cluster LayerNorm, fp32-parity, pooled-product or ragged-N ones) whose outputs the TMA can store.
+        // supports (not the fp32-parity, pooled-product or ragged-N ones) whose outputs the TMA can store.
         // It takes the tile width chosen above, 128 even where that leaves one tile per CTA: 64-wide ping-pong tiles measured slower on H100 SXM
         // (700 W, bf16, 16-bit output, scripts/kernel_bench.py) at 1984x768x768 (9.74 vs 8.20 us), 1984x768x3072 (29.19 vs 20.32) and
         // 2304x1024x1024 (16.71 vs 15.88), and only 4 % faster with GELU at 2304x1024x1024 (18.04 vs 18.81).
-        op.pingpong = gemm_kernel == 1 && tma_store_enabled && !op.ln && !x3 && vb::gemm_pingpong_supports(e, op.block_n) &&
+        op.pingpong = gemm_kernel == 1 && tma_store_enabled && !x3 && vb::gemm_pingpong_supports(e, op.block_n) &&
                       setup_pingpong_store(&op.tc, &op.tc32, e);
-        if (tma_store_enabled && !op.ln && !op.pingpong) setup_tma_store(&op.tc, e);
+        if (tma_store_enabled && !op.pingpong) setup_tma_store(&op.tc, e);
         op.flops = 2.0 * a_rows * W.N * W.K;
         pl.flops += op.flops;
         pl.ops.push_back(op);
-        if (split_ln) {
+        if (ln) {
             Op l{};
             l.kind = Op::LAYERNORM;
             l.stream = stream;
@@ -1088,11 +1079,9 @@ struct vb200_engine {
             pl.v_f32[i] = pl.mem.alloc_n<float>(static_cast<size_t>(Mv) * Hv);
             pl.v_b16[i] = pl.mem.alloc_n<bf16>(static_cast<size_t>(Mv) * Hv * S);
         }
-        if (!fused_ln) {
-            const size_t n0 = std::max({static_cast<size_t>(Mt) * H, static_cast<size_t>(Mv) * Hv, static_cast<size_t>(B) * 2 * Hb});
-            pl.y_scratch[0] = pl.mem.alloc_n<float>(n0);
-            pl.y_scratch[1] = pl.mem.alloc_n<float>(static_cast<size_t>(Mv) * Hv);
-        }
+        pl.y_scratch[0] = pl.mem.alloc_n<float>(std::max({static_cast<size_t>(Mt) * H, static_cast<size_t>(Mv) * Hv,
+                                                          static_cast<size_t>(B) * 2 * Hb}));
+        pl.y_scratch[1] = pl.mem.alloc_n<float>(static_cast<size_t>(Mv) * Hv);
         const int qt = 3 * std::max(H, Hb), qv = 3 * std::max(Hv, Hb);
         // Q | K | V projections: 16-bit for the tensor-core attention kernel, fp32 in fp32-parity mode
         const size_t qe = x3 ? 4 : 2;
@@ -1248,12 +1237,12 @@ struct vb200_engine {
     static constexpr int kTimelineCtas = 304;
     void attach_timeline(Plan& pl) {
         size_t n = 0;
-        for (const Op& op : pl.ops) if (op.kind == Op::GEMM && !op.ln) ++n;
+        for (const Op& op : pl.ops) if (op.kind == Op::GEMM) ++n;
         if (n == 0) return;
         pl.timeline = pl.mem.alloc_n<long long>(n * kTimelineCtas * 16);
         CUDA_CHECK(cudaMemset(pl.timeline, 0, n * kTimelineCtas * 16 * sizeof(long long)));
         size_t i = 0;
-        for (Op& op : pl.ops) if (op.kind == Op::GEMM && !op.ln) op.ep.timing = pl.timeline + (i++) * kTimelineCtas * 16;
+        for (Op& op : pl.ops) if (op.kind == Op::GEMM) op.ep.timing = pl.timeline + (i++) * kTimelineCtas * 16;
     }
 
     // Plan cache bound (a MicroBatchWorker produces many (batch, length, regions) combinations): beyond max_plans the least
@@ -1365,10 +1354,10 @@ struct vb200_engine {
                 e.grid_pct = profile_grid_pct;                        // 0 outside vb200_profile_ops
                 const cudaError_t le = op.pingpong
                     ? vb::launch_gemm_pingpong(op.ta, op.tb, &op.tc, &op.tc32, e, op.block_n, st)
-                    : vb::launch_gemm_persistent(op.ta, op.tb, e, op.block_n, op.ln, st);
+                    : vb::launch_gemm_persistent_plain(op.ta, op.tb, e, op.block_n, st);
                 if (le != cudaSuccess)
-                    fail(VB200_ERR_CUDA, "GEMM launch failed: %s (layer %s, M=%d N=%d K=%d act=%d block_n=%d cluster_ln=%d split16=%d tma_store=%d)",
-                         cudaGetErrorString(le), op.tag ? op.tag : "?", e.M, e.N, e.K, e.act, op.block_n, (int)op.ln, e.split16, e.tma_store);
+                    fail(VB200_ERR_CUDA, "GEMM launch failed: %s (layer %s, M=%d N=%d K=%d act=%d block_n=%d split16=%d tma_store=%d)",
+                         cudaGetErrorString(le), op.tag ? op.tag : "?", e.M, e.N, e.K, e.act, op.block_n, e.split16, e.tma_store);
                 break;
             }
             case Op::SELF_ATTN:
@@ -1782,6 +1771,8 @@ int vb200_create(const char* config_json, int64_t n_tensors, const vb200_tensor*
         vb200_options o{};
         if (opt) o = *opt;
         if (o.ln_fold != 0) fail(VB200_ERR_INVALID, "vb200_options: the LayerNorm fold was removed (its reserved field must be 0)");
+        if (o.fused_layernorm > 0)
+            fail(VB200_ERR_INVALID, "vb200_options: the cluster-LayerNorm GEMM epilogue was removed (fused_layernorm must be 0 or negative)");
         // tri-state flags: 0 = default, 1 = on, -1 = off
         o.use_cuda_graph = o.use_cuda_graph >= 0 ? 1 : 0;
         o.strict = o.strict >= 0 ? 1 : 0;
@@ -1789,7 +1780,6 @@ int vb200_create(const char* config_json, int64_t n_tensors, const vb200_tensor*
         o.use_pdl = o.use_pdl > 0 ? 1 : 0;
         o.split_fp32 = o.split_fp32 > 0 ? 1 : 0;
         o.act_fp16 = (o.act_fp16 >= 0 || o.split_fp32) ? 1 : 0;
-        o.fused_layernorm = (o.fused_layernorm > 0 && !o.split_fp32) ? 1 : 0;
         Config c = parse_config(config_json);
         {   // audit the state_dict (names, shapes, dtypes, strictness) before touching any device
             vb200_engine audit;
@@ -1801,8 +1791,6 @@ int vb200_create(const char* config_json, int64_t n_tensors, const vb200_tensor*
         eng->cfg = c;
         eng->opt = o;
         eng->x3 = o.split_fp32 != 0;
-        eng->fused_ln = o.fused_layernorm != 0;
-        if (const char* v = getenv("VB200_FUSED_LN")) eng->fused_ln = (strcmp(v, "1") == 0) && !eng->x3;
         if (const char* v = getenv("VB200_LONE_ROWS")) eng->lone_rows = std::max(0, atoi(v));
         eng->max_plans = o.max_plans > 0 ? static_cast<size_t>(o.max_plans) : 24;
         if (const char* v = getenv("VB200_MAX_PLANS")) { const int n = atoi(v); if (n > 0) eng->max_plans = static_cast<size_t>(n); }
@@ -2169,7 +2157,7 @@ int vb200_profile_ops(vb200_handle h, int32_t batch, int32_t n_tokens, int32_t n
                 dims[4 * i + 0] = op.kind == Op::GEMM ? op.ep.M : (op.kind == Op::LAYERNORM ? op.ln_M : op.B);
                 dims[4 * i + 1] = op.kind == Op::GEMM ? op.ep.N : (op.kind == Op::LAYERNORM ? op.ln_N : op.La);
                 dims[4 * i + 2] = op.kind == Op::GEMM ? op.ep.K : op.Lb;
-                dims[4 * i + 3] = op.kind == Op::GEMM ? (op.ep.act | (op.ln ? 16 : 0)) : op.heads;
+                dims[4 * i + 3] = op.kind == Op::GEMM ? op.ep.act : op.heads;
             }
         }
     });
@@ -2255,7 +2243,10 @@ int vb200_linear(const void* x_bf16, int64_t ld_x, const void* w_bf16, int64_t l
                  void* y_bf16, int64_t ld_y_bf16, float* y_f32, int64_t ld_y_f32, int64_t M, int64_t N, int64_t K,
                  int32_t block_n, int32_t use_pdl, int32_t act_fp16, int32_t variant, long long* timing, void* cuda_stream) {
     return op_guard([&] {
-        const bool ln = gamma != nullptr;
+        // LayerNorm is the row kernel's job (vb200_layernorm on the fp32 output); eps is ignored
+        if (residual != nullptr || gamma != nullptr || beta != nullptr)
+            fail(VB200_ERR_INVALID, "vb200_linear: residual, gamma and beta must be NULL (the cluster-LayerNorm GEMM epilogue was "
+                                    "removed; run vb200_layernorm on the fp32 output)");
         // Variant 2 named the Blackwell CTA-pair kernel, variants 3 and 4 Blackwell occupancy configurations of the persistent kernel
         // (three CTAs per SM; one CTA with a 6-stage ring); ABI version 2 keeps accepting them, and on sm_90a they select the
         // persistent kernel itself.  block_n 256 (the Blackwell 256-wide tile) runs as 128-wide tiles, which give the same bits: the
@@ -2263,11 +2254,11 @@ int vb200_linear(const void* x_bf16, int64_t ld_x, const void* w_bf16, int64_t l
         if (variant < 0 || variant == 1 || variant > 5)
             fail(VB200_ERR_INVALID, "vb200_linear: variant %d does not exist (0 persistent, 2 / 3 / 4 = 0, 5 ping-pong)", variant);
         if (variant == 5) {
-            const int bn = block_n > 0 ? block_n : vb::gemm_p_pick_block_n(static_cast<int>(N), false);
+            const int bn = block_n > 0 ? block_n : vb::gemm_p_pick_block_n(static_cast<int>(N));
             CUtensorMap ta = make_tmap(x_bf16, M, K, ld_x, 128, act_fp16 != 0);
             CUtensorMap tb = make_tmap(w_bf16, N, K, ld_w, bn, act_fp16 != 0);
             GemmEpilogue e{};
-            e.M = (int)M; e.N = (int)N; e.K = (int)K; e.bias = bias; e.res = residual; e.gamma = gamma; e.act = act; e.pdl = use_pdl;
+            e.M = (int)M; e.N = (int)N; e.K = (int)K; e.bias = bias; e.act = act; e.pdl = use_pdl;
             e.out_bf16 = static_cast<bf16*>(y_bf16); e.ld_bf16 = (int)ld_y_bf16; e.out_f32 = y_f32; e.ld_f32 = (int)ld_y_f32;
             e.a_f16 = act_fp16 ? 1 : 0; e.out_f16 = e.a_f16; e.timing = timing;
             CUtensorMap c16, c32;
@@ -2277,25 +2268,23 @@ int vb200_linear(const void* x_bf16, int64_t ld_x, const void* w_bf16, int64_t l
             CUDA_CHECK(vb::launch_gemm_pingpong(ta, tb, &c16, &c32, e, bn, static_cast<cudaStream_t>(cuda_stream)));
             return;
         }
-        int bn = block_n > 0 ? block_n : vb::gemm_p_pick_block_n(static_cast<int>(N), ln);
-        if (bn == 0) fail(VB200_ERR_INVALID, "no tiling for N=%lld with LayerNorm", (long long)N);
-        if (!ln && bn == 256) bn = 128;
-        if (!ln && bn != 64 && bn != 128 && bn != 192)
+        int bn = block_n > 0 ? block_n : vb::gemm_p_pick_block_n(static_cast<int>(N));
+        if (bn == 256) bn = 128;
+        if (bn != 64 && bn != 128 && bn != 192)
             fail(VB200_ERR_INVALID, "vb200_linear: block_n %d (plain tiles are 64, 128, 192 or 256 wide)", bn);
-        if (variant >= 2 && (ln || (bn != 128 && !(variant == 4 && bn == 64))))
+        if (variant >= 2 && bn != 128 && !(variant == 4 && bn == 64))
             fail(VB200_ERR_INVALID, "vb200_linear: variants 2 and 3 are the plain 128-wide tile, variant 4 the 128- or 64-wide one");
         CUtensorMap ta = make_tmap(x_bf16, M, K, ld_x, 128, act_fp16 != 0);
         CUtensorMap tb = make_tmap(w_bf16, N, K, ld_w, bn, act_fp16 != 0);
         GemmEpilogue e{};
-        e.M = (int)M; e.N = (int)N; e.K = (int)K; e.bias = bias; e.res = residual; e.ld_res = (int)ld_res;
-        e.gamma = gamma; e.beta = beta; e.eps = eps; e.out_bf16 = static_cast<bf16*>(y_bf16); e.ld_bf16 = (int)ld_y_bf16;
+        e.M = (int)M; e.N = (int)N; e.K = (int)K; e.bias = bias; e.out_bf16 = static_cast<bf16*>(y_bf16); e.ld_bf16 = (int)ld_y_bf16;
         e.out_f32 = y_f32; e.ld_f32 = (int)ld_y_f32; e.act = act; e.pdl = use_pdl;
         e.a_f16 = act_fp16 ? 1 : 0; e.out_f16 = e.a_f16; e.timing = timing;
         if (const char* dbg = getenv("VB200_DEBUG")) e.debug = atoi(dbg);          // timing decomposition (kernels.h), op entry only
         CUtensorMap tc;
         const char* ts = getenv("VB200_TMASTORE");
-        if (!ln && !(ts && strcmp(ts, "0") == 0)) { setup_tma_store(&tc, e); e.tmap_c_host = e.tma_store ? &tc : nullptr; }
-        CUDA_CHECK(vb::launch_gemm_persistent(ta, tb, e, bn, ln, static_cast<cudaStream_t>(cuda_stream)));
+        if (!(ts && strcmp(ts, "0") == 0)) { setup_tma_store(&tc, e); e.tmap_c_host = e.tma_store ? &tc : nullptr; }
+        CUDA_CHECK(vb::launch_gemm_persistent_plain(ta, tb, e, bn, static_cast<cudaStream_t>(cuda_stream)));
     });
 }
 
@@ -2304,7 +2293,7 @@ int vb200_linear_rows(const void* x16, int64_t ld_x, const void* w16, int64_t ld
                       const int32_t* m_rows, void* cuda_stream) {
     return op_guard([&] {
         if (m_rows == nullptr) fail(VB200_ERR_INVALID, "vb200_linear_rows: m_rows is NULL");
-        const int bn = block_n > 0 ? block_n : vb::gemm_p_pick_block_n(static_cast<int>(N), false);
+        const int bn = block_n > 0 ? block_n : vb::gemm_p_pick_block_n(static_cast<int>(N));
         if (bn != 64 && bn != 128 && bn != 192) fail(VB200_ERR_INVALID, "vb200_linear_rows: block_n %d (plain tiles are 64, 128 or 192 wide)", bn);
         CUtensorMap ta = make_tmap(x16, M, K, ld_x, 128, act_fp16 != 0);
         CUtensorMap tb = make_tmap(w16, N, K, ld_w, bn, act_fp16 != 0);
@@ -2318,7 +2307,7 @@ int vb200_linear_rows(const void* x16, int64_t ld_x, const void* w16, int64_t ld
         }
         setup_tma_store(&tc, e);
         e.tmap_c_host = e.tma_store ? &tc : nullptr;
-        CUDA_CHECK(vb::launch_gemm_persistent(ta, tb, e, bn, false, static_cast<cudaStream_t>(cuda_stream)));
+        CUDA_CHECK(vb::launch_gemm_persistent_plain(ta, tb, e, bn, static_cast<cudaStream_t>(cuda_stream)));
     });
 }
 
@@ -2345,14 +2334,14 @@ int vb200_linear_split(const void* x16, int64_t ld_x, const void* w16, int64_t l
                        int64_t ld_y16, float* y_f32, int64_t ld_y_f32, int64_t M, int64_t N, int64_t K3, void* cuda_stream) {
     return op_guard([&] {
         if (K3 % 192 != 0) fail(VB200_ERR_INVALID, "vb200_linear_split: K3 = %lld is not 3 x a multiple of 64", (long long)K3);
-        const int bn = vb::gemm_p_pick_block_n(static_cast<int>(N), false);
+        const int bn = vb::gemm_p_pick_block_n(static_cast<int>(N));
         CUtensorMap ta = make_tmap(x16, M, K3, ld_x, 128, true);
         CUtensorMap tb = make_tmap(w16, N, K3, ld_w, bn, true);
         GemmEpilogue e{};
-        e.M = (int)M; e.N = (int)N; e.K = (int)K3; e.bias = bias; e.eps = 0.0f; e.out_bf16 = static_cast<bf16*>(y16);
+        e.M = (int)M; e.N = (int)N; e.K = (int)K3; e.bias = bias; e.out_bf16 = static_cast<bf16*>(y16);
         e.ld_bf16 = (int)ld_y16; e.out_f32 = y_f32; e.ld_f32 = (int)ld_y_f32; e.act = act; e.a_f16 = 1; e.out_f16 = 1;
         e.split16 = y16 != nullptr ? 1 : 0;
-        CUDA_CHECK(vb::launch_gemm_persistent(ta, tb, e, bn, false, static_cast<cudaStream_t>(cuda_stream)));
+        CUDA_CHECK(vb::launch_gemm_persistent_plain(ta, tb, e, bn, static_cast<cudaStream_t>(cuda_stream)));
     });
 }
 
@@ -2419,7 +2408,7 @@ int vb200_linear_product(const void* x16, int64_t ld_x, const void* w16, int64_t
     return op_guard([&] {
         if (mul == nullptr) fail(VB200_ERR_INVALID, "vb200_linear_product: mul is NULL");
         // as add_linear builds the pooled product: the cooperative kernel (ping-pong takes no product), its tile width, its TMA store
-        const int bn = block_n > 0 ? block_n : vb::gemm_p_pick_block_n(static_cast<int>(N), false);
+        const int bn = block_n > 0 ? block_n : vb::gemm_p_pick_block_n(static_cast<int>(N));
         if (bn != 64 && bn != 128 && bn != 192) fail(VB200_ERR_INVALID, "vb200_linear_product: block_n %d (plain tiles are 64, 128 or 192 wide)", bn);
         CUtensorMap ta = make_tmap(x16, M, K, ld_x, 128, act_fp16 != 0);
         CUtensorMap tb = make_tmap(w16, N, K, ld_w, bn, act_fp16 != 0);
@@ -2430,7 +2419,7 @@ int vb200_linear_product(const void* x16, int64_t ld_x, const void* w16, int64_t
         CUtensorMap tc;
         setup_tma_store(&tc, e);
         e.tmap_c_host = e.tma_store ? &tc : nullptr;
-        CUDA_CHECK(vb::launch_gemm_persistent(ta, tb, e, bn, false, static_cast<cudaStream_t>(cuda_stream)));
+        CUDA_CHECK(vb::launch_gemm_persistent_plain(ta, tb, e, bn, static_cast<cudaStream_t>(cuda_stream)));
     });
 }
 

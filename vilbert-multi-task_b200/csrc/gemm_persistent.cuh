@@ -1,6 +1,6 @@
 // Persistent, warp-specialised wgmma GEMM (sm_90a):
-//   * each CTA (each CLUSTER for the LayerNorm variant) loops over output tiles, so barrier init, descriptor prefetch and the
-//     TMA/L2 latency of the first k-block are paid once per kernel, not once per tile;
+//   * each CTA loops over output tiles, so barrier init, descriptor prefetch and the TMA/L2 latency of the first k-block are paid
+//     once per kernel, not once per tile;
 //   * one TMA producer warp runs ahead across tile boundaries (the shared-memory ring never drains);
 //   * two consumer warpgroups accumulate the 128 x BLOCK_N tile in registers (64 rows each, one k-block of wgmma in flight while
 //     the previous stage is handed back), deposit it in a padded fp32 shared-memory tile and then, as eight epilogue warps, read
@@ -8,12 +8,8 @@
 //   * epilogue code is specialised OUTSIDE the per-element loops (activation, 16-bit format); outputs are transposed through a
 //     swizzled 2 KB per-warp buffer so that a store instruction writes 8 rows x 64 bytes; GELU through a polynomial erf;
 //   * launched programmatically (GemmEpilogue::pdl) the producer issues the weight tiles of the first ring pass before
-//     griddepcontrol.wait; every kernel triggers its dependents once its last tile is accumulated;
-//   * LN variant: the fp32 residual of the next 32-column chunk is prefetched while the current chunk is processed, and the
-//     first chunk's residual is requested before the accumulator is even ready;
-//   * LayerNorm (8 epilogue warps, x kept in registers) exchanges ONE (mean, M2) pair per row, column half and CTA through
-//     distributed shared memory (Chan's parallel variance), synchronised by cluster-scope mbarriers that only the epilogue warps
-//     touch -- the producer is never stalled by the normalisation.
+//     griddepcontrol.wait; every kernel triggers its dependents once its last tile is accumulated.
+// A residual LayerNorm is not part of this kernel: the GEMM writes fp32 and the row kernel of layernorm.cu normalises.
 //
 //   D[M,N] = epilogue( A[M,K] (16-bit, row-major)  x  W[N,K]^T (16-bit, nn.Linear layout = K-major) ), fp32 accumulate.
 #pragma once
@@ -37,10 +33,10 @@ constexpr int kMmaK = 16;
 // 16 column tiles instead of 24.
 // One CTA per SM: each consumer thread holds BLOCK_N / 2 fp32 accumulators, and the deposited tile plus a ring deep enough to
 // cover the L2 latency take most of the 227 KB of shared memory.
-template <int BLOCK_N, bool LN, int MODE = 0>
+template <int BLOCK_N, int MODE = 0>
 struct PCfg {
-    static_assert(BLOCK_N == 64 || BLOCK_N == 128 || (LN && BLOCK_N == 96) || (!LN && (MODE == 0 || MODE == 6) && BLOCK_N == 192),
-                  "tile widths: 64 / 128 (LayerNorm also 96, the default plain kernel also 192)");
+    static_assert(BLOCK_N == 64 || BLOCK_N == 128 || ((MODE == 0 || MODE == 6) && BLOCK_N == 192),
+                  "tile widths: 64 / 128 (MODE 0 and 6 also 192)");
     static constexpr int kStageBytesA = kBlockM * kBlockK * 2;
     static constexpr int kStageBytesB = BLOCK_N * kBlockK * 2;
     static constexpr int kStageBytes = kStageBytesA + kStageBytesB;
@@ -57,60 +53,22 @@ struct PCfg {
     // and the fragment-layout float2 writes of the consumer warpgroups (at most) two-way bank conflicted.
     static constexpr int kAccLd = BLOCK_N + 4;
     static constexpr int kAccBytes = kBlockM * kAccLd * 4;
-    // Per-epilogue-warp transpose buffer so global stores are row-contiguous.
-    //   plain: 32 rows x 64 bytes, XOR-swizzled (store16_sw / store_f32_sw);  LN: 32 rows x 33 fp32
-    static constexpr int kXposeBytesPerWarp = LN ? 32 * 33 * 4 : 2048;
+    // Per-epilogue-warp transpose buffer so global stores are row-contiguous: 32 rows x 64 bytes, XOR-swizzled
+    // (store16_sw / store_f32_sw).
+    static constexpr int kXposeBytesPerWarp = 2048;
     static constexpr int kXposeBytes = kEpiWarps * kXposeBytesPerWarp;
-    // LN: chunks per epilogue thread (two column halves per row quarter)
-    static constexpr int kCPT = (kNumChunks + 1) / 2;
-    // LN-only pieces: gamma, beta, cluster partials [2 bufs][2 halves][128] float2
-    static constexpr int kLnAux = LN ? 2 * BLOCK_N * 4 + 4 * kBlockM * 8 : 0;
-    // plain: ONE bias slice (the tile-end barrier of the epilogue warps protects it); LN keeps bias | gamma | beta resident
-    static constexpr int kBiasFloats = LN ? 2 * BLOCK_N : BLOCK_N;
-    static constexpr int kBarBytes = (2 * 8 + 2) * 8 + 16;
-    static constexpr int kFit = (232448 - kAccBytes - kXposeBytes - kBiasFloats * 4 - kLnAux - kBarBytes) / kStageBytes;
+    // ONE bias slice (the tile-end barrier of the epilogue warps protects it)
+    static constexpr int kBiasFloats = BLOCK_N;
+    static constexpr int kBarBytes = 2 * 8 * 8 + 16;
+    static constexpr int kFit = (232448 - kAccBytes - kXposeBytes - kBiasFloats * 4 - kBarBytes) / kStageBytes;
     static constexpr int kStages = kFit > 8 ? 8 : kFit;
-    static constexpr int kNumBars = 2 * kStages + 2;
-    static constexpr int kSmemAux = kBiasFloats * 4 + kLnAux + kNumBars * 8 + 16 + kXposeBytes;
+    static constexpr int kNumBars = 2 * kStages;
+    static constexpr int kSmemAux = kBiasFloats * 4 + kNumBars * 8 + 16 + kXposeBytes;
     // no alignment slack: the dynamic shared-memory window starts 1024-aligned (checked at kernel entry)
     static constexpr int kSmemBytes = kStages * kStageBytes + kAccBytes + kSmemAux;
     static_assert(kStages >= 2 && kSmemBytes <= 232448, "shared memory budget (227 KB per block)");
 };
-// Largest LayerNorm cluster: a row of up to 16 tiles (non-portable cluster size on H100).
-constexpr int kMaxCluster = 16;
 
-// ---- cluster-scope mbarrier helpers (LayerNorm exchange)
-__device__ __forceinline__ uint32_t mapa_u32(const void* local_smem_ptr, uint32_t rank) {
-    uint32_t remote;
-    asm("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(local_smem_ptr)), "r"(rank));
-    return remote;
-}
-__device__ __forceinline__ void mbar_arrive_remote_release(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_acquire_cluster(uint64_t* bar, uint32_t parity) {
-    uint32_t spins = 0, ok = 0;
-    while (true) {
-        asm volatile(
-            "{\n\t"
-            ".reg .pred P;\n\t"
-            "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 P, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, P;\n\t"
-            "}\n"
-            : "=r"(ok)
-            : "r"(smem_u32(bar)), "r"(parity)
-            : "memory");
-        if (ok) break;
-        if (++spins > VB_SPIN_LIMIT) {
-            __trap();                    // no printf: a call in a kernel that issues wgmma serialises it (C7510)
-        }
-    }
-}
-__device__ __forceinline__ float2 dsmem_ld_f32x2(uint32_t cluster_addr) {
-    float2 v;
-    asm volatile("ld.shared::cluster.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(cluster_addr));
-    return v;
-}
 template <int kThreadsInBar>
 __device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kThreadsInBar) : "memory"); }
 
@@ -199,26 +157,6 @@ __device__ __forceinline__ void store_chunk(const GemmEpilogue& p, int m, int nc
         store_chunk_slow(p, m, nc, tmp);
     }
 }
-// residual: 32 fp32 of row m starting at column nc -> 8 float4 (plain loads: res may alias out_f32)
-__device__ __forceinline__ void res_load(const GemmEpilogue& p, int m, int nc, bool fast, float4 (&r)[8]) {
-    const float* rp = p.res + static_cast<size_t>(m) * p.ld_res + nc;
-    if (fast) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) r[j] = reinterpret_cast<const float4*>(rp)[j];
-    } else {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            r[j].x = nc + 4 * j + 0 < p.N ? rp[4 * j + 0] : 0.0f;
-            r[j].y = nc + 4 * j + 1 < p.N ? rp[4 * j + 1] : 0.0f;
-            r[j].z = nc + 4 * j + 2 < p.N ? rp[4 * j + 2] : 0.0f;
-            r[j].w = nc + 4 * j + 3 < p.N ? rp[4 * j + 3] : 0.0f;
-        }
-    }
-}
-__device__ __forceinline__ void res_add(float (&v)[32], const float4 (&r)[8]) {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) { v[4 * j] += r[j].x; v[4 * j + 1] += r[j].y; v[4 * j + 2] += r[j].z; v[4 * j + 3] += r[j].w; }
-}
 
 // ---- row-contiguous stores through a per-warp 2 KB shared-memory transpose (32 rows x 64 bytes, XOR-swizzled)
 // Row r keeps its four 16-byte units j at position j ^ ((r >> 1) & 3): the row-per-lane writes (one unit per instruction) and
@@ -282,48 +220,12 @@ __device__ __forceinline__ void store_f32_sw(uint4* st, float* out, int ld, int 
     }
 }
 
-// LayerNorm outputs (fp32 stream copy and 16-bit GEMM operand) of one chunk from an fp32 [32][33] transpose buffer.
-template <bool F16>
-__device__ __forceinline__ void store_ln_coalesced(float* st, const GemmEpilogue& p, int m_warp, int ncol, const float (&v)[32],
-                                                   int lane) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) st[lane * 33 + j] = v[j];
-    __syncwarp();
-    if (p.out_f32 != nullptr) {
-        const int c4 = lane & 7;
-#pragma unroll
-        for (int it = 0; it < 8; ++it) {                   // 4 rows x 128 contiguous bytes per instruction
-            const int r = it * 4 + (lane >> 3);
-            const float* s4 = st + r * 33 + c4 * 4;
-            if (m_warp + r < p.M)
-                *reinterpret_cast<float4*>(p.out_f32 + static_cast<size_t>(m_warp + r) * p.ld_f32 + ncol + c4 * 4) =
-                    make_float4(s4[0], s4[1], s4[2], s4[3]);
-        }
-    }
-    if (p.out_bf16 != nullptr) {
-        const int piece = lane & 3;
-#pragma unroll
-        for (int it = 0; it < 4; ++it) {                   // 8 rows x 64 contiguous bytes per instruction
-            const int r = it * 8 + (lane >> 2);
-            const float* s8 = st + r * 33 + piece * 8;
-            uint4 u;
-            u.x = F16 ? pack16x2_rt(s8[0], s8[1], 1) : pack_bf16x2(s8[0], s8[1]);
-            u.y = F16 ? pack16x2_rt(s8[2], s8[3], 1) : pack_bf16x2(s8[2], s8[3]);
-            u.z = F16 ? pack16x2_rt(s8[4], s8[5], 1) : pack_bf16x2(s8[4], s8[5]);
-            u.w = F16 ? pack16x2_rt(s8[6], s8[7], 1) : pack_bf16x2(s8[6], s8[7]);
-            if (m_warp + r < p.M)
-                *reinterpret_cast<uint4*>(p.out_bf16 + static_cast<size_t>(m_warp + r) * p.ld_bf16 + ncol + piece * 8) = u;
-        }
-    }
-    __syncwarp();
-}
-
-template <int BLOCK_N, bool LN, int ACT, bool F16, int MODE = 0>
-__global__ void __launch_bounds__(PCfg<BLOCK_N, LN, MODE>::kThreads, PCfg<BLOCK_N, LN, MODE>::kMinBlocks)
+template <int BLOCK_N, int ACT, bool F16, int MODE = 0>
+__global__ void __launch_bounds__(PCfg<BLOCK_N, MODE>::kThreads, PCfg<BLOCK_N, MODE>::kMinBlocks)
 gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                        const __grid_constant__ CUtensorMap tmap_c, const GemmEpilogue p, const int num_m_tiles,
                        const int num_n_tiles) {
-    using Cfg = PCfg<BLOCK_N, LN, MODE>;
+    using Cfg = PCfg<BLOCK_N, MODE>;
     constexpr int kStages = Cfg::kStages;
     constexpr int kNC = Cfg::kNumChunks;
     constexpr int kEpiThreads = Cfg::kEpiThreads;
@@ -338,21 +240,16 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
     }
     uint8_t* ring = smem_raw;
     float* s_acc = reinterpret_cast<float*>(ring + kStages * Cfg::kStageBytes);    // [128][kAccLd] deposited accumulator
-    float* s_bias = s_acc + kBlockM * Cfg::kAccLd;                                  // [BLOCK_N] (LN: [2][BLOCK_N], 2nd half unused)
-    float* s_gamma = s_bias + Cfg::kBiasFloats;                                     // LN only (zero-sized otherwise)
-    float* s_beta = s_gamma + (LN ? BLOCK_N : 0);
-    float2* s_part = reinterpret_cast<float2*>(s_beta + (LN ? BLOCK_N : 0));        // [2 bufs][2 halves][128] (mean, M2)
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(s_part + (LN ? 4 * kBlockM : 0));
+    float* s_bias = s_acc + kBlockM * Cfg::kAccLd;                                  // [BLOCK_N]
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(s_bias + Cfg::kBiasFloats);
     uint64_t* empty_bar = full_bar + kStages;
-    uint64_t* ln_bar = empty_bar + kStages;             // [2] cluster exchange, alternating per tile so that arrivals
-                                                       //     for tile i+1 can never be counted into tile i's phase
-    uint8_t* s_xpose = reinterpret_cast<uint8_t*>(ln_bar + 2) + 16;               // [kEpiWarps][kXposeBytesPerWarp]
+    uint8_t* s_xpose = reinterpret_cast<uint8_t*>(empty_bar + kStages) + 16;       // [kEpiWarps][kXposeBytesPerWarp]
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
     const int num_kb = (p.K + kBlockK - 1) / kBlockK;
     // profiling stamps (first tile of each CTA): 0 entry, 1 setup done, 2 first k-block landed, 3 last k-block accumulated,
-    // 4 accumulator ready, 5 accumulator read + local statistics done, 6 LayerNorm exchange done, 7 epilogue done
+    // 4 accumulator ready, 5 and 7 epilogue done, 6 producer past griddepcontrol.wait (VB200_STAMPS builds)
     long long* stamps = p.timing ? p.timing + 16 * (static_cast<size_t>(blockIdx.y) * gridDim.x + blockIdx.x) : nullptr;
     if (stamps && threadIdx.x == 0) {
         stamps[0] = clock64();
@@ -364,9 +261,8 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
         stamps[12] = smid;                                                         // per-SM occupancy (scripts/step_timeline.py)
     }
 
-    // ---- tile assignment.  Non-LN: CTA b takes tiles b, b+grid, ... with the N index fastest (CTAs that run together
-    // share an A row-panel in L2).  LN: gridDim.x = cluster size = num_n_tiles, blockIdx.y = cluster id; cluster c takes
-    // M tiles c, c + gridDim.y, ... and the CTA's rank in the cluster is its (fixed) N tile.
+    // ---- tile assignment.  CTA b takes tiles b, b+grid, ... with the N index fastest (CTAs that run together share an A row-panel
+    // in L2).
     // Packed batches (p.m_rows): the producer and the consumers derive the same, shorter tile list from the device row count --
     // M tiles whose first row is at or past it do not exist for this launch.  The count is written before the graph starts.  A CTA
     // left without a tile triggers its dependents by exiting.
@@ -375,13 +271,11 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
         const int mr = max(0, min(*p.m_rows, p.M));
         run_m_tiles = min(num_m_tiles, (mr + kBlockM - 1) / kBlockM);
     }
-    const int total_tiles = LN ? num_m_tiles : run_m_tiles * num_n_tiles;
-    const int first_tile = LN ? static_cast<int>(blockIdx.y) : static_cast<int>(blockIdx.x);
-    const int tile_stride = LN ? static_cast<int>(gridDim.y) : static_cast<int>(gridDim.x);
-    const uint32_t cluster_size = LN ? cluster_nctarank() : 1u;
-    const uint32_t my_rank = LN ? cluster_ctarank() : 0u;
-    auto tile_m0 = [&](int tile) { return (LN ? tile : tile / num_n_tiles) * kBlockM; };
-    auto tile_n0 = [&](int tile) { return (LN ? static_cast<int>(my_rank) : tile % num_n_tiles) * BLOCK_N; };
+    const int total_tiles = run_m_tiles * num_n_tiles;
+    const int first_tile = static_cast<int>(blockIdx.x);
+    const int tile_stride = static_cast<int>(gridDim.x);
+    auto tile_m0 = [&](int tile) { return (tile / num_n_tiles) * kBlockM; };
+    auto tile_n0 = [&](int tile) { return (tile % num_n_tiles) * BLOCK_N; };
 
     // ---------------------------------------------------------------- one-time setup
     // The producer thread does not wait for the CTA-wide setup barrier: as soon as ITS barriers exist it puts the first ring
@@ -393,13 +287,10 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
     if (warp == Cfg::kProducerWarp && lane == 0) {
         tma_prefetch_desc(&tmap_a);
         tma_prefetch_desc(&tmap_b);
-        if (!LN && p.tma_store) tma_prefetch_desc(&tmap_c);
+        if (p.tma_store) tma_prefetch_desc(&tmap_c);
         for (int s = 0; s < kStages; ++s) {
             mbar_init(&full_bar[s], 1);
             mbar_init(&empty_bar[s], Cfg::kConsumerWarps);                   // one arrival per consumer warp
-        }
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(&ln_bar[a], LN ? cluster_size : 1u);                   // one arrival per CTA of the cluster
         }
         mbar_fence_init();
 #ifdef VB200_DECOMPOSE
@@ -407,7 +298,7 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
 #else
         constexpr bool early_ok = true;
 #endif
-        if (!LN && first_tile < total_tiles && p.pdl != 1 && early_ok) {
+        if (first_tile < total_tiles && p.pdl != 1 && early_ok) {
             early_a = p.pdl != 5;
             const int m0 = (first_tile / num_n_tiles) * kBlockM, n0 = (first_tile % num_n_tiles) * BLOCK_N;
             early = min(kStages, num_kb);
@@ -418,30 +309,23 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
                 tma_load_2d(sa + Cfg::kStageBytesA, &tmap_b, &full_bar[i], i * kBlockK, n0);
             }
         }
-    } else if (LN && warp < Cfg::kConsumerWarps) {
-        const int n0 = static_cast<int>(my_rank) * BLOCK_N;
-        for (int i = threadIdx.x; i < BLOCK_N; i += kEpiThreads) {
-            s_bias[i] = p.bias ? p.bias[n0 + i] : 0.0f;
-            s_gamma[i] = p.gamma[n0 + i];
-            s_beta[i] = p.beta[n0 + i];
-        }
     }
-    if (LN) cluster_sync_all(); else __syncthreads();           // peers' barriers must be initialised before remote arrives
+    __syncthreads();
     if (stamps && threadIdx.x == 0) stamps[1] = clock64();
 
     // Programmatic dependent launch: everything above overlapped the previous kernel's tail; its outputs are visible after the
     // wait.  (The producer thread of a pdl == 5 kernel waits inside its own branch, right before the first activation tile.)
     const bool producer_thread = warp == Cfg::kProducerWarp && lane == 0;
-    if (p.pdl && !(p.pdl == 5 && !LN && producer_thread)) pdl_wait();
+    if (p.pdl && !(p.pdl == 5 && producer_thread)) pdl_wait();
 
     if (warp == Cfg::kProducerWarp) {
         // ============================================================ TMA producer
         if (lane == 0) {
             int s = 0;
             uint32_t phase = 0;
-            if (p.pdl == 5 && !LN) pdl_wait();
+            if (p.pdl == 5) pdl_wait();
 #ifdef VB200_STAMPS
-            if (stamps && !LN) stamps[6] = clock64();                  // producer past griddepcontrol.wait (non-LN kernels: slot 6 is free)
+            if (stamps) stamps[6] = clock64();                         // producer past griddepcontrol.wait
 #endif
             for (int tile = first_tile; tile < total_tiles; tile += tile_stride) {
                 const int m0 = tile_m0(tile), n0 = tile_n0(tile);
@@ -517,7 +401,6 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
         };
         const int ew = warp;                          // 0..kEpiWarps-1
         const int q = ew & 3;                         // row quarter of the tile this warp owns
-        const int half = LN ? (ew >> 2) : 0;          // LN: column half of the tile
         const int row = q * 32 + lane;
         const int et = threadIdx.x;
         const bool st_fast = (p.out_bf16 == nullptr || (p.ld_bf16 & 7) == 0) && (p.out_f32 == nullptr || (p.ld_f32 & 3) == 0);
@@ -529,223 +412,128 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
             const float* acc_row = s_acc + row * Cfg::kAccLd;
             const bool stamp = stamps && it == 0 && et == 0;
 
-            if constexpr (!LN) {
-                // ------------------------------------------------ plain epilogue: 8 warps, one 32-column chunk at a time
-                const float* bias_t = s_bias;
-                // per-tile bias slice; the barrier below orders it before the reads, the one at the end of the tile orders
-                // the reads before the next tile's writes
-                for (int i = et; i < BLOCK_N; i += kEpiThreads) s_bias[i] = (p.bias && n0 + i < p.N) ? p.bias[n0 + i] : 0.0f;
-                epi_bar_sync<kEpiThreads>();
-                mma_tile(tile, it);
-                if (stamp) stamps[4] = clock64();
-                float* const out_f32 = p.out_f32;
-                // TMA-store path (CTA-uniform): this is the CTA's last tile, so no operand load is or will be in flight and
-                // every MMA that read the ring has completed (mma_tile above)
-                constexpr bool kF32SlabsFit = (BLOCK_N / 32) * (kBlockM * 128) <= kStages * Cfg::kStageBytes;
-                const bool use_tma = p.tma_store != 0 && st_fast && tile + tile_stride >= total_tiles &&
-                                     (p.tma_store == 1 || kF32SlabsFit) &&
-                                     (p.tma_store == 1 ? (p.out_bf16 != nullptr && p.out_f32 == nullptr)
-                                                       : (p.out_f32 != nullptr && p.out_bf16 == nullptr));
-                auto finish_chunk = [&](float (&v)[32], int nc) __attribute__((always_inline)) {
-                    bias_act32<ACT>(v, bias_t + (nc - n0));
+            // ------------------------------------------------ epilogue: 8 warps, one 32-column chunk at a time
+            const float* bias_t = s_bias;
+            // per-tile bias slice; the barrier below orders it before the reads, the one at the end of the tile orders
+            // the reads before the next tile's writes
+            for (int i = et; i < BLOCK_N; i += kEpiThreads) s_bias[i] = (p.bias && n0 + i < p.N) ? p.bias[n0 + i] : 0.0f;
+            epi_bar_sync<kEpiThreads>();
+            mma_tile(tile, it);
+            if (stamp) stamps[4] = clock64();
+            float* const out_f32 = p.out_f32;
+            // TMA-store path (CTA-uniform): this is the CTA's last tile, so no operand load is or will be in flight and
+            // every MMA that read the ring has completed (mma_tile above)
+            constexpr bool kF32SlabsFit = (BLOCK_N / 32) * (kBlockM * 128) <= kStages * Cfg::kStageBytes;
+            const bool use_tma = p.tma_store != 0 && st_fast && tile + tile_stride >= total_tiles &&
+                                 (p.tma_store == 1 || kF32SlabsFit) &&
+                                 (p.tma_store == 1 ? (p.out_bf16 != nullptr && p.out_f32 == nullptr)
+                                                   : (p.out_f32 != nullptr && p.out_bf16 == nullptr));
+            auto finish_chunk = [&](float (&v)[32], int nc) __attribute__((always_inline)) {
+                bias_act32<ACT>(v, bias_t + (nc - n0));
 #ifdef VB200_DECOMPOSE
-                    if ((p.debug & 2) && __float_as_uint(v[0]) != 0x7fc12345u) return;     // timing decomposition: no stores
+                if ((p.debug & 2) && __float_as_uint(v[0]) != 0x7fc12345u) return;     // timing decomposition: no stores
 #endif
-                    if (p.mul != nullptr && m_ok) {
-                        const float* mp = p.mul + static_cast<size_t>(m) * p.ld_mul + nc;
-                        if ((p.ld_mul & 3) == 0 && nc + 32 <= p.N) {          // 8 x 16-byte loads instead of 32 scalar ones
+                if (p.mul != nullptr && m_ok) {
+                    const float* mp = p.mul + static_cast<size_t>(m) * p.ld_mul + nc;
+                    if ((p.ld_mul & 3) == 0 && nc + 32 <= p.N) {          // 8 x 16-byte loads instead of 32 scalar ones
 #pragma unroll
-                            for (int j = 0; j < 8; ++j) {
-                                const float4 f = reinterpret_cast<const float4*>(mp)[j];
-                                v[4 * j] *= f.x; v[4 * j + 1] *= f.y; v[4 * j + 2] *= f.z; v[4 * j + 3] *= f.w;
-                            }
-                        } else {
-#pragma unroll
-                            for (int j = 0; j < 32; ++j) if (nc + j < p.N) v[j] *= mp[j];
+                        for (int j = 0; j < 8; ++j) {
+                            const float4 f = reinterpret_cast<const float4*>(mp)[j];
+                            v[4 * j] *= f.x; v[4 * j + 1] *= f.y; v[4 * j + 2] *= f.z; v[4 * j + 3] *= f.w;
                         }
-                    }
-                    if (use_tma) {
-                        // last tile of this CTA: the operand ring is idle -> stage the tile there in the TMA's SWIZZLE_128B
-                        // layout (16-byte unit u of row r at u ^ (r & 7): row-per-lane writes are bank-conflict free)
-                        const int cl = nc - n0;
-                        if (p.tma_store == 1) {                              // 16-bit: slabs of 64 columns x 128 rows (16 KB)
-                            uint4* slab = reinterpret_cast<uint4*>(ring + (cl >> 6) * (kBlockM * 128)) + row * 8;
-                            const int u0 = (cl & 32) ? 4 : 0;
+                    } else {
 #pragma unroll
-                            for (int j = 0; j < 4; ++j) {
-                                uint4 u;
-                                u.x = F16 ? pack16x2_rt(v[8 * j + 0], v[8 * j + 1], 1) : pack_bf16x2(v[8 * j + 0], v[8 * j + 1]);
-                                u.y = F16 ? pack16x2_rt(v[8 * j + 2], v[8 * j + 3], 1) : pack_bf16x2(v[8 * j + 2], v[8 * j + 3]);
-                                u.z = F16 ? pack16x2_rt(v[8 * j + 4], v[8 * j + 5], 1) : pack_bf16x2(v[8 * j + 4], v[8 * j + 5]);
-                                u.w = F16 ? pack16x2_rt(v[8 * j + 6], v[8 * j + 7], 1) : pack_bf16x2(v[8 * j + 6], v[8 * j + 7]);
-                                slab[(u0 + j) ^ (row & 7)] = u;
-                            }
-                        } else {                                             // fp32: slabs of 32 columns x 128 rows (16 KB)
-                            uint4* slab = reinterpret_cast<uint4*>(ring + (cl >> 5) * (kBlockM * 128)) + row * 8;
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) {
-                                const float4 f = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-                                slab[j ^ (row & 7)] = *reinterpret_cast<const uint4*>(&f);
-                            }
-                        }
-                        return;
-                    }
-                    uint4* xb = reinterpret_cast<uint4*>(s_xpose + ew * Cfg::kXposeBytesPerWarp);
-                    const int nvalid = p.N - nc;                                   // < 32 in a ragged last chunk, <= 0 beyond N
-                    const bool fast16 = st_fast && nvalid >= 32 && p.out_bf16 != nullptr;
-                    const bool fast32 = st_fast && nvalid > 0 && p.out_f32 != nullptr;                 // all warp-uniform
-                    if (fast32) store_f32_sw(xb, out_f32, p.ld_f32, m0 + q * 32, p.M, nc, v, lane, nvalid);
-                    if (fast16) {
-                        if constexpr (MODE == 3) {
-                            // fp32-parity mode: the 16-bit operand is written as fp16 hi | lo | hi per 64 columns (split_col),
-                            // so the consuming GEMM's K' = 3K contraction against W' = hi | hi | lo adds hi.hi + lo.hi + hi.lo
-                            const int c3 = split_col(nc);
-                            store16_sw<F16>(xb, p.out_bf16, p.ld_bf16, m0 + q * 32, p.M, c3, v, lane);
-                            store16_sw<F16>(xb, p.out_bf16, p.ld_bf16, m0 + q * 32, p.M, c3 + 128, v, lane);
-#pragma unroll
-                            for (int j = 0; j < 32; ++j) v[j] = split_lo(v[j]);
-                            store16_sw<F16>(xb, p.out_bf16, p.ld_bf16, m0 + q * 32, p.M, c3 + 64, v, lane);
-                        } else {
-                            store16_sw<F16>(xb, p.out_bf16, p.ld_bf16, m0 + q * 32, p.M, nc, v, lane);
-                        }
-                    }
-                    if (m_ok && nvalid > 0 && ((p.out_f32 != nullptr && !fast32) || (p.out_bf16 != nullptr && !fast16))) {
-                        GemmEpilogue ps = p;                       // per-lane (ragged 16-bit / odd stride) remainder
-                        ps.out_f32 = out_f32;
-                        if (fast32) ps.out_f32 = nullptr;
-                        if (fast16) ps.out_bf16 = nullptr;
-                        store_chunk<F16>(ps, m, nc, false, v);
-                    }
-                };
-                {
-                    // eight warps: column group g = ew / 4 takes chunks [g * kNC/2, (g+1) * kNC/2)
-                    constexpr int kCPG = kNC / 2;
-                    const int g = ew >> 2;
-#pragma unroll
-                    for (int ci = 0; ci < kCPG; ++ci) {
-                        const int c = g * kCPG + ci;
-                        float v[32];
-                        acc_ld32(acc_row + c * 32, v);
-                        if (stamp && ci == 0) stamps[14] = clock64();         // first chunk in registers
-                        finish_chunk(v, n0 + c * 32);
-                        if (stamp && ci == 0) stamps[15] = clock64();         // first chunk stored
+                        for (int j = 0; j < 32; ++j) if (nc + j < p.N) v[j] *= mp[j];
                     }
                 }
                 if (use_tma) {
-                    fence_proxy_async_smem();                        // my staged rows -> visible to the TMA
-                    epi_bar_sync<kEpiThreads>();                     // ... and everybody else's
-                    if (et == 0) {
-                        if (p.tma_store == 1) {
-                            for (int sl = 0; sl < BLOCK_N / 64; ++sl)
-                                if (n0 + sl * 64 < p.N) tma_store_2d(&tmap_c, ring + sl * (kBlockM * 128), n0 + sl * 64, m0);
-                        } else {
-                            for (int sl = 0; sl < BLOCK_N / 32; ++sl)
-                                if (n0 + sl * 32 < p.N) tma_store_2d(&tmap_c, ring + sl * (kBlockM * 128), n0 + sl * 32, m0);
+                    // last tile of this CTA: the operand ring is idle -> stage the tile there in the TMA's SWIZZLE_128B
+                    // layout (16-byte unit u of row r at u ^ (r & 7): row-per-lane writes are bank-conflict free)
+                    const int cl = nc - n0;
+                    if (p.tma_store == 1) {                              // 16-bit: slabs of 64 columns x 128 rows (16 KB)
+                        uint4* slab = reinterpret_cast<uint4*>(ring + (cl >> 6) * (kBlockM * 128)) + row * 8;
+                        const int u0 = (cl & 32) ? 4 : 0;
+#pragma unroll
+                        for (int j = 0; j < 4; ++j) {
+                            uint4 u;
+                            u.x = F16 ? pack16x2_rt(v[8 * j + 0], v[8 * j + 1], 1) : pack_bf16x2(v[8 * j + 0], v[8 * j + 1]);
+                            u.y = F16 ? pack16x2_rt(v[8 * j + 2], v[8 * j + 3], 1) : pack_bf16x2(v[8 * j + 2], v[8 * j + 3]);
+                            u.z = F16 ? pack16x2_rt(v[8 * j + 4], v[8 * j + 5], 1) : pack_bf16x2(v[8 * j + 4], v[8 * j + 5]);
+                            u.w = F16 ? pack16x2_rt(v[8 * j + 6], v[8 * j + 7], 1) : pack_bf16x2(v[8 * j + 6], v[8 * j + 7]);
+                            slab[(u0 + j) ^ (row & 7)] = u;
                         }
-                        tma_store_commit_and_wait_read();            // the ring is read before this CTA tears down
-                    }
-                }
-                if (stamp) { stamps[5] = clock64(); stamps[7] = clock64(); }
-                if (tile + tile_stride < total_tiles) epi_bar_sync<kEpiThreads>();   // bias slice and s_acc free for the next tile
-            } else {
-                // ------------------------------------------------ LayerNorm epilogue: 8 warps, row slice in registers
-                constexpr int kCPT = Cfg::kCPT;
-                const int c_begin = half * kCPT;                                  // this thread's chunks [c_begin, c_end)
-                const int c_end = (c_begin + kCPT < kNC) ? c_begin + kCPT : kNC;
-                const int my_cols = (c_end - c_begin) * 32;
-                const bool has_res = p.res != nullptr && m_ok;
-                float x[kCPT][32];
-                float4 rcur[8];
-                if (has_res) res_load(p, m, n0 + c_begin * 32, true, rcur);       // in flight while the MMAs run
-                mma_tile(tile, it);
-                if (stamp) stamps[4] = clock64();
+                    } else {                                             // fp32: slabs of 32 columns x 128 rows (16 KB)
+                        uint4* slab = reinterpret_cast<uint4*>(ring + (cl >> 5) * (kBlockM * 128)) + row * 8;
 #pragma unroll
-                for (int i = 0; i < kCPT; ++i)
-                    if (c_begin + i < c_end) acc_ld32(acc_row + (c_begin + i) * 32, x[i]);   // the partials barrier below frees s_acc
-                float lsum = 0.0f;
-#pragma unroll
-                for (int i = 0; i < kCPT; ++i) {
-                    if (c_begin + i < c_end) {
-                        if (has_res) {
-                            res_add(x[i], rcur);
-                            // next chunk's residual reuses the same registers and flies behind this chunk's bias / GELU
-                            if (i + 1 < kCPT && c_begin + i + 1 < c_end) res_load(p, m, n0 + (c_begin + i + 1) * 32, true, rcur);
+                        for (int j = 0; j < 8; ++j) {
+                            const float4 f = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+                            slab[j ^ (row & 7)] = *reinterpret_cast<const uint4*>(&f);
                         }
-                        bias_act32<ACT>(x[i], s_bias + (c_begin + i) * 32);
+                    }
+                    return;
+                }
+                uint4* xb = reinterpret_cast<uint4*>(s_xpose + ew * Cfg::kXposeBytesPerWarp);
+                const int nvalid = p.N - nc;                                   // < 32 in a ragged last chunk, <= 0 beyond N
+                const bool fast16 = st_fast && nvalid >= 32 && p.out_bf16 != nullptr;
+                const bool fast32 = st_fast && nvalid > 0 && p.out_f32 != nullptr;                 // all warp-uniform
+                if (fast32) store_f32_sw(xb, out_f32, p.ld_f32, m0 + q * 32, p.M, nc, v, lane, nvalid);
+                if (fast16) {
+                    if constexpr (MODE == 3) {
+                        // fp32-parity mode: the 16-bit operand is written as fp16 hi | lo | hi per 64 columns (split_col),
+                        // so the consuming GEMM's K' = 3K contraction against W' = hi | hi | lo adds hi.hi + lo.hi + hi.lo
+                        const int c3 = split_col(nc);
+                        store16_sw<F16>(xb, p.out_bf16, p.ld_bf16, m0 + q * 32, p.M, c3, v, lane);
+                        store16_sw<F16>(xb, p.out_bf16, p.ld_bf16, m0 + q * 32, p.M, c3 + 128, v, lane);
 #pragma unroll
-                        for (int j = 0; j < 32; ++j) lsum += x[i][j];
+                        for (int j = 0; j < 32; ++j) v[j] = split_lo(v[j]);
+                        store16_sw<F16>(xb, p.out_bf16, p.ld_bf16, m0 + q * 32, p.M, c3 + 64, v, lane);
+                    } else {
+                        store16_sw<F16>(xb, p.out_bf16, p.ld_bf16, m0 + q * 32, p.M, nc, v, lane);
                     }
                 }
-                const float lmean = lsum / static_cast<float>(my_cols);
-                float m2 = 0.0f;
-#pragma unroll
-                for (int i = 0; i < kCPT; ++i) {
-                    if (c_begin + i < c_end) {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) { const float d = x[i][j] - lmean; m2 = fmaf(d, d, m2); }
-                    }
+                if (m_ok && nvalid > 0 && ((p.out_f32 != nullptr && !fast32) || (p.out_bf16 != nullptr && !fast16))) {
+                    GemmEpilogue ps = p;                       // per-lane (ragged 16-bit / odd stride) remainder
+                    ps.out_f32 = out_f32;
+                    if (fast32) ps.out_f32 = nullptr;
+                    if (fast16) ps.out_bf16 = nullptr;
+                    store_chunk<F16>(ps, m, nc, false, v);
                 }
-                if (stamp) stamps[5] = clock64();
-                // ---- ONE exchange of (mean_local, M2_local) per row, column half and CTA
-                float2* part = s_part + (it & 1u) * (2 * kBlockM);                // double-buffered across tiles
-                part[half * kBlockM + row] = make_float2(lmean, m2);
-                epi_bar_sync<kEpiThreads>();                                     // this CTA's partials are all written
-                uint64_t* lb = &ln_bar[it & 1u];
-                // one release-arrive per (CTA, peer), issued by cluster_size lanes in parallel (serialising 8 remote arrives
-                // per warp in one lane cost ~6 k cycles); bar.sync ordered the other threads' writes before it
-                if (ew == 0 && lane < static_cast<int>(cluster_size)) mbar_arrive_remote_release(mapa_u32(lb, lane));
-                mbar_wait_acquire_cluster(lb, (it >> 1) & 1u);                    // every CTA's partials for this tile are visible
-                constexpr float kColsH0 = static_cast<float>(kCPT * 32);          // columns of half 0
-                constexpr float kColsH1 = static_cast<float>(BLOCK_N - kCPT * 32);  // columns of half 1
-                // two passes over the peers' partials (the second re-reads them) keep the register budget independent of the
-                // cluster size; the summation order is fixed, so the result does not depend on timing
-                float tot = 0.0f;
+            };
+            {
+                // eight warps: column group g = ew / 4 takes chunks [g * kNC/2, (g+1) * kNC/2)
+                constexpr int kCPG = kNC / 2;
+                const int g = ew >> 2;
 #pragma unroll
-                for (uint32_t rk = 0; rk < kMaxCluster; ++rk) {
-                    if (rk < cluster_size) {
-                        const float2 a0 = dsmem_ld_f32x2(mapa_u32(&part[row], rk));
-                        const float2 a1 = dsmem_ld_f32x2(mapa_u32(&part[kBlockM + row], rk));
-                        tot += a0.x * kColsH0 + a1.x * kColsH1;
-                    }
+                for (int ci = 0; ci < kCPG; ++ci) {
+                    const int c = g * kCPG + ci;
+                    float v[32];
+                    acc_ld32(acc_row + c * 32, v);
+                    if (stamp && ci == 0) stamps[14] = clock64();         // first chunk in registers
+                    finish_chunk(v, n0 + c * 32);
+                    if (stamp && ci == 0) stamps[15] = clock64();         // first chunk stored
                 }
-                const float mean = tot / static_cast<float>(p.N);
-                float M2 = 0.0f;
-#pragma unroll
-                for (uint32_t rk = 0; rk < kMaxCluster; ++rk) {
-                    if (rk < cluster_size) {
-                        const float2 a0 = dsmem_ld_f32x2(mapa_u32(&part[row], rk));
-                        const float2 a1 = dsmem_ld_f32x2(mapa_u32(&part[kBlockM + row], rk));
-                        const float d0 = a0.x - mean, d1 = a1.x - mean;
-                        M2 += a0.y + kColsH0 * d0 * d0 + a1.y + kColsH1 * d1 * d1;
-                    }
-                }
-                const float rstd = 1.0f / sqrtf(M2 / static_cast<float>(p.N) + p.eps);
-                if (stamp) stamps[6] = clock64();
-#pragma unroll
-                for (int i = 0; i < kCPT; ++i) {
-                    if (c_begin + i < c_end) {
-                        const int cc = (c_begin + i) * 32;
-#pragma unroll
-                        for (int j4 = 0; j4 < 8; ++j4) {
-                            const float4 g = reinterpret_cast<const float4*>(s_gamma + cc)[j4];
-                            const float4 b = reinterpret_cast<const float4*>(s_beta + cc)[j4];
-                            x[i][4 * j4 + 0] = (x[i][4 * j4 + 0] - mean) * rstd * g.x + b.x;
-                            x[i][4 * j4 + 1] = (x[i][4 * j4 + 1] - mean) * rstd * g.y + b.y;
-                            x[i][4 * j4 + 2] = (x[i][4 * j4 + 2] - mean) * rstd * g.z + b.z;
-                            x[i][4 * j4 + 3] = (x[i][4 * j4 + 3] - mean) * rstd * g.w + b.w;
-                        }
-                        store_ln_coalesced<F16>(reinterpret_cast<float*>(s_xpose + ew * Cfg::kXposeBytesPerWarp), p, m0 + q * 32,
-                                                n0 + cc, x[i], lane);                  // output strides are validated on the host
-                    }
-                }
-                if (stamp) stamps[7] = clock64();
             }
+            if (use_tma) {
+                fence_proxy_async_smem();                        // my staged rows -> visible to the TMA
+                epi_bar_sync<kEpiThreads>();                     // ... and everybody else's
+                if (et == 0) {
+                    if (p.tma_store == 1) {
+                        for (int sl = 0; sl < BLOCK_N / 64; ++sl)
+                            if (n0 + sl * 64 < p.N) tma_store_2d(&tmap_c, ring + sl * (kBlockM * 128), n0 + sl * 64, m0);
+                    } else {
+                        for (int sl = 0; sl < BLOCK_N / 32; ++sl)
+                            if (n0 + sl * 32 < p.N) tma_store_2d(&tmap_c, ring + sl * (kBlockM * 128), n0 + sl * 32, m0);
+                    }
+                    tma_store_commit_and_wait_read();            // the ring is read before this CTA tears down
+                }
+            }
+            if (stamp) { stamps[5] = clock64(); stamps[7] = clock64(); }
+            if (tile + tile_stride < total_tiles) epi_bar_sync<kEpiThreads>();   // bias slice and s_acc free for the next tile
         }
     }
 
     // ---------------------------------------------------------------- teardown
-    // nobody exits while a peer may still read its partials (LN)
-    if (LN) cluster_sync_all(); else __syncthreads();
+    __syncthreads();
     if (stamps && threadIdx.x == 0) {
         unsigned long long gt;
         asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt));
@@ -767,21 +555,14 @@ inline int num_sms() {
     return n;
 }
 
-template <typename Cfg, bool LN>
-void fill_cfg(cudaLaunchConfig_t& cfg, cudaLaunchAttribute* attrs, dim3 grid, int cluster, int pdl, cudaStream_t st) {
+template <typename Cfg>
+void fill_cfg(cudaLaunchConfig_t& cfg, cudaLaunchAttribute* attrs, dim3 grid, int pdl, cudaStream_t st) {
     cfg = cudaLaunchConfig_t{};
     cfg.gridDim = grid;
     cfg.blockDim = dim3(Cfg::kThreads, 1, 1);
     cfg.dynamicSmemBytes = Cfg::kSmemBytes;
     cfg.stream = st;
     unsigned na = 0;
-    if (LN || cluster > 1) {
-        attrs[na].id = cudaLaunchAttributeClusterDimension;
-        attrs[na].val.clusterDim.x = cluster;
-        attrs[na].val.clusterDim.y = 1;
-        attrs[na].val.clusterDim.z = 1;
-        ++na;
-    }
     if (pdl) {
         attrs[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
         attrs[na].val.programmaticStreamSerializationAllowed = 1;
@@ -805,32 +586,21 @@ inline int persistent_grid(int tiles, int grid_pct) {
     return g;
 }
 
-// resident: LN only -- how many clusters of this size can be co-resident (grid.y is capped to it)
-template <int BLOCK_N, bool LN, int ACT, bool F16, int MODE = 0>
-cudaError_t launch_p(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilogue& ep, int resident, cudaStream_t st) {
-    using Cfg = PCfg<BLOCK_N, LN, MODE>;
-    auto kern = gemm_persistent_kernel<BLOCK_N, LN, ACT, F16, MODE>;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
-    if (e == cudaSuccess && LN) e = cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+template <int BLOCK_N, int ACT, bool F16, int MODE = 0>
+cudaError_t launch_p(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilogue& ep, cudaStream_t st) {
+    using Cfg = PCfg<BLOCK_N, MODE>;
+    auto kern = gemm_persistent_kernel<BLOCK_N, ACT, F16, MODE>;
+    const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
     if (e != cudaSuccess) return e;
     const int n_tiles = (ep.N + BLOCK_N - 1) / BLOCK_N;
     const int m_tiles = (ep.M + kBlockM - 1) / kBlockM;
-    dim3 grid;
-    int cluster = 1;
-    if (LN) {
-        cluster = n_tiles;
-        if (resident <= 0) return cudaErrorInvalidConfiguration;
-        grid = dim3(cluster, std::min(m_tiles, resident), 1);
-    } else {
-        static_assert(Cfg::kMinBlocks == 1, "persistent_grid assumes one CTA per SM");
-        grid = dim3(persistent_grid(m_tiles * n_tiles, ep.grid_pct), 1, 1);
-    }
+    static_assert(Cfg::kMinBlocks == 1, "persistent_grid assumes one CTA per SM");
     cudaLaunchConfig_t cfg;
-    cudaLaunchAttribute attrs[2];
-    fill_cfg<Cfg, LN>(cfg, attrs, grid, cluster, ep.pdl == 1 || ep.pdl == 5, st);
+    cudaLaunchAttribute attrs[1];
+    fill_cfg<Cfg>(cfg, attrs, dim3(persistent_grid(m_tiles * n_tiles, ep.grid_pct), 1, 1), ep.pdl == 1 || ep.pdl == 5, st);
     GemmEpilogue e2 = ep;
     const CUtensorMap* tc = static_cast<const CUtensorMap*>(ep.tmap_c_host);
-    if (tc == nullptr || LN) { e2.tma_store = 0; tc = &ta; }                       // &ta: any valid map for the unused slot
+    if (tc == nullptr) { e2.tma_store = 0; tc = &ta; }                             // &ta: any valid map for the unused slot
     return cudaLaunchKernelEx(&cfg, kern, ta, tb, *tc, e2, m_tiles, n_tiles);
 }
 

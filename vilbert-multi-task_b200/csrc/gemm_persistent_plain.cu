@@ -1,17 +1,25 @@
-// Plain (bias / GELU / ReLU / pooled-product) instantiations of the persistent wgmma GEMM; see gemm_persistent.cuh.
+// Instantiations (bias / GELU / ReLU / pooled-product) and launcher of the persistent wgmma GEMM; see gemm_persistent.cuh.
 #include <cstdlib>
 #include "gemm_persistent.cuh"
 
 namespace vb {
 using namespace pgemm;
 
+int num_sms_host() { return pgemm::num_sms(); }
+
+int gemm_p_pick_block_n(int N) {
+    static const int forced = [] { const char* e = getenv("VB200_BN"); return e ? atoi(e) : 0; }();   // A/B switch
+    if ((forced == 64 || forced == 128) && N % forced == 0) return forced;
+    return N <= 64 ? 64 : 128;
+}
+
 template <int BN, int MODE>
 static cudaError_t dispatch_act(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilogue& ep, cudaStream_t st) {
     const bool f16 = ep.a_f16 != 0;
     switch (ep.act) {
-        case kActNone: return f16 ? launch_p<BN, false, kActNone, true, MODE>(ta, tb, ep, 0, st) : launch_p<BN, false, kActNone, false, MODE>(ta, tb, ep, 0, st);
-        case kActGelu: return f16 ? launch_p<BN, false, kActGelu, true, MODE>(ta, tb, ep, 0, st) : launch_p<BN, false, kActGelu, false, MODE>(ta, tb, ep, 0, st);
-        case kActRelu: return f16 ? launch_p<BN, false, kActRelu, true, MODE>(ta, tb, ep, 0, st) : launch_p<BN, false, kActRelu, false, MODE>(ta, tb, ep, 0, st);
+        case kActNone: return f16 ? launch_p<BN, kActNone, true, MODE>(ta, tb, ep, st) : launch_p<BN, kActNone, false, MODE>(ta, tb, ep, st);
+        case kActGelu: return f16 ? launch_p<BN, kActGelu, true, MODE>(ta, tb, ep, st) : launch_p<BN, kActGelu, false, MODE>(ta, tb, ep, st);
+        case kActRelu: return f16 ? launch_p<BN, kActRelu, true, MODE>(ta, tb, ep, st) : launch_p<BN, kActRelu, false, MODE>(ta, tb, ep, st);
     }
     return cudaErrorInvalidValue;
 }
@@ -20,17 +28,17 @@ static cudaError_t dispatch_act(const CUtensorMap& ta, const CUtensorMap& tb, co
 template <int BN>
 static cudaError_t dispatch_split(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilogue& ep, cudaStream_t st) {
     switch (ep.act) {
-        case kActNone: return launch_p<BN, false, kActNone, true, 3>(ta, tb, ep, 0, st);
+        case kActNone: return launch_p<BN, kActNone, true, 3>(ta, tb, ep, st);
         case kActGelu:
-        case kActGeluExact: return launch_p<BN, false, kActGeluExact, true, 3>(ta, tb, ep, 0, st);
-        case kActRelu: return launch_p<BN, false, kActRelu, true, 3>(ta, tb, ep, 0, st);
+        case kActGeluExact: return launch_p<BN, kActGeluExact, true, 3>(ta, tb, ep, st);
+        case kActRelu: return launch_p<BN, kActRelu, true, 3>(ta, tb, ep, st);
     }
     return cudaErrorInvalidValue;
 }
 
 cudaError_t launch_gemm_persistent_plain(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilogue& ep, int block_n,
                                          cudaStream_t st) {
-    if (ep.res != nullptr || ep.a_f16 != ep.out_f16) return cudaErrorInvalidValue;   // residual only with LayerNorm
+    if (ep.M < 1 || ep.N < 1 || ep.K < 1 || ep.a_f16 != ep.out_f16) return cudaErrorInvalidValue;
     if (ep.split16 || ep.act == kActGeluExact) {
         // hi | lo | hi output: fp16, whole 64-column groups, no TMA store; narrow tiles only (the mode is for parity, not speed)
         if (!ep.a_f16 || (ep.split16 && (ep.out_bf16 == nullptr || (ep.N & 63) || (ep.ld_bf16 & 7))) || ep.tma_store == 1)

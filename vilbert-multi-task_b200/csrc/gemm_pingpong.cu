@@ -14,9 +14,9 @@ static cudaError_t launch_pp(const CUtensorMap& ta, const CUtensorMap& tb, const
     const int n_tiles = ep.N / BN;
     const int m_tiles = (ep.M + kBlockM - 1) / kBlockM;
     cudaLaunchConfig_t cfg;
-    cudaLaunchAttribute attrs[2];
-    pgemm::fill_cfg<Cfg, false>(cfg, attrs, dim3(pgemm::persistent_grid(m_tiles * n_tiles, ep.grid_pct), 1, 1), 1,
-                                ep.pdl == 1 || ep.pdl == 5, st);
+    cudaLaunchAttribute attrs[1];
+    pgemm::fill_cfg<Cfg>(cfg, attrs, dim3(pgemm::persistent_grid(m_tiles * n_tiles, ep.grid_pct), 1, 1), ep.pdl == 1 || ep.pdl == 5,
+                         st);
     return cudaLaunchKernelEx(&cfg, kern, ta, tb, tc16, tc32, ep, m_tiles, n_tiles);
 }
 
@@ -34,7 +34,7 @@ static cudaError_t dispatch_pp(const CUtensorMap& ta, const CUtensorMap& tb, con
 
 bool gemm_pingpong_supports(const GemmEpilogue& ep, int block_n) {
     return (block_n == 64 || block_n == 128) && ep.M >= 1 && ep.K >= 1 && ep.N >= block_n && ep.N % block_n == 0 &&
-           ep.res == nullptr && ep.gamma == nullptr && ep.mul == nullptr && !ep.split16 && ep.a_f16 == ep.out_f16 &&
+           ep.mul == nullptr && !ep.split16 && ep.a_f16 == ep.out_f16 &&
            (ep.act == kActNone || ep.act == kActGelu || ep.act == kActRelu) && (ep.out_bf16 != nullptr || ep.out_f32 != nullptr);
 }
 

@@ -7,17 +7,12 @@ namespace vb {
 
 enum Act : int { kActNone = 0, kActGelu = 1, kActRelu = 2, kActGeluExact = 3 };   // 3: erf to 1.5e-7 (fp32-parity mode)
 
-// Epilogue of the wgmma GEMM:  x = act(acc + bias + res) * mul ; LN variant: y = LayerNorm(x) * gamma + beta.
+// Epilogue of the wgmma GEMM:  y = act(acc + bias) * mul.
 struct GemmEpilogue {
     int M, N, K;
     const float* bias;            // [N] or null
-    const float* res;             // fp32 [M, ld_res] residual or null (may alias out_f32)
-    int ld_res;
     const float* mul;             // fp32 [M, ld_mul] multiplicand (pooled_t * pooled_v fusion) or null
     int ld_mul;
-    const float* gamma;           // LN only
-    const float* beta;
-    float eps;
     __nv_bfloat16* out_bf16;      // optional
     int ld_bf16;
     float* out_f32;               // optional
@@ -41,21 +36,18 @@ struct GemmEpilogue {
     const int* m_rows;            // optional device row count (packed batches): rows >= min(*m_rows, M) are neither loaded nor
                                   // computed -- the tile list ends at the last 128-row tile holding a row below it.  Written
                                   // before the launch's graph starts, so it is read ahead of griddepcontrol.wait.  Honoured by
-                                  // the plain persistent kernel (PCfg MODE 6 in place of MODE 0); the fp32-parity and
-                                  // cluster-LayerNorm kernels compute every row.
+                                  // the persistent kernel (PCfg MODE 6 in place of MODE 0); the fp32-parity kernel
+                                  // computes every row.
 };
 
-// persistent CTAs / clusters, wgmma consumer warpgroups, single-exchange LayerNorm (gemm_persistent.cuh)
-int gemm_p_pick_block_n(int N, bool ln);
-int gemm_p_max_clusters(int block_n, int cluster);
-cudaError_t launch_gemm_persistent(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b, const GemmEpilogue& ep,
-                                   int block_n, bool ln, cudaStream_t st);
+// persistent CTAs, wgmma consumer warpgroups (gemm_persistent.cuh)
+int gemm_p_pick_block_n(int N);
 int num_sms_host();          // SM count of the current device (132 on H100 SXM)
 cudaError_t launch_gemm_persistent_plain(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b, const GemmEpilogue& ep,
                                          int block_n, cudaStream_t st);
 // ping-pong consumer warpgroups (gemm_pingpong.cuh): plain bias / activation GEMMs with N a multiple of block_n (64 or 128), no
-// residual, LayerNorm, pooled product or fp32-parity output; every output leaves through its TMA map (tmap_c16 for out_bf16,
-// tmap_c32 for out_f32, SWIZZLE_128B boxes of 128 rows x 128 bytes).  Same bits as launch_gemm_persistent.
+// pooled product or fp32-parity output; every output leaves through its TMA map (tmap_c16 for out_bf16, tmap_c32 for out_f32,
+// SWIZZLE_128B boxes of 128 rows x 128 bytes).  Same bits as launch_gemm_persistent_plain.
 bool gemm_pingpong_supports(const GemmEpilogue& ep, int block_n);
 cudaError_t launch_gemm_pingpong(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b, const CUtensorMap* tmap_c16,
                                  const CUtensorMap* tmap_c32, const GemmEpilogue& ep, int block_n, cudaStream_t st);
@@ -75,7 +67,7 @@ cudaError_t launch_co_attention(const __nv_bfloat16* qkv_img, int ld_img, const 
                                 int T, int V, int heads, int head_dim, int pdl, int f16, cudaStream_t st,
                                 const int* offs_t = nullptr, const int* offs_v = nullptr);   // as launch_self_attention, per stream
 
-// un-fused LayerNorm(y + res): fp32 stream out + 16-bit operand out (layernorm.cu); split16: hi | lo | hi operand (fp32-parity mode)
+// LayerNorm(y + res) of a GEMM's fp32 output: fp32 stream out + 16-bit operand out (layernorm.cu); split16: hi | lo | hi operand (fp32-parity mode)
 cudaError_t launch_ln_residual(const float* y, int ld_y, const float* res, int ld_res, const float* gamma, const float* beta,
                                float eps, float* out_f32, int ld_f32, __nv_bfloat16* out16, int ld16, int M, int N, int f16,
                                int split16, int pdl, cudaStream_t st,

@@ -1,10 +1,10 @@
 // Residual-add + LayerNorm row kernel: x = y + res; out = (x - mean) / sqrt(var + eps) * gamma + beta, written as the
 // fp32 residual stream AND the 16-bit operand of the next GEMM.
 //
-// This is the un-fused alternative to the cluster-LayerNorm GEMM epilogue (gemm_persistent_ln.cu): the fused epilogue needs a
-// cluster-wide exchange plus ~2000 dependent instructions per thread, while a plain GEMM that writes fp32 followed by this
-// L2-resident row kernel (one warp per row, 16-byte coalesced accesses, two-pass fp32 statistics in registers) keeps the GEMM
-// epilogue light.  Replaces BertSelfOutput / BertOutput / BertBiOutput `LayerNorm(dense(x) + residual)` and the
+// Every LayerNorm after a GEMM runs here: the GEMM writes fp32, and this L2-resident row kernel (one warp per row, 16-byte
+// coalesced accesses, two-pass fp32 statistics in registers) normalises it.  A row of N columns spans N / BLOCK_N GEMM tiles, so
+// normalising inside the GEMM epilogue would need an exchange of statistics across CTAs; keeping it here keeps the GEMM epilogue
+// light.  Replaces BertSelfOutput / BertOutput / BertBiOutput `LayerNorm(dense(x) + residual)` and the
 // LayerNorm inside SimpleClassifier ([UPSTREAM] vilbert/vilbert.py; anchor worker.py:286-289).
 #include <cstdlib>
 #include "kernels.h"
