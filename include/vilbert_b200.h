@@ -15,8 +15,9 @@
  * in one forward, plans keyed on capacity buckets, GEMM tiles past the call's row totals skipped), detector output in, dense or
  * packed (vb200_region_inputs, vb200_packed_region_inputs: every image at its own box count), caption-image retrieval with reuse, dense or packed (vb200_packed_pairs: captions and images encoded once
  * at their own lengths, pairs scored without padding), the answer decode of every message of a batch in one kernel (vb200_decode_answers:
- * softmax, top N and grounding boxes, so a C host answers a message without re-implementing prediction()'s decode), and kernel-level
- * entry points for the tests.
+ * softmax, top N and grounding boxes, so a C host answers a message without re-implementing prediction()'s decode), the detector's
+ * region selection (vb200_select_regions: per-class NMS, confidence ranking and the top boxes of every image, written into the packed
+ * region inputs), and kernel-level entry points for the tests.
  * The Python shim in vilbert-multi-task_b200/ (ctypes) implements the protocol on top of them; see
  * INTEGRATION.md for the stub a maintainer of the reference would add.
  *
@@ -419,6 +420,62 @@ int vb200_decode_answers(vb200_handle h, const vb200_decode_msg* msgs /* HOST [n
 int vb200_decode_answers_host(vb200_handle h, const vb200_decode_msg* msgs /* HOST [n] */, int32_t n, const vb200_outputs* out,
                               int32_t batch, int32_t vision_rows, const float* spatials, vb200_answer* answers /* HOST [n] */,
                               void* cuda_stream);
+
+/* ---- Detector-region selection: the feature extraction step of the reference worker (worker.py:123-176) on the detector's raw heads,
+ * for every image of a batch in one call, written straight into the packed box_features / boxes that vb200_forward_regions_packed reads.
+ * For image i with n_i proposals, C score columns (column 0 is background) and features [n_i, F]:
+ *   p = softmax(scores_i) per proposal row (fp32: max, expf(x - max), sum, division by the sum);
+ *   dets = proposals_i / (float)im_scale_i (fp32 division: the original-pixel boxes);
+ *   max_conf[b] = the largest p[b, c] over the classes c >= start (start = 0 with background, else 1) whose NMS keeps b and with
+ *     p[b, c] > conf_thresh, else 0.  NMS: greedy in descending score order; IoU with the legacy "+1": w = max(min(x2) - max(x1) + 1, 0),
+ *     the same for h, areas (x2 - x1 + 1)(y2 - y1 + 1), IoU = inter / (Sa + Sb - inter), each step rounded in fp32; suppression when
+ *     IoU > nms_iou;
+ *   keep = the first k_i = min(max_boxes, n_i) indices of max_conf in descending order.
+ * Ties: equal scores rank the lower proposal index first, in every class's NMS order and in the final ranking.
+ * Outputs of image i are rows [dst_row, dst_row + k_i) of each per-row output: box_features = features_i[keep], boxes = dets[keep],
+ * and optionally keep_index, the sorted max_conf, cls_prob = p[keep] (full rows) and objects = argmax over all C columns of each
+ * cls_prob row (ties: lower column).  num_boxes[i] = the count of nonzero max_conf among the k_i.  (The reference's objects is the
+ * argmax of rows start .. k_i - 1 of p[keep]: objects[start:] of this output.)  Rows outside those ranges are not written, so a caller
+ * can leave rows free for the filler images of a packed batch.
+ * Limits: 1 <= n_i <= 2048, 2 <= C <= 2048, F a positive multiple of 4, 1 <= max_boxes <= 255, 0 < nms_iou <= 1, background 0 or 1,
+ * 1 <= n <= 65535, im_scale > 0.  VB200_ERR_INVALID, with a message naming the image where there is one, for a limit broken, a NULL
+ * required pointer, a features or box_features pointer not 16-byte aligned, and destination ranges that overlap or fall outside
+ * [0, out_rows); nothing is enqueued then.
+ * Asynchronous on cuda_stream.  The descriptors reach the device through a pinned staging buffer, and the workspace (row stats, IoU
+ * bitmasks, max_conf) is owned by the engine and grows on demand.  The call blocks only when that workspace grows, or while the previous
+ * call's copy out of the staging buffer is still in flight; a call's kernels wait on the device for the previous call's, so
+ * back-to-back calls need no synchronisation in between. */
+typedef struct {
+    int32_t n_proposals;           /* n_i */
+    int32_t dst_row;               /* first output row of image i */
+    double im_scale;               /* detector input scale: boxes are proposals / (float)im_scale */
+    const float* proposals;        /* DEVICE [n_i, 4] x1, y1, x2, y2 at the detector's input scale */
+    const float* scores;           /* DEVICE [n_i, n_classes] class logits, as the detector returns them */
+    const float* features;         /* DEVICE [n_i, feature_size] (fc6), 16-byte aligned */
+} vb200_detections;
+
+typedef struct {
+    int32_t n_classes;             /* C, background column included (1601) */
+    int32_t feature_size;          /* F (2048) */
+    int32_t max_boxes;             /* K (the worker's num_features, 100) */
+    float conf_thresh;             /* 0 in the worker */
+    float nms_iou;                 /* 0.5 in the worker */
+    int32_t background;            /* 1: class 0 takes part in the NMS (the worker's default is 0) */
+    int32_t out_rows;              /* rows of the per-row outputs */
+} vb200_select_params;
+
+typedef struct {
+    float* box_features;           /* required DEVICE [out_rows, F], 16-byte aligned */
+    float* boxes;                  /* required DEVICE [out_rows, 4] original-pixel x1, y1, x2, y2 */
+    int32_t* num_boxes;            /* required DEVICE [n] */
+    int32_t* keep_index;           /* optional DEVICE [out_rows]: proposal index within its image */
+    float* max_conf;               /* optional DEVICE [out_rows]: the sorted scores */
+    float* cls_prob;               /* optional DEVICE [out_rows, C] */
+    int64_t* objects;              /* optional DEVICE [out_rows] */
+} vb200_selected;
+
+int vb200_select_regions(vb200_handle h, const vb200_detections* imgs /* HOST [n] */, int32_t n, const vb200_select_params* p,
+                         const vb200_selected* out, void* cuda_stream);
 
 /* ---- Kernel-level entry points (device pointers), used by the parity tests and the roofline bench.  ---- */
 /* y = act(x[M,K] (16-bit) . w[N,K]^T (16-bit) + bias); act: 0 none, 1 GELU(erf), 2 ReLU.  residual, gamma and beta are reserved

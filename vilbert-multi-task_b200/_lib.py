@@ -102,6 +102,23 @@ class Answer(C.Structure):
                 ("box", (C.c_int32 * 4) * DECODE_MAX_TOP)]
 
 
+class Detections(C.Structure):
+    """vb200_detections: one image's raw detector heads (device pointers) and its first output row."""
+    _fields_ = [("n_proposals", C.c_int32), ("dst_row", C.c_int32), ("im_scale", C.c_double), ("proposals", C.c_void_p),
+                ("scores", C.c_void_p), ("features", C.c_void_p)]
+
+
+class SelectParams(C.Structure):
+    """vb200_select_params: what vb200_select_regions selects, and the rows of its per-row outputs."""
+    _fields_ = [("n_classes", C.c_int32), ("feature_size", C.c_int32), ("max_boxes", C.c_int32), ("conf_thresh", C.c_float),
+                ("nms_iou", C.c_float), ("background", C.c_int32), ("out_rows", C.c_int32)]
+
+
+class Selected(C.Structure):
+    """vb200_selected: device outputs of vb200_select_regions (the last four may be NULL)."""
+    _fields_ = [(n, C.c_void_p) for n in ("box_features", "boxes", "num_boxes", "keep_index", "max_conf", "cls_prob", "objects")]
+
+
 class Options(C.Structure):
     _fields_ = [("device", C.c_int32), ("num_labels", C.c_int32), ("use_cuda_graph", C.c_int32),
                 ("use_pdl", C.c_int32), ("strict", C.c_int32), ("act_fp16", C.c_int32),
@@ -115,7 +132,7 @@ EXPORTS = ["vb200_abi_version", "vb200_create", "vb200_destroy", "vb200_last_err
            "vb200_encode_text_packed", "vb200_encode_image_packed", "vb200_forward_cached_packed", "vb200_linear", "vb200_linear_rows", "vb200_linear_split", "vb200_layernorm", "vb200_layernorm_split", "vb200_attention_f32",
            "vb200_self_attention", "vb200_co_attention", "vb200_self_attention_packed", "vb200_co_attention_packed",
            "vb200_linear_product", "vb200_text_embed", "vb200_image_pack", "vb200_region_pack", "vb200_rowdot", "vb200_gather_state",
-           "vb200_gather_packed_state", "vb200_decode_answers", "vb200_decode_answers_host"]
+           "vb200_gather_packed_state", "vb200_decode_answers", "vb200_decode_answers_host", "vb200_select_regions"]
 
 _lib = None
 
@@ -185,6 +202,7 @@ def load():
     lib.vb200_gather_packed_state.argtypes = [i32, vp, vp, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp, i32, i32, vp]
     lib.vb200_decode_answers.argtypes = [vp, C.POINTER(DecodeMsg), i32, C.POINTER(Outputs), i32, i32, vp, vp, vp]
     lib.vb200_decode_answers_host.argtypes = [vp, C.POINTER(DecodeMsg), i32, C.POINTER(Outputs), i32, i32, vp, C.POINTER(Answer), vp]
+    lib.vb200_select_regions.argtypes = [vp, C.POINTER(Detections), i32, C.POINTER(SelectParams), C.POINTER(Selected), vp]
     for name in EXPORTS:
         if name not in ("vb200_last_error",):
             getattr(lib, name).restype = C.c_int

@@ -634,8 +634,20 @@ struct vb200_engine {
     cudaEvent_t dec_copied = nullptr;
     vb200_answer* ans_d = nullptr;
     size_t ans_cap = 0;
+    // region selection (vb200_select_regions): descriptors staged in the pinned sel_h (sel_copied: the last copy out of it), the
+    // workspace sel_ws holds the device descriptors, row stats, boxes, bitmasks, max_conf and keep lists; sel_done marks the end of
+    // the last call's kernels.  Both buffers grow on demand.
+    vb::SelectDesc* sel_h = nullptr;
+    size_t sel_h_cap = 0;
+    char* sel_ws = nullptr;
+    size_t sel_ws_bytes = 0;
+    cudaEvent_t sel_copied = nullptr, sel_done = nullptr;
 
     ~vb200_engine() {
+        if (sel_copied) { cudaEventSynchronize(sel_copied); cudaEventDestroy(sel_copied); }
+        if (sel_done) { cudaEventSynchronize(sel_done); cudaEventDestroy(sel_done); }
+        if (sel_h) cudaFreeHost(sel_h);
+        if (sel_ws) cudaFree(sel_ws);
         if (dec_copied) { cudaEventSynchronize(dec_copied); cudaEventDestroy(dec_copied); }
         if (dec_h) cudaFreeHost(dec_h);
         if (dec_d) cudaFree(dec_d);
@@ -1691,6 +1703,117 @@ struct vb200_engine {
         }
         return ans_d;
     }
+    // ---- region selection: every descriptor is checked before anything is enqueued
+    void select_regions(const vb200_detections* imgs, int n, const vb200_select_params* p, const vb200_selected* out, cudaStream_t st) {
+        const char* api = "vb200_select_regions";
+        if (imgs == nullptr || p == nullptr || out == nullptr) fail(VB200_ERR_INVALID, "%s: imgs / p / out is NULL", api);
+        if (n < 1 || n > 65535) fail(VB200_ERR_INVALID, "%s: n = %d outside [1, 65535]", api, n);
+        const int C = p->n_classes, F = p->feature_size, K = p->max_boxes;
+        if (C < 2 || C > 2048) fail(VB200_ERR_INVALID, "%s: n_classes = %d outside [2, 2048]", api, C);
+        if (F < 4 || F % 4 != 0) fail(VB200_ERR_INVALID, "%s: feature_size = %d is not a positive multiple of 4", api, F);
+        if (K < 1 || K > 255) fail(VB200_ERR_INVALID, "%s: max_boxes = %d outside [1, 255]", api, K);
+        if (!(p->nms_iou > 0.f && p->nms_iou <= 1.f)) fail(VB200_ERR_INVALID, "%s: nms_iou = %g outside (0, 1]", api, p->nms_iou);
+        if (std::isnan(p->conf_thresh)) fail(VB200_ERR_INVALID, "%s: conf_thresh is NaN", api);
+        if (p->background != 0 && p->background != 1) fail(VB200_ERR_INVALID, "%s: background = %d is not 0 or 1", api, p->background);
+        if (p->out_rows < 1) fail(VB200_ERR_INVALID, "%s: out_rows = %d", api, p->out_rows);
+        if (out->box_features == nullptr || out->boxes == nullptr || out->num_boxes == nullptr)
+            fail(VB200_ERR_INVALID, "%s: box_features, boxes and num_boxes are required", api);
+        if (reinterpret_cast<uintptr_t>(out->box_features) % 16 != 0) fail(VB200_ERR_INVALID, "%s: box_features is not 16-byte aligned", api);
+        if (reinterpret_cast<uintptr_t>(out->boxes) % 16 != 0) fail(VB200_ERR_INVALID, "%s: boxes is not 16-byte aligned", api);
+        std::vector<vb::SelectDesc> d(n);
+        std::vector<std::pair<int, int>> ranges(n);        // (dst_row, image)
+        size_t rows = 0, words = 0;
+        int max_n = 0, max_npad = 32;
+        for (int i = 0; i < n; ++i) {
+            const vb200_detections& m = imgs[i];
+            if (m.n_proposals < 1 || m.n_proposals > vb::kSelectMaxProposals)
+                fail(VB200_ERR_INVALID, "%s: image %d has %d proposals, outside [1, %d]", api, i, m.n_proposals, vb::kSelectMaxProposals);
+            if (m.proposals == nullptr || m.scores == nullptr || m.features == nullptr)
+                fail(VB200_ERR_INVALID, "%s: image %d has a NULL proposals / scores / features pointer", api, i);
+            if (reinterpret_cast<uintptr_t>(m.features) % 16 != 0) fail(VB200_ERR_INVALID, "%s: image %d's features are not 16-byte aligned", api, i);
+            if (!(m.im_scale > 0.0) || !std::isfinite(static_cast<float>(m.im_scale)))
+                fail(VB200_ERR_INVALID, "%s: image %d has im_scale %g", api, i, m.im_scale);
+            const int k = std::min(K, m.n_proposals);
+            if (m.dst_row < 0 || static_cast<int64_t>(m.dst_row) + k > p->out_rows)
+                fail(VB200_ERR_INVALID, "%s: image %d's rows [%d, %lld) fall outside out_rows %d", api, i, m.dst_row,
+                     static_cast<long long>(static_cast<int64_t>(m.dst_row) + k), p->out_rows);
+            int npad = 32;
+            while (npad < m.n_proposals) npad <<= 1;
+            vb::SelectDesc& s = d[i];
+            s.proposals = m.proposals;
+            s.scores = m.scores;
+            s.features = m.features;
+            s.row0 = rows;
+            s.mask0 = words;
+            s.im_scale = static_cast<float>(m.im_scale);
+            s.n = m.n_proposals;
+            s.npad = npad;
+            s.nw = (m.n_proposals + 31) / 32;
+            s.dst_row = m.dst_row;
+            s.k = k;
+            rows += m.n_proposals;
+            words += static_cast<size_t>(m.n_proposals) * s.nw;
+            max_n = std::max(max_n, m.n_proposals);
+            max_npad = std::max(max_npad, npad);
+            ranges[i] = {m.dst_row, i};
+        }
+        std::sort(ranges.begin(), ranges.end());
+        for (int r = 1; r < n; ++r) {
+            const vb::SelectDesc& a = d[ranges[r - 1].second];
+            if (a.dst_row + a.k > ranges[r].first)
+                fail(VB200_ERR_INVALID, "%s: image %d's rows [%d, %d) overlap image %d's rows starting at %d", api, ranges[r].second,
+                     ranges[r].first, ranges[r].first + d[ranges[r].second].k, ranges[r - 1].second, a.dst_row);
+        }
+        // workspace layout: descriptors, stats [rows] float2, dbox [rows] float4, max_conf [rows], keep [n, K], mask [words]
+        auto up = [](size_t b) { return (b + 255) & ~static_cast<size_t>(255); };
+        const size_t o_desc = 0, o_stats = up(o_desc + n * sizeof(vb::SelectDesc)), o_box = up(o_stats + rows * 8),
+                     o_conf = up(o_box + rows * 16), o_keep = up(o_conf + rows * 4), o_mask = up(o_keep + static_cast<size_t>(n) * K * 4),
+                     need = up(o_mask + words * 4);
+
+        if (sel_copied == nullptr) CUDA_CHECK(cudaEventCreateWithFlags(&sel_copied, cudaEventDisableTiming));
+        if (sel_done == nullptr) CUDA_CHECK(cudaEventCreateWithFlags(&sel_done, cudaEventDisableTiming));
+        CUDA_CHECK(cudaEventSynchronize(sel_copied));               // the previous call's copy has left the staging buffer
+        if (static_cast<size_t>(n) > sel_h_cap) {
+            const size_t cap = std::max<size_t>({static_cast<size_t>(n), 2 * sel_h_cap, 64});
+            if (sel_h) CUDA_CHECK(cudaFreeHost(sel_h));
+            sel_h = nullptr;
+            CUDA_CHECK(cudaMallocHost(&sel_h, cap * sizeof(vb::SelectDesc)));
+            sel_h_cap = cap;
+        }
+        if (need > sel_ws_bytes) {
+            CUDA_CHECK(cudaEventSynchronize(sel_done));             // the previous call's kernels are done with the old workspace
+            if (sel_ws) CUDA_CHECK(cudaFree(sel_ws));
+            sel_ws = nullptr;
+            const size_t cap = std::max(need, 2 * sel_ws_bytes);
+            CUDA_CHECK(cudaMalloc(&sel_ws, cap));
+            sel_ws_bytes = cap;
+        } else {
+            CUDA_CHECK(cudaStreamWaitEvent(st, sel_done, 0));       // the previous call (any stream) is done with the workspace
+        }
+        vb::SelectArgs a{};
+        a.C = C; a.F = F; a.K = K; a.start = p->background ? 0 : 1;
+        a.thr = std::max(p->conf_thresh, 0.f);
+        a.nms_iou = p->nms_iou;
+        a.stats = reinterpret_cast<float2*>(sel_ws + o_stats);
+        a.dbox = reinterpret_cast<float*>(sel_ws + o_box);
+        a.max_conf = reinterpret_cast<unsigned*>(sel_ws + o_conf);
+        a.keep = reinterpret_cast<int*>(sel_ws + o_keep);
+        a.mask = reinterpret_cast<unsigned*>(sel_ws + o_mask);
+        a.box_features = out->box_features;
+        a.boxes = out->boxes;
+        a.num_boxes = out->num_boxes;
+        a.keep_index = out->keep_index;
+        a.max_conf_out = out->max_conf;
+        a.cls_prob = out->cls_prob;
+        a.objects = out->objects;
+        const vb::SelectDesc* descs = reinterpret_cast<const vb::SelectDesc*>(sel_ws + o_desc);
+        memcpy(sel_h, d.data(), n * sizeof(vb::SelectDesc));
+        CUDA_CHECK(cudaMemcpyAsync(sel_ws + o_desc, sel_h, n * sizeof(vb::SelectDesc), cudaMemcpyHostToDevice, st));
+        CUDA_CHECK(cudaEventRecord(sel_copied, st));
+        CUDA_CHECK(cudaMemsetAsync(a.max_conf, 0, rows * 4, st));
+        CUDA_CHECK(vb::launch_select_regions(descs, n, max_n, max_npad, a, st));
+        CUDA_CHECK(cudaEventRecord(sel_done, st));
+    }
     static float* out_ptr(const vb200_outputs& o, int slot) {
         switch (slot) {
             case 0: return o.vil_prediction; case 1: return o.vil_prediction_gqa; case 2: return o.vil_logit;
@@ -2035,6 +2158,15 @@ int vb200_decode_answers_host(vb200_handle h, const vb200_decode_msg* msgs, int3
         h->decode_answers(d, dev, st);
         CUDA_CHECK(cudaMemcpyAsync(answers, dev, d.size() * sizeof(vb200_answer), cudaMemcpyDeviceToHost, st));
         CUDA_CHECK(cudaStreamSynchronize(st));
+    });
+}
+
+int vb200_select_regions(vb200_handle h, const vb200_detections* imgs, int32_t n, const vb200_select_params* p, const vb200_selected* out,
+                         void* cuda_stream) {
+    if (h == nullptr) return VB200_ERR_INVALID;
+    return guard(h, [&] {
+        CUDA_CHECK(cudaSetDevice(h->opt.device));
+        h->select_regions(imgs, n, p, out, static_cast<cudaStream_t>(cuda_stream));
     });
 }
 

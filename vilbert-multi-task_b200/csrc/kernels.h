@@ -141,6 +141,36 @@ struct DecodeDesc {
     int len, top_n;
 };
 cudaError_t launch_answer_decode(const DecodeDesc* descs, int n, vb200_answer* answers, cudaStream_t st);
+// Detector-region selection (regions_select.cu, vb200_select_regions).  Image i's n proposals are workspace rows [row0, row0 + n)
+// of stats / dbox / max_conf and words [mask0, mask0 + n * nw) of the bitmask; its k = min(K, n) selected rows go to output rows
+// [dst_row, dst_row + k).  npad: n rounded up to a power of two >= 32.  Descriptors are validated on the host.
+constexpr int kSelectMaxProposals = 2048;
+struct SelectDesc {
+    const float* proposals;       // [n, 4]
+    const float* scores;          // [n, C] logits
+    const float* features;        // [n, F], 16-byte aligned
+    size_t row0, mask0;
+    float im_scale;
+    int n, npad, nw, dst_row, k;
+};
+struct SelectArgs {
+    int C, F, K, start;           // classes, feature width, max boxes, first class of the NMS (0 with background, else 1)
+    float thr, nms_iou;           // thr = max(conf_thresh, 0)
+    float2* stats;                // workspace [rows]: softmax max, sum
+    float* dbox;                  // workspace [rows, 4]: proposals / im_scale
+    unsigned* mask;               // workspace: per-image suppression bitmasks
+    unsigned* max_conf;           // workspace [rows], zeroed before the NMS: bits of the per-box maximum confidence
+    int* keep;                    // workspace [n_images, K]
+    float* box_features;          // outputs: see vb200_selected
+    float* boxes;
+    int32_t* num_boxes;
+    int32_t* keep_index;
+    float* max_conf_out;
+    float* cls_prob;
+    int64_t* objects;
+};
+size_t select_nms_smem(int npad);
+cudaError_t launch_select_regions(const SelectDesc* descs, int n, int max_n, int max_npad, const SelectArgs& a, cudaStream_t st);
 
 // ---- shared host-side launch helpers
 template <typename K>

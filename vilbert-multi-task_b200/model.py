@@ -617,6 +617,72 @@ class VILBertForVLTasks(object):
             sp = spatials.data_ptr()
         return (msgs, n, C.byref(o), batch, vision_rows, sp), families
 
+    # ------------------------------------------------------------------ detector-region selection (worker.py:123-176)
+    @torch.no_grad()
+    def select_regions(self, detections, max_boxes: int = 100, conf_thresh: float = 0.0, background: bool = False,
+                       nms_iou: float = 0.5, *, dst_rows=None, out_rows: Optional[int] = None, box_features=None, boxes=None,
+                       cls_prob: bool = False, objects: bool = False):
+        """The detector's feature extraction step for every image in one call (vb200_select_regions): per-proposal softmax, per-class
+        NMS on the original-pixel boxes, per-box maximum confidence, the top ``max_boxes`` of each image.
+
+        ``detections`` is a sequence of ``(proposals [n_i, 4], scores [n_i, C], features [n_i, F], im_scale)`` per image: the boxes
+        at the detector's input scale, the class logits (column 0 background) and the fc6 features.  Image i's k_i = min(max_boxes,
+        n_i) rows go to rows ``dst_rows[i] ...`` of the outputs (default: back to back in image order, the layout
+        ``forward_regions_packed`` takes with ``n_boxes = k_i``).  ``box_features`` [out_rows, F] / ``boxes`` [out_rows, 4] may be
+        caller tensors (e.g. a packed batch with rows left free for filler images); rows outside the images' ranges are not
+        written.  Returns a dict of device tensors: box_features, boxes (original pixels), num_boxes [n] int32, keep_index
+        [out_rows] int32, max_conf [out_rows] (the sorted scores), cls_prob [out_rows, C] and objects [out_rows] int64 (the argmax of
+        each cls_prob row) when asked for, else None; and the host lists ``n_boxes`` (k_i) and ``dst_rows``."""
+        if self._handle is None:
+            raise L.VilbertB200Error("call model.cuda(i) first (worker.py:536); there is no CPU path")
+        device = torch.device("cuda", self._device)
+        n = len(detections)
+        if n < 1:
+            raise ValueError("select_regions: no images")
+        heads, k = [], []
+        for prop, sc, ft, scale in detections:
+            prop = torch.as_tensor(prop).to(device=device, dtype=torch.float32).contiguous()
+            sc = torch.as_tensor(sc).to(device=device, dtype=torch.float32).contiguous()
+            ft = torch.as_tensor(ft).to(device=device, dtype=torch.float32).contiguous()
+            if prop.dim() != 2 or prop.shape[1] != 4 or sc.dim() != 2 or ft.dim() != 2 or not prop.shape[0] == sc.shape[0] == ft.shape[0]:
+                raise ValueError(f"select_regions: image {len(heads)} needs proposals [n, 4], scores [n, C] and features [n, F]")
+            heads.append((prop, sc, ft, float(scale)))
+            k.append(min(int(max_boxes), int(prop.shape[0])))
+        Cn, F = int(heads[0][1].shape[1]), int(heads[0][2].shape[1])
+        if any(int(h[1].shape[1]) != Cn or int(h[2].shape[1]) != F for h in heads):
+            raise ValueError("select_regions: every image needs the same number of score columns and feature width")
+        if dst_rows is None:
+            dst_rows = packed_offsets(k)[:-1]
+        dst_rows = [int(r) for r in dst_rows]
+        if len(dst_rows) != n:
+            raise ValueError("select_regions: one dst_row per image")
+        if out_rows is None:
+            out_rows = int(box_features.shape[0]) if box_features is not None else max(r + kk for r, kk in zip(dst_rows, k))
+
+        def buf(t, shape, dtype):
+            if t is None:
+                return torch.empty(shape, dtype=dtype, device=device)
+            if tuple(t.shape) != shape or t.dtype != dtype or t.device != device or not t.is_contiguous():
+                raise ValueError(f"select_regions: output of shape {tuple(t.shape)} / {t.dtype}, need {shape} {dtype} on {device}")
+            return t
+        res = dict(box_features=buf(box_features, (out_rows, F), torch.float32), boxes=buf(boxes, (out_rows, 4), torch.float32),
+                   num_boxes=torch.empty(n, dtype=torch.int32, device=device),
+                   keep_index=torch.empty(out_rows, dtype=torch.int32, device=device),
+                   max_conf=torch.empty(out_rows, dtype=torch.float32, device=device),
+                   cls_prob=torch.empty(out_rows, Cn, dtype=torch.float32, device=device) if cls_prob else None,
+                   objects=torch.empty(out_rows, dtype=torch.int64, device=device) if objects else None)
+        imgs = (L.Detections * n)()
+        for i, ((prop, sc, ft, scale), r) in enumerate(zip(heads, dst_rows)):
+            imgs[i] = L.Detections(int(prop.shape[0]), r, scale, prop.data_ptr(), sc.data_ptr(), ft.data_ptr())
+        params = L.SelectParams(Cn, F, int(max_boxes), float(conf_thresh), float(nms_iou), int(bool(background)), int(out_rows))
+        sel = L.Selected(*[res[name].data_ptr() if res[name] is not None else None for name, _ in L.Selected._fields_])
+        with torch.cuda.device(device):
+            stream = torch.cuda.current_stream(device).cuda_stream
+            L.check(L.load().vb200_select_regions(self._handle, imgs, n, C.byref(params), C.byref(sel), C.c_void_p(stream)),
+                    self._handle)
+        res["n_boxes"], res["dst_rows"] = k, dst_rows
+        return res
+
     # ------------------------------------------------------------------ retrieval reuse (SURVEY.md section 8e)
     @torch.no_grad()
     def encode_text(self, question, segment_ids, input_mask, task_tokens):

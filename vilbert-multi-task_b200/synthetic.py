@@ -7,7 +7,7 @@ shaped like the tensors worker.py:416-419, 452-455 builds.
 """
 from __future__ import annotations
 
-from typing import Dict
+from typing import Dict, Optional
 
 import torch
 
@@ -118,6 +118,45 @@ def synthetic_state_dict(config: BertConfig, num_labels: int = 3129, gqa_labels:
             sd[k] = torch.randn(shape, generator=g) * 0.05
     sd["cls.predictions.decoder.weight"] = sd["bert.embeddings.word_embeddings.weight"]
     return sd
+
+
+def synthetic_detections(n_images: int, n_proposals=1000, n_classes: int = 1601, feature_size: int = 2048, seed: int = 0,
+                         margin: Optional[float] = None, n_clusters: int = 12, n_dominant: int = 24, im_scale: float = 1.6):
+    """Raw detector heads per image, shaped like the Faster R-CNN outputs the reference worker's feature extraction reads
+    (worker.py:123-176): ``[(proposals [n, 4], scores [n, C], features [n, F], im_scale)]``, CPU fp32.  ``n_proposals`` is one count
+    or one per image.
+
+    Boxes (at the detector's input scale, ``im_scale`` times the image) are drawn around ``n_clusters`` centres, so neighbours
+    overlap and the NMS has real work.  Every proposal has a dominant class among ``n_dominant``; features are relu(N(0, 1)) * 1.5.
+    Logits: with ``margin=None`` N(0, 2) plus 6 on the dominant class.  With a ``margin`` d, the dominant logit is 0 and every other
+    one is -26 - d * u for an integer u < 55 / d: the exponentials of the others sum below half an ulp of 1, so every softmax sum
+    is exactly 1 in any summation order, and two probabilities of different logits differ by a factor of at least exp(d), so the
+    selection does not depend on rounding; equal logits give equal probabilities and fall to the index tie rule."""
+    g = torch.Generator().manual_seed(seed)
+    counts = [int(n_proposals)] * n_images if isinstance(n_proposals, int) else [int(n) for n in n_proposals]
+    n_dominant = min(n_dominant, n_classes - 1)
+    dominant = torch.randperm(n_classes - 1, generator=g)[:n_dominant] + 1
+    out = []
+    for n in counts:
+        img = torch.tensor([1333.0, 800.0]) * im_scale
+        centres = torch.rand(n_clusters, 2, generator=g) * img * 0.8 + img * 0.1
+        cl = torch.randint(0, n_clusters, (n,), generator=g)
+        size = (0.05 + torch.rand(n, 2, generator=g) * 0.3) * img
+        c = centres[cl] + torch.randn(n, 2, generator=g) * size * 0.15
+        x1y1 = (c - size / 2).clamp(min=0.0)
+        x2y2 = torch.minimum(c + size / 2, img - 1)
+        proposals = torch.cat([x1y1, torch.maximum(x2y2, x1y1 + 1)], dim=1).float()
+        dom = dominant[torch.randint(0, n_dominant, (n,), generator=g)]
+        if margin is None:
+            scores = torch.randn(n, n_classes, generator=g) * 2.0
+            scores[torch.arange(n), dom] += 6.0
+        else:
+            u = torch.randint(0, max(1, int(55.0 / margin)), (n, n_classes), generator=g).float()
+            scores = -26.0 - float(margin) * u
+            scores[torch.arange(n), dom] = 0.0
+        features = torch.relu(torch.randn(n, feature_size, generator=g)) * 1.5
+        out.append((proposals, scores.float().contiguous(), features, float(im_scale)))
+    return out
 
 
 def synthetic_request(batch: int, n_tokens: int = 30, n_regions: int = 36, seed: int = 1234, task_id: int = 1,

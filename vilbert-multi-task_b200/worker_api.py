@@ -558,6 +558,123 @@ def custom_prediction_packed(requests, bucket: int = 8, select: Optional[int] = 
     return answers
 
 
+def _per_image(x, counts):
+    """A per-image sequence as given, or one tensor over all images' rows split by `counts` (the reference's `.split`)."""
+    if torch.is_tensor(x) or isinstance(x, np.ndarray):
+        return list(torch.as_tensor(x).split(counts))
+    return list(x)
+
+
+def process_feature_extraction(proposals, scores, feats, im_scales, im_infos, conf_thresh=0, background=False, num_features=100):
+    """The detector's feature extraction step (worker.py:123-176) on the device, one `model.select_regions` call for every image.
+
+    `proposals` holds each image's boxes [n_i, 4] at the detector's input scale; `scores` ([n_i, C] logits, column 0 background)
+    and `feats` ([n_i, F] fc6) are per-image sequences or, as the detector returns them, one tensor over all images' rows.
+    `im_scales` / `im_infos` ({"width", "height"}) as the worker's image transform returns them.  Returns the reference's
+    `(feat_list, info_list)`: feat_list[i] the k_i = min(num_features, n_i) kept feature rows (a device tensor), info_list[i] a dict
+    of bbox (float32 [k_i, 4], original pixels), num_boxes (int), objects (int64 [k_i - start], the argmax of kept rows start..,
+    start = 0 with `background` else 1), image_width, image_height and cls_prob (float32 [k_i, C])."""
+    props = list(proposals)
+    counts = [int(torch.as_tensor(p).shape[0]) for p in props]
+    dets = list(zip(props, _per_image(scores, counts), _per_image(feats, counts), im_scales))
+    start = 0 if background else 1
+    with model_lock:
+        r = model.select_regions(dets, num_features, float(conf_thresh), bool(background), cls_prob=True, objects=True)
+    host = {k: r[k].cpu().numpy() for k in ("boxes", "num_boxes", "cls_prob", "objects")}
+    feat_list, info_list = [], []
+    for i, (lo, k) in enumerate(zip(r["dst_rows"], r["n_boxes"])):
+        feat_list.append(r["box_features"][lo:lo + k])
+        info_list.append({"bbox": host["boxes"][lo:lo + k], "num_boxes": int(host["num_boxes"][i]),
+                          "objects": host["objects"][lo + start:lo + k], "image_width": im_infos[i]["width"],
+                          "image_height": im_infos[i]["height"], "cls_prob": host["cls_prob"][lo:lo + k]})
+    return feat_list, info_list
+
+
+def custom_prediction_detections(requests, bucket: int = 8, select: Optional[int] = None, max_boxes: int = 100, *,
+                                 decode: str = "host"):
+    """`custom_prediction_packed` for requests that carry their images' raw detector heads instead of selected features: the
+    region selection (`process_feature_extraction`'s, with the worker's defaults conf_thresh 0, no background class) writes
+    straight into the packed box rows of ONE `forward_regions_packed` call, so no feature row passes through the host.
+
+    `requests` are `(query, task, detections, infos, task_id)`: `detections[j]` = `(proposals [n, 4], scores [n, C], features
+    [n, F], im_scale)` of image j (as `synthetic.synthetic_detections` returns them), `infos[j]` its dict with image_width /
+    image_height.  Each image keeps k = min(max_boxes, n) boxes.  Rows, NLVR2 alignment, fillers (one token, one zero box in a 1 x 1
+    image), capacities and `decode` follow `custom_prediction_packed`; the answers equal `custom_prediction_packed` on the features
+    and boxes `process_feature_extraction` selects.  A request that fails validation gets its exception."""
+    if bucket < 1:
+        raise ValueError("bucket must be >= 1")
+    _check_decode(decode)
+    fixed_select = L.OUT_TASK_HEADS if select is None else int(select)
+    answers = [None] * len(requests)
+    rows, spans, need, CF = [], {}, 0, None        # rows: (tokens, segments, task, detections, (w, h))
+    for i, (query, task, detections, infos, task_id) in enumerate(requests):
+        try:
+            _validate(task_id, infos)
+            if len(detections) != len(infos):
+                raise ValueError(f"{len(detections)} detector outputs for {len(infos)} images")
+            tokens, segs = real_tokens(query)
+            if len(tokens) + 1 > 256:
+                raise ValueError(f"query of {len(tokens)} tokens: packed rows hold at most 255")
+            imgs = []
+            for (prop, sc, ft, scale), info in zip(detections, infos):
+                n = int(prop.shape[0])
+                shape = (int(sc.shape[-1]), int(ft.shape[-1]))
+                if not (1 <= n <= 2048 and tuple(prop.shape) == (n, 4) and tuple(sc.shape) == (n, shape[0])
+                        and tuple(ft.shape) == (n, shape[1])) or (CF is not None and shape != CF):
+                    raise ValueError(f"detector output of shapes {tuple(prop.shape)}, {tuple(sc.shape)}, {tuple(ft.shape)}: need "
+                                     "[n, 4], [n, C], [n, F] with 1 <= n <= 2048" + (f" and (C, F) = {CF}" if CF else ""))
+                imgs.append(((prop, sc, ft, float(scale)), (float(info["image_width"]), float(info["image_height"]))))
+            t = int(np.array(task).reshape(-1)[0])
+        except Exception as e:                      # noqa: BLE001 -- the request's answer, as callback()'s catch-all (worker.py:653-655)
+            answers[i] = e
+            continue
+        CF = (int(imgs[0][0][1].shape[-1]), int(imgs[0][0][2].shape[-1]))
+        if task_id in PAIR_TASKS and len(rows) % 2 == 1:
+            rows.append(None)                       # filler: the pair starts on an even row
+        rep = task_id in PAIR_TASKS + RETRIEVAL_TASKS
+        spans[i] = (len(rows), len(rows) + (len(imgs) if rep else 1))
+        for det, wh in (imgs if rep else imgs[:1]):
+            rows.append((tokens, segs, t, det, wh))
+        need |= TASK_OUTPUT[task_id]
+    if not spans:
+        return answers
+    sel = fixed_select | need
+    target = -(-len(rows) // bucket) * bucket
+    if target % 2 == 1 and (sel & L.OUT_VIL_BINARY_PREDICTION):
+        target += 1                                 # the binary head needs an even number of rows
+    rows += [None] * (target - len(rows))
+    filler = ([0], [0], 0, None, (1.0, 1.0))
+    rows = [filler if r is None else r for r in rows]
+    n_tokens = [len(r[0]) for r in rows]
+    n_boxes = [1 if r[3] is None else min(int(max_boxes), int(r[3][0].shape[0])) for r in rows]
+    offs = np.concatenate([[0], np.cumsum(n_boxes)])
+    device = torch.device("cuda", model._device)
+    box_features = torch.zeros(int(offs[-1]), CF[1], dtype=torch.float32, device=device)   # filler rows keep their zero box
+    boxes = torch.zeros(int(offs[-1]), 4, dtype=torch.float32, device=device)
+    real = [j for j, r in enumerate(rows) if r[3] is not None]
+    question = torch.tensor([x for r in rows for x in r[0]], dtype=torch.long)
+    segment_ids = torch.tensor([x for r in rows for x in r[1]], dtype=torch.long)
+    task_tokens = torch.tensor([[r[2]] for r in rows], dtype=torch.long)
+    image_wh = torch.tensor([list(r[4]) for r in rows], dtype=torch.float32).reshape(-1, 2)
+    with model_lock:
+        model.select_regions([rows[j][3] for j in real], int(max_boxes), dst_rows=[int(offs[j]) for j in real],
+                             box_features=box_features, boxes=boxes)
+        out, spatials = model.forward_regions_packed(question, segment_ids, task_tokens, box_features, boxes, image_wh, n_tokens,
+                                                     n_boxes, select=sel, max_tokens=max([MAX_LENGTH] + n_tokens),
+                                                     max_boxes=max([int(max_boxes)] + n_boxes))
+    if decode == "device":
+        v_off = np.concatenate([[0], np.cumsum([n + 1 for n in n_boxes])])   # packed regions: the global row, then the boxes
+        dec = _decode_device(out, spatials, {i: (requests[i][4], requests[i][3]) for i in spans}, spans, v_off)
+        for i in spans:
+            answers[i] = dec[i]
+        return answers
+    for i, (lo, hi) in spans.items():
+        task_id, infos = requests[i][4], requests[i][3]
+        sl, sp = split_region_outputs(out, spatials, n_tokens, n_boxes, lo, hi, task_id)
+        answers[i] = _decode(task_id, sl, sp, infos)
+    return answers
+
+
 def shape_result(task_id: str, answer, image_path: Sequence[str], image_names: Optional[List[str]] = None):
     """The JSON-able `result` dict callback() pushes to the WebSocket, per task family (worker.py:564-645).
     Box drawing / file writing (cv2, worker.py:596-600) is left to the caller; pass the names it chose."""
