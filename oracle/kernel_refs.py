@@ -47,6 +47,145 @@ def split16(x: torch.Tensor) -> torch.Tensor:
     return torch.stack([hi.view(M, g, 64), lo.view(M, g, 64), hi.view(M, g, 64)], dim=2).reshape(M, 3 * K).contiguous()
 
 
+def split16_w(w: torch.Tensor) -> torch.Tensor:
+    """fp32 [N, K] (K % 64 == 0) -> the fp32-parity weight, fp16 [N, 3K]: per 64 columns hi | hi | lo (engine.cu put_split_w), so
+    that against the activation's hi | lo | hi the K' = 3K contraction adds hi.hi + lo.hi + hi.lo."""
+    w = w.float()
+    hi = sat_rn(w, True)
+    lo = sat_rn(w - hi.float(), True)
+    N, K = w.shape
+    g = K // 64
+    return torch.stack([hi.view(N, g, 64), hi.view(N, g, 64), lo.view(N, g, 64)], dim=2).reshape(N, 3 * K).contiguous()
+
+
+# ---------------------------------------------------------------------------------------------------------------- GELU epilogues
+# gelu_erf (common.cuh): x * sat(0.5 + x Q(x^2)), Q of degree 8 in x^2, evaluated in Horner order with one fp32 FMA per step.
+GELU_Q = (4.547042257e-11, -4.515281038e-09, 1.986152114e-07, -5.147503089e-06, 8.848903963e-05, -1.079077483e-03, 9.718777612e-03,
+          -6.619028002e-02, 3.988192081e-01)
+GELU_BOUND = 4.3e-5             # the documented |gelu_erf - GELU| bound over the whole fp32 range
+# Saturation thresholds of gelu_erf (checked by tests/test_kernel_refs.py on every fp32 value with 2 <= |x| <= 16 and a sample out to
+# FLT_MAX): for x < GELU_ZERO_BELOW the output is -0 (x * 0), for x > GELU_IDENTITY_ABOVE it is x itself.  Each is the last input on
+# its side whose output is neither (gelu(-4.2741566) = -1.44e-6).
+GELU_ZERO_BELOW = float(np.float32(-4.2741566))
+GELU_IDENTITY_ABOVE = float(np.float32(4.2741566))
+
+
+def _fma32(a: np.ndarray, b: np.ndarray, c) -> np.ndarray:
+    """fp32 fmaf(a, b, c): the product of two fp32 values is exact in fp64, the sum is rounded to fp64 and then to fp32 (a double
+    rounding that can differ from the single one of the hardware FMA in rare ties)."""
+    with np.errstate(over="ignore", invalid="ignore"):
+        return (a.astype(np.float64) * b.astype(np.float64) + np.float64(c)).astype(np.float32)
+
+
+def gelu_poly_f32(x) -> np.ndarray:
+    """gelu_erf restated in numpy float32: u = x * x rounded to fp32, Q in the kernel's Horner order with one emulated FMA per step,
+    the FMA's saturation to [0, 1] (NaN -> 0, as __saturatef), then x * Phi rounded to fp32."""
+    x = np.asarray(x, dtype=np.float32)
+    with np.errstate(over="ignore", invalid="ignore"):
+        u = (x * x).astype(np.float32)
+        q = np.full(x.shape, np.float32(GELU_Q[0]), dtype=np.float32)
+        for c in GELU_Q[1:]:
+            q = _fma32(q, u, np.float32(c))
+        t = _fma32(x, q, np.float32(0.5))
+        t = np.clip(np.nan_to_num(t, nan=0.0, posinf=1.0, neginf=0.0), 0.0, 1.0).astype(np.float32)
+        return (x * t).astype(np.float32)
+
+
+def gelu_fp64(x) -> torch.Tensor:
+    """GELU, erf form, in fp64 (torch.erf): the function gelu_erf and the act-3 GELU approximate."""
+    x = torch.as_tensor(x).double()
+    return x * 0.5 * (1.0 + torch.erf(x / math.sqrt(2.0)))
+
+
+def gelu_as_fp64(x) -> torch.Tensor:
+    """The act-3 GELU's formula (common.cuh gelu_erf_as: Abramowitz & Stegun 7.1.26 erf) evaluated in fp64: what the fp32 kernel
+    computes, without its fp32 rounding, __fdividef and exp2f."""
+    x = torch.as_tensor(x).double()
+    z = x / math.sqrt(2.0)
+    ax = z.abs()
+    t = 1.0 / (1.0 + 0.3275911 * ax)
+    p = ((((1.061405429 * t - 1.453152027) * t + 1.421413741) * t - 0.284496736) * t + 0.254829592) * t
+    return x * 0.5 * (1.0 + torch.copysign(1.0 - p * torch.exp(-ax * ax), z))
+
+
+# ---------------------------------------------------------------------------------------------------------------- exact GEMMs
+# Integer-valued operands whose fp32 result does not depend on the order of accumulation: every product is an integer, and the sum of
+# the |products| plus |bias| of each output element stays below 2^24 in units of the smallest power of two anywhere in it (the bias
+# has quarter units, so the budget is 2^22).  Every partial sum in any order is then an exactly representable fp32 value, and the
+# correct fp32 output equals the fp64 one.  The budget is a parameter (`scale`) so that it can be lowered if a tensor core turns out
+# to align its addends more narrowly; H100 wgmma (fp16 and bf16 operands, fp32 accumulation) is exact at the full budget
+# (tests/test_gpu_gemm_exact.py test_exact_accumulation_at_full_budget).
+EXACT_BUDGET_LOG2 = 22          # 2^24 in quarter units
+BIAS_UNIT = 0.25
+W_MAX = 15                      # weights: integers in [-15, 15]
+X_MANT = 255                    # activations: integers in [-255, 255] times a power of two (8 significant bits: exact in bf16)
+BIG_BIAS = 70000.0              # a few columns: fp16 outputs saturate
+
+
+def exact_bound(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor | None) -> torch.Tensor:
+    """Per output element: sum_k |x_k w_k| + |b| (fp64; exact for these integers)."""
+    s = x.double().abs() @ w.double().abs().t()
+    if b is not None:
+        s = s + b.double().abs()
+    return s
+
+
+def exact_operands(M: int, N: int, K: int, ld_x: int | None = None, f16: bool = True, seed: int = 0, scale: int = EXACT_BUDGET_LOG2,
+                   device="cpu"):
+    """(x [M, ld_x] 16-bit, w [N, K] 16-bit, b [N] fp32) of an exact-valued GEMM (see above) with sum |x w| + |b| < 2^scale.
+
+    Row 0 of x and row 0 of w are constant, so element (0, 0) accumulates monotonically to within a factor two of the budget; the
+    other rows take amplitudes from the full budget down by powers of four, so the outputs span many binades.  Biases are odd
+    multiples of 1/4 of 12 or 13 significant bits (exact in neither 16-bit format); every 97th column gets +-70000 instead.  Columns of
+    x past K are NaN: a kernel that reads them writes NaN."""
+    assert scale <= EXACT_BUDGET_LOG2
+    ld_x = ld_x or K
+    dt = torch.float16 if f16 else torch.bfloat16
+    dev = torch.device(device)
+    g = torch.Generator(device=dev).manual_seed(seed)
+    f64 = dict(dtype=torch.float64, device=dev)
+    budget = 2.0 ** scale - BIG_BIAS - 1.0
+    a_max = budget / (K * W_MAX)                                   # largest |x| that keeps every element inside the budget
+    assert a_max >= 1.0, (K, scale)
+    w = torch.randint(-W_MAX, W_MAX + 1, (N, K), generator=g, device=dev).double()
+    w[0] = W_MAX
+    amp = (a_max / 4.0 ** (torch.arange(M, device=dev) % 8).double()).clamp(min=1.0)
+    shift = torch.clamp(torch.ceil(torch.log2(amp / X_MANT)), min=0.0)     # amp = mant * 2^shift, mant <= 255
+    mant = torch.floor(amp / torch.exp2(shift))
+    x = (torch.rand(M, K, generator=g, **f64) * 2.0 - 1.0) * mant[:, None]
+    x = torch.round(x) * torch.exp2(shift)[:, None]
+    x[0] = mant[0] * torch.exp2(shift[0])
+    b = (torch.randint(2048, 4096, (N,), generator=g, device=dev) * 2 + 1).double() * BIAS_UNIT
+    b = b * (torch.randint(0, 2, (N,), generator=g, device=dev) * 2 - 1)
+    b[1::97] = BIG_BIAS
+    b[2::97] = -BIG_BIAS
+    b = b.float()
+    assert torch.equal(x.to(dt).double(), x) and torch.equal(w.to(dt).double(), w)
+    s = exact_bound(x, w, b)
+    assert s.max().item() < 2.0 ** scale, s.max().item()
+    if scale >= 12:
+        assert s.max().item() >= 2.0 ** (scale - 2)
+    xp = torch.full((M, ld_x), float("nan"), **f64)
+    xp[:, :K] = x
+    return xp.to(dt), w.to(dt), b
+
+
+def exact_linear(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor | None, act: int, mul: torch.Tensor | None = None) -> torch.Tensor:
+    """fp32 result of act(x w^T + b) (* mul) for exact-valued operands: fp64 (exact on these integers, on the device too) converted to
+    fp32 without rounding; act 0 or 2 (ReLU of an exact value is exact); mul (fp32 [M, N]) multiplies in fp32, the kernel's one
+    rounding."""
+    assert act in (0, 2)
+    K = w.shape[1]
+    y = x[:, :K].double() @ w.double().t()
+    if b is not None:
+        y = y + b.double()
+    if act == 2:
+        y = torch.relu(y)
+    y32 = y.float()
+    assert torch.equal(y32.double(), y), "the operands are not exact-valued"
+    return y32 * mul.float() if mul is not None else y32
+
+
 # ---------------------------------------------------------------------------------------------------------------- region pack
 def region_rows(box_feats: np.ndarray, boxes: np.ndarray, w: float, h: float, nb: int):
     """One image of the region-pack kernel in float32, in the kernel's order of operations (worker.py:422-455 restated):

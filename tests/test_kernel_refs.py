@@ -56,6 +56,148 @@ def test_split16_matches_gemm_test_helper():
     assert ((back - x).abs()[ok] <= x.abs()[ok] * 2.0 ** -21 + 2.0 ** -24).all()
 
 
+# ---------------------------------------------------------------------------------------------------------------- GELU restatement
+def _all_f32(lo, hi):
+    """Every fp32 value in [lo, hi] for 0 < lo < hi, ascending."""
+    a, b = np.float32(lo).view(np.uint32), np.float32(hi).view(np.uint32)
+    return np.arange(a, b + 1, dtype=np.uint32).view(np.float32)
+
+
+def _all_finite_16(f16):
+    """Every finite fp16 or bf16 value, as fp32."""
+    u = np.arange(1 << 16, dtype=np.uint32)
+    x = u.astype(np.uint16).view(np.float16).astype(np.float32) if f16 else (u << 16).view(np.float32)
+    return x[np.isfinite(x)]
+
+
+def _gelu_err(x):
+    return np.abs(R.gelu_poly_f32(x).astype(np.float64) - R.gelu_fp64(torch.from_numpy(x)).numpy())
+
+
+@pytest.mark.parametrize("f16", [True, False], ids=["fp16", "bf16"])
+def test_gelu_poly_bound_every_16bit_value(f16):
+    """|gelu_erf - GELU| <= 4.3e-5 (common.cuh) on every finite fp16 / bf16 input, and no NaN or inf.  Measured: 4.11e-5 (fp16),
+    3.98e-5 (bf16)."""
+    x = _all_finite_16(f16)
+    assert len(x) == (63488 if f16 else 65280)
+    y = R.gelu_poly_f32(x)
+    assert np.isfinite(y).all()
+    assert _gelu_err(x).max() <= R.GELU_BOUND
+
+
+def test_gelu_poly_bound_dense_grid():
+    """The same bound on a 10^7-point fp32 grid over [-12, 12] and on every fp32 value within 2^-8 of the worst grid point (near
+    x = -4.2645; 4.27e-5 there)."""
+    x = np.linspace(-12.0, 12.0, 10_000_001, dtype=np.float64).astype(np.float32)
+    e = _gelu_err(x)
+    worst = x[np.argmax(e)]
+    assert e.max() <= R.GELU_BOUND and -4.4 < worst < -4.1, (e.max(), worst)
+    near = -_all_f32(-worst - 2.0 ** -8, -worst + 2.0 ** -8)
+    assert _gelu_err(near).max() <= R.GELU_BOUND
+
+
+def test_gelu_poly_saturation_thresholds():
+    """Below GELU_ZERO_BELOW the output is -0, above GELU_IDENTITY_ABOVE it is x bit for bit: every fp32 value with 2 <= |x| <= 16,
+    then every 256th fp32 bit pattern out to FLT_MAX, every value around sqrt(FLT_MAX) (where x * x overflows) and FLT_MAX itself.
+    Both thresholds are tight: the thresholds themselves give neither."""
+    zb, ia = np.float32(R.GELU_ZERO_BELOW), np.float32(R.GELU_IDENTITY_ABOVE)
+    dense = _all_f32(2.0, 16.0)
+    a16 = np.float32(16.0).view(np.uint32)
+    fmax = np.finfo(np.float32).max
+    sparse = np.arange(a16, fmax.view(np.uint32), 256, dtype=np.uint32).view(np.float32)
+    r = np.float32(np.sqrt(fmax)).view(np.uint32)
+    overflow = np.arange(r - (1 << 14), r + (1 << 14), dtype=np.uint32).view(np.float32)
+    pos = np.concatenate([dense, sparse, overflow, np.array([fmax], dtype=np.float32)])
+    yp = R.gelu_poly_f32(pos)
+    yn = R.gelu_poly_f32(-pos)
+    assert np.isfinite(yp).all() and np.isfinite(yn).all()
+    above = pos > ia
+    assert np.array_equal(yp[above].view(np.uint32), pos[above].view(np.uint32))
+    below = -pos < zb
+    assert (yn[below] == 0).all() and np.signbit(yn[below]).all()
+    y_zb, y_ia = R.gelu_poly_f32(np.array([zb, ia], dtype=np.float32))
+    assert y_zb != 0 and y_ia != ia
+
+
+def test_gelu_poly_small_inputs():
+    """Zero gives +0, and small inputs follow x / 2 + x^2 / sqrt(2 pi) (the bound is absolute, so check the relative error too)."""
+    x = np.array([0.0, -0.0, 1e-30, -1e-30, 1e-6, -1e-6, 1e-3], dtype=np.float32)
+    y = R.gelu_poly_f32(x)
+    assert y[0] == 0 and y[1] == 0
+    ref = R.gelu_fp64(torch.from_numpy(x)).numpy()
+    assert (np.abs(y[2:] - ref[2:]) <= np.abs(ref[2:]) * 1e-3).all()
+
+
+# ---------------------------------------------------------------------------------------------------------------- exact GEMM operands
+EXACT_SHAPES = [(1, 64, 64), (129, 1000, 200), (64, 3129, 2048), (300, 1601, 3072), (77, 64, 2112)]
+
+
+@pytest.mark.parametrize("f16", [True, False], ids=["fp16", "bf16"])
+@pytest.mark.parametrize("M,N,K", EXACT_SHAPES)
+def test_exact_operands(M, N, K, f16):
+    """The builder's operands are exact in the 16-bit format, every element stays inside the 2^24-unit budget (quarter-unit biases:
+    sum |x w| + |b| < 2^22) and the largest reaches within a factor four of it; biases have 12 or 13 significant bits (exact in
+    neither 16-bit format) and some are +-70000; columns of x past K are NaN."""
+    ld_x = K + 8
+    x, w, b = R.exact_operands(M, N, K, ld_x, f16, seed=M + N + K)
+    dt = torch.float16 if f16 else torch.bfloat16
+    assert x.dtype == dt and w.dtype == dt and x.shape == (M, ld_x) and w.shape == (N, K) and b.shape == (N,)
+    assert torch.isnan(x[:, K:].float()).all() and not torch.isnan(x[:, :K].float()).any()
+    s = R.exact_bound(x[:, :K], w, b)
+    assert s.max().item() < 2.0 ** 22
+    sxw = R.exact_bound(x[:, :K], w, None)
+    assert 2.0 ** 20 <= sxw.max().item() < 2.0 ** 23
+    if M >= 8:                                                  # amplitudes fall by 4x per row: many binades
+        assert sxw.max().item() / sxw.min().item() > 2.0 ** 8
+    assert ((b.double() * 4).remainder(2) == 1).sum().item() >= N - 2 * ((N + 95) // 97)    # odd quarters
+    small = b.abs() < 70000
+    assert not torch.equal(b[small].half().float(), b[small]) and not torch.equal(b[small].bfloat16().float(), b[small])
+    if N > 2:
+        assert (b == 70000).any() and (b == -70000).any()
+
+
+@pytest.mark.parametrize("M,N,K", EXACT_SHAPES[:3])
+def test_exact_linear_is_order_independent(M, N, K):
+    """exact_linear equals fp32 accumulation in three different orders (forwards, backwards, pairwise by torch's fp32 matmul), bit
+    for bit: the point of the exact-valued operands."""
+    x, w, b = R.exact_operands(M, N, K, None, True, seed=7)
+    ref = R.exact_linear(x, w, b, 0)
+    xf, wf = x.float(), w.float()
+    assert torch.equal((xf @ wf.t()) + b, ref)
+    fwd = torch.zeros(M, N)
+    bwd = torch.zeros(M, N)
+    for k in range(K):
+        fwd += xf[:, k:k + 1] * wf[:, k][None]
+        bwd += xf[:, K - 1 - k:K - k] * wf[:, K - 1 - k][None]
+    assert torch.equal(fwd + b, ref) and torch.equal(bwd + b, ref)
+    assert torch.equal(R.exact_linear(x, w, b, 2), torch.relu(ref))
+    mul = torch.exp2(torch.randint(-3, 4, (M, N)).float())
+    assert torch.equal(R.exact_linear(x, w, b, 0, mul), ref * mul)
+
+
+def test_exact_linear_catches_narrow_accumulators():
+    """A 16-bit bias, or an accumulator rounded to tf32 (10 explicit mantissa bits) before the bias add, changes the result: the
+    operands are built so that the exact tests see such defects."""
+    x, w, b = R.exact_operands(256, 512, 768, None, False, seed=3)
+    ref = R.exact_linear(x, w, b, 0)
+    acc = x.double() @ w.double().t()
+    assert not torch.equal((acc + b.half().double()).float(), ref)
+    assert not torch.equal((acc + b.bfloat16().double()).float(), ref)
+    m, e = torch.frexp(acc)
+    tf32 = torch.ldexp(torch.round(m * 2 ** 11) / 2 ** 11, e)
+    assert not torch.equal((tf32 + b.double()).float(), ref)
+
+
+def test_split16_w_layout():
+    """The weight split is hi | hi | lo per 64 columns and hi + lo carries w to 2^-22 relative."""
+    g = torch.Generator().manual_seed(4)
+    w = torch.randn(5, 128, generator=g)
+    v = R.split16_w(w).view(5, 2, 3, 64).float()
+    assert torch.equal(v[:, :, 0], v[:, :, 1])
+    back = (v[:, :, 0] + v[:, :, 2]).reshape(5, 128)
+    assert ((back - w).abs() <= w.abs() * 2.0 ** -21 + 2.0 ** -24).all()
+
+
 class _Tok:
     def encode(self, s):
         return [5, 6, 7]
