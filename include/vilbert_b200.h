@@ -182,7 +182,7 @@ int vb200_forward_host_slot(vb200_handle h, const vb200_inputs* in, const vb200_
                             int32_t synchronize, void* cuda_stream);
 
 /* Introspection used by the tests / bench: number of kernels one forward of this shape launches,
- * algorithmic FLOPs of it, model dimensions. */
+ * algorithmic FLOPs of it, model dimensions ("max_rows_per_sample": the engine's current bound, see vb200_set_option). */
 int vb200_plan_info(vb200_handle h, int32_t batch, int32_t n_tokens, int32_t n_regions, uint32_t select,
                     int64_t* n_launches, double* flops);
 int vb200_model_dim(vb200_handle h, const char* key, int64_t* value);
@@ -190,7 +190,12 @@ int vb200_model_dim(vb200_handle h, const char* key, int64_t* value);
  * GEMM with this percentage of the resident CTA slots as its persistent grid --
  * for reporting what a launch does when it has the GPU to itself; forwards are never affected.  "gemm_kernel": 1 (default, or 0
  * under VB200_GEMM=coop) runs the plain GEMMs the ping-pong kernel supports on it, 0 runs every GEMM on the cooperative persistent
- * kernel; a change drops the cached plans.  Both give the same bits. */
+ * kernel; a change drops the cached plans.  Both give the same bits.  "max_rows_per_sample" (256..1024, default 256): the longest text
+ * (T = n_tokens + task token) or image (V = regions, boxes + 1) sequence any call of this engine accepts; text is bounded by
+ * max_position_embeddings as well, and vb200_select_regions keeps at most this - 1 boxes per image.  Up to 256 rows per sample a
+ * plan's attention stages each (sample, head) whole in shared memory; a plan with more rows in a stream runs that stream's
+ * attention on the streaming kernels (vb200_self_attention_stream), which give the same bits wherever both run.  The choice
+ * follows from the plan's shape alone, so the bound only changes validation and no cached plan is dropped. */
 int vb200_set_option(vb200_handle h, const char* key, int64_t value);
 /* Profiling: after vb200_set_option(h, "timeline", 1) every persistent GEMM launch of a forward records 16 stamps per CTA (0: clock64 at
  * entry, 1: setup done, 2: first k-block landed [-DVB200_STAMPS builds], 8 / 9: %globaltimer ns at entry / exit, 10: last tile accumulated,
@@ -248,8 +253,8 @@ int vb200_forward_regions(vb200_handle h, const vb200_region_inputs* in, const v
  * keeps one plan and one CUDA graph per batch size whatever the lengths.  The lengths are host arrays (the plan is chosen on the
  * host); the per-sample offsets and row totals are copied to the plan's workspace on cuda_stream through a pinned staging buffer.
  * Attention maps: VB200_OUT_ATTENTION_PACKED, see vb200_attention_layout_packed.
- * VB200_ERR_INVALID for VB200_OUT_ATTENTION, split_fp32 engines, a length < 1 or above a non-zero capacity, T_i or V_i > 256 and
- * Tin_i > max_position_embeddings. */
+ * VB200_ERR_INVALID for VB200_OUT_ATTENTION, split_fp32 engines, a length < 1 or above a non-zero capacity, T_i or V_i above
+ * max_rows_per_sample (see vb200_set_option) and Tin_i > max_position_embeddings. */
 typedef struct {
     int32_t batch;                  /* B */
     int32_t max_tokens;             /* plan capacity: 0 -> max Tin_i of this call; else >= every Tin_i */
@@ -273,7 +278,7 @@ int vb200_forward_packed(vb200_handle h, const vb200_packed_inputs* in, const vb
  * CUDA graph serve both calls at equal capacities.  Outputs follow vb200_forward_packed (per-image outputs [B, ...], per-row outputs
  * packed over sum V_i / sum T_i rows).  Attention maps: VB200_OUT_ATTENTION_PACKED, see vb200_attention_layout_packed (V_i = n_boxes_i + 1).
  * VB200_ERR_INVALID for VB200_OUT_ATTENTION, split_fp32 engines, NULL required pointers,
- * n_boxes_i < 1 or above a non-zero max_boxes, V_i > 256, T_i > 256, Tin_i > max_position_embeddings and negative capacities. */
+ * n_boxes_i < 1 or above a non-zero max_boxes, V_i or T_i above max_rows_per_sample, Tin_i > max_position_embeddings and negative capacities. */
 typedef struct {
     int32_t batch;                  /* B images (rows of the forward); text already repeated per image as for vb200_region_inputs */
     int32_t max_tokens;             /* plan capacity in Tin units: 0 -> this call's maximum */
@@ -298,7 +303,7 @@ int vb200_forward_regions_packed(vb200_handle h, const vb200_packed_region_input
  * inside the entry, with (Lq_b, Lk_b) = (T_b, T_b), (V_b, V_b), (T_b, V_b) or (V_b, T_b) for kinds 0-3 and T_b = Tin_b + 1 (task token).
  * dims[2e] = heads, dims[2e + 1] = kind; total_floats is the buffer size (every float of it is written); arrays may be NULL to query
  * the count only.  Builds no plan and never blocks.  n_tokens / n_regions are HOST arrays of Tin_b and V_b, validated as the
- * packed forwards validate them (a length < 1, T_b or V_b > 256, Tin_b > max_position_embeddings: VB200_ERR_INVALID); for
+ * packed forwards validate them (a length < 1, T_b or V_b above max_rows_per_sample, Tin_b > max_position_embeddings: VB200_ERR_INVALID); for
  * vb200_forward_regions_packed pass V_b = n_boxes_b + 1.
  * A forward with the bit needs vb200_outputs.attention_probs (VB200_ERR_INVALID if NULL): the probability kernels write into it
  * directly, each sample bit-identical to the probabilities of a dense forward of that sample alone, and every other output is
@@ -333,7 +338,7 @@ int vb200_forward_cached(vb200_handle h, int32_t batch, int32_t n_tokens, int32_
  * memory: fp32 [sum rows, hidden] and 16-bit [sum rows, hidden] (2 bytes per element).  Each caption's / image's rows are bit-identical
  * to vb200_encode_text / vb200_encode_image of that item alone at its own length.  Capacities follow vb200_forward_packed: 0 means
  * this call's maximum, and plans are keyed on round16 of the capacity.  VB200_ERR_INVALID for split_fp32 engines, NULL pointers, a
- * length < 1 or above a non-zero capacity, T or V > 256 and Tin > max_position_embeddings. */
+ * length < 1 or above a non-zero capacity, T or V above max_rows_per_sample and Tin > max_position_embeddings. */
 int vb200_encode_text_packed(vb200_handle h, int32_t n, int32_t max_tokens, const int32_t* n_tokens /* HOST [n] Tin_c */,
                              const int64_t* question /* DEVICE [sum Tin_c] */, const int64_t* segment_ids /* DEVICE [sum Tin_c] */,
                              const int64_t* task_tokens /* DEVICE [n, 1] */, float* state_f32, void* state_16, void* cuda_stream);
@@ -346,7 +351,7 @@ int vb200_encode_image_packed(vb200_handle h, int32_t n, int32_t max_regions, co
  * per-pair outputs keep their shapes, per-row outputs come back packed.  Scores are bit-identical to vb200_forward_packed of the same
  * pairs, which is bit-identical to a dense forward of each pair alone at its own (Tin_c, V_i).  VB200_ERR_INVALID for
  * VB200_OUT_ATTENTION, split_fp32 engines, NULL pointers, an index outside [0, n_text) / [0, n_image), offsets that do not increase
- * (a state of 0 rows included), a length above a non-zero capacity, T or V > 256 and Tin > max_position_embeddings. */
+ * (a state of 0 rows included), a length above a non-zero capacity, T or V above max_rows_per_sample and Tin > max_position_embeddings. */
 typedef struct {
     int32_t batch;                  /* B pairs */
     int32_t max_tokens, max_regions;   /* plan capacities (Tin and V units, as vb200_packed_inputs); 0 -> this call's maxima */
@@ -437,7 +442,7 @@ int vb200_decode_answers_host(vb200_handle h, const vb200_decode_msg* msgs /* HO
  * cls_prob row (ties: lower column).  num_boxes[i] = the count of nonzero max_conf among the k_i.  (The reference's objects is the
  * argmax of rows start .. k_i - 1 of p[keep]: objects[start:] of this output.)  Rows outside those ranges are not written, so a caller
  * can leave rows free for the filler images of a packed batch.
- * Limits: 1 <= n_i <= 2048, 2 <= C <= 2048, F a positive multiple of 4, 1 <= max_boxes <= 255, 0 < nms_iou <= 1, background 0 or 1,
+ * Limits: 1 <= n_i <= 2048, 2 <= C <= 2048, F a positive multiple of 4, 1 <= max_boxes <= max_rows_per_sample - 1 (255 by default), 0 < nms_iou <= 1, background 0 or 1,
  * 1 <= n <= 65535, im_scale > 0.  VB200_ERR_INVALID, with a message naming the image where there is one, for a limit broken, a NULL
  * required pointer, a features or box_features pointer not 16-byte aligned, and destination ranges that overlap or fall outside
  * [0, out_rows); nothing is enqueued then.
@@ -531,6 +536,18 @@ int vb200_self_attention_packed(const void* qkv16, int64_t ld_qkv, int32_t hidde
                                 void* cuda_stream);
 /* Packed co-attention: per stream as vb200_self_attention_packed (offs_t text rows, offs_v image rows; T_cap / V_cap capacities). */
 int vb200_co_attention_packed(const void* qkv_img16, int64_t ld_img, const void* qkv_txt16, int64_t ld_txt, int32_t hidden,
+                              const float* img_mask_add, const float* txt_mask_add, void* ctx_txt16, int64_t ld_ctx_txt, void* ctx_img16,
+                              int64_t ld_ctx_img, int32_t B, int32_t T_cap, int32_t V_cap, int32_t heads, int32_t head_dim,
+                              int32_t act_fp16, const int32_t* offs_t, const int32_t* offs_v, void* cuda_stream);
+/* Streaming self- / co-attention, the kernels forwards use when a stream has more than 256 rows per sample: one CTA per 64 query
+ * rows, K and V streamed through shared memory in 64-key blocks, so any length runs.  Arguments as the packed calls above; NULL
+ * offsets mean a dense batch (sample b is rows [b L, b L + L) of its stream; for co-attention offs_t and offs_v are both NULL or
+ * both set).  Wherever vb200_self_attention / vb200_co_attention (or their packed forms) accept the lengths, the context rows are
+ * bit-identical to theirs. */
+int vb200_self_attention_stream(const void* qkv16, int64_t ld_qkv, int32_t hidden, const float* mask_add, void* ctx16, int64_t ld_ctx,
+                                int32_t B, int32_t L_cap, int32_t heads, int32_t head_dim, int32_t act_fp16, const int32_t* offs,
+                                void* cuda_stream);
+int vb200_co_attention_stream(const void* qkv_img16, int64_t ld_img, const void* qkv_txt16, int64_t ld_txt, int32_t hidden,
                               const float* img_mask_add, const float* txt_mask_add, void* ctx_txt16, int64_t ld_ctx_txt, void* ctx_img16,
                               int64_t ld_ctx_img, int32_t B, int32_t T_cap, int32_t V_cap, int32_t heads, int32_t head_dim,
                               int32_t act_fp16, const int32_t* offs_t, const int32_t* offs_v, void* cuda_stream);

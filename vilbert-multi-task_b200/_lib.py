@@ -131,6 +131,7 @@ EXPORTS = ["vb200_abi_version", "vb200_create", "vb200_destroy", "vb200_last_err
            "vb200_attention_layout", "vb200_attention_layout_packed", "vb200_forward_regions", "vb200_forward_packed", "vb200_forward_regions_packed", "vb200_encode_text", "vb200_encode_image", "vb200_forward_cached",
            "vb200_encode_text_packed", "vb200_encode_image_packed", "vb200_forward_cached_packed", "vb200_linear", "vb200_linear_rows", "vb200_linear_split", "vb200_layernorm", "vb200_layernorm_split", "vb200_attention_f32",
            "vb200_self_attention", "vb200_co_attention", "vb200_self_attention_packed", "vb200_co_attention_packed",
+           "vb200_self_attention_stream", "vb200_co_attention_stream",
            "vb200_linear_product", "vb200_text_embed", "vb200_image_pack", "vb200_region_pack", "vb200_rowdot", "vb200_gather_state",
            "vb200_gather_packed_state", "vb200_decode_answers", "vb200_decode_answers_host", "vb200_select_regions"]
 
@@ -192,6 +193,8 @@ def load():
     lib.vb200_co_attention.argtypes = [vp, i64, vp, i64, i32, vp, vp, vp, i64, vp, i64, i32, i32, i32, i32, i32, i32, vp]
     lib.vb200_self_attention_packed.argtypes = [vp, i64, i32, vp, vp, i64, i32, i32, i32, i32, i32, vp, vp]
     lib.vb200_co_attention_packed.argtypes = [vp, i64, vp, i64, i32, vp, vp, vp, i64, vp, i64, i32, i32, i32, i32, i32, i32, vp, vp, vp]
+    lib.vb200_self_attention_stream.argtypes = lib.vb200_self_attention_packed.argtypes
+    lib.vb200_co_attention_stream.argtypes = lib.vb200_co_attention_packed.argtypes
     lib.vb200_linear_product.argtypes = [vp, i64, vp, i64, vp, i32, vp, i64, vp, i64, vp, i64, i64, i64, i64, i32, i32, vp]
     lib.vb200_text_embed.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, f32, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32,
                                      i32, i32, vp, i32, vp]

@@ -4,7 +4,7 @@
 // BertSelfAttention / BertImageSelfAttention, and the 4 bmm + 2 softmax of BertBiAttention
 // ([UPSTREAM] vilbert/vilbert.py; anchor worker.py:286-289).
 //
-// Sequences are tiny (T <= 129, V <= 101) and attention is < 1 % of the FLOPs, so the goals are fusion, launch
+// The worker's sequences are short (T <= 129, V <= 101) and attention is < 1 % of the FLOPs, so the goals are fusion, launch
 // count and instruction count -- not tensor-core tile throughput (a 64-row wgmma tile would be half padding at T = 31).
 // One CTA owns one (sample, head): Q/K/V head slices are staged once in shared memory (16-bit, rows padded by
 // 16 B so ldmatrix is conflict-free); each warp owns 16 query rows and runs a register-resident flash-attention
@@ -12,6 +12,8 @@
 // accumulate), additive key mask, online softmax with quad shuffles in fp32, P V again on mma.sync.
 // The co-attention kernel produces BOTH directions of a (sample, head) in one launch (text-query x image-key -> text
 // context, then image-query x text-key -> image context), re-using one Q/K/V buffer set so five CTAs fit per SM.
+// These staged kernels hold a whole (sample, head) in shared memory, so they serve plans of up to 256 rows per sample; longer
+// plans run the streaming kernels at the end of this file, which give the same bits wherever both run.
 #include <cstdlib>
 #include "kernels.h"
 
@@ -431,6 +433,269 @@ cudaError_t launch_co_attention(const __nv_bfloat16* qkv_img, int ld_img, const 
         return cudaErrorInvalidValue;
 #define VB_CO(D, F) launch_co<D, F>(qkv_img, ld_img, qkv_txt, ld_txt, hidden, img_mask_add, txt_mask_add, ctx_txt, ld_ctx_txt, \
                                     ctx_img, ld_ctx_img, B, T, V, heads, pdl, st, offs_t, offs_v)
+    if (head_dim == 64) return f16 ? VB_CO(64, true) : VB_CO(64, false);
+    return f16 ? VB_CO(128, true) : VB_CO(128, false);
+#undef VB_CO
+}
+
+// ================================================================================================ streaming attention
+// Sequences longer than one CTA's shared memory holds (plans with more than 256 rows per sample in a stream the op reads).  One CTA
+// owns kStreamRows query rows of a (sample, head): its Q tile is staged once, and K / V arrive in kKeyBlock-key blocks through a
+// double-buffered cp.async ring, so shared memory does not depend on the length (D = 128: 17 KB of Q + 2 x 35 KB of ring).  Each
+// warp owns one (16-row tile, 64-column slice) work item -- D / 16 warps -- and runs, per key block, exactly the arithmetic of one
+// block of attend_tile in the same order (stream_block below is that block body): a sample's context rows are bit-identical to the
+// staged kernels' at every length both accept, so which kernel a plan picks never shows in its results.
+constexpr int kStreamRows = 64;           // query rows per CTA
+
+template <int D>
+struct StreamSmem {
+    static constexpr size_t kTile = static_cast<size_t>(kStreamRows) * AttnTile<D>::kStride * 2;     // one 64-row 16-bit tile
+    static constexpr size_t kBytes = 5 * kTile + 2 * kKeyBlock * sizeof(float);                      // Q | 2 x (K | V) | 2 masks
+};
+
+// attend_tile's per-key-block body, keys [kb, kb + nkeys) of Ks / Vs (nkeys a multiple of 16), real below nk (mask_l2[j]).
+template <int D, int OW, bool F16>
+__device__ __forceinline__ void stream_block(const uint32_t (&qa)[D / 16][4], float (&o)[OW / 8][4], float& m0, float& m1, float& l0,
+                                             float& l1, const uint16_t* Ks, const uint16_t* Vs, int kb, int nkeys, int nk,
+                                             const float* mask_l2, float scale_l2, int lane, int oc0) {
+    constexpr int kStride = AttnTile<D>::kStride;
+    constexpr int kKSteps = D / 16;
+    constexpr int kONTiles = OW / 8;
+    const int tq = lane & 3;
+    float s[kKeyBlock / 8][4];
+    // ---- S = Q K^T for this key block
+#pragma unroll
+    for (int nt = 0; nt < kKeyBlock / 8; ++nt) {
+        s[nt][0] = s[nt][1] = s[nt][2] = s[nt][3] = 0.0f;
+        if (nt * 8 < nkeys) {
+#pragma unroll
+            for (int ks2 = 0; ks2 < kKSteps / 2; ++ks2) {
+                uint32_t kf[4];
+                ldsm_x4(kf, Ks + (kb + nt * 8 + (lane & 7)) * kStride + ks2 * 32 + (lane >> 3) * 8);
+                mma16816<F16>(s[nt], qa[2 * ks2], kf[0], kf[1]);
+                mma16816<F16>(s[nt], qa[2 * ks2 + 1], kf[2], kf[3]);
+            }
+        }
+    }
+    // ---- scale + mask (log2 domain), block row max
+    float bm0 = -INFINITY, bm1 = -INFINITY;
+#pragma unroll
+    for (int nt = 0; nt < kKeyBlock / 8; ++nt) {
+        if (nt * 8 < nkeys) {
+            const int j = kb + nt * 8 + tq * 2;
+            const float ma = j < nk ? mask_l2[j] : -INFINITY;
+            const float mb = j + 1 < nk ? mask_l2[j + 1] : -INFINITY;
+            s[nt][0] = fmaf(s[nt][0], scale_l2, ma); s[nt][1] = fmaf(s[nt][1], scale_l2, mb);
+            s[nt][2] = fmaf(s[nt][2], scale_l2, ma); s[nt][3] = fmaf(s[nt][3], scale_l2, mb);
+            bm0 = fmaxf(bm0, fmaxf(s[nt][0], s[nt][1]));
+            bm1 = fmaxf(bm1, fmaxf(s[nt][2], s[nt][3]));
+        }
+    }
+    bm0 = fmaxf(bm0, __shfl_xor_sync(0xffffffffu, bm0, 1)); bm0 = fmaxf(bm0, __shfl_xor_sync(0xffffffffu, bm0, 2));
+    bm1 = fmaxf(bm1, __shfl_xor_sync(0xffffffffu, bm1, 1)); bm1 = fmaxf(bm1, __shfl_xor_sync(0xffffffffu, bm1, 2));
+    const float nm0 = fmaxf(m0, bm0), nm1 = fmaxf(m1, bm1);
+    const float c0 = exp2f(m0 - nm0), c1 = exp2f(m1 - nm1);
+    m0 = nm0; m1 = nm1;
+    float bs0 = 0.0f, bs1 = 0.0f;
+#pragma unroll
+    for (int nt = 0; nt < kKeyBlock / 8; ++nt) {
+        if (nt * 8 < nkeys) {
+            s[nt][0] = exp2f(s[nt][0] - nm0); s[nt][1] = exp2f(s[nt][1] - nm0);
+            s[nt][2] = exp2f(s[nt][2] - nm1); s[nt][3] = exp2f(s[nt][3] - nm1);
+            bs0 += s[nt][0] + s[nt][1];
+            bs1 += s[nt][2] + s[nt][3];
+        }
+    }
+    l0 = l0 * c0 + bs0;
+    l1 = l1 * c1 + bs1;
+#pragma unroll
+    for (int i = 0; i < kONTiles; ++i) { o[i][0] *= c0; o[i][1] *= c0; o[i][2] *= c1; o[i][3] *= c1; }
+    // ---- O += P V
+#pragma unroll
+    for (int kk = 0; kk < kKeyBlock / 16; ++kk) {
+        if (kk * 16 < nkeys) {
+            uint32_t pa[4];
+            pa[0] = pack16x2<F16>(s[2 * kk][0], s[2 * kk][1]);
+            pa[1] = pack16x2<F16>(s[2 * kk][2], s[2 * kk][3]);
+            pa[2] = pack16x2<F16>(s[2 * kk + 1][0], s[2 * kk + 1][1]);
+            pa[3] = pack16x2<F16>(s[2 * kk + 1][2], s[2 * kk + 1][3]);
+#pragma unroll
+            for (int nt2 = 0; nt2 < kONTiles / 2; ++nt2) {
+                uint32_t vf[4];
+                ldsm_x4_trans(vf, Vs + (kb + kk * 16 + (lane & 7) + ((lane >> 3) & 1) * 8) * kStride + oc0 + nt2 * 16 + (lane >> 4) * 8);
+                mma16816<F16>(o[2 * nt2], pa, vf[0], vf[1]);
+                mma16816<F16>(o[2 * nt2 + 1], pa, vf[2], vf[3]);
+            }
+        }
+    }
+}
+
+// One CTA: query rows [q0, q0 + nq) (nq <= kStreamRows) of one (sample, head) against the sample's nk keys.  q: the first query
+// row's head slice; k / v: key row 0's K / V head slices (row stride ld_q / ld_kv); mask: the sample's additive key mask; out:
+// the first query row's context head slice.  Every thread of the CTA calls it.
+template <int D, bool F16>
+__device__ __forceinline__ void stream_attend(const uint16_t* __restrict__ q, int ld_q, int nq, const uint16_t* __restrict__ k,
+                                              const uint16_t* __restrict__ v, int ld_kv, int nk, const float* __restrict__ mask,
+                                              float scale_l2, uint16_t* __restrict__ out, int ld_out, int pdl) {
+    extern __shared__ __align__(16) uint8_t smem_attn[];
+    constexpr int kStride = AttnTile<D>::kStride;
+    constexpr int kTileElems = kStreamRows * kStride;
+    constexpr int kSplit = D / 64, kOW = D / kSplit;             // work item = (16-row tile, 64-column slice of the head)
+    uint16_t* Qs = reinterpret_cast<uint16_t*>(smem_attn);
+    uint16_t* ring = Qs + kTileElems;                            // stage s: K at ring + 2 s tiles, V one tile further
+    float* mask_s = reinterpret_cast<float*>(ring + 4 * kTileElems);   // [2][kKeyBlock]
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int r0 = (warp / kSplit) * 16, oc0 = (warp % kSplit) * kOW;
+    const bool active = r0 < nq;
+    const int nk_pad = pad16(nk);
+    const int nblocks = (nk + kKeyBlock - 1) / kKeyBlock;
+
+    auto issue = [&](int blk) {                                  // key block blk -> ring stage blk & 1, as one cp.async group
+        const int kb = blk * kKeyBlock, n = min(kKeyBlock, nk - kb), st = blk & 1;
+        uint16_t* Ks = ring + 2 * st * kTileElems;
+        load_tile<D>(Ks, k + static_cast<size_t>(kb) * ld_kv, n, pad16(n), ld_kv);
+        load_tile<D>(Ks + kTileElems, v + static_cast<size_t>(kb) * ld_kv, n, pad16(n), ld_kv);
+        for (int j = threadIdx.x; j < n; j += blockDim.x) mask_s[st * kKeyBlock + j] = mask[kb + j] * kLog2e;
+        asm volatile("cp.async.commit_group;" ::: "memory");
+    };
+
+    if (pdl) pdl_wait();
+    load_tile<D>(Qs, q, nq, pad16(nq), ld_q);                    // rows [nq, pad16(nq)) zero-filled
+    issue(0);                                                    // Q joins block 0's group
+
+    uint32_t qa[D / 16][4];
+    float o[kOW / 8][4];
+#pragma unroll
+    for (int i = 0; i < kOW / 8; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.0f;
+    float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.0f, l1 = 0.0f;
+    for (int blk = 0; blk < nblocks; ++blk) {
+        if (blk + 1 < nblocks) {
+            issue(blk + 1);                                      // its stage was last read in iteration blk - 1
+            asm volatile("cp.async.wait_group 1;" ::: "memory");
+        } else {
+            asm volatile("cp.async.wait_group 0;" ::: "memory");
+        }
+        __syncthreads();
+        if (blk == 0) {
+            if (pdl) pdl_launch_dependents();
+#pragma unroll
+            for (int ks = 0; ks < D / 16; ++ks)
+                ldsm_x4(qa[ks], Qs + (r0 + (lane & 15)) * kStride + ks * 16 + (lane >> 4) * 8);
+        }
+        const int kb = blk * kKeyBlock, st = blk & 1;
+        // block-relative key indices: the same keys, masks and nkeys = min(kKeyBlock, nk_pad - kb) as attend_tile's block kb
+        if (active)
+            stream_block<D, kOW, F16>(qa, o, m0, m1, l0, l1, ring + 2 * st * kTileElems, ring + (2 * st + 1) * kTileElems, 0,
+                                      min(kKeyBlock, nk_pad - kb), nk - kb, mask_s + st * kKeyBlock, scale_l2, lane, oc0);
+        __syncthreads();                                         // stage st is free for block blk + 2
+    }
+    if (!active) return;
+    const int g = lane >> 2, tq = lane & 3;
+    l0 += __shfl_xor_sync(0xffffffffu, l0, 1); l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+    l1 += __shfl_xor_sync(0xffffffffu, l1, 1); l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+    const float i0 = 1.0f / l0, i1 = 1.0f / l1;
+    const int row0 = r0 + g, row1 = r0 + g + 8;
+#pragma unroll
+    for (int nt = 0; nt < kOW / 8; ++nt) {
+        const int col = oc0 + nt * 8 + tq * 2;
+        if (row0 < nq) *reinterpret_cast<uint32_t*>(out + static_cast<size_t>(row0) * ld_out + col) = pack16x2<F16>(o[nt][0] * i0, o[nt][1] * i0);
+        if (row1 < nq) *reinterpret_cast<uint32_t*>(out + static_cast<size_t>(row1) * ld_out + col) = pack16x2<F16>(o[nt][2] * i1, o[nt][3] * i1);
+    }
+}
+
+// grid (heads, B, ceil(L_cap / kStreamRows)), D / 16 warps.  Arguments as self_attention_kernel.
+template <int D, bool F16>
+__global__ void __launch_bounds__(256, 2)
+self_attention_stream_kernel(const uint16_t* __restrict__ qkv, int ld_qkv, int hidden, const float* __restrict__ key_mask_add,
+                             uint16_t* __restrict__ ctx, int ld_ctx, int L_cap, float scale_l2, int pdl, const int* __restrict__ offs) {
+    const int h = blockIdx.x, b = blockIdx.y, q0 = blockIdx.z * kStreamRows;
+    const int r0 = offs ? offs[b] : b * L_cap;
+    const int L = offs ? offs[b + 1] - r0 : L_cap;
+    if (q0 >= L) return;                                         // a tile past this sample's length: no barrier reached yet
+    const uint16_t* base = qkv + static_cast<size_t>(r0) * ld_qkv + h * D;
+    stream_attend<D, F16>(base + static_cast<size_t>(q0) * ld_qkv, ld_qkv, min(kStreamRows, L - q0), base + hidden, base + 2 * hidden,
+                          ld_qkv, L, key_mask_add + r0, scale_l2, ctx + static_cast<size_t>(r0 + q0) * ld_ctx + h * D, ld_ctx, pdl);
+}
+
+// grid (heads, B, ceil(T_cap / kStreamRows) + ceil(V_cap / kStreamRows)), D / 16 warps: blockIdx.z first walks the text-query
+// tiles (text queries Q2 over image keys K1 / V1 -> ctx_txt), then the image-query tiles (Q1 over K2 / V2 -> ctx_img).  Arguments
+// as co_attention_kernel.
+template <int D, bool F16>
+__global__ void __launch_bounds__(256, 2)
+co_attention_stream_kernel(const uint16_t* __restrict__ qkv_img, int ld_img, const uint16_t* __restrict__ qkv_txt, int ld_txt,
+                           int hidden, const float* __restrict__ img_mask_add, const float* __restrict__ txt_mask_add,
+                           uint16_t* __restrict__ ctx_txt, int ld_ctx_txt, uint16_t* __restrict__ ctx_img, int ld_ctx_img, int T_cap,
+                           int V_cap, float scale_l2, int pdl, const int* __restrict__ offs_t, const int* __restrict__ offs_v) {
+    const int h = blockIdx.x, b = blockIdx.y;
+    const int t0 = offs_t ? offs_t[b] : b * T_cap, T = offs_t ? offs_t[b + 1] - t0 : T_cap;
+    const int v0 = offs_v ? offs_v[b] : b * V_cap, V = offs_v ? offs_v[b + 1] - v0 : V_cap;
+    const int t_tiles = (T_cap + kStreamRows - 1) / kStreamRows;
+    const bool text_q = static_cast<int>(blockIdx.z) < t_tiles;
+    const int q0 = (text_q ? blockIdx.z : blockIdx.z - t_tiles) * kStreamRows;
+    const int nq = text_q ? T : V;
+    if (q0 >= nq) return;
+    const uint16_t* bi = qkv_img + static_cast<size_t>(v0) * ld_img + h * D;
+    const uint16_t* bt = qkv_txt + static_cast<size_t>(t0) * ld_txt + h * D;
+    if (text_q)
+        stream_attend<D, F16>(bt + static_cast<size_t>(q0) * ld_txt, ld_txt, min(kStreamRows, T - q0), bi + hidden, bi + 2 * hidden,
+                              ld_img, V, img_mask_add + v0, scale_l2, ctx_txt + static_cast<size_t>(t0 + q0) * ld_ctx_txt + h * D,
+                              ld_ctx_txt, pdl);
+    else
+        stream_attend<D, F16>(bi + static_cast<size_t>(q0) * ld_img, ld_img, min(kStreamRows, V - q0), bt + hidden, bt + 2 * hidden,
+                              ld_txt, T, txt_mask_add + t0, scale_l2, ctx_img + static_cast<size_t>(v0 + q0) * ld_ctx_img + h * D,
+                              ld_ctx_img, pdl);
+}
+
+template <int D, bool F16>
+static cudaError_t launch_self_stream(const __nv_bfloat16* qkv, int ld_qkv, int hidden, const float* key_mask_add, __nv_bfloat16* ctx,
+                                      int ld_ctx, int B, int L, int heads, int pdl, cudaStream_t st, const int* offs) {
+    constexpr size_t smem = StreamSmem<D>::kBytes;
+    cudaError_t e = set_smem(self_attention_stream_kernel<D, F16>, smem);
+    if (e != cudaSuccess) return e;
+    const float scale_l2 = kLog2e / sqrtf(static_cast<float>(D));
+    return launch_ex(self_attention_stream_kernel<D, F16>, dim3(heads, B, (L + kStreamRows - 1) / kStreamRows), dim3(32 * (D / 16)),
+                     smem, pdl, st, reinterpret_cast<const uint16_t*>(qkv), ld_qkv, hidden, key_mask_add,
+                     reinterpret_cast<uint16_t*>(ctx), ld_ctx, L, scale_l2, pdl, offs);
+}
+
+cudaError_t launch_self_attention_stream(const __nv_bfloat16* qkv, int ld_qkv, int hidden, const float* key_mask_add,
+                                         __nv_bfloat16* ctx, int ld_ctx, int B, int L, int heads, int head_dim, int pdl,
+                                         int f16, cudaStream_t st, const int* offs) {
+    if (L < 1 || (head_dim != 64 && head_dim != 128) || (ld_qkv & 7) || (ld_ctx & 1) || (hidden & 7))
+        return cudaErrorInvalidValue;
+    if (head_dim == 64)
+        return f16 ? launch_self_stream<64, true>(qkv, ld_qkv, hidden, key_mask_add, ctx, ld_ctx, B, L, heads, pdl, st, offs)
+                   : launch_self_stream<64, false>(qkv, ld_qkv, hidden, key_mask_add, ctx, ld_ctx, B, L, heads, pdl, st, offs);
+    return f16 ? launch_self_stream<128, true>(qkv, ld_qkv, hidden, key_mask_add, ctx, ld_ctx, B, L, heads, pdl, st, offs)
+               : launch_self_stream<128, false>(qkv, ld_qkv, hidden, key_mask_add, ctx, ld_ctx, B, L, heads, pdl, st, offs);
+}
+
+template <int D, bool F16>
+static cudaError_t launch_co_stream(const __nv_bfloat16* qkv_img, int ld_img, const __nv_bfloat16* qkv_txt, int ld_txt, int hidden,
+                                    const float* img_mask_add, const float* txt_mask_add, __nv_bfloat16* ctx_txt, int ld_ctx_txt,
+                                    __nv_bfloat16* ctx_img, int ld_ctx_img, int B, int T, int V, int heads, int pdl, cudaStream_t st,
+                                    const int* offs_t, const int* offs_v) {
+    constexpr size_t smem = StreamSmem<D>::kBytes;
+    cudaError_t e = set_smem(co_attention_stream_kernel<D, F16>, smem);
+    if (e != cudaSuccess) return e;
+    const float scale_l2 = kLog2e / sqrtf(static_cast<float>(D));
+    const int tiles = (T + kStreamRows - 1) / kStreamRows + (V + kStreamRows - 1) / kStreamRows;
+    return launch_ex(co_attention_stream_kernel<D, F16>, dim3(heads, B, tiles), dim3(32 * (D / 16)), smem, pdl, st,
+                     reinterpret_cast<const uint16_t*>(qkv_img), ld_img, reinterpret_cast<const uint16_t*>(qkv_txt), ld_txt,
+                     hidden, img_mask_add, txt_mask_add, reinterpret_cast<uint16_t*>(ctx_txt), ld_ctx_txt,
+                     reinterpret_cast<uint16_t*>(ctx_img), ld_ctx_img, T, V, scale_l2, pdl, offs_t, offs_v);
+}
+
+cudaError_t launch_co_attention_stream(const __nv_bfloat16* qkv_img, int ld_img, const __nv_bfloat16* qkv_txt, int ld_txt,
+                                       int hidden, const float* img_mask_add, const float* txt_mask_add,
+                                       __nv_bfloat16* ctx_txt, int ld_ctx_txt, __nv_bfloat16* ctx_img, int ld_ctx_img, int B,
+                                       int T, int V, int heads, int head_dim, int pdl, int f16, cudaStream_t st,
+                                       const int* offs_t, const int* offs_v) {
+    if (T < 1 || V < 1 || (head_dim != 64 && head_dim != 128) || (ld_img & 7) || (ld_txt & 7) || (hidden & 7) ||
+        (ld_ctx_txt & 1) || (ld_ctx_img & 1))
+        return cudaErrorInvalidValue;
+#define VB_CO(D, F) launch_co_stream<D, F>(qkv_img, ld_img, qkv_txt, ld_txt, hidden, img_mask_add, txt_mask_add, ctx_txt, ld_ctx_txt, \
+                                           ctx_img, ld_ctx_img, B, T, V, heads, pdl, st, offs_t, offs_v)
     if (head_dim == 64) return f16 ? VB_CO(64, true) : VB_CO(64, false);
     return f16 ? VB_CO(128, true) : VB_CO(128, false);
 #undef VB_CO

@@ -358,6 +358,15 @@ int default_gemm_kernel() {
 }
 
 // ------------------------------------------------------------------------------------------ launch list
+// Rows per sample: up to kStagedAttnRows a plan's attention stages whole (sample, head) tiles in shared memory (attention.cu), above
+// it it streams K / V in key blocks.  kMaxRowsPerSample caps vb200_set_option("max_rows_per_sample"): region selection ranks at most
+// 2048 proposals and the fp32 attention kernel holds 8 probability rows of up to 1024 keys in shared memory.
+constexpr int kStagedAttnRows = 256;
+constexpr int kMaxRowsPerSample = 1024;
+// What a rejection above the bound names: the default bound is the staged kernels' limit, a raised one the engine's option.
+inline const char* bound_name(int max_rows) {
+    return max_rows == kStagedAttnRows ? "the small-sequence attention kernels" : "this engine's max_rows_per_sample";
+}
 struct Op {
     enum Kind { GEMM, SELF_ATTN, CO_ATTN, ROWDOT, LAYERNORM, ATTN_F32, GATHER } kind;
     int stream = 0;                // 0 main, 1 side (image branch) inside the captured graph
@@ -395,6 +404,8 @@ struct Op {
     // of ctx_a, b < B, clamped to M rows
     const int* m_rows = nullptr;
     const int *offs_a = nullptr, *offs_b = nullptr;
+    // SELF_ATTN / CO_ATTN: the streaming kernels (a stream the op reads has more than 256 rows per sample in this plan)
+    bool stream_kv = false;
     // fork/join markers for the two-stream graph
     enum Sync { NONE, FORK, JOIN } sync = NONE;
     double flops = 0;
@@ -486,10 +497,11 @@ struct PackedBatch {
     int rows_v() const { return meta[layout.rows_v()]; }
 };
 // Validates a packed call's lengths and lays out its rows: offs[i + 1] = offs[i] + rows_i per stream (text: T_i = Tin_i + task
-// token).  Rejects a batch < 1, a negative capacity, a length < 1 or above a non-zero capacity, more than 256 rows (the
-// small-sequence attention kernels) and Tin_i > max_position_embeddings.  maps (non-null): where the plan's kernels write the packed
+// token).  Rejects a batch < 1, a negative capacity, a length < 1 or above a non-zero capacity, more than max_rows rows per sample
+// (the engine's max_rows_per_sample) and Tin_i > max_position_embeddings.  maps (non-null): where the plan's kernels write the packed
 // attention probabilities, whose layout then joins the meta.
-PackedBatch pack_batch(const char* api, const Config& c, const std::vector<std::string>& schedule, const PackedLengths& in, float* maps) {
+PackedBatch pack_batch(const char* api, const Config& c, const std::vector<std::string>& schedule, const PackedLengths& in, float* maps,
+                       int max_rows) {
     if (in.B < 1) fail(VB200_ERR_INVALID, "%s: batch must be positive", api);
     if (in.max_tokens < 0) fail(VB200_ERR_INVALID, "%s: negative capacity max_tokens %d", api, in.max_tokens);
     if (in.max_regions < 0) fail(VB200_ERR_INVALID, "%s: negative capacity max_regions %d", api, in.max_regions);
@@ -506,16 +518,17 @@ PackedBatch pack_batch(const char* api, const Config& c, const std::vector<std::
             const int l = len[i];
             if (l < 1) fail(VB200_ERR_INVALID, "%s: %s %d has %s %d (must be >= 1)", api, in.item, i, name, l);
             if (cap > 0 && l > cap) fail(VB200_ERR_INVALID, "%s: %s %d has %s %d, above the capacity %d", api, in.item, i, name, l, cap);
-            if (l + extra > 256)
-                fail(VB200_ERR_INVALID, "%s: %s %d too long for the small-sequence attention kernels (%s=%d, max 256)", api, in.item, i,
-                     text ? "T" : "V", l + extra);
+            if (l + extra > max_rows)
+                fail(VB200_ERR_INVALID, "%s: %s %d too long for %s (%s=%d, max %d)", api, in.item, i, bound_name(max_rows),
+                     text ? "T" : "V", l + extra, max_rows);
             if (text && l > c.max_pos)
                 fail(VB200_ERR_INVALID, "%s: %s %d has n_tokens %d > max_position_embeddings %d", api, in.item, i, l, c.max_pos);
             offs[i + 1] = offs[i] + l + extra;
             longest = std::max(longest, l);
         }
         const int rows = (cap > 0 ? cap : longest) + extra;                     // rounded up to the attention kernels' 16-row buckets
-        if (rows > 256) fail(VB200_ERR_INVALID, "%s: capacity above 256 rows per sample (%s=%d)", api, text ? "T" : "V", rows);
+        if (rows > max_rows)
+            fail(VB200_ERR_INVALID, "%s: capacity above %d rows per sample (%s=%d)", api, max_rows, text ? "T" : "V", rows);
         return (rows + 15) / 16 * 16;
     };
     if (in.n_tokens) b.Tin = pack(true, in.n_tokens, in.max_tokens, b.layout.offs_t()) - task;
@@ -594,6 +607,9 @@ struct vb200_engine {
     bool dry = false;          // audit pass: check names / shapes / dtypes only, touch no device
     int lone_rows = 320;       // VB200_LONE_ROWS (0 = off): forwards with at most this many rows in either stream (batch <= 8 at the default
                                // shapes) run their plain GEMMs with 64-wide tiles while those still fit one CTA per SM
+    // vb200_set_option("max_rows_per_sample"), 256..1024: the longest text (T = Tin + task token) or image (V) sequence a call may
+    // bring.  Validation only -- a plan's attention kernels follow from its shape (streaming above 256 rows), so no plan is dropped.
+    int max_rows = 256;
     bool x3 = false;           // fp32-parity mode (vb200_options::split_fp32): fp16 hi/lo split operands, K' = 3K GEMMs, fp32 attention
     // Programmatic dependent launch (opt.use_pdl): every kernel triggers its dependents once its main work is issued, and a
     // dependent GEMM's producer puts its first weight tiles in flight before griddepcontrol.wait.  On by default;
@@ -1045,15 +1061,19 @@ struct vb200_engine {
         const bool packed = mode >= PACKED;
         const int schedule_mode = packed ? mode - PACKED : mode;     // which part of the schedule: FULL, a prefix or the suffix
         if (schedule_mode == TEXT_PREFIX || schedule_mode == IMAGE_PREFIX) { select = 0; want_attn = false; }
+        const int T = Tin + (cfg.task_tokens ? 1 : 0);
+        // ahead of the cache: a plan built under a higher max_rows_per_sample must not outlive the bound being lowered.  Packed
+        // capacities are the call's longest rows rounded up to 16 (pack_batch has checked the rows themselves against the bound)
+        const int cap = mode >= PACKED ? (max_rows + 15) / 16 * 16 : max_rows;
+        if (T > cap || V > cap)
+            fail(VB200_ERR_INVALID, "sequence too long for %s (T=%d, V=%d, max %d)", bound_name(max_rows), T, V, cap);
         std::vector<int64_t> key{B, Tin, V, static_cast<int64_t>(select), slot, mode, want_attn ? 1 : 0};
         auto it = plans.find(key);
         if (it != plans.end()) { it->second->last_use = ++use_clock; return it->second.get(); }
         std::unique_ptr<Plan> up(new Plan());
         Plan& pl = *up;
         const Config& c = cfg;
-        const int T = Tin + (c.task_tokens ? 1 : 0);
         if (B < 1 || Tin < 1 || V < 1) fail(VB200_ERR_INVALID, "batch, n_tokens and n_regions must be positive");
-        if (T > 256 || V > 256) fail(VB200_ERR_INVALID, "sequence too long for the small-sequence attention kernels (T=%d, V=%d, max 256)", T, V);
         if (Tin > c.max_pos && !packed) fail(VB200_ERR_INVALID, "n_tokens %d exceeds max_position_embeddings %d", Tin, c.max_pos);
         pl.B = B; pl.Tin = Tin; pl.T = T; pl.V = V; pl.select = select;
         if (packed) {
@@ -1143,6 +1163,7 @@ struct vb200_engine {
                 a.stream = stream;
                 a.qkv_a = qb; a.ld_a = 3 * hid; a.hidden = hid; a.mask_a = st.mask; a.ctx_a = st.ctx; a.ld_ctx_a = hid;
                 a.B = B; a.La = st.seq; a.heads = heads; a.head_dim = hid / heads; a.offs_a = st.offs;
+                a.stream_kv = st.seq > kStagedAttnRows;
                 a.flops = 4.0 * B * heads * st.seq * st.seq * (hid / heads);
                 pl.flops += a.flops;
                 ops.push_back(a);
@@ -1190,6 +1211,7 @@ struct vb200_engine {
                     a.qkv_a = qvb; a.ld_a = 3 * Hb; a.qkv_b = qtb; a.ld_b = 3 * Hb; a.hidden = Hb;
                     a.mask_a = pl.mask_v; a.mask_b = pl.mask_t; a.ctx_a = ctx_t; a.ld_ctx_a = Hb; a.ctx_b = ctx_v; a.ld_ctx_b = Hb;
                     a.B = B; a.La = T; a.Lb = V; a.heads = c.bi_heads; a.head_dim = Hb / c.bi_heads; a.offs_a = offs_t; a.offs_b = offs_v;
+                    a.stream_kv = T > kStagedAttnRows || V > kStagedAttnRows;
                     a.flops = 8.0 * B * c.bi_heads * T * V * (Hb / c.bi_heads);
                     pl.flops += a.flops;
                     ops.push_back(a);
@@ -1373,13 +1395,14 @@ struct vb200_engine {
                 break;
             }
             case Op::SELF_ATTN:
-                CUDA_CHECK(vb::launch_self_attention(op.qkv_a, op.ld_a, op.hidden, op.mask_a, op.ctx_a, op.ld_ctx_a, op.B, op.La,
-                                                     op.heads, op.head_dim, opt.use_pdl, opt.act_fp16, st, op.offs_a));
+                CUDA_CHECK((op.stream_kv ? vb::launch_self_attention_stream : vb::launch_self_attention)(
+                    op.qkv_a, op.ld_a, op.hidden, op.mask_a, op.ctx_a, op.ld_ctx_a, op.B, op.La, op.heads, op.head_dim, opt.use_pdl,
+                    opt.act_fp16, st, op.offs_a));
                 break;
             case Op::CO_ATTN:
-                CUDA_CHECK(vb::launch_co_attention(op.qkv_a, op.ld_a, op.qkv_b, op.ld_b, op.hidden, op.mask_a, op.mask_b, op.ctx_a,
-                                                   op.ld_ctx_a, op.ctx_b, op.ld_ctx_b, op.B, op.La, op.Lb, op.heads, op.head_dim,
-                                                   opt.use_pdl, opt.act_fp16, st, op.offs_a, op.offs_b));
+                CUDA_CHECK((op.stream_kv ? vb::launch_co_attention_stream : vb::launch_co_attention)(
+                    op.qkv_a, op.ld_a, op.qkv_b, op.ld_b, op.hidden, op.mask_a, op.mask_b, op.ctx_a, op.ld_ctx_a, op.ctx_b, op.ld_ctx_b,
+                    op.B, op.La, op.Lb, op.heads, op.head_dim, opt.use_pdl, opt.act_fp16, st, op.offs_a, op.offs_b));
                 break;
             case Op::LAYERNORM:
                 CUDA_CHECK(vb::launch_ln_residual(op.ln_y, op.ln_ld, op.ln_res, op.ld_x, op.ln_g, op.ln_b, cfg.ln_eps, op.ln_out_f,
@@ -1582,7 +1605,7 @@ struct vb200_engine {
         if (maps && out->attention_probs == nullptr)
             fail(VB200_ERR_INVALID, "%s: VB200_OUT_ATTENTION_PACKED needs vb200_outputs.attention_probs (NULL)", api);
         if (x3) fail(VB200_ERR_INVALID, "%s: packed batches are not supported in split_fp32 (fp32x) mode", api);
-        const PackedBatch b = pack_batch(api, cfg, schedule, len, maps ? out->attention_probs : nullptr);
+        const PackedBatch b = pack_batch(api, cfg, schedule, len, maps ? out->attention_probs : nullptr, max_rows);
         CUDA_CHECK(cudaSetDevice(opt.device));
         Plan& pl = *get_plan(len.B, b.Tin, b.V, select & VB200_OUT_ALL, slot, mode, maps);
         const cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
@@ -1711,7 +1734,7 @@ struct vb200_engine {
         const int C = p->n_classes, F = p->feature_size, K = p->max_boxes;
         if (C < 2 || C > 2048) fail(VB200_ERR_INVALID, "%s: n_classes = %d outside [2, 2048]", api, C);
         if (F < 4 || F % 4 != 0) fail(VB200_ERR_INVALID, "%s: feature_size = %d is not a positive multiple of 4", api, F);
-        if (K < 1 || K > 255) fail(VB200_ERR_INVALID, "%s: max_boxes = %d outside [1, 255]", api, K);
+        if (K < 1 || K > max_rows - 1) fail(VB200_ERR_INVALID, "%s: max_boxes = %d outside [1, %d]", api, K, max_rows - 1);
         if (!(p->nms_iou > 0.f && p->nms_iou <= 1.f)) fail(VB200_ERR_INVALID, "%s: nms_iou = %g outside (0, 1]", api, p->nms_iou);
         if (std::isnan(p->conf_thresh)) fail(VB200_ERR_INVALID, "%s: conf_thresh is NaN", api);
         if (p->background != 0 && p->background != 1) fail(VB200_ERR_INVALID, "%s: background = %d is not 0 or 1", api, p->background);
@@ -1990,7 +2013,9 @@ int vb200_forward_regions_packed(vb200_handle h, const vb200_packed_region_input
             (task && !in->task_tokens))
             fail(VB200_ERR_INVALID, "vb200_packed_region_inputs has a NULL required pointer");
         if (in->max_boxes < 0) fail(VB200_ERR_INVALID, "%s: negative capacity max_boxes %d", api, in->max_boxes);
-        if (in->max_boxes > 255) fail(VB200_ERR_INVALID, "%s: capacity max_boxes %d above 255 (V = boxes + 1 <= 256)", api, in->max_boxes);
+        const int max_rows = h->max_rows;
+        if (in->max_boxes > max_rows - 1)
+            fail(VB200_ERR_INVALID, "%s: capacity max_boxes %d above %d (V = boxes + 1 <= %d)", api, in->max_boxes, max_rows - 1, max_rows);
         // regions per image = boxes + the global mean row; these checks name the caller's fields before pack_batch sees V_i / T_i
         std::vector<int32_t> nv;
         for (int i = 0; i < in->batch; ++i) {
@@ -1998,8 +2023,10 @@ int vb200_forward_regions_packed(vb200_handle h, const vb200_packed_region_input
             if (n < 1) fail(VB200_ERR_INVALID, "%s: image %d has n_boxes %d (must be >= 1)", api, i, n);
             if (in->max_boxes > 0 && n > in->max_boxes)
                 fail(VB200_ERR_INVALID, "%s: image %d has n_boxes %d, above the capacity max_boxes %d", api, i, n, in->max_boxes);
-            if (n + 1 > 256) fail(VB200_ERR_INVALID, "%s: image %d has n_boxes %d (V = n_boxes + 1 must be <= 256)", api, i, n);
-            if (t + task > 256) fail(VB200_ERR_INVALID, "%s: image %d has n_tokens %d (T = n_tokens + 1 must be <= 256)", api, i, t);
+            if (n + 1 > max_rows)
+                fail(VB200_ERR_INVALID, "%s: image %d has n_boxes %d (V = n_boxes + 1 must be <= %d)", api, i, n, max_rows);
+            if (t + task > max_rows)
+                fail(VB200_ERR_INVALID, "%s: image %d has n_tokens %d (T = n_tokens + 1 must be <= %d)", api, i, t, max_rows);
             nv.push_back(n + 1);
         }
         h->run_packed(api, vb200_engine::PACKED,
@@ -2204,7 +2231,7 @@ int vb200_attention_layout_packed(vb200_handle h, int32_t batch, const int32_t* 
         // from the lengths and the layer schedule alone (no plan is built), validated as the packed forwards validate them
         const char* api = "vb200_attention_layout_packed";
         if (!n_tokens || !n_regions) fail(VB200_ERR_INVALID, "%s: NULL length array", api);
-        const PackedBatch b = pack_batch(api, h->cfg, h->schedule, {"sample", batch, n_tokens, 0, n_regions, 0}, nullptr);
+        const PackedBatch b = pack_batch(api, h->cfg, h->schedule, {"sample", batch, n_tokens, 0, n_regions, 0}, nullptr, h->max_rows);
         const PackedAttnLayout l = packed_attn_layout(h->cfg, h->schedule, batch, b.offs_t(), b.offs_v());
         const int n = static_cast<int>(l.heads.size());
         for (int e = 0; e < n && e < max_entries; ++e) {
@@ -2318,6 +2345,10 @@ int vb200_set_option(vb200_handle h, const char* key, int64_t value) {
                 h->plans.clear();
                 h->gemm_kernel = static_cast<int>(value);
             }
+        } else if (k == "max_rows_per_sample") {
+            if (value < kStagedAttnRows || value > kMaxRowsPerSample)
+                fail(VB200_ERR_INVALID, "max_rows_per_sample must be in [%d, %d]", kStagedAttnRows, kMaxRowsPerSample);
+            h->max_rows = static_cast<int>(value);       // validation only: every cached plan stays valid
         } else fail(VB200_ERR_INVALID, "unknown option \"%s\"", key);
     });
 }
@@ -2358,6 +2389,7 @@ int vb200_model_dim(vb200_handle h, const char* key, int64_t* value) {
         else if (k == "operand_width_factor") *value = h->x3 ? 3 : 1;
         else if (k == "n_plans") *value = static_cast<int64_t>(h->plans.size());
         else if (k == "n_layers_scheduled") *value = static_cast<int64_t>(h->schedule.size());
+        else if (k == "max_rows_per_sample") *value = h->max_rows;
         else fail(VB200_ERR_INVALID, "unknown model dimension \"%s\"", key);
     });
 }
@@ -2531,6 +2563,31 @@ int vb200_co_attention_packed(const void* qkv_img16, int64_t ld_img, const void*
                                            (int)ld_txt, hidden, img_mask_add, txt_mask_add, static_cast<bf16*>(ctx_txt16),
                                            (int)ld_ctx_txt, static_cast<bf16*>(ctx_img16), (int)ld_ctx_img, B, T_cap, V_cap, heads,
                                            head_dim, 0, act_fp16 ? 1 : 0, static_cast<cudaStream_t>(cuda_stream), offs_t, offs_v));
+    });
+}
+
+int vb200_self_attention_stream(const void* qkv16, int64_t ld_qkv, int32_t hidden, const float* mask_add, void* ctx16, int64_t ld_ctx,
+                                int32_t B, int32_t L_cap, int32_t heads, int32_t head_dim, int32_t act_fp16, const int32_t* offs,
+                                void* cuda_stream) {
+    return op_guard([&] {
+        CUDA_CHECK(vb::launch_self_attention_stream(static_cast<const bf16*>(qkv16), (int)ld_qkv, hidden, mask_add,
+                                                    static_cast<bf16*>(ctx16), (int)ld_ctx, B, L_cap, heads, head_dim, 0,
+                                                    act_fp16 ? 1 : 0, static_cast<cudaStream_t>(cuda_stream), offs));
+    });
+}
+
+int vb200_co_attention_stream(const void* qkv_img16, int64_t ld_img, const void* qkv_txt16, int64_t ld_txt, int32_t hidden,
+                              const float* img_mask_add, const float* txt_mask_add, void* ctx_txt16, int64_t ld_ctx_txt, void* ctx_img16,
+                              int64_t ld_ctx_img, int32_t B, int32_t T_cap, int32_t V_cap, int32_t heads, int32_t head_dim,
+                              int32_t act_fp16, const int32_t* offs_t, const int32_t* offs_v, void* cuda_stream) {
+    return op_guard([&] {
+        if ((offs_t == nullptr) != (offs_v == nullptr))
+            fail(VB200_ERR_INVALID, "vb200_co_attention_stream: offs_t and offs_v must both be NULL (dense) or both be set (packed)");
+        CUDA_CHECK(vb::launch_co_attention_stream(static_cast<const bf16*>(qkv_img16), (int)ld_img, static_cast<const bf16*>(qkv_txt16),
+                                                  (int)ld_txt, hidden, img_mask_add, txt_mask_add, static_cast<bf16*>(ctx_txt16),
+                                                  (int)ld_ctx_txt, static_cast<bf16*>(ctx_img16), (int)ld_ctx_img, B, T_cap, V_cap,
+                                                  heads, head_dim, 0, act_fp16 ? 1 : 0, static_cast<cudaStream_t>(cuda_stream), offs_t,
+                                                  offs_v));
     });
 }
 

@@ -66,6 +66,17 @@ cudaError_t launch_co_attention(const __nv_bfloat16* qkv_img, int ld_img, const 
                                 __nv_bfloat16* ctx_txt, int ld_ctx_txt, __nv_bfloat16* ctx_img, int ld_ctx_img, int B,
                                 int T, int V, int heads, int head_dim, int pdl, int f16, cudaStream_t st,
                                 const int* offs_t = nullptr, const int* offs_v = nullptr);   // as launch_self_attention, per stream
+// Streaming K4 / K5 (any length): same arguments and the same bits as the two above wherever those accept the length, but K and V
+// stream through shared memory in 64-key blocks, one CTA per 64 query rows.  The engine uses them for plans with more than 256 rows
+// per sample in a stream the op reads.
+cudaError_t launch_self_attention_stream(const __nv_bfloat16* qkv, int ld_qkv, int hidden, const float* key_mask_add,
+                                         __nv_bfloat16* ctx, int ld_ctx, int B, int L, int heads, int head_dim, int pdl,
+                                         int f16, cudaStream_t st, const int* offs = nullptr);
+cudaError_t launch_co_attention_stream(const __nv_bfloat16* qkv_img, int ld_img, const __nv_bfloat16* qkv_txt, int ld_txt,
+                                       int hidden, const float* img_mask_add, const float* txt_mask_add,
+                                       __nv_bfloat16* ctx_txt, int ld_ctx_txt, __nv_bfloat16* ctx_img, int ld_ctx_img, int B,
+                                       int T, int V, int heads, int head_dim, int pdl, int f16, cudaStream_t st,
+                                       const int* offs_t = nullptr, const int* offs_v = nullptr);
 
 // LayerNorm(y + res) of a GEMM's fp32 output: fp32 stream out + 16-bit operand out (layernorm.cu); split16: hi | lo | hi operand (fp32-parity mode)
 cudaError_t launch_ln_residual(const float* y, int ld_y, const float* res, int ld_res, const float* gamma, const float* beta,

@@ -156,17 +156,22 @@ select_rank_kernel(const SelectDesc* __restrict__ descs, SelectArgs a) {
             __syncthreads();
         }
     }
-    const bool on = tid < d.k;
-    const unsigned long long kk = on ? keys[tid] : 0ull;
-    const int nonzero = __syncthreads_count(on && (kk >> 32) != 0);
+    // kept rank r = r0 + tid, kRankThreads at a time (k may exceed the block: up to 1023 boxes)
+    int nonzero = 0;
+    for (int r0 = 0; r0 < d.k; r0 += kRankThreads) {
+        const int r = r0 + tid;
+        const bool on = r < d.k;
+        const unsigned long long kk = on ? keys[r] : 0ull;
+        nonzero += __syncthreads_count(on && (kk >> 32) != 0);
+        if (!on) continue;
+        const int j = key_index(kk);
+        const size_t o = static_cast<size_t>(d.dst_row) + r;
+        a.keep[static_cast<size_t>(blockIdx.x) * a.K + r] = j;
+        if (a.keep_index) a.keep_index[o] = j;
+        if (a.max_conf_out) a.max_conf_out[o] = __uint_as_float(static_cast<unsigned>(kk >> 32));
+        reinterpret_cast<float4*>(a.boxes)[o] = reinterpret_cast<const float4*>(a.dbox)[d.row0 + j];
+    }
     if (tid == 0) a.num_boxes[blockIdx.x] = nonzero;
-    if (!on) return;
-    const int j = key_index(kk);
-    const size_t o = static_cast<size_t>(d.dst_row) + tid;
-    a.keep[static_cast<size_t>(blockIdx.x) * a.K + tid] = j;
-    if (a.keep_index) a.keep_index[o] = j;
-    if (a.max_conf_out) a.max_conf_out[o] = __uint_as_float(static_cast<unsigned>(kk >> 32));
-    reinterpret_cast<float4*>(a.boxes)[o] = reinterpret_cast<const float4*>(a.dbox)[d.row0 + j];
 }
 
 // One CTA per output row: the kept proposal's feature row (16-byte copies), and with cls_prob / objects its probability row and

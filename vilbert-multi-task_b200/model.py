@@ -81,7 +81,7 @@ class VILBertForVLTasks(object):
 
     def __init__(self, config: BertConfig, num_labels: int = 3129, state_dict=None, default_gpu: bool = True,
                  use_cuda_graph: bool = True, use_pdl: Optional[bool] = None, strict: bool = True, compute_dtype: str = "fp16",
-                 fused_layernorm: bool = False, return_attention: bool = False, max_plans: int = 0):
+                 fused_layernorm: bool = False, return_attention: bool = False, max_plans: int = 0, max_rows_per_sample: int = 256):
         self.config = config
         self.num_labels = num_labels
         self._sd = _normalise_state_dict(state_dict) if state_dict is not None else None
@@ -96,8 +96,13 @@ class VILBertForVLTasks(object):
         # every operand as an fp16 hi/lo pair, three tensor-core products per k-step, fp32 attention (<= 1e-3 per logit against
         # the reference's fp32 forward, 3x the tensor work).  Accumulation, residual stream, LayerNorm, softmax and logits are
         # fp32 in every mode.
+        # max_rows_per_sample (256..1024): the longest text (tokens + task token) or image (regions) sequence a call may bring.
+        # Plans of up to 256 rows per sample keep their kernels; longer ones stream keys through the attention kernels.  Text is
+        # bounded by max_position_embeddings (+ the task token) as well.
+        if not 256 <= int(max_rows_per_sample) <= 1024:
+            raise ValueError(f"max_rows_per_sample must be in [256, 1024], got {max_rows_per_sample}")
         self._opts = dict(use_cuda_graph=use_cuda_graph, use_pdl=use_pdl, strict=strict, compute_dtype=compute_dtype,
-                          max_plans=int(max_plans))
+                          max_plans=int(max_plans), max_rows_per_sample=int(max_rows_per_sample))
         # attn_data_list (element 9 of the tuple): the reference returns the 24 layers' attention probabilities when called with
         # output_all_attention_masks=True (worker.py:287-288) and never reads them; here they are computed only when this flag
         # is set as well (model.return_attention = True), otherwise element 9 is [].
@@ -191,6 +196,7 @@ class VILBertForVLTasks(object):
             rc = lib.vb200_create(self._config_json(), len(self._sd), arr, C.byref(opt), C.byref(h))
         L.check(rc, None)
         self._handle, self._device = h, device
+        L.check(lib.vb200_set_option(h, b"max_rows_per_sample", self._opts["max_rows_per_sample"]), h)
         for key in ("hidden_size", "v_hidden_size", "bi_hidden_size", "vocab_size", "v_target_size",
                     "v_feature_size", "num_labels", "gqa_labels", "task_specific_tokens", "weight_bytes",
                     "operand_width_factor"):
@@ -233,8 +239,15 @@ class VILBertForVLTasks(object):
 
     def set_option(self, key, value):
         """Run-time knobs of the engine (include/vilbert_b200.h, vb200_set_option): "max_plans", "timeline", "profile_grid_pct",
-        "gemm_kernel"."""
+        "gemm_kernel", "max_rows_per_sample" (also applied to the engine a later .cuda() creates)."""
         L.check(L.load().vb200_set_option(self._handle, key.encode(), int(value)), self._handle)
+        if key == "max_rows_per_sample":
+            self._opts["max_rows_per_sample"] = int(value)
+
+    @property
+    def max_rows_per_sample(self) -> int:
+        """Longest text (tokens + task token) or image (regions) sequence a call of this model may bring."""
+        return self._opts["max_rows_per_sample"]
 
     def profile_ops(self, batch, n_tokens, n_regions, select=L.OUT_TASK_HEADS, iters=5, grid_pct=0):
         """Per-launch device times (ms) of one forward: every kernel replayed alone from its own CUDA graph between two events.

@@ -51,8 +51,10 @@ TASK_NAMES = {"1": "VQA", "2": "VG-QA", "15": "GQA", "12": "NLVR2", "13": "SNLI-
 
 
 def load_vilbert_model(from_pretrained, config_file, num_labels: int = 3129, device: int = 0, vocab_file=None,
-                       label2ans: Optional[Dict[str, str]] = None, tokenizer_obj=None, **engine_kw):
-    """worker.py:463-539 without the detector: config mutation (worker.py:509-522), from_pretrained, eval, cuda."""
+                       label2ans: Optional[Dict[str, str]] = None, tokenizer_obj=None, max_rows_per_sample: int = 256, **engine_kw):
+    """worker.py:463-539 without the detector: config mutation (worker.py:509-522), from_pretrained, eval, cuda.
+    max_rows_per_sample (256..1024): the longest query (wordpieces + the task token) or image (boxes + the global row) the model
+    serves; text stays bounded by max_position_embeddings as well."""
     global model, tokenizer
     from .config import BertConfig
     from .model import VILBertForVLTasks
@@ -62,7 +64,7 @@ def load_vilbert_model(from_pretrained, config_file, num_labels: int = 3129, dev
     config.task_specific_tokens = True     # worker.py:516-517
     config.visualization = True            # worker.py:522
     m = VILBertForVLTasks.from_pretrained(from_pretrained, config=config, num_labels=num_labels, default_gpu=True,
-                                          **engine_kw)
+                                          max_rows_per_sample=max_rows_per_sample, **engine_kw)
     m.eval()
     m = m.cuda(device)
     model = m
@@ -444,6 +446,12 @@ def real_tokens(query, tok=None):
     return tokens[:k], segment_ids[:k]
 
 
+def _max_rows() -> int:
+    """Rows per sample the loaded model accepts in either stream (its max_rows_per_sample; 256 for a model without the knob): a
+    query holds at most this - 1 tokens (+ the task token), an image this - 1 boxes (+ the global mean row)."""
+    return int(getattr(model, "max_rows_per_sample", 256))
+
+
 def pack_region_requests(requests, bucket: int = 8, select: Optional[int] = None, max_boxes: int = 100, tok=None):
     """The host half of `custom_prediction_packed`: `custom_prediction` argument tuples `(query, task, features, infos, task_id)` ->
     the inputs of ONE `forward_regions_packed` call, as CPU tensors.
@@ -457,6 +465,7 @@ def pack_region_requests(requests, bucket: int = 8, select: Optional[int] = None
     if bucket < 1:
         raise ValueError("bucket must be >= 1")
     fixed_select = L.OUT_TASK_HEADS if select is None else int(select)
+    max_rows = _max_rows()
     answers = [None] * len(requests)
     rows, spans, need, F = [], {}, 0, None        # rows: (tokens, segments, task, box features [n, F], boxes [n, 4], (w, h))
     for i, (query, task, features, infos, task_id) in enumerate(requests):
@@ -465,14 +474,14 @@ def pack_region_requests(requests, bucket: int = 8, select: Optional[int] = None
             if len(features) != len(infos):
                 raise ValueError(f"{len(features)} feature arrays for {len(infos)} images")
             tokens, segs = real_tokens(query, tok)
-            if len(tokens) + 1 > 256:
-                raise ValueError(f"query of {len(tokens)} tokens: packed rows hold at most 255")
+            if len(tokens) + 1 > max_rows:
+                raise ValueError(f"query of {len(tokens)} tokens: packed rows hold at most {max_rows - 1}")
             imgs = []
             for f, info in zip(features, infos):
                 f = torch.as_tensor(f, dtype=torch.float32)
                 n = int(f.shape[0]) if f.dim() == 2 else 0
-                if n < 1 or n + 1 > 256 or (F is not None and f.shape[1] != F):
-                    raise ValueError(f"box features of shape {tuple(f.shape)}: need [n, F] with 1 <= n <= 255"
+                if n < 1 or n + 1 > max_rows or (F is not None and f.shape[1] != F):
+                    raise ValueError(f"box features of shape {tuple(f.shape)}: need [n, F] with 1 <= n <= {max_rows - 1}"
                                      + (f" and F = {F}" if F is not None else ""))
                 bx = torch.as_tensor(np.asarray(info["bbox"], dtype=np.float32))
                 if bx.dim() != 2 or bx.shape[0] < n or bx.shape[1] < 4:
@@ -605,6 +614,7 @@ def custom_prediction_detections(requests, bucket: int = 8, select: Optional[int
         raise ValueError("bucket must be >= 1")
     _check_decode(decode)
     fixed_select = L.OUT_TASK_HEADS if select is None else int(select)
+    max_rows = _max_rows()
     answers = [None] * len(requests)
     rows, spans, need, CF = [], {}, 0, None        # rows: (tokens, segments, task, detections, (w, h))
     for i, (query, task, detections, infos, task_id) in enumerate(requests):
@@ -613,8 +623,8 @@ def custom_prediction_detections(requests, bucket: int = 8, select: Optional[int
             if len(detections) != len(infos):
                 raise ValueError(f"{len(detections)} detector outputs for {len(infos)} images")
             tokens, segs = real_tokens(query)
-            if len(tokens) + 1 > 256:
-                raise ValueError(f"query of {len(tokens)} tokens: packed rows hold at most 255")
+            if len(tokens) + 1 > max_rows:
+                raise ValueError(f"query of {len(tokens)} tokens: packed rows hold at most {max_rows - 1}")
             imgs = []
             for (prop, sc, ft, scale), info in zip(detections, infos):
                 n = int(prop.shape[0])
