@@ -15,6 +15,7 @@ full sort + per-element `.item()`; label maps are loaded once instead of per req
 """
 from __future__ import annotations
 
+import functools
 import os
 import pickle
 import re
@@ -609,12 +610,15 @@ def custom_prediction_detections(requests, bucket: int = 8, select: Optional[int
     [n, F], im_scale)` of image j (as `synthetic.synthetic_detections` returns them), `infos[j]` its dict with image_width /
     image_height.  Each image keeps k = min(max_boxes, n) boxes.  Rows, NLVR2 alignment, fillers (one token, one zero box in a 1 x 1
     image), capacities and `decode` follow `custom_prediction_packed`; the answers equal `custom_prediction_packed` on the features
-    and boxes `process_feature_extraction` selects.  A request that fails validation gets its exception."""
+    and boxes `process_feature_extraction` selects.  A request that fails validation gets its exception: every limit of
+    `vb200_select_regions` on an image (1 <= n <= 2048 proposals, 2 <= C <= 2048 score columns, F the model's feature width, a
+    positive finite im_scale, C the same as every other image of the call) is checked here, so one bad image does not fail the call."""
     if bucket < 1:
         raise ValueError("bucket must be >= 1")
     _check_decode(decode)
     fixed_select = L.OUT_TASK_HEADS if select is None else int(select)
     max_rows = _max_rows()
+    F = int(model._dims["v_feature_size"])
     answers = [None] * len(requests)
     rows, spans, need, CF = [], {}, 0, None        # rows: (tokens, segments, task, detections, (w, h))
     for i, (query, task, detections, infos, task_id) in enumerate(requests):
@@ -625,20 +629,25 @@ def custom_prediction_detections(requests, bucket: int = 8, select: Optional[int
             tokens, segs = real_tokens(query)
             if len(tokens) + 1 > max_rows:
                 raise ValueError(f"query of {len(tokens)} tokens: packed rows hold at most {max_rows - 1}")
-            imgs = []
+            imgs, cf = [], CF                       # cf: the (C, F) this request's images must share with the call
             for (prop, sc, ft, scale), info in zip(detections, infos):
                 n = int(prop.shape[0])
                 shape = (int(sc.shape[-1]), int(ft.shape[-1]))
-                if not (1 <= n <= 2048 and tuple(prop.shape) == (n, 4) and tuple(sc.shape) == (n, shape[0])
-                        and tuple(ft.shape) == (n, shape[1])) or (CF is not None and shape != CF):
+                if not (1 <= n <= 2048 and 2 <= shape[0] <= 2048 and shape[1] == F
+                        and tuple(prop.shape) == (n, 4) and tuple(sc.shape) == (n, shape[0]) and tuple(ft.shape) == (n, F)) \
+                        or (cf is not None and shape != cf):
                     raise ValueError(f"detector output of shapes {tuple(prop.shape)}, {tuple(sc.shape)}, {tuple(ft.shape)}: need "
-                                     "[n, 4], [n, C], [n, F] with 1 <= n <= 2048" + (f" and (C, F) = {CF}" if CF else ""))
+                                     f"[n, 4], [n, C], [n, F] with 1 <= n <= 2048, 2 <= C <= 2048 and F = {F} (the model's feature "
+                                     "width)" + (f" and C = {cf[0]}" if cf else ""))
+                if not 0.0 < float(scale) <= float(np.finfo(np.float32).max):
+                    raise ValueError(f"im_scale {scale}: need a positive finite scale")
+                cf = shape
                 imgs.append(((prop, sc, ft, float(scale)), (float(info["image_width"]), float(info["image_height"]))))
             t = int(np.array(task).reshape(-1)[0])
         except Exception as e:                      # noqa: BLE001 -- the request's answer, as callback()'s catch-all (worker.py:653-655)
             answers[i] = e
             continue
-        CF = (int(imgs[0][0][1].shape[-1]), int(imgs[0][0][2].shape[-1]))
+        CF = cf
         if task_id in PAIR_TASKS and len(rows) % 2 == 1:
             rows.append(None)                       # filler: the pair starts on an even row
         rep = task_id in PAIR_TASKS + RETRIEVAL_TASKS
@@ -658,7 +667,8 @@ def custom_prediction_detections(requests, bucket: int = 8, select: Optional[int
     n_tokens = [len(r[0]) for r in rows]
     n_boxes = [1 if r[3] is None else min(int(max_boxes), int(r[3][0].shape[0])) for r in rows]
     offs = np.concatenate([[0], np.cumsum(n_boxes)])
-    device = torch.device("cuda", model._device)
+    # the engine needs a GPU; the CPU is only ever reached by a stand-in model when no GPU is visible (as in MicroBatchWorker._run)
+    device = torch.device("cuda", model._device) if torch.cuda.is_available() else torch.device("cpu")
     box_features = torch.zeros(int(offs[-1]), CF[1], dtype=torch.float32, device=device)   # filler rows keep their zero box
     boxes = torch.zeros(int(offs[-1]), 4, dtype=torch.float32, device=device)
     real = [j for j, r in enumerate(rows) if r[3] is not None]
@@ -734,15 +744,33 @@ class MicroBatchWorker(object):
     branch is a follow-up, to be decided on the A/B of scripts/regions_packed_bench.py.
 
     `decode="device"` decodes every answer of a model call in one kernel (`model.decode_answers`) instead of one softmax, top-N
-    and host synchronisation per message; the default stays on the host."""
+    and host synchronisation per message; the default stays on the host.
 
-    def __init__(self, max_rows: int = 64, max_wait_ms: float = 2.0, bucket: int = 8, packed: bool = False, *, decode: str = "host"):
+    `source="detections"` serves messages that carry the detector network's raw heads instead of selected features:
+    `submit(body, detections, infos)` takes per image `(proposals [n, 4], scores [n, C], features [n, F], im_scale)` (the layout of
+    `synthetic.synthetic_detections`) and `infos[j]` with image_width / image_height.  Each micro-batch goes through
+    `custom_prediction_detections`: ONE region selection (the top `max_boxes` boxes per image, the detector's num_features) straight
+    into the packed rows of ONE `forward_regions_packed`, and with `decode="device"` one decode.  `packed` only applies to
+    `source="features"`.  Heads may be device tensors on any GPU: for each GPU that holds some, `submit` records an event on the
+    submitting thread's current stream there and the worker's stream there waits for it before the selection, so heads written on
+    any stream need no synchronisation, and the worker keeps them alive until its reads are done, so the caller may drop its
+    references right after `submit`.  A message whose heads
+    break a limit of the selection resolves to its own `ValueError`; the rest of its micro-batch is answered.  The default source
+    stays "features"; changing it, like the dense default, waits for an A/B (scripts/worker_detections_bench.py)."""
+
+    def __init__(self, max_rows: int = 64, max_wait_ms: float = 2.0, bucket: int = 8, packed: bool = False, *, decode: str = "host",
+                 source: str = "features", max_boxes: int = 100):
         import queue
         import threading
         _check_decode(decode)
+        if source not in ("features", "detections"):
+            raise ValueError(f"source must be 'features' or 'detections', not {source!r}")
+        if not 1 <= int(max_boxes) <= _max_rows() - 1:
+            raise ValueError(f"max_boxes = {max_boxes} outside [1, {_max_rows() - 1}]")
         self.max_rows, self.max_wait, self.bucket = int(max_rows), float(max_wait_ms) * 1e-3, int(bucket)
         self.packed = bool(packed)
         self.decode = decode
+        self.source, self.max_boxes = source, int(max_boxes)
         self._q = queue.Queue()
         self._stop = False
         self.batches = []                      # rows per model call group, for tests / monitoring
@@ -750,12 +778,24 @@ class MicroBatchWorker(object):
         self._thread.start()
 
     def submit(self, body: dict, features, infos):
+        """Queue one message; `features` are the selected box features per image, or with `source="detections"` the raw heads."""
         from concurrent.futures import CancelledError, Future
         fut = Future()
         if self._stop:
             fut.set_exception(CancelledError("MicroBatchWorker closed"))
             return fut
-        self._q.put((body, features, infos, fut))
+        ready = []                             # per GPU: (event, heads) the worker's stream there waits for and keeps alive
+        if self.source == "detections":
+            by_device = {}
+            for det in features:
+                for t in (det[:3] if isinstance(det, (tuple, list)) else ()):
+                    if torch.is_tensor(t) and t.is_cuda:
+                        by_device.setdefault(t.device, []).append(t)
+            for dev, heads in by_device.items():
+                ev = torch.cuda.Event()
+                ev.record(torch.cuda.current_stream(dev))
+                ready.append((ev, heads))
+        self._q.put((body, features, infos, fut, ready))
         return fut
 
     def close(self):
@@ -799,11 +839,13 @@ class MicroBatchWorker(object):
             self._run(pending)
 
     def _run(self, pending):
+        if self.source == "detections":
+            return self._run_detections(pending)
         if self.packed:
-            return self._run_packed(pending)
+            return self._run_packed(pending, custom_prediction_packed)
         device = torch.device("cuda", model._device) if torch.cuda.is_available() else torch.device("cpu")
         reqs, live = [], []
-        for body, features, infos, fut in pending:
+        for body, features, infos, fut, _ in pending:
             try:
                 task_id = str(body["task_id"])
                 reqs.append(build_inputs(body["question"], [int(task_id)], features, infos, device) + (task_id, infos))
@@ -821,9 +863,22 @@ class MicroBatchWorker(object):
         self.batches.append(sum(r[1].shape[0] for r in reqs))
         self._resolve(live, answers)
 
-    def _run_packed(self, pending):
+    def _run_detections(self, pending):
+        """Order this thread's stream on each GPU that holds heads after the message's event there (the selection reads heads on
+        the model's GPU in place, and copies heads on another GPU on this thread's stream of that GPU), keep the heads alive until
+        the work enqueued on them is done (`record_stream`: the allocator does not reuse their memory before that, even when the
+        call raises after enqueuing), then answer the micro-batch."""
+        for *_, ready in pending:
+            for ev, heads in ready:
+                stream = torch.cuda.current_stream(heads[0].device)
+                stream.wait_event(ev)
+                for t in heads:
+                    t.record_stream(stream)
+        self._run_packed(pending, functools.partial(custom_prediction_detections, max_boxes=self.max_boxes))
+
+    def _run_packed(self, pending, predict):
         reqs, live = [], []
-        for body, features, infos, fut in pending:
+        for body, features, infos, fut, _ in pending:
             try:
                 task_id = str(body["task_id"])
                 reqs.append((body["question"], [int(task_id)], features, infos, task_id))
@@ -833,7 +888,7 @@ class MicroBatchWorker(object):
         if not reqs:
             return
         try:
-            answers = custom_prediction_packed(reqs, bucket=self.bucket, decode=self.decode)
+            answers = predict(reqs, bucket=self.bucket, decode=self.decode)
         except Exception as e:                 # noqa: BLE001
             for _, fut, _ in live:
                 fut.set_exception(e)
