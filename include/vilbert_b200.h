@@ -14,7 +14,7 @@
  * Beyond the protocol: packed variable-length batches (vb200_packed_inputs: samples with their own text lengths and region counts
  * in one forward, plans keyed on capacity buckets, GEMM tiles past the call's row totals skipped), detector output in, dense or
  * packed (vb200_region_inputs, vb200_packed_region_inputs: every image at its own box count), caption-image retrieval with reuse, dense or packed (vb200_packed_pairs: captions and images encoded once
- * at their own lengths, pairs scored without padding), the answer decode of every message of a batch in one kernel (vb200_decode_answers:
+ * at their own lengths, pairs scored without padding; vb200_encode_regions_packed: image states from detector output), the answer decode of every message of a batch in one kernel (vb200_decode_answers:
  * softmax, top N and grounding boxes, so a C host answers a message without re-implementing prediction()'s decode), the detector's
  * region selection (vb200_select_regions: per-class NMS, confidence ranking and the top boxes of every image, written into the packed
  * region inputs), and kernel-level entry points for the tests.
@@ -345,6 +345,17 @@ int vb200_encode_text_packed(vb200_handle h, int32_t n, int32_t max_tokens, cons
 int vb200_encode_image_packed(vb200_handle h, int32_t n, int32_t max_regions, const int32_t* n_regions /* HOST [n] V_i */,
                               const float* features /* DEVICE [sum V_i, v_feature_size] */, const float* spatials /* DEVICE [sum V_i, 5] */,
                               float* state_f32, void* state_16, void* cuda_stream);
+/* vb200_encode_image_packed from detector output, as vb200_forward_regions_packed takes it: image i has n_boxes_i box feature rows and
+ * pixel boxes, back to back, and its size in image_wh.  Its state is V_i = n_boxes_i + 1 rows, the global mean row first, in the layout
+ * above (vb200_forward_cached_packed reads it unchanged).  The same region-pack kernel as vb200_forward_regions_packed writes the rows,
+ * in front of the plan of vb200_encode_image_packed at max_regions = max_boxes + 1 (one plan serves both calls), so scores from these
+ * states are bit-identical to vb200_forward_regions_packed of the same (caption, image) pairs.  max_boxes: plan capacity in boxes,
+ * 0 -> this call's maximum.  VB200_ERR_INVALID, with nothing enqueued, for split_fp32 engines, NULL pointers, n_boxes_i < 1 or above
+ * a non-zero max_boxes, a negative max_boxes and V_i above max_rows_per_sample. */
+int vb200_encode_regions_packed(vb200_handle h, int32_t n, int32_t max_boxes, const int32_t* n_boxes /* HOST [n] */,
+                                const float* box_features /* DEVICE [sum n_boxes_i, v_feature_size] */,
+                                const float* boxes /* DEVICE [sum n_boxes_i, 4] pixels */, const float* image_wh /* DEVICE [n, 2] */,
+                                float* state_f32, void* state_16, void* cuda_stream);
 /* Pair b = (caption text_index[b], image image_index[b]) from packed states.  The index arrays and state offsets are HOST arrays (the
  * engine validates them and builds the plan's offsets on the host); the per-call offsets reach the plan's workspace on cuda_stream
  * through a pinned staging buffer, and one kernel gathers every pair's rows from the states.  Outputs follow vb200_forward_packed:

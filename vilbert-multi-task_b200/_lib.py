@@ -129,7 +129,7 @@ class Options(C.Structure):
 EXPORTS = ["vb200_abi_version", "vb200_create", "vb200_destroy", "vb200_last_error", "vb200_forward", "vb200_forward_slot",
            "vb200_forward_host", "vb200_forward_host_slot", "vb200_plan_info", "vb200_model_dim", "vb200_set_option", "vb200_timeline", "vb200_profile_ops",
            "vb200_attention_layout", "vb200_attention_layout_packed", "vb200_forward_regions", "vb200_forward_packed", "vb200_forward_regions_packed", "vb200_encode_text", "vb200_encode_image", "vb200_forward_cached",
-           "vb200_encode_text_packed", "vb200_encode_image_packed", "vb200_forward_cached_packed", "vb200_linear", "vb200_linear_rows", "vb200_linear_split", "vb200_layernorm", "vb200_layernorm_split", "vb200_attention_f32",
+           "vb200_encode_text_packed", "vb200_encode_image_packed", "vb200_encode_regions_packed", "vb200_forward_cached_packed", "vb200_linear", "vb200_linear_rows", "vb200_linear_split", "vb200_layernorm", "vb200_layernorm_split", "vb200_attention_f32",
            "vb200_self_attention", "vb200_co_attention", "vb200_self_attention_packed", "vb200_co_attention_packed",
            "vb200_self_attention_stream", "vb200_co_attention_stream",
            "vb200_linear_product", "vb200_text_embed", "vb200_image_pack", "vb200_region_pack", "vb200_rowdot", "vb200_gather_state",
@@ -182,6 +182,7 @@ def load():
     lib.vb200_forward_cached.argtypes = [vp, i32, i32, i32, vp, i32, vp, vp, vp, vp, i32, vp, vp, vp, C.POINTER(Outputs), u32, i32, vp]
     lib.vb200_encode_text_packed.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp, vp, vp]
     lib.vb200_encode_image_packed.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp, vp]
+    lib.vb200_encode_regions_packed.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp, vp, vp]
     lib.vb200_forward_cached_packed.argtypes = [vp, C.POINTER(PackedPairs), C.POINTER(Outputs), u32, i32, vp]
     lib.vb200_linear_split.argtypes = [vp, i64, vp, i64, vp, i32, vp, i64, vp, i64, i64, i64, i64, vp]
     lib.vb200_layernorm_split.argtypes = [vp, i64, vp, i64, vp, vp, f32, vp, i64, vp, i64, i64, i64, vp]

@@ -1577,10 +1577,14 @@ struct vb200_engine {
     // offsets (the same rows forward_regions writes for that image alone), then the packed forward runs as above
     void forward_regions_packed(Plan& pl, const vb200_packed_region_inputs& in, const PackedBatch& b, cudaStream_t st) {
         embed_text(pl, in.question, in.segment_ids, nullptr, in.task_tokens, b.rows_t(), st);
-        CUDA_CHECK(vb::launch_region_pack(in.box_features, in.boxes, in.image_wh, nullptr, pl.img_a, pl.mask_v, in.spatials_out, pl.B, 0,
-                                          cfg.v_feat, pl.kp, opt.act_fp16, 0, st, pl.offs_v()));
-        zero_tail(pl.img_a, b.rows_v(), pl.B * pl.V, pl.kp, st);
+        pack_regions_packed(pl, in.box_features, in.boxes, in.image_wh, in.spatials_out, b.rows_v(), st);
         run_plan(pl, st);
+    }
+    void pack_regions_packed(Plan& pl, const float* box_feats, const float* boxes, const float* image_wh, float* spatials_out, int rows,
+                             cudaStream_t st) {
+        CUDA_CHECK(vb::launch_region_pack(box_feats, boxes, image_wh, nullptr, pl.img_a, pl.mask_v, spatials_out, pl.B, 0, cfg.v_feat,
+                                          pl.kp, opt.act_fp16, 0, st, pl.offs_v()));
+        zero_tail(pl.img_a, rows, pl.B * pl.V, pl.kp, st);
     }
     // packed pair suffix: every pair's rows are gathered from the packed caption / image states into the plan's packed buffers
     void forward_cached_packed(Plan& pl, const vb200_packed_pairs& in, const PackedBatch& b, cudaStream_t st) {
@@ -1634,6 +1638,13 @@ struct vb200_engine {
         pack_image(pl, feats, loc, vmask, rows, st);
         run_plan(pl, st);
         copy_state(pl.v_f32[pl.v_cur], pl.v_b16[pl.v_cur], pl.mask_v, rows, cfg.v_hidden, st_f32, st_16, st_mask, st);
+    }
+    // packed image prefix from detector output: the region pack of forward_regions_packed in front of the image prefix
+    void encode_regions(Plan& pl, const float* box_feats, const float* boxes, const float* image_wh, int rows, float* st_f32, void* st_16,
+                        cudaStream_t st) {
+        pack_regions_packed(pl, box_feats, boxes, image_wh, nullptr, rows, st);
+        run_plan(pl, st);
+        copy_state(pl.v_f32[pl.v_cur], pl.v_b16[pl.v_cur], pl.mask_v, rows, cfg.v_hidden, st_f32, st_16, nullptr, st);
     }
     void copy_state(const float* f32, const bf16* b16, const float* mask, size_t rows, size_t H, float* st_f32, void* st_16,
                     float* st_mask, cudaStream_t st) {
@@ -2120,6 +2131,36 @@ int vb200_encode_image_packed(vb200_handle h, int32_t n, int32_t max_regions, co
         h->run_packed(api, vb200_engine::PACKED_IMAGE_PREFIX, {"image", n, nullptr, 0, n_regions, max_regions}, 0, 0, nullptr, cuda_stream,
                       [&](Plan& pl, const PackedBatch& b, cudaStream_t st) {
                           h->encode_image(pl, features, spatials, nullptr, b.rows_v(), state_f32, state_16, nullptr, st);
+                      });
+    });
+}
+
+int vb200_encode_regions_packed(vb200_handle h, int32_t n, int32_t max_boxes, const int32_t* n_boxes, const float* box_features,
+                                const float* boxes, const float* image_wh, float* state_f32, void* state_16, void* cuda_stream) {
+    if (h == nullptr) return VB200_ERR_INVALID;
+    return guard(h, [&] {
+        const char* api = "vb200_encode_regions_packed";
+        if (!n_boxes || !box_features || !boxes || !image_wh || !state_f32 || !state_16) fail(VB200_ERR_INVALID, "%s: NULL pointer", api);
+        if (max_boxes < 0) fail(VB200_ERR_INVALID, "%s: negative capacity max_boxes %d", api, max_boxes);
+        const int max_rows = h->max_rows;
+        if (max_boxes > max_rows - 1)
+            fail(VB200_ERR_INVALID, "%s: capacity max_boxes %d above %d (V = boxes + 1 <= %d)", api, max_boxes, max_rows - 1, max_rows);
+        // regions per image = boxes + the global mean row, checked in the caller's units before pack_batch sees V_i
+        std::vector<int32_t> nv;
+        for (int i = 0; i < n; ++i) {
+            const int k = n_boxes[i];
+            if (k < 1) fail(VB200_ERR_INVALID, "%s: image %d has n_boxes %d (must be >= 1)", api, i, k);
+            if (max_boxes > 0 && k > max_boxes)
+                fail(VB200_ERR_INVALID, "%s: image %d has n_boxes %d, above the capacity max_boxes %d", api, i, k, max_boxes);
+            if (k + 1 > max_rows)
+                fail(VB200_ERR_INVALID, "%s: image %d has n_boxes %d (V = n_boxes + 1 must be <= %d)", api, i, k, max_rows);
+            nv.push_back(k + 1);
+        }
+        // the PACKED_IMAGE_PREFIX plan of vb200_encode_image_packed at max_regions = max_boxes + 1, fed by the region pack of
+        // vb200_forward_regions_packed: each image's rows are the rows that forward writes for it
+        h->run_packed(api, vb200_engine::PACKED_IMAGE_PREFIX, {"image", n, nullptr, 0, nv.data(), max_boxes > 0 ? max_boxes + 1 : 0}, 0, 0,
+                      nullptr, cuda_stream, [&](Plan& pl, const PackedBatch& b, cudaStream_t st) {
+                          h->encode_regions(pl, box_features, boxes, image_wh, b.rows_v(), state_f32, state_16, st);
                       });
     });
 }

@@ -816,6 +816,47 @@ class VILBertForVLTasks(object):
         return st
 
     @torch.no_grad()
+    def encode_regions_packed(self, box_features, boxes, image_wh, n_boxes, max_boxes: int = 0):
+        """``encode_image_packed`` from detector output, as ``forward_regions_packed`` takes it: ``box_features`` ``[sum n_boxes_i, F]``,
+        pixel ``boxes`` ``[sum n_boxes_i, 4]``, ``image_wh`` ``[n, 2]``, ``n_boxes`` (list or CPU tensor) the box counts.  Image i's
+        state is V_i = n_boxes_i + 1 rows, its global mean row first, built on the device by the region pack of
+        ``forward_regions_packed``: ``forward_cached_packed`` on these states gives that forward's scores bit for bit.
+        ``max_boxes`` (0: this call's maximum) is the plan capacity; the plan is ``encode_image_packed``'s at ``max_regions =
+        max_boxes + 1``."""
+        if self._handle is None:
+            raise L.VilbertB200Error("call model.cuda(i) first (worker.py:536); there is no CPU path")
+        lib = L.load()
+        device = torch.device("cuda", self._device)
+        nb = _host_ints(n_boxes)
+        n = len(nb)
+        bf = torch.as_tensor(box_features).to(device=device, dtype=torch.float32).reshape(-1, self._dims["v_feature_size"]).contiguous()
+        bx = torch.as_tensor(boxes).to(device=device, dtype=torch.float32).reshape(-1, 4).contiguous()
+        wh = torch.as_tensor(image_wh).to(device=device, dtype=torch.float32).contiguous()
+        if n < 1 or bf.shape[0] != sum(nb) or bx.shape[0] != sum(nb) or tuple(wh.shape) != (n, 2):
+            raise ValueError("encode_regions_packed: box_features / boxes need sum(n_boxes) rows and image_wh [n, 2] for n >= 1 images")
+        offs = packed_offsets(nb, 1)
+        Hv = self._dims["v_hidden_size"]
+        st = dict(kind="image", n=n, offsets=torch.tensor(offs, dtype=torch.int32), max_len=max(nb) + 1,
+                  f32=torch.empty(offs[-1], Hv, dtype=torch.float32, device=device),
+                  h16=torch.empty(offs[-1], Hv, dtype=torch.int16, device=device))
+        nb_c = (C.c_int32 * n)(*nb)
+        with torch.cuda.device(device):
+            stream = torch.cuda.current_stream(device).cuda_stream
+            L.check(lib.vb200_encode_regions_packed(self._handle, n, int(max_boxes), C.cast(nb_c, C.c_void_p), bf.data_ptr(), bx.data_ptr(),
+                                                    wh.data_ptr(), st["f32"].data_ptr(), st["h16"].data_ptr(), C.c_void_p(stream)),
+                    self._handle)
+        return st
+
+    @torch.no_grad()
+    def encode_detections_packed(self, detections, image_wh, max_boxes: int = 100, conf_thresh: float = 0.0, background: bool = False):
+        """A retrieval gallery from the detector's raw heads: one ``select_regions`` of every image (``detections`` as there) into a
+        packed device buffer, then one ``encode_regions_packed`` of the k_i = min(max_boxes, n_i) selected boxes with the images'
+        ``image_wh`` ``[n, 2]``.  No feature row passes through the host.  Returns the ``encode_regions_packed`` state; the plan
+        capacity is ``max_boxes``, so galleries of any proposal counts share one plan."""
+        r = self.select_regions(detections, max_boxes, conf_thresh, background)
+        return self.encode_regions_packed(r["box_features"], r["boxes"], image_wh, r["n_boxes"], max_boxes=max_boxes)
+
+    @torch.no_grad()
     def forward_cached_packed(self, text_state, text_index, image_state, image_index, select: int = L.OUT_VIL_LOGIT, slot: int = 0,
                               max_tokens: Optional[int] = None, max_regions: Optional[int] = None, debug_taps: bool = False):
         """Pair b = (caption text_index[b], image image_index[b]) from packed states, every pair at its own lengths.  Index tensors may

@@ -184,20 +184,41 @@ def retrieval_scores_packed(model, captions, images, task_id: int = 7, pair_batc
     `pair_batch` from the packed states (`model.forward_cached_packed`, one plan per chunk size).  Each score equals the
     unpadded forward of its pair; with uniform lengths and no padding it is bit-identical to `retrieval_scores_cached`.  One
     all-gather at the end.  `timings` (dict) receives CUDA-event milliseconds: encode / pairs / gather."""
+    f, s, vm = images
+    v_lens = strip_padding(vm, "image_mask")
+    return _score_packed_states(model, captions, lambda: model.encode_image_packed(pack_rows(f, v_lens), pack_rows(s, v_lens), v_lens),
+                                f.shape[0], task_id, pair_batch, group, comm, timings)
+
+
+def retrieval_scores_regions(model, captions, gallery, task_id: int = 7, pair_batch: int = 256, max_boxes: int = 0, group=None,
+                             comm=None, timings=None) -> torch.Tensor:
+    """`retrieval_scores_packed` with the gallery as the detector returns it: `gallery` = (box_features [sum n_boxes_i, F], pixel
+    boxes [sum n_boxes_i, 4], image_wh [n_img, 2], n_boxes), the images' selected boxes back to back, on the model's device.  The
+    gallery is encoded once with `model.encode_regions_packed` (capacity `max_boxes`, 0: the largest image), which builds each
+    image's global mean row and locations on the device as `forward_regions_packed` does, so every score is bit-identical to that
+    forward of its (caption, image) pair.  `captions` (padded, prefix masks), sharding, pair chunks, the all-gather and `timings`
+    follow `retrieval_scores_packed`."""
+    bf, bx, wh, n_boxes = gallery
+    return _score_packed_states(model, captions, lambda: model.encode_regions_packed(bf, bx, wh, n_boxes, max_boxes=max_boxes),
+                                len(n_boxes), task_id, pair_batch, group, comm, timings)
+
+
+def _score_packed_states(model, captions, encode_gallery, n_img, task_id, pair_batch, group, comm, timings) -> torch.Tensor:
+    """What the packed retrieval calls share: this rank's block of the padded `captions` (prefix masks), the gallery states of
+    `encode_gallery()`, every pair scored in chunks of `pair_batch` from the packed states (`model.forward_cached_packed`), and one
+    all-gather."""
     from . import _lib as L
     world = dist.get_world_size(group) if dist.is_initialized() else 1
     rank = dist.get_rank(group) if dist.is_initialized() else 0
     q, seg, im = captions
-    f, s, vm = images
-    n_cap, n_img = q.shape[0], f.shape[0]
+    n_cap, dev = q.shape[0], q.device
     lo, hi = shard_range(n_cap, rank, world)
-    dev = f.device
-    t_lens, v_lens = strip_padding(im[lo:hi], "input_mask"), strip_padding(vm, "image_mask")
+    t_lens = strip_padding(im[lo:hi], "input_mask")
     ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)] if timings is not None else None
     if ev:
         ev[0].record()
     task = torch.full((hi - lo, 1), task_id, dtype=torch.long, device=dev)
-    vs = model.encode_image_packed(pack_rows(f, v_lens), pack_rows(s, v_lens), v_lens)
+    vs = encode_gallery()
     ts = model.encode_text_packed(pack_rows(q[lo:hi], t_lens), pack_rows(seg[lo:hi], t_lens), task, t_lens)
     if ev:
         ev[1].record()
