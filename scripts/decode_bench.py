@@ -2,8 +2,9 @@
 
 (a) Decode only.  64 mixed messages -- 16 VQA, 16 GQA, 12 NLVR2 pairs, 12 grounding images with 100 boxes (101 vision rows) and 8
     retrievals over 10 images -- packed into one `forward_regions_packed` call, run once.  Then, alternating, the per-message
-    `_decode` loop of `custom_prediction_packed` and one device decode of the same outputs (`worker_api._decode_device`); both end
-    in a host synchronisation.  Wall time on the host thread, median over --rounds windows of --reps calls each.
+    `_decode` loop of `custom_prediction_packed` and one device decode of the same outputs (`worker_api._answer_regions` with
+    decode="host" and "device"); both end in a host synchronisation.  Wall time on the host thread, median over --rounds windows
+    of --reps calls each.
 (b) The worker window of scripts/regions_packed_bench.py: 64 single-image VQA messages with 100 boxes.  First the real
     `MicroBatchWorker(packed=True)` with decode="host" and decode="device", alternating (messages/s from the first submit to the last
     result).  Then the same steps inline on this thread, split into pack (`pack_region_requests`), forward (`forward_regions_packed`
@@ -67,21 +68,14 @@ def decode_only(model, F, args):
     out, spatials = model.forward_regions_packed(p["question"], p["segment_ids"], p["task_tokens"], p["box_features"], p["boxes"],
                                                  p["image_wh"], p["n_tokens"], p["n_boxes"], select=p["select"],
                                                  max_tokens=p["max_tokens"], max_boxes=p["max_boxes"])
-    import numpy as np
     import torch
     torch.cuda.synchronize()
-    v_off = np.concatenate([[0], np.cumsum([n + 1 for n in p["n_boxes"]])])
-    tasks = {i: (r[4], r[3]) for i, r in enumerate(reqs)}
 
     def host():
-        res = {}
-        for i, (lo, hi) in p["spans"].items():
-            sl, sp = W.split_region_outputs(out, spatials, p["n_tokens"], p["n_boxes"], lo, hi, reqs[i][4])
-            res[i] = W._decode(reqs[i][4], sl, sp, reqs[i][3])
-        return res
+        return W._answer_regions({}, reqs, out, spatials, p["spans"], p["n_tokens"], p["n_boxes"], "host")
 
     def device():
-        return W._decode_device(out, spatials, tasks, p["spans"], v_off)
+        return W._answer_regions({}, reqs, out, spatials, p["spans"], p["n_tokens"], p["n_boxes"], "device")
 
     a, b = host(), device()
     same_idx = 0
@@ -100,7 +94,7 @@ def decode_only(model, F, args):
     res = {name: {"ms_per_batch": 1e3 * statistics.median(s), "windows_ms": [1e3 * x for x in s]} for name, s in secs.items()}
     res["speedup"] = res["host"]["ms_per_batch"] / res["device"]["ms_per_batch"]
     res["answers_agree"] = f"{same_idx}/{len(a)}"
-    res["messages"], res["forward_rows"], res["vision_rows"] = len(reqs), len(p["n_boxes"]), int(v_off[-1])
+    res["messages"], res["forward_rows"], res["vision_rows"] = len(reqs), len(p["n_boxes"]), sum(p["n_boxes"]) + len(p["n_boxes"])
     return res
 
 
@@ -147,15 +141,7 @@ def worker_window(model, F, args):
                                                      max_tokens=p["max_tokens"], max_boxes=p["max_boxes"])
         torch.cuda.synchronize()
         t.append(time.perf_counter())
-        if decode == "device":
-            import numpy as np
-            v_off = np.concatenate([[0], np.cumsum([n + 1 for n in p["n_boxes"]])])
-            dec = W._decode_device(out, spatials, {i: (r[4], r[3]) for i, r in enumerate(reqs)}, p["spans"], v_off)
-        else:
-            dec = {}
-            for i, (lo, hi) in p["spans"].items():
-                sl, sp = W.split_region_outputs(out, spatials, p["n_tokens"], p["n_boxes"], lo, hi, reqs[i][4])
-                dec[i] = W._decode(reqs[i][4], sl, sp, reqs[i][3])
+        dec = W._answer_regions({}, reqs, out, spatials, p["spans"], p["n_tokens"], p["n_boxes"], decode)
         t.append(time.perf_counter())
         for i, (b, _, _) in enumerate(msgs):
             W.shape_result(b["task_id"], dec[i], b["image_path"])

@@ -1,4 +1,4 @@
-"""Packed detector-output batches on CPU: worker_api.pack_region_requests / split_region_outputs / custom_prediction_packed and
+"""Packed detector-output batches on CPU: worker_api.pack_region_requests / _split_outputs / custom_prediction_packed and
 MicroBatchWorker(packed=True) with a stub in place of the engine, plus the C ABI surface of vb200_forward_regions_packed
 (vb200_packed_region_inputs layout, export, NULL handle).  The engine call itself is covered by tests/test_gpu_regions_packed.py."""
 import ctypes as C
@@ -140,14 +140,16 @@ def test_offsets_and_filler_rows_through_custom_prediction_packed():
     assert np.allclose(ans[2]["top3_confidence"], conf.tolist())
 
 
-def test_split_region_outputs_layout():
+def test_split_outputs_layout():
     out, sp = StubRegionModel().forward_regions_packed(torch.zeros(12, dtype=torch.long), torch.zeros(12, dtype=torch.long),
                                                        torch.zeros(4, 1, dtype=torch.long), torch.zeros(14, 8), torch.zeros(14, 4),
                                                        torch.ones(4, 2), [3, 2, 2, 5], [1, 4, 6, 3])
-    sl, s = W.split_region_outputs(out, sp, [3, 2, 2, 5], [1, 4, 6, 3], 1, 3, "12")
+    v_off = [0, 2, 7, 14, 18]                                         # boxes [1, 4, 6, 3], each with its global row
+    t_off = [0, 4, 7, 10, 16]                                         # tokens [3, 2, 2, 5], each with its task token
+    sl, s = W._split_outputs(out, sp, 1, 3, v_off, t_off, "12")
     assert torch.equal(sl[0], out[0][1:3]) and torch.equal(sl[3], out[3][0:1])
     assert torch.equal(sl[6], out[6][2:14]) and torch.equal(sl[8], out[8][4:10]) and torch.equal(s, sp[2:14])
-    sl, s = W.split_region_outputs(out, sp, [3, 2, 2, 5], [1, 4, 6, 3], 3, 4, "11")
+    sl, s = W._split_outputs(out, sp, 3, 4, v_off, t_off, "11")
     assert sl[6].shape == (1, 4, 1) and torch.equal(sl[6][0], out[6][14:18]) and s.shape == (1, 4, 5)
     assert sl[3].numel() == 0
 

@@ -20,6 +20,7 @@ import os
 import pickle
 import re
 import unicodedata
+from itertools import accumulate
 from typing import Dict, List, Optional, Sequence
 
 import numpy as np
@@ -110,33 +111,18 @@ def _expand_text(task_id, n_rows, question, input_mask, segment_ids, task_tokens
 
 
 def _decode(task_id, out, spatials, infos):
-    """Logits of ONE request -> the reference's answer (worker.py:295-386)."""
-    N = len(infos) if task_id == "7" else 3                      # worker.py:250-253
-    (vil_prediction, vil_prediction_gqa, vil_logit, vil_binary_prediction, vil_tri_prediction, _vision_prediction,
-     vision_logit, _linguisic_prediction, _linguisic_logit, _attn) = out
-    if task_id in ("1", "2"):
-        conf, idx = _top(torch.softmax(vil_prediction.view(-1), dim=0), N)
-        return {"top3_answer": [_label("vqa", i) for i in idx], "top3_confidence": conf}
-    if task_id == "15":
-        conf, idx = _top(torch.softmax(vil_prediction_gqa.view(-1), dim=0), N)
-        return {"top3_answer": [_label("gqa", i) for i in idx], "top3_confidence": conf}
-    if task_id == "12":
-        names = {0: "False", 1: "True"}
-        conf, idx = _top(torch.softmax(vil_binary_prediction.view(-1), dim=0), 2)
-        return {"top3_answer": [names[i] for i in idx], "top3_confidence": conf}
-    if task_id == "13":
-        names = {0: "contradiction (false)", 1: "neutral", 2: "entailment (true)"}
-        conf, idx = _top(torch.softmax(vil_tri_prediction.view(-1), dim=0), 3)
-        return {"top3_answer": [names[i] for i in idx], "top3_confidence": conf}
-    if task_id == "7":
-        conf, idx = _top(torch.softmax(vil_logit.view(-1), dim=0), N)
-        return {"top3_answer": idx, "top3_confidence": conf}
-    # grounding: softmax over ALL rows of vision_logit, the synthetic global box included (worker.py:374-385)
-    image_w, image_h = infos[0]["image_width"], infos[0]["image_height"]
-    conf, idx = _top(torch.softmax(vision_logit.view(-1), dim=0), N)
-    boxes = spatials[0][torch.as_tensor(idx, device=spatials.device)][:, :4].tolist()
-    return [{"y1": int(b[1] * image_h), "y2": int(b[3] * image_h), "x1": int(b[0] * image_w), "x2": int(b[2] * image_w),
-             "confidence": c * 100} for b, c in zip(boxes, conf)]
+    """Logits of ONE request -> the reference's answer (worker.py:295-386): softmax over the task's output flattened, top-N, and
+    for grounding the top rows' boxes in pixels.  Grounding ranks ALL rows of vision_logit, the synthetic global box included
+    (worker.py:374-385), and reads the boxes from the image's spatials [1, V, 5]."""
+    top = len(infos) if task_id == "7" else 2 if task_id == "12" else 3          # worker.py:250-253
+    # OUT_* bit k selects element k of the 10-tuple
+    conf, idx = _top(torch.softmax(out[TASK_OUTPUT[task_id].bit_length() - 1].view(-1), dim=0), top)
+    boxes = None
+    if task_id in GROUNDING_TASKS:
+        w, h = infos[0]["image_width"], infos[0]["image_height"]
+        boxes = [[int(b[0] * w), int(b[1] * h), int(b[2] * w), int(b[3] * h)]
+                 for b in spatials[0][torch.as_tensor(idx, device=spatials.device)][:, :4].tolist()]
+    return _answer(task_id, idx, conf, boxes)
 
 
 def _check_decode(decode):
@@ -168,7 +154,8 @@ def decode_messages(tasks, spans, v_off):
 
 
 def _answer(task_id, idx, conf, boxes):
-    """`_decode`'s answer for one request from a device decode's indices, probabilities and boxes."""
+    """The answer dict of one request from its top-N indices, probabilities and, for grounding, pixel boxes [x1, y1, x2, y2]
+    (as `_decode` and `model.decode_answers` rank them)."""
     if task_id in ("1", "2"):
         return {"top3_answer": [_label("vqa", i) for i in idx], "top3_confidence": conf}
     if task_id == "15":
@@ -184,16 +171,64 @@ def _answer(task_id, idx, conf, boxes):
     return [{"y1": b[1], "y2": b[3], "x1": b[0], "x2": b[2], "confidence": c * 100} for b, c in zip(boxes, conf)]
 
 
-def _decode_device(out, spatials, tasks, spans, v_off):
-    """Every request of one forward decoded by one `model.decode_answers` call -> {request: `_decode`'s answer}."""
-    msgs = decode_messages(tasks, spans, v_off)
-    if not msgs:
-        return {}
-    if spatials is not None:
-        spatials = spatials.to(device=torch.device("cuda", model._device), dtype=torch.float32).contiguous()
-    with model_lock:
-        res = model.decode_answers(out, [m for _, m in msgs], spatials)
-    return {i: _answer(m[0], *r) for (i, m), r in zip(msgs, res)}
+def _row_layout(accepted, bucket, select):
+    """The batch rows of one model call.  `accepted` lists the requests in order as `(request, task_id, its rows)`.
+
+    An NLVR2 pair starts on an even row -- the binary head consumes adjacent rows as one pair (worker.py:266-276) -- with ONE
+    filler row in front when needed.  The engine keeps one plan per batch size and select, so that a long-running worker sees a
+    small, fixed set of plans: the batch is padded with filler rows to a multiple of `bucket` (and to an even count when the pair
+    head is computed), and `select` (default: the seven task heads) is ORed with the heads the requests read.
+    Returns (the rows, None at filler positions; spans {request: (first row, end row)}; the select mask)."""
+    rows, spans, need = [], {}, 0
+    for i, task_id, own in accepted:
+        if task_id in PAIR_TASKS and len(rows) % 2 == 1:
+            rows.append(None)
+        spans[i] = (len(rows), len(rows) + len(own))
+        rows += own
+        need |= TASK_OUTPUT[task_id]
+    sel = (L.OUT_TASK_HEADS if select is None else int(select)) | need
+    target = -(-len(rows) // bucket) * bucket
+    if target % 2 == 1 and (sel & L.OUT_VIL_BINARY_PREDICTION):
+        target += 1
+    return rows + [None] * (target - len(rows)), spans, sel
+
+
+def _split_outputs(out, spatials, lo, hi, v_off, t_off, task_id):
+    """Rows [lo, hi) of a forward's outputs -> the 10-tuple and spatials `_decode` reads for one request.  Per-image outputs are
+    sliced and the pair head keeps the request's pair.  Per-row outputs and spatials, packed [rows, ...], keep the request's vision
+    rows [v_off[lo], v_off[hi]) and text rows [t_off[lo], t_off[hi]), shaped [1, rows, ...] for a single image."""
+    sl = [None if o is None else o[lo:hi] for o in out[:5]] + [None] * 4 + [[]]
+    if out[3] is not None:
+        sl[3] = out[3][lo // 2:hi // 2] if task_id == "12" else out[3][0:0]
+    one = hi - lo == 1
+    for k, offs in ((5, v_off), (6, v_off), (7, t_off), (8, t_off)):
+        if out[k] is not None:
+            r = out[k][int(offs[lo]):int(offs[hi])]
+            sl[k] = r.reshape(1, -1, r.shape[-1]) if one else r
+    sp = spatials[int(v_off[lo]):int(v_off[hi])]
+    return tuple(sl), (sp.reshape(1, -1, 5) if one else sp)
+
+
+def _answer_spans(answers, out, spatials, tasks, spans, v_off, t_off, decode):
+    """Fill in `answers[i]` for every request i of `spans` from one forward's outputs; `tasks` maps a request to `(task_id, infos)`
+    and `v_off` / `t_off` give the first vision / text row of every batch row (see `_split_outputs`).  decode="device": one
+    `model.decode_answers` call for all of them, given the spatials only when a grounding request reads them; "host": `_decode`
+    per request on its slice of the outputs and spatials."""
+    if decode == "device":
+        msgs = decode_messages(tasks, spans, v_off)
+        sp = None
+        if any(m[0] in GROUNDING_TASKS for _, m in msgs):
+            sp = spatials.to(device=torch.device("cuda", model._device), dtype=torch.float32).contiguous()
+        with model_lock:
+            res = model.decode_answers(out, [m for _, m in msgs], sp)
+        for (i, m), r in zip(msgs, res):
+            answers[i] = _answer(m[0], *r)
+        return answers
+    for i, (lo, hi) in spans.items():
+        task_id, infos = tasks[i]
+        sl, sp = _split_outputs(out, spatials, lo, hi, v_off, t_off, task_id)
+        answers[i] = _decode(task_id, sl, sp, infos)
+    return answers
 
 
 def prediction(question, features, spatials, segment_ids, input_mask, image_mask, co_attention_mask, task_tokens,
@@ -226,7 +261,6 @@ def prediction_batch(requests, bucket: int = 8, select: Optional[int] = None, *,
     if bucket < 1:
         raise ValueError("bucket must be >= 1")
     _check_decode(decode)
-    fixed_select = L.OUT_TASK_HEADS if select is None else int(select)
     answers = [None] * len(requests)
     groups = {}
     for i, r in enumerate(requests):
@@ -239,46 +273,29 @@ def prediction_batch(requests, bucket: int = 8, select: Optional[int] = None, *,
         key = (question.shape[1], features.shape[1], features.shape[2])
         groups.setdefault(key, []).append(i)
     for idxs in groups.values():
-        rows, spans, need = [], {}, 0
-        n = 0
+        accepted = []
         for i in idxs:
             (question, features, spatials, segment_ids, input_mask, image_mask, co_mask, task_tokens, task_id, infos) = requests[i]
             q, im, seg, tk = _expand_text(task_id, features.size(0), question, input_mask, segment_ids, task_tokens)
-            if task_id == "12" and n % 2 == 1:            # ONE filler row so that the pair starts on an even row
-                rows.append(tuple(t[-1:] for t in rows[-1]))
-                n += 1
             if co_mask is None:
                 co_mask = torch.zeros(features.size(0), features.size(1), question.size(1), device=features.device)
-            rows.append((q, features, spatials, seg, im, image_mask, co_mask, tk))
-            spans[i] = (n, n + features.size(0))
-            n += features.size(0)
-            need |= TASK_OUTPUT[task_id]
-        sel = fixed_select | need
-        target = -(-n // bucket) * bucket
-        if target % 2 == 1 and (sel & L.OUT_VIL_BINARY_PREDICTION):
-            target += 1                                    # the binary head needs an even number of rows
-        if target > n:                                     # filler rows: copies of the last row, results discarded
-            last = tuple(t[-1:] for t in rows[-1])
-            rows.append(tuple(t.expand(target - n, *t.shape[1:]) for t in last))
-            n = target
-        cat = [torch.cat([r[k] for r in rows], dim=0) for k in range(8)]
+            # every row of the request refers to the request's tensors, which go into the batch once
+            accepted.append((i, task_id, [(q, features, spatials, seg, im, image_mask, co_mask, tk)] * features.size(0)))
+        rows, spans, sel = _row_layout(accepted, bucket, select)
+        parts = []                                         # filler rows: copies of the row before them, results discarded
+        for r in rows:
+            if r is None:
+                parts.append(tuple(t[-1:] for t in parts[-1]))
+            elif not parts or r is not parts[-1]:
+                parts.append(r)
+        cat = [torch.cat([r[k] for r in parts], dim=0) for k in range(8)]
         with model_lock:
             out = model(*cat, output_all_attention_masks=True, select=sel)
-        if decode == "device":
-            V = cat[1].shape[1]
-            ground = any(requests[i][8] in GROUNDING_TASKS for i in idxs)
-            dec = _decode_device(out, cat[2] if ground else None, {i: (requests[i][8], requests[i][9]) for i in idxs}, spans,
-                                 [k * V for k in range(n + 1)])
-            for i in idxs:
-                answers[i] = dec[i]
-            continue
-        for i in idxs:
-            lo, hi = spans[i]
-            task_id, infos, spatials = requests[i][8], requests[i][9], requests[i][2]
-            sl = [None if o is None or isinstance(o, list) else o[lo:hi] for o in out[:9]] + [[]]
-            if out[3] is not None:
-                sl[3] = out[3][lo // 2:hi // 2] if task_id == "12" else out[3][0:0]
-            answers[i] = _decode(task_id, tuple(sl), spatials, infos)
+        # the per-row outputs [B, rows, ...] and the spatials in the packed layout [B * rows, ...]
+        V, T = cat[1].shape[1], next((o.shape[1] for o in out[7:9] if o is not None), 0)
+        out = tuple(o.flatten(0, 1) if 5 <= k <= 8 and o is not None else o for k, o in enumerate(out))
+        _answer_spans(answers, out, cat[2].flatten(0, 1), {i: (requests[i][8], requests[i][9]) for i in idxs}, spans,
+                      [k * V for k in range(len(rows) + 1)], [k * T for k in range(len(rows) + 1)], decode)
     return answers
 
 
@@ -300,9 +317,8 @@ def prediction_packed(requests, bucket: int = 8, select: Optional[int] = None, *
     if bucket < 1:
         raise ValueError("bucket must be >= 1")
     _check_decode(decode)
-    fixed_select = L.OUT_TASK_HEADS if select is None else int(select)
     answers = [None] * len(requests)
-    samples, spans, need = [], {}, 0            # samples: (tokens [Tin], segments [Tin], task [1], features [V, F], spatials [V, 5])
+    accepted = []                               # rows: (tokens [Tin], segments [Tin], task [1], features [V, F], spatials [V, 5])
     max_tin, max_v, F, dev = 1, 1, None, None
     for i, r in enumerate(requests):
         (question, features, spatials, segment_ids, input_mask, image_mask, co_mask, task_tokens, task_id, infos) = r
@@ -318,20 +334,11 @@ def prediction_packed(requests, bucket: int = 8, select: Optional[int] = None, *
             answers[i] = e
             continue
         F, dev = features.size(2), features.device
-        if task_id == "12" and len(samples) % 2 == 1:
-            samples.append(None)                    # filler: the pair starts on an even row
-        spans[i] = (len(samples), len(samples) + features.size(0))
-        for j, k in enumerate(lens):
-            samples.append((q[j, :k], seg[j, :k], tk[j].reshape(1), features[j], spatials[j]))
+        accepted.append((i, task_id, [(q[j, :k], seg[j, :k], tk[j].reshape(1), features[j], spatials[j]) for j, k in enumerate(lens)]))
         max_tin, max_v = max(max_tin, q.size(1)), max(max_v, features.size(1))
-        need |= TASK_OUTPUT[task_id]
-    if not spans:
+    if not accepted:
         return answers
-    sel = fixed_select | need
-    target = -(-len(samples) // bucket) * bucket
-    if target % 2 == 1 and (sel & L.OUT_VIL_BINARY_PREDICTION):
-        target += 1                                  # the binary head needs an even number of rows
-    samples += [None] * (target - len(samples))
+    samples, spans, sel = _row_layout(accepted, bucket, select)
     filler = (torch.zeros(1, dtype=torch.long, device=dev), torch.zeros(1, dtype=torch.long, device=dev),
               torch.zeros(1, dtype=torch.long, device=dev), torch.zeros(1, F, device=dev), torch.zeros(1, 5, device=dev))
     samples = [filler if smp is None else smp for smp in samples]
@@ -341,27 +348,10 @@ def prediction_packed(requests, bucket: int = 8, select: Optional[int] = None, *
     with model_lock:
         out = model.forward_packed(cat[0], cat[3], cat[4], cat[1], cat[2].view(-1, 1), n_tokens, n_regions, select=sel,
                                    max_tokens=max_tin, max_regions=max_v)
-    t_off = np.concatenate([[0], np.cumsum([n + 1 for n in n_tokens])])   # packed text rows (task token included)
-    v_off = np.concatenate([[0], np.cumsum(n_regions)])
-    if decode == "device":
-        ground = any(requests[i][8] in GROUNDING_TASKS for i in spans)
-        dec = _decode_device(out, cat[4] if ground else None, {i: (requests[i][8], requests[i][9]) for i in spans}, spans, v_off)
-        for i in spans:
-            answers[i] = dec[i]
-        return answers
-    for i, (lo, hi) in spans.items():
-        task_id, infos, spatials = requests[i][8], requests[i][9], requests[i][2]
-        sl = [None if o is None or isinstance(o, list) else o[lo:hi] for o in out[:9]] + [[]]
-        if out[3] is not None:
-            sl[3] = out[3][lo // 2:hi // 2] if task_id == "12" else out[3][0:0]
-        for k in (5, 6):                             # per-region rows: [images, V, ...] (the request's images share V)
-            if out[k] is not None:
-                sl[k] = out[k][int(v_off[lo]):int(v_off[hi])].reshape(hi - lo, -1, out[k].shape[-1])
-        for k in (7, 8):                             # per-token rows
-            if out[k] is not None:
-                sl[k] = out[k][int(t_off[lo]):int(t_off[hi])].reshape(hi - lo, -1, out[k].shape[-1])
-        answers[i] = _decode(task_id, tuple(sl), spatials, infos)
-    return answers
+    return _answer_spans(answers, out, cat[4], {i: (requests[i][8], requests[i][9]) for i in spans}, spans,
+                         list(accumulate(n_regions, initial=0)),
+                         list(accumulate([n + 1 for n in n_tokens], initial=0)),    # each text: its tokens and the task token
+                         decode)
 
 
 def build_inputs(query, task, features, infos, device, tok=None):
@@ -453,6 +443,21 @@ def _max_rows() -> int:
     return int(getattr(model, "max_rows_per_sample", 256))
 
 
+def _region_text(query, tok, max_rows):
+    """The text half of a packed region request: the query's real tokens and segments, at most `max_rows` - 1 of them."""
+    tokens, segs = real_tokens(query, tok)
+    if len(tokens) + 1 > max_rows:
+        raise ValueError(f"query of {len(tokens)} tokens: packed rows hold at most {max_rows - 1}")
+    return tokens, segs
+
+
+def _region_rows(task_id, task, tokens, segs, imgs):
+    """The rows of a packed region request, `(tokens, segments, task token) + image half`: the text repeated per image for NLVR2
+    and retrieval (worker.py:266-284), else with the first image only."""
+    t = int(np.array(task).reshape(-1)[0])
+    return [(tokens, segs, t) + img for img in (imgs if task_id in PAIR_TASKS + RETRIEVAL_TASKS else imgs[:1])]
+
+
 def pack_region_requests(requests, bucket: int = 8, select: Optional[int] = None, max_boxes: int = 100, tok=None):
     """The host half of `custom_prediction_packed`: `custom_prediction` argument tuples `(query, task, features, infos, task_id)` ->
     the inputs of ONE `forward_regions_packed` call, as CPU tensors.
@@ -465,18 +470,15 @@ def pack_region_requests(requests, bucket: int = 8, select: Optional[int] = None
     n_tokens, n_boxes, question, segment_ids, task_tokens [B, 1], box_features, boxes, image_wh, select, max_tokens, max_boxes."""
     if bucket < 1:
         raise ValueError("bucket must be >= 1")
-    fixed_select = L.OUT_TASK_HEADS if select is None else int(select)
     max_rows = _max_rows()
     answers = [None] * len(requests)
-    rows, spans, need, F = [], {}, 0, None        # rows: (tokens, segments, task, box features [n, F], boxes [n, 4], (w, h))
+    accepted, F = [], None                        # rows: (tokens, segments, task, box features [n, F], boxes [n, 4], (w, h))
     for i, (query, task, features, infos, task_id) in enumerate(requests):
         try:
             _validate(task_id, infos)
             if len(features) != len(infos):
                 raise ValueError(f"{len(features)} feature arrays for {len(infos)} images")
-            tokens, segs = real_tokens(query, tok)
-            if len(tokens) + 1 > max_rows:
-                raise ValueError(f"query of {len(tokens)} tokens: packed rows hold at most {max_rows - 1}")
+            tokens, segs = _region_text(query, tok, max_rows)
             imgs = []
             for f, info in zip(features, infos):
                 f = torch.as_tensor(f, dtype=torch.float32)
@@ -488,23 +490,13 @@ def pack_region_requests(requests, bucket: int = 8, select: Optional[int] = None
                 if bx.dim() != 2 or bx.shape[0] < n or bx.shape[1] < 4:
                     raise ValueError(f"bbox of shape {tuple(bx.shape)} for {n} boxes")
                 imgs.append((f, bx[:n, :4], (float(info["image_width"]), float(info["image_height"]))))
-            t = int(np.array(task).reshape(-1)[0])
+            own = _region_rows(task_id, task, tokens, segs, imgs)
         except Exception as e:                      # noqa: BLE001 -- the request's answer, as callback()'s catch-all (worker.py:653-655)
             answers[i] = e
             continue
         F = int(imgs[0][0].shape[1])
-        if task_id in PAIR_TASKS and len(rows) % 2 == 1:
-            rows.append(None)                       # filler: the pair starts on an even row
-        rep = task_id in PAIR_TASKS + RETRIEVAL_TASKS
-        spans[i] = (len(rows), len(rows) + (len(imgs) if rep else 1))
-        for f, bx, wh in (imgs if rep else imgs[:1]):
-            rows.append((tokens, segs, t, f, bx, wh))
-        need |= TASK_OUTPUT[task_id]
-    sel = fixed_select | need
-    target = -(-len(rows) // bucket) * bucket
-    if target % 2 == 1 and (sel & L.OUT_VIL_BINARY_PREDICTION):
-        target += 1                                 # the binary head needs an even number of rows
-    rows += [None] * (target - len(rows))
+        accepted.append((i, task_id, own))
+    rows, spans, sel = _row_layout(accepted, bucket, select)
     filler = ([0], [0], 0, torch.zeros(1, F or 1), torch.zeros(1, 4), (1.0, 1.0))
     rows = [filler if r is None else r for r in rows]
     n_tokens = [len(r[0]) for r in rows]
@@ -519,25 +511,12 @@ def pack_region_requests(requests, bucket: int = 8, select: Optional[int] = None
                 select=sel, max_tokens=max([MAX_LENGTH] + n_tokens), max_boxes=max([int(max_boxes)] + n_boxes))
 
 
-def split_region_outputs(out, spatials, n_tokens, n_boxes, lo, hi, task_id):
-    """Rows [lo, hi) of a `forward_regions_packed` result -> the 10-tuple and spatials `_decode` reads for one request.  Per-image
-    outputs are sliced; the pair head keeps the request's pair; per-row outputs (and spatials) keep the request's packed rows, shaped
-    [1, V, ...] for a single-image request (the grounding decode reads its own vision_logit and spatials rows)."""
-    t_off = np.concatenate([[0], np.cumsum([n + 1 for n in n_tokens])])   # packed text rows (task token included)
-    v_off = np.concatenate([[0], np.cumsum([n + 1 for n in n_boxes])])    # packed regions: the global row, then the boxes
-    sl = [None if o is None or isinstance(o, list) else o[lo:hi] for o in out[:9]] + [[]]
-    if out[3] is not None:
-        sl[3] = out[3][lo // 2:hi // 2] if task_id == "12" else out[3][0:0]
-    one = hi - lo == 1
-    for k, offs in ((5, v_off), (6, v_off), (7, t_off), (8, t_off)):
-        if out[k] is not None:
-            r = out[k][int(offs[lo]):int(offs[hi])]
-            sl[k] = r.reshape(1, -1, r.shape[-1]) if one else r
-    sp = None
-    if spatials is not None:
-        sp = spatials[int(v_off[lo]):int(v_off[hi])]
-        sp = sp.reshape(1, -1, 5) if one else sp
-    return tuple(sl), sp
+def _answer_regions(answers, requests, out, spatials, spans, n_tokens, n_boxes, decode):
+    """`_answer_spans` for a `forward_regions_packed` call on `custom_prediction` argument tuples."""
+    return _answer_spans(answers, out, spatials, {i: (requests[i][4], requests[i][3]) for i in spans}, spans,
+                         list(accumulate([n + 1 for n in n_boxes], initial=0)),     # each image: the global row, then the boxes
+                         list(accumulate([n + 1 for n in n_tokens], initial=0)),    # each text: its tokens and the task token
+                         decode)
 
 
 def custom_prediction_packed(requests, bucket: int = 8, select: Optional[int] = None, max_boxes: int = 100, *, decode: str = "host"):
@@ -555,17 +534,7 @@ def custom_prediction_packed(requests, bucket: int = 8, select: Optional[int] = 
         out, spatials = model.forward_regions_packed(p["question"], p["segment_ids"], p["task_tokens"], p["box_features"], p["boxes"],
                                                      p["image_wh"], p["n_tokens"], p["n_boxes"], select=p["select"],
                                                      max_tokens=p["max_tokens"], max_boxes=p["max_boxes"])
-    if decode == "device":
-        v_off = np.concatenate([[0], np.cumsum([n + 1 for n in p["n_boxes"]])])   # packed regions: the global row, then the boxes
-        dec = _decode_device(out, spatials, {i: (requests[i][4], requests[i][3]) for i in p["spans"]}, p["spans"], v_off)
-        for i in p["spans"]:
-            answers[i] = dec[i]
-        return answers
-    for i, (lo, hi) in p["spans"].items():
-        task_id, infos = requests[i][4], requests[i][3]
-        sl, sp = split_region_outputs(out, spatials, p["n_tokens"], p["n_boxes"], lo, hi, task_id)
-        answers[i] = _decode(task_id, sl, sp, infos)
-    return answers
+    return _answer_regions(answers, requests, out, spatials, p["spans"], p["n_tokens"], p["n_boxes"], decode)
 
 
 def _per_image(x, counts):
@@ -616,19 +585,16 @@ def custom_prediction_detections(requests, bucket: int = 8, select: Optional[int
     if bucket < 1:
         raise ValueError("bucket must be >= 1")
     _check_decode(decode)
-    fixed_select = L.OUT_TASK_HEADS if select is None else int(select)
     max_rows = _max_rows()
     F = int(model._dims["v_feature_size"])
     answers = [None] * len(requests)
-    rows, spans, need, CF = [], {}, 0, None        # rows: (tokens, segments, task, detections, (w, h))
+    accepted, CF = [], None                        # rows: (tokens, segments, task, detections, (w, h))
     for i, (query, task, detections, infos, task_id) in enumerate(requests):
         try:
             _validate(task_id, infos)
             if len(detections) != len(infos):
                 raise ValueError(f"{len(detections)} detector outputs for {len(infos)} images")
-            tokens, segs = real_tokens(query)
-            if len(tokens) + 1 > max_rows:
-                raise ValueError(f"query of {len(tokens)} tokens: packed rows hold at most {max_rows - 1}")
+            tokens, segs = _region_text(query, None, max_rows)
             imgs, cf = [], CF                       # cf: the (C, F) this request's images must share with the call
             for (prop, sc, ft, scale), info in zip(detections, infos):
                 n = int(prop.shape[0])
@@ -643,25 +609,15 @@ def custom_prediction_detections(requests, bucket: int = 8, select: Optional[int
                     raise ValueError(f"im_scale {scale}: need a positive finite scale")
                 cf = shape
                 imgs.append(((prop, sc, ft, float(scale)), (float(info["image_width"]), float(info["image_height"]))))
-            t = int(np.array(task).reshape(-1)[0])
+            own = _region_rows(task_id, task, tokens, segs, imgs)
         except Exception as e:                      # noqa: BLE001 -- the request's answer, as callback()'s catch-all (worker.py:653-655)
             answers[i] = e
             continue
         CF = cf
-        if task_id in PAIR_TASKS and len(rows) % 2 == 1:
-            rows.append(None)                       # filler: the pair starts on an even row
-        rep = task_id in PAIR_TASKS + RETRIEVAL_TASKS
-        spans[i] = (len(rows), len(rows) + (len(imgs) if rep else 1))
-        for det, wh in (imgs if rep else imgs[:1]):
-            rows.append((tokens, segs, t, det, wh))
-        need |= TASK_OUTPUT[task_id]
-    if not spans:
+        accepted.append((i, task_id, own))
+    if not accepted:
         return answers
-    sel = fixed_select | need
-    target = -(-len(rows) // bucket) * bucket
-    if target % 2 == 1 and (sel & L.OUT_VIL_BINARY_PREDICTION):
-        target += 1                                 # the binary head needs an even number of rows
-    rows += [None] * (target - len(rows))
+    rows, spans, sel = _row_layout(accepted, bucket, select)
     filler = ([0], [0], 0, None, (1.0, 1.0))
     rows = [filler if r is None else r for r in rows]
     n_tokens = [len(r[0]) for r in rows]
@@ -682,17 +638,7 @@ def custom_prediction_detections(requests, bucket: int = 8, select: Optional[int
         out, spatials = model.forward_regions_packed(question, segment_ids, task_tokens, box_features, boxes, image_wh, n_tokens,
                                                      n_boxes, select=sel, max_tokens=max([MAX_LENGTH] + n_tokens),
                                                      max_boxes=max([int(max_boxes)] + n_boxes))
-    if decode == "device":
-        v_off = np.concatenate([[0], np.cumsum([n + 1 for n in n_boxes])])   # packed regions: the global row, then the boxes
-        dec = _decode_device(out, spatials, {i: (requests[i][4], requests[i][3]) for i in spans}, spans, v_off)
-        for i in spans:
-            answers[i] = dec[i]
-        return answers
-    for i, (lo, hi) in spans.items():
-        task_id, infos = requests[i][4], requests[i][3]
-        sl, sp = split_region_outputs(out, spatials, n_tokens, n_boxes, lo, hi, task_id)
-        answers[i] = _decode(task_id, sl, sp, infos)
-    return answers
+    return _answer_regions(answers, requests, out, spatials, spans, n_tokens, n_boxes, decode)
 
 
 def shape_result(task_id: str, answer, image_path: Sequence[str], image_names: Optional[List[str]] = None):
