@@ -548,6 +548,24 @@ PackedBatch pack_batch(const char* api, const Config& c, const std::vector<std::
     }
     return b;
 }
+// Detector box counts of a packed region call -> regions per image, V_i = n_boxes_i + 1 (the boxes and the global mean row), and
+// the region capacity (max_boxes + 1, or 0: the call's longest).  Checked in the caller's units before pack_batch sees V_i.
+struct BoxRows { std::vector<int32_t> v; int max_regions; };
+BoxRows box_rows(const char* api, int n, const int32_t* n_boxes, int max_boxes, int max_rows) {
+    if (max_boxes < 0) fail(VB200_ERR_INVALID, "%s: negative capacity max_boxes %d", api, max_boxes);
+    if (max_boxes > max_rows - 1)
+        fail(VB200_ERR_INVALID, "%s: capacity max_boxes %d above %d (V = boxes + 1 <= %d)", api, max_boxes, max_rows - 1, max_rows);
+    BoxRows r{{}, max_boxes > 0 ? max_boxes + 1 : 0};
+    for (int i = 0; i < n; ++i) {
+        const int k = n_boxes[i];
+        if (k < 1) fail(VB200_ERR_INVALID, "%s: image %d has n_boxes %d (must be >= 1)", api, i, k);
+        if (max_boxes > 0 && k > max_boxes)
+            fail(VB200_ERR_INVALID, "%s: image %d has n_boxes %d, above the capacity max_boxes %d", api, i, k, max_boxes);
+        if (k + 1 > max_rows) fail(VB200_ERR_INVALID, "%s: image %d has n_boxes %d (V = n_boxes + 1 must be <= %d)", api, i, k, max_rows);
+        r.v.push_back(k + 1);
+    }
+    return r;
+}
 
 struct Plan {
     int B = 0, Tin = 0, T = 0, V = 0;
@@ -1521,14 +1539,15 @@ struct vb200_engine {
         CUDA_CHECK(cudaGraphInstantiate(&pl.exec, pl.graph, 0));
     }
 
-    void forward_device(Plan& pl, const vb200_inputs& in, cudaStream_t st) {
-        const Config& c = cfg;
+    void check_inputs(const vb200_inputs& in) const {
         if (!in.question || !in.features || !in.spatials || !in.segment_ids || !in.input_mask || !in.image_mask ||
-            (c.task_tokens && !in.task_tokens))
+            (cfg.task_tokens && !in.task_tokens))
             fail(VB200_ERR_INVALID, "vb200_inputs has a NULL required pointer");
+    }
+    // the dense forward's input kernels, on inputs check_inputs has accepted
+    void embed_inputs(Plan& pl, const vb200_inputs& in, cudaStream_t st) {
         embed_text(pl, in.question, in.segment_ids, in.input_mask, in.task_tokens, pl.B * pl.T, st);
         pack_image(pl, in.features, in.spatials, in.image_mask, pl.B * pl.V, st);
-        run_plan(pl, st);
     }
     // The input kernels of every plan.  `rows`: the text / image rows of the call -- B x T / B x V on dense plans (padding from the
     // masks), the call's row totals on packed plans (no masks: every row is real; the rows up to the next 128-row GEMM tile are
@@ -1556,8 +1575,8 @@ struct vb200_engine {
         if (pl.exec) CUDA_CHECK(cudaGraphLaunch(pl.exec, st));
         else run_ops(pl, st);
     }
-    // worker.py:422-455 on the device: detector output -> operand rows / masks, then the same plan as forward_device
-    void forward_regions(Plan& pl, const vb200_region_inputs& in, cudaStream_t st) {
+    // worker.py:422-455 on the device: detector output -> operand rows / masks for the same plan as the dense forward
+    void embed_regions(Plan& pl, const vb200_region_inputs& in, cudaStream_t st) {
         const Config& c = cfg;
         if (!in.question || !in.segment_ids || !in.input_mask || (c.task_tokens && !in.task_tokens) || !in.box_features || !in.boxes ||
             !in.image_wh)
@@ -1565,21 +1584,10 @@ struct vb200_engine {
         embed_text(pl, in.question, in.segment_ids, in.input_mask, in.task_tokens, pl.B * pl.T, st);
         CUDA_CHECK(vb::launch_region_pack(in.box_features, in.boxes, in.image_wh, in.num_boxes, pl.img_a, pl.mask_v, in.spatials_out,
                                           pl.B, pl.V - 1, c.v_feat, pl.kp, opt.act_fp16, x3 ? 1 : 0, st));
-        run_plan(pl, st);
     }
     // ---- packed batches (run_packed has staged the call's d_meta ahead of these, in stream order)
-    void forward_packed(Plan& pl, const vb200_packed_inputs& in, const PackedBatch& b, cudaStream_t st) {
-        embed_text(pl, in.question, in.segment_ids, nullptr, in.task_tokens, b.rows_t(), st);
-        pack_image(pl, in.features, in.spatials, nullptr, b.rows_v(), st);
-        run_plan(pl, st);
-    }
-    // Packed detector output on a PACKED plan: the region-pack kernel writes every image's mean row and boxes at the plan's image
-    // offsets (the same rows forward_regions writes for that image alone), then the packed forward runs as above
-    void forward_regions_packed(Plan& pl, const vb200_packed_region_inputs& in, const PackedBatch& b, cudaStream_t st) {
-        embed_text(pl, in.question, in.segment_ids, nullptr, in.task_tokens, b.rows_t(), st);
-        pack_regions_packed(pl, in.box_features, in.boxes, in.image_wh, in.spatials_out, b.rows_v(), st);
-        run_plan(pl, st);
-    }
+    // Packed detector output: the region-pack kernel writes every image's mean row and boxes at the plan's image offsets (the same
+    // rows embed_regions writes for that image alone)
     void pack_regions_packed(Plan& pl, const float* box_feats, const float* boxes, const float* image_wh, float* spatials_out, int rows,
                              cudaStream_t st) {
         CUDA_CHECK(vb::launch_region_pack(box_feats, boxes, image_wh, nullptr, pl.img_a, pl.mask_v, spatials_out, pl.B, 0, cfg.v_feat,
@@ -1587,7 +1595,7 @@ struct vb200_engine {
         zero_tail(pl.img_a, rows, pl.B * pl.V, pl.kp, st);
     }
     // packed pair suffix: every pair's rows are gathered from the packed caption / image states into the plan's packed buffers
-    void forward_cached_packed(Plan& pl, const vb200_packed_pairs& in, const PackedBatch& b, cudaStream_t st) {
+    void gather_packed_state(Plan& pl, const vb200_packed_pairs& in, const PackedBatch& b, cudaStream_t st) {
         const Config& c = cfg;
         const vb::PackedStateCopy text{pl.offs_t(), pl.src_t(), in.text_f32, in.text_16, pl.t_f32[0], pl.t_b16[0], c.hidden / 4, c.hidden / 8};
         const vb::PackedStateCopy image{pl.offs_v(), pl.src_v(), in.image_f32, in.image_16, pl.v_f32[0], pl.v_b16[0], c.v_hidden / 4,
@@ -1595,13 +1603,47 @@ struct vb200_engine {
         CUDA_CHECK(vb::launch_gather_packed_state(text, image, pl.B, st));
         zero_tail(pl.t_b16[0], b.rows_t(), pl.B * pl.T, c.hidden, st);
         zero_tail(pl.v_b16[0], b.rows_v(), pl.B * pl.V, c.v_hidden, st);
+    }
+    // ---- retrieval reuse (PlanMode): per-caption / per-image prefixes and the pair suffix.  A prefix leaves its stream's state after
+    // the layers ahead of the first connection layer in the caller's buffers: B x T / B x V rows with the mask on dense plans, the
+    // call's rows back to back and no mask (mask null) on packed plans
+    struct PrefixState { float* f32; void* b16; float* mask; };
+    void copy_state(const Plan& pl, bool text, size_t rows, const PrefixState& to, cudaStream_t st) {
+        const size_t H = text ? cfg.hidden : cfg.v_hidden, S = x3 ? 3 : 1;
+        const float* f32 = text ? pl.t_f32[pl.t_cur] : pl.v_f32[pl.v_cur];
+        const bf16* b16 = text ? pl.t_b16[pl.t_cur] : pl.v_b16[pl.v_cur];
+        CUDA_CHECK(cudaMemcpyAsync(to.f32, f32, rows * H * 4, cudaMemcpyDeviceToDevice, st));
+        CUDA_CHECK(cudaMemcpyAsync(to.b16, b16, rows * H * S * 2, cudaMemcpyDeviceToDevice, st));
+        if (to.mask != nullptr) CUDA_CHECK(cudaMemcpyAsync(to.mask, text ? pl.mask_t : pl.mask_v, rows * 4, cudaMemcpyDeviceToDevice, st));
+    }
+    void gather_state(Plan& pl, const int32_t* t_idx, int n_text, const float* t_f32, const void* t_16, const float* t_mask,
+                      const int32_t* v_idx, int n_img, const float* v_f32, const void* v_16, const float* v_mask, cudaStream_t st) {
+        const Config& c = cfg;
+        if (!t_idx || !t_f32 || !t_16 || !t_mask || !v_idx || !v_f32 || !v_16 || !v_mask) fail(VB200_ERR_INVALID, "vb200_forward_cached: NULL pointer");
+        const int S = x3 ? 3 : 1;
+        CUDA_CHECK(vb::launch_gather_state(t_idx, n_text, t_f32, t_16, t_mask, pl.t_f32[0], pl.t_b16[0], pl.mask_t, pl.B, pl.T,
+                                           c.hidden, c.hidden * S, st));
+        CUDA_CHECK(vb::launch_gather_state(v_idx, n_img, v_f32, v_16, v_mask, pl.v_f32[0], pl.v_b16[0], pl.mask_v, pl.B, pl.V,
+                                           c.v_hidden, c.v_hidden * S, st));
+    }
+    // What every dense entry point shares once it has checked its own inputs: the packed-map rejection, the call's plan, its input
+    // kernels (`input`), the plan and then the forward's outputs (out != null, copied with `kind`) or the prefix's state (`state`).
+    void run_dense(const char* api, int B, int Tin, int V, uint32_t select, int slot, int mode, const vb200_outputs* out,
+                   const PrefixState& state, cudaMemcpyKind kind, void* cuda_stream, const std::function<void(Plan&, cudaStream_t)>& input) {
+        reject_packed_attention(select, api);
+        CUDA_CHECK(cudaSetDevice(opt.device));
+        Plan& pl = *get_plan(B, Tin, V, select & VB200_OUT_ALL, slot, mode, (select & VB200_OUT_ATTENTION) != 0);
+        const cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+        input(pl, st);
         run_plan(pl, st);
+        if (out != nullptr) copy_outputs(pl, *out, st, kind);
+        else copy_state(pl, mode == TEXT_PREFIX, mode == TEXT_PREFIX ? pl.B * pl.T : pl.B * pl.V, state, st);
     }
     // What every packed entry point shares once it has checked its own inputs: the engine-wide rejections, the call's rows
-    // (pack_batch), its plan, the d_meta staged ahead of `run` (the call's input kernels and the plan) and, for the forwards
-    // (out != null), the outputs at the call's row totals.
+    // (pack_batch), its plan, the d_meta staged ahead of `input` (the call's input kernels), the plan and then, for the forwards
+    // (out != null), the outputs at the call's row totals or, for the prefixes, the state of the call's rows.
     void run_packed(const char* api, int mode, const PackedLengths& len, uint32_t select, int slot, const vb200_outputs* out,
-                    void* cuda_stream, const std::function<void(Plan&, const PackedBatch&, cudaStream_t)>& run) {
+                    const PrefixState& state, void* cuda_stream, const std::function<void(Plan&, const PackedBatch&, cudaStream_t)>& input) {
         if (select & VB200_OUT_ATTENTION)
             fail(VB200_ERR_INVALID, "%s: the attention-probability output (VB200_OUT_ATTENTION) is not supported", api);
         if (mode != PACKED) reject_packed_attention(select, api);
@@ -1614,8 +1656,10 @@ struct vb200_engine {
         Plan& pl = *get_plan(len.B, b.Tin, b.V, select & VB200_OUT_ALL, slot, mode, maps);
         const cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
         stage_meta(pl, b.meta, st);
-        run(pl, b, st);
+        input(pl, b, st);
+        run_plan(pl, st);
         if (out != nullptr) copy_outputs(pl, *out, st, cudaMemcpyDeviceToDevice, b.rows_t(), b.rows_v());
+        else copy_state(pl, mode == PACKED_TEXT_PREFIX, mode == PACKED_TEXT_PREFIX ? b.rows_t() : b.rows_v(), state, st);
     }
     // meta (host, in the plan's d_meta layout) -> d_meta, in stream order ahead of the plan's kernels
     void stage_meta(Plan& pl, const std::vector<int>& meta, cudaStream_t st) {
@@ -1623,46 +1667,6 @@ struct vb200_engine {
         memcpy(pl.h_meta, meta.data(), meta.size() * sizeof(int));
         CUDA_CHECK(cudaMemcpyAsync(pl.d_meta, pl.h_meta, meta.size() * sizeof(int), cudaMemcpyHostToDevice, st));
         CUDA_CHECK(cudaEventRecord(pl.meta_copied, st));
-    }
-    // ---- retrieval reuse (PlanMode): per-caption / per-image prefixes and the pair suffix.  A prefix leaves its stream's state after
-    // the layers ahead of the first connection layer in the caller's buffers: `rows` rows, B x T / B x V with the mask on dense
-    // plans, the call's rows back to back and no mask (st_mask null) on packed plans
-    void encode_text(Plan& pl, const int64_t* q, const int64_t* seg, const int64_t* im, const int64_t* tk, int rows, float* st_f32,
-                     void* st_16, float* st_mask, cudaStream_t st) {
-        embed_text(pl, q, seg, im, tk, rows, st);
-        run_plan(pl, st);
-        copy_state(pl.t_f32[pl.t_cur], pl.t_b16[pl.t_cur], pl.mask_t, rows, cfg.hidden, st_f32, st_16, st_mask, st);
-    }
-    void encode_image(Plan& pl, const float* feats, const float* loc, const uint8_t* vmask, int rows, float* st_f32, void* st_16,
-                      float* st_mask, cudaStream_t st) {
-        pack_image(pl, feats, loc, vmask, rows, st);
-        run_plan(pl, st);
-        copy_state(pl.v_f32[pl.v_cur], pl.v_b16[pl.v_cur], pl.mask_v, rows, cfg.v_hidden, st_f32, st_16, st_mask, st);
-    }
-    // packed image prefix from detector output: the region pack of forward_regions_packed in front of the image prefix
-    void encode_regions(Plan& pl, const float* box_feats, const float* boxes, const float* image_wh, int rows, float* st_f32, void* st_16,
-                        cudaStream_t st) {
-        pack_regions_packed(pl, box_feats, boxes, image_wh, nullptr, rows, st);
-        run_plan(pl, st);
-        copy_state(pl.v_f32[pl.v_cur], pl.v_b16[pl.v_cur], pl.mask_v, rows, cfg.v_hidden, st_f32, st_16, nullptr, st);
-    }
-    void copy_state(const float* f32, const bf16* b16, const float* mask, size_t rows, size_t H, float* st_f32, void* st_16,
-                    float* st_mask, cudaStream_t st) {
-        const size_t S = x3 ? 3 : 1;
-        CUDA_CHECK(cudaMemcpyAsync(st_f32, f32, rows * H * 4, cudaMemcpyDeviceToDevice, st));
-        CUDA_CHECK(cudaMemcpyAsync(st_16, b16, rows * H * S * 2, cudaMemcpyDeviceToDevice, st));
-        if (st_mask != nullptr) CUDA_CHECK(cudaMemcpyAsync(st_mask, mask, rows * 4, cudaMemcpyDeviceToDevice, st));
-    }
-    void forward_cached(Plan& pl, const int32_t* t_idx, int n_text, const float* t_f32, const void* t_16, const float* t_mask,
-                        const int32_t* v_idx, int n_img, const float* v_f32, const void* v_16, const float* v_mask, cudaStream_t st) {
-        const Config& c = cfg;
-        if (!t_idx || !t_f32 || !t_16 || !t_mask || !v_idx || !v_f32 || !v_16 || !v_mask) fail(VB200_ERR_INVALID, "vb200_forward_cached: NULL pointer");
-        const int S = x3 ? 3 : 1;
-        CUDA_CHECK(vb::launch_gather_state(t_idx, n_text, t_f32, t_16, t_mask, pl.t_f32[0], pl.t_b16[0], pl.mask_t, pl.B, pl.T,
-                                           c.hidden, c.hidden * S, st));
-        CUDA_CHECK(vb::launch_gather_state(v_idx, n_img, v_f32, v_16, v_mask, pl.v_f32[0], pl.v_b16[0], pl.mask_v, pl.B, pl.V,
-                                           c.v_hidden, c.v_hidden * S, st));
-        run_plan(pl, st);
     }
     // ---- answer decode: every descriptor is resolved and bounds-checked before anything is enqueued
     std::vector<vb::DecodeDesc> decode_descs(const char* api, const vb200_decode_msg* msgs, int n, const vb200_outputs* out, int batch,
@@ -1989,13 +1993,11 @@ int vb200_forward_slot(vb200_handle h, const vb200_inputs* in, const vb200_outpu
     if (h == nullptr) return VB200_ERR_INVALID;
     return guard(h, [&] {
         if (in == nullptr || out == nullptr) fail(VB200_ERR_INVALID, "inputs/outputs struct is NULL");
-        reject_packed_attention(select, "vb200_forward");
-        CUDA_CHECK(cudaSetDevice(h->opt.device));
-        Plan* pl = h->get_plan(in->batch, in->n_tokens, in->n_regions, select & VB200_OUT_ALL, slot, vb200_engine::FULL,
-                               (select & VB200_OUT_ATTENTION) != 0);
-        cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-        h->forward_device(*pl, *in, st);
-        h->copy_outputs(*pl, *out, st, cudaMemcpyDeviceToDevice);
+        h->run_dense("vb200_forward", in->batch, in->n_tokens, in->n_regions, select, slot, vb200_engine::FULL, out, {},
+                     cudaMemcpyDeviceToDevice, cuda_stream, [&](Plan& pl, cudaStream_t st) {
+                         h->check_inputs(*in);
+                         h->embed_inputs(pl, *in, st);
+                     });
     });
 }
 
@@ -2008,8 +2010,11 @@ int vb200_forward_packed(vb200_handle h, const vb200_packed_inputs* in, const vb
             (h->cfg.task_tokens && !in->task_tokens))
             fail(VB200_ERR_INVALID, "vb200_packed_inputs has a NULL required pointer");
         h->run_packed("vb200_forward_packed", vb200_engine::PACKED,
-                      {"sample", in->batch, in->n_tokens, in->max_tokens, in->n_regions, in->max_regions}, select, slot, out, cuda_stream,
-                      [&](Plan& pl, const PackedBatch& b, cudaStream_t st) { h->forward_packed(pl, *in, b, st); });
+                      {"sample", in->batch, in->n_tokens, in->max_tokens, in->n_regions, in->max_regions}, select, slot, out, {},
+                      cuda_stream, [&](Plan& pl, const PackedBatch& b, cudaStream_t st) {
+                          h->embed_text(pl, in->question, in->segment_ids, nullptr, in->task_tokens, b.rows_t(), st);
+                          h->pack_image(pl, in->features, in->spatials, nullptr, b.rows_v(), st);
+                      });
     });
 }
 
@@ -2023,26 +2028,16 @@ int vb200_forward_regions_packed(vb200_handle h, const vb200_packed_region_input
         if (!in->n_tokens || !in->n_boxes || !in->question || !in->segment_ids || !in->box_features || !in->boxes || !in->image_wh ||
             (task && !in->task_tokens))
             fail(VB200_ERR_INVALID, "vb200_packed_region_inputs has a NULL required pointer");
-        if (in->max_boxes < 0) fail(VB200_ERR_INVALID, "%s: negative capacity max_boxes %d", api, in->max_boxes);
-        const int max_rows = h->max_rows;
-        if (in->max_boxes > max_rows - 1)
-            fail(VB200_ERR_INVALID, "%s: capacity max_boxes %d above %d (V = boxes + 1 <= %d)", api, in->max_boxes, max_rows - 1, max_rows);
-        // regions per image = boxes + the global mean row; these checks name the caller's fields before pack_batch sees V_i / T_i
-        std::vector<int32_t> nv;
-        for (int i = 0; i < in->batch; ++i) {
-            const int n = in->n_boxes[i], t = in->n_tokens[i];
-            if (n < 1) fail(VB200_ERR_INVALID, "%s: image %d has n_boxes %d (must be >= 1)", api, i, n);
-            if (in->max_boxes > 0 && n > in->max_boxes)
-                fail(VB200_ERR_INVALID, "%s: image %d has n_boxes %d, above the capacity max_boxes %d", api, i, n, in->max_boxes);
-            if (n + 1 > max_rows)
-                fail(VB200_ERR_INVALID, "%s: image %d has n_boxes %d (V = n_boxes + 1 must be <= %d)", api, i, n, max_rows);
-            if (t + task > max_rows)
-                fail(VB200_ERR_INVALID, "%s: image %d has n_tokens %d (T = n_tokens + 1 must be <= %d)", api, i, t, max_rows);
-            nv.push_back(n + 1);
-        }
-        h->run_packed(api, vb200_engine::PACKED,
-                      {"image", in->batch, in->n_tokens, in->max_tokens, nv.data(), in->max_boxes > 0 ? in->max_boxes + 1 : 0}, select, slot,
-                      out, cuda_stream, [&](Plan& pl, const PackedBatch& b, cudaStream_t st) { h->forward_regions_packed(pl, *in, b, st); });
+        const BoxRows v = box_rows(api, in->batch, in->n_boxes, in->max_boxes, h->max_rows);
+        // named in the caller's field before pack_batch sees T_i
+        for (int i = 0; i < in->batch; ++i)
+            if (in->n_tokens[i] + task > h->max_rows)
+                fail(VB200_ERR_INVALID, "%s: image %d has n_tokens %d (T = n_tokens + 1 must be <= %d)", api, i, in->n_tokens[i], h->max_rows);
+        h->run_packed(api, vb200_engine::PACKED, {"image", in->batch, in->n_tokens, in->max_tokens, v.v.data(), v.max_regions}, select,
+                      slot, out, {}, cuda_stream, [&](Plan& pl, const PackedBatch& b, cudaStream_t st) {
+                          h->embed_text(pl, in->question, in->segment_ids, nullptr, in->task_tokens, b.rows_t(), st);
+                          h->pack_regions_packed(pl, in->box_features, in->boxes, in->image_wh, in->spatials_out, b.rows_v(), st);
+                      });
     });
 }
 
@@ -2052,13 +2047,8 @@ int vb200_forward_regions(vb200_handle h, const vb200_region_inputs* in, const v
     return guard(h, [&] {
         if (in == nullptr || out == nullptr) fail(VB200_ERR_INVALID, "inputs/outputs struct is NULL");
         if (in->n_boxes < 1) fail(VB200_ERR_INVALID, "n_boxes must be positive");
-        reject_packed_attention(select, "vb200_forward_regions");
-        CUDA_CHECK(cudaSetDevice(h->opt.device));
-        Plan* pl = h->get_plan(in->batch, in->n_tokens, in->n_boxes + 1, select & VB200_OUT_ALL, slot, vb200_engine::FULL,
-                               (select & VB200_OUT_ATTENTION) != 0);
-        cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-        h->forward_regions(*pl, *in, st);
-        h->copy_outputs(*pl, *out, st, cudaMemcpyDeviceToDevice);
+        h->run_dense("vb200_forward_regions", in->batch, in->n_tokens, in->n_boxes + 1, select, slot, vb200_engine::FULL, out, {},
+                     cudaMemcpyDeviceToDevice, cuda_stream, [&](Plan& pl, cudaStream_t st) { h->embed_regions(pl, *in, st); });
     });
 }
 
@@ -2067,12 +2057,12 @@ int vb200_encode_text(vb200_handle h, int32_t n, int32_t n_tokens, const int64_t
                       void* cuda_stream) {
     if (h == nullptr) return VB200_ERR_INVALID;
     return guard(h, [&] {
-        CUDA_CHECK(cudaSetDevice(h->opt.device));
         if (!question || !segment_ids || !input_mask || (h->cfg.task_tokens && !task_tokens) || !state_f32 || !state_16 || !state_mask)
             fail(VB200_ERR_INVALID, "vb200_encode_text: NULL pointer");
-        Plan& pl = *h->get_plan(n, n_tokens, 1, 0, 0, vb200_engine::TEXT_PREFIX);
-        h->encode_text(pl, question, segment_ids, input_mask, task_tokens, pl.B * pl.T, state_f32, state_16, state_mask,
-                       static_cast<cudaStream_t>(cuda_stream));
+        h->run_dense("vb200_encode_text", n, n_tokens, 1, 0, 0, vb200_engine::TEXT_PREFIX, nullptr, {state_f32, state_16, state_mask},
+                     cudaMemcpyDeviceToDevice, cuda_stream, [&](Plan& pl, cudaStream_t st) {
+                         h->embed_text(pl, question, segment_ids, input_mask, task_tokens, pl.B * pl.T, st);
+                     });
     });
 }
 
@@ -2080,12 +2070,12 @@ int vb200_encode_image(vb200_handle h, int32_t n, int32_t n_regions, const float
                        const uint8_t* image_mask, float* state_f32, void* state_16, float* state_mask, void* cuda_stream) {
     if (h == nullptr) return VB200_ERR_INVALID;
     return guard(h, [&] {
-        CUDA_CHECK(cudaSetDevice(h->opt.device));
         if (!features || !spatials || !image_mask || !state_f32 || !state_16 || !state_mask)
             fail(VB200_ERR_INVALID, "vb200_encode_image: NULL pointer");
-        Plan& pl = *h->get_plan(n, 1, n_regions, 0, 0, vb200_engine::IMAGE_PREFIX);
-        h->encode_image(pl, features, spatials, image_mask, pl.B * pl.V, state_f32, state_16, state_mask,
-                        static_cast<cudaStream_t>(cuda_stream));
+        h->run_dense("vb200_encode_image", n, 1, n_regions, 0, 0, vb200_engine::IMAGE_PREFIX, nullptr, {state_f32, state_16, state_mask},
+                     cudaMemcpyDeviceToDevice, cuda_stream, [&](Plan& pl, cudaStream_t st) {
+                         h->pack_image(pl, features, spatials, image_mask, pl.B * pl.V, st);
+                     });
     });
 }
 
@@ -2097,14 +2087,11 @@ int vb200_forward_cached(vb200_handle h, int32_t batch, int32_t n_tokens, int32_
     return guard(h, [&] {
         if (out == nullptr) fail(VB200_ERR_INVALID, "outputs struct is NULL");
         if (n_text < 1 || n_image < 1) fail(VB200_ERR_INVALID, "cached state counts must be positive");
-        reject_packed_attention(select, "vb200_forward_cached");
-        CUDA_CHECK(cudaSetDevice(h->opt.device));
-        Plan* pl = h->get_plan(batch, n_tokens, n_regions, select & VB200_OUT_ALL, slot, vb200_engine::SUFFIX,
-                               (select & VB200_OUT_ATTENTION) != 0);
-        cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-        h->forward_cached(*pl, text_index, n_text, text_f32, text_16, text_mask, image_index, n_image, image_f32, image_16,
-                          image_mask, st);
-        h->copy_outputs(*pl, *out, st, cudaMemcpyDeviceToDevice);
+        h->run_dense("vb200_forward_cached", batch, n_tokens, n_regions, select, slot, vb200_engine::SUFFIX, out, {},
+                     cudaMemcpyDeviceToDevice, cuda_stream, [&](Plan& pl, cudaStream_t st) {
+                         h->gather_state(pl, text_index, n_text, text_f32, text_16, text_mask, image_index, n_image, image_f32, image_16,
+                                         image_mask, st);
+                     });
     });
 }
 
@@ -2115,9 +2102,9 @@ int vb200_encode_text_packed(vb200_handle h, int32_t n, int32_t max_tokens, cons
         const char* api = "vb200_encode_text_packed";
         if (!n_tokens || !question || !segment_ids || (h->cfg.task_tokens && !task_tokens) || !state_f32 || !state_16)
             fail(VB200_ERR_INVALID, "%s: NULL pointer", api);
-        h->run_packed(api, vb200_engine::PACKED_TEXT_PREFIX, {"caption", n, n_tokens, max_tokens, nullptr, 0}, 0, 0, nullptr, cuda_stream,
-                      [&](Plan& pl, const PackedBatch& b, cudaStream_t st) {
-                          h->encode_text(pl, question, segment_ids, nullptr, task_tokens, b.rows_t(), state_f32, state_16, nullptr, st);
+        h->run_packed(api, vb200_engine::PACKED_TEXT_PREFIX, {"caption", n, n_tokens, max_tokens, nullptr, 0}, 0, 0, nullptr,
+                      {state_f32, state_16, nullptr}, cuda_stream, [&](Plan& pl, const PackedBatch& b, cudaStream_t st) {
+                          h->embed_text(pl, question, segment_ids, nullptr, task_tokens, b.rows_t(), st);
                       });
     });
 }
@@ -2128,9 +2115,9 @@ int vb200_encode_image_packed(vb200_handle h, int32_t n, int32_t max_regions, co
     return guard(h, [&] {
         const char* api = "vb200_encode_image_packed";
         if (!n_regions || !features || !spatials || !state_f32 || !state_16) fail(VB200_ERR_INVALID, "%s: NULL pointer", api);
-        h->run_packed(api, vb200_engine::PACKED_IMAGE_PREFIX, {"image", n, nullptr, 0, n_regions, max_regions}, 0, 0, nullptr, cuda_stream,
-                      [&](Plan& pl, const PackedBatch& b, cudaStream_t st) {
-                          h->encode_image(pl, features, spatials, nullptr, b.rows_v(), state_f32, state_16, nullptr, st);
+        h->run_packed(api, vb200_engine::PACKED_IMAGE_PREFIX, {"image", n, nullptr, 0, n_regions, max_regions}, 0, 0, nullptr,
+                      {state_f32, state_16, nullptr}, cuda_stream, [&](Plan& pl, const PackedBatch& b, cudaStream_t st) {
+                          h->pack_image(pl, features, spatials, nullptr, b.rows_v(), st);
                       });
     });
 }
@@ -2141,26 +2128,12 @@ int vb200_encode_regions_packed(vb200_handle h, int32_t n, int32_t max_boxes, co
     return guard(h, [&] {
         const char* api = "vb200_encode_regions_packed";
         if (!n_boxes || !box_features || !boxes || !image_wh || !state_f32 || !state_16) fail(VB200_ERR_INVALID, "%s: NULL pointer", api);
-        if (max_boxes < 0) fail(VB200_ERR_INVALID, "%s: negative capacity max_boxes %d", api, max_boxes);
-        const int max_rows = h->max_rows;
-        if (max_boxes > max_rows - 1)
-            fail(VB200_ERR_INVALID, "%s: capacity max_boxes %d above %d (V = boxes + 1 <= %d)", api, max_boxes, max_rows - 1, max_rows);
-        // regions per image = boxes + the global mean row, checked in the caller's units before pack_batch sees V_i
-        std::vector<int32_t> nv;
-        for (int i = 0; i < n; ++i) {
-            const int k = n_boxes[i];
-            if (k < 1) fail(VB200_ERR_INVALID, "%s: image %d has n_boxes %d (must be >= 1)", api, i, k);
-            if (max_boxes > 0 && k > max_boxes)
-                fail(VB200_ERR_INVALID, "%s: image %d has n_boxes %d, above the capacity max_boxes %d", api, i, k, max_boxes);
-            if (k + 1 > max_rows)
-                fail(VB200_ERR_INVALID, "%s: image %d has n_boxes %d (V = n_boxes + 1 must be <= %d)", api, i, k, max_rows);
-            nv.push_back(k + 1);
-        }
+        const BoxRows v = box_rows(api, n, n_boxes, max_boxes, h->max_rows);
         // the PACKED_IMAGE_PREFIX plan of vb200_encode_image_packed at max_regions = max_boxes + 1, fed by the region pack of
         // vb200_forward_regions_packed: each image's rows are the rows that forward writes for it
-        h->run_packed(api, vb200_engine::PACKED_IMAGE_PREFIX, {"image", n, nullptr, 0, nv.data(), max_boxes > 0 ? max_boxes + 1 : 0}, 0, 0,
-                      nullptr, cuda_stream, [&](Plan& pl, const PackedBatch& b, cudaStream_t st) {
-                          h->encode_regions(pl, box_features, boxes, image_wh, b.rows_v(), state_f32, state_16, st);
+        h->run_packed(api, vb200_engine::PACKED_IMAGE_PREFIX, {"image", n, nullptr, 0, v.v.data(), v.max_regions}, 0, 0, nullptr,
+                      {state_f32, state_16, nullptr}, cuda_stream, [&](Plan& pl, const PackedBatch& b, cudaStream_t st) {
+                          h->pack_regions_packed(pl, box_features, boxes, image_wh, nullptr, b.rows_v(), st);
                       });
     });
 }
@@ -2197,7 +2170,7 @@ int vb200_forward_cached_packed(vb200_handle h, const vb200_packed_pairs* in, co
         }
         h->run_packed(api, vb200_engine::PACKED_SUFFIX,
                       {"pair", in->batch, tin.data(), in->max_tokens, nv.data(), in->max_regions, src_t.data(), src_v.data()}, select, slot,
-                      out, cuda_stream, [&](Plan& pl, const PackedBatch& b, cudaStream_t st) { h->forward_cached_packed(pl, *in, b, st); });
+                      out, {}, cuda_stream, [&](Plan& pl, const PackedBatch& b, cudaStream_t st) { h->gather_packed_state(pl, *in, b, st); });
     });
 }
 
@@ -2293,34 +2266,29 @@ int vb200_forward_host_slot(vb200_handle h, const vb200_inputs* in, const vb200_
     if (h == nullptr) return VB200_ERR_INVALID;
     return guard(h, [&] {
         if (in == nullptr || out == nullptr) fail(VB200_ERR_INVALID, "inputs/outputs struct is NULL");
-        reject_packed_attention(select, "vb200_forward_host");
-        CUDA_CHECK(cudaSetDevice(h->opt.device));
-        Plan* pl = h->get_plan(in->batch, in->n_tokens, in->n_regions, select & VB200_OUT_ALL, slot, vb200_engine::FULL,
-                               (select & VB200_OUT_ATTENTION) != 0);
-        cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-        const size_t B = pl->B, Tin = pl->Tin, V = pl->V, F = h->cfg.v_feat;
-        if (pl->d_q == nullptr) {
-            pl->d_q = pl->mem.alloc_n<int64_t>(B * Tin); pl->d_seg = pl->mem.alloc_n<int64_t>(B * Tin);
-            pl->d_mask = pl->mem.alloc_n<int64_t>(B * Tin); pl->d_task = pl->mem.alloc_n<int64_t>(B);
-            pl->d_feat = pl->mem.alloc_n<float>(B * V * F); pl->d_loc = pl->mem.alloc_n<float>(B * V * 5);
-            pl->d_imask = pl->mem.alloc_n<uint8_t>(B * V);
-        }
-        if (!in->question || !in->features || !in->spatials || !in->segment_ids || !in->input_mask || !in->image_mask ||
-            (h->cfg.task_tokens && !in->task_tokens))
-            fail(VB200_ERR_INVALID, "vb200_inputs has a NULL required pointer");
-        CUDA_CHECK(cudaMemcpyAsync(pl->d_q, in->question, B * Tin * 8, cudaMemcpyHostToDevice, st));
-        CUDA_CHECK(cudaMemcpyAsync(pl->d_seg, in->segment_ids, B * Tin * 8, cudaMemcpyHostToDevice, st));
-        CUDA_CHECK(cudaMemcpyAsync(pl->d_mask, in->input_mask, B * Tin * 8, cudaMemcpyHostToDevice, st));
-        if (in->task_tokens) CUDA_CHECK(cudaMemcpyAsync(pl->d_task, in->task_tokens, B * 8, cudaMemcpyHostToDevice, st));
-        CUDA_CHECK(cudaMemcpyAsync(pl->d_feat, in->features, B * V * F * 4, cudaMemcpyHostToDevice, st));
-        CUDA_CHECK(cudaMemcpyAsync(pl->d_loc, in->spatials, B * V * 5 * 4, cudaMemcpyHostToDevice, st));
-        CUDA_CHECK(cudaMemcpyAsync(pl->d_imask, in->image_mask, B * V, cudaMemcpyHostToDevice, st));
-        vb200_inputs dev = *in;
-        dev.question = pl->d_q; dev.segment_ids = pl->d_seg; dev.input_mask = pl->d_mask; dev.task_tokens = pl->d_task;
-        dev.features = pl->d_feat; dev.spatials = pl->d_loc; dev.image_mask = pl->d_imask; dev.co_attention_mask = nullptr;
-        h->forward_device(*pl, dev, st);
-        h->copy_outputs(*pl, *out, st, cudaMemcpyDeviceToHost);
-        if (synchronize) CUDA_CHECK(cudaStreamSynchronize(st));
+        h->run_dense("vb200_forward_host", in->batch, in->n_tokens, in->n_regions, select, slot, vb200_engine::FULL, out, {},
+                     cudaMemcpyDeviceToHost, cuda_stream, [&](Plan& pl, cudaStream_t st) {
+            const size_t B = pl.B, Tin = pl.Tin, V = pl.V, F = h->cfg.v_feat;
+            if (pl.d_q == nullptr) {
+                pl.d_q = pl.mem.alloc_n<int64_t>(B * Tin); pl.d_seg = pl.mem.alloc_n<int64_t>(B * Tin);
+                pl.d_mask = pl.mem.alloc_n<int64_t>(B * Tin); pl.d_task = pl.mem.alloc_n<int64_t>(B);
+                pl.d_feat = pl.mem.alloc_n<float>(B * V * F); pl.d_loc = pl.mem.alloc_n<float>(B * V * 5);
+                pl.d_imask = pl.mem.alloc_n<uint8_t>(B * V);
+            }
+            h->check_inputs(*in);
+            CUDA_CHECK(cudaMemcpyAsync(pl.d_q, in->question, B * Tin * 8, cudaMemcpyHostToDevice, st));
+            CUDA_CHECK(cudaMemcpyAsync(pl.d_seg, in->segment_ids, B * Tin * 8, cudaMemcpyHostToDevice, st));
+            CUDA_CHECK(cudaMemcpyAsync(pl.d_mask, in->input_mask, B * Tin * 8, cudaMemcpyHostToDevice, st));
+            if (in->task_tokens) CUDA_CHECK(cudaMemcpyAsync(pl.d_task, in->task_tokens, B * 8, cudaMemcpyHostToDevice, st));
+            CUDA_CHECK(cudaMemcpyAsync(pl.d_feat, in->features, B * V * F * 4, cudaMemcpyHostToDevice, st));
+            CUDA_CHECK(cudaMemcpyAsync(pl.d_loc, in->spatials, B * V * 5 * 4, cudaMemcpyHostToDevice, st));
+            CUDA_CHECK(cudaMemcpyAsync(pl.d_imask, in->image_mask, B * V, cudaMemcpyHostToDevice, st));
+            vb200_inputs dev = *in;
+            dev.question = pl.d_q; dev.segment_ids = pl.d_seg; dev.input_mask = pl.d_mask; dev.task_tokens = pl.d_task;
+            dev.features = pl.d_feat; dev.spatials = pl.d_loc; dev.image_mask = pl.d_imask; dev.co_attention_mask = nullptr;
+            h->embed_inputs(pl, dev, st);
+        });
+        if (synchronize) CUDA_CHECK(cudaStreamSynchronize(static_cast<cudaStream_t>(cuda_stream)));
     });
 }
 

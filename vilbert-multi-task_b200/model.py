@@ -46,6 +46,27 @@ def _host_ints(x):
     return [int(v) for v in (x.tolist() if torch.is_tensor(x) else x)]
 
 
+def _int32s(values):
+    """Host ints as the ``int32_t*`` of a C ABI length array (the array lives as long as the returned pointer)."""
+    return C.cast((C.c_int32 * max(len(values), 1))(*values), C.c_void_p)
+
+
+def _to_device(t, dtype, device):
+    """``t`` as a contiguous ``dtype`` tensor on ``device``; a tensor that already is one is passed through without a copy."""
+    if not torch.is_tensor(t):
+        t = torch.as_tensor(t)
+    if t.dtype != dtype:
+        t = t.to(dtype)
+    if t.device != device:
+        t = t.to(device, non_blocking=True)
+    return t.contiguous()
+
+
+def _task_rows(task_tokens, n, device):
+    """The task token of each of n samples as [n, 1] int64 on ``device`` (the first entry of each sample's row)."""
+    return _to_device(task_tokens, torch.int64, device).reshape(n, -1)[:, :1].contiguous()
+
+
 def packed_offsets(lengths, extra: int = 0):
     """Row offsets [n + 1] of n items stored back to back with lengths[i] + extra rows each (extra = 1: the task-token row of
     a caption state)."""
@@ -215,6 +236,19 @@ class VILBertForVLTasks(object):
         except Exception:
             pass
 
+    def _engine_device(self) -> torch.device:
+        """The engine's device; raises when the model has no engine (before any CUDA tensor or library call)."""
+        if self._handle is None:
+            raise L.VilbertB200Error("call model.cuda(i) first (worker.py:536); there is no CPU path")
+        return torch.device("cuda", self._device)
+
+    def _call(self, fn: str, *args):
+        """``fn(handle, *args, stream)`` of the C ABI on the current stream of the engine's device; raises on a failed status."""
+        device = self._engine_device()
+        with torch.cuda.device(device):
+            stream = torch.cuda.current_stream(device).cuda_stream
+            L.check(getattr(L.load(), fn)(self._handle, *args, C.c_void_p(stream)), self._handle)
+
     # ------------------------------------------------------------------ forward
     def _out_shapes(self, B, T, V, select):
         d = self._dims
@@ -232,6 +266,7 @@ class VILBertForVLTasks(object):
         return {k: s for k, (bit, s) in shapes.items() if select & bit}
 
     def plan_info(self, batch, n_tokens, n_regions, select=L.OUT_TASK_HEADS):
+        self._engine_device()
         n, f = C.c_int64(), C.c_double()
         L.check(L.load().vb200_plan_info(self._handle, batch, n_tokens, n_regions, select, C.byref(n), C.byref(f)),
                 self._handle)
@@ -240,6 +275,7 @@ class VILBertForVLTasks(object):
     def set_option(self, key, value):
         """Run-time knobs of the engine (include/vilbert_b200.h, vb200_set_option): "max_plans", "timeline", "profile_grid_pct",
         "gemm_kernel", "max_rows_per_sample" (also applied to the engine a later .cuda() creates)."""
+        self._engine_device()
         L.check(L.load().vb200_set_option(self._handle, key.encode(), int(value)), self._handle)
         if key == "max_rows_per_sample":
             self._opts["max_rows_per_sample"] = int(value)
@@ -252,6 +288,7 @@ class VILBertForVLTasks(object):
     def profile_ops(self, batch, n_tokens, n_regions, select=L.OUT_TASK_HEADS, iters=5, grid_pct=0):
         """Per-launch device times (ms) of one forward: every kernel replayed alone from its own CUDA graph between two events.
         grid_pct (10..100): persistent-grid size of the GEMMs for THIS measurement only (production: 2/3 of the CTA slots)."""
+        self._engine_device()
         if grid_pct:
             L.check(L.load().vb200_set_option(self._handle, b"profile_grid_pct", int(grid_pct)), self._handle)
         cap = 2048
@@ -267,25 +304,15 @@ class VILBertForVLTasks(object):
                 for i in range(min(n.value, cap))]
 
     def _prep(self, question, features, spatials, segment_ids, input_mask, image_mask, task_tokens, device):
-        def dev(t, dtype):
-            if not torch.is_tensor(t):
-                t = torch.as_tensor(t)
-            if t.dtype != dtype:
-                t = t.to(dtype)
-            if t.device != device:
-                t = t.to(device, non_blocking=True)
-            return t.contiguous()
         B, Tin = question.shape
         V = features.shape[1]
-        q = dev(question, torch.int64)
-        f = dev(features, torch.float32)
-        s = dev(spatials, torch.float32)
-        seg = dev(segment_ids if segment_ids is not None else torch.zeros_like(question), torch.int64)
-        im = dev(input_mask if input_mask is not None else torch.ones_like(question), torch.int64)
-        vm = dev(image_mask if image_mask is not None else torch.ones(B, V, dtype=torch.uint8), torch.uint8)
-        if task_tokens is None:
-            task_tokens = torch.zeros(B, 1, dtype=torch.int64)
-        tk = dev(task_tokens, torch.int64).reshape(B, -1)[:, :1].contiguous()
+        q = _to_device(question, torch.int64, device)
+        f = _to_device(features, torch.float32, device)
+        s = _to_device(spatials, torch.float32, device)
+        seg = _to_device(segment_ids if segment_ids is not None else torch.zeros_like(question), torch.int64, device)
+        im = _to_device(input_mask if input_mask is not None else torch.ones_like(question), torch.int64, device)
+        vm = _to_device(image_mask if image_mask is not None else torch.ones(B, V, dtype=torch.uint8), torch.uint8, device)
+        tk = _task_rows(task_tokens if task_tokens is not None else torch.zeros(B, 1, dtype=torch.int64), B, device)
         if tuple(f.shape) != (B, V, self._dims["v_feature_size"]) or tuple(s.shape) != (B, V, 5) \
                 or tuple(seg.shape) != (B, Tin) or tuple(im.shape) != (B, Tin) or tuple(vm.shape) != (B, V):
             raise ValueError("input shapes do not match the worker.py:416-455 layout")
@@ -309,13 +336,9 @@ class VILBertForVLTasks(object):
         are set, else ``[]``.  ``slot`` selects one of 16 independent workspaces: calls on different slots may be in flight
         concurrently on different CUDA streams.
         """
-        if self._handle is None:
-            if torch.is_tensor(input_txt) and input_txt.is_cuda:
-                self.cuda(input_txt.device.index)
-            else:
-                raise L.VilbertB200Error("call model.cuda(i) first (worker.py:536); there is no CPU path")
-        lib = L.load()
-        device = torch.device("cuda", self._device)
+        if self._handle is None and torch.is_tensor(input_txt) and input_txt.is_cuda:
+            self.cuda(input_txt.device.index)
+        device = self._engine_device()
         if select is None:
             select = L.OUT_ALL if compute_pretraining_heads else L.OUT_TASK_HEADS
         q, f, s, seg, im, vm, tk = self._prep(input_txt, input_imgs, image_loc, token_type_ids, attention_mask,
@@ -326,14 +349,13 @@ class VILBertForVLTasks(object):
                        vm.data_ptr(), None, tk.data_ptr())
         want_attn = bool(output_all_attention_masks and self.return_attention)
         outs, o, select = self._alloc_outputs(B, Tin, V, select, debug_taps, want_attn, device)
-        with torch.cuda.device(device):
-            stream = torch.cuda.current_stream(device).cuda_stream
-            L.check(lib.vb200_forward_slot(self._handle, C.byref(inp), C.byref(o), select, slot, C.c_void_p(stream)), self._handle)
+        self._call("vb200_forward_slot", C.byref(inp), C.byref(o), select, slot)
         return self._result(outs, B, Tin, V, debug_taps)
 
     # ------------------------------------------------------------------ shared output plumbing
     def attention_layout(self, B, Tin, V):
         """[(heads, Lq, Lk, kind, float_offset)] of the flat attention buffer + its size (vb200_attention_layout)."""
+        self._engine_device()
         lib = L.load()
         n = C.c_int32()
         total = C.c_int64()
@@ -346,13 +368,12 @@ class VILBertForVLTasks(object):
     def attention_layout_packed(self, n_tokens, n_regions):
         """[(heads, kind, float_offset)] of the packed attention buffer of a batch with these Tin_b / V_b (for
         ``forward_regions_packed``, V_b = n_boxes_b + 1) + its size in floats (vb200_attention_layout_packed)."""
+        self._engine_device()
         lib = L.load()
         nt, nr = _host_ints(n_tokens), _host_ints(n_regions)
         if len(nt) != len(nr):
             raise ValueError("attention_layout_packed: n_tokens and n_regions must have the same length")
-        B = len(nt)
-        nt_c, nr_c = (C.c_int32 * max(B, 1))(*nt), (C.c_int32 * max(B, 1))(*nr)
-        args = (self._handle, B, C.cast(nt_c, C.c_void_p), C.cast(nr_c, C.c_void_p))
+        args = (self._handle, len(nt), _int32s(nt), _int32s(nr))
         n, total = C.c_int32(), C.c_int64()
         L.check(lib.vb200_attention_layout_packed(*args, 0, C.byref(n), None, None, C.byref(total)), self._handle)
         dims = (C.c_int32 * (2 * n.value))()
@@ -421,23 +442,16 @@ class VILBertForVLTasks(object):
         """``custom_prediction``'s tensor construction fused into the forward: ``box_features [B, n, F]`` (what the detector
         returned, no global row), pixel ``boxes [B, n, 4]``, ``image_wh [B, 2]`` -> the 10-tuple (and the ``spatials``
         tensor ``[B, n+1, 5]`` the reference would have built: the grounding decode reads it, worker.py:379)."""
-        if self._handle is None:
-            raise L.VilbertB200Error("call model.cuda(i) first (worker.py:536); there is no CPU path")
-        lib = L.load()
-        device = torch.device("cuda", self._device)
-
-        def dev(t, dtype):
-            t = torch.as_tensor(t)
-            return t.to(device=device, dtype=dtype, non_blocking=True).contiguous()
-        q, seg, im = dev(question, torch.int64), dev(segment_ids, torch.int64), dev(input_mask, torch.int64)
+        device = self._engine_device()
+        q, seg, im = (_to_device(t, torch.int64, device) for t in (question, segment_ids, input_mask))
         B, Tin = q.shape
-        tk = dev(task_tokens, torch.int64).reshape(B, -1)[:, :1].contiguous()
-        bf, bx, wh = dev(box_features, torch.float32), dev(boxes, torch.float32), dev(image_wh, torch.float32)
+        tk = _task_rows(task_tokens, B, device)
+        bf, bx, wh = (_to_device(t, torch.float32, device) for t in (box_features, boxes, image_wh))
         n = bf.shape[1]
         if tuple(bf.shape) != (B, n, self._dims["v_feature_size"]) or tuple(bx.shape) != (B, n, 4) or tuple(wh.shape) != (B, 2) \
                 or tuple(seg.shape) != (B, Tin) or tuple(im.shape) != (B, Tin):
             raise ValueError("forward_regions: box_features [B,n,F], boxes [B,n,4], image_wh [B,2], text [B,Tin] expected")
-        nb = dev(num_boxes, torch.int32) if num_boxes is not None else None
+        nb = _to_device(num_boxes, torch.int32, device) if num_boxes is not None else None
         sp = torch.empty(B, n + 1, 5, dtype=torch.float32, device=device) if return_spatials else None
         if select is None:
             select = L.OUT_TASK_HEADS
@@ -445,9 +459,7 @@ class VILBertForVLTasks(object):
                              wh.data_ptr(), nb.data_ptr() if nb is not None else None, sp.data_ptr() if sp is not None else None)
         want_attn = bool(output_all_attention_masks and self.return_attention)
         outs, o, select = self._alloc_outputs(B, Tin, n + 1, select, False, want_attn, device)
-        with torch.cuda.device(device):
-            stream = torch.cuda.current_stream(device).cuda_stream
-            L.check(lib.vb200_forward_regions(self._handle, C.byref(inp), C.byref(o), select, slot, C.c_void_p(stream)), self._handle)
+        self._call("vb200_forward_regions", C.byref(inp), C.byref(o), select, slot)
         return self._result(outs, B, Tin, n + 1, False), sp
 
     # ------------------------------------------------------------------ packed variable-length batches
@@ -464,24 +476,17 @@ class VILBertForVLTasks(object):
         lengths (``split_packed_attention``: per layer a list of B ``[heads, L_i, L_i]`` tensors, a connection layer a tuple of two
         such lists), views of one flat buffer.  ``max_tokens`` / ``max_regions`` (0: this call's maxima) are the plan's capacities:
         calls with the same batch size and capacities share one plan and CUDA graph whatever their lengths."""
-        if self._handle is None:
-            raise L.VilbertB200Error("call model.cuda(i) first (worker.py:536); there is no CPU path")
-        lib = L.load()
-        device = torch.device("cuda", self._device)
+        device = self._engine_device()
         nt, nr = _host_ints(n_tokens), _host_ints(n_regions)
         B = len(nt)
         if len(nr) != B or B < 1:
             raise ValueError("forward_packed: n_tokens and n_regions must have the same, positive length")
-
-        def dev(t, dtype):
-            return torch.as_tensor(t).to(device=device, dtype=dtype, non_blocking=True).contiguous()
         F = self._dims["v_feature_size"]
-        q = dev(question, torch.int64).reshape(-1)
-        seg = dev(segment_ids if segment_ids is not None else torch.zeros_like(q), torch.int64).reshape(-1)
-        f = dev(features, torch.float32).reshape(-1, F)
-        s = dev(spatials, torch.float32).reshape(-1, 5)
-        tk = dev(task_tokens if task_tokens is not None else torch.zeros(B, 1, dtype=torch.int64), torch.int64).reshape(B, -1)[:, :1]
-        tk = tk.contiguous()
+        q = _to_device(question, torch.int64, device).reshape(-1)
+        seg = _to_device(segment_ids if segment_ids is not None else torch.zeros_like(q), torch.int64, device).reshape(-1)
+        f = _to_device(features, torch.float32, device).reshape(-1, F)
+        s = _to_device(spatials, torch.float32, device).reshape(-1, 5)
+        tk = _task_rows(task_tokens if task_tokens is not None else torch.zeros(B, 1, dtype=torch.int64), B, device)
         sum_tin, sum_v = sum(nt), sum(nr)
         if q.numel() != sum_tin or seg.numel() != sum_tin or f.shape[0] != sum_v or s.shape[0] != sum_v:
             raise ValueError("forward_packed: question / segment_ids need sum(n_tokens) rows, features / spatials sum(n_regions)")
@@ -490,12 +495,9 @@ class VILBertForVLTasks(object):
         want_attn = bool(output_all_attention_masks and self.return_attention)
         if want_attn:
             select, maps = self._packed_attention(nt, nr, select, o, device)
-        nt_c, nr_c = (C.c_int32 * B)(*nt), (C.c_int32 * B)(*nr)
-        inp = L.PackedInputs(B, int(max_tokens), int(max_regions), C.cast(nt_c, C.c_void_p), C.cast(nr_c, C.c_void_p), q.data_ptr(),
-                             seg.data_ptr(), f.data_ptr(), s.data_ptr(), tk.data_ptr())
-        with torch.cuda.device(device):
-            stream = torch.cuda.current_stream(device).cuda_stream
-            L.check(lib.vb200_forward_packed(self._handle, C.byref(inp), C.byref(o), select, slot, C.c_void_p(stream)), self._handle)
+        inp = L.PackedInputs(B, int(max_tokens), int(max_regions), _int32s(nt), _int32s(nr), q.data_ptr(), seg.data_ptr(), f.data_ptr(),
+                             s.data_ptr(), tk.data_ptr())
+        self._call("vb200_forward_packed", C.byref(inp), C.byref(o), select, slot)
         result = self._result(outs, B, 0, 0, debug_taps)
         return self._with_attention(result, maps(), debug_taps) if want_attn else result
 
@@ -514,23 +516,18 @@ class VILBertForVLTasks(object):
         plan's capacities; the plan is the one ``forward_packed`` uses at ``max_regions = max_boxes + 1``.  Element 9 follows
         ``forward_packed``: the attention maps at each image's own T_i / V_i with ``output_all_attention_masks`` and
         ``self.return_attention``, else ``[]``."""
-        if self._handle is None:
-            raise L.VilbertB200Error("call model.cuda(i) first (worker.py:536); there is no CPU path")
-        lib = L.load()
-        device = torch.device("cuda", self._device)
+        device = self._engine_device()
         nt, nb = _host_ints(n_tokens), _host_ints(n_boxes)
         B = len(nt)
         if len(nb) != B or B < 1:
             raise ValueError("forward_regions_packed: n_tokens and n_boxes must have the same, positive length")
-
-        def dev(t, dtype):
-            return torch.as_tensor(t).to(device=device, dtype=dtype, non_blocking=True).contiguous()
         F = self._dims["v_feature_size"]
-        q = dev(question, torch.int64).reshape(-1)
-        seg = dev(segment_ids if segment_ids is not None else torch.zeros_like(q), torch.int64).reshape(-1)
-        tk = dev(task_tokens if task_tokens is not None else torch.zeros(B, 1, dtype=torch.int64), torch.int64).reshape(B, -1)[:, :1]
-        tk = tk.contiguous()
-        bf, bx, wh = dev(box_features, torch.float32).reshape(-1, F), dev(boxes, torch.float32).reshape(-1, 4), dev(image_wh, torch.float32)
+        q = _to_device(question, torch.int64, device).reshape(-1)
+        seg = _to_device(segment_ids if segment_ids is not None else torch.zeros_like(q), torch.int64, device).reshape(-1)
+        tk = _task_rows(task_tokens if task_tokens is not None else torch.zeros(B, 1, dtype=torch.int64), B, device)
+        bf = _to_device(box_features, torch.float32, device).reshape(-1, F)
+        bx = _to_device(boxes, torch.float32, device).reshape(-1, 4)
+        wh = _to_device(image_wh, torch.float32, device)
         sum_tin, sum_n = sum(nt), sum(nb)
         if q.numel() != sum_tin or seg.numel() != sum_tin or bf.shape[0] != sum_n or bx.shape[0] != sum_n or tuple(wh.shape) != (B, 2):
             raise ValueError("forward_regions_packed: question / segment_ids need sum(n_tokens) entries, box_features / boxes "
@@ -542,14 +539,9 @@ class VILBertForVLTasks(object):
         want_attn = bool(output_all_attention_masks and self.return_attention)
         if want_attn:
             select, maps = self._packed_attention(nt, [n + 1 for n in nb], select, o, device)
-        nt_c, nb_c = (C.c_int32 * B)(*nt), (C.c_int32 * B)(*nb)
-        inp = L.PackedRegionInputs(B, int(max_tokens), int(max_boxes), C.cast(nt_c, C.c_void_p), C.cast(nb_c, C.c_void_p),
-                                   q.data_ptr(), seg.data_ptr(), tk.data_ptr(), bf.data_ptr(), bx.data_ptr(), wh.data_ptr(),
-                                   sp.data_ptr() if sp is not None else None)
-        with torch.cuda.device(device):
-            stream = torch.cuda.current_stream(device).cuda_stream
-            L.check(lib.vb200_forward_regions_packed(self._handle, C.byref(inp), C.byref(o), select, slot, C.c_void_p(stream)),
-                    self._handle)
+        inp = L.PackedRegionInputs(B, int(max_tokens), int(max_boxes), _int32s(nt), _int32s(nb), q.data_ptr(), seg.data_ptr(),
+                                   tk.data_ptr(), bf.data_ptr(), bx.data_ptr(), wh.data_ptr(), sp.data_ptr() if sp is not None else None)
+        self._call("vb200_forward_regions_packed", C.byref(inp), C.byref(o), select, slot)
         result = self._result(outs, B, 0, 0, debug_taps)
         return (self._with_attention(result, maps(), debug_taps) if want_attn else result), sp
 
@@ -581,15 +573,11 @@ class VILBertForVLTasks(object):
         Returns one ``(indices, probs, boxes)`` per message: top_n indices in the segment, best first (equal probabilities: lower
         index first), the fp32 softmax probabilities as Python floats, and for grounding top_n ``[x1, y1, x2, y2]`` pixel boxes
         (``int(spatial * size)``, worker.py:381-384), else None."""
-        if self._handle is None:
-            raise L.VilbertB200Error("call model.cuda(i) first (worker.py:536); there is no CPU path")
+        self._engine_device()
         args, families = self._decode_args(out, messages, spatials)
         n = len(messages)
         answers = (L.Answer * max(n, 1))()
-        device = torch.device("cuda", self._device)
-        with torch.cuda.device(device):
-            stream = torch.cuda.current_stream(device).cuda_stream
-            L.check(L.load().vb200_decode_answers_host(self._handle, *args, answers, C.c_void_p(stream)), self._handle)
+        self._call("vb200_decode_answers_host", *args, answers)
         res = []
         for a, fam in zip(answers[:n], families):
             k = a.n
@@ -646,17 +634,13 @@ class VILBertForVLTasks(object):
         written.  Returns a dict of device tensors: box_features, boxes (original pixels), num_boxes [n] int32, keep_index
         [out_rows] int32, max_conf [out_rows] (the sorted scores), cls_prob [out_rows, C] and objects [out_rows] int64 (the argmax of
         each cls_prob row) when asked for, else None; and the host lists ``n_boxes`` (k_i) and ``dst_rows``."""
-        if self._handle is None:
-            raise L.VilbertB200Error("call model.cuda(i) first (worker.py:536); there is no CPU path")
-        device = torch.device("cuda", self._device)
+        device = self._engine_device()
         n = len(detections)
         if n < 1:
             raise ValueError("select_regions: no images")
         heads, k = [], []
         for prop, sc, ft, scale in detections:
-            prop = torch.as_tensor(prop).to(device=device, dtype=torch.float32).contiguous()
-            sc = torch.as_tensor(sc).to(device=device, dtype=torch.float32).contiguous()
-            ft = torch.as_tensor(ft).to(device=device, dtype=torch.float32).contiguous()
+            prop, sc, ft = (_to_device(t, torch.float32, device) for t in (prop, sc, ft))
             if prop.dim() != 2 or prop.shape[1] != 4 or sc.dim() != 2 or ft.dim() != 2 or not prop.shape[0] == sc.shape[0] == ft.shape[0]:
                 raise ValueError(f"select_regions: image {len(heads)} needs proposals [n, 4], scores [n, C] and features [n, F]")
             heads.append((prop, sc, ft, float(scale)))
@@ -689,76 +673,68 @@ class VILBertForVLTasks(object):
             imgs[i] = L.Detections(int(prop.shape[0]), r, scale, prop.data_ptr(), sc.data_ptr(), ft.data_ptr())
         params = L.SelectParams(Cn, F, int(max_boxes), float(conf_thresh), float(nms_iou), int(bool(background)), int(out_rows))
         sel = L.Selected(*[res[name].data_ptr() if res[name] is not None else None for name, _ in L.Selected._fields_])
-        with torch.cuda.device(device):
-            stream = torch.cuda.current_stream(device).cuda_stream
-            L.check(L.load().vb200_select_regions(self._handle, imgs, n, C.byref(params), C.byref(sel), C.c_void_p(stream)),
-                    self._handle)
+        self._call("vb200_select_regions", imgs, n, C.byref(params), C.byref(sel))
         res["n_boxes"], res["dst_rows"] = k, dst_rows
         return res
 
     # ------------------------------------------------------------------ retrieval reuse (SURVEY.md section 8e)
+    def _dense_state(self, kind, n, rows, device, **lengths):
+        """An empty prefix state of n items with ``rows`` rows each: f32 and 16-bit rows of the ``kind`` stream and the key mask."""
+        H = self._dims["hidden_size" if kind == "text" else "v_hidden_size"]
+        S = self._dims["operand_width_factor"]
+        return dict(kind=kind, n=n, **lengths, f32=torch.empty(n, rows, H, dtype=torch.float32, device=device),
+                    h16=torch.empty(n, rows, H * S, dtype=torch.int16, device=device),
+                    mask=torch.empty(n, rows, dtype=torch.float32, device=device))
+
+    def _packed_state(self, kind, lengths, device, extra=0):
+        """An empty packed prefix state: item i's rows (lengths[i] + extra) back to back from ``offsets[i]``, no mask; ``max_len`` is
+        the longest of ``lengths``."""
+        offs = packed_offsets(lengths, extra)
+        H = self._dims["hidden_size" if kind == "text" else "v_hidden_size"]
+        return dict(kind=kind, n=len(lengths), offsets=torch.tensor(offs, dtype=torch.int32), max_len=max(lengths),
+                    f32=torch.empty(offs[-1], H, dtype=torch.float32, device=device),
+                    h16=torch.empty(offs[-1], H, dtype=torch.int16, device=device))
+
     @torch.no_grad()
     def encode_text(self, question, segment_ids, input_mask, task_tokens):
         """Everything ahead of the first connection layer that depends on the caption alone (embeddings + text layers T0..),
         once per caption.  Returns an opaque state for ``forward_cached``."""
-        lib = L.load()
-        device = torch.device("cuda", self._device)
-        q = question.to(device=device, dtype=torch.int64).contiguous()
+        device = self._engine_device()
+        q = _to_device(question, torch.int64, device)
         n, Tin = q.shape
-        seg = segment_ids.to(device=device, dtype=torch.int64).contiguous()
-        im = input_mask.to(device=device, dtype=torch.int64).contiguous()
-        tk = task_tokens.to(device=device, dtype=torch.int64).reshape(n, -1)[:, :1].contiguous()
-        T = Tin + (1 if self._dims["task_specific_tokens"] else 0)
-        H, S = self._dims["hidden_size"], self._dims["operand_width_factor"]
-        st = dict(kind="text", n=n, Tin=Tin, f32=torch.empty(n, T, H, dtype=torch.float32, device=device),
-                  h16=torch.empty(n, T, H * S, dtype=torch.int16, device=device),
-                  mask=torch.empty(n, T, dtype=torch.float32, device=device))
-        with torch.cuda.device(device):
-            stream = torch.cuda.current_stream(device).cuda_stream
-            L.check(lib.vb200_encode_text(self._handle, n, Tin, q.data_ptr(), seg.data_ptr(), im.data_ptr(), tk.data_ptr(),
-                                          st["f32"].data_ptr(), st["h16"].data_ptr(), st["mask"].data_ptr(), C.c_void_p(stream)),
-                    self._handle)
+        seg, im = _to_device(segment_ids, torch.int64, device), _to_device(input_mask, torch.int64, device)
+        tk = _task_rows(task_tokens, n, device)
+        st = self._dense_state("text", n, Tin + (1 if self._dims["task_specific_tokens"] else 0), device, Tin=Tin)
+        self._call("vb200_encode_text", n, Tin, q.data_ptr(), seg.data_ptr(), im.data_ptr(), tk.data_ptr(), st["f32"].data_ptr(),
+                   st["h16"].data_ptr(), st["mask"].data_ptr())
         return st
 
     @torch.no_grad()
     def encode_image(self, features, spatials, image_mask):
         """The image-side prefix (image embedding, plus image layers scheduled ahead of the first connection layer), once per image."""
-        lib = L.load()
-        device = torch.device("cuda", self._device)
-        f = features.to(device=device, dtype=torch.float32).contiguous()
+        device = self._engine_device()
+        f = _to_device(features, torch.float32, device)
         n, V = f.shape[0], f.shape[1]
-        s = spatials.to(device=device, dtype=torch.float32).contiguous()
-        vm = image_mask.to(device=device, dtype=torch.uint8).contiguous()
-        Hv, S = self._dims["v_hidden_size"], self._dims["operand_width_factor"]
-        st = dict(kind="image", n=n, V=V, f32=torch.empty(n, V, Hv, dtype=torch.float32, device=device),
-                  h16=torch.empty(n, V, Hv * S, dtype=torch.int16, device=device),
-                  mask=torch.empty(n, V, dtype=torch.float32, device=device))
-        with torch.cuda.device(device):
-            stream = torch.cuda.current_stream(device).cuda_stream
-            L.check(lib.vb200_encode_image(self._handle, n, V, f.data_ptr(), s.data_ptr(), vm.data_ptr(), st["f32"].data_ptr(),
-                                           st["h16"].data_ptr(), st["mask"].data_ptr(), C.c_void_p(stream)), self._handle)
+        s, vm = _to_device(spatials, torch.float32, device), _to_device(image_mask, torch.uint8, device)
+        st = self._dense_state("image", n, V, device, V=V)
+        self._call("vb200_encode_image", n, V, f.data_ptr(), s.data_ptr(), vm.data_ptr(), st["f32"].data_ptr(), st["h16"].data_ptr(),
+                   st["mask"].data_ptr())
         return st
 
     @torch.no_grad()
     def forward_cached(self, text_state, text_index, image_state, image_index, select: int = L.OUT_VIL_LOGIT, slot: int = 0):
         """Pair b = (caption text_index[b], image image_index[b]) from cached states: the connection layers onwards.  Results are
         bit-identical to the full forward of the same pairs."""
-        lib = L.load()
-        device = torch.device("cuda", self._device)
-        ti = text_index.to(device=device, dtype=torch.int32).contiguous()
-        vi = image_index.to(device=device, dtype=torch.int32).contiguous()
+        device = self._engine_device()
+        ti, vi = _to_device(text_index, torch.int32, device), _to_device(image_index, torch.int32, device)
         B = ti.numel()
         if vi.numel() != B:
             raise ValueError("text_index and image_index must have the same length")
         Tin, V = text_state["Tin"], image_state["V"]
         outs, o, select = self._alloc_outputs(B, Tin, V, select, False, False, device)
-        with torch.cuda.device(device):
-            stream = torch.cuda.current_stream(device).cuda_stream
-            L.check(lib.vb200_forward_cached(self._handle, B, Tin, V, ti.data_ptr(), text_state["n"], text_state["f32"].data_ptr(),
-                                             text_state["h16"].data_ptr(), text_state["mask"].data_ptr(), vi.data_ptr(),
-                                             image_state["n"], image_state["f32"].data_ptr(), image_state["h16"].data_ptr(),
-                                             image_state["mask"].data_ptr(), C.byref(o), select, slot, C.c_void_p(stream)),
-                    self._handle)
+        self._call("vb200_forward_cached", B, Tin, V, ti.data_ptr(), text_state["n"], text_state["f32"].data_ptr(),
+                   text_state["h16"].data_ptr(), text_state["mask"].data_ptr(), vi.data_ptr(), image_state["n"],
+                   image_state["f32"].data_ptr(), image_state["h16"].data_ptr(), image_state["mask"].data_ptr(), C.byref(o), select, slot)
         return self._result(outs, B, Tin, V, False)
 
     # ------------------------------------------------------------------ packed retrieval: every caption / image at its own length
@@ -768,26 +744,17 @@ class VILBertForVLTasks(object):
         ``task_tokens`` ``[n, 1]``, ``n_tokens`` (list or CPU tensor) the Tin_c.  Returns an opaque state for
         ``forward_cached_packed``: caption c's rows sit at ``offsets[c]`` (T_c = Tin_c + 1 rows with the task token) and equal
         ``encode_text`` of that caption alone.  ``max_tokens`` (0: this call's maximum) is the plan capacity."""
-        lib = L.load()
-        device = torch.device("cuda", self._device)
+        device = self._engine_device()
         nt = _host_ints(n_tokens)
         n = len(nt)
-        q = torch.as_tensor(question).to(device=device, dtype=torch.int64).reshape(-1).contiguous()
-        seg = torch.as_tensor(segment_ids).to(device=device, dtype=torch.int64).reshape(-1).contiguous()
-        tk = torch.as_tensor(task_tokens).to(device=device, dtype=torch.int64).reshape(n, -1)[:, :1].contiguous()
+        q = _to_device(question, torch.int64, device).reshape(-1)
+        seg = _to_device(segment_ids, torch.int64, device).reshape(-1)
+        tk = _task_rows(task_tokens, n, device)
         if n < 1 or q.numel() != sum(nt) or seg.numel() != sum(nt):
             raise ValueError("encode_text_packed: question / segment_ids need sum(n_tokens) entries for n >= 1 captions")
-        offs = packed_offsets(nt, 1 if self._dims["task_specific_tokens"] else 0)
-        H = self._dims["hidden_size"]
-        st = dict(kind="text", n=n, offsets=torch.tensor(offs, dtype=torch.int32), max_len=max(nt),
-                  f32=torch.empty(offs[-1], H, dtype=torch.float32, device=device),
-                  h16=torch.empty(offs[-1], H, dtype=torch.int16, device=device))
-        nt_c = (C.c_int32 * n)(*nt)
-        with torch.cuda.device(device):
-            stream = torch.cuda.current_stream(device).cuda_stream
-            L.check(lib.vb200_encode_text_packed(self._handle, n, int(max_tokens), C.cast(nt_c, C.c_void_p), q.data_ptr(), seg.data_ptr(),
-                                                 tk.data_ptr(), st["f32"].data_ptr(), st["h16"].data_ptr(), C.c_void_p(stream)),
-                    self._handle)
+        st = self._packed_state("text", nt, device, extra=1 if self._dims["task_specific_tokens"] else 0)
+        self._call("vb200_encode_text_packed", n, int(max_tokens), _int32s(nt), q.data_ptr(), seg.data_ptr(), tk.data_ptr(),
+                   st["f32"].data_ptr(), st["h16"].data_ptr())
         return st
 
     @torch.no_grad()
@@ -795,24 +762,16 @@ class VILBertForVLTasks(object):
         """``encode_image`` of n images stored back to back without padding: ``features`` ``[sum V_i, F]``, ``spatials``
         ``[sum V_i, 5]``, ``n_regions`` the V_i.  Image i's state rows sit at ``offsets[i]`` and equal ``encode_image`` of that
         image alone."""
-        lib = L.load()
-        device = torch.device("cuda", self._device)
+        device = self._engine_device()
         nr = _host_ints(n_regions)
         n = len(nr)
-        f = torch.as_tensor(features).to(device=device, dtype=torch.float32).reshape(-1, self._dims["v_feature_size"]).contiguous()
-        s = torch.as_tensor(spatials).to(device=device, dtype=torch.float32).reshape(-1, 5).contiguous()
+        f = _to_device(features, torch.float32, device).reshape(-1, self._dims["v_feature_size"])
+        s = _to_device(spatials, torch.float32, device).reshape(-1, 5)
         if n < 1 or f.shape[0] != sum(nr) or s.shape[0] != sum(nr):
             raise ValueError("encode_image_packed: features / spatials need sum(n_regions) rows for n >= 1 images")
-        offs = packed_offsets(nr)
-        Hv = self._dims["v_hidden_size"]
-        st = dict(kind="image", n=n, offsets=torch.tensor(offs, dtype=torch.int32), max_len=max(nr),
-                  f32=torch.empty(offs[-1], Hv, dtype=torch.float32, device=device),
-                  h16=torch.empty(offs[-1], Hv, dtype=torch.int16, device=device))
-        nr_c = (C.c_int32 * n)(*nr)
-        with torch.cuda.device(device):
-            stream = torch.cuda.current_stream(device).cuda_stream
-            L.check(lib.vb200_encode_image_packed(self._handle, n, int(max_regions), C.cast(nr_c, C.c_void_p), f.data_ptr(), s.data_ptr(),
-                                                  st["f32"].data_ptr(), st["h16"].data_ptr(), C.c_void_p(stream)), self._handle)
+        st = self._packed_state("image", nr, device)
+        self._call("vb200_encode_image_packed", n, int(max_regions), _int32s(nr), f.data_ptr(), s.data_ptr(), st["f32"].data_ptr(),
+                   st["h16"].data_ptr())
         return st
 
     @torch.no_grad()
@@ -823,28 +782,17 @@ class VILBertForVLTasks(object):
         ``forward_regions_packed``: ``forward_cached_packed`` on these states gives that forward's scores bit for bit.
         ``max_boxes`` (0: this call's maximum) is the plan capacity; the plan is ``encode_image_packed``'s at ``max_regions =
         max_boxes + 1``."""
-        if self._handle is None:
-            raise L.VilbertB200Error("call model.cuda(i) first (worker.py:536); there is no CPU path")
-        lib = L.load()
-        device = torch.device("cuda", self._device)
+        device = self._engine_device()
         nb = _host_ints(n_boxes)
         n = len(nb)
-        bf = torch.as_tensor(box_features).to(device=device, dtype=torch.float32).reshape(-1, self._dims["v_feature_size"]).contiguous()
-        bx = torch.as_tensor(boxes).to(device=device, dtype=torch.float32).reshape(-1, 4).contiguous()
-        wh = torch.as_tensor(image_wh).to(device=device, dtype=torch.float32).contiguous()
+        bf = _to_device(box_features, torch.float32, device).reshape(-1, self._dims["v_feature_size"])
+        bx = _to_device(boxes, torch.float32, device).reshape(-1, 4)
+        wh = _to_device(image_wh, torch.float32, device)
         if n < 1 or bf.shape[0] != sum(nb) or bx.shape[0] != sum(nb) or tuple(wh.shape) != (n, 2):
             raise ValueError("encode_regions_packed: box_features / boxes need sum(n_boxes) rows and image_wh [n, 2] for n >= 1 images")
-        offs = packed_offsets(nb, 1)
-        Hv = self._dims["v_hidden_size"]
-        st = dict(kind="image", n=n, offsets=torch.tensor(offs, dtype=torch.int32), max_len=max(nb) + 1,
-                  f32=torch.empty(offs[-1], Hv, dtype=torch.float32, device=device),
-                  h16=torch.empty(offs[-1], Hv, dtype=torch.int16, device=device))
-        nb_c = (C.c_int32 * n)(*nb)
-        with torch.cuda.device(device):
-            stream = torch.cuda.current_stream(device).cuda_stream
-            L.check(lib.vb200_encode_regions_packed(self._handle, n, int(max_boxes), C.cast(nb_c, C.c_void_p), bf.data_ptr(), bx.data_ptr(),
-                                                    wh.data_ptr(), st["f32"].data_ptr(), st["h16"].data_ptr(), C.c_void_p(stream)),
-                    self._handle)
+        st = self._packed_state("image", [k + 1 for k in nb], device)
+        self._call("vb200_encode_regions_packed", n, int(max_boxes), _int32s(nb), bf.data_ptr(), bx.data_ptr(), wh.data_ptr(),
+                   st["f32"].data_ptr(), st["h16"].data_ptr())
         return st
 
     @torch.no_grad()
@@ -866,8 +814,7 @@ class VILBertForVLTasks(object):
         if text_state.get("kind") != "text" or image_state.get("kind") != "image" or "offsets" not in text_state \
                 or "offsets" not in image_state:
             raise ValueError("forward_cached_packed: pass the states of encode_text_packed and encode_image_packed")
-        lib = L.load()
-        device = torch.device("cuda", self._device)
+        device = self._engine_device()
         ti = torch.as_tensor(text_index).to(device="cpu", dtype=torch.int32).reshape(-1).contiguous()
         vi = torch.as_tensor(image_index).to(device="cpu", dtype=torch.int32).reshape(-1).contiguous()
         B = ti.numel()
@@ -883,10 +830,7 @@ class VILBertForVLTasks(object):
         pairs = L.PackedPairs(B, mt, mr, ti.data_ptr(), vi.data_ptr(), text_state["n"], toffs.data_ptr(), text_state["f32"].data_ptr(),
                               text_state["h16"].data_ptr(), image_state["n"], voffs.data_ptr(), image_state["f32"].data_ptr(),
                               image_state["h16"].data_ptr())
-        with torch.cuda.device(device):
-            stream = torch.cuda.current_stream(device).cuda_stream
-            L.check(lib.vb200_forward_cached_packed(self._handle, C.byref(pairs), C.byref(o), select, slot, C.c_void_p(stream)),
-                    self._handle)
+        self._call("vb200_forward_cached_packed", C.byref(pairs), C.byref(o), select, slot)
         return self._result(outs, B, 0, 0, debug_taps)
 
     # ------------------------------------------------------------------ host-buffer entry (bench e2e, serving)
@@ -895,7 +839,6 @@ class VILBertForVLTasks(object):
         """vb200_forward_host[_slot]: HOST (ideally pinned) tensors in, HOST tensors out; H2D + forward + D2H (+ stream sync).
         With ``synchronize=False`` the call returns after enqueueing on the current stream; synchronise that stream before
         reading ``out`` or re-using the input buffers."""
-        lib = L.load()
         B, Tin = question.shape
         V = features.shape[1]
         inp = L.Inputs(B, Tin, V, question.data_ptr(), features.data_ptr(), spatials.data_ptr(),
@@ -904,9 +847,5 @@ class VILBertForVLTasks(object):
         o = L.Outputs()
         for k, t in out.items():
             setattr(o, k, t.data_ptr())
-        device = torch.device("cuda", self._device)
-        with torch.cuda.device(device):
-            stream = torch.cuda.current_stream(device).cuda_stream
-            L.check(lib.vb200_forward_host_slot(self._handle, C.byref(inp), C.byref(o), select, slot, 1 if synchronize else 0,
-                                                C.c_void_p(stream)), self._handle)
+        self._call("vb200_forward_host_slot", C.byref(inp), C.byref(o), select, slot, 1 if synchronize else 0)
         return out
