@@ -17,7 +17,8 @@
  * at their own lengths, pairs scored without padding; vb200_encode_regions_packed: image states from detector output), the answer decode of every message of a batch in one kernel (vb200_decode_answers:
  * softmax, top N and grounding boxes, so a C host answers a message without re-implementing prediction()'s decode), the detector's
  * region selection (vb200_select_regions: per-class NMS, confidence ranking and the top boxes of every image, written into the packed
- * region inputs), and kernel-level entry points for the tests.
+ * region inputs), the pre-training heads at the rows a caller lists (vb200_pretraining_heads: masked-token and masked-region logits and
+ * the image-text alignment score from a forward's final states, ranked on the device), and kernel-level entry points for the tests.
  * The Python shim in vilbert-multi-task_b200/ (ctypes) implements the protocol on top of them; see
  * INTEGRATION.md for the stub a maintainer of the reference would add.
  *
@@ -492,6 +493,48 @@ typedef struct {
 
 int vb200_select_regions(vb200_handle h, const vb200_detections* imgs /* HOST [n] */, int32_t n, const vb200_select_params* p,
                          const vb200_selected* out, void* cuda_stream);
+
+/* ---- Pre-training heads at chosen rows: the three ViLBERT objectives of the checkpoint's `cls` heads on the rows a caller lists, from
+ * the fp32 final states a forward returns as taps (vb200_outputs.sequence_output_t / _v and pooled_output, dense B x T / B x V rows
+ * or packed sum T_i / sum V_i rows; any forward that writes them).
+ *   token_logits[i]  = cls.predictions (768 -> 768 GELU + LayerNorm, tied 768 -> vocab decoder + bias) of text row text_rows[i];
+ *   region_logits[i] = cls.imagePredictions (1024 -> 1024 GELU + LayerNorm, 1024 -> v_target_size) of image row image_rows[i];
+ *   alignment[i]     = cls.bi_seq_relationship (bi_hidden -> 2) of pooled row pair_rows[i] (pooled_output = pooled_t * pooled_v).
+ * Each logits row is bit-identical to that row of the same forward run with VB200_OUT_LINGUISIC_PREDICTION / VB200_OUT_VISION_PREDICTION,
+ * and each alignment row to element 3 (vil_binary_prediction) of a batch-1 forward of that pair: one kernel gathers the listed rows into
+ * the 16-bit operand the forward's final LayerNorm writes, and the forward's GEMMs, LayerNorm and narrow-head kernels run on them at the
+ * bucket of the listed rows (128 rows times a power of two; tiles past the call's count are skipped).  Which alignment column means
+ * "matched" is upstream's convention; the engine returns both logits in the head's order.
+ * token_top / region_top: per listed row, the softmax over its logits and the top_k indices (columns) and probabilities, in the
+ * vb200_answer convention of vb200_decode_answers (equal probabilities: lower index first; box unused, 0).
+ * Every group is optional: a list of 0 rows, or NULL outputs, skips it.  Duplicate rows are allowed.  Everything is checked on the
+ * host before anything is enqueued: VB200_ERR_INVALID, with a message naming the list and the index, for a negative count, a row outside
+ * its state's rows, a NULL state for a non-empty list, top_k < 0, above VB200_DECODE_MAX_TOP or above the width of a head whose top
+ * output is requested, and a top output with top_k = 0.
+ * Asynchronous on cuda_stream; no forward plan is built, used or evicted.  The row lists reach the device through a pinned staging
+ * buffer: a call blocks only while the previous call's copy out of it is in flight, and when a larger bucket of rows appears for the
+ * first time (its workspace and TMA descriptors are built once and kept), so back-to-back calls need no synchronisation in between. */
+typedef struct {
+    const float* text_state;       /* DEVICE fp32 [t_rows, hidden]: a forward's sequence_output_t */
+    const float* image_state;      /* DEVICE fp32 [v_rows, v_hidden]: sequence_output_v */
+    const float* pooled_state;     /* DEVICE fp32 [p_rows, bi_hidden]: pooled_output */
+    int32_t t_rows, v_rows, p_rows;
+    int32_t n_t, n_v, n_p;         /* entries of the three row lists */
+    const int32_t* text_rows;      /* HOST [n_t] rows of text_state */
+    const int32_t* image_rows;     /* HOST [n_v] rows of image_state */
+    const int32_t* pair_rows;      /* HOST [n_p] rows of pooled_state */
+    int32_t top_k;                 /* 0: no ranking; else 1 .. VB200_DECODE_MAX_TOP */
+} vb200_pretrain_rows;
+
+typedef struct {                   /* DEVICE outputs, each optional (NULL skips it) */
+    float* token_logits;           /* [n_t, vocab] */
+    float* region_logits;          /* [n_v, v_target_size] */
+    float* alignment;              /* [n_p, 2] */
+    vb200_answer* token_top;       /* [n_t] */
+    vb200_answer* region_top;      /* [n_v] */
+} vb200_pretrain_out;
+
+int vb200_pretraining_heads(vb200_handle h, const vb200_pretrain_rows* in, const vb200_pretrain_out* out, void* cuda_stream);
 
 /* ---- Kernel-level entry points (device pointers), used by the parity tests and the roofline bench.  ---- */
 /* y = act(x[M,K] (16-bit) . w[N,K]^T (16-bit) + bias); act: 0 none, 1 GELU(erf), 2 ReLU.  residual, gamma and beta are reserved

@@ -119,6 +119,19 @@ class Selected(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("box_features", "boxes", "num_boxes", "keep_index", "max_conf", "cls_prob", "objects")]
 
 
+class PretrainRows(C.Structure):
+    """vb200_pretrain_rows: fp32 final states (device) and the HOST int32 row lists of vb200_pretraining_heads."""
+    _fields_ = [("text_state", C.c_void_p), ("image_state", C.c_void_p), ("pooled_state", C.c_void_p),
+                ("t_rows", C.c_int32), ("v_rows", C.c_int32), ("p_rows", C.c_int32),
+                ("n_t", C.c_int32), ("n_v", C.c_int32), ("n_p", C.c_int32),
+                ("text_rows", C.c_void_p), ("image_rows", C.c_void_p), ("pair_rows", C.c_void_p), ("top_k", C.c_int32)]
+
+
+class PretrainOut(C.Structure):
+    """vb200_pretrain_out: optional device outputs of vb200_pretraining_heads (logits fp32, top-k as vb200_answer)."""
+    _fields_ = [(n, C.c_void_p) for n in ("token_logits", "region_logits", "alignment", "token_top", "region_top")]
+
+
 class Options(C.Structure):
     _fields_ = [("device", C.c_int32), ("num_labels", C.c_int32), ("use_cuda_graph", C.c_int32),
                 ("use_pdl", C.c_int32), ("strict", C.c_int32), ("act_fp16", C.c_int32),
@@ -133,7 +146,8 @@ EXPORTS = ["vb200_abi_version", "vb200_create", "vb200_destroy", "vb200_last_err
            "vb200_self_attention", "vb200_co_attention", "vb200_self_attention_packed", "vb200_co_attention_packed",
            "vb200_self_attention_stream", "vb200_co_attention_stream",
            "vb200_linear_product", "vb200_text_embed", "vb200_image_pack", "vb200_region_pack", "vb200_rowdot", "vb200_gather_state",
-           "vb200_gather_packed_state", "vb200_decode_answers", "vb200_decode_answers_host", "vb200_select_regions"]
+           "vb200_gather_packed_state", "vb200_decode_answers", "vb200_decode_answers_host", "vb200_select_regions",
+           "vb200_pretraining_heads"]
 
 _lib = None
 
@@ -207,6 +221,7 @@ def load():
     lib.vb200_decode_answers.argtypes = [vp, C.POINTER(DecodeMsg), i32, C.POINTER(Outputs), i32, i32, vp, vp, vp]
     lib.vb200_decode_answers_host.argtypes = [vp, C.POINTER(DecodeMsg), i32, C.POINTER(Outputs), i32, i32, vp, C.POINTER(Answer), vp]
     lib.vb200_select_regions.argtypes = [vp, C.POINTER(Detections), i32, C.POINTER(SelectParams), C.POINTER(Selected), vp]
+    lib.vb200_pretraining_heads.argtypes = [vp, C.POINTER(PretrainRows), C.POINTER(PretrainOut), vp]
     for name in EXPORTS:
         if name not in ("vb200_last_error",):
             getattr(lib, name).restype = C.c_int

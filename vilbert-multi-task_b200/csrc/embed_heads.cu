@@ -267,6 +267,44 @@ gather_packed_state_kernel(PackedStateCopy text, PackedStateCopy image) {
     else copy_packed_rows(image, blockIdx.x);
 }
 
+// Pre-training heads at chosen rows (vb200_pretraining_heads): row rows[i] of a forward's fp32 final state -> row i of the heads'
+// compact operand.  The 16-bit forms are what ln_residual_kernel writes as the final LayerNorm's operand from the same fp32 value
+// (pack16x2<F16>, or in fp32-parity mode the hi | lo | hi split through pack16x2_rt and split_lo), so every head row sees the bits the
+// forward's full-row heads see.  MODE 0 bf16, 1 fp16, 2 fp16 hi | lo | hi, 3 fp32 copy (the pooled rows of the alignment head).
+// Rows [n, rows_out) -- the rest of the last 128-row GEMM tile -- are zeroed.  One thread per 8 columns: two 16-byte loads, one
+// 16-byte store per copy.
+template <int MODE>
+__global__ void __launch_bounds__(256)
+gather_rows_kernel(const float* __restrict__ src, const int32_t* __restrict__ rows, int n, int rows_out, int H, void* __restrict__ dst,
+                   int ld_dst) {
+    const int per_row = H >> 3;
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    const int r = t / per_row, c = (t - r * per_row) * 8;
+    if (r >= rows_out) return;
+    float4 a = make_float4(0.f, 0.f, 0.f, 0.f), b = a;
+    if (r < n) {
+        const float4* s = reinterpret_cast<const float4*>(src + static_cast<size_t>(rows[r]) * H + c);
+        a = s[0];
+        b = s[1];
+    }
+    if constexpr (MODE == 3) {
+        float4* d = reinterpret_cast<float4*>(static_cast<float*>(dst) + static_cast<size_t>(r) * ld_dst + c);
+        d[0] = a;
+        d[1] = b;
+    } else if constexpr (MODE == 2) {
+        uint4* d = reinterpret_cast<uint4*>(static_cast<uint16_t*>(dst) + static_cast<size_t>(r) * ld_dst + split_col(c));
+        const uint4 hi = make_uint4(pack16x2_rt(a.x, a.y, 1), pack16x2_rt(a.z, a.w, 1), pack16x2_rt(b.x, b.y, 1), pack16x2_rt(b.z, b.w, 1));
+        d[0] = hi;
+        d[8] = make_uint4(pack16x2_rt(split_lo(a.x), split_lo(a.y), 1), pack16x2_rt(split_lo(a.z), split_lo(a.w), 1),
+                          pack16x2_rt(split_lo(b.x), split_lo(b.y), 1), pack16x2_rt(split_lo(b.z), split_lo(b.w), 1));
+        d[16] = hi;
+    } else {
+        constexpr bool F16 = MODE == 1;
+        uint4* d = reinterpret_cast<uint4*>(static_cast<uint16_t*>(dst) + static_cast<size_t>(r) * ld_dst + c);
+        d[0] = make_uint4(pack16x2<F16>(a.x, a.y), pack16x2<F16>(a.z, a.w), pack16x2<F16>(b.x, b.y), pack16x2<F16>(b.z, b.w));
+    }
+}
+
 // one warp per row; n_out <= 4
 __global__ void __launch_bounds__(128)
 rowdot_kernel(const float* __restrict__ x, int ld_x, const float* __restrict__ W, const float* __restrict__ bias,
@@ -344,6 +382,22 @@ cudaError_t launch_gather_packed_state(const PackedStateCopy& text, const Packed
                                          reinterpret_cast<uintptr_t>(c->dst_f32) | reinterpret_cast<uintptr_t>(c->dst_16)) & 15)
             return cudaErrorInvalidValue;
     gather_packed_state_kernel<<<dim3(B, 2), 256, 0, st>>>(text, image);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_gather_rows(const float* src, const int32_t* rows, int n, int rows_out, int H, void* dst, int ld_dst, int mode,
+                                cudaStream_t st) {
+    if (n < 0 || rows_out < n || rows_out < 1 || H < 8 || H % 8 != 0 || mode < 0 || mode > 3 || (mode == 2 && H % 64 != 0) ||
+        ld_dst % 8 != 0 || ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15))
+        return cudaErrorInvalidValue;
+    const int64_t threads = static_cast<int64_t>(rows_out) * (H / 8);
+    const dim3 grid(static_cast<unsigned>((threads + 255) / 256)), block(256);
+    switch (mode) {
+        case 0: gather_rows_kernel<0><<<grid, block, 0, st>>>(src, rows, n, rows_out, H, dst, ld_dst); break;
+        case 1: gather_rows_kernel<1><<<grid, block, 0, st>>>(src, rows, n, rows_out, H, dst, ld_dst); break;
+        case 2: gather_rows_kernel<2><<<grid, block, 0, st>>>(src, rows, n, rows_out, H, dst, ld_dst); break;
+        default: gather_rows_kernel<3><<<grid, block, 0, st>>>(src, rows, n, rows_out, H, dst, ld_dst); break;
+    }
     return cudaGetLastError();
 }
 

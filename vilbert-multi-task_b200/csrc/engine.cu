@@ -615,6 +615,21 @@ struct Plan {
     }
 };
 
+// One pre-training head at one bucket of M listed rows (vb200_pretraining_heads): the device row list (the call's count first, which
+// bounds the GEMM, LayerNorm and rowdot rows), the gathered operand, the forward's launch list for that head built by add_linear /
+// rowdot_op at M rows (TMA descriptors included) and its fp32 logits.  Built once per bucket and kept, apart from the forward plans:
+// never captured, counted against max_plans or evicted.
+enum { kHeadText = 0, kHeadImage = 1, kHeadPair = 2 };
+constexpr int kMaxHeadRows = 1 << 20;   // rows per list of one call (the largest bucket's logits: 1M x 30522 fp32 = 125 GB is already
+                                        // past any device; the bound keeps the bucket arithmetic in int)
+struct RowHeads {
+    Plan pl;                       // workspace (pl.mem), launch list (pl.ops), GEMM scratch (pl.y_scratch[0]); B = 1, T = V = M
+    int M = 0;
+    int* d_rows = nullptr;         // [1 + M]: count, then the rows
+    void* a = nullptr;             // [M, width]: 16-bit operand (x3: hi | lo | hi) of the transform GEMM, fp32 pooled rows (pair head)
+    OutBuf logits;                 // [M, N] fp32, row stride logits.ld
+};
+
 }  // namespace
 
 // =========================================================================================== engine
@@ -676,8 +691,19 @@ struct vb200_engine {
     char* sel_ws = nullptr;
     size_t sel_ws_bytes = 0;
     cudaEvent_t sel_copied = nullptr, sel_done = nullptr;
+    // pre-training heads at chosen rows (vb200_pretraining_heads): per head (kHeadText / kHeadImage / kHeadPair) the RowHeads of every
+    // bucket seen so far; row lists staged in the pinned pre_h (pre_copied: the last copy out of it), pre_done marks the end of the
+    // last call's kernels.
+    std::map<int, std::unique_ptr<RowHeads>> row_heads[3];
+    int32_t* pre_h = nullptr;
+    size_t pre_h_cap = 0;
+    cudaEvent_t pre_copied = nullptr, pre_done = nullptr;
 
     ~vb200_engine() {
+        if (pre_copied) { cudaEventSynchronize(pre_copied); cudaEventDestroy(pre_copied); }
+        if (pre_done) { cudaEventSynchronize(pre_done); cudaEventDestroy(pre_done); }
+        if (pre_h) cudaFreeHost(pre_h);
+        for (auto& m : row_heads) m.clear();
         if (sel_copied) { cudaEventSynchronize(sel_copied); cudaEventDestroy(sel_copied); }
         if (sel_done) { cudaEventSynchronize(sel_done); cudaEventDestroy(sel_done); }
         if (sel_h) cudaFreeHost(sel_h);
@@ -1713,6 +1739,9 @@ struct vb200_engine {
     }
     // descriptors -> dec_d through the pinned dec_h (in stream order), then the decode kernel writes answers [n]
     void decode_answers(const std::vector<vb::DecodeDesc>& d, vb200_answer* answers, cudaStream_t st) {
+        CUDA_CHECK(vb::launch_answer_decode(stage_decode(d, st), static_cast<int>(d.size()), answers, st));
+    }
+    const vb::DecodeDesc* stage_decode(const std::vector<vb::DecodeDesc>& d, cudaStream_t st) {
         const size_t n = d.size();
         if (dec_copied == nullptr) CUDA_CHECK(cudaEventCreateWithFlags(&dec_copied, cudaEventDisableTiming));
         CUDA_CHECK(cudaEventSynchronize(dec_copied));                // the previous call's copy has left the staging buffer
@@ -1729,7 +1758,7 @@ struct vb200_engine {
         memcpy(dec_h, d.data(), n * sizeof(vb::DecodeDesc));
         CUDA_CHECK(cudaMemcpyAsync(dec_d, dec_h, n * sizeof(vb::DecodeDesc), cudaMemcpyHostToDevice, st));
         CUDA_CHECK(cudaEventRecord(dec_copied, st));
-        CUDA_CHECK(vb::launch_answer_decode(dec_d, static_cast<int>(n), answers, st));
+        return dec_d;
     }
     vb200_answer* answer_scratch(size_t n, cudaStream_t st) {
         if (n > ans_cap) {
@@ -1851,6 +1880,131 @@ struct vb200_engine {
         CUDA_CHECK(cudaMemsetAsync(a.max_conf, 0, rows * 4, st));
         CUDA_CHECK(vb::launch_select_regions(descs, n, max_n, max_npad, a, st));
         CUDA_CHECK(cudaEventRecord(sel_done, st));
+    }
+    // ---- pre-training heads at chosen rows
+    // The RowHeads of `head` for n rows: bucket M = 128 * 2^k >= n, built on its first use with the forward's head launches (build_heads)
+    // at M rows and the device row count as their m_rows.
+    RowHeads& row_heads_for(int head, int n) {
+        int M = 128;
+        while (M < n) M *= 2;
+        std::unique_ptr<RowHeads>& slot = row_heads[head][M];
+        if (slot) return *slot;
+        std::unique_ptr<RowHeads> r(new RowHeads());
+        Plan& pl = r->pl;
+        pl.B = 1; pl.T = pl.V = M;
+        r->M = M;
+        r->d_rows = pl.mem.alloc_n<int>(static_cast<size_t>(M) + 1);
+        const int* count = r->d_rows;
+        const size_t S = x3 ? 3 : 1;
+        if (head == kHeadPair) {
+            const int Hb = cfg.bi_hidden;
+            float* a = pl.mem.alloc_n<float>(static_cast<size_t>(M) * Hb);
+            r->a = a;
+            r->logits = make_out(pl, M, 2);
+            pl.ops.push_back(rowdot_op(a, Hb, seq_rel, nullptr, r->logits.p, r->logits.ld, M, count));
+        } else {
+            const bool text = head == kHeadText;
+            const int H = text ? cfg.hidden : cfg.v_hidden;
+            const LinearW& transform = text ? lm_transform : img_transform;
+            const LinearW& decoder = text ? lm_decoder : img_decoder;
+            bf16* a = pl.mem.alloc_n<bf16>(static_cast<size_t>(M) * H * S);
+            bf16* hid = pl.mem.alloc_n<bf16>(static_cast<size_t>(M) * H * S);
+            r->a = a;
+            pl.y_scratch[0] = pl.mem.alloc_n<float>(static_cast<size_t>(M) * H);
+            add_linear(pl, a, M, H, transform, vb::kActGelu, nullptr, 0, text ? &lm_ln : &img_ln, hid, H, nullptr, 0, 0, Op::NONE,
+                       nullptr, 0, count);
+            r->logits = make_out(pl, M, decoder.N);
+            add_linear(pl, hid, M, H, decoder, vb::kActNone, nullptr, 0, nullptr, nullptr, 0, r->logits.p, r->logits.ld, 0, Op::NONE,
+                       nullptr, 0, count);
+        }
+        for (Op& op : pl.ops) op.tag = "pretraining heads";
+        slot = std::move(r);
+        return *slot;
+    }
+    void pretraining_heads(const vb200_pretrain_rows* in, const vb200_pretrain_out* out, cudaStream_t st) {
+        const char* api = "vb200_pretraining_heads";
+        if (in == nullptr || out == nullptr) fail(VB200_ERR_INVALID, "%s: in / out is NULL", api);
+        const int k = in->top_k;
+        if (k < 0 || k > VB200_DECODE_MAX_TOP) fail(VB200_ERR_INVALID, "%s: top_k %d outside [0, %d]", api, k, VB200_DECODE_MAX_TOP);
+        struct Group {
+            const char* list; const char* state; const float* src; int src_rows, width; int n; const int32_t* rows;
+            float* logits; int N; vb200_answer* top; const char* top_name;
+        };
+        Group g[3] = {
+            {"text_rows", "text_state", in->text_state, in->t_rows, cfg.hidden, in->n_t, in->text_rows, out->token_logits, cfg.vocab,
+             out->token_top, "token_top"},
+            {"image_rows", "image_state", in->image_state, in->v_rows, cfg.v_hidden, in->n_v, in->image_rows, out->region_logits,
+             cfg.v_target, out->region_top, "region_top"},
+            {"pair_rows", "pooled_state", in->pooled_state, in->p_rows, cfg.bi_hidden, in->n_p, in->pair_rows, out->alignment, 2, nullptr,
+             nullptr},
+        };
+        size_t staged = 0;
+        for (const Group& x : g) {
+            if (x.n < 0 || x.n > kMaxHeadRows)
+                fail(VB200_ERR_INVALID, "%s: %s has a count of %d (must be in [0, %d])", api, x.list, x.n, kMaxHeadRows);
+            if (x.top != nullptr && k == 0) fail(VB200_ERR_INVALID, "%s: %s is requested with top_k = 0", api, x.top_name);
+            if (x.top != nullptr && k > x.N)
+                fail(VB200_ERR_INVALID, "%s: top_k %d is above the %d logits of a %s row", api, k, x.N, x.top_name);
+            if (x.n == 0) continue;
+            if (x.rows == nullptr) fail(VB200_ERR_INVALID, "%s: %s is NULL for %d rows", api, x.list, x.n);
+            if (x.src == nullptr) fail(VB200_ERR_INVALID, "%s: %s is NULL for a non-empty %s", api, x.state, x.list);
+            if (reinterpret_cast<uintptr_t>(x.src) & 15) fail(VB200_ERR_INVALID, "%s: %s is not 16-byte aligned", api, x.state);
+            for (int i = 0; i < x.n; ++i)
+                if (x.rows[i] < 0 || x.rows[i] >= x.src_rows)
+                    fail(VB200_ERR_INVALID, "%s: %s[%d] = %d is outside the %d rows of %s", api, x.list, i, x.rows[i], x.src_rows, x.state);
+            if (x.logits != nullptr || x.top != nullptr) staged += 1 + static_cast<size_t>(x.n);
+        }
+        if (staged == 0) return;
+        CUDA_CHECK(cudaSetDevice(opt.device));
+        RowHeads* rh[3] = {nullptr, nullptr, nullptr};
+        std::vector<vb::DecodeDesc> descs;
+        for (int i = 0; i < 3; ++i) {
+            if (g[i].n == 0 || (g[i].logits == nullptr && g[i].top == nullptr)) continue;
+            rh[i] = &row_heads_for(i, g[i].n);
+            if (g[i].top != nullptr)
+                for (int r = 0; r < g[i].n; ++r)
+                    descs.push_back(vb::DecodeDesc{rh[i]->logits.p + static_cast<size_t>(r) * rh[i]->logits.ld, nullptr, 0.0, 0.0, g[i].N, k});
+        }
+        if (pre_copied == nullptr) CUDA_CHECK(cudaEventCreateWithFlags(&pre_copied, cudaEventDisableTiming));
+        if (pre_done == nullptr) CUDA_CHECK(cudaEventCreateWithFlags(&pre_done, cudaEventDisableTiming));
+        CUDA_CHECK(cudaEventSynchronize(pre_copied));                // the previous call's copies have left the staging buffer
+        if (staged > pre_h_cap) {
+            const size_t cap = std::max<size_t>({staged, 2 * pre_h_cap, 1024});
+            if (pre_h) CUDA_CHECK(cudaFreeHost(pre_h));
+            pre_h = nullptr;
+            CUDA_CHECK(cudaMallocHost(&pre_h, cap * sizeof(int32_t)));
+            pre_h_cap = cap;
+        }
+        CUDA_CHECK(cudaStreamWaitEvent(st, pre_done, 0));            // the previous call (any stream) is done with the workspace
+        size_t at = 0;
+        for (int i = 0; i < 3; ++i) {
+            if (rh[i] == nullptr) continue;
+            pre_h[at] = g[i].n;
+            memcpy(pre_h + at + 1, g[i].rows, static_cast<size_t>(g[i].n) * sizeof(int32_t));
+            CUDA_CHECK(cudaMemcpyAsync(rh[i]->d_rows, pre_h + at, (1 + static_cast<size_t>(g[i].n)) * sizeof(int32_t),
+                                       cudaMemcpyHostToDevice, st));
+            at += 1 + static_cast<size_t>(g[i].n);
+        }
+        CUDA_CHECK(cudaEventRecord(pre_copied, st));
+        const vb::DecodeDesc* dd = descs.empty() ? nullptr : stage_decode(descs, st);
+        for (int i = 0; i < 3; ++i) {
+            if (rh[i] == nullptr) continue;
+            RowHeads& r = *rh[i];
+            const Group& x = g[i];
+            const int rows_out = (x.n + 127) / 128 * 128;          // the rest of the last 128-row tile is zeroed
+            const int mode = i == kHeadPair ? 3 : (x3 ? 2 : (opt.act_fp16 ? 1 : 0));
+            const int ld = i == kHeadPair ? x.width : x.width * (x3 ? 3 : 1);
+            CUDA_CHECK(vb::launch_gather_rows(x.src, r.d_rows + 1, x.n, rows_out, x.width, r.a, ld, mode, st));
+            for (const Op& op : r.pl.ops) launch_op(op, st);
+            if (x.logits != nullptr)
+                CUDA_CHECK(cudaMemcpy2DAsync(x.logits, static_cast<size_t>(x.N) * 4, r.logits.p, static_cast<size_t>(r.logits.ld) * 4,
+                                             static_cast<size_t>(x.N) * 4, x.n, cudaMemcpyDeviceToDevice, st));
+            if (x.top != nullptr) {
+                CUDA_CHECK(vb::launch_answer_decode(dd, x.n, x.top, st));
+                dd += x.n;
+            }
+        }
+        CUDA_CHECK(cudaEventRecord(pre_done, st));
     }
     static float* out_ptr(const vb200_outputs& o, int slot) {
         switch (slot) {
@@ -2211,6 +2365,11 @@ int vb200_select_regions(vb200_handle h, const vb200_detections* imgs, int32_t n
     });
 }
 
+int vb200_pretraining_heads(vb200_handle h, const vb200_pretrain_rows* in, const vb200_pretrain_out* out, void* cuda_stream) {
+    if (h == nullptr) return VB200_ERR_INVALID;
+    return guard(h, [&] { h->pretraining_heads(in, out, static_cast<cudaStream_t>(cuda_stream)); });
+}
+
 int vb200_attention_layout(vb200_handle h, int32_t batch, int32_t n_tokens, int32_t n_regions, int32_t max_entries,
                            int32_t* n_entries, int32_t* dims, int64_t* offsets, int64_t* total_floats) {
     if (h == nullptr || n_entries == nullptr) return VB200_ERR_INVALID;
@@ -2352,6 +2511,7 @@ int vb200_set_option(vb200_handle h, const char* key, int64_t value) {
             if (value != h->gemm_kernel) {              // the kernel is chosen when a plan is built
                 CUDA_CHECK(cudaDeviceSynchronize());
                 h->plans.clear();
+                for (auto& m : h->row_heads) m.clear();
                 h->gemm_kernel = static_cast<int>(value);
             }
         } else if (k == "max_rows_per_sample") {

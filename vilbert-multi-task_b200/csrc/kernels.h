@@ -139,6 +139,11 @@ struct PackedProbs {
 cudaError_t launch_attention_f32(const void* q, int ld_q, const void* k, const void* v, int ld_kv, int in_kind,
                                  const float* key_mask_add, int B, int Lq, int Lk, int heads, int D, __nv_bfloat16* ctx, int ld_ctx,
                                  int ctx_mode, float* probs, int pdl, cudaStream_t st, const PackedProbs* packed = nullptr);
+// Pre-training heads at chosen rows: row rows[i] (device int32, i < n) of an fp32 state [*, H] -> row i of dst, in the 16-bit operand
+// form the final LayerNorm writes (mode 0 bf16, 1 fp16, 2 fp16 hi | lo | hi with ld_dst the 3x wide stride) or as fp32 (mode 3); rows
+// [n, rows_out) are zeroed.  H a multiple of 8 (64 in mode 2), 16-byte aligned src / dst; rows are bounds-checked on the host.
+cudaError_t launch_gather_rows(const float* src, const int32_t* rows, int n, int rows_out, int H, void* dst, int ld_dst, int mode,
+                               cudaStream_t st);
 // K8 (narrow heads): out[m, j] = dot(x[m, :K], W[j, :K]) + b[j] + (add ? add[m] : 0), j < n_out <= 4.
 cudaError_t launch_rowdot(const float* x, int ld_x, const float* W, const float* b, const float* add, float* out,
                           int ld_out, int M, int K, int n_out, int pdl, cudaStream_t st, const int* m_rows = nullptr);

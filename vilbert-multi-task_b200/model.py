@@ -618,6 +618,62 @@ class VILBertForVLTasks(object):
             sp = spatials.data_ptr()
         return (msgs, n, C.byref(o), batch, vision_rows, sp), families
 
+    # ------------------------------------------------------------------ pre-training heads at chosen rows
+    @torch.no_grad()
+    def pretraining_heads(self, taps, text_rows=None, image_rows=None, pair_rows=None, top_k: int = 0):
+        """The checkpoint's three pre-training objectives at the rows a caller lists (vb200_pretraining_heads), from the final states
+        a forward returned as taps: ``taps`` is the dict of ``forward(..., debug_taps=True)``, ``forward_packed``,
+        ``forward_regions_packed`` or ``forward_cached_packed`` with ``debug_taps=True``.  Rows index the flattened states: dense text
+        row b * T + t of ``sequence_output_t`` [B, T, hidden] (T = Tin + 1 with the task token), packed rows as the packed taps hold
+        them; image rows likewise in ``sequence_output_v``, pair rows in ``pooled_output`` [B, bi_hidden].
+
+        Returns a dict of device tensors: ``token_logits`` [n_t, vocab] (masked-token prediction, ``cls.predictions``),
+        ``region_logits`` [n_v, v_target_size] (masked-region prediction, ``cls.imagePredictions``) and ``alignment`` [n_p, 2]
+        (``cls.bi_seq_relationship`` on pooled_t * pooled_v) for each list given, each row bit-identical to that row of the forward's
+        full-row heads (element 3 of a batch-1 forward for the alignment).  Which alignment column means "matched" is an upstream
+        convention not confirmed here: both logits are returned in the head's order.  With ``top_k`` (1..10), ``token_top`` /
+        ``region_top`` are ``(indices [n, top_k] int32, probabilities [n, top_k] fp32)``: each row's softmax over its logits, best
+        first, equal probabilities ranking the lower index first -- computed on the device, like everything else here, so the call
+        returns as soon as its work is enqueued."""
+        device = self._engine_device()
+        d = self._dims
+        # (list, its rows, tap, width, logits columns, vb200_pretrain_rows fields: state, state rows, count, list; outputs: logits, top)
+        groups = (("text_rows", text_rows, "sequence_output_t", d["hidden_size"], d["vocab_size"],
+                   ("text_state", "t_rows", "n_t", "text_rows"), ("token_logits", "token_top")),
+                  ("image_rows", image_rows, "sequence_output_v", d["v_hidden_size"], d["v_target_size"],
+                   ("image_state", "v_rows", "n_v", "image_rows"), ("region_logits", "region_top")),
+                  ("pair_rows", pair_rows, "pooled_output", d["bi_hidden_size"], 2,
+                   ("pooled_state", "p_rows", "n_p", "pair_rows"), ("alignment", None)))
+        inp, out = L.PretrainRows(), L.PretrainOut()
+        inp.top_k = int(top_k)
+        res, keep = {}, []
+        for name, rows, tap, width, n_out, fields, (logits, top) in groups:
+            if rows is None:
+                continue
+            rows = _host_ints(rows)
+            state = taps.get(tap)
+            if state is None:
+                raise ValueError(f"pretraining_heads: {name} needs the {tap} tap")
+            if state.dtype != torch.float32 or state.device != device or not state.is_contiguous() or state.shape[-1] != width:
+                raise ValueError(f"pretraining_heads: {tap} must be a contiguous fp32 [..., {width}] tensor on {device}")
+            state = state.view(-1, width)
+            arr = _int32s(rows)
+            keep += [state, arr]
+            for field, value in zip(fields, (state.data_ptr(), state.shape[0], len(rows), arr)):
+                setattr(inp, field, value)
+            res[logits] = torch.empty(len(rows), n_out, dtype=torch.float32, device=device)
+            setattr(out, logits, res[logits].data_ptr())
+            if top is not None and top_k:
+                res[top] = torch.empty(len(rows), C.sizeof(L.Answer) // 4, dtype=torch.int32, device=device)
+                setattr(out, top, res[top].data_ptr())
+        self._call("vb200_pretraining_heads", C.byref(inp), C.byref(out))
+        k = int(top_k)
+        for head in ("token", "region"):
+            ans = res.get(head + "_top")
+            if ans is not None:            # vb200_answer as int32 words: n, index[10], prob[10], box[10][4]
+                res[head + "_top"] = (ans[:, 1:1 + k], ans[:, 1 + L.DECODE_MAX_TOP:1 + L.DECODE_MAX_TOP + k].view(torch.float32))
+        return res
+
     # ------------------------------------------------------------------ detector-region selection (worker.py:123-176)
     @torch.no_grad()
     def select_regions(self, detections, max_boxes: int = 100, conf_thresh: float = 0.0, background: bool = False,

@@ -177,37 +177,44 @@ def retrieval_pairs(n_captions: int, n_images: int, pair_batch: int):
 
 
 def retrieval_scores_packed(model, captions, images, task_id: int = 7, pair_batch: int = 256, group=None, comm=None,
-                            timings=None) -> torch.Tensor:
+                            timings=None, score: str = "vil_logit") -> torch.Tensor:
     """`retrieval_scores_cached` without padding: the same padded inputs, but every caption and image runs at its own length.
     `input_mask` and `image_mask` must have every row a prefix of ones (ValueError otherwise).  The real rows are packed, this rank's
     captions and all images are encoded once (`model.encode_text_packed` / `encode_image_packed`), and pairs are scored in chunks of
     `pair_batch` from the packed states (`model.forward_cached_packed`, one plan per chunk size).  Each score equals the
     unpadded forward of its pair; with uniform lengths and no padding it is bit-identical to `retrieval_scores_cached`.  One
-    all-gather at the end.  `timings` (dict) receives CUDA-event milliseconds: encode / pairs / gather."""
+    all-gather at the end.  `timings` (dict) receives CUDA-event milliseconds: encode / pairs / gather.
+
+    `score`: "vil_logit" (default) returns the retrieval head's [n_captions, n_images] matrix; "alignment" returns the pre-training
+    image-text alignment head instead (`cls.bi_seq_relationship`, the score of ViLBERT's zero-shot caption-based retrieval) as
+    [n_captions, n_images, 2], both logits of each pair computed from the pair's pooled state (`model.pretraining_heads`).  Which
+    column means "matched" is an upstream convention this code does not fix."""
     f, s, vm = images
     v_lens = strip_padding(vm, "image_mask")
     return _score_packed_states(model, captions, lambda: model.encode_image_packed(pack_rows(f, v_lens), pack_rows(s, v_lens), v_lens),
-                                f.shape[0], task_id, pair_batch, group, comm, timings)
+                                f.shape[0], task_id, pair_batch, group, comm, timings, score)
 
 
 def retrieval_scores_regions(model, captions, gallery, task_id: int = 7, pair_batch: int = 256, max_boxes: int = 0, group=None,
-                             comm=None, timings=None) -> torch.Tensor:
+                             comm=None, timings=None, score: str = "vil_logit") -> torch.Tensor:
     """`retrieval_scores_packed` with the gallery as the detector returns it: `gallery` = (box_features [sum n_boxes_i, F], pixel
     boxes [sum n_boxes_i, 4], image_wh [n_img, 2], n_boxes), the images' selected boxes back to back, on the model's device.  The
     gallery is encoded once with `model.encode_regions_packed` (capacity `max_boxes`, 0: the largest image), which builds each
     image's global mean row and locations on the device as `forward_regions_packed` does, so every score is bit-identical to that
     forward of its (caption, image) pair.  `captions` (padded, prefix masks), sharding, pair chunks, the all-gather and `timings`
-    follow `retrieval_scores_packed`."""
+    and `score` follow `retrieval_scores_packed`."""
     bf, bx, wh, n_boxes = gallery
     return _score_packed_states(model, captions, lambda: model.encode_regions_packed(bf, bx, wh, n_boxes, max_boxes=max_boxes),
-                                len(n_boxes), task_id, pair_batch, group, comm, timings)
+                                len(n_boxes), task_id, pair_batch, group, comm, timings, score)
 
 
-def _score_packed_states(model, captions, encode_gallery, n_img, task_id, pair_batch, group, comm, timings) -> torch.Tensor:
+def _score_packed_states(model, captions, encode_gallery, n_img, task_id, pair_batch, group, comm, timings, score) -> torch.Tensor:
     """What the packed retrieval calls share: this rank's block of the padded `captions` (prefix masks), the gallery states of
-    `encode_gallery()`, every pair scored in chunks of `pair_batch` from the packed states (`model.forward_cached_packed`), and one
-    all-gather."""
+    `encode_gallery()`, every pair scored in chunks of `pair_batch` from the packed states (`model.forward_cached_packed`; with
+    score="alignment" its pooled tap through `model.pretraining_heads`), and one all-gather."""
     from . import _lib as L
+    if score not in ("vil_logit", "alignment"):
+        raise ValueError(f'score must be "vil_logit" or "alignment", got {score!r}')
     world = dist.get_world_size(group) if dist.is_initialized() else 1
     rank = dist.get_rank(group) if dist.is_initialized() else 0
     q, seg, im = captions
@@ -223,11 +230,18 @@ def _score_packed_states(model, captions, encode_gallery, n_img, task_id, pair_b
     if ev:
         ev[1].record()
     ci, ii, total = retrieval_pairs(hi - lo, n_img, pair_batch)
-    scores = torch.empty(ci.numel(), dtype=torch.float32, device=dev)
-    for s0 in range(0, ci.numel(), pair_batch):
-        out = model.forward_cached_packed(ts, ci[s0:s0 + pair_batch], vs, ii[s0:s0 + pair_batch], select=L.OUT_VIL_LOGIT)
-        scores[s0:s0 + pair_batch] = out[2].view(-1)
-    local = scores[:total].view(hi - lo, n_img)
+    if score == "alignment":
+        scores = torch.empty(ci.numel(), 2, dtype=torch.float32, device=dev)
+        for s0 in range(0, ci.numel(), pair_batch):
+            _, taps = model.forward_cached_packed(ts, ci[s0:s0 + pair_batch], vs, ii[s0:s0 + pair_batch], select=0, debug_taps=True)
+            scores[s0:s0 + pair_batch] = model.pretraining_heads(taps, pair_rows=range(pair_batch))["alignment"]
+        local = scores[:total].view(hi - lo, n_img, 2)
+    else:
+        scores = torch.empty(ci.numel(), dtype=torch.float32, device=dev)
+        for s0 in range(0, ci.numel(), pair_batch):
+            out = model.forward_cached_packed(ts, ci[s0:s0 + pair_batch], vs, ii[s0:s0 + pair_batch], select=L.OUT_VIL_LOGIT)
+            scores[s0:s0 + pair_batch] = out[2].view(-1)
+        local = scores[:total].view(hi - lo, n_img)
     if ev:
         ev[2].record()
     full = all_gather_rows(local, n_cap, group, comm)
