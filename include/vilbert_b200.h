@@ -18,7 +18,9 @@
  * softmax, top N and grounding boxes, so a C host answers a message without re-implementing prediction()'s decode), the detector's
  * region selection (vb200_select_regions: per-class NMS, confidence ranking and the top boxes of every image, written into the packed
  * region inputs), the pre-training heads at the rows a caller lists (vb200_pretraining_heads: masked-token and masked-region logits and
- * the image-text alignment score from a forward's final states, ranked on the device), and kernel-level entry points for the tests.
+ * the image-text alignment score from a forward's final states, ranked on the device), upstream's pre-training model
+ * (vb200_create_pretraining: a checkpoint with the encoder and the `cls` heads but no task heads; vb200_pretraining_objectives: the
+ * masked-token, masked-region and alignment losses from labels, on the device), and kernel-level entry points for the tests.
  * The Python shim in vilbert-multi-task_b200/ (ctypes) implements the protocol on top of them; see
  * INTEGRATION.md for the stub a maintainer of the reference would add.
  *
@@ -154,6 +156,18 @@ int vb200_abi_version(void);
  * fp16 hi/lo pairs of split_fp32 -- and fp32 LayerNorm / bias / embedding tables). */
 int vb200_create(const char* config_json, int64_t n_tensors, const vb200_tensor* tensors, const vb200_options* opt,
                  vb200_handle* out);
+/* BertForMultiModalPreTraining.from_pretrained + cuda(device): the same arguments, options and audit rules as vb200_create (`module.`
+ * prefixes, gamma / beta, the ignored keys, strict vs strict = -1 for extra keys), against upstream's pre-training key set: `bert.*`
+ * plus cls.predictions.*, cls.imagePredictions.* and cls.bi_seq_relationship.*.  Task-head keys are extra keys.  The audit runs
+ * before any device is touched.  task_specific_tokens may be off (the pre-training config carries no task embeddings).
+ * VB200_ERR_CONFIG for visual_target != 0 or predict_feature (feature regression / NCE are not implemented: the masked-region head is
+ * the KL objective over v_target_size classes); VB200_ERR_INVALID for num_labels != 0.
+ * The engine has no task head: every forward, encode and cached entry point accepts a `select` of the pre-training heads
+ * (VB200_OUT_LINGUISIC_PREDICTION, VB200_OUT_VISION_PREDICTION), the taps and the attention maps, and returns VB200_ERR_INVALID, naming
+ * the head, for any bit of VB200_OUT_TASK_HEADS; so does vb200_decode_answers for every family.  vb200_model_dim("num_labels") and
+ * ("gqa_labels") are 0.  vb200_pretraining_heads and vb200_pretraining_objectives work as on any engine. */
+int vb200_create_pretraining(const char* config_json, int64_t n_tensors, const vb200_tensor* tensors, const vb200_options* opt,
+                             vb200_handle* out);
 int vb200_destroy(vb200_handle h);
 const char* vb200_last_error(vb200_handle h);
 
@@ -535,6 +549,38 @@ typedef struct {                   /* DEVICE outputs, each optional (NULL skips 
 } vb200_pretrain_out;
 
 int vb200_pretraining_heads(vb200_handle h, const vb200_pretrain_rows* in, const vb200_pretrain_out* out, void* cuda_stream);
+
+/* ---- The three pre-training objectives at the rows a caller lists (upstream BertForMultiModalPreTraining's losses, visual_target 0),
+ * from the same row lists and the same head launches as vb200_pretraining_heads (in->top_k must be 0).  With z the listed row's
+ * logits, bit-identical to that row of vb200_pretraining_heads:
+ *   token_loss[i]  = logsumexp(z) - z[token_labels[i]]                 (masked-token cross-entropy, text_rows[i])
+ *   region_loss[i] = sum_c t_c (log t_c - log_softmax(z)_c), 0 log 0 = 0, t = image_targets row i   (KL divergence as
+ *                    torch.nn.functional.kl_div computes it: a negative target gives NaN)
+ *   pair_loss[i]   = logsumexp(z) - z[pair_labels[i]]                  (alignment cross-entropy, pair_rows[i])
+ *   reduced[0..2]  = the mean of token_loss, region_loss and pair_loss: upstream's masked_lm_loss and next_sentence_loss
+ *                    (CrossEntropyLoss over the rows whose label is not -1) and masked_img_loss (the KL summed over the classes of the
+ *                    rows whose image_label is 1, divided by their count).  An empty list gives NaN (0 / 0, as upstream).
+ * One CTA per listed row reads that row's logits; one CTA sums each list in a fixed order, so repeated calls give the same bits.
+ * Every output is optional.  Everything is checked on the host before anything is enqueued: VB200_ERR_INVALID, naming the list or
+ * the label and the index, for the row-list faults of vb200_pretraining_heads, top_k != 0, a token label outside [0, vocab), a pair
+ * label other than 0 / 1, a NULL label list or target pointer for a non-empty list, a target or reduced pointer that is not 4-byte
+ * aligned.  Asynchronous on cuda_stream; rows and labels are staged as vb200_pretraining_heads stages its rows, so back-to-back calls
+ * need no synchronisation; no forward plan is built, used or evicted. */
+typedef struct {
+    const int32_t* token_labels;   /* HOST [n_t]: the vocabulary id of each text row */
+    const float* image_targets;    /* DEVICE fp32 [n_v, v_target_size]: the target distribution of each image row */
+    const int32_t* pair_labels;    /* HOST [n_p]: 0 / 1, the cross-entropy class of each pair row */
+} vb200_pretrain_targets;
+
+typedef struct {                   /* DEVICE fp32 outputs, each optional (NULL skips it) */
+    float* token_loss;             /* [n_t] */
+    float* region_loss;            /* [n_v] */
+    float* pair_loss;              /* [n_p] */
+    float* reduced;                /* [3]: masked_lm_loss, masked_img_loss, next_sentence_loss */
+} vb200_pretrain_losses;
+
+int vb200_pretraining_objectives(vb200_handle h, const vb200_pretrain_rows* in, const vb200_pretrain_targets* targets,
+                                 const vb200_pretrain_losses* out, void* cuda_stream);
 
 /* ---- Kernel-level entry points (device pointers), used by the parity tests and the roofline bench.  ---- */
 /* y = act(x[M,K] (16-bit) . w[N,K]^T (16-bit) + bias); act: 0 none, 1 GELU(erf), 2 ReLU.  residual, gamma and beta are reserved

@@ -132,6 +132,16 @@ class PretrainOut(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("token_logits", "region_logits", "alignment", "token_top", "region_top")]
 
 
+class PretrainTargets(C.Structure):
+    """vb200_pretrain_targets: HOST int32 token / pair labels, DEVICE fp32 image target rows of vb200_pretraining_objectives."""
+    _fields_ = [(n, C.c_void_p) for n in ("token_labels", "image_targets", "pair_labels")]
+
+
+class PretrainLosses(C.Structure):
+    """vb200_pretrain_losses: optional device fp32 outputs of vb200_pretraining_objectives."""
+    _fields_ = [(n, C.c_void_p) for n in ("token_loss", "region_loss", "pair_loss", "reduced")]
+
+
 class Options(C.Structure):
     _fields_ = [("device", C.c_int32), ("num_labels", C.c_int32), ("use_cuda_graph", C.c_int32),
                 ("use_pdl", C.c_int32), ("strict", C.c_int32), ("act_fp16", C.c_int32),
@@ -147,7 +157,7 @@ EXPORTS = ["vb200_abi_version", "vb200_create", "vb200_destroy", "vb200_last_err
            "vb200_self_attention_stream", "vb200_co_attention_stream",
            "vb200_linear_product", "vb200_text_embed", "vb200_image_pack", "vb200_region_pack", "vb200_rowdot", "vb200_gather_state",
            "vb200_gather_packed_state", "vb200_decode_answers", "vb200_decode_answers_host", "vb200_select_regions",
-           "vb200_pretraining_heads"]
+           "vb200_pretraining_heads", "vb200_create_pretraining", "vb200_pretraining_objectives"]
 
 _lib = None
 
@@ -222,6 +232,8 @@ def load():
     lib.vb200_decode_answers_host.argtypes = [vp, C.POINTER(DecodeMsg), i32, C.POINTER(Outputs), i32, i32, vp, C.POINTER(Answer), vp]
     lib.vb200_select_regions.argtypes = [vp, C.POINTER(Detections), i32, C.POINTER(SelectParams), C.POINTER(Selected), vp]
     lib.vb200_pretraining_heads.argtypes = [vp, C.POINTER(PretrainRows), C.POINTER(PretrainOut), vp]
+    lib.vb200_create_pretraining.argtypes = lib.vb200_create.argtypes
+    lib.vb200_pretraining_objectives.argtypes = [vp, C.POINTER(PretrainRows), C.POINTER(PretrainTargets), C.POINTER(PretrainLosses), vp]
     for name in EXPORTS:
         if name not in ("vb200_last_error",):
             getattr(lib, name).restype = C.c_int

@@ -305,6 +305,84 @@ gather_rows_kernel(const float* __restrict__ src, const int32_t* __restrict__ ro
     }
 }
 
+// Pre-training objectives (vb200_pretraining_objectives): one CTA per listed row of the three heads' compact logits, in list order
+// text | image | pair.  With z the row's logits, m = max z and s = sum exp(z - m), log_softmax(z)_c = (z_c - m) - log s:
+//   token / pair row: cross-entropy log s - (z_label - m);
+//   image row: KL(t || softmax z) = sum_c xlogy(t_c, t_c) - t_c log_softmax(z)_c (0 log 0 = 0), as torch.nn.functional.kl_div.
+// Each thread takes the columns tid, tid + 256, ... and the partial sums meet in a fixed shuffle tree, so a row's loss has the same
+// bits on every call.
+constexpr int kLossThreads = 256, kLossWarps = kLossThreads / 32;
+template <bool MAX>
+__device__ __forceinline__ float loss_block_reduce(float v, float* s_f) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    v = MAX ? warp_max(v) : warp_sum(v);
+    if (lane == 0) s_f[warp] = v;
+    __syncthreads();
+    const float w = lane < kLossWarps ? s_f[lane] : (MAX ? -INFINITY : 0.f);
+    v = MAX ? warp_max(w) : warp_sum(w);
+    __syncthreads();                                      // s_f is reused by the next reduction
+    return v;
+}
+
+// row r of list g (inlined once per list, so every field is read from the kernel parameters directly)
+__device__ __forceinline__ void loss_row(const LossRows& g, int r, float* s_f) {
+    const float* __restrict__ z = g.logits + static_cast<size_t>(r) * g.ld;
+    const int tid = threadIdx.x;
+    float m = -INFINITY;
+    for (int c = tid; c < g.N; c += kLossThreads) m = fmaxf(m, z[c]);
+    m = loss_block_reduce<true>(m, s_f);
+    float s = 0.f;
+    for (int c = tid; c < g.N; c += kLossThreads) s += expf(z[c] - m);
+    const float log_s = logf(loss_block_reduce<false>(s, s_f));
+    float loss;
+    if (g.targets != nullptr) {
+        const float* __restrict__ tr = g.targets + static_cast<size_t>(r) * g.N;
+        float k = 0.f;
+        for (int c = tid; c < g.N; c += kLossThreads) {
+            const float tc = tr[c];
+            k += (tc == 0.f ? 0.f : tc * logf(tc)) - tc * ((z[c] - m) - log_s);
+        }
+        loss = loss_block_reduce<false>(k, s_f);
+    } else {
+        loss = log_s - (z[g.labels[r]] - m);
+    }
+    if (tid == 0) g.loss[r] = loss;
+}
+
+__global__ void __launch_bounds__(kLossThreads)
+pretrain_loss_rows_kernel(LossRows t, LossRows v, LossRows p) {
+    __shared__ float s_f[kLossWarps];
+    const int r = blockIdx.x;
+    if (r < t.n) loss_row(t, r, s_f);
+    else if (r < t.n + v.n) loss_row(v, r - t.n, s_f);
+    else loss_row(p, r - t.n - v.n, s_f);
+}
+
+// The reduced objectives: reduced[k] = (sum of list k's row losses) / n_k, summed in double in a fixed order by one CTA; an empty list
+// gives 0 / 0 = NaN.
+__device__ __forceinline__ void loss_mean(const LossRows& g, float* out, double* s_d) {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    double a = 0.0;
+    for (int i = tid; i < g.n; i += 1024) a += static_cast<double>(g.loss[i]);
+    for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
+    if (lane == 0) s_d[warp] = a;
+    __syncthreads();
+    if (warp == 0) {
+        a = s_d[lane];
+        for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
+        if (lane == 0) *out = static_cast<float>(a / static_cast<double>(g.n));
+    }
+    __syncthreads();
+}
+
+__global__ void __launch_bounds__(1024)
+pretrain_loss_reduce_kernel(LossRows t, LossRows v, LossRows p, float* __restrict__ reduced) {
+    __shared__ double s_d[32];
+    loss_mean(t, reduced, s_d);
+    loss_mean(v, reduced + 1, s_d);
+    loss_mean(p, reduced + 2, s_d);
+}
+
 // one warp per row; n_out <= 4
 __global__ void __launch_bounds__(128)
 rowdot_kernel(const float* __restrict__ x, int ld_x, const float* __restrict__ W, const float* __restrict__ bias,
@@ -398,6 +476,21 @@ cudaError_t launch_gather_rows(const float* src, const int32_t* rows, int n, int
         case 2: gather_rows_kernel<2><<<grid, block, 0, st>>>(src, rows, n, rows_out, H, dst, ld_dst); break;
         default: gather_rows_kernel<3><<<grid, block, 0, st>>>(src, rows, n, rows_out, H, dst, ld_dst); break;
     }
+    return cudaGetLastError();
+}
+
+cudaError_t launch_pretrain_losses(const LossRows* g, float* reduced, cudaStream_t st) {
+    int64_t blocks = 0;
+    for (int k = 0; k < 3; ++k) {
+        const LossRows& x = g[k];
+        if (x.n < 0 || (x.n > 0 && (x.logits == nullptr || x.loss == nullptr || x.N < 1 || x.ld < x.N ||
+                                    ((k == 1) != (x.targets != nullptr)) || ((k != 1) != (x.labels != nullptr)))))
+            return cudaErrorInvalidValue;
+        blocks += x.n;
+    }
+    if (blocks > 0x7fffffff) return cudaErrorInvalidValue;
+    if (blocks > 0) pretrain_loss_rows_kernel<<<static_cast<unsigned>(blocks), kLossThreads, 0, st>>>(g[0], g[1], g[2]);
+    if (reduced != nullptr) pretrain_loss_reduce_kernel<<<1, 1024, 0, st>>>(g[0], g[1], g[2], reduced);
     return cudaGetLastError();
 }
 

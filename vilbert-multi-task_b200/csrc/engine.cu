@@ -161,6 +161,7 @@ struct Config {
     int v_feat = 2048, v_target = 1601, v_hidden = 1024, v_layers = 6, v_heads = 8, v_inter = 1024;
     int bi_hidden = 1024, bi_heads = 8;
     int task_tokens = 1, n_task = 20;
+    int visual_target = 0, predict_feature = 0;   // pre-training options: read here, accepted only at 0 by vb200_create_pretraining
     std::vector<int> v_bi_id{0, 1, 2, 3, 4, 5}, t_bi_id{6, 7, 8, 9, 10, 11};
     std::string hidden_act = "gelu", v_hidden_act = "gelu", fusion = "mul";
     float ln_eps = 1e-12f;
@@ -184,6 +185,7 @@ Config parse_config(const char* json) {
     geti("v_num_attention_heads", c.v_heads); geti("v_intermediate_size", c.v_inter);
     geti("bi_hidden_size", c.bi_hidden); geti("bi_num_attention_heads", c.bi_heads);
     geti("task_specific_tokens", c.task_tokens); geti("num_task_tokens", c.n_task);
+    geti("visual_target", c.visual_target); geti("predict_feature", c.predict_feature);
     auto geta = [&](const char* k, std::vector<int>& dst) {
         auto it = m.find(k);
         if (it == m.end() || it->second.kind != JVal::ARR) return;
@@ -625,9 +627,10 @@ constexpr int kMaxHeadRows = 1 << 20;   // rows per list of one call (the larges
 struct RowHeads {
     Plan pl;                       // workspace (pl.mem), launch list (pl.ops), GEMM scratch (pl.y_scratch[0]); B = 1, T = V = M
     int M = 0;
-    int* d_rows = nullptr;         // [1 + M]: count, then the rows
+    int* d_rows = nullptr;         // [1 + 2M]: count, then the rows, then (vb200_pretraining_objectives) their labels
     void* a = nullptr;             // [M, width]: 16-bit operand (x3: hi | lo | hi) of the transform GEMM, fp32 pooled rows (pair head)
     OutBuf logits;                 // [M, N] fp32, row stride logits.ld
+    float* loss = nullptr;         // [M]: each listed row's objective (vb200_pretraining_objectives)
 };
 
 }  // namespace
@@ -637,6 +640,9 @@ struct vb200_engine {
     Config cfg;
     vb200_options opt{};
     int num_labels = 0, gqa_labels = 0;
+    // vb200_create_pretraining: the checkpoint holds the encoder and the `cls` heads only.  No task head is loaded, and asking for one
+    // (a select bit, a decode family) is VB200_ERR_INVALID; num_labels and gqa_labels stay 0.
+    bool pretraining = false;
     bool dry = false;          // audit pass: check names / shapes / dtypes only, touch no device
     int lone_rows = 320;       // VB200_LONE_ROWS (0 = off): forwards with at most this many rows in either stream (batch <= 8 at the default
                                // shapes) run their plain GEMMs with 64-wide tiles while those still fit one CTA per SM
@@ -877,7 +883,7 @@ struct vb200_engine {
         }
         const Config& c = cfg;
         // vil_prediction width comes from the checkpoint unless the caller pins it (worker.py:523 passes 3129)
-        {
+        if (!pretraining) {
             auto it = sd.find("vil_prediction.logit_fc.3.weight");
             if (it == sd.end()) fail(VB200_ERR_CHECKPOINT, "checkpoint is missing key \"vil_prediction.logit_fc.3.weight\"");
             const int ck = static_cast<int>(it->second.shape[0]);
@@ -937,13 +943,15 @@ struct vb200_engine {
         }
         t_pool = load_linear1("bert.t_pooler.dense", c.bi_hidden, c.hidden);
         v_pool = load_linear1("bert.v_pooler.dense", c.bi_hidden, c.v_hidden);
-        vqa = load_cls("vil_prediction", c.bi_hidden, 2 * c.bi_hidden, num_labels, false);
-        gqa = load_cls("vil_prediction_gqa", c.bi_hidden, 2 * c.bi_hidden, gqa_labels, false);
-        binary = load_cls("vil_binary_prediction", 2 * c.bi_hidden, 2 * c.bi_hidden, 2, true);
-        vil_logit = load_row("vil_logit", 1, c.bi_hidden);
-        vil_tri = load_row("vil_tri_prediction", 3, c.bi_hidden);
-        vision_logit = load_row("vision_logit", 1, c.v_hidden);
-        ling_logit = load_row("linguisic_logit", 1, c.hidden);
+        if (!pretraining) {   // task heads; on a pre-training engine their keys are unexpected ones (strict) like any other
+            vqa = load_cls("vil_prediction", c.bi_hidden, 2 * c.bi_hidden, num_labels, false);
+            gqa = load_cls("vil_prediction_gqa", c.bi_hidden, 2 * c.bi_hidden, gqa_labels, false);
+            binary = load_cls("vil_binary_prediction", 2 * c.bi_hidden, 2 * c.bi_hidden, 2, true);
+            vil_logit = load_row("vil_logit", 1, c.bi_hidden);
+            vil_tri = load_row("vil_tri_prediction", 3, c.bi_hidden);
+            vision_logit = load_row("vision_logit", 1, c.v_hidden);
+            ling_logit = load_row("linguisic_logit", 1, c.hidden);
+        }
         seq_rel = load_row("cls.bi_seq_relationship", 2, c.bi_hidden);
         lm_transform = load_linear1("cls.predictions.transform.dense", c.hidden, c.hidden);
         lm_ln = load_ln("cls.predictions.transform.LayerNorm", c.hidden);
@@ -1099,12 +1107,30 @@ struct vb200_engine {
     enum PlanMode { FULL = 0, TEXT_PREFIX = 1, IMAGE_PREFIX = 2, SUFFIX = 3, PACKED = 4,
                     PACKED_TEXT_PREFIX = 5, PACKED_IMAGE_PREFIX = 6, PACKED_SUFFIX = 7 };
 
+    // A pre-training engine has no task head: every select bit of VB200_OUT_TASK_HEADS is rejected, naming the head.
+    static void reject_task_heads(uint32_t select) {
+        static const struct { uint32_t bit; const char* name; } heads[] = {
+            {VB200_OUT_VIL_PREDICTION, "vil_prediction (VB200_OUT_VIL_PREDICTION)"},
+            {VB200_OUT_VIL_PREDICTION_GQA, "vil_prediction_gqa (VB200_OUT_VIL_PREDICTION_GQA)"},
+            {VB200_OUT_VIL_LOGIT, "vil_logit (VB200_OUT_VIL_LOGIT)"},
+            {VB200_OUT_VIL_BINARY_PREDICTION, "vil_binary_prediction (VB200_OUT_VIL_BINARY_PREDICTION)"},
+            {VB200_OUT_VIL_TRI_PREDICTION, "vil_tri_prediction (VB200_OUT_VIL_TRI_PREDICTION)"},
+            {VB200_OUT_VISION_LOGIT, "vision_logit (VB200_OUT_VISION_LOGIT)"},
+            {VB200_OUT_LINGUISIC_LOGIT, "linguisic_logit (VB200_OUT_LINGUISIC_LOGIT)"},
+        };
+        for (const auto& h : heads)
+            if (select & h.bit)
+                fail(VB200_ERR_INVALID, "the task head %s is not part of a pre-training engine (select only the pre-training heads, "
+                     "taps or attention maps)", h.name);
+    }
+
     Plan* get_plan(int B, int Tin, int V, uint32_t select, int slot = 0, int mode = FULL, bool want_attn = false) {
         if (slot < 0 || slot > 15) fail(VB200_ERR_INVALID, "slot %d out of range (0..15)", slot);
         if (slot > 0 && !opt.use_cuda_graph) fail(VB200_ERR_INVALID, "concurrent slots need CUDA-graph plans (use_cuda_graph)");
         const bool packed = mode >= PACKED;
         const int schedule_mode = packed ? mode - PACKED : mode;     // which part of the schedule: FULL, a prefix or the suffix
         if (schedule_mode == TEXT_PREFIX || schedule_mode == IMAGE_PREFIX) { select = 0; want_attn = false; }
+        if (pretraining) reject_task_heads(select);
         const int T = Tin + (cfg.task_tokens ? 1 : 0);
         // ahead of the cache: a plan built under a higher max_rows_per_sample must not outlive the bound being lowered.  Packed
         // capacities are the call's longest rows rounded up to 16 (pack_batch has checked the rows themselves against the bound)
@@ -1717,6 +1743,9 @@ struct vb200_engine {
                 case VB200_DECODE_GROUNDING: field = "vision_logit"; src = out->vision_logit; rows = vision_rows; break;
                 default: fail(VB200_ERR_INVALID, "%s: message %d has unknown family %d", api, i, m.family);
             }
+            if (pretraining)
+                fail(VB200_ERR_INVALID, "%s: message %d (family %d) reads the task head %s, which is not part of a pre-training engine", api,
+                     i, m.family, field);
             if (src == nullptr) fail(VB200_ERR_INVALID, "%s: message %d (family %d) reads vb200_outputs.%s, which is NULL", api, i, m.family, field);
             const bool grounding = m.family == VB200_DECODE_GROUNDING;
             if (grounding && spatials == nullptr) fail(VB200_ERR_INVALID, "%s: message %d is a grounding message and spatials is NULL", api, i);
@@ -1893,7 +1922,8 @@ struct vb200_engine {
         Plan& pl = r->pl;
         pl.B = 1; pl.T = pl.V = M;
         r->M = M;
-        r->d_rows = pl.mem.alloc_n<int>(static_cast<size_t>(M) + 1);
+        r->d_rows = pl.mem.alloc_n<int>(2 * static_cast<size_t>(M) + 1);
+        r->loss = pl.mem.alloc_n<float>(M);
         const int* count = r->d_rows;
         const size_t S = x3 ? 3 : 1;
         if (head == kHeadPair) {
@@ -1921,49 +1951,37 @@ struct vb200_engine {
         slot = std::move(r);
         return *slot;
     }
-    void pretraining_heads(const vb200_pretrain_rows* in, const vb200_pretrain_out* out, cudaStream_t st) {
-        const char* api = "vb200_pretraining_heads";
-        if (in == nullptr || out == nullptr) fail(VB200_ERR_INVALID, "%s: in / out is NULL", api);
-        const int k = in->top_k;
-        if (k < 0 || k > VB200_DECODE_MAX_TOP) fail(VB200_ERR_INVALID, "%s: top_k %d outside [0, %d]", api, k, VB200_DECODE_MAX_TOP);
-        struct Group {
-            const char* list; const char* state; const float* src; int src_rows, width; int n; const int32_t* rows;
-            float* logits; int N; vb200_answer* top; const char* top_name;
-        };
-        Group g[3] = {
-            {"text_rows", "text_state", in->text_state, in->t_rows, cfg.hidden, in->n_t, in->text_rows, out->token_logits, cfg.vocab,
-             out->token_top, "token_top"},
-            {"image_rows", "image_state", in->image_state, in->v_rows, cfg.v_hidden, in->n_v, in->image_rows, out->region_logits,
-             cfg.v_target, out->region_top, "region_top"},
-            {"pair_rows", "pooled_state", in->pooled_state, in->p_rows, cfg.bi_hidden, in->n_p, in->pair_rows, out->alignment, 2, nullptr,
-             nullptr},
-        };
+    // One head's list of a vb200_pretraining_heads / vb200_pretraining_objectives call: the fp32 state it gathers from, the rows, the
+    // head's logits per row, the objectives' HOST labels (staged after the rows: token and pair heads) and whether any output reads it.
+    struct HeadGroup {
+        const char* list; const char* state; const float* src; int src_rows, width, n; const int32_t* rows; int N;
+        const int32_t* labels; bool run;
+    };
+    HeadGroup head_group(int head, const vb200_pretrain_rows& in) const {
+        if (head == kHeadText)
+            return {"text_rows", "text_state", in.text_state, in.t_rows, cfg.hidden, in.n_t, in.text_rows, cfg.vocab, nullptr, false};
+        if (head == kHeadImage)
+            return {"image_rows", "image_state", in.image_state, in.v_rows, cfg.v_hidden, in.n_v, in.image_rows, cfg.v_target, nullptr, false};
+        return {"pair_rows", "pooled_state", in.pooled_state, in.p_rows, cfg.bi_hidden, in.n_p, in.pair_rows, 2, nullptr, false};
+    }
+    static void check_group(const char* api, const HeadGroup& x) {
+        if (x.n < 0 || x.n > kMaxHeadRows) fail(VB200_ERR_INVALID, "%s: %s has a count of %d (must be in [0, %d])", api, x.list, x.n, kMaxHeadRows);
+        if (x.n == 0) return;
+        if (x.rows == nullptr) fail(VB200_ERR_INVALID, "%s: %s is NULL for %d rows", api, x.list, x.n);
+        if (x.src == nullptr) fail(VB200_ERR_INVALID, "%s: %s is NULL for a non-empty %s", api, x.state, x.list);
+        if (reinterpret_cast<uintptr_t>(x.src) & 15) fail(VB200_ERR_INVALID, "%s: %s is not 16-byte aligned", api, x.state);
+        for (int i = 0; i < x.n; ++i)
+            if (x.rows[i] < 0 || x.rows[i] >= x.src_rows)
+                fail(VB200_ERR_INVALID, "%s: %s[%d] = %d is outside the %d rows of %s", api, x.list, i, x.rows[i], x.src_rows, x.state);
+    }
+    // The RowHeads of every group that runs, with its count, rows and labels staged through the pinned pre_h into rh->d_rows, in stream
+    // order after the previous call (any stream) is done with the workspace.  Records pre_copied; the caller records pre_done.
+    void stage_rows(const HeadGroup (&g)[3], RowHeads* (&rh)[3], cudaStream_t st) {
         size_t staged = 0;
-        for (const Group& x : g) {
-            if (x.n < 0 || x.n > kMaxHeadRows)
-                fail(VB200_ERR_INVALID, "%s: %s has a count of %d (must be in [0, %d])", api, x.list, x.n, kMaxHeadRows);
-            if (x.top != nullptr && k == 0) fail(VB200_ERR_INVALID, "%s: %s is requested with top_k = 0", api, x.top_name);
-            if (x.top != nullptr && k > x.N)
-                fail(VB200_ERR_INVALID, "%s: top_k %d is above the %d logits of a %s row", api, k, x.N, x.top_name);
-            if (x.n == 0) continue;
-            if (x.rows == nullptr) fail(VB200_ERR_INVALID, "%s: %s is NULL for %d rows", api, x.list, x.n);
-            if (x.src == nullptr) fail(VB200_ERR_INVALID, "%s: %s is NULL for a non-empty %s", api, x.state, x.list);
-            if (reinterpret_cast<uintptr_t>(x.src) & 15) fail(VB200_ERR_INVALID, "%s: %s is not 16-byte aligned", api, x.state);
-            for (int i = 0; i < x.n; ++i)
-                if (x.rows[i] < 0 || x.rows[i] >= x.src_rows)
-                    fail(VB200_ERR_INVALID, "%s: %s[%d] = %d is outside the %d rows of %s", api, x.list, i, x.rows[i], x.src_rows, x.state);
-            if (x.logits != nullptr || x.top != nullptr) staged += 1 + static_cast<size_t>(x.n);
-        }
-        if (staged == 0) return;
-        CUDA_CHECK(cudaSetDevice(opt.device));
-        RowHeads* rh[3] = {nullptr, nullptr, nullptr};
-        std::vector<vb::DecodeDesc> descs;
         for (int i = 0; i < 3; ++i) {
-            if (g[i].n == 0 || (g[i].logits == nullptr && g[i].top == nullptr)) continue;
+            if (!g[i].run) continue;
             rh[i] = &row_heads_for(i, g[i].n);
-            if (g[i].top != nullptr)
-                for (int r = 0; r < g[i].n; ++r)
-                    descs.push_back(vb::DecodeDesc{rh[i]->logits.p + static_cast<size_t>(r) * rh[i]->logits.ld, nullptr, 0.0, 0.0, g[i].N, k});
+            staged += 1 + static_cast<size_t>(g[i].n) * (g[i].labels ? 2 : 1);
         }
         if (pre_copied == nullptr) CUDA_CHECK(cudaEventCreateWithFlags(&pre_copied, cudaEventDisableTiming));
         if (pre_done == nullptr) CUDA_CHECK(cudaEventCreateWithFlags(&pre_done, cudaEventDisableTiming));
@@ -1979,31 +1997,119 @@ struct vb200_engine {
         size_t at = 0;
         for (int i = 0; i < 3; ++i) {
             if (rh[i] == nullptr) continue;
+            const size_t n = static_cast<size_t>(g[i].n), len = 1 + n * (g[i].labels ? 2 : 1);
             pre_h[at] = g[i].n;
-            memcpy(pre_h + at + 1, g[i].rows, static_cast<size_t>(g[i].n) * sizeof(int32_t));
-            CUDA_CHECK(cudaMemcpyAsync(rh[i]->d_rows, pre_h + at, (1 + static_cast<size_t>(g[i].n)) * sizeof(int32_t),
-                                       cudaMemcpyHostToDevice, st));
-            at += 1 + static_cast<size_t>(g[i].n);
+            memcpy(pre_h + at + 1, g[i].rows, n * sizeof(int32_t));
+            if (g[i].labels) memcpy(pre_h + at + 1 + n, g[i].labels, n * sizeof(int32_t));
+            CUDA_CHECK(cudaMemcpyAsync(rh[i]->d_rows, pre_h + at, len * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+            at += len;
         }
         CUDA_CHECK(cudaEventRecord(pre_copied, st));
+    }
+    // One running group's gather and the forward's head launches: its logits land in r.logits.
+    void run_row_heads(int head, const HeadGroup& x, RowHeads& r, cudaStream_t st) {
+        const int rows_out = (x.n + 127) / 128 * 128;                // the rest of the last 128-row tile is zeroed
+        const int mode = head == kHeadPair ? 3 : (x3 ? 2 : (opt.act_fp16 ? 1 : 0));
+        const int ld = head == kHeadPair ? x.width : x.width * (x3 ? 3 : 1);
+        CUDA_CHECK(vb::launch_gather_rows(x.src, r.d_rows + 1, x.n, rows_out, x.width, r.a, ld, mode, st));
+        for (const Op& op : r.pl.ops) launch_op(op, st);
+    }
+    void pretraining_heads(const vb200_pretrain_rows* in, const vb200_pretrain_out* out, cudaStream_t st) {
+        const char* api = "vb200_pretraining_heads";
+        if (in == nullptr || out == nullptr) fail(VB200_ERR_INVALID, "%s: in / out is NULL", api);
+        const int k = in->top_k;
+        if (k < 0 || k > VB200_DECODE_MAX_TOP) fail(VB200_ERR_INVALID, "%s: top_k %d outside [0, %d]", api, k, VB200_DECODE_MAX_TOP);
+        float* logits[3] = {out->token_logits, out->region_logits, out->alignment};
+        vb200_answer* top[3] = {out->token_top, out->region_top, nullptr};
+        const char* top_name[3] = {"token_top", "region_top", nullptr};
+        HeadGroup g[3];
+        bool any = false;
+        for (int i = 0; i < 3; ++i) {
+            g[i] = head_group(i, *in);
+            if (top[i] != nullptr && k == 0) fail(VB200_ERR_INVALID, "%s: %s is requested with top_k = 0", api, top_name[i]);
+            if (top[i] != nullptr && k > g[i].N)
+                fail(VB200_ERR_INVALID, "%s: top_k %d is above the %d logits of a %s row", api, k, g[i].N, top_name[i]);
+            check_group(api, g[i]);
+            g[i].run = g[i].n > 0 && (logits[i] != nullptr || top[i] != nullptr);
+            any = any || g[i].run;
+        }
+        if (!any) return;
+        CUDA_CHECK(cudaSetDevice(opt.device));
+        RowHeads* rh[3] = {nullptr, nullptr, nullptr};
+        stage_rows(g, rh, st);
+        std::vector<vb::DecodeDesc> descs;
+        for (int i = 0; i < 3; ++i)
+            if (rh[i] != nullptr && top[i] != nullptr)
+                for (int r = 0; r < g[i].n; ++r)
+                    descs.push_back(vb::DecodeDesc{rh[i]->logits.p + static_cast<size_t>(r) * rh[i]->logits.ld, nullptr, 0.0, 0.0, g[i].N, k});
         const vb::DecodeDesc* dd = descs.empty() ? nullptr : stage_decode(descs, st);
         for (int i = 0; i < 3; ++i) {
             if (rh[i] == nullptr) continue;
-            RowHeads& r = *rh[i];
-            const Group& x = g[i];
-            const int rows_out = (x.n + 127) / 128 * 128;          // the rest of the last 128-row tile is zeroed
-            const int mode = i == kHeadPair ? 3 : (x3 ? 2 : (opt.act_fp16 ? 1 : 0));
-            const int ld = i == kHeadPair ? x.width : x.width * (x3 ? 3 : 1);
-            CUDA_CHECK(vb::launch_gather_rows(x.src, r.d_rows + 1, x.n, rows_out, x.width, r.a, ld, mode, st));
-            for (const Op& op : r.pl.ops) launch_op(op, st);
-            if (x.logits != nullptr)
-                CUDA_CHECK(cudaMemcpy2DAsync(x.logits, static_cast<size_t>(x.N) * 4, r.logits.p, static_cast<size_t>(r.logits.ld) * 4,
-                                             static_cast<size_t>(x.N) * 4, x.n, cudaMemcpyDeviceToDevice, st));
-            if (x.top != nullptr) {
-                CUDA_CHECK(vb::launch_answer_decode(dd, x.n, x.top, st));
+            const HeadGroup& x = g[i];
+            run_row_heads(i, x, *rh[i], st);
+            if (logits[i] != nullptr)
+                CUDA_CHECK(cudaMemcpy2DAsync(logits[i], static_cast<size_t>(x.N) * 4, rh[i]->logits.p,
+                                             static_cast<size_t>(rh[i]->logits.ld) * 4, static_cast<size_t>(x.N) * 4, x.n,
+                                             cudaMemcpyDeviceToDevice, st));
+            if (top[i] != nullptr) {
+                CUDA_CHECK(vb::launch_answer_decode(dd, x.n, top[i], st));
                 dd += x.n;
             }
         }
+        CUDA_CHECK(cudaEventRecord(pre_done, st));
+    }
+    // The three pre-training objectives at the listed rows: the heads of pretraining_heads, then one CTA per listed row computes its
+    // loss from the compact logits and one CTA reduces each list in a fixed order.
+    void pretraining_objectives(const vb200_pretrain_rows* in, const vb200_pretrain_targets* tg, const vb200_pretrain_losses* out,
+                                cudaStream_t st) {
+        const char* api = "vb200_pretraining_objectives";
+        if (in == nullptr || tg == nullptr || out == nullptr) fail(VB200_ERR_INVALID, "%s: in / targets / out is NULL", api);
+        if (in->top_k != 0) fail(VB200_ERR_INVALID, "%s: top_k %d (the objectives rank nothing: it must be 0)", api, in->top_k);
+        if (reinterpret_cast<uintptr_t>(out->reduced) & 3) fail(VB200_ERR_INVALID, "%s: reduced is not 4-byte aligned", api);
+        float* per_row[3] = {out->token_loss, out->region_loss, out->pair_loss};
+        HeadGroup g[3];
+        for (int i = 0; i < 3; ++i) {
+            g[i] = head_group(i, *in);
+            check_group(api, g[i]);
+            g[i].run = g[i].n > 0 && (per_row[i] != nullptr || out->reduced != nullptr);
+        }
+        const HeadGroup& t = g[kHeadText];
+        const HeadGroup& v = g[kHeadImage];
+        const HeadGroup& p = g[kHeadPair];
+        if (t.n > 0) {
+            if (tg->token_labels == nullptr) fail(VB200_ERR_INVALID, "%s: token_labels is NULL for %d text rows", api, t.n);
+            for (int i = 0; i < t.n; ++i)
+                if (tg->token_labels[i] < 0 || tg->token_labels[i] >= cfg.vocab)
+                    fail(VB200_ERR_INVALID, "%s: token_labels[%d] = %d is outside [0, %d)", api, i, tg->token_labels[i], cfg.vocab);
+        }
+        if (v.n > 0) {
+            if (tg->image_targets == nullptr) fail(VB200_ERR_INVALID, "%s: image_targets is NULL for %d image rows", api, v.n);
+            if (reinterpret_cast<uintptr_t>(tg->image_targets) & 3) fail(VB200_ERR_INVALID, "%s: image_targets is not 4-byte aligned", api);
+        }
+        if (p.n > 0) {
+            if (tg->pair_labels == nullptr) fail(VB200_ERR_INVALID, "%s: pair_labels is NULL for %d pair rows", api, p.n);
+            for (int i = 0; i < p.n; ++i)
+                if (tg->pair_labels[i] != 0 && tg->pair_labels[i] != 1)
+                    fail(VB200_ERR_INVALID, "%s: pair_labels[%d] = %d is not 0 or 1", api, i, tg->pair_labels[i]);
+        }
+        if (!t.run && !v.run && !p.run && out->reduced == nullptr) return;
+        g[kHeadText].labels = tg->token_labels;
+        g[kHeadPair].labels = tg->pair_labels;
+        CUDA_CHECK(cudaSetDevice(opt.device));
+        RowHeads* rh[3] = {nullptr, nullptr, nullptr};
+        stage_rows(g, rh, st);
+        vb::LossRows rows[3] = {};
+        for (int i = 0; i < 3; ++i) {
+            if (rh[i] == nullptr) continue;
+            run_row_heads(i, g[i], *rh[i], st);
+            rows[i] = vb::LossRows{rh[i]->logits.p, rh[i]->logits.ld, g[i].N, g[i].n,
+                                   g[i].labels ? rh[i]->d_rows + 1 + g[i].n : nullptr, i == kHeadImage ? tg->image_targets : nullptr,
+                                   rh[i]->loss};
+        }
+        CUDA_CHECK(vb::launch_pretrain_losses(rows, out->reduced, st));
+        for (int i = 0; i < 3; ++i)
+            if (rh[i] != nullptr && per_row[i] != nullptr)
+                CUDA_CHECK(cudaMemcpyAsync(per_row[i], rh[i]->loss, static_cast<size_t>(g[i].n) * 4, cudaMemcpyDeviceToDevice, st));
         CUDA_CHECK(cudaEventRecord(pre_done, st));
     }
     static float* out_ptr(const vb200_outputs& o, int slot) {
@@ -2076,15 +2182,22 @@ extern "C" {
 
 int vb200_abi_version(void) { return VB200_ABI_VERSION; }
 
-int vb200_create(const char* config_json, int64_t n_tensors, const vb200_tensor* tensors, const vb200_options* opt,
-                 vb200_handle* out) {
-    if (out == nullptr) { g_create_error = "vb200_create: out handle pointer is NULL"; return VB200_ERR_INVALID; }
+}  // extern "C"
+
+namespace {
+// vb200_create (multi-task checkpoint, every task head) and vb200_create_pretraining (encoder + `cls` heads): the same options, audit and
+// ingestion; `pretraining` selects the key set.
+int create_engine(const char* api, bool pretraining, const char* config_json, int64_t n_tensors, const vb200_tensor* tensors,
+                  const vb200_options* opt, vb200_handle* out) {
+    if (out == nullptr) { g_create_error = std::string(api) + ": out handle pointer is NULL"; return VB200_ERR_INVALID; }
     *out = nullptr;
     vb200_engine* eng = nullptr;
     int rc = guard(nullptr, [&] {
         if (tensors == nullptr || n_tensors <= 0) fail(VB200_ERR_CHECKPOINT, "empty state_dict");
         vb200_options o{};
         if (opt) o = *opt;
+        if (pretraining && o.num_labels != 0)
+            fail(VB200_ERR_INVALID, "%s: num_labels must be 0 (a pre-training checkpoint has no vil_prediction head)", api);
         if (o.ln_fold != 0) fail(VB200_ERR_INVALID, "vb200_options: the LayerNorm fold was removed (its reserved field must be 0)");
         if (o.fused_layernorm > 0)
             fail(VB200_ERR_INVALID, "vb200_options: the cluster-LayerNorm GEMM epilogue was removed (fused_layernorm must be 0 or negative)");
@@ -2096,15 +2209,20 @@ int vb200_create(const char* config_json, int64_t n_tensors, const vb200_tensor*
         o.split_fp32 = o.split_fp32 > 0 ? 1 : 0;
         o.act_fp16 = (o.act_fp16 >= 0 || o.split_fp32) ? 1 : 0;
         Config c = parse_config(config_json);
+        if (pretraining && c.visual_target != 0)
+            fail(VB200_ERR_CONFIG, "visual_target=%d is not supported (the masked-region head is the KL objective over v_target_size "
+                 "classes, visual_target 0)", c.visual_target);
+        if (pretraining && c.predict_feature) fail(VB200_ERR_CONFIG, "predict_feature=true is not supported (visual_target 0 only)");
         {   // audit the state_dict (names, shapes, dtypes, strictness) before touching any device
             vb200_engine audit;
-            audit.cfg = c; audit.opt = o; audit.dry = true; audit.x3 = o.split_fp32 != 0;
+            audit.cfg = c; audit.opt = o; audit.dry = true; audit.x3 = o.split_fp32 != 0; audit.pretraining = pretraining;
             audit.ingest(n_tensors, tensors);
         }
         require_device(o.device);
         eng = new vb200_engine();
         eng->cfg = c;
         eng->opt = o;
+        eng->pretraining = pretraining;
         eng->x3 = o.split_fp32 != 0;
         if (const char* v = getenv("VB200_LONE_ROWS")) eng->lone_rows = std::max(0, atoi(v));
         eng->max_plans = o.max_plans > 0 ? static_cast<size_t>(o.max_plans) : 24;
@@ -2126,6 +2244,19 @@ int vb200_create(const char* config_json, int64_t n_tensors, const vb200_tensor*
     if (rc != VB200_OK) { delete eng; return rc; }
     *out = eng;
     return VB200_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int vb200_create(const char* config_json, int64_t n_tensors, const vb200_tensor* tensors, const vb200_options* opt,
+                 vb200_handle* out) {
+    return create_engine("vb200_create", false, config_json, n_tensors, tensors, opt, out);
+}
+
+int vb200_create_pretraining(const char* config_json, int64_t n_tensors, const vb200_tensor* tensors, const vb200_options* opt,
+                             vb200_handle* out) {
+    return create_engine("vb200_create_pretraining", true, config_json, n_tensors, tensors, opt, out);
 }
 
 int vb200_destroy(vb200_handle h) {
@@ -2368,6 +2499,12 @@ int vb200_select_regions(vb200_handle h, const vb200_detections* imgs, int32_t n
 int vb200_pretraining_heads(vb200_handle h, const vb200_pretrain_rows* in, const vb200_pretrain_out* out, void* cuda_stream) {
     if (h == nullptr) return VB200_ERR_INVALID;
     return guard(h, [&] { h->pretraining_heads(in, out, static_cast<cudaStream_t>(cuda_stream)); });
+}
+
+int vb200_pretraining_objectives(vb200_handle h, const vb200_pretrain_rows* in, const vb200_pretrain_targets* targets,
+                                 const vb200_pretrain_losses* out, void* cuda_stream) {
+    if (h == nullptr) return VB200_ERR_INVALID;
+    return guard(h, [&] { h->pretraining_objectives(in, targets, out, static_cast<cudaStream_t>(cuda_stream)); });
 }
 
 int vb200_attention_layout(vb200_handle h, int32_t batch, int32_t n_tokens, int32_t n_regions, int32_t max_entries,

@@ -144,6 +144,12 @@ cudaError_t launch_attention_f32(const void* q, int ld_q, const void* k, const v
 // [n, rows_out) are zeroed.  H a multiple of 8 (64 in mode 2), 16-byte aligned src / dst; rows are bounds-checked on the host.
 cudaError_t launch_gather_rows(const float* src, const int32_t* rows, int n, int rows_out, int H, void* dst, int ld_dst, int mode,
                                cudaStream_t st);
+// Pre-training objectives: per listed row i < n of a head's fp32 logits [n, N] (row stride ld), loss[i] = the cross-entropy
+// logsumexp(z) - z[labels[i]] (labels: device int32, token and pair heads) or KL(targets[i] || softmax z) (targets: device fp32 [n, N],
+// image head); g = {token, image, pair}.  With `reduced` (device fp32 [3]) reduced[k] = mean of list k's losses (NaN for n_k = 0),
+// in a fixed order.  Labels are range-checked on the host.
+struct LossRows { const float* logits; int ld, N, n; const int32_t* labels; const float* targets; float* loss; };
+cudaError_t launch_pretrain_losses(const LossRows* g, float* reduced, cudaStream_t st);
 // K8 (narrow heads): out[m, j] = dot(x[m, :K], W[j, :K]) + b[j] + (add ? add[m] : 0), j < n_out <= 4.
 cudaError_t launch_rowdot(const float* x, int ld_x, const float* W, const float* b, const float* add, float* out,
                           int ld_out, int M, int K, int n_out, int pdl, cudaStream_t st, const int* m_rows = nullptr);

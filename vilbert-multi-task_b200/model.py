@@ -100,6 +100,8 @@ def split_packed_attention(flat, layout, t_rows, v_rows):
 class VILBertForVLTasks(object):
     """Drop-in for ``vilbert.vilbert.VILBertForVLTasks`` on the inference path the worker uses."""
 
+    _create_fn = "vb200_create"            # the C ABI constructor of this model's checkpoint kind
+
     def __init__(self, config: BertConfig, num_labels: int = 3129, state_dict=None, default_gpu: bool = True,
                  use_cuda_graph: bool = True, use_pdl: Optional[bool] = None, strict: bool = True, compute_dtype: str = "fp16",
                  fused_layernorm: bool = False, return_attention: bool = False, max_plans: int = 0, max_rows_per_sample: int = 256):
@@ -214,7 +216,7 @@ class VILBertForVLTasks(object):
         opt.max_plans = self._opts["max_plans"]
         h = C.c_void_p()
         with torch.cuda.device(device):
-            rc = lib.vb200_create(self._config_json(), len(self._sd), arr, C.byref(opt), C.byref(h))
+            rc = getattr(lib, self._create_fn)(self._config_json(), len(self._sd), arr, C.byref(opt), C.byref(h))
         L.check(rc, None)
         self._handle, self._device = h, device
         L.check(lib.vb200_set_option(h, b"max_rows_per_sample", self._opts["max_rows_per_sample"]), h)
@@ -636,35 +638,15 @@ class VILBertForVLTasks(object):
         first, equal probabilities ranking the lower index first -- computed on the device, like everything else here, so the call
         returns as soon as its work is enqueued."""
         device = self._engine_device()
-        d = self._dims
-        # (list, its rows, tap, width, logits columns, vb200_pretrain_rows fields: state, state rows, count, list; outputs: logits, top)
-        groups = (("text_rows", text_rows, "sequence_output_t", d["hidden_size"], d["vocab_size"],
-                   ("text_state", "t_rows", "n_t", "text_rows"), ("token_logits", "token_top")),
-                  ("image_rows", image_rows, "sequence_output_v", d["v_hidden_size"], d["v_target_size"],
-                   ("image_state", "v_rows", "n_v", "image_rows"), ("region_logits", "region_top")),
-                  ("pair_rows", pair_rows, "pooled_output", d["bi_hidden_size"], 2,
-                   ("pooled_state", "p_rows", "n_p", "pair_rows"), ("alignment", None)))
-        inp, out = L.PretrainRows(), L.PretrainOut()
+        inp, groups, keep = self._pretrain_rows("pretraining_heads", taps, text_rows, image_rows, pair_rows, device)
         inp.top_k = int(top_k)
-        res, keep = {}, []
-        for name, rows, tap, width, n_out, fields, (logits, top) in groups:
-            if rows is None:
-                continue
-            rows = _host_ints(rows)
-            state = taps.get(tap)
-            if state is None:
-                raise ValueError(f"pretraining_heads: {name} needs the {tap} tap")
-            if state.dtype != torch.float32 or state.device != device or not state.is_contiguous() or state.shape[-1] != width:
-                raise ValueError(f"pretraining_heads: {tap} must be a contiguous fp32 [..., {width}] tensor on {device}")
-            state = state.view(-1, width)
-            arr = _int32s(rows)
-            keep += [state, arr]
-            for field, value in zip(fields, (state.data_ptr(), state.shape[0], len(rows), arr)):
-                setattr(inp, field, value)
-            res[logits] = torch.empty(len(rows), n_out, dtype=torch.float32, device=device)
+        out = L.PretrainOut()
+        res = {}
+        for n, n_out, (logits, top) in groups:
+            res[logits] = torch.empty(n, n_out, dtype=torch.float32, device=device)
             setattr(out, logits, res[logits].data_ptr())
             if top is not None and top_k:
-                res[top] = torch.empty(len(rows), C.sizeof(L.Answer) // 4, dtype=torch.int32, device=device)
+                res[top] = torch.empty(n, C.sizeof(L.Answer) // 4, dtype=torch.int32, device=device)
                 setattr(out, top, res[top].data_ptr())
         self._call("vb200_pretraining_heads", C.byref(inp), C.byref(out))
         k = int(top_k)
@@ -672,6 +654,77 @@ class VILBertForVLTasks(object):
             ans = res.get(head + "_top")
             if ans is not None:            # vb200_answer as int32 words: n, index[10], prob[10], box[10][4]
                 res[head + "_top"] = (ans[:, 1:1 + k], ans[:, 1 + L.DECODE_MAX_TOP:1 + L.DECODE_MAX_TOP + k].view(torch.float32))
+        return res
+
+    def _pretrain_rows(self, api, taps, text_rows, image_rows, pair_rows, device):
+        """vb200_pretrain_rows of the lists given (None: not part of the call) over the taps' flattened states; returns it, one
+        ``(count, logits columns, (logits output, top output))`` per list given, and the host arrays the struct points to."""
+        d = self._dims
+        # (list, its rows, tap, width, logits columns, vb200_pretrain_rows fields: state, state rows, count, list; outputs: logits, top)
+        specs = (("text_rows", text_rows, "sequence_output_t", d["hidden_size"], d["vocab_size"],
+                  ("text_state", "t_rows", "n_t", "text_rows"), ("token_logits", "token_top")),
+                 ("image_rows", image_rows, "sequence_output_v", d["v_hidden_size"], d["v_target_size"],
+                  ("image_state", "v_rows", "n_v", "image_rows"), ("region_logits", "region_top")),
+                 ("pair_rows", pair_rows, "pooled_output", d["bi_hidden_size"], 2,
+                  ("pooled_state", "p_rows", "n_p", "pair_rows"), ("alignment", None)))
+        inp, groups, keep = L.PretrainRows(), [], []
+        for name, rows, tap, width, n_out, fields, outputs in specs:
+            if rows is None:
+                continue
+            rows = _host_ints(rows)
+            state = taps.get(tap)
+            if state is None:
+                raise ValueError(f"{api}: {name} needs the {tap} tap")
+            if state.dtype != torch.float32 or state.device != device or not state.is_contiguous() or state.shape[-1] != width:
+                raise ValueError(f"{api}: {tap} must be a contiguous fp32 [..., {width}] tensor on {device}")
+            state = state.view(-1, width)
+            arr = _int32s(rows)
+            keep += [state, arr]
+            for field, value in zip(fields, (state.data_ptr(), state.shape[0], len(rows), arr)):
+                setattr(inp, field, value)
+            groups.append((len(rows), n_out, outputs))
+        return inp, groups, keep
+
+    @torch.no_grad()
+    def pretraining_objectives(self, taps, text_rows=None, token_labels=None, image_rows=None, image_targets=None, pair_rows=None,
+                               pair_labels=None):
+        """The three pre-training objectives at the rows a caller lists (vb200_pretraining_objectives), on the device: the heads of
+        ``pretraining_heads`` at those rows, then each row's loss from its logits and each list's mean.  ``taps`` and the row lists
+        are as for ``pretraining_heads``; ``token_labels`` gives one vocabulary id per text row, ``image_targets`` one
+        [v_target_size] target distribution per image row (any float tensor, [n_v, v_target_size]), ``pair_labels`` one 0 / 1 class
+        per pair row.
+
+        Returns a dict of device tensors: ``token_loss`` [n_t] (masked-token cross-entropy), ``region_loss`` [n_v] (KL divergence of
+        the target from the row's softmax, as ``torch.nn.functional.kl_div`` computes it), ``pair_loss`` [n_p] (alignment
+        cross-entropy), and ``masked_lm_loss``, ``masked_img_loss``, ``next_sentence_loss`` ([1] each): the mean of each list, NaN for
+        an empty list, as upstream's losses are for batches without a masked token, region or labelled pair."""
+        device = self._engine_device()
+        lists = (text_rows, image_rows, pair_rows)
+        inp, _, keep = self._pretrain_rows("pretraining_objectives", taps, *lists, device)
+        n_t, n_v, n_p = (len(_host_ints(r)) if r is not None else 0 for r in lists)
+        tg = L.PretrainTargets()
+        for field, labels, n in (("token_labels", token_labels, n_t), ("pair_labels", pair_labels, n_p)):
+            if n:
+                values = _host_ints(labels if labels is not None else [])
+                if len(values) != n:
+                    raise ValueError(f"pretraining_objectives: {field} needs one label per row ({n}), got {len(values)}")
+                arr = _int32s(values)
+                keep.append(arr)
+                setattr(tg, field, arr)
+        if n_v:
+            t = _to_device(image_targets, torch.float32, device) if image_targets is not None else None
+            if t is None or tuple(t.shape) != (n_v, self._dims["v_target_size"]):
+                raise ValueError(f"pretraining_objectives: image_targets must be [{n_v}, {self._dims['v_target_size']}]")
+            keep.append(t)
+            tg.image_targets = t.data_ptr()
+        res = {"token_loss": torch.empty(n_t, dtype=torch.float32, device=device),
+               "region_loss": torch.empty(n_v, dtype=torch.float32, device=device),
+               "pair_loss": torch.empty(n_p, dtype=torch.float32, device=device)}
+        reduced = torch.empty(3, dtype=torch.float32, device=device)
+        out = L.PretrainLosses(*(res[k].data_ptr() if res[k].numel() else None for k in ("token_loss", "region_loss", "pair_loss")),
+                               reduced.data_ptr())
+        self._call("vb200_pretraining_objectives", C.byref(inp), C.byref(tg), C.byref(out))
+        res.update(masked_lm_loss=reduced[0:1], masked_img_loss=reduced[1:2], next_sentence_loss=reduced[2:3])
         return res
 
     # ------------------------------------------------------------------ detector-region selection (worker.py:123-176)

@@ -120,6 +120,49 @@ def synthetic_state_dict(config: BertConfig, num_labels: int = 3129, gqa_labels:
     return sd
 
 
+# the task heads of a multi-task checkpoint: absent from a pre-training one (upstream BertForMultiModalPreTraining has bert + cls)
+TASK_HEAD_PREFIXES = ("vil_prediction.", "vil_prediction_gqa.", "vil_binary_prediction.", "vil_logit.", "vil_tri_prediction.",
+                      "vision_logit.", "linguisic_logit.")
+
+
+def synthetic_pretraining_state_dict(config: BertConfig, seed: int = 42, bf16_exact: bool = True) -> Dict[str, torch.Tensor]:
+    """Random-init pre-training checkpoint (``bert.*`` and ``cls.*``, no task heads) drawn as ``synthetic_state_dict``.  The
+    config must have ``task_specific_tokens`` off, as upstream's pre-training config does (no task embedding table)."""
+    if getattr(config, "task_specific_tokens", False):
+        raise ValueError("a pre-training checkpoint has no task embeddings: set task_specific_tokens = False")
+    sd = synthetic_state_dict(config, num_labels=2, gqa_labels=2, seed=seed, bf16_exact=bf16_exact)
+    return {k: v for k, v in sd.items() if not k.startswith(TASK_HEAD_PREFIXES)}
+
+
+def synthetic_masked_batch(batch: int, n_tokens: int = 36, n_regions: int = 37, seed: int = 0, vocab_size: int = 30522,
+                           v_feature_size: int = 2048, v_target_size: int = 1601, mask_prob: float = 0.15):
+    """A masked pre-training batch shaped like upstream's Conceptual Captions loader output, for BertForMultiModalPreTraining.forward:
+    dict of ``input_ids`` / ``token_type_ids`` / ``attention_mask`` [B, n_tokens], ``image_feat`` [B, V, F] / ``image_loc`` [B, V, 5]
+    / ``image_attention_mask`` [B, V] (V = n_regions, the global row first), ``masked_lm_labels`` [B, n_tokens] (the original id at
+    about ``mask_prob`` of the word tokens, now [MASK] = 103; -1 elsewhere), ``image_label`` [B, V - 1] (1 at about ``mask_prob`` of
+    the regions, whose features are zeroed; -1 elsewhere), ``image_target`` [B, V - 1, v_target_size] (detector class distributions:
+    softmax rows with some classes exactly 0, renormalised) and ``next_sentence_label`` [B] (0 / 1, some -1)."""
+    B, V = batch, n_regions
+    q, feats, spatials, segment_ids, input_mask, image_mask, _, _ = synthetic_request(
+        B, n_tokens, V, seed=seed, v_feature_size=v_feature_size, vocab_size=vocab_size, full_masks=False)
+    g = torch.Generator().manual_seed(seed + 1)
+    words = (q != 101) & (q != 102) & (input_mask == 1)
+    masked = words & (torch.rand(q.shape, generator=g) < mask_prob)
+    lm_labels = torch.where(masked, q, torch.full_like(q, -1))
+    q = torch.where(masked, torch.full_like(q, 103), q)
+    region = torch.rand(B, V - 1, generator=g) < mask_prob
+    image_label = torch.where(region, torch.ones(B, V - 1, dtype=torch.long), torch.full((B, V - 1), -1, dtype=torch.long))
+    feats[:, 1:][region] = 0.0
+    target = torch.softmax(torch.randn(B, V - 1, v_target_size, generator=g) * 3.0, dim=-1)
+    target = target * (torch.rand(B, V - 1, v_target_size, generator=g) > 0.2)
+    target = target / target.sum(-1, keepdim=True)
+    nsp = torch.randint(0, 2, (B,), generator=g)
+    nsp[torch.rand(B, generator=g) < 0.1] = -1
+    return dict(input_ids=q, image_feat=feats, image_loc=spatials, token_type_ids=segment_ids, attention_mask=input_mask,
+                image_attention_mask=image_mask, masked_lm_labels=lm_labels, image_label=image_label, image_target=target,
+                next_sentence_label=nsp)
+
+
 def synthetic_detections(n_images: int, n_proposals=1000, n_classes: int = 1601, feature_size: int = 2048, seed: int = 0,
                          margin: Optional[float] = None, n_clusters: int = 12, n_dominant: int = 24, im_scale: float = 1.6):
     """Raw detector heads per image, shaped like the Faster R-CNN outputs the reference worker's feature extraction reads
