@@ -76,6 +76,10 @@ def main():
         ("vqa_fc0_gelu_f32", B, 2048, 1024, 1, True, 0), ("vqa_fc3", B, 3129, 2048, 0, False, 0),
         ("plain_text_ffn_out", Mt, 768, 3072, 0, False, 0), ("plain_img_out", Mv, 1024, 1024, 0, False, 0),
         ("plain_text_attn_out", Mt, 768, 768, 0, False, 0),
+        # the pruned tails of the last text and image layer: one row per sample
+        ("tail_text_attn_out_f32", B, 768, 768, 0, True, 0), ("tail_text_ffn_in_gelu", B, 3072, 768, 1, False, 0),
+        ("tail_text_ffn_out_f32", B, 768, 3072, 0, True, 0), ("tail_img_attn_out_f32", B, 1024, 1024, 0, True, 0),
+        ("tail_img_ffn_in_gelu", B, 1024, 1024, 1, False, 0), ("tail_img_ffn_out_f32", B, 1024, 1024, 0, True, 0),
     ]
     res = []
     for name, M, N, K, actf, f32, bn in gemms:

@@ -403,7 +403,7 @@ struct Op {
     int ld_x = 0, ld_out = 0, M = 0, K = 0, n_out = 0;
     // packed plans: device row count of the GEMM / LayerNorm / rowdot rows (ep.m_rows for GEMMs), per-sample row offsets of
     // the attention operands (offs_a: La stream, offs_b: Lb stream); GATHER: row offs_a[b] of qkv_a (16-bit, ld_a wide) -> row b
-    // of ctx_a, b < B, clamped to M rows
+    // of ctx_a, b < B, clamped to M rows, and with x non-null the same row of x (fp32, `hidden` wide) -> row b of out
     const int* m_rows = nullptr;
     const int *offs_a = nullptr, *offs_b = nullptr;
     // SELF_ATTN / CO_ATTN: the streaming kernels (a stream the op reads has more than 256 rows per sample in this plan)
@@ -580,6 +580,9 @@ struct Plan {
     float* v_f32[2]; bf16* v_b16[2];
     float* y_scratch[2] = {nullptr, nullptr};   // per-stream fp32 GEMM output feeding the row LayerNorm kernel
     int t_cur = 0, v_cur = 0;
+    // pruned tail of a stream (get_plan): its last layer's compact 16-bit output [B, hidden], each sample's first row; null when the
+    // stream's full final rows are in t_b16[t_cur] / v_b16[v_cur]
+    bf16 *tail_t = nullptr, *tail_v = nullptr;
     std::vector<Op> ops;
     OutBuf outs[12];
     struct AttnOut { float* p; int heads, Lq, Lk; };   // attention probabilities [B, heads, Lq, Lk] in schedule order
@@ -1026,7 +1029,11 @@ struct vb200_engine {
         // supports (not the fp32-parity, pooled-product or ragged-N ones) whose outputs the TMA can store.
         // It takes the tile width chosen above, 128 even where that leaves one tile per CTA: 64-wide ping-pong tiles measured slower on H100 SXM
         // (700 W, bf16, 16-bit output, scripts/kernel_bench.py) at 1984x768x768 (9.74 vs 8.20 us), 1984x768x3072 (29.19 vs 20.32) and
-        // 2304x1024x1024 (16.71 vs 15.88), and only 4 % faster with GELU at 2304x1024x1024 (18.04 vs 18.81).
+        // 2304x1024x1024 (16.71 vs 15.88), and only 4 % faster with GELU at 2304x1024x1024 (18.04 vs 18.81).  The single-panel
+        // launches of a batch-64 forward (poolers, fc0, the pruned tails) keep 128 too: 64-wide was slower at 64x768x768 (8.71 vs
+        // 8.45 / 8.41 us, two 128-wide runs), 64x3072x768 GELU (9.54 vs 9.13 / 9.07), 64x1024x1024 (10.18 vs 10.04 / 9.97; GELU 10.40
+        // vs 10.21 / 10.10), 64x1024x768 ReLU (8.53 vs 8.08 / 8.05) and 64x2048x1024 GELU (10.57 vs 10.47 / 10.42), and 2 % faster
+        // only at 64x768x3072 (20.74 vs 21.23 / 21.12); same card, bf16.
         op.pingpong = gemm_kernel == 1 && tma_store_enabled && !x3 && vb::gemm_pingpong_supports(e, op.block_n) &&
                       setup_pingpong_store(&op.tc, &op.tc32, e);
         if (tma_store_enabled && !op.pingpong) setup_tma_store(&op.tc, e);
@@ -1107,6 +1114,14 @@ struct vb200_engine {
     enum PlanMode { FULL = 0, TEXT_PREFIX = 1, IMAGE_PREFIX = 2, SUFFIX = 3, PACKED = 4,
                     PACKED_TEXT_PREFIX = 5, PACKED_IMAGE_PREFIX = 6, PACKED_SUFFIX = 7 };
 
+    // Plan-key bits above the public select bits: the call reads every final text / image row (its sequence_output_t / _v tap).
+    // A forward whose select and taps read no final row of a stream prunes that stream's tail (get_plan).
+    static constexpr uint32_t kTextRows = 1u << 30, kImageRows = 1u << 31;
+    static uint32_t rows_read(const vb200_outputs* out) {
+        if (out == nullptr) return 0;
+        return (out->sequence_output_t ? kTextRows : 0) | (out->sequence_output_v ? kImageRows : 0);
+    }
+
     // A pre-training engine has no task head: every select bit of VB200_OUT_TASK_HEADS is rejected, naming the head.
     static void reject_task_heads(uint32_t select) {
         static const struct { uint32_t bit; const char* name; } heads[] = {
@@ -1165,6 +1180,16 @@ struct vb200_engine {
         const bool full = schedule_mode == FULL;
         const bool do_t = full || schedule_mode == TEXT_PREFIX, do_v = full || schedule_mode == IMAGE_PREFIX;
         const bool do_s = full || schedule_mode == SUFFIX;
+        // Pruned tail: the poolers read one row per sample of each final state.  A stream no per-row head and no tap reads runs its
+        // last layer's row-local half (everything after the self-attention) on those B rows only; bit-identical rows, since no
+        // kernel's per-element result depends on M.  A stream whose last layer is a connection layer keeps its full rows.
+        const bool prune_t = do_s && !(select & (kTextRows | VB200_OUT_LINGUISIC_PREDICTION | VB200_OUT_LINGUISIC_LOGIT));
+        const bool prune_v = do_s && !(select & (kImageRows | VB200_OUT_VISION_PREDICTION | VB200_OUT_VISION_LOGIT));
+        size_t last_t = 0, last_v = 0;                 // the last schedule step writing each stream
+        for (size_t i = 0; i < schedule.size(); ++i) {
+            if (schedule[i][0] != 'V') last_t = i;
+            if (schedule[i][0] != 'T') last_v = i;
+        }
         pl.kp = img_emb.ldw;
         pl.img_a = pl.mem.alloc_n<bf16>(static_cast<size_t>(Mv) * pl.kp * S);
         pl.mask_t = pl.mem.alloc_n<float>(Mt);
@@ -1220,8 +1245,10 @@ struct vb200_engine {
             add_linear(pl, pl.img_a, Mv, pl.kp, img_emb, vb::kActNone, nullptr, 0, &vemb_ln, pl.v_b16[0], Hv, pl.v_f32[0], Hv,
                        1, Op::NONE, nullptr, 0, vs.m_rows);   // side stream: overlaps the text layers ahead of the first co-attention
 
-        // one BertLayer / BertImageLayer
-        auto single_layer = [&](const LayerW& L, StreamSt& st, int inter, int heads) {
+        // one BertLayer / BertImageLayer.  `tail` (the pruned tail): Q, K, V and the attention on every row (each is a key and a
+        // value), the rest on each sample's first row -- read at stride seq rows on dense plans, gathered from the sample offsets on
+        // packed ones -- into compact [B, hid] rows; returns their 16-bit copy (null without `tail`).
+        auto single_layer = [&](const LayerW& L, StreamSt& st, int inter, int heads, bool tail) -> bf16* {
             const int hid = st.hid, cur = st.cur, M = st.rows, stream = st.stream;
             bf16* qb; float* qf;
             qkv_out(st.qkv, qb, qf);
@@ -1241,18 +1268,41 @@ struct vb200_engine {
             if (x3 || want_attn)
                 add_attn_f32(pl, qkv_at(st.qkv, 0), 3 * hid, qkv_at(st.qkv, hid), qkv_at(st.qkv, 2 * hid), 3 * hid, st.mask, st.seq, st.seq,
                              heads, hid, st.ctx, want_attn, stream, st.offs, st.offs, stream);   // prefix: stream 0 T^2, 1 V^2
+            if (tail) {
+                const bf16* ctx = st.ctx;
+                const float* res = st.f32[cur];
+                int ld = st.seq * hid;
+                if (pl.packed) {
+                    bf16* ctx_c = pl.mem.alloc_n<bf16>(static_cast<size_t>(B) * hid * S);
+                    float* res_c = pl.mem.alloc_n<float>(static_cast<size_t>(B) * hid);
+                    Op g{};
+                    g.kind = Op::GATHER; g.stream = stream; g.B = B; g.offs_a = st.offs; g.M = M;
+                    g.qkv_a = st.ctx; g.ctx_a = ctx_c; g.ld_a = static_cast<int>(hid * S); g.x = res; g.out = res_c; g.hidden = hid;
+                    ops.push_back(g);
+                    ctx = ctx_c; res = res_c; ld = hid;
+                }
+                float* ln1_f = pl.mem.alloc_n<float>(static_cast<size_t>(B) * hid);
+                bf16* ln1_b = pl.mem.alloc_n<bf16>(static_cast<size_t>(B) * hid * S);
+                bf16* out_b = pl.mem.alloc_n<bf16>(static_cast<size_t>(B) * hid * S);
+                add_linear(pl, ctx, B, ld, L.attn_out, vb::kActNone, res, ld, &L.ln1, ln1_b, hid, ln1_f, hid, stream);
+                add_linear(pl, ln1_b, B, hid, L.inter, vb::kActGelu, nullptr, 0, nullptr, st.inter, inter, nullptr, 0, stream);
+                add_linear(pl, st.inter, B, inter, L.out, vb::kActNone, ln1_f, hid, &L.ln2, out_b, hid, nullptr, 0, stream);
+                return out_b;                // no fp32 copy: nothing reads the pruned stream's final fp32 rows
+            }
             // attention output + LayerNorm1 (residual: the layer input) -> buffers [1 - cur]
             ln_linear(st, st.ctx, hid, L.attn_out, L.ln1, cur, 1 - cur, Op::NONE);
             add_linear(pl, st.b16[1 - cur], M, hid, L.inter, vb::kActGelu, nullptr, 0, nullptr, st.inter, inter, nullptr, 0, stream,
                        Op::NONE, nullptr, 0, st.m_rows);
             // FFN output + LayerNorm2 (residual: LayerNorm1's output) -> buffers [cur]
             ln_linear(st, st.inter, inter, L.out, L.ln2, 1 - cur, cur, Op::NONE);
+            return nullptr;
         };
 
         for (Op& op : ops) op.tag = "embed";
         bool in_suffix = false;
         size_t tagged = ops.size();
-        for (const std::string& step : schedule) {
+        for (size_t si = 0; si < schedule.size(); ++si) {
+            const std::string& step = schedule[si];
             for (; tagged < ops.size(); ++tagged) if (ops[tagged].tag == nullptr) ops[tagged].tag = "?";
             const int idx = atoi(step.c_str() + 1);
             if (step[0] == 'C') in_suffix = true;
@@ -1261,9 +1311,9 @@ struct vb200_engine {
                 ~Tagger() { for (size_t i = from; i < ops.size(); ++i) ops[i].tag = name; }
             } tagger{ops, ops.size(), step.c_str()};
             if (step[0] == 'T') {
-                if (in_suffix ? do_s : do_t) single_layer(t_layers[idx], ts, c.inter, c.heads);
+                if (in_suffix ? do_s : do_t) pl.tail_t = single_layer(t_layers[idx], ts, c.inter, c.heads, prune_t && si == last_t);
             } else if (step[0] == 'V') {
-                if (in_suffix ? do_s : do_v) single_layer(v_layers[idx], vs, c.v_inter, c.v_heads);
+                if (in_suffix ? do_s : do_v) pl.tail_v = single_layer(v_layers[idx], vs, c.v_inter, c.v_heads, prune_v && si == last_v);
             } else if (do_s) {
                 const ConnW& W = c_layers[idx];
                 const int tcur = ts.cur, vcur = vs.cur;
@@ -1308,8 +1358,8 @@ struct vb200_engine {
         }
         const int tc = ts.cur, vc = vs.cur;
         pl.t_cur = tc; pl.v_cur = vc;
-        pl.outs[9] = OutBuf{pl.t_f32[tc], Mt, H, H};
-        pl.outs[10] = OutBuf{pl.v_f32[vc], Mv, Hv, Hv};
+        if (pl.tail_t == nullptr) pl.outs[9] = OutBuf{pl.t_f32[tc], Mt, H, H};
+        if (pl.tail_v == nullptr) pl.outs[10] = OutBuf{pl.v_f32[vc], Mv, Hv, Hv};
 
         const size_t n_before_heads = ops.size();
         if (do_s) build_heads(pl, select);
@@ -1373,24 +1423,26 @@ struct vb200_engine {
         float* pooled_t = pl.mem.alloc_n<float>(static_cast<size_t>(B) * Hb);
         float* pooled = pl.mem.alloc_n<float>(static_cast<size_t>(B) * Hb);
         bf16* pooled_b = pl.mem.alloc_n<bf16>(static_cast<size_t>(B) * Hb * S);
-        if (pl.packed) {
-            // a sample's first row sits at a per-call offset, not at a fixed stride: gather the B first rows of each stream into
-            // compact [B, hidden] operands for the poolers
-            bf16* first_t = pl.mem.alloc_n<bf16>(static_cast<size_t>(B) * H * S);
-            bf16* first_v = pl.mem.alloc_n<bf16>(static_cast<size_t>(B) * Hv * S);
+        // The poolers' operand, each sample's first row of a final state: a pruned tail's compact rows, the full state at stride
+        // L rows on dense plans, or on packed plans (a sample's first row sits at a per-call offset) the B first rows gathered into
+        // compact [B, hidden] rows.  Returns the operand and its row stride.
+        const size_t first_op = ops.size();
+        auto first_rows = [&](const bf16* tail, const bf16* state, int hid, int L, bool text, int M) -> std::pair<const bf16*, int64_t> {
+            if (tail != nullptr) return {tail, hid};
+            if (!pl.packed) return {state, static_cast<int64_t>(L) * hid};
+            bf16* first = pl.mem.alloc_n<bf16>(static_cast<size_t>(B) * hid * S);
             Op g{};
-            g.kind = Op::GATHER; g.sync = Op::JOIN; g.B = B;
-            g.qkv_a = pl.t_b16[tc]; g.ctx_a = first_t; g.ld_a = static_cast<int>(H * S); g.offs_a = pl.offs_t(); g.M = Mt;
+            g.kind = Op::GATHER; g.B = B; g.qkv_a = state; g.ctx_a = first; g.ld_a = static_cast<int>(hid * S);
+            g.offs_a = text ? pl.offs_t() : pl.offs_v(); g.M = M;
             ops.push_back(g);
-            g.sync = Op::NONE;
-            g.qkv_a = pl.v_b16[vc]; g.ctx_a = first_v; g.ld_a = static_cast<int>(Hv * S); g.offs_a = pl.offs_v(); g.M = Mv;
-            ops.push_back(g);
-            add_linear(pl, first_t, B, H, t_pool, vb::kActRelu, nullptr, 0, nullptr, nullptr, 0, pooled_t, Hb, 0, Op::NONE);
-            add_linear(pl, first_v, B, Hv, v_pool, vb::kActRelu, nullptr, 0, nullptr, pooled_b, Hb, pooled, Hb, 0, Op::NONE, pooled_t, Hb);
-        } else {
-            add_linear(pl, pl.t_b16[tc], B, static_cast<int64_t>(T) * H, t_pool, vb::kActRelu, nullptr, 0, nullptr, nullptr, 0, pooled_t, Hb, 0, Op::JOIN);
-            add_linear(pl, pl.v_b16[vc], B, static_cast<int64_t>(V) * Hv, v_pool, vb::kActRelu, nullptr, 0, nullptr, pooled_b, Hb, pooled, Hb, 0, Op::NONE, pooled_t, Hb);
-        }
+            return {first, hid};
+        };
+        const auto first_t = first_rows(pl.tail_t, pl.t_b16[tc], H, T, true, Mt);
+        const auto first_v = first_rows(pl.tail_v, pl.v_b16[vc], Hv, V, false, Mv);
+        add_linear(pl, first_t.first, B, first_t.second, t_pool, vb::kActRelu, nullptr, 0, nullptr, nullptr, 0, pooled_t, Hb, 0, Op::NONE);
+        add_linear(pl, first_v.first, B, first_v.second, v_pool, vb::kActRelu, nullptr, 0, nullptr, pooled_b, Hb, pooled, Hb, 0, Op::NONE,
+                   pooled_t, Hb);
+        ops[first_op].sync = Op::JOIN;       // the heads start after the image branch
         const int* rows_t = pl.packed ? pl.rows_t() : nullptr;
         const int* rows_v = pl.packed ? pl.rows_v() : nullptr;
         pl.outs[11] = OutBuf{pooled, B, Hb, Hb};
@@ -1489,8 +1541,8 @@ struct vb200_engine {
                                              op.m_rows));
                 break;
             case Op::GATHER:
-                CUDA_CHECK(vb::launch_gather_state(op.offs_a, op.M, nullptr, op.qkv_a, nullptr, nullptr, op.ctx_a, nullptr, op.B, 1,
-                                                   op.ld_a, op.ld_a, st));
+                CUDA_CHECK(vb::launch_gather_state(op.offs_a, op.M, op.x, op.qkv_a, nullptr, op.out, op.ctx_a, nullptr, op.B, 1,
+                                                   op.hidden, op.ld_a, st));
                 break;
         }
     }
@@ -1684,7 +1736,7 @@ struct vb200_engine {
                    const PrefixState& state, cudaMemcpyKind kind, void* cuda_stream, const std::function<void(Plan&, cudaStream_t)>& input) {
         reject_packed_attention(select, api);
         CUDA_CHECK(cudaSetDevice(opt.device));
-        Plan& pl = *get_plan(B, Tin, V, select & VB200_OUT_ALL, slot, mode, (select & VB200_OUT_ATTENTION) != 0);
+        Plan& pl = *get_plan(B, Tin, V, (select & VB200_OUT_ALL) | rows_read(out), slot, mode, (select & VB200_OUT_ATTENTION) != 0);
         const cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
         input(pl, st);
         run_plan(pl, st);
@@ -1705,7 +1757,7 @@ struct vb200_engine {
         if (x3) fail(VB200_ERR_INVALID, "%s: packed batches are not supported in split_fp32 (fp32x) mode", api);
         const PackedBatch b = pack_batch(api, cfg, schedule, len, maps ? out->attention_probs : nullptr, max_rows);
         CUDA_CHECK(cudaSetDevice(opt.device));
-        Plan& pl = *get_plan(len.B, b.Tin, b.V, select & VB200_OUT_ALL, slot, mode, maps);
+        Plan& pl = *get_plan(len.B, b.Tin, b.V, (select & VB200_OUT_ALL) | rows_read(out), slot, mode, maps);
         const cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
         stage_meta(pl, b.meta, st);
         input(pl, b, st);
