@@ -7,6 +7,7 @@
 #include "../../include/vilbert_b200.h"
 
 #include <algorithm>
+#include <array>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
@@ -17,6 +18,7 @@
 #include <memory>
 #include <stdexcept>
 #include <string>
+#include <variant>
 #include <vector>
 
 #include <nvtx3/nvToolsExt.h>      // header-only NVTX v3: ranges per layer / per forward for nsys and ncu --nvtx (SURVEY.md section 5)
@@ -336,27 +338,51 @@ bool make_tmap_out(CUtensorMap* m, const void* base, int64_t rows, int64_t cols,
                            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
-// Decide whether a plain GEMM may use the TMA-store epilogue and build its output map (exactly one output, aligned).
-void setup_tma_store(CUtensorMap* tc, GemmEpilogue& e) {
-    e.tma_store = 0;
-    if (e.split16) return;
-    if (e.out_bf16 != nullptr && e.out_f32 == nullptr) {
-        if (make_tmap_out(tc, e.out_bf16, e.M, e.N, e.ld_bf16, false, e.out_f16 != 0)) e.tma_store = 1;
-    } else if (e.out_f32 != nullptr && e.out_bf16 == nullptr) {
-        if (make_tmap_out(tc, e.out_f32, e.M, e.N, e.ld_f32, true, false)) e.tma_store = 2;
-    }
-}
-// Output maps of the ping-pong kernel (every output leaves through the TMA); false when an output does not meet the TMA's rules.
-bool setup_pingpong_store(CUtensorMap* c16, CUtensorMap* c32, const GemmEpilogue& e) {
-    if (e.out_bf16 != nullptr && !make_tmap_out(c16, e.out_bf16, e.M, e.N, e.ld_bf16, false, e.out_f16 != 0)) return false;
-    if (e.out_f32 != nullptr && !make_tmap_out(c32, e.out_f32, e.M, e.N, e.ld_f32, true, false)) return false;
-    return true;
-}
 // Which kernel takes the plain GEMMs it supports: 1 ping-pong (default), 0 the cooperative gemm_persistent_kernel.
 // VB200_GEMM=coop|pingpong is the A/B switch; vb200_set_option("gemm_kernel") changes it per engine.
 int default_gemm_kernel() {
     static const int v = [] { const char* e = getenv("VB200_GEMM"); return (e && strcmp(e, "coop") == 0) ? 0 : 1; }();
     return v;
+}
+
+// One GEMM launch: operand maps, output maps, epilogue, tile width and kernel (make_gemm).
+struct GemmCall {
+    CUtensorMap ta{}, tb{};
+    CUtensorMap tc16{}, tc32{};    // output maps of the TMA store: 16-bit and fp32 output (cooperative kernel: the one ep.tma_store names)
+    GemmEpilogue ep{};
+    int block_n = 128;
+    bool pingpong = false;         // the ping-pong kernel (gemm_pingpong.cuh), else the cooperative one (gemm_persistent.cuh)
+    // grid_pct: 0 the default persistent grid, 10..100 this percentage of the SMs (vb200_profile_ops)
+    cudaError_t launch(cudaStream_t st, int grid_pct = 0) const {
+        if (pingpong) return vb::launch_gemm_pingpong(ta, tb, &tc16, &tc32, ep, block_n, grid_pct, st);
+        const CUtensorMap* tc = ep.tma_store == 1 ? &tc16 : (ep.tma_store == 2 ? &tc32 : nullptr);
+        return vb::launch_gemm_persistent_plain(ta, tb, tc, ep, block_n, grid_pct, st);
+    }
+};
+// What a caller fixes of a GEMM launch: the tile width (0: gemm_p_pick_block_n(N)) and the kernel -- 0 the cooperative one, 1 the
+// ping-pong one wherever it takes the GEMM and the TMA can store every output (else the cooperative one), -1 as 1 or 0 by the process
+// default (default_gemm_kernel).
+struct GemmSpec { int block_n = 0; int kernel = -1; };
+// A = [ep.M, ep.K] with row stride lda, W = [ep.N, ep.K] with row stride ldw (elements); ep names the outputs, activation and the
+// rest of the epilogue but not the TMA store, which is decided here: ping-pong outputs all leave through the TMA, a cooperative
+// GEMM with exactly one aligned output and no hi | lo | hi split stores its last tile through it.
+GemmCall make_gemm(const void* A, int64_t lda, const void* W, int64_t ldw, const GemmEpilogue& ep, GemmSpec spec = {}) {
+    GemmCall g;
+    g.ep = ep;
+    g.ep.tma_store = 0;
+    g.block_n = spec.block_n > 0 ? spec.block_n : vb::gemm_p_pick_block_n(ep.N);
+    g.ta = make_tmap(A, ep.M, ep.K, lda, 128, ep.a_f16 != 0);
+    g.tb = make_tmap(W, ep.N, ep.K, ldw, g.block_n, ep.a_f16 != 0);
+    auto out16 = [&](CUtensorMap* m) { return make_tmap_out(m, ep.out_bf16, ep.M, ep.N, ep.ld_bf16, false, ep.out_f16 != 0); };
+    auto out32 = [&](CUtensorMap* m) { return make_tmap_out(m, ep.out_f32, ep.M, ep.N, ep.ld_f32, true, false); };
+    const int kernel = spec.kernel < 0 ? default_gemm_kernel() : spec.kernel;
+    g.pingpong = kernel == 1 && vb::gemm_pingpong_supports(ep, g.block_n) && (ep.out_bf16 == nullptr || out16(&g.tc16)) &&
+                 (ep.out_f32 == nullptr || out32(&g.tc32));
+    if (!g.pingpong && !ep.split16) {
+        if (ep.out_bf16 != nullptr && ep.out_f32 == nullptr && out16(&g.tc16)) g.ep.tma_store = 1;
+        else if (ep.out_f32 != nullptr && ep.out_bf16 == nullptr && out32(&g.tc32)) g.ep.tma_store = 2;
+    }
+    return g;
 }
 
 // ------------------------------------------------------------------------------------------ launch list
@@ -369,50 +395,39 @@ constexpr int kMaxRowsPerSample = 1024;
 inline const char* bound_name(int max_rows) {
     return max_rows == kStagedAttnRows ? "the small-sequence attention kernels" : "this engine's max_rows_per_sample";
 }
+// Launch-list entries.  Each kind's arguments are the named arguments of its launcher (kernels.h); packed plans add the device row
+// count of the rows an op computes (m_rows) and the per-sample row offsets of the attention operands (offs*).
+struct SelfAttnArgs {
+    const bf16* qkv; int ld_qkv, hidden; const float* mask; bf16* ctx; int ld_ctx, B, L, heads, head_dim; const int* offs;
+    bool stream_kv;                // the streaming kernel (more than kStagedAttnRows rows per sample)
+};
+struct CoAttnArgs {
+    const bf16 *qkv_img, *qkv_txt; int ld_img, ld_txt, hidden; const float *img_mask, *txt_mask;
+    bf16 *ctx_txt, *ctx_img; int ld_ctx_txt, ld_ctx_img, B, T, V, heads, head_dim; const int *offs_t, *offs_v;
+    bool stream_kv;                // the streaming kernel (either stream above kStagedAttnRows rows per sample)
+};
+struct RowdotArgs { const float *x, *W, *bias, *add; float* out; int ld_x, ld_out, M, K, n_out; const int* m_rows; };
+struct LayerNormArgs {             // out = LN(y + res)
+    const float *y, *res, *gamma, *beta; int ld_y, ld_res; float* out_f32; int ld_f32; bf16* out16; int ld16, M, N; const int* m_rows;
+};
+// fp32 attention (attention_f32.cu): fp32-parity mode and the attention-probability output; packed: probabilities per sample (pk)
+struct AttnF32Args {
+    const void *q, *k, *v; int ld_q, ld_kv, in_kind; const float* mask; int B, Lq, Lk, heads, head_dim;
+    bf16* ctx; int ld_ctx, ctx_mode; float* probs; bool packed; vb::PackedProbs pk;
+};
+// Row offs[b] of src16 (ld16 wide) -> row b of dst16, b < B, clamped to n_src rows; with src_f32 the same row (`hidden` wide) -> dst_f32.
+struct GatherArgs { const int* offs; int n_src, B; const bf16* src16; bf16* dst16; int ld16; const float* src_f32; float* dst_f32; int hidden; };
+
 struct Op {
-    enum Kind { GEMM, SELF_ATTN, CO_ATTN, ROWDOT, LAYERNORM, ATTN_F32, GATHER } kind;
+    // the index of the alternative is the kind number vb200_profile_ops reports
+    std::variant<GemmCall, SelfAttnArgs, CoAttnArgs, RowdotArgs, LayerNormArgs, AttnF32Args, GatherArgs> args;
     int stream = 0;                // 0 main, 1 side (image branch) inside the captured graph
-    // GEMM
-    CUtensorMap ta, tb, tc;        // operands, and the output (TMA-store epilogue, ep.tma_store != 0; ping-pong: the 16-bit output)
-    CUtensorMap tc32;              // ping-pong: the fp32 output
-    GemmEpilogue ep;
-    int block_n = 128;
-    bool pingpong = false;         // launched as the ping-pong kernel (gemm_pingpong.cuh)
-    // fp32 attention (attention_f32.cu): fp32-parity mode and the attention-probability output
-    const void *f_q = nullptr, *f_k = nullptr, *f_v = nullptr;
-    int f_ld_q = 0, f_ld_kv = 0, f_in = 0, f_Lq = 0, f_Lk = 0, f_ctx_mode = 0, f_ld_ctx = 0;
-    const float* f_mask = nullptr;
-    bf16* f_ctx = nullptr;
-    float* f_probs = nullptr;
-    bool f_packed = false;         // packed plan with VB200_OUT_ATTENTION_PACKED: per-sample rows and destination from f_pk
-    vb::PackedProbs f_pk{};
-    // attention
-    const bf16 *qkv_a = nullptr, *qkv_b = nullptr;
-    int ld_a = 0, ld_b = 0, hidden = 0;
-    const float *mask_a = nullptr, *mask_b = nullptr;
-    bf16 *ctx_a = nullptr, *ctx_b = nullptr;
-    int ld_ctx_a = 0, ld_ctx_b = 0, B = 0, La = 0, Lb = 0, heads = 0, head_dim = 0;
-    // layernorm: out = LN(ln_y + ln_res)
-    const float *ln_y = nullptr, *ln_res = nullptr, *ln_g = nullptr, *ln_b = nullptr;
-    float* ln_out_f = nullptr;
-    bf16* ln_out_h = nullptr;
-    int ln_ld = 0, ln_M = 0, ln_N = 0;
-    // rowdot
-    const float *x = nullptr, *W = nullptr, *bias = nullptr, *add = nullptr;
-    float* out = nullptr;
-    int ld_x = 0, ld_out = 0, M = 0, K = 0, n_out = 0;
-    // packed plans: device row count of the GEMM / LayerNorm / rowdot rows (ep.m_rows for GEMMs), per-sample row offsets of
-    // the attention operands (offs_a: La stream, offs_b: Lb stream); GATHER: row offs_a[b] of qkv_a (16-bit, ld_a wide) -> row b
-    // of ctx_a, b < B, clamped to M rows, and with x non-null the same row of x (fp32, `hidden` wide) -> row b of out
-    const int* m_rows = nullptr;
-    const int *offs_a = nullptr, *offs_b = nullptr;
-    // SELF_ATTN / CO_ATTN: the streaming kernels (a stream the op reads has more than 256 rows per sample in this plan)
-    bool stream_kv = false;
-    // fork/join markers for the two-stream graph
-    enum Sync { NONE, FORK, JOIN } sync = NONE;
     double flops = 0;
+    enum Sync { NONE, FORK, JOIN } sync = NONE;   // fork/join markers for the two-stream graph
     const char* tag = nullptr;     // layer this launch belongs to ("T3", "V0", "C2", "embed", "heads"): NVTX range name
 };
+template <class... F> struct Overloaded : F... { using F::operator()...; };
+template <class... F> Overloaded(F...) -> Overloaded<F...>;
 
 struct OutBuf { float* p = nullptr; int rows = 0, cols = 0, ld = 0; };
 
@@ -656,8 +671,6 @@ struct vb200_engine {
     // Programmatic dependent launch (opt.use_pdl): every kernel triggers its dependents once its main work is issued, and a
     // dependent GEMM's producer puts its first weight tiles in flight before griddepcontrol.wait.  On by default;
     // VB200_PDL=off|full, use_pdl < 0 = off.
-    bool tma_store_enabled = true;  // VB200_TMASTORE=0: every tile leaves through the register / LSU epilogue
-    bool early_w = true;            // VB200_EARLYW=0: no weight loads ahead of griddepcontrol.wait
     int gemm_kernel = 1;       // default_gemm_kernel(): 1 = plain GEMMs the ping-pong kernel supports run on it, 0 = all on the cooperative one
     Arena weights;
     std::string last_error;
@@ -1000,22 +1013,10 @@ struct vb200_engine {
                     const LNW* ln, bf16* out_b, int ld_b, float* out_f, int ld_f, int stream = 0, Op::Sync sync = Op::NONE,
                     const float* mul = nullptr, int ld_mul = 0, const int* m_rows = nullptr) {
         const int S = x3 ? 3 : 1;
-        if (x3 && act == vb::kActGelu) act = vb::kActGeluExact;
-        Op op{};
-        op.kind = Op::GEMM;
-        op.stream = stream;
-        op.sync = sync;
-        op.block_n = vb::gemm_p_pick_block_n(W.N);
-        // Small forwards (<= lone_rows rows in either stream, batch <= 8): 64-wide tiles while they still fit one CTA per SM -- twice
-        // the CTAs, half the epilogue each.  The tile width never changes an element's accumulation order.
-        if (lone_rows > 0 && !x3 && op.block_n == 128 && W.N % 64 == 0 &&
-            std::max(pl.B * pl.T, pl.B * pl.V) <= lone_rows && ((a_rows + 127) / 128) * (W.N / 64) <= vb::num_sms_host())
-            op.block_n = 64;
-        op.ta = make_tmap(A, a_rows, static_cast<int64_t>(W.ldw) * S, lda * S, 128, opt.act_fp16 != 0);
-        op.tb = make_tmap(W.w, W.N, static_cast<int64_t>(W.ldw) * S, static_cast<int64_t>(W.ldw) * S, op.block_n, opt.act_fp16 != 0);
-        GemmEpilogue& e = op.ep;
+        GemmEpilogue e{};
         e.M = static_cast<int>(a_rows); e.N = W.N; e.K = W.ldw * S;
-        e.bias = W.bias; e.mul = mul; e.ld_mul = ld_mul; e.act = act; e.pdl = opt.use_pdl ? (early_w ? 5 : 1) : 0;
+        e.bias = W.bias; e.mul = mul; e.ld_mul = ld_mul; e.act = x3 && act == vb::kActGelu ? vb::kActGeluExact : act;
+        e.pdl = opt.use_pdl ? 5 : 0;
         e.a_f16 = opt.act_fp16; e.out_f16 = opt.act_fp16;
         e.m_rows = m_rows;
         if (ln) {
@@ -1025,6 +1026,13 @@ struct vb200_engine {
             e.split16 = (x3 && out_b != nullptr) ? 1 : 0;
             if (e.split16 && (W.N & 63)) fail(VB200_ERR_INVALID, "fp32-parity mode: 16-bit GEMM output of width %d is not a multiple of 64", W.N);
         }
+        // Small forwards (<= lone_rows rows in either stream, batch <= 8): 64-wide tiles while they still fit one CTA per SM -- twice
+        // the CTAs, half the epilogue each.  The tile width never changes an element's accumulation order.  RowHeads plans bring
+        // their bucket M as pl.B = 1, pl.T = pl.V = M.
+        int block_n = vb::gemm_p_pick_block_n(W.N);
+        if (lone_rows > 0 && !x3 && block_n == 128 && W.N % 64 == 0 &&
+            std::max(pl.B * pl.T, pl.B * pl.V) <= lone_rows && ((a_rows + 127) / 128) * (W.N / 64) <= vb::num_sms_host())
+            block_n = 64;
         // Ping-pong kernel: each consumer warpgroup's epilogue runs under the other's mainloop.  It takes every plain GEMM it
         // supports (not the fp32-parity, pooled-product or ragged-N ones) whose outputs the TMA can store.
         // It takes the tile width chosen above, 128 even where that leaves one tile per CTA: 64-wide ping-pong tiles measured slower on H100 SXM
@@ -1034,22 +1042,14 @@ struct vb200_engine {
         // 8.45 / 8.41 us, two 128-wide runs), 64x3072x768 GELU (9.54 vs 9.13 / 9.07), 64x1024x1024 (10.18 vs 10.04 / 9.97; GELU 10.40
         // vs 10.21 / 10.10), 64x1024x768 ReLU (8.53 vs 8.08 / 8.05) and 64x2048x1024 GELU (10.57 vs 10.47 / 10.42), and 2 % faster
         // only at 64x768x3072 (20.74 vs 21.23 / 21.12); same card, bf16.
-        op.pingpong = gemm_kernel == 1 && tma_store_enabled && !x3 && vb::gemm_pingpong_supports(e, op.block_n) &&
-                      setup_pingpong_store(&op.tc, &op.tc32, e);
-        if (tma_store_enabled && !op.pingpong) setup_tma_store(&op.tc, e);
-        op.flops = 2.0 * a_rows * W.N * W.K;
-        pl.flops += op.flops;
-        pl.ops.push_back(op);
+        const GemmCall g = make_gemm(A, lda * S, W.w, static_cast<int64_t>(W.ldw) * S, e, {block_n, x3 ? 0 : gemm_kernel});
+        pl.ops.push_back({g, stream, 2.0 * a_rows * W.N * W.K, sync});
         if (ln) {
-            Op l{};
-            l.kind = Op::LAYERNORM;
-            l.stream = stream;
-            l.ln_y = pl.y_scratch[stream]; l.ln_res = res; l.ld_x = ld_res;
-            l.ln_g = ln->g; l.ln_b = ln->b; l.ln_out_f = out_f; l.ln_out_h = out_b; l.ln_ld = W.N;
-            l.ld_out = out_f ? ld_f : 0; l.ld_a = out_b ? ld_b * S : 0;
-            l.ln_M = static_cast<int>(a_rows); l.ln_N = W.N;
-            l.m_rows = m_rows;
-            pl.ops.push_back(l);
+            LayerNormArgs l{};
+            l.y = pl.y_scratch[stream]; l.ld_y = W.N; l.res = res; l.ld_res = ld_res; l.gamma = ln->g; l.beta = ln->b;
+            l.out_f32 = out_f; l.ld_f32 = out_f ? ld_f : 0; l.out16 = out_b; l.ld16 = out_b ? ld_b * S : 0;
+            l.M = static_cast<int>(a_rows); l.N = W.N; l.m_rows = m_rows;
+            pl.ops.push_back({l, stream});
         }
     }
     // softmax(Q K^T / sqrt(d) + mask) V of one stream (self) or one direction of a connection layer.  Default: the tensor-core
@@ -1060,34 +1060,25 @@ struct vb200_engine {
     void add_attn_f32(Plan& pl, const void* q, int ld_q, const void* k, const void* v, int ld_kv, const float* mask, int Lq, int Lk,
                       int heads, int hid, bf16* ctx, bool want_probs, int stream, const int* offs_q = nullptr,
                       const int* offs_k = nullptr, int prefix = 0) {
-        Op a{};
-        a.kind = Op::ATTN_F32;
-        a.stream = stream;
-        a.f_q = q; a.f_k = k; a.f_v = v; a.f_ld_q = ld_q; a.f_ld_kv = ld_kv; a.f_mask = mask; a.f_Lq = Lq; a.f_Lk = Lk;
-        a.f_in = x3 ? 0 : (opt.act_fp16 ? 1 : 2);
+        AttnF32Args a{};
+        a.q = q; a.k = k; a.v = v; a.ld_q = ld_q; a.ld_kv = ld_kv; a.mask = mask; a.Lq = Lq; a.Lk = Lk;
+        a.in_kind = x3 ? 0 : (opt.act_fp16 ? 1 : 2);
         a.B = pl.B; a.heads = heads; a.head_dim = hid / heads;
-        a.f_ctx = x3 ? ctx : nullptr; a.f_ctx_mode = x3 ? 3 : 0; a.f_ld_ctx = x3 ? 3 * hid : 0;
+        a.ctx = x3 ? ctx : nullptr; a.ctx_mode = x3 ? 3 : 0; a.ld_ctx = x3 ? 3 * hid : 0;
         if (want_probs && pl.packed) {
             const MetaLayout& m = pl.layout;
-            a.f_packed = true;
-            a.f_pk = vb::PackedProbs{offs_q, offs_k, pl.meta64(m.probs_dst()), pl.meta64(m.probs_entry(pl.n_probs)),
-                                     pl.meta64(m.probs_prefix(prefix))};
+            a.packed = true;
+            a.pk = vb::PackedProbs{offs_q, offs_k, pl.meta64(m.probs_dst()), pl.meta64(m.probs_entry(pl.n_probs)),
+                                   pl.meta64(m.probs_prefix(prefix))};
             ++pl.n_probs;
         } else if (want_probs) {
-            a.f_probs = pl.mem.alloc_n<float>(static_cast<size_t>(pl.B) * heads * Lq * Lk);
-            pl.attn.push_back(Plan::AttnOut{a.f_probs, heads, Lq, Lk});
+            a.probs = pl.mem.alloc_n<float>(static_cast<size_t>(pl.B) * heads * Lq * Lk);
+            pl.attn.push_back(Plan::AttnOut{a.probs, heads, Lq, Lk});
         }
-        if (x3) { a.flops = 4.0 * pl.B * heads * Lq * Lk * (hid / heads); pl.flops += a.flops; }
-        pl.ops.push_back(a);
+        pl.ops.push_back({a, stream, x3 ? 4.0 * pl.B * heads * Lq * Lk * (hid / heads) : 0.0});
     }
     Op rowdot_op(const float* x, int ld_x, const RowW& w, const float* add, float* out, int ld_out, int M, const int* m_rows = nullptr) {
-        Op op{};
-        op.m_rows = m_rows;
-        op.kind = Op::ROWDOT;
-        op.x = x; op.ld_x = ld_x; op.W = w.w; op.bias = w.b; op.add = add; op.out = out; op.ld_out = ld_out;
-        op.M = M; op.K = w.K; op.n_out = w.n_out;
-        op.flops = 2.0 * M * w.K * w.n_out;
-        return op;
+        return {RowdotArgs{x, w.w, w.b, add, out, ld_x, ld_out, M, w.K, w.n_out, m_rows}, 0, 2.0 * M * w.K * w.n_out};
     }
     // attention-probability entries of one forward: one per text / image layer, two per connection layer
     int attention_entries() const {
@@ -1255,15 +1246,11 @@ struct vb200_engine {
             add_linear(pl, st.b16[cur], M, hid, L.qkv, vb::kActNone, nullptr, 0, nullptr, qb, 3 * hid, qf, 3 * hid, stream, Op::NONE,
                        nullptr, 0, st.m_rows);
             if (!x3) {
-                Op a{};
-                a.kind = Op::SELF_ATTN;
-                a.stream = stream;
-                a.qkv_a = qb; a.ld_a = 3 * hid; a.hidden = hid; a.mask_a = st.mask; a.ctx_a = st.ctx; a.ld_ctx_a = hid;
-                a.B = B; a.La = st.seq; a.heads = heads; a.head_dim = hid / heads; a.offs_a = st.offs;
+                SelfAttnArgs a{};
+                a.qkv = qb; a.ld_qkv = 3 * hid; a.hidden = hid; a.mask = st.mask; a.ctx = st.ctx; a.ld_ctx = hid;
+                a.B = B; a.L = st.seq; a.heads = heads; a.head_dim = hid / heads; a.offs = st.offs;
                 a.stream_kv = st.seq > kStagedAttnRows;
-                a.flops = 4.0 * B * heads * st.seq * st.seq * (hid / heads);
-                pl.flops += a.flops;
-                ops.push_back(a);
+                ops.push_back({a, stream, 4.0 * B * heads * st.seq * st.seq * (hid / heads)});
             }
             if (x3 || want_attn)
                 add_attn_f32(pl, qkv_at(st.qkv, 0), 3 * hid, qkv_at(st.qkv, hid), qkv_at(st.qkv, 2 * hid), 3 * hid, st.mask, st.seq, st.seq,
@@ -1275,10 +1262,10 @@ struct vb200_engine {
                 if (pl.packed) {
                     bf16* ctx_c = pl.mem.alloc_n<bf16>(static_cast<size_t>(B) * hid * S);
                     float* res_c = pl.mem.alloc_n<float>(static_cast<size_t>(B) * hid);
-                    Op g{};
-                    g.kind = Op::GATHER; g.stream = stream; g.B = B; g.offs_a = st.offs; g.M = M;
-                    g.qkv_a = st.ctx; g.ctx_a = ctx_c; g.ld_a = static_cast<int>(hid * S); g.x = res; g.out = res_c; g.hidden = hid;
-                    ops.push_back(g);
+                    GatherArgs g{};
+                    g.offs = st.offs; g.n_src = M; g.B = B; g.src16 = st.ctx; g.dst16 = ctx_c; g.ld16 = static_cast<int>(hid * S);
+                    g.src_f32 = res; g.dst_f32 = res_c; g.hidden = hid;
+                    ops.push_back({g, stream});
                     ctx = ctx_c; res = res_c; ld = hid;
                 }
                 float* ln1_f = pl.mem.alloc_n<float>(static_cast<size_t>(B) * hid);
@@ -1326,15 +1313,12 @@ struct vb200_engine {
                            nullptr, 0, ts.m_rows);
                 const size_t first_co = ops.size();
                 if (!x3) {
-                    Op a{};
-                    a.kind = Op::CO_ATTN;
-                    a.qkv_a = qvb; a.ld_a = 3 * Hb; a.qkv_b = qtb; a.ld_b = 3 * Hb; a.hidden = Hb;
-                    a.mask_a = pl.mask_v; a.mask_b = pl.mask_t; a.ctx_a = ctx_t; a.ld_ctx_a = Hb; a.ctx_b = ctx_v; a.ld_ctx_b = Hb;
-                    a.B = B; a.La = T; a.Lb = V; a.heads = c.bi_heads; a.head_dim = Hb / c.bi_heads; a.offs_a = offs_t; a.offs_b = offs_v;
+                    CoAttnArgs a{};
+                    a.qkv_img = qvb; a.ld_img = 3 * Hb; a.qkv_txt = qtb; a.ld_txt = 3 * Hb; a.hidden = Hb;
+                    a.img_mask = pl.mask_v; a.txt_mask = pl.mask_t; a.ctx_txt = ctx_t; a.ld_ctx_txt = Hb; a.ctx_img = ctx_v; a.ld_ctx_img = Hb;
+                    a.B = B; a.T = T; a.V = V; a.heads = c.bi_heads; a.head_dim = Hb / c.bi_heads; a.offs_t = offs_t; a.offs_v = offs_v;
                     a.stream_kv = T > kStagedAttnRows || V > kStagedAttnRows;
-                    a.flops = 8.0 * B * c.bi_heads * T * V * (Hb / c.bi_heads);
-                    pl.flops += a.flops;
-                    ops.push_back(a);
+                    ops.push_back({a, 0, 8.0 * B * c.bi_heads * T * V * (Hb / c.bi_heads)});
                 }
                 if (x3 || want_attn) {
                     // text queries (Q2) over image keys / values (K1, V1) -> text context; then image queries (Q1) over K2, V2
@@ -1364,7 +1348,7 @@ struct vb200_engine {
         const size_t n_before_heads = ops.size();
         if (do_s) build_heads(pl, select);
         for (size_t i = n_before_heads; i < ops.size(); ++i) ops[i].tag = "heads";
-        for (Op& op : ops) if (op.kind == Op::ROWDOT) pl.flops += op.flops;
+        for (const Op& op : ops) pl.flops += op.flops;
 
         if (timeline) attach_timeline(pl);
         // One eager pass first: opts kernels into their shared-memory sizes and surfaces launch-configuration
@@ -1391,12 +1375,13 @@ struct vb200_engine {
     static constexpr int kTimelineCtas = 304;
     void attach_timeline(Plan& pl) {
         size_t n = 0;
-        for (const Op& op : pl.ops) if (op.kind == Op::GEMM) ++n;
+        for (const Op& op : pl.ops) n += std::holds_alternative<GemmCall>(op.args);
         if (n == 0) return;
         pl.timeline = pl.mem.alloc_n<long long>(n * kTimelineCtas * 16);
         CUDA_CHECK(cudaMemset(pl.timeline, 0, n * kTimelineCtas * 16 * sizeof(long long)));
         size_t i = 0;
-        for (Op& op : pl.ops) if (op.kind == Op::GEMM) op.ep.timing = pl.timeline + (i++) * kTimelineCtas * 16;
+        for (Op& op : pl.ops)
+            if (GemmCall* g = std::get_if<GemmCall>(&op.args)) g->ep.timing = pl.timeline + (i++) * kTimelineCtas * 16;
     }
 
     // Plan cache bound (a MicroBatchWorker produces many (batch, length, regions) combinations): beyond max_plans the least
@@ -1431,10 +1416,10 @@ struct vb200_engine {
             if (tail != nullptr) return {tail, hid};
             if (!pl.packed) return {state, static_cast<int64_t>(L) * hid};
             bf16* first = pl.mem.alloc_n<bf16>(static_cast<size_t>(B) * hid * S);
-            Op g{};
-            g.kind = Op::GATHER; g.B = B; g.qkv_a = state; g.ctx_a = first; g.ld_a = static_cast<int>(hid * S);
-            g.offs_a = text ? pl.offs_t() : pl.offs_v(); g.M = M;
-            ops.push_back(g);
+            GatherArgs g{};
+            g.offs = text ? pl.offs_t() : pl.offs_v(); g.n_src = M; g.B = B;
+            g.src16 = state; g.dst16 = first; g.ld16 = static_cast<int>(hid * S);
+            ops.push_back({g});
             return {first, hid};
         };
         const auto first_t = first_rows(pl.tail_t, pl.t_b16[tc], H, T, true, Mt);
@@ -1503,48 +1488,53 @@ struct vb200_engine {
 
     // ---------------------------------------------------------------- execution
     void launch_op(const Op& op, cudaStream_t st) {
-        switch (op.kind) {
-            case Op::GEMM: {
-                GemmEpilogue e = op.ep;
-                e.tmap_c_host = e.tma_store ? &op.tc : nullptr;       // Op objects move when the list grows: bind here
-                e.grid_pct = profile_grid_pct;                        // 0 outside vb200_profile_ops
-                const cudaError_t le = op.pingpong
-                    ? vb::launch_gemm_pingpong(op.ta, op.tb, &op.tc, &op.tc32, e, op.block_n, st)
-                    : vb::launch_gemm_persistent_plain(op.ta, op.tb, e, op.block_n, st);
+        const int pdl = opt.use_pdl, f16 = opt.act_fp16;
+        std::visit(Overloaded{
+            [&](const GemmCall& g) {
+                const cudaError_t le = g.launch(st, profile_grid_pct);   // profile_grid_pct: 0 outside vb200_profile_ops
+                const GemmEpilogue& e = g.ep;
                 if (le != cudaSuccess)
                     fail(VB200_ERR_CUDA, "GEMM launch failed: %s (layer %s, M=%d N=%d K=%d act=%d block_n=%d split16=%d tma_store=%d)",
-                         cudaGetErrorString(le), op.tag ? op.tag : "?", e.M, e.N, e.K, e.act, op.block_n, e.split16, e.tma_store);
-                break;
-            }
-            case Op::SELF_ATTN:
-                CUDA_CHECK((op.stream_kv ? vb::launch_self_attention_stream : vb::launch_self_attention)(
-                    op.qkv_a, op.ld_a, op.hidden, op.mask_a, op.ctx_a, op.ld_ctx_a, op.B, op.La, op.heads, op.head_dim, opt.use_pdl,
-                    opt.act_fp16, st, op.offs_a));
-                break;
-            case Op::CO_ATTN:
-                CUDA_CHECK((op.stream_kv ? vb::launch_co_attention_stream : vb::launch_co_attention)(
-                    op.qkv_a, op.ld_a, op.qkv_b, op.ld_b, op.hidden, op.mask_a, op.mask_b, op.ctx_a, op.ld_ctx_a, op.ctx_b, op.ld_ctx_b,
-                    op.B, op.La, op.Lb, op.heads, op.head_dim, opt.use_pdl, opt.act_fp16, st, op.offs_a, op.offs_b));
-                break;
-            case Op::LAYERNORM:
-                CUDA_CHECK(vb::launch_ln_residual(op.ln_y, op.ln_ld, op.ln_res, op.ld_x, op.ln_g, op.ln_b, cfg.ln_eps, op.ln_out_f,
-                                                  op.ld_out, op.ln_out_h, op.ld_a, op.ln_M, op.ln_N, opt.act_fp16, x3 ? 1 : 0,
-                                                  opt.use_pdl, st, op.m_rows));
-                break;
-            case Op::ATTN_F32:
-                CUDA_CHECK(vb::launch_attention_f32(op.f_q, op.f_ld_q, op.f_k, op.f_v, op.f_ld_kv, op.f_in, op.f_mask, op.B, op.f_Lq,
-                                                    op.f_Lk, op.heads, op.head_dim, op.f_ctx, op.f_ld_ctx, op.f_ctx_mode, op.f_probs,
-                                                    opt.use_pdl, st, op.f_packed ? &op.f_pk : nullptr));
-                break;
-            case Op::ROWDOT:
-                CUDA_CHECK(vb::launch_rowdot(op.x, op.ld_x, op.W, op.bias, op.add, op.out, op.ld_out, op.M, op.K, op.n_out, opt.use_pdl, st,
-                                             op.m_rows));
-                break;
-            case Op::GATHER:
-                CUDA_CHECK(vb::launch_gather_state(op.offs_a, op.M, op.x, op.qkv_a, nullptr, op.out, op.ctx_a, nullptr, op.B, 1,
-                                                   op.hidden, op.ld_a, st));
-                break;
-        }
+                         cudaGetErrorString(le), op.tag ? op.tag : "?", e.M, e.N, e.K, e.act, g.block_n, e.split16, e.tma_store);
+            },
+            [&](const SelfAttnArgs& a) {
+                CUDA_CHECK((a.stream_kv ? vb::launch_self_attention_stream : vb::launch_self_attention)(
+                    a.qkv, a.ld_qkv, a.hidden, a.mask, a.ctx, a.ld_ctx, a.B, a.L, a.heads, a.head_dim, pdl, f16, st, a.offs));
+            },
+            [&](const CoAttnArgs& a) {
+                CUDA_CHECK((a.stream_kv ? vb::launch_co_attention_stream : vb::launch_co_attention)(
+                    a.qkv_img, a.ld_img, a.qkv_txt, a.ld_txt, a.hidden, a.img_mask, a.txt_mask, a.ctx_txt, a.ld_ctx_txt, a.ctx_img,
+                    a.ld_ctx_img, a.B, a.T, a.V, a.heads, a.head_dim, pdl, f16, st, a.offs_t, a.offs_v));
+            },
+            [&](const RowdotArgs& a) {
+                CUDA_CHECK(vb::launch_rowdot(a.x, a.ld_x, a.W, a.bias, a.add, a.out, a.ld_out, a.M, a.K, a.n_out, pdl, st, a.m_rows));
+            },
+            [&](const LayerNormArgs& a) {
+                CUDA_CHECK(vb::launch_ln_residual(a.y, a.ld_y, a.res, a.ld_res, a.gamma, a.beta, cfg.ln_eps, a.out_f32, a.ld_f32, a.out16,
+                                                  a.ld16, a.M, a.N, f16, x3 ? 1 : 0, pdl, st, a.m_rows));
+            },
+            [&](const AttnF32Args& a) {
+                CUDA_CHECK(vb::launch_attention_f32(a.q, a.ld_q, a.k, a.v, a.ld_kv, a.in_kind, a.mask, a.B, a.Lq, a.Lk, a.heads,
+                                                    a.head_dim, a.ctx, a.ld_ctx, a.ctx_mode, a.probs, pdl, st,
+                                                    a.packed ? &a.pk : nullptr));
+            },
+            [&](const GatherArgs& a) {
+                CUDA_CHECK(vb::launch_gather_state(a.offs, a.n_src, a.src_f32, a.src16, nullptr, a.dst_f32, a.dst16, nullptr, a.B, 1,
+                                                   a.hidden, a.ld16, st));
+            },
+        }, op.args);
+    }
+    // vb200_profile_ops' dims of a launch-list entry
+    static std::array<int, 4> op_dims(const Op& op) {
+        return std::visit(Overloaded{
+            [](const GemmCall& g) { return std::array<int, 4>{g.ep.M, g.ep.N, g.ep.K, g.ep.act}; },
+            [](const SelfAttnArgs& a) { return std::array<int, 4>{a.B, a.L, 0, a.heads}; },
+            [](const CoAttnArgs& a) { return std::array<int, 4>{a.B, a.T, a.V, a.heads}; },
+            [](const RowdotArgs&) { return std::array<int, 4>{0, 0, 0, 0}; },
+            [](const LayerNormArgs& a) { return std::array<int, 4>{a.M, a.N, 0, 0}; },
+            [](const AttnF32Args& a) { return std::array<int, 4>{a.B, 0, 0, a.heads}; },
+            [](const GatherArgs& a) { return std::array<int, 4>{a.B, 0, 0, 0}; },
+        }, op.args);
     }
     // Text-stream ops go to `st`, image-stream ops to the side stream so the two ViLBERT streams overlap
     // (T_k || V_k between co-attentions, and the two halves of a connection layer).  Dependencies across the
@@ -2284,8 +2274,6 @@ int create_engine(const char* api, bool pretraining, const char* config_json, in
             if (strcmp(v, "full") == 0) eng->opt.use_pdl = 1;
             if (strcmp(v, "off") == 0) eng->opt.use_pdl = 0;
         }
-        if (const char* v = getenv("VB200_TMASTORE")) eng->tma_store_enabled = (strcmp(v, "0") != 0);
-        if (const char* v = getenv("VB200_EARLYW")) eng->early_w = (strcmp(v, "0") != 0);
         eng->gemm_kernel = default_gemm_kernel();
         CUDA_CHECK(cudaStreamCreateWithFlags(&eng->side_stream, cudaStreamNonBlocking));
         CUDA_CHECK(cudaEventCreateWithFlags(&eng->ev_fork, cudaEventDisableTiming));
@@ -2666,14 +2654,12 @@ int vb200_profile_ops(vb200_handle h, int32_t batch, int32_t n_tokens, int32_t n
         *n_ops = n;
         for (int i = 0; i < n && i < max_ops; ++i) {
             const Op& op = pl->ops[i];
-            if (kinds) kinds[i] = static_cast<int>(op.kind);
+            if (kinds) kinds[i] = static_cast<int>(op.args.index());
             if (ms) ms[i] = t[i];
             if (flops) flops[i] = op.flops;
             if (dims) {
-                dims[4 * i + 0] = op.kind == Op::GEMM ? op.ep.M : (op.kind == Op::LAYERNORM ? op.ln_M : op.B);
-                dims[4 * i + 1] = op.kind == Op::GEMM ? op.ep.N : (op.kind == Op::LAYERNORM ? op.ln_N : op.La);
-                dims[4 * i + 2] = op.kind == Op::GEMM ? op.ep.K : op.Lb;
-                dims[4 * i + 3] = op.kind == Op::GEMM ? op.ep.act : op.heads;
+                const std::array<int, 4> d = vb200_engine::op_dims(op);
+                std::copy(d.begin(), d.end(), dims + 4 * i);
             }
         }
     });
@@ -2721,10 +2707,11 @@ int vb200_timeline(vb200_handle h, int32_t batch, int32_t n_tokens, int32_t n_re
         CUDA_CHECK(cudaDeviceSynchronize());
         int n = 0;
         for (const Op& op : pl->ops) {
-            if (op.ep.timing == nullptr || op.kind != Op::GEMM) continue;
+            const GemmCall* g = std::get_if<GemmCall>(&op.args);
+            if (g == nullptr || g->ep.timing == nullptr) continue;
             if (n < max_ops) {
-                if (dims) { dims[4 * n] = op.ep.M; dims[4 * n + 1] = op.ep.N; dims[4 * n + 2] = op.ep.K; dims[4 * n + 3] = op.stream; }
-                if (stamps) CUDA_CHECK(cudaMemcpy(stamps + static_cast<size_t>(n) * vb200_engine::kTimelineCtas * 16, op.ep.timing,
+                if (dims) { dims[4 * n] = g->ep.M; dims[4 * n + 1] = g->ep.N; dims[4 * n + 2] = g->ep.K; dims[4 * n + 3] = op.stream; }
+                if (stamps) CUDA_CHECK(cudaMemcpy(stamps + static_cast<size_t>(n) * vb200_engine::kTimelineCtas * 16, g->ep.timing,
                                                   sizeof(long long) * vb200_engine::kTimelineCtas * 16, cudaMemcpyDeviceToHost));
             }
             ++n;
@@ -2775,38 +2762,27 @@ int vb200_linear(const void* x_bf16, int64_t ld_x, const void* w_bf16, int64_t l
         // tile width never changes an element's accumulation order.
         if (variant < 0 || variant == 1 || variant > 5)
             fail(VB200_ERR_INVALID, "vb200_linear: variant %d does not exist (0 persistent, 2 / 3 / 4 = 0, 5 ping-pong)", variant);
+        GemmEpilogue e{};
+        e.M = (int)M; e.N = (int)N; e.K = (int)K; e.bias = bias; e.out_bf16 = static_cast<bf16*>(y_bf16); e.ld_bf16 = (int)ld_y_bf16;
+        e.out_f32 = y_f32; e.ld_f32 = (int)ld_y_f32; e.act = act; e.pdl = use_pdl;
+        e.a_f16 = act_fp16 ? 1 : 0; e.out_f16 = e.a_f16; e.timing = timing;
+        const cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+        int bn = block_n > 0 ? block_n : vb::gemm_p_pick_block_n(static_cast<int>(N));
         if (variant == 5) {
-            const int bn = block_n > 0 ? block_n : vb::gemm_p_pick_block_n(static_cast<int>(N));
-            CUtensorMap ta = make_tmap(x_bf16, M, K, ld_x, 128, act_fp16 != 0);
-            CUtensorMap tb = make_tmap(w_bf16, N, K, ld_w, bn, act_fp16 != 0);
-            GemmEpilogue e{};
-            e.M = (int)M; e.N = (int)N; e.K = (int)K; e.bias = bias; e.act = act; e.pdl = use_pdl;
-            e.out_bf16 = static_cast<bf16*>(y_bf16); e.ld_bf16 = (int)ld_y_bf16; e.out_f32 = y_f32; e.ld_f32 = (int)ld_y_f32;
-            e.a_f16 = act_fp16 ? 1 : 0; e.out_f16 = e.a_f16; e.timing = timing;
-            CUtensorMap c16, c32;
-            if (!vb::gemm_pingpong_supports(e, bn) || !setup_pingpong_store(&c16, &c32, e))
+            const GemmCall g = make_gemm(x_bf16, ld_x, w_bf16, ld_w, e, {bn, 1});
+            if (!g.pingpong)
                 fail(VB200_ERR_INVALID, "vb200_linear: variant 5 (ping-pong) takes plain GEMMs with N a multiple of block_n 64 / 128 and "
                                         "TMA-storable outputs (N=%lld block_n=%d)", (long long)N, bn);
-            CUDA_CHECK(vb::launch_gemm_pingpong(ta, tb, &c16, &c32, e, bn, static_cast<cudaStream_t>(cuda_stream)));
+            CUDA_CHECK(g.launch(st));
             return;
         }
-        int bn = block_n > 0 ? block_n : vb::gemm_p_pick_block_n(static_cast<int>(N));
         if (bn == 256) bn = 128;
         if (bn != 64 && bn != 128 && bn != 192)
             fail(VB200_ERR_INVALID, "vb200_linear: block_n %d (plain tiles are 64, 128, 192 or 256 wide)", bn);
         if (variant >= 2 && bn != 128 && !(variant == 4 && bn == 64))
             fail(VB200_ERR_INVALID, "vb200_linear: variants 2 and 3 are the plain 128-wide tile, variant 4 the 128- or 64-wide one");
-        CUtensorMap ta = make_tmap(x_bf16, M, K, ld_x, 128, act_fp16 != 0);
-        CUtensorMap tb = make_tmap(w_bf16, N, K, ld_w, bn, act_fp16 != 0);
-        GemmEpilogue e{};
-        e.M = (int)M; e.N = (int)N; e.K = (int)K; e.bias = bias; e.out_bf16 = static_cast<bf16*>(y_bf16); e.ld_bf16 = (int)ld_y_bf16;
-        e.out_f32 = y_f32; e.ld_f32 = (int)ld_y_f32; e.act = act; e.pdl = use_pdl;
-        e.a_f16 = act_fp16 ? 1 : 0; e.out_f16 = e.a_f16; e.timing = timing;
         if (const char* dbg = getenv("VB200_DEBUG")) e.debug = atoi(dbg);          // timing decomposition (kernels.h), op entry only
-        CUtensorMap tc;
-        const char* ts = getenv("VB200_TMASTORE");
-        if (!(ts && strcmp(ts, "0") == 0)) { setup_tma_store(&tc, e); e.tmap_c_host = e.tma_store ? &tc : nullptr; }
-        CUDA_CHECK(vb::launch_gemm_persistent_plain(ta, tb, e, bn, static_cast<cudaStream_t>(cuda_stream)));
+        CUDA_CHECK(make_gemm(x_bf16, ld_x, w_bf16, ld_w, e, {bn, 0}).launch(st));
     });
 }
 
@@ -2817,19 +2793,10 @@ int vb200_linear_rows(const void* x16, int64_t ld_x, const void* w16, int64_t ld
         if (m_rows == nullptr) fail(VB200_ERR_INVALID, "vb200_linear_rows: m_rows is NULL");
         const int bn = block_n > 0 ? block_n : vb::gemm_p_pick_block_n(static_cast<int>(N));
         if (bn != 64 && bn != 128 && bn != 192) fail(VB200_ERR_INVALID, "vb200_linear_rows: block_n %d (plain tiles are 64, 128 or 192 wide)", bn);
-        CUtensorMap ta = make_tmap(x16, M, K, ld_x, 128, act_fp16 != 0);
-        CUtensorMap tb = make_tmap(w16, N, K, ld_w, bn, act_fp16 != 0);
         GemmEpilogue e{};
         e.M = (int)M; e.N = (int)N; e.K = (int)K; e.bias = bias; e.act = act; e.a_f16 = act_fp16 ? 1 : 0; e.out_f16 = e.a_f16;
         e.out_bf16 = static_cast<bf16*>(y16); e.ld_bf16 = (int)ld_y16; e.out_f32 = y_f32; e.ld_f32 = (int)ld_y_f32; e.m_rows = m_rows;
-        CUtensorMap tc, tc32;
-        if (default_gemm_kernel() == 1 && vb::gemm_pingpong_supports(e, bn) && setup_pingpong_store(&tc, &tc32, e)) {   // as the engine
-            CUDA_CHECK(vb::launch_gemm_pingpong(ta, tb, &tc, &tc32, e, bn, static_cast<cudaStream_t>(cuda_stream)));
-            return;
-        }
-        setup_tma_store(&tc, e);
-        e.tmap_c_host = e.tma_store ? &tc : nullptr;
-        CUDA_CHECK(vb::launch_gemm_persistent_plain(ta, tb, e, bn, static_cast<cudaStream_t>(cuda_stream)));
+        CUDA_CHECK(make_gemm(x16, ld_x, w16, ld_w, e, {bn, -1}).launch(static_cast<cudaStream_t>(cuda_stream)));   // as the engine
     });
 }
 
@@ -2856,14 +2823,12 @@ int vb200_linear_split(const void* x16, int64_t ld_x, const void* w16, int64_t l
                        int64_t ld_y16, float* y_f32, int64_t ld_y_f32, int64_t M, int64_t N, int64_t K3, void* cuda_stream) {
     return op_guard([&] {
         if (K3 % 192 != 0) fail(VB200_ERR_INVALID, "vb200_linear_split: K3 = %lld is not 3 x a multiple of 64", (long long)K3);
-        const int bn = vb::gemm_p_pick_block_n(static_cast<int>(N));
-        CUtensorMap ta = make_tmap(x16, M, K3, ld_x, 128, true);
-        CUtensorMap tb = make_tmap(w16, N, K3, ld_w, bn, true);
         GemmEpilogue e{};
         e.M = (int)M; e.N = (int)N; e.K = (int)K3; e.bias = bias; e.out_bf16 = static_cast<bf16*>(y16);
         e.ld_bf16 = (int)ld_y16; e.out_f32 = y_f32; e.ld_f32 = (int)ld_y_f32; e.act = act; e.a_f16 = 1; e.out_f16 = 1;
         e.split16 = y16 != nullptr ? 1 : 0;
-        CUDA_CHECK(vb::launch_gemm_persistent_plain(ta, tb, e, bn, static_cast<cudaStream_t>(cuda_stream)));
+        // as the engine's fp32-parity GEMMs: the cooperative kernel, the TMA store for an fp32-only output
+        CUDA_CHECK(make_gemm(x16, ld_x, w16, ld_w, e, {0, 0}).launch(static_cast<cudaStream_t>(cuda_stream)));
     });
 }
 
@@ -2957,16 +2922,11 @@ int vb200_linear_product(const void* x16, int64_t ld_x, const void* w16, int64_t
         // as add_linear builds the pooled product: the cooperative kernel (ping-pong takes no product), its tile width, its TMA store
         const int bn = block_n > 0 ? block_n : vb::gemm_p_pick_block_n(static_cast<int>(N));
         if (bn != 64 && bn != 128 && bn != 192) fail(VB200_ERR_INVALID, "vb200_linear_product: block_n %d (plain tiles are 64, 128 or 192 wide)", bn);
-        CUtensorMap ta = make_tmap(x16, M, K, ld_x, 128, act_fp16 != 0);
-        CUtensorMap tb = make_tmap(w16, N, K, ld_w, bn, act_fp16 != 0);
         GemmEpilogue e{};
         e.M = (int)M; e.N = (int)N; e.K = (int)K; e.bias = bias; e.act = act; e.mul = mul; e.ld_mul = (int)ld_mul;
         e.a_f16 = act_fp16 ? 1 : 0; e.out_f16 = e.a_f16;
         e.out_bf16 = static_cast<bf16*>(y16); e.ld_bf16 = (int)ld_y16; e.out_f32 = y_f32; e.ld_f32 = (int)ld_y_f32;
-        CUtensorMap tc;
-        setup_tma_store(&tc, e);
-        e.tmap_c_host = e.tma_store ? &tc : nullptr;
-        CUDA_CHECK(vb::launch_gemm_persistent_plain(ta, tb, e, bn, static_cast<cudaStream_t>(cuda_stream)));
+        CUDA_CHECK(make_gemm(x16, ld_x, w16, ld_w, e, {bn, -1}).launch(static_cast<cudaStream_t>(cuda_stream)));
     });
 }
 

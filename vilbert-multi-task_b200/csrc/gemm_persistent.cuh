@@ -587,7 +587,8 @@ inline int persistent_grid(int tiles, int grid_pct) {
 }
 
 template <int BLOCK_N, int ACT, bool F16, int MODE = 0>
-cudaError_t launch_p(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilogue& ep, cudaStream_t st) {
+cudaError_t launch_p(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap* tc, const GemmEpilogue& ep, int grid_pct,
+                     cudaStream_t st) {
     using Cfg = PCfg<BLOCK_N, MODE>;
     auto kern = gemm_persistent_kernel<BLOCK_N, ACT, F16, MODE>;
     const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
@@ -597,9 +598,8 @@ cudaError_t launch_p(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpi
     static_assert(Cfg::kMinBlocks == 1, "persistent_grid assumes one CTA per SM");
     cudaLaunchConfig_t cfg;
     cudaLaunchAttribute attrs[1];
-    fill_cfg<Cfg>(cfg, attrs, dim3(persistent_grid(m_tiles * n_tiles, ep.grid_pct), 1, 1), ep.pdl == 1 || ep.pdl == 5, st);
+    fill_cfg<Cfg>(cfg, attrs, dim3(persistent_grid(m_tiles * n_tiles, grid_pct), 1, 1), ep.pdl == 1 || ep.pdl == 5, st);
     GemmEpilogue e2 = ep;
-    const CUtensorMap* tc = static_cast<const CUtensorMap*>(ep.tmap_c_host);
     if (tc == nullptr) { e2.tma_store = 0; tc = &ta; }                             // &ta: any valid map for the unused slot
     return cudaLaunchKernelEx(&cfg, kern, ta, tb, *tc, e2, m_tiles, n_tiles);
 }

@@ -27,10 +27,8 @@ struct GemmEpilogue {
     int split16;                  // fp32-parity mode: the 16-bit output is written as fp16 hi | lo | hi per 64 columns
                                   // (common.cuh split_col; ld_bf16 is the stride of that 3x wider buffer); plain kernel only
     long long* timing;            // optional (profiling): 8 clock64 stamps per CTA, see gemm_persistent.cu; null in production
-    const void* tmap_c_host;      // host pointer to the CUtensorMap of the output (launchers copy it into a kernel parameter)
     int tma_store;                // 0: register/LSU stores only; 1: 16-bit output, 2: fp32 output may leave through a TMA store
                                   // (plain persistent kernel: the LAST tile of every CTA is staged in the idle operand ring)
-    int grid_pct;                 // 0: default persistent grid (2/3 of the CTA slots, launch_p); 10..100: this percentage of them
     int debug;                    // timing decomposition only (VB200_DEBUG through vb200_linear): 1 = issue no MMA, 2 = no epilogue
                                   // stores, 4 = no operand loads (the ring is "filled" by plain arrives); results are garbage
     const int* m_rows;            // optional device row count (packed batches): rows >= min(*m_rows, M) are neither loaded nor
@@ -43,14 +41,16 @@ struct GemmEpilogue {
 // persistent CTAs, wgmma consumer warpgroups (gemm_persistent.cuh)
 int gemm_p_pick_block_n(int N);
 int num_sms_host();          // SM count of the current device (132 on H100 SXM)
-cudaError_t launch_gemm_persistent_plain(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b, const GemmEpilogue& ep,
-                                         int block_n, cudaStream_t st);
+// tmap_c: the output map of the TMA store (ep.tma_store != 0), or null.  grid_pct (all GEMM launchers): 0 the default persistent
+// grid (persistent_grid), 10..100 this percentage of the SMs.
+cudaError_t launch_gemm_persistent_plain(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b, const CUtensorMap* tmap_c,
+                                         const GemmEpilogue& ep, int block_n, int grid_pct, cudaStream_t st);
 // ping-pong consumer warpgroups (gemm_pingpong.cuh): plain bias / activation GEMMs with N a multiple of block_n (64 or 128), no
 // pooled product or fp32-parity output; every output leaves through its TMA map (tmap_c16 for out_bf16, tmap_c32 for out_f32,
 // SWIZZLE_128B boxes of 128 rows x 128 bytes).  Same bits as launch_gemm_persistent_plain.
 bool gemm_pingpong_supports(const GemmEpilogue& ep, int block_n);
 cudaError_t launch_gemm_pingpong(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b, const CUtensorMap* tmap_c16,
-                                 const CUtensorMap* tmap_c32, const GemmEpilogue& ep, int block_n, cudaStream_t st);
+                                 const CUtensorMap* tmap_c32, const GemmEpilogue& ep, int block_n, int grid_pct, cudaStream_t st);
 
 // 16-bit activation buffers are typed __nv_bfloat16* throughout; `f16` says the bits are IEEE fp16 instead.
 // K4: softmax(Q K^T / sqrt(d) + mask) V per (sample, head); qkv row = [Q | K | V], each `hidden` wide.
