@@ -67,7 +67,8 @@ class BertForMultiModalPreTraining(nn.Module):
             attention_mask = torch.ones_like(input_ids)
         if image_attention_mask is None:
             image_attention_mask = torch.ones(image_feat.size(0), image_feat.size(1), dtype=torch.long)
-        t, v, pooled_t, pooled_v, attn = self.bert(input_ids, image_feat.float(), image_loc.float(), token_type_ids, attention_mask,
+        dt = self.cls.bi_seq_relationship.weight.dtype
+        t, v, pooled_t, pooled_v, attn = self.bert(input_ids, image_feat.to(dt), image_loc.to(dt), token_type_ids, attention_mask,
                                                    image_attention_mask, None, collect)
         if collect is not None:
             collect["final"] = (t, v, pooled_t, pooled_v)

@@ -389,8 +389,9 @@ class BertModel(nn.Module):
         if self.task_specific_tokens:
             ones = attention_mask.new_ones(attention_mask.size(0), 1)
             attention_mask = torch.cat([ones, attention_mask], dim=1)
-        t_mask = (1.0 - attention_mask[:, None, None, :].to(torch.float32)) * -10000.0
-        v_mask = (1.0 - image_attention_mask[:, None, None, :].to(torch.float32)) * -10000.0
+        dt = self.embeddings.word_embeddings.weight.dtype              # fp32, or fp64 for an fp64 copy of the oracle
+        t_mask = (1.0 - attention_mask[:, None, None, :].to(dt)) * -10000.0
+        v_mask = (1.0 - image_attention_mask[:, None, None, :].to(dt)) * -10000.0
         t = self.embeddings(input_txt, token_type_ids, task_ids)
         v = self.v_embeddings(input_imgs, image_loc)
         if collect is not None:
@@ -484,7 +485,8 @@ class VILBertForVLTasks(nn.Module):
             attention_mask = torch.ones_like(input_txt)
         if image_attention_mask is None:
             image_attention_mask = torch.ones(input_imgs.size(0), input_imgs.size(1), dtype=torch.long)
-        t, v, pooled_t, pooled_v, attn = self.bert(input_txt, input_imgs.float(), image_loc.float(),
+        dt = self.vil_logit.weight.dtype
+        t, v, pooled_t, pooled_v, attn = self.bert(input_txt, input_imgs.to(dt), image_loc.to(dt),
                                                    token_type_ids, attention_mask, image_attention_mask,
                                                    task_ids, collect)
         if compute_pretraining_heads:
@@ -500,7 +502,7 @@ class VILBertForVLTasks(nn.Module):
             vil_binary_prediction = self.vil_binary_prediction(pooled.view(-1, pooled.size(1) * 2))
         vil_logit = self.vil_logit(pooled)
         vil_tri_prediction = self.vil_tri_prediction(pooled)
-        vision_logit = self.vision_logit(v) + ((1.0 - image_attention_mask.float()) * -10000.0).unsqueeze(2)
+        vision_logit = self.vision_logit(v) + ((1.0 - image_attention_mask.to(dt)) * -10000.0).unsqueeze(2)
         linguisic_logit = self.linguisic_logit(t)
         if collect is not None:
             collect["final"] = (t, v, pooled_t, pooled_v)

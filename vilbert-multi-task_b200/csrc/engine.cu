@@ -1019,6 +1019,7 @@ struct vb200_engine {
         e.pdl = opt.use_pdl ? 5 : 0;
         e.a_f16 = opt.act_fp16; e.out_f16 = opt.act_fp16;
         e.m_rows = m_rows;
+        e.split_acc = x3 ? 1 : 0;
         if (ln) {
             e.out_f32 = pl.y_scratch[stream]; e.ld_f32 = W.N;
         } else {
@@ -1029,7 +1030,7 @@ struct vb200_engine {
         // Small forwards (<= lone_rows rows in either stream, batch <= 8): 64-wide tiles while they still fit one CTA per SM -- twice
         // the CTAs, half the epilogue each.  The tile width never changes an element's accumulation order.  RowHeads plans bring
         // their bucket M as pl.B = 1, pl.T = pl.V = M.
-        int block_n = vb::gemm_p_pick_block_n(W.N);
+        int block_n = x3 ? 64 : vb::gemm_p_pick_block_n(W.N);      // the fp32-parity kernel runs 64-wide tiles only
         if (lone_rows > 0 && !x3 && block_n == 128 && W.N % 64 == 0 &&
             std::max(pl.B * pl.T, pl.B * pl.V) <= lone_rows && ((a_rows + 127) / 128) * (W.N / 64) <= vb::num_sms_host())
             block_n = 64;
@@ -2827,8 +2828,9 @@ int vb200_linear_split(const void* x16, int64_t ld_x, const void* w16, int64_t l
         e.M = (int)M; e.N = (int)N; e.K = (int)K3; e.bias = bias; e.out_bf16 = static_cast<bf16*>(y16);
         e.ld_bf16 = (int)ld_y16; e.out_f32 = y_f32; e.ld_f32 = (int)ld_y_f32; e.act = act; e.a_f16 = 1; e.out_f16 = 1;
         e.split16 = y16 != nullptr ? 1 : 0;
-        // as the engine's fp32-parity GEMMs: the cooperative kernel, the TMA store for an fp32-only output
-        CUDA_CHECK(make_gemm(x16, ld_x, w16, ld_w, e, {0, 0}).launch(static_cast<cudaStream_t>(cuda_stream)));
+        e.split_acc = 1;
+        // as the engine's fp32-parity GEMMs: the cooperative kernel at 64-wide tiles, the TMA store for an fp32-only output
+        CUDA_CHECK(make_gemm(x16, ld_x, w16, ld_w, e, {64, 0}).launch(static_cast<cudaStream_t>(cuda_stream)));
     });
 }
 

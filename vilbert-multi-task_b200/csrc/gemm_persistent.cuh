@@ -27,7 +27,8 @@ constexpr int kBlockK = 64;
 constexpr int kMmaK = 16;
 
 // MODE 0: default.  MODE 3: the same kernel with the fp32-parity mode's hi | lo | hi 16-bit output (a compile-time variant so the
-// default kernel's register budget is untouched).  MODE 6 ("ROWS"): MODE 0 whose tile list ends at a device row count
+// default kernel's register budget is untouched).  MODE 7: MODE 3 summing each k-block's wgmma result in round-to-nearest fp32 on
+// the CUDA cores (GemmEpilogue::split_acc, the engine's fp32-parity GEMMs; 64-wide tiles).  MODE 6 ("ROWS"): MODE 0 whose tile list ends at a device row count
 // (GemmEpilogue::m_rows, packed batches) -- a variant of its own so that MODE 0 keeps its register allocation.
 // MODE 0 and 6 also come 192 wide (96 accumulators per consumer thread, a 2-stage ring): 128 x 192 tiles cover an N = 3072 GEMM in
 // 16 column tiles instead of 24.
@@ -370,6 +371,28 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
         auto mma_tile = [&](int tile, uint32_t it) __attribute__((always_inline)) {
             float d[BLOCK_N / 2];
             int prev = -1;
+            if constexpr (MODE == 7) {
+                // fp32-parity mode (GemmEpilogue::split_acc): every k-block (one of hi.hi, lo.hi, hi.lo over 64 columns) starts from zero in the wgmma
+                // accumulator and is added to `sum` on the CUDA cores, round to nearest.  Accumulating all K' = 3K products in the
+                // wgmma accumulator loses bits at every k step instead, an error that grows with K: on the 268 M model (K = 768 ...
+                // 3072) it put the forward ~15x further from fp64 than fp32 arithmetic is.  One k-block in flight at a time.
+                float sum[BLOCK_N / 2];
+                for (int kb = 0; kb < num_kb; ++kb) {
+                    mbar_wait_nocall(&full_bar[ks], kphase);
+                    const uint64_t da = da0 + kDescStage * static_cast<uint64_t>(ks);
+                    const uint64_t db = db0 + kDescStage * static_cast<uint64_t>(ks);
+                    mma_kblock<BLOCK_N, F16>(d, da, db, true);
+                    wgmma_wait<0>();
+                    release(ks);
+                    if (++ks == kStages) { ks = 0; kphase ^= 1u; }
+#pragma unroll
+                    for (int j = 0; j < BLOCK_N / 2; ++j) sum[j] = kb == 0 ? d[j] : __fadd_rn(sum[j], d[j]);
+                }
+                if (p.pdl && threadIdx.x == 0 && tile + tile_stride >= total_tiles) pdl_launch_dependents();
+                acc_deposit<BLOCK_N>(s_acc, sum, threadIdx.x);
+                epi_bar_sync<kEpiThreads>();
+                return;
+            }
             for (int kb = 0; kb < num_kb; ++kb) {
                 mbar_wait_nocall(&full_bar[ks], kphase);
 #ifdef VB200_STAMPS
@@ -478,7 +501,7 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
                 const bool fast32 = st_fast && nvalid > 0 && p.out_f32 != nullptr;                 // all warp-uniform
                 if (fast32) store_f32_sw(xb, out_f32, p.ld_f32, m0 + q * 32, p.M, nc, v, lane, nvalid);
                 if (fast16) {
-                    if constexpr (MODE == 3) {
+                    if constexpr (MODE == 3 || MODE == 7) {
                         // fp32-parity mode: the 16-bit operand is written as fp16 hi | lo | hi per 64 columns (split_col),
                         // so the consuming GEMM's K' = 3K contraction against W' = hi | hi | lo adds hi.hi + lo.hi + hi.lo
                         const int c3 = split_col(nc);

@@ -20,15 +20,16 @@ static cudaError_t dispatch_act(const CUtensorMap& ta, const CUtensorMap& tb, co
     return cudaErrorInvalidValue;
 }
 
-// fp32-parity mode (fp16 hi/lo operands, K' = 3K): PCfg MODE 3 writes the 16-bit output as hi | lo | hi; GELU with the 1.5e-7 erf
-template <int BN>
+// fp32-parity mode (fp16 hi/lo operands, K' = 3K): PCfg MODE 3 writes the 16-bit output as hi | lo | hi; GELU with the 1.5e-7 erf.
+// MODE 7 is MODE 3 whose k-blocks are summed with round-to-nearest fp32 adds (GemmEpilogue::split_acc).
+template <int BN, int MODE>
 static cudaError_t dispatch_split(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap* tc, const GemmEpilogue& ep, int pct,
                                 cudaStream_t st) {
     switch (ep.act) {
-        case kActNone: return launch_p<BN, kActNone, true, 3>(ta, tb, tc, ep, pct, st);
+        case kActNone: return launch_p<BN, kActNone, true, MODE>(ta, tb, tc, ep, pct, st);
         case kActGelu:
-        case kActGeluExact: return launch_p<BN, kActGeluExact, true, 3>(ta, tb, tc, ep, pct, st);
-        case kActRelu: return launch_p<BN, kActRelu, true, 3>(ta, tb, tc, ep, pct, st);
+        case kActGeluExact: return launch_p<BN, kActGeluExact, true, MODE>(ta, tb, tc, ep, pct, st);
+        case kActRelu: return launch_p<BN, kActRelu, true, MODE>(ta, tb, tc, ep, pct, st);
     }
     return cudaErrorInvalidValue;
 }
@@ -36,11 +37,14 @@ static cudaError_t dispatch_split(const CUtensorMap& ta, const CUtensorMap& tb, 
 cudaError_t launch_gemm_persistent_plain(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap* tc, const GemmEpilogue& ep,
                                          int block_n, int pct, cudaStream_t st) {
     if (ep.M < 1 || ep.N < 1 || ep.K < 1 || ep.a_f16 != ep.out_f16) return cudaErrorInvalidValue;
-    if (ep.split16 || ep.act == kActGeluExact) {
-        // hi | lo | hi output: fp16, whole 64-column groups, no TMA store; narrow tiles only (the mode is for parity, not speed)
-        if (!ep.a_f16 || (ep.split16 && (ep.out_bf16 == nullptr || (ep.N & 63) || (ep.ld_bf16 & 7))) || ep.tma_store == 1)
+    if (ep.split16 || ep.split_acc || ep.act == kActGeluExact) {
+        // hi | lo | hi output: fp16, whole 64-column groups, no TMA store; narrow tiles only (the mode is for parity, not speed).
+        // The k-block sums of MODE 7 take 64-wide tiles only (128-wide ones spill).
+        if (!ep.a_f16 || (ep.split16 && (ep.out_bf16 == nullptr || (ep.N & 63) || (ep.ld_bf16 & 7))) || ep.tma_store == 1 ||
+            (ep.split_acc && block_n != 64))
             return cudaErrorInvalidValue;
-        return block_n == 64 ? dispatch_split<64>(ta, tb, tc, ep, pct, st) : dispatch_split<128>(ta, tb, tc, ep, pct, st);
+        if (ep.split_acc) return dispatch_split<64, 7>(ta, tb, tc, ep, pct, st);
+        return block_n == 64 ? dispatch_split<64, 3>(ta, tb, tc, ep, pct, st) : dispatch_split<128, 3>(ta, tb, tc, ep, pct, st);
     }
     const bool rows = ep.m_rows != nullptr;          // MODE 6: the tile list ends at a device row count (packed batches)
     switch (block_n) {

@@ -36,6 +36,9 @@ struct GemmEpilogue {
                                   // before the launch's graph starts, so it is read ahead of griddepcontrol.wait.  Honoured by
                                   // the persistent kernel (PCfg MODE 6 in place of MODE 0); the fp32-parity kernel
                                   // computes every row.
+    int split_acc;                // fp32-parity mode: A and W are hi / lo split operands over K' = 3K.  The kernel (PCfg MODE 7,
+                                  // 64-wide tiles) sums each 64-wide k-block's wgmma result into a separate fp32 accumulator with
+                                  // round-to-nearest adds: the tensor cores' own fp32 accumulation over K' drifts with K.
 };
 
 // persistent CTAs, wgmma consumer warpgroups (gemm_persistent.cuh)
