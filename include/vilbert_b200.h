@@ -196,8 +196,9 @@ int vb200_forward_host(vb200_handle h, const vb200_inputs* in, const vb200_outpu
 int vb200_forward_host_slot(vb200_handle h, const vb200_inputs* in, const vb200_outputs* out, uint32_t select, int32_t slot,
                             int32_t synchronize, void* cuda_stream);
 
-/* Introspection used by the tests / bench: number of kernels one forward of this shape launches,
- * algorithmic FLOPs of it, model dimensions ("max_rows_per_sample": the engine's current bound, see vb200_set_option). */
+/* Introspection used by the tests / bench: number of kernels one forward of this shape launches (with VB200_OUT_ATTENTION: one with
+ * the current map selection), algorithmic FLOPs of it, model dimensions ("max_rows_per_sample": the engine's current bound;
+ * "attention_entries" (-1 above 63 entries) and "attention_heads": the map selection; see vb200_set_option). */
 int vb200_plan_info(vb200_handle h, int32_t batch, int32_t n_tokens, int32_t n_regions, uint32_t select,
                     int64_t* n_launches, double* flops);
 int vb200_model_dim(vb200_handle h, const char* key, int64_t* value);
@@ -210,7 +211,15 @@ int vb200_model_dim(vb200_handle h, const char* key, int64_t* value);
  * max_position_embeddings as well, and vb200_select_regions keeps at most this - 1 boxes per image.  Up to 256 rows per sample a
  * plan's attention stages each (sample, head) whole in shared memory; a plan with more rows in a stream runs that stream's
  * attention on the streaming kernels (vb200_self_attention_stream), which give the same bits wherever both run.  The choice
- * follows from the plan's shape alone, so the bound only changes validation and no cached plan is dropped. */
+ * follows from the plan's shape alone, so the bound only changes validation and no cached plan is dropped.
+ * Attention maps by selection (VB200_OUT_ATTENTION and VB200_OUT_ATTENTION_PACKED): "attention_entries" is a bitmask over the entries
+ * of the full list in execution order (bit e: entry e of vb200_attention_selection; default every entry) and "attention_heads" 0
+ * (default) writes every head, 1 each selected entry averaged over its heads: (sum over h = 0..heads-1 of p_h, added left to right in
+ * fp32) / heads, each p_h bit-identical to the per-head map.  A zero mask, a bit at or past the entry count, a configuration with more
+ * than 63 entries (the default then stays every entry) or attention_heads outside {0, 1} is VB200_ERR_INVALID.  Both stay in force
+ * until changed and both are readable through vb200_model_dim.  The selection is part of the plan key of a forward with maps: the first
+ * call after a change builds (or finds) the plan of the new selection, and a plan without maps is unaffected.  Every other output is
+ * bit-identical whatever the selection. */
 int vb200_set_option(vb200_handle h, const char* key, int64_t value);
 /* Profiling: after vb200_set_option(h, "timeline", 1) every persistent GEMM launch of a forward records 16 stamps per CTA (0: clock64 at
  * entry, 1: setup done, 2: first k-block landed [-DVB200_STAMPS builds], 8 / 9: %globaltimer ns at entry / exit, 10: last tile accumulated,
@@ -229,9 +238,17 @@ int vb200_profile_ops(vb200_handle h, int32_t batch, int32_t n_tokens, int32_t n
  * (heads, query length, key length) at float offset offsets[i]; dims[4i+3] is the layer kind: 0 text layer, 1 image layer,
  * 2 connection layer, text queries over image keys, 3 connection layer, image queries over text keys (kinds 2 and 3 of one layer
  * are adjacent: the reference's per-layer tuple).  *n_entries receives the entry count (30 for the 12/6/6 configuration: 24
- * layers, two tensors per connection layer), total_floats the buffer size.  Arrays may be NULL to query the count only. */
+ * layers, two tensors per connection layer), total_floats the buffer size.  Arrays may be NULL to query the count only.
+ * Under a map selection (vb200_set_option "attention_entries" / "attention_heads") the layout holds the selected entries only, in
+ * execution order: *n_entries is the mask's popcount, heads is 1 under the head mean, the kind is unchanged; each entry's index in
+ * the full list is vb200_attention_selection's. */
 int vb200_attention_layout(vb200_handle h, int32_t batch, int32_t n_tokens, int32_t n_regions, int32_t max_entries,
                            int32_t* n_entries, int32_t* dims, int64_t* offsets, int64_t* total_floats);
+/* The full list of attention-map entries in execution order and the engine's current selection of it: *n_entries receives the full
+ * count (30 for the 12/6/6 configuration), kinds[e] entry e's kind (as dims[4i+3] above) and layout_entry[e] its index in the
+ * layouts of vb200_attention_layout / vb200_attention_layout_packed, or -1 when "attention_entries" leaves it out.  Arrays (up to
+ * max_entries) may be NULL to query the count only. */
+int vb200_attention_selection(vb200_handle h, int32_t max_entries, int32_t* n_entries, int32_t* kinds, int32_t* layout_entry);
 
 /* custom_prediction()'s tensor construction fused into the forward (worker.py:422-455): instead of features [B, V, F] /
  * spatials [B, V, 5] / image_mask the caller passes what the detector produced -- box features, pixel boxes, image sizes -- and one
@@ -317,7 +334,10 @@ int vb200_forward_regions_packed(vb200_handle h, const vb200_packed_region_input
  * offsets[e] and holds, for sample b in batch order, a contiguous [heads, Lq_b, Lk_b] block at heads * sum_{b' < b} Lq_b' * Lk_b'
  * inside the entry, with (Lq_b, Lk_b) = (T_b, T_b), (V_b, V_b), (T_b, V_b) or (V_b, T_b) for kinds 0-3 and T_b = Tin_b + 1 (task token).
  * dims[2e] = heads, dims[2e + 1] = kind; total_floats is the buffer size (every float of it is written); arrays may be NULL to query
- * the count only.  Builds no plan and never blocks.  n_tokens / n_regions are HOST arrays of Tin_b and V_b, validated as the
+ * the count only.  Under a map selection (vb200_set_option "attention_entries" / "attention_heads") the entries are the selected ones
+ * only, in execution order, with heads 1 under the head mean (sample b's block is then [Lq_b, Lk_b] at prefix[b]); each entry's index
+ * in the full list is vb200_attention_selection's.
+ * Builds no plan and never blocks.  n_tokens / n_regions are HOST arrays of Tin_b and V_b, validated as the
  * packed forwards validate them (a length < 1, T_b or V_b above max_rows_per_sample, Tin_b > max_position_embeddings: VB200_ERR_INVALID); for
  * vb200_forward_regions_packed pass V_b = n_boxes_b + 1.
  * A forward with the bit needs vb200_outputs.attention_probs (VB200_ERR_INVALID if NULL): the probability kernels write into it

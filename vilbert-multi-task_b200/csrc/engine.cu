@@ -414,6 +414,7 @@ struct LayerNormArgs {             // out = LN(y + res)
 struct AttnF32Args {
     const void *q, *k, *v; int ld_q, ld_kv, in_kind; const float* mask; int B, Lq, Lk, heads, head_dim;
     bf16* ctx; int ld_ctx, ctx_mode; float* probs; bool packed; vb::PackedProbs pk;
+    bool mean;                     // the head-mean kernel: maps only, [B, Lq, Lk] (packed: heads factor 1)
 };
 // Row offs[b] of src16 (ld16 wide) -> row b of dst16, b < B, clamped to n_src rows; with src_f32 the same row (`hidden` wide) -> dst_f32.
 struct GatherArgs { const int* offs; int n_src, B; const bf16* src16; bf16* dst16; int ld16; const float* src_f32; float* dst_f32; int hidden; };
@@ -453,17 +454,38 @@ struct MetaLayout {
     size_t size() const { return n_entries ? probs_prefix(3) : rows_end(); }
 };
 
-// Layout of the packed attention probabilities (VB200_OUT_ATTENTION_PACKED) from the two streams' row offsets [B + 1]: entries in
-// execution order (the order get_plan adds the probability ops in), each holding sample b's [heads, Lq_b, Lk_b] block at
-// heads * prefix[b]; prefix = sum over b' < b of T_b'^2 (text layers), V_b'^2 (image layers) or T_b' V_b' (both directions of a
-// connection layer).  int64 throughout: at batch 512 with 256 rows per sample one call holds more than 2^31 floats.
+// Which attention maps a forward writes (vb200_set_option "attention_entries" / "attention_heads"): bit e of `mask` selects entry e
+// of the full list (execution order; a configuration with more than 63 entries always writes every entry), `mean` writes each
+// selected entry averaged over heads (heads 1 in the layouts).  The default is every entry, every head.
+struct AttnSelect {
+    uint64_t mask = ~0ull;
+    bool mean = false;
+    bool has(int e) const { return e > 63 || ((mask >> e) & 1); }
+    int heads(int h) const { return mean ? 1 : h; }
+};
+// The full list's entries in execution order: kinds 0 text layer, 1 image layer, 2 / 3 the two directions of a connection layer.
+std::vector<int> attention_kinds(const std::vector<std::string>& schedule) {
+    std::vector<int> k;
+    for (const std::string& step : schedule) {
+        if (step[0] == 'T') k.push_back(0);
+        else if (step[0] == 'V') k.push_back(1);
+        else { k.push_back(2); k.push_back(3); }
+    }
+    return k;
+}
+
+// Layout of the packed attention probabilities (VB200_OUT_ATTENTION_PACKED) from the two streams' row offsets [B + 1]: the selected
+// entries in execution order (the order get_plan adds the probability ops in), each holding sample b's [heads, Lq_b, Lk_b] block at
+// heads * prefix[b] (heads 1 under the head mean); prefix = sum over b' < b of T_b'^2 (text layers), V_b'^2 (image layers) or
+// T_b' V_b' (both directions of a connection layer).  int64 throughout: at batch 512 with 256 rows per sample one call holds more than 2^31 floats.
 struct PackedAttnLayout {
     std::vector<int32_t> heads, kind;
     std::vector<int64_t> offset;
     std::vector<int64_t> prefix;       // [3][B + 1]
     int64_t total = 0;
 };
-PackedAttnLayout packed_attn_layout(const Config& c, const std::vector<std::string>& schedule, int B, const int* offs_t, const int* offs_v) {
+PackedAttnLayout packed_attn_layout(const Config& c, const std::vector<std::string>& schedule, const AttnSelect& sel, int B,
+                                    const int* offs_t, const int* offs_v) {
     PackedAttnLayout l;
     const size_t n = static_cast<size_t>(B) + 1;
     l.prefix.assign(3 * n, 0);
@@ -473,16 +495,14 @@ PackedAttnLayout packed_attn_layout(const Config& c, const std::vector<std::stri
         l.prefix[n + b + 1] = l.prefix[n + b] + V * V;
         l.prefix[2 * n + b + 1] = l.prefix[2 * n + b] + T * V;
     }
-    auto put = [&](int heads, int kind) {
+    const std::vector<int> kinds = attention_kinds(schedule);
+    for (int e = 0; e < static_cast<int>(kinds.size()); ++e) {
+        if (!sel.has(e)) continue;
+        const int kind = kinds[e], heads = sel.heads(kind == 0 ? c.heads : kind == 1 ? c.v_heads : c.bi_heads);
         l.heads.push_back(heads);
         l.kind.push_back(kind);
         l.offset.push_back(l.total);
         l.total += heads * l.prefix[(kind < 2 ? kind : 2) * n + B];
-    };
-    for (const std::string& step : schedule) {
-        if (step[0] == 'T') put(c.heads, 0);
-        else if (step[0] == 'V') put(c.v_heads, 1);
-        else { put(c.bi_heads, 2); put(c.bi_heads, 3); }
     }
     return l;
 }
@@ -516,9 +536,9 @@ struct PackedBatch {
 // Validates a packed call's lengths and lays out its rows: offs[i + 1] = offs[i] + rows_i per stream (text: T_i = Tin_i + task
 // token).  Rejects a batch < 1, a negative capacity, a length < 1 or above a non-zero capacity, more than max_rows rows per sample
 // (the engine's max_rows_per_sample) and Tin_i > max_position_embeddings.  maps (non-null): where the plan's kernels write the packed
-// attention probabilities, whose layout then joins the meta.
+// attention probabilities of the entries `sel` selects, whose layout then joins the meta.
 PackedBatch pack_batch(const char* api, const Config& c, const std::vector<std::string>& schedule, const PackedLengths& in, float* maps,
-                       int max_rows) {
+                       int max_rows, const AttnSelect& sel = {}) {
     if (in.B < 1) fail(VB200_ERR_INVALID, "%s: batch must be positive", api);
     if (in.max_tokens < 0) fail(VB200_ERR_INVALID, "%s: negative capacity max_tokens %d", api, in.max_tokens);
     if (in.max_regions < 0) fail(VB200_ERR_INVALID, "%s: negative capacity max_regions %d", api, in.max_regions);
@@ -555,7 +575,7 @@ PackedBatch pack_batch(const char* api, const Config& c, const std::vector<std::
         std::copy(in.src_v, in.src_v + in.B, b.meta.begin() + b.layout.src_v());
     }
     if (maps) {
-        const PackedAttnLayout l = packed_attn_layout(c, schedule, in.B, b.offs_t(), b.offs_v());
+        const PackedAttnLayout l = packed_attn_layout(c, schedule, sel, in.B, b.offs_t(), b.offs_v());
         const int64_t dst = static_cast<int64_t>(reinterpret_cast<uintptr_t>(maps));
         b.layout.n_entries = l.offset.size();
         b.meta.resize(b.layout.size(), 0);
@@ -667,6 +687,7 @@ struct vb200_engine {
     // vb200_set_option("max_rows_per_sample"), 256..1024: the longest text (T = Tin + task token) or image (V) sequence a call may
     // bring.  Validation only -- a plan's attention kernels follow from its shape (streaming above 256 rows), so no plan is dropped.
     int max_rows = 256;
+    AttnSelect attn_sel;       // vb200_set_option("attention_entries" / "attention_heads"): the maps a forward with the map bit writes
     bool x3 = false;           // fp32-parity mode (vb200_options::split_fp32): fp16 hi/lo split operands, K' = 3K GEMMs, fp32 attention
     // Programmatic dependent launch (opt.use_pdl): every kernel triggers its dependents once its main work is issued, and a
     // dependent GEMM's producer puts its first weight tiles in flight before griddepcontrol.wait.  On by default;
@@ -1057,34 +1078,51 @@ struct vb200_engine {
     // kernel writes the context (callers push that op themselves); this adds the fp32 kernel -- as THE attention in fp32-parity
     // mode (context out as hi | lo | hi), and/or as the producer of the attention-probability output.  Packed plans: the
     // probabilities of every sample at its own lengths (query rows offs_q, key rows offs_k) straight into the caller's buffer, at
-    // the entry's offset and the sample's prefix sum `prefix` (0 T^2, 1 V^2, 2 T V) of the plan's probability meta.
+    // the entry's offset and the sample's prefix sum `prefix` (0 T^2, 1 V^2, 2 T V) of the plan's probability meta.  want_probs: the
+    // entry is selected (attn_sel); under the head mean its maps come from a maps-only head-mean launch, after the fp32-parity
+    // mode's context launch.  Adds nothing outside fp32-parity mode for an entry that is not selected.
     void add_attn_f32(Plan& pl, const void* q, int ld_q, const void* k, const void* v, int ld_kv, const float* mask, int Lq, int Lk,
                       int heads, int hid, bf16* ctx, bool want_probs, int stream, const int* offs_q = nullptr,
                       const int* offs_k = nullptr, int prefix = 0) {
+        const bool mean = want_probs && attn_sel.mean;
         AttnF32Args a{};
         a.q = q; a.k = k; a.v = v; a.ld_q = ld_q; a.ld_kv = ld_kv; a.mask = mask; a.Lq = Lq; a.Lk = Lk;
         a.in_kind = x3 ? 0 : (opt.act_fp16 ? 1 : 2);
         a.B = pl.B; a.heads = heads; a.head_dim = hid / heads;
-        a.ctx = x3 ? ctx : nullptr; a.ctx_mode = x3 ? 3 : 0; a.ld_ctx = x3 ? 3 * hid : 0;
-        if (want_probs && pl.packed) {
+        if (x3) {
+            AttnF32Args c = a;
+            c.ctx = ctx; c.ctx_mode = 3; c.ld_ctx = 3 * hid;
+            if (want_probs && !mean) c.probs = attn_out(pl, heads, Lq, Lk);
+            pl.ops.push_back({c, stream, 4.0 * pl.B * heads * Lq * Lk * (hid / heads)});
+        }
+        if (!want_probs || (x3 && !mean)) return;
+        a.mean = mean;
+        if (pl.packed) {
             const MetaLayout& m = pl.layout;
             a.packed = true;
             a.pk = vb::PackedProbs{offs_q, offs_k, pl.meta64(m.probs_dst()), pl.meta64(m.probs_entry(pl.n_probs)),
                                    pl.meta64(m.probs_prefix(prefix))};
             ++pl.n_probs;
-        } else if (want_probs) {
-            a.probs = pl.mem.alloc_n<float>(static_cast<size_t>(pl.B) * heads * Lq * Lk);
-            pl.attn.push_back(Plan::AttnOut{a.probs, heads, Lq, Lk});
+        } else {
+            a.probs = attn_out(pl, mean ? 1 : heads, Lq, Lk);
         }
-        pl.ops.push_back({a, stream, x3 ? 4.0 * pl.B * heads * Lq * Lk * (hid / heads) : 0.0});
+        pl.ops.push_back({a, stream, 0.0});
+    }
+    // a dense plan's next attention-probability output [B, heads, Lq, Lk]
+    static float* attn_out(Plan& pl, int heads, int Lq, int Lk) {
+        float* p = pl.mem.alloc_n<float>(static_cast<size_t>(pl.B) * heads * Lq * Lk);
+        pl.attn.push_back(Plan::AttnOut{p, heads, Lq, Lk});
+        return p;
     }
     Op rowdot_op(const float* x, int ld_x, const RowW& w, const float* add, float* out, int ld_out, int M, const int* m_rows = nullptr) {
         return {RowdotArgs{x, w.w, w.b, add, out, ld_x, ld_out, M, w.K, w.n_out, m_rows}, 0, 2.0 * M * w.K * w.n_out};
     }
-    // attention-probability entries of one forward: one per text / image layer, two per connection layer
-    int attention_entries() const {
+    // attention-probability entries one forward with maps writes: the selected ones of the full list (one per text / image layer,
+    // two per connection layer)
+    int selected_entries() const {
+        const int all = static_cast<int>(attention_kinds(schedule).size());
         int n = 0;
-        for (const std::string& step : schedule) n += step[0] == 'C' ? 2 : 1;
+        for (int e = 0; e < all; ++e) n += attn_sel.has(e) ? 1 : 0;
         return n;
     }
     OutBuf make_out(Plan& pl, int rows, int cols) {
@@ -1144,7 +1182,9 @@ struct vb200_engine {
         const int cap = mode >= PACKED ? (max_rows + 15) / 16 * 16 : max_rows;
         if (T > cap || V > cap)
             fail(VB200_ERR_INVALID, "sequence too long for %s (T=%d, V=%d, max %d)", bound_name(max_rows), T, V, cap);
-        std::vector<int64_t> key{B, Tin, V, static_cast<int64_t>(select), slot, mode, want_attn ? 1 : 0};
+        // the map selection is part of the key of a plan with maps: a call never replays a plan built for another selection
+        std::vector<int64_t> key{B, Tin, V, static_cast<int64_t>(select), slot, mode, want_attn ? 1 : 0,
+                                 want_attn ? static_cast<int64_t>(attn_sel.mask) : 0, want_attn && attn_sel.mean ? 1 : 0};
         auto it = plans.find(key);
         if (it != plans.end()) { it->second->last_use = ++use_clock; return it->second.get(); }
         std::unique_ptr<Plan> up(new Plan());
@@ -1156,7 +1196,7 @@ struct vb200_engine {
         if (packed) {
             // zero offsets until the first call: the validation pass and the capture below then touch no row
             pl.packed = true;
-            pl.layout = MetaLayout{static_cast<size_t>(B), want_attn ? static_cast<size_t>(attention_entries()) : 0, mode == PACKED_SUFFIX};
+            pl.layout = MetaLayout{static_cast<size_t>(B), want_attn ? static_cast<size_t>(selected_entries()) : 0, mode == PACKED_SUFFIX};
             const size_t n_meta = pl.layout.size();
             pl.d_meta = pl.mem.alloc_n<int>(n_meta);
             CUDA_CHECK(cudaMemset(pl.d_meta, 0, n_meta * sizeof(int)));
@@ -1240,7 +1280,7 @@ struct vb200_engine {
         // one BertLayer / BertImageLayer.  `tail` (the pruned tail): Q, K, V and the attention on every row (each is a key and a
         // value), the rest on each sample's first row -- read at stride seq rows on dense plans, gathered from the sample offsets on
         // packed ones -- into compact [B, hid] rows; returns their 16-bit copy (null without `tail`).
-        auto single_layer = [&](const LayerW& L, StreamSt& st, int inter, int heads, bool tail) -> bf16* {
+        auto single_layer = [&](const LayerW& L, StreamSt& st, int inter, int heads, bool tail, int entry) -> bf16* {
             const int hid = st.hid, cur = st.cur, M = st.rows, stream = st.stream;
             bf16* qb; float* qf;
             qkv_out(st.qkv, qb, qf);
@@ -1255,7 +1295,8 @@ struct vb200_engine {
             }
             if (x3 || want_attn)
                 add_attn_f32(pl, qkv_at(st.qkv, 0), 3 * hid, qkv_at(st.qkv, hid), qkv_at(st.qkv, 2 * hid), 3 * hid, st.mask, st.seq, st.seq,
-                             heads, hid, st.ctx, want_attn, stream, st.offs, st.offs, stream);   // prefix: stream 0 T^2, 1 V^2
+                             heads, hid, st.ctx, want_attn && attn_sel.has(entry), stream, st.offs, st.offs,
+                             stream);                                      // prefix: stream 0 T^2, 1 V^2
             if (tail) {
                 const bf16* ctx = st.ctx;
                 const float* res = st.f32[cur];
@@ -1289,8 +1330,11 @@ struct vb200_engine {
         for (Op& op : ops) op.tag = "embed";
         bool in_suffix = false;
         size_t tagged = ops.size();
+        int n_entry = 0;                               // the step's first attention-map entry in the full list
         for (size_t si = 0; si < schedule.size(); ++si) {
             const std::string& step = schedule[si];
+            const int entry = n_entry;
+            n_entry += step[0] == 'C' ? 2 : 1;
             for (; tagged < ops.size(); ++tagged) if (ops[tagged].tag == nullptr) ops[tagged].tag = "?";
             const int idx = atoi(step.c_str() + 1);
             if (step[0] == 'C') in_suffix = true;
@@ -1299,9 +1343,9 @@ struct vb200_engine {
                 ~Tagger() { for (size_t i = from; i < ops.size(); ++i) ops[i].tag = name; }
             } tagger{ops, ops.size(), step.c_str()};
             if (step[0] == 'T') {
-                if (in_suffix ? do_s : do_t) pl.tail_t = single_layer(t_layers[idx], ts, c.inter, c.heads, prune_t && si == last_t);
+                if (in_suffix ? do_s : do_t) pl.tail_t = single_layer(t_layers[idx], ts, c.inter, c.heads, prune_t && si == last_t, entry);
             } else if (step[0] == 'V') {
-                if (in_suffix ? do_s : do_v) pl.tail_v = single_layer(v_layers[idx], vs, c.v_inter, c.v_heads, prune_v && si == last_v);
+                if (in_suffix ? do_s : do_v) pl.tail_v = single_layer(v_layers[idx], vs, c.v_inter, c.v_heads, prune_v && si == last_v, entry);
             } else if (do_s) {
                 const ConnW& W = c_layers[idx];
                 const int tcur = ts.cur, vcur = vs.cur;
@@ -1324,9 +1368,9 @@ struct vb200_engine {
                 if (x3 || want_attn) {
                     // text queries (Q2) over image keys / values (K1, V1) -> text context; then image queries (Q1) over K2, V2
                     add_attn_f32(pl, qkv_at(qkv_t, 0), 3 * Hb, qkv_at(qkv_v, Hb), qkv_at(qkv_v, 2 * Hb), 3 * Hb, pl.mask_v, T, V,
-                                 c.bi_heads, Hb, ctx_t, want_attn, 0, offs_t, offs_v, 2);
+                                 c.bi_heads, Hb, ctx_t, want_attn && attn_sel.has(entry), 0, offs_t, offs_v, 2);
                     add_attn_f32(pl, qkv_at(qkv_v, 0), 3 * Hb, qkv_at(qkv_t, Hb), qkv_at(qkv_t, 2 * Hb), 3 * Hb, pl.mask_t, V, T,
-                                 c.bi_heads, Hb, ctx_v, want_attn, 0, offs_v, offs_t, 2);
+                                 c.bi_heads, Hb, ctx_v, want_attn && attn_sel.has(entry + 1), 0, offs_v, offs_t, 2);
                 }
                 ops[first_co].sync = Op::JOIN;              // needs both projections
                 // image branch (side stream; forks from the co-attention): biOutput.dense1 + LayerNorm1, v_intermediate, v_output + LayerNorm
@@ -1515,6 +1559,11 @@ struct vb200_engine {
                                                   a.ld16, a.M, a.N, f16, x3 ? 1 : 0, pdl, st, a.m_rows));
             },
             [&](const AttnF32Args& a) {
+                if (a.mean) {
+                    CUDA_CHECK(vb::launch_attention_f32_mean(a.q, a.ld_q, a.k, a.ld_kv, a.in_kind, a.mask, a.B, a.Lq, a.Lk, a.heads,
+                                                             a.head_dim, a.probs, pdl, st, a.packed ? &a.pk : nullptr));
+                    return;
+                }
                 CUDA_CHECK(vb::launch_attention_f32(a.q, a.ld_q, a.k, a.v, a.ld_kv, a.in_kind, a.mask, a.B, a.Lq, a.Lk, a.heads,
                                                     a.head_dim, a.ctx, a.ld_ctx, a.ctx_mode, a.probs, pdl, st,
                                                     a.packed ? &a.pk : nullptr));
@@ -1746,7 +1795,7 @@ struct vb200_engine {
         if (maps && out->attention_probs == nullptr)
             fail(VB200_ERR_INVALID, "%s: VB200_OUT_ATTENTION_PACKED needs vb200_outputs.attention_probs (NULL)", api);
         if (x3) fail(VB200_ERR_INVALID, "%s: packed batches are not supported in split_fp32 (fp32x) mode", api);
-        const PackedBatch b = pack_batch(api, cfg, schedule, len, maps ? out->attention_probs : nullptr, max_rows);
+        const PackedBatch b = pack_batch(api, cfg, schedule, len, maps ? out->attention_probs : nullptr, max_rows, attn_sel);
         CUDA_CHECK(cudaSetDevice(opt.device));
         Plan& pl = *get_plan(len.B, b.Tin, b.V, (select & VB200_OUT_ALL) | rows_read(out), slot, mode, maps);
         const cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
@@ -2552,23 +2601,23 @@ int vb200_attention_layout(vb200_handle h, int32_t batch, int32_t n_tokens, int3
                            int32_t* n_entries, int32_t* dims, int64_t* offsets, int64_t* total_floats) {
     if (h == nullptr || n_entries == nullptr) return VB200_ERR_INVALID;
     return guard(h, [&] {
-        // derived from the layer schedule alone (no plan is built): the order add_attn_f32 is called in by get_plan
+        // derived from the layer schedule and the map selection alone (no plan is built): the order add_attn_f32 is called in by
+        // get_plan
         const Config& c = h->cfg;
         const int T = n_tokens + (c.task_tokens ? 1 : 0), V = n_regions;
+        const std::vector<int> kinds = attention_kinds(h->schedule);
         int n = 0;
         int64_t off = 0;
-        auto put = [&](int heads, int lq, int lk, int kind) {
+        for (int e = 0; e < static_cast<int>(kinds.size()); ++e) {
+            if (!h->attn_sel.has(e)) continue;
+            const int kind = kinds[e], heads = h->attn_sel.heads(kind == 0 ? c.heads : kind == 1 ? c.v_heads : c.bi_heads);
+            const int lq = kind == 0 || kind == 2 ? T : V, lk = kind == 0 || kind == 3 ? T : V;
             if (n < max_entries) {
                 if (dims) { dims[4 * n] = heads; dims[4 * n + 1] = lq; dims[4 * n + 2] = lk; dims[4 * n + 3] = kind; }
                 if (offsets) offsets[n] = off;
             }
             off += static_cast<int64_t>(batch) * heads * lq * lk;
             ++n;
-        };
-        for (const std::string& step : h->schedule) {
-            if (step[0] == 'T') put(c.heads, T, T, 0);
-            else if (step[0] == 'V') put(c.v_heads, V, V, 1);
-            else { put(c.bi_heads, T, V, 2); put(c.bi_heads, V, T, 3); }
         }
         *n_entries = n;
         if (total_floats) *total_floats = off;
@@ -2583,7 +2632,7 @@ int vb200_attention_layout_packed(vb200_handle h, int32_t batch, const int32_t* 
         const char* api = "vb200_attention_layout_packed";
         if (!n_tokens || !n_regions) fail(VB200_ERR_INVALID, "%s: NULL length array", api);
         const PackedBatch b = pack_batch(api, h->cfg, h->schedule, {"sample", batch, n_tokens, 0, n_regions, 0}, nullptr, h->max_rows);
-        const PackedAttnLayout l = packed_attn_layout(h->cfg, h->schedule, batch, b.offs_t(), b.offs_v());
+        const PackedAttnLayout l = packed_attn_layout(h->cfg, h->schedule, h->attn_sel, batch, b.offs_t(), b.offs_v());
         const int n = static_cast<int>(l.heads.size());
         for (int e = 0; e < n && e < max_entries; ++e) {
             if (dims) { dims[2 * e] = l.heads[e]; dims[2 * e + 1] = l.kind[e]; }
@@ -2591,6 +2640,23 @@ int vb200_attention_layout_packed(vb200_handle h, int32_t batch, const int32_t* 
         }
         *n_entries = n;
         if (total_floats) *total_floats = l.total;
+    });
+}
+
+int vb200_attention_selection(vb200_handle h, int32_t max_entries, int32_t* n_entries, int32_t* kinds, int32_t* layout_entry) {
+    if (h == nullptr || n_entries == nullptr) return VB200_ERR_INVALID;
+    return guard(h, [&] {
+        const std::vector<int> k = attention_kinds(h->schedule);
+        int selected = 0;
+        for (int e = 0; e < static_cast<int>(k.size()); ++e) {
+            const bool has = h->attn_sel.has(e);
+            if (e < max_entries) {
+                if (kinds) kinds[e] = k[e];
+                if (layout_entry) layout_entry[e] = has ? selected : -1;
+            }
+            selected += has ? 1 : 0;
+        }
+        *n_entries = static_cast<int32_t>(k.size());
     });
 }
 
@@ -2634,7 +2700,8 @@ int vb200_plan_info(vb200_handle h, int32_t batch, int32_t n_tokens, int32_t n_r
     if (h == nullptr) return VB200_ERR_INVALID;
     return guard(h, [&] {
         CUDA_CHECK(cudaSetDevice(h->opt.device));
-        Plan* pl = h->get_plan(batch, n_tokens, n_regions, select & VB200_OUT_ALL);
+        Plan* pl = h->get_plan(batch, n_tokens, n_regions, select & VB200_OUT_ALL, 0, vb200_engine::FULL,
+                               (select & VB200_OUT_ATTENTION) != 0);
         if (n_launches) *n_launches = static_cast<int64_t>(pl->ops.size()) + 2;   // + text-embed + image-pack
         if (flops) *flops = pl->flops;
     });
@@ -2694,6 +2761,20 @@ int vb200_set_option(vb200_handle h, const char* key, int64_t value) {
             if (value < kStagedAttnRows || value > kMaxRowsPerSample)
                 fail(VB200_ERR_INVALID, "max_rows_per_sample must be in [%d, %d]", kStagedAttnRows, kMaxRowsPerSample);
             h->max_rows = static_cast<int>(value);       // validation only: every cached plan stays valid
+        } else if (k == "attention_entries") {
+            // the selection is part of the plan key of a plan with maps: no cached plan is dropped
+            const int n = static_cast<int>(attention_kinds(h->schedule).size());
+            if (n > 63)
+                fail(VB200_ERR_INVALID, "attention_entries: this configuration has %d attention entries, more than the 63 a mask holds", n);
+            const uint64_t full = (1ull << n) - 1;
+            if (value == 0 || (static_cast<uint64_t>(value) & ~full) != 0)
+                fail(VB200_ERR_INVALID, "attention_entries: mask 0x%llx must be non-zero and select only entries 0..%d",
+                     (unsigned long long)value, n - 1);
+            h->attn_sel.mask = static_cast<uint64_t>(value) == full ? ~0ull : static_cast<uint64_t>(value);
+        } else if (k == "attention_heads") {
+            if (value != 0 && value != 1)
+                fail(VB200_ERR_INVALID, "attention_heads must be 0 (every head) or 1 (the mean over heads), got %lld", (long long)value);
+            h->attn_sel.mean = value == 1;
         } else fail(VB200_ERR_INVALID, "unknown option \"%s\"", key);
     });
 }
@@ -2736,6 +2817,10 @@ int vb200_model_dim(vb200_handle h, const char* key, int64_t* value) {
         else if (k == "n_plans") *value = static_cast<int64_t>(h->plans.size());
         else if (k == "n_layers_scheduled") *value = static_cast<int64_t>(h->schedule.size());
         else if (k == "max_rows_per_sample") *value = h->max_rows;
+        else if (k == "attention_entries") {
+            const size_t n = attention_kinds(h->schedule).size();
+            *value = n > 63 ? -1 : static_cast<int64_t>(h->attn_sel.mask & ((1ull << n) - 1));
+        } else if (k == "attention_heads") *value = h->attn_sel.mean ? 1 : 0;
         else fail(VB200_ERR_INVALID, "unknown model dimension \"%s\"", key);
     });
 }

@@ -142,6 +142,12 @@ struct PackedProbs {
 cudaError_t launch_attention_f32(const void* q, int ld_q, const void* k, const void* v, int ld_kv, int in_kind,
                                  const float* key_mask_add, int B, int Lq, int Lk, int heads, int D, __nv_bfloat16* ctx, int ld_ctx,
                                  int ctx_mode, float* probs, int pdl, cudaStream_t st, const PackedProbs* packed = nullptr);
+// Head mean of the same probabilities (attention_f32.cu): probs [B, Lq, Lk] = (sum over heads in increasing order, in fp32) / heads,
+// each head's row computed as launch_attention_f32 computes it; no context.  packed: a PackedProbs entry whose per-sample blocks
+// are [Lq_b, Lk_b] (heads factor 1), probs NULL.
+cudaError_t launch_attention_f32_mean(const void* q, int ld_q, const void* k, int ld_kv, int in_kind, const float* key_mask_add, int B,
+                                      int Lq, int Lk, int heads, int D, float* probs, int pdl, cudaStream_t st,
+                                      const PackedProbs* packed = nullptr);
 // Pre-training heads at chosen rows: row rows[i] (device int32, i < n) of an fp32 state [*, H] -> row i of dst, in the 16-bit operand
 // form the final LayerNorm writes (mode 0 bf16, 1 fp16, 2 fp16 hi | lo | hi with ld_dst the 3x wide stride) or as fp32 (mode 3); rows
 // [n, rows_out) are zeroed.  H a multiple of 8 (64 in mode 2), 16-byte aligned src / dst; rows are bounds-checked on the host.

@@ -76,25 +76,63 @@ def packed_offsets(lengths, extra: int = 0):
     return offs
 
 
-def split_packed_attention(flat, layout, t_rows, v_rows):
+def attention_list(kinds, layout_entry, entries):
+    """The reference's attn_data_list from the maps of the selected entries: ``kinds`` / ``layout_entry`` are the full entry list's
+    kinds and each entry's index in ``entries`` (-1: not selected) as ``attention_selection`` returns them.  One position per layer in
+    execution order: a text or image layer (kinds 0 / 1) holds its entry, a connection layer (kinds 2 and 3, adjacent) the tuple
+    ``(text->image, image->text)``; an entry left out of the selection is None, each direction of a connection layer on its own."""
+    def get(e):
+        return entries[layout_entry[e]] if layout_entry[e] >= 0 else None
+    attn, e = [], 0
+    while e < len(kinds):
+        if kinds[e] == 2:
+            attn.append((get(e), get(e + 1)))
+            e += 2
+        else:
+            attn.append(get(e))
+            e += 1
+    return attn
+
+
+def _full_selection(layout):
+    """``attention_selection``'s (kinds, layout_entry) of a layout that holds every entry."""
+    return [entry[-2] for entry in layout], list(range(len(layout)))
+
+
+def split_packed_attention(flat, layout, t_rows, v_rows, selection=None):
     """The packed attention buffer (VB200_OUT_ATTENTION_PACKED) as the reference's attn_data_list: ``layout`` is
     ``[(heads, kind, float_offset)]`` of ``attention_layout_packed``, ``t_rows`` / ``v_rows`` the samples' T_b / V_b.  A text or image
     layer (kinds 0 / 1) gives a list of B views ``[heads, L_b, L_b]``; a connection layer (kinds 2 and 3, adjacent) a tuple of two
-    such lists, ``[heads, T_b, V_b]`` and ``[heads, V_b, T_b]``.  Inside an entry sample b's block follows sample b - 1's."""
+    such lists, ``[heads, T_b, V_b]`` and ``[heads, V_b, T_b]``.  Inside an entry sample b's block follows sample b - 1's.
+    ``selection``: ``attention_selection``'s (kinds, layout_entry) when the layout holds a selection of the entries (None: every
+    entry); positions follow ``attention_list`` (heads 1 under the head mean)."""
     dims = {0: (t_rows, t_rows), 1: (v_rows, v_rows), 2: (t_rows, v_rows), 3: (v_rows, t_rows)}
-    attn, pending = [], None
+    entries = []
     for heads, kind, off in layout:
         shapes = [(heads, lq, lk) for lq, lk in zip(*dims[kind])]
         sizes = [h * lq * lk for h, lq, lk in shapes]
         parts = torch.split(flat[int(off):int(off) + sum(sizes)], sizes)
-        per = [p.view(s) for p, s in zip(parts, shapes)]
-        if kind == 2:
-            pending = per
-        elif kind == 3:
-            attn.append((pending, per))
-        else:
-            attn.append(per)
-    return attn
+        entries.append([p.view(s) for p, s in zip(parts, shapes)])
+    return attention_list(*(selection or _full_selection(layout)), entries)
+
+
+def attention_mask_bits(entries) -> int:
+    """The "attention_entries" bitmask of an iterable of entry indices (``from_pretrained(attention_entries=...)``)."""
+    if isinstance(entries, (str, bytes)) or not hasattr(entries, "__iter__"):
+        raise TypeError(f"attention_entries must be an iterable of entry indices or None, got {entries!r}")
+    mask = 0
+    for e in entries:
+        if isinstance(e, bool) or not isinstance(e, int):
+            raise TypeError(f"attention_entries: entry index {e!r} is not an int")
+        if not 0 <= e < 63:
+            raise ValueError(f"attention_entries: entry index {e} outside [0, 63)")
+        mask |= 1 << e
+    if mask == 0:
+        raise ValueError("attention_entries: select at least one entry (None selects every entry)")
+    return mask
+
+
+_ATTENTION_HEADS = {"all": 0, "mean": 1}
 
 
 class VILBertForVLTasks(object):
@@ -104,7 +142,8 @@ class VILBertForVLTasks(object):
 
     def __init__(self, config: BertConfig, num_labels: int = 3129, state_dict=None, default_gpu: bool = True,
                  use_cuda_graph: bool = True, use_pdl: Optional[bool] = None, strict: bool = True, compute_dtype: str = "fp16",
-                 fused_layernorm: bool = False, return_attention: bool = False, max_plans: int = 0, max_rows_per_sample: int = 256):
+                 fused_layernorm: bool = False, return_attention: bool = False, max_plans: int = 0, max_rows_per_sample: int = 256,
+                 attention_entries=None, attention_heads: str = "all"):
         self.config = config
         self.num_labels = num_labels
         self._sd = _normalise_state_dict(state_dict) if state_dict is not None else None
@@ -124,8 +163,15 @@ class VILBertForVLTasks(object):
         # bounded by max_position_embeddings (+ the task token) as well.
         if not 256 <= int(max_rows_per_sample) <= 1024:
             raise ValueError(f"max_rows_per_sample must be in [256, 1024], got {max_rows_per_sample}")
+        # Which attention maps element 9 carries: attention_entries (entry indices of the full list in execution order, see
+        # attention_selection; None: every entry) and attention_heads ("all", or "mean": each entry averaged over its heads, the
+        # head axis kept as size 1).  Engine state, set when the engine is created and by set_option.
+        if attention_heads not in _ATTENTION_HEADS:
+            raise ValueError(f"attention_heads must be 'all' or 'mean', got {attention_heads!r}")
         self._opts = dict(use_cuda_graph=use_cuda_graph, use_pdl=use_pdl, strict=strict, compute_dtype=compute_dtype,
-                          max_plans=int(max_plans), max_rows_per_sample=int(max_rows_per_sample))
+                          max_plans=int(max_plans), max_rows_per_sample=int(max_rows_per_sample),
+                          attention_entries=None if attention_entries is None else attention_mask_bits(attention_entries),
+                          attention_heads=_ATTENTION_HEADS[attention_heads])
         # attn_data_list (element 9 of the tuple): the reference returns the 24 layers' attention probabilities when called with
         # output_all_attention_masks=True (worker.py:287-288) and never reads them; here they are computed only when this flag
         # is set as well (model.return_attention = True), otherwise element 9 is [].
@@ -220,6 +266,9 @@ class VILBertForVLTasks(object):
         L.check(rc, None)
         self._handle, self._device = h, device
         L.check(lib.vb200_set_option(h, b"max_rows_per_sample", self._opts["max_rows_per_sample"]), h)
+        for key in ("attention_entries", "attention_heads"):
+            if self._opts[key]:
+                L.check(lib.vb200_set_option(h, key.encode(), self._opts[key]), h)
         for key in ("hidden_size", "v_hidden_size", "bi_hidden_size", "vocab_size", "v_target_size",
                     "v_feature_size", "num_labels", "gqa_labels", "task_specific_tokens", "weight_bytes",
                     "operand_width_factor"):
@@ -276,11 +325,12 @@ class VILBertForVLTasks(object):
 
     def set_option(self, key, value):
         """Run-time knobs of the engine (include/vilbert_b200.h, vb200_set_option): "max_plans", "timeline", "profile_grid_pct",
-        "gemm_kernel", "max_rows_per_sample" (also applied to the engine a later .cuda() creates)."""
+        "gemm_kernel", "max_rows_per_sample", "attention_entries" (a bitmask) and "attention_heads" (0 / 1) -- the last three also
+        applied to the engine a later .cuda() creates."""
         self._engine_device()
         L.check(L.load().vb200_set_option(self._handle, key.encode(), int(value)), self._handle)
-        if key == "max_rows_per_sample":
-            self._opts["max_rows_per_sample"] = int(value)
+        if key in ("max_rows_per_sample", "attention_entries", "attention_heads"):
+            self._opts[key] = int(value)
 
     @property
     def max_rows_per_sample(self) -> int:
@@ -335,8 +385,9 @@ class VILBertForVLTasks(object):
         ``attn_data_list`` (element 9, never read by the worker) is the list of the 24 layers' attention probabilities in
         execution order -- ``[B, heads, L, L]`` for a text / image layer, a ``(text->image [B, heads, T, V], image->text
         [B, heads, V, T])`` tuple for a connection layer -- when ``output_all_attention_masks`` AND ``self.return_attention``
-        are set, else ``[]``.  ``slot`` selects one of 16 independent workspaces: calls on different slots may be in flight
-        concurrently on different CUDA streams.
+        are set, else ``[]``; with ``attention_entries`` / ``attention_heads`` an entry left out is None (each direction of a
+        connection layer on its own) and a head-mean entry is ``[B, 1, Lq, Lk]``.  ``slot`` selects one of 16 independent
+        workspaces: calls on different slots may be in flight concurrently on different CUDA streams.
         """
         if self._handle is None and torch.is_tensor(input_txt) and input_txt.is_cuda:
             self.cuda(input_txt.device.index)
@@ -367,6 +418,18 @@ class VILBertForVLTasks(object):
         L.check(lib.vb200_attention_layout(self._handle, B, Tin, V, n.value, C.byref(n), dims, offs, C.byref(total)), self._handle)
         return [(dims[4 * i], dims[4 * i + 1], dims[4 * i + 2], dims[4 * i + 3], offs[i]) for i in range(n.value)], total.value
 
+    def attention_selection(self):
+        """(kinds, layout_entry) of the full attention-map entry list in execution order (vb200_attention_selection): each entry's
+        kind (0 text, 1 image, 2 / 3 the text->image / image->text direction of a connection layer) and its index in the layouts of
+        the current selection, -1 when it is not selected."""
+        self._engine_device()
+        lib = L.load()
+        n = C.c_int32()
+        L.check(lib.vb200_attention_selection(self._handle, 0, C.byref(n), None, None), self._handle)
+        kinds, where = (C.c_int32 * n.value)(), (C.c_int32 * n.value)()
+        L.check(lib.vb200_attention_selection(self._handle, n.value, C.byref(n), kinds, where), self._handle)
+        return list(kinds), list(where)
+
     def attention_layout_packed(self, n_tokens, n_regions):
         """[(heads, kind, float_offset)] of the packed attention buffer of a batch with these Tin_b / V_b (for
         ``forward_regions_packed``, V_b = n_boxes_b + 1) + its size in floats (vb200_attention_layout_packed)."""
@@ -389,7 +452,8 @@ class VILBertForVLTasks(object):
         flat = torch.empty(total, dtype=torch.float32, device=device)
         o.attention_probs = flat.data_ptr()
         task = 1 if self._dims["task_specific_tokens"] else 0
-        return select | L.OUT_ATTENTION_PACKED, lambda: split_packed_attention(flat, layout, [t + task for t in nt], nv)
+        sel = self.attention_selection()
+        return select | L.OUT_ATTENTION_PACKED, lambda: split_packed_attention(flat, layout, [t + task for t in nt], nv, sel)
 
     @staticmethod
     def _with_attention(result, attn, debug_taps):
@@ -421,15 +485,8 @@ class VILBertForVLTasks(object):
         if "attention_probs" in outs:
             flat = outs["attention_probs"]
             layout, _ = self.attention_layout(B, Tin, V)
-            pending = None
-            for heads, lq, lk, kind, off in layout:
-                t = flat[off:off + B * heads * lq * lk].view(B, heads, lq, lk)
-                if kind == 2:
-                    pending = t
-                elif kind == 3:
-                    attn.append((pending, t))
-                else:
-                    attn.append(t)
+            entries = [flat[off:off + B * heads * lq * lk].view(B, heads, lq, lk) for heads, lq, lk, kind, off in layout]
+            attn = attention_list(*self.attention_selection(), entries)
         result = (g("vil_prediction"), g("vil_prediction_gqa"), g("vil_logit"), g("vil_binary_prediction"),
                   g("vil_tri_prediction"), g("vision_prediction"), g("vision_logit"), g("linguisic_prediction"),
                   g("linguisic_logit"), attn)
