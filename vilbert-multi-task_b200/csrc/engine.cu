@@ -18,6 +18,7 @@
 #include <memory>
 #include <stdexcept>
 #include <string>
+#include <utility>
 #include <variant>
 #include <vector>
 
@@ -431,6 +432,35 @@ template <class... F> struct Overloaded : F... { using F::operator()...; };
 template <class... F> Overloaded(F...) -> Overloaded<F...>;
 
 struct OutBuf { float* p = nullptr; int rows = 0, cols = 0, ld = 0; };
+// The twelve outputs of a forward, in vb200_outputs' order: per slot its field, the plan-key bit of a call that reads it -- a head's
+// select bit, kTextRows / kImageRows (above the public bits) for a sequence tap, none for pooled_output, which every suffix plan
+// writes -- what its rows are and its name in messages.  A packed plan holds its per-row outputs at the call's row totals.
+constexpr uint32_t kTextRows = 1u << 30, kImageRows = 1u << 31;
+enum OutRows { kPerSample, kPerPair, kTextRow, kImageRow };   // kPerPair: B / 2 rows, B at an odd batch
+using OutField = float* vb200_outputs::*;
+struct OutSlot { OutField field; uint32_t bit; OutRows rows; const char* name; };
+enum { kOutVqa, kOutGqa, kOutVilLogit, kOutBinary, kOutTri, kOutVisionPred, kOutVisionLogit, kOutLingPred, kOutLingLogit, kOutSeqT,
+       kOutSeqV, kOutPooled, kNumOuts };
+constexpr OutSlot kOutSlots[kNumOuts] = {
+    {&vb200_outputs::vil_prediction, VB200_OUT_VIL_PREDICTION, kPerSample, "vil_prediction (VB200_OUT_VIL_PREDICTION)"},
+    {&vb200_outputs::vil_prediction_gqa, VB200_OUT_VIL_PREDICTION_GQA, kPerSample, "vil_prediction_gqa (VB200_OUT_VIL_PREDICTION_GQA)"},
+    {&vb200_outputs::vil_logit, VB200_OUT_VIL_LOGIT, kPerSample, "vil_logit (VB200_OUT_VIL_LOGIT)"},
+    {&vb200_outputs::vil_binary_prediction, VB200_OUT_VIL_BINARY_PREDICTION, kPerPair, "vil_binary_prediction (VB200_OUT_VIL_BINARY_PREDICTION)"},
+    {&vb200_outputs::vil_tri_prediction, VB200_OUT_VIL_TRI_PREDICTION, kPerSample, "vil_tri_prediction (VB200_OUT_VIL_TRI_PREDICTION)"},
+    {&vb200_outputs::vision_prediction, VB200_OUT_VISION_PREDICTION, kImageRow, "vision_prediction (VB200_OUT_VISION_PREDICTION)"},
+    {&vb200_outputs::vision_logit, VB200_OUT_VISION_LOGIT, kImageRow, "vision_logit (VB200_OUT_VISION_LOGIT)"},
+    {&vb200_outputs::linguisic_prediction, VB200_OUT_LINGUISIC_PREDICTION, kTextRow, "linguisic_prediction (VB200_OUT_LINGUISIC_PREDICTION)"},
+    {&vb200_outputs::linguisic_logit, VB200_OUT_LINGUISIC_LOGIT, kTextRow, "linguisic_logit (VB200_OUT_LINGUISIC_LOGIT)"},
+    {&vb200_outputs::sequence_output_t, kTextRows, kTextRow, "sequence_output_t"},
+    {&vb200_outputs::sequence_output_v, kImageRows, kImageRow, "sequence_output_v"},
+    {&vb200_outputs::pooled_output, 0, kPerSample, "pooled_output"},
+};
+// the plan-key bits of the outputs whose rows are `rows`
+constexpr uint32_t out_bits(OutRows rows) {
+    uint32_t m = 0;
+    for (const OutSlot& o : kOutSlots) if (o.rows == rows) m |= o.bit;
+    return m;
+}
 
 // ------------------------------------------------------------------------------------------ packed batches
 // The d_meta format of a packed plan, in ints: text row offsets [B + 1] | image row offsets [B + 1]; with `src` (a packed pair suffix)
@@ -606,20 +636,14 @@ BoxRows box_rows(const char* api, int n, const int32_t* n_boxes, int max_boxes, 
 
 struct Plan {
     int B = 0, Tin = 0, T = 0, V = 0;
-    uint32_t select = 0;
     Arena mem;
     // input-side buffers
     bf16* img_a = nullptr; int kp = 0;
     float *mask_t = nullptr, *mask_v = nullptr;
-    float* t_f32[2]; bf16* t_b16[2];
+    float* t_f32[2]; bf16* t_b16[2];              // each stream's state: [0] between layers, [1] a layer's attention LayerNorm output
     float* v_f32[2]; bf16* v_b16[2];
-    float* y_scratch[2] = {nullptr, nullptr};   // per-stream fp32 GEMM output feeding the row LayerNorm kernel
-    int t_cur = 0, v_cur = 0;
-    // pruned tail of a stream (get_plan): its last layer's compact 16-bit output [B, hidden], each sample's first row; null when the
-    // stream's full final rows are in t_b16[t_cur] / v_b16[v_cur]
-    bf16 *tail_t = nullptr, *tail_v = nullptr;
     std::vector<Op> ops;
-    OutBuf outs[12];
+    OutBuf outs[kNumOuts];
     struct AttnOut { float* p; int heads, Lq, Lk; };   // attention probabilities [B, heads, Lq, Lk] in schedule order
     std::vector<AttnOut> attn;                         //   (T / V layers: one entry; connection layers: text->image, image->text)
     uint64_t last_use = 0;                             // plan-cache LRU stamp
@@ -639,7 +663,6 @@ struct Plan {
     int* d_meta = nullptr;
     int* h_meta = nullptr;
     cudaEvent_t meta_copied = nullptr;
-    int n_probs = 0;                                   // packed attention-probability ops added so far (their entry index)
     const int* offs_t() const { return d_meta + layout.offs_t(); }
     const int* offs_v() const { return d_meta + layout.offs_v(); }
     const int* rows_t() const { return d_meta + layout.rows_t(); }
@@ -656,14 +679,14 @@ struct Plan {
 };
 
 // One pre-training head at one bucket of M listed rows (vb200_pretraining_heads): the device row list (the call's count first, which
-// bounds the GEMM, LayerNorm and rowdot rows), the gathered operand, the forward's launch list for that head built by add_linear /
-// rowdot_op at M rows (TMA descriptors included) and its fp32 logits.  Built once per bucket and kept, apart from the forward plans:
+// bounds the GEMM, LayerNorm and rowdot rows), the gathered operand, the forward's launch list for that head built by PlanBuilder
+// at M rows (TMA descriptors included) and its fp32 logits.  Built once per bucket and kept, apart from the forward plans:
 // never captured, counted against max_plans or evicted.
 enum { kHeadText = 0, kHeadImage = 1, kHeadPair = 2 };
 constexpr int kMaxHeadRows = 1 << 20;   // rows per list of one call (the largest bucket's logits: 1M x 30522 fp32 = 125 GB is already
                                         // past any device; the bound keeps the bucket arithmetic in int)
 struct RowHeads {
-    Plan pl;                       // workspace (pl.mem), launch list (pl.ops), GEMM scratch (pl.y_scratch[0]); B = 1, T = V = M
+    Plan pl;                       // workspace (pl.mem) and launch list (pl.ops)
     int M = 0;
     int* d_rows = nullptr;         // [1 + 2M]: count, then the rows, then (vb200_pretraining_objectives) their labels
     void* a = nullptr;             // [M, width]: 16-bit operand (x3: hi | lo | hi) of the transform GEMM, fp32 pooled rows (pair head)
@@ -1025,98 +1048,307 @@ struct vb200_engine {
     }
 
     // ---------------------------------------------------------------- plan construction
-    // One nn.Linear (+ activation, + residual LayerNorm) -> one or two launch-list entries on `stream`: the GEMM (+bias,
-    // +activation), and with `ln` it writes fp32 to the stream's scratch and the row LayerNorm kernel (adds the residual) follows.
-    // All sizes are LOGICAL (elements of the mathematical matrices).  In fp32-parity mode (x3) every 16-bit operand buffer is
-    // physically 3x as wide (fp16 hi | lo | hi per 64 columns), so operand strides, the contraction length and the 16-bit
-    // output stride are multiplied by S = 3 here and nowhere else.
-    void add_linear(Plan& pl, const bf16* A, int64_t a_rows, int64_t lda, const LinearW& W, int act, const float* res, int ld_res,
-                    const LNW* ln, bf16* out_b, int ld_b, float* out_f, int ld_f, int stream = 0, Op::Sync sync = Op::NONE,
-                    const float* mul = nullptr, int ld_mul = 0, const int* m_rows = nullptr) {
-        const int S = x3 ? 3 : 1;
-        GemmEpilogue e{};
-        e.M = static_cast<int>(a_rows); e.N = W.N; e.K = W.ldw * S;
-        e.bias = W.bias; e.mul = mul; e.ld_mul = ld_mul; e.act = x3 && act == vb::kActGelu ? vb::kActGeluExact : act;
-        e.pdl = opt.use_pdl ? 5 : 0;
-        e.a_f16 = opt.act_fp16; e.out_f16 = opt.act_fp16;
-        e.m_rows = m_rows;
-        e.split_acc = x3 ? 1 : 0;
-        if (ln) {
-            e.out_f32 = pl.y_scratch[stream]; e.ld_f32 = W.N;
-        } else {
-            e.out_bf16 = out_b; e.ld_bf16 = ld_b * S; e.out_f32 = out_f; e.ld_f32 = ld_f;
-            e.split16 = (x3 && out_b != nullptr) ? 1 : 0;
-            if (e.split16 && (W.N & 63)) fail(VB200_ERR_INVALID, "fp32-parity mode: 16-bit GEMM output of width %d is not a multiple of 64", W.N);
+    // One ViLBERT stream of a forward plan under construction: every layer kind and the heads read the stream's facts from here.
+    struct StreamRec {
+        float** f32; bf16** b16;            // the plan's t_f32 / t_b16 or v_f32 / v_b16
+        int hid, seq, rows;                 // width, rows per sample (a packed plan's capacity), B x seq
+        int branch, prefix;                 // graph branch of its layers; prefix sums of its packed self-attention maps (0 T^2, 1 V^2)
+        const float* mask;
+        uint8_t* qkv; bf16* ctx; bf16* inter;   // scratch: Q | K | V projections, attention context, FFN intermediate
+        const int* m_rows; const int* offs;     // packed plans: device row count and per-sample row offsets
+        bf16* tail;                         // pruned tail: its last layer's compact 16-bit output [B, hid], each sample's first row
+    };
+    // One nn.Linear's arguments (PlanBuilder::linear): the weight and the operand [rows, w.K] at row stride lda are fixed, the rest
+    // named.  All sizes are LOGICAL (elements of the mathematical matrices).  Over a stream: every row of it, on its branch.
+    struct LinearArgs {
+        const LinearW& w; const bf16* a; int64_t lda, rows;
+        int act = vb::kActNone;
+        bf16* out16 = nullptr; int ld16 = 0;
+        float* out32 = nullptr; int ld32 = 0;
+        const LNW* ln = nullptr; const float* res = nullptr; int ld_res = 0;   // LayerNorm(GEMM + res): the row kernel writes the outputs
+        const float* mul = nullptr; int ld_mul = 0;                           // epilogue product operand (the pooled product)
+        const int* m_rows = nullptr;                                          // packed plans: device count of the rows computed
+        int branch = 0;                                                       // graph branch: 0 main, 1 side (image)
+        Op::Sync sync = Op::NONE;
+        LinearArgs(const LinearW& w_, const bf16* a_, int64_t lda_, int64_t rows_) : w(w_), a(a_), lda(lda_), rows(rows_) {}
+        LinearArgs(const StreamRec& s, const LinearW& w_, const bf16* a_, int64_t lda_)
+            : w(w_), a(a_), lda(lda_), rows(s.rows), m_rows(s.m_rows), branch(s.branch) {}
+    };
+    // Builds one launch list into `pl` (get_plan, row_heads_for) and holds what only construction needs.  Every op it adds takes the
+    // current tag: the NVTX range name, also named by a failed GEMM launch's message.
+    struct PlanBuilder {
+        vb200_engine& eng;
+        Plan& pl;
+        int lone_m;                         // the rows the lone-rows tile rule compares: a forward's larger stream, a RowHeads bucket
+        const char* tag;
+        float* y[2] = {nullptr, nullptr};   // per-branch fp32 GEMM output feeding the row LayerNorm kernel
+        StreamRec t{}, v{};
+        bool maps = false;                  // the forward writes the attention maps attn_sel selects
+        int entry = 0;                      // the current schedule step's first attention-map entry in the full list
+        int n_probs = 0;                    // packed attention-probability ops added so far (their entry index)
+
+        // Physical width factor of the 16-bit operand buffers: in fp32-parity mode (x3) each is 3x as wide (fp16 hi | lo | hi per 64
+        // columns).  buf16 sizes them, linear and gather scale their strides and K; nothing else applies it.
+        int S() const { return eng.x3 ? 3 : 1; }
+        bf16* buf16(size_t rows, size_t width) { return pl.mem.alloc_n<bf16>(rows * width * S()); }
+        float* buf32(size_t rows, size_t width) { return pl.mem.alloc_n<float>(rows * width); }
+        void push(Op op) { op.tag = tag; pl.ops.push_back(op); }
+        OutBuf make_out(int rows, int cols) { const int ld = (cols + 3) / 4 * 4; return OutBuf{buf32(rows, ld), rows, cols, ld}; }
+        // output slot `slot` of a forward, `cols` wide, at the rows kOutSlots gives it
+        const OutBuf& out(int slot, int cols) {
+            const int B = pl.B, r = kOutSlots[slot].rows;
+            const int rows = r == kPerSample ? B : r == kPerPair ? (B % 2 == 0 ? B / 2 : B) : r == kTextRow ? t.rows : v.rows;
+            return pl.outs[slot] = make_out(rows, cols);
         }
-        // Small forwards (<= lone_rows rows in either stream, batch <= 8): 64-wide tiles while they still fit one CTA per SM -- twice
-        // the CTAs, half the epilogue each.  The tile width never changes an element's accumulation order.  RowHeads plans bring
-        // their bucket M as pl.B = 1, pl.T = pl.V = M.
-        int block_n = x3 ? 64 : vb::gemm_p_pick_block_n(W.N);      // the fp32-parity kernel runs 64-wide tiles only
-        if (lone_rows > 0 && !x3 && block_n == 128 && W.N % 64 == 0 &&
-            std::max(pl.B * pl.T, pl.B * pl.V) <= lone_rows && ((a_rows + 127) / 128) * (W.N / 64) <= vb::num_sms_host())
-            block_n = 64;
-        // Ping-pong kernel: each consumer warpgroup's epilogue runs under the other's mainloop.  It takes every plain GEMM it
-        // supports (not the fp32-parity, pooled-product or ragged-N ones) whose outputs the TMA can store.
-        // It takes the tile width chosen above, 128 even where that leaves one tile per CTA: 64-wide ping-pong tiles measured slower on H100 SXM
-        // (700 W, bf16, 16-bit output, scripts/kernel_bench.py) at 1984x768x768 (9.74 vs 8.20 us), 1984x768x3072 (29.19 vs 20.32) and
-        // 2304x1024x1024 (16.71 vs 15.88), and only 4 % faster with GELU at 2304x1024x1024 (18.04 vs 18.81).  The single-panel
-        // launches of a batch-64 forward (poolers, fc0, the pruned tails) keep 128 too: 64-wide was slower at 64x768x768 (8.71 vs
-        // 8.45 / 8.41 us, two 128-wide runs), 64x3072x768 GELU (9.54 vs 9.13 / 9.07), 64x1024x1024 (10.18 vs 10.04 / 9.97; GELU 10.40
-        // vs 10.21 / 10.10), 64x1024x768 ReLU (8.53 vs 8.08 / 8.05) and 64x2048x1024 GELU (10.57 vs 10.47 / 10.42), and 2 % faster
-        // only at 64x768x3072 (20.74 vs 21.23 / 21.12); same card, bf16.
-        const GemmCall g = make_gemm(A, lda * S, W.w, static_cast<int64_t>(W.ldw) * S, e, {block_n, x3 ? 0 : gemm_kernel});
-        pl.ops.push_back({g, stream, 2.0 * a_rows * W.N * W.K, sync});
-        if (ln) {
-            LayerNormArgs l{};
-            l.y = pl.y_scratch[stream]; l.ld_y = W.N; l.res = res; l.ld_res = ld_res; l.gamma = ln->g; l.beta = ln->b;
-            l.out_f32 = out_f; l.ld_f32 = out_f ? ld_f : 0; l.out16 = out_b; l.ld16 = out_b ? ld_b * S : 0;
-            l.M = static_cast<int>(a_rows); l.N = W.N; l.m_rows = m_rows;
-            pl.ops.push_back({l, stream});
+
+        // One nn.Linear (+ activation, + residual LayerNorm) -> one or two launch-list entries on a.branch: the GEMM (+bias,
+        // +activation), and with a.ln it writes fp32 to the branch's scratch and the row LayerNorm kernel (adds the residual) follows.
+        void linear(const LinearArgs& a) {
+            const LinearW& W = a.w;
+            const int S = this->S();
+            GemmEpilogue e{};
+            e.M = static_cast<int>(a.rows); e.N = W.N; e.K = W.ldw * S;
+            e.bias = W.bias; e.mul = a.mul; e.ld_mul = a.ld_mul; e.act = eng.x3 && a.act == vb::kActGelu ? vb::kActGeluExact : a.act;
+            e.pdl = eng.opt.use_pdl ? 5 : 0;
+            e.a_f16 = eng.opt.act_fp16; e.out_f16 = eng.opt.act_fp16;
+            e.m_rows = a.m_rows;
+            e.split_acc = eng.x3 ? 1 : 0;
+            if (a.ln) {
+                e.out_f32 = y[a.branch]; e.ld_f32 = W.N;
+            } else {
+                e.out_bf16 = a.out16; e.ld_bf16 = a.ld16 * S; e.out_f32 = a.out32; e.ld_f32 = a.ld32;
+                e.split16 = (eng.x3 && a.out16 != nullptr) ? 1 : 0;
+                if (e.split16 && (W.N & 63)) fail(VB200_ERR_INVALID, "fp32-parity mode: 16-bit GEMM output of width %d is not a multiple of 64", W.N);
+            }
+            // Small forwards (<= lone_rows rows in either stream, batch <= 8): 64-wide tiles while they still fit one CTA per SM -- twice
+            // the CTAs, half the epilogue each.  The tile width never changes an element's accumulation order.  RowHeads plans compare
+            // their bucket M.
+            int block_n = eng.x3 ? 64 : vb::gemm_p_pick_block_n(W.N);      // the fp32-parity kernel runs 64-wide tiles only
+            if (eng.lone_rows > 0 && !eng.x3 && block_n == 128 && W.N % 64 == 0 && lone_m <= eng.lone_rows &&
+                ((a.rows + 127) / 128) * (W.N / 64) <= vb::num_sms_host())
+                block_n = 64;
+            // Ping-pong kernel: each consumer warpgroup's epilogue runs under the other's mainloop.  It takes every plain GEMM it
+            // supports (not the fp32-parity, pooled-product or ragged-N ones) whose outputs the TMA can store.
+            // It takes the tile width chosen above, 128 even where that leaves one tile per CTA: 64-wide ping-pong tiles measured slower on H100 SXM
+            // (700 W, bf16, 16-bit output, scripts/kernel_bench.py) at 1984x768x768 (9.74 vs 8.20 us), 1984x768x3072 (29.19 vs 20.32) and
+            // 2304x1024x1024 (16.71 vs 15.88), and only 4 % faster with GELU at 2304x1024x1024 (18.04 vs 18.81).  The single-panel
+            // launches of a batch-64 forward (poolers, fc0, the pruned tails) keep 128 too: 64-wide was slower at 64x768x768 (8.71 vs
+            // 8.45 / 8.41 us, two 128-wide runs), 64x3072x768 GELU (9.54 vs 9.13 / 9.07), 64x1024x1024 (10.18 vs 10.04 / 9.97; GELU 10.40
+            // vs 10.21 / 10.10), 64x1024x768 ReLU (8.53 vs 8.08 / 8.05) and 64x2048x1024 GELU (10.57 vs 10.47 / 10.42), and 2 % faster
+            // only at 64x768x3072 (20.74 vs 21.23 / 21.12); same card, bf16.
+            const GemmCall g = make_gemm(a.a, a.lda * S, W.w, static_cast<int64_t>(W.ldw) * S, e, {block_n, eng.x3 ? 0 : eng.gemm_kernel});
+            push({g, a.branch, 2.0 * a.rows * W.N * W.K, a.sync});
+            if (a.ln) {
+                LayerNormArgs l{};
+                l.y = y[a.branch]; l.ld_y = W.N; l.res = a.res; l.ld_res = a.ld_res; l.gamma = a.ln->g; l.beta = a.ln->b;
+                l.out_f32 = a.out32; l.ld_f32 = a.out32 ? a.ld32 : 0; l.out16 = a.out16; l.ld16 = a.out16 ? a.ld16 * S : 0;
+                l.M = static_cast<int>(a.rows); l.N = W.N; l.m_rows = a.m_rows;
+                push({l, a.branch});
+            }
         }
-    }
-    // softmax(Q K^T / sqrt(d) + mask) V of one stream (self) or one direction of a connection layer.  Default: the tensor-core
-    // kernel writes the context (callers push that op themselves); this adds the fp32 kernel -- as THE attention in fp32-parity
-    // mode (context out as hi | lo | hi), and/or as the producer of the attention-probability output.  Packed plans: the
-    // probabilities of every sample at its own lengths (query rows offs_q, key rows offs_k) straight into the caller's buffer, at
-    // the entry's offset and the sample's prefix sum `prefix` (0 T^2, 1 V^2, 2 T V) of the plan's probability meta.  want_probs: the
-    // entry is selected (attn_sel); under the head mean its maps come from a maps-only head-mean launch, after the fp32-parity
-    // mode's context launch.  Adds nothing outside fp32-parity mode for an entry that is not selected.
-    void add_attn_f32(Plan& pl, const void* q, int ld_q, const void* k, const void* v, int ld_kv, const float* mask, int Lq, int Lk,
-                      int heads, int hid, bf16* ctx, bool want_probs, int stream, const int* offs_q = nullptr,
-                      const int* offs_k = nullptr, int prefix = 0) {
-        const bool mean = want_probs && attn_sel.mean;
-        AttnF32Args a{};
-        a.q = q; a.k = k; a.v = v; a.ld_q = ld_q; a.ld_kv = ld_kv; a.mask = mask; a.Lq = Lq; a.Lk = Lk;
-        a.in_kind = x3 ? 0 : (opt.act_fp16 ? 1 : 2);
-        a.B = pl.B; a.heads = heads; a.head_dim = hid / heads;
-        if (x3) {
-            AttnF32Args c = a;
-            c.ctx = ctx; c.ctx_mode = 3; c.ld_ctx = 3 * hid;
-            if (want_probs && !mean) c.probs = attn_out(pl, heads, Lq, Lk);
-            pl.ops.push_back({c, stream, 4.0 * pl.B * heads * Lq * Lk * (hid / heads)});
+        // Row offs[b] of stream s's src16 (and src32) -> row b of the compact [B, hid] dst16 (and dst32): each sample's first row.
+        void gather(const StreamRec& s, int branch, Op::Sync sync, const bf16* src16, bf16* dst16, const float* src32 = nullptr,
+                    float* dst32 = nullptr) {
+            GatherArgs g{};
+            g.offs = s.offs; g.n_src = s.rows; g.B = pl.B; g.src16 = src16; g.dst16 = dst16; g.ld16 = s.hid * S();
+            g.src_f32 = src32; g.dst_f32 = dst32; g.hidden = src32 ? s.hid : 0;
+            push({g, branch, 0.0, sync});
         }
-        if (!want_probs || (x3 && !mean)) return;
-        a.mean = mean;
-        if (pl.packed) {
-            const MetaLayout& m = pl.layout;
-            a.packed = true;
-            a.pk = vb::PackedProbs{offs_q, offs_k, pl.meta64(m.probs_dst()), pl.meta64(m.probs_entry(pl.n_probs)),
-                                   pl.meta64(m.probs_prefix(prefix))};
-            ++pl.n_probs;
-        } else {
-            a.probs = attn_out(pl, mean ? 1 : heads, Lq, Lk);
+        void rowdot(const float* x, int ld_x, const RowW& w, const float* add, const OutBuf& o, const int* m_rows = nullptr) {
+            push({RowdotArgs{x, w.w, w.b, add, o.p, ld_x, o.ld, o.rows, w.K, w.n_out, m_rows}, 0, 2.0 * o.rows * w.K * w.n_out});
         }
-        pl.ops.push_back({a, stream, 0.0});
-    }
-    // a dense plan's next attention-probability output [B, heads, Lq, Lk]
-    static float* attn_out(Plan& pl, int heads, int Lq, int Lk) {
-        float* p = pl.mem.alloc_n<float>(static_cast<size_t>(pl.B) * heads * Lq * Lk);
-        pl.attn.push_back(Plan::AttnOut{p, heads, Lq, Lk});
-        return p;
-    }
-    Op rowdot_op(const float* x, int ld_x, const RowW& w, const float* add, float* out, int ld_out, int M, const int* m_rows = nullptr) {
-        return {RowdotArgs{x, w.w, w.b, add, out, ld_x, ld_out, M, w.K, w.n_out, m_rows}, 0, 2.0 * M * w.K * w.n_out};
-    }
+        // Q | K | V of stream s (w: 3 x its attention width): 16-bit for the tensor-core attention kernels, fp32 in fp32-parity mode
+        void qkv(const StreamRec& s, const LinearW& w) {
+            LinearArgs g(s, w, s.b16[0], s.hid);
+            g.out16 = eng.x3 ? nullptr : reinterpret_cast<bf16*>(s.qkv); g.ld16 = w.N;
+            g.out32 = eng.x3 ? reinterpret_cast<float*>(s.qkv) : nullptr; g.ld32 = w.N;
+            linear(g);
+        }
+        // softmax(Q K^T / sqrt(d) + mask) V of stream q's queries over stream kv's keys and values (Q | K | V projections hid wide).
+        // A self-attention (q == kv) runs on its stream's branch, both directions of a connection layer on the main one.  Default:
+        // the tensor-core kernel writes the context (callers push that op themselves); this adds the fp32 kernel -- as THE attention
+        // in fp32-parity mode (context out as hi | lo | hi; `sync` is that launch's), and/or as the producer of the attention-probability
+        // output.  Packed plans: the probabilities of every sample at its own lengths straight into the caller's buffer, at the entry's
+        // offset and the sample's prefix sum (0 T^2, 1 V^2, 2 T V) of the plan's probability meta.  The entry is written when it is
+        // selected (attn_sel); under the head mean its maps come from a maps-only head-mean launch, after the fp32-parity mode's context
+        // launch.  Adds nothing outside fp32-parity mode for an entry that is not selected.
+        void attention_f32(const StreamRec& q, const StreamRec& kv, int hid, int heads, int entry, Op::Sync sync = Op::NONE) {
+            const bool self = &q == &kv, want_probs = maps && eng.attn_sel.has(entry), mean = want_probs && eng.attn_sel.mean;
+            const int branch = self ? q.branch : 0;
+            const size_t qe = eng.x3 ? 4 : 2;
+            AttnF32Args a{};
+            a.q = q.qkv; a.k = kv.qkv + hid * qe; a.v = kv.qkv + 2 * hid * qe; a.ld_q = 3 * hid; a.ld_kv = 3 * hid; a.mask = kv.mask;
+            a.Lq = q.seq; a.Lk = kv.seq;
+            a.in_kind = eng.x3 ? 0 : (eng.opt.act_fp16 ? 1 : 2);
+            a.B = pl.B; a.heads = heads; a.head_dim = hid / heads;
+            if (eng.x3) {
+                AttnF32Args c = a;
+                c.ctx = q.ctx; c.ctx_mode = 3; c.ld_ctx = 3 * hid;
+                if (want_probs && !mean) c.probs = attn_out(heads, a.Lq, a.Lk);
+                push({c, branch, 4.0 * pl.B * heads * a.Lq * a.Lk * (hid / heads), sync});
+            }
+            if (!want_probs || (eng.x3 && !mean)) return;
+            a.mean = mean;
+            if (pl.packed) {
+                const MetaLayout& m = pl.layout;
+                a.packed = true;
+                a.pk = vb::PackedProbs{q.offs, kv.offs, pl.meta64(m.probs_dst()), pl.meta64(m.probs_entry(n_probs)),
+                                       pl.meta64(m.probs_prefix(self ? q.prefix : 2))};
+                ++n_probs;
+            } else {
+                a.probs = attn_out(mean ? 1 : heads, a.Lq, a.Lk);
+            }
+            push({a, branch, 0.0});
+        }
+        // a dense plan's next attention-probability output [B, heads, Lq, Lk]
+        float* attn_out(int heads, int Lq, int Lk) {
+            float* p = pl.mem.alloc_n<float>(static_cast<size_t>(pl.B) * heads * Lq * Lk);
+            pl.attn.push_back(Plan::AttnOut{p, heads, Lq, Lk});
+            return p;
+        }
+        // A layer's row-local half on stream s: the attention output (ctx, ctx_w wide) + LayerNorm with the layer input -> [1], the
+        // FFN and its LayerNorm with that output -> [0].  `sync` is the first GEMM's.
+        void row_local(StreamRec& s, int ctx_w, const LinearW& wo, const LNW& ln1, const LinearW& wi, const LinearW& wf, const LNW& ln2,
+                       Op::Sync sync) {
+            auto ln_linear = [&](const bf16* a, int64_t lda, const LinearW& w, const LNW& ln, int from, int to, Op::Sync sy) {
+                LinearArgs g(s, w, a, lda);
+                g.ln = &ln; g.res = s.f32[from]; g.ld_res = s.hid; g.sync = sy;
+                g.out16 = s.b16[to]; g.ld16 = s.hid; g.out32 = s.f32[to]; g.ld32 = s.hid;
+                linear(g);
+            };
+            ln_linear(s.ctx, ctx_w, wo, ln1, 0, 1, sync);
+            LinearArgs g(s, wi, s.b16[1], s.hid);
+            g.act = vb::kActGelu; g.out16 = s.inter; g.ld16 = wi.N;
+            linear(g);
+            ln_linear(s.inter, wi.N, wf, ln2, 1, 0, Op::NONE);
+        }
+        // One BertLayer / BertImageLayer.  `tail` (the pruned tail): Q, K, V and the attention on every row (each is a key and a
+        // value), the rest on each sample's first row -- read at stride seq rows on dense plans, gathered from the sample offsets on
+        // packed ones -- into compact [B, hid] rows, s.tail.
+        void layer(const LayerW& L, StreamRec& s, int heads, bool tail) {
+            const int hid = s.hid, B = pl.B;
+            qkv(s, L.qkv);
+            if (!eng.x3) {
+                SelfAttnArgs a{};
+                a.qkv = reinterpret_cast<bf16*>(s.qkv); a.ld_qkv = 3 * hid; a.hidden = hid; a.mask = s.mask; a.ctx = s.ctx; a.ld_ctx = hid;
+                a.B = B; a.L = s.seq; a.heads = heads; a.head_dim = hid / heads; a.offs = s.offs;
+                a.stream_kv = s.seq > kStagedAttnRows;
+                push({a, s.branch, 4.0 * B * heads * s.seq * s.seq * (hid / heads)});
+            }
+            if (eng.x3 || maps) attention_f32(s, s, hid, heads, entry);
+            if (!tail) {
+                row_local(s, hid, L.attn_out, L.ln1, L.inter, L.out, L.ln2, Op::NONE);
+                return;
+            }
+            const bf16* ctx = s.ctx;
+            const float* res = s.f32[0];
+            int ld = s.seq * hid;
+            if (pl.packed) {
+                bf16* ctx_c = buf16(B, hid);
+                float* res_c = buf32(B, hid);
+                gather(s, s.branch, Op::NONE, s.ctx, ctx_c, res, res_c);
+                ctx = ctx_c; res = res_c; ld = hid;
+            }
+            float* ln1_f = buf32(B, hid);
+            bf16* ln1_b = buf16(B, hid);
+            s.tail = buf16(B, hid);
+            LinearArgs o(L.attn_out, ctx, ld, B);
+            o.ln = &L.ln1; o.res = res; o.ld_res = ld; o.out16 = ln1_b; o.ld16 = hid; o.out32 = ln1_f; o.ld32 = hid; o.branch = s.branch;
+            linear(o);
+            LinearArgs i(L.inter, ln1_b, hid, B);
+            i.act = vb::kActGelu; i.out16 = s.inter; i.ld16 = L.inter.N; i.branch = s.branch;
+            linear(i);
+            LinearArgs f(L.out, s.inter, L.inter.N, B);     // no fp32 copy: nothing reads the pruned stream's final fp32 rows
+            f.ln = &L.ln2; f.res = ln1_f; f.ld_res = hid; f.out16 = s.tail; f.ld16 = hid; f.branch = s.branch;
+            linear(f);
+        }
+        // One connection layer: both projections, the co-attention after joining the image branch, then the image branch's row-local
+        // half on the side stream (forking from the co-attention) and the text branch's on the main one.
+        void connection(const ConnW& W) {
+            const int B = pl.B, Hb = eng.cfg.bi_hidden, heads = eng.cfg.bi_heads;
+            qkv(v, W.qkv_img);
+            qkv(t, W.qkv_txt);
+            if (!eng.x3) {
+                CoAttnArgs a{};
+                a.qkv_img = reinterpret_cast<bf16*>(v.qkv); a.ld_img = 3 * Hb; a.qkv_txt = reinterpret_cast<bf16*>(t.qkv); a.ld_txt = 3 * Hb;
+                a.hidden = Hb; a.img_mask = v.mask; a.txt_mask = t.mask; a.ctx_txt = t.ctx; a.ld_ctx_txt = Hb; a.ctx_img = v.ctx; a.ld_ctx_img = Hb;
+                a.B = B; a.T = t.seq; a.V = v.seq; a.heads = heads; a.head_dim = Hb / heads; a.offs_t = t.offs; a.offs_v = v.offs;
+                a.stream_kv = t.seq > kStagedAttnRows || v.seq > kStagedAttnRows;
+                push({a, 0, 8.0 * B * heads * t.seq * v.seq * (Hb / heads), Op::JOIN});
+            }
+            if (eng.x3 || maps) {
+                // text queries (Q2) over image keys / values (K1, V1) -> text context; then image queries (Q1) over K2, V2
+                attention_f32(t, v, Hb, heads, entry, Op::JOIN);
+                attention_f32(v, t, Hb, heads, entry + 1);
+            }
+            row_local(v, Hb, W.dense1, W.ln1, W.v_inter, W.v_out, W.v_ln, Op::FORK);
+            row_local(t, Hb, W.dense2, W.ln2, W.t_inter, W.t_out, W.t_ln, Op::NONE);
+        }
+        // A two-GEMM head on `rows` rows of a (row stride lda): the transform (GELU, LayerNorm) into hid16, the decoder's logits into
+        // a new *logits -- a task head's logit_fc, a pre-training prediction head.
+        void predict(const LinearW& transform, const LNW& ln, const LinearW& decoder, const bf16* a, int lda, bf16* hid16, int rows,
+                     const int* m_rows, OutBuf* logits) {
+            LinearArgs g0(transform, a, lda, rows);
+            g0.act = vb::kActGelu; g0.ln = &ln; g0.out16 = hid16; g0.ld16 = transform.N; g0.m_rows = m_rows;
+            linear(g0);
+            *logits = make_out(rows, decoder.N);
+            LinearArgs g1(decoder, hid16, transform.N, rows);
+            g1.out32 = logits->p; g1.ld32 = logits->ld; g1.m_rows = m_rows;
+            linear(g1);
+        }
+        // ---- poolers + heads (main stream, after joining the image branch)
+        void heads(uint32_t select) {
+            const vb200_engine& E = eng;
+            const int B = pl.B, Hb = E.cfg.bi_hidden;
+            float* pooled_t = buf32(B, Hb);
+            float* pooled = buf32(B, Hb);
+            bf16* pooled_b = buf16(B, Hb);
+            Op::Sync join = Op::JOIN;       // the heads' first launch waits for the image branch
+            // The poolers' operand, each sample's first row of a final state: a pruned tail's compact rows, the full state at stride
+            // seq rows on dense plans, or on packed plans (a sample's first row sits at a per-call offset) the B first rows gathered
+            // into compact [B, hid] rows.  Returns the operand and its row stride.
+            auto first_rows = [&](const StreamRec& s) -> std::pair<const bf16*, int64_t> {
+                if (s.tail != nullptr) return {s.tail, s.hid};
+                if (!pl.packed) return {s.b16[0], static_cast<int64_t>(s.seq) * s.hid};
+                bf16* first = buf16(B, s.hid);
+                gather(s, 0, std::exchange(join, Op::NONE), s.b16[0], first);
+                return {first, s.hid};
+            };
+            const auto first_t = first_rows(t);
+            const auto first_v = first_rows(v);
+            LinearArgs pt(E.t_pool, first_t.first, first_t.second, B);
+            pt.act = vb::kActRelu; pt.out32 = pooled_t; pt.ld32 = Hb; pt.sync = join;
+            linear(pt);
+            LinearArgs pv(E.v_pool, first_v.first, first_v.second, B);
+            pv.act = vb::kActRelu; pv.out16 = pooled_b; pv.ld16 = Hb; pv.out32 = pooled; pv.ld32 = Hb; pv.mul = pooled_t; pv.ld_mul = Hb;
+            linear(pv);
+            pl.outs[kOutPooled] = OutBuf{pooled, B, Hb, Hb};
+            auto cls_head = [&](const ClsW& w, int slot) { predict(w.fc0, w.ln, w.fc3, pooled_b, Hb, buf16(B, 2 * Hb), B, nullptr, &pl.outs[slot]); };
+            if (select & VB200_OUT_VIL_PREDICTION) cls_head(E.vqa, kOutVqa);
+            if (select & VB200_OUT_VIL_PREDICTION_GQA) cls_head(E.gqa, kOutGqa);
+            if (select & VB200_OUT_VIL_LOGIT) rowdot(pooled, Hb, E.vil_logit, nullptr, out(kOutVilLogit, 1));
+            if (select & VB200_OUT_VIL_BINARY_PREDICTION) {
+                if (B % 2 == 0) {
+                    // pooled.view(-1, 2*bi_hidden): adjacent samples form one NLVR2 pair (worker.py:266-276)
+                    float* hid = buf32(B / 2, 2 * Hb);
+                    LinearArgs g0(E.binary.fc0, pooled_b, 2 * Hb, B / 2);
+                    g0.act = vb::kActGelu; g0.ln = &E.binary.ln; g0.out32 = hid; g0.ld32 = 2 * Hb;
+                    linear(g0);
+                    rowdot(hid, 2 * Hb, E.binary.fc3_row, nullptr, out(kOutBinary, 2));
+                } else {
+                    // [UPSTREAM] odd batch: element 3 stays the pre-training bi_seq_relationship score
+                    rowdot(pooled, Hb, E.seq_rel, nullptr, out(kOutBinary, 2));
+                }
+            }
+            if (select & VB200_OUT_VIL_TRI_PREDICTION) rowdot(pooled, Hb, E.vil_tri, nullptr, out(kOutTri, 3));
+            if (select & VB200_OUT_VISION_PREDICTION)
+                predict(E.img_transform, E.img_ln, E.img_decoder, v.b16[0], v.hid, buf16(v.rows, v.hid), v.rows, v.m_rows, &pl.outs[kOutVisionPred]);
+            if (select & VB200_OUT_VISION_LOGIT) rowdot(v.f32[0], v.hid, E.vision_logit, v.mask, out(kOutVisionLogit, 1), v.m_rows);
+            if (select & VB200_OUT_LINGUISIC_PREDICTION)
+                predict(E.lm_transform, E.lm_ln, E.lm_decoder, t.b16[0], t.hid, buf16(t.rows, t.hid), t.rows, t.m_rows, &pl.outs[kOutLingPred]);
+            if (select & VB200_OUT_LINGUISIC_LOGIT) rowdot(t.f32[0], t.hid, E.ling_logit, nullptr, out(kOutLingLogit, 1), t.m_rows);
+        }
+    };
     // attention-probability entries one forward with maps writes: the selected ones of the full list (one per text / image layer,
     // two per connection layer)
     int selected_entries() const {
@@ -1124,11 +1356,6 @@ struct vb200_engine {
         int n = 0;
         for (int e = 0; e < all; ++e) n += attn_sel.has(e) ? 1 : 0;
         return n;
-    }
-    OutBuf make_out(Plan& pl, int rows, int cols) {
-        OutBuf o; o.rows = rows; o.cols = cols; o.ld = (cols + 3) / 4 * 4;
-        o.p = pl.mem.alloc_n<float>(static_cast<size_t>(rows) * o.ld);
-        return o;
     }
 
     // Plan modes.  FULL is the reference's forward (worker.py:286-289).  The other three split it at the first connection layer
@@ -1144,27 +1371,18 @@ struct vb200_engine {
     enum PlanMode { FULL = 0, TEXT_PREFIX = 1, IMAGE_PREFIX = 2, SUFFIX = 3, PACKED = 4,
                     PACKED_TEXT_PREFIX = 5, PACKED_IMAGE_PREFIX = 6, PACKED_SUFFIX = 7 };
 
-    // Plan-key bits above the public select bits: the call reads every final text / image row (its sequence_output_t / _v tap).
-    // A forward whose select and taps read no final row of a stream prunes that stream's tail (get_plan).
-    static constexpr uint32_t kTextRows = 1u << 30, kImageRows = 1u << 31;
+    // The plan-key bits of the taps a call reads (kTextRows / kImageRows): a forward whose select and taps read no final row of a
+    // stream prunes that stream's tail (get_plan).
     static uint32_t rows_read(const vb200_outputs* out) {
-        if (out == nullptr) return 0;
-        return (out->sequence_output_t ? kTextRows : 0) | (out->sequence_output_v ? kImageRows : 0);
+        uint32_t r = 0;
+        for (const OutSlot& o : kOutSlots) r |= out != nullptr && out->*o.field ? o.bit & (kTextRows | kImageRows) : 0;
+        return r;
     }
 
     // A pre-training engine has no task head: every select bit of VB200_OUT_TASK_HEADS is rejected, naming the head.
     static void reject_task_heads(uint32_t select) {
-        static const struct { uint32_t bit; const char* name; } heads[] = {
-            {VB200_OUT_VIL_PREDICTION, "vil_prediction (VB200_OUT_VIL_PREDICTION)"},
-            {VB200_OUT_VIL_PREDICTION_GQA, "vil_prediction_gqa (VB200_OUT_VIL_PREDICTION_GQA)"},
-            {VB200_OUT_VIL_LOGIT, "vil_logit (VB200_OUT_VIL_LOGIT)"},
-            {VB200_OUT_VIL_BINARY_PREDICTION, "vil_binary_prediction (VB200_OUT_VIL_BINARY_PREDICTION)"},
-            {VB200_OUT_VIL_TRI_PREDICTION, "vil_tri_prediction (VB200_OUT_VIL_TRI_PREDICTION)"},
-            {VB200_OUT_VISION_LOGIT, "vision_logit (VB200_OUT_VISION_LOGIT)"},
-            {VB200_OUT_LINGUISIC_LOGIT, "linguisic_logit (VB200_OUT_LINGUISIC_LOGIT)"},
-        };
-        for (const auto& h : heads)
-            if (select & h.bit)
+        for (const OutSlot& h : kOutSlots)
+            if (select & h.bit & VB200_OUT_TASK_HEADS)
                 fail(VB200_ERR_INVALID, "the task head %s is not part of a pre-training engine (select only the pre-training heads, "
                      "taps or attention maps)", h.name);
     }
@@ -1192,7 +1410,7 @@ struct vb200_engine {
         const Config& c = cfg;
         if (B < 1 || Tin < 1 || V < 1) fail(VB200_ERR_INVALID, "batch, n_tokens and n_regions must be positive");
         if (Tin > c.max_pos && !packed) fail(VB200_ERR_INVALID, "n_tokens %d exceeds max_position_embeddings %d", Tin, c.max_pos);
-        pl.B = B; pl.Tin = Tin; pl.T = T; pl.V = V; pl.select = select;
+        pl.B = B; pl.Tin = Tin; pl.T = T; pl.V = V;
         if (packed) {
             // zero offsets until the first call: the validation pass and the capture below then touch no row
             pl.packed = true;
@@ -1203,27 +1421,23 @@ struct vb200_engine {
             CUDA_CHECK(cudaMallocHost(&pl.h_meta, n_meta * sizeof(int)));
             CUDA_CHECK(cudaEventCreateWithFlags(&pl.meta_copied, cudaEventDisableTiming));
         }
-        const int* rows_t = pl.packed ? pl.rows_t() : nullptr;
-        const int* rows_v = pl.packed ? pl.rows_v() : nullptr;
-        const int* offs_t = pl.packed ? pl.offs_t() : nullptr;
-        const int* offs_v = pl.packed ? pl.offs_v() : nullptr;
         const int Mt = B * T, Mv = B * V, H = c.hidden, Hv = c.v_hidden, Hb = c.bi_hidden;
-        const size_t S = x3 ? 3 : 1;                 // physical width factor of the 16-bit operand buffers (fp32-parity mode)
         const bool full = schedule_mode == FULL;
         const bool do_t = full || schedule_mode == TEXT_PREFIX, do_v = full || schedule_mode == IMAGE_PREFIX;
         const bool do_s = full || schedule_mode == SUFFIX;
         // Pruned tail: the poolers read one row per sample of each final state.  A stream no per-row head and no tap reads runs its
         // last layer's row-local half (everything after the self-attention) on those B rows only; bit-identical rows, since no
         // kernel's per-element result depends on M.  A stream whose last layer is a connection layer keeps its full rows.
-        const bool prune_t = do_s && !(select & (kTextRows | VB200_OUT_LINGUISIC_PREDICTION | VB200_OUT_LINGUISIC_LOGIT));
-        const bool prune_v = do_s && !(select & (kImageRows | VB200_OUT_VISION_PREDICTION | VB200_OUT_VISION_LOGIT));
+        const bool prune_t = do_s && !(select & out_bits(kTextRow));
+        const bool prune_v = do_s && !(select & out_bits(kImageRow));
         size_t last_t = 0, last_v = 0;                 // the last schedule step writing each stream
         for (size_t i = 0; i < schedule.size(); ++i) {
             if (schedule[i][0] != 'V') last_t = i;
             if (schedule[i][0] != 'T') last_v = i;
         }
+        PlanBuilder b{*this, pl, std::max(Mt, Mv), "embed"};
         pl.kp = img_emb.ldw;
-        pl.img_a = pl.mem.alloc_n<bf16>(static_cast<size_t>(Mv) * pl.kp * S);
+        pl.img_a = b.buf16(Mv, pl.kp);
         pl.mask_t = pl.mem.alloc_n<float>(Mt);
         pl.mask_v = pl.mem.alloc_n<float>(Mv);
         if (mode == PACKED_SUFFIX) {
@@ -1233,172 +1447,59 @@ struct vb200_engine {
             CUDA_CHECK(cudaMemset(pl.mask_v, 0, static_cast<size_t>(Mv) * sizeof(float)));
         }
         for (int i = 0; i < 2; ++i) {
-            pl.t_f32[i] = pl.mem.alloc_n<float>(static_cast<size_t>(Mt) * H);
-            pl.t_b16[i] = pl.mem.alloc_n<bf16>(static_cast<size_t>(Mt) * H * S);
-            pl.v_f32[i] = pl.mem.alloc_n<float>(static_cast<size_t>(Mv) * Hv);
-            pl.v_b16[i] = pl.mem.alloc_n<bf16>(static_cast<size_t>(Mv) * Hv * S);
+            pl.t_f32[i] = b.buf32(Mt, H);
+            pl.t_b16[i] = b.buf16(Mt, H);
+            pl.v_f32[i] = b.buf32(Mv, Hv);
+            pl.v_b16[i] = b.buf16(Mv, Hv);
         }
-        pl.y_scratch[0] = pl.mem.alloc_n<float>(std::max({static_cast<size_t>(Mt) * H, static_cast<size_t>(Mv) * Hv,
-                                                          static_cast<size_t>(B) * 2 * Hb}));
-        pl.y_scratch[1] = pl.mem.alloc_n<float>(static_cast<size_t>(Mv) * Hv);
-        const int qt = 3 * std::max(H, Hb), qv = 3 * std::max(Hv, Hb);
+        b.y[0] = pl.mem.alloc_n<float>(std::max({static_cast<size_t>(Mt) * H, static_cast<size_t>(Mv) * Hv, static_cast<size_t>(B) * 2 * Hb}));
+        b.y[1] = b.buf32(Mv, Hv);
         // Q | K | V projections: 16-bit for the tensor-core attention kernel, fp32 in fp32-parity mode
         const size_t qe = x3 ? 4 : 2;
-        uint8_t* qkv_t = static_cast<uint8_t*>(pl.mem.alloc(static_cast<size_t>(Mt) * qt * qe));
-        uint8_t* qkv_v = static_cast<uint8_t*>(pl.mem.alloc(static_cast<size_t>(Mv) * qv * qe));
-        bf16* ctx_t = pl.mem.alloc_n<bf16>(static_cast<size_t>(Mt) * std::max(H, Hb) * S);
-        bf16* ctx_v = pl.mem.alloc_n<bf16>(static_cast<size_t>(Mv) * std::max(Hv, Hb) * S);
-        bf16* inter_t = pl.mem.alloc_n<bf16>(static_cast<size_t>(Mt) * c.inter * S);
-        bf16* inter_v = pl.mem.alloc_n<bf16>(static_cast<size_t>(Mv) * c.v_inter * S);
-        auto& ops = pl.ops;
-        auto qkv_out = [&](uint8_t* q, bf16*& ob, float*& of) {       // where a QKV GEMM writes
-            ob = x3 ? nullptr : reinterpret_cast<bf16*>(q);
-            of = x3 ? reinterpret_cast<float*>(q) : nullptr;
-        };
-        auto qkv_at = [&](const uint8_t* q, int col) -> const void* { return q + static_cast<size_t>(col) * qe; };
+        uint8_t* qkv_t = static_cast<uint8_t*>(pl.mem.alloc(static_cast<size_t>(Mt) * 3 * std::max(H, Hb) * qe));
+        uint8_t* qkv_v = static_cast<uint8_t*>(pl.mem.alloc(static_cast<size_t>(Mv) * 3 * std::max(Hv, Hb) * qe));
+        bf16* ctx_t = b.buf16(Mt, std::max(H, Hb));
+        bf16* ctx_v = b.buf16(Mv, std::max(Hv, Hb));
+        bf16* inter_t = b.buf16(Mt, c.inter);
+        bf16* inter_v = b.buf16(Mv, c.v_inter);
+        b.t = StreamRec{pl.t_f32, pl.t_b16, H, T, Mt, 0, 0, pl.mask_t, qkv_t, ctx_t, inter_t, packed ? pl.rows_t() : nullptr,
+                        packed ? pl.offs_t() : nullptr, nullptr};
+        b.v = StreamRec{pl.v_f32, pl.v_b16, Hv, V, Mv, 1, 1, pl.mask_v, qkv_v, ctx_v, inter_v, packed ? pl.rows_v() : nullptr,
+                        packed ? pl.offs_v() : nullptr, nullptr};
+        b.maps = want_attn;
 
-        // ---- the two streams: activations ping-pong between buffers [cur] and [1 - cur]
-        struct StreamSt {
-            float** f32; bf16** b16; int cur; int hid, rows, stream; const float* mask; int seq;
-            uint8_t* qkv; bf16* ctx; bf16* inter;
-            const int* m_rows; const int* offs;     // packed plans: device row count and per-sample row offsets of the stream
-        };
-        StreamSt ts{pl.t_f32, pl.t_b16, 0, H, Mt, 0, pl.mask_t, T, qkv_t, ctx_t, inter_t, rows_t, offs_t};
-        StreamSt vs{pl.v_f32, pl.v_b16, 0, Hv, Mv, 1, pl.mask_v, V, qkv_v, ctx_v, inter_v, rows_v, offs_v};
-        // GEMM + LayerNorm whose residual is buffers[rwhich] of stream st; the result lands in buffers[owhich]
-        auto ln_linear = [&](StreamSt& st, const bf16* A, int64_t lda, const LinearW& W, const LNW& ln, int rwhich, int owhich,
-                             Op::Sync sync) {
-            add_linear(pl, A, st.rows, lda, W, vb::kActNone, st.f32[rwhich], st.hid, &ln, st.b16[owhich], st.hid, st.f32[owhich], st.hid,
-                       st.stream, sync, nullptr, 0, st.m_rows);
-        };
-
-        // ---- image embedding: LayerNorm(feat.W_img^T + loc.W_loc^T + b) as ONE GEMM over K = v_feat + 64
-        if (do_v)
-            add_linear(pl, pl.img_a, Mv, pl.kp, img_emb, vb::kActNone, nullptr, 0, &vemb_ln, pl.v_b16[0], Hv, pl.v_f32[0], Hv,
-                       1, Op::NONE, nullptr, 0, vs.m_rows);   // side stream: overlaps the text layers ahead of the first co-attention
-
-        // one BertLayer / BertImageLayer.  `tail` (the pruned tail): Q, K, V and the attention on every row (each is a key and a
-        // value), the rest on each sample's first row -- read at stride seq rows on dense plans, gathered from the sample offsets on
-        // packed ones -- into compact [B, hid] rows; returns their 16-bit copy (null without `tail`).
-        auto single_layer = [&](const LayerW& L, StreamSt& st, int inter, int heads, bool tail, int entry) -> bf16* {
-            const int hid = st.hid, cur = st.cur, M = st.rows, stream = st.stream;
-            bf16* qb; float* qf;
-            qkv_out(st.qkv, qb, qf);
-            add_linear(pl, st.b16[cur], M, hid, L.qkv, vb::kActNone, nullptr, 0, nullptr, qb, 3 * hid, qf, 3 * hid, stream, Op::NONE,
-                       nullptr, 0, st.m_rows);
-            if (!x3) {
-                SelfAttnArgs a{};
-                a.qkv = qb; a.ld_qkv = 3 * hid; a.hidden = hid; a.mask = st.mask; a.ctx = st.ctx; a.ld_ctx = hid;
-                a.B = B; a.L = st.seq; a.heads = heads; a.head_dim = hid / heads; a.offs = st.offs;
-                a.stream_kv = st.seq > kStagedAttnRows;
-                ops.push_back({a, stream, 4.0 * B * heads * st.seq * st.seq * (hid / heads)});
-            }
-            if (x3 || want_attn)
-                add_attn_f32(pl, qkv_at(st.qkv, 0), 3 * hid, qkv_at(st.qkv, hid), qkv_at(st.qkv, 2 * hid), 3 * hid, st.mask, st.seq, st.seq,
-                             heads, hid, st.ctx, want_attn && attn_sel.has(entry), stream, st.offs, st.offs,
-                             stream);                                      // prefix: stream 0 T^2, 1 V^2
-            if (tail) {
-                const bf16* ctx = st.ctx;
-                const float* res = st.f32[cur];
-                int ld = st.seq * hid;
-                if (pl.packed) {
-                    bf16* ctx_c = pl.mem.alloc_n<bf16>(static_cast<size_t>(B) * hid * S);
-                    float* res_c = pl.mem.alloc_n<float>(static_cast<size_t>(B) * hid);
-                    GatherArgs g{};
-                    g.offs = st.offs; g.n_src = M; g.B = B; g.src16 = st.ctx; g.dst16 = ctx_c; g.ld16 = static_cast<int>(hid * S);
-                    g.src_f32 = res; g.dst_f32 = res_c; g.hidden = hid;
-                    ops.push_back({g, stream});
-                    ctx = ctx_c; res = res_c; ld = hid;
-                }
-                float* ln1_f = pl.mem.alloc_n<float>(static_cast<size_t>(B) * hid);
-                bf16* ln1_b = pl.mem.alloc_n<bf16>(static_cast<size_t>(B) * hid * S);
-                bf16* out_b = pl.mem.alloc_n<bf16>(static_cast<size_t>(B) * hid * S);
-                add_linear(pl, ctx, B, ld, L.attn_out, vb::kActNone, res, ld, &L.ln1, ln1_b, hid, ln1_f, hid, stream);
-                add_linear(pl, ln1_b, B, hid, L.inter, vb::kActGelu, nullptr, 0, nullptr, st.inter, inter, nullptr, 0, stream);
-                add_linear(pl, st.inter, B, inter, L.out, vb::kActNone, ln1_f, hid, &L.ln2, out_b, hid, nullptr, 0, stream);
-                return out_b;                // no fp32 copy: nothing reads the pruned stream's final fp32 rows
-            }
-            // attention output + LayerNorm1 (residual: the layer input) -> buffers [1 - cur]
-            ln_linear(st, st.ctx, hid, L.attn_out, L.ln1, cur, 1 - cur, Op::NONE);
-            add_linear(pl, st.b16[1 - cur], M, hid, L.inter, vb::kActGelu, nullptr, 0, nullptr, st.inter, inter, nullptr, 0, stream,
-                       Op::NONE, nullptr, 0, st.m_rows);
-            // FFN output + LayerNorm2 (residual: LayerNorm1's output) -> buffers [cur]
-            ln_linear(st, st.inter, inter, L.out, L.ln2, 1 - cur, cur, Op::NONE);
-            return nullptr;
-        };
-
-        for (Op& op : ops) op.tag = "embed";
+        // image embedding: LayerNorm(feat.W_img^T + loc.W_loc^T + b) as ONE GEMM over K = v_feat + 64, on the side stream: it
+        // overlaps the text layers ahead of the first co-attention
+        if (do_v) {
+            LinearArgs g(b.v, img_emb, pl.img_a, pl.kp);
+            g.ln = &vemb_ln; g.out16 = pl.v_b16[0]; g.ld16 = Hv; g.out32 = pl.v_f32[0]; g.ld32 = Hv;
+            b.linear(g);
+        }
         bool in_suffix = false;
-        size_t tagged = ops.size();
-        int n_entry = 0;                               // the step's first attention-map entry in the full list
         for (size_t si = 0; si < schedule.size(); ++si) {
             const std::string& step = schedule[si];
-            const int entry = n_entry;
-            n_entry += step[0] == 'C' ? 2 : 1;
-            for (; tagged < ops.size(); ++tagged) if (ops[tagged].tag == nullptr) ops[tagged].tag = "?";
             const int idx = atoi(step.c_str() + 1);
+            b.tag = step.c_str();          // engine.schedule outlives every plan
             if (step[0] == 'C') in_suffix = true;
-            struct Tagger {          // names the launches this step appends after its layer (engine.schedule outlives every plan)
-                std::vector<Op>& ops; size_t from; const char* name;
-                ~Tagger() { for (size_t i = from; i < ops.size(); ++i) ops[i].tag = name; }
-            } tagger{ops, ops.size(), step.c_str()};
             if (step[0] == 'T') {
-                if (in_suffix ? do_s : do_t) pl.tail_t = single_layer(t_layers[idx], ts, c.inter, c.heads, prune_t && si == last_t, entry);
+                if (in_suffix ? do_s : do_t) b.layer(t_layers[idx], b.t, c.heads, prune_t && si == last_t);
             } else if (step[0] == 'V') {
-                if (in_suffix ? do_s : do_v) pl.tail_v = single_layer(v_layers[idx], vs, c.v_inter, c.v_heads, prune_v && si == last_v, entry);
+                if (in_suffix ? do_s : do_v) b.layer(v_layers[idx], b.v, c.v_heads, prune_v && si == last_v);
             } else if (do_s) {
-                const ConnW& W = c_layers[idx];
-                const int tcur = ts.cur, vcur = vs.cur;
-                bf16 *qvb, *qtb; float *qvf, *qtf;
-                qkv_out(qkv_v, qvb, qvf);
-                qkv_out(qkv_t, qtb, qtf);
-                add_linear(pl, pl.v_b16[vcur], Mv, Hv, W.qkv_img, vb::kActNone, nullptr, 0, nullptr, qvb, 3 * Hb, qvf, 3 * Hb, 1, Op::NONE,
-                           nullptr, 0, vs.m_rows);
-                add_linear(pl, pl.t_b16[tcur], Mt, H, W.qkv_txt, vb::kActNone, nullptr, 0, nullptr, qtb, 3 * Hb, qtf, 3 * Hb, 0, Op::NONE,
-                           nullptr, 0, ts.m_rows);
-                const size_t first_co = ops.size();
-                if (!x3) {
-                    CoAttnArgs a{};
-                    a.qkv_img = qvb; a.ld_img = 3 * Hb; a.qkv_txt = qtb; a.ld_txt = 3 * Hb; a.hidden = Hb;
-                    a.img_mask = pl.mask_v; a.txt_mask = pl.mask_t; a.ctx_txt = ctx_t; a.ld_ctx_txt = Hb; a.ctx_img = ctx_v; a.ld_ctx_img = Hb;
-                    a.B = B; a.T = T; a.V = V; a.heads = c.bi_heads; a.head_dim = Hb / c.bi_heads; a.offs_t = offs_t; a.offs_v = offs_v;
-                    a.stream_kv = T > kStagedAttnRows || V > kStagedAttnRows;
-                    ops.push_back({a, 0, 8.0 * B * c.bi_heads * T * V * (Hb / c.bi_heads)});
-                }
-                if (x3 || want_attn) {
-                    // text queries (Q2) over image keys / values (K1, V1) -> text context; then image queries (Q1) over K2, V2
-                    add_attn_f32(pl, qkv_at(qkv_t, 0), 3 * Hb, qkv_at(qkv_v, Hb), qkv_at(qkv_v, 2 * Hb), 3 * Hb, pl.mask_v, T, V,
-                                 c.bi_heads, Hb, ctx_t, want_attn && attn_sel.has(entry), 0, offs_t, offs_v, 2);
-                    add_attn_f32(pl, qkv_at(qkv_v, 0), 3 * Hb, qkv_at(qkv_t, Hb), qkv_at(qkv_t, 2 * Hb), 3 * Hb, pl.mask_t, V, T,
-                                 c.bi_heads, Hb, ctx_v, want_attn && attn_sel.has(entry + 1), 0, offs_v, offs_t, 2);
-                }
-                ops[first_co].sync = Op::JOIN;              // needs both projections
-                // image branch (side stream; forks from the co-attention): biOutput.dense1 + LayerNorm1, v_intermediate, v_output + LayerNorm
-                ln_linear(vs, ctx_v, Hb, W.dense1, W.ln1, vcur, 1 - vcur, Op::FORK);
-                add_linear(pl, pl.v_b16[1 - vcur], Mv, Hv, W.v_inter, vb::kActGelu, nullptr, 0, nullptr, inter_v, c.v_inter, nullptr, 0, 1,
-                           Op::NONE, nullptr, 0, vs.m_rows);
-                ln_linear(vs, inter_v, c.v_inter, W.v_out, W.v_ln, 1 - vcur, vcur, Op::NONE);
-                // text branch (main stream)
-                ln_linear(ts, ctx_t, Hb, W.dense2, W.ln2, tcur, 1 - tcur, Op::NONE);
-                add_linear(pl, pl.t_b16[1 - tcur], Mt, H, W.t_inter, vb::kActGelu, nullptr, 0, nullptr, inter_t, c.inter, nullptr, 0, 0,
-                           Op::NONE, nullptr, 0, ts.m_rows);
-                ln_linear(ts, inter_t, c.inter, W.t_out, W.t_ln, 1 - tcur, tcur, Op::NONE);
+                b.connection(c_layers[idx]);
             }
+            b.entry += step[0] == 'C' ? 2 : 1;
         }
-        const int tc = ts.cur, vc = vs.cur;
-        pl.t_cur = tc; pl.v_cur = vc;
-        if (pl.tail_t == nullptr) pl.outs[9] = OutBuf{pl.t_f32[tc], Mt, H, H};
-        if (pl.tail_v == nullptr) pl.outs[10] = OutBuf{pl.v_f32[vc], Mv, Hv, Hv};
-
-        const size_t n_before_heads = ops.size();
-        if (do_s) build_heads(pl, select);
-        for (size_t i = n_before_heads; i < ops.size(); ++i) ops[i].tag = "heads";
-        for (const Op& op : ops) pl.flops += op.flops;
+        if (b.t.tail == nullptr) pl.outs[kOutSeqT] = OutBuf{pl.t_f32[0], Mt, H, H};
+        if (b.v.tail == nullptr) pl.outs[kOutSeqV] = OutBuf{pl.v_f32[0], Mv, Hv, Hv};
+        b.tag = "heads";
+        if (do_s) b.heads(select);
+        for (const Op& op : pl.ops) pl.flops += op.flops;
 
         if (timeline) attach_timeline(pl);
         // One eager pass first: opts kernels into their shared-memory sizes and surfaces launch-configuration
         // errors with a real message (errors inside a capture only invalidate the capture).
-        if (!ops.empty()) {
+        if (!pl.ops.empty()) {
             cudaStream_t ws;
             CUDA_CHECK(cudaStreamCreateWithFlags(&ws, cudaStreamNonBlocking));
             try { run_ops(pl, ws); } catch (...) { cudaStreamSynchronize(ws); cudaStreamDestroy(ws); throw; }
@@ -1440,94 +1541,6 @@ struct vb200_engine {
             if (victim == plans.end()) break;
             cudaDeviceSynchronize();
             plans.erase(victim);
-        }
-    }
-
-    // ---- poolers + heads (main stream, after joining the image branch)
-    void build_heads(Plan& pl, uint32_t select) {
-        const Config& c = cfg;
-        const int B = pl.B, T = pl.T, V = pl.V, tc = pl.t_cur, vc = pl.v_cur;
-        const int Mt = B * T, Mv = B * V, H = c.hidden, Hv = c.v_hidden, Hb = c.bi_hidden;
-        const size_t S = x3 ? 3 : 1;
-        auto& ops = pl.ops;
-        float* pooled_t = pl.mem.alloc_n<float>(static_cast<size_t>(B) * Hb);
-        float* pooled = pl.mem.alloc_n<float>(static_cast<size_t>(B) * Hb);
-        bf16* pooled_b = pl.mem.alloc_n<bf16>(static_cast<size_t>(B) * Hb * S);
-        // The poolers' operand, each sample's first row of a final state: a pruned tail's compact rows, the full state at stride
-        // L rows on dense plans, or on packed plans (a sample's first row sits at a per-call offset) the B first rows gathered into
-        // compact [B, hidden] rows.  Returns the operand and its row stride.
-        const size_t first_op = ops.size();
-        auto first_rows = [&](const bf16* tail, const bf16* state, int hid, int L, bool text, int M) -> std::pair<const bf16*, int64_t> {
-            if (tail != nullptr) return {tail, hid};
-            if (!pl.packed) return {state, static_cast<int64_t>(L) * hid};
-            bf16* first = pl.mem.alloc_n<bf16>(static_cast<size_t>(B) * hid * S);
-            GatherArgs g{};
-            g.offs = text ? pl.offs_t() : pl.offs_v(); g.n_src = M; g.B = B;
-            g.src16 = state; g.dst16 = first; g.ld16 = static_cast<int>(hid * S);
-            ops.push_back({g});
-            return {first, hid};
-        };
-        const auto first_t = first_rows(pl.tail_t, pl.t_b16[tc], H, T, true, Mt);
-        const auto first_v = first_rows(pl.tail_v, pl.v_b16[vc], Hv, V, false, Mv);
-        add_linear(pl, first_t.first, B, first_t.second, t_pool, vb::kActRelu, nullptr, 0, nullptr, nullptr, 0, pooled_t, Hb, 0, Op::NONE);
-        add_linear(pl, first_v.first, B, first_v.second, v_pool, vb::kActRelu, nullptr, 0, nullptr, pooled_b, Hb, pooled, Hb, 0, Op::NONE,
-                   pooled_t, Hb);
-        ops[first_op].sync = Op::JOIN;       // the heads start after the image branch
-        const int* rows_t = pl.packed ? pl.rows_t() : nullptr;
-        const int* rows_v = pl.packed ? pl.rows_v() : nullptr;
-        pl.outs[11] = OutBuf{pooled, B, Hb, Hb};
-        auto cls_head = [&](const ClsW& w, int n_out, int slot) {
-            bf16* hid = pl.mem.alloc_n<bf16>(static_cast<size_t>(B) * 2 * Hb * S);
-            add_linear(pl, pooled_b, B, Hb, w.fc0, vb::kActGelu, nullptr, 0, &w.ln, hid, 2 * Hb, nullptr, 0);
-            pl.outs[slot] = make_out(pl, B, n_out);
-            add_linear(pl, hid, B, 2 * Hb, w.fc3, vb::kActNone, nullptr, 0, nullptr, nullptr, 0, pl.outs[slot].p, pl.outs[slot].ld);
-        };
-        if (select & VB200_OUT_VIL_PREDICTION) cls_head(vqa, num_labels, 0);
-        if (select & VB200_OUT_VIL_PREDICTION_GQA) cls_head(gqa, gqa_labels, 1);
-        if (select & VB200_OUT_VIL_LOGIT) {
-            pl.outs[2] = make_out(pl, B, 1);
-            ops.push_back(rowdot_op(pooled, Hb, vil_logit, nullptr, pl.outs[2].p, pl.outs[2].ld, B));
-        }
-        if (select & VB200_OUT_VIL_BINARY_PREDICTION) {
-            if (B % 2 == 0) {
-                // pooled.view(-1, 2*bi_hidden): adjacent samples form one NLVR2 pair (worker.py:266-276)
-                float* hid_f = pl.mem.alloc_n<float>(static_cast<size_t>(B / 2) * 2 * Hb);
-                add_linear(pl, pooled_b, B / 2, 2 * Hb, binary.fc0, vb::kActGelu, nullptr, 0, &binary.ln, nullptr, 0, hid_f, 2 * Hb);
-                pl.outs[3] = make_out(pl, B / 2, 2);
-                ops.push_back(rowdot_op(hid_f, 2 * Hb, binary.fc3_row, nullptr, pl.outs[3].p, pl.outs[3].ld, B / 2));
-            } else {
-                // [UPSTREAM] odd batch: element 3 stays the pre-training bi_seq_relationship score
-                pl.outs[3] = make_out(pl, B, 2);
-                ops.push_back(rowdot_op(pooled, Hb, seq_rel, nullptr, pl.outs[3].p, pl.outs[3].ld, B));
-            }
-        }
-        if (select & VB200_OUT_VIL_TRI_PREDICTION) {
-            pl.outs[4] = make_out(pl, B, 3);
-            ops.push_back(rowdot_op(pooled, Hb, vil_tri, nullptr, pl.outs[4].p, pl.outs[4].ld, B));
-        }
-        if (select & VB200_OUT_VISION_PREDICTION) {
-            bf16* hid = pl.mem.alloc_n<bf16>(static_cast<size_t>(Mv) * Hv * S);
-            add_linear(pl, pl.v_b16[vc], Mv, Hv, img_transform, vb::kActGelu, nullptr, 0, &img_ln, hid, Hv, nullptr, 0, 0, Op::NONE,
-                       nullptr, 0, rows_v);
-            pl.outs[5] = make_out(pl, Mv, c.v_target);
-            add_linear(pl, hid, Mv, Hv, img_decoder, vb::kActNone, nullptr, 0, nullptr, nullptr, 0, pl.outs[5].p, pl.outs[5].ld, 0, Op::NONE,
-                       nullptr, 0, rows_v);
-        }
-        if (select & VB200_OUT_VISION_LOGIT) {
-            pl.outs[6] = make_out(pl, Mv, 1);
-            ops.push_back(rowdot_op(pl.v_f32[vc], Hv, vision_logit, pl.mask_v, pl.outs[6].p, pl.outs[6].ld, Mv, rows_v));
-        }
-        if (select & VB200_OUT_LINGUISIC_PREDICTION) {
-            bf16* hid = pl.mem.alloc_n<bf16>(static_cast<size_t>(Mt) * H * S);
-            add_linear(pl, pl.t_b16[tc], Mt, H, lm_transform, vb::kActGelu, nullptr, 0, &lm_ln, hid, H, nullptr, 0, 0, Op::NONE,
-                       nullptr, 0, rows_t);
-            pl.outs[7] = make_out(pl, Mt, c.vocab);
-            add_linear(pl, hid, Mt, H, lm_decoder, vb::kActNone, nullptr, 0, nullptr, nullptr, 0, pl.outs[7].p, pl.outs[7].ld, 0, Op::NONE,
-                       nullptr, 0, rows_t);
-        }
-        if (select & VB200_OUT_LINGUISIC_LOGIT) {
-            pl.outs[8] = make_out(pl, Mt, 1);
-            ops.push_back(rowdot_op(pl.t_f32[tc], H, ling_logit, nullptr, pl.outs[8].p, pl.outs[8].ld, Mt, rows_t));
         }
     }
 
@@ -1754,8 +1767,8 @@ struct vb200_engine {
     struct PrefixState { float* f32; void* b16; float* mask; };
     void copy_state(const Plan& pl, bool text, size_t rows, const PrefixState& to, cudaStream_t st) {
         const size_t H = text ? cfg.hidden : cfg.v_hidden, S = x3 ? 3 : 1;
-        const float* f32 = text ? pl.t_f32[pl.t_cur] : pl.v_f32[pl.v_cur];
-        const bf16* b16 = text ? pl.t_b16[pl.t_cur] : pl.v_b16[pl.v_cur];
+        const float* f32 = text ? pl.t_f32[0] : pl.v_f32[0];
+        const bf16* b16 = text ? pl.t_b16[0] : pl.v_b16[0];
         CUDA_CHECK(cudaMemcpyAsync(to.f32, f32, rows * H * 4, cudaMemcpyDeviceToDevice, st));
         CUDA_CHECK(cudaMemcpyAsync(to.b16, b16, rows * H * S * 2, cudaMemcpyDeviceToDevice, st));
         if (to.mask != nullptr) CUDA_CHECK(cudaMemcpyAsync(to.mask, text ? pl.mask_t : pl.mask_v, rows * 4, cudaMemcpyDeviceToDevice, st));
@@ -2003,8 +2016,8 @@ struct vb200_engine {
         CUDA_CHECK(cudaEventRecord(sel_done, st));
     }
     // ---- pre-training heads at chosen rows
-    // The RowHeads of `head` for n rows: bucket M = 128 * 2^k >= n, built on its first use with the forward's head launches (build_heads)
-    // at M rows and the device row count as their m_rows.
+    // The RowHeads of `head` for n rows: bucket M = 128 * 2^k >= n, built on its first use with the forward's head launches
+    // (PlanBuilder::heads) at M rows and the device row count as their m_rows.
     RowHeads& row_heads_for(int head, int n) {
         int M = 128;
         while (M < n) M *= 2;
@@ -2012,34 +2025,28 @@ struct vb200_engine {
         if (slot) return *slot;
         std::unique_ptr<RowHeads> r(new RowHeads());
         Plan& pl = r->pl;
-        pl.B = 1; pl.T = pl.V = M;
+        PlanBuilder b{*this, pl, M, "pretraining heads"};
         r->M = M;
         r->d_rows = pl.mem.alloc_n<int>(2 * static_cast<size_t>(M) + 1);
         r->loss = pl.mem.alloc_n<float>(M);
         const int* count = r->d_rows;
-        const size_t S = x3 ? 3 : 1;
         if (head == kHeadPair) {
             const int Hb = cfg.bi_hidden;
-            float* a = pl.mem.alloc_n<float>(static_cast<size_t>(M) * Hb);
+            float* a = b.buf32(M, Hb);
             r->a = a;
-            r->logits = make_out(pl, M, 2);
-            pl.ops.push_back(rowdot_op(a, Hb, seq_rel, nullptr, r->logits.p, r->logits.ld, M, count));
+            r->logits = b.make_out(M, 2);
+            b.rowdot(a, Hb, seq_rel, nullptr, r->logits, count);
         } else {
             const bool text = head == kHeadText;
             const int H = text ? cfg.hidden : cfg.v_hidden;
             const LinearW& transform = text ? lm_transform : img_transform;
             const LinearW& decoder = text ? lm_decoder : img_decoder;
-            bf16* a = pl.mem.alloc_n<bf16>(static_cast<size_t>(M) * H * S);
-            bf16* hid = pl.mem.alloc_n<bf16>(static_cast<size_t>(M) * H * S);
+            bf16* a = b.buf16(M, H);
+            bf16* hid = b.buf16(M, H);
             r->a = a;
-            pl.y_scratch[0] = pl.mem.alloc_n<float>(static_cast<size_t>(M) * H);
-            add_linear(pl, a, M, H, transform, vb::kActGelu, nullptr, 0, text ? &lm_ln : &img_ln, hid, H, nullptr, 0, 0, Op::NONE,
-                       nullptr, 0, count);
-            r->logits = make_out(pl, M, decoder.N);
-            add_linear(pl, hid, M, H, decoder, vb::kActNone, nullptr, 0, nullptr, nullptr, 0, r->logits.p, r->logits.ld, 0, Op::NONE,
-                       nullptr, 0, count);
+            b.y[0] = b.buf32(M, H);
+            b.predict(transform, text ? lm_ln : img_ln, decoder, a, H, hid, M, count, &r->logits);
         }
-        for (Op& op : pl.ops) op.tag = "pretraining heads";
         slot = std::move(r);
         return *slot;
     }
@@ -2204,30 +2211,21 @@ struct vb200_engine {
                 CUDA_CHECK(cudaMemcpyAsync(per_row[i], rh[i]->loss, static_cast<size_t>(g[i].n) * 4, cudaMemcpyDeviceToDevice, st));
         CUDA_CHECK(cudaEventRecord(pre_done, st));
     }
-    static float* out_ptr(const vb200_outputs& o, int slot) {
-        switch (slot) {
-            case 0: return o.vil_prediction; case 1: return o.vil_prediction_gqa; case 2: return o.vil_logit;
-            case 3: return o.vil_binary_prediction; case 4: return o.vil_tri_prediction; case 5: return o.vision_prediction;
-            case 6: return o.vision_logit; case 7: return o.linguisic_prediction; case 8: return o.linguisic_logit;
-            case 9: return o.sequence_output_t; case 10: return o.sequence_output_v; case 11: return o.pooled_output;
-        }
-        return nullptr;
-    }
     // rows_t / rows_v (packed plans): the call's row totals -- the per-row outputs hold that many packed rows
     void copy_outputs(Plan& pl, const vb200_outputs& out, cudaStream_t st, cudaMemcpyKind kind, int rows_t = 0, int rows_v = 0) {
-        for (int s = 0; s < 12; ++s) {
-            float* dst = out_ptr(out, s);
+        for (int s = 0; s < kNumOuts; ++s) {
+            float* dst = out.*kOutSlots[s].field;
             const OutBuf& o = pl.outs[s];
             if (dst == nullptr) continue;
             if (o.p == nullptr) fail(VB200_ERR_INVALID, "output slot %d requested but not selected in the `select` mask", s);
             int rows = o.rows;
-            if (pl.packed && (s == 5 || s == 6 || s == 10)) rows = rows_v;
-            if (pl.packed && (s == 7 || s == 8 || s == 9)) rows = rows_t;
+            if (pl.packed && kOutSlots[s].rows == kImageRow) rows = rows_v;
+            if (pl.packed && kOutSlots[s].rows == kTextRow) rows = rows_t;
             CUDA_CHECK(cudaMemcpy2DAsync(dst, static_cast<size_t>(o.cols) * 4, o.p, static_cast<size_t>(o.ld) * 4,
                                          static_cast<size_t>(o.cols) * 4, rows, kind, st));
         }
-        // packed probabilities (pl.n_probs > 0) were written into out.attention_probs by the plan's kernels: nothing to copy
-        if (out.attention_probs != nullptr && pl.n_probs == 0) {
+        // packed probabilities (layout entries) were written into out.attention_probs by the plan's kernels: nothing to copy
+        if (out.attention_probs != nullptr && pl.layout.n_entries == 0) {
             if (pl.attn.empty()) fail(VB200_ERR_INVALID, "attention_probs requested but VB200_OUT_ATTENTION is not set in `select`");
             float* dst = out.attention_probs;
             for (const Plan::AttnOut& a : pl.attn) {
@@ -2601,8 +2599,8 @@ int vb200_attention_layout(vb200_handle h, int32_t batch, int32_t n_tokens, int3
                            int32_t* n_entries, int32_t* dims, int64_t* offsets, int64_t* total_floats) {
     if (h == nullptr || n_entries == nullptr) return VB200_ERR_INVALID;
     return guard(h, [&] {
-        // derived from the layer schedule and the map selection alone (no plan is built): the order add_attn_f32 is called in by
-        // get_plan
+        // derived from the layer schedule and the map selection alone (no plan is built): the order get_plan's builder
+        // calls PlanBuilder::attention_f32 in
         const Config& c = h->cfg;
         const int T = n_tokens + (c.task_tokens ? 1 : 0), V = n_regions;
         const std::vector<int> kinds = attention_kinds(h->schedule);
@@ -3006,7 +3004,7 @@ int vb200_linear_product(const void* x16, int64_t ld_x, const void* w16, int64_t
                          int32_t block_n, int32_t act_fp16, void* cuda_stream) {
     return op_guard([&] {
         if (mul == nullptr) fail(VB200_ERR_INVALID, "vb200_linear_product: mul is NULL");
-        // as add_linear builds the pooled product: the cooperative kernel (ping-pong takes no product), its tile width, its TMA store
+        // as PlanBuilder::linear builds the pooled product: the cooperative kernel (ping-pong takes no product), its tile width, its TMA store
         const int bn = block_n > 0 ? block_n : vb::gemm_p_pick_block_n(static_cast<int>(N));
         if (bn != 64 && bn != 128 && bn != 192) fail(VB200_ERR_INVALID, "vb200_linear_product: block_n %d (plain tiles are 64, 128 or 192 wide)", bn);
         GemmEpilogue e{};
