@@ -81,9 +81,15 @@ enum {
                                                   (worker.py:287-288; the reference returns them because config.visualization is set,
                                                   worker.py:522, and never reads them).  Off unless requested: see
                                                   vb200_attention_layout and vb200_outputs.attention_probs. */
-    VB200_OUT_ATTENTION_PACKED = 1 << 10       /* the same probabilities for a packed batch, every sample at its own lengths: accepted by
+    VB200_OUT_ATTENTION_PACKED = 1 << 10,      /* the same probabilities for a packed batch, every sample at its own lengths: accepted by
                                                   vb200_forward_packed and vb200_forward_regions_packed only (see there and
                                                   vb200_attention_layout_packed); VB200_ERR_INVALID on every other forward */
+    VB200_OUT_LAYER_STATES = 1 << 11           /* the fp32 state after every step that writes a stream, by selection ("state_entries",
+                                                  "state_rows": see vb200_set_option), written by the forward's kernels into
+                                                  vb200_outputs.layer_states at the offsets of vb200_state_layout (dense forwards) or
+                                                  vb200_state_layout_packed (packed forwards).  Accepted by vb200_forward[_slot],
+                                                  vb200_forward_regions, vb200_forward_packed and vb200_forward_regions_packed;
+                                                  VB200_ERR_INVALID on every other entry point */
 };
 
 /* Inputs of one forward, in the dtypes the worker builds them (worker.py:416-419, 452-455).
@@ -121,6 +127,10 @@ typedef struct {
                                       [B, heads, Lq, Lk] back to back in execution order (vb200_attention_layout gives the
                                       offsets); NULL skips the copy.  VB200_OUT_ATTENTION_PACKED: required, device memory of
                                       vb200_attention_layout_packed's total_floats, written in place by the forward's kernels */
+    float* layer_states;           /* VB200_OUT_LAYER_STATES: required, 16-byte aligned (VB200_ERR_INVALID if NULL or not),
+                                      device memory of vb200_state_layout's / vb200_state_layout_packed's total_floats, written in
+                                      place by the forward's kernels with 16-byte stores.  Read only when the bit is set, so a host built against a header without
+                                      this field stays correct as long as it never sets the bit. */
 } vb200_outputs;
 
 /* Engine options (all optional; zero-initialise for defaults).  Flags are tri-state: 0 default, 1 on, -1 off. */
@@ -198,7 +208,8 @@ int vb200_forward_host_slot(vb200_handle h, const vb200_inputs* in, const vb200_
 
 /* Introspection used by the tests / bench: number of kernels one forward of this shape launches (with VB200_OUT_ATTENTION: one with
  * the current map selection), algorithmic FLOPs of it, model dimensions ("max_rows_per_sample": the engine's current bound;
- * "attention_entries" (-1 above 63 entries) and "attention_heads": the map selection; see vb200_set_option). */
+ * "attention_entries" (-1 above 63 entries) and "attention_heads": the map selection; "state_entries" and "state_rows": the
+ * layer-state selection; see vb200_set_option).  With VB200_OUT_LAYER_STATES the count includes one launch per selected entry. */
 int vb200_plan_info(vb200_handle h, int32_t batch, int32_t n_tokens, int32_t n_regions, uint32_t select,
                     int64_t* n_launches, double* flops);
 int vb200_model_dim(vb200_handle h, const char* key, int64_t* value);
@@ -219,7 +230,13 @@ int vb200_model_dim(vb200_handle h, const char* key, int64_t* value);
  * than 63 entries (the default then stays every entry) or attention_heads outside {0, 1} is VB200_ERR_INVALID.  Both stay in force
  * until changed and both are readable through vb200_model_dim.  The selection is part of the plan key of a forward with maps: the first
  * call after a change builds (or finds) the plan of the new selection, and a plan without maps is unaffected.  Every other output is
- * bit-identical whatever the selection. */
+ * bit-identical whatever the selection.
+ * Layer states by selection (VB200_OUT_LAYER_STATES): "state_entries" is a bitmask over the full state list in execution order (bit e:
+ * entry e of vb200_state_selection; default every entry) and "state_rows" 0 (default) writes every row of each selected entry, 1 each
+ * sample's first row, 2 each sample's mean over its real rows.  A zero mask, a bit at or past the entry count, a configuration with
+ * more than 63 entries or state_rows outside {0, 1, 2} is VB200_ERR_INVALID.  Both are engine-wide, readable through vb200_model_dim,
+ * and part of the plan key of a forward with states only.  A selection with a stream's last entry reads that stream's final rows, so
+ * that stream's last layer runs on every row, as with a sequence_output tap. */
 int vb200_set_option(vb200_handle h, const char* key, int64_t value);
 /* Profiling: after vb200_set_option(h, "timeline", 1) every persistent GEMM launch of a forward records 16 stamps per CTA (0: clock64 at
  * entry, 1: setup done, 2: first k-block landed [-DVB200_STAMPS builds], 8 / 9: %globaltimer ns at entry / exit, 10: last tile accumulated,
@@ -249,6 +266,25 @@ int vb200_attention_layout(vb200_handle h, int32_t batch, int32_t n_tokens, int3
  * layouts of vb200_attention_layout / vb200_attention_layout_packed, or -1 when "attention_entries" leaves it out.  Arrays (up to
  * max_entries) may be NULL to query the count only. */
 int vb200_attention_selection(vb200_handle h, int32_t max_entries, int32_t* n_entries, int32_t* kinds, int32_t* layout_entry);
+
+/* ---- Layer states (VB200_OUT_LAYER_STATES).  The full list holds the fp32 residual-stream state after every step that writes a
+ * stream, in execution order: the text embedding, the image embedding, then per schedule step one text entry (text layer), one
+ * image entry (image layer) or two, text then image (connection layer): 32 entries for the 12/6/6 configuration, 19 text and 13
+ * image.  An entry's value is the row the step's last LayerNorm writes; the last text / image entries equal sequence_output_t / _v.
+ * Layout of vb200_outputs.layer_states for a dense forward of this shape: selected entry i is kinds[i] (0 text, 1 image),
+ * dims[2i] rows of dims[2i + 1] floats at float offset offsets[i]: rows B x L (state_rows 0, L = T or V, padding rows included)
+ * or B (state_rows 1 and 2; a sample without a real row has NaN means).  Arrays may be NULL to query the count only.  Builds no
+ * plan and never blocks. */
+int vb200_state_layout(vb200_handle h, int32_t batch, int32_t n_tokens, int32_t n_regions, int32_t max_entries, int32_t* n_entries,
+                       int32_t* kinds, int32_t* dims, int64_t* offsets, int64_t* total_floats);
+/* The same for a packed forward with these Tin_b / V_b (HOST arrays, validated as vb200_attention_layout_packed validates them;
+ * V_b = n_boxes_b + 1 for vb200_forward_regions_packed): under state_rows 0 an entry holds sum T_b (T_b = Tin_b + task token) or
+ * sum V_b rows, sample b's rows after sample b - 1's, the layout of the packed sequence_output taps; under 1 and 2 B rows. */
+int vb200_state_layout_packed(vb200_handle h, int32_t batch, const int32_t* n_tokens, const int32_t* n_regions, int32_t max_entries,
+                              int32_t* n_entries, int32_t* kinds, int32_t* dims, int64_t* offsets, int64_t* total_floats);
+/* The full state list and the current selection: *n_entries receives the full count, kinds[e] entry e's kind (0 text, 1 image) and
+ * layout_entry[e] its index in the layouts above, or -1 when "state_entries" leaves it out.  Arrays may be NULL. */
+int vb200_state_selection(vb200_handle h, int32_t max_entries, int32_t* n_entries, int32_t* kinds, int32_t* layout_entry);
 
 /* custom_prediction()'s tensor construction fused into the forward (worker.py:422-455): instead of features [B, V, F] /
  * spatials [B, V, 5] / image_mask the caller passes what the detector produced -- box features, pixel boxes, image sizes -- and one

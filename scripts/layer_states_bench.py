@@ -1,0 +1,147 @@
+"""Cost of layer states by selection on the packed detector-output path (one JSON line).
+
+Workload: attention_maps_bench.py's -- batch 64 VQA rows in the given dtype (default bf16), U{5..20} question tokens, U{10..100}
+detector boxes per image, forward_regions_packed at fixed capacities 37 tokens / 100 boxes.  Four variants of the same call on one
+engine, the state selection set (vb200_set_option "state_entries" / "state_rows") before each window:
+  no_states      -- output_layer_states=False;
+  all_rows       -- every entry, every row (the default selection);
+  all_mean       -- every entry, each sample's mean over its rows;
+  last4_rows     -- the last four entries of the full list, every row.
+The variants alternate window by window after every plan is warm; each is timed with CUDA events around a loop of whole calls and the
+median of --rounds windows is reported, with the fp32 state floats written per call and, from a torch.profiler pass of its own, the
+device time per call of the state kernels (layer_state_kernel).  The card name, power limit and the SM clock sampled while the
+windows run are read in the same run.
+
+    python scripts/layer_states_bench.py [--batch 64] [--steps 50] [--dtype bf16]
+"""
+import argparse
+import json
+import os
+import statistics
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "scripts"))
+
+T_CAP, BOX_CAP = 37, 100
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--batch", type=int, default=64)
+    ap.add_argument("--steps", type=int, default=50)
+    ap.add_argument("--warmup", type=int, default=5)
+    ap.add_argument("--rounds", type=int, default=5, help="alternating timing windows per variant; the median is reported")
+    ap.add_argument("--dtype", default="bf16", choices=["fp16", "bf16"])
+    ap.add_argument("--seed", type=int, default=0)
+    args = ap.parse_args()
+
+    import torch
+    import vilbert_b200 as vb
+    from vilbert_b200 import synthetic as S
+    from bench import ClockSampler
+    from packed_attention_bench import detector_rows
+
+    if not torch.cuda.is_available():
+        raise SystemExit("layer_states_bench.py needs an H100: there is no CPU path")
+    cfg = vb.BertConfig(task_specific_tokens=True, visualization=True)
+    model = vb.VILBertForVLTasks.from_pretrained(S.synthetic_state_dict(cfg, seed=42), config=cfg, num_labels=3129,
+                                                 compute_dtype=args.dtype).eval().cuda(0)
+    rows = detector_rows(args.batch, args.seed, cfg.v_feature_size, cfg.vocab_size)
+    B = len(rows)
+    tin, nb = [len(r[0]) for r in rows], [r[1].shape[0] for r in rows]
+    dev = torch.device("cuda", 0)
+    pq = torch.cat([r[0] for r in rows]).to(dev)
+    packed_in = (pq, torch.zeros_like(pq), torch.ones(B, 1, dtype=torch.long, device=dev), torch.cat([r[1] for r in rows]).to(dev),
+                 torch.cat([r[2] for r in rows]).to(dev), torch.tensor([list(r[3]) for r in rows]).to(dev), tin, nb)
+
+    kinds, _ = model.state_selection()
+    n = len(kinds)
+    full = (1 << n) - 1
+    last4 = sum(1 << e for e in range(n - 4, n))
+    # variant -> (states, state_entries, state_rows)
+    variants = {"no_states": (False, full, 0), "all_rows": (True, full, 0), "all_mean": (True, full, 2), "last4_rows": (True, last4, 0)}
+
+    def select(name):
+        _, mask, rows_mode = variants[name]
+        model.set_option("state_entries", mask)
+        model.set_option("state_rows", rows_mode)
+
+    def call(name):
+        out = model.forward_regions_packed(*packed_in, select=vb.OUT_VIL_PREDICTION, max_tokens=T_CAP, max_boxes=BOX_CAP,
+                                           return_spatials=False, output_layer_states=variants[name][0])
+        return out[0] if variants[name][0] else out
+
+    floats, logits = {}, {}
+    for name, (states, _, _) in variants.items():
+        select(name)
+        floats[name] = model.state_layout_packed(tin, [n + 1 for n in nb])[1] if states else 0
+        logits[name] = call(name)[0][0]
+    torch.cuda.synchronize()
+    for name in variants:
+        if not torch.equal(logits[name], logits["no_states"]):
+            raise SystemExit(f"VQA logits of {name} differ from the call without states")
+
+    def timed(name):
+        select(name)
+        for _ in range(args.warmup):
+            call(name)
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        torch.cuda.synchronize()
+        e0.record()
+        for _ in range(args.steps):
+            call(name)
+        e1.record()
+        e1.synchronize()
+        return e0.elapsed_time(e1) / args.steps
+
+    clock = ClockSampler(0)
+    clock.start()
+    ms = {k: [] for k in variants}
+    for _ in range(args.rounds):
+        for k in variants:
+            ms[k].append(timed(k))
+    clock.stop_flag = True
+    clock.join()
+
+    from torch.profiler import ProfilerActivity, profile
+
+    def state_kernel_ms(name, n=5):
+        """Device ms per call of the state kernels, from CUPTI kernel records."""
+        select(name)
+        call(name)
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(n):
+                call(name)
+            torch.cuda.synchronize()
+        t = 0.0
+        for ev in prof.key_averages():
+            d = getattr(ev, "device_time_total", None)
+            d = ev.cuda_time_total if d is None else d
+            if "layer_state_kernel" in ev.key and ev.device_type is not None and "cuda" in str(ev.device_type).lower():
+                t += d
+        return t / n / 1e3
+    kernel_ms = {k: state_kernel_ms(k) for k in variants}
+
+    try:
+        import pynvml as nv_
+        nv_.nvmlInit()
+        h = nv_.nvmlDeviceGetHandleByIndex(0)
+        name = nv_.nvmlDeviceGetName(h)
+        card = {"name": name.decode() if isinstance(name, bytes) else name,
+                "power_limit_w": nv_.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0}
+    except Exception as e:          # NVML missing: report it
+        card = {"name": torch.cuda.get_device_name(0), "nvml_error": repr(e)}
+    card.update(clock.result())
+    result = {k: {"ms_per_call": statistics.median(v), "windows_ms": [min(v), max(v)], "state_floats_per_call": floats[k],
+                  "device_ms_per_call_state_kernels": kernel_ms[k]} for k, v in ms.items()}
+    print(json.dumps({"workload": f"batch {B} VQA rows, U{{5..20}} tokens, U{{10..100}} boxes, seed {args.seed}, {args.dtype}, "
+                                  f"forward_regions_packed at capacities {T_CAP} / {BOX_CAP}", **result, "steps": args.steps,
+                      "rounds": args.rounds, "card": card}), flush=True)
+    model.close()
+
+
+if __name__ == "__main__":
+    main()

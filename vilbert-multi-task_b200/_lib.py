@@ -28,6 +28,7 @@ OUT_TASK_HEADS = 0x15F
 OUT_ALL = 0x1FF
 OUT_ATTENTION = 1 << 9
 OUT_ATTENTION_PACKED = 1 << 10
+OUT_LAYER_STATES = 1 << 11
 
 
 class Tensor(C.Structure):
@@ -79,7 +80,14 @@ class PackedPairs(C.Structure):
 
 
 class Outputs(C.Structure):
+    """vb200_outputs up to attention_probs: the struct of hosts built before the layer_states field, which the engine accepts for
+    every call without VB200_OUT_LAYER_STATES."""
     _fields_ = [(n, C.c_void_p) for n in OUTPUT_FIELDS]
+
+
+class StateOutputs(Outputs):
+    """The full vb200_outputs: Outputs and the last field, layer_states (VB200_OUT_LAYER_STATES)."""
+    _fields_ = [("layer_states", C.c_void_p)]
 
 
 # vb200_decode_family: which output a decode message reads (include/vilbert_b200.h, vb200_decode_answers)
@@ -151,7 +159,8 @@ class Options(C.Structure):
 # every symbol include/vilbert_b200.h declares (tests/test_cabi.py checks the list against the header)
 EXPORTS = ["vb200_abi_version", "vb200_create", "vb200_destroy", "vb200_last_error", "vb200_forward", "vb200_forward_slot",
            "vb200_forward_host", "vb200_forward_host_slot", "vb200_plan_info", "vb200_model_dim", "vb200_set_option", "vb200_timeline", "vb200_profile_ops",
-           "vb200_attention_layout", "vb200_attention_layout_packed", "vb200_attention_selection", "vb200_forward_regions", "vb200_forward_packed", "vb200_forward_regions_packed", "vb200_encode_text", "vb200_encode_image", "vb200_forward_cached",
+           "vb200_attention_layout", "vb200_attention_layout_packed", "vb200_attention_selection", "vb200_state_layout", "vb200_state_layout_packed", "vb200_state_selection",
+           "vb200_forward_regions", "vb200_forward_packed", "vb200_forward_regions_packed", "vb200_encode_text", "vb200_encode_image", "vb200_forward_cached",
            "vb200_encode_text_packed", "vb200_encode_image_packed", "vb200_encode_regions_packed", "vb200_forward_cached_packed", "vb200_linear", "vb200_linear_rows", "vb200_linear_split", "vb200_layernorm", "vb200_layernorm_split", "vb200_attention_f32",
            "vb200_self_attention", "vb200_co_attention", "vb200_self_attention_packed", "vb200_co_attention_packed",
            "vb200_self_attention_stream", "vb200_co_attention_stream",
@@ -198,6 +207,11 @@ def load():
     lib.vb200_attention_layout.argtypes = [vp, i32, i32, i32, i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(i64), C.POINTER(i64)]
     lib.vb200_attention_layout_packed.argtypes = [vp, i32, vp, vp, i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(i64), C.POINTER(i64)]
     lib.vb200_attention_selection.argtypes = [vp, i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)]
+    lib.vb200_state_layout.argtypes = [vp, i32, i32, i32, i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), C.POINTER(i64),
+                                       C.POINTER(i64)]
+    lib.vb200_state_layout_packed.argtypes = [vp, i32, vp, vp, i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), C.POINTER(i64),
+                                              C.POINTER(i64)]
+    lib.vb200_state_selection.argtypes = lib.vb200_attention_selection.argtypes
     lib.vb200_forward_regions.argtypes = [vp, C.POINTER(RegionInputs), C.POINTER(Outputs), u32, i32, vp]
     lib.vb200_forward_packed.argtypes = [vp, C.POINTER(PackedInputs), C.POINTER(Outputs), u32, i32, vp]
     lib.vb200_forward_regions_packed.argtypes = [vp, C.POINTER(PackedRegionInputs), C.POINTER(Outputs), u32, i32, vp]

@@ -412,6 +412,59 @@ rowdot_kernel(const float* __restrict__ x, int ld_x, const float* __restrict__ W
     }
 }
 
+// Layer states: REDUCE 0 copies rows with a grid-stride loop of 16-byte accesses, 1 one CTA per sample copies its first row, 2 one
+// CTA per (sample, 128 columns) where each thread owns one column and walks the sample's rows in order.  Every launch waits for the
+// op that wrote src before looking at the destination, so the dependents of a launch that writes nothing still see that op's rows.
+constexpr int kStateThreads = 128;
+template <int REDUCE>
+__global__ void __launch_bounds__(kStateThreads)
+layer_state_kernel(StateArgs a, int pdl) {
+    if (pdl) { pdl_wait(); pdl_launch_dependents(); }
+    float* dst = reinterpret_cast<float*>(static_cast<uintptr_t>(a.dst[0]));
+    if (dst == nullptr) return;
+    const int b = blockIdx.x;
+    if constexpr (REDUCE == 0) {
+        const int rows = a.offs != nullptr ? *a.m_rows : a.B * a.L;
+        const int64_t n4 = static_cast<int64_t>(rows) * (a.H / 4);
+        const float4* src = reinterpret_cast<const float4*>(a.src);
+        float4* out = reinterpret_cast<float4*>(dst);
+        for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n4; i += static_cast<int64_t>(gridDim.x) * blockDim.x)
+            out[i] = src[i];
+    } else if constexpr (REDUCE == 1) {
+        const int64_t row = a.offs != nullptr ? a.offs[b] : static_cast<int64_t>(b) * a.L;
+        const float4* src = reinterpret_cast<const float4*>(a.src + row * a.H);
+        float4* out = reinterpret_cast<float4*>(dst + static_cast<int64_t>(b) * a.H);
+        for (int c = threadIdx.x; c < a.H / 4; c += blockDim.x) out[c] = src[c];
+    } else {
+        const int col = blockIdx.y * kStateThreads + threadIdx.x;
+        if (col >= a.H) return;
+        const int r0 = a.offs != nullptr ? a.offs[b] : b * a.L;
+        const int r1 = a.offs != nullptr ? a.offs[b + 1] : r0 + a.L;
+        float sum = 0.0f;
+        int count = 0;
+        for (int r = r0; r < r1; ++r) {
+            if (a.mask != nullptr && a.mask[r] != 0.0f) continue;
+            sum = __fadd_rn(sum, a.src[static_cast<int64_t>(r) * a.H + col]);
+            ++count;
+        }
+        dst[static_cast<int64_t>(b) * a.H + col] = count > 0 ? __fdiv_rn(sum, static_cast<float>(count)) : __int_as_float(0x7fc00000);
+    }
+}
+
+cudaError_t launch_layer_state(const StateArgs& a, int pdl, cudaStream_t st) {
+    if (a.B < 1 || a.L < 1 || a.H < 4 || a.H % 4 != 0 || a.dst == nullptr || (a.offs != nullptr) != (a.m_rows != nullptr) ||
+        (reinterpret_cast<uintptr_t>(a.src) & 15) || a.reduce < 0 || a.reduce > 2)
+        return cudaErrorInvalidValue;
+    const dim3 block(kStateThreads);
+    if (a.reduce == 0) {
+        const int64_t n4 = static_cast<int64_t>(a.B) * a.L * (a.H / 4);
+        const dim3 grid(static_cast<unsigned>(std::min<int64_t>((n4 + kStateThreads - 1) / kStateThreads, 2048)));
+        return launch_ex(layer_state_kernel<0>, grid, block, 0, pdl, st, a, pdl);
+    }
+    if (a.reduce == 1) return launch_ex(layer_state_kernel<1>, dim3(a.B), block, 0, pdl, st, a, pdl);
+    return launch_ex(layer_state_kernel<2>, dim3(a.B, (a.H + kStateThreads - 1) / kStateThreads), block, 0, pdl, st, a, pdl);
+}
+
 cudaError_t launch_text_embed(const int64_t* ids, const int64_t* seg, const int64_t* input_mask, const int64_t* task,
                               const float* word, const float* pos, const float* type, const float* task_tab,
                               const float* gamma, const float* beta, float eps, float* out_f32,

@@ -422,7 +422,7 @@ struct GatherArgs { const int* offs; int n_src, B; const bf16* src16; bf16* dst1
 
 struct Op {
     // the index of the alternative is the kind number vb200_profile_ops reports
-    std::variant<GemmCall, SelfAttnArgs, CoAttnArgs, RowdotArgs, LayerNormArgs, AttnF32Args, GatherArgs> args;
+    std::variant<GemmCall, SelfAttnArgs, CoAttnArgs, RowdotArgs, LayerNormArgs, AttnF32Args, GatherArgs, vb::StateArgs> args;
     int stream = 0;                // 0 main, 1 side (image branch) inside the captured graph
     double flops = 0;
     enum Sync { NONE, FORK, JOIN } sync = NONE;   // fork/join markers for the two-stream graph
@@ -466,11 +466,13 @@ constexpr uint32_t out_bits(OutRows rows) {
 // The d_meta format of a packed plan, in ints: text row offsets [B + 1] | image row offsets [B + 1]; with `src` (a packed pair suffix)
 // then the pairs' first rows in the cached text states [B] | image states [B]; with n_entries > 0 (the packed attention
 // probabilities, VB200_OUT_ATTENTION_PACKED) then, 8-byte aligned, the int64 destination pointer | entry float offsets [n_entries] |
-// per-sample prefix sums [3][B + 1] (sum T_b'^2, sum V_b'^2, sum T_b' V_b' over b' < b).  A stream's row total, which bounds its GEMM,
-// LayerNorm and rowdot rows, is its last offset.
+// per-sample prefix sums [3][B + 1] (sum T_b'^2, sum V_b'^2, sum T_b' V_b' over b' < b); with n_states > 0 (the layer states,
+// VB200_OUT_LAYER_STATES, which dense plans stage in the same format) then, 8-byte aligned, one int64 destination pointer per selected
+// state entry.  A stream's row total, which bounds its GEMM, LayerNorm and rowdot rows, is its last offset.
 struct MetaLayout {
     size_t B = 0, n_entries = 0;
     bool src = false;
+    size_t n_states = 0;
     size_t offs_t() const { return 0; }
     size_t offs_v() const { return B + 1; }
     size_t rows_t() const { return offs_t() + B; }
@@ -481,7 +483,9 @@ struct MetaLayout {
     size_t probs_dst() const { return (rows_end() + 1) & ~static_cast<size_t>(1); }
     size_t probs_entry(size_t e) const { return probs_dst() + 2 * (1 + e); }
     size_t probs_prefix(int k) const { return probs_entry(n_entries) + 2 * static_cast<size_t>(k) * (B + 1); }
-    size_t size() const { return n_entries ? probs_prefix(3) : rows_end(); }
+    size_t probs_end() const { return n_entries ? probs_prefix(3) : rows_end(); }
+    size_t state_dst(size_t e) const { return ((probs_end() + 1) & ~static_cast<size_t>(1)) + 2 * e; }
+    size_t size() const { return n_states ? state_dst(n_states) : probs_end(); }
 };
 
 // Which attention maps a forward writes (vb200_set_option "attention_entries" / "attention_heads"): bit e of `mask` selects entry e
@@ -502,6 +506,69 @@ std::vector<int> attention_kinds(const std::vector<std::string>& schedule) {
         else { k.push_back(2); k.push_back(3); }
     }
     return k;
+}
+
+// Which layer states a forward writes (vb200_set_option "state_entries" / "state_rows"): bit e of `mask` selects entry e of the full
+// list (state_kinds; a configuration with more than 63 entries always writes every entry), `rows` 0 every row, 1 each sample's first
+// row, 2 each sample's mean over its real rows.  The default is every entry, every row.
+struct StateSelect {
+    uint64_t mask = ~0ull;
+    int rows = 0;
+    bool has(int e) const { return e > 63 || ((mask >> e) & 1); }
+    int index(int e) const { return e > 63 ? e : __builtin_popcountll(mask & ((1ull << e) - 1)); }   // e's place in the layouts
+};
+// The full layer-state list in execution order, 0 a text state and 1 an image state: the text and the image embedding, then per
+// schedule step the state of each stream it writes, text first.  Built next to attention_kinds so both lists follow the schedule.
+std::vector<int> state_kinds(const std::vector<std::string>& schedule) {
+    std::vector<int> k{0, 1};
+    for (const std::string& step : schedule) {
+        if (step[0] != 'V') k.push_back(0);
+        if (step[0] != 'T') k.push_back(1);
+    }
+    return k;
+}
+// Layout of vb200_outputs.layer_states: the selected entries in execution order, each `rows` x width floats back to back.  rows_t /
+// rows_v are a stream's rows under state_rows 0 (dense: B x T / B x V, packed: the call's row totals); state_rows 1 and 2 give B.
+struct StateLayout {
+    std::vector<int32_t> kind, rows, width;
+    std::vector<int64_t> offset;
+    int64_t total = 0;
+};
+StateLayout state_layout(const Config& c, const std::vector<std::string>& schedule, const StateSelect& sel, int B, int64_t rows_t,
+                         int64_t rows_v) {
+    StateLayout l;
+    const std::vector<int> kinds = state_kinds(schedule);
+    for (int e = 0; e < static_cast<int>(kinds.size()); ++e) {
+        if (!sel.has(e)) continue;
+        const int kind = kinds[e], width = kind == 0 ? c.hidden : c.v_hidden;
+        const int64_t rows = sel.rows == 0 ? (kind == 0 ? rows_t : rows_v) : B;
+        l.kind.push_back(kind);
+        l.rows.push_back(static_cast<int32_t>(rows));
+        l.width.push_back(width);
+        l.offset.push_back(l.total);
+        l.total += rows * width;
+    }
+    return l;
+}
+// Each selected entry's destination (dst + its offset) into meta, in the layout's state section (resized to hold it)
+void put_state_dsts(MetaLayout& layout, std::vector<int>& meta, const StateLayout& l, float* dst) {
+    layout.n_states = l.offset.size();
+    meta.resize(layout.size(), 0);
+    for (size_t e = 0; e < l.offset.size(); ++e) {
+        const int64_t p = static_cast<int64_t>(reinterpret_cast<uintptr_t>(dst + l.offset[e]));
+        memcpy(meta.data() + layout.state_dst(e), &p, sizeof(p));
+    }
+}
+// A forward with VB200_OUT_LAYER_STATES needs the caller's buffer, 16-byte aligned: the state kernels write it with 16-byte stores.
+void check_state_buffer(const char* api, const float* states) {
+    if (states == nullptr) fail(VB200_ERR_INVALID, "%s: VB200_OUT_LAYER_STATES needs vb200_outputs.layer_states (NULL)", api);
+    if (reinterpret_cast<uintptr_t>(states) & 15) fail(VB200_ERR_INVALID, "%s: vb200_outputs.layer_states is not 16-byte aligned", api);
+}
+// The layer states exist for the dense and packed device-pointer forwards only; every other entry point rejects their select bit.
+void reject_layer_states(uint32_t select, const char* api) {
+    if (select & VB200_OUT_LAYER_STATES)
+        fail(VB200_ERR_INVALID, "%s: VB200_OUT_LAYER_STATES is only supported by vb200_forward, vb200_forward_slot, vb200_forward_regions, "
+             "vb200_forward_packed and vb200_forward_regions_packed", api);
 }
 
 // Layout of the packed attention probabilities (VB200_OUT_ATTENTION_PACKED) from the two streams' row offsets [B + 1]: the selected
@@ -566,9 +633,10 @@ struct PackedBatch {
 // Validates a packed call's lengths and lays out its rows: offs[i + 1] = offs[i] + rows_i per stream (text: T_i = Tin_i + task
 // token).  Rejects a batch < 1, a negative capacity, a length < 1 or above a non-zero capacity, more than max_rows rows per sample
 // (the engine's max_rows_per_sample) and Tin_i > max_position_embeddings.  maps (non-null): where the plan's kernels write the packed
-// attention probabilities of the entries `sel` selects, whose layout then joins the meta.
+// attention probabilities of the entries `sel` selects, whose layout then joins the meta; states (non-null): the same for the layer
+// states `ssel` selects.
 PackedBatch pack_batch(const char* api, const Config& c, const std::vector<std::string>& schedule, const PackedLengths& in, float* maps,
-                       int max_rows, const AttnSelect& sel = {}) {
+                       int max_rows, const AttnSelect& sel = {}, float* states = nullptr, const StateSelect& ssel = {}) {
     if (in.B < 1) fail(VB200_ERR_INVALID, "%s: batch must be positive", api);
     if (in.max_tokens < 0) fail(VB200_ERR_INVALID, "%s: negative capacity max_tokens %d", api, in.max_tokens);
     if (in.max_regions < 0) fail(VB200_ERR_INVALID, "%s: negative capacity max_regions %d", api, in.max_regions);
@@ -613,6 +681,7 @@ PackedBatch pack_batch(const char* api, const Config& c, const std::vector<std::
         memcpy(b.meta.data() + b.layout.probs_entry(0), l.offset.data(), l.offset.size() * sizeof(int64_t));
         memcpy(b.meta.data() + b.layout.probs_prefix(0), l.prefix.data(), l.prefix.size() * sizeof(int64_t));
     }
+    if (states) put_state_dsts(b.layout, b.meta, state_layout(c, schedule, ssel, in.B, b.rows_t(), b.rows_v()), states);
     return b;
 }
 // Detector box counts of a packed region call -> regions per image, V_i = n_boxes_i + 1 (the boxes and the global mean row), and
@@ -711,6 +780,7 @@ struct vb200_engine {
     // bring.  Validation only -- a plan's attention kernels follow from its shape (streaming above 256 rows), so no plan is dropped.
     int max_rows = 256;
     AttnSelect attn_sel;       // vb200_set_option("attention_entries" / "attention_heads"): the maps a forward with the map bit writes
+    StateSelect state_sel;     // vb200_set_option("state_entries" / "state_rows"): the layer states a forward with the state bit writes
     bool x3 = false;           // fp32-parity mode (vb200_options::split_fp32): fp16 hi/lo split operands, K' = 3K GEMMs, fp32 attention
     // Programmatic dependent launch (opt.use_pdl): every kernel triggers its dependents once its main work is issued, and a
     // dependent GEMM's producer puts its first weight tiles in flight before griddepcontrol.wait.  On by default;
@@ -1086,6 +1156,7 @@ struct vb200_engine {
         bool maps = false;                  // the forward writes the attention maps attn_sel selects
         int entry = 0;                      // the current schedule step's first attention-map entry in the full list
         int n_probs = 0;                    // packed attention-probability ops added so far (their entry index)
+        bool states = false;                // the forward writes the layer states state_sel selects
 
         // Physical width factor of the 16-bit operand buffers: in fp32-parity mode (x3) each is 3x as wide (fp16 hi | lo | hi per 64
         // columns).  buf16 sizes them, linear and gather scale their strides and K; nothing else applies it.
@@ -1199,6 +1270,15 @@ struct vb200_engine {
                 a.probs = attn_out(mean ? 1 : heads, a.Lq, a.Lk);
             }
             push({a, branch, 0.0});
+        }
+        // Layer-state entry e of the full list (state_kinds), stream s's fp32 state, when the forward writes it and state_sel selects
+        // it: one launch on s's branch, added right after the op that wrote the state, so the stream's next layer cannot overwrite it
+        // first.  Its destination is the entry's pointer in the plan's staged meta.
+        void state(const StreamRec& s, int e) {
+            if (!states || !eng.state_sel.has(e)) return;
+            const vb::StateArgs a{s.f32[0], s.offs, s.m_rows, pl.packed ? nullptr : s.mask,
+                                  pl.meta64(pl.layout.state_dst(eng.state_sel.index(e))), pl.B, s.seq, s.hid, eng.state_sel.rows};
+            push({a, s.branch, 0.0});
         }
         // a dense plan's next attention-probability output [B, heads, Lq, Lk]
         float* attn_out(int heads, int Lq, int Lk) {
@@ -1358,6 +1438,14 @@ struct vb200_engine {
         return n;
     }
 
+    // layer-state entries one forward with states writes
+    int selected_states() const {
+        const int all = static_cast<int>(state_kinds(schedule).size());
+        int n = 0;
+        for (int e = 0; e < all; ++e) n += state_sel.has(e) ? 1 : 0;
+        return n;
+    }
+
     // Plan modes.  FULL is the reference's forward (worker.py:286-289).  The other three split it at the first connection layer
     // for caption-image retrieval (SURVEY.md section 8e): everything before it depends on the caption alone (text embeddings +
     // the text layers scheduled ahead of C0) or on the image alone (image embedding + any image layer ahead of C0), so a
@@ -1387,12 +1475,20 @@ struct vb200_engine {
                      "taps or attention maps)", h.name);
     }
 
-    Plan* get_plan(int B, int Tin, int V, uint32_t select, int slot = 0, int mode = FULL, bool want_attn = false) {
+    // The plan-key bits of the final rows a layer-state selection reads: a selected last entry of a stream keeps its tail unpruned.
+    uint32_t states_read() const {
+        const std::vector<int> k = state_kinds(schedule);
+        int last[2] = {0, 0};
+        for (int e = 0; e < static_cast<int>(k.size()); ++e) last[k[e]] = e;
+        return (state_sel.has(last[0]) ? kTextRows : 0) | (state_sel.has(last[1]) ? kImageRows : 0);
+    }
+    Plan* get_plan(int B, int Tin, int V, uint32_t select, int slot = 0, int mode = FULL, bool want_attn = false, bool want_states = false) {
         if (slot < 0 || slot > 15) fail(VB200_ERR_INVALID, "slot %d out of range (0..15)", slot);
         if (slot > 0 && !opt.use_cuda_graph) fail(VB200_ERR_INVALID, "concurrent slots need CUDA-graph plans (use_cuda_graph)");
         const bool packed = mode >= PACKED;
         const int schedule_mode = packed ? mode - PACKED : mode;     // which part of the schedule: FULL, a prefix or the suffix
-        if (schedule_mode == TEXT_PREFIX || schedule_mode == IMAGE_PREFIX) { select = 0; want_attn = false; }
+        if (schedule_mode == TEXT_PREFIX || schedule_mode == IMAGE_PREFIX) { select = 0; want_attn = false; want_states = false; }
+        if (want_states) select |= states_read();
         if (pretraining) reject_task_heads(select);
         const int T = Tin + (cfg.task_tokens ? 1 : 0);
         // ahead of the cache: a plan built under a higher max_rows_per_sample must not outlive the bound being lowered.  Packed
@@ -1401,8 +1497,11 @@ struct vb200_engine {
         if (T > cap || V > cap)
             fail(VB200_ERR_INVALID, "sequence too long for %s (T=%d, V=%d, max %d)", bound_name(max_rows), T, V, cap);
         // the map selection is part of the key of a plan with maps: a call never replays a plan built for another selection
+        // and so is the state selection of a plan with layer states
         std::vector<int64_t> key{B, Tin, V, static_cast<int64_t>(select), slot, mode, want_attn ? 1 : 0,
-                                 want_attn ? static_cast<int64_t>(attn_sel.mask) : 0, want_attn && attn_sel.mean ? 1 : 0};
+                                 want_attn ? static_cast<int64_t>(attn_sel.mask) : 0, want_attn && attn_sel.mean ? 1 : 0,
+                                 want_states ? 1 : 0, want_states ? static_cast<int64_t>(state_sel.mask) : 0,
+                                 want_states ? state_sel.rows : 0};
         auto it = plans.find(key);
         if (it != plans.end()) { it->second->last_use = ++use_clock; return it->second.get(); }
         std::unique_ptr<Plan> up(new Plan());
@@ -1411,10 +1510,12 @@ struct vb200_engine {
         if (B < 1 || Tin < 1 || V < 1) fail(VB200_ERR_INVALID, "batch, n_tokens and n_regions must be positive");
         if (Tin > c.max_pos && !packed) fail(VB200_ERR_INVALID, "n_tokens %d exceeds max_position_embeddings %d", Tin, c.max_pos);
         pl.B = B; pl.Tin = Tin; pl.T = T; pl.V = V;
-        if (packed) {
-            // zero offsets until the first call: the validation pass and the capture below then touch no row
-            pl.packed = true;
-            pl.layout = MetaLayout{static_cast<size_t>(B), want_attn ? static_cast<size_t>(selected_entries()) : 0, mode == PACKED_SUFFIX};
+        if (packed || want_states) {
+            // zero offsets and destinations until the first call: the validation pass and the capture below then touch no row and
+            // write no state.  Dense plans hold only the layer states' destinations.
+            pl.packed = packed;
+            pl.layout = MetaLayout{static_cast<size_t>(B), packed && want_attn ? static_cast<size_t>(selected_entries()) : 0,
+                                   mode == PACKED_SUFFIX, want_states ? static_cast<size_t>(selected_states()) : 0};
             const size_t n_meta = pl.layout.size();
             pl.d_meta = pl.mem.alloc_n<int>(n_meta);
             CUDA_CHECK(cudaMemset(pl.d_meta, 0, n_meta * sizeof(int)));
@@ -1467,6 +1568,7 @@ struct vb200_engine {
         b.v = StreamRec{pl.v_f32, pl.v_b16, Hv, V, Mv, 1, 1, pl.mask_v, qkv_v, ctx_v, inter_v, packed ? pl.rows_v() : nullptr,
                         packed ? pl.offs_v() : nullptr, nullptr};
         b.maps = want_attn;
+        b.states = want_states;
 
         // image embedding: LayerNorm(feat.W_img^T + loc.W_loc^T + b) as ONE GEMM over K = v_feat + 64, on the side stream: it
         // overlaps the text layers ahead of the first co-attention
@@ -1475,6 +1577,11 @@ struct vb200_engine {
             g.ln = &vemb_ln; g.out16 = pl.v_b16[0]; g.ld16 = Hv; g.out32 = pl.v_f32[0]; g.ld32 = Hv;
             b.linear(g);
         }
+        // layer states (FULL and PACKED plans only): the embeddings are entries 0 (text, written by the input kernels ahead of the
+        // plan) and 1, then each step's text state before its image state
+        b.state(b.v, 1);
+        b.state(b.t, 0);
+        int state_e = 2;
         bool in_suffix = false;
         for (size_t si = 0; si < schedule.size(); ++si) {
             const std::string& step = schedule[si];
@@ -1488,6 +1595,8 @@ struct vb200_engine {
             } else if (do_s) {
                 b.connection(c_layers[idx]);
             }
+            if (step[0] != 'V') b.state(b.t, state_e++);
+            if (step[0] != 'T') b.state(b.v, state_e++);
             b.entry += step[0] == 'C' ? 2 : 1;
         }
         if (b.t.tail == nullptr) pl.outs[kOutSeqT] = OutBuf{pl.t_f32[0], Mt, H, H};
@@ -1585,6 +1694,7 @@ struct vb200_engine {
                 CUDA_CHECK(vb::launch_gather_state(a.offs, a.n_src, a.src_f32, a.src16, nullptr, a.dst_f32, a.dst16, nullptr, a.B, 1,
                                                    a.hidden, a.ld16, st));
             },
+            [&](const vb::StateArgs& a) { CUDA_CHECK(vb::launch_layer_state(a, pdl, st)); },
         }, op.args);
     }
     // vb200_profile_ops' dims of a launch-list entry
@@ -1597,6 +1707,7 @@ struct vb200_engine {
             [](const LayerNormArgs& a) { return std::array<int, 4>{a.M, a.N, 0, 0}; },
             [](const AttnF32Args& a) { return std::array<int, 4>{a.B, 0, 0, a.heads}; },
             [](const GatherArgs& a) { return std::array<int, 4>{a.B, 0, 0, 0}; },
+            [](const vb::StateArgs& a) { return std::array<int, 4>{a.B, a.L, a.H, 0}; },
         }, op.args);
     }
     // Text-stream ops go to `st`, image-stream ops to the side stream so the two ViLBERT streams overlap
@@ -1788,9 +1899,19 @@ struct vb200_engine {
     void run_dense(const char* api, int B, int Tin, int V, uint32_t select, int slot, int mode, const vb200_outputs* out,
                    const PrefixState& state, cudaMemcpyKind kind, void* cuda_stream, const std::function<void(Plan&, cudaStream_t)>& input) {
         reject_packed_attention(select, api);
+        if (mode != FULL || kind != cudaMemcpyDeviceToDevice) reject_layer_states(select, api);
+        const bool states = (select & VB200_OUT_LAYER_STATES) != 0;
+        if (states) check_state_buffer(api, out->layer_states);
         CUDA_CHECK(cudaSetDevice(opt.device));
-        Plan& pl = *get_plan(B, Tin, V, (select & VB200_OUT_ALL) | rows_read(out), slot, mode, (select & VB200_OUT_ATTENTION) != 0);
+        Plan& pl = *get_plan(B, Tin, V, (select & VB200_OUT_ALL) | rows_read(out), slot, mode, (select & VB200_OUT_ATTENTION) != 0, states);
         const cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+        if (states) {
+            MetaLayout layout{static_cast<size_t>(pl.B)};
+            std::vector<int> meta(layout.size(), 0);
+            put_state_dsts(layout, meta, state_layout(cfg, schedule, state_sel, pl.B, static_cast<int64_t>(pl.B) * pl.T,
+                                                      static_cast<int64_t>(pl.B) * pl.V), out->layer_states);
+            stage_meta(pl, meta, st);
+        }
         input(pl, st);
         run_plan(pl, st);
         if (out != nullptr) copy_outputs(pl, *out, st, kind);
@@ -1804,13 +1925,17 @@ struct vb200_engine {
         if (select & VB200_OUT_ATTENTION)
             fail(VB200_ERR_INVALID, "%s: the attention-probability output (VB200_OUT_ATTENTION) is not supported", api);
         if (mode != PACKED) reject_packed_attention(select, api);
+        if (mode != PACKED) reject_layer_states(select, api);
         const bool maps = (select & VB200_OUT_ATTENTION_PACKED) != 0;
         if (maps && out->attention_probs == nullptr)
             fail(VB200_ERR_INVALID, "%s: VB200_OUT_ATTENTION_PACKED needs vb200_outputs.attention_probs (NULL)", api);
         if (x3) fail(VB200_ERR_INVALID, "%s: packed batches are not supported in split_fp32 (fp32x) mode", api);
-        const PackedBatch b = pack_batch(api, cfg, schedule, len, maps ? out->attention_probs : nullptr, max_rows, attn_sel);
+        const bool states = (select & VB200_OUT_LAYER_STATES) != 0;
+        if (states) check_state_buffer(api, out->layer_states);
+        const PackedBatch b = pack_batch(api, cfg, schedule, len, maps ? out->attention_probs : nullptr, max_rows, attn_sel,
+                                         states ? out->layer_states : nullptr, state_sel);
         CUDA_CHECK(cudaSetDevice(opt.device));
-        Plan& pl = *get_plan(len.B, b.Tin, b.V, (select & VB200_OUT_ALL) | rows_read(out), slot, mode, maps);
+        Plan& pl = *get_plan(len.B, b.Tin, b.V, (select & VB200_OUT_ALL) | rows_read(out), slot, mode, maps, states);
         const cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
         stage_meta(pl, b.meta, st);
         input(pl, b, st);
@@ -2658,6 +2783,60 @@ int vb200_attention_selection(vb200_handle h, int32_t max_entries, int32_t* n_en
     });
 }
 
+}  // extern "C"
+
+namespace {
+// the arrays of vb200_state_layout / vb200_state_layout_packed
+void put_state_layout(const StateLayout& l, int32_t max_entries, int32_t* n_entries, int32_t* kinds, int32_t* dims, int64_t* offsets,
+                      int64_t* total_floats) {
+    const int n = static_cast<int>(l.offset.size());
+    for (int e = 0; e < n && e < max_entries; ++e) {
+        if (kinds) kinds[e] = l.kind[e];
+        if (dims) { dims[2 * e] = l.rows[e]; dims[2 * e + 1] = l.width[e]; }
+        if (offsets) offsets[e] = l.offset[e];
+    }
+    *n_entries = n;
+    if (total_floats) *total_floats = l.total;
+}
+}  // namespace
+
+extern "C" {
+
+int vb200_state_layout(vb200_handle h, int32_t batch, int32_t n_tokens, int32_t n_regions, int32_t max_entries, int32_t* n_entries,
+                       int32_t* kinds, int32_t* dims, int64_t* offsets, int64_t* total_floats) {
+    if (h == nullptr || n_entries == nullptr) return VB200_ERR_INVALID;
+    return guard(h, [&] {
+        if (batch < 1 || n_tokens < 1 || n_regions < 1) fail(VB200_ERR_INVALID, "vb200_state_layout: batch, n_tokens and n_regions must be positive");
+        const int64_t T = n_tokens + (h->cfg.task_tokens ? 1 : 0);
+        put_state_layout(state_layout(h->cfg, h->schedule, h->state_sel, batch, batch * T, static_cast<int64_t>(batch) * n_regions),
+                         max_entries, n_entries, kinds, dims, offsets, total_floats);
+    });
+}
+
+int vb200_state_layout_packed(vb200_handle h, int32_t batch, const int32_t* n_tokens, const int32_t* n_regions, int32_t max_entries,
+                              int32_t* n_entries, int32_t* kinds, int32_t* dims, int64_t* offsets, int64_t* total_floats) {
+    if (h == nullptr || n_entries == nullptr) return VB200_ERR_INVALID;
+    return guard(h, [&] {
+        const char* api = "vb200_state_layout_packed";
+        if (!n_tokens || !n_regions) fail(VB200_ERR_INVALID, "%s: NULL length array", api);
+        const PackedBatch b = pack_batch(api, h->cfg, h->schedule, {"sample", batch, n_tokens, 0, n_regions, 0}, nullptr, h->max_rows);
+        put_state_layout(state_layout(h->cfg, h->schedule, h->state_sel, batch, b.rows_t(), b.rows_v()), max_entries, n_entries, kinds,
+                         dims, offsets, total_floats);
+    });
+}
+
+int vb200_state_selection(vb200_handle h, int32_t max_entries, int32_t* n_entries, int32_t* kinds, int32_t* layout_entry) {
+    if (h == nullptr || n_entries == nullptr) return VB200_ERR_INVALID;
+    return guard(h, [&] {
+        const std::vector<int> k = state_kinds(h->schedule);
+        for (int e = 0; e < static_cast<int>(k.size()) && e < max_entries; ++e) {
+            if (kinds) kinds[e] = k[e];
+            if (layout_entry) layout_entry[e] = h->state_sel.has(e) ? h->state_sel.index(e) : -1;
+        }
+        *n_entries = static_cast<int32_t>(k.size());
+    });
+}
+
 int vb200_forward_host(vb200_handle h, const vb200_inputs* in, const vb200_outputs* out, uint32_t select, void* cuda_stream) {
     return vb200_forward_host_slot(h, in, out, select, 0, 1, cuda_stream);
 }
@@ -2699,7 +2878,7 @@ int vb200_plan_info(vb200_handle h, int32_t batch, int32_t n_tokens, int32_t n_r
     return guard(h, [&] {
         CUDA_CHECK(cudaSetDevice(h->opt.device));
         Plan* pl = h->get_plan(batch, n_tokens, n_regions, select & VB200_OUT_ALL, 0, vb200_engine::FULL,
-                               (select & VB200_OUT_ATTENTION) != 0);
+                               (select & VB200_OUT_ATTENTION) != 0, (select & VB200_OUT_LAYER_STATES) != 0);
         if (n_launches) *n_launches = static_cast<int64_t>(pl->ops.size()) + 2;   // + text-embed + image-pack
         if (flops) *flops = pl->flops;
     });
@@ -2773,6 +2952,20 @@ int vb200_set_option(vb200_handle h, const char* key, int64_t value) {
             if (value != 0 && value != 1)
                 fail(VB200_ERR_INVALID, "attention_heads must be 0 (every head) or 1 (the mean over heads), got %lld", (long long)value);
             h->attn_sel.mean = value == 1;
+        } else if (k == "state_entries") {
+            // part of the plan key of a plan with states: no cached plan is dropped
+            const int n = static_cast<int>(state_kinds(h->schedule).size());
+            if (n > 63) fail(VB200_ERR_INVALID, "state_entries: this configuration has %d state entries, more than the 63 a mask holds", n);
+            const uint64_t full = (1ull << n) - 1;
+            if (value == 0 || (static_cast<uint64_t>(value) & ~full) != 0)
+                fail(VB200_ERR_INVALID, "state_entries: mask 0x%llx must be non-zero and select only entries 0..%d", (unsigned long long)value,
+                     n - 1);
+            h->state_sel.mask = static_cast<uint64_t>(value) == full ? ~0ull : static_cast<uint64_t>(value);
+        } else if (k == "state_rows") {
+            if (value < 0 || value > 2)
+                fail(VB200_ERR_INVALID, "state_rows must be 0 (every row), 1 (each sample's first row) or 2 (each sample's mean), got %lld",
+                     (long long)value);
+            h->state_sel.rows = static_cast<int>(value);
         } else fail(VB200_ERR_INVALID, "unknown option \"%s\"", key);
     });
 }
@@ -2819,6 +3012,10 @@ int vb200_model_dim(vb200_handle h, const char* key, int64_t* value) {
             const size_t n = attention_kinds(h->schedule).size();
             *value = n > 63 ? -1 : static_cast<int64_t>(h->attn_sel.mask & ((1ull << n) - 1));
         } else if (k == "attention_heads") *value = h->attn_sel.mean ? 1 : 0;
+        else if (k == "state_entries") {
+            const size_t n = state_kinds(h->schedule).size();
+            *value = n > 63 ? -1 : static_cast<int64_t>(h->state_sel.mask & ((1ull << n) - 1));
+        } else if (k == "state_rows") *value = h->state_sel.rows;
         else fail(VB200_ERR_INVALID, "unknown model dimension \"%s\"", key);
     });
 }

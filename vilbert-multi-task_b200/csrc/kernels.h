@@ -159,6 +159,14 @@ cudaError_t launch_gather_rows(const float* src, const int32_t* rows, int n, int
 // in a fixed order.  Labels are range-checked on the host.
 struct LossRows { const float* logits; int ld, N, n; const int32_t* labels; const float* targets; float* loss; };
 cudaError_t launch_pretrain_losses(const LossRows* g, float* reduced, cudaStream_t st);
+// Layer states (VB200_OUT_LAYER_STATES): one entry of an fp32 residual stream src [B x L rows, H] (dense: sample b's rows
+// [b L, b L + L), mask the additive key mask, 0 on real rows; packed: rows [offs[b], offs[b + 1]), m_rows the device row count) into
+// the float buffer whose address is *dst (0: no write; dst lives in the plan's staged meta).  reduce 0: every row (dense: B x L
+// rows, padding included; packed: *m_rows rows); 1: each sample's first row, [B, H]; 2: [B, H], the mean over each sample's real
+// rows, summed in increasing row order in fp32 and divided once by the count (NaN for a sample without one).  H a multiple of 4;
+// src and *dst 16-byte aligned (the host checks the caller's buffer).
+struct StateArgs { const float* src; const int* offs; const int* m_rows; const float* mask; const int64_t* dst; int B, L, H, reduce; };
+cudaError_t launch_layer_state(const StateArgs& a, int pdl, cudaStream_t st);
 // K8 (narrow heads): out[m, j] = dot(x[m, :K], W[j, :K]) + b[j] + (add ? add[m] : 0), j < n_out <= 4.
 cudaError_t launch_rowdot(const float* x, int ld_x, const float* W, const float* b, const float* add, float* out,
                           int ld_out, int M, int K, int n_out, int pdl, cudaStream_t st, const int* m_rows = nullptr);

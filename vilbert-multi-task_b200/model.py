@@ -116,23 +116,47 @@ def split_packed_attention(flat, layout, t_rows, v_rows, selection=None):
     return attention_list(*(selection or _full_selection(layout)), entries)
 
 
-def attention_mask_bits(entries) -> int:
-    """The "attention_entries" bitmask of an iterable of entry indices (``from_pretrained(attention_entries=...)``)."""
+def entry_mask_bits(entries, name: str = "attention_entries") -> int:
+    """The bitmask of option ``name`` ("attention_entries" / "state_entries") from an iterable of entry indices."""
     if isinstance(entries, (str, bytes)) or not hasattr(entries, "__iter__"):
-        raise TypeError(f"attention_entries must be an iterable of entry indices or None, got {entries!r}")
+        raise TypeError(f"{name} must be an iterable of entry indices or None, got {entries!r}")
     mask = 0
     for e in entries:
         if isinstance(e, bool) or not isinstance(e, int):
-            raise TypeError(f"attention_entries: entry index {e!r} is not an int")
+            raise TypeError(f"{name}: entry index {e!r} is not an int")
         if not 0 <= e < 63:
-            raise ValueError(f"attention_entries: entry index {e} outside [0, 63)")
+            raise ValueError(f"{name}: entry index {e} outside [0, 63)")
         mask |= 1 << e
     if mask == 0:
-        raise ValueError("attention_entries: select at least one entry (None selects every entry)")
+        raise ValueError(f"{name}: select at least one entry (None selects every entry)")
     return mask
 
 
+def attention_mask_bits(entries) -> int:
+    """The "attention_entries" bitmask of an iterable of entry indices (``from_pretrained(attention_entries=...)``)."""
+    return entry_mask_bits(entries, "attention_entries")
+
+
+def state_list(layout_entry, entries):
+    """The layer states as ``output_layer_states`` returns them: one position per entry of the full list (``state_selection``'s
+    ``layout_entry``), ``entries[i]`` for an entry at layout index i and None for an entry left out."""
+    return [entries[i] if i >= 0 else None for i in layout_entry]
+
+
+def split_packed_states(flat, layout, t_rows, v_rows, rows_mode):
+    """The entries of a packed layer-state buffer (VB200_OUT_LAYER_STATES): ``layout`` is ``[(kind, rows, width, float_offset)]`` of
+    ``state_layout_packed``, ``t_rows`` / ``v_rows`` the samples' T_b / V_b.  Under ``rows_mode`` 0 an entry is a list of B
+    ``[L_b, width]`` views, else a ``[B, width]`` view.  One ``torch.split`` of the entry's ``[rows, width]`` view along the rows:
+    views made one by one cost about four times the host time, which at batch 64 was most of a call with every entry."""
+    entries = []
+    for kind, rows, width, off in layout:
+        entry = flat[int(off):int(off) + rows * width].view(rows, width)
+        entries.append(list(torch.split(entry, t_rows if kind == 0 else v_rows)) if rows_mode == 0 else entry)
+    return entries
+
+
 _ATTENTION_HEADS = {"all": 0, "mean": 1}
+_STATE_ROWS = {"all": 0, "first": 1, "mean": 2}
 
 
 class VILBertForVLTasks(object):
@@ -143,7 +167,7 @@ class VILBertForVLTasks(object):
     def __init__(self, config: BertConfig, num_labels: int = 3129, state_dict=None, default_gpu: bool = True,
                  use_cuda_graph: bool = True, use_pdl: Optional[bool] = None, strict: bool = True, compute_dtype: str = "fp16",
                  fused_layernorm: bool = False, return_attention: bool = False, max_plans: int = 0, max_rows_per_sample: int = 256,
-                 attention_entries=None, attention_heads: str = "all"):
+                 attention_entries=None, attention_heads: str = "all", state_entries=None, state_rows: str = "all"):
         self.config = config
         self.num_labels = num_labels
         self._sd = _normalise_state_dict(state_dict) if state_dict is not None else None
@@ -168,10 +192,16 @@ class VILBertForVLTasks(object):
         # head axis kept as size 1).  Engine state, set when the engine is created and by set_option.
         if attention_heads not in _ATTENTION_HEADS:
             raise ValueError(f"attention_heads must be 'all' or 'mean', got {attention_heads!r}")
+        # Which layer states output_layer_states returns: state_entries (entry indices of the full list, see state_selection; None:
+        # every entry) and state_rows ("all" rows, each sample's "first" row, or each sample's "mean" over its real rows).
+        if state_rows not in _STATE_ROWS:
+            raise ValueError(f"state_rows must be 'all', 'first' or 'mean', got {state_rows!r}")
         self._opts = dict(use_cuda_graph=use_cuda_graph, use_pdl=use_pdl, strict=strict, compute_dtype=compute_dtype,
                           max_plans=int(max_plans), max_rows_per_sample=int(max_rows_per_sample),
                           attention_entries=None if attention_entries is None else attention_mask_bits(attention_entries),
-                          attention_heads=_ATTENTION_HEADS[attention_heads])
+                          attention_heads=_ATTENTION_HEADS[attention_heads],
+                          state_entries=None if state_entries is None else entry_mask_bits(state_entries, "state_entries"),
+                          state_rows=_STATE_ROWS[state_rows])
         # attn_data_list (element 9 of the tuple): the reference returns the 24 layers' attention probabilities when called with
         # output_all_attention_masks=True (worker.py:287-288) and never reads them; here they are computed only when this flag
         # is set as well (model.return_attention = True), otherwise element 9 is [].
@@ -266,7 +296,7 @@ class VILBertForVLTasks(object):
         L.check(rc, None)
         self._handle, self._device = h, device
         L.check(lib.vb200_set_option(h, b"max_rows_per_sample", self._opts["max_rows_per_sample"]), h)
-        for key in ("attention_entries", "attention_heads"):
+        for key in ("attention_entries", "attention_heads", "state_entries", "state_rows"):
             if self._opts[key]:
                 L.check(lib.vb200_set_option(h, key.encode(), self._opts[key]), h)
         for key in ("hidden_size", "v_hidden_size", "bi_hidden_size", "vocab_size", "v_target_size",
@@ -325,11 +355,11 @@ class VILBertForVLTasks(object):
 
     def set_option(self, key, value):
         """Run-time knobs of the engine (include/vilbert_b200.h, vb200_set_option): "max_plans", "timeline", "profile_grid_pct",
-        "gemm_kernel", "max_rows_per_sample", "attention_entries" (a bitmask) and "attention_heads" (0 / 1) -- the last three also
-        applied to the engine a later .cuda() creates."""
+        "gemm_kernel", "max_rows_per_sample", "attention_entries" (a bitmask), "attention_heads" (0 / 1), "state_entries" (a bitmask)
+        and "state_rows" (0 / 1 / 2) -- the last five also applied to the engine a later .cuda() creates."""
         self._engine_device()
         L.check(L.load().vb200_set_option(self._handle, key.encode(), int(value)), self._handle)
-        if key in ("max_rows_per_sample", "attention_entries", "attention_heads"):
+        if key in ("max_rows_per_sample", "attention_entries", "attention_heads", "state_entries", "state_rows"):
             self._opts[key] = int(value)
 
     @property
@@ -351,7 +381,7 @@ class VILBertForVLTasks(object):
         dims = (C.c_int32 * (4 * cap))()
         L.check(L.load().vb200_profile_ops(self._handle, batch, n_tokens, n_regions, select, iters, cap, C.byref(n), kinds, ms,
                                            fl, dims), self._handle)
-        names = {0: "gemm", 1: "self_attention", 2: "co_attention", 3: "rowdot", 4: "layernorm", 5: "attention_f32"}
+        names = {0: "gemm", 1: "self_attention", 2: "co_attention", 3: "rowdot", 4: "layernorm", 5: "attention_f32", 7: "layer_state"}
         return [dict(kind=names.get(kinds[i], "?"), ms=ms[i], flops=fl[i], dims=list(dims[4 * i:4 * i + 4]))
                 for i in range(min(n.value, cap))]
 
@@ -377,7 +407,8 @@ class VILBertForVLTasks(object):
     def forward(self, input_txt, input_imgs, image_loc, token_type_ids=None, attention_mask=None,
                 image_attention_mask=None, co_attention_mask=None, task_ids=None,
                 output_all_encoded_layers=False, output_all_attention_masks=False,
-                compute_pretraining_heads=False, select: Optional[int] = None, debug_taps: bool = False, slot: int = 0):
+                compute_pretraining_heads=False, select: Optional[int] = None, debug_taps: bool = False, slot: int = 0,
+                output_layer_states: bool = False):
         """Positional signature and 10-tuple of worker.py:286-289.
 
         ``vision_prediction`` / ``linguisic_prediction`` (the pre-training heads, elements 5 and 7, never read
@@ -387,7 +418,10 @@ class VILBertForVLTasks(object):
         [B, heads, V, T])`` tuple for a connection layer -- when ``output_all_attention_masks`` AND ``self.return_attention``
         are set, else ``[]``; with ``attention_entries`` / ``attention_heads`` an entry left out is None (each direction of a
         connection layer on its own) and a head-mean entry is ``[B, 1, Lq, Lk]``.  ``slot`` selects one of 16 independent
-        workspaces: calls on different slots may be in flight concurrently on different CUDA streams.
+        workspaces: calls on different slots may be in flight concurrently on different CUDA streams.  ``output_all_encoded_layers``
+        is accepted and ignored.  With ``output_layer_states`` the call returns ``(result, states)``: ``result`` as without it,
+        ``states`` the layer states of ``state_selection`` (None for an entry left out), ``[B, L, hidden]`` under ``state_rows="all"``
+        (padding rows included), else ``[B, hidden]``.
         """
         if self._handle is None and torch.is_tensor(input_txt) and input_txt.is_cuda:
             self.cuda(input_txt.device.index)
@@ -402,8 +436,11 @@ class VILBertForVLTasks(object):
                        vm.data_ptr(), None, tk.data_ptr())
         want_attn = bool(output_all_attention_masks and self.return_attention)
         outs, o, select = self._alloc_outputs(B, Tin, V, select, debug_taps, want_attn, device)
+        if output_layer_states:
+            select, states = self._dense_states(B, Tin, V, select, o, device)
         self._call("vb200_forward_slot", C.byref(inp), C.byref(o), select, slot)
-        return self._result(outs, B, Tin, V, debug_taps)
+        result = self._result(outs, B, Tin, V, debug_taps)
+        return (result, states()) if output_layer_states else result
 
     # ------------------------------------------------------------------ shared output plumbing
     def attention_layout(self, B, Tin, V):
@@ -446,6 +483,59 @@ class VILBertForVLTasks(object):
         L.check(lib.vb200_attention_layout_packed(*args, n.value, C.byref(n), dims, offs, C.byref(total)), self._handle)
         return [(dims[2 * i], dims[2 * i + 1], offs[i]) for i in range(n.value)], total.value
 
+    def state_selection(self):
+        """(kinds, layout_entry) of the full layer-state list in execution order (vb200_state_selection): each entry's kind (0 text,
+        1 image) and its index in the layouts of the current selection, -1 when it is not selected."""
+        self._engine_device()
+        lib = L.load()
+        n = C.c_int32()
+        L.check(lib.vb200_state_selection(self._handle, 0, C.byref(n), None, None), self._handle)
+        kinds, where = (C.c_int32 * n.value)(), (C.c_int32 * n.value)()
+        L.check(lib.vb200_state_selection(self._handle, n.value, C.byref(n), kinds, where), self._handle)
+        return list(kinds), list(where)
+
+    def _state_layout(self, fn, *args):
+        """[(kind, rows, width, float_offset)] of the selected layer states and the buffer size (vb200_state_layout[_packed])."""
+        self._engine_device()
+        lib = L.load()
+        n, total = C.c_int32(), C.c_int64()
+        L.check(getattr(lib, fn)(self._handle, *args, 0, C.byref(n), None, None, None, C.byref(total)), self._handle)
+        kinds, dims, offs = (C.c_int32 * n.value)(), (C.c_int32 * (2 * n.value))(), (C.c_int64 * n.value)()
+        L.check(getattr(lib, fn)(self._handle, *args, n.value, C.byref(n), kinds, dims, offs, C.byref(total)), self._handle)
+        return [(kinds[i], dims[2 * i], dims[2 * i + 1], offs[i]) for i in range(n.value)], total.value
+
+    def state_layout(self, B, Tin, V):
+        """[(kind, rows, width, float_offset)] of a dense forward's layer-state buffer + its size in floats."""
+        return self._state_layout("vb200_state_layout", B, Tin, V)
+
+    def state_layout_packed(self, n_tokens, n_regions):
+        """[(kind, rows, width, float_offset)] of a packed forward's layer-state buffer for these Tin_b / V_b + its size in floats."""
+        nt, nr = _host_ints(n_tokens), _host_ints(n_regions)
+        if len(nt) != len(nr):
+            raise ValueError("state_layout_packed: n_tokens and n_regions must have the same length")
+        return self._state_layout("vb200_state_layout_packed", len(nt), _int32s(nt), _int32s(nr))
+
+    def _dense_states(self, B, Tin, V, select, o, device):
+        """Flat layer-state buffer of a dense forward bound to ``o.layer_states``: (select, states)."""
+        layout, total = self.state_layout(B, Tin, V)
+        flat = torch.empty(total, dtype=torch.float32, device=device)
+        o.layer_states = flat.data_ptr()
+        every_row = self._opts["state_rows"] == 0
+        entries = [flat[off:off + rows * width].view((B, rows // B, width) if every_row else (B, width))
+                   for kind, rows, width, off in layout]
+        where = self.state_selection()[1]
+        return select | L.OUT_LAYER_STATES, lambda: state_list(where, entries)
+
+    def _packed_states(self, nt, nv, select, o, device):
+        """Flat layer-state buffer of a packed forward with Tin_b = nt, V_b = nv bound to ``o.layer_states``: (select, states)."""
+        layout, total = self.state_layout_packed(nt, nv)
+        flat = torch.empty(total, dtype=torch.float32, device=device)
+        o.layer_states = flat.data_ptr()
+        task = 1 if self._dims["task_specific_tokens"] else 0
+        entries = split_packed_states(flat, layout, [t + task for t in nt], nv, self._opts["state_rows"])
+        where = self.state_selection()[1]
+        return select | L.OUT_LAYER_STATES, lambda: state_list(where, entries)
+
     def _packed_attention(self, nt, nv, select, o, device):
         """Flat buffer of the packed attention maps for Tin_b = nt, V_b = nv, bound to ``o.attention_probs``: (select, flat, split)."""
         layout, total = self.attention_layout_packed(nt, nv)
@@ -474,7 +564,7 @@ class VILBertForVLTasks(object):
             _, total = self.attention_layout(B, Tin, V)
             outs["attention_probs"] = torch.empty(total, dtype=torch.float32, device=device)
             select |= L.OUT_ATTENTION
-        o = L.Outputs()
+        o = L.StateOutputs()
         for k, t in outs.items():
             setattr(o, k, t.data_ptr())
         return outs, o, select
@@ -497,10 +587,12 @@ class VILBertForVLTasks(object):
     # ------------------------------------------------------------------ detector output in, logits out (worker.py:388-458)
     @torch.no_grad()
     def forward_regions(self, question, segment_ids, input_mask, task_tokens, box_features, boxes, image_wh, num_boxes=None,
-                        select: Optional[int] = None, output_all_attention_masks=False, slot: int = 0, return_spatials=True):
+                        select: Optional[int] = None, output_all_attention_masks=False, slot: int = 0, return_spatials=True,
+                        output_layer_states: bool = False):
         """``custom_prediction``'s tensor construction fused into the forward: ``box_features [B, n, F]`` (what the detector
         returned, no global row), pixel ``boxes [B, n, 4]``, ``image_wh [B, 2]`` -> the 10-tuple (and the ``spatials``
-        tensor ``[B, n+1, 5]`` the reference would have built: the grounding decode reads it, worker.py:379)."""
+        tensor ``[B, n+1, 5]`` the reference would have built: the grounding decode reads it, worker.py:379).  With
+        ``output_layer_states``: ``(result, states)`` as ``forward`` returns them."""
         device = self._engine_device()
         q, seg, im = (_to_device(t, torch.int64, device) for t in (question, segment_ids, input_mask))
         B, Tin = q.shape
@@ -518,14 +610,17 @@ class VILBertForVLTasks(object):
                              wh.data_ptr(), nb.data_ptr() if nb is not None else None, sp.data_ptr() if sp is not None else None)
         want_attn = bool(output_all_attention_masks and self.return_attention)
         outs, o, select = self._alloc_outputs(B, Tin, n + 1, select, False, want_attn, device)
+        if output_layer_states:
+            select, states = self._dense_states(B, Tin, n + 1, select, o, device)
         self._call("vb200_forward_regions", C.byref(inp), C.byref(o), select, slot)
-        return self._result(outs, B, Tin, n + 1, False), sp
+        result = self._result(outs, B, Tin, n + 1, False), sp
+        return (result, states()) if output_layer_states else result
 
     # ------------------------------------------------------------------ packed variable-length batches
     @torch.no_grad()
     def forward_packed(self, question, features, spatials, segment_ids, task_tokens, n_tokens, n_regions,
                        select: int = L.OUT_TASK_HEADS, slot: int = 0, debug_taps: bool = False, max_tokens: int = 0,
-                       max_regions: int = 0, output_all_attention_masks: bool = False):
+                       max_regions: int = 0, output_all_attention_masks: bool = False, output_layer_states: bool = False):
         """One forward of B samples with their own text lengths and region counts, stored back to back without padding:
         ``question`` / ``segment_ids`` ``[sum Tin_i]``, ``features`` ``[sum V_i, F]``, ``spatials`` ``[sum V_i, 5]``,
         ``task_tokens`` ``[B, 1]``; ``n_tokens`` / ``n_regions`` (lists or CPU int tensors) give Tin_i and V_i.  Every row is real
@@ -534,7 +629,9 @@ class VILBertForVLTasks(object):
         ``output_all_attention_masks`` AND ``self.return_attention`` the 24 layers' attention probabilities at each sample's own
         lengths (``split_packed_attention``: per layer a list of B ``[heads, L_i, L_i]`` tensors, a connection layer a tuple of two
         such lists), views of one flat buffer.  ``max_tokens`` / ``max_regions`` (0: this call's maxima) are the plan's capacities:
-        calls with the same batch size and capacities share one plan and CUDA graph whatever their lengths."""
+        calls with the same batch size and capacities share one plan and CUDA graph whatever their lengths.  With
+        ``output_layer_states``: ``(result, states)``, each selected entry a list of B ``[L_i, hidden]`` views of one flat buffer
+        under ``state_rows="all"``, else ``[B, hidden]``; None for an entry left out."""
         device = self._engine_device()
         nt, nr = _host_ints(n_tokens), _host_ints(n_regions)
         B = len(nt)
@@ -554,16 +651,20 @@ class VILBertForVLTasks(object):
         want_attn = bool(output_all_attention_masks and self.return_attention)
         if want_attn:
             select, maps = self._packed_attention(nt, nr, select, o, device)
+        if output_layer_states:
+            select, states = self._packed_states(nt, nr, select, o, device)
         inp = L.PackedInputs(B, int(max_tokens), int(max_regions), _int32s(nt), _int32s(nr), q.data_ptr(), seg.data_ptr(), f.data_ptr(),
                              s.data_ptr(), tk.data_ptr())
         self._call("vb200_forward_packed", C.byref(inp), C.byref(o), select, slot)
         result = self._result(outs, B, 0, 0, debug_taps)
-        return self._with_attention(result, maps(), debug_taps) if want_attn else result
+        result = self._with_attention(result, maps(), debug_taps) if want_attn else result
+        return (result, states()) if output_layer_states else result
 
     @torch.no_grad()
     def forward_regions_packed(self, question, segment_ids, task_tokens, box_features, boxes, image_wh, n_tokens, n_boxes,
                                select: int = L.OUT_TASK_HEADS, slot: int = 0, max_tokens: int = 0, max_boxes: int = 0,
-                               debug_taps: bool = False, return_spatials: bool = True, output_all_attention_masks: bool = False):
+                               debug_taps: bool = False, return_spatials: bool = True, output_all_attention_masks: bool = False,
+                               output_layer_states: bool = False):
         """``forward_regions`` with every image at its own box count and every text at its own length, stored back to back without
         padding: ``question`` / ``segment_ids`` ``[sum Tin_i]`` (text already repeated per image), ``task_tokens`` ``[B, 1]``,
         ``box_features`` ``[sum n_boxes_i, F]`` and pixel ``boxes`` ``[sum n_boxes_i, 4]`` as the detector returned them,
@@ -574,7 +675,7 @@ class VILBertForVLTasks(object):
         bit-identical to ``forward_regions`` of that image alone.  ``max_tokens`` / ``max_boxes`` (0: this call's maxima) are the
         plan's capacities; the plan is the one ``forward_packed`` uses at ``max_regions = max_boxes + 1``.  Element 9 follows
         ``forward_packed``: the attention maps at each image's own T_i / V_i with ``output_all_attention_masks`` and
-        ``self.return_attention``, else ``[]``."""
+        ``self.return_attention``, else ``[]``.  ``output_layer_states`` returns ``(result, states)`` as ``forward_packed`` does."""
         device = self._engine_device()
         nt, nb = _host_ints(n_tokens), _host_ints(n_boxes)
         B = len(nt)
@@ -598,11 +699,14 @@ class VILBertForVLTasks(object):
         want_attn = bool(output_all_attention_masks and self.return_attention)
         if want_attn:
             select, maps = self._packed_attention(nt, [n + 1 for n in nb], select, o, device)
+        if output_layer_states:
+            select, states = self._packed_states(nt, [n + 1 for n in nb], select, o, device)
         inp = L.PackedRegionInputs(B, int(max_tokens), int(max_boxes), _int32s(nt), _int32s(nb), q.data_ptr(), seg.data_ptr(),
                                    tk.data_ptr(), bf.data_ptr(), bx.data_ptr(), wh.data_ptr(), sp.data_ptr() if sp is not None else None)
         self._call("vb200_forward_regions_packed", C.byref(inp), C.byref(o), select, slot)
         result = self._result(outs, B, 0, 0, debug_taps)
-        return (self._with_attention(result, maps(), debug_taps) if want_attn else result), sp
+        result = (self._with_attention(result, maps(), debug_taps) if want_attn else result), sp
+        return (result, states()) if output_layer_states else result
 
     def _alloc_packed_outputs(self, B, rows_t, rows_v, select, debug_taps, device):
         """Outputs of a packed call: per-sample outputs [B, ...], per-row outputs and taps [rows_t or rows_v, ...]."""
@@ -615,7 +719,7 @@ class VILBertForVLTasks(object):
             outs["sequence_output_t"] = torch.empty(rows_t, d["hidden_size"], dtype=torch.float32, device=device)
             outs["sequence_output_v"] = torch.empty(rows_v, d["v_hidden_size"], dtype=torch.float32, device=device)
             outs["pooled_output"] = torch.empty(B, d["bi_hidden_size"], dtype=torch.float32, device=device)
-        o = L.Outputs()
+        o = L.StateOutputs()
         for k, t in outs.items():
             setattr(o, k, t.data_ptr())
         return outs, o
