@@ -241,10 +241,11 @@ def attention_fp64(q, k, v, mask_add, heads):
 
 
 def attention_emulated(q, k, v, mask_add, heads, f16: bool):
-    """The tensor-core attention's rounding points on the CPU: fp32 scores and softmax numerators p = exp2(s - max) (log2 domain,
-    as attention.cu), the denominator summed from the fp32 p, P rounded to the 16-bit format before P V, the context rounded to the
-    16-bit format.  One key block (the kernel's online softmax over 64-key blocks only rescales by exact powers of the running
-    max, which this ignores).  Returns the 16-bit context as fp64 [B, Lq, H]."""
+    """The tensor-core attention's rounding points on the CPU: fp32 scores s = fmaf(q.k, kLog2e / sqrtf(d), mask * kLog2e) and
+    softmax numerators p = exp2(s - max) (log2 domain, as attention.cu), the denominator summed from the fp32 p, P rounded to the
+    16-bit format before P V, the context rounded to the 16-bit format.  One key block, as attend_tile_short: past 64 keys the
+    kernel's online softmax rounds P against the running max of each block (oracle/step_ref.py attention_blockwise restates
+    that).  Returns the 16-bit context as fp64 [B, Lq, H]."""
     B, Lq, H = q.shape
     Lk = k.shape[1]
     d = H // heads
@@ -252,8 +253,10 @@ def attention_emulated(q, k, v, mask_add, heads, f16: bool):
     qh = q.float().reshape(B, Lq, heads, d).permute(0, 2, 1, 3)
     kh = k.float().reshape(B, Lk, heads, d).permute(0, 2, 1, 3)
     vh = v.float().reshape(B, Lk, heads, d).permute(0, 2, 1, 3)
-    log2e = 1.4426950408889634
-    s = (qh.double() @ kh.double().transpose(-1, -2)).float() * (log2e / math.sqrt(d)) + (mask_add.float() * log2e)[:, None, None, :]
+    log2e = torch.tensor(1.4426950408889634, dtype=torch.float32)
+    scale = log2e / torch.sqrt(torch.tensor(float(d), dtype=torch.float32))
+    raw = (qh.double() @ kh.double().transpose(-1, -2)).float()
+    s = (raw.double() * scale.double() + (mask_add.float() * log2e).double()[:, None, None, :]).float()
     p = torch.exp2(s - s.amax(-1, keepdim=True))
     l = p.sum(-1, keepdim=True)
     o = (p.to(dt).double() @ vh.double()).float() * (1.0 / l)
