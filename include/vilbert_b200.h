@@ -266,6 +266,25 @@ int vb200_attention_layout(vb200_handle h, int32_t batch, int32_t n_tokens, int3
  * layouts of vb200_attention_layout / vb200_attention_layout_packed, or -1 when "attention_entries" leaves it out.  Arrays (up to
  * max_entries) may be NULL to query the count only. */
 int vb200_attention_selection(vb200_handle h, int32_t max_entries, int32_t* n_entries, int32_t* kinds, int32_t* layout_entry);
+/* Attention relevance: the residual-weighted attention rollout (Abnar & Zuidema 2020) of one forward's maps through both streams,
+ * for the two rows the answer heads read, the text CLS row (t_pooler) and the image global row (v_pooler).  For a sample with T text
+ * rows (task token included) and V image rows, a step -- one text layer, one image layer, or both directions of one connection
+ * layer, which read the same pre-layer streams -- maps each row i it writes to 0.5 (e_i + Abar[i, :]), Abar its map averaged over
+ * heads (fp32, heads summed left to right, then divided once: the engine's head mean, so maps kept with every head and maps written
+ * as the mean give the same bits) in its block of the T + V positions, and leaves the other rows e_i.  The output per sample is
+ * rows 0 and T of W_n ... W_1, each T + V floats (text columns first) summing to 1; padded positions of a dense forward are 0.
+ * Evaluated from the last step to the first on the two row vectors, each column's sum over the step's query rows in increasing order
+ * with separate fp32 products and adds (relevance.cu states the order).
+ * attention_probs: DEVICE, the maps one forward wrote under the engine's CURRENT map selection, which must hold every entry (heads
+ * kept or averaged).  packed = 0: the layout of vb200_attention_layout for n_tokens = &Tin, n_regions = &V (one HOST value each);
+ * relevance is DEVICE [batch, 2, T + V].  packed = 1: the layout of vb200_attention_layout_packed for the HOST arrays n_tokens /
+ * n_regions [batch] (V_b = n_boxes_b + 1 for region forwards), validated as it validates them; sample b's [2, T_b + V_b] block
+ * starts at float 2 sum_{b' < b} (T_b' + V_b').  VB200_ERR_INVALID, before anything is enqueued and with relevance untouched, for a
+ * NULL pointer, batch < 1, bad lengths, packed not 0 / 1, and a selection that leaves out an entry (the message names the first).
+ * Asynchronous on cuda_stream; builds no plan; the descriptors reach the device through engine-owned pinned staging in stream order,
+ * so back-to-back calls need no synchronisation.  One CTA per sample. */
+int vb200_attention_relevance(vb200_handle h, const float* attention_probs, int32_t batch, const int32_t* n_tokens,
+                              const int32_t* n_regions, int32_t packed, float* relevance, void* cuda_stream);
 
 /* ---- Layer states (VB200_OUT_LAYER_STATES).  The full list holds the fp32 residual-stream state after every step that writes a
  * stream, in execution order: the text embedding, the image embedding, then per schedule step one text entry (text layer), one

@@ -159,7 +159,7 @@ class Options(C.Structure):
 # every symbol include/vilbert_b200.h declares (tests/test_cabi.py checks the list against the header)
 EXPORTS = ["vb200_abi_version", "vb200_create", "vb200_destroy", "vb200_last_error", "vb200_forward", "vb200_forward_slot",
            "vb200_forward_host", "vb200_forward_host_slot", "vb200_plan_info", "vb200_model_dim", "vb200_set_option", "vb200_timeline", "vb200_profile_ops",
-           "vb200_attention_layout", "vb200_attention_layout_packed", "vb200_attention_selection", "vb200_state_layout", "vb200_state_layout_packed", "vb200_state_selection",
+           "vb200_attention_layout", "vb200_attention_layout_packed", "vb200_attention_selection", "vb200_attention_relevance", "vb200_state_layout", "vb200_state_layout_packed", "vb200_state_selection",
            "vb200_forward_regions", "vb200_forward_packed", "vb200_forward_regions_packed", "vb200_encode_text", "vb200_encode_image", "vb200_forward_cached",
            "vb200_encode_text_packed", "vb200_encode_image_packed", "vb200_encode_regions_packed", "vb200_forward_cached_packed", "vb200_linear", "vb200_linear_rows", "vb200_linear_split", "vb200_layernorm", "vb200_layernorm_split", "vb200_attention_f32",
            "vb200_self_attention", "vb200_co_attention", "vb200_self_attention_packed", "vb200_co_attention_packed",
@@ -207,6 +207,7 @@ def load():
     lib.vb200_attention_layout.argtypes = [vp, i32, i32, i32, i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(i64), C.POINTER(i64)]
     lib.vb200_attention_layout_packed.argtypes = [vp, i32, vp, vp, i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(i64), C.POINTER(i64)]
     lib.vb200_attention_selection.argtypes = [vp, i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)]
+    lib.vb200_attention_relevance.argtypes = [vp, vp, i32, vp, vp, i32, vp, vp]
     lib.vb200_state_layout.argtypes = [vp, i32, i32, i32, i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), C.POINTER(i64),
                                        C.POINTER(i64)]
     lib.vb200_state_layout_packed.argtypes = [vp, i32, vp, vp, i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), C.POINTER(i64),

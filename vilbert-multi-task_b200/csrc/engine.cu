@@ -819,6 +819,12 @@ struct vb200_engine {
     cudaEvent_t dec_copied = nullptr;
     vb200_answer* ans_d = nullptr;
     size_t ans_cap = 0;
+    // attention relevance (vb200_attention_relevance): each call's entry and sample descriptors go to rel_d through the pinned rel_h,
+    // rel_copied marks when the last copy out of rel_h has been made.  Both grow on demand.
+    char* rel_h = nullptr;
+    char* rel_d = nullptr;
+    size_t rel_cap = 0;
+    cudaEvent_t rel_copied = nullptr;
     // region selection (vb200_select_regions): descriptors staged in the pinned sel_h (sel_copied: the last copy out of it), the
     // workspace sel_ws holds the device descriptors, row stats, boxes, bitmasks, max_conf and keep lists; sel_done marks the end of
     // the last call's kernels.  Both buffers grow on demand.
@@ -848,6 +854,9 @@ struct vb200_engine {
         if (dec_h) cudaFreeHost(dec_h);
         if (dec_d) cudaFree(dec_d);
         if (ans_d) cudaFree(ans_d);
+        if (rel_copied) { cudaEventSynchronize(rel_copied); cudaEventDestroy(rel_copied); }
+        if (rel_h) cudaFreeHost(rel_h);
+        if (rel_d) cudaFree(rel_d);
         plans.clear();
         if (side_stream) cudaStreamDestroy(side_stream);
         if (ev_fork) cudaEventDestroy(ev_fork);
@@ -2029,6 +2038,58 @@ struct vb200_engine {
         }
         return ans_d;
     }
+    // ---- attention relevance: lengths and the map selection are checked, and the descriptors built, before anything is enqueued
+    void attention_relevance(const float* maps, int batch, const int32_t* n_tokens, const int32_t* n_regions, int packed,
+                             float* relevance, cudaStream_t st) {
+        const char* api = "vb200_attention_relevance";
+        if (maps == nullptr || relevance == nullptr) fail(VB200_ERR_INVALID, "%s: attention_probs / relevance is NULL", api);
+        if (n_tokens == nullptr || n_regions == nullptr) fail(VB200_ERR_INVALID, "%s: n_tokens / n_regions is NULL", api);
+        if (packed != 0 && packed != 1) fail(VB200_ERR_INVALID, "%s: packed must be 0 or 1 (got %d)", api, packed);
+        if (batch < 1) fail(VB200_ERR_INVALID, "%s: batch must be positive", api);
+        const std::vector<int> kinds = attention_kinds(schedule);
+        for (int e = 0; e < static_cast<int>(kinds.size()); ++e)
+            if (!attn_sel.has(e))
+                fail(VB200_ERR_INVALID, "%s: attention entry %d is not selected (\"attention_entries\"); the rollout needs every entry", api, e);
+        // a dense batch is a packed one whose samples all have the padded lengths: the same validation, and the same layout
+        // (entry e's offset sum_{e' < e} B heads Lq Lk, sample b's block at heads * b Lq Lk)
+        std::vector<int32_t> tin, nv;
+        if (!packed) { tin.assign(batch, *n_tokens); nv.assign(batch, *n_regions); }
+        const PackedBatch b = pack_batch(api, cfg, schedule, {"sample", batch, packed ? n_tokens : tin.data(), 0,
+                                                              packed ? n_regions : nv.data(), 0}, nullptr, max_rows);
+        const PackedAttnLayout l = packed_attn_layout(cfg, schedule, attn_sel, batch, b.offs_t(), b.offs_v());
+        const size_t n = l.offset.size(), n1 = static_cast<size_t>(batch) + 1;
+        std::vector<vb::RelevanceEntry> ents(n);
+        for (size_t e = 0; e < n; ++e) ents[e] = {l.offset[e], l.kind[e], l.heads[e]};
+        std::vector<vb::RelevanceSample> smp(batch);
+        int64_t out = 0;
+        int max_cols = 0;
+        for (int i = 0; i < batch; ++i) {
+            const int T = b.offs_t()[i + 1] - b.offs_t()[i], V = b.offs_v()[i + 1] - b.offs_v()[i];
+            smp[i] = {{l.prefix[i], l.prefix[n1 + i], l.prefix[2 * n1 + i]}, out, T, V};
+            out += 2 * static_cast<int64_t>(T + V);
+            max_cols = std::max(max_cols, T + V);
+        }
+        // stage entries then samples (both 8-byte aligned) through the pinned rel_h, in stream order
+        const size_t eb = n * sizeof(vb::RelevanceEntry), bytes = eb + smp.size() * sizeof(vb::RelevanceSample);
+        if (rel_copied == nullptr) CUDA_CHECK(cudaEventCreateWithFlags(&rel_copied, cudaEventDisableTiming));
+        CUDA_CHECK(cudaEventSynchronize(rel_copied));                // the previous call's copy has left the staging buffer
+        if (bytes > rel_cap) {
+            const size_t cap = std::max<size_t>({bytes, 2 * rel_cap, 4096});
+            if (rel_h) CUDA_CHECK(cudaFreeHost(rel_h));
+            rel_h = nullptr;
+            CUDA_CHECK(cudaMallocHost(&rel_h, cap));
+            if (rel_d) CUDA_CHECK(cudaFreeAsync(rel_d, st));          // after the kernels already enqueued on st have read it
+            rel_d = nullptr;
+            CUDA_CHECK(cudaMallocAsync(&rel_d, cap, st));
+            rel_cap = cap;
+        }
+        memcpy(rel_h, ents.data(), eb);
+        memcpy(rel_h + eb, smp.data(), bytes - eb);
+        CUDA_CHECK(cudaMemcpyAsync(rel_d, rel_h, bytes, cudaMemcpyHostToDevice, st));
+        CUDA_CHECK(cudaEventRecord(rel_copied, st));
+        CUDA_CHECK(vb::launch_attention_relevance(maps, reinterpret_cast<const vb::RelevanceEntry*>(rel_d), static_cast<int>(n),
+                                                  reinterpret_cast<const vb::RelevanceSample*>(rel_d + eb), batch, max_cols, relevance, st));
+    }
     // ---- region selection: every descriptor is checked before anything is enqueued
     void select_regions(const vb200_detections* imgs, int n, const vb200_select_params* p, const vb200_selected* out, cudaStream_t st) {
         const char* api = "vb200_select_regions";
@@ -2697,6 +2758,15 @@ int vb200_decode_answers_host(vb200_handle h, const vb200_decode_msg* msgs, int3
         h->decode_answers(d, dev, st);
         CUDA_CHECK(cudaMemcpyAsync(answers, dev, d.size() * sizeof(vb200_answer), cudaMemcpyDeviceToHost, st));
         CUDA_CHECK(cudaStreamSynchronize(st));
+    });
+}
+
+int vb200_attention_relevance(vb200_handle h, const float* attention_probs, int32_t batch, const int32_t* n_tokens,
+                              const int32_t* n_regions, int32_t packed, float* relevance, void* cuda_stream) {
+    if (h == nullptr) return VB200_ERR_INVALID;
+    return guard(h, [&] {
+        CUDA_CHECK(cudaSetDevice(h->opt.device));
+        h->attention_relevance(attention_probs, batch, n_tokens, n_regions, packed, relevance, static_cast<cudaStream_t>(cuda_stream));
     });
 }
 

@@ -180,6 +180,14 @@ struct DecodeDesc {
     int len, top_n;
 };
 cudaError_t launch_answer_decode(const DecodeDesc* descs, int n, vb200_answer* answers, cudaStream_t st);
+// Attention relevance (relevance.cu, vb200_attention_relevance): per sample b (one CTA) the rollout rows of the text CLS row and the
+// image global row, [2, T_b + V_b] at relevance + out.  Entry e of the maps starts at float `offset` and holds sample b's
+// [heads, Lq_b, Lk_b] block at heads * prefix[k] (k 0 text layers, 1 image layers, 2 both directions of a connection layer); kinds
+// follow the full list's execution order, every kind 3 right after a kind 2.  max_cols: the largest T_b + V_b (<= 2048).
+struct RelevanceEntry { int64_t offset; int32_t kind, heads; };
+struct RelevanceSample { int64_t prefix[3]; int64_t out; int32_t T, V; };
+cudaError_t launch_attention_relevance(const float* maps, const RelevanceEntry* entries, int n_entries, const RelevanceSample* samples,
+                                       int B, int max_cols, float* relevance, cudaStream_t st);
 // Detector-region selection (regions_select.cu, vb200_select_regions).  Image i's n proposals are workspace rows [row0, row0 + n)
 // of stats / dbox / max_conf and words [mask0, mask0 + n * nw) of the bitmask; its k = min(K, n) selected rows go to output rows
 // [dst_row, dst_row + k).  npad: n rounded up to a power of two >= 32.  Descriptors are validated on the host.

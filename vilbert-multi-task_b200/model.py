@@ -155,6 +155,49 @@ def split_packed_states(flat, layout, t_rows, v_rows, rows_mode):
     return entries
 
 
+def relevance_entries(attn, kinds):
+    """The maps of element 9 (``attention_list`` order) as ``attention_relevance`` reads them: (entries, packed, t_rows, v_rows).
+    ``kinds`` is the full entry list's kinds (``attention_selection``); ``entries`` one tensor ``[B, heads, Lq, Lk]`` (dense) or one
+    list of B ``[heads, Lq_b, Lk_b]`` views (packed) per entry in execution order; ``t_rows`` / ``v_rows`` each sample's T_b / V_b
+    (dense: B copies of T / V), read from the shapes.  ValueError for an entry left out by the selection (None)."""
+    entries = []
+    for pos in attn:
+        entries.extend(pos if isinstance(pos, tuple) else (pos,))
+    if len(entries) != len(kinds):
+        raise ValueError(f"attention_relevance: {len(entries)} attention entries, the model has {len(kinds)}")
+    for e, x in enumerate(entries):
+        if x is None:
+            raise ValueError(f"attention_relevance: attention entry {e} is None (left out by attention_entries); "
+                             "the rollout needs every entry")
+    packed = not torch.is_tensor(entries[0])
+    rows = {}                                             # stream (0 text, 1 image) -> per-sample rows
+    for kind, x in zip(kinds, entries):
+        lq, lk = {0: (0, 0), 1: (1, 1), 2: (0, 1), 3: (1, 0)}[kind]
+        for stream, axis in ((lq, -2), (lk, -1)):
+            if stream not in rows:
+                rows[stream] = [int(m.shape[axis]) for m in x] if packed else [int(x.shape[axis])] * int(x.shape[0])
+        if len(rows) == 2:
+            break
+    return entries, packed, rows[0], rows[1]
+
+
+def maps_pointer(entries, packed, layout):
+    """Device address of the flat map buffer behind ``entries`` (``relevance_entries``), checked against ``layout``: per entry
+    (heads, float offset) of the buffer the engine's current selection describes.  Entry e (packed: its sample 0) must be a
+    contiguous fp32 view at that offset of one buffer with that head count; ValueError otherwise."""
+    if len(layout) != len(entries):
+        raise ValueError(f"attention_relevance: {len(entries)} entries, the current map selection lays out {len(layout)}")
+    first = [x[0] if packed else x for x in entries]
+    base = first[0].data_ptr() - 4 * int(layout[0][1])
+    for e, (x, (heads, off)) in enumerate(zip(first, layout)):
+        if x.dtype != torch.float32 or not x.is_contiguous() or x.device != first[0].device:
+            raise ValueError(f"attention_relevance: attention entry {e} is not a contiguous fp32 map on {first[0].device}")
+        if x.data_ptr() != base + 4 * int(off) or int(x.shape[-3]) != heads:
+            raise ValueError(f"attention_relevance: attention entry {e} is not where the current map selection puts it "
+                             "(the maps must be element 9 of one forward under this selection)")
+    return base
+
+
 _ATTENTION_HEADS = {"all": 0, "mean": 1}
 _STATE_ROWS = {"all": 0, "first": 1, "mean": 2}
 
@@ -482,6 +525,35 @@ class VILBertForVLTasks(object):
         offs = (C.c_int64 * n.value)()
         L.check(lib.vb200_attention_layout_packed(*args, n.value, C.byref(n), dims, offs, C.byref(total)), self._handle)
         return [(dims[2 * i], dims[2 * i + 1], offs[i]) for i in range(n.value)], total.value
+
+    def attention_relevance(self, attn):
+        """Relevance of every text and image position to the two rows the answer heads read, from element 9 of ``forward`` /
+        ``forward_regions`` (dense) or ``forward_packed`` / ``forward_regions_packed`` (packed), on the device
+        (vb200_attention_relevance): the residual-weighted attention rollout through both streams, row 0 the text CLS row and row 1
+        the image global row, each ``T + V`` floats (text columns first) that sum to 1.  Returns a device tensor ``[B, 2, T + V]``
+        (dense; padded positions are 0) or a list of B ``[2, T_b + V_b]`` views of one buffer (packed).  Every entry must be in the
+        maps (ValueError for a None entry); heads may be kept or averaged.  Asynchronous on the current stream."""
+        kinds, _ = self.attention_selection()
+        entries, packed, t_rows, v_rows = relevance_entries(attn, kinds)
+        task = 1 if self._dims["task_specific_tokens"] else 0
+        tin = [t - task for t in t_rows]
+        B = len(t_rows)
+        if packed:
+            layout = [(h, off) for h, kind, off in self.attention_layout_packed(tin, v_rows)[0]]
+            nt, nv = _int32s(tin), _int32s(v_rows)
+        else:
+            layout = [(h, off) for h, lq, lk, kind, off in self.attention_layout(B, tin[0], v_rows[0])[0]]
+            nt, nv = _int32s(tin[:1]), _int32s(v_rows[:1])
+        ptr = maps_pointer(entries, packed, layout)
+        device = self._engine_device()
+        if (entries[0][0] if packed else entries[0]).device != device:
+            raise ValueError(f"attention_relevance: the maps are not on the engine's device {device}")
+        sizes = [2 * (t + v) for t, v in zip(t_rows, v_rows)]
+        out = torch.empty(sum(sizes), dtype=torch.float32, device=device)
+        self._call("vb200_attention_relevance", C.c_void_p(ptr), B, nt, nv, int(packed), out.data_ptr())
+        if packed:
+            return [p.view(2, s // 2) for p, s in zip(torch.split(out, sizes), sizes)]
+        return out.view(B, 2, t_rows[0] + v_rows[0])
 
     def state_selection(self):
         """(kinds, layout_entry) of the full layer-state list in execution order (vb200_state_selection): each entry's kind (0 text,
