@@ -25,6 +25,16 @@ BOUNDS = {
     "losses": 2.5e-7,     # [6.1e-8] the three pre-training losses
 }
 
+# The same families at checkpoint-like weights (oracle/trained_like.py, tests/test_gpu_trained_like.py), where BOUNDS do not hold on the
+# 268 M model: sharp heads over 24 layers amplify fp32 rounding, and the fp32 oracle itself sits at 1.7e-4 (logits), 2.8e-4 (final
+# states) and 5.9e-2 (attention, T11) from fp64 on that case, further than the mode.  ~4x the worst value measured on an H100 80GB
+# HBM3 at a 700 W power limit over tests/test_gpu_trained_like.py's fp32x cases; in brackets the value, its case and its output.
+BOUNDS_TRAINED = {
+    "logits": 2e-4,       # [5.1e-5 full_B2 (2, 30, 101), linguisic_prediction]
+    "states": 3.7e-4,     # [9.2e-5 full_B2, sequence_output_t]
+    "attention": 1.1e-1,  # [2.8e-2 full_B2, T11]
+}
+
 OUTPUT_NAMES = ("vil_prediction", "vil_prediction_gqa", "vil_logit", "vil_binary_prediction", "vil_tri_prediction",
                 "vision_prediction", "vision_logit", "linguisic_prediction", "linguisic_logit")
 

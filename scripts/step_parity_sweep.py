@@ -5,7 +5,10 @@ at B = 2 and at the bench shape B = 64) in fp16 and bf16 for --seeds seeds each 
 --heavy-seeds), and prints one JSON line per mode and family with the worst value, its case, step and row, the worst value per step,
 and the card's name, power limit and maximum SM clock read in the same run.
 
-    python scripts/step_parity_sweep.py [--seeds 20] [--heavy-seeds 3] [--out FILE]   (--out: append the lines to FILE too)
+    python scripts/step_parity_sweep.py [--seeds 20] [--heavy-seeds 3] [--weights synthetic|trained] [--out FILE]
+
+--out appends the lines to FILE too.  --weights trained runs every case on oracle/trained_like.py's checkpoint-like weights (seed
+trained_like.SEED), the measurement behind step_ref.STEP_BOUNDS_TRAINED; the default is the seeded synthetic checkpoint of STEP_BOUNDS.
 """
 import argparse
 import importlib.util
@@ -43,6 +46,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--seeds", type=int, default=20)
     ap.add_argument("--heavy-seeds", type=int, default=3, help="seeds of the long-sequence and 268 M model cases")
+    ap.add_argument("--weights", choices=("synthetic", "trained"), default="synthetic")
     ap.add_argument("--out", default=None, help="also append the JSON lines to this file")
     args = ap.parse_args()
 
@@ -69,6 +73,9 @@ def main():
     tiny_oracle = R.build(R.tiny_config(), seed=7, num_labels=200)
     long_oracle = T.long_oracle()
     full_oracle = R.build(seed=42)
+    if args.weights == "trained":
+        from oracle import trained_like as TL
+        tiny_oracle, long_oracle, full_oracle = (TL.trained_like(o, TL.SEED) for o in (tiny_oracle, long_oracle, full_oracle))
     for mode in T.MODES:
         model = T.engine(tiny_oracle, mode)
         for s in range(args.seeds):
@@ -92,7 +99,7 @@ def main():
 
     card = _card()
     lines = [json.dumps({"mode": mode, "family": fam, "worst": w["max"][0], "case": w["max"][1], "step": w["max"][2],
-                         "where": w["max"][3], "seeds": args.seeds, "heavy_seeds": args.heavy_seeds, "per_step": w["steps"],
+                         "where": w["max"][3], "weights": args.weights, "seeds": args.seeds, "heavy_seeds": args.heavy_seeds, "per_step": w["steps"],
                          "card": card}) for (mode, fam), w in sorted(worst.items())]
     for line in lines:
         print(line, flush=True)

@@ -187,10 +187,11 @@ __device__ __forceinline__ uint32_t pack16x2_rt(float lo, float hi, int f16) {
 }
 __device__ __forceinline__ uint16_t cvt16_rt(float v, int f16) { return static_cast<uint16_t>(pack16x2_rt(v, 0.0f, f16) & 0xffffu); }
 
-// ---- fp32-parity mode ("fp32x"): a value x travels as TWO fp16 numbers hi = fp16(x), lo = fp16(x - hi) (22 significand bits;
-// lo may be an fp16 subnormal, which the tensor cores handle).  16-bit operand buffers then hold, per 64 logical columns,
-// 192 physical ones: hi | lo | hi for activations, hi | hi | lo for weights, so that an ordinary K' = 3K GEMM computes
-// hi.hi + lo.hi + hi.lo (the dropped lo.lo term is 2^-22 relative) with fp32 accumulation.
+// ---- fp32-parity mode ("fp32x"): a value x travels as TWO fp16 numbers hi = fp16(x), lo = fp16(x - hi).  hi + lo is x to about
+// |x| 2^-22 relative, with an absolute floor of 2^-25 (half the fp16 subnormal step, where lo is a subnormal, which the tensor cores
+// handle): 22 significand bits for |x| >= 2^-3, 25 + log2|x| below that, about 19.4 for a weight of 0.02.  16-bit operand
+// buffers then hold, per 64 logical columns, 192 physical ones: hi | lo | hi for activations, hi | hi | lo for weights, so that an
+// ordinary K' = 3K GEMM computes hi.hi + lo.hi + hi.lo (the dropped lo.lo term is 2^-22 relative) with fp32 accumulation.
 __host__ __device__ __forceinline__ int split_col(int c) { return (c >> 6) * 192 + (c & 63); }   // column of the first hi
 __device__ __forceinline__ float split_hi(float x) {
     return __half2float(__float2half_rn(fminf(fmaxf(x, -65504.0f), 65504.0f)));
