@@ -548,9 +548,9 @@ int vb200_decode_answers_host(vb200_handle h, const vb200_decode_msg* msgs /* HO
  * required pointer, a features or box_features pointer not 16-byte aligned, and destination ranges that overlap or fall outside
  * [0, out_rows); nothing is enqueued then.
  * Asynchronous on cuda_stream.  The descriptors reach the device through a pinned staging buffer, and the workspace (row stats, IoU
- * bitmasks, max_conf) is owned by the engine and grows on demand.  The call blocks only when that workspace grows, or while the previous
- * call's copy out of the staging buffer is still in flight; a call's kernels wait on the device for the previous call's, so
- * back-to-back calls need no synchronisation in between. */
+ * bitmasks, max_conf) is owned by the engine and grows on demand, in stream order.  The call blocks only while the previous call's copy
+ * out of the staging buffer is still in flight (and when a batch larger than any before grows that buffer); a call's kernels wait on
+ * the device for the previous call's, so back-to-back calls need no synchronisation in between. */
 typedef struct {
     int32_t n_proposals;           /* n_i */
     int32_t dst_row;               /* first output row of image i */

@@ -235,6 +235,107 @@ struct Arena {   // owns every device allocation of an engine / plan
     ~Arena() { for (void* p : ptrs) cudaFree(p); }
 };
 
+// Owners of the runtime's handles.  A stream is drained before it is destroyed: a launch list that throws midway leaves kernels
+// that still read the workspace its plan is about to free.
+struct EventDel { void operator()(cudaEvent_t e) const { cudaEventDestroy(e); } };
+struct StreamDel { void operator()(cudaStream_t s) const { cudaStreamSynchronize(s); cudaStreamDestroy(s); } };
+struct GraphDel { void operator()(cudaGraph_t g) const { cudaGraphDestroy(g); } };
+struct GraphExecDel { void operator()(cudaGraphExec_t g) const { cudaGraphExecDestroy(g); } };
+struct PinnedDel { void operator()(char* p) const { cudaFreeHost(p); } };
+using Event = std::unique_ptr<CUevent_st, EventDel>;
+using Stream = std::unique_ptr<CUstream_st, StreamDel>;
+using Graph = std::unique_ptr<CUgraph_st, GraphDel>;
+using GraphExec = std::unique_ptr<CUgraphExec_st, GraphExecDel>;
+
+Event make_event(unsigned flags = cudaEventDisableTiming) {
+    cudaEvent_t e;
+    CUDA_CHECK(cudaEventCreateWithFlags(&e, flags));
+    return Event(e);
+}
+Stream make_stream() {
+    cudaStream_t s;
+    CUDA_CHECK(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
+    return Stream(s);
+}
+// What `enqueue` launches on st, as a graph.  A throw from enqueue ends the capture it aborted before it propagates.
+Graph capture_graph(cudaStream_t st, const std::function<void()>& enqueue) {
+    CUDA_CHECK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+    cudaGraph_t g = nullptr;
+    try {
+        enqueue();
+    } catch (...) {
+        cudaStreamEndCapture(st, &g);
+        Graph partial(g);
+        throw;
+    }
+    const cudaError_t e = cudaStreamEndCapture(st, &g);
+    Graph owned(g);
+    CUDA_CHECK(e);
+    return owned;
+}
+GraphExec instantiate(cudaGraph_t g) {
+    cudaGraphExec_t x;
+    CUDA_CHECK(cudaGraphInstantiate(&x, g, 0));
+    return GraphExec(x);
+}
+
+// What a call builds on the host (a packed forward's row layout, the descriptors of the calls beside the forward) reaches the device
+// through two owners.  Both grow on demand to at least twice their last size (and kMinGrowBytes), and set the pointer and the size
+// together, once the allocation has succeeded.
+//   Staging: a pinned host buffer and `copied`, recorded once the call's copies out of it are enqueued.  stage() waits on the host
+//     until the previous call's copies have left the buffer, grows it, and lets the caller fill it and put its parts on the device.
+//   Workspace: a device buffer and `done`, which the call records (release) after its last kernel that reads the buffer.  acquire()
+//     makes the call's stream wait for the previous call's `done` before anything writes the buffer, so growth is stream-ordered
+//     (cudaFreeAsync / cudaMallocAsync on that stream) and never blocks the host.
+// Their events are created with the engine (a plan's Staging with its plan), never in the audit pass.
+constexpr size_t kMinGrowBytes = 4096;
+inline size_t grown(size_t have, size_t need) { return std::max({need, 2 * have, kMinGrowBytes}); }
+
+struct Staging {
+    Event copied;
+    std::unique_ptr<char, PinnedDel> buf;
+    size_t size = 0;
+    ~Staging() { if (copied) cudaEventSynchronize(copied.get()); }
+    void reserve(size_t bytes) {
+        if (bytes <= size) return;
+        char* p;
+        CUDA_CHECK(cudaMallocHost(&p, bytes));
+        buf.reset(p);
+        size = bytes;
+    }
+    // fill(h, put): h holds `bytes`; put(dst, at, n) copies bytes [at, at + n) of h to the device at dst on st
+    template <typename Fill> void stage(size_t bytes, cudaStream_t st, Fill&& fill) {
+        CUDA_CHECK(cudaEventSynchronize(copied.get()));
+        if (bytes > size) reserve(grown(size, bytes));
+        char* h = buf.get();
+        fill(h, [&](void* dst, size_t at, size_t n) { CUDA_CHECK(cudaMemcpyAsync(dst, h + at, n, cudaMemcpyHostToDevice, st)); });
+        CUDA_CHECK(cudaEventRecord(copied.get(), st));
+    }
+};
+
+struct Workspace {
+    Event done;
+    char* p = nullptr;
+    size_t size = 0;
+    ~Workspace() {
+        if (done) cudaEventSynchronize(done.get());
+        if (p) cudaFree(p);
+    }
+    char* acquire(size_t bytes, cudaStream_t st) {
+        CUDA_CHECK(cudaStreamWaitEvent(st, done.get(), 0));
+        if (bytes > size) {
+            const size_t n = grown(size, bytes);
+            void* q;
+            CUDA_CHECK(cudaMallocAsync(&q, n, st));
+            char* old = std::exchange(p, static_cast<char*>(q));
+            size = n;
+            if (old) CUDA_CHECK(cudaFreeAsync(old, st));
+        }
+        return p;
+    }
+    void release(cudaStream_t st) { CUDA_CHECK(cudaEventRecord(done.get(), st)); }
+};
+
 inline uint16_t f32_to_f16_bits(float f) {          // IEEE half, round to nearest even, saturating to +-65504
     const __half h = __float2half_rn(f);            // host-callable conversion from cuda_fp16.h
     uint16_t b;
@@ -718,20 +819,19 @@ struct Plan {
     uint64_t last_use = 0;                             // plan-cache LRU stamp
     long long* timeline = nullptr;                     // profiling (set_option "timeline"): [GEMM op][kTimelineCtas][16] stamps of the LAST replay
     double flops = 0;
-    cudaGraph_t graph = nullptr;
-    cudaGraphExec_t exec = nullptr;
+    Graph graph;
+    GraphExec exec;
     // host-API staging (device copies of the inputs)
     int64_t *d_q = nullptr, *d_seg = nullptr, *d_mask = nullptr, *d_task = nullptr;
     float *d_feat = nullptr, *d_loc = nullptr;
     uint8_t* d_imask = nullptr;
     float* d_out[12] = {nullptr};
-    // packed plans (the packed forwards and retrieval calls): d_meta in the format `layout` describes, filled per call from the
-    // pinned h_meta (stage_meta); meta_copied marks when the last copy out of h_meta has been made
+    // packed plans (the packed forwards and retrieval calls): d_meta in the format `layout` describes, filled per call through
+    // `meta` (stage_meta), reserved at plan build so that a forward never allocates
     bool packed = false;
     MetaLayout layout;
     int* d_meta = nullptr;
-    int* h_meta = nullptr;
-    cudaEvent_t meta_copied = nullptr;
+    Staging meta;
     const int* offs_t() const { return d_meta + layout.offs_t(); }
     const int* offs_v() const { return d_meta + layout.offs_v(); }
     const int* rows_t() const { return d_meta + layout.rows_t(); }
@@ -739,12 +839,6 @@ struct Plan {
     const int* src_t() const { return d_meta + layout.src_t(); }
     const int* src_v() const { return d_meta + layout.src_v(); }
     const int64_t* meta64(size_t at) const { return reinterpret_cast<const int64_t*>(d_meta + at); }
-    ~Plan() {
-        if (exec) cudaGraphExecDestroy(exec);
-        if (graph) cudaGraphDestroy(graph);
-        if (meta_copied) { cudaEventSynchronize(meta_copied); cudaEventDestroy(meta_copied); }
-        if (h_meta) cudaFreeHost(h_meta);
-    }
 };
 
 // One pre-training head at one bucket of M listed rows (vb200_pretraining_heads): the device row list (the call's count first, which
@@ -808,60 +902,21 @@ struct vb200_engine {
     int profile_grid_pct = 0;       // vb200_set_option("profile_grid_pct"): persistent-grid override for vb200_profile_ops only
     uint64_t use_clock = 0;         // LRU clock of the plan cache
     size_t max_plans = 24;          // VB200_MAX_PLANS: least-recently-used plans beyond this are destroyed (workspace + graph)
-    cudaStream_t side_stream = nullptr;
-    cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
     std::vector<std::string> schedule;
-    // answer decode (vb200_decode_answers): descriptors go to dec_d through the pinned dec_h, dec_copied marks when the last copy out
-    // of dec_h has been made; ans_d holds vb200_decode_answers_host's device answers.  All three grow on demand.
-    vb::DecodeDesc* dec_h = nullptr;
-    vb::DecodeDesc* dec_d = nullptr;
-    size_t dec_cap = 0;
-    cudaEvent_t dec_copied = nullptr;
-    vb200_answer* ans_d = nullptr;
-    size_t ans_cap = 0;
-    // attention relevance (vb200_attention_relevance): each call's entry and sample descriptors go to rel_d through the pinned rel_h,
-    // rel_copied marks when the last copy out of rel_h has been made.  Both grow on demand.
-    char* rel_h = nullptr;
-    char* rel_d = nullptr;
-    size_t rel_cap = 0;
-    cudaEvent_t rel_copied = nullptr;
-    // region selection (vb200_select_regions): descriptors staged in the pinned sel_h (sel_copied: the last copy out of it), the
-    // workspace sel_ws holds the device descriptors, row stats, boxes, bitmasks, max_conf and keep lists; sel_done marks the end of
-    // the last call's kernels.  Both buffers grow on demand.
-    vb::SelectDesc* sel_h = nullptr;
-    size_t sel_h_cap = 0;
-    char* sel_ws = nullptr;
-    size_t sel_ws_bytes = 0;
-    cudaEvent_t sel_copied = nullptr, sel_done = nullptr;
     // pre-training heads at chosen rows (vb200_pretraining_heads): per head (kHeadText / kHeadImage / kHeadPair) the RowHeads of every
-    // bucket seen so far; row lists staged in the pinned pre_h (pre_copied: the last copy out of it), pre_done marks the end of the
-    // last call's kernels.
+    // bucket seen so far
     std::map<int, std::unique_ptr<RowHeads>> row_heads[3];
-    int32_t* pre_h = nullptr;
-    size_t pre_h_cap = 0;
-    cudaEvent_t pre_copied = nullptr, pre_done = nullptr;
-
-    ~vb200_engine() {
-        if (pre_copied) { cudaEventSynchronize(pre_copied); cudaEventDestroy(pre_copied); }
-        if (pre_done) { cudaEventSynchronize(pre_done); cudaEventDestroy(pre_done); }
-        if (pre_h) cudaFreeHost(pre_h);
-        for (auto& m : row_heads) m.clear();
-        if (sel_copied) { cudaEventSynchronize(sel_copied); cudaEventDestroy(sel_copied); }
-        if (sel_done) { cudaEventSynchronize(sel_done); cudaEventDestroy(sel_done); }
-        if (sel_h) cudaFreeHost(sel_h);
-        if (sel_ws) cudaFree(sel_ws);
-        if (dec_copied) { cudaEventSynchronize(dec_copied); cudaEventDestroy(dec_copied); }
-        if (dec_h) cudaFreeHost(dec_h);
-        if (dec_d) cudaFree(dec_d);
-        if (ans_d) cudaFree(ans_d);
-        if (rel_copied) { cudaEventSynchronize(rel_copied); cudaEventDestroy(rel_copied); }
-        if (rel_h) cudaFreeHost(rel_h);
-        if (rel_d) cudaFree(rel_d);
-        plans.clear();
-        if (side_stream) cudaStreamDestroy(side_stream);
-        if (ev_fork) cudaEventDestroy(ev_fork);
-        if (ev_join) cudaEventDestroy(ev_join);
-    }
+    // Members are destroyed in reverse order: the owners below go before the plans and RowHeads above, and each Staging waits for
+    // its copies before the workspaces they fill are freed.
+    // The calls beside the forward: answer decode's descriptors (pretraining_heads' top-k ones too) and vb200_decode_answers_host's
+    // device answers, attention relevance's entry and sample descriptors, region selection's descriptors and workspace (device
+    // descriptors, row stats, boxes, bitmasks, max_conf, keep lists), and pre-training's row lists, staged into the RowHeads' d_rows.
+    // The RowHeads never grow, so pre_done alone orders those calls, as a Workspace's `done` does.
+    Workspace dec_ws, ans_ws, rel_ws, sel_ws;
+    Staging dec_in, rel_in, sel_in, pre_in;
+    Event pre_done;
+    Stream side_stream;
+    Event ev_fork, ev_join;
 
     // ---------------------------------------------------------------- checkpoint ingestion
     HostTensor& need(const std::string& name, int ndim, int64_t d0, int64_t d1 = 0) {
@@ -1528,8 +1583,8 @@ struct vb200_engine {
             const size_t n_meta = pl.layout.size();
             pl.d_meta = pl.mem.alloc_n<int>(n_meta);
             CUDA_CHECK(cudaMemset(pl.d_meta, 0, n_meta * sizeof(int)));
-            CUDA_CHECK(cudaMallocHost(&pl.h_meta, n_meta * sizeof(int)));
-            CUDA_CHECK(cudaEventCreateWithFlags(&pl.meta_copied, cudaEventDisableTiming));
+            pl.meta.copied = make_event();
+            pl.meta.reserve(n_meta * sizeof(int));
         }
         const int Mt = B * T, Mv = B * V, H = c.hidden, Hv = c.v_hidden, Hb = c.bi_hidden;
         const bool full = schedule_mode == FULL;
@@ -1618,12 +1673,9 @@ struct vb200_engine {
         // One eager pass first: opts kernels into their shared-memory sizes and surfaces launch-configuration
         // errors with a real message (errors inside a capture only invalidate the capture).
         if (!pl.ops.empty()) {
-            cudaStream_t ws;
-            CUDA_CHECK(cudaStreamCreateWithFlags(&ws, cudaStreamNonBlocking));
-            try { run_ops(pl, ws); } catch (...) { cudaStreamSynchronize(ws); cudaStreamDestroy(ws); throw; }
-            cudaError_t e = cudaStreamSynchronize(ws);
-            cudaStreamDestroy(ws);
-            CUDA_CHECK(e);
+            const Stream ws = make_stream();
+            run_ops(pl, ws.get());
+            CUDA_CHECK(cudaStreamSynchronize(ws.get()));
             if (opt.use_cuda_graph) capture(pl);
         }
         Plan* raw = up.get();
@@ -1735,24 +1787,24 @@ struct vb200_engine {
             }
             if (op.stream == 1) {
                 if (!side_started || op.sync == Op::FORK) {
-                    CUDA_CHECK(cudaEventRecord(ev_fork, st));
-                    CUDA_CHECK(cudaStreamWaitEvent(side_stream, ev_fork, 0));
+                    CUDA_CHECK(cudaEventRecord(ev_fork.get(), st));
+                    CUDA_CHECK(cudaStreamWaitEvent(side_stream.get(), ev_fork.get(), 0));
                     side_started = true;
                 }
-                launch_op(op, side_stream);
+                launch_op(op, side_stream.get());
                 side_dirty = true;
             } else {
                 if (op.sync == Op::JOIN && side_dirty) {
-                    CUDA_CHECK(cudaEventRecord(ev_join, side_stream));
-                    CUDA_CHECK(cudaStreamWaitEvent(st, ev_join, 0));
+                    CUDA_CHECK(cudaEventRecord(ev_join.get(), side_stream.get()));
+                    CUDA_CHECK(cudaStreamWaitEvent(st, ev_join.get(), 0));
                     side_dirty = false;
                 }
                 launch_op(op, st);
             }
         }
         if (side_dirty) {
-            CUDA_CHECK(cudaEventRecord(ev_join, side_stream));
-            CUDA_CHECK(cudaStreamWaitEvent(st, ev_join, 0));
+            CUDA_CHECK(cudaEventRecord(ev_join.get(), side_stream.get()));
+            CUDA_CHECK(cudaStreamWaitEvent(st, ev_join.get(), 0));
         }
     }
     // Per-op device time: each launch-list entry is captured `kRep` times into its own CUDA graph and the graph replayed
@@ -1761,59 +1813,29 @@ struct vb200_engine {
     // the plan's workspace, which must hold a previous forward's data.  Used by bench.py for the per-kernel roofline.
     void profile_ops(Plan& pl, int iters, std::vector<double>& ms_out) {
         constexpr int kRep = 8;
-        cudaStream_t st;
-        CUDA_CHECK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-        cudaEvent_t e0, e1;
-        CUDA_CHECK(cudaEventCreate(&e0));
-        CUDA_CHECK(cudaEventCreate(&e1));
+        const Stream owned = make_stream();
+        const cudaStream_t st = owned.get();
+        const Event e0 = make_event(cudaEventDefault), e1 = make_event(cudaEventDefault);
         const size_t n = pl.ops.size();
         ms_out.assign(n, 0.0);
-        cudaGraph_t g = nullptr;
-        cudaGraphExec_t ge = nullptr;
-        try {
-            for (size_t i = 0; i < n; ++i) {
-                CUDA_CHECK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-                for (int r = 0; r < kRep; ++r) launch_op(pl.ops[i], st);
-                CUDA_CHECK(cudaStreamEndCapture(st, &g));
-                CUDA_CHECK(cudaGraphInstantiate(&ge, g, 0));
-                CUDA_CHECK(cudaGraphLaunch(ge, st));                    // warm-up
-                CUDA_CHECK(cudaEventRecord(e0, st));
-                for (int it = 0; it < iters; ++it) CUDA_CHECK(cudaGraphLaunch(ge, st));
-                CUDA_CHECK(cudaEventRecord(e1, st));
-                CUDA_CHECK(cudaStreamSynchronize(st));
-                float ms = 0.0f;
-                CUDA_CHECK(cudaEventElapsedTime(&ms, e0, e1));
-                ms_out[i] = ms / (static_cast<double>(iters) * kRep);
-                cudaGraphExecDestroy(ge); ge = nullptr;
-                cudaGraphDestroy(g); g = nullptr;
-            }
-        } catch (...) {
-            if (ge) cudaGraphExecDestroy(ge);
-            if (g) cudaGraphDestroy(g);
-            cudaEventDestroy(e0); cudaEventDestroy(e1); cudaStreamDestroy(st);
-            throw;
+        for (size_t i = 0; i < n; ++i) {
+            const Graph g = capture_graph(st, [&] { for (int r = 0; r < kRep; ++r) launch_op(pl.ops[i], st); });
+            const GraphExec ge = instantiate(g.get());
+            CUDA_CHECK(cudaGraphLaunch(ge.get(), st));                  // warm-up
+            CUDA_CHECK(cudaEventRecord(e0.get(), st));
+            for (int it = 0; it < iters; ++it) CUDA_CHECK(cudaGraphLaunch(ge.get(), st));
+            CUDA_CHECK(cudaEventRecord(e1.get(), st));
+            CUDA_CHECK(cudaStreamSynchronize(st));
+            float ms = 0.0f;
+            CUDA_CHECK(cudaEventElapsedTime(&ms, e0.get(), e1.get()));
+            ms_out[i] = ms / (static_cast<double>(iters) * kRep);
         }
-        cudaEventDestroy(e0); cudaEventDestroy(e1); cudaStreamDestroy(st);
     }
 
     void capture(Plan& pl) {
-        cudaStream_t cs;
-        CUDA_CHECK(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
-        cudaError_t e = cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal);
-        if (e != cudaSuccess) { cudaStreamDestroy(cs); CUDA_CHECK(e); }
-        try {
-            run_ops(pl, cs);
-        } catch (...) {
-            cudaGraph_t g = nullptr;
-            cudaStreamEndCapture(cs, &g);
-            if (g) cudaGraphDestroy(g);
-            cudaStreamDestroy(cs);
-            throw;
-        }
-        e = cudaStreamEndCapture(cs, &pl.graph);
-        cudaStreamDestroy(cs);
-        CUDA_CHECK(e);
-        CUDA_CHECK(cudaGraphInstantiate(&pl.exec, pl.graph, 0));
+        const Stream cs = make_stream();
+        pl.graph = capture_graph(cs.get(), [&] { run_ops(pl, cs.get()); });
+        pl.exec = instantiate(pl.graph.get());
     }
 
     void check_inputs(const vb200_inputs& in) const {
@@ -1849,7 +1871,7 @@ struct vb200_engine {
         if (pl.ops.empty()) return;
         struct R { R(const Plan& p) { char b[96]; snprintf(b, sizeof(b), "vb200 forward B=%d T=%d V=%d", p.B, p.T, p.V); nvtxRangePushA(b); }
                    ~R() { nvtxRangePop(); } } range(pl);
-        if (pl.exec) CUDA_CHECK(cudaGraphLaunch(pl.exec, st));
+        if (pl.exec) CUDA_CHECK(cudaGraphLaunch(pl.exec.get(), st));
         else run_ops(pl, st);
     }
     // worker.py:422-455 on the device: detector output -> operand rows / masks for the same plan as the dense forward
@@ -1954,10 +1976,8 @@ struct vb200_engine {
     }
     // meta (host, in the plan's d_meta layout) -> d_meta, in stream order ahead of the plan's kernels
     void stage_meta(Plan& pl, const std::vector<int>& meta, cudaStream_t st) {
-        CUDA_CHECK(cudaEventSynchronize(pl.meta_copied));           // the previous call's copy has left the staging buffer
-        memcpy(pl.h_meta, meta.data(), meta.size() * sizeof(int));
-        CUDA_CHECK(cudaMemcpyAsync(pl.d_meta, pl.h_meta, meta.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-        CUDA_CHECK(cudaEventRecord(pl.meta_copied, st));
+        const size_t bytes = meta.size() * sizeof(int);
+        pl.meta.stage(bytes, st, [&](char* h, const auto& put) { memcpy(h, meta.data(), bytes); put(pl.d_meta, 0, bytes); });
     }
     // ---- answer decode: every descriptor is resolved and bounds-checked before anything is enqueued
     std::vector<vb::DecodeDesc> decode_descs(const char* api, const vb200_decode_msg* msgs, int n, const vb200_outputs* out, int batch,
@@ -2005,38 +2025,17 @@ struct vb200_engine {
         }
         return d;
     }
-    // descriptors -> dec_d through the pinned dec_h (in stream order), then the decode kernel writes answers [n]
+    // descriptors -> dec_ws through dec_in (in stream order), then the decode kernel writes answers [n]
     void decode_answers(const std::vector<vb::DecodeDesc>& d, vb200_answer* answers, cudaStream_t st) {
         CUDA_CHECK(vb::launch_answer_decode(stage_decode(d, st), static_cast<int>(d.size()), answers, st));
+        dec_ws.release(st);
     }
+    // the caller releases dec_ws after its last decode kernel
     const vb::DecodeDesc* stage_decode(const std::vector<vb::DecodeDesc>& d, cudaStream_t st) {
-        const size_t n = d.size();
-        if (dec_copied == nullptr) CUDA_CHECK(cudaEventCreateWithFlags(&dec_copied, cudaEventDisableTiming));
-        CUDA_CHECK(cudaEventSynchronize(dec_copied));                // the previous call's copy has left the staging buffer
-        if (n > dec_cap) {
-            const size_t cap = std::max<size_t>({n, 2 * dec_cap, 256});
-            if (dec_h) CUDA_CHECK(cudaFreeHost(dec_h));
-            dec_h = nullptr;
-            CUDA_CHECK(cudaMallocHost(&dec_h, cap * sizeof(vb::DecodeDesc)));
-            if (dec_d) CUDA_CHECK(cudaFreeAsync(dec_d, st));          // after the kernels already enqueued on st have read it
-            dec_d = nullptr;
-            CUDA_CHECK(cudaMallocAsync(&dec_d, cap * sizeof(vb::DecodeDesc), st));
-            dec_cap = cap;
-        }
-        memcpy(dec_h, d.data(), n * sizeof(vb::DecodeDesc));
-        CUDA_CHECK(cudaMemcpyAsync(dec_d, dec_h, n * sizeof(vb::DecodeDesc), cudaMemcpyHostToDevice, st));
-        CUDA_CHECK(cudaEventRecord(dec_copied, st));
-        return dec_d;
-    }
-    vb200_answer* answer_scratch(size_t n, cudaStream_t st) {
-        if (n > ans_cap) {
-            const size_t cap = std::max<size_t>({n, 2 * ans_cap, 256});
-            if (ans_d) CUDA_CHECK(cudaFreeAsync(ans_d, st));
-            ans_d = nullptr;
-            CUDA_CHECK(cudaMallocAsync(&ans_d, cap * sizeof(vb200_answer), st));
-            ans_cap = cap;
-        }
-        return ans_d;
+        const size_t bytes = d.size() * sizeof(vb::DecodeDesc);
+        char* dst = dec_ws.acquire(bytes, st);
+        dec_in.stage(bytes, st, [&](char* h, const auto& put) { memcpy(h, d.data(), bytes); put(dst, 0, bytes); });
+        return reinterpret_cast<const vb::DecodeDesc*>(dst);
     }
     // ---- attention relevance: lengths and the map selection are checked, and the descriptors built, before anything is enqueued
     void attention_relevance(const float* maps, int batch, const int32_t* n_tokens, const int32_t* n_regions, int packed,
@@ -2069,26 +2068,17 @@ struct vb200_engine {
             out += 2 * static_cast<int64_t>(T + V);
             max_cols = std::max(max_cols, T + V);
         }
-        // stage entries then samples (both 8-byte aligned) through the pinned rel_h, in stream order
+        // stage entries then samples (both 8-byte aligned) in one copy, in stream order
         const size_t eb = n * sizeof(vb::RelevanceEntry), bytes = eb + smp.size() * sizeof(vb::RelevanceSample);
-        if (rel_copied == nullptr) CUDA_CHECK(cudaEventCreateWithFlags(&rel_copied, cudaEventDisableTiming));
-        CUDA_CHECK(cudaEventSynchronize(rel_copied));                // the previous call's copy has left the staging buffer
-        if (bytes > rel_cap) {
-            const size_t cap = std::max<size_t>({bytes, 2 * rel_cap, 4096});
-            if (rel_h) CUDA_CHECK(cudaFreeHost(rel_h));
-            rel_h = nullptr;
-            CUDA_CHECK(cudaMallocHost(&rel_h, cap));
-            if (rel_d) CUDA_CHECK(cudaFreeAsync(rel_d, st));          // after the kernels already enqueued on st have read it
-            rel_d = nullptr;
-            CUDA_CHECK(cudaMallocAsync(&rel_d, cap, st));
-            rel_cap = cap;
-        }
-        memcpy(rel_h, ents.data(), eb);
-        memcpy(rel_h + eb, smp.data(), bytes - eb);
-        CUDA_CHECK(cudaMemcpyAsync(rel_d, rel_h, bytes, cudaMemcpyHostToDevice, st));
-        CUDA_CHECK(cudaEventRecord(rel_copied, st));
-        CUDA_CHECK(vb::launch_attention_relevance(maps, reinterpret_cast<const vb::RelevanceEntry*>(rel_d), static_cast<int>(n),
-                                                  reinterpret_cast<const vb::RelevanceSample*>(rel_d + eb), batch, max_cols, relevance, st));
+        char* dst = rel_ws.acquire(bytes, st);
+        rel_in.stage(bytes, st, [&](char* h, const auto& put) {
+            memcpy(h, ents.data(), eb);
+            memcpy(h + eb, smp.data(), bytes - eb);
+            put(dst, 0, bytes);
+        });
+        CUDA_CHECK(vb::launch_attention_relevance(maps, reinterpret_cast<const vb::RelevanceEntry*>(dst), static_cast<int>(n),
+                                                  reinterpret_cast<const vb::RelevanceSample*>(dst + eb), batch, max_cols, relevance, st));
+        rel_ws.release(st);
     }
     // ---- region selection: every descriptor is checked before anything is enqueued
     void select_regions(const vb200_detections* imgs, int n, const vb200_select_params* p, const vb200_selected* out, cudaStream_t st) {
@@ -2156,36 +2146,16 @@ struct vb200_engine {
         const size_t o_desc = 0, o_stats = up(o_desc + n * sizeof(vb::SelectDesc)), o_box = up(o_stats + rows * 8),
                      o_conf = up(o_box + rows * 16), o_keep = up(o_conf + rows * 4), o_mask = up(o_keep + static_cast<size_t>(n) * K * 4),
                      need = up(o_mask + words * 4);
-
-        if (sel_copied == nullptr) CUDA_CHECK(cudaEventCreateWithFlags(&sel_copied, cudaEventDisableTiming));
-        if (sel_done == nullptr) CUDA_CHECK(cudaEventCreateWithFlags(&sel_done, cudaEventDisableTiming));
-        CUDA_CHECK(cudaEventSynchronize(sel_copied));               // the previous call's copy has left the staging buffer
-        if (static_cast<size_t>(n) > sel_h_cap) {
-            const size_t cap = std::max<size_t>({static_cast<size_t>(n), 2 * sel_h_cap, 64});
-            if (sel_h) CUDA_CHECK(cudaFreeHost(sel_h));
-            sel_h = nullptr;
-            CUDA_CHECK(cudaMallocHost(&sel_h, cap * sizeof(vb::SelectDesc)));
-            sel_h_cap = cap;
-        }
-        if (need > sel_ws_bytes) {
-            CUDA_CHECK(cudaEventSynchronize(sel_done));             // the previous call's kernels are done with the old workspace
-            if (sel_ws) CUDA_CHECK(cudaFree(sel_ws));
-            sel_ws = nullptr;
-            const size_t cap = std::max(need, 2 * sel_ws_bytes);
-            CUDA_CHECK(cudaMalloc(&sel_ws, cap));
-            sel_ws_bytes = cap;
-        } else {
-            CUDA_CHECK(cudaStreamWaitEvent(st, sel_done, 0));       // the previous call (any stream) is done with the workspace
-        }
+        char* ws = sel_ws.acquire(need, st);
         vb::SelectArgs a{};
         a.C = C; a.F = F; a.K = K; a.start = p->background ? 0 : 1;
         a.thr = std::max(p->conf_thresh, 0.f);
         a.nms_iou = p->nms_iou;
-        a.stats = reinterpret_cast<float2*>(sel_ws + o_stats);
-        a.dbox = reinterpret_cast<float*>(sel_ws + o_box);
-        a.max_conf = reinterpret_cast<unsigned*>(sel_ws + o_conf);
-        a.keep = reinterpret_cast<int*>(sel_ws + o_keep);
-        a.mask = reinterpret_cast<unsigned*>(sel_ws + o_mask);
+        a.stats = reinterpret_cast<float2*>(ws + o_stats);
+        a.dbox = reinterpret_cast<float*>(ws + o_box);
+        a.max_conf = reinterpret_cast<unsigned*>(ws + o_conf);
+        a.keep = reinterpret_cast<int*>(ws + o_keep);
+        a.mask = reinterpret_cast<unsigned*>(ws + o_mask);
         a.box_features = out->box_features;
         a.boxes = out->boxes;
         a.num_boxes = out->num_boxes;
@@ -2193,13 +2163,11 @@ struct vb200_engine {
         a.max_conf_out = out->max_conf;
         a.cls_prob = out->cls_prob;
         a.objects = out->objects;
-        const vb::SelectDesc* descs = reinterpret_cast<const vb::SelectDesc*>(sel_ws + o_desc);
-        memcpy(sel_h, d.data(), n * sizeof(vb::SelectDesc));
-        CUDA_CHECK(cudaMemcpyAsync(sel_ws + o_desc, sel_h, n * sizeof(vb::SelectDesc), cudaMemcpyHostToDevice, st));
-        CUDA_CHECK(cudaEventRecord(sel_copied, st));
+        const size_t db = n * sizeof(vb::SelectDesc);
+        sel_in.stage(db, st, [&](char* h, const auto& put) { memcpy(h, d.data(), db); put(ws + o_desc, 0, db); });
         CUDA_CHECK(cudaMemsetAsync(a.max_conf, 0, rows * 4, st));
-        CUDA_CHECK(vb::launch_select_regions(descs, n, max_n, max_npad, a, st));
-        CUDA_CHECK(cudaEventRecord(sel_done, st));
+        CUDA_CHECK(vb::launch_select_regions(reinterpret_cast<const vb::SelectDesc*>(ws + o_desc), n, max_n, max_npad, a, st));
+        sel_ws.release(st);
     }
     // ---- pre-training heads at chosen rows
     // The RowHeads of `head` for n rows: bucket M = 128 * 2^k >= n, built on its first use with the forward's head launches
@@ -2259,8 +2227,8 @@ struct vb200_engine {
             if (x.rows[i] < 0 || x.rows[i] >= x.src_rows)
                 fail(VB200_ERR_INVALID, "%s: %s[%d] = %d is outside the %d rows of %s", api, x.list, i, x.rows[i], x.src_rows, x.state);
     }
-    // The RowHeads of every group that runs, with its count, rows and labels staged through the pinned pre_h into rh->d_rows, in stream
-    // order after the previous call (any stream) is done with the workspace.  Records pre_copied; the caller records pre_done.
+    // The RowHeads of every group that runs, with its count, rows and labels staged through pre_in into rh->d_rows, in stream order
+    // after the previous call (any stream) is done with them.  The caller records pre_done.
     void stage_rows(const HeadGroup (&g)[3], RowHeads* (&rh)[3], cudaStream_t st) {
         size_t staged = 0;
         for (int i = 0; i < 3; ++i) {
@@ -2268,28 +2236,20 @@ struct vb200_engine {
             rh[i] = &row_heads_for(i, g[i].n);
             staged += 1 + static_cast<size_t>(g[i].n) * (g[i].labels ? 2 : 1);
         }
-        if (pre_copied == nullptr) CUDA_CHECK(cudaEventCreateWithFlags(&pre_copied, cudaEventDisableTiming));
-        if (pre_done == nullptr) CUDA_CHECK(cudaEventCreateWithFlags(&pre_done, cudaEventDisableTiming));
-        CUDA_CHECK(cudaEventSynchronize(pre_copied));                // the previous call's copies have left the staging buffer
-        if (staged > pre_h_cap) {
-            const size_t cap = std::max<size_t>({staged, 2 * pre_h_cap, 1024});
-            if (pre_h) CUDA_CHECK(cudaFreeHost(pre_h));
-            pre_h = nullptr;
-            CUDA_CHECK(cudaMallocHost(&pre_h, cap * sizeof(int32_t)));
-            pre_h_cap = cap;
-        }
-        CUDA_CHECK(cudaStreamWaitEvent(st, pre_done, 0));            // the previous call (any stream) is done with the workspace
-        size_t at = 0;
-        for (int i = 0; i < 3; ++i) {
-            if (rh[i] == nullptr) continue;
-            const size_t n = static_cast<size_t>(g[i].n), len = 1 + n * (g[i].labels ? 2 : 1);
-            pre_h[at] = g[i].n;
-            memcpy(pre_h + at + 1, g[i].rows, n * sizeof(int32_t));
-            if (g[i].labels) memcpy(pre_h + at + 1 + n, g[i].labels, n * sizeof(int32_t));
-            CUDA_CHECK(cudaMemcpyAsync(rh[i]->d_rows, pre_h + at, len * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-            at += len;
-        }
-        CUDA_CHECK(cudaEventRecord(pre_copied, st));
+        CUDA_CHECK(cudaStreamWaitEvent(st, pre_done.get(), 0));
+        pre_in.stage(staged * sizeof(int32_t), st, [&](char* hb, const auto& put) {
+            int32_t* h = reinterpret_cast<int32_t*>(hb);
+            size_t at = 0;
+            for (int i = 0; i < 3; ++i) {
+                if (rh[i] == nullptr) continue;
+                const size_t n = static_cast<size_t>(g[i].n), len = 1 + n * (g[i].labels ? 2 : 1);
+                h[at] = g[i].n;
+                memcpy(h + at + 1, g[i].rows, n * sizeof(int32_t));
+                if (g[i].labels) memcpy(h + at + 1 + n, g[i].labels, n * sizeof(int32_t));
+                put(rh[i]->d_rows, at * sizeof(int32_t), len * sizeof(int32_t));
+                at += len;
+            }
+        });
     }
     // One running group's gather and the forward's head launches: its logits land in r.logits.
     void run_row_heads(int head, const HeadGroup& x, RowHeads& r, cudaStream_t st) {
@@ -2341,7 +2301,8 @@ struct vb200_engine {
                 dd += x.n;
             }
         }
-        CUDA_CHECK(cudaEventRecord(pre_done, st));
+        if (!descs.empty()) dec_ws.release(st);
+        CUDA_CHECK(cudaEventRecord(pre_done.get(), st));
     }
     // The three pre-training objectives at the listed rows: the heads of pretraining_heads, then one CTA per listed row computes its
     // loss from the compact logits and one CTA reduces each list in a fixed order.
@@ -2395,7 +2356,7 @@ struct vb200_engine {
         for (int i = 0; i < 3; ++i)
             if (rh[i] != nullptr && per_row[i] != nullptr)
                 CUDA_CHECK(cudaMemcpyAsync(per_row[i], rh[i]->loss, static_cast<size_t>(g[i].n) * 4, cudaMemcpyDeviceToDevice, st));
-        CUDA_CHECK(cudaEventRecord(pre_done, st));
+        CUDA_CHECK(cudaEventRecord(pre_done.get(), st));
     }
     // rows_t / rows_v (packed plans): the call's row totals -- the per-row outputs hold that many packed rows
     void copy_outputs(Plan& pl, const vb200_outputs& out, cudaStream_t st, cudaMemcpyKind kind, int rows_t = 0, int rows_v = 0) {
@@ -2467,7 +2428,7 @@ int create_engine(const char* api, bool pretraining, const char* config_json, in
                   const vb200_options* opt, vb200_handle* out) {
     if (out == nullptr) { g_create_error = std::string(api) + ": out handle pointer is NULL"; return VB200_ERR_INVALID; }
     *out = nullptr;
-    vb200_engine* eng = nullptr;
+    std::unique_ptr<vb200_engine> eng;
     int rc = guard(nullptr, [&] {
         if (tensors == nullptr || n_tensors <= 0) fail(VB200_ERR_CHECKPOINT, "empty state_dict");
         vb200_options o{};
@@ -2495,7 +2456,7 @@ int create_engine(const char* api, bool pretraining, const char* config_json, in
             audit.ingest(n_tensors, tensors);
         }
         require_device(o.device);
-        eng = new vb200_engine();
+        eng.reset(new vb200_engine());
         eng->cfg = c;
         eng->opt = o;
         eng->pretraining = pretraining;
@@ -2509,14 +2470,15 @@ int create_engine(const char* api, bool pretraining, const char* config_json, in
             if (strcmp(v, "off") == 0) eng->opt.use_pdl = 0;
         }
         eng->gemm_kernel = default_gemm_kernel();
-        CUDA_CHECK(cudaStreamCreateWithFlags(&eng->side_stream, cudaStreamNonBlocking));
-        CUDA_CHECK(cudaEventCreateWithFlags(&eng->ev_fork, cudaEventDisableTiming));
-        CUDA_CHECK(cudaEventCreateWithFlags(&eng->ev_join, cudaEventDisableTiming));
+        eng->side_stream = make_stream();
+        for (Event* e : {&eng->ev_fork, &eng->ev_join, &eng->pre_done}) *e = make_event();
+        for (Staging* s : {&eng->dec_in, &eng->rel_in, &eng->sel_in, &eng->pre_in}) s->copied = make_event();
+        for (Workspace* w : {&eng->dec_ws, &eng->ans_ws, &eng->rel_ws, &eng->sel_ws}) w->done = make_event();
         eng->ingest(n_tensors, tensors);
         CUDA_CHECK(cudaDeviceSynchronize());
     });
-    if (rc != VB200_OK) { delete eng; return rc; }
-    *out = eng;
+    if (rc != VB200_OK) return rc;
+    *out = eng.release();
     return VB200_OK;
 }
 }  // namespace
@@ -2754,9 +2716,11 @@ int vb200_decode_answers_host(vb200_handle h, const vb200_decode_msg* msgs, int3
         if (answers == nullptr) fail(VB200_ERR_INVALID, "%s: answers is NULL", api);
         CUDA_CHECK(cudaSetDevice(h->opt.device));
         cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-        vb200_answer* dev = h->answer_scratch(d.size(), st);
+        const size_t bytes = d.size() * sizeof(vb200_answer);
+        vb200_answer* dev = reinterpret_cast<vb200_answer*>(h->ans_ws.acquire(bytes, st));
         h->decode_answers(d, dev, st);
-        CUDA_CHECK(cudaMemcpyAsync(answers, dev, d.size() * sizeof(vb200_answer), cudaMemcpyDeviceToHost, st));
+        CUDA_CHECK(cudaMemcpyAsync(answers, dev, bytes, cudaMemcpyDeviceToHost, st));
+        h->ans_ws.release(st);
         CUDA_CHECK(cudaStreamSynchronize(st));
     });
 }
