@@ -527,6 +527,51 @@ int vb200_decode_answers_host(vb200_handle h, const vb200_decode_msg* msgs /* HO
                               int32_t batch, int32_t vision_rows, const float* spatials, vb200_answer* answers /* HOST [n] */,
                               void* cuda_stream);
 
+/* ---- Answer ablation: how much each question token and each detector box holds up one answer, from forwards alone.  For every
+ * sample of a packed detector-output batch (laid out exactly as for vb200_forward_regions_packed), the engine builds on the device the
+ * variants below, runs them all as one packed forward and scores each variant's head row against the attributed answer.
+ *   Variants of sample i, in this order: the unablated input; then for each question position p in [token_begin, token_end) the
+ *   input with question[p] replaced by mask_token (segment and task ids unchanged); then for each box j in [box_begin, box_end) the
+ *   detector output without box j: n_boxes_i - 1 boxes, the ones after j moved up, the global mean row the mean of the remaining
+ *   boxes summed in the order the region pack sums them.  Samples follow each other in batch order; the variant count is
+ *   sum_i (1 + (token_end - token_begin) + (box_end - box_begin)) <= VB200_ABLATION_MAX_VARIANTS.
+ *   Bit-identity: every variant's logits equal those of vb200_forward_regions_packed run on that variant's input alone.
+ *   family: VB200_DECODE_VQA, _GQA or _SNLI_VE (one row of one image per answer).  NLVR2 (two images per answer), retrieval (many
+ *   images per answer) and grounding (the answer is a box a variant may remove) are rejected.
+ *   variant_logits (DEVICE, required): fp32 [n_variants, width], each variant's row of the family's head (width num_labels,
+ *   gqa_labels or 3).  scores (DEVICE, optional, NULL skips them): one vb200_ablation_score per variant.  The softmax follows
+ *   vb200_decode_answers (max, expf(x - max), the sum, a division; equal probabilities rank the lower index first), so every
+ *   probability equals what vb200_decode_answers reports for that index of the same logits.  answer = -1 resolves to the
+ *   unablated variant's top-1, and every variant of the sample reports against that column.
+ * The variants run on the PACKED plan of vb200_forward_packed: the count is rounded up to a multiple of 64 with filler variants
+ * (sample 0's first token and first box, outputs discarded), so a server keeps one plan per bucket and capacities.  max_tokens /
+ * max_boxes are the plan's capacities as for vb200_forward_regions_packed (0: this call's maxima); spatials_out is not used.  The
+ * plan's workspace grows with the bucket times the capacities: at 1024 variants and the default 256-row bound, some GB.  A caller
+ * with more variants splits the ranges across calls.
+ * VB200_ERR_INVALID, with nothing enqueued, no output written and a message naming the sample, for: split_fp32 and pre-training
+ * engines; an excluded or unknown family; a range outside [0, Tin_i] / [0, n_boxes_i] or reversed; box ablation on an image with
+ * fewer than 2 boxes; mask_token outside [0, vocab); answer outside [-1, width); more than VB200_ABLATION_MAX_VARIANTS variants;
+ * NULL required pointers; box_features not 16-byte aligned; and every length rule of vb200_forward_regions_packed.
+ * Asynchronous on cuda_stream: the variant descriptors reach the device through engine-owned pinned staging and the variants' ids
+ * live in an engine-owned workspace, both stream-ordered, so back-to-back calls need no synchronisation. */
+#define VB200_ABLATION_MAX_VARIANTS 1024
+typedef struct {
+    int32_t answer;                   /* column of the family's head to attribute; -1: the unablated forward's top-1 */
+    int32_t token_begin, token_end;   /* mask question positions [token_begin, token_end) of the sample's Tin ids, one at a time */
+    int32_t box_begin, box_end;       /* drop boxes [box_begin, box_end) of the sample's n_boxes, one at a time */
+} vb200_ablation_msg;
+
+typedef struct {
+    int32_t answer;                   /* the attributed column (answer -1 resolved) */
+    float prob;                       /* its softmax probability in this variant */
+    int32_t top1;                     /* this variant's own top-1 column */
+    float top1_prob;                  /* and its probability */
+} vb200_ablation_score;
+
+int vb200_answer_ablation(vb200_handle h, const vb200_packed_region_inputs* in, const vb200_ablation_msg* msgs /* HOST [batch] */,
+                          int32_t family, int64_t mask_token, float* variant_logits, vb200_ablation_score* scores, int32_t slot,
+                          void* cuda_stream);
+
 /* ---- Detector-region selection: the feature extraction step of the reference worker (worker.py:123-176) on the detector's raw heads,
  * for every image of a batch in one call, written straight into the packed box_features / boxes that vb200_forward_regions_packed reads.
  * For image i with n_i proposals, C score columns (column 0 is background) and features [n_i, F]:

@@ -110,6 +110,20 @@ class Answer(C.Structure):
                 ("box", (C.c_int32 * 4) * DECODE_MAX_TOP)]
 
 
+ABLATION_MAX_VARIANTS = 1024
+
+
+class AblationMsg(C.Structure):
+    """vb200_ablation_msg: the attributed column (-1: the unablated top-1) and the token and box ranges ablated one unit at a time."""
+    _fields_ = [("answer", C.c_int32), ("token_begin", C.c_int32), ("token_end", C.c_int32), ("box_begin", C.c_int32),
+                ("box_end", C.c_int32)]
+
+
+class AblationScore(C.Structure):
+    """vb200_ablation_score: per variant the attributed column and its probability, and the variant's own top-1 and probability."""
+    _fields_ = [("answer", C.c_int32), ("prob", C.c_float), ("top1", C.c_int32), ("top1_prob", C.c_float)]
+
+
 class Detections(C.Structure):
     """vb200_detections: one image's raw detector heads (device pointers) and its first output row."""
     _fields_ = [("n_proposals", C.c_int32), ("dst_row", C.c_int32), ("im_scale", C.c_double), ("proposals", C.c_void_p),
@@ -166,7 +180,7 @@ EXPORTS = ["vb200_abi_version", "vb200_create", "vb200_destroy", "vb200_last_err
            "vb200_self_attention_stream", "vb200_co_attention_stream",
            "vb200_linear_product", "vb200_text_embed", "vb200_image_pack", "vb200_region_pack", "vb200_rowdot", "vb200_gather_state",
            "vb200_gather_packed_state", "vb200_decode_answers", "vb200_decode_answers_host", "vb200_select_regions",
-           "vb200_pretraining_heads", "vb200_create_pretraining", "vb200_pretraining_objectives"]
+           "vb200_pretraining_heads", "vb200_create_pretraining", "vb200_pretraining_objectives", "vb200_answer_ablation"]
 
 _lib = None
 
@@ -250,6 +264,7 @@ def load():
     lib.vb200_pretraining_heads.argtypes = [vp, C.POINTER(PretrainRows), C.POINTER(PretrainOut), vp]
     lib.vb200_create_pretraining.argtypes = lib.vb200_create.argtypes
     lib.vb200_pretraining_objectives.argtypes = [vp, C.POINTER(PretrainRows), C.POINTER(PretrainTargets), C.POINTER(PretrainLosses), vp]
+    lib.vb200_answer_ablation.argtypes = [vp, C.POINTER(PackedRegionInputs), C.POINTER(AblationMsg), i32, i64, vp, vp, i32, vp]
     for name in EXPORTS:
         if name not in ("vb200_last_error",):
             getattr(lib, name).restype = C.c_int

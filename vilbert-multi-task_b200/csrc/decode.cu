@@ -29,17 +29,11 @@ __device__ __forceinline__ unsigned long long rank_key(float p, int i) {
     return (static_cast<unsigned long long>(__float_as_uint(p)) << 32) | (0xffffffffu - static_cast<unsigned>(i));
 }
 
-__global__ void __launch_bounds__(kDecodeThreads)
-answer_decode_kernel(const DecodeDesc* __restrict__ descs, vb200_answer* __restrict__ answers) {
-    __shared__ float s_f[kDecodeWarps];
-    __shared__ unsigned long long s_k[kDecodeWarps];
-    __shared__ unsigned long long s_pick[VB200_DECODE_MAX_TOP];
-    const DecodeDesc d = descs[blockIdx.x];
-    const float* __restrict__ x = d.src;
+// The softmax's max and sum of the `len` logits at x (every thread gets both), as torch.softmax computes them up to the order of the sum.
+__device__ __forceinline__ float2 softmax_stats(const float* __restrict__ x, int len, float* s_f) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-
     float m = -INFINITY;
-    for (int i = tid; i < d.len; i += kDecodeThreads) m = fmaxf(m, x[i]);
+    for (int i = tid; i < len; i += kDecodeThreads) m = fmaxf(m, x[i]);
     m = warp_max(m);
     if (lane == 0) s_f[warp] = m;
     __syncthreads();
@@ -47,18 +41,25 @@ answer_decode_kernel(const DecodeDesc* __restrict__ descs, vb200_answer* __restr
     __syncthreads();
 
     float s = 0.f;
-    for (int i = tid; i < d.len; i += kDecodeThreads) s += expf(x[i] - m);
+    for (int i = tid; i < len; i += kDecodeThreads) s += expf(x[i] - m);
     s = warp_sum(s);
     if (lane == 0) s_f[warp] = s;
     __syncthreads();
     s = warp_sum(lane < kDecodeWarps ? s_f[lane] : 0.f);
+    __syncthreads();                                  // s_f is reused by the next row's statistics
+    return make_float2(m, s);
+}
 
-    // pick k is the largest key below pick k - 1's: N passes over the segment, each recomputing the same probabilities
+// s_pick[k] for k < top_n: the rank key of pick k, the largest key below pick k - 1's -- top_n passes over the row, each recomputing
+// the same probabilities
+__device__ __forceinline__ void pick_top(const float* __restrict__ x, int len, float2 ms, int top_n, unsigned long long* s_k,
+                                         unsigned long long* s_pick) {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     unsigned long long prev = ~0ull;
-    for (int k = 0; k < d.top_n; ++k) {
+    for (int k = 0; k < top_n; ++k) {
         unsigned long long best = 0;
-        for (int i = tid; i < d.len; i += kDecodeThreads) {
-            const unsigned long long key = rank_key(expf(x[i] - m) / s, i);
+        for (int i = tid; i < len; i += kDecodeThreads) {
+            const unsigned long long key = rank_key(expf(x[i] - ms.x) / ms.y, i);
             if (key < prev && key > best) best = key;
         }
         best = warp_max_u64(best);
@@ -69,19 +70,53 @@ answer_decode_kernel(const DecodeDesc* __restrict__ descs, vb200_answer* __restr
         __syncthreads();
         prev = best;
     }
+}
+
+__device__ __forceinline__ int key_index(unsigned long long key) { return static_cast<int>(0xffffffffu - static_cast<unsigned>(key & 0xffffffffu)); }
+
+__global__ void __launch_bounds__(kDecodeThreads)
+answer_decode_kernel(const DecodeDesc* __restrict__ descs, vb200_answer* __restrict__ answers) {
+    __shared__ float s_f[kDecodeWarps];
+    __shared__ unsigned long long s_k[kDecodeWarps];
+    __shared__ unsigned long long s_pick[VB200_DECODE_MAX_TOP];
+    const DecodeDesc d = descs[blockIdx.x];
+    const float* __restrict__ x = d.src;
+    const int tid = threadIdx.x;
+
+    const float2 ms = softmax_stats(x, d.len, s_f);
+    pick_top(x, d.len, ms, d.top_n, s_k, s_pick);
+
+    if (d.score != nullptr) {                         // answer ablation: one score, no answer
+        const unsigned long long top1 = s_pick[0];
+        int col = d.column;
+        if (col < 0) {                                // the unablated row's top-1, as its own decode ranks it
+            const float2 ref = softmax_stats(d.ref, d.len, s_f);
+            pick_top(d.ref, d.len, ref, 1, s_k, s_pick);
+            col = key_index(s_pick[0]);
+        }
+        if (tid == 0) {
+            vb200_ablation_score sc;
+            sc.answer = col;
+            sc.prob = expf(x[col] - ms.x) / ms.y;
+            sc.top1 = key_index(top1);
+            sc.top1_prob = __uint_as_float(static_cast<unsigned>(top1 >> 32));
+            *d.score = sc;
+        }
+        return;
+    }
 
     vb200_answer* a = answers + blockIdx.x;
     if (tid == 0) a->n = d.top_n;
     if (tid < VB200_DECODE_MAX_TOP) {
         const bool on = tid < d.top_n;
-        a->index[tid] = on ? static_cast<int32_t>(0xffffffffu - static_cast<unsigned>(s_pick[tid] & 0xffffffffu)) : -1;
+        a->index[tid] = on ? key_index(s_pick[tid]) : -1;
         a->prob[tid] = on ? __uint_as_float(static_cast<unsigned>(s_pick[tid] >> 32)) : 0.f;
     }
     if (tid < 4 * VB200_DECODE_MAX_TOP) {
         const int k = tid >> 2, c = tid & 3;       // box k, coordinate c of x1, y1, x2, y2 (spatials columns 0-3)
         int v = 0;
         if (d.spatials != nullptr && k < d.top_n) {
-            const int row = static_cast<int>(0xffffffffu - static_cast<unsigned>(s_pick[k] & 0xffffffffu));
+            const int row = key_index(s_pick[k]);
             const double size = (c & 1) ? d.image_h : d.image_w;
             v = __double2int_rz(static_cast<double>(d.spatials[static_cast<size_t>(row) * 5 + c]) * size);
         }

@@ -153,21 +153,27 @@ image_pack_kernel(const float* __restrict__ feats, const float* __restrict__ loc
 // grid (B, ceil(F / 1024) + 1): the last grid row writes the location columns, the masks and the optional spatials copy.
 // Packed batch (offs = the plan's image row offsets [B + 1]): image b owns regions [offs[b], offs[b+1]) -- its mean row, then its
 // offs[b+1] - offs[b] - 1 boxes, which start at detector row offs[b] - b (one global row per image) -- every row is real, and
-// spatials_out is packed [sum V_i, 5].
+// spatials_out is packed [sum V_i, 5].  With src (answer ablation), output image b is instead source image src[b].image's boxes from
+// detector row src[b].box0 on, with box src[b].skip (>= 0) left out: the boxes after it move up one row, and the mean sums the kept
+// boxes in the same order, so the rows are those of the reduced image packed alone.
 __global__ void __launch_bounds__(128)
 region_pack_kernel(const float* __restrict__ box_feats, const float* __restrict__ boxes, const float* __restrict__ image_wh,
                    const int32_t* __restrict__ num_boxes, __nv_bfloat16* __restrict__ a_out, float* __restrict__ mask_add,
-                   float* __restrict__ spatials_out, int n, int F, int Kp, int f16, int split16, const int* __restrict__ offs) {
+                   float* __restrict__ spatials_out, int n, int F, int Kp, int f16, int split16, const int* __restrict__ offs,
+                   const RegionSrc* __restrict__ src_img) {
     const int b = blockIdx.x;
-    int row0, box0, nb;                                              // first operand row, first detector row, valid boxes
-    if (offs == nullptr) {
+    int row0, box0, nb, img = b, skip = -1;                          // first operand row, first detector row, valid boxes, source
+    if (offs == nullptr) {                                           //   image, skipped detector box
         row0 = b * (n + 1); box0 = b * n;
         nb = num_boxes ? num_boxes[b] : n;
         nb = nb < 0 ? 0 : (nb > n ? n : nb);
     } else {
         row0 = offs[b]; box0 = row0 - b;
         n = nb = offs[b + 1] - row0 - 1;
+        if (src_img != nullptr) { const RegionSrc s = src_img[b]; img = s.image; box0 = s.box0; skip = s.skip; }
     }
+    // detector row of output box r
+    auto det_row = [&](int r) { return static_cast<size_t>(box0) + r + (skip >= 0 && r >= skip ? 1 : 0); };
     const int V = n + 1;
     const size_t ld = static_cast<size_t>(split16 ? 3 * Kp : Kp);
     auto put = [&](int row, int i, const float (&x)[8]) {           // 8 columns [8i, 8i+8) of operand row `row`
@@ -186,12 +192,12 @@ region_pack_kernel(const float* __restrict__ box_feats, const float* __restrict_
         const int i = blockIdx.y * blockDim.x + threadIdx.x;           // 8-column group
         if (i * 8 >= F) return;
         float sum[8] = {0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f};
-        const float* src = box_feats + static_cast<size_t>(box0) * F + i * 8;
         for (int r = 0; r < n; ++r) {
             float x[8] = {0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f};
             if (r < nb) {
-                const float4 a = __ldg(reinterpret_cast<const float4*>(src + static_cast<size_t>(r) * F));
-                const float4 c = __ldg(reinterpret_cast<const float4*>(src + static_cast<size_t>(r) * F) + 1);
+                const float* src = box_feats + det_row(r) * F + i * 8;
+                const float4 a = __ldg(reinterpret_cast<const float4*>(src));
+                const float4 c = __ldg(reinterpret_cast<const float4*>(src) + 1);
                 x[0] = a.x; x[1] = a.y; x[2] = a.z; x[3] = a.w; x[4] = c.x; x[5] = c.y; x[6] = c.z; x[7] = c.w;
 #pragma unroll
                 for (int j = 0; j < 8; ++j) sum[j] += x[j];
@@ -204,7 +210,7 @@ region_pack_kernel(const float* __restrict__ box_feats, const float* __restrict_
         put(row0, i, sum);
         return;
     }
-    const float w = image_wh[2 * b], h = image_wh[2 * b + 1];
+    const float w = image_wh[2 * img], h = image_wh[2 * img + 1];
     const float wh = static_cast<float>(static_cast<double>(w) * static_cast<double>(h));     // float(image_w) * float(image_h)
     const int tail_groups = (Kp - F) / 8;
     for (int r = threadIdx.x; r < V; r += blockDim.x) {
@@ -212,7 +218,7 @@ region_pack_kernel(const float* __restrict__ box_feats, const float* __restrict_
         const bool real = r == 0 || r - 1 < nb;
         if (r == 0) { loc[2] = loc[3] = loc[4] = 1.0f; }               // g_location = [0, 0, 1, 1, 1] (worker.py:443)
         else if (real) {
-            const float* bx = boxes + (static_cast<size_t>(box0) + (r - 1)) * 4;
+            const float* bx = boxes + det_row(r - 1) * 4;
             const float x1 = bx[0], y1 = bx[1], x2 = bx[2], y2 = bx[3];
             loc[4] = (y2 - y1) * (x2 - x1) / wh;                       // computed before the coordinates are normalised (worker.py:438)
             loc[0] = x1 / w; loc[1] = y1 / h; loc[2] = x2 / w; loc[3] = y2 / h;
@@ -488,13 +494,37 @@ cudaError_t launch_image_pack(const float* feats, const float* loc, const uint8_
 
 cudaError_t launch_region_pack(const float* box_feats, const float* boxes, const float* image_wh, const int32_t* num_boxes,
                                __nv_bfloat16* a_out, float* mask_add, float* spatials_out, int B, int n, int F, int Kp, int f16,
-                               int split16, cudaStream_t st, const int* offs) {
+                               int split16, cudaStream_t st, const int* offs, const RegionSrc* src) {
     if (B < 1 || (offs == nullptr && n < 1) || F % 8 != 0 || Kp % 8 != 0 || Kp < F + 8 || (split16 && (!f16 || (Kp & 63))) ||
-        (offs != nullptr && (num_boxes != nullptr || split16)))
+        (offs != nullptr && (num_boxes != nullptr || split16)) || (src != nullptr && offs == nullptr))
         return cudaErrorInvalidValue;
     const dim3 grid(B, (F / 8 + 127) / 128 + 1);
     region_pack_kernel<<<grid, 128, 0, st>>>(box_feats, boxes, image_wh, num_boxes, a_out, mask_add, spatials_out, n, F, Kp, f16, split16,
-                                             offs);
+                                             offs, src);
+    return cudaGetLastError();
+}
+
+// Answer ablation's text inputs: variant k's token ids, segment ids and task id copied from its sample's single copy, position
+// `masked` (>= 0) replaced by mask_token, written where the packed text embedding reads variant k (offs[k] - k task_tokens).
+__global__ void __launch_bounds__(128)
+variant_text_kernel(const TextSrc* __restrict__ v, const int* __restrict__ offs, int task_tokens, const int64_t* __restrict__ q,
+                    const int64_t* __restrict__ seg, const int64_t* __restrict__ task, int64_t mask_token, int64_t* __restrict__ q_out,
+                    int64_t* __restrict__ seg_out, int64_t* __restrict__ task_out) {
+    const int k = blockIdx.x;
+    const TextSrc d = v[k];
+    const int out0 = offs[k] - k * task_tokens;
+    for (int t = threadIdx.x; t < d.len; t += blockDim.x) {
+        q_out[out0 + t] = t == d.masked ? mask_token : q[d.first + t];
+        seg_out[out0 + t] = seg[d.first + t];
+    }
+    if (threadIdx.x == 0 && task_tokens) task_out[k] = task[d.sample];
+}
+
+cudaError_t launch_variant_text(const TextSrc* v, int n, const int* offs, int task_tokens, const int64_t* q, const int64_t* seg,
+                                const int64_t* task, int64_t mask_token, int64_t* q_out, int64_t* seg_out, int64_t* task_out,
+                                cudaStream_t st) {
+    if (n < 1 || (task_tokens && (task == nullptr || task_out == nullptr))) return cudaErrorInvalidValue;
+    variant_text_kernel<<<n, 128, 0, st>>>(v, offs, task_tokens, q, seg, task, mask_token, q_out, seg_out, task_out);
     return cudaGetLastError();
 }
 

@@ -16,6 +16,7 @@
 #include <functional>
 #include <map>
 #include <memory>
+#include <numeric>
 #include <stdexcept>
 #include <string>
 #include <utility>
@@ -911,9 +912,10 @@ struct vb200_engine {
     // The calls beside the forward: answer decode's descriptors (pretraining_heads' top-k ones too) and vb200_decode_answers_host's
     // device answers, attention relevance's entry and sample descriptors, region selection's descriptors and workspace (device
     // descriptors, row stats, boxes, bitmasks, max_conf, keep lists), and pre-training's row lists, staged into the RowHeads' d_rows.
-    // The RowHeads never grow, so pre_done alone orders those calls, as a Workspace's `done` does.
-    Workspace dec_ws, ans_ws, rel_ws, sel_ws;
-    Staging dec_in, rel_in, sel_in, pre_in;
+    // The RowHeads never grow, so pre_done alone orders those calls, as a Workspace's `done` does.  Answer ablation: the variant
+    // descriptors (staged through abl_in), the variants' text ids and the head rows of the padded batch.
+    Workspace dec_ws, ans_ws, rel_ws, sel_ws, abl_ws;
+    Staging dec_in, rel_in, sel_in, pre_in, abl_in;
     Event pre_done;
     Stream side_stream;
     Event ev_fork, ev_join;
@@ -1887,10 +1889,11 @@ struct vb200_engine {
     // ---- packed batches (run_packed has staged the call's d_meta ahead of these, in stream order)
     // Packed detector output: the region-pack kernel writes every image's mean row and boxes at the plan's image offsets (the same
     // rows embed_regions writes for that image alone)
+    // (src: answer ablation's per-image sources, see launch_region_pack)
     void pack_regions_packed(Plan& pl, const float* box_feats, const float* boxes, const float* image_wh, float* spatials_out, int rows,
-                             cudaStream_t st) {
+                             cudaStream_t st, const vb::RegionSrc* src = nullptr) {
         CUDA_CHECK(vb::launch_region_pack(box_feats, boxes, image_wh, nullptr, pl.img_a, pl.mask_v, spatials_out, pl.B, 0, cfg.v_feat,
-                                          pl.kp, opt.act_fp16, 0, st, pl.offs_v()));
+                                          pl.kp, opt.act_fp16, 0, st, pl.offs_v(), src));
         zero_tail(pl.img_a, rows, pl.B * pl.V, pl.kp, st);
     }
     // packed pair suffix: every pair's rows are gathered from the packed caption / image states into the plan's packed buffers
@@ -2079,6 +2082,125 @@ struct vb200_engine {
         CUDA_CHECK(vb::launch_attention_relevance(maps, reinterpret_cast<const vb::RelevanceEntry*>(dst), static_cast<int>(n),
                                                   reinterpret_cast<const vb::RelevanceSample*>(dst + eb), batch, max_cols, relevance, st));
         rel_ws.release(st);
+    }
+    // ---- answer ablation: the samples, their ranges and the variant count are checked, and the variants laid out, before anything
+    // is enqueued.  abl_ws holds the variant descriptors (staged through abl_in), the variants' text ids and the padded batch's head rows.
+    void answer_ablation(const vb200_packed_region_inputs* in, const vb200_ablation_msg* msgs, int family, int64_t mask_token,
+                         float* variant_logits, vb200_ablation_score* scores, int slot, cudaStream_t st) {
+        const char* api = "vb200_answer_ablation";
+        if (in == nullptr || msgs == nullptr || variant_logits == nullptr) fail(VB200_ERR_INVALID, "%s: in / msgs / variant_logits is NULL", api);
+        if (x3) fail(VB200_ERR_INVALID, "%s: packed batches are not supported in split_fp32 (fp32x) mode", api);
+        if (pretraining) fail(VB200_ERR_INVALID, "%s: a pre-training engine has no task head to attribute an answer of", api);
+        uint32_t bit = 0;
+        float* vb200_outputs::*field = nullptr;
+        int width = 0;
+        switch (family) {
+            case VB200_DECODE_VQA: bit = VB200_OUT_VIL_PREDICTION; field = &vb200_outputs::vil_prediction; width = num_labels; break;
+            case VB200_DECODE_GQA: bit = VB200_OUT_VIL_PREDICTION_GQA; field = &vb200_outputs::vil_prediction_gqa; width = gqa_labels; break;
+            case VB200_DECODE_SNLI_VE: bit = VB200_OUT_VIL_TRI_PREDICTION; field = &vb200_outputs::vil_tri_prediction; width = 3; break;
+            case VB200_DECODE_NLVR2: fail(VB200_ERR_INVALID, "%s: family NLVR2 is not supported (an answer reads two images)", api);
+            case VB200_DECODE_RETRIEVAL: fail(VB200_ERR_INVALID, "%s: family retrieval is not supported (an answer ranks many images)", api);
+            case VB200_DECODE_GROUNDING:
+                fail(VB200_ERR_INVALID, "%s: family grounding is not supported (the answer is a box a variant may remove)", api);
+            default: fail(VB200_ERR_INVALID, "%s: unknown family %d", api, family);
+        }
+        if (width < 1) fail(VB200_ERR_INVALID, "%s: family %d's head has no columns on this engine", api, family);
+        const int task = cfg.task_tokens ? 1 : 0;
+        if (!in->n_tokens || !in->n_boxes || !in->question || !in->segment_ids || !in->box_features || !in->boxes || !in->image_wh ||
+            (task && !in->task_tokens))
+            fail(VB200_ERR_INVALID, "%s: vb200_packed_region_inputs has a NULL required pointer", api);
+        if (reinterpret_cast<uintptr_t>(in->box_features) & 15) fail(VB200_ERR_INVALID, "%s: box_features is not 16-byte aligned", api);
+        if (mask_token < 0 || mask_token >= cfg.vocab)
+            fail(VB200_ERR_INVALID, "%s: mask_token %lld outside [0, %d)", api, static_cast<long long>(mask_token), cfg.vocab);
+        if (slot < 0 || slot > 15) fail(VB200_ERR_INVALID, "%s: slot %d out of range (0..15)", api, slot);
+        if (slot > 0 && !opt.use_cuda_graph) fail(VB200_ERR_INVALID, "%s: concurrent slots need CUDA-graph plans (use_cuda_graph)", api);
+        // the length rules of vb200_forward_regions_packed, on the samples: every variant is no longer than its sample
+        const BoxRows v = box_rows(api, in->batch, in->n_boxes, in->max_boxes, max_rows);
+        for (int i = 0; i < in->batch; ++i)
+            if (in->n_tokens[i] + task > max_rows)
+                fail(VB200_ERR_INVALID, "%s: image %d has n_tokens %d (T = n_tokens + 1 must be <= %d)", api, i, in->n_tokens[i], max_rows);
+        pack_batch(api, cfg, schedule, {"image", in->batch, in->n_tokens, in->max_tokens, v.v.data(), v.max_regions}, nullptr, max_rows);
+
+        // the variants: text source and masked position, image source and dropped box, lengths, the sample's unablated variant
+        std::vector<vb::TextSrc> text;
+        std::vector<vb::RegionSrc> img;
+        std::vector<int32_t> tin, nv, base, column;
+        auto add = [&](int sample, int tok0, int t, int masked, int box0, int boxes, int skip, int b, int col) {
+            text.push_back({tok0, t, masked, sample});
+            img.push_back({sample, box0, skip});
+            tin.push_back(t);
+            nv.push_back(boxes - (skip >= 0 ? 1 : 0) + 1);
+            base.push_back(b);
+            column.push_back(col);
+        };
+        int64_t count = 0;
+        for (int i = 0, tok0 = 0, box0 = 0; i < in->batch; tok0 += in->n_tokens[i], box0 += in->n_boxes[i], ++i) {
+            const vb200_ablation_msg& m = msgs[i];
+            const int T = in->n_tokens[i], nb = in->n_boxes[i];
+            if (m.answer < -1 || m.answer >= width)
+                fail(VB200_ERR_INVALID, "%s: sample %d has answer %d outside [-1, %d)", api, i, m.answer, width);
+            if (m.token_begin < 0 || m.token_begin > m.token_end || m.token_end > T)
+                fail(VB200_ERR_INVALID, "%s: sample %d has the token range [%d, %d), reversed or outside [0, %d]", api, i, m.token_begin,
+                     m.token_end, T);
+            if (m.box_begin < 0 || m.box_begin > m.box_end || m.box_end > nb)
+                fail(VB200_ERR_INVALID, "%s: sample %d has the box range [%d, %d), reversed or outside [0, %d]", api, i, m.box_begin, m.box_end,
+                     nb);
+            if (m.box_end > m.box_begin && nb < 2)
+                fail(VB200_ERR_INVALID, "%s: sample %d drops a box of an image with %d box (box ablation needs >= 2)", api, i, nb);
+            count += 1 + (m.token_end - m.token_begin) + (m.box_end - m.box_begin);
+            if (count > VB200_ABLATION_MAX_VARIANTS)
+                fail(VB200_ERR_INVALID, "%s: the variants of samples 0..%d number %lld, above %d (split the ranges across calls)", api, i,
+                     static_cast<long long>(count), VB200_ABLATION_MAX_VARIANTS);
+            const int b = static_cast<int>(text.size());
+            add(i, tok0, T, -1, box0, nb, -1, b, m.answer);
+            for (int p = m.token_begin; p < m.token_end; ++p) add(i, tok0, T, p, box0, nb, -1, b, m.answer);
+            for (int j = m.box_begin; j < m.box_end; ++j) add(i, tok0, T, -1, box0, nb, j, b, m.answer);
+        }
+        const int n = static_cast<int>(count), n_pad = (n + 63) / 64 * 64;
+        while (static_cast<int>(text.size()) < n_pad) add(0, 0, 1, -1, 0, 1, -1, 0, 0);     // fillers: sample 0's first token and box
+        const int64_t sum_tin = std::accumulate(tin.begin(), tin.end(), int64_t{0});
+
+        size_t at = 0;
+        auto carve = [&](size_t bytes) { const size_t a = at; at += (bytes + 255) / 256 * 256; return a; };
+        const size_t o_text = carve(n_pad * sizeof(vb::TextSrc)), o_img = carve(n_pad * sizeof(vb::RegionSrc)), staged = at;
+        const size_t o_q = carve(sum_tin * 8), o_seg = carve(sum_tin * 8), o_task = carve(static_cast<size_t>(n_pad) * 8);
+        const size_t o_logits = carve(static_cast<size_t>(n_pad) * width * 4);
+        CUDA_CHECK(cudaSetDevice(opt.device));
+        char* ws = abl_ws.acquire(at, st);
+        abl_in.stage(staged, st, [&](char* h, const auto& put) {
+            memcpy(h + o_text, text.data(), n_pad * sizeof(vb::TextSrc));
+            memcpy(h + o_img, img.data(), n_pad * sizeof(vb::RegionSrc));
+            put(ws, 0, staged);
+        });
+        const auto* text_d = reinterpret_cast<const vb::TextSrc*>(ws + o_text);
+        const auto* img_d = reinterpret_cast<const vb::RegionSrc*>(ws + o_img);
+        int64_t *q = reinterpret_cast<int64_t*>(ws + o_q), *seg = reinterpret_cast<int64_t*>(ws + o_seg);
+        int64_t* tk = reinterpret_cast<int64_t*>(ws + o_task);
+        float* logits = reinterpret_cast<float*>(ws + o_logits);
+        vb200_outputs out{};
+        out.*field = logits;
+        run_packed(api, PACKED, {"variant", n_pad, tin.data(), in->max_tokens, nv.data(), v.max_regions}, bit, slot, &out, {}, st,
+                   [&](Plan& pl, const PackedBatch& b, cudaStream_t s) {
+                       CUDA_CHECK(vb::launch_variant_text(text_d, n_pad, pl.offs_t(), task, in->question, in->segment_ids, in->task_tokens,
+                                                          mask_token, q, seg, tk, s));
+                       embed_text(pl, q, seg, nullptr, tk, b.rows_t(), s);
+                       pack_regions_packed(pl, in->box_features, in->boxes, in->image_wh, nullptr, b.rows_v(), s, img_d);
+                   });
+        if (scores != nullptr) {
+            std::vector<vb::DecodeDesc> d(n);
+            for (int k = 0; k < n; ++k) {
+                d[k].src = logits + static_cast<size_t>(k) * width;
+                d[k].len = width;
+                d[k].top_n = 1;
+                d[k].ref = logits + static_cast<size_t>(base[k]) * width;
+                d[k].score = scores + k;
+                d[k].column = column[k];
+            }
+            CUDA_CHECK(vb::launch_answer_decode(stage_decode(d, st), n, nullptr, st));
+            dec_ws.release(st);
+        }
+        CUDA_CHECK(cudaMemcpyAsync(variant_logits, logits, static_cast<size_t>(n) * width * 4, cudaMemcpyDeviceToDevice, st));
+        abl_ws.release(st);
     }
     // ---- region selection: every descriptor is checked before anything is enqueued
     void select_regions(const vb200_detections* imgs, int n, const vb200_select_params* p, const vb200_selected* out, cudaStream_t st) {
@@ -2472,8 +2594,8 @@ int create_engine(const char* api, bool pretraining, const char* config_json, in
         eng->gemm_kernel = default_gemm_kernel();
         eng->side_stream = make_stream();
         for (Event* e : {&eng->ev_fork, &eng->ev_join, &eng->pre_done}) *e = make_event();
-        for (Staging* s : {&eng->dec_in, &eng->rel_in, &eng->sel_in, &eng->pre_in}) s->copied = make_event();
-        for (Workspace* w : {&eng->dec_ws, &eng->ans_ws, &eng->rel_ws, &eng->sel_ws}) w->done = make_event();
+        for (Staging* s : {&eng->dec_in, &eng->rel_in, &eng->sel_in, &eng->pre_in, &eng->abl_in}) s->copied = make_event();
+        for (Workspace* w : {&eng->dec_ws, &eng->ans_ws, &eng->rel_ws, &eng->sel_ws, &eng->abl_ws}) w->done = make_event();
         eng->ingest(n_tensors, tensors);
         CUDA_CHECK(cudaDeviceSynchronize());
     });
@@ -2731,6 +2853,14 @@ int vb200_attention_relevance(vb200_handle h, const float* attention_probs, int3
     return guard(h, [&] {
         CUDA_CHECK(cudaSetDevice(h->opt.device));
         h->attention_relevance(attention_probs, batch, n_tokens, n_regions, packed, relevance, static_cast<cudaStream_t>(cuda_stream));
+    });
+}
+
+int vb200_answer_ablation(vb200_handle h, const vb200_packed_region_inputs* in, const vb200_ablation_msg* msgs, int32_t family,
+                          int64_t mask_token, float* variant_logits, vb200_ablation_score* scores, int32_t slot, void* cuda_stream) {
+    if (h == nullptr) return VB200_ERR_INVALID;
+    return guard(h, [&] {
+        h->answer_ablation(in, msgs, family, mask_token, variant_logits, scores, slot, static_cast<cudaStream_t>(cuda_stream));
     });
 }
 

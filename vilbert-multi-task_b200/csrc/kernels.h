@@ -105,9 +105,19 @@ cudaError_t launch_image_pack(const float* feats, const float* loc, const uint8_
 // Packed batches (offs != nullptr): offs = device [B + 1] image row offsets (V_b = boxes_b + 1 regions per image), box_features /
 // boxes hold image b's V_b - 1 boxes from detector row offs[b] - b, every row is real, n and num_boxes are unused (num_boxes must be
 // null, and split16 0), spatials_out is [offs[B], 5].
+// src (packed only, answer ablation): output image b is image src[b].image's offs[b+1] - offs[b] - 1 + (skip >= 0) detector boxes
+// from row src[b].box0, box src[b].skip left out (-1: none).
+struct RegionSrc { int32_t image, box0, skip; };
 cudaError_t launch_region_pack(const float* box_feats, const float* boxes, const float* image_wh, const int32_t* num_boxes,
                                __nv_bfloat16* a_out, float* mask_add, float* spatials_out, int B, int n, int F, int Kp, int f16,
-                               int split16, cudaStream_t st, const int* offs = nullptr);
+                               int split16, cudaStream_t st, const int* offs = nullptr, const RegionSrc* src = nullptr);
+// Answer ablation's text ids: variant k (one CTA each, n of them) = tokens [first, first + len) of the packed question / segment
+// ids, position `masked` (-1: none) replaced by mask_token, and task id task[sample] -> the packed layout of the plan's text
+// offsets offs (device [n + 1]) in q_out / seg_out / task_out.
+struct TextSrc { int32_t first, len, masked, sample; };
+cudaError_t launch_variant_text(const TextSrc* v, int n, const int* offs, int task_tokens, const int64_t* q, const int64_t* seg,
+                                const int64_t* task, int64_t mask_token, int64_t* q_out, int64_t* seg_out, int64_t* task_out,
+                                cudaStream_t st);
 // retrieval reuse: cached encoder state rows idx[b] -> sample b of a pair plan (fp32 stream [L, H], 16-bit operand [L, H16], mask [L]);
 // the fp32 and mask copies are skipped when their pointers are null (packed poolers: the first 16-bit row of every sample)
 cudaError_t launch_gather_state(const int32_t* idx, int n_src, const float* src_f32, const void* src_16, const float* src_mask,
@@ -173,11 +183,17 @@ cudaError_t launch_rowdot(const float* x, int ld_x, const float* W, const float*
 // Answer decode (decode.cu, vb200_decode_answers): message b's softmax over the `len` logits at src, its top_n (<= 10)
 // probabilities and indices, and for grounding (spatials != null: the segment's first [len, 5] spatials row) the pixel boxes of
 // the picked rows.  One CTA per message; the descriptors are resolved and bounds-checked on the host.
+// Answer ablation (score != null, top_n 1): the CTA writes *score instead of an answer -- column `column` of src, or for column -1
+// the top-1 of the `len` logits at ref (the sample's unablated row, recomputed by every CTA), with its probability in src, and src's
+// own top-1; answers may then be null.
 struct DecodeDesc {
     const float* src;
     const float* spatials;
     double image_w, image_h;
     int len, top_n;
+    const float* ref;
+    vb200_ablation_score* score;
+    int column;
 };
 cudaError_t launch_answer_decode(const DecodeDesc* descs, int n, vb200_answer* answers, cudaStream_t st);
 // Attention relevance (relevance.cu, vb200_attention_relevance): per sample b (one CTA) the rollout rows of the text CLS row and the

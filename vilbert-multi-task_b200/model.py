@@ -76,6 +76,76 @@ def packed_offsets(lengths, extra: int = 0):
     return offs
 
 
+# the families whose answer is one row of one image (vb200_answer_ablation)
+ABLATION_FAMILIES = {"vqa": L.DECODE_VQA, "gqa": L.DECODE_GQA, "snli_ve": L.DECODE_SNLI_VE}
+
+
+def ablation_ranges(n_tokens, n_boxes, tokens=None, boxes_range=None):
+    """Each sample's (token_begin, token_end, box_begin, box_end) for answer ablation.  By default the question positions
+    1 .. Tin - 2 are masked (the [CLS] and [SEP] kept) and every box of an image with at least two boxes is dropped.  ``tokens`` /
+    ``boxes_range``: None (the default), one (begin, end) pair for every sample, or a list of one pair or None per sample."""
+    n = len(n_tokens)
+
+    def per_sample(r, name):
+        if r is None:
+            return [None] * n
+        if len(r) == 2 and all(isinstance(x, int) for x in r):
+            return [tuple(r)] * n
+        if len(r) != n:
+            raise ValueError(f"answer_ablation: {name} needs one (begin, end) pair, or one per sample ({n}), got {len(r)} entries")
+        return [None if x is None else tuple(x) for x in r]
+
+    tk, bx = per_sample(tokens, "tokens"), per_sample(boxes_range, "boxes_range")
+    out = []
+    for i, (tin, nb) in enumerate(zip(n_tokens, n_boxes)):
+        tb, te = tk[i] if tk[i] is not None else (1, max(1, tin - 1))
+        bb, be = bx[i] if bx[i] is not None else (0, nb if nb >= 2 else 0)
+        if not 0 <= tb <= te <= tin:
+            raise ValueError(f"answer_ablation: sample {i} has the token range [{tb}, {te}), reversed or outside [0, {tin}]")
+        if not 0 <= bb <= be <= nb:
+            raise ValueError(f"answer_ablation: sample {i} has the box range [{bb}, {be}), reversed or outside [0, {nb}]")
+        if be > bb and nb < 2:
+            raise ValueError(f"answer_ablation: sample {i} drops a box of an image with {nb} box (box ablation needs >= 2)")
+        out.append((int(tb), int(te), int(bb), int(be)))
+    return out
+
+
+def ablation_calls(ranges, cap: int = L.ABLATION_MAX_VARIANTS):
+    """The engine calls for these per-sample ranges: each call a list of (sample, (token_begin, token_end, box_begin, box_end))
+    pieces whose variants (1 + tokens + boxes each) number at most ``cap``.  A batch is split at sample boundaries; a sample with more
+    than ``cap`` variants is split into pieces of its units (tokens first, then boxes), each with its own unablated variant."""
+    pieces = []
+    for i, (tb, te, bb, be) in enumerate(ranges):
+        units = [("t", p) for p in range(tb, te)] + [("b", j) for j in range(bb, be)]
+        for c in range(0, max(len(units), 1), cap - 1):
+            chunk = units[c:c + cap - 1]
+            toks = [p for k, p in chunk if k == "t"]
+            bxs = [j for k, j in chunk if k == "b"]
+            r = (toks[0], toks[-1] + 1) if toks else (0, 0)
+            r += (bxs[0], bxs[-1] + 1) if bxs else (0, 0)
+            pieces.append((i, r))
+    calls, size = [], cap
+    for i, r in pieces:
+        k = 1 + (r[1] - r[0]) + (r[3] - r[2])
+        if size + k > cap:
+            calls.append([])
+            size = 0
+        calls[-1].append((i, r))
+        size += k
+    return calls
+
+
+def ablation_variants(call):
+    """The variants of one engine call in the engine's order: (sample, kind, unit) with kind "base" (unit None), "token" (the masked
+    position) or "box" (the dropped box)."""
+    out = []
+    for i, (tb, te, bb, be) in call:
+        out.append((i, "base", None))
+        out += [(i, "token", p) for p in range(tb, te)]
+        out += [(i, "box", j) for j in range(bb, be)]
+    return out
+
+
 def attention_list(kinds, layout_entry, entries):
     """The reference's attn_data_list from the maps of the selected entries: ``kinds`` / ``layout_entry`` are the full entry list's
     kinds and each entry's index in ``entries`` (-1: not selected) as ``attention_selection`` returns them.  One position per layer in
@@ -795,6 +865,96 @@ class VILBertForVLTasks(object):
         for k, t in outs.items():
             setattr(o, k, t.data_ptr())
         return outs, o
+
+    # ------------------------------------------------------------------ answer ablation
+    @torch.no_grad()
+    def answer_ablation(self, question, segment_ids, task_tokens, box_features, boxes, image_wh, n_tokens, n_boxes, family="vqa",
+                        answer=None, tokens=None, boxes_range=None, mask_token: int = 103, max_tokens: int = 0, max_boxes: int = 0,
+                        slot: int = 0, return_logits: bool = False):
+        """How much each question token and each detector box holds up an answer (vb200_answer_ablation): for every image of a
+        packed detector-output batch (the inputs of ``forward_regions_packed``), the answer's probability with each question position
+        replaced by ``mask_token`` in turn and with each box dropped in turn, every variant a forward of the engine built and scored
+        on the device.  ``family``: "vqa", "gqa" or "snli_ve" (or the ``_lib.DECODE_*`` value).  ``answer``: None (each sample's
+        unablated top-1), one column for every sample, or a list with one column (or None) per sample.  ``tokens`` / ``boxes_range``:
+        see ``ablation_ranges`` (default: positions 1 .. Tin - 2 and every box).  Batches above the engine's 1024 variants per call
+        are split across calls (``ablation_calls``).
+        Returns one dict per sample: ``answer`` (the attributed column), ``prob`` / ``top1`` / ``top1_prob`` of the unablated input,
+        ``tokens`` / ``boxes`` (the ablated positions and boxes) with ``token_prob`` / ``box_prob`` (the answer's probability without
+        that unit) and ``token_top1`` / ``box_top1`` (the variant's own top-1), CPU tensors; with ``return_logits`` also ``logits``,
+        a device tensor [1 + tokens + boxes, width] in that variant order."""
+        nt, nb = _host_ints(n_tokens), _host_ints(n_boxes)
+        B = len(nt)
+        if len(nb) != B or B < 1:
+            raise ValueError("answer_ablation: n_tokens and n_boxes must have the same, positive length")
+        fam = ABLATION_FAMILIES.get(family, 0) if isinstance(family, str) else int(family)
+        if fam not in ABLATION_FAMILIES.values():
+            raise ValueError(f"answer_ablation: family {family!r} is not one of {sorted(ABLATION_FAMILIES)} (NLVR2, retrieval and "
+                             "grounding answers are not ablated)")
+        if answer is None or isinstance(answer, int):
+            answers = [-1 if answer is None else int(answer)] * B
+        else:
+            answers = [-1 if a is None else int(a) for a in answer]
+            if len(answers) != B:
+                raise ValueError(f"answer_ablation: answer has {len(answers)} entries for {B} samples")
+        if any(a < -1 for a in answers):
+            raise ValueError("answer_ablation: an answer column must be >= 0 (or None / -1: the unablated top-1)")
+        calls = ablation_calls(ablation_ranges(nt, nb, tokens, boxes_range))
+        device = self._engine_device()
+        d = self._dims
+        width = {L.DECODE_VQA: d["num_labels"], L.DECODE_GQA: d["gqa_labels"], L.DECODE_SNLI_VE: 3}[fam]
+        F = d["v_feature_size"]
+        q = _to_device(question, torch.int64, device).reshape(-1)
+        seg = _to_device(segment_ids if segment_ids is not None else torch.zeros_like(q), torch.int64, device).reshape(-1)
+        tk = _task_rows(task_tokens if task_tokens is not None else torch.zeros(B, 1, dtype=torch.int64), B, device)
+        bf = _to_device(box_features, torch.float32, device).reshape(-1, F)
+        bx = _to_device(boxes, torch.float32, device).reshape(-1, 4)
+        wh = _to_device(image_wh, torch.float32, device)
+        t_off, b_off = packed_offsets(nt), packed_offsets(nb)
+        if q.numel() != t_off[-1] or seg.numel() != t_off[-1] or bf.shape[0] != b_off[-1] or bx.shape[0] != b_off[-1] \
+                or tuple(wh.shape) != (B, 2):
+            raise ValueError("answer_ablation: question / segment_ids need sum(n_tokens) entries, box_features / boxes sum(n_boxes) "
+                             "rows, image_wh [B, 2]")
+        res = [dict(tokens=[], token_prob=[], token_top1=[], boxes=[], box_prob=[], box_top1=[], logits=[]) for _ in range(B)]
+        for call in calls:
+            samples = [i for i, _ in call]
+            if len(calls) == 1:
+                cq, cseg, ctk, cbf, cbx, cwh = q, seg, tk, bf, bx, wh
+            else:                            # this call's samples (or pieces of one), packed back to back
+                tcat = lambda t: torch.cat([t[t_off[i]:t_off[i + 1]] for i in samples])
+                bcat = lambda t: torch.cat([t[b_off[i]:b_off[i + 1]] for i in samples])
+                cq, cseg, cbf, cbx = tcat(q), tcat(seg), bcat(bf), bcat(bx)
+                ctk, cwh = tk[samples].contiguous(), wh[samples].contiguous()
+            msgs = (L.AblationMsg * len(call))(*[L.AblationMsg(answers[i], *r) for i, r in call])
+            variants = ablation_variants(call)
+            logits = torch.empty(len(variants), width, dtype=torch.float32, device=device)
+            scores = torch.empty(len(variants), 4, dtype=torch.int32, device=device)       # vb200_ablation_score
+            inp = L.PackedRegionInputs(len(call), int(max_tokens), int(max_boxes), _int32s([nt[i] for i in samples]),
+                                       _int32s([nb[i] for i in samples]), cq.data_ptr(), cseg.data_ptr(), ctk.data_ptr(), cbf.data_ptr(),
+                                       cbx.data_ptr(), cwh.data_ptr(), None)
+            self._call("vb200_answer_ablation", C.byref(inp), msgs, fam, int(mask_token), logits.data_ptr(), scores.data_ptr(), int(slot))
+            sc = scores.cpu()
+            col, top1 = sc[:, 0].tolist(), sc[:, 2].tolist()
+            prob, top1_prob = sc[:, 1].view(torch.float32).tolist(), sc[:, 3].view(torch.float32).tolist()
+            for k, (i, kind, unit) in enumerate(variants):
+                r = res[i]
+                if kind == "base":
+                    if "answer" not in r:
+                        r.update(answer=col[k], prob=prob[k], top1=top1[k], top1_prob=top1_prob[k])
+                        r["logits"].append(logits[k:k + 1])
+                    continue
+                r["tokens" if kind == "token" else "boxes"].append(unit)
+                r[kind + "_prob"].append(prob[k])
+                r[kind + "_top1"].append(top1[k])
+                r["logits"].append(logits[k:k + 1])
+        for r in res:
+            for k in ("token_prob", "box_prob"):
+                r[k] = torch.tensor(r[k], dtype=torch.float32)
+            for k in ("token_top1", "box_top1"):
+                r[k] = torch.tensor(r[k], dtype=torch.int64)
+            logits = r.pop("logits")
+            if return_logits:
+                r["logits"] = torch.cat(logits)
+        return res
 
     # ------------------------------------------------------------------ answer decode (worker.py:295-386)
     def decode_answers(self, out, messages, spatials=None):
