@@ -572,6 +572,59 @@ int vb200_answer_ablation(vb200_handle h, const vb200_packed_region_inputs* in, 
                           int32_t family, int64_t mask_token, float* variant_logits, vb200_ablation_score* scores, int32_t slot,
                           void* cuda_stream);
 
+/* ---- Message ablation: answer ablation for every decode family, the answers of several images included.  The batch is a packed
+ * detector-output batch laid out as the worker lays it out for vb200_forward_regions_packed (the text repeated per image, an NLVR2
+ * pair on an even sample); each message names one answer by its images and is ablated one unit at a time.
+ *   Message m reads samples [image_begin, image_begin + n_images) of the batch: VQA / GQA / SNLI-VE and grounding 1 image, NLVR2 2,
+ *   retrieval K >= 1.  Its question, segment ids and task id are image_begin's (the other samples' text is not read).  Its segment
+ *   is what vb200_decode_answers reads for it: the head row (width num_labels / gqa_labels / 3), the pair's vil_binary_prediction row
+ *   (2), the K vil_logit values (K), or the image's vision_logit rows, the global row first (n_boxes + 1).  answer: an index in the
+ *   segment (-1: the unablated top-1).  Boxes are numbered across the message's images in order.
+ *   Variants of message m, in this order: the unablated input; each masked question position of [token_begin, token_end) (every
+ *   image of the message with the masked question); each dropped box of [box_begin, box_end).  A dropped box runs both images for
+ *   NLVR2 (the pair head reads adjacent pooled rows) and only the changed image otherwise: a retrieval box variant's segment is the
+ *   unablated segment with element k (the changed image) replaced by that sample's vil_logit, exact because a packed sample's outputs
+ *   do not depend on its neighbours; a grounding box variant's segment has n_boxes rows.
+ *   vb200_message_ablation_layout owns the variant order: it writes one vb200_ablation_variant per variant (variants HOST, or NULL
+ *   for the counts alone) and the totals: variants, floats of variant_logits and forward samples.  It checks the messages against
+ *   the lengths as vb200_message_ablation does, without the sample cap.
+ *   variant_logits (DEVICE, required): the segments back to back in layout order.  Bit-identity: every segment equals the same
+ *   floats of vb200_forward_regions_packed run on that variant's input in the worker's layout (a retrieval box variant: all K images).
+ *   scores (DEVICE, optional): one vb200_ablation_score per variant, with the arithmetic of vb200_answer_ablation.  Grounding reports
+ *   answer and top1 in the unablated image's row numbering (a row after the dropped box maps back by +1); a variant that drops the
+ *   attributed box reports answer -1 and prob 0.
+ * The forward samples (at most VB200_ABLATION_MAX_VARIANTS per call; NLVR2 variants first, so each pair starts on an even sample) run
+ * as one forward of the PACKED plan, rounded up to a multiple of 64 with fillers.  The plan selects the five pooled task heads, and
+ * vision_logit as well when a message is a grounding message, so a server keeps at most two plans per bucket and capacities.
+ * VB200_ERR_INVALID, with nothing enqueued, no output written and a message naming the message, for: split_fp32 and pre-training
+ * engines; n_msgs < 1; an unknown family; n_images wrong for the family; an image range outside the batch; answer outside [-1,
+ * segment length); a token range outside [0, Tin] or a box range outside [0, the message's boxes], or reversed; dropping a box of an
+ * image with fewer than 2 boxes; mask_token outside [0, vocab); more than VB200_ABLATION_MAX_VARIANTS samples; NULL required pointers;
+ * box_features not 16-byte aligned; and every length rule of vb200_forward_regions_packed.
+ * Asynchronous and stream-ordered as vb200_answer_ablation. */
+typedef struct {
+    int32_t family;                   /* VB200_DECODE_* */
+    int32_t image_begin, n_images;    /* the message's images: samples [image_begin, image_begin + n_images) of the batch */
+    int32_t answer;                   /* attributed index in the message's segment; -1: the unablated top-1 */
+    int32_t token_begin, token_end;   /* mask question positions [token_begin, token_end) of image_begin's Tin ids, one at a time */
+    int32_t box_begin, box_end;       /* drop boxes [box_begin, box_end), numbered across the message's images in order, one at a time */
+} vb200_ablation_message;
+
+typedef struct {
+    int32_t message, kind, unit;      /* kind 0: the unablated input (unit -1); 1: masked position `unit`; 2: dropped box `unit` */
+    int32_t samples;                  /* forward samples this variant runs */
+    int64_t offset;                   /* its segment: floats [offset, offset + length) of variant_logits */
+    int32_t length;
+} vb200_ablation_variant;
+
+int vb200_message_ablation_layout(vb200_handle h, int32_t batch, const int32_t* n_tokens /* HOST [batch] */,
+                                  const int32_t* n_boxes /* HOST [batch] */, const vb200_ablation_message* msgs /* HOST [n_msgs] */,
+                                  int32_t n_msgs, vb200_ablation_variant* variants /* HOST, NULL: counts only */, int64_t* n_variants,
+                                  int64_t* n_floats, int64_t* n_samples);
+int vb200_message_ablation(vb200_handle h, const vb200_packed_region_inputs* in, const vb200_ablation_message* msgs /* HOST [n_msgs] */,
+                           int32_t n_msgs, int64_t mask_token, float* variant_logits, vb200_ablation_score* scores, int32_t slot,
+                           void* cuda_stream);
+
 /* ---- Detector-region selection: the feature extraction step of the reference worker (worker.py:123-176) on the detector's raw heads,
  * for every image of a batch in one call, written straight into the packed box_features / boxes that vb200_forward_regions_packed reads.
  * For image i with n_i proposals, C score columns (column 0 is background) and features [n_i, F]:

@@ -124,6 +124,20 @@ class AblationScore(C.Structure):
     _fields_ = [("answer", C.c_int32), ("prob", C.c_float), ("top1", C.c_int32), ("top1_prob", C.c_float)]
 
 
+class AblationMessage(C.Structure):
+    """vb200_ablation_message: one answer of any decode family by its images, the attributed index in its segment (-1: the
+    unablated top-1) and the token and box ranges ablated one unit at a time (boxes numbered across the message's images)."""
+    _fields_ = [("family", C.c_int32), ("image_begin", C.c_int32), ("n_images", C.c_int32), ("answer", C.c_int32),
+                ("token_begin", C.c_int32), ("token_end", C.c_int32), ("box_begin", C.c_int32), ("box_end", C.c_int32)]
+
+
+class AblationVariant(C.Structure):
+    """vb200_ablation_variant: one variant in the engine's order -- its message, kind (0 unablated, 1 masked position, 2 dropped
+    box) and unit, the forward samples it runs and its segment [offset, offset + length) of variant_logits."""
+    _fields_ = [("message", C.c_int32), ("kind", C.c_int32), ("unit", C.c_int32), ("samples", C.c_int32), ("offset", C.c_int64),
+                ("length", C.c_int32)]
+
+
 class Detections(C.Structure):
     """vb200_detections: one image's raw detector heads (device pointers) and its first output row."""
     _fields_ = [("n_proposals", C.c_int32), ("dst_row", C.c_int32), ("im_scale", C.c_double), ("proposals", C.c_void_p),
@@ -180,7 +194,8 @@ EXPORTS = ["vb200_abi_version", "vb200_create", "vb200_destroy", "vb200_last_err
            "vb200_self_attention_stream", "vb200_co_attention_stream",
            "vb200_linear_product", "vb200_text_embed", "vb200_image_pack", "vb200_region_pack", "vb200_rowdot", "vb200_gather_state",
            "vb200_gather_packed_state", "vb200_decode_answers", "vb200_decode_answers_host", "vb200_select_regions",
-           "vb200_pretraining_heads", "vb200_create_pretraining", "vb200_pretraining_objectives", "vb200_answer_ablation"]
+           "vb200_pretraining_heads", "vb200_create_pretraining", "vb200_pretraining_objectives", "vb200_answer_ablation",
+           "vb200_message_ablation_layout", "vb200_message_ablation"]
 
 _lib = None
 
@@ -265,6 +280,9 @@ def load():
     lib.vb200_create_pretraining.argtypes = lib.vb200_create.argtypes
     lib.vb200_pretraining_objectives.argtypes = [vp, C.POINTER(PretrainRows), C.POINTER(PretrainTargets), C.POINTER(PretrainLosses), vp]
     lib.vb200_answer_ablation.argtypes = [vp, C.POINTER(PackedRegionInputs), C.POINTER(AblationMsg), i32, i64, vp, vp, i32, vp]
+    lib.vb200_message_ablation_layout.argtypes = [vp, i32, vp, vp, C.POINTER(AblationMessage), i32, vp, C.POINTER(C.c_int64),
+                                                  C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
+    lib.vb200_message_ablation.argtypes = [vp, C.POINTER(PackedRegionInputs), C.POINTER(AblationMessage), i32, i64, vp, vp, i32, vp]
     for name in EXPORTS:
         if name not in ("vb200_last_error",):
             getattr(lib, name).restype = C.c_int

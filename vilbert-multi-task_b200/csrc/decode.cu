@@ -89,16 +89,21 @@ answer_decode_kernel(const DecodeDesc* __restrict__ descs, vb200_answer* __restr
     if (d.score != nullptr) {                         // answer ablation: one score, no answer
         const unsigned long long top1 = s_pick[0];
         int col = d.column;
-        if (col < 0) {                                // the unablated row's top-1, as its own decode ranks it
-            const float2 ref = softmax_stats(d.ref, d.len, s_f);
-            pick_top(d.ref, d.len, ref, 1, s_k, s_pick);
+        if (col < 0) {                                // the unablated segment's top-1, as its own decode ranks it
+            const int ref_len = d.len + (d.drop >= 0 ? 1 : 0);
+            const float2 ref = softmax_stats(d.ref, ref_len, s_f);
+            pick_top(d.ref, ref_len, ref, 1, s_k, s_pick);
             col = key_index(s_pick[0]);
         }
         if (tid == 0) {
+            // a dropped row: the attributed row of the unablated numbering maps into src, or is gone
+            const bool gone = d.drop >= 0 && col == d.drop;
+            const int at = d.drop >= 0 && col > d.drop ? col - 1 : col;
+            const int t = key_index(top1);
             vb200_ablation_score sc;
-            sc.answer = col;
-            sc.prob = expf(x[col] - ms.x) / ms.y;
-            sc.top1 = key_index(top1);
+            sc.answer = gone ? -1 : col;
+            sc.prob = gone ? 0.f : expf(x[at] - ms.x) / ms.y;
+            sc.top1 = d.drop >= 0 && t >= d.drop ? t + 1 : t;
             sc.top1_prob = __uint_as_float(static_cast<unsigned>(top1 >> 32));
             *d.score = sc;
         }
@@ -126,6 +131,24 @@ answer_decode_kernel(const DecodeDesc* __restrict__ descs, vb200_answer* __restr
 
 cudaError_t launch_answer_decode(const DecodeDesc* descs, int n, vb200_answer* answers, cudaStream_t st) {
     return launch_ex(answer_decode_kernel, dim3(n), dim3(kDecodeThreads), 0, 0, st, descs, answers);
+}
+
+__global__ void __launch_bounds__(128)
+segment_gather_kernel(const SegmentDesc* __restrict__ descs, const __grid_constant__ SegmentHeads heads, float* __restrict__ out) {
+    const SegmentDesc d = descs[blockIdx.x];
+    const float* __restrict__ p = heads.p[d.head];
+    const int64_t ld = heads.ld[d.head];
+    const bool run = heads.cols[d.head] == 1;         // a one-column head: the segment is a run of rows
+    float* __restrict__ dst = out + d.dst;
+    for (int i = threadIdx.x; i < d.len; i += blockDim.x) {
+        const int64_t at = i == d.sub ? d.sub_row * ld : run ? (d.row + i) * ld : d.row * ld + i;
+        dst[i] = p[at];
+    }
+}
+
+cudaError_t launch_segment_gather(const SegmentDesc* descs, int n, const SegmentHeads& heads, float* out, cudaStream_t st) {
+    if (n < 1) return cudaErrorInvalidValue;
+    return launch_ex(segment_gather_kernel, dim3(n), dim3(128), 0, 0, st, descs, heads, out);
 }
 
 }  // namespace vb

@@ -912,8 +912,8 @@ struct vb200_engine {
     // The calls beside the forward: answer decode's descriptors (pretraining_heads' top-k ones too) and vb200_decode_answers_host's
     // device answers, attention relevance's entry and sample descriptors, region selection's descriptors and workspace (device
     // descriptors, row stats, boxes, bitmasks, max_conf, keep lists), and pre-training's row lists, staged into the RowHeads' d_rows.
-    // The RowHeads never grow, so pre_done alone orders those calls, as a Workspace's `done` does.  Answer ablation: the variant
-    // descriptors (staged through abl_in), the variants' text ids and the head rows of the padded batch.
+    // The RowHeads never grow, so pre_done alone orders those calls, as a Workspace's `done` does.  Answer and message ablation:
+    // the sample and segment descriptors (staged through abl_in) and the samples' text ids.
     Workspace dec_ws, ans_ws, rel_ws, sel_ws, abl_ws;
     Staging dec_in, rel_in, sel_in, pre_in, abl_in;
     Event pre_done;
@@ -1953,9 +1953,10 @@ struct vb200_engine {
     }
     // What every packed entry point shares once it has checked its own inputs: the engine-wide rejections, the call's rows
     // (pack_batch), its plan, the d_meta staged ahead of `input` (the call's input kernels), the plan and then, for the forwards
-    // (out != null), the outputs at the call's row totals or, for the prefixes, the state of the call's rows.
-    void run_packed(const char* api, int mode, const PackedLengths& len, uint32_t select, int slot, const vb200_outputs* out,
-                    const PrefixState& state, void* cuda_stream, const std::function<void(Plan&, const PackedBatch&, cudaStream_t)>& input) {
+    // (out != null), the outputs at the call's row totals or, for the prefixes, the state of the call's rows.  Returns the plan,
+    // whose outputs stay valid in stream order until the plan's next run.
+    Plan& run_packed(const char* api, int mode, const PackedLengths& len, uint32_t select, int slot, const vb200_outputs* out,
+                     const PrefixState& state, void* cuda_stream, const std::function<void(Plan&, const PackedBatch&, cudaStream_t)>& input) {
         if (select & VB200_OUT_ATTENTION)
             fail(VB200_ERR_INVALID, "%s: the attention-probability output (VB200_OUT_ATTENTION) is not supported", api);
         if (mode != PACKED) reject_packed_attention(select, api);
@@ -1976,6 +1977,7 @@ struct vb200_engine {
         run_plan(pl, st);
         if (out != nullptr) copy_outputs(pl, *out, st, cudaMemcpyDeviceToDevice, b.rows_t(), b.rows_v());
         else copy_state(pl, mode == PACKED_TEXT_PREFIX, mode == PACKED_TEXT_PREFIX ? b.rows_t() : b.rows_v(), state, st);
+        return pl;
     }
     // meta (host, in the plan's d_meta layout) -> d_meta, in stream order ahead of the plan's kernels
     void stage_meta(Plan& pl, const std::vector<int>& meta, cudaStream_t st) {
@@ -2083,28 +2085,11 @@ struct vb200_engine {
                                                   reinterpret_cast<const vb::RelevanceSample*>(dst + eb), batch, max_cols, relevance, st));
         rel_ws.release(st);
     }
-    // ---- answer ablation: the samples, their ranges and the variant count are checked, and the variants laid out, before anything
-    // is enqueued.  abl_ws holds the variant descriptors (staged through abl_in), the variants' text ids and the padded batch's head rows.
-    void answer_ablation(const vb200_packed_region_inputs* in, const vb200_ablation_msg* msgs, int family, int64_t mask_token,
-                         float* variant_logits, vb200_ablation_score* scores, int slot, cudaStream_t st) {
-        const char* api = "vb200_answer_ablation";
-        if (in == nullptr || msgs == nullptr || variant_logits == nullptr) fail(VB200_ERR_INVALID, "%s: in / msgs / variant_logits is NULL", api);
-        if (x3) fail(VB200_ERR_INVALID, "%s: packed batches are not supported in split_fp32 (fp32x) mode", api);
-        if (pretraining) fail(VB200_ERR_INVALID, "%s: a pre-training engine has no task head to attribute an answer of", api);
-        uint32_t bit = 0;
-        float* vb200_outputs::*field = nullptr;
-        int width = 0;
-        switch (family) {
-            case VB200_DECODE_VQA: bit = VB200_OUT_VIL_PREDICTION; field = &vb200_outputs::vil_prediction; width = num_labels; break;
-            case VB200_DECODE_GQA: bit = VB200_OUT_VIL_PREDICTION_GQA; field = &vb200_outputs::vil_prediction_gqa; width = gqa_labels; break;
-            case VB200_DECODE_SNLI_VE: bit = VB200_OUT_VIL_TRI_PREDICTION; field = &vb200_outputs::vil_tri_prediction; width = 3; break;
-            case VB200_DECODE_NLVR2: fail(VB200_ERR_INVALID, "%s: family NLVR2 is not supported (an answer reads two images)", api);
-            case VB200_DECODE_RETRIEVAL: fail(VB200_ERR_INVALID, "%s: family retrieval is not supported (an answer ranks many images)", api);
-            case VB200_DECODE_GROUNDING:
-                fail(VB200_ERR_INVALID, "%s: family grounding is not supported (the answer is a box a variant may remove)", api);
-            default: fail(VB200_ERR_INVALID, "%s: unknown family %d", api, family);
-        }
-        if (width < 1) fail(VB200_ERR_INVALID, "%s: family %d's head has no columns on this engine", api, family);
+    // ---- answer and message ablation.  Both entry points check their inputs, describe every variant as a message ablation layout
+    // (AblLayout) and run it through run_ablation: one packed forward of every variant's samples, one segment gather, one scoring.
+    // The rejections every ablation call shares: the batch's pointers, mask_token, slot and the length rules of
+    // vb200_forward_regions_packed on the samples (every variant is no longer than its samples).  Returns the region capacity.
+    int check_ablation_inputs(const char* api, const vb200_packed_region_inputs* in, int64_t mask_token, int slot) const {
         const int task = cfg.task_tokens ? 1 : 0;
         if (!in->n_tokens || !in->n_boxes || !in->question || !in->segment_ids || !in->box_features || !in->boxes || !in->image_wh ||
             (task && !in->task_tokens))
@@ -2114,93 +2099,284 @@ struct vb200_engine {
             fail(VB200_ERR_INVALID, "%s: mask_token %lld outside [0, %d)", api, static_cast<long long>(mask_token), cfg.vocab);
         if (slot < 0 || slot > 15) fail(VB200_ERR_INVALID, "%s: slot %d out of range (0..15)", api, slot);
         if (slot > 0 && !opt.use_cuda_graph) fail(VB200_ERR_INVALID, "%s: concurrent slots need CUDA-graph plans (use_cuda_graph)", api);
-        // the length rules of vb200_forward_regions_packed, on the samples: every variant is no longer than its sample
         const BoxRows v = box_rows(api, in->batch, in->n_boxes, in->max_boxes, max_rows);
         for (int i = 0; i < in->batch; ++i)
             if (in->n_tokens[i] + task > max_rows)
                 fail(VB200_ERR_INVALID, "%s: image %d has n_tokens %d (T = n_tokens + 1 must be <= %d)", api, i, in->n_tokens[i], max_rows);
         pack_batch(api, cfg, schedule, {"image", in->batch, in->n_tokens, in->max_tokens, v.v.data(), v.max_regions}, nullptr, max_rows);
-
-        // the variants: text source and masked position, image source and dropped box, lengths, the sample's unablated variant
+        return v.max_regions;
+    }
+    // One variant: its layout record, where its segment is gathered from (seg.dst = rec.offset), and its score -- against the
+    // message's unablated variant `base`, index `column`, without segment row `drop` (-1: none).
+    struct AblVariant { vb200_ablation_variant rec; vb::SegmentDesc seg; int base, column, drop; };
+    // The variants in layout order and the forward samples they run: text and image sources, lengths.  NLVR2 variants take the first
+    // samples, two each, so every pair starts on an even sample with no filler.
+    struct AblLayout {
+        std::vector<AblVariant> v;
         std::vector<vb::TextSrc> text;
         std::vector<vb::RegionSrc> img;
-        std::vector<int32_t> tin, nv, base, column;
-        auto add = [&](int sample, int tok0, int t, int masked, int box0, int boxes, int skip, int b, int col) {
-            text.push_back({tok0, t, masked, sample});
-            img.push_back({sample, box0, skip});
-            tin.push_back(t);
-            nv.push_back(boxes - (skip >= 0 ? 1 : 0) + 1);
-            base.push_back(b);
-            column.push_back(col);
-        };
-        int64_t count = 0;
-        for (int i = 0, tok0 = 0, box0 = 0; i < in->batch; tok0 += in->n_tokens[i], box0 += in->n_boxes[i], ++i) {
-            const vb200_ablation_msg& m = msgs[i];
-            const int T = in->n_tokens[i], nb = in->n_boxes[i];
-            if (m.answer < -1 || m.answer >= width)
-                fail(VB200_ERR_INVALID, "%s: sample %d has answer %d outside [-1, %d)", api, i, m.answer, width);
-            if (m.token_begin < 0 || m.token_begin > m.token_end || m.token_end > T)
-                fail(VB200_ERR_INVALID, "%s: sample %d has the token range [%d, %d), reversed or outside [0, %d]", api, i, m.token_begin,
-                     m.token_end, T);
-            if (m.box_begin < 0 || m.box_begin > m.box_end || m.box_end > nb)
-                fail(VB200_ERR_INVALID, "%s: sample %d has the box range [%d, %d), reversed or outside [0, %d]", api, i, m.box_begin, m.box_end,
-                     nb);
-            if (m.box_end > m.box_begin && nb < 2)
-                fail(VB200_ERR_INVALID, "%s: sample %d drops a box of an image with %d box (box ablation needs >= 2)", api, i, nb);
-            count += 1 + (m.token_end - m.token_begin) + (m.box_end - m.box_begin);
-            if (count > VB200_ABLATION_MAX_VARIANTS)
-                fail(VB200_ERR_INVALID, "%s: the variants of samples 0..%d number %lld, above %d (split the ranges across calls)", api, i,
-                     static_cast<long long>(count), VB200_ABLATION_MAX_VARIANTS);
-            const int b = static_cast<int>(text.size());
-            add(i, tok0, T, -1, box0, nb, -1, b, m.answer);
-            for (int p = m.token_begin; p < m.token_end; ++p) add(i, tok0, T, p, box0, nb, -1, b, m.answer);
-            for (int j = m.box_begin; j < m.box_end; ++j) add(i, tok0, T, -1, box0, nb, j, b, m.answer);
+        std::vector<int32_t> tin, nv;
+        int64_t n_floats = 0;
+        bool grounding = false;
+    };
+    // The messages checked against the batch's lengths and laid out; no sample cap (run_ablation applies it).
+    AblLayout ablation_layout(const char* api, int batch, const int32_t* n_tokens, const int32_t* n_boxes, const vb200_ablation_message* msgs,
+                              int n_msgs) const {
+        if (n_tokens == nullptr || n_boxes == nullptr || msgs == nullptr) fail(VB200_ERR_INVALID, "%s: n_tokens / n_boxes / msgs is NULL", api);
+        if (batch < 1) fail(VB200_ERR_INVALID, "%s: batch must be positive (batch = %d)", api, batch);
+        if (n_msgs < 1) fail(VB200_ERR_INVALID, "%s: n_msgs must be positive (n_msgs = %d)", api, n_msgs);
+        std::vector<int> tok0(batch + 1, 0), box0(batch + 1, 0);
+        for (int i = 0; i < batch; ++i) {
+            if (n_tokens[i] < 1 || n_boxes[i] < 1)
+                fail(VB200_ERR_INVALID, "%s: image %d has n_tokens %d / n_boxes %d (both must be >= 1)", api, i, n_tokens[i], n_boxes[i]);
+            if (tok0[i] > INT32_MAX - n_tokens[i] || box0[i] > INT32_MAX - n_boxes[i])
+                fail(VB200_ERR_INVALID, "%s: the batch's tokens or boxes overflow int32", api);
+            tok0[i + 1] = tok0[i] + n_tokens[i];
+            box0[i + 1] = box0[i] + n_boxes[i];
         }
-        const int n = static_cast<int>(count), n_pad = (n + 63) / 64 * 64;
-        while (static_cast<int>(text.size()) < n_pad) add(0, 0, 1, -1, 0, 1, -1, 0, 0);     // fillers: sample 0's first token and box
-        const int64_t sum_tin = std::accumulate(tin.begin(), tin.end(), int64_t{0});
+        AblLayout L;
+        std::vector<std::vector<AblVariant>> per(n_msgs);
+        auto sample = [&](const vb200_ablation_message& m, int masked, int image, int skip) {
+            L.text.push_back({tok0[m.image_begin], n_tokens[m.image_begin], masked, m.image_begin});
+            L.img.push_back({image, box0[image], skip});
+            L.tin.push_back(n_tokens[m.image_begin]);
+            L.nv.push_back(n_boxes[image] - (skip >= 0 ? 1 : 0) + 1);
+            return static_cast<int>(L.text.size()) - 1;
+        };
+        for (int pass = 0; pass < 2; ++pass)
+            for (int i = 0; i < n_msgs; ++i) {
+                const vb200_ablation_message& m = msgs[i];
+                const int f = m.family, K = m.n_images, ib = m.image_begin;
+                int head = 0, width = 0, images = 1;
+                switch (f) {
+                    case VB200_DECODE_VQA: head = kOutVqa; width = num_labels; break;
+                    case VB200_DECODE_GQA: head = kOutGqa; width = gqa_labels; break;
+                    case VB200_DECODE_SNLI_VE: head = kOutTri; width = 3; break;
+                    case VB200_DECODE_NLVR2: head = kOutBinary; width = 2; images = 2; break;
+                    case VB200_DECODE_RETRIEVAL: head = kOutVilLogit; width = K; images = 0; break;
+                    case VB200_DECODE_GROUNDING: head = kOutVisionLogit; break;
+                    default: fail(VB200_ERR_INVALID, "%s: message %d has unknown family %d", api, i, f);
+                }
+                if (pass == 0) {               // every message is checked before any sample is laid out
+                    if (images ? K != images : K < 1)
+                        fail(VB200_ERR_INVALID, "%s: message %d (family %d) has n_images %d (the family reads %s)", api, i, f, K,
+                             images == 2 ? "2" : images ? "1" : ">= 1");
+                    if (ib < 0 || ib > batch - K)
+                        fail(VB200_ERR_INVALID, "%s: message %d has images [%d, %lld) outside the batch of %d", api, i, ib,
+                             static_cast<long long>(ib) + K, batch);
+                    const int len = f == VB200_DECODE_GROUNDING ? n_boxes[ib] + 1 : width;
+                    if (len < 1) fail(VB200_ERR_INVALID, "%s: message %d: family %d's head has no columns on this engine", api, i, f);
+                    if (m.answer < -1 || m.answer >= len)
+                        fail(VB200_ERR_INVALID, "%s: message %d has answer %d outside [-1, %d)", api, i, m.answer, len);
+                    const int T = n_tokens[ib], nb = box0[ib + K] - box0[ib];
+                    if (m.token_begin < 0 || m.token_begin > m.token_end || m.token_end > T)
+                        fail(VB200_ERR_INVALID, "%s: message %d has the token range [%d, %d), reversed or outside [0, %d]", api, i,
+                             m.token_begin, m.token_end, T);
+                    if (m.box_begin < 0 || m.box_begin > m.box_end || m.box_end > nb)
+                        fail(VB200_ERR_INVALID, "%s: message %d has the box range [%d, %d), reversed or outside [0, %d]", api, i,
+                             m.box_begin, m.box_end, nb);
+                    for (int k = 0; k < K; ++k)
+                        if (n_boxes[ib + k] < 2 && m.box_begin < box0[ib + k + 1] - box0[ib] && m.box_end > box0[ib + k] - box0[ib])
+                            fail(VB200_ERR_INVALID, "%s: message %d drops a box of its image %d, which has %d box (box ablation needs >= 2)",
+                                 api, i, k, n_boxes[ib + k]);
+                }
+                if ((f == VB200_DECODE_NLVR2) != (pass == 0)) continue;
+                std::vector<AblVariant>& out = per[i];
+                // kind, unit, samples, segment (row: the first sample's head row; a grounding one's vision row is set below), drop
+                auto variant = [&](int kind, int unit, int samples, vb::SegmentDesc seg, int drop) {
+                    out.push_back({{i, kind, unit, samples, 0, seg.len}, seg, 0, m.answer, drop});
+                };
+                auto seg = [&](int first) -> vb::SegmentDesc {
+                    if (f == VB200_DECODE_NLVR2) return {head, first / 2, 2, -1, 0, 0};
+                    if (f == VB200_DECODE_GROUNDING) return {head, first, L.nv[first], -1, 0, 0};
+                    return {head, first, width, -1, 0, 0};
+                };
+                auto all_images = [&](int masked) {
+                    const int first = sample(m, masked, ib, -1);
+                    for (int k = 1; k < K; ++k) sample(m, masked, ib + k, -1);
+                    return first;
+                };
+                const int base = all_images(-1);
+                variant(0, -1, K, seg(base), -1);
+                for (int p = m.token_begin; p < m.token_end; ++p) {
+                    const int first = all_images(p);
+                    variant(1, p, K, seg(first), -1);
+                }
+                for (int u = m.box_begin; u < m.box_end; ++u) {
+                    int k = 0;
+                    while (box0[ib + k + 1] - box0[ib] <= u) ++k;
+                    const int j = u - (box0[ib + k] - box0[ib]);
+                    if (f == VB200_DECODE_NLVR2) {
+                        const int first = sample(m, -1, ib, k == 0 ? j : -1);
+                        sample(m, -1, ib + 1, k == 1 ? j : -1);
+                        variant(2, u, 2, seg(first), -1);
+                    } else if (f == VB200_DECODE_RETRIEVAL) {     // the unablated segment, element k from the changed image alone
+                        vb::SegmentDesc s = seg(base);
+                        s.sub = k;
+                        s.sub_row = sample(m, -1, ib + k, j);
+                        variant(2, u, 1, s, -1);
+                    } else {
+                        const int first = sample(m, -1, ib, j);
+                        variant(2, u, 1, seg(first), f == VB200_DECODE_GROUNDING ? j + 1 : -1);
+                    }
+                }
+                L.grounding |= f == VB200_DECODE_GROUNDING;
+            }
+        std::vector<int64_t> vrow(L.nv.size() + 1, 0);       // each sample's first vision_logit row
+        for (size_t s = 0; s < L.nv.size(); ++s) vrow[s + 1] = vrow[s] + L.nv[s];
+        for (int i = 0; i < n_msgs; ++i) {
+            const int base = static_cast<int>(L.v.size());
+            for (AblVariant a : per[i]) {
+                if (msgs[i].family == VB200_DECODE_GROUNDING) a.seg.row = static_cast<int32_t>(vrow[a.seg.row]);
+                a.rec.offset = a.seg.dst = L.n_floats;
+                a.base = base;
+                L.n_floats += a.rec.length;
+                L.v.push_back(a);
+            }
+        }
+        return L;
+    }
+    // Every sample of L as one PACKED forward (rounded up to a multiple of 64 with fillers: sample 0's first token and box), each
+    // variant's segment gathered into variant_logits, and with scores one score per variant.  abl_ws holds the sample and segment
+    // descriptors (staged through abl_in) and the samples' text ids.
+    void run_ablation(const char* api, const vb200_packed_region_inputs* in, AblLayout L, int max_regions, int64_t mask_token,
+                      float* variant_logits, vb200_ablation_score* scores, int slot, cudaStream_t st) {
+        const int64_t count = static_cast<int64_t>(L.text.size());
+        if (count > VB200_ABLATION_MAX_VARIANTS)
+            fail(VB200_ERR_INVALID, "%s: the variants run %lld forward samples, above %d (split the messages across calls)", api,
+                 static_cast<long long>(count), VB200_ABLATION_MAX_VARIANTS);
+        const int task = cfg.task_tokens ? 1 : 0;
+        const int n_pad = static_cast<int>((count + 63) / 64 * 64), n_var = static_cast<int>(L.v.size());
+        for (int64_t s = count; s < n_pad; ++s) {
+            L.text.push_back({0, 1, -1, 0});
+            L.img.push_back({0, 0, -1});
+            L.tin.push_back(1);
+            L.nv.push_back(2);
+        }
+        std::vector<vb::SegmentDesc> seg(n_var);
+        for (int k = 0; k < n_var; ++k) seg[k] = L.v[k].seg;
+        const int64_t sum_tin = std::accumulate(L.tin.begin(), L.tin.end(), int64_t{0});
 
         size_t at = 0;
         auto carve = [&](size_t bytes) { const size_t a = at; at += (bytes + 255) / 256 * 256; return a; };
-        const size_t o_text = carve(n_pad * sizeof(vb::TextSrc)), o_img = carve(n_pad * sizeof(vb::RegionSrc)), staged = at;
-        const size_t o_q = carve(sum_tin * 8), o_seg = carve(sum_tin * 8), o_task = carve(static_cast<size_t>(n_pad) * 8);
-        const size_t o_logits = carve(static_cast<size_t>(n_pad) * width * 4);
+        const size_t o_text = carve(n_pad * sizeof(vb::TextSrc)), o_img = carve(n_pad * sizeof(vb::RegionSrc));
+        const size_t o_seg = carve(n_var * sizeof(vb::SegmentDesc)), staged = at;
+        const size_t o_q = carve(sum_tin * 8), o_ids = carve(sum_tin * 8), o_task = carve(static_cast<size_t>(n_pad) * 8);
         CUDA_CHECK(cudaSetDevice(opt.device));
         char* ws = abl_ws.acquire(at, st);
         abl_in.stage(staged, st, [&](char* h, const auto& put) {
-            memcpy(h + o_text, text.data(), n_pad * sizeof(vb::TextSrc));
-            memcpy(h + o_img, img.data(), n_pad * sizeof(vb::RegionSrc));
+            memcpy(h + o_text, L.text.data(), n_pad * sizeof(vb::TextSrc));
+            memcpy(h + o_img, L.img.data(), n_pad * sizeof(vb::RegionSrc));
+            memcpy(h + o_seg, seg.data(), n_var * sizeof(vb::SegmentDesc));
             put(ws, 0, staged);
         });
         const auto* text_d = reinterpret_cast<const vb::TextSrc*>(ws + o_text);
         const auto* img_d = reinterpret_cast<const vb::RegionSrc*>(ws + o_img);
-        int64_t *q = reinterpret_cast<int64_t*>(ws + o_q), *seg = reinterpret_cast<int64_t*>(ws + o_seg);
+        int64_t *q = reinterpret_cast<int64_t*>(ws + o_q), *ids = reinterpret_cast<int64_t*>(ws + o_ids);
         int64_t* tk = reinterpret_cast<int64_t*>(ws + o_task);
-        float* logits = reinterpret_cast<float*>(ws + o_logits);
-        vb200_outputs out{};
-        out.*field = logits;
-        run_packed(api, PACKED, {"variant", n_pad, tin.data(), in->max_tokens, nv.data(), v.max_regions}, bit, slot, &out, {}, st,
-                   [&](Plan& pl, const PackedBatch& b, cudaStream_t s) {
-                       CUDA_CHECK(vb::launch_variant_text(text_d, n_pad, pl.offs_t(), task, in->question, in->segment_ids, in->task_tokens,
-                                                          mask_token, q, seg, tk, s));
-                       embed_text(pl, q, seg, nullptr, tk, b.rows_t(), s);
-                       pack_regions_packed(pl, in->box_features, in->boxes, in->image_wh, nullptr, b.rows_v(), s, img_d);
-                   });
+        // the pooled task heads always, vision_logit for a grounding message: at most two plans per bucket and capacities
+        const uint32_t select = VB200_OUT_VIL_PREDICTION | VB200_OUT_VIL_PREDICTION_GQA | VB200_OUT_VIL_LOGIT | VB200_OUT_VIL_BINARY_PREDICTION |
+                                VB200_OUT_VIL_TRI_PREDICTION | (L.grounding ? VB200_OUT_VISION_LOGIT : 0u);
+        const vb200_outputs none{};                   // the segments are gathered from the plan's heads, not copied out
+        const Plan& pl = run_packed(api, PACKED, {"variant", n_pad, L.tin.data(), in->max_tokens, L.nv.data(), max_regions}, select, slot,
+                                    &none, {}, st, [&](Plan& p, const PackedBatch& b, cudaStream_t s) {
+            CUDA_CHECK(vb::launch_variant_text(text_d, n_pad, p.offs_t(), task, in->question, in->segment_ids, in->task_tokens, mask_token,
+                                               q, ids, tk, s));
+            embed_text(p, q, ids, nullptr, tk, b.rows_t(), s);
+            pack_regions_packed(p, in->box_features, in->boxes, in->image_wh, nullptr, b.rows_v(), s, img_d);
+        });
+        vb::SegmentHeads heads{};
+        for (int h = 0; h < vb::kSegmentHeads; ++h) {
+            heads.p[h] = pl.outs[h].p;
+            heads.ld[h] = pl.outs[h].ld;
+            heads.cols[h] = pl.outs[h].cols;
+        }
+        CUDA_CHECK(vb::launch_segment_gather(reinterpret_cast<const vb::SegmentDesc*>(ws + o_seg), n_var, heads, variant_logits, st));
+        abl_ws.release(st);
         if (scores != nullptr) {
-            std::vector<vb::DecodeDesc> d(n);
-            for (int k = 0; k < n; ++k) {
-                d[k].src = logits + static_cast<size_t>(k) * width;
-                d[k].len = width;
+            std::vector<vb::DecodeDesc> d(n_var);
+            for (int k = 0; k < n_var; ++k) {
+                const AblVariant& a = L.v[k];
+                d[k].src = variant_logits + a.rec.offset;
+                d[k].len = a.rec.length;
                 d[k].top_n = 1;
-                d[k].ref = logits + static_cast<size_t>(base[k]) * width;
+                d[k].ref = variant_logits + L.v[a.base].rec.offset;
                 d[k].score = scores + k;
-                d[k].column = column[k];
+                d[k].column = a.column;
+                d[k].drop = a.drop;
             }
-            CUDA_CHECK(vb::launch_answer_decode(stage_decode(d, st), n, nullptr, st));
+            CUDA_CHECK(vb::launch_answer_decode(stage_decode(d, st), n_var, nullptr, st));
             dec_ws.release(st);
         }
-        CUDA_CHECK(cudaMemcpyAsync(variant_logits, logits, static_cast<size_t>(n) * width * 4, cudaMemcpyDeviceToDevice, st));
-        abl_ws.release(st);
+    }
+    // vb200_answer_ablation: one single-image message of `family` per sample, checked in the samples' terms first
+    void answer_ablation(const vb200_packed_region_inputs* in, const vb200_ablation_msg* msgs, int family, int64_t mask_token,
+                         float* variant_logits, vb200_ablation_score* scores, int slot, cudaStream_t st) {
+        const char* api = "vb200_answer_ablation";
+        if (in == nullptr || msgs == nullptr || variant_logits == nullptr) fail(VB200_ERR_INVALID, "%s: in / msgs / variant_logits is NULL", api);
+        if (x3) fail(VB200_ERR_INVALID, "%s: packed batches are not supported in split_fp32 (fp32x) mode", api);
+        if (pretraining) fail(VB200_ERR_INVALID, "%s: a pre-training engine has no task head to attribute an answer of", api);
+        int width = 0;
+        switch (family) {
+            case VB200_DECODE_VQA: width = num_labels; break;
+            case VB200_DECODE_GQA: width = gqa_labels; break;
+            case VB200_DECODE_SNLI_VE: width = 3; break;
+            case VB200_DECODE_NLVR2: fail(VB200_ERR_INVALID, "%s: family NLVR2 is not supported (an answer reads two images)", api);
+            case VB200_DECODE_RETRIEVAL: fail(VB200_ERR_INVALID, "%s: family retrieval is not supported (an answer ranks many images)", api);
+            case VB200_DECODE_GROUNDING:
+                fail(VB200_ERR_INVALID, "%s: family grounding is not supported (the answer is a box a variant may remove)", api);
+            default: fail(VB200_ERR_INVALID, "%s: unknown family %d", api, family);
+        }
+        if (width < 1) fail(VB200_ERR_INVALID, "%s: family %d's head has no columns on this engine", api, family);
+        const int max_regions = check_ablation_inputs(api, in, mask_token, slot);
+        std::vector<vb200_ablation_message> m(in->batch);
+        int64_t count = 0;
+        for (int i = 0; i < in->batch; ++i) {
+            const vb200_ablation_msg& a = msgs[i];
+            const int T = in->n_tokens[i], nb = in->n_boxes[i];
+            if (a.answer < -1 || a.answer >= width)
+                fail(VB200_ERR_INVALID, "%s: sample %d has answer %d outside [-1, %d)", api, i, a.answer, width);
+            if (a.token_begin < 0 || a.token_begin > a.token_end || a.token_end > T)
+                fail(VB200_ERR_INVALID, "%s: sample %d has the token range [%d, %d), reversed or outside [0, %d]", api, i, a.token_begin,
+                     a.token_end, T);
+            if (a.box_begin < 0 || a.box_begin > a.box_end || a.box_end > nb)
+                fail(VB200_ERR_INVALID, "%s: sample %d has the box range [%d, %d), reversed or outside [0, %d]", api, i, a.box_begin, a.box_end,
+                     nb);
+            if (a.box_end > a.box_begin && nb < 2)
+                fail(VB200_ERR_INVALID, "%s: sample %d drops a box of an image with %d box (box ablation needs >= 2)", api, i, nb);
+            count += 1 + (a.token_end - a.token_begin) + (a.box_end - a.box_begin);
+            if (count > VB200_ABLATION_MAX_VARIANTS)
+                fail(VB200_ERR_INVALID, "%s: the variants of samples 0..%d number %lld, above %d (split the ranges across calls)", api, i,
+                     static_cast<long long>(count), VB200_ABLATION_MAX_VARIANTS);
+            m[i] = {family, i, 1, a.answer, a.token_begin, a.token_end, a.box_begin, a.box_end};
+        }
+        run_ablation(api, in, ablation_layout(api, in->batch, in->n_tokens, in->n_boxes, m.data(), in->batch), max_regions, mask_token,
+                     variant_logits, scores, slot, st);
+    }
+    void message_ablation(const vb200_packed_region_inputs* in, const vb200_ablation_message* msgs, int n_msgs, int64_t mask_token,
+                          float* variant_logits, vb200_ablation_score* scores, int slot, cudaStream_t st) {
+        const char* api = "vb200_message_ablation";
+        if (in == nullptr || msgs == nullptr || variant_logits == nullptr) fail(VB200_ERR_INVALID, "%s: in / msgs / variant_logits is NULL", api);
+        if (x3) fail(VB200_ERR_INVALID, "%s: packed batches are not supported in split_fp32 (fp32x) mode", api);
+        if (pretraining) fail(VB200_ERR_INVALID, "%s: a pre-training engine has no task head to attribute an answer of", api);
+        if (reinterpret_cast<uintptr_t>(variant_logits) & 3) fail(VB200_ERR_INVALID, "%s: variant_logits is not 4-byte aligned", api);
+        if (reinterpret_cast<uintptr_t>(scores) & 3) fail(VB200_ERR_INVALID, "%s: scores is not 4-byte aligned", api);
+        const int max_regions = check_ablation_inputs(api, in, mask_token, slot);
+        run_ablation(api, in, ablation_layout(api, in->batch, in->n_tokens, in->n_boxes, msgs, n_msgs), max_regions, mask_token,
+                     variant_logits, scores, slot, st);
+    }
+    void message_ablation_layout(int batch, const int32_t* n_tokens, const int32_t* n_boxes, const vb200_ablation_message* msgs, int n_msgs,
+                                 vb200_ablation_variant* variants, int64_t* n_variants, int64_t* n_floats, int64_t* n_samples) const {
+        const char* api = "vb200_message_ablation_layout";
+        if (n_variants == nullptr || n_floats == nullptr || n_samples == nullptr)
+            fail(VB200_ERR_INVALID, "%s: n_variants / n_floats / n_samples is NULL", api);
+        if (pretraining) fail(VB200_ERR_INVALID, "%s: a pre-training engine has no task head to attribute an answer of", api);
+        const AblLayout L = ablation_layout(api, batch, n_tokens, n_boxes, msgs, n_msgs);
+        if (variants != nullptr)
+            for (size_t k = 0; k < L.v.size(); ++k) variants[k] = L.v[k].rec;
+        *n_variants = static_cast<int64_t>(L.v.size());
+        *n_floats = L.n_floats;
+        *n_samples = static_cast<int64_t>(L.text.size());
     }
     // ---- region selection: every descriptor is checked before anything is enqueued
     void select_regions(const vb200_detections* imgs, int n, const vb200_select_params* p, const vb200_selected* out, cudaStream_t st) {
@@ -2861,6 +3037,21 @@ int vb200_answer_ablation(vb200_handle h, const vb200_packed_region_inputs* in, 
     if (h == nullptr) return VB200_ERR_INVALID;
     return guard(h, [&] {
         h->answer_ablation(in, msgs, family, mask_token, variant_logits, scores, slot, static_cast<cudaStream_t>(cuda_stream));
+    });
+}
+
+int vb200_message_ablation_layout(vb200_handle h, int32_t batch, const int32_t* n_tokens, const int32_t* n_boxes,
+                                  const vb200_ablation_message* msgs, int32_t n_msgs, vb200_ablation_variant* variants, int64_t* n_variants,
+                                  int64_t* n_floats, int64_t* n_samples) {
+    if (h == nullptr) return VB200_ERR_INVALID;
+    return guard(h, [&] { h->message_ablation_layout(batch, n_tokens, n_boxes, msgs, n_msgs, variants, n_variants, n_floats, n_samples); });
+}
+
+int vb200_message_ablation(vb200_handle h, const vb200_packed_region_inputs* in, const vb200_ablation_message* msgs, int32_t n_msgs,
+                           int64_t mask_token, float* variant_logits, vb200_ablation_score* scores, int32_t slot, void* cuda_stream) {
+    if (h == nullptr) return VB200_ERR_INVALID;
+    return guard(h, [&] {
+        h->message_ablation(in, msgs, n_msgs, mask_token, variant_logits, scores, slot, static_cast<cudaStream_t>(cuda_stream));
     });
 }
 

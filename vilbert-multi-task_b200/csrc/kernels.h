@@ -105,7 +105,7 @@ cudaError_t launch_image_pack(const float* feats, const float* loc, const uint8_
 // Packed batches (offs != nullptr): offs = device [B + 1] image row offsets (V_b = boxes_b + 1 regions per image), box_features /
 // boxes hold image b's V_b - 1 boxes from detector row offs[b] - b, every row is real, n and num_boxes are unused (num_boxes must be
 // null, and split16 0), spatials_out is [offs[B], 5].
-// src (packed only, answer ablation): output image b is image src[b].image's offs[b+1] - offs[b] - 1 + (skip >= 0) detector boxes
+// src (packed only, answer and message ablation): output image b is image src[b].image's offs[b+1] - offs[b] - 1 + (skip >= 0) detector boxes
 // from row src[b].box0, box src[b].skip left out (-1: none).
 struct RegionSrc { int32_t image, box0, skip; };
 cudaError_t launch_region_pack(const float* box_feats, const float* boxes, const float* image_wh, const int32_t* num_boxes,
@@ -184,8 +184,10 @@ cudaError_t launch_rowdot(const float* x, int ld_x, const float* W, const float*
 // probabilities and indices, and for grounding (spatials != null: the segment's first [len, 5] spatials row) the pixel boxes of
 // the picked rows.  One CTA per message; the descriptors are resolved and bounds-checked on the host.
 // Answer ablation (score != null, top_n 1): the CTA writes *score instead of an answer -- column `column` of src, or for column -1
-// the top-1 of the `len` logits at ref (the sample's unablated row, recomputed by every CTA), with its probability in src, and src's
-// own top-1; answers may then be null.
+// the top-1 of the logits at ref (the message's unablated segment, recomputed by every CTA), with its probability in src, and src's
+// own top-1; answers may then be null.  drop >= 0 (a grounding box variant): src is ref without row `drop`, ref has len + 1 logits,
+// and column and top-1 are reported in ref's numbering -- the attributed row maps into src, a dropped one reports column -1 with
+// probability 0, and src's top-1 maps back by +1 from row `drop` on.
 struct DecodeDesc {
     const float* src;
     const float* spatials;
@@ -193,9 +195,16 @@ struct DecodeDesc {
     int len, top_n;
     const float* ref;
     vb200_ablation_score* score;
-    int column;
+    int column, drop;
 };
 cudaError_t launch_answer_decode(const DecodeDesc* descs, int n, vb200_answer* answers, cudaStream_t st);
+// Message ablation's segments (decode.cu): variant k (one CTA each) copies `len` floats of head `head` into out + dst -- element i
+// is heads.p[head][row * ld + i] for a head of several columns (one row), heads.p[head][(row + i) * ld] for a one-column head (a
+// run of rows) -- with element `sub` (>= 0) read from row sub_row instead.  Heads are indexed as the engine's output slots.
+constexpr int kSegmentHeads = 7;
+struct SegmentHeads { const float* p[kSegmentHeads]; int ld[kSegmentHeads], cols[kSegmentHeads]; };
+struct SegmentDesc { int32_t head, row, len, sub, sub_row; int64_t dst; };
+cudaError_t launch_segment_gather(const SegmentDesc* descs, int n, const SegmentHeads& heads, float* out, cudaStream_t st);
 // Attention relevance (relevance.cu, vb200_attention_relevance): per sample b (one CTA) the rollout rows of the text CLS row and the
 // image global row, [2, T_b + V_b] at relevance + out.  Entry e of the maps starts at float `offset` and holds sample b's
 // [heads, Lq_b, Lk_b] block at heads * prefix[k] (k 0 text layers, 1 image layers, 2 both directions of a connection layer); kinds

@@ -146,6 +146,110 @@ def ablation_variants(call):
     return out
 
 
+# every decode family by name (vb200_message_ablation); a worker task id (_lib.TASK_DECODE_FAMILY) or a DECODE_* value works too
+MESSAGE_FAMILIES = {"vqa": L.DECODE_VQA, "gqa": L.DECODE_GQA, "nlvr2": L.DECODE_NLVR2, "snli_ve": L.DECODE_SNLI_VE,
+                    "retrieval": L.DECODE_RETRIEVAL, "grounding": L.DECODE_GROUNDING}
+_FAMILY_IMAGES = {L.DECODE_VQA: 1, L.DECODE_GQA: 1, L.DECODE_NLVR2: 2, L.DECODE_SNLI_VE: 1, L.DECODE_GROUNDING: 1}
+
+
+def message_family(family):
+    """A decode family from its name, a worker task id or its ``_lib.DECODE_*`` value."""
+    if isinstance(family, str):
+        f = MESSAGE_FAMILIES.get(family, L.TASK_DECODE_FAMILY.get(family))
+    else:
+        f = int(family)
+    if f not in MESSAGE_FAMILIES.values():
+        raise ValueError(f"message_ablation: unknown family {family!r} (one of {sorted(MESSAGE_FAMILIES)}, a task id or a DECODE_* value)")
+    return f
+
+
+def message_pieces(messages, n_tokens, n_boxes):
+    """The engine messages (``_lib.AblationMessage`` fields as tuples) for ``message_ablation``'s ``messages`` and the batch's
+    lengths, and for each the index of the message it belongs to.  A message is ``(family, image_begin, n_images, answer=None,
+    tokens=None, boxes=None)``; by default positions 1 .. Tin - 2 of image_begin's question are masked and every box of the
+    message's images with at least two boxes is dropped (boxes numbered across the message's images).  The default boxes of a
+    message with a one-box image between others run as separate pieces, each with its own unablated variant."""
+    B = len(n_tokens)
+    out = []
+    for i, m in enumerate(messages):
+        m = tuple(m) + (None,) * (6 - len(m))
+        if len(m) != 6:
+            raise ValueError(f"message_ablation: message {i} has {len(m)} fields (family, image_begin, n_images, answer, tokens, boxes)")
+        fam, ib, k, answer, tokens, boxes = m
+        f = message_family(fam)
+        ib, k = int(ib), int(k)
+        want = _FAMILY_IMAGES.get(f)
+        if (k != want) if want else k < 1:
+            raise ValueError(f"message_ablation: message {i} has n_images {k} (the family reads {want or '>= 1'})")
+        if ib < 0 or ib + k > B:
+            raise ValueError(f"message_ablation: message {i} has images [{ib}, {ib + k}) outside the batch of {B}")
+        a = -1 if answer is None else int(answer)
+        if a < -1:
+            raise ValueError(f"message_ablation: message {i} has answer {a} (an index >= 0, or None / -1: the unablated top-1)")
+        tin, nb = int(n_tokens[ib]), [int(n) for n in n_boxes[ib:ib + k]]
+        first = [sum(nb[:j]) for j in range(k + 1)]            # each image's first box in the message's numbering
+        tb, te = (1, max(1, tin - 1)) if tokens is None else (int(tokens[0]), int(tokens[1]))
+        if not 0 <= tb <= te <= tin:
+            raise ValueError(f"message_ablation: message {i} has the token range [{tb}, {te}), reversed or outside [0, {tin}]")
+        if boxes is None:                                      # runs of adjacent images with >= 2 boxes
+            runs = []
+            for j in range(k):
+                if nb[j] < 2:
+                    continue
+                if runs and runs[-1][1] == first[j]:
+                    runs[-1] = (runs[-1][0], first[j + 1])
+                else:
+                    runs.append((first[j], first[j + 1]))
+        else:
+            bb, be = int(boxes[0]), int(boxes[1])
+            if not 0 <= bb <= be <= first[k]:
+                raise ValueError(f"message_ablation: message {i} has the box range [{bb}, {be}), reversed or outside [0, {first[k]}]")
+            for j in range(k):
+                if nb[j] < 2 and bb < first[j + 1] and be > first[j]:
+                    raise ValueError(f"message_ablation: message {i} drops a box of its image {j}, which has {nb[j]} box")
+            runs = [(bb, be)] if be > bb else []
+        runs = runs or [(0, 0)]
+        out.append(((f, ib, k, a, tb, te) + runs[0], i))
+        out += [((f, ib, k, a, 0, 0) + r, i) for r in runs[1:]]
+    return out
+
+
+def message_calls(variants, cap: int = L.ABLATION_MAX_VARIANTS):
+    """The engine calls for a message ablation layout: ``variants`` are its records ``(message, kind, unit, samples)`` in layout order
+    (``vb200_message_ablation_layout``).  Each call is a list of pieces ``(message, (token_begin, token_end, box_begin, box_end))``
+    whose variants run at most ``cap`` forward samples.  Messages are kept whole where they fit; a message above ``cap`` is split
+    into pieces of its units (positions first, then boxes), each with its own unablated variant."""
+    groups = []
+    for m, kind, unit, samples in variants:
+        if kind == 0:
+            groups.append((m, samples, []))
+        else:
+            groups[-1][2].append((kind, unit, samples))
+    pieces = []
+    for m, base, units in groups:
+        if base + max([s for _, _, s in units], default=0) > cap:
+            raise ValueError(f"message_ablation: message {m} runs {base} samples per unablated variant, too many for {cap} per call")
+        chunk, size = [], base
+        for u in units:
+            if size + u[2] > cap:
+                pieces.append((m, chunk, size))
+                chunk, size = [], base
+            chunk.append(u)
+            size += u[2]
+        pieces.append((m, chunk, size))
+    calls, size = [], cap + 1
+    for m, chunk, n in pieces:
+        if size + n > cap:
+            calls.append([])
+            size = 0
+        toks = [u for k, u, _ in chunk if k == 1]
+        bxs = [u for k, u, _ in chunk if k == 2]
+        r = ((toks[0], toks[-1] + 1) if toks else (0, 0)) + ((bxs[0], bxs[-1] + 1) if bxs else (0, 0))
+        calls[-1].append((m, r))
+        size += n
+    return calls
+
+
 def attention_list(kinds, layout_entry, entries):
     """The reference's attn_data_list from the maps of the selected entries: ``kinds`` / ``layout_entry`` are the full entry list's
     kinds and each entry's index in ``entries`` (-1: not selected) as ``attention_selection`` returns them.  One position per layer in
@@ -954,6 +1058,93 @@ class VILBertForVLTasks(object):
             logits = r.pop("logits")
             if return_logits:
                 r["logits"] = torch.cat(logits)
+        return res
+
+    def _message_layout(self, n_tokens, n_boxes, msgs):
+        """vb200_message_ablation_layout: the records ``(message, kind, unit, samples, offset, length)`` and the floats they need."""
+        arr = (L.AblationMessage * len(msgs))(*[L.AblationMessage(*m) for m in msgs])
+        lib, nv, nf, ns = L.load(), C.c_int64(), C.c_int64(), C.c_int64()
+        args = (len(n_tokens), _int32s(n_tokens), _int32s(n_boxes), arr, len(msgs))
+        L.check(lib.vb200_message_ablation_layout(self._handle, *args, None, C.byref(nv), C.byref(nf), C.byref(ns)), self._handle)
+        recs = (L.AblationVariant * max(nv.value, 1))()
+        L.check(lib.vb200_message_ablation_layout(self._handle, *args, recs, C.byref(nv), C.byref(nf), C.byref(ns)), self._handle)
+        return [(r.message, r.kind, r.unit, r.samples, r.offset, r.length) for r in recs[:nv.value]], nf.value, arr
+
+    @torch.no_grad()
+    def message_ablation(self, question, segment_ids, task_tokens, box_features, boxes, image_wh, n_tokens, n_boxes, messages,
+                         mask_token: int = 103, max_tokens: int = 0, max_boxes: int = 0, slot: int = 0, return_logits: bool = False):
+        """Answer ablation for every decode family (vb200_message_ablation): the packed detector-output batch of ``answer_ablation``
+        (laid out as the worker lays it out: the text repeated per image, an NLVR2 pair on an even sample) and ``messages``, each
+        ``(family or task id, image_begin, n_images, answer=None, tokens=None, boxes=None)`` -- see ``message_pieces`` for the
+        defaults.  ``answer`` indexes the message's segment: a head column, 0 / 1 for NLVR2, the image for retrieval, the row of
+        ``vision_logit`` (0: the global box) for grounding.  Calls above the engine's 1024 forward samples are split along the
+        engine's own layout records (``message_calls``).
+        Returns one dict per message: ``answer``, ``prob``, ``top1``, ``top1_prob`` of the unablated input; ``tokens`` with
+        ``token_prob`` / ``token_top1``; ``boxes`` as ``(image of the message, box)`` pairs with ``box_prob`` / ``box_top1`` (CPU
+        tensors; grounding reports rows in the unablated image's numbering, answer -1 / prob 0 where the attributed box is dropped);
+        with ``return_logits`` also ``logits``, the variants' segments (device tensors) in that order."""
+        nt, nb = _host_ints(n_tokens), _host_ints(n_boxes)
+        B = len(nt)
+        if len(nb) != B or B < 1:
+            raise ValueError("message_ablation: n_tokens and n_boxes must have the same, positive length")
+        if not messages:
+            raise ValueError("message_ablation: no messages")
+        pieces = message_pieces(messages, nt, nb)
+        device = self._engine_device()
+        F = self._dims["v_feature_size"]
+        q = _to_device(question, torch.int64, device).reshape(-1)
+        seg = _to_device(segment_ids if segment_ids is not None else torch.zeros_like(q), torch.int64, device).reshape(-1)
+        tk = _task_rows(task_tokens if task_tokens is not None else torch.zeros(B, 1, dtype=torch.int64), B, device)
+        bf = _to_device(box_features, torch.float32, device).reshape(-1, F)
+        bx = _to_device(boxes, torch.float32, device).reshape(-1, 4)
+        wh = _to_device(image_wh, torch.float32, device)
+        if q.numel() != sum(nt) or seg.numel() != sum(nt) or bf.shape[0] != sum(nb) or bx.shape[0] != sum(nb) or tuple(wh.shape) != (B, 2):
+            raise ValueError("message_ablation: question / segment_ids need sum(n_tokens) entries, box_features / boxes sum(n_boxes) "
+                             "rows, image_wh [B, 2]")
+        msgs = [p for p, _ in pieces]
+        recs, _, _ = self._message_layout(nt, nb, msgs)
+        inp = L.PackedRegionInputs(B, int(max_tokens), int(max_boxes), _int32s(nt), _int32s(nb), q.data_ptr(), seg.data_ptr(),
+                                   tk.data_ptr(), bf.data_ptr(), bx.data_ptr(), wh.data_ptr(), None)
+        res = [dict(tokens=[], token_prob=[], token_top1=[], boxes=[], box_prob=[], box_top1=[], logits=[]) for _ in messages]
+        for call in message_calls([r[:4] for r in recs]):
+            cmsgs = [msgs[p][:4] + r for p, r in call]
+            crecs, n_floats, arr = self._message_layout(nt, nb, cmsgs)
+            logits = torch.empty(n_floats, dtype=torch.float32, device=device)
+            scores = torch.empty(len(crecs), 4, dtype=torch.int32, device=device)       # vb200_ablation_score
+            self._call("vb200_message_ablation", C.byref(inp), arr, len(cmsgs), int(mask_token), logits.data_ptr(), scores.data_ptr(),
+                       int(slot))
+            sc = scores.cpu()
+            col, top1 = sc[:, 0].tolist(), sc[:, 2].tolist()
+            prob, top1_prob = sc[:, 1].view(torch.float32).tolist(), sc[:, 3].view(torch.float32).tolist()
+            for k, (m, kind, unit, _, off, n) in enumerate(crecs):
+                p = call[m][0]
+                r = res[pieces[p][1]]
+                seg_k = logits[off:off + n]
+                if kind == 0:
+                    if "answer" not in r:
+                        r.update(answer=col[k], prob=prob[k], top1=top1[k], top1_prob=top1_prob[k])
+                        r["logits"].append(seg_k)
+                    continue
+                if kind == 1:
+                    r["tokens"].append(unit)
+                else:
+                    first = [0]
+                    for j in range(msgs[p][2]):
+                        first.append(first[-1] + nb[msgs[p][1] + j])
+                    img = max(j for j in range(msgs[p][2]) if first[j] <= unit)
+                    r["boxes"].append((img, unit - first[img]))
+                name = "token" if kind == 1 else "box"
+                r[name + "_prob"].append(prob[k])
+                r[name + "_top1"].append(top1[k])
+                r["logits"].append(seg_k)
+        for r in res:
+            for k in ("token_prob", "box_prob"):
+                r[k] = torch.tensor(r[k], dtype=torch.float32)
+            for k in ("token_top1", "box_top1"):
+                r[k] = torch.tensor(r[k], dtype=torch.int64)
+            logits = r.pop("logits")
+            if return_logits:
+                r["logits"] = logits
         return res
 
     # ------------------------------------------------------------------ answer decode (worker.py:295-386)

@@ -537,6 +537,49 @@ def custom_prediction_packed(requests, bucket: int = 8, select: Optional[int] = 
     return _answer_regions(answers, requests, out, spatials, p["spans"], p["n_tokens"], p["n_boxes"], decode)
 
 
+def ablation_messages(requests, spans, tokens=None, boxes=None):
+    """The `model.message_ablation` messages of packed region requests: request i, which took batch rows `spans[i] = (lo, hi)`,
+    attributes its answer over images [lo, hi) -- one for VQA, GQA, SNLI-VE and grounding, the pair for NLVR2, every candidate for
+    retrieval -- with its task id as the family.  Returns `{request: (task_id, lo, hi - lo, None, tokens, boxes)}`."""
+    return {i: (requests[i][4], lo, hi - lo, None, tokens, boxes) for i, (lo, hi) in spans.items()}
+
+
+def _pixel_box(info, row):
+    """Row `row` of a grounding segment as a pixel box [x1, y1, x2, y2]: row 0 is the whole image, row r >= 1 box r - 1 of `info`."""
+    if row == 0:
+        return [0.0, 0.0, float(info["image_width"]), float(info["image_height"])]
+    return [float(v) for v in np.asarray(info["bbox"], dtype=np.float32)[row - 1, :4]]
+
+
+def custom_ablation_packed(requests, max_boxes: int = 100, *, tokens=None, boxes=None):
+    """Why each answer: `custom_prediction_packed` (decode="device") for `custom_prediction` argument tuples
+    `(query, task, features, infos, task_id)`, plus the answer's ablation over its question tokens and detector boxes
+    (`model.message_ablation`) for every task: one image for VQA, GQA, SNLI-VE and grounding, the pair for NLVR2, every candidate for
+    retrieval.  `tokens` / `boxes`: one (begin, end) range for every request, or None for the defaults (positions 1 .. Tin - 2, every
+    box of an image with at least two).  The rows are those of `pack_region_requests`, unchanged.
+    Returns per request `{"answer": <custom_prediction_packed's answer>, "ablation": <message_ablation's dict>}` -- whose `boxes` are
+    `(image, box)` pairs, with `box_pixels` their [x1, y1, x2, y2] from `infos`, and for grounding `answer_box` the pixel box of the
+    attributed row -- or the exception of a request that fails validation."""
+    p = pack_region_requests(requests, max_boxes=max_boxes)
+    answers = p["answers"]
+    if not p["spans"]:
+        return answers
+    args = (p["question"], p["segment_ids"], p["task_tokens"], p["box_features"], p["boxes"], p["image_wh"], p["n_tokens"], p["n_boxes"])
+    msgs = ablation_messages(requests, p["spans"], tokens, boxes)
+    mask = (tokenizer.vocab.get("[MASK]", 103) if tokenizer is not None and hasattr(tokenizer, "vocab") else 103)
+    with model_lock:
+        out, spatials = model.forward_regions_packed(*args, select=p["select"], max_tokens=p["max_tokens"], max_boxes=p["max_boxes"])
+        ab = model.message_ablation(*args, list(msgs.values()), mask_token=mask, max_tokens=p["max_tokens"], max_boxes=p["max_boxes"])
+    answers = _answer_regions(answers, requests, out, spatials, p["spans"], p["n_tokens"], p["n_boxes"], "device")
+    for i, a in zip(msgs, ab):
+        infos = requests[i][3]
+        a["box_pixels"] = [_pixel_box(infos[img], b + 1) for img, b in a["boxes"]]
+        if requests[i][4] in GROUNDING_TASKS:
+            a["answer_box"] = _pixel_box(infos[0], a["answer"])
+        answers[i] = {"answer": answers[i], "ablation": a}
+    return answers
+
+
 def _per_image(x, counts):
     """A per-image sequence as given, or one tensor over all images' rows split by `counts` (the reference's `.split`)."""
     if torch.is_tensor(x) or isinstance(x, np.ndarray):
