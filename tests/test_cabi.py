@@ -10,17 +10,9 @@ import torch
 import vilbert_b200 as vb
 from vilbert_b200 import _lib as L
 from vilbert_b200 import synthetic as S
+import support
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _tiny_cfg(**kw):
-    d = dict(hidden_size=128, num_attention_heads=2, intermediate_size=256, v_hidden_size=256,
-             v_num_attention_heads=2, v_intermediate_size=256, bi_hidden_size=256, bi_num_attention_heads=2,
-             bi_intermediate_size=256, vocab_size=512, v_feature_size=64, v_target_size=32,
-             max_position_embeddings=64, task_specific_tokens=True)
-    d.update(kw)
-    return vb.BertConfig(**d)
 
 
 def test_header_symbols_all_exported():
@@ -70,7 +62,7 @@ needs_no_gpu = pytest.mark.skipif(torch.cuda.is_available(), reason="checks the 
 
 @needs_no_gpu
 def test_good_checkpoint_fails_loudly_without_gpu():
-    cfg = _tiny_cfg()
+    cfg = support.tiny_cfg()
     sd = S.synthetic_state_dict(cfg, num_labels=40, gqa_labels=24, seed=1)
     rc, msg = _create(cfg, sd)
     assert rc == -5 and "no CPU fallback" in msg          # audit passed, then VB200_ERR_NO_DEVICE
@@ -79,7 +71,7 @@ def test_good_checkpoint_fails_loudly_without_gpu():
 
 
 def test_checkpoint_audit_missing_key():
-    cfg = _tiny_cfg()
+    cfg = support.tiny_cfg()
     sd = S.synthetic_state_dict(cfg, num_labels=40, gqa_labels=24, seed=1)
     del sd["bert.encoder.c_layer.3.biattention.query2.weight"]
     rc, msg = _create(cfg, sd)
@@ -87,7 +79,7 @@ def test_checkpoint_audit_missing_key():
 
 
 def test_checkpoint_audit_wrong_shape():
-    cfg = _tiny_cfg()
+    cfg = support.tiny_cfg()
     sd = S.synthetic_state_dict(cfg, num_labels=40, gqa_labels=24, seed=1)
     sd["bert.encoder.v_layer.0.output.dense.weight"] = torch.zeros(256, 128)
     rc, msg = _create(cfg, sd)
@@ -95,7 +87,7 @@ def test_checkpoint_audit_wrong_shape():
 
 
 def test_checkpoint_audit_unexpected_key_strict_and_lenient():
-    cfg = _tiny_cfg()
+    cfg = support.tiny_cfg()
     sd = S.synthetic_state_dict(cfg, num_labels=40, gqa_labels=24, seed=1)
     sd["bert.encoder.layer.0.some_new_thing.weight"] = torch.zeros(4, 4)
     rc, msg = _create(cfg, sd)
@@ -105,7 +97,7 @@ def test_checkpoint_audit_unexpected_key_strict_and_lenient():
 
 
 def test_checkpoint_audit_num_labels_mismatch():
-    cfg = _tiny_cfg()
+    cfg = support.tiny_cfg()
     sd = S.synthetic_state_dict(cfg, num_labels=40, gqa_labels=24, seed=1)
     rc, msg = _create(cfg, sd, num_labels=3129)
     assert rc == -3 and "num_labels" in msg
@@ -114,7 +106,7 @@ def test_checkpoint_audit_num_labels_mismatch():
 def test_reserved_ln_fold_option_rejected():
     """vb200_options::ln_fold is reserved since the LayerNorm fold was removed: a non-zero value is refused before the checkpoint
     audit, so with or without a device."""
-    cfg = _tiny_cfg()
+    cfg = support.tiny_cfg()
     sd = S.synthetic_state_dict(cfg, num_labels=40, gqa_labels=24, seed=1)
     rc, msg = _create(cfg, sd, ln_fold=1)
     assert rc == -1 and "LayerNorm fold was removed" in msg, (rc, msg)
@@ -124,7 +116,7 @@ def test_reserved_ln_fold_option_rejected():
 def test_reserved_fused_layernorm_option_rejected(split_fp32):
     """vb200_options::fused_layernorm is reserved since the cluster-LayerNorm GEMM epilogue was removed: a positive value is
     refused before the checkpoint audit, so with or without a device, and in fp32-parity mode too."""
-    cfg = _tiny_cfg()
+    cfg = support.tiny_cfg()
     sd = S.synthetic_state_dict(cfg, num_labels=40, gqa_labels=24, seed=1)
     rc, msg = _create(cfg, sd, fused_layernorm=1, split_fp32=split_fp32)
     assert rc == -1 and "cluster-LayerNorm GEMM epilogue was removed" in msg, (rc, msg)
@@ -134,7 +126,7 @@ def test_reserved_fused_layernorm_option_rejected(split_fp32):
 def test_fused_layernorm_off_values_accepted(value):
     """0 and negative fused_layernorm values ("off" in the tri-state convention) get past the option check: the checkpoint
     audit, which needs no device, then reports the missing key."""
-    cfg = _tiny_cfg()
+    cfg = support.tiny_cfg()
     sd = S.synthetic_state_dict(cfg, num_labels=40, gqa_labels=24, seed=1)
     del sd["bert.encoder.c_layer.3.biattention.query2.weight"]
     rc, msg = _create(cfg, sd, fused_layernorm=value)
@@ -156,7 +148,7 @@ def test_linear_rejects_layernorm_arguments(arg):
 
 
 def test_model_rejects_fused_layernorm():
-    cfg = _tiny_cfg()
+    cfg = support.tiny_cfg()
     sd = S.synthetic_state_dict(cfg, num_labels=40, gqa_labels=24, seed=1)
     with pytest.raises(ValueError, match="cluster-LayerNorm GEMM epilogue was removed"):
         vb.VILBertForVLTasks.from_pretrained(sd, config=cfg, num_labels=40, fused_layernorm=True)
@@ -164,7 +156,7 @@ def test_model_rejects_fused_layernorm():
 
 def test_checkpoint_legacy_names_accepted():
     """`module.` prefixes (DataParallel) and gamma/beta LayerNorm names ([UPSTREAM] from_pretrained fix-ups)."""
-    cfg = _tiny_cfg()
+    cfg = support.tiny_cfg()
     sd = S.synthetic_state_dict(cfg, num_labels=40, gqa_labels=24, seed=1)
     legacy = {}
     for k, v in sd.items():
@@ -185,8 +177,8 @@ def test_checkpoint_legacy_names_accepted():
     (dict(fusion_method="sum"), "fusion_method"),
 ])
 def test_config_rejections(kw, needle):
-    cfg = _tiny_cfg(**kw)
-    sd = S.synthetic_state_dict(_tiny_cfg(), num_labels=40, gqa_labels=24, seed=1)
+    cfg = support.tiny_cfg(**kw)
+    sd = S.synthetic_state_dict(support.tiny_cfg(), num_labels=40, gqa_labels=24, seed=1)
     rc, msg = _create(cfg, sd)
     assert rc == -2 and needle in msg, (rc, msg)
 
@@ -234,7 +226,7 @@ def test_bertconfig_protocol(tmp_path):
 
 
 def test_model_protocol_without_engine():
-    cfg = _tiny_cfg()
+    cfg = support.tiny_cfg()
     sd = S.synthetic_state_dict(cfg, num_labels=40, gqa_labels=24, seed=1)
     m = vb.VILBertForVLTasks.from_pretrained(sd, config=cfg, num_labels=40)
     assert m.eval() is m

@@ -15,15 +15,10 @@ from torch import nn
 
 from oracle import fp64 as X
 from oracle import vilbert_ref as R
+import support
 
 FLOOR = 1e-5             # fp32 oracle vs fp64 oracle: outputs and final states (rel_err)
 FLOOR_ATTENTION = 1e-6   # ... and attention maps (max abs)
-
-
-def _tiny_inputs(oracle, B, Tin, V, seed, pad=0):
-    inp = list(R.make_inputs(B, Tin, V, seed=seed, vocab_size=oracle.config.vocab_size, pad_regions=pad))
-    inp[1] = inp[1][..., :oracle.config.v_feature_size].contiguous()
-    return inp
 
 
 def _run(model, inp, pretraining=True):
@@ -59,7 +54,7 @@ def test_fp64_copy_leaves_the_oracle(tiny_oracle, tiny64):
 
 
 def test_fp64_oracle_runs_in_fp64(tiny64):
-    inp = _tiny_inputs(tiny64, 3, 16, 10, 9, pad=3)
+    inp = support.tiny_inputs(tiny64, 3, 16, 10, 9, pad=3)
     out, final = _run(tiny64, inp)
     for i, name in enumerate(X.OUTPUT_NAMES):
         assert out[i].dtype == torch.float64, name
@@ -83,7 +78,7 @@ def _check_floor(oracle, oracle64, inp, tag):
 
 @pytest.mark.parametrize("B,Tin,V,pad", [(2, 30, 36, 0), (3, 16, 10, 3), (1, 12, 37, 0), (4, 37, 101, 7), (2, 70, 100, 0)])
 def test_fp32_floor_tiny(tiny_oracle, tiny64, B, Tin, V, pad):
-    _check_floor(tiny_oracle, tiny64, _tiny_inputs(tiny_oracle, B, Tin, V, 500 + B, pad), f"tiny_B{B}_T{Tin}_V{V}")
+    _check_floor(tiny_oracle, tiny64, support.tiny_inputs(tiny_oracle, B, Tin, V, 500 + B, pad), f"tiny_B{B}_T{Tin}_V{V}")
 
 
 def test_fp32_floor_full(full_oracle):
@@ -173,7 +168,7 @@ DEFECTS = {
 
 @pytest.fixture(scope="module")
 def catalog_run(tiny64):
-    inp = _tiny_inputs(tiny64, 4, 37, 101, 504, pad=7)
+    inp = support.tiny_inputs(tiny64, 4, 37, 101, 504, pad=7)
     return inp, _run(tiny64, inp)
 
 

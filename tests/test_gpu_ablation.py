@@ -10,6 +10,8 @@ import ctypes as C
 import pytest
 import torch
 
+import support
+
 pytestmark = pytest.mark.gpu
 
 TOL = 1e-2                 # fp16 / bf16 vs the fp32 oracle (test_gpu_regions_packed.py)
@@ -18,61 +20,28 @@ VOCAB = {t: i for i, t in enumerate(["[PAD]", "[UNK]", "[CLS]", "[SEP]"])}     #
 FAMILY_OUT = {"vqa": 0, "gqa": 1, "snli_ve": 4}          # element of the 10-tuple each family's head is
 
 
-def _engine(oracle, **kw):
-    import vilbert_b200 as vb
-    cfg = vb.BertConfig.from_dict(oracle.config.to_dict())
-    return vb.VILBertForVLTasks.from_pretrained(oracle.state_dict(), config=cfg, num_labels=oracle.num_labels, **kw).eval().cuda(0)
-
-
 @pytest.fixture(scope="module")
 def tiny(tiny_oracle):
-    e = {k: _engine(tiny_oracle, compute_dtype=k) for k in ("fp16", "bf16")}
-    yield e
-    for m in e.values():
-        m.close()
+    yield from support.engines(tiny_oracle, ("fp16", "bf16"))
 
 
 @pytest.fixture(scope="module")
 def tiny_long(tiny_oracle):
-    m = _engine(tiny_oracle, compute_dtype="bf16", max_rows_per_sample=1024)
-    yield m
-    m.close()
+    yield from support.one_engine(tiny_oracle, compute_dtype="bf16", max_rows_per_sample=1024)
 
 
 @pytest.fixture(scope="module")
 def full(full_oracle):
-    m = _engine(full_oracle, compute_dtype="bf16")
-    yield m
-    m.close()
-
-
-def _image(tin, n, seed, F, vocab, wh=(640, 480)):
-    """One sample: tin token ids ([CLS] ... [SEP] shaped: ids >= 1) and segments, n detector boxes, the image size, a task id."""
-    g = torch.Generator().manual_seed(seed)
-    q = torch.randint(1, vocab, (tin,), generator=g)
-    seg = torch.randint(0, 2, (tin,), generator=g)
-    f = torch.relu(torch.randn(n, F, generator=g)) * 1.5
-    w, h = wh
-    x1, y1 = torch.rand(n, generator=g) * 0.7 * w, torch.rand(n, generator=g) * 0.7 * h
-    x2 = torch.minimum(x1 + (0.05 + 0.25 * torch.rand(n, generator=g)) * w, torch.tensor(float(w)))
-    y2 = torch.minimum(y1 + (0.05 + 0.25 * torch.rand(n, generator=g)) * h, torch.tensor(float(h)))
-    task = int(torch.randint(0, 20, (1,), generator=g))
-    return q, seg, f, torch.stack([x1, y1, x2, y2], 1), torch.tensor([float(w), float(h)]), task
+    yield from support.one_engine(full_oracle, compute_dtype="bf16")
 
 
 def _images(model, lens, seed):
     F, vocab = model._dims["v_feature_size"], model._dims["vocab_size"]
-    return [_image(t, n, seed + i, F, vocab, ((640, 480), (500, 375))[i % 2]) for i, (t, n) in enumerate(lens)]
-
-
-def _packed_args(imgs):
-    cat = lambda k: torch.cat([im[k] for im in imgs], dim=0).cuda()
-    return (cat(0), cat(1), torch.tensor([[im[5]] for im in imgs]).cuda(), cat(2), cat(3), torch.stack([im[4] for im in imgs]).cuda(),
-            [len(im[0]) for im in imgs], [im[2].shape[0] for im in imgs])
+    return [support.image(t, n, seed + i, F, vocab, ((640, 480), (500, 375))[i % 2]) for i, (t, n) in enumerate(lens)]
 
 
 def _ablate(model, imgs, **kw):
-    out = model.answer_ablation(*_packed_args(imgs), return_logits=True, mask_token=MASK, **kw)
+    out = model.answer_ablation(*support.packed_image_args(imgs), return_logits=True, mask_token=MASK, **kw)
     torch.cuda.synchronize()
     return out
 
@@ -97,7 +66,7 @@ def _forward(model, variants, family, **kw):
     """forward_regions_packed of the host-built variants: their head rows [n, width]."""
     import vilbert_b200 as vb
     bit = {"vqa": vb.OUT_VIL_PREDICTION, "gqa": vb.OUT_VIL_PREDICTION_GQA, "snli_ve": vb.OUT_VIL_TRI_PREDICTION}[family]
-    out, _ = model.forward_regions_packed(*_packed_args(variants), select=bit, return_spatials=False, **kw)
+    out, _ = model.forward_regions_packed(*support.packed_image_args(variants), select=bit, return_spatials=False, **kw)
     torch.cuda.synchronize()
     return out[FAMILY_OUT[family]]
 
@@ -234,13 +203,6 @@ def test_against_the_oracle(tiny, tiny_oracle):
     assert err < TOL, f"variant logits vs fp32 oracle: {err} >= {TOL}"
 
 
-def _n_plans(model):
-    from vilbert_b200 import _lib as L
-    v = C.c_int64()
-    L.check(L.load().vb200_model_dim(model._handle, b"n_plans", C.byref(v)), model._handle)
-    return v.value
-
-
 def test_plans_are_shared_and_forwards_unchanged(tiny):
     """Calls with other lengths in the same bucket and capacities build no plan; forwards around a call keep their bits."""
     model = tiny["bf16"]
@@ -248,9 +210,9 @@ def test_plans_are_shared_and_forwards_unchanged(tiny):
     fwd = lambda: _forward(model, imgs, "vqa", max_tokens=20, max_boxes=30)
     before = fwd()
     _ablate(model, imgs[:2], family="vqa", max_tokens=20, max_boxes=30)          # 1+10+20 + 1+5+9 = 46 -> 64
-    n = _n_plans(model)
+    n = support.n_plans(model)
     _ablate(model, imgs[1:], family="vqa", tokens=(1, 3), boxes_range=[(0, 9), (0, 20)], max_tokens=20, max_boxes=30)   # 13+23 -> 64
-    assert _n_plans(model) == n
+    assert support.n_plans(model) == n
     assert torch.equal(fwd(), before)
 
 
@@ -259,7 +221,7 @@ def test_back_to_back_calls_need_no_synchronisation(tiny):
     import vilbert_b200 as vb
     model = tiny["fp16"]
     sets = [_images(model, lens, seed=s) for s, lens in ((71, [(8, 5), (3, 2)]), (72, [(15, 40)]), (73, [(6, 3), (9, 9), (4, 2)]))]
-    args = [_packed_args(imgs) for imgs in sets]
+    args = [support.packed_image_args(imgs) for imgs in sets]
 
     def run(sync):
         outs = []
@@ -289,7 +251,7 @@ def test_rejections(tiny, tiny_oracle):
     from vilbert_b200 import _lib as L
     model = tiny["fp16"]
     imgs = _images(model, [(6, 3), (5, 1)], seed=81)
-    a = list(_packed_args(imgs))
+    a = list(support.packed_image_args(imgs))
     width = model._dims["num_labels"]
     logits = torch.full((64, width), 7.0, device="cuda")
     scores = torch.full((64, 4), 7, dtype=torch.int32, device="cuda")
@@ -333,13 +295,13 @@ def test_rejections(tiny, tiny_oracle):
         assert bool((logits == 7.0).all()) and bool((scores == 7).all()), kw
     # more than 1024 variants: 8 samples of 1 + 35 + 100 = 136
     big = _images(model, [(37, 100)] * 8, seed=90)
-    b = _packed_args(big)
+    b = support.packed_image_args(big)
     arr = (L.AblationMsg * 8)(*[L.AblationMsg(-1, 1, 36, 0, 100)] * 8)
     inp = L.PackedRegionInputs(8, 0, 0, vb.model._int32s(b[6]), vb.model._int32s(b[7]), *[t.data_ptr() for t in b[:6]], None)
     rc = lib.vb200_answer_ablation(model._handle, C.byref(inp), arr, L.DECODE_VQA, MASK, logits.data_ptr(), scores.data_ptr(), 0, stream)
     assert rc == -1 and "above 1024" in lib.vb200_last_error(model._handle).decode()
     # split_fp32 engines
-    x = _engine(tiny_oracle, compute_dtype="fp32x")
+    x = support.engine(tiny_oracle, compute_dtype="fp32x")
     try:
         rc, msg = call(m=x)
         assert rc == -1 and "split_fp32" in msg
@@ -357,7 +319,7 @@ def test_pretraining_engine_is_rejected():
     m = vb.BertForMultiModalPreTraining.from_pretrained(ref.state_dict(), config=cfg).eval().cuda(0)
     try:
         imgs = _images(m, [(5, 3)], seed=1)
-        a = _packed_args(imgs)
+        a = support.packed_image_args(imgs)
         arr = (L.AblationMsg * 1)(L.AblationMsg(-1, 1, 4, 0, 3))
         inp = L.PackedRegionInputs(1, 0, 0, vb.model._int32s(a[6]), vb.model._int32s(a[7]), *[t.data_ptr() for t in a[:6]], None)
         logits = torch.full((8, 4), 7.0, device="cuda")

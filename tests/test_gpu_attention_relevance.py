@@ -14,6 +14,7 @@ import pytest
 import torch
 
 from relevance_ref import attention_relevance_f32, attention_relevance_f64, sample_maps
+import support
 
 pytestmark = pytest.mark.gpu
 
@@ -24,24 +25,9 @@ TOL_ORACLE = 4e-5          # per entry, the bf16 engine's relevance vs the fp32 
 SENTINEL = -7.0
 
 
-def _lib():
-    from vilbert_b200 import _lib as L
-    return L
-
-
-def _engine(oracle, **kw):
-    import vilbert_b200 as vb
-    cfg = vb.BertConfig.from_dict(oracle.config.to_dict())
-    return vb.VILBertForVLTasks.from_pretrained(oracle.state_dict(), config=cfg, num_labels=oracle.num_labels, return_attention=True,
-                                                **kw).eval().cuda(0)
-
-
 @pytest.fixture(scope="module")
 def tiny(tiny_oracle):
-    e = {k: _engine(tiny_oracle, compute_dtype=k) for k in ("fp16", "bf16", "fp32x")}
-    yield e
-    for m in e.values():
-        m.close()
+    yield from support.engines(tiny_oracle, ("fp16", "bf16", "fp32x"), return_attention=True)
 
 
 def _kinds(model):
@@ -50,13 +36,6 @@ def _kinds(model):
 
 def _task(model):
     return 1 if model._dims["task_specific_tokens"] else 0
-
-
-def _tiny_inputs(oracle, B, Tin, V, seed, pad=0):
-    from oracle import vilbert_ref as R
-    inp = list(R.make_inputs(B, Tin, V, seed=seed, vocab_size=oracle.config.vocab_size, pad_regions=pad))
-    inp[1] = inp[1][..., :oracle.config.v_feature_size].contiguous()
-    return [t.cuda() for t in inp]
 
 
 def _dense(model, inp):
@@ -91,7 +70,7 @@ def _check_refs(model, attn, rel, packed, tol_f64=TOL_F64):
 @pytest.mark.parametrize("B,pad", [(2, 0), (3, 4)])
 def test_dense_bitwise(tiny, tiny_oracle, mode, B, pad):
     model = tiny[mode]
-    inp = _tiny_inputs(tiny_oracle, B, 16, 12, seed=31 + B, pad=pad)
+    inp = [t.cuda() for t in support.tiny_inputs(tiny_oracle, B, 16, 12, seed=31 + B, pad=pad)]
     attn = _dense(model, inp)
     rel = model.attention_relevance(attn)
     torch.cuda.synchronize()
@@ -106,8 +85,8 @@ def test_dense_bitwise(tiny, tiny_oracle, mode, B, pad):
 
 def test_heads_all_and_mean_same_bits(tiny, tiny_oracle):
     model = tiny["bf16"]
-    inp = _tiny_inputs(tiny_oracle, 2, 9, 7, seed=5, pad=2)
-    samples = _batch(model, [(4, 9), (13, 2)], seed=3)
+    inp = [t.cuda() for t in support.tiny_inputs(tiny_oracle, 2, 9, 7, seed=5, pad=2)]
+    samples = support.batch(model, [(4, 9), (13, 2)], seed=3)
     full_d = model.attention_relevance(_dense(model, inp))
     full_p = model.attention_relevance(_packed(model, samples))
     model.set_option("attention_heads", 1)
@@ -123,41 +102,15 @@ def test_heads_all_and_mean_same_bits(tiny, tiny_oracle):
 
 
 # ------------------------------------------------------------------------------------------------------------ packed
-def _sample(tin, v, seed, F, vocab):
-    g = torch.Generator().manual_seed(seed)
-    q = torch.randint(1, vocab, (tin,), generator=g)
-    f = torch.relu(torch.randn(v, F, generator=g)) * 1.5
-    x1, y1 = torch.rand(v, generator=g) * 0.7, torch.rand(v, generator=g) * 0.7
-    x2, y2 = x1 + 0.05 + torch.rand(v, generator=g) * 0.25, y1 + 0.05 + torch.rand(v, generator=g) * 0.25
-    s = torch.stack([x1, y1, x2.clamp(max=1.0), y2.clamp(max=1.0), (x2 - x1) * (y2 - y1)], dim=-1)
-    s[0] = torch.tensor([0.0, 0.0, 1.0, 1.0, 1.0])
-    seg = torch.randint(0, 2, (tin,), generator=g)
-    return q, seg, f, s, int(torch.randint(0, 20, (1,), generator=g))
-
-
-def _batch(model, lens, seed):
-    F, vocab = model._dims["v_feature_size"], model._dims["vocab_size"]
-    return [_sample(t, v, seed + i, F, vocab) for i, (t, v) in enumerate(lens)]
-
-
-def _packed_args(samples):
-    cat = lambda k: torch.cat([s[k] for s in samples], dim=0).cuda()
-    task = torch.tensor([[s[4]] for s in samples]).cuda()
-    return cat(0), cat(2), cat(3), cat(1), task, [len(s[0]) for s in samples], [s[2].shape[0] for s in samples]
-
-
 def _packed(model, samples):
-    out = model.forward_packed(*_packed_args(samples), output_all_attention_masks=True)
+    out = model.forward_packed(*support.packed_sample_args(samples), output_all_attention_masks=True)
     torch.cuda.synchronize()
     return out[9]
 
 
 def _alone(model, smp):
     """Relevance of a batch-1 dense forward of one packed sample: [2, T + V]."""
-    q, seg, f, s, task = smp
-    out = model(q[None].cuda(), f[None].cuda(), s[None].cuda(), seg[None].cuda(), torch.ones(1, len(q), dtype=torch.long).cuda(),
-                torch.ones(1, f.shape[0], dtype=torch.uint8).cuda(), None, torch.tensor([[task]]).cuda(), output_all_attention_masks=True)
-    return model.attention_relevance(out[9])[0]
+    return model.attention_relevance(support.dense_alone(model, smp, output_all_attention_masks=True)[9])[0]
 
 
 LENS = [(1, 40), (31, 1), (12, 64), (5, 17)]
@@ -166,7 +119,7 @@ LENS = [(1, 40), (31, 1), (12, 64), (5, 17)]
 @pytest.mark.parametrize("mode", ("fp16", "bf16"))
 def test_packed_bitwise_and_alone(tiny, mode):
     model = tiny[mode]
-    samples = _batch(model, LENS, seed=11)
+    samples = support.batch(model, LENS, seed=11)
     attn = _packed(model, samples)
     rel = model.attention_relevance(attn)
     torch.cuda.synchronize()
@@ -202,9 +155,9 @@ def test_long_rows(tiny_oracle):
     alone, and within the derived L1 bound of float64."""
     from oracle import vilbert_ref as R
     oracle = R.build(R.tiny_config(max_position_embeddings=1024), seed=7, num_labels=200)
-    model = _engine(oracle, compute_dtype="bf16", max_rows_per_sample=1024)
+    model = support.engine(oracle, compute_dtype="bf16", max_rows_per_sample=1024, return_attention=True)
     try:
-        samples = _batch(model, [(300, 20), (10, 1024), (3, 3)], seed=50)
+        samples = support.batch(model, [(300, 20), (10, 1024), (3, 3)], seed=50)
         attn = _packed(model, samples)
         rel = model.attention_relevance(attn)
         torch.cuda.synchronize()
@@ -225,7 +178,7 @@ def test_long_rows(tiny_oracle):
 # ------------------------------------------------------------------------------------------------------------ full model
 def test_full_model_bf16(full_oracle, parity_log):
     from oracle import vilbert_ref as R
-    model = _engine(full_oracle, compute_dtype="bf16")
+    model = support.engine(full_oracle, compute_dtype="bf16", return_attention=True)
     try:
         kinds = _kinds(model)
         assert len(kinds) == 30
@@ -247,7 +200,7 @@ def test_full_model_bf16(full_oracle, parity_log):
         parity_log(test="relevance_full_bf16_vs_oracle_maps", max_abs_err=d_oracle)
         assert d_oracle < TOL_ORACLE, d_oracle
         # packed samples == each sample's dense forward alone
-        samples = _batch(model, [(37, 101), (5, 10), (20, 36)], seed=90)
+        samples = support.batch(model, [(37, 101), (5, 10), (20, 36)], seed=90)
         prel = model.attention_relevance(_packed(model, samples))
         for b, smp in enumerate(samples):
             assert torch.equal(prel[b], _alone(model, smp)), b
@@ -271,28 +224,22 @@ def _raw_args(model, attn):
 
 
 def _call(model, ptr, B, nt, nv, packed, out):
-    L = _lib()
+    L = support.lib()
     stream = torch.cuda.current_stream().cuda_stream
     return L.load().vb200_attention_relevance(model._handle, C.c_void_p(ptr), B, C.cast(nt, C.c_void_p), C.cast(nv, C.c_void_p),
                                               packed, C.c_void_p(out.data_ptr() if out is not None else None), C.c_void_p(stream))
 
 
-def _n_plans(model):
-    L = _lib()
-    v = C.c_int64()
-    L.check(L.load().vb200_model_dim(model._handle, b"n_plans", C.byref(v)), model._handle)
-    return v.value
-
-
 def test_every_float_written_maps_unchanged_repeatable(tiny, tiny_oracle):
     model = tiny["fp16"]
-    for attn in (_dense(model, _tiny_inputs(tiny_oracle, 3, 10, 9, seed=2, pad=3)), _packed(model, _batch(model, LENS, seed=4))):
+    for attn in (_dense(model, [t.cuda() for t in support.tiny_inputs(tiny_oracle, 3, 10, 9, seed=2, pad=3)]),
+                 _packed(model, support.batch(model, LENS, seed=4))):
         ptr, B, nt, nv, packed, n = _raw_args(model, attn)
         flat = attn[0] if not packed else attn[0][0]
         storage = flat.untyped_storage()
         before = torch.empty(storage.nbytes() // 4, dtype=torch.float32, device="cuda")
         before.untyped_storage().copy_(storage)
-        plans = _n_plans(model)
+        plans = support.n_plans(model)
         outs = [torch.full((n,), float("nan"), device="cuda") for _ in range(3)]
         for o in outs:                                         # back to back, no synchronisation in between
             assert _call(model, ptr, B, nt, nv, packed, o) == 0
@@ -302,13 +249,13 @@ def test_every_float_written_maps_unchanged_repeatable(tiny, tiny_oracle):
         after = torch.empty_like(before)
         after.untyped_storage().copy_(storage)
         assert torch.equal(before, after)
-        assert _n_plans(model) == plans
+        assert support.n_plans(model) == plans
 
 
 def test_rejections_leave_output_untouched(tiny, tiny_oracle):
-    L = _lib()
+    L = support.lib()
     model = tiny["fp16"]
-    attn = _packed(model, _batch(model, LENS, seed=4))
+    attn = _packed(model, support.batch(model, LENS, seed=4))
     ptr, B, nt, nv, packed, n = _raw_args(model, attn)
     out = torch.full((n,), SENTINEL, device="cuda")
 
@@ -332,7 +279,7 @@ def test_rejections_leave_output_untouched(tiny, tiny_oracle):
     model.set_option("attention_entries", ((1 << 30) - 1) & ~(1 << 3))
     try:
         rejected(_call(model, ptr, B, nt, nv, 1, out), "entry 3 ")
-        sel = model.forward_packed(*_packed_args(_batch(model, LENS, seed=4)), output_all_attention_masks=True)[9]
+        sel = model.forward_packed(*support.packed_sample_args(support.batch(model, LENS, seed=4)), output_all_attention_masks=True)[9]
         with pytest.raises(ValueError, match="None"):
             model.attention_relevance(sel)
     finally:

@@ -11,6 +11,8 @@ import numpy as np
 import pytest
 import torch
 
+import support
+
 pytestmark = pytest.mark.gpu
 
 MODES = ("fp16", "bf16", "fp32x")
@@ -18,24 +20,9 @@ TOL_ATTN = 5e-3            # engine (fp16) vs the fp32 oracle's attention probab
 NAN = float("nan")
 
 
-def _lib():
-    from vilbert_b200 import _lib as L
-    return L
-
-
-def _engine(oracle, **kw):
-    import vilbert_b200 as vb
-    cfg = vb.BertConfig.from_dict(oracle.config.to_dict())
-    return vb.VILBertForVLTasks.from_pretrained(oracle.state_dict(), config=cfg, num_labels=oracle.num_labels, return_attention=True,
-                                                **kw).eval().cuda(0)
-
-
 @pytest.fixture(scope="module")
 def tiny(tiny_oracle):
-    e = {k: _engine(tiny_oracle, compute_dtype=k) for k in MODES}
-    yield e
-    for m in e.values():
-        m.close()
+    yield from support.engines(tiny_oracle, MODES, return_attention=True)
 
 
 class _Selected:
@@ -92,13 +79,6 @@ def _entry(attn, where):
     return attn[pos] if d is None else attn[pos][d]
 
 
-def _tiny_inputs(oracle, B, Tin, V, seed, pad=0):
-    from oracle import vilbert_ref as R
-    inp = list(R.make_inputs(B, Tin, V, seed=seed, vocab_size=oracle.config.vocab_size, pad_regions=pad))
-    inp[1] = inp[1][..., :oracle.config.v_feature_size].contiguous()
-    return [t.cuda() for t in inp]
-
-
 def _dense(model, inp, maps=True):
     out = model(*inp, output_all_attention_masks=maps, debug_taps=True)
     torch.cuda.synchronize()
@@ -146,9 +126,9 @@ def _check_selected(attn, full, kinds, entries, mean, axis=1):
 @pytest.mark.parametrize("mode", MODES)
 @pytest.mark.parametrize("B,pad", [(2, 0), (3, 2)])
 def test_dense_selected_entries_bitwise(tiny, tiny_oracle, mode, B, pad):
-    L = _lib()
+    L = support.lib()
     model = tiny[mode]
-    inp = _tiny_inputs(tiny_oracle, B, 14, 11, seed=300 + B, pad=pad)
+    inp = [t.cuda() for t in support.tiny_inputs(tiny_oracle, B, 14, 11, seed=300 + B, pad=pad)]
     full = _dense(model, inp)
     plain = _dense(model, inp, maps=False)
     _same_outputs(full, plain)
@@ -167,9 +147,9 @@ def test_dense_selected_entries_bitwise(tiny, tiny_oracle, mode, B, pad):
 # ------------------------------------------------------------------------------------------------------------ dense, head mean
 @pytest.mark.parametrize("mode", MODES)
 def test_dense_head_mean_bitwise(tiny, tiny_oracle, mode):
-    L = _lib()
+    L = support.lib()
     model = tiny[mode]
-    inp = _tiny_inputs(tiny_oracle, 3, 20, 12, seed=61, pad=2)
+    inp = [t.cuda() for t in support.tiny_inputs(tiny_oracle, 3, 20, 12, seed=61, pad=2)]
     full = _dense(model, inp)
     plain = _dense(model, inp, maps=False)
     kinds = _kinds(model)
@@ -186,7 +166,7 @@ def test_dense_head_mean_bitwise(tiny, tiny_oracle, mode):
 
 def test_head_mean_vs_oracle(tiny, tiny_oracle, parity_log):
     """The fp32 oracle's maps averaged over heads, at the tolerance of the per-head maps."""
-    inp = _tiny_inputs(tiny_oracle, 3, 20, 12, seed=61, pad=2)
+    inp = [t.cuda() for t in support.tiny_inputs(tiny_oracle, 3, 20, 12, seed=61, pad=2)]
     ref = tiny_oracle(*[t.cpu() for t in inp], output_all_attention_masks=True)[9]
     model = tiny["fp16"]
     with _Selected(model, None, "mean"):
@@ -202,45 +182,16 @@ def test_head_mean_vs_oracle(tiny, tiny_oracle, parity_log):
 
 
 # ------------------------------------------------------------------------------------------------------------ packed
-def _sample(tin, v, seed, F, vocab):
-    g = torch.Generator().manual_seed(seed)
-    q = torch.randint(1, vocab, (tin,), generator=g)
-    f = torch.relu(torch.randn(v, F, generator=g)) * 1.5
-    x1, y1 = torch.rand(v, generator=g) * 0.7, torch.rand(v, generator=g) * 0.7
-    x2, y2 = x1 + 0.05 + torch.rand(v, generator=g) * 0.25, y1 + 0.05 + torch.rand(v, generator=g) * 0.25
-    s = torch.stack([x1, y1, x2.clamp(max=1.0), y2.clamp(max=1.0), (x2 - x1) * (y2 - y1)], dim=-1)
-    s[0] = torch.tensor([0.0, 0.0, 1.0, 1.0, 1.0])
-    seg = torch.randint(0, 2, (tin,), generator=g)
-    return q, seg, f, s, int(torch.randint(0, 20, (1,), generator=g))
-
-
-def _batch(model, lens, seed):
-    F, vocab = model._dims["v_feature_size"], model._dims["vocab_size"]
-    return [_sample(t, v, seed + i, F, vocab) for i, (t, v) in enumerate(lens)]
-
-
-def _packed_args(samples):
-    cat = lambda k: torch.cat([s[k] for s in samples], dim=0).cuda()
-    task = torch.tensor([[s[4]] for s in samples]).cuda()
-    return cat(0), cat(2), cat(3), cat(1), task, [len(s[0]) for s in samples], [s[2].shape[0] for s in samples]
-
-
 def _packed(model, samples, maps=True, sync=True):
-    L = _lib()
-    out = model.forward_packed(*_packed_args(samples), select=L.OUT_TASK_HEADS, debug_taps=True, output_all_attention_masks=maps)
+    L = support.lib()
+    out = model.forward_packed(*support.packed_sample_args(samples), select=L.OUT_TASK_HEADS, debug_taps=True, output_all_attention_masks=maps)
     if sync:
         torch.cuda.synchronize()
     return out
 
 
 def _alone(model, smp):
-    L = _lib()
-    q, seg, f, s, task = smp
-    out = model(q[None].cuda(), f[None].cuda(), s[None].cuda(), seg[None].cuda(), torch.ones(1, len(q), dtype=torch.long).cuda(),
-                torch.ones(1, f.shape[0], dtype=torch.uint8).cuda(), None, torch.tensor([[task]]).cuda(), select=L.OUT_TASK_HEADS,
-                output_all_attention_masks=True)
-    torch.cuda.synchronize()
-    return out[9]
+    return support.dense_alone(model, smp, select=support.lib().OUT_TASK_HEADS, output_all_attention_masks=True)[9]
 
 
 def _check_packed_vs_alone(attn, alone, kinds, entries):
@@ -260,7 +211,7 @@ LENS = [(1, 40), (31, 1), (12, 64), (5, 17)]
 @pytest.mark.parametrize("mode", ("fp16", "bf16"))
 def test_packed_selection(tiny, mode):
     model = tiny[mode]
-    samples = _batch(model, LENS, seed=900)
+    samples = support.batch(model, LENS, seed=900)
     full = _packed(model, samples)
     plain = _packed(model, samples, maps=False)
     kinds = _kinds(model)
@@ -276,7 +227,7 @@ def test_packed_selection(tiny, mode):
 
 
 def test_regions_packed_selection(tiny):
-    L = _lib()
+    L = support.lib()
     model = tiny["bf16"]
     F, vocab = model._dims["v_feature_size"], model._dims["vocab_size"]
     imgs = []
@@ -313,10 +264,10 @@ def test_long_rows_head_mean(tiny_oracle):
     1024-key accumulators; each packed sample equals its dense forward alone, and the dense mean equals the per-head maps' mean."""
     from oracle import vilbert_ref as R
     oracle = R.build(R.tiny_config(max_position_embeddings=1024), seed=7, num_labels=200)
-    model = _engine(oracle, compute_dtype="bf16", max_rows_per_sample=1024)
+    model = support.engine(oracle, compute_dtype="bf16", max_rows_per_sample=1024, return_attention=True)
     try:
         kinds = _kinds(model)
-        samples = _batch(model, [(300, 20), (10, 1024), (3, 3)], seed=50)
+        samples = support.batch(model, [(300, 20), (10, 1024), (3, 3)], seed=50)
         full_alone = [_alone(model, s) for s in samples]
         entries = list(range(len(kinds)))
         with _Selected(model, entries, "mean"):
@@ -331,7 +282,7 @@ def test_long_rows_head_mean(tiny_oracle):
 
 def test_full_model_bf16_selection(full_oracle):
     from oracle import vilbert_ref as R
-    model = _engine(full_oracle, compute_dtype="bf16")
+    model = support.engine(full_oracle, compute_dtype="bf16", return_attention=True)
     try:
         inp = [t.cuda() for t in R.make_inputs(2, 30, 36, seed=808, pad_regions=3)]
         full = _dense(model, inp)
@@ -380,7 +331,7 @@ def test_layouts_follow_selection(tiny):
                 off += h * sum(a * b for a, b in zip(lq, lk))
             assert total_p == off
             v = C.c_int64()
-            L = _lib()
+            L = support.lib()
             L.check(L.load().vb200_model_dim(model._handle, b"attention_entries", C.byref(v)), model._handle)
             assert v.value == sum(1 << e for e in entries)
             L.check(L.load().vb200_model_dim(model._handle, b"attention_heads", C.byref(v)), model._handle)
@@ -390,13 +341,13 @@ def test_layouts_follow_selection(tiny):
 
 def test_every_float_written(tiny, tiny_oracle):
     """A NaN-filled buffer has no NaN left after a dense or packed forward under a selection."""
-    L = _lib()
+    L = support.lib()
     model = tiny["bf16"]
     dev = torch.device("cuda", 0)
     entries = _selections(model)["first_last"] + _selections(model)["one_t2i"]
     for heads in ("all", "mean"):
         with _Selected(model, entries, heads):
-            q, f, s, seg, im, vm, co, tk = _tiny_inputs(tiny_oracle, 3, 9, 7, seed=5, pad=2)
+            q, f, s, seg, im, vm, co, tk = [t.cuda() for t in support.tiny_inputs(tiny_oracle, 3, 9, 7, seed=5, pad=2)]
             outs, o, select = model._alloc_outputs(3, 9, 7, L.OUT_TASK_HEADS, False, True, dev)
             outs["attention_probs"].fill_(NAN)
             inp = L.Inputs(3, 9, 7, q.data_ptr(), f.data_ptr(), s.data_ptr(), seg.data_ptr(), im.data_ptr(), vm.data_ptr(), None,
@@ -405,8 +356,8 @@ def test_every_float_written(tiny, tiny_oracle):
             torch.cuda.synchronize()
             assert not torch.isnan(outs["attention_probs"]).any()
 
-            samples = _batch(model, LENS, seed=11)
-            qp, fp, sp, segp, tkp, nt, nv = _packed_args(samples)
+            samples = support.batch(model, LENS, seed=11)
+            qp, fp, sp, segp, tkp, nt, nv = support.packed_sample_args(samples)
             _, total = model.attention_layout_packed(nt, nv)
             flat = torch.full((total,), NAN, device=dev)
             rows_t = sum(nt) + len(nt)
@@ -421,41 +372,34 @@ def test_every_float_written(tiny, tiny_oracle):
 
 
 # ------------------------------------------------------------------------------------------------------------ changing the selection
-def _n_plans(model):
-    L = _lib()
-    v = C.c_int64()
-    L.check(L.load().vb200_model_dim(model._handle, b"n_plans", C.byref(v)), model._handle)
-    return v.value
-
-
 def test_change_selection_between_calls(tiny_oracle):
-    model = _engine(tiny_oracle, compute_dtype="fp16")
+    model = support.engine(tiny_oracle, compute_dtype="fp16", return_attention=True)
     try:
-        inp = _tiny_inputs(tiny_oracle, 2, 8, 6, seed=3)
+        inp = [t.cuda() for t in support.tiny_inputs(tiny_oracle, 2, 8, 6, seed=3)]
         kinds = _kinds(model)
         full = _dense(model, inp)[0][9]
-        plans = _n_plans(model)
+        plans = support.n_plans(model)
         sel = _selections(model)
         with _Selected(model, sel["connection"]):
             _check_selected(_dense(model, inp)[0][9], full, kinds, sel["connection"], mean=False)
-        assert _n_plans(model) == plans + 1
+        assert support.n_plans(model) == plans + 1
         _check_selected(_dense(model, inp)[0][9], full, kinds, list(range(len(kinds))), mean=False)
-        assert _n_plans(model) == plans + 1                   # the default selection's plan is reused
+        assert support.n_plans(model) == plans + 1                   # the default selection's plan is reused
         with _Selected(model, sel["connection"], "mean"):
             _check_selected(_dense(model, inp)[0][9], full, kinds, sel["connection"], mean=True)
-        assert _n_plans(model) == plans + 2
+        assert support.n_plans(model) == plans + 2
         with _Selected(model, sel["connection"]):
             _dense(model, inp)
-        assert _n_plans(model) == plans + 2                   # and so is the first selection's
+        assert support.n_plans(model) == plans + 2                   # and so is the first selection's
 
         # unsynchronised back-to-back packed calls under different selections, each into its own buffer
-        samples = _batch(model, LENS, seed=21)
+        samples = support.batch(model, LENS, seed=21)
         pfull = _packed(model, samples)[0][9]
-        a = model.forward_packed(*_packed_args(samples), debug_taps=True, output_all_attention_masks=True)
+        a = model.forward_packed(*support.packed_sample_args(samples), debug_taps=True, output_all_attention_masks=True)
         model.set_option("attention_entries", 1 << 3)
-        b = model.forward_packed(*_packed_args(samples), debug_taps=True, output_all_attention_masks=True)
+        b = model.forward_packed(*support.packed_sample_args(samples), debug_taps=True, output_all_attention_masks=True)
         model.set_option("attention_heads", 1)
-        c = model.forward_packed(*_packed_args(samples), debug_taps=True, output_all_attention_masks=True)
+        c = model.forward_packed(*support.packed_sample_args(samples), debug_taps=True, output_all_attention_masks=True)
         torch.cuda.synchronize()
         _check_selected(a[0][9], pfull, kinds, list(range(len(kinds))), mean=False, axis=0)
         _check_selected(b[0][9], pfull, kinds, [3], mean=False, axis=0)
@@ -466,7 +410,7 @@ def test_change_selection_between_calls(tiny_oracle):
 
 # ------------------------------------------------------------------------------------------------------------ rejections
 def test_rejections(tiny):
-    L = _lib()
+    L = support.lib()
     model = tiny["fp16"]
     n = len(_kinds(model))
     for key, value, msg in (("attention_entries", 0, "attention_entries"), ("attention_entries", 1 << n, "attention_entries"),

@@ -11,6 +11,8 @@ import numpy as np
 import pytest
 import torch
 
+import support
+
 pytestmark = pytest.mark.gpu
 
 WIDTHS = {"1": 3129, "15": 1533, "12": 2, "13": 3}
@@ -19,46 +21,26 @@ VOCAB = {t: i for i, t in enumerate(["[PAD]", "[UNK]", "[CLS]", "[SEP]", "what",
                                      "?", "color", "of", "un", "##aff", "##able", ",", "a", "dog", "on", "grass"])}
 
 
-def _tiny_cfg():
-    import vilbert_b200 as vb
-    return vb.BertConfig(hidden_size=128, num_attention_heads=2, intermediate_size=256, v_hidden_size=256, v_num_attention_heads=2,
-                         v_intermediate_size=256, bi_hidden_size=256, bi_num_attention_heads=2, bi_intermediate_size=256,
-                         vocab_size=512, v_feature_size=64, v_target_size=32, max_position_embeddings=64, task_specific_tokens=True)
-
-
 @pytest.fixture(scope="module")
 def eng():
     """A small engine with the worker's head widths (3129 VQA labels, 1533 GQA labels): the decode reads widths from the engine."""
     import vilbert_b200 as vb
     from vilbert_b200 import synthetic as S
-    cfg = _tiny_cfg()
+    cfg = support.tiny_cfg()
     m = vb.VILBertForVLTasks.from_pretrained(S.synthetic_state_dict(cfg, num_labels=3129, gqa_labels=1533, seed=3), config=cfg,
                                              num_labels=3129).eval().cuda(0)
     yield m
     m.close()
 
 
-def _oracle_engine(oracle, dtype):
-    import vilbert_b200 as vb
-    cfg = vb.BertConfig.from_dict(oracle.config.to_dict())
-    return vb.VILBertForVLTasks.from_pretrained(oracle.state_dict(), config=cfg, num_labels=oracle.num_labels,
-                                                compute_dtype=dtype).eval().cuda(0)
-
-
 @pytest.fixture(scope="module")
 def tiny(tiny_oracle):
-    e = {k: _oracle_engine(tiny_oracle, k) for k in DT}
-    yield e
-    for m in e.values():
-        m.close()
+    yield from support.engines(tiny_oracle, DT)
 
 
 @pytest.fixture(scope="module")
 def full(full_oracle):
-    e = {k: _oracle_engine(full_oracle, k) for k in DT}
-    yield e
-    for m in e.values():
-        m.close()
+    yield from support.engines(full_oracle, DT)
 
 
 def _gapped(n, g, planted=11):
@@ -238,19 +220,6 @@ def test_decode_real_forwards(which, request):
 
 
 # ----------------------------------------------------------------------------------------------- the worker
-def _detector_output(n_boxes, F, seed):
-    g = torch.Generator().manual_seed(seed)
-    feats, infos = [], []
-    for i, n in enumerate(n_boxes):
-        w, h = WHS[i % 4]
-        feats.append(torch.relu(torch.randn(n, F, generator=g)) * 1.5)
-        x1, y1 = torch.rand(n, generator=g) * 0.7 * w, torch.rand(n, generator=g) * 0.7 * h
-        bw, bh = (0.05 + 0.25 * torch.rand(n, generator=g)) * w, (0.05 + 0.25 * torch.rand(n, generator=g)) * h
-        bbox = torch.stack([x1, y1, torch.minimum(x1 + bw, torch.tensor(float(w))), torch.minimum(y1 + bh, torch.tensor(float(h)))], 1)
-        infos.append({"image_width": w, "image_height": h, "bbox": bbox.numpy().astype(np.float32)})
-    return feats, infos
-
-
 MESSAGES = [("1", [36], "what is the man holding?"), ("12", [20, 20], "the man is holding a dog"), ("7", [30, 30, 30], "a dog on the grass"),
             ("11", [25], "the man"), ("13", [8], "a dog"), ("15", [100], "what is the color of the dog"), ("4", [50], "a dog"),
             ("16", [12], "the grass")]
@@ -278,7 +247,7 @@ def test_worker_device_decode_matches_host(full):
     F = model._dims["v_feature_size"]
     msgs = []
     for k, (task_id, counts, q) in enumerate(MESSAGES):
-        feats, infos = _detector_output(counts, F, seed=700 + k)
+        feats, infos = support.detector_output(counts, F, wh=WHS, seed=700 + k)
         body = {"image_path": [f"/m/demo/i{j}.jpg" for j in range(len(counts))], "question": q, "socket_id": f"s{k}", "task_id": task_id}
         msgs.append((body, feats, infos))
     res = {}
@@ -298,7 +267,7 @@ def test_worker_device_decode_matches_host(full):
             assert ra["image_name_list"] == rb["image_name_list"]
             assert ra["confidence_list"] == pytest.approx(rb["confidence_list"], abs=1e-4)
     # the answer dicts themselves: custom_prediction_packed and prediction_batch (dense), device against host
-    reqs = [(q, [int(t)], *_detector_output(c, F, seed=800 + k), t) for k, (t, c, q) in enumerate(MESSAGES)]
+    reqs = [(q, [int(t)], *support.detector_output(c, F, wh=WHS, seed=800 + k), t) for k, (t, c, q) in enumerate(MESSAGES)]
     for a, b in zip(W.custom_prediction_packed(reqs, decode="device"), W.custom_prediction_packed(reqs, decode="host")):
         _same(a, b)
     dev = torch.device("cuda", 0)

@@ -21,27 +21,12 @@ import pytest
 import torch
 
 from oracle import fp64 as X
+import support
 
 pytestmark = pytest.mark.gpu
 
 VOCAB = {t: i for i, t in enumerate(["[PAD]", "[UNK]", "[CLS]", "[SEP]", "what", "is", "the", "man", "hold", "##ing",
                                      "?", "color", "of", "un", "##aff", "##able", ",", "a", "dog", "on", "grass"])}
-
-
-def _engine(oracle, cls=None, **kw):
-    import vilbert_b200 as vb
-    cfg = vb.BertConfig.from_dict(oracle.config.to_dict())
-    if cls is None:
-        return vb.VILBertForVLTasks.from_pretrained(oracle.state_dict(), config=cfg, num_labels=oracle.num_labels,
-                                                    compute_dtype="fp32x", **kw).eval().cuda(0)
-    return cls.from_pretrained(oracle.state_dict(), config=cfg, compute_dtype="fp32x", **kw).eval().cuda(0)
-
-
-def _tiny_inputs(oracle, B, Tin, V, seed, pad=0):
-    from oracle import vilbert_ref as R
-    inp = list(R.make_inputs(B, Tin, V, seed=seed, vocab_size=oracle.config.vocab_size, pad_regions=pad))
-    inp[1] = inp[1][..., :oracle.config.v_feature_size].contiguous()
-    return inp
 
 
 def _check(tag, parity_log, logits=None, states=None, attention=None, losses=None):
@@ -84,16 +69,12 @@ def full64(full_oracle):
 
 @pytest.fixture(scope="module")
 def tiny_x(tiny_oracle):
-    m = _engine(tiny_oracle, return_attention=True)
-    yield m
-    m.close()
+    yield from support.one_engine(tiny_oracle, compute_dtype="fp32x", return_attention=True)
 
 
 @pytest.fixture(scope="module")
 def full_x(full_oracle):
-    m = _engine(full_oracle, return_attention=True)
-    yield m
-    m.close()
+    yield from support.one_engine(full_oracle, compute_dtype="fp32x", return_attention=True)
 
 
 # ------------------------------------------------------------------ the split GEMM
@@ -131,7 +112,7 @@ def test_split_gemm_error_does_not_grow_with_k(K, parity_log):
                                          (1, 3, 1, 0), (1, 155, 256, 11), (5, 3, 7, 2)])
 def test_tiny_dense(tiny_oracle, tiny64, tiny_x, parity_log, B, Tin, V, pad):
     """The shapes of test_fp32x_tiny_all_outputs and the corners of test_tiny_model_all_outputs, with the pre-training heads."""
-    _forward(tiny64, tiny_x, _tiny_inputs(tiny_oracle, B, Tin, V, 500 + B, pad), f"tiny_B{B}_T{Tin}_V{V}", parity_log)
+    _forward(tiny64, tiny_x, support.tiny_inputs(tiny_oracle, B, Tin, V, 500 + B, pad), f"tiny_B{B}_T{Tin}_V{V}", parity_log)
 
 
 @pytest.mark.parametrize("B,seed,pad,pretraining", [(1, 1235, 0, False), (2, 1236, 0, False), (3, 99, 4, False), (4, 314, 0, True)])
@@ -149,28 +130,12 @@ def test_full_model_without_attention_output(full64, full_x, parity_log):
 
 
 # ------------------------------------------------------------------ detector output in (forward_regions)
-def _detector_output(n_img, n, F, seed, wh=((640, 480), (500, 375), (320, 240))):
-    import numpy as np
-    g = torch.Generator().manual_seed(seed)
-    feats = [torch.relu(torch.randn(n, F, generator=g)) * 1.5 for _ in range(n_img)]
-    infos = []
-    for i in range(n_img):
-        w, h = wh[i % len(wh)]
-        x1 = torch.rand(n, generator=g) * 0.7 * w
-        y1 = torch.rand(n, generator=g) * 0.7 * h
-        bw = (0.05 + 0.25 * torch.rand(n, generator=g)) * w
-        bh = (0.05 + 0.25 * torch.rand(n, generator=g)) * h
-        bbox = torch.stack([x1, y1, torch.minimum(x1 + bw, torch.tensor(float(w))), torch.minimum(y1 + bh, torch.tensor(float(h)))], 1)
-        infos.append({"image_width": w, "image_height": h, "bbox": bbox.numpy().astype(np.float32)})
-    return feats, infos
-
-
 def test_forward_regions(tiny_oracle, tiny64, tiny_x, parity_log):
     """vb200_forward_regions against the fp64 oracle on the host construction of the same detector output (build_inputs), with all
     boxes valid and with image 1 holding 13 valid boxes of 20 (padded boxes zero, masked, left out of the mean row)."""
     from vilbert_b200 import worker_api as W
     tok = W.WordpieceTokenizer(VOCAB)
-    feats, infos = _detector_output(3, 20, tiny_oracle.config.v_feature_size, seed=12)
+    feats, infos = support.detector_output_features_first(3, 20, tiny_oracle.config.v_feature_size, seed=12)
     text, f, s, seg, im, vm, _, task = W.build_inputs("what is the man holding?", [7], feats, infos, torch.device("cpu"), tok)
     rep = lambda t: t.repeat(3, 1)
     boxes = torch.stack([torch.from_numpy(i["bbox"]) for i in infos])
@@ -197,7 +162,7 @@ def test_forward_regions(tiny_oracle, tiny64, tiny_x, parity_log):
 def test_cached_states(tiny_oracle, tiny64, tiny_x, parity_log):
     """encode_text / encode_image once, forward_cached on nine pairs (repeats included) against the fp64 oracle on those pairs."""
     from vilbert_b200 import _lib as L
-    cap, img = _tiny_inputs(tiny_oracle, 5, 22, 14, 71), _tiny_inputs(tiny_oracle, 4, 22, 14, 72, pad=2)
+    cap, img = support.tiny_inputs(tiny_oracle, 5, 22, 14, 71), support.tiny_inputs(tiny_oracle, 4, 22, 14, 72, pad=2)
     q, seg, im = (cap[i] for i in (0, 3, 4))
     f, s, vm = (img[i] for i in (1, 2, 5))
     task = torch.full((5, 1), 7, dtype=torch.long)
@@ -218,10 +183,10 @@ def test_long_sequences(parity_log):
     from oracle import vilbert_ref as R
     oracle = R.build(R.tiny_config(max_position_embeddings=1024), seed=7, num_labels=200)
     o64 = X.fp64(oracle)
-    m = _engine(oracle, max_rows_per_sample=1024, return_attention=True)
+    m = support.engine(oracle, compute_dtype="fp32x", max_rows_per_sample=1024, return_attention=True)
     try:
         for Tin, V in [(300, 36), (511, 257), (30, 1000)]:
-            _forward(o64, m, _tiny_inputs(oracle, 1, Tin, V, Tin + V), f"long_T{Tin}_V{V}", parity_log)
+            _forward(o64, m, support.tiny_inputs(oracle, 1, Tin, V, Tin + V), f"long_T{Tin}_V{V}", parity_log)
     finally:
         m.close()
 
@@ -231,7 +196,7 @@ def test_pretraining_heads_at_rows(tiny64, tiny_x, parity_log):
     """pretraining_heads on an fp32x forward's taps, at listed rows (the 128-row bucket edges, the last row, duplicates), against the
     fp64 cls heads on the fp64 final states."""
     B, Tin, V = 3, 60, 50
-    inp = _tiny_inputs(tiny64, B, Tin, V, 103, pad=2)
+    inp = support.tiny_inputs(tiny64, B, Tin, V, 103, pad=2)
     _, taps = tiny_x(*[t.cuda() for t in inp], select=0, debug_taps=True)
     last_t, last_v = B * (Tin + 1) - 1, B * V - 1
     tr, vr, pr = [0, 127, 128, last_t, 5, 5, last_t], [0, 127, 128, last_v, 3, 3], [2, 0, 1, 1]
@@ -254,7 +219,7 @@ def pt():
     from oracle import pretraining_ref as P
     import vilbert_b200 as vb
     oracle = P.build(P.tiny_pretraining_config(), seed=7)
-    m = _engine(oracle, vb.BertForMultiModalPreTraining, return_attention=True)
+    m = support.engine(oracle, vb.BertForMultiModalPreTraining, return_attention=True, compute_dtype="fp32x")
     yield X.fp64(oracle), m
     m.close()
 

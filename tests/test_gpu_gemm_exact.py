@@ -11,12 +11,11 @@ must keep the NaN.
 The activation sweep feeds every finite fp16 and bf16 value through identity weights, so the accumulator holds the input exactly and
 the epilogue's bias add, activation and 16-bit conversion are compared, value by value, with their references: pre = fp32(x + b), the
 documented 4.3e-5 bound and saturation thresholds of gelu_erf, and its float32 restatement gelu_poly_f32."""
-import ctypes as C
-
 import pytest
 import torch
 
 from oracle import kernel_refs as R
+import support
 
 pytestmark = pytest.mark.gpu
 
@@ -25,29 +24,8 @@ DT_IDS = ["fp16", "bf16"]
 NAN = float("nan")
 
 
-def _lib():
-    from vilbert_b200 import _lib as L
-    return L, L.load()
-
-
-def _call(name, *args):
-    """Call a C-ABI hook on the current stream; tensors are passed as themselves so that they stay alive until the launch is
-    enqueued."""
-    L, lib = _lib()
-    ptrs = [a.data_ptr() if torch.is_tensor(a) else a for a in args]
-    L.check(getattr(lib, name)(*ptrs, C.c_void_p(torch.cuda.current_stream().cuda_stream)), None)
-
-
 def _f16(dt):
     return dt == torch.float16
-
-
-def _eq16(a, b):
-    return torch.equal(a.contiguous().view(torch.int16), b.contiguous().view(torch.int16))
-
-
-def _eq32(a, b):
-    return torch.equal(a.contiguous().view(torch.int32), b.contiguous().view(torch.int32))
 
 
 def _all_nan(t):
@@ -72,8 +50,8 @@ def _linear(x, w, b, M, N, K, dt, act=0, outs="16+32", variant=0, bn=0, pdl=0, s
         y16, ld16, y32, ld32 = _buffers(M, N, dt, outs)
     else:
         y32, ld32 = None, 0
-    _call("vb200_linear", x, x.stride(0), w, w.stride(0), b, None, 0, None, None, 1e-12, act, y16, ld16 if y16 is not None else 0,
-          y32, ld32 if y32 is not None else 0, M, N, K, bn, pdl, int(_f16(dt)), variant, None)
+    support.call("vb200_linear", x, x.stride(0), w, w.stride(0), b, None, 0, None, None, 1e-12, act, y16, ld16 if y16 is not None else 0,
+                 y32, ld32 if y32 is not None else 0, M, N, K, bn, pdl, int(_f16(dt)), variant, None)
     if sync:
         torch.cuda.synchronize()
     return y16, y32
@@ -83,11 +61,11 @@ def _check(y16, y32, ref, N, dt, rows=None, what=""):
     """y32 == ref and y16 == sat_rn(ref) bit for bit on rows [0, rows); padding columns past N keep their NaN."""
     m = ref.shape[0] if rows is None else rows
     if y32 is not None:
-        assert _eq32(y32[:m, :N], ref[:m]), f"{what}: fp32 output differs from the exact result " \
+        assert support.eq32(y32[:m, :N], ref[:m]), f"{what}: fp32 output differs from the exact result " \
             f"({int((y32[:m, :N] != ref[:m]).sum())} elements)"
         assert _all_nan(y32[:, N:]), f"{what}: fp32 padding columns written"
     if y16 is not None:
-        assert _eq16(y16[:m, :N], R.sat_rn(ref[:m], _f16(dt))), f"{what}: 16-bit output is not sat_rn(exact)"
+        assert support.eq16(y16[:m, :N], R.sat_rn(ref[:m], _f16(dt))), f"{what}: 16-bit output is not sat_rn(exact)"
         assert _all_nan(y16[:, N:]), f"{what}: 16-bit padding columns written"
 
 
@@ -147,8 +125,8 @@ def test_linear_rows_exact(N, K, m, dt):
     x, w, b = _operands(M, N, K, dt, seed=N + m)
     ref = R.exact_linear(x, w, b, 0)
     y16, ld16, y32, ld32 = _buffers(M, N, dt, "16+32")
-    _call("vb200_linear_rows", x, K, w, K, b, 0, y16, ld16, y32, ld32, M, N, K, 0, int(_f16(dt)),
-          torch.tensor([m], dtype=torch.int32, device="cuda"))
+    support.call("vb200_linear_rows", x, K, w, K, b, 0, y16, ld16, y32, ld32, M, N, K, 0, int(_f16(dt)),
+                 torch.tensor([m], dtype=torch.int32, device="cuda"))
     torch.cuda.synchronize()
     _check(y16, y32, ref, N, dt, rows=m, what=f"m_rows {m}")
     boundary = (m + 127) // 128 * 128
@@ -176,8 +154,8 @@ def test_linear_product_exact(case, dt):
         ref = R.exact_linear(x, w, b, act, mul[:, :N])
         for outs in ("16+32", "16"):
             y16, ld16, y32, ld32 = _buffers(M, N, dt, outs)
-            _call("vb200_linear_product", x, ld_x, w, K, b, act, mul, ld_mul, y16, ld16, y32, ld32 if y32 is not None else 0, M, N, K,
-                  0, int(_f16(dt)))
+            support.call("vb200_linear_product", x, ld_x, w, K, b, act, mul, ld_mul, y16, ld16, y32, ld32 if y32 is not None else 0, M, N, K,
+                         0, int(_f16(dt)))
             torch.cuda.synchronize()
             _check(y16, y32, ref, N, dt, what=f"act {act} outputs {outs}")
 
@@ -226,11 +204,11 @@ def test_linear_split_exact(M, N, K, act):
     x3, w3, b = R.split16(x).cuda(), R.split16_w(w).cuda(), b.cuda()
     y3 = torch.full((M, 3 * N + 64), NAN, dtype=torch.float16, device="cuda")
     y32 = torch.full((M, N + 4), NAN, device="cuda")
-    _call("vb200_linear_split", x3, 3 * K, w3, 3 * K, b, act, y3, 3 * N + 64, y32, N + 4, M, N, 3 * K)
+    support.call("vb200_linear_split", x3, 3 * K, w3, 3 * K, b, act, y3, 3 * N + 64, y32, N + 4, M, N, 3 * K)
     torch.cuda.synchronize()
     ref = ref.cuda()
-    assert _eq32(y32[:, :N], ref), int((y32[:, :N] != ref).sum())
-    assert _eq16(y3[:, :3 * N], R.split16(ref))
+    assert support.eq32(y32[:, :N], ref), int((y32[:, :N] != ref).sum())
+    assert support.eq16(y3[:, :3 * N], R.split16(ref))
     assert _all_nan(y32[:, N:]) and _all_nan(y3[:, 3 * N:])
 
 
@@ -307,9 +285,9 @@ def test_unaligned_fp32_output_exact(dt):
     x, w, b = _operands(M, N, K, dt, seed=3)
     ref = R.exact_linear(x, w, b, 0)
     y32 = torch.full((M + 1, N), NAN, device="cuda")
-    _call("vb200_linear", x, K, w, K, b, None, 0, None, None, 1e-12, 0, None, 0, y32, N, M, N, K, 0, 0, int(_f16(dt)), 0, None)
+    support.call("vb200_linear", x, K, w, K, b, None, 0, None, None, 1e-12, 0, None, 0, y32, N, M, N, K, 0, 0, int(_f16(dt)), 0, None)
     torch.cuda.synchronize()
-    assert _eq32(y32[:M], ref) and _all_nan(y32[M:])
+    assert support.eq32(y32[:M], ref) and _all_nan(y32[M:])
 
 
 # M = 128 x (tiles - 1) + 1 .. 128 x tiles, one column tile: 131 / 132 / 133 and 263 / 264 / 265 tiles against 132 SMs
@@ -397,7 +375,7 @@ def test_pingpong_pdl_chain_exact(dt):
             _linear(cur, w, b, M, 768, K, dt, act=act, variant=5, bn=64, pdl=pdl, sync=False, y16=y, ld16=768)
             cur = y
         torch.cuda.synchronize()
-        assert _eq16(cur, R.sat_rn(ref, _f16(dt))), f"pdl {pdl}"
+        assert support.eq16(cur, R.sat_rn(ref, _f16(dt))), f"pdl {pdl}"
 
 
 # ================================================================================================================ activation sweep
@@ -452,7 +430,7 @@ def test_activation_epilogue_every_16bit_input(variant, bn, dt, parity_log):
         for act in (0, 2, 1):
             y16, y32 = _linear(x, w, b, 256, 256, 256, dt, act=act, variant=variant, bn=bn)
             y16, y32 = y16[:, :256], y32[:, :256]
-            assert _eq16(y16, R.sat_rn(y32, f16)), act
+            assert support.eq16(y16, R.sat_rn(y32, f16)), act
             assert bool(torch.isfinite(y32).all()), act
             if act == 0:
                 sub = (x.float().abs() < (2.0 ** -14 if f16 else 2.0 ** -126)) & (x.float() != 0)
@@ -465,7 +443,7 @@ def test_activation_epilogue_every_16bit_input(variant, bn, dt, parity_log):
                 worst = max(worst, err.max().item())
                 assert err.max().item() <= R.GELU_BOUND, err.max().item()
                 lo, hi = pre < R.GELU_ZERO_BELOW, pre > R.GELU_IDENTITY_ABOVE
-                assert bool((y32[lo] == 0).all()) and _eq32(y32[hi], pre[hi])
+                assert bool((y32[lo] == 0).all()) and support.eq32(y32[hi], pre[hi])
                 emu = torch.from_numpy(R.gelu_poly_f32(pre.cpu().numpy())).cuda()
                 assert _ulp_distance(y32, emu).max().item() <= 1
     parity_log(test="gemm_exact_gelu_sweep", dtype=str(dt), variant=variant, block_n=bn, values=n, max_abs_err=worst, bound=R.GELU_BOUND)
@@ -496,10 +474,10 @@ def test_act3_gelu_every_fp16_input(parity_log):
         pre = a.float().cuda() + b
         y3 = torch.full((256, 768), NAN, dtype=torch.float16, device="cuda")
         y32 = torch.full((256, 256), NAN, device="cuda")
-        _call("vb200_linear_split", x3, 768, w3, 768, b, 3, y3, 768, y32, 256, 256, 256, 768)
+        support.call("vb200_linear_split", x3, 768, w3, 768, b, 3, y3, 768, y32, 256, 256, 256, 768)
         torch.cuda.synchronize()
         assert bool(torch.isfinite(y32).all())
-        assert _eq16(y3, R.split16(y32))
+        assert support.eq16(y3, R.split16(y32))
         err = (y32.double() - R.gelu_fp64(pre.double())).abs()
         worst = max(worst, err.max().item())
         near = pre.abs() <= 2.0
@@ -538,8 +516,8 @@ def test_rowdot_exact(n_out, K, add, bias):
         ref, scale = ref + a.double()[:, None], scale + a.double().abs()[:, None]
     assert scale.max().item() < 2.0 ** R.EXACT_BUDGET_LOG2 and scale.max().item() > 2.0 ** 20
     out = torch.full((M, ld_out), NAN, device="cuda")
-    _call("vb200_rowdot", x.cuda(), ld_x, w.cuda(), b.cuda() if b is not None else None, a.cuda() if a is not None else None, out, ld_out,
-          M, K, n_out, None)
+    support.call("vb200_rowdot", x.cuda(), ld_x, w.cuda(), b.cuda() if b is not None else None, a.cuda() if a is not None else None, out,
+                 ld_out, M, K, n_out, None)
     torch.cuda.synchronize()
-    assert _eq32(out[:, :n_out], ref.float().cuda())
+    assert support.eq32(out[:, :n_out], ref.float().cuda())
     assert _all_nan(out[:, n_out:])

@@ -8,12 +8,9 @@ import ctypes as C
 import pytest
 import torch
 
+import support
+
 pytestmark = pytest.mark.gpu
-
-
-def _lib():
-    from vilbert_b200 import _lib as L
-    return L, L.load()
 
 
 def _stream():
@@ -30,7 +27,8 @@ def _operands(M, N, K, f16, seed):
 
 
 def _linear(x, w, b, act, yb, yf, bn, variant, f16, pdl=0, m=None):
-    L, lib = _lib()
+    L = support.lib()
+    lib = L.load()
     M, K = x.shape
     N = w.shape[0]
     L.check(lib.vb200_linear(x.data_ptr(), K, w.data_ptr(), K, b.data_ptr() if b is not None else None, None, 0, None, None, 1e-12,
@@ -99,7 +97,8 @@ def test_pingpong_without_bias(f16):
 def test_pingpong_device_row_count(bn, m):
     """vb200_linear_rows (the ping-pong kernel by default) with m_rows = m at M = 1000: rows < m equal variant 0; every tile that starts
     at or past m is skipped, so rows from the next 128-row boundary on keep the sentinel."""
-    L, lib = _lib()
+    L = support.lib()
+    lib = L.load()
     M, N, K = 1000, 256, 192
     x, w, b = _operands(M, N, K, True, 5)
     rows = torch.tensor([m], dtype=torch.int32, device="cuda")
@@ -136,13 +135,6 @@ def test_pingpong_pdl_chain(f16):
 
 
 # ---------------------------------------------------------------- the full model: gemm_kernel 0 (cooperative) against 1 (ping-pong)
-def _engine(oracle, dtype):
-    import vilbert_b200 as vb
-    cfg = vb.BertConfig.from_dict(oracle.config.to_dict())
-    return vb.VILBertForVLTasks.from_pretrained(oracle.state_dict(), config=cfg, num_labels=oracle.num_labels,
-                                                compute_dtype=dtype).eval().cuda(0)
-
-
 def _tensors(x):
     if torch.is_tensor(x):
         return [x.clone()]
@@ -172,7 +164,7 @@ def test_full_model_pingpong_bitwise(full_oracle, dtype):
     same bits with either GEMM kernel."""
     import vilbert_b200 as vb
     from oracle import vilbert_ref as R
-    model = _engine(full_oracle, dtype)
+    model = support.engine(full_oracle, compute_dtype=dtype)
     try:
         inp = [t.cuda() for t in R.make_inputs(64, 30, 36, seed=3)]
         _ab(model, lambda: model(*inp, select=vb.OUT_TASK_HEADS, debug_taps=True))

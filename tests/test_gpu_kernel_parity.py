@@ -6,7 +6,6 @@ programmatic dependent launch.  `-m gpu` only.
 Output buffers start out filled with a sentinel (NaN, or a marker value) so that a write outside a kernel's contract shows up.  Where
 a kernel writes an fp32 value and its 16-bit copy, the 16-bit bits must equal sat_rn(fp32): fp16 clamps to +-65504 and rounds to
 nearest even, bf16 rounds to nearest even."""
-import ctypes as C
 import math
 
 import numpy as np
@@ -14,33 +13,13 @@ import pytest
 import torch
 
 from oracle import kernel_refs as R
+import support
 
 pytestmark = pytest.mark.gpu
 
 DTS = [torch.float16, torch.bfloat16]
 DT_IDS = ["fp16", "bf16"]
 NAN = float("nan")
-
-
-def _lib():
-    from vilbert_b200 import _lib as L
-    return L, L.load()
-
-
-def _call(name, *args):
-    """Call a C-ABI hook on the current stream.  Tensors are passed as themselves and turned into pointers here, so that every
-    temporary stays alive until its launch is enqueued (later allocations are then ordered after the kernel on the stream)."""
-    L, lib = _lib()
-    ptrs = [a.data_ptr() if torch.is_tensor(a) else a for a in args]
-    L.check(getattr(lib, name)(*ptrs, C.c_void_p(torch.cuda.current_stream().cuda_stream)), None)
-
-
-def _eq16(a, b):
-    return torch.equal(a.contiguous().view(torch.int16), b.contiguous().view(torch.int16))
-
-
-def _eq32(a, b):
-    return torch.equal(a.contiguous().view(torch.int32), b.contiguous().view(torch.int32))
 
 
 def _is_nan(t):
@@ -81,9 +60,9 @@ class _Tables:
         o16 = torch.full((n + extra, 3 * self.H if split16 else self.H), NAN, device="cuda",
                          dtype=torch.float16 if f16 else torch.bfloat16)
         mask = torch.full((n + extra,), NAN, device="cuda")
-        _call("vb200_text_embed", ids, seg, imask, task, self.word, self.pos, self.type, self.task,
-              self.gamma, self.beta, 1e-12, out, o16, mask, B, Tin, self.H, self.vocab, self.max_pos, self.n_type,
-              self.n_task, tt, f16, split16, offs, rows)
+        support.call("vb200_text_embed", ids, seg, imask, task, self.word, self.pos, self.type, self.task,
+                     self.gamma, self.beta, 1e-12, out, o16, mask, B, Tin, self.H, self.vocab, self.max_pos, self.n_type,
+                     self.n_task, tt, f16, split16, offs, rows)
         torch.cuda.synchronize()
         return out, o16, mask, n
 
@@ -143,7 +122,7 @@ def test_text_embed_dense(H, Tin, B, tt, dt, parity_log):
     err = (out[:n].double() - ref).abs().max().item()
     parity_log(test="kp_text_embed", H=H, Tin=Tin, B=B, tt=tt, dtype=str(dt), max_abs_err=err, bound=1e-5)
     assert err < 1e-5, err
-    assert _eq16(o16[:n], R.sat_rn(out[:n], dt == torch.float16))
+    assert support.eq16(o16[:n], R.sat_rn(out[:n], dt == torch.float16))
     assert torch.equal(mask[:n].cpu(), _mask_ref(imask, tt))
     assert _is_nan(out[n:]) and _is_nan(o16[n:]) and _is_nan(mask[n:])
 
@@ -162,7 +141,7 @@ def test_text_embed_clamping(Tin, dt, parity_log):
         err = (out[:n].double() - ref).abs().max().item()
         parity_log(test="kp_text_embed_clamp", Tin=Tin, tt=tt, dtype=str(dt), max_abs_err=err, bound=1e-5)
         assert err < 1e-5, err
-        assert _eq16(o16[:n], R.sat_rn(out[:n], dt == torch.float16))
+        assert support.eq16(o16[:n], R.sat_rn(out[:n], dt == torch.float16))
         assert torch.equal(mask[:n].cpu(), _mask_ref(imask, tt))
 
 
@@ -191,7 +170,7 @@ def test_text_embed_packed(H, tt, dt, parity_log):
         d_out, d16, d_mask, dn = tb.run(ids_l[b].view(1, -1).cuda(), seg_l[b].view(1, -1).cuda(),
                                         torch.ones(1, Tin, dtype=torch.long, device="cuda"), task[b:b + 1].cuda(), 1, Tin, tt, _f16(dt))
         sl = slice(offs[b], offs[b + 1])
-        assert _eq32(out[sl], d_out[:dn]) and _eq16(o16[sl], d16[:dn]) and torch.equal(mask[sl], d_mask[:dn]), b
+        assert support.eq32(out[sl], d_out[:dn]) and support.eq16(o16[sl], d16[:dn]) and torch.equal(mask[sl], d_mask[:dn]), b
 
 
 @pytest.mark.parametrize("packed", [False, True], ids=["dense", "packed"])
@@ -206,7 +185,7 @@ def test_text_embed_split16(packed):
                                 offs=_dev_i32(offs), rows=60)
     else:
         out, o16, _, n = tb.run(ids.cuda(), seg.cuda(), imask.cuda(), task.cuda(), B, Tin, 1, 1, split16=1)
-    assert _eq16(o16[:n], R.split16(out[:n]))
+    assert support.eq16(o16[:n], R.split16(out[:n]))
     assert _is_nan(o16[n:])
 
 
@@ -231,10 +210,10 @@ def test_image_pack(F, Kp, with_mask, dt):
     im = (torch.arange(rows, device="cuda") % 4 != 3).to(torch.uint8) if with_mask else None
     a = torch.full((rows + 2, Kp), NAN, dtype=dt, device="cuda")
     mask = torch.full((rows + 2,), NAN, device="cuda")
-    _call("vb200_image_pack", feats, loc, im, a, mask, rows, F, Kp, _f16(dt), 0)
+    support.call("vb200_image_pack", feats, loc, im, a, mask, rows, F, Kp, _f16(dt), 0)
     torch.cuda.synchronize()
     ref = torch.from_numpy(R.operand_rows(feats.cpu().numpy(), loc.cpu().numpy(), Kp)).cuda()
-    assert _eq16(a[:rows], R.sat_rn(ref, dt == torch.float16))
+    assert support.eq16(a[:rows], R.sat_rn(ref, dt == torch.float16))
     want = (1.0 - im.float()) * -10000.0 if with_mask else torch.zeros(rows, device="cuda")
     assert torch.equal(mask[:rows], want)
     assert _is_nan(a[rows:]) and _is_nan(mask[rows:])
@@ -247,10 +226,10 @@ def test_image_pack_split16(F, Kp):
     loc = torch.rand(rows, 5, generator=_gen(2), device="cuda")
     a = torch.full((rows + 1, 3 * Kp), NAN, dtype=torch.float16, device="cuda")
     mask = torch.full((rows + 1,), NAN, device="cuda")
-    _call("vb200_image_pack", feats, loc, None, a, mask, rows, F, Kp, 1, 1)
+    support.call("vb200_image_pack", feats, loc, None, a, mask, rows, F, Kp, 1, 1)
     torch.cuda.synchronize()
     ref = torch.from_numpy(R.operand_rows(feats.cpu().numpy(), loc.cpu().numpy(), Kp)).cuda()
-    assert _eq16(a[:rows], R.split16(ref)) and _is_nan(a[rows:])
+    assert support.eq16(a[:rows], R.split16(ref)) and _is_nan(a[rows:])
 
 
 # ================================================================================================================ region pack
@@ -292,8 +271,8 @@ def test_region_pack_dense(F, Kp, num_boxes, dt):
     mask = torch.full((R_ + 2,), NAN, device="cuda")
     sp = torch.full((R_ + 2, 5), NAN, device="cuda")
     nb_t = _dev_i32(nbs) if num_boxes else None
-    _call("vb200_region_pack", torch.from_numpy(feats).cuda(), torch.from_numpy(boxes).cuda(), torch.from_numpy(wh).cuda(),
-          nb_t, a, mask, sp, B, n, F, Kp, _f16(dt), 0, None)
+    support.call("vb200_region_pack", torch.from_numpy(feats).cuda(), torch.from_numpy(boxes).cuda(), torch.from_numpy(wh).cuda(),
+                 nb_t, a, mask, sp, B, n, F, Kp, _f16(dt), 0, None)
     torch.cuda.synchronize()
     f16 = dt == torch.float16
     assert _is_nan(a[R_:]) and _is_nan(mask[R_:]) and _is_nan(sp[R_:])
@@ -301,15 +280,15 @@ def test_region_pack_dense(F, Kp, num_boxes, dt):
         rows, loc, real = R.region_rows(feats[b], boxes[b], wh[b, 0], wh[b, 1], nbs[b])
         sl = slice(b * (n + 1), (b + 1) * (n + 1))
         ref = torch.from_numpy(R.operand_rows(rows, loc, Kp)).cuda()
-        assert _eq16(a[sl], R.sat_rn(ref, f16)), b
-        assert _eq32(sp[sl], torch.from_numpy(loc).cuda()), b
+        assert support.eq16(a[sl], R.sat_rn(ref, f16)), b
+        assert support.eq32(sp[sl], torch.from_numpy(loc).cuda()), b
         assert torch.equal(mask[sl].cpu(), torch.from_numpy(np.where(real, 0.0, -10000.0).astype(np.float32))), b
         if nbs[b] == n:
             info = {"image_width": float(wh[b, 0]), "image_height": float(wh[b, 1]), "bbox": boxes[b]}
             _, f_bi, s_bi, *_ = W.build_inputs("q", [1], [torch.from_numpy(feats[b])], [info], torch.device("cpu"), _Tok())
             got = a[sl][:, :F]
-            assert _eq16(got[1:], R.sat_rn(f_bi[0, 1:].cuda(), f16))
-            assert _eq32(sp[sl], s_bi[0].cuda())
+            assert support.eq16(got[1:], R.sat_rn(f_bi[0, 1:].cuda(), f16))
+            assert support.eq32(sp[sl], s_bi[0].cuda())
             d = (got[0].view(torch.int16).int() - R.sat_rn(f_bi[0, 0].cuda(), f16).view(torch.int16).int()).abs()
             assert int(d.max()) <= 1
 
@@ -320,13 +299,13 @@ def test_region_pack_split16():
     R_ = B * (n + 1)
     a = torch.full((R_, 3 * Kp), NAN, dtype=torch.float16, device="cuda")
     mask = torch.full((R_,), NAN, device="cuda")
-    _call("vb200_region_pack", torch.from_numpy(feats).cuda(), torch.from_numpy(boxes).cuda(), torch.from_numpy(wh).cuda(),
-          _dev_i32([n, 4]), a, mask, None, B, n, F, Kp, 1, 1, None)
+    support.call("vb200_region_pack", torch.from_numpy(feats).cuda(), torch.from_numpy(boxes).cuda(), torch.from_numpy(wh).cuda(),
+                 _dev_i32([n, 4]), a, mask, None, B, n, F, Kp, 1, 1, None)
     torch.cuda.synchronize()
     for b, nb in enumerate([n, 4]):
         rows, loc, _ = R.region_rows(feats[b], boxes[b], wh[b, 0], wh[b, 1], nb)
         ref = torch.from_numpy(R.operand_rows(rows, loc, Kp)).cuda()
-        assert _eq16(a[b * (n + 1):(b + 1) * (n + 1)], R.split16(ref)), b
+        assert support.eq16(a[b * (n + 1):(b + 1) * (n + 1)], R.split16(ref)), b
 
 
 @pytest.mark.parametrize("dt", DTS, ids=DT_IDS)
@@ -346,16 +325,16 @@ def test_region_pack_packed(F, Kp, dt):
     a = torch.full((R_ + 3, Kp), NAN, dtype=dt, device="cuda")
     mask = torch.full((R_ + 3,), NAN, device="cuda")
     sp = torch.full((R_ + 3, 5), NAN, device="cuda")
-    _call("vb200_region_pack", torch.from_numpy(feats).cuda(), torch.from_numpy(boxes).cuda(), torch.from_numpy(wh).cuda(),
-          None, a, mask, sp, B, 0, F, Kp, _f16(dt), 0, _dev_i32(offs))
+    support.call("vb200_region_pack", torch.from_numpy(feats).cuda(), torch.from_numpy(boxes).cuda(), torch.from_numpy(wh).cuda(),
+                 None, a, mask, sp, B, 0, F, Kp, _f16(dt), 0, _dev_i32(offs))
     torch.cuda.synchronize()
     assert _is_nan(a[R_:]) and _is_nan(mask[R_:]) and _is_nan(sp[R_:])
     assert bool((mask[:R_] == 0).all())
     for b, c in enumerate(counts):
         rows, loc, _ = R.region_rows(per[b][0][0], per[b][1][0], wh[b, 0], wh[b, 1], c)
         sl = slice(offs[b], offs[b + 1])
-        assert _eq16(a[sl], R.sat_rn(torch.from_numpy(R.operand_rows(rows, loc, Kp)).cuda(), dt == torch.float16)), b
-        assert _eq32(sp[sl], torch.from_numpy(loc).cuda()), b
+        assert support.eq16(a[sl], R.sat_rn(torch.from_numpy(R.operand_rows(rows, loc, Kp)).cuda(), dt == torch.float16)), b
+        assert support.eq32(sp[sl], torch.from_numpy(loc).cuda()), b
 
 
 # ================================================================================================================ narrow heads
@@ -377,7 +356,7 @@ def test_rowdot(n_out, K, add, bias, cut, parity_log):
         a[::3] = -10000.0
     out = torch.full((M, ld_out), NAN, device="cuda")
     rows = _dev_i32([cut]) if cut is not None else None
-    _call("vb200_rowdot", x, ld_x, w, b, a, out, ld_out, M, K, n_out, rows)
+    support.call("vb200_rowdot", x, ld_x, w, b, a, out, ld_out, M, K, n_out, rows)
     torch.cuda.synchronize()
     m = cut if cut is not None else M
     terms = x[:, :K].double()[:, None, :] * w.double()[None]
@@ -406,10 +385,10 @@ def test_gather_state():
     d32 = torch.full((B + 1, L, H), NAN, device="cuda")
     d16 = torch.full((B + 1, L, H16), 0x7E01, dtype=torch.int16, device="cuda")
     dmask = torch.full((B + 1, L), NAN, device="cuda")
-    _call("vb200_gather_state", _dev_i32(idx), n_src, s32, s16, smask, d32, d16, dmask, B, L, H, H16)
+    support.call("vb200_gather_state", _dev_i32(idx), n_src, s32, s16, smask, d32, d16, dmask, B, L, H, H16)
     torch.cuda.synchronize()
     src = torch.tensor([min(max(i, 0), n_src - 1) for i in idx], device="cuda")
-    assert _eq32(d32[:B], s32[src]) and torch.equal(d16[:B], s16[src]) and _eq32(dmask[:B], smask[src])
+    assert support.eq32(d32[:B], s32[src]) and torch.equal(d16[:B], s16[src]) and support.eq32(dmask[:B], smask[src])
     assert _is_nan(d32[B:]) and bool((d16[B:] == 0x7E01).all()) and _is_nan(dmask[B:])
 
 
@@ -422,7 +401,7 @@ def test_gather_state_packed_pooler_form():
     M = offs[-1]
     s16 = torch.randint(-32768, 32767, (M, ld), generator=_gen(12), device="cuda", dtype=torch.int32).to(torch.int16)
     d16 = torch.full((len(lens) + 1, ld), 0x7E01, dtype=torch.int16, device="cuda")
-    _call("vb200_gather_state", _dev_i32(offs), M, None, s16, None, None, d16, None, len(lens), 1, ld, ld)
+    support.call("vb200_gather_state", _dev_i32(offs), M, None, s16, None, None, d16, None, len(lens), 1, ld, ld)
     torch.cuda.synchronize()
     assert torch.equal(d16[:len(lens)], s16[torch.tensor(offs[:-1], device="cuda")])
     assert bool((d16[len(lens):] == 0x7E01).all())
@@ -444,13 +423,13 @@ def test_gather_packed_state():
     td16 = torch.full((to[-1] + 2, Ht), NAN, dtype=torch.float16, device="cuda")
     vd32 = torch.full((vo[-1] + 2, Hv), NAN, device="cuda")
     vd16 = torch.full((vo[-1] + 2, Hv), NAN, dtype=torch.float16, device="cuda")
-    _call("vb200_gather_packed_state", len(t_lens), _dev_i32(to), _dev_i32(t_src_start), ts32, ts16, td32, td16,
-          Ht // 4, Ht // 8, _dev_i32(vo), _dev_i32(v_src_start), vs32, vs16, vd32, vd16, Hv // 4, Hv // 8)
+    support.call("vb200_gather_packed_state", len(t_lens), _dev_i32(to), _dev_i32(t_src_start), ts32, ts16, td32, td16,
+                 Ht // 4, Ht // 8, _dev_i32(vo), _dev_i32(v_src_start), vs32, vs16, vd32, vd16, Hv // 4, Hv // 8)
     torch.cuda.synchronize()
     for b in range(len(t_lens)):
         st, sv = t_src_start[b], v_src_start[b]
-        assert _eq32(td32[to[b]:to[b + 1]], ts32[st:st + t_lens[b]]) and _eq16(td16[to[b]:to[b + 1]], ts16[st:st + t_lens[b]]), b
-        assert _eq32(vd32[vo[b]:vo[b + 1]], vs32[sv:sv + v_lens[b]]) and _eq16(vd16[vo[b]:vo[b + 1]], vs16[sv:sv + v_lens[b]]), b
+        assert support.eq32(td32[to[b]:to[b + 1]], ts32[st:st + t_lens[b]]) and support.eq16(td16[to[b]:to[b + 1]], ts16[st:st + t_lens[b]]), b
+        assert support.eq32(vd32[vo[b]:vo[b + 1]], vs32[sv:sv + v_lens[b]]) and support.eq16(vd16[vo[b]:vo[b + 1]], vs16[sv:sv + v_lens[b]]), b
     assert _is_nan(td32[to[-1]:]) and _is_nan(td16[to[-1]:]) and _is_nan(vd32[vo[-1]:]) and _is_nan(vd16[vo[-1]:])
 
 
@@ -480,14 +459,14 @@ def _attn_err(ctx, ref):
 
 def _self_dense(qkv, ld_qkv, H, mask, B, L, heads, d, dt, ld_ctx):
     ctx = torch.full((B * L, ld_ctx), NAN, dtype=dt, device="cuda")
-    _call("vb200_self_attention", qkv, ld_qkv, H, mask, ctx, ld_ctx, B, L, heads, d, _f16(dt))
+    support.call("vb200_self_attention", qkv, ld_qkv, H, mask, ctx, ld_ctx, B, L, heads, d, _f16(dt))
     return ctx
 
 
 def _co_dense(qi, ld_i, qt, ld_t, H, mi, mt, B, T, V, heads, d, dt, ld_ct, ld_ci):
     ct = torch.full((B * T, ld_ct), NAN, dtype=dt, device="cuda")
     ci = torch.full((B * V, ld_ci), NAN, dtype=dt, device="cuda")
-    _call("vb200_co_attention", qi, ld_i, qt, ld_t, H, mi, mt, ct, ld_ct, ci, ld_ci, B, T, V, heads, d, _f16(dt))
+    support.call("vb200_co_attention", qi, ld_i, qt, ld_t, H, mi, mt, ct, ld_ct, ci, ld_ci, B, T, V, heads, d, _f16(dt))
     return ct, ci
 
 
@@ -546,14 +525,14 @@ def test_self_attention_packed(d, dt, parity_log):
     qkv = torch.randn(M, ld_qkv, generator=_gen(d), device="cuda").to(dt)
     mask = torch.cat([_key_mask(L, b) for b, L in enumerate(LENGTHS)]).cuda()
     ctx = torch.full((M + 16, ld_ctx), NAN, dtype=dt, device="cuda")
-    _call("vb200_self_attention_packed", qkv, ld_qkv, H, mask, ctx, ld_ctx, len(LENGTHS), max(LENGTHS), heads, d, _f16(dt),
-          _dev_i32(offs))
+    support.call("vb200_self_attention_packed", qkv, ld_qkv, H, mask, ctx, ld_ctx, len(LENGTHS), max(LENGTHS), heads, d, _f16(dt),
+                 _dev_i32(offs))
     worst = 0.0
     for b, L in enumerate(LENGTHS):
         sl = slice(offs[b], offs[b + 1])
         dense = _self_dense(qkv[sl], ld_qkv, H, mask[sl].contiguous(), 1, L, heads, d, dt, ld_ctx)
         torch.cuda.synchronize()
-        assert _eq16(ctx[sl, :H], dense[:, :H]), f"sample {b} (L = {L})"
+        assert support.eq16(ctx[sl, :H], dense[:, :H]), f"sample {b} (L = {L})"
         x = qkv[sl, :3 * H].view(1, L, 3 * H)
         ref = R.attention_fp64(x[..., :H], x[..., H:2 * H], x[..., 2 * H:], mask[sl].view(1, L), heads)
         worst = max(worst, _attn_err(ctx[sl, :H].view(1, L, H), ref))
@@ -580,15 +559,15 @@ def test_co_attention_packed(d, dt, parity_log):
     mt = torch.cat([_key_mask(T, b + 1) for b, T in enumerate(T_l)]).cuda()
     ct = torch.full((ot[-1] + 16, ld_ct), NAN, dtype=dt, device="cuda")
     ci = torch.full((ov[-1] + 16, ld_ci), NAN, dtype=dt, device="cuda")
-    _call("vb200_co_attention_packed", qi, ld_i, qt, ld_t, H, mi, mt, ct, ld_ct, ci, ld_ci, B, max(T_l), max(V_l),
-          heads, d, _f16(dt), _dev_i32(ot), _dev_i32(ov))
+    support.call("vb200_co_attention_packed", qi, ld_i, qt, ld_t, H, mi, mt, ct, ld_ct, ci, ld_ci, B, max(T_l), max(V_l),
+                 heads, d, _f16(dt), _dev_i32(ot), _dev_i32(ov))
     worst = 0.0
     for b in range(B):
         T, V = T_l[b], V_l[b]
         st, sv = slice(ot[b], ot[b + 1]), slice(ov[b], ov[b + 1])
         dt_, di_ = _co_dense(qi[sv], ld_i, qt[st], ld_t, H, mi[sv].contiguous(), mt[st].contiguous(), 1, T, V, heads, d, dt, ld_ct, ld_ci)
         torch.cuda.synchronize()
-        assert _eq16(ct[st, :H], dt_[:, :H]) and _eq16(ci[sv, :H], di_[:, :H]), f"sample {b} (T = {T}, V = {V})"
+        assert support.eq16(ct[st, :H], dt_[:, :H]) and support.eq16(ci[sv, :H], di_[:, :H]), f"sample {b} (T = {T}, V = {V})"
         xi, xt = qi[sv, :3 * H].view(1, V, 3 * H), qt[st, :3 * H].view(1, T, 3 * H)
         ref_t = R.attention_fp64(xt[..., :H], xi[..., H:2 * H], xi[..., 2 * H:], mi[sv].view(1, V), heads)
         ref_i = R.attention_fp64(xi[..., :H], xt[..., H:2 * H], xt[..., 2 * H:], mt[st].view(1, T), heads)
@@ -637,16 +616,16 @@ def test_attention_structured(d, dt):
     expect = torch.cat([p[1] for p in parts]).cuda()
     mask = torch.zeros(offs[-1], device="cuda")
     ctx = torch.full((offs[-1], H), NAN, dtype=dt, device="cuda")
-    _call("vb200_self_attention_packed", qkv, 3 * H, H, mask, ctx, H, len(STRUCT_LENGTHS), max(STRUCT_LENGTHS), heads, d,
-          _f16(dt), _dev_i32(offs))
+    support.call("vb200_self_attention_packed", qkv, 3 * H, H, mask, ctx, H, len(STRUCT_LENGTHS), max(STRUCT_LENGTHS), heads, d,
+                 _f16(dt), _dev_i32(offs))
     torch.cuda.synchronize()
     assert (ctx.float() - expect).abs().max().item() < 0.5, "packed self"
     # co-attention: text queries over image keys built for them (T = V per sample), and the image direction over the text keys
     ct = torch.full((offs[-1], H), NAN, dtype=dt, device="cuda")
     ci = torch.full((offs[-1], H), NAN, dtype=dt, device="cuda")
     o = _dev_i32(offs)
-    _call("vb200_co_attention_packed", qkv, 3 * H, qkv, 3 * H, H, mask, mask, ct, H, ci, H, len(STRUCT_LENGTHS),
-          max(STRUCT_LENGTHS), max(STRUCT_LENGTHS), heads, d, _f16(dt), o, o)
+    support.call("vb200_co_attention_packed", qkv, 3 * H, qkv, 3 * H, H, mask, mask, ct, H, ci, H, len(STRUCT_LENGTHS),
+                 max(STRUCT_LENGTHS), max(STRUCT_LENGTHS), heads, d, _f16(dt), o, o)
     torch.cuda.synchronize()
     assert (ct.float() - expect).abs().max().item() < 0.5 and (ci.float() - expect).abs().max().item() < 0.5, "packed co"
     for L in (17, 129):
@@ -673,8 +652,8 @@ def _linear(x, w, b, M, N, K, dt, outs="16+32", variant=0, bn=0, act=0, pdl=0, l
         y16 = torch.full((M, ld16), NAN, dtype=dt, device="cuda")
     if y32 is None and "32" in outs:
         y32 = torch.full((M, ld32), NAN, device="cuda")
-    _call("vb200_linear", x, x.stride(0), w, w.stride(0), b, None, 0, None, None, 1e-12, act, y16, ld16, y32, ld32, M, N, K, bn, pdl,
-          _f16(dt), variant, None)
+    support.call("vb200_linear", x, x.stride(0), w, w.stride(0), b, None, 0, None, None, 1e-12, act, y16, ld16, y32, ld32, M, N, K, bn, pdl,
+                 _f16(dt), variant, None)
     if sync:
         torch.cuda.synchronize()
     return (y16[:, :N] if y16 is not None else None), (y32[:, :N] if y32 is not None else None)
@@ -700,10 +679,10 @@ def test_linear_16bit_is_sat_rn(path, dt):
     x, w, b = _operands(M, N, K, dt, seed=M + N)
     for act in (0, 1):
         y16, y32 = _linear(x, w, b, M, N, K, dt, variant=variant, bn=bn, act=act)
-        assert _eq16(y16, R.sat_rn(y32, dt == torch.float16)), act
+        assert support.eq16(y16, R.sat_rn(y32, dt == torch.float16)), act
         if N % 8 == 0:
             y16b, _ = _linear(x, w, b, M, N, K, dt, outs="16", variant=variant, bn=bn, act=act)
-            assert _eq16(y16b, y16), act
+            assert support.eq16(y16b, y16), act
 
 
 @pytest.mark.parametrize("path", STORE_PATHS, ids=[p[0] for p in STORE_PATHS])
@@ -715,11 +694,11 @@ def test_linear_fp16_saturates(path):
     b[1::3] = -1e5
     y16, y32 = _linear(x, w, b, M, N, K, torch.float16, variant=variant, bn=bn)
     assert bool((y32[:, 0::3] > 65504).all()) and bool((y32[:, 1::3] < -65504).all())
-    assert _eq16(y16, R.sat_rn(y32, True))
+    assert support.eq16(y16, R.sat_rn(y32, True))
     assert bool((y16[:, 0::3] == 65504).all()) and bool((y16[:, 1::3] == -65504).all())
     if N % 8 == 0:
         y16b, _ = _linear(x, w, b, M, N, K, torch.float16, outs="16", variant=variant, bn=bn)
-        assert _eq16(y16b, y16) and not bool(torch.isinf(y16b.float()).any())
+        assert support.eq16(y16b, y16) and not bool(torch.isinf(y16b.float()).any())
 
 
 @pytest.mark.parametrize("dt", DTS, ids=DT_IDS)
@@ -733,10 +712,10 @@ def test_layernorm_row_kernel_16bit_rounding(dt):
     gamma, beta = 1 + 0.1 * torch.randn(N, generator=g, device="cuda"), 0.1 * torch.randn(N, generator=g, device="cuda")
     of = torch.full((M, N), NAN, device="cuda")
     oh = torch.full((M, N), NAN, dtype=dt, device="cuda")
-    _call("vb200_layernorm", y, N, res, N, gamma, beta, 1e-12, of, N, oh, N, M, N, _f16(dt))
+    support.call("vb200_layernorm", y, N, res, N, gamma, beta, 1e-12, of, N, oh, N, M, N, _f16(dt))
     torch.cuda.synchronize()
     assert bool((of.abs() < 65504).all())
-    assert _eq16(oh, R.sat_rn(of, dt == torch.float16))
+    assert support.eq16(oh, R.sat_rn(of, dt == torch.float16))
 
 
 def _ref_product(x, w, b, act, mul):
@@ -764,15 +743,15 @@ def test_linear_product(case, dt, parity_log):
     ld16, ld32 = (N + 7) // 8 * 8, (N + 3) // 4 * 4
     y16 = torch.full((M, ld16), NAN, dtype=dt, device="cuda")
     y32 = torch.full((M, ld32), NAN, device="cuda")
-    _call("vb200_linear_product", x, ld_x, w, K, b, 2, mul, ld_mul, y16, ld16, y32, ld32, M, N, K, 0, _f16(dt))
+    support.call("vb200_linear_product", x, ld_x, w, K, b, 2, mul, ld_mul, y16, ld16, y32, ld32, M, N, K, 0, _f16(dt))
     y16o = torch.full((M, ld16), NAN, dtype=dt, device="cuda")
-    _call("vb200_linear_product", x, ld_x, w, K, b, 2, mul, ld_mul, y16o, ld16, None, 0, M, N, K, 0, _f16(dt))
+    support.call("vb200_linear_product", x, ld_x, w, K, b, 2, mul, ld_mul, y16o, ld16, None, 0, M, N, K, 0, _f16(dt))
     torch.cuda.synchronize()
     err = (y32[:, :N].double() - ref).abs().max().item()
     parity_log(test="kp_linear_product", M=M, N=N, K=K, ld_mul=ld_mul, dtype=str(dt), max_abs_err=err, bound=2e-3)
     assert err < 2e-3, err
-    assert _eq16(y16[:, :N], R.sat_rn(y32[:, :N], dt == torch.float16))
-    assert _eq16(y16o[:, :N], y16[:, :N])
+    assert support.eq16(y16[:, :N], R.sat_rn(y32[:, :N], dt == torch.float16))
+    assert support.eq16(y16o[:, :N], y16[:, :N])
     assert _is_nan(y32[:, N:]) and _is_nan(y16[:, N:])
 
 
@@ -787,9 +766,9 @@ def test_coop_device_row_count(N, m, dt):
     ld16, ld32 = (N + 7) // 8 * 8, (N + 3) // 4 * 4
     y16 = torch.full((M, ld16), NAN, dtype=dt, device="cuda")
     y32 = torch.full((M, ld32), NAN, device="cuda")
-    _call("vb200_linear_rows", x, K, w, K, b, 0, y16, ld16, y32, ld32, M, N, K, 0, _f16(dt), _dev_i32([m]))
+    support.call("vb200_linear_rows", x, K, w, K, b, 0, y16, ld16, y32, ld32, M, N, K, 0, _f16(dt), _dev_i32([m]))
     r16, r32 = _linear(x, w, b, M, N, K, dt)
-    assert _eq32(y32[:m, :N], r32[:m]) and _eq16(y16[:m, :N], r16[:m])
+    assert support.eq32(y32[:m, :N], r32[:m]) and support.eq16(y16[:m, :N], r16[:m])
     boundary = (m + 127) // 128 * 128
     assert _is_nan(y32[boundary:]) and _is_nan(y16[boundary:])
     assert _is_nan(y32[:, N:]) and _is_nan(y16[:, N:])
@@ -817,6 +796,7 @@ def test_coop_plain_gemm_pdl_chain(dt):
     for o in outs:
         assert not _is_nan(o[3]) and not bool(torch.isnan(o[3]).any())
     for o in outs[1:]:
-        assert _eq16(o[0], outs[0][0]) and _eq16(o[1], outs[0][1]) and _eq16(o[2], outs[0][2]) and _eq32(o[3], outs[0][3])
+        assert support.eq16(o[0], outs[0][0]) and support.eq16(o[1], outs[0][1]) and support.eq16(o[2], outs[0][2]) \
+            and support.eq32(o[3], outs[0][3])
     ref = R.sat_rn(outs[0][3], dt == torch.float16)
-    assert _eq16(outs[0][2], ref)
+    assert support.eq16(outs[0][2], ref)

@@ -11,30 +11,17 @@ import numpy as np
 import pytest
 import torch
 
+import support
+
 pytestmark = pytest.mark.gpu
 
 ROWS = {"all": 0, "first": 1, "mean": 2}
 TOL = {"fp16": 1e-2, "bf16": 3.5e-2}     # rel_err of oracle/fp64.py against the fp32 oracle, the model tests' logit tolerances
 
 
-def _lib():
-    from vilbert_b200 import _lib as L
-    return L
-
-
-def _engine(oracle, **kw):
-    import vilbert_b200 as vb
-    cfg = vb.BertConfig.from_dict(oracle.config.to_dict())
-    return vb.VILBertForVLTasks.from_pretrained(oracle.state_dict(), config=cfg, num_labels=oracle.num_labels, return_attention=True,
-                                                **kw).eval().cuda(0)
-
-
 @pytest.fixture(scope="module")
 def tiny(tiny_oracle):
-    e = {k: _engine(tiny_oracle, compute_dtype=k) for k in ("fp16", "bf16", "fp32x")}
-    yield e
-    for m in e.values():
-        m.close()
+    yield from support.engines(tiny_oracle, ("fp16", "bf16", "fp32x"), return_attention=True)
 
 
 class _States:
@@ -54,13 +41,6 @@ class _States:
     def __exit__(self, *exc):
         self.model.set_option("state_entries", (1 << len(self.model.state_selection()[0])) - 1)
         self.model.set_option("state_rows", 0)
-
-
-def _tiny_inputs(oracle, B, Tin, V, seed, pad=0):
-    from oracle import vilbert_ref as R
-    inp = list(R.make_inputs(B, Tin, V, seed=seed, vocab_size=oracle.config.vocab_size, pad_regions=pad))
-    inp[1] = inp[1][..., :oracle.config.v_feature_size].contiguous()
-    return inp
 
 
 def _oracle_entries(oracle, inp):
@@ -114,7 +94,7 @@ def _eq_nan(a, b):
 def test_oracle_parity_tiny(tiny, tiny_oracle, mode, parity_log):
     from oracle import fp64 as X
     model = tiny[mode]
-    inp = _tiny_inputs(tiny_oracle, 3, 14, 20, seed=31, pad=4)
+    inp = support.tiny_inputs(tiny_oracle, 3, 14, 20, seed=31, pad=4)
     _, states = _dense(model, inp)
     ref = _oracle_entries(tiny_oracle, inp)
     assert len(states) == len(ref) == 32
@@ -125,7 +105,7 @@ def test_oracle_parity_tiny(tiny, tiny_oracle, mode, parity_log):
 
 def test_oracle_parity_fp32x_vs_fp64(tiny, tiny_oracle, parity_log):
     from oracle import fp64 as X
-    inp = _tiny_inputs(tiny_oracle, 2, 12, 17, seed=32, pad=3)
+    inp = support.tiny_inputs(tiny_oracle, 2, 12, 17, seed=32, pad=3)
     _, states = _dense(tiny["fp32x"], inp)
     ref = _oracle_entries(X.fp64(tiny_oracle), inp)
     errs = [X.rel_err(s, r) for s, r in zip(states, ref)]
@@ -136,7 +116,7 @@ def test_oracle_parity_fp32x_vs_fp64(tiny, tiny_oracle, parity_log):
 def test_oracle_parity_full_model_bf16(full_oracle, parity_log):
     from oracle import fp64 as X
     from oracle import vilbert_ref as R
-    model = _engine(full_oracle, compute_dtype="bf16")
+    model = support.engine(full_oracle, compute_dtype="bf16", return_attention=True)
     try:
         inp = list(R.make_inputs(2, 20, 36, seed=33, pad_regions=5))
         _, states = _dense(model, inp)
@@ -145,7 +125,7 @@ def test_oracle_parity_full_model_bf16(full_oracle, parity_log):
         parity_log(test="layer_states_full_bf16", max_rel_err=max(errs))
         assert max(errs) < TOL["bf16"], errs
         # per-sample identity on the full model: packed regions of each sample vs that sample alone
-        samples = _batch(model, [(9, 30), (20, 12)], seed=34)
+        samples = support.batch(model, [(9, 30), (20, 12)], seed=34)
         for rows in ROWS:
             with _States(model, rows=rows):
                 _check_packed_vs_alone(model, samples, rows)
@@ -157,7 +137,7 @@ def test_oracle_parity_full_model_bf16(full_oracle, parity_log):
 @pytest.mark.parametrize("mode", ("fp16", "bf16"))
 def test_reductions_dense_exact(tiny, tiny_oracle, mode):
     model = tiny[mode]
-    inp = _tiny_inputs(tiny_oracle, 3, 14, 20, seed=41, pad=6)
+    inp = support.tiny_inputs(tiny_oracle, 3, 14, 20, seed=41, pad=6)
     (_, taps), rows = _dense(model, inp)
     lt, lv = _last(model)
     _eq(rows[lt], taps["sequence_output_t"])
@@ -178,45 +158,12 @@ def test_reductions_dense_exact(tiny, tiny_oracle, mode):
         _eq(mean[e], ref)
 
 
-def _sample(tin, v, seed, F, vocab):
-    g = torch.Generator().manual_seed(seed)
-    q = torch.randint(1, vocab, (tin,), generator=g)
-    f = torch.relu(torch.randn(v, F, generator=g)) * 1.5
-    x1, y1 = torch.rand(v, generator=g) * 0.7, torch.rand(v, generator=g) * 0.7
-    x2, y2 = x1 + 0.05 + torch.rand(v, generator=g) * 0.25, y1 + 0.05 + torch.rand(v, generator=g) * 0.25
-    s = torch.stack([x1, y1, x2.clamp(max=1.0), y2.clamp(max=1.0), (x2 - x1) * (y2 - y1)], dim=-1)
-    s[0] = torch.tensor([0.0, 0.0, 1.0, 1.0, 1.0])
-    seg = torch.randint(0, 2, (tin,), generator=g)
-    return q, seg, f, s, int(torch.randint(0, 20, (1,), generator=g))
-
-
-def _batch(model, lens, seed):
-    F, vocab = model._dims["v_feature_size"], model._dims["vocab_size"]
-    return [_sample(t, v, seed + i, F, vocab) for i, (t, v) in enumerate(lens)]
-
-
-def _packed_args(samples):
-    cat = lambda k: torch.cat([s[k] for s in samples], dim=0).cuda()
-    task = torch.tensor([[s[4]] for s in samples]).cuda()
-    return cat(0), cat(2), cat(3), cat(1), task, [len(s[0]) for s in samples], [s[2].shape[0] for s in samples]
-
-
 def _packed(model, samples, states=True, sync=True, **kw):
-    L = _lib()
-    out = model.forward_packed(*_packed_args(samples), select=L.OUT_TASK_HEADS, debug_taps=True, output_layer_states=states, **kw)
+    L = support.lib()
+    out = model.forward_packed(*support.packed_sample_args(samples), select=L.OUT_TASK_HEADS, debug_taps=True, output_layer_states=states, **kw)
     if sync:
         torch.cuda.synchronize()
     return out
-
-
-def _alone(model, smp):
-    L = _lib()
-    q, seg, f, s, task = smp
-    (_, states) = model(q[None].cuda(), f[None].cuda(), s[None].cuda(), seg[None].cuda(), torch.ones(1, len(q), dtype=torch.long).cuda(),
-                        torch.ones(1, f.shape[0], dtype=torch.uint8).cuda(), None, torch.tensor([[task]]).cuda(), select=L.OUT_TASK_HEADS,
-                        output_layer_states=True)
-    torch.cuda.synchronize()
-    return states
 
 
 def _check_packed_vs_alone(model, samples, rows, regions=False):
@@ -226,7 +173,7 @@ def _check_packed_vs_alone(model, samples, rows, regions=False):
         got, alone = _regions(model, samples)
     else:
         (_, got) = _packed(model, samples)
-        alone = [_alone(model, s) for s in samples]
+        alone = [support.dense_alone(model, s, select=support.lib().OUT_TASK_HEADS, output_layer_states=True)[1] for s in samples]
     for e, entry in enumerate(got):
         for b, ref in enumerate(alone):
             _eq_nan(entry[b], ref[e][0])      # rows: sample b's [L_b, H] view vs [1, L_b, H]; first / mean: [H] vs [1, H]
@@ -238,7 +185,7 @@ LENS = [(1, 40), (31, 1), (12, 64), (5, 17)]
 @pytest.mark.parametrize("mode", ("fp16", "bf16"))
 def test_reductions_packed_exact(tiny, mode):
     model = tiny[mode]
-    samples = _batch(model, LENS, seed=500)
+    samples = support.batch(model, LENS, seed=500)
     (_, taps), rows = _packed(model, samples)
     lt, lv = _last(model)
     _eq(torch.cat(rows[lt]), taps["sequence_output_t"])
@@ -257,7 +204,7 @@ def test_reductions_packed_exact(tiny, mode):
 def test_packed_per_sample_identity(tiny, mode, rows):
     model = tiny[mode]
     with _States(model, rows=rows):
-        _check_packed_vs_alone(model, _batch(model, LENS, seed=600), rows)
+        _check_packed_vs_alone(model, support.batch(model, LENS, seed=600), rows)
 
 
 def test_packed_per_sample_identity_past_256_rows(tiny):
@@ -266,13 +213,13 @@ def test_packed_per_sample_identity_past_256_rows(tiny):
     try:
         for rows in ROWS:
             with _States(model, rows=rows):
-                _check_packed_vs_alone(model, _batch(model, [(150, 300), (3, 512), (40, 20)], seed=650), rows)
+                _check_packed_vs_alone(model, support.batch(model, [(150, 300), (3, 512), (40, 20)], seed=650), rows)
     finally:
         model.set_option("max_rows_per_sample", 256)
 
 
 def _regions(model, imgs_lens):
-    L = _lib()
+    L = support.lib()
     F, vocab = model._dims["v_feature_size"], model._dims["vocab_size"]
     imgs = []
     for i, (tin, n) in enumerate(imgs_lens):
@@ -316,7 +263,7 @@ def _same(a, b):
 @pytest.mark.parametrize("mode", ("fp16", "bf16", "fp32x"))
 def test_selection_and_no_side_effects_dense(tiny, tiny_oracle, mode):
     model = tiny[mode]
-    inp = _tiny_inputs(tiny_oracle, 2, 10, 15, seed=51, pad=2)
+    inp = support.tiny_inputs(tiny_oracle, 2, 10, 15, seed=51, pad=2)
     plain = _dense(model, inp, states=False, output_all_attention_masks=True)
     res, every = _dense(model, inp, output_all_attention_masks=True)
     _same(res, plain)
@@ -336,7 +283,7 @@ def test_selection_and_no_side_effects_dense(tiny, tiny_oracle, mode):
 
 def test_no_side_effects_packed(tiny):
     model = tiny["fp16"]
-    samples = _batch(model, LENS, seed=700)
+    samples = support.batch(model, LENS, seed=700)
     plain = _packed(model, samples, states=False, output_all_attention_masks=True)
     res, every = _packed(model, samples, output_all_attention_masks=True)
     _same(res, plain)
@@ -352,7 +299,7 @@ def test_no_side_effects_packed(tiny):
 
 # ------------------------------------------------------------------------------------------------------------ pruning
 def test_pruning(tiny):
-    L = _lib()
+    L = support.lib()
     model = tiny["fp16"]
     lt, lv = _last(model)
     base_n, base_f = model.plan_info(4, 12, 20, L.OUT_VIL_PREDICTION)
@@ -381,20 +328,20 @@ def test_pruning(tiny):
 
 # ------------------------------------------------------------------------------------------------------------ plans and buffers
 def test_plans_and_buffers(tiny, tiny_oracle):
-    L = _lib()
+    L = support.lib()
     model = tiny["bf16"]
     model.set_option("max_plans", 1024)           # no eviction hides a plan built or reused below
-    samples = _batch(model, LENS, seed=800)
+    samples = support.batch(model, LENS, seed=800)
     _packed(model, samples)
-    n0 = _n_plans(model)
+    n0 = support.n_plans(model)
     _packed(model, samples)
-    assert _n_plans(model) == n0                      # same selection: the plan is reused
+    assert support.n_plans(model) == n0                      # same selection: the plan is reused
     with _States(model, [4, 6]):
         _packed(model, samples)
-        assert _n_plans(model) == n0 + 1              # changed selection: a plan of its own
+        assert support.n_plans(model) == n0 + 1              # changed selection: a plan of its own
     ref = _packed(model, samples)[1]
     # unsynchronised back-to-back calls into different buffers each get their own states
-    other = _batch(model, [(3, 5), (20, 33), (7, 7), (2, 60)], seed=801)
+    other = support.batch(model, [(3, 5), (20, 33), (7, 7), (2, 60)], seed=801)
     a = _packed(model, samples, sync=False)[1]
     b = _packed(model, other, sync=False)[1]
     c = _packed(model, samples, sync=False)[1]
@@ -413,7 +360,7 @@ def test_plans_and_buffers(tiny, tiny_oracle):
             flat = torch.full((total,), float("nan"), device="cuda")
             o = L.StateOutputs()
             o.layer_states = flat.data_ptr()
-            q, f, s, seg, task, _, _ = _packed_args(samples)
+            q, f, s, seg, task, _, _ = support.packed_sample_args(samples)
             pin = L.PackedInputs(len(samples), 0, 0, C.cast((C.c_int32 * 4)(*nt), C.c_void_p), C.cast((C.c_int32 * 4)(*nr), C.c_void_p),
                                  q.data_ptr(), seg.data_ptr(), f.data_ptr(), s.data_ptr(), task.data_ptr())
             model._call("vb200_forward_packed", C.byref(pin), C.byref(o), L.OUT_TASK_HEADS | L.OUT_LAYER_STATES, 0)
@@ -421,14 +368,14 @@ def test_plans_and_buffers(tiny, tiny_oracle):
             assert not torch.isnan(flat).any(), rows
             _, total_d = model.state_layout(2, 9, 13)
             flat_d = torch.full((total_d,), float("nan"), device="cuda")
-            assert _dense_raw(model, _tiny_inputs(tiny_oracle, 2, 9, 13, seed=802, pad=3), flat_d.data_ptr()) == 0
+            assert _dense_raw(model, support.tiny_inputs(tiny_oracle, 2, 9, 13, seed=802, pad=3), flat_d.data_ptr()) == 0
             torch.cuda.synchronize()
             assert not torch.isnan(flat_d).any(), rows
 
 
 def _dense_raw(model, inp, states_ptr, select=None, fn="vb200_forward"):
     """vb200_forward (or the host-buffer ``fn``) of make_inputs tensors with vb200_outputs.layer_states = states_ptr; the status."""
-    L = _lib()
+    L = support.lib()
     q, f, s, seg, im, vm = inp[:6]
     B, Tin = q.shape
     dev = "cpu" if fn.startswith("vb200_forward_host") else "cuda"
@@ -444,15 +391,9 @@ def _dense_raw(model, inp, states_ptr, select=None, fn="vb200_forward"):
     return getattr(lib, fn)(model._handle, C.byref(di), C.byref(o), sel, None)
 
 
-def _n_plans(model):
-    v = C.c_int64()
-    _lib().check(_lib().load().vb200_model_dim(model._handle, b"n_plans", C.byref(v)), model._handle)
-    return v.value
-
-
 # ------------------------------------------------------------------------------------------------------------ options and rejections
 def test_options_read_back_and_validation(tiny, tiny_oracle):
-    L = _lib()
+    L = support.lib()
     model = tiny["fp16"]
     # the engine's full list is the specified one: embeddings, then per step its text state before its image state
     spec = [0, 1]
@@ -475,12 +416,12 @@ def test_options_read_back_and_validation(tiny, tiny_oracle):
 
 
 def test_rejections(tiny, tiny_oracle):
-    L = _lib()
+    L = support.lib()
     model = tiny["fp16"]
     lib = L.load()
     h = model._handle
     flat = torch.full((64,), -7.0, device="cuda")
-    inp = _tiny_inputs(tiny_oracle, 1, 6, 5, seed=90)
+    inp = support.tiny_inputs(tiny_oracle, 1, 6, 5, seed=90)
     bit = L.OUT_VIL_LOGIT | L.OUT_LAYER_STATES
 
     def rejects(rc, name):
@@ -506,8 +447,8 @@ def test_rejections(tiny, tiny_oracle):
     # the bit without a buffer, or with one the 16-byte state stores cannot write: dense and packed
     rejects(_dense_raw(model, inp, None, bit), "layer_states (NULL)")
     rejects(_dense_raw(model, inp, flat[1:].data_ptr(), bit), "vb200_forward: vb200_outputs.layer_states is not 16-byte aligned")
-    samples = _batch(model, [(3, 4), (5, 2)], seed=92)
-    q, f, s, seg, task, nt, nr = _packed_args(samples)
+    samples = support.batch(model, [(3, 4), (5, 2)], seed=92)
+    q, f, s, seg, task, nt, nr = support.packed_sample_args(samples)
     pin = L.PackedInputs(2, 0, 0, C.cast((C.c_int32 * 2)(*nt), C.c_void_p), C.cast((C.c_int32 * 2)(*nr), C.c_void_p),
                          q.data_ptr(), seg.data_ptr(), f.data_ptr(), s.data_ptr(), task.data_ptr())
     o.layer_states = flat[2:].data_ptr()
@@ -516,7 +457,7 @@ def test_rejections(tiny, tiny_oracle):
     # fp32x keeps rejecting packed calls as before
     x = tiny["fp32x"]
     with pytest.raises(L.VilbertB200Error, match="split_fp32"):
-        x.forward_packed(*_packed_args(_batch(model, [(3, 4)], seed=91)), output_layer_states=True)
+        x.forward_packed(*support.packed_sample_args(support.batch(model, [(3, 4)], seed=91)), output_layer_states=True)
 
 
 def test_pretraining_engine_accepts_states():
@@ -528,15 +469,15 @@ def test_pretraining_engine_accepts_states():
                                                            compute_dtype="bf16").eval().cuda(0)
     try:
         lt, lv = _last(model)
-        samples = _batch(model, [(4, 9), (11, 3)], seed=93)
-        (_, taps), states = model.forward_packed(*_packed_args(samples), select=0, debug_taps=True, output_layer_states=True)
+        samples = support.batch(model, [(4, 9), (11, 3)], seed=93)
+        (_, taps), states = model.forward_packed(*support.packed_sample_args(samples), select=0, debug_taps=True, output_layer_states=True)
         _eq(torch.cat(states[lt]), taps["sequence_output_t"])
         _eq(torch.cat(states[lv]), taps["sequence_output_v"])
         q, seg, f, s, task = samples[0]
         (_, taps_d), states_d = vb.VILBertForVLTasks.forward(
             model, q[None].cuda(), f[None].cuda(), s[None].cuda(), seg[None].cuda(), torch.ones(1, len(q), dtype=torch.long).cuda(),
-            torch.ones(1, f.shape[0], dtype=torch.uint8).cuda(), None, torch.tensor([[task]]).cuda(), select=_lib().OUT_LINGUISIC_PREDICTION | _lib().OUT_VISION_PREDICTION,
-            debug_taps=True, output_layer_states=True)
+            torch.ones(1, f.shape[0], dtype=torch.uint8).cuda(), None, torch.tensor([[task]]).cuda(),
+            select=support.lib().OUT_LINGUISIC_PREDICTION | support.lib().OUT_VISION_PREDICTION, debug_taps=True, output_layer_states=True)
         torch.cuda.synchronize()
         _eq(states_d[lt], taps_d["sequence_output_t"])
         _eq(states_d[lv], taps_d["sequence_output_v"])

@@ -13,6 +13,7 @@ import torch
 
 from oracle import kernel_refs as KR
 from oracle import detections_ref as D
+import support
 
 pytestmark = pytest.mark.gpu
 
@@ -29,17 +30,6 @@ LONG = [257, 300, 511, 513, 777, 1024]
 
 
 # ------------------------------------------------------------------------------------------------------------------ op hooks
-def _call(name, *args):
-    from vilbert_b200 import _lib as L
-    lib = L.load()
-    ptrs = [a.data_ptr() if torch.is_tensor(a) else a for a in args]
-    L.check(getattr(lib, name)(*ptrs, C.c_void_p(torch.cuda.current_stream().cuda_stream)), None)
-
-
-def _eq16(a, b):
-    return torch.equal(a.contiguous().view(torch.int16), b.contiguous().view(torch.int16))
-
-
 def _f16(dt):
     return 1 if dt == torch.float16 else 0
 
@@ -68,14 +58,14 @@ def _key_mask(L, b):
 
 def _self(hook, qkv, ld_qkv, H, mask, B, L, heads, d, dt, ld_ctx, offs=None, rows=None):
     ctx = torch.full(((rows if rows is not None else B * L) + 16, ld_ctx), NAN, dtype=dt, device="cuda")
-    _call(hook, qkv, ld_qkv, H, mask, ctx, ld_ctx, B, L, heads, d, _f16(dt), offs)
+    support.call(hook, qkv, ld_qkv, H, mask, ctx, ld_ctx, B, L, heads, d, _f16(dt), offs)
     return ctx
 
 
 def _co(hook, qi, ld_i, qt, ld_t, H, mi, mt, B, T, V, heads, d, dt, ot=None, ov=None, rows_t=None, rows_v=None):
     ct = torch.full(((rows_t if rows_t is not None else B * T) + 16, H + 8), NAN, dtype=dt, device="cuda")
     ci = torch.full(((rows_v if rows_v is not None else B * V) + 16, H), NAN, dtype=dt, device="cuda")
-    _call(hook, qi, ld_i, qt, ld_t, H, mi, mt, ct, H + 8, ci, H, B, T, V, heads, d, _f16(dt), ot, ov)
+    support.call(hook, qi, ld_i, qt, ld_t, H, mi, mt, ct, H + 8, ci, H, B, T, V, heads, d, _f16(dt), ot, ov)
     return ct, ci
 
 
@@ -96,7 +86,7 @@ def test_stream_self_equals_staged(d, dt):
         a = _self("vb200_self_attention_stream", qkv, ld_qkv, H, mask, 2, L, heads, d, dt, ld_ctx)
         b = _self("vb200_self_attention_packed", qkv, ld_qkv, H, mask, 2, L, heads, d, dt, ld_ctx, _dev_i32([0, L, 2 * L]))
         torch.cuda.synchronize()
-        assert _eq16(a, b), f"dense L = {L}"
+        assert support.eq16(a, b), f"dense L = {L}"
     offs = _offs(BOTH_SIDES)
     qkv = torch.randn(offs[-1], ld_qkv, generator=_gen(d), device="cuda").to(dt)
     mask = torch.cat([_key_mask(L, b) for b, L in enumerate(BOTH_SIDES)]).cuda()
@@ -104,7 +94,7 @@ def test_stream_self_equals_staged(d, dt):
     a = _self("vb200_self_attention_stream", qkv, ld_qkv, H, mask, len(BOTH_SIDES), 256, heads, d, dt, ld_ctx, o, offs[-1])
     b = _self("vb200_self_attention_packed", qkv, ld_qkv, H, mask, len(BOTH_SIDES), 256, heads, d, dt, ld_ctx, o, offs[-1])
     torch.cuda.synchronize()
-    assert _eq16(a, b)
+    assert support.eq16(a, b)
 
 
 CO_PAIRS = [(1, 1), (15, 65), (65, 15), (16, 17), (63, 64), (64, 63), (129, 17), (17, 129), (256, 31), (31, 256), (128, 256)]
@@ -125,7 +115,7 @@ def test_stream_co_equals_staged(d, dt):
         a = _co("vb200_co_attention_stream", qi, ld_i, qt, ld_t, H, mi, mt, 2, T, V, heads, d, dt)
         b = _co("vb200_co_attention", qi, ld_i, qt, ld_t, H, mi, mt, 2, T, V, heads, d, dt)
         torch.cuda.synchronize()
-        assert _eq16(a[0], b[0]) and _eq16(a[1], b[1]), f"dense T = {T}, V = {V}"
+        assert support.eq16(a[0], b[0]) and support.eq16(a[1], b[1]), f"dense T = {T}, V = {V}"
     T_l, V_l = [t for t, _ in CO_PAIRS], [v for _, v in CO_PAIRS]
     ot, ov = _offs(T_l), _offs(V_l)
     g = _gen(d + 5)
@@ -136,7 +126,7 @@ def test_stream_co_equals_staged(d, dt):
     args = (qi, ld_i, qt, ld_t, H, mi, mt, len(T_l), 256, 256, heads, d, dt, _dev_i32(ot), _dev_i32(ov), ot[-1], ov[-1])
     a, b = _co("vb200_co_attention_stream", *args), _co("vb200_co_attention_packed", *args)
     torch.cuda.synchronize()
-    assert _eq16(a[0], b[0]) and _eq16(a[1], b[1])
+    assert support.eq16(a[0], b[0]) and support.eq16(a[1], b[1])
 
 
 @pytest.mark.parametrize("dt", DTS, ids=DT_IDS)
@@ -196,20 +186,12 @@ def test_stream_packed_mix_equals_dense(d, dt):
         dt_, di_ = _co("vb200_co_attention_stream", qi[sv], ld, qkv[sl], ld, H, mi[sv].contiguous(), mask[sl].contiguous(), 1, L,
                        rev[b], heads, d, dt)
         torch.cuda.synchronize()
-        assert _eq16(packed[sl], dense[:L]), f"self sample {b} (L = {L})"
-        assert _eq16(ct[sl], dt_[:L]) and _eq16(ci[sv], di_[:rev[b]]), f"co sample {b} (T = {L}, V = {rev[b]})"
+        assert support.eq16(packed[sl], dense[:L]), f"self sample {b} (L = {L})"
+        assert support.eq16(ct[sl], dt_[:L]) and support.eq16(ci[sv], di_[:rev[b]]), f"co sample {b} (T = {L}, V = {rev[b]})"
     assert torch.isnan(packed[offs[-1]:].float()).all()
 
 
 # ------------------------------------------------------------------------------------------------------------------ engines
-def _engine(oracle, rows=None, **kw):
-    import vilbert_b200 as vb
-    cfg = vb.BertConfig.from_dict(oracle.config.to_dict())
-    if rows is not None:
-        kw["max_rows_per_sample"] = rows
-    return vb.VILBertForVLTasks.from_pretrained(oracle.state_dict(), config=cfg, num_labels=oracle.num_labels, **kw).eval().cuda(0)
-
-
 @pytest.fixture(scope="module")
 def long_oracle():
     from oracle import vilbert_ref as R
@@ -218,16 +200,13 @@ def long_oracle():
 
 @pytest.fixture(scope="module")
 def long_tiny(long_oracle):
-    e = {k: _engine(long_oracle, 1024, compute_dtype=k) for k in ("fp16", "bf16")}
-    yield e
-    for m in e.values():
-        m.close()
+    yield from support.engines(long_oracle, ("fp16", "bf16"), max_rows_per_sample=1024)
 
 
 def test_defaults_unchanged(long_oracle):
     """A default engine keeps the 256-row bound and its messages; the option accepts 256 ... 1024 only."""
     from vilbert_b200 import _lib as L
-    m = _engine(long_oracle)
+    m = support.engine(long_oracle)
     try:
         v = C.c_int64()
         L.check(L.load().vb200_model_dim(m._handle, b"max_rows_per_sample", C.byref(v)), m._handle)
@@ -247,7 +226,7 @@ def test_defaults_unchanged(long_oracle):
                 m.set_option("max_rows_per_sample", bad)
         assert m.max_rows_per_sample == 256
         with pytest.raises(ValueError):
-            _engine(long_oracle, 1025)
+            support.engine(long_oracle, max_rows_per_sample=1025)
         # raising and lowering the bound is validation only
         m.set_option("max_rows_per_sample", 300)
         m.plan_info(1, 256, 36)
@@ -260,7 +239,7 @@ def test_defaults_unchanged(long_oracle):
 
 def test_default_plan_launches_unchanged(tiny_oracle):
     """The plan of a short shape is the same launch list whatever the bound."""
-    a, b = _engine(tiny_oracle), _engine(tiny_oracle, 1024)
+    a, b = support.engine(tiny_oracle), support.engine(tiny_oracle, max_rows_per_sample=1024)
     try:
         for shape in [(2, 30, 36), (1, 155, 256)]:
             assert a.plan_info(*shape) == b.plan_info(*shape)
@@ -271,13 +250,6 @@ def test_default_plan_launches_unchanged(tiny_oracle):
 
 NAMES = ["vil_prediction", "vil_prediction_gqa", "vil_logit", "vil_binary_prediction", "vil_tri_prediction",
          "vision_prediction", "vision_logit", "linguisic_prediction", "linguisic_logit"]
-
-
-def _inputs(oracle, B, Tin, V, seed):
-    from oracle import vilbert_ref as R
-    inp = list(R.make_inputs(B, Tin, V, seed=seed, vocab_size=oracle.config.vocab_size))
-    inp[1] = inp[1][..., :oracle.config.v_feature_size].contiguous()
-    return inp
 
 
 def _check_vs_oracle(oracle, model, inputs, tol_fn, tag, parity_log):
@@ -301,15 +273,16 @@ def _check_vs_oracle(oracle, model, inputs, tol_fn, tag, parity_log):
 def test_long_model_vs_oracle(long_oracle, long_tiny, mode, Tin, V, parity_log):
     """Tiny 12/6/6 model with 1024 positions and the bound at 1024: all nine outputs of dense long forwards vs the fp32 oracle."""
     tol = (lambda s: TOL) if mode == "fp16" else (lambda s: TOL_BF16_VS_FP32 * max(1.0, s))
-    _check_vs_oracle(long_oracle, long_tiny[mode], _inputs(long_oracle, 1, Tin, V, Tin + V), tol, f"long_{mode}_T{Tin}_V{V}", parity_log)
+    _check_vs_oracle(long_oracle, long_tiny[mode], support.tiny_inputs(long_oracle, 1, Tin, V, Tin + V), tol, f"long_{mode}_T{Tin}_V{V}",
+                     parity_log)
 
 
 def test_long_model_fp32x_vs_oracle(long_oracle, parity_log):
     """fp32-parity mode (fp32 attention kernel) on dense long forwards: 1e-3 against the fp32 oracle."""
-    m = _engine(long_oracle, 1024, compute_dtype="fp32x")
+    m = support.engine(long_oracle, compute_dtype="fp32x", max_rows_per_sample=1024)
     try:
         for Tin, V in [(300, 36), (511, 257), (30, 1000)]:
-            _check_vs_oracle(long_oracle, m, _inputs(long_oracle, 1, Tin, V, Tin + V), lambda s: TOL_FP32X, f"long_fp32x_T{Tin}_V{V}",
+            _check_vs_oracle(long_oracle, m, support.tiny_inputs(long_oracle, 1, Tin, V, Tin + V), lambda s: TOL_FP32X, f"long_fp32x_T{Tin}_V{V}",
                              parity_log)
     finally:
         m.close()
@@ -317,35 +290,15 @@ def test_long_model_fp32x_vs_oracle(long_oracle, parity_log):
 
 def test_full_model_long(full_oracle, parity_log):
     """The 268 M model once at (Tin, V) = (511, 300) in bf16."""
-    m = _engine(full_oracle, 1024, compute_dtype="bf16")
+    m = support.engine(full_oracle, compute_dtype="bf16", max_rows_per_sample=1024)
     try:
-        _check_vs_oracle(full_oracle, m, list(_inputs(full_oracle, 1, 511, 300, 5)), lambda s: TOL_BF16_VS_FP32 * max(1.0, s),
+        _check_vs_oracle(full_oracle, m, list(support.tiny_inputs(full_oracle, 1, 511, 300, 5)), lambda s: TOL_BF16_VS_FP32 * max(1.0, s),
                          "long_full_bf16", parity_log)
     finally:
         m.close()
 
 
 # ------------------------------------------------------------------------------------------------------------------ packed
-def _sample(tin, v, seed, F, vocab):
-    g = torch.Generator().manual_seed(seed)
-    q = torch.randint(1, vocab, (tin,), generator=g)
-    f = torch.relu(torch.randn(v, F, generator=g)) * 1.5
-    x1, y1 = torch.rand(v, generator=g) * 0.7, torch.rand(v, generator=g) * 0.7
-    x2, y2 = x1 + 0.05 + torch.rand(v, generator=g) * 0.25, y1 + 0.05 + torch.rand(v, generator=g) * 0.25
-    s = torch.stack([x1, y1, x2.clamp(max=1.0), y2.clamp(max=1.0), (x2 - x1) * (y2 - y1)], dim=-1)
-    s[0] = torch.tensor([0.0, 0.0, 1.0, 1.0, 1.0])
-    seg = torch.randint(0, 2, (tin,), generator=g)
-    return q, seg, f, s, int(torch.randint(0, 20, (1,), generator=g))
-
-
-def _dense_alone(model, smp, select):
-    q, seg, f, s, task = smp
-    out = model(q[None].cuda(), f[None].cuda(), s[None].cuda(), seg[None].cuda(), torch.ones(1, len(q), dtype=torch.long).cuda(),
-                torch.ones(1, f.shape[0], dtype=torch.uint8).cuda(), None, torch.tensor([[task]]).cuda(), select=select)
-    torch.cuda.synchronize()
-    return out
-
-
 def _rows(t, counts):
     o = _offs(counts)
     return [t[o[i]:o[i + 1]] for i in range(len(counts))]
@@ -359,7 +312,7 @@ def _assert_per_sample(out, samples, dense_models, select_all):
     v_rows = [s[2].shape[0] for s in samples]
     for i, smp in enumerate(samples):
         for model in dense_models(smp):
-            ref = _dense_alone(model, smp, select_all)
+            ref = support.dense_alone(model, smp, select=select_all)
             for k in range(9):
                 if k == 3 or out[k] is None:
                     continue            # the pair head reads two samples
@@ -375,10 +328,10 @@ def test_packed_long_equals_dense(tiny_oracle, long_oracle, long_tiny):
     it alone; samples of at most 256 rows also equal a dense forward on a default engine (staged kernels)."""
     import vilbert_b200 as vb
     model = long_tiny["bf16"]
-    default = _engine(long_oracle, compute_dtype="bf16")
+    default = support.engine(long_oracle, compute_dtype="bf16")
     try:
         F, vocab = model._dims["v_feature_size"], model._dims["vocab_size"]
-        samples = [_sample(t, v, 30 + i, F, vocab) for i, (t, v) in enumerate(LENS)]
+        samples = [support.sample(t, v, 30 + i, F, vocab) for i, (t, v) in enumerate(LENS)]
         cat = lambda k: torch.cat([s[k] for s in samples], dim=0).cuda()
         task = torch.tensor([[s[4]] for s in samples]).cuda()
         out = model.forward_packed(cat(0), cat(2), cat(3), cat(1), task, [len(s[0]) for s in samples],
@@ -393,11 +346,11 @@ def test_packed_long_equals_dense(tiny_oracle, long_oracle, long_tiny):
 def test_packed_long_attention_maps(long_oracle):
     """Packed attention maps at lengths past 256 equal each sample's dense maps."""
     import vilbert_b200 as vb
-    model = _engine(long_oracle, 1024, compute_dtype="bf16", return_attention=True)
+    model = support.engine(long_oracle, compute_dtype="bf16", max_rows_per_sample=1024, return_attention=True)
     try:
         F, vocab = model._dims["v_feature_size"], model._dims["vocab_size"]
         lens = [(300, 20), (10, 280), (3, 3)]
-        samples = [_sample(t, v, 50 + i, F, vocab) for i, (t, v) in enumerate(lens)]
+        samples = [support.sample(t, v, 50 + i, F, vocab) for i, (t, v) in enumerate(lens)]
         cat = lambda k: torch.cat([s[k] for s in samples], dim=0).cuda()
         task = torch.tensor([[s[4]] for s in samples]).cuda()
         out = model.forward_packed(cat(0), cat(2), cat(3), cat(1), task, [len(s[0]) for s in samples],
@@ -418,31 +371,13 @@ def test_packed_long_attention_maps(long_oracle):
         model.close()
 
 
-def _regions_alone(model, im, select):
-    """vb200_forward_regions of one image (batch 1, its own Tin and box count, no padding): (10-tuple, spatials [1, V, 5])."""
-    from vilbert_b200 import _lib as L
-    q, seg, f, bx, wh, task = im
-    dev = lambda t, dt: torch.as_tensor(t).to(device="cuda", dtype=dt).contiguous()
-    q, seg, ones = dev(q[None], torch.int64), dev(seg[None], torch.int64), torch.ones(1, len(q), dtype=torch.int64, device="cuda")
-    tk, f, bx, wh = dev([[task]], torch.int64), dev(f[None], torch.float32), dev(bx[None], torch.float32), dev([wh], torch.float32)
-    n = f.shape[1]
-    sp = torch.empty(1, n + 1, 5, device="cuda")
-    inp = L.RegionInputs(1, q.shape[1], n, q.data_ptr(), seg.data_ptr(), ones.data_ptr(), tk.data_ptr(), f.data_ptr(), bx.data_ptr(),
-                         wh.data_ptr(), None, sp.data_ptr())
-    outs, o, select = model._alloc_outputs(1, q.shape[1], n + 1, select, False, False, torch.device("cuda", 0))
-    L.check(L.load().vb200_forward_regions(model._handle, C.byref(inp), C.byref(o), select, 0,
-                                           C.c_void_p(torch.cuda.current_stream().cuda_stream)), model._handle)
-    torch.cuda.synchronize()
-    return model._result(outs, 1, q.shape[1], n + 1, False), sp
-
-
 def test_regions_packed_long_equals_dense(long_oracle, long_tiny):
     """forward_regions_packed with images of up to 700 boxes and texts on both sides of 256 rows: each image's outputs and spatials
     equal a dense forward_regions of that image alone; images of at most 256 rows also equal it on a default engine (staged
     kernels), so the kernel the packed plan picked does not show."""
     import vilbert_b200 as vb
     model = long_tiny["fp16"]
-    default = _engine(long_oracle, compute_dtype="fp16")
+    default = support.engine(long_oracle, compute_dtype="fp16")
     F = model._dims["v_feature_size"]
     g = torch.Generator().manual_seed(3)
     cases = [(300, 400), (20, 100), (5, 700), (254, 255), (255, 40)]
@@ -463,7 +398,7 @@ def test_regions_packed_long_equals_dense(long_oracle, long_tiny):
         for i, b in enumerate(imgs):
             engines = [model] + ([default] if t_rows[i] <= 256 and v_rows[i] <= 256 else [])
             for eng in engines:
-                ref, rsp = _regions_alone(eng, b, vb.OUT_ALL)
+                ref, rsp = support.regions_alone(eng, b, vb.OUT_ALL)
                 assert torch.equal(_rows(sp, v_rows)[i], rsp[0]), i
                 for k in range(9):
                     if k == 3 or out[k] is None:
@@ -479,10 +414,10 @@ def test_packed_bound_not_multiple_of_16(long_oracle):
     bound run and equal dense forwards; one row more is rejected, naming the option."""
     import vilbert_b200 as vb
     from vilbert_b200 import _lib as L
-    m = _engine(long_oracle, 300, compute_dtype="fp16")
+    m = support.engine(long_oracle, compute_dtype="fp16", max_rows_per_sample=300)
     try:
         F, vocab = m._dims["v_feature_size"], m._dims["vocab_size"]
-        samples = [_sample(299, 300, 90, F, vocab), _sample(7, 291, 91, F, vocab), _sample(290, 3, 92, F, vocab)]
+        samples = [support.sample(299, 300, 90, F, vocab), support.sample(7, 291, 91, F, vocab), support.sample(290, 3, 92, F, vocab)]
         cat = lambda k: torch.cat([s[k] for s in samples], dim=0).cuda()
         task = torch.tensor([[s[4]] for s in samples]).cuda()
         nt, nv = [len(s[0]) for s in samples], [s[2].shape[0] for s in samples]
@@ -514,8 +449,8 @@ def test_retrieval_long_equals_forward_packed(long_tiny):
     import vilbert_b200 as vb
     model = long_tiny["fp16"]
     F, vocab = model._dims["v_feature_size"], model._dims["vocab_size"]
-    caps = [_sample(t, 1, 70 + i, F, vocab) for i, t in enumerate([400, 12, 256])]
-    ims = [_sample(1, v, 80 + i, F, vocab) for i, v in enumerate([300, 36, 257])]
+    caps = [support.sample(t, 1, 70 + i, F, vocab) for i, t in enumerate([400, 12, 256])]
+    ims = [support.sample(1, v, 80 + i, F, vocab) for i, v in enumerate([300, 36, 257])]
     pairs = [(0, 0), (1, 2), (2, 1), (0, 1), (2, 2)]
     task = 7
     nt = [len(c[0]) for c in caps]
@@ -552,7 +487,7 @@ def test_select_regions_600_boxes(long_tiny, tiny_oracle):
         np.testing.assert_array_equal(r["objects"][lo:lo + k].cpu().numpy(), ref["argmax"])
         assert torch.equal(r["boxes"][lo:lo + k].cpu(), torch.from_numpy(ref["bbox"]))
         assert torch.equal(r["box_features"][lo:lo + k].cpu(), torch.from_numpy(ref["features"]))
-    default = _engine(tiny_oracle, compute_dtype="bf16")
+    default = support.engine(tiny_oracle, compute_dtype="bf16")
     try:
         for K in (100, 255):
             a = m.select_regions(dets, K, cls_prob=True, objects=True)

@@ -11,6 +11,8 @@ import random
 import pytest
 import torch
 
+import support
+
 pytestmark = pytest.mark.gpu
 
 TOL = 1e-2                 # fp16 / bf16 vs the fp32 oracle (test_gpu_regions_packed.py)
@@ -22,46 +24,19 @@ VOCAB = {t: i for i, t in enumerate(["[PAD]", "[UNK]", "[CLS]", "[SEP]", "what",
                                      "dog", "on", "grass"])}
 
 
-def _engine(oracle, **kw):
-    import vilbert_b200 as vb
-    cfg = vb.BertConfig.from_dict(oracle.config.to_dict())
-    return vb.VILBertForVLTasks.from_pretrained(oracle.state_dict(), config=cfg, num_labels=oracle.num_labels, **kw).eval().cuda(0)
-
-
 @pytest.fixture(scope="module")
 def tiny(tiny_oracle):
-    e = {k: _engine(tiny_oracle, compute_dtype=k) for k in ("fp16", "bf16")}
-    yield e
-    for m in e.values():
-        m.close()
+    yield from support.engines(tiny_oracle, ("fp16", "bf16"))
 
 
 @pytest.fixture(scope="module")
 def tiny_long(tiny_oracle):
-    m = _engine(tiny_oracle, compute_dtype="bf16", max_rows_per_sample=1024)
-    yield m
-    m.close()
+    yield from support.one_engine(tiny_oracle, compute_dtype="bf16", max_rows_per_sample=1024)
 
 
 @pytest.fixture(scope="module")
 def full(full_oracle):
-    m = _engine(full_oracle, compute_dtype="bf16")
-    yield m
-    m.close()
-
-
-def _image(tin, n, seed, F, vocab, wh=(640, 480)):
-    """One sample: tin token ids and segments, n detector boxes, the image size, a task id."""
-    g = torch.Generator().manual_seed(seed)
-    q = torch.randint(1, vocab, (tin,), generator=g)
-    seg = torch.randint(0, 2, (tin,), generator=g)
-    f = torch.relu(torch.randn(n, F, generator=g)) * 1.5
-    w, h = wh
-    x1, y1 = torch.rand(n, generator=g) * 0.7 * w, torch.rand(n, generator=g) * 0.7 * h
-    x2 = torch.minimum(x1 + (0.05 + 0.25 * torch.rand(n, generator=g)) * w, torch.tensor(float(w)))
-    y2 = torch.minimum(y1 + (0.05 + 0.25 * torch.rand(n, generator=g)) * h, torch.tensor(float(h)))
-    task = int(torch.randint(0, 20, (1,), generator=g))
-    return q, seg, f, torch.stack([x1, y1, x2, y2], 1), torch.tensor([float(w), float(h)]), task
+    yield from support.one_engine(full_oracle, compute_dtype="bf16")
 
 
 def _batch(model, groups, seed):
@@ -72,21 +47,15 @@ def _batch(model, groups, seed):
     for gi, (tin, counts) in enumerate(groups):
         first.append(len(imgs))
         for k, n in enumerate(counts):
-            q, seg, f, bx, wh, task = _image(tin, n, seed + 31 * gi + k, F, vocab, ((640, 480), (500, 375))[k % 2])
+            q, seg, f, bx, wh, task = support.image(tin, n, seed + 31 * gi + k, F, vocab, ((640, 480), (500, 375))[k % 2])
             if k > 0:
                 q, seg, task = imgs[first[-1]][0], imgs[first[-1]][1], imgs[first[-1]][5]
             imgs.append((q, seg, f, bx, wh, task))
     return imgs, first
 
 
-def _packed_args(imgs):
-    cat = lambda k: torch.cat([im[k] for im in imgs], dim=0).cuda()
-    return (cat(0), cat(1), torch.tensor([[im[5]] for im in imgs]).cuda(), cat(2), cat(3), torch.stack([im[4] for im in imgs]).cuda(),
-            [len(im[0]) for im in imgs], [im[2].shape[0] for im in imgs])
-
-
 def _ablate(model, imgs, messages, **kw):
-    out = model.message_ablation(*_packed_args(imgs), messages, return_logits=True, mask_token=MASK, **kw)
+    out = model.message_ablation(*support.packed_image_args(imgs), messages, return_logits=True, mask_token=MASK, **kw)
     torch.cuda.synchronize()
     return out
 
@@ -115,7 +84,7 @@ def _reference(model, imgs, fam, ib, K, r):
     var = _variants(imgs, fam, ib, K, r)
     samples = [s for v, _ in var for s in v]
     sel = POOLED | (vb.OUT_VISION_LOGIT if fam == GRD else 0)
-    out, _ = model.forward_regions_packed(*_packed_args(samples), select=sel, return_spatials=False)
+    out, _ = model.forward_regions_packed(*support.packed_image_args(samples), select=sel, return_spatials=False)
     torch.cuda.synchronize()
     segs, at = [], 0
     voff = [0]
@@ -235,7 +204,7 @@ def _raw_answers(model, imgs, msgs):
     """The answer field of every box variant's score, read through the C ABI."""
     from vilbert_b200 import _lib as L
     import vilbert_b200 as vb
-    a = _packed_args(imgs)
+    a = support.packed_image_args(imgs)
     arr = (L.AblationMessage * len(msgs))(*[L.AblationMessage(m[0], m[1], m[2], -1 if m[3] is None else m[3], *m[4],
                                                                   0, int(a[7][m[1]])) for m in msgs])
     recs, n_floats, _ = model._message_layout(a[6], a[7], [tuple(getattr(x, f) for f, _ in L.AblationMessage._fields_) for x in arr])
@@ -265,7 +234,7 @@ def test_agrees_with_answer_ablation(tiny):
     model = tiny["fp16"]
     imgs, first = _batch(model, [(9, [6]), (14, [3]), (5, [1])], seed=17)
     for fam, name in ((VQA, "vqa"), (GQA, "gqa"), (SNLI, "snli_ve")):
-        old = model.answer_ablation(*_packed_args(imgs), family=name, return_logits=True, mask_token=MASK)
+        old = model.answer_ablation(*support.packed_image_args(imgs), family=name, return_logits=True, mask_token=MASK)
         new = _ablate(model, imgs, [(fam, i, 1) for i in range(3)])
         for o, n in zip(old, new):
             assert torch.equal(o["logits"], torch.stack(n["logits"]))
@@ -328,7 +297,7 @@ def test_against_the_oracle(tiny, tiny_oracle):
 def _call(model, imgs, msgs, logits, scores, mask=MASK, handle=None, n_msgs=None, inp_kw=None, bf=None):
     from vilbert_b200 import _lib as L
     import vilbert_b200 as vb
-    a = _packed_args(imgs)
+    a = support.packed_image_args(imgs)
     kw = dict(nt=a[6], nb=a[7], max_boxes=0)
     kw.update(inp_kw or {})
     arr = (L.AblationMessage * max(len(msgs), 1))(*[L.AblationMessage(*m) for m in msgs])
@@ -350,7 +319,7 @@ def test_layout_matches_the_call(tiny):
     imgs, first = _batch(model, GROUPS, seed=23)
     msgs = [(NLVR2, first[0], 2, -1, 1, 3, 5, 7), (RET, first[1], 3, 2, 0, 2, 4, 6), (GRD, first[2], 1, 0, 1, 2, 0, 2),
             (VQA, first[3], 1, -1, 0, 1, 0, 1)]
-    a = _packed_args(imgs)
+    a = support.packed_image_args(imgs)
     recs, n_floats, _ = model._message_layout(a[6], a[7], msgs)
     K = {0: 2, 1: 3, 2: 1, 3: 1}
     length = {0: 2, 1: 3, 2: 5, 3: model._dims["num_labels"]}
@@ -374,26 +343,19 @@ def test_layout_matches_the_call(tiny):
     assert not (scores[:len(recs)] == 7).all(1).any() and (scores[len(recs):] == 7).all()
 
 
-def _n_plans(model):
-    from vilbert_b200 import _lib as L
-    v = C.c_int64()
-    L.check(L.load().vb200_model_dim(model._handle, b"n_plans", C.byref(v)), model._handle)
-    return v.value
-
-
 def test_plans_are_shared_and_forwards_unchanged(tiny):
     """Repeated calls in the same bucket and capacities add no plans; forwards around a call keep their bits."""
     model = tiny["bf16"]
     imgs, first = _batch(model, GROUPS, seed=61)
-    fwd = lambda: model.forward_regions_packed(*_packed_args(imgs), max_tokens=20, max_boxes=30)[0][0].clone()
+    fwd = lambda: model.forward_regions_packed(*support.packed_image_args(imgs), max_tokens=20, max_boxes=30)[0][0].clone()
     before = fwd()
     msgs = _messages(first)
     _ablate(model, imgs, msgs, max_tokens=20, max_boxes=30)
     _ablate(model, imgs, msgs[3:5], max_tokens=20, max_boxes=30)          # pooled only
-    n = _n_plans(model)
+    n = support.n_plans(model)
     _ablate(model, imgs, msgs[::-1], max_tokens=20, max_boxes=30)
     _ablate(model, imgs, msgs[4:6], max_tokens=20, max_boxes=30)
-    assert _n_plans(model) == n
+    assert support.n_plans(model) == n
     assert torch.equal(fwd(), before)
 
 
@@ -406,7 +368,7 @@ def test_back_to_back_calls_need_no_synchronisation(tiny):
         imgs, first = _batch(model, groups, seed=s)
         msgs = [(m[0], m[1], m[2], -1 if m[3] is None else m[3]) + (m[4] or (0, 0)) + (m[5] or (0, 2)) for m in _messages(first)] \
             if s == 71 else ([(NLVR2, 0, 2, -1, 1, 14, 0, 43)] if s == 72 else [(GRD, 0, 1, -1, 1, 5, 0, 3), (RET, 1, 3, -1, 0, 9, 0, 15)])
-        a = _packed_args(imgs)
+        a = support.packed_image_args(imgs)
         recs, n_floats, arr = model._message_layout(a[6], a[7], msgs)
         inp = L.PackedRegionInputs(len(a[6]), 0, 0, vb.model._int32s(a[6]), vb.model._int32s(a[7]), *[t.data_ptr() for t in a[:6]], None)
         sets.append((inp, arr, len(msgs), n_floats, len(recs), a))
@@ -434,7 +396,7 @@ def test_rejections(tiny, tiny_oracle):
     logits = torch.full((4096,), 7.0, device="cuda")
     scores = torch.full((256, 4), 7, dtype=torch.int32, device="cuda")
     ok = [(NLVR2, 0, 2, -1, 1, 5, 0, 7), (VQA, 2, 1, -1, 0, 0, 0, 0)]
-    a = _packed_args(imgs)
+    a = support.packed_image_args(imgs)
     cases = [
         (dict(msgs=[(99, 0, 1, -1, 0, 0, 0, 0)]), "message 0 has unknown family"),
         (dict(msgs=[(NLVR2, 0, 1, -1, 0, 0, 0, 0)]), "message 0 (family 3) has n_images 1"),
@@ -468,7 +430,7 @@ def test_rejections(tiny, tiny_oracle):
     big, _ = _batch(model, [(37, [100, 100, 100])], seed=90)
     rc, msg = _call(model, big, [(RET, 0, 3, -1, 1, 36, 0, 300)] * 4, logits, scores)
     assert rc == -1 and "above 1024" in msg, msg
-    x = _engine(tiny_oracle, compute_dtype="fp32x")
+    x = support.engine(tiny_oracle, compute_dtype="fp32x")
     try:
         rc, msg = _call(x, imgs, ok, logits, scores)
         assert rc == -1 and "split_fp32" in msg

@@ -25,6 +25,8 @@ import numpy as np
 import pytest
 import torch
 
+import support
+
 pytestmark = pytest.mark.gpu
 
 TOL = 1e-2                 # north_star, default mode vs fp32 oracle
@@ -39,28 +41,14 @@ NAMES = ["vil_prediction", "vil_prediction_gqa", "vil_logit", "vil_binary_predic
 DT = {"fp16": torch.float16, "bf16": torch.bfloat16}
 
 
-def _engine(oracle, **kw):
-    import vilbert_b200 as vb
-    cfg = vb.BertConfig.from_dict(oracle.config.to_dict())
-    m = vb.VILBertForVLTasks.from_pretrained(oracle.state_dict(), config=cfg, num_labels=oracle.num_labels, **kw)
-    m.eval()
-    return m.cuda(0)
-
-
 @pytest.fixture(scope="module")
 def tiny_engines(tiny_oracle):
-    e = {k: _engine(tiny_oracle, compute_dtype=k) for k in DT}
-    yield e
-    for m in e.values():
-        m.close()
+    yield from support.engines(tiny_oracle, DT)
 
 
 @pytest.fixture(scope="module")
 def full_engines(full_oracle):
-    e = {k: _engine(full_oracle, compute_dtype=k) for k in DT}
-    yield e
-    for m in e.values():
-        m.close()
+    yield from support.engines(full_oracle, DT)
 
 
 def _errs(ref, out):
@@ -100,13 +88,6 @@ def _check(oracle, engines, inputs, parity_log, tag, pretraining):
             assert e32[name][0] < tol32, f"{tag}/{mode}: {name} vs fp32 oracle: {e32[name][0]} >= {tol32}"
 
 
-def _tiny_inputs(oracle, B, Tin, V, seed, pad=0):
-    from oracle import vilbert_ref as R
-    inp = list(R.make_inputs(B, Tin, V, seed=seed, vocab_size=oracle.config.vocab_size, pad_regions=pad))
-    inp[1] = inp[1][..., :oracle.config.v_feature_size].contiguous()
-    return inp
-
-
 @pytest.mark.parametrize("B,Tin,V,pad", [(2, 30, 36, 0), (3, 16, 10, 3), (4, 37, 101, 7), (1, 12, 37, 0), (2, 128, 100, 0),
                                          (1, 3, 1, 0), (1, 155, 256, 11), (5, 3, 7, 2)])
 def test_tiny_model_all_outputs(tiny_oracle, tiny_engines, parity_log, B, Tin, V, pad):
@@ -114,14 +95,14 @@ def test_tiny_model_all_outputs(tiny_oracle, tiny_engines, parity_log, B, Tin, V
     lengths, masked regions, odd batch (binary head falls back to the seq-relationship score), and the corner of the
     BASELINE sweep (text 128, regions 100); extremes: three tokens ([CLS] id [SEP]) + one region, 155 tokens (the tiny model has 160 positions)
     x 256 regions (four key blocks in every attention kernel), an odd batch of tiny sequences."""
-    _check(tiny_oracle, tiny_engines, _tiny_inputs(tiny_oracle, B, Tin, V, 100 + B, pad), parity_log,
+    _check(tiny_oracle, tiny_engines, support.tiny_inputs(tiny_oracle, B, Tin, V, 100 + B, pad), parity_log,
            f"tiny_B{B}_T{Tin}_V{V}", pretraining=True)
 
 
 def test_tiny_model_eager_equals_graph(tiny_oracle, tiny_engines):
     """CUDA-graph replay and eager launches of the same plan give bit-identical outputs."""
-    dev = [t.cuda() for t in _tiny_inputs(tiny_oracle, 2, 20, 12, 5)]
-    eager = _engine(tiny_oracle, use_cuda_graph=False)
+    dev = [t.cuda() for t in support.tiny_inputs(tiny_oracle, 2, 20, 12, 5)]
+    eager = support.engine(tiny_oracle, use_cuda_graph=False)
     a = tiny_engines["fp16"](*dev)
     b = eager(*dev)
     c = tiny_engines["fp16"](*dev)
@@ -135,10 +116,10 @@ def test_tiny_model_eager_equals_graph(tiny_oracle, tiny_engines):
 def test_tiny_model_pdl(tiny_oracle, tiny_engines):
     """Programmatic dependent launch changes scheduling only, never results: the default (every kernel), forced on
     (use_pdl=True) and none (use_pdl=False) agree bit for bit."""
-    dev = [t.cuda() for t in _tiny_inputs(tiny_oracle, 2, 20, 12, 6)]
+    dev = [t.cuda() for t in support.tiny_inputs(tiny_oracle, 2, 20, 12, 6)]
     a = tiny_engines["fp16"](*dev, compute_pretraining_heads=True)
     for mode in (True, False):
-        other = _engine(tiny_oracle, use_pdl=mode)
+        other = support.engine(tiny_oracle, use_pdl=mode)
         for rep in range(3):
             b = other(*dev, compute_pretraining_heads=True)
             torch.cuda.synchronize()
@@ -151,7 +132,7 @@ def test_tiny_model_pdl(tiny_oracle, tiny_engines):
 def test_tiny_model_host_api(tiny_oracle, tiny_engines):
     """vb200_forward_host (pinned host buffers in/out) == vb200_forward (device pointers)."""
     from vilbert_b200 import _lib as L
-    inp = _tiny_inputs(tiny_oracle, 4, 20, 12, 8)
+    inp = support.tiny_inputs(tiny_oracle, 4, 20, 12, 8)
     eng = tiny_engines["fp16"]
     ref = eng(*[t.cuda() for t in inp])
     hin = [t.pin_memory() for i, t in enumerate(inp) if i != 6]
@@ -166,7 +147,7 @@ def test_tiny_model_workspace_slots(tiny_oracle, tiny_engines):
     other -- every slot returns bit-for-bit what slot 0 returns for the same batch."""
     from vilbert_b200 import _lib as L
     eng = tiny_engines["fp16"]
-    batches = [_tiny_inputs(tiny_oracle, 3, 20, 12, 40 + i, pad=i % 2) for i in range(6)]
+    batches = [support.tiny_inputs(tiny_oracle, 3, 20, 12, 40 + i, pad=i % 2) for i in range(6)]
     want = []
     for b in batches:
         want.append(eng(*[t.cuda() for t in b])[0].clone())
@@ -273,7 +254,7 @@ def test_checkpoint_file_ingestion(tiny_oracle, tiny_engines, tmp_path):
     m = vb.VILBertForVLTasks.from_pretrained(str(ckpt), config=config, num_labels=tiny_oracle.num_labels, default_gpu=True)
     m.eval()
     m.cuda(0)
-    dev = [t.cuda() for t in _tiny_inputs(tiny_oracle, 3, 20, 12, 77, pad=1)]
+    dev = [t.cuda() for t in support.tiny_inputs(tiny_oracle, 3, 20, 12, 77, pad=1)]
     a = tiny_engines["fp16"](*dev, compute_pretraining_heads=True)
     b = m(*dev, compute_pretraining_heads=True)
     torch.cuda.synchronize()

@@ -6,12 +6,9 @@ import math
 import pytest
 import torch
 
+import support
+
 pytestmark = pytest.mark.gpu
-
-
-def _lib():
-    from vilbert_b200 import _lib as L
-    return L, L.load()
 
 
 def _ptr(t):
@@ -31,7 +28,8 @@ def variant(request):
 
 def run_linear(x, w, bias=None, act=0, block_n=0, want_bf16=True, want_f32=True, ld_f32=None, pdl=0):
     """x, w: both fp16 or both bf16 (wgmma needs matching operand formats); same format for the 16-bit output."""
-    L, lib = _lib()
+    L = support.lib()
+    lib = L.load()
     M, K = x.shape
     N = w.shape[0]
     dev = x.device
@@ -135,7 +133,8 @@ def _attn_ref(q, k, v, mask_add, heads):
 @pytest.mark.parametrize("B,L,heads,d", [(3, 31, 12, 64), (2, 38, 12, 64), (2, 36, 8, 128), (2, 101, 8, 128),
                                          (1, 129, 2, 64), (2, 17, 2, 128), (1, 256, 2, 128), (2, 1, 2, 64), (1, 2, 1, 128)])
 def test_self_attention(B, L, heads, d, act_dt, parity_log):
-    Lm, lib = _lib()
+    Lm = support.lib()
+    lib = Lm.load()
     H = heads * d
     g = torch.Generator(device="cuda").manual_seed(5)
     qkv = torch.randn(B * L, 3 * H, generator=g, device="cuda").to(act_dt)
@@ -158,7 +157,8 @@ def test_self_attention(B, L, heads, d, act_dt, parity_log):
 @pytest.mark.parametrize("B,T,V,heads,d", [(3, 31, 36, 8, 128), (2, 38, 101, 8, 128), (2, 17, 10, 2, 128),
                                            (1, 129, 100, 8, 128), (1, 256, 256, 2, 128), (2, 2, 1, 2, 128), (1, 1, 200, 1, 64)])
 def test_co_attention(B, T, V, heads, d, act_dt, parity_log):
-    Lm, lib = _lib()
+    Lm = support.lib()
+    lib = Lm.load()
     H = heads * d
     g = torch.Generator(device="cuda").manual_seed(6)
     qkv_i = torch.randn(B * V, 3 * H, generator=g, device="cuda").to(act_dt)
@@ -187,7 +187,8 @@ def test_co_attention(B, T, V, heads, d, act_dt, parity_log):
 @pytest.mark.parametrize("M,N,with_res", [(1984, 768, True), (2304, 1024, True), (64, 2048, False), (37, 128, True), (5, 256, False)])
 def test_layernorm_row_kernel(M, N, with_res, act_dt, parity_log):
     """vb200_layernorm: LayerNorm(y + residual) with fp32 and 16-bit outputs (the LayerNorm after every residual GEMM)."""
-    L, lib = _lib()
+    L = support.lib()
+    lib = L.load()
     g = torch.Generator(device="cuda").manual_seed(9)
     y = torch.randn(M, N, generator=g, device="cuda") * 3 + 0.5
     res = torch.randn(M, N, generator=g, device="cuda") if with_res else None
@@ -263,7 +264,8 @@ def _unsplit(y3):
                                         (77, 64, 128, 0)])
 def test_linear_split_operands(M, N, K, act, parity_log):
     """fp32-parity mode GEMM: fp16 hi/lo split operands, K' = 3K; against fp64 math on the ORIGINAL fp32 operands."""
-    L, lib = _lib()
+    L = support.lib()
+    lib = L.load()
     g = torch.Generator(device="cuda").manual_seed(5)
     x = torch.randn(M, K, generator=g, device="cuda") * 1.7
     w = torch.randn(N, K, generator=g, device="cuda") / math.sqrt(K)
@@ -284,7 +286,8 @@ def test_linear_split_operands(M, N, K, act, parity_log):
 
 
 def test_layernorm_split_output(parity_log):
-    L, lib = _lib()
+    L = support.lib()
+    lib = L.load()
     g = torch.Generator(device="cuda").manual_seed(6)
     M, N = 333, 768
     y, r = torch.randn(M, N, generator=g, device="cuda"), torch.randn(M, N, generator=g, device="cuda")
@@ -306,7 +309,8 @@ def test_layernorm_split_output(parity_log):
                                              (2, 5, 200, 3, 64)])
 def test_attention_f32(B, Lq, Lk, heads, d, in_kind, parity_log):
     """fp32 CUDA-core attention: context in every output format + the probability output, against fp64 torch math."""
-    L, lib = _lib()
+    L = support.lib()
+    lib = L.load()
     g = torch.Generator(device="cuda").manual_seed(7)
     hid = heads * d
     dt = [torch.float32, torch.float16, torch.bfloat16][in_kind]

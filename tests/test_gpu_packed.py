@@ -8,9 +8,10 @@ batch at the tolerances of test_gpu_model.py.
 """
 import ctypes as C
 
-import numpy as np
 import pytest
 import torch
+
+import support
 
 pytestmark = pytest.mark.gpu
 
@@ -20,66 +21,20 @@ DT = ("fp16", "bf16")
 ROW_OUT = {5: "regions", 6: "regions", 7: "tokens", 8: "tokens"}    # per-row outputs of the 10-tuple
 
 
-def _engine(oracle, **kw):
-    import vilbert_b200 as vb
-    cfg = vb.BertConfig.from_dict(oracle.config.to_dict())
-    return vb.VILBertForVLTasks.from_pretrained(oracle.state_dict(), config=cfg, num_labels=oracle.num_labels, **kw).eval().cuda(0)
-
-
 @pytest.fixture(scope="module")
 def tiny(tiny_oracle):
-    e = {k: _engine(tiny_oracle, compute_dtype=k) for k in DT}
-    yield e
-    for m in e.values():
-        m.close()
+    yield from support.engines(tiny_oracle, DT)
 
 
 @pytest.fixture(scope="module")
 def full(full_oracle):
-    m = _engine(full_oracle)
-    yield m
-    m.close()
-
-
-def _sample(tin, v, seed, F, vocab):
-    """One request's real rows: tin token ids, v regions (relu features, boxes in [0, 1], global box first)."""
-    g = torch.Generator().manual_seed(seed)
-    q = torch.randint(1, vocab, (tin,), generator=g)
-    f = torch.relu(torch.randn(v, F, generator=g)) * 1.5
-    x1, y1 = torch.rand(v, generator=g) * 0.7, torch.rand(v, generator=g) * 0.7
-    x2, y2 = x1 + 0.05 + torch.rand(v, generator=g) * 0.25, y1 + 0.05 + torch.rand(v, generator=g) * 0.25
-    s = torch.stack([x1, y1, x2.clamp(max=1.0), y2.clamp(max=1.0), (x2 - x1) * (y2 - y1)], dim=-1)
-    s[0] = torch.tensor([0.0, 0.0, 1.0, 1.0, 1.0])
-    seg = torch.randint(0, 2, (tin,), generator=g)
-    task = int(torch.randint(0, 20, (1,), generator=g))
-    return q, seg, f, s, task
-
-
-def _batch(model, lens, seed):
-    F, vocab = model._dims["v_feature_size"], model._dims["vocab_size"]
-    return [_sample(t, v, seed + i, F, vocab) for i, (t, v) in enumerate(lens)]
+    yield from support.one_engine(full_oracle)
 
 
 def _packed(model, samples, select, **kw):
-    cat = lambda k: torch.cat([s[k] for s in samples], dim=0).cuda()
-    task = torch.tensor([[s[4]] for s in samples]).cuda()
-    out = model.forward_packed(cat(0), cat(2), cat(3), cat(1), task, [len(s[0]) for s in samples], [s[2].shape[0] for s in samples],
-                               select=select, debug_taps=True, **kw)
+    out = model.forward_packed(*support.packed_sample_args(samples), select=select, debug_taps=True, **kw)
     torch.cuda.synchronize()
     return out
-
-
-def _dense_alone(model, smp, select):
-    q, seg, f, s, task = smp
-    out = model(q[None].cuda(), f[None].cuda(), s[None].cuda(), seg[None].cuda(), torch.ones(1, len(q), dtype=torch.long).cuda(),
-                torch.ones(1, f.shape[0], dtype=torch.uint8).cuda(), None, torch.tensor([[task]]).cuda(), select=select, debug_taps=True)
-    torch.cuda.synchronize()
-    return out
-
-
-def _split_rows(t, counts):
-    offs = np.concatenate([[0], np.cumsum(counts)])
-    return [t[offs[i]:offs[i + 1]] for i in range(len(counts))]
 
 
 def _check_bitwise(model, samples, packed):
@@ -89,10 +44,10 @@ def _check_bitwise(model, samples, packed):
     t_rows = [len(s[0]) + 1 for s in samples]
     v_rows = [s[2].shape[0] for s in samples]
     for i, smp in enumerate(samples):
-        ref, rtaps = _dense_alone(model, smp, vb.OUT_ALL)
+        ref, rtaps = support.dense_alone(model, smp, select=vb.OUT_ALL, debug_taps=True)
         for k in range(9):
             if k in ROW_OUT:
-                got = _split_rows(out[k], v_rows if ROW_OUT[k] == "regions" else t_rows)[i]
+                got = support.split_rows(out[k], v_rows if ROW_OUT[k] == "regions" else t_rows)[i]
                 want = ref[k][0]
             elif k == 3:
                 if B % 2 == 0:
@@ -101,8 +56,8 @@ def _check_bitwise(model, samples, packed):
             else:
                 got, want = out[k][i], ref[k][0]
             assert torch.equal(got, want), f"sample {i}: output {k} differs from the sample's own dense forward"
-        assert torch.equal(_split_rows(taps["sequence_output_t"], t_rows)[i], rtaps["sequence_output_t"][0]), f"sample {i}: text tap"
-        assert torch.equal(_split_rows(taps["sequence_output_v"], v_rows)[i], rtaps["sequence_output_v"][0]), f"sample {i}: image tap"
+        assert torch.equal(support.split_rows(taps["sequence_output_t"], t_rows)[i], rtaps["sequence_output_t"][0]), f"sample {i}: text tap"
+        assert torch.equal(support.split_rows(taps["sequence_output_v"], v_rows)[i], rtaps["sequence_output_v"][0]), f"sample {i}: image tap"
         assert torch.equal(taps["pooled_output"][i], rtaps["pooled_output"][0]), f"sample {i}: pooled tap"
 
 
@@ -116,7 +71,7 @@ def test_packed_bitwise_equals_dense_per_sample(tiny, mode, B):
     taps of every sample equal the dense forward of that sample alone, bit for bit."""
     import vilbert_b200 as vb
     model = tiny[mode]
-    samples = _batch(model, CORNERS[:B], seed=40 + B)
+    samples = support.batch(model, CORNERS[:B], seed=40 + B)
     _check_bitwise(model, samples, _packed(model, samples, vb.OUT_ALL))
 
 
@@ -124,7 +79,7 @@ def test_packed_bitwise_full_model(full):
     """The 268 M model with an 8-sample mix of worker-like lengths (VQA head plus the per-row heads)."""
     import vilbert_b200 as vb
     lens = [(9, 37), (30, 101), (14, 11), (37, 64), (7, 100), (22, 18), (5, 2), (28, 73)]
-    samples = _batch(full, lens, seed=7)
+    samples = support.batch(full, lens, seed=7)
     _check_bitwise(full, samples, _packed(full, samples, vb.OUT_ALL))
 
 
@@ -135,7 +90,7 @@ def test_packed_matches_oracle_on_padded_batch(tiny_oracle, tiny, mode):
     import vilbert_b200 as vb
     model = tiny[mode]
     lens = [(5, 36), (30, 10), (12, 101), (1, 1), (37, 7), (20, 64)]
-    samples = _batch(model, lens, seed=3)
+    samples = support.batch(model, lens, seed=3)
     out, _ = _packed(model, samples, vb.OUT_ALL)
     B, Tm, Vm = len(samples), max(t for t, _ in lens), max(v for _, v in lens)
     F = model._dims["v_feature_size"]
@@ -157,33 +112,26 @@ def test_packed_matches_oracle_on_padded_batch(tiny_oracle, tiny, mode):
         assert err < tol, f"{mode}: output {k} vs fp32 oracle: {err} >= {tol}"
 
 
-def _n_plans(model):
-    from vilbert_b200 import _lib as L
-    v = C.c_int64()
-    L.check(L.load().vb200_model_dim(model._handle, b"n_plans", C.byref(v)), model._handle)
-    return v.value
-
-
 def test_packed_plan_reuse_and_capacity(tiny):
     """Lengths in one 16-row bucket share a plan; fixed capacities share one plan across quite different maxima, and capacity
     changes no bit."""
     import vilbert_b200 as vb
     model = tiny["fp16"]
     sel = vb.OUT_TASK_HEADS
-    a = _batch(model, [(20, 40), (3, 33), (25, 12), (8, 47)], seed=11)       # maxima T = 26, V = 47 -> bucket (32, 48)
-    b = _batch(model, [(30, 35), (30, 48), (2, 5), (17, 20)], seed=12)       # maxima T = 31, V = 48 -> the same bucket
+    a = support.batch(model, [(20, 40), (3, 33), (25, 12), (8, 47)], seed=11)       # maxima T = 26, V = 47 -> bucket (32, 48)
+    b = support.batch(model, [(30, 35), (30, 48), (2, 5), (17, 20)], seed=12)       # maxima T = 31, V = 48 -> the same bucket
     _packed(model, a, sel)
-    n = _n_plans(model)
+    n = support.n_plans(model)
     _packed(model, b, sel)
-    assert _n_plans(model) == n
+    assert support.n_plans(model) == n
     cap = dict(max_tokens=37, max_regions=101)
-    small = _batch(model, [(2, 3), (5, 1), (4, 9), (1, 2)], seed=13)
-    large = _batch(model, [(37, 101), (12, 60), (30, 7), (36, 100)], seed=14)
+    small = support.batch(model, [(2, 3), (5, 1), (4, 9), (1, 2)], seed=13)
+    large = support.batch(model, [(37, 101), (12, 60), (30, 7), (36, 100)], seed=14)
     ref_small, ref_large = _packed(model, small, sel), _packed(model, large, sel)
     got_small = _packed(model, small, sel, **cap)
-    n = _n_plans(model)
+    n = support.n_plans(model)
     got_large = _packed(model, large, sel, **cap)
-    assert _n_plans(model) == n
+    assert support.n_plans(model) == n
     for got, ref in ((got_small, ref_small), (got_large, ref_large)):
         for k in range(9):
             assert (got[0][k] is None) == (ref[0][k] is None)
@@ -197,17 +145,17 @@ def test_packed_rejections(tiny_oracle, tiny):
     import vilbert_b200 as vb
     from vilbert_b200 import _lib as L
     model = tiny["fp16"]
-    ok = _batch(model, [(5, 3), (4, 2)], seed=21)
+    ok = support.batch(model, [(5, 3), (4, 2)], seed=21)
     with pytest.raises(L.VilbertB200Error, match=r"error -1: .*VB200_OUT_ATTENTION"):
         _packed(model, ok, L.OUT_TASK_HEADS | L.OUT_ATTENTION)
     with pytest.raises(L.VilbertB200Error, match=r"error -1: .*n_tokens 0"):
         model.forward_packed(torch.zeros(4, dtype=torch.long).cuda(), torch.zeros(5, model._dims["v_feature_size"]).cuda(),
                              torch.zeros(5, 5).cuda(), None, torch.zeros(2, 1, dtype=torch.long).cuda(), [0, 4], [3, 2])
     with pytest.raises(L.VilbertB200Error, match=r"error -1: .*T=257"):
-        _packed(model, _batch(model, [(256, 3)], seed=22), vb.OUT_TASK_HEADS)
+        _packed(model, support.batch(model, [(256, 3)], seed=22), vb.OUT_TASK_HEADS)
     with pytest.raises(L.VilbertB200Error, match=r"error -1: .*capacity"):
         _packed(model, ok, vb.OUT_TASK_HEADS, max_tokens=4)
-    x = _engine(tiny_oracle, compute_dtype="fp32x")
+    x = support.engine(tiny_oracle, compute_dtype="fp32x")
     try:
         with pytest.raises(L.VilbertB200Error, match=r"error -1: .*fp32x"):
             _packed(x, ok, vb.OUT_TASK_HEADS)

@@ -10,74 +10,30 @@ import ctypes as C
 import pytest
 import torch
 
+import support
+
 pytestmark = pytest.mark.gpu
 
 DT = ("fp16", "bf16")
 TOL_ATTN = 5e-3            # engine (fp16) vs the fp32 oracle's attention probabilities (test_gpu_round2.py)
 
 
-def _engine(oracle, **kw):
-    import vilbert_b200 as vb
-    cfg = vb.BertConfig.from_dict(oracle.config.to_dict())
-    return vb.VILBertForVLTasks.from_pretrained(oracle.state_dict(), config=cfg, num_labels=oracle.num_labels, return_attention=True,
-                                                **kw).eval().cuda(0)
-
-
 @pytest.fixture(scope="module")
 def tiny(tiny_oracle):
-    e = {k: _engine(tiny_oracle, compute_dtype=k) for k in DT}
-    yield e
-    for m in e.values():
-        m.close()
+    yield from support.engines(tiny_oracle, DT, return_attention=True)
 
 
 @pytest.fixture(scope="module")
 def full(full_oracle):
-    m = _engine(full_oracle)
-    yield m
-    m.close()
-
-
-def _sample(tin, v, seed, F, vocab):
-    """One request's real rows: tin token ids, v regions (relu features, boxes in [0, 1], global box first)."""
-    g = torch.Generator().manual_seed(seed)
-    q = torch.randint(1, vocab, (tin,), generator=g)
-    f = torch.relu(torch.randn(v, F, generator=g)) * 1.5
-    x1, y1 = torch.rand(v, generator=g) * 0.7, torch.rand(v, generator=g) * 0.7
-    x2, y2 = x1 + 0.05 + torch.rand(v, generator=g) * 0.25, y1 + 0.05 + torch.rand(v, generator=g) * 0.25
-    s = torch.stack([x1, y1, x2.clamp(max=1.0), y2.clamp(max=1.0), (x2 - x1) * (y2 - y1)], dim=-1)
-    s[0] = torch.tensor([0.0, 0.0, 1.0, 1.0, 1.0])
-    seg = torch.randint(0, 2, (tin,), generator=g)
-    task = int(torch.randint(0, 20, (1,), generator=g))
-    return q, seg, f, s, task
-
-
-def _batch(model, lens, seed):
-    F, vocab = model._dims["v_feature_size"], model._dims["vocab_size"]
-    return [_sample(t, v, seed + i, F, vocab) for i, (t, v) in enumerate(lens)]
-
-
-def _dev_args(samples):
-    """forward_packed's positional arguments, on the device."""
-    cat = lambda k: torch.cat([s[k] for s in samples], dim=0).cuda()
-    task = torch.tensor([[s[4]] for s in samples]).cuda()
-    return cat(0), cat(2), cat(3), cat(1), task, [len(s[0]) for s in samples], [s[2].shape[0] for s in samples]
+    yield from support.one_engine(full_oracle, return_attention=True)
 
 
 def _packed(model, samples, select=None, maps=True, **kw):
     import vilbert_b200 as vb
-    out = model.forward_packed(*_dev_args(samples), select=vb.OUT_TASK_HEADS if select is None else select, debug_taps=True,
+    out = model.forward_packed(*support.packed_sample_args(samples), select=vb.OUT_TASK_HEADS if select is None else select, debug_taps=True,
                                output_all_attention_masks=maps, **kw)
     torch.cuda.synchronize()
     return out
-
-
-def _dense_alone(model, smp):
-    q, seg, f, s, task = smp
-    out = model(q[None].cuda(), f[None].cuda(), s[None].cuda(), seg[None].cuda(), torch.ones(1, len(q), dtype=torch.long).cuda(),
-                torch.ones(1, f.shape[0], dtype=torch.uint8).cuda(), None, torch.tensor([[task]]).cuda(), output_all_attention_masks=True)
-    torch.cuda.synchronize()
-    return out[9]
 
 
 def _check_maps_bitwise(attn, refs):
@@ -104,31 +60,15 @@ CORNERS = [(1, 256), (31, 1), (32, 33), (63, 31), (64, 65), (12, 64), (1, 1)]
 @pytest.mark.parametrize("B", [1, 7, 6])
 def test_packed_maps_bitwise_equal_dense_per_sample(tiny, mode, B):
     model = tiny[mode]
-    samples = _batch(model, CORNERS[:B], seed=80 + B)
+    samples = support.batch(model, CORNERS[:B], seed=80 + B)
     (out, _) = _packed(model, samples)
-    _check_maps_bitwise(out[9], [_dense_alone(model, s) for s in samples])
+    _check_maps_bitwise(out[9], [support.dense_alone(model, s, output_all_attention_masks=True)[9] for s in samples])
 
 
 # ------------------------------------------------------------------------------------------------ detector output
-def _image(tin, n, seed, F, vocab, wh=(640, 480)):
-    g = torch.Generator().manual_seed(seed)
-    q = torch.randint(1, vocab, (tin,), generator=g)
-    seg = torch.randint(0, 2, (tin,), generator=g)
-    f = torch.relu(torch.randn(n, F, generator=g)) * 1.5
-    w, h = wh
-    x1, y1 = torch.rand(n, generator=g) * 0.7 * w, torch.rand(n, generator=g) * 0.7 * h
-    x2 = torch.minimum(x1 + (0.05 + 0.25 * torch.rand(n, generator=g)) * w, torch.tensor(float(w)))
-    y2 = torch.minimum(y1 + (0.05 + 0.25 * torch.rand(n, generator=g)) * h, torch.tensor(float(h)))
-    task = int(torch.randint(0, 20, (1,), generator=g))
-    return q, seg, f, torch.stack([x1, y1, x2, y2], 1), torch.tensor([float(w), float(h)]), task
-
-
 def _regions_packed(model, imgs, maps=True, **kw):
     import vilbert_b200 as vb
-    cat = lambda k: torch.cat([im[k] for im in imgs], dim=0).cuda()
-    (out, sp) = model.forward_regions_packed(cat(0), cat(1), torch.tensor([[im[5]] for im in imgs]).cuda(), cat(2), cat(3),
-                                             torch.stack([im[4] for im in imgs]).cuda(), [len(im[0]) for im in imgs],
-                                             [im[2].shape[0] for im in imgs], select=vb.OUT_TASK_HEADS, output_all_attention_masks=maps,
+    (out, sp) = model.forward_regions_packed(*support.packed_image_args(imgs), select=vb.OUT_TASK_HEADS, output_all_attention_masks=maps,
                                              **kw)
     torch.cuda.synchronize()
     return out
@@ -152,7 +92,7 @@ REGION_CORNERS = [(1, 255), (31, 1), (32, 31), (63, 32), (64, 63), (5, 64), (2, 
 def test_regions_packed_maps_bitwise_equal_regions_per_image(tiny, mode, B):
     model = tiny[mode]
     F, vocab = model._dims["v_feature_size"], model._dims["vocab_size"]
-    imgs = [_image(t, n, 90 + B + i, F, vocab) for i, (t, n) in enumerate(REGION_CORNERS[:B])]
+    imgs = [support.image(t, n, 90 + B + i, F, vocab) for i, (t, n) in enumerate(REGION_CORNERS[:B])]
     out = _regions_packed(model, imgs)
     _check_maps_bitwise(out[9], [_regions_alone(model, im) for im in imgs])
 
@@ -160,9 +100,9 @@ def test_regions_packed_maps_bitwise_equal_regions_per_image(tiny, mode, B):
 # ------------------------------------------------------------------------------------------------ full model, oracle
 def test_full_model_maps_bitwise_and_oracle(full_oracle, full):
     lens = [(9, 37), (30, 101), (14, 11), (37, 64), (5, 2), (22, 18)]
-    samples = _batch(full, lens, seed=17)
+    samples = support.batch(full, lens, seed=17)
     (out, _) = _packed(full, samples)
-    _check_maps_bitwise(out[9], [_dense_alone(full, s) for s in samples])
+    _check_maps_bitwise(out[9], [support.dense_alone(full, s, output_all_attention_masks=True)[9] for s in samples])
     B, Tm, Vm = len(samples), max(t for t, _ in lens), max(v for _, v in lens)
     F = full._dims["v_feature_size"]
     q, seg, im = (torch.zeros(B, Tm, dtype=torch.long) for _ in range(3))
@@ -192,7 +132,7 @@ def test_full_model_maps_bitwise_and_oracle(full_oracle, full):
 def test_maps_change_no_other_output(tiny, mode):
     import vilbert_b200 as vb
     model = tiny[mode]
-    samples = _batch(model, [(5, 36), (30, 10), (12, 101), (1, 1), (37, 7)], seed=3)
+    samples = support.batch(model, [(5, 36), (30, 10), (12, 101), (1, 1), (37, 7)], seed=3)
     (a, ta) = _packed(model, samples, select=vb.OUT_ALL, maps=True)
     (b, tb) = _packed(model, samples, select=vb.OUT_ALL, maps=False)
     assert b[9] == [] and len(a[9]) > 0
@@ -207,13 +147,6 @@ def test_maps_change_no_other_output(tiny, mode):
         assert _packed(model, samples, maps=True)[0][9] == []
     finally:
         model.return_attention = True
-
-
-def _n_plans(model):
-    from vilbert_b200 import _lib as L
-    v = C.c_int64()
-    L.check(L.load().vb200_model_dim(model._handle, b"n_plans", C.byref(v)), model._handle)
-    return v.value
 
 
 def _call_c(model, samples, buf, select, max_tokens=0, max_regions=0):
@@ -240,7 +173,7 @@ def test_layout_total_and_untouched_tail(tiny):
     from vilbert_b200 import _lib as L
     model = tiny["fp16"]
     lens = [(3, 40), (20, 1), (1, 70), (33, 9)]
-    samples = _batch(model, lens, seed=23)
+    samples = support.batch(model, lens, seed=23)
     layout, total = model.attention_layout_packed([t for t, _ in lens], [v for _, v in lens])
     T, V = [t + 1 for t, _ in lens], [v for _, v in lens]
     sums = {0: sum(t * t for t in T), 1: sum(v * v for v in V), 2: sum(t * v for t, v in zip(T, V)), 3: sum(t * v for t, v in zip(T, V))}
@@ -271,15 +204,15 @@ def _check_maps_equal(a, b):
 def test_plans_shared_across_lengths(tiny):
     model = tiny["bf16"]
     cap = dict(max_tokens=40, max_regions=120)
-    a = _batch(model, [(5, 36), (30, 10), (12, 101), (1, 1)], seed=41)
-    b = _batch(model, [(40, 120), (2, 3), (7, 64), (19, 33)], seed=42)
+    a = support.batch(model, [(5, 36), (30, 10), (12, 101), (1, 1)], seed=41)
+    b = support.batch(model, [(40, 120), (2, 3), (7, 64), (19, 33)], seed=42)
     _packed(model, a, maps=False, **cap)
-    n = _n_plans(model)
+    n = support.n_plans(model)
     _packed(model, a, maps=True, **cap)
-    assert _n_plans(model) == n + 1, "the first call with maps adds exactly one plan"
+    assert support.n_plans(model) == n + 1, "the first call with maps adds exactly one plan"
     _packed(model, b, maps=True, **cap)
     _packed(model, b, maps=False, **cap)
-    assert _n_plans(model) == n + 1, "calls at the same capacities share the plans whatever the lengths"
+    assert support.n_plans(model) == n + 1, "calls at the same capacities share the plans whatever the lengths"
 
 
 def test_back_to_back_calls_stage_their_own_destination(tiny):
@@ -287,10 +220,10 @@ def test_back_to_back_calls_stage_their_own_destination(tiny):
     travels with each call's staged meta, so both get their own maps."""
     model = tiny["fp16"]
     cap = dict(max_tokens=40, max_regions=120)
-    a = _batch(model, [(5, 36), (30, 10), (12, 101), (1, 1)], seed=51)
-    b = _batch(model, [(40, 120), (2, 3), (7, 64), (19, 33)], seed=52)
+    a = support.batch(model, [(5, 36), (30, 10), (12, 101), (1, 1)], seed=51)
+    b = support.batch(model, [(40, 120), (2, 3), (7, 64), (19, 33)], seed=52)
     want_a, want_b = _packed(model, a, **cap)[0][9], _packed(model, b, **cap)[0][9]
-    args_a, args_b = _dev_args(a), _dev_args(b)          # inputs on the device first: nothing below synchronises
+    args_a, args_b = support.packed_sample_args(a), support.packed_sample_args(b)      # inputs on the device first: nothing below synchronises
     torch.cuda.synchronize()
     got_a = model.forward_packed(*args_a, output_all_attention_masks=True, **cap)[9]
     got_b = model.forward_packed(*args_b, output_all_attention_masks=True, **cap)[9]
@@ -306,13 +239,13 @@ def test_rejections(tiny_oracle, tiny):
     model = tiny["fp16"]
     err = lambda pat: pytest.raises(L.VilbertB200Error, match=r"error -1: .*" + pat)
     lib = L.load()
-    ok = _batch(model, [(5, 3), (4, 2)], seed=61)
+    ok = support.batch(model, [(5, 3), (4, 2)], seed=61)
     sel = L.OUT_VIL_PREDICTION | L.OUT_ATTENTION_PACKED
     # the bit without a destination
     assert _call_c(model, ok, None, sel) == -1
     assert b"attention_probs" in lib.vb200_last_error(model._handle)
     F, vocab = model._dims["v_feature_size"], model._dims["vocab_size"]
-    im = _image(5, 3, 62, F, vocab)
+    im = support.image(5, 3, 62, F, vocab)
     nt, nb = (C.c_int32 * 1)(5), (C.c_int32 * 1)(3)
     dev = [t.cuda().contiguous() for t in (im[0], im[1], torch.tensor([[im[5]]]), im[2], im[3], im[4][None])]
     inp = L.PackedRegionInputs(1, 0, 0, C.cast(nt, C.c_void_p), C.cast(nb, C.c_void_p), *[t.data_ptr() for t in dev], None)
@@ -350,7 +283,7 @@ def test_rejections(tiny_oracle, tiny):
     with err("T=257"):
         model.attention_layout_packed([256], [4])
     # fp32x engines keep rejecting packed calls
-    x = _engine(tiny_oracle, compute_dtype="fp32x")
+    x = support.engine(tiny_oracle, compute_dtype="fp32x", return_attention=True)
     try:
         with err("fp32x"):
             _packed(x, ok)

@@ -7,12 +7,15 @@ and row by row, bit for bit, against vb200_pretraining_heads on the same taps; t
 against dense forwards of each sample alone.  The objectives are checked against fp64 torch on the engine's own logits and against the
 oracle's losses.
 """
+import contextlib
 import ctypes as C
 import math
 
 import pytest
 import torch
 import torch.nn.functional as F
+
+import support
 
 pytestmark = pytest.mark.gpu
 
@@ -23,20 +26,9 @@ KEYS = ("input_ids", "image_feat", "image_loc", "token_type_ids", "attention_mas
 LABELS = ("masked_lm_labels", "image_label", "image_target", "next_sentence_label")
 
 
-def _lib():
-    from vilbert_b200 import _lib as L
-    return L
-
-
 def _both():
-    L = _lib()
+    L = support.lib()
     return L.OUT_LINGUISIC_PREDICTION | L.OUT_VISION_PREDICTION
-
-
-def _engine(oracle, **kw):
-    import vilbert_b200 as vb
-    cfg = vb.BertConfig.from_dict(oracle.config.to_dict())
-    return vb.BertForMultiModalPreTraining.from_pretrained(oracle.state_dict(), config=cfg, **kw).eval().cuda(0)
 
 
 @pytest.fixture(scope="module")
@@ -47,19 +39,17 @@ def pt_oracle():
 
 @pytest.fixture(scope="module")
 def tiny(pt_oracle):
-    e = {k: _engine(pt_oracle, compute_dtype=k) for k in MODES}
-    yield e
-    for m in e.values():
-        m.close()
+    import vilbert_b200 as vb
+    yield from support.engines(pt_oracle, MODES, vb.BertForMultiModalPreTraining)
 
 
 @pytest.fixture(scope="module")
 def full_pt():
     from oracle import pretraining_ref as P
+    import vilbert_b200 as vb
     oracle = P.build(seed=42)
-    m = _engine(oracle, compute_dtype="bf16")
-    yield oracle, m
-    m.close()
+    with contextlib.closing(support.engine(oracle, vb.BertForMultiModalPreTraining, compute_dtype="bf16")) as m:
+        yield oracle, m
 
 
 def _batch(model, B, Tin, V, seed):
@@ -68,13 +58,6 @@ def _batch(model, B, Tin, V, seed):
     b = S.synthetic_masked_batch(B, Tin, V, seed=seed, vocab_size=d["vocab_size"], v_feature_size=d["v_feature_size"],
                                  v_target_size=d["v_target_size"])
     return b
-
-
-def _n_plans(model):
-    L = _lib()
-    v = C.c_int64()
-    L.check(L.load().vb200_model_dim(model._handle, b"n_plans", C.byref(v)), model._handle)
-    return v.value
 
 
 def _dense(model, inputs, select):
@@ -89,7 +72,7 @@ def _err(a, r):
 
 # ------------------------------------------------------------------ engine flags
 def test_engine_dims(tiny):
-    L = _lib()
+    L = support.lib()
     for m in tiny.values():
         assert m._dims["task_specific_tokens"] == 0 and m._dims["num_labels"] == 0 and m._dims["gqa_labels"] == 0
         v = C.c_int64()
@@ -335,7 +318,7 @@ def test_repeated_and_back_to_back_calls_same_bits(tiny, mode):
         vr = torch.randint(0, 150, (n_v,), generator=g)
         calls.append(dict(text_rows=tr, token_labels=torch.randint(0, vocab, (n_t,), generator=g), image_rows=vr,
                           image_targets=_targets(n_v, vt, n_v), pair_rows=[2, 0], pair_labels=[1, 0]))
-    plans = _n_plans(model)
+    plans = support.n_plans(model)
     alone = []
     for c in calls:
         alone.append(model.pretraining_objectives(taps, **c))
@@ -345,7 +328,7 @@ def test_repeated_and_back_to_back_calls_same_bits(tiny, mode):
     for a, r in zip(alone, again):
         for k in a:
             assert torch.equal(a[k], r[k]) or (torch.isnan(a[k]).all() and torch.isnan(r[k]).all()), k
-    assert _n_plans(model) == plans
+    assert support.n_plans(model) == plans
 
 
 def test_objectives_on_multitask_engine(tiny_oracle):
@@ -397,7 +380,7 @@ def test_zero_shot_retrieval_alignment(tiny):
 
 # ------------------------------------------------------------------ rejections
 def test_task_head_select_bits_rejected(tiny):
-    L = _lib()
+    L = support.lib()
     model = tiny["fp16"]
     b = _batch(model, 2, 10, 6, seed=17)
     names = {L.OUT_VIL_PREDICTION: "vil_prediction", L.OUT_VIL_PREDICTION_GQA: "vil_prediction_gqa", L.OUT_VIL_LOGIT: "vil_logit",
@@ -414,16 +397,16 @@ def test_task_head_select_bits_rejected(tiny):
         "cached_packed": lambda sel: model.forward_cached_packed(ts, one, vs, one, select=sel),
         "plan_info": lambda sel: model.plan_info(1, 10, 6, select=sel),
     }
-    plans = _n_plans(model)
+    plans = support.n_plans(model)
     for bit, name in names.items():
         for kind, call in calls.items():
             with pytest.raises(L.VilbertB200Error, match=f"task head {name} "):
                 call(bit)
-    assert _n_plans(model) == plans
+    assert support.n_plans(model) == plans
 
 
 def test_decode_families_rejected(tiny):
-    L = _lib()
+    L = support.lib()
     model = tiny["fp16"]
     t = torch.zeros(4, 3, device="cuda")
     fields = {L.DECODE_VQA: "vil_prediction", L.DECODE_GQA: "vil_prediction_gqa", L.DECODE_NLVR2: "vil_binary_prediction",
@@ -441,7 +424,7 @@ def test_decode_families_rejected(tiny):
 
 
 def _raw_objectives(model, taps, t_rows=(), t_labels=(), v_rows=(), targets=None, p_rows=(), p_labels=(), top_k=0):
-    L = _lib()
+    L = support.lib()
     keep = []
 
     def arr(v):
@@ -456,10 +439,10 @@ def _raw_objectives(model, taps, t_rows=(), t_labels=(), v_rows=(), targets=None
     outs = [torch.full((max(len(x), 1),), 7.0, device="cuda") for x in rows] + [torch.full((3,), 7.0, device="cuda")]
     o = L.PretrainLosses(*(x.data_ptr() for x in outs))
     torch.cuda.synchronize()
-    plans = _n_plans(model)
+    plans = support.n_plans(model)
     rc = L.load().vb200_pretraining_objectives(model._handle, C.byref(r), C.byref(tg), C.byref(o), None)
     torch.cuda.synchronize()
-    assert _n_plans(model) == plans
+    assert support.n_plans(model) == plans
     return rc, L.load().vb200_last_error(model._handle).decode(), outs
 
 

@@ -11,48 +11,27 @@ import ctypes as C
 import pytest
 import torch
 
+import support
+
 pytestmark = pytest.mark.gpu
 
 MODES = ("fp16", "bf16", "fp32x")
 TOL = {"fp16": 1e-2, "bf16": 2e-2, "fp32x": 1e-3}   # vs the oracle's heads (16-bit modes: with the engine's operand rounding emulated)
 
 
-def _lib():
-    from vilbert_b200 import _lib as L
-    return L
-
-
-def _engine(oracle, **kw):
-    import vilbert_b200 as vb
-    cfg = vb.BertConfig.from_dict(oracle.config.to_dict())
-    return vb.VILBertForVLTasks.from_pretrained(oracle.state_dict(), config=cfg, num_labels=oracle.num_labels, **kw).eval().cuda(0)
-
-
 @pytest.fixture(scope="module")
 def tiny(tiny_oracle):
-    e = {k: _engine(tiny_oracle, compute_dtype=k) for k in MODES}
-    yield e
-    for m in e.values():
-        m.close()
+    yield from support.engines(tiny_oracle, MODES)
 
 
 @pytest.fixture(scope="module")
 def full(full_oracle):
-    m = _engine(full_oracle, compute_dtype="bf16")
-    yield m
-    m.close()
+    yield from support.one_engine(full_oracle, compute_dtype="bf16")
 
 
 def _both_heads():
-    L = _lib()
+    L = support.lib()
     return L.OUT_LINGUISIC_PREDICTION | L.OUT_VISION_PREDICTION
-
-
-def _n_plans(model):
-    v = C.c_int64()
-    L = _lib()
-    L.check(L.load().vb200_model_dim(model._handle, b"n_plans", C.byref(v)), model._handle)
-    return v.value
 
 
 def _row_lists(total, seed):
@@ -154,7 +133,7 @@ def test_full_model_rows_bit_identical(full):
 
 # ------------------------------------------------------------------ alignment = element 3 of a batch-1 forward
 def _element3_alone(model, inp, b):
-    L = _lib()
+    L = support.lib()
     one = [t[b:b + 1] for t in inp]
     return model(*[t.cuda() for t in one], select=L.OUT_VIL_BINARY_PREDICTION)[3]
 
@@ -180,7 +159,7 @@ def _dense_alone(model, q, f, s, seg, tk, nt, nv, b):
 
 @pytest.mark.parametrize("mode", ("fp16", "bf16"))
 def test_alignment_from_packed_and_cached_packed(tiny, mode):
-    L = _lib()
+    L = support.lib()
     model = tiny[mode]
     nt, nv = [12, 30, 5, 22], [20, 9, 36, 14]
     q, f, s, seg, tk = _packed_inputs(model, nt, nv, 41)
@@ -257,13 +236,13 @@ def test_top_k_matches_softmax_of_logits(tiny, mode, k):
 # ------------------------------------------------------------------ independence and isolation
 @pytest.mark.parametrize("mode", ("fp16", "fp32x"))
 def test_back_to_back_calls_and_isolation(tiny, mode):
-    L = _lib()
+    L = support.lib()
     model = tiny[mode]
     inp = _dense(model, 3, 60, 50, seed=71)
     sel = L.OUT_TASK_HEADS
     before, taps = _run_dense(model, inp, sel)
     before = [x.clone() if torch.is_tensor(x) else x for x in before]
-    plans = _n_plans(model)
+    plans = support.n_plans(model)
     lists = [([0, 1, 2], [5]), (list(range(150)), list(range(140, 0, -1))), ([182, 182], [149]), (list(range(183)), [0] * 300)]
     alone = []
     for tr, vr in lists:
@@ -276,19 +255,19 @@ def test_back_to_back_calls_and_isolation(tiny, mode):
             assert torch.equal(a[key], b[key]), key
         for key in ("token_top", "region_top"):
             assert torch.equal(a[key][0], b[key][0]) and torch.equal(a[key][1], b[key][1]), key
-    assert _n_plans(model) == plans
+    assert support.n_plans(model) == plans
     after, _ = _run_dense(model, inp, sel)
     torch.cuda.synchronize()
     for x, y in zip(before[:9], after[:9]):
         assert (x is None and y is None) or torch.equal(x, y)
-    assert _n_plans(model) == plans
+    assert support.n_plans(model) == plans
 
 
 # ------------------------------------------------------------------ rejections
 def _raw_call(model, t_rows=None, v_rows=None, p_rows=None, top_k=0, states=(True, True, True), tops=(False, False), n_override=None):
     """vb200_pretraining_heads on a B=2 dense forward's taps with sentinel-filled outputs; returns (status, message, outputs).  The
     call leaves the forward-plan count as it was."""
-    L = _lib()
+    L = support.lib()
     inp = _dense(model, 2, 20, 16, seed=81)
     _, taps = _run_dense(model, inp, 0)
     d = model._dims
@@ -311,11 +290,11 @@ def _raw_call(model, t_rows=None, v_rows=None, p_rows=None, top_k=0, states=(Tru
     o = L.PretrainOut(outs["token_logits"].data_ptr(), outs["region_logits"].data_ptr(), outs["alignment"].data_ptr(),
                       outs["token_top"].data_ptr() if tops[0] else None, outs["region_top"].data_ptr() if tops[1] else None)
     torch.cuda.synchronize()
-    plans = _n_plans(model)
+    plans = support.n_plans(model)
     rc = L.load().vb200_pretraining_heads(model._handle, C.byref(r), C.byref(o), None)
     torch.cuda.synchronize()
     msg = L.load().vb200_last_error(model._handle).decode()
-    assert _n_plans(model) == plans
+    assert support.n_plans(model) == plans
     return rc, msg, outs
 
 
@@ -342,7 +321,7 @@ def test_rejections_name_list_and_index(tiny, case, needle):
 def test_top_k_above_width_rejected():
     from oracle import vilbert_ref as R
     oracle = R.build(R.tiny_config(v_target_size=8), seed=7, num_labels=200)
-    model = _engine(oracle)
+    model = support.engine(oracle)
     try:
         rc, msg, outs = _raw_call(model, v_rows=[0, 1], top_k=9, tops=(False, True))
         assert rc == -1 and "top_k 9 is above the 8 logits of a region_top row" in msg, msg

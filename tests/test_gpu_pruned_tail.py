@@ -6,10 +6,11 @@ each case compares a pooled-only call with the same call made to keep every row 
 pooled-based outputs and pooled_output must be bit-identical.
 """
 import contextlib
-import ctypes as C
 
 import pytest
 import torch
+
+import support
 
 pytestmark = pytest.mark.gpu
 
@@ -18,25 +19,9 @@ POOLED = 0x1F           # VIL_PREDICTION | VIL_PREDICTION_GQA | VIL_LOGIT | VIL_
 ROW_HEADS = (1 << 6) | (1 << 8)     # VISION_LOGIT | LINGUISIC_LOGIT: every final row of both streams is read
 
 
-def _engine(oracle, **kw):
-    import vilbert_b200 as vb
-    cfg = vb.BertConfig.from_dict(oracle.config.to_dict())
-    return vb.VILBertForVLTasks.from_pretrained(oracle.state_dict(), config=cfg, num_labels=oracle.num_labels, **kw).eval().cuda(0)
-
-
 @pytest.fixture(scope="module")
 def tiny(tiny_oracle):
-    e = {k: _engine(tiny_oracle, compute_dtype=k, return_attention=True, max_plans=256) for k in ("fp16", "bf16", "fp32x")}
-    yield e
-    for m in e.values():
-        m.close()
-
-
-def _n_plans(model):
-    from vilbert_b200 import _lib as L
-    v = C.c_int64()
-    L.check(L.load().vb200_model_dim(model._handle, b"n_plans", C.byref(v)), model._handle)
-    return v.value
+    yield from support.engines(tiny_oracle, ("fp16", "bf16", "fp32x"), return_attention=True, max_plans=256)
 
 
 @contextlib.contextmanager
@@ -62,12 +47,12 @@ def _pooled_tap_only(model):
 
 def _pruned_and_full(model, call, select=POOLED):
     """call(select, debug_taps) -> (10-tuple, taps), once with only pooled_output bound, once with every tap bound."""
-    n = _n_plans(model)
+    n = support.n_plans(model)
     with _pooled_tap_only(model):
         pruned = call(select, True)
     full = call(select, True)
     torch.cuda.synchronize()
-    assert _n_plans(model) == n + 2, "the pooled-only call and the taps call share a plan"
+    assert support.n_plans(model) == n + 2, "the pooled-only call and the taps call share a plan"
     return pruned, full
 
 
@@ -197,9 +182,9 @@ def test_taps_after_pruned_plan(tiny):
     model = tiny["bf16"]
     inp = _dense_inputs(model, 3, 11, 19, 29, 0)
     model(*inp, select=POOLED)
-    n = _n_plans(model)
+    n = support.n_plans(model)
     out, taps = model(*inp, select=POOLED, debug_taps=True)
-    assert _n_plans(model) == n + 1
+    assert support.n_plans(model) == n + 1
     ref_out, ref_taps = model(*inp, select=POOLED | ROW_HEADS, debug_taps=True)
     torch.cuda.synchronize()
     for k in ("sequence_output_t", "sequence_output_v", "pooled_output"):
@@ -210,9 +195,7 @@ def test_taps_after_pruned_plan(tiny):
 
 @pytest.fixture(scope="module")
 def full_bf16(full_oracle):
-    m = _engine(full_oracle, compute_dtype="bf16", max_plans=256)
-    yield m
-    m.close()
+    yield from support.one_engine(full_oracle, compute_dtype="bf16", max_plans=256)
 
 
 def test_full_model_bench_shape(full_bf16):

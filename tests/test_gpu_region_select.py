@@ -13,6 +13,7 @@ import pytest
 import torch
 
 from oracle import detections_ref as D
+import support
 
 pytestmark = pytest.mark.gpu
 
@@ -20,26 +21,14 @@ VOCAB = {t: i for i, t in enumerate(["[PAD]", "[UNK]", "[CLS]", "[SEP]", "what",
                                      "?", "color", "of", "a", "dog", "on", "grass"])}
 
 
-def _engine(oracle, dtype):
-    import vilbert_b200 as vb
-    cfg = vb.BertConfig.from_dict(oracle.config.to_dict())
-    return vb.VILBertForVLTasks.from_pretrained(oracle.state_dict(), config=cfg, num_labels=oracle.num_labels,
-                                                compute_dtype=dtype).eval().cuda(0)
-
-
 @pytest.fixture(scope="module")
 def tiny(tiny_oracle):
-    e = {k: _engine(tiny_oracle, k) for k in ("fp16", "bf16")}
-    yield e
-    for m in e.values():
-        m.close()
+    yield from support.engines(tiny_oracle, ("fp16", "bf16"))
 
 
 @pytest.fixture(scope="module")
 def full(full_oracle):
-    m = _engine(full_oracle, "bf16")
-    yield m
-    m.close()
+    yield from support.one_engine(full_oracle, compute_dtype="bf16")
 
 
 def _heads(counts, seed, F=2048, Cn=1601):

@@ -8,9 +8,10 @@ padded batch at the tolerances of test_gpu_packed.py.
 """
 import ctypes as C
 
-import numpy as np
 import pytest
 import torch
+
+import support
 
 pytestmark = pytest.mark.gpu
 
@@ -22,78 +23,26 @@ VOCAB = {t: i for i, t in enumerate(["[PAD]", "[UNK]", "[CLS]", "[SEP]", "what",
                                      "?", "color", "of", "un", "##aff", "##able", ",", "a", "dog", "on", "grass"])}
 
 
-def _engine(oracle, **kw):
-    import vilbert_b200 as vb
-    cfg = vb.BertConfig.from_dict(oracle.config.to_dict())
-    return vb.VILBertForVLTasks.from_pretrained(oracle.state_dict(), config=cfg, num_labels=oracle.num_labels, **kw).eval().cuda(0)
-
-
 @pytest.fixture(scope="module")
 def tiny(tiny_oracle):
-    e = {k: _engine(tiny_oracle, compute_dtype=k) for k in DT}
-    yield e
-    for m in e.values():
-        m.close()
+    yield from support.engines(tiny_oracle, DT)
 
 
 @pytest.fixture(scope="module")
 def full(full_oracle):
-    m = _engine(full_oracle)
-    yield m
-    m.close()
-
-
-def _image(tin, n, seed, F, vocab, wh=(640, 480)):
-    """One image row: tin token ids and segments, n detector boxes (relu features, pixel boxes inside the image), its size, a task."""
-    g = torch.Generator().manual_seed(seed)
-    q = torch.randint(1, vocab, (tin,), generator=g)
-    seg = torch.randint(0, 2, (tin,), generator=g)
-    f = torch.relu(torch.randn(n, F, generator=g)) * 1.5
-    w, h = wh
-    x1, y1 = torch.rand(n, generator=g) * 0.7 * w, torch.rand(n, generator=g) * 0.7 * h
-    x2 = torch.minimum(x1 + (0.05 + 0.25 * torch.rand(n, generator=g)) * w, torch.tensor(float(w)))
-    y2 = torch.minimum(y1 + (0.05 + 0.25 * torch.rand(n, generator=g)) * h, torch.tensor(float(h)))
-    task = int(torch.randint(0, 20, (1,), generator=g))
-    return q, seg, f, torch.stack([x1, y1, x2, y2], 1), torch.tensor([float(w), float(h)]), task
+    yield from support.one_engine(full_oracle)
 
 
 def _images(model, lens, seed):
     F, vocab = model._dims["v_feature_size"], model._dims["vocab_size"]
     whs = ((640, 480), (500, 375), (320, 240))
-    return [_image(t, n, seed + i, F, vocab, whs[i % 3]) for i, (t, n) in enumerate(lens)]
+    return [support.image(t, n, seed + i, F, vocab, whs[i % 3]) for i, (t, n) in enumerate(lens)]
 
 
 def _packed(model, imgs, select, **kw):
-    cat = lambda k: torch.cat([im[k] for im in imgs], dim=0).cuda()
-    out = model.forward_regions_packed(cat(0), cat(1), torch.tensor([[im[5]] for im in imgs]).cuda(), cat(2), cat(3),
-                                       torch.stack([im[4] for im in imgs]).cuda(), [len(im[0]) for im in imgs],
-                                       [im[2].shape[0] for im in imgs], select=select, **kw)
+    out = model.forward_regions_packed(*support.packed_image_args(imgs), select=select, **kw)
     torch.cuda.synchronize()
     return out
-
-
-def _regions_alone(model, im, select):
-    """vb200_forward_regions of one image (batch 1, its own Tin and box count, no padding) with the debug taps."""
-    from vilbert_b200 import _lib as L
-    q, seg, f, bx, wh, task = im
-    dev = lambda t, dt: t.to(device="cuda", dtype=dt).contiguous()
-    q, seg, ones = dev(q[None], torch.int64), dev(seg[None], torch.int64), torch.ones(1, len(q), dtype=torch.int64, device="cuda")
-    tk, f, bx, wh = dev(torch.tensor([[task]]), torch.int64), dev(f[None], torch.float32), dev(bx[None], torch.float32), dev(wh[None], torch.float32)
-    n = f.shape[1]
-    sp = torch.empty(1, n + 1, 5, device="cuda")
-    inp = L.RegionInputs(1, q.shape[1], n, q.data_ptr(), seg.data_ptr(), ones.data_ptr(), tk.data_ptr(), f.data_ptr(), bx.data_ptr(),
-                         wh.data_ptr(), None, sp.data_ptr())
-    outs, o, select = model._alloc_outputs(1, q.shape[1], n + 1, select, True, False, torch.device("cuda", 0))
-    L.check(L.load().vb200_forward_regions(model._handle, C.byref(inp), C.byref(o), select, 0,
-                                           C.c_void_p(torch.cuda.current_stream().cuda_stream)), model._handle)
-    torch.cuda.synchronize()
-    out, taps = model._result(outs, 1, q.shape[1], n + 1, True)
-    return out, taps, sp
-
-
-def _split_rows(t, counts):
-    offs = np.concatenate([[0], np.cumsum(counts)])
-    return [t[offs[i]:offs[i + 1]] for i in range(len(counts))]
 
 
 def _check_bitwise(model, imgs, packed):
@@ -103,10 +52,10 @@ def _check_bitwise(model, imgs, packed):
     t_rows = [len(im[0]) + 1 for im in imgs]
     v_rows = [im[2].shape[0] + 1 for im in imgs]
     for i, im in enumerate(imgs):
-        ref, rtaps, rsp = _regions_alone(model, im, vb.OUT_ALL)
+        (ref, rtaps), rsp = support.regions_alone(model, im, vb.OUT_ALL, debug_taps=True)
         for k in range(9):
             if k in ROW_OUT:
-                got = _split_rows(out[k], v_rows if ROW_OUT[k] == "regions" else t_rows)[i]
+                got = support.split_rows(out[k], v_rows if ROW_OUT[k] == "regions" else t_rows)[i]
                 want = ref[k][0]
             elif k == 3:
                 if B % 2 == 0:
@@ -115,10 +64,10 @@ def _check_bitwise(model, imgs, packed):
             else:
                 got, want = out[k][i], ref[k][0]
             assert torch.equal(got, want), f"image {i}: output {k} differs from forward_regions of the image alone"
-        assert torch.equal(_split_rows(taps["sequence_output_t"], t_rows)[i], rtaps["sequence_output_t"][0]), f"image {i}: text tap"
-        assert torch.equal(_split_rows(taps["sequence_output_v"], v_rows)[i], rtaps["sequence_output_v"][0]), f"image {i}: image tap"
+        assert torch.equal(support.split_rows(taps["sequence_output_t"], t_rows)[i], rtaps["sequence_output_t"][0]), f"image {i}: text tap"
+        assert torch.equal(support.split_rows(taps["sequence_output_v"], v_rows)[i], rtaps["sequence_output_v"][0]), f"image {i}: image tap"
         assert torch.equal(taps["pooled_output"][i], rtaps["pooled_output"][0]), f"image {i}: pooled tap"
-        assert torch.equal(_split_rows(sp, v_rows)[i], rsp[0]), f"image {i}: spatials"
+        assert torch.equal(support.split_rows(sp, v_rows)[i], rsp[0]), f"image {i}: spatials"
 
 
 # (Tin, boxes): Tin in {1, 3, 12, 37, 155}, boxes in {1, 9, 35, 100, 255} (V = 256, the attention kernels' limit)
@@ -189,13 +138,6 @@ def test_regions_packed_spatials_match_host_construction(tiny):
     assert float((sp.cpu() - want).abs().max()) < 1e-6
 
 
-def _n_plans(model):
-    from vilbert_b200 import _lib as L
-    v = C.c_int64()
-    L.check(L.load().vb200_model_dim(model._handle, b"n_plans", C.byref(v)), model._handle)
-    return v.value
-
-
 def test_regions_packed_shares_the_packed_plan(tiny):
     """At fixed capacities (37 tokens, 100 boxes) calls with different lengths share one plan, and forward_packed at the same
     capacities (101 regions) uses that plan too."""
@@ -204,14 +146,14 @@ def test_regions_packed_shares_the_packed_plan(tiny):
     sel = vb.OUT_TASK_HEADS
     cap = dict(max_tokens=37, max_boxes=100)
     _packed(model, _images(model, [(3, 10), (20, 99), (37, 1), (8, 40)], seed=61), sel, **cap)
-    n = _n_plans(model)
+    n = support.n_plans(model)
     _packed(model, _images(model, [(1, 2), (5, 5), (12, 7), (2, 3)], seed=62), sel, **cap)
-    assert _n_plans(model) == n
+    assert support.n_plans(model) == n
     F = model._dims["v_feature_size"]
     model.forward_packed(torch.ones(4 * 6, dtype=torch.long).cuda(), torch.rand(4 * 30, F).cuda(), torch.rand(4 * 30, 5).cuda(), None,
                          torch.zeros(4, 1, dtype=torch.long).cuda(), [6] * 4, [30] * 4, select=sel, max_tokens=37, max_regions=101)
     torch.cuda.synchronize()
-    assert _n_plans(model) == n
+    assert support.n_plans(model) == n
 
 
 def test_regions_packed_rejections(tiny_oracle, tiny):
@@ -253,7 +195,7 @@ def test_regions_packed_rejections(tiny_oracle, tiny):
     o = L.Outputs()
     assert L.load().vb200_forward_regions_packed(model._handle, C.byref(inp), C.byref(o), sel, 0, None) == -1
     assert b"vb200_packed_region_inputs has a NULL required pointer" in L.load().vb200_last_error(model._handle)
-    x = _engine(tiny_oracle, compute_dtype="fp32x")
+    x = support.engine(tiny_oracle, compute_dtype="fp32x")
     try:
         with err("fp32x"):
             _packed(x, ok, sel)
@@ -262,19 +204,6 @@ def test_regions_packed_rejections(tiny_oracle, tiny):
 
 
 # ----------------------------------------------------------------------------------------------- the worker on the engine
-def _detector_output(n_boxes, F, seed, wh=((640, 480), (500, 375), (320, 240))):
-    g = torch.Generator().manual_seed(seed)
-    feats, infos = [], []
-    for i, n in enumerate(n_boxes):
-        w, h = wh[i % len(wh)]
-        feats.append(torch.relu(torch.randn(n, F, generator=g)) * 1.5)
-        x1, y1 = torch.rand(n, generator=g) * 0.7 * w, torch.rand(n, generator=g) * 0.7 * h
-        bw, bh = (0.05 + 0.25 * torch.rand(n, generator=g)) * w, (0.05 + 0.25 * torch.rand(n, generator=g)) * h
-        bbox = torch.stack([x1, y1, torch.minimum(x1 + bw, torch.tensor(float(w))), torch.minimum(y1 + bh, torch.tensor(float(h)))], 1)
-        infos.append({"image_width": w, "image_height": h, "bbox": bbox.numpy().astype(np.float32)})
-    return feats, infos
-
-
 def _same_answer(a, b):
     """The tolerances of test_gpu_round2.py: same labels / boxes, confidences within 5e-3 (boxes: 0.5 percentage points)."""
     if isinstance(a, list):
@@ -297,9 +226,9 @@ def test_custom_prediction_packed_matches_custom_prediction(full):
     for k, (task_id, counts, q) in enumerate([("1", [36], "what is the man holding?"), ("12", [20, 33], "the man is holding a dog"),
                                                ("7", [20, 11, 57], "a dog on the grass"), ("11", [45], "the man"),
                                                ("13", [10], "a dog"), ("15", [100], "what is the color of the dog")]):
-        feats, infos = _detector_output(counts, F, seed=300 + k)
+        feats, infos = support.detector_output(counts, F, seed=300 + k)
         reqs.append((q, [int(task_id)], feats, infos, task_id))
-    bad_feats, bad_infos = _detector_output([5, 5], F, seed=399)
+    bad_feats, bad_infos = support.detector_output([5, 5], F, seed=399)
     reqs.insert(3, ("what", [1], bad_feats, bad_infos, "1"))          # VQA with two images
     calls = []
     orig = full.forward_regions_packed
@@ -332,7 +261,7 @@ def test_micro_batch_worker_packed_on_engine(full):
     for k, (task_id, counts, q) in enumerate([("1", [36], "what is the man holding?"), ("12", [20, 20], "the man is holding a dog"),
                                                ("7", [30, 12, 64], "a dog on the grass"), ("11", [25], "the man"), ("13", [8], "a dog"),
                                                ("15", [100], "what is the color of the dog")]):
-        feats, infos = _detector_output(counts, F, seed=600 + k)
+        feats, infos = support.detector_output(counts, F, seed=600 + k)
         body = {"image_path": [f"/m/demo/i{j}.jpg" for j in range(len(counts))], "question": q, "socket_id": f"s{k}", "task_id": task_id}
         msgs.append((body, feats, infos))
     want = [W.handle_request(*m) for m in msgs]

@@ -10,31 +10,22 @@ import ctypes as C
 import pytest
 import torch
 
+import support
+
 pytestmark = pytest.mark.gpu
 
 TOL = 1e-2                 # fp16 mode vs the fp32 oracle, and packed vs dense padded retrieval (test_gpu_model.py)
 DT = ("fp16", "bf16")
 
 
-def _engine(oracle, **kw):
-    import vilbert_b200 as vb
-    cfg = vb.BertConfig.from_dict(oracle.config.to_dict())
-    return vb.VILBertForVLTasks.from_pretrained(oracle.state_dict(), config=cfg, num_labels=oracle.num_labels, **kw).eval().cuda(0)
-
-
 @pytest.fixture(scope="module")
 def tiny(tiny_oracle):
-    e = {k: _engine(tiny_oracle, compute_dtype=k) for k in DT}
-    yield e
-    for m in e.values():
-        m.close()
+    yield from support.engines(tiny_oracle, DT)
 
 
 @pytest.fixture(scope="module")
 def full(full_oracle):
-    m = _engine(full_oracle)
-    yield m
-    m.close()
+    yield from support.one_engine(full_oracle)
 
 
 def _captions(model, lens, seed):
@@ -195,13 +186,6 @@ def test_retrieval_scores_packed_vs_cached(full):
     assert timings["pairs"] == 35 and timings["local_captions"] == 5
 
 
-def _n_plans(model):
-    from vilbert_b200 import _lib as L
-    v = C.c_int64()
-    L.check(L.load().vb200_model_dim(model._handle, b"n_plans", C.byref(v)), model._handle)
-    return v.value
-
-
 def test_packed_retrieval_plan_reuse(tiny):
     """Further chunks reuse the pair plan; a second run with other lengths under the same capacities builds no plan."""
     import vilbert_b200 as vb
@@ -209,15 +193,15 @@ def test_packed_retrieval_plan_reuse(tiny):
     caps, imgs = _captions(model, [5, 30, 12], seed=6), _images(model, [36, 101, 10, 7], seed=6)
     ts, vs = _encode(model, caps, imgs, max_tokens=30, max_regions=101)
     model.forward_cached_packed(ts, torch.tensor([0, 1, 2, 0]), vs, torch.tensor([0, 1, 2, 3]), select=vb.OUT_VIL_LOGIT)
-    n = _n_plans(model)
+    n = support.n_plans(model)
     model.forward_cached_packed(ts, torch.tensor([2, 2, 1, 0]), vs, torch.tensor([3, 1, 0, 2]), select=vb.OUT_VIL_LOGIT)
-    assert _n_plans(model) == n
+    assert support.n_plans(model) == n
     caps2, imgs2 = _captions(model, [2, 17, 9], seed=7), _images(model, [3, 50, 1, 88], seed=7)
     ts2, vs2 = _encode(model, caps2, imgs2, max_tokens=30, max_regions=101)
     got = model.forward_cached_packed(ts2, torch.tensor([1, 0, 2, 1]), vs2, torch.tensor([2, 3, 0, 1]), select=vb.OUT_VIL_LOGIT,
                                       max_tokens=30, max_regions=101)
     torch.cuda.synchronize()
-    assert _n_plans(model) == n
+    assert support.n_plans(model) == n
     # capacity changes no bit: the same pairs at this call's own maxima (another plan)
     ref = model.forward_cached_packed(ts2, torch.tensor([1, 0, 2, 1]), vs2, torch.tensor([2, 3, 0, 1]), select=vb.OUT_VIL_LOGIT)
     torch.cuda.synchronize()
@@ -265,7 +249,7 @@ def test_packed_retrieval_rejections(tiny_oracle, tiny):
                           ts["h16"].data_ptr(), 2, vs["offsets"].data_ptr(), vs["f32"].data_ptr(), vs["h16"].data_ptr())
     assert lib.vb200_forward_cached_packed(model._handle, C.byref(pairs), C.byref(L.Outputs()), L.OUT_VIL_LOGIT, 0, None) == -1
     assert b"NULL" in lib.vb200_last_error(model._handle)
-    x = _engine(tiny_oracle, compute_dtype="fp32x")
+    x = support.engine(tiny_oracle, compute_dtype="fp32x")
     try:
         with err("fp32x"):
             _encode(x, caps, imgs)

@@ -11,6 +11,8 @@ import ctypes as C
 import pytest
 import torch
 
+import support
+
 pytestmark = pytest.mark.gpu
 
 TOL = 1e-2                 # the packed retrieval tests' tolerance against the fp32 oracle
@@ -19,25 +21,14 @@ TAPS = ("sequence_output_t", "sequence_output_v", "pooled_output")
 VOCAB = {t: i for i, t in enumerate(["[PAD]", "[UNK]", "[CLS]", "[SEP]", "a", "dog", "on", "the", "grass", "man"])}
 
 
-def _engine(oracle, **kw):
-    import vilbert_b200 as vb
-    cfg = vb.BertConfig.from_dict(oracle.config.to_dict())
-    return vb.VILBertForVLTasks.from_pretrained(oracle.state_dict(), config=cfg, num_labels=oracle.num_labels, **kw).eval().cuda(0)
-
-
 @pytest.fixture(scope="module")
 def tiny(tiny_oracle):
-    e = {k: _engine(tiny_oracle, compute_dtype=k) for k in DT}
-    yield e
-    for m in e.values():
-        m.close()
+    yield from support.engines(tiny_oracle, DT)
 
 
 @pytest.fixture(scope="module")
 def full(full_oracle):
-    m = _engine(full_oracle)
-    yield m
-    m.close()
+    yield from support.one_engine(full_oracle)
 
 
 def _captions(model, lens, seed):
@@ -256,13 +247,6 @@ def test_full_model_bitwise_oracle_and_multi_gpu_path(full, full_oracle):
     assert err < TOL, f"vil_logit vs fp32 oracle: {err}"
 
 
-def _n_plans(model):
-    from vilbert_b200 import _lib as L
-    v = C.c_int64()
-    L.check(L.load().vb200_model_dim(model._handle, b"n_plans", C.byref(v)), model._handle)
-    return v.value
-
-
 def test_plan_shared_with_encode_image_packed(tiny):
     """encode_image_packed at max_regions = k + 1 and encode_regions_packed at max_boxes = k (same image count) use one plan."""
     model = tiny["fp16"]
@@ -270,10 +254,10 @@ def test_plan_shared_with_encode_image_packed(tiny):
     k, lens = 40, [41, 3, 17, 30]
     model.encode_image_packed(torch.rand(sum(lens), F).cuda(), torch.rand(sum(lens), 5).cuda(), lens, max_regions=k + 1)
     torch.cuda.synchronize()
-    n = _n_plans(model)
+    n = support.n_plans(model)
     _encode_gallery(model, _gallery(model, [40, 1, 22, 7], seed=5), max_boxes=k)
     torch.cuda.synchronize()
-    assert _n_plans(model) == n
+    assert support.n_plans(model) == n
 
 
 def test_back_to_back_calls(tiny):
@@ -316,7 +300,7 @@ def test_encode_regions_packed_rejections(tiny_oracle, tiny):
         args[null] = None
         assert lib.vb200_encode_regions_packed(model._handle, 1, 0, *args, None) == -1
         assert b"vb200_encode_regions_packed: NULL pointer" in lib.vb200_last_error(model._handle)
-    x = _engine(tiny_oracle, compute_dtype="fp32x")
+    x = support.engine(tiny_oracle, compute_dtype="fp32x")
     try:
         with err("packed batches are not supported in split_fp32"):
             _encode_gallery(x, ok)

@@ -14,25 +14,13 @@ import numpy as np
 import pytest
 import torch
 
+import support
+
 pytestmark = pytest.mark.gpu
 
 TOL_FP32X = 1e-3            # north_star: "within 1e-3 fp32 ... per logit"
 NAMES = ["vil_prediction", "vil_prediction_gqa", "vil_logit", "vil_binary_prediction", "vil_tri_prediction",
          "vision_prediction", "vision_logit", "linguisic_prediction", "linguisic_logit"]
-
-
-def _engine(oracle, **kw):
-    import vilbert_b200 as vb
-    cfg = vb.BertConfig.from_dict(oracle.config.to_dict())
-    m = vb.VILBertForVLTasks.from_pretrained(oracle.state_dict(), config=cfg, num_labels=oracle.num_labels, **kw)
-    return m.eval().cuda(0)
-
-
-def _tiny_inputs(oracle, B, Tin, V, seed, pad=0):
-    from oracle import vilbert_ref as R
-    inp = list(R.make_inputs(B, Tin, V, seed=seed, vocab_size=oracle.config.vocab_size, pad_regions=pad))
-    inp[1] = inp[1][..., :oracle.config.v_feature_size].contiguous()
-    return inp
 
 
 def _max_err(ref, out):
@@ -49,36 +37,28 @@ def _max_err(ref, out):
 
 @pytest.fixture(scope="module")
 def tiny_x(tiny_oracle):
-    m = _engine(tiny_oracle, compute_dtype="fp32x", return_attention=True)
-    yield m
-    m.close()
+    yield from support.one_engine(tiny_oracle, compute_dtype="fp32x", return_attention=True)
 
 
 @pytest.fixture(scope="module")
 def full_x(full_oracle):
-    m = _engine(full_oracle, compute_dtype="fp32x")
-    yield m
-    m.close()
+    yield from support.one_engine(full_oracle, compute_dtype="fp32x")
 
 
 @pytest.fixture(scope="module")
 def full_h(full_oracle):
-    m = _engine(full_oracle, return_attention=True)
-    yield m
-    m.close()
+    yield from support.one_engine(full_oracle, return_attention=True)
 
 
 @pytest.fixture(scope="module")
 def tiny_h(tiny_oracle):
-    m = _engine(tiny_oracle, return_attention=True)
-    yield m
-    m.close()
+    yield from support.one_engine(tiny_oracle, return_attention=True)
 
 
 # ----------------------------------------------------------------------------------------------- fp32-parity mode
 @pytest.mark.parametrize("B,Tin,V,pad", [(2, 30, 36, 0), (3, 16, 10, 3), (1, 12, 37, 0), (4, 37, 101, 7), (2, 70, 100, 0)])
 def test_fp32x_tiny_all_outputs(tiny_oracle, tiny_x, parity_log, B, Tin, V, pad):
-    inp = _tiny_inputs(tiny_oracle, B, Tin, V, 500 + B, pad)
+    inp = support.tiny_inputs(tiny_oracle, B, Tin, V, 500 + B, pad)
     ref = tiny_oracle(*inp, compute_pretraining_heads=True)
     out = tiny_x(*[t.cuda() for t in inp], compute_pretraining_heads=True)
     torch.cuda.synchronize()
@@ -141,7 +121,7 @@ def _check_attn(attn, ref_attn, tol, tag, parity_log):
 
 
 def test_attention_probabilities_tiny(tiny_oracle, tiny_h, tiny_x, parity_log):
-    inp = _tiny_inputs(tiny_oracle, 3, 20, 12, 61, pad=2)
+    inp = support.tiny_inputs(tiny_oracle, 3, 20, 12, 61, pad=2)
     ref = tiny_oracle(*inp, output_all_attention_masks=True)
     dev = [t.cuda() for t in inp]
     out = tiny_h(*dev, output_all_attention_masks=True)
@@ -169,21 +149,6 @@ def test_attention_probabilities_full(full_oracle, full_h, parity_log):
 
 
 # ----------------------------------------------------------------------------------------------- device-side input builder
-def _detector_output(n_img, n, F, seed, wh=((640, 480), (500, 375), (320, 240))):
-    g = torch.Generator().manual_seed(seed)
-    feats = [torch.relu(torch.randn(n, F, generator=g)) * 1.5 for _ in range(n_img)]
-    infos = []
-    for i in range(n_img):
-        w, h = wh[i % len(wh)]
-        x1 = torch.rand(n, generator=g) * 0.7 * w
-        y1 = torch.rand(n, generator=g) * 0.7 * h
-        bw = (0.05 + 0.25 * torch.rand(n, generator=g)) * w
-        bh = (0.05 + 0.25 * torch.rand(n, generator=g)) * h
-        bbox = torch.stack([x1, y1, torch.minimum(x1 + bw, torch.tensor(float(w))), torch.minimum(y1 + bh, torch.tensor(float(h)))], 1)
-        infos.append({"image_width": w, "image_height": h, "bbox": bbox.numpy().astype(np.float32)})
-    return feats, infos
-
-
 VOCAB = {t: i for i, t in enumerate(["[PAD]", "[UNK]", "[CLS]", "[SEP]", "what", "is", "the", "man", "hold", "##ing",
                                      "?", "color", "of", "un", "##aff", "##able", ",", "a", "dog", "on", "grass"])}
 
@@ -192,7 +157,7 @@ def test_forward_regions_matches_host_construction(full_oracle, full_x, full_h, 
     """One region-pack kernel == worker.py:422-455 on the host (build_inputs) followed by the ordinary forward."""
     from vilbert_b200 import worker_api as W
     tok = W.WordpieceTokenizer(VOCAB)
-    feats, infos = _detector_output(3, 20, 2048, seed=12)
+    feats, infos = support.detector_output_features_first(3, 20, 2048, seed=12)
     text, f, s, seg, im, vm, co, task = W.build_inputs("what is the man holding?", [7], feats, infos, torch.device("cuda", 0), tok)
     rep = lambda t: t.repeat(3, 1)
     boxes = torch.stack([torch.from_numpy(i["bbox"]) for i in infos])
@@ -227,7 +192,7 @@ def test_cached_states_are_bit_identical(which, request, tiny_oracle, full_oracl
     from vilbert_b200 import _lib as L
     if which.startswith("tiny"):
         eng = request.getfixturevalue("tiny_h" if which == "tiny_fp16" else "tiny_x")
-        cap, img = _tiny_inputs(tiny_oracle, 5, 22, 14, 71), _tiny_inputs(tiny_oracle, 4, 22, 14, 72, pad=2)
+        cap, img = support.tiny_inputs(tiny_oracle, 5, 22, 14, 71), support.tiny_inputs(tiny_oracle, 4, 22, 14, 72, pad=2)
     else:
         eng = request.getfixturevalue("full_h")
         cap, img = R.make_inputs(5, 30, 36, seed=71), R.make_inputs(4, 30, 36, seed=72, pad_regions=2)
@@ -251,10 +216,10 @@ def test_cached_states_are_bit_identical(which, request, tiny_oracle, full_oracl
 def test_plan_cache_is_bounded(tiny_oracle):
     import ctypes as C
     from vilbert_b200 import _lib as L
-    eng = _engine(tiny_oracle, max_plans=3)
+    eng = support.engine(tiny_oracle, max_plans=3)
     first = None
     for k, B in enumerate([1, 2, 3, 4, 5, 1]):
-        inp = [t.cuda() for t in _tiny_inputs(tiny_oracle, B, 20, 12, 31)]
+        inp = [t.cuda() for t in support.tiny_inputs(tiny_oracle, B, 20, 12, 31)]
         out = eng(*inp)[0].clone()
         if k == 0:
             first = out
@@ -294,7 +259,7 @@ def test_custom_prediction_on_engine(full_oracle, full_h, task_id, n_img):
     from vilbert_b200 import worker_api as W
     W.label_maps.update(vqa=None, gqa=None)
     W.tokenizer = W.WordpieceTokenizer(VOCAB)
-    feats, infos = _detector_output(n_img, 20, 2048, seed=40 + n_img)
+    feats, infos = support.detector_output_features_first(n_img, 20, 2048, seed=40 + n_img)
     W.model = full_h
     ans = W.custom_prediction("what is the man holding?", [int(task_id)], feats, infos, task_id)
     W.model = _OracleAsModel(full_oracle)
@@ -314,7 +279,7 @@ def test_custom_prediction_unequal_box_counts(full_oracle, full_h):
     W.label_maps.update(vqa=None, gqa=None)
     W.tokenizer = W.WordpieceTokenizer(VOCAB)
     W.model = full_h
-    feats, infos = _detector_output(3, 20, 2048, seed=9)
+    feats, infos = support.detector_output_features_first(3, 20, 2048, seed=9)
     feats[1] = feats[1][:11]
     infos[1] = dict(infos[1], bbox=infos[1]["bbox"][:11])
     ans = W.custom_prediction("a dog on the grass", [7], feats, infos, "7")
@@ -343,7 +308,7 @@ def test_micro_batch_worker_on_engine(full_oracle, full_h):
     for k, (task_id, n_img, q) in enumerate([("1", 1, "what is the man holding?"), ("12", 2, "the man is holding a dog"),
                                               ("7", 3, "a dog on the grass"), ("11", 1, "the man"), ("13", 1, "a dog"),
                                               ("12", 2, "what color"), ("15", 1, "what is the color of the dog")]):
-        feats, infos = _detector_output(n_img, 20, 2048, seed=600 + k)
+        feats, infos = support.detector_output_features_first(n_img, 20, 2048, seed=600 + k)
         body = {"image_path": [f"/m/demo/i{j}.jpg" for j in range(n_img)], "question": q, "socket_id": f"s{k}", "task_id": task_id}
         msgs.append((body, feats, infos))
     want = [W.handle_request(*m) for m in msgs]
@@ -369,9 +334,9 @@ def test_timeline_records_every_gemm_cta(tiny_oracle):
     import ctypes as C
     import numpy as np
     from vilbert_b200 import _lib as L
-    inp = _tiny_inputs(tiny_oracle, 4, 30, 36, 94)
+    inp = support.tiny_inputs(tiny_oracle, 4, 30, 36, 94)
     dev = [t.cuda() for t in inp]
-    eng = _engine(tiny_oracle)
+    eng = support.engine(tiny_oracle)
     sel = L.OUT_VIL_PREDICTION
     plain = eng(*dev, select=sel)[0].clone()
     eng.set_option("timeline", 1)

@@ -8,16 +8,14 @@
 import pytest
 import torch
 
+import support
+
 pytestmark = pytest.mark.gpu
 
 
 @pytest.fixture(scope="module")
 def engine(full_oracle):
-    import vilbert_b200 as vb
-    cfg = vb.BertConfig.from_dict(full_oracle.config.to_dict())
-    m = vb.VILBertForVLTasks.from_pretrained(full_oracle.state_dict(), config=cfg, num_labels=full_oracle.num_labels).eval().cuda(0)
-    yield m
-    m.close()
+    yield from support.one_engine(full_oracle)
 
 
 def test_multitask_batch_sharded(full_oracle, engine, parity_log):

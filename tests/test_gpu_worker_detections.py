@@ -8,6 +8,8 @@ before (process_feature_extraction per message, then MicroBatchWorker(packed=Tru
 import pytest
 import torch
 
+import support
+
 pytestmark = pytest.mark.gpu
 
 VOCAB = {t: i for i, t in enumerate(["[PAD]", "[UNK]", "[CLS]", "[SEP]", "what", "is", "the", "man", "hold", "##ing",
@@ -16,26 +18,14 @@ MIXED = [("1", [1000], "what is the man holding?"), ("12", [300, 80], "the man i
          ("7", [60, 1000, 40], "a dog on the grass"), ("11", [500], "the man"), ("13", [37], "a dog"), ("1", [7], "what color")]
 
 
-def _engine(oracle, dtype):
-    import vilbert_b200 as vb
-    cfg = vb.BertConfig.from_dict(oracle.config.to_dict())
-    return vb.VILBertForVLTasks.from_pretrained(oracle.state_dict(), config=cfg, num_labels=oracle.num_labels,
-                                                compute_dtype=dtype).eval().cuda(0)
-
-
 @pytest.fixture(scope="module")
 def tiny(tiny_oracle):
-    e = {k: _engine(tiny_oracle, k) for k in ("fp16", "bf16")}
-    yield e
-    for m in e.values():
-        m.close()
+    yield from support.engines(tiny_oracle, ("fp16", "bf16"))
 
 
 @pytest.fixture(scope="module")
 def full(full_oracle):
-    m = _engine(full_oracle, "bf16")
-    yield m
-    m.close()
+    yield from support.one_engine(full_oracle, compute_dtype="bf16")
 
 
 def _worker_api(m):

@@ -1,7 +1,6 @@
 """Host-side multi-GPU logic on CPU: sharding arithmetic, and a world_size-2 gloo run of the retrieval
 all-gather and of batch-sharded execution (the N>1 path of bench.py / vilbert_b200.parallel)."""
 import os
-import socket
 
 import pytest
 import torch
@@ -9,6 +8,7 @@ import torch.distributed as dist
 import torch.multiprocessing as mp
 
 from vilbert_b200 import parallel as P
+import support
 
 
 def test_shard_range_covers_and_balances():
@@ -28,14 +28,6 @@ def test_shard_range_pair_aligned():
             assert spans[-1][1] == n and all(lo % 2 == 0 and hi % 2 == 0 for lo, hi in spans)
     with pytest.raises(ValueError):
         P.shard_range(7, 0, 2, pair_aligned=True)
-
-
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
 
 
 def _worker(rank, world, port, n_cap, n_img, q):
@@ -67,7 +59,7 @@ def _worker(rank, world, port, n_cap, n_img, q):
 def test_retrieval_allgather_gloo_world2(n_cap, n_img):
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    port = _free_port()
+    port = support.free_port()
     procs = [ctx.Process(target=_worker, args=(r, 2, port, n_cap, n_img, q)) for r in range(2)]
     for p in procs:
         p.start()

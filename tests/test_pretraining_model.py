@@ -5,7 +5,6 @@ model under a gloo world of 2.  The engine calls themselves are covered on the G
 import ctypes as C
 import os
 import shutil
-import socket
 import subprocess
 
 import pytest
@@ -19,6 +18,7 @@ from vilbert_b200 import _lib as L
 from vilbert_b200 import parallel as P
 from vilbert_b200 import synthetic as S
 from vilbert_b200.model import packed_offsets
+import support
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 TARGET_FIELDS = ["token_labels", "image_targets", "pair_labels"]
@@ -311,14 +311,6 @@ def _check(rank, world, n_cap, n_img, pair_batch):
     return True
 
 
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
 def _worker(rank, world, port, n_cap, n_img, pair_batch, q):
     os.environ["MASTER_ADDR"] = "127.0.0.1"
     os.environ["MASTER_PORT"] = str(port)
@@ -336,7 +328,7 @@ def _worker(rank, world, port, n_cap, n_img, pair_batch, q):
 def test_alignment_routing_gloo_world2():
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    port = _free_port()
+    port = support.free_port()
     procs = [ctx.Process(target=_worker, args=(r, 2, port, 5, 6, 4, q)) for r in range(2)]
     for p in procs:
         p.start()

@@ -5,7 +5,6 @@ import ctypes as C
 import os
 import re
 import shutil
-import socket
 import subprocess
 
 import pytest
@@ -16,6 +15,7 @@ import torch.multiprocessing as mp
 from vilbert_b200 import _lib as L
 from vilbert_b200 import parallel as P
 from vilbert_b200.model import packed_offsets
+import support
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 F = 8
@@ -129,14 +129,6 @@ def _gallery(n_img):
     return (bf, torch.rand(sum(n_boxes), 4), torch.full((n_img, 2), 100.0), n_boxes)
 
 
-def _padded_gallery(n_img, v_pad=5):
-    lens = [1 + (7 * i) % v_pad for i in range(n_img)]
-    f, s, vm = torch.zeros(n_img, v_pad, F), torch.rand(n_img, v_pad, 5), torch.zeros(n_img, v_pad, dtype=torch.uint8)
-    for i, k in enumerate(lens):
-        f[i, :k], vm[i, :k] = float(i), 1
-    return (f, s, vm), lens
-
-
 def _check(rank, world, n_cap, n_img, pair_batch):
     g = torch.Generator().manual_seed(5)
     table, align = torch.randn(n_cap, n_img, generator=g), torch.randn(n_cap, n_img, 2, generator=g)
@@ -149,7 +141,7 @@ def _check(rank, world, n_cap, n_img, pair_batch):
     aligned = []
     for c, i in chunks:
         aligned += [("forward_cached_packed", c, i, 0, True), ("pretraining_heads", list(range(pair_batch)), None, None, 0)]
-    images, v_lens = _padded_gallery(n_img)
+    images, v_lens = support.padded_gallery(n_img, F)
     gallery = _gallery(n_img)
     for score, expect, calls in ((None, table, default), ("vil_logit", table, default), ("alignment", align, aligned)):
         kw = {} if score is None else {"score": score}
@@ -162,14 +154,6 @@ def _check(rank, world, n_cap, n_img, pair_batch):
         assert torch.equal(full, expect), score
         assert m.calls == [("encode_regions_packed", gallery[3], 6), text_call] + calls, score
     return True
-
-
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
 
 
 def _worker(rank, world, port, n_cap, n_img, pair_batch, q):
@@ -190,7 +174,7 @@ def _worker(rank, world, port, n_cap, n_img, pair_batch, q):
 def test_score_routing_gloo_world2(n_cap, n_img, pair_batch):
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    port = _free_port()
+    port = support.free_port()
     procs = [ctx.Process(target=_worker, args=(r, 2, port, n_cap, n_img, pair_batch, q)) for r in range(2)]
     for p in procs:
         p.start()

@@ -4,7 +4,6 @@ retrieval_scores_packed makes the calls it made before its pair loop was shared.
 tests/test_gpu_retrieval_regions.py."""
 import os
 import re
-import socket
 
 import pytest
 import torch
@@ -14,6 +13,7 @@ import torch.multiprocessing as mp
 from vilbert_b200 import _lib as L
 from vilbert_b200 import parallel as P
 from vilbert_b200.model import packed_offsets
+import support
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 F = 8
@@ -67,14 +67,6 @@ def _gallery(n_img):
     return (bf, torch.rand(sum(n_boxes), 4), torch.full((n_img, 2), 100.0), n_boxes)
 
 
-def _padded_gallery(n_img, v_pad=5):
-    lens = [1 + (7 * i) % v_pad for i in range(n_img)]
-    f, s, vm = torch.zeros(n_img, v_pad, F), torch.rand(n_img, v_pad, 5), torch.zeros(n_img, v_pad, dtype=torch.uint8)
-    for i, k in enumerate(lens):
-        f[i, :k], vm[i, :k] = float(i), 1
-    return (f, s, vm), lens
-
-
 def _expected_pairs(lo, hi, n_img, pair_batch):
     ci, ii, _ = P.retrieval_pairs(hi - lo, n_img, pair_batch)
     return [("forward_cached_packed", ci[s:s + pair_batch].tolist(), ii[s:s + pair_batch].tolist(), L.OUT_VIL_LOGIT)
@@ -98,19 +90,11 @@ def _check(rank, world, n_cap, n_img, pair_batch):
     assert m.calls == [("encode_regions_packed", gallery[3], 6), text_call] + pairs
 
     m = StubModel(table)
-    images, v_lens = _padded_gallery(n_img)
+    images, v_lens = support.padded_gallery(n_img, F)
     full = P.retrieval_scores_packed(m, caps, images, pair_batch=pair_batch)
     assert torch.equal(full, table)
     assert m.calls == [("encode_image_packed", v_lens), text_call] + pairs
     return True
-
-
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
 
 
 def _worker(rank, world, port, n_cap, n_img, pair_batch, q):
@@ -131,7 +115,7 @@ def _worker(rank, world, port, n_cap, n_img, pair_batch, q):
 def test_retrieval_regions_gloo_world2(n_cap, n_img, pair_batch):
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    port = _free_port()
+    port = support.free_port()
     procs = [ctx.Process(target=_worker, args=(r, 2, port, n_cap, n_img, pair_batch, q)) for r in range(2)]
     for p in procs:
         p.start()

@@ -16,15 +16,10 @@ from oracle import fp64 as X
 from oracle import kernel_refs as K
 from oracle import step_ref as S
 from oracle import vilbert_ref as R
+import support
 
 EXACT = 1e-12
 E2E_TOL = {"fp16": 1e-2, "bf16": 3.5e-2}    # tests/test_gpu_model.py: fp16 max abs, bf16 max abs / max(1, logit std)
-
-
-def _tiny_inputs(oracle, B, Tin, V, seed, pad=0):
-    inp = list(R.make_inputs(B, Tin, V, seed=seed, vocab_size=oracle.config.vocab_size, pad_regions=pad))
-    inp[1] = inp[1][..., :oracle.config.v_feature_size].contiguous()
-    return inp
 
 
 def _oracle_run(oracle64, inp):
@@ -68,7 +63,7 @@ def _check_restatement(oracle, inp, tag):
 
 @pytest.mark.parametrize("B,Tin,V,pad", [(3, 16, 10, 3), (4, 37, 101, 7), (1, 3, 1, 0), (5, 70, 66, 2)])
 def test_restatement_tiny(tiny_oracle, B, Tin, V, pad):
-    _check_restatement(tiny_oracle, _tiny_inputs(tiny_oracle, B, Tin, V, 900 + B, pad), f"tiny_B{B}_T{Tin}_V{V}")
+    _check_restatement(tiny_oracle, support.tiny_inputs(tiny_oracle, B, Tin, V, 900 + B, pad), f"tiny_B{B}_T{Tin}_V{V}")
 
 
 def test_restatement_full(full_oracle):
@@ -157,7 +152,7 @@ def catalog(full_oracle):
 
 @pytest.fixture(scope="module")
 def end_to_end(tiny_oracle):
-    inp = _tiny_inputs(tiny_oracle, 4, 37, 101, seed=905, pad=7)
+    inp = support.tiny_inputs(tiny_oracle, 4, 37, 101, seed=905, pad=7)
     tm, vm = _masks(inp)
     cache = {}
 
