@@ -1,6 +1,7 @@
 """Plain references for the op-level kernel tests (tests/test_gpu_kernel_parity.py): the exact 16-bit conversions the kernels apply,
 the fp16 hi / lo split of the fp32-parity mode, a float32 restatement of the detector-output input builder in the region-pack
-kernel's order, and an emulation of the tensor-core attention's rounding points.  CPU only; checked by tests/test_kernel_refs.py."""
+kernel's order, fp64 attention with its probabilities, key masks at the attention kernels' block edges, and an emulation of the
+tensor-core attention's rounding points.  CPU only; checked by tests/test_kernel_refs.py."""
 from __future__ import annotations
 
 import math
@@ -228,8 +229,9 @@ def operand_rows(feat: np.ndarray, loc: np.ndarray, Kp: int) -> np.ndarray:
 
 
 # ---------------------------------------------------------------------------------------------------------------- attention
-def attention_fp64(q, k, v, mask_add, heads):
-    """softmax(Q K^T / sqrt(d) + mask) V in fp64; q [B, Lq, H], k / v [B, Lk, H], mask_add [B, Lk] -> [B, Lq, H] fp64."""
+def attention_probs_fp64(q, k, v, mask_add, heads):
+    """softmax(Q K^T / sqrt(d) + mask) and its product with V, in fp64; q [B, Lq, H], k / v [B, Lk, H], mask_add [B, Lk] ->
+    (probabilities [B, heads, Lq, Lk], context [B, Lq, H])."""
     B, Lq, H = q.shape
     Lk = k.shape[1]
     d = H // heads
@@ -237,7 +239,92 @@ def attention_fp64(q, k, v, mask_add, heads):
     kh = k.double().reshape(B, Lk, heads, d).permute(0, 2, 1, 3)
     vh = v.double().reshape(B, Lk, heads, d).permute(0, 2, 1, 3)
     s = qh @ kh.transpose(-1, -2) / math.sqrt(d) + mask_add.double()[:, None, None, :]
-    return (torch.softmax(s, dim=-1) @ vh).permute(0, 2, 1, 3).reshape(B, Lq, H)
+    p = torch.softmax(s, dim=-1)
+    return p, (p @ vh).permute(0, 2, 1, 3).reshape(B, Lq, H)
+
+
+def attention_fp64(q, k, v, mask_add, heads):
+    """softmax(Q K^T / sqrt(d) + mask) V in fp64; q [B, Lq, H], k / v [B, Lk, H], mask_add [B, Lk] -> [B, Lq, H] fp64."""
+    return attention_probs_fp64(q, k, v, mask_add, heads)[1]
+
+
+# Key masks at the places the attention kernels skip or predicate work (tests/test_gpu_attention_edges.py): the 64-key blocks of the
+# online softmax, the 16-key padding of the staged tiles, the 32-key chunks of the fp32 kernel, the key pairs of one mma column.
+# A pattern is "kind" or "kind@position"; positions past the sample's length clamp to it.
+MASKED = -10000.0               # the additive mask of a masked key (BERT's extended attention mask)
+EDGE_MASKS = ("all_real", "key0_masked",
+              "single@0", "single@last", "single@63", "single@64", "single@65",       # one real key
+              "masked_below@63", "masked_below@64", "masked_below@65",                # first block masked, later keys real
+              "masked_block@64", "masked_block@192",                                  # one middle block masked
+              "straddle",                                                             # keys n - 1 and n masked at every n = 16 i
+              "real_below@15", "real_below@17", "real_below@31", "real_below@33",     # real prefix ending one key either side of a
+              "real_below@63", "real_below@65", "real_below@127", "real_below@129",   # 16 / 32 / 64 boundary
+              "all_masked")
+
+
+def edge_mask(pattern: str, L: int) -> torch.Tensor:
+    """The additive key mask [L] (fp32, 0 or MASKED) of one EDGE_MASKS pattern."""
+    kind, _, at = pattern.partition("@")
+    m = torch.zeros(L)
+    if kind == "all_real":
+        pass
+    elif kind == "all_masked":
+        m[:] = MASKED
+    elif kind == "key0_masked":
+        m[0] = MASKED
+    elif kind == "single":
+        m[:] = MASKED
+        m[L - 1 if at == "last" else min(int(at), L - 1)] = 0.0
+    elif kind == "masked_below":
+        m[:int(at)] = MASKED
+    elif kind == "masked_block":
+        m[int(at):int(at) + 64] = MASKED
+    elif kind == "straddle":
+        for n in range(16, L, 16):
+            m[n - 1:n + 1] = MASKED
+    elif kind == "real_below":
+        m[int(at):] = MASKED
+    else:
+        raise ValueError(pattern)
+    return m
+
+
+# A masked score is s - 10000 (fp32 kernel, natural log) or s log2(e) - 14427 (tensor-core kernels, log2 domain), rounded to fp32
+# where the ulp is 2^-10: each masked key's exponent carries up to 2^-11 of error.  Only rows with no real key give masked keys any
+# weight; there that error is real (an fp32 PyTorch forward has it too) and comes on top of each kernel's rounding floor.
+MASKED_SCORE_ERR = {"f32": 2.0 ** -11, "tc": 2.0 ** -11 * math.log(2.0)}     # natural-log units
+
+
+def masked_score_slack(p, masked, v, ctx, heads, err):
+    """Context error allowed for the rounding of masked scores, per element [B, Lq, H]: each weight p_j of a masked key is off by a
+    factor exp(delta_j), |delta_j| <= err, so to first order the context moves by sum_j p_j (delta_j - mean delta) (v_j - c), at most
+    2 err sum_j p_j |v_j - c| <= 2 err sqrt(sum_j p_j (v_j - c)^2) (Cauchy-Schwarz, sum_j p_j <= 1), summed over masked keys.  p: fp64
+    probabilities [B, heads, Lq, Lk]; masked [B, Lk] bool; v [B, Lk, H]; ctx: the fp64 context [B, Lq, H].  Zero for rows with a
+    real key (their masked weights underflow to 0 in fp64)."""
+    B, Lq, H = ctx.shape
+    Lk = v.shape[1]
+    d = H // heads
+    pm = p * masked.double()[:, None, None, :]
+    vh = v.double().reshape(B, Lk, heads, d).permute(0, 2, 1, 3)
+    ch = ctx.double().reshape(B, Lq, heads, d).permute(0, 2, 1, 3)
+    var = pm @ (vh * vh) - 2.0 * ch * (pm @ vh) + ch * ch * pm.sum(-1, keepdim=True)
+    return (2.0 * err * var.clamp(min=0.0).sqrt()).permute(0, 2, 1, 3).reshape(B, Lq, H)
+
+
+def single_real_key(mask: torch.Tensor) -> int | None:
+    """The index of the only real key of a mask [L], or None when it has none or several."""
+    real = (mask == 0).nonzero().flatten()
+    return int(real[0]) if real.numel() == 1 else None
+
+
+def grid_qk(rows: int, cols: int, amp: float, generator: torch.Generator) -> torch.Tensor:
+    """[rows, cols] fp32 multiples of 1/4 in [-amp, amp], amp <= 8: Q elements at amp <= 8, K elements at amp = 1.  Each product q k
+    is then a multiple of 2^-4 of magnitude <= 8, and every partial sum of a head's dot product (d <= 128) stays below 2^10 = 2^14
+    units, so a score q . k is exact in fp32 in any order of accumulation; the values themselves are exact in fp16 and bf16 (at most
+    6 significant bits).  Scores have a standard deviation of about amp / 3."""
+    assert amp <= 8.0
+    n = int(amp * 4)
+    return torch.randint(-n, n + 1, (rows, cols), generator=generator, device=generator.device).float() / 4.0
 
 
 def attention_emulated(q, k, v, mask_add, heads, f16: bool):

@@ -259,3 +259,95 @@ def test_attention_rounding_floor(L, d):
         ref = R.attention_fp64(q, k, v, mask, heads)
         err = ((R.attention_emulated(q, k, v, mask, heads, f16) - ref).abs() / ref.abs().clamp(min=1.0)).max().item()
         assert err < bound / 2, (f16, err)
+
+
+def _edge_masks(L):
+    return torch.stack([R.edge_mask(p, L) for p in R.EDGE_MASKS])
+
+
+def test_attention_probs_fp64_matches_softmax():
+    """attention_probs_fp64 against an independent fp64 restatement (per-head scores, torch.softmax, P V as a sum over keys), at every
+    edge mask: probabilities and context to fp64 rounding, rows summing to 1, and attention_fp64 returning the same context."""
+    heads, d, Lq, Lk = 2, 64, 5, 130
+    H = heads * d
+    g = torch.Generator().manual_seed(11)
+    mask = _edge_masks(Lk)
+    B = mask.shape[0]
+    q, k, v = (torch.randn(B, n, H, generator=g, dtype=torch.float64) for n in (Lq, Lk, Lk))
+    p, ctx = R.attention_probs_fp64(q, k, v, mask, heads)
+    assert p.shape == (B, heads, Lq, Lk) and ctx.shape == (B, Lq, H) and p.dtype == ctx.dtype == torch.float64
+    for h in range(heads):
+        c = slice(h * d, (h + 1) * d)
+        s = torch.einsum("bid,bjd->bij", q[..., c], k[..., c]) / d ** 0.5 + mask.double()[:, None, :]
+        ph = torch.softmax(s, dim=-1)
+        assert torch.allclose(p[:, h], ph, rtol=0, atol=1e-15)
+        assert torch.allclose(ctx[..., c], (ph[..., None] * v[:, None, :, c]).sum(2), rtol=0, atol=1e-13)
+    assert torch.allclose(p.sum(-1), torch.ones(B, heads, Lq, dtype=torch.float64), rtol=0, atol=1e-14)
+    assert torch.equal(R.attention_fp64(q, k, v, mask, heads), ctx)
+
+
+def test_edge_masks():
+    """The edge mask builder: one real key where the pattern puts it (clamped to the length), masks exactly 0 or -10000, and the
+    straddle pattern masking the two keys around every multiple of 16."""
+    for L in (1, 2, 16, 17, 64, 65, 129, 512):
+        m = _edge_masks(L)
+        assert ((m == 0) | (m == R.MASKED)).all()
+        for p, row in zip(R.EDGE_MASKS, m):
+            if p.startswith("single@"):
+                at = p.split("@")[1]
+                assert R.single_real_key(row) == (L - 1 if at == "last" else min(int(at), L - 1)), (p, L)
+        assert (m[R.EDGE_MASKS.index("all_masked")] == R.MASKED).all() and (m[R.EDGE_MASKS.index("all_real")] == 0).all()
+    s = R.edge_mask("straddle", 70)
+    assert (s == R.MASKED).nonzero().flatten().tolist() == [15, 16, 31, 32, 47, 48, 63, 64]
+    assert (R.edge_mask("real_below@17", 40) == 0).nonzero().flatten().tolist() == list(range(17))
+
+
+def test_fully_masked_row_is_unmasked_softmax():
+    """Every key masked: softmax(s - 10000) is softmax(s), so the fp64 reference of a fully masked sample is its unmasked one."""
+    heads, d, L = 2, 64, 67
+    H = heads * d
+    g = torch.Generator().manual_seed(12)
+    q, k, v = (torch.randn(1, L, H, generator=g) * 2 for _ in range(3))
+    pm, cm = R.attention_probs_fp64(q, k, v, R.edge_mask("all_masked", L)[None], heads)
+    pr, cr = R.attention_probs_fp64(q, k, v, R.edge_mask("all_real", L)[None], heads)
+    assert torch.allclose(pm, pr, rtol=1e-10, atol=0) and torch.allclose(cm, cr, rtol=0, atol=1e-10)
+
+
+@pytest.mark.parametrize("L,d", [(1, 64), (2, 128), (15, 64), (17, 128), (33, 64), (63, 128), (64, 64)])
+def test_attention_rounding_floor_edge_masks(L, d):
+    """test_attention_rounding_floor at every edge mask (one sample per pattern): the emulated rounding points stay within half the
+    GPU attention bound of fp64, once the fully masked samples are allowed the rounding of their masked scores
+    (masked_score_slack).  Without that allowance they exceed it (7.9e-4 at L = 2, fp16), so the slack is needed, and it is no
+    licence for the others: the samples with a real key stay within half the bound on their own."""
+    heads = 2
+    H = heads * d
+    g = torch.Generator().manual_seed(L * 3 + d)
+    mask = _edge_masks(L)
+    B = mask.shape[0]
+    for f16, bound in ((False, 1.2e-2), (True, 1.5e-3)):
+        dt = torch.float16 if f16 else torch.bfloat16
+        qkv = torch.randn(B, L, 3 * H, generator=g).to(dt)
+        q, k, v = qkv[..., :H], qkv[..., H:2 * H], qkv[..., 2 * H:]
+        p, ref = R.attention_probs_fp64(q, k, v, mask, heads)
+        slack = R.masked_score_slack(p, mask == R.MASKED, v, ref, heads, R.MASKED_SCORE_ERR["tc"])
+        assert not slack[~(mask == R.MASKED).all(1)].any()
+        err = (R.attention_emulated(q, k, v, mask, heads, f16) - ref).abs()
+        assert (err <= bound / 2 * ref.abs().clamp(min=1.0) + slack).all(), (f16, (err - slack).max().item())
+
+
+@pytest.mark.parametrize("d", [64, 128])
+def test_grid_qk_scores_exact(d):
+    """The fp32 attention test's Q / K grid: fp32 scores accumulated key by key in the kernel's order (one fmaf per element) and in
+    reverse equal the fp64 ones, at the largest Q amplitude and at the all-extreme corner; the values survive fp16 and bf16."""
+    g = torch.Generator().manual_seed(d)
+    q, k = R.grid_qk(64, d, 8.0, g), R.grid_qk(256, d, 1.0, g)
+    q[0], k[0] = 8.0, -1.0
+    exact = q.double() @ k.double().t()
+    fwd, bwd = torch.zeros(64, 256), torch.zeros(64, 256)
+    for i in range(d):
+        fwd = torch.addcmul(fwd, q[:, i:i + 1], k[:, i][None])
+        bwd = torch.addcmul(bwd, q[:, d - 1 - i:d - i], k[:, d - 1 - i][None])
+    assert torch.equal(fwd.double(), exact) and torch.equal(bwd.double(), exact)
+    assert exact[0, 0].item() == -8.0 * d
+    for dt in (torch.float16, torch.bfloat16):
+        assert torch.equal(q.to(dt).float(), q) and torch.equal(k.to(dt).float(), k)
