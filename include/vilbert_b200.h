@@ -405,6 +405,25 @@ int vb200_attention_layout_packed(vb200_handle h, int32_t batch, const int32_t* 
                                   const int32_t* n_regions /* HOST [batch] V_b */, int32_t max_entries, int32_t* n_entries,
                                   int32_t* dims, int64_t* offsets, int64_t* total_floats);
 
+/* ---- Head masks: the two packed forwards with a per-sample, per-head gate on every attention head (pytorch_transformers'
+ * head_mask).  head_mask is DEVICE fp32 [batch, E, H] with E = vb200_model_dim "head_mask_entries" (the full list of
+ * vb200_attention_selection in execution order, each connection layer's text-query then image-query direction: 30 for 12/6/6) and
+ * H = "head_mask_heads" (the configuration's largest head count, 12); slots past an entry's own head count are ignored.  Sample b's
+ * head h context rows at entry e are multiplied in fp32 by head_mask[b][e][h] before the 16-bit store -- attention_probs * head_mask
+ * applied after the P V product -- so 1.0 gives the ungated bits exactly and 0 an exact zero context.  Packed attention maps
+ * (VB200_OUT_ATTENTION_PACKED) report g * p, and under the head mean the mean of the gated maps.  The gate also holds in the pruned
+ * last layers.  The mask is copied into the plan's gate table with one device-to-device copy on cuda_stream ahead of the forward, so
+ * back-to-back calls may pass different masks without synchronising.  Gate values are device memory and are not checked.
+ * A gated call runs a plan of its own (the PACKED plan's key plus gating), which launches the same kernels as the ungated plan and no
+ * more; ungated calls keep their plans.  Everything else -- arguments, outputs, rejections -- follows vb200_forward_packed /
+ * vb200_forward_regions_packed; a NULL head_mask is VB200_ERR_INVALID as well, and split_fp32 engines reject both calls as they
+ * reject every packed call.  Dense, cached and retrieval forwards have no head mask. */
+int vb200_forward_packed_gated(vb200_handle h, const vb200_packed_inputs* in, const float* head_mask /* DEVICE [batch, E, H] */,
+                               const vb200_outputs* out, uint32_t select, int32_t slot, void* cuda_stream);
+int vb200_forward_regions_packed_gated(vb200_handle h, const vb200_packed_region_inputs* in,
+                                       const float* head_mask /* DEVICE [batch, E, H] */, const vb200_outputs* out, uint32_t select,
+                                       int32_t slot, void* cuda_stream);
+
 /* ---- Caption-image retrieval with reuse (SURVEY.md section 8e; reference semantics worker.py:278-284, 359).  Everything ahead of
  * the first connection layer depends on the caption alone or on the image alone: encode each caption / image ONCE, then score
  * pairs from the cached states.  Same kernels on the same rows as the full forward: scores are bit-identical to vb200_forward.
@@ -611,7 +630,8 @@ typedef struct {
 } vb200_ablation_message;
 
 typedef struct {
-    int32_t message, kind, unit;      /* kind 0: the unablated input (unit -1); 1: masked position `unit`; 2: dropped box `unit` */
+    int32_t message, kind, unit;      /* kind 0: the unablated input (unit -1); 1: masked position `unit`; 2: dropped box `unit`;
+                                         3 (head ablation): gate `unit` = entry * head_mask_heads + head at 0 */
     int32_t samples;                  /* forward samples this variant runs */
     int64_t offset;                   /* its segment: floats [offset, offset + length) of variant_logits */
     int32_t length;
@@ -624,6 +644,33 @@ int vb200_message_ablation_layout(vb200_handle h, int32_t batch, const int32_t* 
 int vb200_message_ablation(vb200_handle h, const vb200_packed_region_inputs* in, const vb200_ablation_message* msgs /* HOST [n_msgs] */,
                            int32_t n_msgs, int64_t mask_token, float* variant_logits, vb200_ablation_score* scores, int32_t slot,
                            void* cuda_stream);
+
+/* ---- Head ablation (Michel et al. 2019): which attention heads an answer depends on.  Messages follow vb200_message_ablation (every
+ * decode family, the same images per message and answer rule) with an entry range instead of token and box ranges.  A message's
+ * variants, in order: the unablated input (kind 0, unit -1), then for each entry e in [entry_begin, entry_end) (the head mask's entry
+ * order, see vb200_forward_packed_gated) and each of that entry's heads h, the message's samples unablated with gate (e, h) at 0 and
+ * every other gate at 1 (kind 3, unit e * head_mask_heads + h).  Every sample of the message runs in each variant: an NLVR2 variant is
+ * a pair on an even sample, a retrieval variant all K images.  The variants are built on the device (text and regions as message
+ * ablation builds its unablated input, one kernel writing each sample's gate row) and run as one forward of the gated PACKED plan,
+ * rounded up to a multiple of 64 samples with fillers (gate 1), at most VB200_ABLATION_MAX_VARIANTS samples per call.  Segments and
+ * scores follow vb200_message_ablation: every segment is bit-identical to the same floats of vb200_forward_regions_packed_gated run on
+ * the variant's input and gate row alone.  vb200_head_ablation_layout owns the variant order, as vb200_message_ablation_layout does.
+ * Every head of one message: 1 + 288 = 289 forward samples for 12/6/6 (578 for NLVR2).
+ * VB200_ERR_INVALID, with nothing enqueued, for every rejection of vb200_message_ablation that applies (mask_token aside) and an
+ * entry range reversed or outside [0, head_mask_entries]. */
+typedef struct {
+    int32_t family;                   /* VB200_DECODE_* */
+    int32_t image_begin, n_images;    /* the message's images in the batch, as vb200_ablation_message */
+    int32_t answer;                   /* attributed index, -1: the unablated top-1 */
+    int32_t entry_begin, entry_end;   /* remove each head of entries [entry_begin, entry_end), one at a time */
+} vb200_head_ablation_message;
+
+int vb200_head_ablation_layout(vb200_handle h, int32_t batch, const int32_t* n_tokens /* HOST [batch] */,
+                               const int32_t* n_boxes /* HOST [batch] */, const vb200_head_ablation_message* msgs /* HOST [n_msgs] */,
+                               int32_t n_msgs, vb200_ablation_variant* variants /* HOST, NULL: counts only */, int64_t* n_variants,
+                               int64_t* n_floats, int64_t* n_samples);
+int vb200_head_ablation(vb200_handle h, const vb200_packed_region_inputs* in, const vb200_head_ablation_message* msgs /* HOST [n_msgs] */,
+                        int32_t n_msgs, float* variant_logits, vb200_ablation_score* scores, int32_t slot, void* cuda_stream);
 
 /* ---- Detector-region selection: the feature extraction step of the reference worker (worker.py:123-176) on the detector's raw heads,
  * for every image of a batch in one call, written straight into the packed box_features / boxes that vb200_forward_regions_packed reads.

@@ -124,6 +124,13 @@ class AblationScore(C.Structure):
     _fields_ = [("answer", C.c_int32), ("prob", C.c_float), ("top1", C.c_int32), ("top1_prob", C.c_float)]
 
 
+class HeadAblationMessage(C.Structure):
+    """vb200_head_ablation_message: one answer of any decode family by its images, the attributed index (-1: the unablated top-1)
+    and the attention entries whose heads are removed one at a time."""
+    _fields_ = [("family", C.c_int32), ("image_begin", C.c_int32), ("n_images", C.c_int32), ("answer", C.c_int32),
+                ("entry_begin", C.c_int32), ("entry_end", C.c_int32)]
+
+
 class AblationMessage(C.Structure):
     """vb200_ablation_message: one answer of any decode family by its images, the attributed index in its segment (-1: the
     unablated top-1) and the token and box ranges ablated one unit at a time (boxes numbered across the message's images)."""
@@ -195,7 +202,8 @@ EXPORTS = ["vb200_abi_version", "vb200_create", "vb200_destroy", "vb200_last_err
            "vb200_linear_product", "vb200_text_embed", "vb200_image_pack", "vb200_region_pack", "vb200_rowdot", "vb200_gather_state",
            "vb200_gather_packed_state", "vb200_decode_answers", "vb200_decode_answers_host", "vb200_select_regions",
            "vb200_pretraining_heads", "vb200_create_pretraining", "vb200_pretraining_objectives", "vb200_answer_ablation",
-           "vb200_message_ablation_layout", "vb200_message_ablation"]
+           "vb200_message_ablation_layout", "vb200_message_ablation", "vb200_forward_packed_gated", "vb200_forward_regions_packed_gated",
+           "vb200_head_ablation_layout", "vb200_head_ablation"]
 
 _lib = None
 
@@ -245,6 +253,8 @@ def load():
     lib.vb200_forward_regions.argtypes = [vp, C.POINTER(RegionInputs), C.POINTER(Outputs), u32, i32, vp]
     lib.vb200_forward_packed.argtypes = [vp, C.POINTER(PackedInputs), C.POINTER(Outputs), u32, i32, vp]
     lib.vb200_forward_regions_packed.argtypes = [vp, C.POINTER(PackedRegionInputs), C.POINTER(Outputs), u32, i32, vp]
+    lib.vb200_forward_packed_gated.argtypes = [vp, C.POINTER(PackedInputs), vp, C.POINTER(Outputs), u32, i32, vp]
+    lib.vb200_forward_regions_packed_gated.argtypes = [vp, C.POINTER(PackedRegionInputs), vp, C.POINTER(Outputs), u32, i32, vp]
     lib.vb200_linear_rows.argtypes = [vp, i64, vp, i64, vp, i32, vp, i64, vp, i64, i64, i64, i64, i32, i32, vp, vp]
     lib.vb200_encode_text.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp]
     lib.vb200_encode_image.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp, vp, vp]
@@ -283,6 +293,9 @@ def load():
     lib.vb200_message_ablation_layout.argtypes = [vp, i32, vp, vp, C.POINTER(AblationMessage), i32, vp, C.POINTER(C.c_int64),
                                                   C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     lib.vb200_message_ablation.argtypes = [vp, C.POINTER(PackedRegionInputs), C.POINTER(AblationMessage), i32, i64, vp, vp, i32, vp]
+    lib.vb200_head_ablation_layout.argtypes = [vp, i32, vp, vp, C.POINTER(HeadAblationMessage), i32, vp, C.POINTER(C.c_int64),
+                                               C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
+    lib.vb200_head_ablation.argtypes = [vp, C.POINTER(PackedRegionInputs), C.POINTER(HeadAblationMessage), i32, vp, vp, i32, vp]
     for name in EXPORTS:
         if name not in ("vb200_last_error",):
             getattr(lib, name).restype = C.c_int

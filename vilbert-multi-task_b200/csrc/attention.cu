@@ -79,7 +79,7 @@ __device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], 
 template <int D, int OW, bool F16>
 __device__ __forceinline__ void attend_tile(const uint16_t* Qs, const uint16_t* Ks, const uint16_t* Vs, int r0, int nq,
                                             int nk, const float* mask_l2, float scale_l2, uint16_t* out, int ld_out,
-                                            int lane, int oc0) {
+                                            int lane, int oc0, const float& gate) {
     constexpr int kStride = AttnTile<D>::kStride;
     constexpr int kKSteps = D / 16;         // k-steps of Q K^T
     constexpr int kONTiles = OW / 8;        // 8-wide output column tiles of this work item
@@ -167,7 +167,7 @@ __device__ __forceinline__ void attend_tile(const uint16_t* Qs, const uint16_t* 
     }
     l0 += __shfl_xor_sync(0xffffffffu, l0, 1); l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
     l1 += __shfl_xor_sync(0xffffffffu, l1, 1); l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
-    const float i0 = 1.0f / l0, i1 = 1.0f / l1;
+    const float i0 = (1.0f / l0) * gate, i1 = (1.0f / l1) * gate;   // the head gate: 1 gives the ungated bits (x * 1.0f is exact)
     const int row0 = r0 + g, row1 = r0 + g + 8;
 #pragma unroll
     for (int nt = 0; nt < kONTiles; ++nt) {
@@ -183,7 +183,7 @@ __device__ __forceinline__ void attend_tile(const uint16_t* Qs, const uint16_t* 
 template <int D, bool F16>
 __device__ __forceinline__ void attend_tile_short(const uint16_t* Qs, const uint16_t* Ks, const uint16_t* Vs, int r0, int nq,
                                                   int nk, const float* mask_l2, float scale_l2, uint16_t* out, int ld_out,
-                                                  int lane) {
+                                                  int lane, const float& gate) {
     constexpr int kStride = AttnTile<D>::kStride;
     constexpr int kKSteps = D / 16;
     const int g = lane >> 2, tq = lane & 3;
@@ -243,7 +243,7 @@ __device__ __forceinline__ void attend_tile_short(const uint16_t* Qs, const uint
     }
     l0 += __shfl_xor_sync(0xffffffffu, l0, 1); l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
     l1 += __shfl_xor_sync(0xffffffffu, l1, 1); l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
-    const float i0 = 1.0f / l0, i1 = 1.0f / l1;
+    const float i0 = (1.0f / l0) * gate, i1 = (1.0f / l1) * gate;   // the head gate: 1 gives the ungated bits (x * 1.0f is exact)
     const int row0 = r0 + g, row1 = r0 + g + 8;
 #pragma unroll
     for (int oc0 = 0; oc0 < D; oc0 += 64) {                       // 64 output columns at a time: 32 accumulator registers
@@ -274,7 +274,8 @@ __device__ __forceinline__ void attend_tile_short(const uint16_t* Qs, const uint
 template <int D, bool F16>
 __global__ void __launch_bounds__(256, 2)     // <= 128 registers: 5 CTAs of 3-4 warps per SM -> one wave at batch 64
 self_attention_kernel(const uint16_t* __restrict__ qkv, int ld_qkv, int hidden, const float* __restrict__ key_mask_add,
-                      uint16_t* __restrict__ ctx, int ld_ctx, int L_cap, float scale_l2, int pdl, const int* __restrict__ offs) {
+                      uint16_t* __restrict__ ctx, int ld_ctx, int L_cap, float scale_l2, int pdl, const int* __restrict__ offs,
+                      HeadGate gate) {
     extern __shared__ __align__(16) uint8_t smem_attn[];
     constexpr int kStride = AttnTile<D>::kStride;
     const int h = blockIdx.x, b = blockIdx.y;
@@ -296,6 +297,8 @@ self_attention_kernel(const uint16_t* __restrict__ qkv, int ld_qkv, int hidden, 
     load_tile<D>(Ks, base + hidden, L, Lp, ld_qkv);
     load_tile<D>(Vs, base + 2 * hidden, L, Lp, ld_qkv);
     for (int j = threadIdx.x; j < L; j += blockDim.x) mask_s[j] = key_mask_add[r0 + j] * kLog2e;
+    __shared__ float gate_s[1];              // read once more per warp at the store: no register holds it through the math
+    if (threadIdx.x == 0) gate_s[0] = gate.at(b, h);
     cp_async_wait_all();
     __syncthreads();
     if (pdl) pdl_launch_dependents();       // tiles are staged: the next kernel's prologue may overlap the math
@@ -303,11 +306,11 @@ self_attention_kernel(const uint16_t* __restrict__ qkv, int ld_qkv, int hidden, 
     constexpr int kSplit = D / 64, kOW = D / kSplit;             // work item = (16-row tile, 64-column slice of the head)
     if (L <= kKeyBlock) {                                        // one key block: S and the softmax once per row tile
         for (int t = warp; t * 16 < L; t += nwarps)
-            attend_tile_short<D, F16>(Qs, Ks, Vs, t * 16, L, L, mask_s, scale_l2, outp, ld_ctx, lane);
+            attend_tile_short<D, F16>(Qs, Ks, Vs, t * 16, L, L, mask_s, scale_l2, outp, ld_ctx, lane, gate_s[0]);
         return;
     }
     for (int w = warp; (w / kSplit) * 16 < L; w += nwarps)
-        attend_tile<D, kOW, F16>(Qs, Ks, Vs, (w / kSplit) * 16, L, L, mask_s, scale_l2, outp, ld_ctx, lane, (w % kSplit) * kOW);
+        attend_tile<D, kOW, F16>(Qs, Ks, Vs, (w / kSplit) * 16, L, L, mask_s, scale_l2, outp, ld_ctx, lane, (w % kSplit) * kOW, gate_s[0]);
 }
 
 template <int D, bool F16>
@@ -315,7 +318,7 @@ __global__ void __launch_bounds__(256, 2)
 co_attention_kernel(const uint16_t* __restrict__ qkv_img, int ld_img, const uint16_t* __restrict__ qkv_txt, int ld_txt,
                     int hidden, const float* __restrict__ img_mask_add, const float* __restrict__ txt_mask_add,
                     uint16_t* __restrict__ ctx_txt, int ld_ctx_txt, uint16_t* __restrict__ ctx_img, int ld_ctx_img, int T_cap,
-                    int V_cap, float scale_l2, int pdl, const int* __restrict__ offs_t, const int* __restrict__ offs_v) {
+                    int V_cap, float scale_l2, int pdl, const int* __restrict__ offs_t, const int* __restrict__ offs_v, HeadGate gate) {
     // Two phases over ONE set of Q/K/V buffers sized for the longer sequence (39 KB at T=31/V=36 instead of 65 KB for all
     // six tiles: 5 CTAs per SM, so the 512 (sample, head) CTAs of a batch-64 layer are resident in a single wave).
     //   phase 1: text queries (Q2) over image keys/values (K1, V1) -> context for the text stream
@@ -344,16 +347,18 @@ co_attention_kernel(const uint16_t* __restrict__ qkv_img, int ld_img, const uint
     load_tile<D>(Vs, bi + 2 * hidden, V, Vp, ld_img);            // V1
     for (int j = threadIdx.x; j < V; j += blockDim.x) mask_img[j] = img_mask_add[v0 + j] * kLog2e;
     for (int j = threadIdx.x; j < T; j += blockDim.x) mask_txt[j] = txt_mask_add[t0 + j] * kLog2e;
+    __shared__ float gate_s[2];              // per direction, as in self_attention_kernel
+    if (threadIdx.x < 2) gate_s[threadIdx.x] = gate.at(b, h, threadIdx.x);
     cp_async_wait_all();
     __syncthreads();
     uint16_t* out_t = ctx_txt + static_cast<size_t>(t0) * ld_ctx_txt + h * D;
     constexpr int kSplit = D / 64, kOW = D / kSplit;
     if (V <= kKeyBlock) {
         for (int t = warp; t * 16 < T; t += nwarps)
-            attend_tile_short<D, F16>(Qs, Ks, Vs, t * 16, T, V, mask_img, scale_l2, out_t, ld_ctx_txt, lane);
+            attend_tile_short<D, F16>(Qs, Ks, Vs, t * 16, T, V, mask_img, scale_l2, out_t, ld_ctx_txt, lane, gate_s[0]);
     } else {
         for (int w = warp; (w / kSplit) * 16 < T; w += nwarps)
-            attend_tile<D, kOW, F16>(Qs, Ks, Vs, (w / kSplit) * 16, T, V, mask_img, scale_l2, out_t, ld_ctx_txt, lane, (w % kSplit) * kOW);
+            attend_tile<D, kOW, F16>(Qs, Ks, Vs, (w / kSplit) * 16, T, V, mask_img, scale_l2, out_t, ld_ctx_txt, lane, (w % kSplit) * kOW, gate_s[0]);
     }
     __syncthreads();                                             // everyone is done reading phase-1 tiles
     load_tile<D>(Qs, bi, V, Vp, ld_img);                         // Q1
@@ -365,17 +370,17 @@ co_attention_kernel(const uint16_t* __restrict__ qkv_img, int ld_img, const uint
     uint16_t* out_v = ctx_img + static_cast<size_t>(v0) * ld_ctx_img + h * D;
     if (T <= kKeyBlock) {
         for (int t = warp; t * 16 < V; t += nwarps)
-            attend_tile_short<D, F16>(Qs, Ks, Vs, t * 16, V, T, mask_txt, scale_l2, out_v, ld_ctx_img, lane);
+            attend_tile_short<D, F16>(Qs, Ks, Vs, t * 16, V, T, mask_txt, scale_l2, out_v, ld_ctx_img, lane, gate_s[1]);
     } else {
         for (int w = warp; (w / kSplit) * 16 < V; w += nwarps)
-            attend_tile<D, kOW, F16>(Qs, Ks, Vs, (w / kSplit) * 16, V, T, mask_txt, scale_l2, out_v, ld_ctx_img, lane, (w % kSplit) * kOW);
+            attend_tile<D, kOW, F16>(Qs, Ks, Vs, (w / kSplit) * 16, V, T, mask_txt, scale_l2, out_v, ld_ctx_img, lane, (w % kSplit) * kOW, gate_s[1]);
     }
 }
 
 template <int D, bool F16>
 static cudaError_t launch_self(const __nv_bfloat16* qkv, int ld_qkv, int hidden, const float* key_mask_add,
                                __nv_bfloat16* ctx, int ld_ctx, int B, int L, int heads, int pdl, cudaStream_t st,
-                               const int* offs) {
+                               const int* offs, HeadGate gate) {
     const int Lp = pad16(L);
     const size_t smem = 3 * AttnTile<D>::bytes(Lp) + sizeof(float) * L;
     if (smem > 227 * 1024) return cudaErrorInvalidValue;
@@ -388,26 +393,26 @@ static cudaError_t launch_self(const __nv_bfloat16* qkv, int ld_qkv, int hidden,
     const float scale_l2 = kLog2e / sqrtf(static_cast<float>(D));
     return launch_ex(self_attention_kernel<D, F16>, dim3(heads, B), dim3(32 * nwarps), smem, pdl, st,
                      reinterpret_cast<const uint16_t*>(qkv), ld_qkv, hidden, key_mask_add, reinterpret_cast<uint16_t*>(ctx),
-                     ld_ctx, L, scale_l2, pdl, offs);
+                     ld_ctx, L, scale_l2, pdl, offs, gate);
 }
 
 cudaError_t launch_self_attention(const __nv_bfloat16* qkv, int ld_qkv, int hidden, const float* key_mask_add,
                                   __nv_bfloat16* ctx, int ld_ctx, int B, int L, int heads, int head_dim, int pdl,
-                                  int f16, cudaStream_t st, const int* offs) {
+                                  int f16, cudaStream_t st, const int* offs, HeadGate gate) {
     if (L < 1 || (head_dim != 64 && head_dim != 128) || (ld_qkv & 7) || (ld_ctx & 1) || (hidden & 7))
         return cudaErrorInvalidValue;
     if (head_dim == 64)
-        return f16 ? launch_self<64, true>(qkv, ld_qkv, hidden, key_mask_add, ctx, ld_ctx, B, L, heads, pdl, st, offs)
-                   : launch_self<64, false>(qkv, ld_qkv, hidden, key_mask_add, ctx, ld_ctx, B, L, heads, pdl, st, offs);
-    return f16 ? launch_self<128, true>(qkv, ld_qkv, hidden, key_mask_add, ctx, ld_ctx, B, L, heads, pdl, st, offs)
-               : launch_self<128, false>(qkv, ld_qkv, hidden, key_mask_add, ctx, ld_ctx, B, L, heads, pdl, st, offs);
+        return f16 ? launch_self<64, true>(qkv, ld_qkv, hidden, key_mask_add, ctx, ld_ctx, B, L, heads, pdl, st, offs, gate)
+                   : launch_self<64, false>(qkv, ld_qkv, hidden, key_mask_add, ctx, ld_ctx, B, L, heads, pdl, st, offs, gate);
+    return f16 ? launch_self<128, true>(qkv, ld_qkv, hidden, key_mask_add, ctx, ld_ctx, B, L, heads, pdl, st, offs, gate)
+               : launch_self<128, false>(qkv, ld_qkv, hidden, key_mask_add, ctx, ld_ctx, B, L, heads, pdl, st, offs, gate);
 }
 
 template <int D, bool F16>
 static cudaError_t launch_co(const __nv_bfloat16* qkv_img, int ld_img, const __nv_bfloat16* qkv_txt, int ld_txt, int hidden,
                              const float* img_mask_add, const float* txt_mask_add, __nv_bfloat16* ctx_txt, int ld_ctx_txt,
                              __nv_bfloat16* ctx_img, int ld_ctx_img, int B, int T, int V, int heads, int pdl,
-                             cudaStream_t st, const int* offs_t, const int* offs_v) {
+                             cudaStream_t st, const int* offs_t, const int* offs_v, HeadGate gate) {
     const int Tp = pad16(T), Vp = pad16(V);
     const int Lp = Tp > Vp ? Tp : Vp;
     const size_t smem = 3 * AttnTile<D>::bytes(Lp) + sizeof(float) * (T + V);
@@ -420,19 +425,19 @@ static cudaError_t launch_co(const __nv_bfloat16* qkv_img, int ld_img, const __n
     return launch_ex(co_attention_kernel<D, F16>, dim3(heads, B), dim3(32 * nwarps), smem, pdl, st,
                      reinterpret_cast<const uint16_t*>(qkv_img), ld_img, reinterpret_cast<const uint16_t*>(qkv_txt), ld_txt,
                      hidden, img_mask_add, txt_mask_add, reinterpret_cast<uint16_t*>(ctx_txt), ld_ctx_txt,
-                     reinterpret_cast<uint16_t*>(ctx_img), ld_ctx_img, T, V, scale_l2, pdl, offs_t, offs_v);
+                     reinterpret_cast<uint16_t*>(ctx_img), ld_ctx_img, T, V, scale_l2, pdl, offs_t, offs_v, gate);
 }
 
 cudaError_t launch_co_attention(const __nv_bfloat16* qkv_img, int ld_img, const __nv_bfloat16* qkv_txt, int ld_txt,
                                 int hidden, const float* img_mask_add, const float* txt_mask_add,
                                 __nv_bfloat16* ctx_txt, int ld_ctx_txt, __nv_bfloat16* ctx_img, int ld_ctx_img, int B,
                                 int T, int V, int heads, int head_dim, int pdl, int f16, cudaStream_t st,
-                                const int* offs_t, const int* offs_v) {
+                                const int* offs_t, const int* offs_v, HeadGate gate) {
     if (T < 1 || V < 1 || (head_dim != 64 && head_dim != 128) || (ld_img & 7) || (ld_txt & 7) || (hidden & 7) ||
         (ld_ctx_txt & 1) || (ld_ctx_img & 1))
         return cudaErrorInvalidValue;
 #define VB_CO(D, F) launch_co<D, F>(qkv_img, ld_img, qkv_txt, ld_txt, hidden, img_mask_add, txt_mask_add, ctx_txt, ld_ctx_txt, \
-                                    ctx_img, ld_ctx_img, B, T, V, heads, pdl, st, offs_t, offs_v)
+                                    ctx_img, ld_ctx_img, B, T, V, heads, pdl, st, offs_t, offs_v, gate)
     if (head_dim == 64) return f16 ? VB_CO(64, true) : VB_CO(64, false);
     return f16 ? VB_CO(128, true) : VB_CO(128, false);
 #undef VB_CO
@@ -536,7 +541,8 @@ __device__ __forceinline__ void stream_block(const uint32_t (&qa)[D / 16][4], fl
 template <int D, bool F16>
 __device__ __forceinline__ void stream_attend(const uint16_t* __restrict__ q, int ld_q, int nq, const uint16_t* __restrict__ k,
                                               const uint16_t* __restrict__ v, int ld_kv, int nk, const float* __restrict__ mask,
-                                              float scale_l2, uint16_t* __restrict__ out, int ld_out, int pdl) {
+                                              float scale_l2, uint16_t* __restrict__ out, int ld_out, int pdl, HeadGate gate,
+                                              int b, int h, int dir) {
     extern __shared__ __align__(16) uint8_t smem_attn[];
     constexpr int kStride = AttnTile<D>::kStride;
     constexpr int kTileElems = kStreamRows * kStride;
@@ -559,6 +565,8 @@ __device__ __forceinline__ void stream_attend(const uint16_t* __restrict__ q, in
         asm volatile("cp.async.commit_group;" ::: "memory");
     };
 
+    __shared__ float gate_s;                                     // as in self_attention_kernel
+    if (threadIdx.x == 0) gate_s = gate.at(b, h, dir);
     if (pdl) pdl_wait();
     load_tile<D>(Qs, q, nq, pad16(nq), ld_q);                    // rows [nq, pad16(nq)) zero-filled
     issue(0);                                                    // Q joins block 0's group
@@ -593,7 +601,7 @@ __device__ __forceinline__ void stream_attend(const uint16_t* __restrict__ q, in
     const int g = lane >> 2, tq = lane & 3;
     l0 += __shfl_xor_sync(0xffffffffu, l0, 1); l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
     l1 += __shfl_xor_sync(0xffffffffu, l1, 1); l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
-    const float i0 = 1.0f / l0, i1 = 1.0f / l1;
+    const float i0 = (1.0f / l0) * gate_s, i1 = (1.0f / l1) * gate_s;   // as in attend_tile
     const int row0 = r0 + g, row1 = r0 + g + 8;
 #pragma unroll
     for (int nt = 0; nt < kOW / 8; ++nt) {
@@ -607,14 +615,16 @@ __device__ __forceinline__ void stream_attend(const uint16_t* __restrict__ q, in
 template <int D, bool F16>
 __global__ void __launch_bounds__(256, 2)
 self_attention_stream_kernel(const uint16_t* __restrict__ qkv, int ld_qkv, int hidden, const float* __restrict__ key_mask_add,
-                             uint16_t* __restrict__ ctx, int ld_ctx, int L_cap, float scale_l2, int pdl, const int* __restrict__ offs) {
+                             uint16_t* __restrict__ ctx, int ld_ctx, int L_cap, float scale_l2, int pdl, const int* __restrict__ offs,
+                             HeadGate gate) {
     const int h = blockIdx.x, b = blockIdx.y, q0 = blockIdx.z * kStreamRows;
     const int r0 = offs ? offs[b] : b * L_cap;
     const int L = offs ? offs[b + 1] - r0 : L_cap;
     if (q0 >= L) return;                                         // a tile past this sample's length: no barrier reached yet
     const uint16_t* base = qkv + static_cast<size_t>(r0) * ld_qkv + h * D;
     stream_attend<D, F16>(base + static_cast<size_t>(q0) * ld_qkv, ld_qkv, min(kStreamRows, L - q0), base + hidden, base + 2 * hidden,
-                          ld_qkv, L, key_mask_add + r0, scale_l2, ctx + static_cast<size_t>(r0 + q0) * ld_ctx + h * D, ld_ctx, pdl);
+                          ld_qkv, L, key_mask_add + r0, scale_l2, ctx + static_cast<size_t>(r0 + q0) * ld_ctx + h * D, ld_ctx, pdl,
+                          gate, b, h, 0);
 }
 
 // grid (heads, B, ceil(T_cap / kStreamRows) + ceil(V_cap / kStreamRows)), D / 16 warps: blockIdx.z first walks the text-query
@@ -625,7 +635,8 @@ __global__ void __launch_bounds__(256, 2)
 co_attention_stream_kernel(const uint16_t* __restrict__ qkv_img, int ld_img, const uint16_t* __restrict__ qkv_txt, int ld_txt,
                            int hidden, const float* __restrict__ img_mask_add, const float* __restrict__ txt_mask_add,
                            uint16_t* __restrict__ ctx_txt, int ld_ctx_txt, uint16_t* __restrict__ ctx_img, int ld_ctx_img, int T_cap,
-                           int V_cap, float scale_l2, int pdl, const int* __restrict__ offs_t, const int* __restrict__ offs_v) {
+                           int V_cap, float scale_l2, int pdl, const int* __restrict__ offs_t, const int* __restrict__ offs_v,
+                           HeadGate gate) {
     const int h = blockIdx.x, b = blockIdx.y;
     const int t0 = offs_t ? offs_t[b] : b * T_cap, T = offs_t ? offs_t[b + 1] - t0 : T_cap;
     const int v0 = offs_v ? offs_v[b] : b * V_cap, V = offs_v ? offs_v[b + 1] - v0 : V_cap;
@@ -639,42 +650,42 @@ co_attention_stream_kernel(const uint16_t* __restrict__ qkv_img, int ld_img, con
     if (text_q)
         stream_attend<D, F16>(bt + static_cast<size_t>(q0) * ld_txt, ld_txt, min(kStreamRows, T - q0), bi + hidden, bi + 2 * hidden,
                               ld_img, V, img_mask_add + v0, scale_l2, ctx_txt + static_cast<size_t>(t0 + q0) * ld_ctx_txt + h * D,
-                              ld_ctx_txt, pdl);
+                              ld_ctx_txt, pdl, gate, b, h, 0);
     else
         stream_attend<D, F16>(bi + static_cast<size_t>(q0) * ld_img, ld_img, min(kStreamRows, V - q0), bt + hidden, bt + 2 * hidden,
                               ld_txt, T, txt_mask_add + t0, scale_l2, ctx_img + static_cast<size_t>(v0 + q0) * ld_ctx_img + h * D,
-                              ld_ctx_img, pdl);
+                              ld_ctx_img, pdl, gate, b, h, 1);
 }
 
 template <int D, bool F16>
 static cudaError_t launch_self_stream(const __nv_bfloat16* qkv, int ld_qkv, int hidden, const float* key_mask_add, __nv_bfloat16* ctx,
-                                      int ld_ctx, int B, int L, int heads, int pdl, cudaStream_t st, const int* offs) {
+                                      int ld_ctx, int B, int L, int heads, int pdl, cudaStream_t st, const int* offs, HeadGate gate) {
     constexpr size_t smem = StreamSmem<D>::kBytes;
     cudaError_t e = set_smem(self_attention_stream_kernel<D, F16>, smem);
     if (e != cudaSuccess) return e;
     const float scale_l2 = kLog2e / sqrtf(static_cast<float>(D));
     return launch_ex(self_attention_stream_kernel<D, F16>, dim3(heads, B, (L + kStreamRows - 1) / kStreamRows), dim3(32 * (D / 16)),
                      smem, pdl, st, reinterpret_cast<const uint16_t*>(qkv), ld_qkv, hidden, key_mask_add,
-                     reinterpret_cast<uint16_t*>(ctx), ld_ctx, L, scale_l2, pdl, offs);
+                     reinterpret_cast<uint16_t*>(ctx), ld_ctx, L, scale_l2, pdl, offs, gate);
 }
 
 cudaError_t launch_self_attention_stream(const __nv_bfloat16* qkv, int ld_qkv, int hidden, const float* key_mask_add,
                                          __nv_bfloat16* ctx, int ld_ctx, int B, int L, int heads, int head_dim, int pdl,
-                                         int f16, cudaStream_t st, const int* offs) {
+                                         int f16, cudaStream_t st, const int* offs, HeadGate gate) {
     if (L < 1 || (head_dim != 64 && head_dim != 128) || (ld_qkv & 7) || (ld_ctx & 1) || (hidden & 7))
         return cudaErrorInvalidValue;
     if (head_dim == 64)
-        return f16 ? launch_self_stream<64, true>(qkv, ld_qkv, hidden, key_mask_add, ctx, ld_ctx, B, L, heads, pdl, st, offs)
-                   : launch_self_stream<64, false>(qkv, ld_qkv, hidden, key_mask_add, ctx, ld_ctx, B, L, heads, pdl, st, offs);
-    return f16 ? launch_self_stream<128, true>(qkv, ld_qkv, hidden, key_mask_add, ctx, ld_ctx, B, L, heads, pdl, st, offs)
-               : launch_self_stream<128, false>(qkv, ld_qkv, hidden, key_mask_add, ctx, ld_ctx, B, L, heads, pdl, st, offs);
+        return f16 ? launch_self_stream<64, true>(qkv, ld_qkv, hidden, key_mask_add, ctx, ld_ctx, B, L, heads, pdl, st, offs, gate)
+                   : launch_self_stream<64, false>(qkv, ld_qkv, hidden, key_mask_add, ctx, ld_ctx, B, L, heads, pdl, st, offs, gate);
+    return f16 ? launch_self_stream<128, true>(qkv, ld_qkv, hidden, key_mask_add, ctx, ld_ctx, B, L, heads, pdl, st, offs, gate)
+               : launch_self_stream<128, false>(qkv, ld_qkv, hidden, key_mask_add, ctx, ld_ctx, B, L, heads, pdl, st, offs, gate);
 }
 
 template <int D, bool F16>
 static cudaError_t launch_co_stream(const __nv_bfloat16* qkv_img, int ld_img, const __nv_bfloat16* qkv_txt, int ld_txt, int hidden,
                                     const float* img_mask_add, const float* txt_mask_add, __nv_bfloat16* ctx_txt, int ld_ctx_txt,
                                     __nv_bfloat16* ctx_img, int ld_ctx_img, int B, int T, int V, int heads, int pdl, cudaStream_t st,
-                                    const int* offs_t, const int* offs_v) {
+                                    const int* offs_t, const int* offs_v, HeadGate gate) {
     constexpr size_t smem = StreamSmem<D>::kBytes;
     cudaError_t e = set_smem(co_attention_stream_kernel<D, F16>, smem);
     if (e != cudaSuccess) return e;
@@ -683,19 +694,19 @@ static cudaError_t launch_co_stream(const __nv_bfloat16* qkv_img, int ld_img, co
     return launch_ex(co_attention_stream_kernel<D, F16>, dim3(heads, B, tiles), dim3(32 * (D / 16)), smem, pdl, st,
                      reinterpret_cast<const uint16_t*>(qkv_img), ld_img, reinterpret_cast<const uint16_t*>(qkv_txt), ld_txt,
                      hidden, img_mask_add, txt_mask_add, reinterpret_cast<uint16_t*>(ctx_txt), ld_ctx_txt,
-                     reinterpret_cast<uint16_t*>(ctx_img), ld_ctx_img, T, V, scale_l2, pdl, offs_t, offs_v);
+                     reinterpret_cast<uint16_t*>(ctx_img), ld_ctx_img, T, V, scale_l2, pdl, offs_t, offs_v, gate);
 }
 
 cudaError_t launch_co_attention_stream(const __nv_bfloat16* qkv_img, int ld_img, const __nv_bfloat16* qkv_txt, int ld_txt,
                                        int hidden, const float* img_mask_add, const float* txt_mask_add,
                                        __nv_bfloat16* ctx_txt, int ld_ctx_txt, __nv_bfloat16* ctx_img, int ld_ctx_img, int B,
                                        int T, int V, int heads, int head_dim, int pdl, int f16, cudaStream_t st,
-                                       const int* offs_t, const int* offs_v) {
+                                       const int* offs_t, const int* offs_v, HeadGate gate) {
     if (T < 1 || V < 1 || (head_dim != 64 && head_dim != 128) || (ld_img & 7) || (ld_txt & 7) || (hidden & 7) ||
         (ld_ctx_txt & 1) || (ld_ctx_img & 1))
         return cudaErrorInvalidValue;
 #define VB_CO(D, F) launch_co_stream<D, F>(qkv_img, ld_img, qkv_txt, ld_txt, hidden, img_mask_add, txt_mask_add, ctx_txt, ld_ctx_txt, \
-                                           ctx_img, ld_ctx_img, B, T, V, heads, pdl, st, offs_t, offs_v)
+                                           ctx_img, ld_ctx_img, B, T, V, heads, pdl, st, offs_t, offs_v, gate)
     if (head_dim == 64) return f16 ? VB_CO(64, true) : VB_CO(64, false);
     return f16 ? VB_CO(128, true) : VB_CO(128, false);
 #undef VB_CO

@@ -130,7 +130,9 @@ attention_f32_kernel(const typename InT<IN>::type* __restrict__ q, int ld_q, con
     __syncwarp();
     const float inv = softmax_row(pr, Lk);
     float* gp = nullptr;
+    float g = 1.0f;
     if constexpr (PACKED) {
+        g = pk.gate.at(b, h);                          // gated plans report g * p
         // entry offset + heads * sum_{b' < b} Lq_b' Lk_b' + (h, i) inside the sample's [heads, Lq, Lk] block, in int64: one call's
         // entries hold more than 2^31 floats at large batches
         float* dst = reinterpret_cast<float*>(pk.dst[0]);
@@ -141,7 +143,7 @@ attention_f32_kernel(const typename InT<IN>::type* __restrict__ q, int ld_q, con
     for (int j = lane; j < Lk; j += 32) {
         const float pj = pr[j] * inv;
         pr[j] = pj;
-        if (gp) gp[j] = pj;
+        if (gp) gp[j] = pj * g;
     }
     __syncwarp();
     if (PACKED || ctx_mode == 0) return;
@@ -208,7 +210,8 @@ attention_f32_mean_kernel(const typename InT<IN>::type* __restrict__ q, int ld_q
         if (row_ok) {                                  // rows past Lq keep staging keys with the CTA: no return before the last head
             __syncwarp();
             const float inv = softmax_row(pr, Lk);
-            for (int j = lane; j < Lk; j += 32) ar[j] = __fadd_rn(ar[j], __fmul_rn(pr[j], inv));
+            const float g = PACKED ? pk.gate.at(b, h) : 1.0f;     // gated plans average g * p (x * 1.0f is exact)
+            for (int j = lane; j < Lk; j += 32) ar[j] = __fadd_rn(ar[j], __fmul_rn(__fmul_rn(pr[j], inv), g));
         }
     }
     if (pdl) pdl_launch_dependents();

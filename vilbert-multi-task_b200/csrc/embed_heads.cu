@@ -528,6 +528,20 @@ cudaError_t launch_variant_text(const TextSrc* v, int n, const int* offs, int ta
     return cudaGetLastError();
 }
 
+// Head ablation's gate rows: row b of the [n, stride] gate table is all ones, with element zero[b] set to 0 (-1: none).  One CTA per
+// row; every float of the row is written, so the table holds nothing from an earlier call.
+__global__ void gate_rows_kernel(const int32_t* __restrict__ zero, int stride, float* __restrict__ gate) {
+    const int b = blockIdx.x, z = zero[b];
+    float* row = gate + static_cast<size_t>(b) * stride;
+    for (int i = threadIdx.x; i < stride; i += blockDim.x) row[i] = i == z ? 0.0f : 1.0f;
+}
+
+cudaError_t launch_gate_rows(const int32_t* zero, int n, int stride, float* gate, cudaStream_t st) {
+    if (n < 1 || stride < 1 || zero == nullptr || gate == nullptr) return cudaErrorInvalidValue;
+    gate_rows_kernel<<<n, 128, 0, st>>>(zero, stride, gate);
+    return cudaGetLastError();
+}
+
 cudaError_t launch_gather_state(const int32_t* idx, int n_src, const float* src_f32, const void* src_16, const float* src_mask,
                                 float* dst_f32, void* dst_16, float* dst_mask, int B, int L, int H, int H16, cudaStream_t st) {
     if (B < 1 || n_src < 1 || (static_cast<long long>(L) * H) % 4 != 0 || (static_cast<long long>(L) * H16) % 8 != 0) return cudaErrorInvalidValue;

@@ -503,11 +503,13 @@ inline const char* bound_name(int max_rows) {
 struct SelfAttnArgs {
     const bf16* qkv; int ld_qkv, hidden; const float* mask; bf16* ctx; int ld_ctx, B, L, heads, head_dim; const int* offs;
     bool stream_kv;                // the streaming kernel (more than kStagedAttnRows rows per sample)
+    vb::HeadGate gate;             // gated packed plans: the entry's column of the plan's gate table
 };
 struct CoAttnArgs {
     const bf16 *qkv_img, *qkv_txt; int ld_img, ld_txt, hidden; const float *img_mask, *txt_mask;
     bf16 *ctx_txt, *ctx_img; int ld_ctx_txt, ld_ctx_img, B, T, V, heads, head_dim; const int *offs_t, *offs_v;
     bool stream_kv;                // the streaming kernel (either stream above kStagedAttnRows rows per sample)
+    vb::HeadGate gate;             // gated packed plans: the text-query entry's column, the image-query one at gate.next
 };
 struct RowdotArgs { const float *x, *W, *bias, *add; float* out; int ld_x, ld_out, M, K, n_out; const int* m_rows; };
 struct LayerNormArgs {             // out = LN(y + res)
@@ -840,6 +842,14 @@ struct Plan {
     const int* src_t() const { return d_meta + layout.src_t(); }
     const int* src_v() const { return d_meta + layout.src_v(); }
     const int64_t* meta64(size_t at) const { return reinterpret_cast<const int64_t*>(d_meta + at); }
+    // gated packed plans (vb200_forward_packed_gated): the head gate table [B, n_entries, max_heads] fp32, written per call ahead of
+    // the plan's kernels; every attention launch reads its entry's column
+    float* gate = nullptr;
+    int gate_entries = 0, gate_heads = 0;
+    vb::HeadGate gate_at(int e) const {
+        if (gate == nullptr) return {};
+        return vb::HeadGate{gate + static_cast<size_t>(e) * gate_heads, gate_entries * gate_heads, gate_heads};
+    }
 };
 
 // One pre-training head at one bucket of M listed rows (vb200_pretraining_heads): the device row list (the call's count first, which
@@ -1330,7 +1340,7 @@ struct vb200_engine {
                 const MetaLayout& m = pl.layout;
                 a.packed = true;
                 a.pk = vb::PackedProbs{q.offs, kv.offs, pl.meta64(m.probs_dst()), pl.meta64(m.probs_entry(n_probs)),
-                                       pl.meta64(m.probs_prefix(self ? q.prefix : 2))};
+                                       pl.meta64(m.probs_prefix(self ? q.prefix : 2)), pl.gate_at(entry)};
                 ++n_probs;
             } else {
                 a.probs = attn_out(mean ? 1 : heads, a.Lq, a.Lk);
@@ -1379,6 +1389,7 @@ struct vb200_engine {
                 a.qkv = reinterpret_cast<bf16*>(s.qkv); a.ld_qkv = 3 * hid; a.hidden = hid; a.mask = s.mask; a.ctx = s.ctx; a.ld_ctx = hid;
                 a.B = B; a.L = s.seq; a.heads = heads; a.head_dim = hid / heads; a.offs = s.offs;
                 a.stream_kv = s.seq > kStagedAttnRows;
+                a.gate = pl.gate_at(entry);
                 push({a, s.branch, 4.0 * B * heads * s.seq * s.seq * (hid / heads)});
             }
             if (eng.x3 || maps) attention_f32(s, s, hid, heads, entry);
@@ -1420,6 +1431,7 @@ struct vb200_engine {
                 a.hidden = Hb; a.img_mask = v.mask; a.txt_mask = t.mask; a.ctx_txt = t.ctx; a.ld_ctx_txt = Hb; a.ctx_img = v.ctx; a.ld_ctx_img = Hb;
                 a.B = B; a.T = t.seq; a.V = v.seq; a.heads = heads; a.head_dim = Hb / heads; a.offs_t = t.offs; a.offs_v = v.offs;
                 a.stream_kv = t.seq > kStagedAttnRows || v.seq > kStagedAttnRows;
+                a.gate = pl.gate_at(entry);
                 push({a, 0, 8.0 * B * heads * t.seq * v.seq * (Hb / heads), Op::JOIN});
             }
             if (eng.x3 || maps) {
@@ -1548,7 +1560,13 @@ struct vb200_engine {
         for (int e = 0; e < static_cast<int>(k.size()); ++e) last[k[e]] = e;
         return (state_sel.has(last[0]) ? kTextRows : 0) | (state_sel.has(last[1]) ? kImageRows : 0);
     }
-    Plan* get_plan(int B, int Tin, int V, uint32_t select, int slot = 0, int mode = FULL, bool want_attn = false, bool want_states = false) {
+    // The head gate table's shape: every entry of the full attention list, the configuration's largest head count.
+    int gate_entries() const { return static_cast<int>(attention_kinds(schedule).size()); }
+    int gate_heads() const { return std::max({cfg.heads, cfg.v_heads, cfg.bi_heads}); }
+
+    // gated (PACKED plans only): the plan owns a head gate table and its attention launches read it
+    Plan* get_plan(int B, int Tin, int V, uint32_t select, int slot = 0, int mode = FULL, bool want_attn = false, bool want_states = false,
+                   bool gated = false) {
         if (slot < 0 || slot > 15) fail(VB200_ERR_INVALID, "slot %d out of range (0..15)", slot);
         if (slot > 0 && !opt.use_cuda_graph) fail(VB200_ERR_INVALID, "concurrent slots need CUDA-graph plans (use_cuda_graph)");
         const bool packed = mode >= PACKED;
@@ -1567,7 +1585,7 @@ struct vb200_engine {
         std::vector<int64_t> key{B, Tin, V, static_cast<int64_t>(select), slot, mode, want_attn ? 1 : 0,
                                  want_attn ? static_cast<int64_t>(attn_sel.mask) : 0, want_attn && attn_sel.mean ? 1 : 0,
                                  want_states ? 1 : 0, want_states ? static_cast<int64_t>(state_sel.mask) : 0,
-                                 want_states ? state_sel.rows : 0};
+                                 want_states ? state_sel.rows : 0, gated ? 1 : 0};
         auto it = plans.find(key);
         if (it != plans.end()) { it->second->last_use = ++use_clock; return it->second.get(); }
         std::unique_ptr<Plan> up(new Plan());
@@ -1587,6 +1605,12 @@ struct vb200_engine {
             CUDA_CHECK(cudaMemset(pl.d_meta, 0, n_meta * sizeof(int)));
             pl.meta.copied = make_event();
             pl.meta.reserve(n_meta * sizeof(int));
+        }
+        if (gated) {
+            if (mode != PACKED) fail(VB200_ERR_INVALID, "head gates exist for the PACKED forwards only");
+            pl.gate_entries = gate_entries();
+            pl.gate_heads = gate_heads();
+            pl.gate = pl.mem.alloc_n<float>(static_cast<size_t>(B) * pl.gate_entries * pl.gate_heads);
         }
         const int Mt = B * T, Mv = B * V, H = c.hidden, Hv = c.v_hidden, Hb = c.bi_hidden;
         const bool full = schedule_mode == FULL;
@@ -1729,12 +1753,12 @@ struct vb200_engine {
             },
             [&](const SelfAttnArgs& a) {
                 CUDA_CHECK((a.stream_kv ? vb::launch_self_attention_stream : vb::launch_self_attention)(
-                    a.qkv, a.ld_qkv, a.hidden, a.mask, a.ctx, a.ld_ctx, a.B, a.L, a.heads, a.head_dim, pdl, f16, st, a.offs));
+                    a.qkv, a.ld_qkv, a.hidden, a.mask, a.ctx, a.ld_ctx, a.B, a.L, a.heads, a.head_dim, pdl, f16, st, a.offs, a.gate));
             },
             [&](const CoAttnArgs& a) {
                 CUDA_CHECK((a.stream_kv ? vb::launch_co_attention_stream : vb::launch_co_attention)(
                     a.qkv_img, a.ld_img, a.qkv_txt, a.ld_txt, a.hidden, a.img_mask, a.txt_mask, a.ctx_txt, a.ld_ctx_txt, a.ctx_img,
-                    a.ld_ctx_img, a.B, a.T, a.V, a.heads, a.head_dim, pdl, f16, st, a.offs_t, a.offs_v));
+                    a.ld_ctx_img, a.B, a.T, a.V, a.heads, a.head_dim, pdl, f16, st, a.offs_t, a.offs_v, a.gate));
             },
             [&](const RowdotArgs& a) {
                 CUDA_CHECK(vb::launch_rowdot(a.x, a.ld_x, a.W, a.bias, a.add, a.out, a.ld_out, a.M, a.K, a.n_out, pdl, st, a.m_rows));
@@ -1954,9 +1978,12 @@ struct vb200_engine {
     // What every packed entry point shares once it has checked its own inputs: the engine-wide rejections, the call's rows
     // (pack_batch), its plan, the d_meta staged ahead of `input` (the call's input kernels), the plan and then, for the forwards
     // (out != null), the outputs at the call's row totals or, for the prefixes, the state of the call's rows.  Returns the plan,
-    // whose outputs stay valid in stream order until the plan's next run.
+    // whose outputs stay valid in stream order until the plan's next run.  head_mask (DEVICE [B, gate_entries, gate_heads], the gated
+    // forwards): the call runs the gated plan, and one copy puts the mask into the plan's gate table ahead of `input`.  gated without
+    // a head_mask (head ablation): the gated plan, whose table `input` writes.
     Plan& run_packed(const char* api, int mode, const PackedLengths& len, uint32_t select, int slot, const vb200_outputs* out,
-                     const PrefixState& state, void* cuda_stream, const std::function<void(Plan&, const PackedBatch&, cudaStream_t)>& input) {
+                     const PrefixState& state, void* cuda_stream, const std::function<void(Plan&, const PackedBatch&, cudaStream_t)>& input,
+                     const float* head_mask = nullptr, bool gated = false) {
         if (select & VB200_OUT_ATTENTION)
             fail(VB200_ERR_INVALID, "%s: the attention-probability output (VB200_OUT_ATTENTION) is not supported", api);
         if (mode != PACKED) reject_packed_attention(select, api);
@@ -1970,9 +1997,13 @@ struct vb200_engine {
         const PackedBatch b = pack_batch(api, cfg, schedule, len, maps ? out->attention_probs : nullptr, max_rows, attn_sel,
                                          states ? out->layer_states : nullptr, state_sel);
         CUDA_CHECK(cudaSetDevice(opt.device));
-        Plan& pl = *get_plan(len.B, b.Tin, b.V, (select & VB200_OUT_ALL) | rows_read(out), slot, mode, maps, states);
+        Plan& pl = *get_plan(len.B, b.Tin, b.V, (select & VB200_OUT_ALL) | rows_read(out), slot, mode, maps, states,
+                             gated || head_mask != nullptr);
         const cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
         stage_meta(pl, b.meta, st);
+        if (head_mask != nullptr)
+            CUDA_CHECK(cudaMemcpyAsync(pl.gate, head_mask, static_cast<size_t>(pl.B) * pl.gate_entries * pl.gate_heads * sizeof(float),
+                                       cudaMemcpyDeviceToDevice, st));
         input(pl, b, st);
         run_plan(pl, st);
         if (out != nullptr) copy_outputs(pl, *out, st, cudaMemcpyDeviceToDevice, b.rows_t(), b.rows_v());
@@ -2116,12 +2147,16 @@ struct vb200_engine {
         std::vector<vb::TextSrc> text;
         std::vector<vb::RegionSrc> img;
         std::vector<int32_t> tin, nv;
+        std::vector<int32_t> gate;     // head ablation: per sample the gate table element (entry * gate_heads + head) set to 0, or -1
         int64_t n_floats = 0;
         bool grounding = false;
+        bool gated = false;            // head ablation: the samples run the gated plan
     };
-    // The messages checked against the batch's lengths and laid out; no sample cap (run_ablation applies it).
+    // The messages checked against the batch's lengths and laid out; no sample cap (run_ablation applies it).  entries (head
+    // ablation, one [begin, end) per message): after its token and box variants, each message gets one variant per head of every
+    // entry in the range (kind 3, unit entry * gate_heads + head): the message's samples, unablated, with that one gate at 0.
     AblLayout ablation_layout(const char* api, int batch, const int32_t* n_tokens, const int32_t* n_boxes, const vb200_ablation_message* msgs,
-                              int n_msgs) const {
+                              int n_msgs, const std::vector<std::array<int, 2>>* entries = nullptr) const {
         if (n_tokens == nullptr || n_boxes == nullptr || msgs == nullptr) fail(VB200_ERR_INVALID, "%s: n_tokens / n_boxes / msgs is NULL", api);
         if (batch < 1) fail(VB200_ERR_INVALID, "%s: batch must be positive (batch = %d)", api, batch);
         if (n_msgs < 1) fail(VB200_ERR_INVALID, "%s: n_msgs must be positive (n_msgs = %d)", api, n_msgs);
@@ -2136,7 +2171,13 @@ struct vb200_engine {
         }
         AblLayout L;
         std::vector<std::vector<AblVariant>> per(n_msgs);
-        auto sample = [&](const vb200_ablation_message& m, int masked, int image, int skip) {
+        std::vector<int> entry_heads;
+        if (entries != nullptr) {
+            L.gated = true;
+            for (int kind : attention_kinds(schedule)) entry_heads.push_back(kind == 0 ? cfg.heads : kind == 1 ? cfg.v_heads : cfg.bi_heads);
+        }
+        auto sample = [&](const vb200_ablation_message& m, int masked, int image, int skip, int gate = -1) {
+            L.gate.push_back(gate);
             L.text.push_back({tok0[m.image_begin], n_tokens[m.image_begin], masked, m.image_begin});
             L.img.push_back({image, box0[image], skip});
             L.tin.push_back(n_tokens[m.image_begin]);
@@ -2179,6 +2220,12 @@ struct vb200_engine {
                         if (n_boxes[ib + k] < 2 && m.box_begin < box0[ib + k + 1] - box0[ib] && m.box_end > box0[ib + k] - box0[ib])
                             fail(VB200_ERR_INVALID, "%s: message %d drops a box of its image %d, which has %d box (box ablation needs >= 2)",
                                  api, i, k, n_boxes[ib + k]);
+                    if (entries != nullptr) {
+                        const auto& r = (*entries)[i];
+                        if (r[0] < 0 || r[0] > r[1] || r[1] > static_cast<int>(entry_heads.size()))
+                            fail(VB200_ERR_INVALID, "%s: message %d has the entry range [%d, %d), reversed or outside [0, %d]", api, i, r[0],
+                                 r[1], static_cast<int>(entry_heads.size()));
+                    }
                 }
                 if ((f == VB200_DECODE_NLVR2) != (pass == 0)) continue;
                 std::vector<AblVariant>& out = per[i];
@@ -2191,9 +2238,9 @@ struct vb200_engine {
                     if (f == VB200_DECODE_GROUNDING) return {head, first, L.nv[first], -1, 0, 0};
                     return {head, first, width, -1, 0, 0};
                 };
-                auto all_images = [&](int masked) {
-                    const int first = sample(m, masked, ib, -1);
-                    for (int k = 1; k < K; ++k) sample(m, masked, ib + k, -1);
+                auto all_images = [&](int masked, int gate = -1) {
+                    const int first = sample(m, masked, ib, -1, gate);
+                    for (int k = 1; k < K; ++k) sample(m, masked, ib + k, -1, gate);
                     return first;
                 };
                 const int base = all_images(-1);
@@ -2220,6 +2267,12 @@ struct vb200_engine {
                         variant(2, u, 1, seg(first), f == VB200_DECODE_GROUNDING ? j + 1 : -1);
                     }
                 }
+                if (entries != nullptr)
+                    for (int e = (*entries)[i][0]; e < (*entries)[i][1]; ++e)
+                        for (int h = 0; h < entry_heads[e]; ++h) {
+                            const int unit = e * gate_heads() + h;
+                            variant(3, unit, K, seg(all_images(-1, unit)), -1);
+                        }
                 L.grounding |= f == VB200_DECODE_GROUNDING;
             }
         std::vector<int64_t> vrow(L.nv.size() + 1, 0);       // each sample's first vision_logit row
@@ -2252,6 +2305,7 @@ struct vb200_engine {
             L.img.push_back({0, 0, -1});
             L.tin.push_back(1);
             L.nv.push_back(2);
+            L.gate.push_back(-1);
         }
         std::vector<vb::SegmentDesc> seg(n_var);
         for (int k = 0; k < n_var; ++k) seg[k] = L.v[k].seg;
@@ -2260,7 +2314,8 @@ struct vb200_engine {
         size_t at = 0;
         auto carve = [&](size_t bytes) { const size_t a = at; at += (bytes + 255) / 256 * 256; return a; };
         const size_t o_text = carve(n_pad * sizeof(vb::TextSrc)), o_img = carve(n_pad * sizeof(vb::RegionSrc));
-        const size_t o_seg = carve(n_var * sizeof(vb::SegmentDesc)), staged = at;
+        const size_t o_seg = carve(n_var * sizeof(vb::SegmentDesc));
+        const size_t o_gate = L.gated ? carve(n_pad * sizeof(int32_t)) : 0, staged = at;
         const size_t o_q = carve(sum_tin * 8), o_ids = carve(sum_tin * 8), o_task = carve(static_cast<size_t>(n_pad) * 8);
         CUDA_CHECK(cudaSetDevice(opt.device));
         char* ws = abl_ws.acquire(at, st);
@@ -2268,6 +2323,7 @@ struct vb200_engine {
             memcpy(h + o_text, L.text.data(), n_pad * sizeof(vb::TextSrc));
             memcpy(h + o_img, L.img.data(), n_pad * sizeof(vb::RegionSrc));
             memcpy(h + o_seg, seg.data(), n_var * sizeof(vb::SegmentDesc));
+            if (L.gated) memcpy(h + o_gate, L.gate.data(), n_pad * sizeof(int32_t));
             put(ws, 0, staged);
         });
         const auto* text_d = reinterpret_cast<const vb::TextSrc*>(ws + o_text);
@@ -2284,7 +2340,9 @@ struct vb200_engine {
                                                q, ids, tk, s));
             embed_text(p, q, ids, nullptr, tk, b.rows_t(), s);
             pack_regions_packed(p, in->box_features, in->boxes, in->image_wh, nullptr, b.rows_v(), s, img_d);
-        });
+            if (L.gated)
+                CUDA_CHECK(vb::launch_gate_rows(reinterpret_cast<const int32_t*>(ws + o_gate), n_pad, p.gate_entries * p.gate_heads, p.gate, s));
+        }, nullptr, L.gated);
         vb::SegmentHeads heads{};
         for (int h = 0; h < vb::kSegmentHeads; ++h) {
             heads.p[h] = pl.outs[h].p;
@@ -2365,18 +2423,57 @@ struct vb200_engine {
         run_ablation(api, in, ablation_layout(api, in->batch, in->n_tokens, in->n_boxes, msgs, n_msgs), max_regions, mask_token,
                      variant_logits, scores, slot, st);
     }
+    // vb200_head_ablation[_layout]: each head message as a message with no token or box range, plus its entry range
+    static std::vector<vb200_ablation_message> head_messages(const vb200_head_ablation_message* msgs, int n,
+                                                             std::vector<std::array<int, 2>>& entries) {
+        std::vector<vb200_ablation_message> m;
+        for (int i = 0; i < n; ++i) {
+            m.push_back({msgs[i].family, msgs[i].image_begin, msgs[i].n_images, msgs[i].answer, 0, 0, 0, 0});
+            entries.push_back({msgs[i].entry_begin, msgs[i].entry_end});
+        }
+        return m;
+    }
+    void head_ablation(const vb200_packed_region_inputs* in, const vb200_head_ablation_message* msgs, int n_msgs, float* variant_logits,
+                       vb200_ablation_score* scores, int slot, cudaStream_t st) {
+        const char* api = "vb200_head_ablation";
+        if (in == nullptr || msgs == nullptr || variant_logits == nullptr) fail(VB200_ERR_INVALID, "%s: in / msgs / variant_logits is NULL", api);
+        if (x3) fail(VB200_ERR_INVALID, "%s: packed batches are not supported in split_fp32 (fp32x) mode", api);
+        if (pretraining) fail(VB200_ERR_INVALID, "%s: a pre-training engine has no task head to attribute an answer of", api);
+        if (reinterpret_cast<uintptr_t>(variant_logits) & 3) fail(VB200_ERR_INVALID, "%s: variant_logits is not 4-byte aligned", api);
+        if (reinterpret_cast<uintptr_t>(scores) & 3) fail(VB200_ERR_INVALID, "%s: scores is not 4-byte aligned", api);
+        if (n_msgs < 1) fail(VB200_ERR_INVALID, "%s: n_msgs must be positive (n_msgs = %d)", api, n_msgs);
+        const int max_regions = check_ablation_inputs(api, in, 0, slot);     // no position is masked: any valid token id
+        std::vector<std::array<int, 2>> entries;
+        const std::vector<vb200_ablation_message> m = head_messages(msgs, n_msgs, entries);
+        run_ablation(api, in, ablation_layout(api, in->batch, in->n_tokens, in->n_boxes, m.data(), n_msgs, &entries), max_regions, 0,
+                     variant_logits, scores, slot, st);
+    }
+    void head_ablation_layout(int batch, const int32_t* n_tokens, const int32_t* n_boxes, const vb200_head_ablation_message* msgs, int n_msgs,
+                              vb200_ablation_variant* variants, int64_t* n_variants, int64_t* n_floats, int64_t* n_samples) const {
+        const char* api = "vb200_head_ablation_layout";
+        if (n_variants == nullptr || n_floats == nullptr || n_samples == nullptr)
+            fail(VB200_ERR_INVALID, "%s: n_variants / n_floats / n_samples is NULL", api);
+        if (pretraining) fail(VB200_ERR_INVALID, "%s: a pre-training engine has no task head to attribute an answer of", api);
+        if (msgs == nullptr) fail(VB200_ERR_INVALID, "%s: msgs is NULL", api);
+        if (n_msgs < 1) fail(VB200_ERR_INVALID, "%s: n_msgs must be positive (n_msgs = %d)", api, n_msgs);
+        std::vector<std::array<int, 2>> entries;
+        const std::vector<vb200_ablation_message> m = head_messages(msgs, n_msgs, entries);
+        put_layout(ablation_layout(api, batch, n_tokens, n_boxes, m.data(), n_msgs, &entries), variants, n_variants, n_floats, n_samples);
+    }
+    static void put_layout(const AblLayout& L, vb200_ablation_variant* variants, int64_t* n_variants, int64_t* n_floats, int64_t* n_samples) {
+        if (variants != nullptr)
+            for (size_t k = 0; k < L.v.size(); ++k) variants[k] = L.v[k].rec;
+        *n_variants = static_cast<int64_t>(L.v.size());
+        *n_floats = L.n_floats;
+        *n_samples = static_cast<int64_t>(L.text.size());
+    }
     void message_ablation_layout(int batch, const int32_t* n_tokens, const int32_t* n_boxes, const vb200_ablation_message* msgs, int n_msgs,
                                  vb200_ablation_variant* variants, int64_t* n_variants, int64_t* n_floats, int64_t* n_samples) const {
         const char* api = "vb200_message_ablation_layout";
         if (n_variants == nullptr || n_floats == nullptr || n_samples == nullptr)
             fail(VB200_ERR_INVALID, "%s: n_variants / n_floats / n_samples is NULL", api);
         if (pretraining) fail(VB200_ERR_INVALID, "%s: a pre-training engine has no task head to attribute an answer of", api);
-        const AblLayout L = ablation_layout(api, batch, n_tokens, n_boxes, msgs, n_msgs);
-        if (variants != nullptr)
-            for (size_t k = 0; k < L.v.size(); ++k) variants[k] = L.v[k].rec;
-        *n_variants = static_cast<int64_t>(L.v.size());
-        *n_floats = L.n_floats;
-        *n_samples = static_cast<int64_t>(L.text.size());
+        put_layout(ablation_layout(api, batch, n_tokens, n_boxes, msgs, n_msgs), variants, n_variants, n_floats, n_samples);
     }
     // ---- region selection: every descriptor is checked before anything is enqueued
     void select_regions(const vb200_detections* imgs, int n, const vb200_select_params* p, const vb200_selected* out, cudaStream_t st) {
@@ -2820,28 +2917,30 @@ int vb200_forward_slot(vb200_handle h, const vb200_inputs* in, const vb200_outpu
     });
 }
 
-int vb200_forward_packed(vb200_handle h, const vb200_packed_inputs* in, const vb200_outputs* out, uint32_t select, int32_t slot,
-                         void* cuda_stream) {
+namespace {
+// vb200_forward_packed and its gated form (head_mask non-null; `api` names the entry point)
+int forward_packed(vb200_handle h, const char* api, const vb200_packed_inputs* in, const float* head_mask, const vb200_outputs* out,
+                   uint32_t select, int32_t slot, void* cuda_stream) {
     if (h == nullptr) return VB200_ERR_INVALID;
     return guard(h, [&] {
         if (in == nullptr || out == nullptr) fail(VB200_ERR_INVALID, "inputs/outputs struct is NULL");
         if (!in->n_tokens || !in->n_regions || !in->question || !in->segment_ids || !in->features || !in->spatials ||
             (h->cfg.task_tokens && !in->task_tokens))
             fail(VB200_ERR_INVALID, "vb200_packed_inputs has a NULL required pointer");
-        h->run_packed("vb200_forward_packed", vb200_engine::PACKED,
+        h->run_packed(api, vb200_engine::PACKED,
                       {"sample", in->batch, in->n_tokens, in->max_tokens, in->n_regions, in->max_regions}, select, slot, out, {},
                       cuda_stream, [&](Plan& pl, const PackedBatch& b, cudaStream_t st) {
                           h->embed_text(pl, in->question, in->segment_ids, nullptr, in->task_tokens, b.rows_t(), st);
                           h->pack_image(pl, in->features, in->spatials, nullptr, b.rows_v(), st);
-                      });
+                      }, head_mask);
     });
 }
 
-int vb200_forward_regions_packed(vb200_handle h, const vb200_packed_region_inputs* in, const vb200_outputs* out, uint32_t select,
-                                 int32_t slot, void* cuda_stream) {
+// vb200_forward_regions_packed and its gated form (head_mask non-null)
+int forward_regions_packed(vb200_handle h, const char* api, const vb200_packed_region_inputs* in, const float* head_mask,
+                           const vb200_outputs* out, uint32_t select, int32_t slot, void* cuda_stream) {
     if (h == nullptr) return VB200_ERR_INVALID;
     return guard(h, [&] {
-        const char* api = "vb200_forward_regions_packed";
         if (in == nullptr || out == nullptr) fail(VB200_ERR_INVALID, "inputs/outputs struct is NULL");
         const int task = h->cfg.task_tokens ? 1 : 0;
         if (!in->n_tokens || !in->n_boxes || !in->question || !in->segment_ids || !in->box_features || !in->boxes || !in->image_wh ||
@@ -2856,8 +2955,38 @@ int vb200_forward_regions_packed(vb200_handle h, const vb200_packed_region_input
                       slot, out, {}, cuda_stream, [&](Plan& pl, const PackedBatch& b, cudaStream_t st) {
                           h->embed_text(pl, in->question, in->segment_ids, nullptr, in->task_tokens, b.rows_t(), st);
                           h->pack_regions_packed(pl, in->box_features, in->boxes, in->image_wh, in->spatials_out, b.rows_v(), st);
-                      });
+                      }, head_mask);
     });
+}
+// the gated forwards' own rejection, ahead of everything else: a gated call without a gate table
+int reject_null_mask(vb200_handle h, const char* api, const float* head_mask) {
+    if (h == nullptr) return VB200_ERR_INVALID;
+    return guard(h, [&] { if (head_mask == nullptr) fail(VB200_ERR_INVALID, "%s: head_mask is NULL", api); });
+}
+}  // namespace
+
+int vb200_forward_packed(vb200_handle h, const vb200_packed_inputs* in, const vb200_outputs* out, uint32_t select, int32_t slot,
+                         void* cuda_stream) {
+    return forward_packed(h, "vb200_forward_packed", in, nullptr, out, select, slot, cuda_stream);
+}
+
+int vb200_forward_packed_gated(vb200_handle h, const vb200_packed_inputs* in, const float* head_mask, const vb200_outputs* out,
+                               uint32_t select, int32_t slot, void* cuda_stream) {
+    const char* api = "vb200_forward_packed_gated";
+    const int r = reject_null_mask(h, api, head_mask);
+    return r != VB200_OK ? r : forward_packed(h, api, in, head_mask, out, select, slot, cuda_stream);
+}
+
+int vb200_forward_regions_packed(vb200_handle h, const vb200_packed_region_inputs* in, const vb200_outputs* out, uint32_t select,
+                                 int32_t slot, void* cuda_stream) {
+    return forward_regions_packed(h, "vb200_forward_regions_packed", in, nullptr, out, select, slot, cuda_stream);
+}
+
+int vb200_forward_regions_packed_gated(vb200_handle h, const vb200_packed_region_inputs* in, const float* head_mask,
+                                       const vb200_outputs* out, uint32_t select, int32_t slot, void* cuda_stream) {
+    const char* api = "vb200_forward_regions_packed_gated";
+    const int r = reject_null_mask(h, api, head_mask);
+    return r != VB200_OK ? r : forward_regions_packed(h, api, in, head_mask, out, select, slot, cuda_stream);
 }
 
 int vb200_forward_regions(vb200_handle h, const vb200_region_inputs* in, const vb200_outputs* out, uint32_t select, int32_t slot,
@@ -3045,6 +3174,21 @@ int vb200_message_ablation_layout(vb200_handle h, int32_t batch, const int32_t* 
                                   int64_t* n_floats, int64_t* n_samples) {
     if (h == nullptr) return VB200_ERR_INVALID;
     return guard(h, [&] { h->message_ablation_layout(batch, n_tokens, n_boxes, msgs, n_msgs, variants, n_variants, n_floats, n_samples); });
+}
+
+int vb200_head_ablation_layout(vb200_handle h, int32_t batch, const int32_t* n_tokens, const int32_t* n_boxes,
+                               const vb200_head_ablation_message* msgs, int32_t n_msgs, vb200_ablation_variant* variants, int64_t* n_variants,
+                               int64_t* n_floats, int64_t* n_samples) {
+    if (h == nullptr) return VB200_ERR_INVALID;
+    return guard(h, [&] { h->head_ablation_layout(batch, n_tokens, n_boxes, msgs, n_msgs, variants, n_variants, n_floats, n_samples); });
+}
+
+int vb200_head_ablation(vb200_handle h, const vb200_packed_region_inputs* in, const vb200_head_ablation_message* msgs, int32_t n_msgs,
+                        float* variant_logits, vb200_ablation_score* scores, int32_t slot, void* cuda_stream) {
+    if (h == nullptr) return VB200_ERR_INVALID;
+    return guard(h, [&] {
+        h->head_ablation(in, msgs, n_msgs, variant_logits, scores, slot, static_cast<cudaStream_t>(cuda_stream));
+    });
 }
 
 int vb200_message_ablation(vb200_handle h, const vb200_packed_region_inputs* in, const vb200_ablation_message* msgs, int32_t n_msgs,
@@ -3363,6 +3507,8 @@ int vb200_model_dim(vb200_handle h, const char* key, int64_t* value) {
         else if (k == "n_plans") *value = static_cast<int64_t>(h->plans.size());
         else if (k == "n_layers_scheduled") *value = static_cast<int64_t>(h->schedule.size());
         else if (k == "max_rows_per_sample") *value = h->max_rows;
+        else if (k == "head_mask_entries") *value = h->gate_entries();
+        else if (k == "head_mask_heads") *value = h->gate_heads();
         else if (k == "attention_entries") {
             const size_t n = attention_kinds(h->schedule).size();
             *value = n > 63 ? -1 : static_cast<int64_t>(h->attn_sel.mask & ((1ull << n) - 1));

@@ -55,11 +55,22 @@ bool gemm_pingpong_supports(const GemmEpilogue& ep, int block_n);
 cudaError_t launch_gemm_pingpong(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b, const CUtensorMap* tmap_c16,
                                  const CUtensorMap* tmap_c32, const GemmEpilogue& ep, int block_n, int grid_pct, cudaStream_t st);
 
+// Head gate of the gated packed forwards (vb200_forward_packed_gated): sample b's head h context rows -- or its probabilities -- are
+// scaled in fp32 by p[b * ld + h], p being one attention entry's column of the plan's [B, n_entries, max_heads] gate table.  A
+// co-attention launch runs two entries: its image-query direction reads the column at p + next.  p null: no gate, today's bits
+// (a gate of 1.0f gives them too).
+struct HeadGate {
+    const float* p; int ld, next;
+    __device__ __forceinline__ float at(int b, int h, int dir = 0) const {
+        return p ? p[static_cast<size_t>(b) * ld + dir * next + h] : 1.0f;
+    }
+};
 // 16-bit activation buffers are typed __nv_bfloat16* throughout; `f16` says the bits are IEEE fp16 instead.
-// K4: softmax(Q K^T / sqrt(d) + mask) V per (sample, head); qkv row = [Q | K | V], each `hidden` wide.
+// K4: softmax(Q K^T / sqrt(d) + mask) V per (sample, head); qkv row = [Q | K | V], each `hidden` wide.  Every attention launcher takes
+// an optional HeadGate (default: none).
 cudaError_t launch_self_attention(const __nv_bfloat16* qkv, int ld_qkv, int hidden, const float* key_mask_add,
                                   __nv_bfloat16* ctx, int ld_ctx, int B, int L, int heads, int head_dim, int pdl,
-                                  int f16, cudaStream_t st, const int* offs = nullptr);
+                                  int f16, cudaStream_t st, const int* offs = nullptr, HeadGate gate = {});
 // offs (packed batches, optional): device [B + 1] row offsets; sample b is rows [offs[b], offs[b+1]) of qkv / mask / ctx, and
 // L is the shared-memory capacity (>= every sample's length).  nullptr: sample b is rows [b L, b L + L).
 // K5: both co-attention directions in one kernel.  qkv_img rows = [Q1|K1|V1], qkv_txt rows = [Q2|K2|V2].
@@ -68,18 +79,19 @@ cudaError_t launch_co_attention(const __nv_bfloat16* qkv_img, int ld_img, const 
                                 int hidden, const float* img_mask_add, const float* txt_mask_add,
                                 __nv_bfloat16* ctx_txt, int ld_ctx_txt, __nv_bfloat16* ctx_img, int ld_ctx_img, int B,
                                 int T, int V, int heads, int head_dim, int pdl, int f16, cudaStream_t st,
-                                const int* offs_t = nullptr, const int* offs_v = nullptr);   // as launch_self_attention, per stream
+                                const int* offs_t = nullptr, const int* offs_v = nullptr,   // as launch_self_attention, per stream
+                                HeadGate gate = {});                                         // dir 0 ctx_txt, 1 ctx_img
 // Streaming K4 / K5 (any length): same arguments and the same bits as the two above wherever those accept the length, but K and V
 // stream through shared memory in 64-key blocks, one CTA per 64 query rows.  The engine uses them for plans with more than 256 rows
 // per sample in a stream the op reads.
 cudaError_t launch_self_attention_stream(const __nv_bfloat16* qkv, int ld_qkv, int hidden, const float* key_mask_add,
                                          __nv_bfloat16* ctx, int ld_ctx, int B, int L, int heads, int head_dim, int pdl,
-                                         int f16, cudaStream_t st, const int* offs = nullptr);
+                                         int f16, cudaStream_t st, const int* offs = nullptr, HeadGate gate = {});
 cudaError_t launch_co_attention_stream(const __nv_bfloat16* qkv_img, int ld_img, const __nv_bfloat16* qkv_txt, int ld_txt,
                                        int hidden, const float* img_mask_add, const float* txt_mask_add,
                                        __nv_bfloat16* ctx_txt, int ld_ctx_txt, __nv_bfloat16* ctx_img, int ld_ctx_img, int B,
                                        int T, int V, int heads, int head_dim, int pdl, int f16, cudaStream_t st,
-                                       const int* offs_t = nullptr, const int* offs_v = nullptr);
+                                       const int* offs_t = nullptr, const int* offs_v = nullptr, HeadGate gate = {});
 
 // LayerNorm(y + res) of a GEMM's fp32 output: fp32 stream out + 16-bit operand out (layernorm.cu); split16: hi | lo | hi operand (fp32-parity mode)
 cudaError_t launch_ln_residual(const float* y, int ld_y, const float* res, int ld_res, const float* gamma, const float* beta,
@@ -118,6 +130,8 @@ struct TextSrc { int32_t first, len, masked, sample; };
 cudaError_t launch_variant_text(const TextSrc* v, int n, const int* offs, int task_tokens, const int64_t* q, const int64_t* seg,
                                 const int64_t* task, int64_t mask_token, int64_t* q_out, int64_t* seg_out, int64_t* task_out,
                                 cudaStream_t st);
+// Head ablation: row b of the [n, stride] gate table = ones with element zero[b] at 0 (zero[b] = -1: all ones), every float written.
+cudaError_t launch_gate_rows(const int32_t* zero, int n, int stride, float* gate, cudaStream_t st);
 // retrieval reuse: cached encoder state rows idx[b] -> sample b of a pair plan (fp32 stream [L, H], 16-bit operand [L, H16], mask [L]);
 // the fp32 and mask copies are skipped when their pointers are null (packed poolers: the first 16-bit row of every sample)
 cudaError_t launch_gather_state(const int32_t* idx, int n_src, const float* src_f32, const void* src_16, const float* src_mask,
@@ -138,13 +152,15 @@ cudaError_t launch_gather_packed_state(const PackedStateCopy& text, const Packed
 // Packed probabilities of the fp32 attention kernel (VB200_OUT_ATTENTION_PACKED).  Sample b's query rows are [offs_q[b],
 // offs_q[b + 1]) of Q, its key rows [offs_k[b], offs_k[b + 1]) of K and of the key mask; its [heads, Lq_b, Lk_b] block goes to
 // float dst[0] + entry[0] + heads * prefix[b], where dst[0] is the destination pointer (0: no write), entry[0] the entry's float
-// offset and prefix[b] = sum over b' < b of Lq_b' * Lk_b'.  All of it lives in the plan's d_meta, filled per call.
+// offset and prefix[b] = sum over b' < b of Lq_b' * Lk_b'.  All of it lives in the plan's d_meta, filled per call.  gate: the
+// entry's head gate (gated plans); the maps are then g * p, and the head mean averages the gated maps.
 struct PackedProbs {
     const int* offs_q;
     const int* offs_k;
     const int64_t* dst;
     const int64_t* entry;
     const int64_t* prefix;
+    HeadGate gate;
 };
 // fp32 CUDA-core attention (attention_f32.cu): in_kind 0 fp32 / 1 fp16 / 2 bf16 Q, K, V; ctx_mode 0 none / 1 fp16 / 2 bf16 /
 // 3 fp16 hi | lo | hi; probs: optional [B, heads, Lq, Lk] fp32 attention probabilities.  packed (optional): a packed batch --

@@ -67,6 +67,26 @@ def _task_rows(task_tokens, n, device):
     return _to_device(task_tokens, torch.int64, device).reshape(n, -1)[:, :1].contiguous()
 
 
+def head_mask_shape(config):
+    """``(n_entries, max_heads)`` of a head mask (vb200_model_dim "head_mask_entries" / "head_mask_heads"): one entry per text
+    and image layer and two per connection layer (text-query, then image-query direction) in execution order, each with a slot
+    for every head of the configuration's widest attention."""
+    entries = config.num_hidden_layers + config.v_num_hidden_layers + 2 * len(config.v_biattention_id)
+    return entries, max(config.num_attention_heads, config.v_num_attention_heads, config.bi_num_attention_heads)
+
+
+def head_mask_rows(head_mask, batch: int, shape, device):
+    """A packed forward's ``head_mask`` as the engine's contiguous fp32 ``[batch, n_entries, max_heads]`` on ``device``:
+    ``[n_entries, max_heads]`` applies to every sample, ``[batch, n_entries, max_heads]`` gives each sample its own."""
+    m = head_mask if torch.is_tensor(head_mask) else torch.as_tensor(head_mask)
+    if tuple(m.shape) == tuple(shape):
+        m = m.unsqueeze(0).expand(batch, *shape)
+    elif tuple(m.shape) != (batch, *shape):
+        raise ValueError(f"head_mask has shape {tuple(m.shape)}: expected {tuple(shape)} (every sample) or "
+                         f"{(batch, *shape)} (per sample)")
+    return _to_device(m, torch.float32, device)
+
+
 def packed_offsets(lengths, extra: int = 0):
     """Row offsets [n + 1] of n items stored back to back with lengths[i] + extra rows each (extra = 1: the task-token row of
     a caption state)."""
@@ -246,6 +266,67 @@ def message_calls(variants, cap: int = L.ABLATION_MAX_VARIANTS):
         bxs = [u for k, u, _ in chunk if k == 2]
         r = ((toks[0], toks[-1] + 1) if toks else (0, 0)) + ((bxs[0], bxs[-1] + 1) if bxs else (0, 0))
         calls[-1].append((m, r))
+        size += n
+    return calls
+
+
+def head_messages(messages, batch: int, n_entries: int):
+    """The engine messages (``_lib.HeadAblationMessage`` fields as tuples) for ``head_ablation``'s ``messages``: each is
+    ``(family, image_begin, n_images, answer=None, entries=None)``, entries a ``(begin, end)`` range of the head mask's entry
+    order (None: every entry)."""
+    out = []
+    for i, m in enumerate(messages):
+        m = tuple(m)
+        if not 3 <= len(m) <= 5:
+            raise ValueError(f"head_ablation: message {i} has {len(m)} fields (family, image_begin, n_images, answer, entries)")
+        fam, ib, k, answer, entries = m + (None,) * (5 - len(m))
+        f = message_family(fam)
+        ib, k = int(ib), int(k)
+        want = _FAMILY_IMAGES.get(f)
+        if (k != want) if want else k < 1:
+            raise ValueError(f"head_ablation: message {i} has n_images {k} (the family reads {want or '>= 1'})")
+        if ib < 0 or ib + k > batch:
+            raise ValueError(f"head_ablation: message {i} has images [{ib}, {ib + k}) outside the batch of {batch}")
+        a = -1 if answer is None else int(answer)
+        if a < -1:
+            raise ValueError(f"head_ablation: message {i} has answer {a} (an index >= 0, or None / -1: the unablated top-1)")
+        eb, ee = (0, n_entries) if entries is None else (int(entries[0]), int(entries[1]))
+        if not 0 <= eb <= ee <= n_entries:
+            raise ValueError(f"head_ablation: message {i} has the entry range [{eb}, {ee}), reversed or outside [0, {n_entries}]")
+        out.append((f, ib, k, a, eb, ee))
+    return out
+
+
+def head_calls(variants, max_heads: int, cap: int = L.ABLATION_MAX_VARIANTS):
+    """The engine calls for a head ablation layout: ``variants`` are its records ``(message, kind, unit, samples)`` in layout order
+    (``vb200_head_ablation_layout``).  Each call is a list of pieces ``(message, (entry_begin, entry_end))`` whose variants run at
+    most ``cap`` forward samples.  Messages are kept whole where they fit; a message above ``cap`` is split at entry boundaries, each
+    piece with its own unablated variant."""
+    groups = []
+    for m, kind, unit, samples in variants:
+        if kind == 0:
+            groups.append((m, samples, {}))
+        else:
+            e = unit // max_heads
+            groups[-1][2][e] = groups[-1][2].get(e, 0) + samples
+    pieces = []
+    for m, base, entries in groups:
+        if base + max(entries.values(), default=0) > cap:
+            raise ValueError(f"head_ablation: message {m} runs {base} samples per variant, too many for {cap} per call")
+        chunk, size = [], base
+        for e, n in sorted(entries.items()):
+            if size + n > cap:
+                pieces.append((m, chunk, size))
+                chunk, size = [], base
+            chunk.append(e)
+            size += n
+        pieces.append((m, chunk, size))
+    calls, size = [], cap + 1
+    for m, chunk, n in pieces:
+        if size + n > cap:
+            calls.append([])
+            size = 0
+        calls[-1].append((m, (chunk[0], chunk[-1] + 1) if chunk else (0, 0)))
         size += n
     return calls
 
@@ -866,7 +947,8 @@ class VILBertForVLTasks(object):
     @torch.no_grad()
     def forward_packed(self, question, features, spatials, segment_ids, task_tokens, n_tokens, n_regions,
                        select: int = L.OUT_TASK_HEADS, slot: int = 0, debug_taps: bool = False, max_tokens: int = 0,
-                       max_regions: int = 0, output_all_attention_masks: bool = False, output_layer_states: bool = False):
+                       max_regions: int = 0, output_all_attention_masks: bool = False, output_layer_states: bool = False,
+                       head_mask=None):
         """One forward of B samples with their own text lengths and region counts, stored back to back without padding:
         ``question`` / ``segment_ids`` ``[sum Tin_i]``, ``features`` ``[sum V_i, F]``, ``spatials`` ``[sum V_i, 5]``,
         ``task_tokens`` ``[B, 1]``; ``n_tokens`` / ``n_regions`` (lists or CPU int tensors) give Tin_i and V_i.  Every row is real
@@ -877,7 +959,10 @@ class VILBertForVLTasks(object):
         such lists), views of one flat buffer.  ``max_tokens`` / ``max_regions`` (0: this call's maxima) are the plan's capacities:
         calls with the same batch size and capacities share one plan and CUDA graph whatever their lengths.  With
         ``output_layer_states``: ``(result, states)``, each selected entry a list of B ``[L_i, hidden]`` views of one flat buffer
-        under ``state_rows="all"``, else ``[B, hidden]``; None for an entry left out."""
+        under ``state_rows="all"``, else ``[B, hidden]``; None for an entry left out.  ``head_mask`` (``head_mask_shape(config)``
+        for every sample, or ``[B, *that]`` per sample; None: no gate) scales each attention head's context by its factor, as
+        ``pytorch_transformers``' ``attention_probs * head_mask`` does, through vb200_forward_packed_gated; the maps are then the
+        gated ones."""
         device = self._engine_device()
         nt, nr = _host_ints(n_tokens), _host_ints(n_regions)
         B = len(nt)
@@ -901,7 +986,11 @@ class VILBertForVLTasks(object):
             select, states = self._packed_states(nt, nr, select, o, device)
         inp = L.PackedInputs(B, int(max_tokens), int(max_regions), _int32s(nt), _int32s(nr), q.data_ptr(), seg.data_ptr(), f.data_ptr(),
                              s.data_ptr(), tk.data_ptr())
-        self._call("vb200_forward_packed", C.byref(inp), C.byref(o), select, slot)
+        if head_mask is None:
+            self._call("vb200_forward_packed", C.byref(inp), C.byref(o), select, slot)
+        else:
+            gate = head_mask_rows(head_mask, B, head_mask_shape(self.config), device)
+            self._call("vb200_forward_packed_gated", C.byref(inp), gate.data_ptr(), C.byref(o), select, slot)
         result = self._result(outs, B, 0, 0, debug_taps)
         result = self._with_attention(result, maps(), debug_taps) if want_attn else result
         return (result, states()) if output_layer_states else result
@@ -910,7 +999,7 @@ class VILBertForVLTasks(object):
     def forward_regions_packed(self, question, segment_ids, task_tokens, box_features, boxes, image_wh, n_tokens, n_boxes,
                                select: int = L.OUT_TASK_HEADS, slot: int = 0, max_tokens: int = 0, max_boxes: int = 0,
                                debug_taps: bool = False, return_spatials: bool = True, output_all_attention_masks: bool = False,
-                               output_layer_states: bool = False):
+                               output_layer_states: bool = False, head_mask=None):
         """``forward_regions`` with every image at its own box count and every text at its own length, stored back to back without
         padding: ``question`` / ``segment_ids`` ``[sum Tin_i]`` (text already repeated per image), ``task_tokens`` ``[B, 1]``,
         ``box_features`` ``[sum n_boxes_i, F]`` and pixel ``boxes`` ``[sum n_boxes_i, 4]`` as the detector returned them,
@@ -921,7 +1010,8 @@ class VILBertForVLTasks(object):
         bit-identical to ``forward_regions`` of that image alone.  ``max_tokens`` / ``max_boxes`` (0: this call's maxima) are the
         plan's capacities; the plan is the one ``forward_packed`` uses at ``max_regions = max_boxes + 1``.  Element 9 follows
         ``forward_packed``: the attention maps at each image's own T_i / V_i with ``output_all_attention_masks`` and
-        ``self.return_attention``, else ``[]``.  ``output_layer_states`` returns ``(result, states)`` as ``forward_packed`` does."""
+        ``self.return_attention``, else ``[]``.  ``output_layer_states`` returns ``(result, states)`` and ``head_mask`` gates the
+        heads as in ``forward_packed`` (vb200_forward_regions_packed_gated)."""
         device = self._engine_device()
         nt, nb = _host_ints(n_tokens), _host_ints(n_boxes)
         B = len(nt)
@@ -949,7 +1039,11 @@ class VILBertForVLTasks(object):
             select, states = self._packed_states(nt, [n + 1 for n in nb], select, o, device)
         inp = L.PackedRegionInputs(B, int(max_tokens), int(max_boxes), _int32s(nt), _int32s(nb), q.data_ptr(), seg.data_ptr(),
                                    tk.data_ptr(), bf.data_ptr(), bx.data_ptr(), wh.data_ptr(), sp.data_ptr() if sp is not None else None)
-        self._call("vb200_forward_regions_packed", C.byref(inp), C.byref(o), select, slot)
+        if head_mask is None:
+            self._call("vb200_forward_regions_packed", C.byref(inp), C.byref(o), select, slot)
+        else:
+            gate = head_mask_rows(head_mask, B, head_mask_shape(self.config), device)
+            self._call("vb200_forward_regions_packed_gated", C.byref(inp), gate.data_ptr(), C.byref(o), select, slot)
         result = self._result(outs, B, 0, 0, debug_taps)
         result = (self._with_attention(result, maps(), debug_taps) if want_attn else result), sp
         return (result, states()) if output_layer_states else result
@@ -1069,6 +1163,76 @@ class VILBertForVLTasks(object):
         recs = (L.AblationVariant * max(nv.value, 1))()
         L.check(lib.vb200_message_ablation_layout(self._handle, *args, recs, C.byref(nv), C.byref(nf), C.byref(ns)), self._handle)
         return [(r.message, r.kind, r.unit, r.samples, r.offset, r.length) for r in recs[:nv.value]], nf.value, arr
+
+    def _head_layout(self, n_tokens, n_boxes, msgs):
+        """vb200_head_ablation_layout: the records ``(message, kind, unit, samples, offset, length)`` and the floats they need."""
+        arr = (L.HeadAblationMessage * len(msgs))(*[L.HeadAblationMessage(*m) for m in msgs])
+        lib, nv, nf, ns = L.load(), C.c_int64(), C.c_int64(), C.c_int64()
+        args = (len(n_tokens), _int32s(n_tokens), _int32s(n_boxes), arr, len(msgs))
+        L.check(lib.vb200_head_ablation_layout(self._handle, *args, None, C.byref(nv), C.byref(nf), C.byref(ns)), self._handle)
+        recs = (L.AblationVariant * max(nv.value, 1))()
+        L.check(lib.vb200_head_ablation_layout(self._handle, *args, recs, C.byref(nv), C.byref(nf), C.byref(ns)), self._handle)
+        return [(r.message, r.kind, r.unit, r.samples, r.offset, r.length) for r in recs[:nv.value]], nf.value, arr
+
+    @torch.no_grad()
+    def head_ablation(self, question, segment_ids, task_tokens, box_features, boxes, image_wh, n_tokens, n_boxes, messages,
+                      max_tokens: int = 0, max_boxes: int = 0, slot: int = 0, return_logits: bool = False):
+        """Head ablation for every decode family (vb200_head_ablation): the packed detector-output batch of ``message_ablation`` and
+        messages ``(family, image_begin, n_images, answer=None, entries=None)``; each head of each entry in ``entries`` (a ``(begin,
+        end)`` range of ``head_mask_shape``'s entry order, None: all) is removed in turn from every sample of the message, all variants
+        in packed forwards of at most 1024 samples (a message above that is split at entry boundaries).  Returns per message a dict:
+        ``answer`` / ``prob`` / ``top1`` / ``top1_prob`` of the unablated input and, as ``[n_entries, max_heads]`` tensors,
+        ``head_prob`` (the attributed answer's probability with that head removed) and ``head_top1`` (the variant's top-1), NaN / -1
+        where no variant ran (an entry outside the range, or a slot past the entry's head count); with ``return_logits`` the segments
+        in layout order."""
+        nt, nb = _host_ints(n_tokens), _host_ints(n_boxes)
+        B = len(nt)
+        if len(nb) != B or B < 1:
+            raise ValueError("head_ablation: n_tokens and n_boxes must have the same, positive length")
+        if not messages:
+            raise ValueError("head_ablation: no messages")
+        E, H = head_mask_shape(self.config)
+        msgs = head_messages(messages, B, E)
+        device = self._engine_device()
+        F = self._dims["v_feature_size"]
+        q = _to_device(question, torch.int64, device).reshape(-1)
+        seg = _to_device(segment_ids if segment_ids is not None else torch.zeros_like(q), torch.int64, device).reshape(-1)
+        tk = _task_rows(task_tokens if task_tokens is not None else torch.zeros(B, 1, dtype=torch.int64), B, device)
+        bf = _to_device(box_features, torch.float32, device).reshape(-1, F)
+        bx = _to_device(boxes, torch.float32, device).reshape(-1, 4)
+        wh = _to_device(image_wh, torch.float32, device)
+        if q.numel() != sum(nt) or seg.numel() != sum(nt) or bf.shape[0] != sum(nb) or bx.shape[0] != sum(nb) or tuple(wh.shape) != (B, 2):
+            raise ValueError("head_ablation: question / segment_ids need sum(n_tokens) entries, box_features / boxes sum(n_boxes) "
+                             "rows, image_wh [B, 2]")
+        recs, _, _ = self._head_layout(nt, nb, msgs)
+        inp = L.PackedRegionInputs(B, int(max_tokens), int(max_boxes), _int32s(nt), _int32s(nb), q.data_ptr(), seg.data_ptr(),
+                                   tk.data_ptr(), bf.data_ptr(), bx.data_ptr(), wh.data_ptr(), None)
+        res = [dict(head_prob=torch.full((E, H), float("nan")), head_top1=torch.full((E, H), -1, dtype=torch.int64), logits=[])
+               for _ in msgs]
+        for call in head_calls([r[:4] for r in recs], H):
+            cmsgs = [msgs[p][:4] + r for p, r in call]
+            crecs, n_floats, arr = self._head_layout(nt, nb, cmsgs)
+            logits = torch.empty(n_floats, dtype=torch.float32, device=device)
+            scores = torch.empty(len(crecs), 4, dtype=torch.int32, device=device)       # vb200_ablation_score
+            self._call("vb200_head_ablation", C.byref(inp), arr, len(cmsgs), logits.data_ptr(), scores.data_ptr(), int(slot))
+            sc = scores.cpu()
+            col, top1 = sc[:, 0].tolist(), sc[:, 2].tolist()
+            prob, top1_prob = sc[:, 1].view(torch.float32).tolist(), sc[:, 3].view(torch.float32).tolist()
+            for k, (m, kind, unit, _, off, n) in enumerate(crecs):
+                r = res[call[m][0]]
+                if kind == 0:
+                    if "answer" in r:
+                        continue
+                    r.update(answer=col[k], prob=prob[k], top1=top1[k], top1_prob=top1_prob[k])
+                else:
+                    r["head_prob"][unit // H, unit % H] = prob[k]
+                    r["head_top1"][unit // H, unit % H] = top1[k]
+                r["logits"].append(logits[off:off + n])
+        for r in res:
+            logits = r.pop("logits")
+            if return_logits:
+                r["logits"] = logits
+        return res
 
     @torch.no_grad()
     def message_ablation(self, question, segment_ids, task_tokens, box_features, boxes, image_wh, n_tokens, n_boxes, messages,

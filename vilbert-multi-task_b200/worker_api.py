@@ -580,6 +580,27 @@ def custom_ablation_packed(requests, max_boxes: int = 100, *, tokens=None, boxes
     return answers
 
 
+def custom_head_ablation_packed(requests, max_boxes: int = 100, *, entries=None):
+    """Which attention heads each answer depends on: `custom_prediction_packed` (decode="device") for `custom_prediction` argument
+    tuples `(query, task, features, infos, task_id)`, plus the answer's head ablation (`model.head_ablation`) over the images the
+    answer reads, as `custom_ablation_packed` chooses them.  `entries`: one (begin, end) range of attention entries for every
+    request, or None for all.  Returns per request `{"answer": <custom_prediction_packed's answer>, "ablation": <head_ablation's
+    dict>}`, or the exception of a request that fails validation."""
+    p = pack_region_requests(requests, max_boxes=max_boxes)
+    answers = p["answers"]
+    if not p["spans"]:
+        return answers
+    args = (p["question"], p["segment_ids"], p["task_tokens"], p["box_features"], p["boxes"], p["image_wh"], p["n_tokens"], p["n_boxes"])
+    msgs = {i: m[:4] + (entries,) for i, m in ablation_messages(requests, p["spans"]).items()}
+    with model_lock:
+        out, spatials = model.forward_regions_packed(*args, select=p["select"], max_tokens=p["max_tokens"], max_boxes=p["max_boxes"])
+        ab = model.head_ablation(*args, list(msgs.values()), max_tokens=p["max_tokens"], max_boxes=p["max_boxes"])
+    answers = _answer_regions(answers, requests, out, spatials, p["spans"], p["n_tokens"], p["n_boxes"], "device")
+    for i, a in zip(msgs, ab):
+        answers[i] = {"answer": answers[i], "ablation": a}
+    return answers
+
+
 def _per_image(x, counts):
     """A per-image sequence as given, or one tensor over all images' rows split by `counts` (the reference's `.split`)."""
     if torch.is_tensor(x) or isinstance(x, np.ndarray):
