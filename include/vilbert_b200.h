@@ -631,7 +631,8 @@ typedef struct {
 
 typedef struct {
     int32_t message, kind, unit;      /* kind 0: the unablated input (unit -1); 1: masked position `unit`; 2: dropped box `unit`;
-                                         3 (head ablation): gate `unit` = entry * head_mask_heads + head at 0 */
+                                         3 (head ablation): gate `unit` = entry * head_mask_heads + head at 0;
+                                         4 (coalition ablation): coalition `unit` of the message */
     int32_t samples;                  /* forward samples this variant runs */
     int64_t offset;                   /* its segment: floats [offset, offset + length) of variant_logits */
     int32_t length;
@@ -671,6 +672,79 @@ int vb200_head_ablation_layout(vb200_handle h, int32_t batch, const int32_t* n_t
                                int64_t* n_floats, int64_t* n_samples);
 int vb200_head_ablation(vb200_handle h, const vb200_packed_region_inputs* in, const vb200_head_ablation_message* msgs /* HOST [n_msgs] */,
                         int32_t n_msgs, float* variant_logits, vb200_ablation_score* scores, int32_t slot, void* cuda_stream);
+
+/* ---- Coalition ablation: the answer with any set of units removed at once, the inputs of Shapley values and of any other
+ * coalition-based attribution.  Messages follow vb200_message_ablation (family, images, answer) for VQA, GQA, SNLI-VE, NLVR2 and
+ * retrieval; grounding is rejected (its answer is a box, which a coalition would renumber).
+ *   Units: unit u of a message is a non-empty set of question positions of image_begin's Tin ids (positions[position_offsets[u] ..
+ *   position_offsets[u + 1])) plus a set of boxes numbered across the message's images in order (boxes[box_offsets[u] ..
+ *   box_offsets[u + 1])).  No position or box belongs to two units, or twice to one; 1 <= n_units <= VB200_COALITION_MAX_UNITS.
+ *   Positions and boxes in no unit are never removed.
+ *   Coalitions: coalition c is words [c * W, c * W + W) of `coalitions`, W = ceil(n_units / 64): bit u % 64 of word u / 64 set marks
+ *   unit u PRESENT.  A coalition input removes every absent unit: its positions are replaced by mask_token in every image's question
+ *   (segment and task ids unchanged), and each of its boxes is dropped from its own image -- the kept boxes stay in their order, and
+ *   the global mean row is their mean summed in the order the region pack sums any image.  An image left with no box is the global
+ *   row alone: zero features and location [0, 0, 1, 1, 1] (the mean divides by max(boxes, 1)).
+ *   Variants of message m, in order: the full input (kind 0, unit -1), then its coalitions in the caller's order (kind 4, unit = the
+ *   coalition's index).  Every variant runs every sample of the message (an NLVR2 pair on an even sample, all K retrieval images),
+ *   and its segment is the message's segment as vb200_message_ablation gathers it.  Bit-identity: every segment equals the same
+ *   floats of vb200_forward_regions_packed run on that coalition's input in the worker's layout.
+ *   scores (DEVICE, optional): one vb200_ablation_score per variant with the arithmetic of vb200_answer_ablation; answer -1 resolves
+ *   to the full input's top-1, and a coalition's prob is its value v(S).
+ * vb200_coalition_ablation_layout writes the records and totals as vb200_message_ablation_layout does.  The samples (at most
+ * VB200_ABLATION_MAX_VARIANTS per call, NLVR2 messages first) run as one forward of the PACKED plan message ablation uses, rounded up
+ * to a multiple of 64 with fillers; the masked-position bitmaps and kept-box lists are staged with the other descriptors.
+ * VB200_ERR_INVALID, with nothing enqueued and a message naming the message or unit, for every rejection of vb200_message_ablation
+ * that applies (split_fp32 and pre-training engines included), grounding, n_units outside [1, VB200_COALITION_MAX_UNITS], n_coalitions
+ * < 0, an empty unit, a position outside [0, Tin) or a box outside [0, the message's boxes), a position or box in two units, a
+ * coalition bit at or past n_units, and NULL unit or coalition arrays.  Asynchronous and stream-ordered as vb200_answer_ablation. */
+#define VB200_COALITION_MAX_UNITS 1024
+typedef struct {
+    int32_t family;                   /* VB200_DECODE_* except grounding */
+    int32_t image_begin, n_images;    /* the message's images in the batch, as vb200_ablation_message */
+    int32_t answer;                   /* attributed index in the message's segment; -1: the full input's top-1 */
+    int32_t n_units;
+    const int32_t* position_offsets;  /* HOST [n_units + 1], from 0 */
+    const int32_t* positions;         /* HOST: each unit's question positions */
+    const int32_t* box_offsets;       /* HOST [n_units + 1], from 0 */
+    const int32_t* boxes;             /* HOST: each unit's boxes, numbered across the message's images */
+    int32_t n_coalitions;
+    const uint64_t* coalitions;       /* HOST [n_coalitions, ceil(n_units / 64)] presence bitmaps */
+} vb200_coalition_message;
+
+int vb200_coalition_ablation_layout(vb200_handle h, int32_t batch, const int32_t* n_tokens /* HOST [batch] */,
+                                    const int32_t* n_boxes /* HOST [batch] */, const vb200_coalition_message* msgs /* HOST [n_msgs] */,
+                                    int32_t n_msgs, vb200_ablation_variant* variants /* HOST, NULL: counts only */, int64_t* n_variants,
+                                    int64_t* n_floats, int64_t* n_samples);
+int vb200_coalition_ablation(vb200_handle h, const vb200_packed_region_inputs* in, const vb200_coalition_message* msgs /* HOST [n_msgs] */,
+                             int32_t n_msgs, int64_t mask_token, float* variant_logits, vb200_ablation_score* scores, int32_t slot,
+                             void* cuda_stream);
+
+/* ---- Shapley values from permutation-sampled coalition values, on the device (one CTA per message, float64 throughout).
+ * Message i has n = n_units units, P = n_perm permutations and groups of g = group consecutive permutations (1, or 2 for antithetic
+ * pairs; g divides P).  perm + perm_offset: DEVICE int32 [P, n], each row a permutation of 0 .. n-1.  values + value_offset: DEVICE
+ * fp32 [2 + P (n - 1)]: v(empty), v(all), then for p = 0 .. P-1 the chain v(S^p_1) .. v(S^p_{n-1}), S^p_j the first j units of row p.
+ * With c[p][0] = v(empty), c[p][n] = v(all), c[p][j] = chain value j of row p, every value widened to double:
+ *   d[p][u] = c[p][j + 1] - c[p][j] for u = perm[p][j];
+ *   s = 0; for p = 0 .. P-1: s = s + d[p][u];              phi_u = s / P;
+ *   G = P / g; for q = 0 .. G-1: m = 0; for i = 0 .. g-1: m = m + d[q g + i][u];  m = m / g;  t = m - phi_u;  ss = ss + t * t
+ *     (ss from 0);
+ *   stderr_u = sqrt((ss / (G - 1)) / G), NaN when G < 2.
+ * Each step is one correctly rounded float64 operation in that order (no fused multiply-add), so a numpy restatement in float64
+ * reproduces it bit for bit.  phi + out_offset and stderr + out_offset: DEVICE fp32 [n], the float64 results rounded to nearest.  A
+ * permutation row that is not a permutation gives NaN in both outputs for every unit of its message.
+ * VB200_ERR_INVALID, with nothing enqueued, for n_msgs < 1, n_units outside [1, VB200_COALITION_MAX_UNITS], n_perm < 1, group not 1
+ * or 2, n_perm not a multiple of group, a negative offset, NULL pointers, or phi / stderr / values not 4-byte aligned.  The
+ * descriptors are staged as vb200_decode_answers stages its messages; asynchronous on cuda_stream. */
+typedef struct {
+    int32_t n_units, n_perm, group;
+    int64_t perm_offset;              /* int32 elements of perm where the message's [n_perm, n_units] table starts */
+    int64_t value_offset;             /* floats of values where its 2 + n_perm * (n_units - 1) values start */
+    int64_t out_offset;               /* floats of phi and of stderr where its n_units outputs start */
+} vb200_shapley_message;
+
+int vb200_shapley_values(vb200_handle h, const vb200_shapley_message* msgs /* HOST [n_msgs] */, int32_t n_msgs, const int32_t* perm,
+                         const float* values, float* phi, float* stderr_out, void* cuda_stream);
 
 /* ---- Detector-region selection: the feature extraction step of the reference worker (worker.py:123-176) on the detector's raw heads,
  * for every image of a batch in one call, written straight into the packed box_features / boxes that vb200_forward_regions_packed reads.

@@ -140,9 +140,28 @@ class AblationMessage(C.Structure):
 
 class AblationVariant(C.Structure):
     """vb200_ablation_variant: one variant in the engine's order -- its message, kind (0 unablated, 1 masked position, 2 dropped
-    box) and unit, the forward samples it runs and its segment [offset, offset + length) of variant_logits."""
+    box, 3 removed head, 4 coalition) and unit, the forward samples it runs and its segment [offset, offset + length) of variant_logits."""
     _fields_ = [("message", C.c_int32), ("kind", C.c_int32), ("unit", C.c_int32), ("samples", C.c_int32), ("offset", C.c_int64),
                 ("length", C.c_int32)]
+
+
+COALITION_MAX_UNITS = 1024
+
+
+class CoalitionMessage(C.Structure):
+    """vb200_coalition_message: one answer by its images and attributed index (-1: the full input's top-1), its units (HOST int32
+    offset / item arrays of question positions and boxes) and its coalitions (HOST uint64 presence bitmaps, ceil(n_units / 64) words
+    each)."""
+    _fields_ = [("family", C.c_int32), ("image_begin", C.c_int32), ("n_images", C.c_int32), ("answer", C.c_int32),
+                ("n_units", C.c_int32), ("position_offsets", C.c_void_p), ("positions", C.c_void_p), ("box_offsets", C.c_void_p),
+                ("boxes", C.c_void_p), ("n_coalitions", C.c_int32), ("coalitions", C.c_void_p)]
+
+
+class ShapleyMessage(C.Structure):
+    """vb200_shapley_message: units, permutations and group size of one message, and where its permutation table, values and
+    outputs start in the call's device arrays."""
+    _fields_ = [("n_units", C.c_int32), ("n_perm", C.c_int32), ("group", C.c_int32), ("perm_offset", C.c_int64),
+                ("value_offset", C.c_int64), ("out_offset", C.c_int64)]
 
 
 class Detections(C.Structure):
@@ -203,7 +222,8 @@ EXPORTS = ["vb200_abi_version", "vb200_create", "vb200_destroy", "vb200_last_err
            "vb200_gather_packed_state", "vb200_decode_answers", "vb200_decode_answers_host", "vb200_select_regions",
            "vb200_pretraining_heads", "vb200_create_pretraining", "vb200_pretraining_objectives", "vb200_answer_ablation",
            "vb200_message_ablation_layout", "vb200_message_ablation", "vb200_forward_packed_gated", "vb200_forward_regions_packed_gated",
-           "vb200_head_ablation_layout", "vb200_head_ablation"]
+           "vb200_head_ablation_layout", "vb200_head_ablation", "vb200_coalition_ablation_layout", "vb200_coalition_ablation",
+           "vb200_shapley_values"]
 
 _lib = None
 
@@ -296,6 +316,10 @@ def load():
     lib.vb200_head_ablation_layout.argtypes = [vp, i32, vp, vp, C.POINTER(HeadAblationMessage), i32, vp, C.POINTER(C.c_int64),
                                                C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     lib.vb200_head_ablation.argtypes = [vp, C.POINTER(PackedRegionInputs), C.POINTER(HeadAblationMessage), i32, vp, vp, i32, vp]
+    lib.vb200_coalition_ablation_layout.argtypes = [vp, i32, vp, vp, C.POINTER(CoalitionMessage), i32, vp, C.POINTER(C.c_int64),
+                                                    C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
+    lib.vb200_coalition_ablation.argtypes = [vp, C.POINTER(PackedRegionInputs), C.POINTER(CoalitionMessage), i32, i64, vp, vp, i32, vp]
+    lib.vb200_shapley_values.argtypes = [vp, C.POINTER(ShapleyMessage), i32, vp, vp, vp, vp, vp]
     for name in EXPORTS:
         if name not in ("vb200_last_error",):
             getattr(lib, name).restype = C.c_int

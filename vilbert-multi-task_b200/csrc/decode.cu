@@ -151,4 +151,59 @@ cudaError_t launch_segment_gather(const SegmentDesc* descs, int n, const Segment
     return launch_ex(segment_gather_kernel, dim3(n), dim3(128), 0, 0, st, descs, heads, out);
 }
 
+// Permutation-sampled Shapley values: one CTA per message, thread u owns unit u.  For each permutation p the CTA inverts row p into
+// shared memory (inv[perm[p][j]] = j), so unit u finds its position j and its marginal c[p][j+1] - c[p][j] in float64.  Pass 1 sums
+// the marginals over p in order; pass 2 recomputes them group by group for the two-pass standard error.  Every float64 operation is
+// an explicitly rounded intrinsic, so no multiply-add is contracted and numpy's sequential float64 arithmetic gives the same bits.  A
+// row that is not a permutation of 0 .. n-1 (some unit has no position) gives NaN for every unit of the message.
+__global__ void __launch_bounds__(kShapleyMaxUnits)
+shapley_values_kernel(const ShapleyDesc* __restrict__ descs) {
+    __shared__ int inv[kShapleyMaxUnits];
+    const ShapleyDesc d = descs[blockIdx.x];
+    const int n = d.n_units, P = d.n_perm, g = d.group, u = threadIdx.x;
+    const float* __restrict__ v = d.values;
+    auto chain = [&](int p, int j) -> double {                 // c[p][j]: v(empty) at 0, v(all) at n, the chain in between
+        return static_cast<double>(j == 0 ? v[0] : j == n ? v[1] : v[2 + static_cast<int64_t>(p) * (n - 1) + (j - 1)]);
+    };
+    bool bad = false;
+    auto marginal = [&](int p) -> double {                     // unit u's marginal in permutation p (every thread must call)
+        const int32_t* __restrict__ row = d.perm + static_cast<int64_t>(p) * n;
+        __syncthreads();                                       // the previous permutation's reads of inv are done
+        if (u < n) inv[u] = -1;
+        __syncthreads();
+        if (u < n) {
+            const int w = row[u];
+            if (w >= 0 && w < n) inv[w] = u;
+        }
+        __syncthreads();
+        if (u >= n) return 0.0;
+        const int j = inv[u];
+        if (j < 0 || row[j] != u) { bad = true; return 0.0; }
+        return __dsub_rn(chain(p, j + 1), chain(p, j));
+    };
+    double sum = 0.0;
+    for (int p = 0; p < P; ++p) sum = __dadd_rn(sum, marginal(p));
+    const double phi = __ddiv_rn(sum, static_cast<double>(P));
+    const int G = P / g;
+    double ss = 0.0;
+    for (int q = 0; q < G; ++q) {
+        double m = 0.0;
+        for (int i = 0; i < g; ++i) m = __dadd_rn(m, marginal(q * g + i));
+        m = __ddiv_rn(m, static_cast<double>(g));
+        const double t = __dsub_rn(m, phi);
+        ss = __dadd_rn(ss, __dmul_rn(t, t));
+    }
+    bad = __syncthreads_or(bad) != 0;
+    if (u >= n) return;
+    const double nan = __longlong_as_double(0x7ff8000000000000ll);
+    const double se = G < 2 ? nan : __dsqrt_rn(__ddiv_rn(__ddiv_rn(ss, static_cast<double>(G - 1)), static_cast<double>(G)));
+    d.phi[u] = static_cast<float>(bad ? nan : phi);
+    d.stderr_out[u] = static_cast<float>(bad ? nan : se);
+}
+
+cudaError_t launch_shapley_values(const ShapleyDesc* descs, int n, cudaStream_t st) {
+    if (n < 1) return cudaErrorInvalidValue;
+    return launch_ex(shapley_values_kernel, dim3(n), dim3(kShapleyMaxUnits), 0, 0, st, descs);
+}
+
 }  // namespace vb

@@ -153,27 +153,33 @@ image_pack_kernel(const float* __restrict__ feats, const float* __restrict__ loc
 // grid (B, ceil(F / 1024) + 1): the last grid row writes the location columns, the masks and the optional spatials copy.
 // Packed batch (offs = the plan's image row offsets [B + 1]): image b owns regions [offs[b], offs[b+1]) -- its mean row, then its
 // offs[b+1] - offs[b] - 1 boxes, which start at detector row offs[b] - b (one global row per image) -- every row is real, and
-// spatials_out is packed [sum V_i, 5].  With src (answer ablation), output image b is instead source image src[b].image's boxes from
-// detector row src[b].box0 on, with box src[b].skip (>= 0) left out: the boxes after it move up one row, and the mean sums the kept
-// boxes in the same order, so the rows are those of the reduced image packed alone.
+// spatials_out is packed [sum V_i, 5].  With src (the ablation calls), output image b is instead source image src[b].image's boxes
+// named by its kept list (kept + src[b].kept, detector rows relative to src[b].box0, in order; src[b].kept = -1: every box): the
+// mean sums the kept boxes in the order any image's boxes are summed, so the rows are those of the reduced image packed alone.
+// No kept box gives the global row alone (zero features, location [0, 0, 1, 1, 1]).
 __global__ void __launch_bounds__(128)
 region_pack_kernel(const float* __restrict__ box_feats, const float* __restrict__ boxes, const float* __restrict__ image_wh,
                    const int32_t* __restrict__ num_boxes, __nv_bfloat16* __restrict__ a_out, float* __restrict__ mask_add,
                    float* __restrict__ spatials_out, int n, int F, int Kp, int f16, int split16, const int* __restrict__ offs,
-                   const RegionSrc* __restrict__ src_img) {
+                   const RegionSrc* __restrict__ src_img, const int32_t* __restrict__ kept) {
     const int b = blockIdx.x;
-    int row0, box0, nb, img = b, skip = -1;                          // first operand row, first detector row, valid boxes, source
-    if (offs == nullptr) {                                           //   image, skipped detector box
+    int row0, box0, nb, img = b;                                     // first operand row, first detector row, valid boxes, source image
+    const int32_t* rows = nullptr;                                   // kept detector rows (relative to box0), null: every box in order
+    if (offs == nullptr) {
         row0 = b * (n + 1); box0 = b * n;
         nb = num_boxes ? num_boxes[b] : n;
         nb = nb < 0 ? 0 : (nb > n ? n : nb);
     } else {
         row0 = offs[b]; box0 = row0 - b;
         n = nb = offs[b + 1] - row0 - 1;
-        if (src_img != nullptr) { const RegionSrc s = src_img[b]; img = s.image; box0 = s.box0; skip = s.skip; }
+        if (src_img != nullptr) {
+            const RegionSrc s = src_img[b];
+            img = s.image; box0 = s.box0;
+            if (s.kept >= 0) rows = kept + s.kept;
+        }
     }
     // detector row of output box r
-    auto det_row = [&](int r) { return static_cast<size_t>(box0) + r + (skip >= 0 && r >= skip ? 1 : 0); };
+    auto det_row = [&](int r) { return static_cast<size_t>(box0) + (rows != nullptr ? rows[r] : r); };
     const int V = n + 1;
     const size_t ld = static_cast<size_t>(split16 ? 3 * Kp : Kp);
     auto put = [&](int row, int i, const float (&x)[8]) {           // 8 columns [8i, 8i+8) of operand row `row`
@@ -494,27 +500,30 @@ cudaError_t launch_image_pack(const float* feats, const float* loc, const uint8_
 
 cudaError_t launch_region_pack(const float* box_feats, const float* boxes, const float* image_wh, const int32_t* num_boxes,
                                __nv_bfloat16* a_out, float* mask_add, float* spatials_out, int B, int n, int F, int Kp, int f16,
-                               int split16, cudaStream_t st, const int* offs, const RegionSrc* src) {
+                               int split16, cudaStream_t st, const int* offs, const RegionSrc* src, const int32_t* kept) {
     if (B < 1 || (offs == nullptr && n < 1) || F % 8 != 0 || Kp % 8 != 0 || Kp < F + 8 || (split16 && (!f16 || (Kp & 63))) ||
-        (offs != nullptr && (num_boxes != nullptr || split16)) || (src != nullptr && offs == nullptr))
+        (offs != nullptr && (num_boxes != nullptr || split16)) || (src != nullptr && offs == nullptr) || (kept != nullptr && src == nullptr))
         return cudaErrorInvalidValue;
     const dim3 grid(B, (F / 8 + 127) / 128 + 1);
     region_pack_kernel<<<grid, 128, 0, st>>>(box_feats, boxes, image_wh, num_boxes, a_out, mask_add, spatials_out, n, F, Kp, f16, split16,
-                                             offs, src);
+                                             offs, src, kept);
     return cudaGetLastError();
 }
 
-// Answer ablation's text inputs: variant k's token ids, segment ids and task id copied from its sample's single copy, position
-// `masked` (>= 0) replaced by mask_token, written where the packed text embedding reads variant k (offs[k] - k task_tokens).
+// The ablation calls' text inputs: variant k's token ids, segment ids and task id copied from its sample's single copy, every
+// position whose bit is set in the call's bitmap (words from mask + masked, masked >= 0) replaced by mask_token, written where the
+// packed text embedding reads variant k (offs[k] - k task_tokens).
 __global__ void __launch_bounds__(128)
 variant_text_kernel(const TextSrc* __restrict__ v, const int* __restrict__ offs, int task_tokens, const int64_t* __restrict__ q,
                     const int64_t* __restrict__ seg, const int64_t* __restrict__ task, int64_t mask_token, int64_t* __restrict__ q_out,
-                    int64_t* __restrict__ seg_out, int64_t* __restrict__ task_out) {
+                    int64_t* __restrict__ seg_out, int64_t* __restrict__ task_out, const uint32_t* __restrict__ mask) {
     const int k = blockIdx.x;
     const TextSrc d = v[k];
     const int out0 = offs[k] - k * task_tokens;
+    const uint32_t* bits = d.masked >= 0 ? mask + d.masked : nullptr;
     for (int t = threadIdx.x; t < d.len; t += blockDim.x) {
-        q_out[out0 + t] = t == d.masked ? mask_token : q[d.first + t];
+        const bool masked = bits != nullptr && ((bits[t >> 5] >> (t & 31)) & 1u);
+        q_out[out0 + t] = masked ? mask_token : q[d.first + t];
         seg_out[out0 + t] = seg[d.first + t];
     }
     if (threadIdx.x == 0 && task_tokens) task_out[k] = task[d.sample];
@@ -522,9 +531,9 @@ variant_text_kernel(const TextSrc* __restrict__ v, const int* __restrict__ offs,
 
 cudaError_t launch_variant_text(const TextSrc* v, int n, const int* offs, int task_tokens, const int64_t* q, const int64_t* seg,
                                 const int64_t* task, int64_t mask_token, int64_t* q_out, int64_t* seg_out, int64_t* task_out,
-                                cudaStream_t st) {
+                                cudaStream_t st, const uint32_t* mask) {
     if (n < 1 || (task_tokens && (task == nullptr || task_out == nullptr))) return cudaErrorInvalidValue;
-    variant_text_kernel<<<n, 128, 0, st>>>(v, offs, task_tokens, q, seg, task, mask_token, q_out, seg_out, task_out);
+    variant_text_kernel<<<n, 128, 0, st>>>(v, offs, task_tokens, q, seg, task, mask_token, q_out, seg_out, task_out, mask);
     return cudaGetLastError();
 }
 

@@ -1913,11 +1913,11 @@ struct vb200_engine {
     // ---- packed batches (run_packed has staged the call's d_meta ahead of these, in stream order)
     // Packed detector output: the region-pack kernel writes every image's mean row and boxes at the plan's image offsets (the same
     // rows embed_regions writes for that image alone)
-    // (src: answer ablation's per-image sources, see launch_region_pack)
+    // (src / kept: the ablation calls' per-image sources and kept-box lists, see launch_region_pack)
     void pack_regions_packed(Plan& pl, const float* box_feats, const float* boxes, const float* image_wh, float* spatials_out, int rows,
-                             cudaStream_t st, const vb::RegionSrc* src = nullptr) {
+                             cudaStream_t st, const vb::RegionSrc* src = nullptr, const int32_t* kept = nullptr) {
         CUDA_CHECK(vb::launch_region_pack(box_feats, boxes, image_wh, nullptr, pl.img_a, pl.mask_v, spatials_out, pl.B, 0, cfg.v_feat,
-                                          pl.kp, opt.act_fp16, 0, st, pl.offs_v(), src));
+                                          pl.kp, opt.act_fp16, 0, st, pl.offs_v(), src, kept));
         zero_tail(pl.img_a, rows, pl.B * pl.V, pl.kp, st);
     }
     // packed pair suffix: every pair's rows are gathered from the packed caption / image states into the plan's packed buffers
@@ -2067,11 +2067,12 @@ struct vb200_engine {
         dec_ws.release(st);
     }
     // the caller releases dec_ws after its last decode kernel
-    const vb::DecodeDesc* stage_decode(const std::vector<vb::DecodeDesc>& d, cudaStream_t st) {
-        const size_t bytes = d.size() * sizeof(vb::DecodeDesc);
+    template <typename Desc>
+    const Desc* stage_decode(const std::vector<Desc>& d, cudaStream_t st) {
+        const size_t bytes = d.size() * sizeof(Desc);
         char* dst = dec_ws.acquire(bytes, st);
         dec_in.stage(bytes, st, [&](char* h, const auto& put) { memcpy(h, d.data(), bytes); put(dst, 0, bytes); });
-        return reinterpret_cast<const vb::DecodeDesc*>(dst);
+        return reinterpret_cast<const Desc*>(dst);
     }
     // ---- attention relevance: lengths and the map selection are checked, and the descriptors built, before anything is enqueued
     void attention_relevance(const float* maps, int batch, const int32_t* n_tokens, const int32_t* n_regions, int packed,
@@ -2146,17 +2147,66 @@ struct vb200_engine {
         std::vector<AblVariant> v;
         std::vector<vb::TextSrc> text;
         std::vector<vb::RegionSrc> img;
+        std::vector<uint32_t> mask;    // masked-position bitmaps, one word-aligned run per masked question (TextSrc::masked)
+        std::vector<int32_t> kept;     // kept-box lists, one run per reduced image (RegionSrc::kept)
         std::vector<int32_t> tin, nv;
         std::vector<int32_t> gate;     // head ablation: per sample the gate table element (entry * gate_heads + head) set to 0, or -1
         int64_t n_floats = 0;
         bool grounding = false;
         bool gated = false;            // head ablation: the samples run the gated plan
     };
+    // Coalition message i's units and coalitions checked against its question length T and box count nb; pos_unit / box_unit get
+    // each position's and box's unit (-1: in none).
+    static void check_coalitions(const char* api, int i, const vb200_coalition_message& c, int T, int nb, std::vector<int>& pos_unit,
+                                 std::vector<int>& box_unit) {
+        if (c.family == VB200_DECODE_GROUNDING)
+            fail(VB200_ERR_INVALID, "%s: message %d is a grounding message (its answer is a box, which a coalition would renumber)", api, i);
+        if (c.n_units < 1 || c.n_units > VB200_COALITION_MAX_UNITS)
+            fail(VB200_ERR_INVALID, "%s: message %d has n_units %d outside [1, %d]", api, i, c.n_units, VB200_COALITION_MAX_UNITS);
+        if (c.n_coalitions < 0) fail(VB200_ERR_INVALID, "%s: message %d has n_coalitions %d (must be >= 0)", api, i, c.n_coalitions);
+        if (!c.position_offsets || !c.box_offsets || (c.n_coalitions > 0 && !c.coalitions))
+            fail(VB200_ERR_INVALID, "%s: message %d has a NULL position_offsets / box_offsets / coalitions array", api, i);
+        pos_unit.assign(T, -1);
+        box_unit.assign(nb, -1);
+        for (int pass = 0; pass < 2; ++pass) {
+            const bool text = pass == 0;
+            const int32_t* offs = text ? c.position_offsets : c.box_offsets;
+            const int32_t* item = text ? c.positions : c.boxes;
+            std::vector<int>& owner = text ? pos_unit : box_unit;
+            const char* what = text ? "position" : "box";
+            if (offs[0] != 0) fail(VB200_ERR_INVALID, "%s: message %d: %s_offsets[0] is %d (must be 0)", api, i, what, offs[0]);
+            for (int u = 0; u < c.n_units; ++u) {
+                if (offs[u + 1] < offs[u])
+                    fail(VB200_ERR_INVALID, "%s: message %d unit %d: %s_offsets decrease (%d after %d)", api, i, u, what, offs[u + 1], offs[u]);
+                if (offs[u + 1] > offs[u] && item == nullptr)
+                    fail(VB200_ERR_INVALID, "%s: message %d unit %d lists %ss, but the %ss array is NULL", api, i, u, what, what);
+                for (int32_t k = offs[u]; k < offs[u + 1]; ++k) {
+                    const int x = item[k], lim = text ? T : nb;
+                    if (x < 0 || x >= lim)
+                        fail(VB200_ERR_INVALID, "%s: message %d unit %d has %s %d outside [0, %d)", api, i, u, what, x, lim);
+                    if (owner[x] >= 0)
+                        fail(VB200_ERR_INVALID, "%s: message %d unit %d has %s %d, which unit %d already holds", api, i, u, what, x, owner[x]);
+                    owner[x] = u;
+                }
+            }
+        }
+        for (int u = 0; u < c.n_units; ++u)
+            if (c.position_offsets[u + 1] == c.position_offsets[u] && c.box_offsets[u + 1] == c.box_offsets[u])
+                fail(VB200_ERR_INVALID, "%s: message %d unit %d is empty (no position and no box)", api, i, u);
+        const size_t W = (static_cast<size_t>(c.n_units) + 63) / 64;
+        const uint64_t past = c.n_units % 64 ? ~0ull << (c.n_units % 64) : 0ull;
+        for (int s = 0; s < c.n_coalitions; ++s)
+            if (c.coalitions[s * W + W - 1] & past)
+                fail(VB200_ERR_INVALID, "%s: message %d coalition %d sets a bit at or past n_units %d", api, i, s, c.n_units);
+    }
     // The messages checked against the batch's lengths and laid out; no sample cap (run_ablation applies it).  entries (head
     // ablation, one [begin, end) per message): after its token and box variants, each message gets one variant per head of every
     // entry in the range (kind 3, unit entry * gate_heads + head): the message's samples, unablated, with that one gate at 0.
+    // coal (coalition ablation, one per message, whose token and box ranges are empty): after the full input, one variant per
+    // coalition (kind 4, unit = its index): every sample of the message with the coalition's absent units removed.
     AblLayout ablation_layout(const char* api, int batch, const int32_t* n_tokens, const int32_t* n_boxes, const vb200_ablation_message* msgs,
-                              int n_msgs, const std::vector<std::array<int, 2>>* entries = nullptr) const {
+                              int n_msgs, const std::vector<std::array<int, 2>>* entries = nullptr,
+                              const vb200_coalition_message* coal = nullptr) const {
         if (n_tokens == nullptr || n_boxes == nullptr || msgs == nullptr) fail(VB200_ERR_INVALID, "%s: n_tokens / n_boxes / msgs is NULL", api);
         if (batch < 1) fail(VB200_ERR_INVALID, "%s: batch must be positive (batch = %d)", api, batch);
         if (n_msgs < 1) fail(VB200_ERR_INVALID, "%s: n_msgs must be positive (n_msgs = %d)", api, n_msgs);
@@ -2176,13 +2226,35 @@ struct vb200_engine {
             L.gated = true;
             for (int kind : attention_kinds(schedule)) entry_heads.push_back(kind == 0 ? cfg.heads : kind == 1 ? cfg.v_heads : cfg.bi_heads);
         }
-        auto sample = [&](const vb200_ablation_message& m, int masked, int image, int skip, int gate = -1) {
+        std::vector<std::vector<int>> pos_unit(coal ? n_msgs : 0), box_unit(coal ? n_msgs : 0);   // owning unit, -1: none
+        // one sample: message m's question with the positions of bitmap run `masked` replaced (-1: none), image `image` with the
+        // nbox boxes of kept-list run `kept` (-1: all its boxes)
+        auto sample = [&](const vb200_ablation_message& m, int masked, int image, int kept = -1, int nbox = -1, int gate = -1) {
             L.gate.push_back(gate);
             L.text.push_back({tok0[m.image_begin], n_tokens[m.image_begin], masked, m.image_begin});
-            L.img.push_back({image, box0[image], skip});
+            L.img.push_back({image, box0[image], kept});
             L.tin.push_back(n_tokens[m.image_begin]);
-            L.nv.push_back(n_boxes[image] - (skip >= 0 ? 1 : 0) + 1);
+            L.nv.push_back((kept < 0 ? n_boxes[image] : nbox) + 1);
             return static_cast<int>(L.text.size()) - 1;
+        };
+        auto mask_run = [&](int tin, const std::vector<int>& pos) {          // a bitmap run of tin bits, `pos` set
+            if (pos.empty()) return -1;
+            const int at = static_cast<int>(L.mask.size());
+            L.mask.resize(L.mask.size() + (tin + 31) / 32, 0u);
+            for (int p : pos) L.mask[at + p / 32] |= 1u << (p % 32);
+            return at;
+        };
+        auto reduced = [&](const vb200_ablation_message& m, int masked, int image, const std::vector<int32_t>& rows) {   // `rows` kept
+            if (static_cast<int>(rows.size()) == n_boxes[image]) return sample(m, masked, image);
+            const int at = static_cast<int>(L.kept.size());
+            L.kept.insert(L.kept.end(), rows.begin(), rows.end());
+            return sample(m, masked, image, at, static_cast<int>(rows.size()));
+        };
+        auto without = [&](const vb200_ablation_message& m, int image, int skip) {   // image without box `skip`
+            std::vector<int32_t> rows;
+            for (int r = 0; r < n_boxes[image]; ++r)
+                if (r != skip) rows.push_back(r);
+            return reduced(m, -1, image, rows);
         };
         for (int pass = 0; pass < 2; ++pass)
             for (int i = 0; i < n_msgs; ++i) {
@@ -2226,6 +2298,7 @@ struct vb200_engine {
                             fail(VB200_ERR_INVALID, "%s: message %d has the entry range [%d, %d), reversed or outside [0, %d]", api, i, r[0],
                                  r[1], static_cast<int>(entry_heads.size()));
                     }
+                    if (coal != nullptr) check_coalitions(api, i, coal[i], T, nb, pos_unit[i], box_unit[i]);
                 }
                 if ((f == VB200_DECODE_NLVR2) != (pass == 0)) continue;
                 std::vector<AblVariant>& out = per[i];
@@ -2239,14 +2312,14 @@ struct vb200_engine {
                     return {head, first, width, -1, 0, 0};
                 };
                 auto all_images = [&](int masked, int gate = -1) {
-                    const int first = sample(m, masked, ib, -1, gate);
-                    for (int k = 1; k < K; ++k) sample(m, masked, ib + k, -1, gate);
+                    const int first = sample(m, masked, ib, -1, -1, gate);
+                    for (int k = 1; k < K; ++k) sample(m, masked, ib + k, -1, -1, gate);
                     return first;
                 };
                 const int base = all_images(-1);
                 variant(0, -1, K, seg(base), -1);
                 for (int p = m.token_begin; p < m.token_end; ++p) {
-                    const int first = all_images(p);
+                    const int first = all_images(mask_run(n_tokens[ib], {p}));
                     variant(1, p, K, seg(first), -1);
                 }
                 for (int u = m.box_begin; u < m.box_end; ++u) {
@@ -2254,16 +2327,16 @@ struct vb200_engine {
                     while (box0[ib + k + 1] - box0[ib] <= u) ++k;
                     const int j = u - (box0[ib + k] - box0[ib]);
                     if (f == VB200_DECODE_NLVR2) {
-                        const int first = sample(m, -1, ib, k == 0 ? j : -1);
-                        sample(m, -1, ib + 1, k == 1 ? j : -1);
+                        const int first = k == 0 ? without(m, ib, j) : sample(m, -1, ib);
+                        if (k == 1) without(m, ib + 1, j); else sample(m, -1, ib + 1);
                         variant(2, u, 2, seg(first), -1);
                     } else if (f == VB200_DECODE_RETRIEVAL) {     // the unablated segment, element k from the changed image alone
                         vb::SegmentDesc s = seg(base);
                         s.sub = k;
-                        s.sub_row = sample(m, -1, ib + k, j);
+                        s.sub_row = without(m, ib + k, j);
                         variant(2, u, 1, s, -1);
                     } else {
-                        const int first = sample(m, -1, ib, j);
+                        const int first = without(m, ib, j);
                         variant(2, u, 1, seg(first), f == VB200_DECODE_GROUNDING ? j + 1 : -1);
                     }
                 }
@@ -2273,6 +2346,28 @@ struct vb200_engine {
                             const int unit = e * gate_heads() + h;
                             variant(3, unit, K, seg(all_images(-1, unit)), -1);
                         }
+                if (coal != nullptr) {
+                    const vb200_coalition_message& c = coal[i];
+                    const size_t W = (static_cast<size_t>(c.n_units) + 63) / 64;
+                    for (int s = 0; s < c.n_coalitions; ++s) {
+                        const uint64_t* bits = c.coalitions + s * W;
+                        auto absent = [&](int unit) { return unit >= 0 && !((bits[unit >> 6] >> (unit & 63)) & 1u); };
+                        std::vector<int> masked;
+                        for (int t = 0; t < n_tokens[ib]; ++t)
+                            if (absent(pos_unit[i][t])) masked.push_back(t);
+                        const int mw = mask_run(n_tokens[ib], masked);
+                        int first = -1;
+                        for (int k = 0; k < K; ++k) {
+                            const int b0 = box0[ib + k] - box0[ib];
+                            std::vector<int32_t> rows;
+                            for (int r = 0; r < n_boxes[ib + k]; ++r)
+                                if (!absent(box_unit[i][b0 + r])) rows.push_back(r);
+                            const int x = reduced(m, mw, ib + k, rows);
+                            if (k == 0) first = x;
+                        }
+                        variant(4, s, K, seg(first), -1);
+                    }
+                }
                 L.grounding |= f == VB200_DECODE_GROUNDING;
             }
         std::vector<int64_t> vrow(L.nv.size() + 1, 0);       // each sample's first vision_logit row
@@ -2315,7 +2410,8 @@ struct vb200_engine {
         auto carve = [&](size_t bytes) { const size_t a = at; at += (bytes + 255) / 256 * 256; return a; };
         const size_t o_text = carve(n_pad * sizeof(vb::TextSrc)), o_img = carve(n_pad * sizeof(vb::RegionSrc));
         const size_t o_seg = carve(n_var * sizeof(vb::SegmentDesc));
-        const size_t o_gate = L.gated ? carve(n_pad * sizeof(int32_t)) : 0, staged = at;
+        const size_t o_gate = L.gated ? carve(n_pad * sizeof(int32_t)) : 0;
+        const size_t o_mask = carve(L.mask.size() * sizeof(uint32_t)), o_kept = carve(L.kept.size() * sizeof(int32_t)), staged = at;
         const size_t o_q = carve(sum_tin * 8), o_ids = carve(sum_tin * 8), o_task = carve(static_cast<size_t>(n_pad) * 8);
         CUDA_CHECK(cudaSetDevice(opt.device));
         char* ws = abl_ws.acquire(at, st);
@@ -2324,6 +2420,8 @@ struct vb200_engine {
             memcpy(h + o_img, L.img.data(), n_pad * sizeof(vb::RegionSrc));
             memcpy(h + o_seg, seg.data(), n_var * sizeof(vb::SegmentDesc));
             if (L.gated) memcpy(h + o_gate, L.gate.data(), n_pad * sizeof(int32_t));
+            if (!L.mask.empty()) memcpy(h + o_mask, L.mask.data(), L.mask.size() * sizeof(uint32_t));
+            if (!L.kept.empty()) memcpy(h + o_kept, L.kept.data(), L.kept.size() * sizeof(int32_t));
             put(ws, 0, staged);
         });
         const auto* text_d = reinterpret_cast<const vb::TextSrc*>(ws + o_text);
@@ -2337,9 +2435,10 @@ struct vb200_engine {
         const Plan& pl = run_packed(api, PACKED, {"variant", n_pad, L.tin.data(), in->max_tokens, L.nv.data(), max_regions}, select, slot,
                                     &none, {}, st, [&](Plan& p, const PackedBatch& b, cudaStream_t s) {
             CUDA_CHECK(vb::launch_variant_text(text_d, n_pad, p.offs_t(), task, in->question, in->segment_ids, in->task_tokens, mask_token,
-                                               q, ids, tk, s));
+                                               q, ids, tk, s, reinterpret_cast<const uint32_t*>(ws + o_mask)));
             embed_text(p, q, ids, nullptr, tk, b.rows_t(), s);
-            pack_regions_packed(p, in->box_features, in->boxes, in->image_wh, nullptr, b.rows_v(), s, img_d);
+            pack_regions_packed(p, in->box_features, in->boxes, in->image_wh, nullptr, b.rows_v(), s, img_d,
+                                reinterpret_cast<const int32_t*>(ws + o_kept));
             if (L.gated)
                 CUDA_CHECK(vb::launch_gate_rows(reinterpret_cast<const int32_t*>(ws + o_gate), n_pad, p.gate_entries * p.gate_heads, p.gate, s));
         }, nullptr, L.gated);
@@ -2474,6 +2573,61 @@ struct vb200_engine {
             fail(VB200_ERR_INVALID, "%s: n_variants / n_floats / n_samples is NULL", api);
         if (pretraining) fail(VB200_ERR_INVALID, "%s: a pre-training engine has no task head to attribute an answer of", api);
         put_layout(ablation_layout(api, batch, n_tokens, n_boxes, msgs, n_msgs), variants, n_variants, n_floats, n_samples);
+    }
+    // vb200_coalition_ablation[_layout]: each coalition message as a message with no token or box range, plus its units and coalitions
+    AblLayout coalition_layout(const char* api, int batch, const int32_t* n_tokens, const int32_t* n_boxes, const vb200_coalition_message* msgs,
+                               int n_msgs) const {
+        if (msgs == nullptr) fail(VB200_ERR_INVALID, "%s: msgs is NULL", api);
+        if (n_msgs < 1) fail(VB200_ERR_INVALID, "%s: n_msgs must be positive (n_msgs = %d)", api, n_msgs);
+        std::vector<vb200_ablation_message> m;
+        for (int i = 0; i < n_msgs; ++i) m.push_back({msgs[i].family, msgs[i].image_begin, msgs[i].n_images, msgs[i].answer, 0, 0, 0, 0});
+        return ablation_layout(api, batch, n_tokens, n_boxes, m.data(), n_msgs, nullptr, msgs);
+    }
+    void coalition_ablation_layout(int batch, const int32_t* n_tokens, const int32_t* n_boxes, const vb200_coalition_message* msgs, int n_msgs,
+                                   vb200_ablation_variant* variants, int64_t* n_variants, int64_t* n_floats, int64_t* n_samples) const {
+        const char* api = "vb200_coalition_ablation_layout";
+        if (n_variants == nullptr || n_floats == nullptr || n_samples == nullptr)
+            fail(VB200_ERR_INVALID, "%s: n_variants / n_floats / n_samples is NULL", api);
+        if (pretraining) fail(VB200_ERR_INVALID, "%s: a pre-training engine has no task head to attribute an answer of", api);
+        put_layout(coalition_layout(api, batch, n_tokens, n_boxes, msgs, n_msgs), variants, n_variants, n_floats, n_samples);
+    }
+    void coalition_ablation(const vb200_packed_region_inputs* in, const vb200_coalition_message* msgs, int n_msgs, int64_t mask_token,
+                            float* variant_logits, vb200_ablation_score* scores, int slot, cudaStream_t st) {
+        const char* api = "vb200_coalition_ablation";
+        if (in == nullptr || msgs == nullptr || variant_logits == nullptr) fail(VB200_ERR_INVALID, "%s: in / msgs / variant_logits is NULL", api);
+        if (x3) fail(VB200_ERR_INVALID, "%s: packed batches are not supported in split_fp32 (fp32x) mode", api);
+        if (pretraining) fail(VB200_ERR_INVALID, "%s: a pre-training engine has no task head to attribute an answer of", api);
+        if (reinterpret_cast<uintptr_t>(variant_logits) & 3) fail(VB200_ERR_INVALID, "%s: variant_logits is not 4-byte aligned", api);
+        if (reinterpret_cast<uintptr_t>(scores) & 3) fail(VB200_ERR_INVALID, "%s: scores is not 4-byte aligned", api);
+        const int max_regions = check_ablation_inputs(api, in, mask_token, slot);
+        run_ablation(api, in, coalition_layout(api, in->batch, in->n_tokens, in->n_boxes, msgs, n_msgs), max_regions, mask_token,
+                     variant_logits, scores, slot, st);
+    }
+    // vb200_shapley_values: every descriptor is checked before anything is enqueued
+    void shapley_values(const vb200_shapley_message* msgs, int n_msgs, const int32_t* perm, const float* values, float* phi, float* se,
+                        cudaStream_t st) {
+        const char* api = "vb200_shapley_values";
+        if (msgs == nullptr || perm == nullptr || values == nullptr || phi == nullptr || se == nullptr)
+            fail(VB200_ERR_INVALID, "%s: msgs / perm / values / phi / stderr is NULL", api);
+        if (n_msgs < 1) fail(VB200_ERR_INVALID, "%s: n_msgs must be positive (n_msgs = %d)", api, n_msgs);
+        if ((reinterpret_cast<uintptr_t>(perm) | reinterpret_cast<uintptr_t>(values) | reinterpret_cast<uintptr_t>(phi) |
+             reinterpret_cast<uintptr_t>(se)) & 3)
+            fail(VB200_ERR_INVALID, "%s: perm / values / phi / stderr is not 4-byte aligned", api);
+        std::vector<vb::ShapleyDesc> d(n_msgs);
+        for (int i = 0; i < n_msgs; ++i) {
+            const vb200_shapley_message& m = msgs[i];
+            if (m.n_units < 1 || m.n_units > VB200_COALITION_MAX_UNITS)
+                fail(VB200_ERR_INVALID, "%s: message %d has n_units %d outside [1, %d]", api, i, m.n_units, VB200_COALITION_MAX_UNITS);
+            if (m.n_perm < 1) fail(VB200_ERR_INVALID, "%s: message %d has n_perm %d (must be >= 1)", api, i, m.n_perm);
+            if (m.group != 1 && m.group != 2) fail(VB200_ERR_INVALID, "%s: message %d has group %d (1 or 2)", api, i, m.group);
+            if (m.n_perm % m.group) fail(VB200_ERR_INVALID, "%s: message %d has n_perm %d, not a multiple of group %d", api, i, m.n_perm, m.group);
+            if (m.perm_offset < 0 || m.value_offset < 0 || m.out_offset < 0)
+                fail(VB200_ERR_INVALID, "%s: message %d has a negative offset", api, i);
+            d[i] = {perm + m.perm_offset, values + m.value_offset, phi + m.out_offset, se + m.out_offset, m.n_units, m.n_perm, m.group};
+        }
+        CUDA_CHECK(cudaSetDevice(opt.device));
+        CUDA_CHECK(vb::launch_shapley_values(stage_decode(d, st), n_msgs, st));
+        dec_ws.release(st);
     }
     // ---- region selection: every descriptor is checked before anything is enqueued
     void select_regions(const vb200_detections* imgs, int n, const vb200_select_params* p, const vb200_selected* out, cudaStream_t st) {
@@ -3181,6 +3335,27 @@ int vb200_head_ablation_layout(vb200_handle h, int32_t batch, const int32_t* n_t
                                int64_t* n_floats, int64_t* n_samples) {
     if (h == nullptr) return VB200_ERR_INVALID;
     return guard(h, [&] { h->head_ablation_layout(batch, n_tokens, n_boxes, msgs, n_msgs, variants, n_variants, n_floats, n_samples); });
+}
+
+int vb200_coalition_ablation_layout(vb200_handle h, int32_t batch, const int32_t* n_tokens, const int32_t* n_boxes,
+                                    const vb200_coalition_message* msgs, int32_t n_msgs, vb200_ablation_variant* variants,
+                                    int64_t* n_variants, int64_t* n_floats, int64_t* n_samples) {
+    if (h == nullptr) return VB200_ERR_INVALID;
+    return guard(h, [&] { h->coalition_ablation_layout(batch, n_tokens, n_boxes, msgs, n_msgs, variants, n_variants, n_floats, n_samples); });
+}
+
+int vb200_coalition_ablation(vb200_handle h, const vb200_packed_region_inputs* in, const vb200_coalition_message* msgs, int32_t n_msgs,
+                             int64_t mask_token, float* variant_logits, vb200_ablation_score* scores, int32_t slot, void* cuda_stream) {
+    if (h == nullptr) return VB200_ERR_INVALID;
+    return guard(h, [&] {
+        h->coalition_ablation(in, msgs, n_msgs, mask_token, variant_logits, scores, slot, static_cast<cudaStream_t>(cuda_stream));
+    });
+}
+
+int vb200_shapley_values(vb200_handle h, const vb200_shapley_message* msgs, int32_t n_msgs, const int32_t* perm, const float* values,
+                         float* phi, float* stderr_out, void* cuda_stream) {
+    if (h == nullptr) return VB200_ERR_INVALID;
+    return guard(h, [&] { h->shapley_values(msgs, n_msgs, perm, values, phi, stderr_out, static_cast<cudaStream_t>(cuda_stream)); });
 }
 
 int vb200_head_ablation(vb200_handle h, const vb200_packed_region_inputs* in, const vb200_head_ablation_message* msgs, int32_t n_msgs,

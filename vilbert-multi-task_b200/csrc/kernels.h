@@ -117,19 +117,23 @@ cudaError_t launch_image_pack(const float* feats, const float* loc, const uint8_
 // Packed batches (offs != nullptr): offs = device [B + 1] image row offsets (V_b = boxes_b + 1 regions per image), box_features /
 // boxes hold image b's V_b - 1 boxes from detector row offs[b] - b, every row is real, n and num_boxes are unused (num_boxes must be
 // null, and split16 0), spatials_out is [offs[B], 5].
-// src (packed only, answer and message ablation): output image b is image src[b].image's offs[b+1] - offs[b] - 1 + (skip >= 0) detector boxes
-// from row src[b].box0, box src[b].skip left out (-1: none).
-struct RegionSrc { int32_t image, box0, skip; };
+// src (packed only, the ablation calls): output image b holds nb = offs[b+1] - offs[b] - 1 detector boxes of source image
+// src[b].image, box r being detector row src[b].box0 + kept[src[b].kept + r] (src[b].kept = -1: box0 + r, every box in order).  A kept
+// list names any subset of the image's boxes in their original order; nb = 0 is the "no boxes" input: the global row alone, with
+// zero features (the mean divides by max(nb, 1)) and location [0, 0, 1, 1, 1].
+struct RegionSrc { int32_t image, box0, kept; };
 cudaError_t launch_region_pack(const float* box_feats, const float* boxes, const float* image_wh, const int32_t* num_boxes,
                                __nv_bfloat16* a_out, float* mask_add, float* spatials_out, int B, int n, int F, int Kp, int f16,
-                               int split16, cudaStream_t st, const int* offs = nullptr, const RegionSrc* src = nullptr);
-// Answer ablation's text ids: variant k (one CTA each, n of them) = tokens [first, first + len) of the packed question / segment
-// ids, position `masked` (-1: none) replaced by mask_token, and task id task[sample] -> the packed layout of the plan's text
-// offsets offs (device [n + 1]) in q_out / seg_out / task_out.
+                               int split16, cudaStream_t st, const int* offs = nullptr, const RegionSrc* src = nullptr,
+                               const int32_t* kept = nullptr);
+// The ablation calls' text ids: variant k (one CTA each, n of them) = tokens [first, first + len) of the packed question / segment
+// ids, every position t whose bit is set in the call's bitmap replaced by mask_token, and task id task[sample] -> the packed layout
+// of the plan's text offsets offs (device [n + 1]) in q_out / seg_out / task_out.  Position t's bit is bit t % 32 of word
+// mask[masked + t / 32]; masked = -1: no position is replaced.
 struct TextSrc { int32_t first, len, masked, sample; };
 cudaError_t launch_variant_text(const TextSrc* v, int n, const int* offs, int task_tokens, const int64_t* q, const int64_t* seg,
                                 const int64_t* task, int64_t mask_token, int64_t* q_out, int64_t* seg_out, int64_t* task_out,
-                                cudaStream_t st);
+                                cudaStream_t st, const uint32_t* mask = nullptr);
 // Head ablation: row b of the [n, stride] gate table = ones with element zero[b] at 0 (zero[b] = -1: all ones), every float written.
 cudaError_t launch_gate_rows(const int32_t* zero, int n, int stride, float* gate, cudaStream_t st);
 // retrieval reuse: cached encoder state rows idx[b] -> sample b of a pair plan (fp32 stream [L, H], 16-bit operand [L, H16], mask [L]);
@@ -221,6 +225,11 @@ constexpr int kSegmentHeads = 7;
 struct SegmentHeads { const float* p[kSegmentHeads]; int ld[kSegmentHeads], cols[kSegmentHeads]; };
 struct SegmentDesc { int32_t head, row, len, sub, sub_row; int64_t dst; };
 cudaError_t launch_segment_gather(const SegmentDesc* descs, int n, const SegmentHeads& heads, float* out, cudaStream_t st);
+// Shapley estimates (decode.cu, vb200_shapley_values): one CTA per message, the arithmetic documented at vb200_shapley_values.
+// perm: [n_perm, n_units] int32, values: 2 + n_perm * (n_units - 1) floats, phi / stderr: n_units floats each.
+struct ShapleyDesc { const int32_t* perm; const float* values; float* phi; float* stderr_out; int32_t n_units, n_perm, group; };
+constexpr int kShapleyMaxUnits = 1024;
+cudaError_t launch_shapley_values(const ShapleyDesc* descs, int n, cudaStream_t st);
 // Attention relevance (relevance.cu, vb200_attention_relevance): per sample b (one CTA) the rollout rows of the text CLS row and the
 // image global row, [2, T_b + V_b] at relevance + out.  Entry e of the maps starts at float `offset` and holds sample b's
 // [heads, Lq_b, Lk_b] block at heads * prefix[k] (k 0 text layers, 1 image layers, 2 both directions of a connection layer); kinds

@@ -15,8 +15,10 @@ from __future__ import annotations
 
 import ctypes as C
 import json
+import math
 from typing import Dict, Optional
 
+import numpy as np
 import torch
 
 from . import _lib as L
@@ -329,6 +331,164 @@ def head_calls(variants, max_heads: int, cap: int = L.ABLATION_MAX_VARIANTS):
         calls[-1].append((m, (chunk[0], chunk[-1] + 1) if chunk else (0, 0)))
         size += n
     return calls
+
+
+# the families a coalition can attribute (grounding's answer is a box, which a coalition would renumber)
+COALITION_FAMILIES = {L.DECODE_VQA, L.DECODE_GQA, L.DECODE_NLVR2, L.DECODE_SNLI_VE, L.DECODE_RETRIEVAL}
+
+
+def coalition_messages(messages, batch: int):
+    """The engine messages ``(family, image_begin, n_images, answer)`` for ``coalition_ablation`` / ``shapley``'s ``messages``:
+    each is ``(family or task id, image_begin, n_images, answer=None)``, any decode family except grounding."""
+    out = []
+    for i, m in enumerate(messages):
+        m = tuple(m)
+        if not 3 <= len(m) <= 4:
+            raise ValueError(f"coalition_ablation: message {i} has {len(m)} fields (family, image_begin, n_images, answer)")
+        fam, ib, k, answer = m + (None,) * (4 - len(m))
+        f = message_family(fam)
+        if f not in COALITION_FAMILIES:
+            raise ValueError(f"coalition_ablation: message {i} is a grounding message (its answer is a box, which a coalition would "
+                             "renumber)")
+        ib, k = int(ib), int(k)
+        want = _FAMILY_IMAGES.get(f)
+        if (k != want) if want else k < 1:
+            raise ValueError(f"coalition_ablation: message {i} has n_images {k} (the family reads {want or '>= 1'})")
+        if ib < 0 or ib + k > batch:
+            raise ValueError(f"coalition_ablation: message {i} has images [{ib}, {ib + k}) outside the batch of {batch}")
+        a = -1 if answer is None else int(answer)
+        if a < -1:
+            raise ValueError(f"coalition_ablation: message {i} has answer {a} (an index >= 0, or None / -1: the full input's top-1)")
+        out.append((f, ib, k, a))
+    return out
+
+
+def coalition_units(units, tin: int, boxes: int, i: int = 0):
+    """One message's units as ``(positions, boxes)`` tuples of ints.  ``units`` None: one unit per question position 1 .. Tin - 2 and
+    one per box of the message's ``boxes`` (numbered across its images); else a list of ``(positions, boxes)`` groups, e.g. the word
+    pieces of one word or the boxes of one class.  Each unit non-empty, no position or box in two units, at most
+    ``_lib.COALITION_MAX_UNITS`` units."""
+    if units is None:
+        out = [((p,), ()) for p in range(1, max(1, tin - 1))] + [((), (b,)) for b in range(boxes)]
+    else:
+        out = []
+        for u, g in enumerate(units):
+            if len(g) != 2:
+                raise ValueError(f"coalition_ablation: message {i} unit {u} needs (positions, boxes), got {g!r}")
+            out.append((tuple(int(x) for x in g[0]), tuple(int(x) for x in g[1])))
+    if not 1 <= len(out) <= L.COALITION_MAX_UNITS:
+        raise ValueError(f"coalition_ablation: message {i} has {len(out)} units (1 .. {L.COALITION_MAX_UNITS})")
+    seen_p, seen_b = {}, {}
+    for u, (ps, bs) in enumerate(out):
+        if not ps and not bs:
+            raise ValueError(f"coalition_ablation: message {i} unit {u} is empty (no position and no box)")
+        for x, lim, seen, what in [(p, tin, seen_p, "position") for p in ps] + [(b, boxes, seen_b, "box") for b in bs]:
+            if not 0 <= x < lim:
+                raise ValueError(f"coalition_ablation: message {i} unit {u} has {what} {x} outside [0, {lim})")
+            if x in seen:
+                raise ValueError(f"coalition_ablation: message {i} unit {u} has {what} {x}, which unit {seen[x]} already holds")
+            seen[x] = u
+    return out
+
+
+def coalition_bitmaps(present, n_units: int):
+    """Presence bitmaps of coalitions: ``present`` is a bool / 0-1 array [n_coalitions, n_units] (True: the unit is present).
+    Returns a uint64 numpy array [n_coalitions, ceil(n_units / 64)], bit u % 64 of word u // 64 for unit u."""
+    a = np.asarray(present, dtype=bool)
+    if a.ndim != 2 or a.shape[1] != n_units:
+        raise ValueError(f"coalition_ablation: coalitions need shape [n_coalitions, {n_units}], got {tuple(a.shape)}")
+    W = (n_units + 63) // 64
+    padded = np.zeros((a.shape[0], W * 64), dtype=np.uint64)
+    padded[:, :n_units] = a
+    weights = np.left_shift(np.uint64(1), np.arange(64, dtype=np.uint64))
+    return (padded.reshape(-1, W, 64) * weights).sum(axis=2, dtype=np.uint64)
+
+
+def coalition_calls(variants, cap: int = L.ABLATION_MAX_VARIANTS):
+    """The engine calls for a coalition ablation layout: ``variants`` are its records ``(message, kind, unit, samples)`` in layout
+    order (``vb200_coalition_ablation_layout``).  Each call is a list of pieces ``(message, (coalition_begin, coalition_end))``
+    whose variants run at most ``cap`` forward samples; a message above that is split into runs of its coalitions, each piece with
+    its own full-input variant."""
+    groups = []
+    for m, kind, unit, samples in variants:
+        if kind == 0:
+            groups.append((m, samples, 0))
+        else:
+            groups[-1] = groups[-1][:2] + (groups[-1][2] + 1,)
+    pieces = []
+    for m, base, n in groups:
+        if base * (2 if n else 1) > cap:
+            raise ValueError(f"coalition_ablation: message {m} runs {base} samples per variant, too many for {cap} per call")
+        per = max(1, (cap - base) // base)                 # coalitions beside the full input in one piece
+        for c in range(0, max(n, 1), per):
+            pieces.append((m, (c, min(n, c + per)), base * (1 + min(n, c + per) - c)))
+    calls, size = [], cap + 1
+    for m, r, n in pieces:
+        if size + n > cap:
+            calls.append([])
+            size = 0
+        calls[-1].append((m, r))
+        size += n
+    return calls
+
+
+def shapley_permutations(n_units: int, permutations: int, generator, antithetic: bool = True):
+    """``permutations`` rows of a permutation of 0 .. n_units - 1 drawn with ``torch.randperm`` from ``generator`` (a CPU
+    ``torch.Generator``); with ``antithetic`` row 2i + 1 is row 2i reversed and ``permutations`` must be even.  int64 [P, n]."""
+    P = int(permutations)
+    if P < 1:
+        raise ValueError(f"shapley: permutations must be >= 1, got {P}")
+    if antithetic and P % 2:
+        raise ValueError(f"shapley: antithetic sampling needs an even number of permutations, got {P}")
+    rows = []
+    for _ in range(P // 2 if antithetic else P):
+        r = torch.randperm(n_units, generator=generator)
+        rows += [r, r.flip(0)] if antithetic else [r]
+    return torch.stack(rows)
+
+
+def shapley_chain(perm):
+    """The coalitions a permutation estimate evaluates beyond the full input: the empty coalition, then for each row p of ``perm``
+    the chain S^p_1 .. S^p_{n-1} (the first j units of row p).  bool [1 + P (n - 1), n], True: present."""
+    perm = torch.as_tensor(perm, dtype=torch.int64)
+    P, n = perm.shape
+    rank = torch.empty_like(perm)
+    rank.scatter_(1, perm, torch.arange(n).expand(P, n).contiguous())        # rank[p, u]: position of unit u in row p
+    j = torch.arange(1, n).view(1, -1, 1)
+    chain = rank.view(P, 1, n) < j                                            # [P, n - 1, n]
+    return torch.cat([torch.zeros(1, n, dtype=torch.bool), chain.reshape(-1, n)])
+
+
+def shapley_reference(values, perm, group: int, dtype=np.float32):
+    """numpy float64 restatement of vb200_shapley_values for one message: ``values`` [2 + P (n - 1)] (v(empty), v(all), the chains),
+    ``perm`` [P, n].  Returns (phi, stderr), each step the header's, in its order, rounded to ``dtype`` (float32: the device's
+    outputs; float64: before that rounding)."""
+    v = np.asarray(values, dtype=np.float32).astype(np.float64)
+    perm = np.asarray(perm, dtype=np.int64)
+    P, n = perm.shape
+    c = np.empty((P, n + 1), dtype=np.float64)
+    c[:, 0], c[:, n] = v[0], v[1]
+    c[:, 1:n] = v[2:].reshape(P, n - 1)
+    d = np.empty((P, n), dtype=np.float64)
+    for p in range(P):
+        for j in range(n):
+            d[p, perm[p, j]] = c[p, j + 1] - c[p, j]
+    G = P // group
+    phi, se = np.empty(n), np.empty(n)
+    for u in range(n):
+        s = 0.0
+        for p in range(P):
+            s = s + float(d[p, u])
+        phi[u] = s / P
+        ss = 0.0
+        for q in range(G):
+            m = 0.0
+            for i in range(group):
+                m = m + float(d[q * group + i, u])
+            t = m / group - phi[u]
+            ss = ss + t * t
+        se[u] = math.sqrt(ss / (G - 1) / G) if G >= 2 else float("nan")
+    return phi.astype(dtype), se.astype(dtype)
 
 
 def attention_list(kinds, layout_entry, entries):
@@ -1310,6 +1470,166 @@ class VILBertForVLTasks(object):
             if return_logits:
                 r["logits"] = logits
         return res
+
+    # ------------------------------------------------------------------ coalition ablation and Shapley values
+    def _coalition_layout(self, n_tokens, n_boxes, arr):
+        """vb200_coalition_ablation_layout: the records ``(message, kind, unit, samples, offset, length)`` and the floats they need."""
+        lib, nv, nf, ns = L.load(), C.c_int64(), C.c_int64(), C.c_int64()
+        args = (len(n_tokens), _int32s(n_tokens), _int32s(n_boxes), arr, len(arr))
+        L.check(lib.vb200_coalition_ablation_layout(self._handle, *args, None, C.byref(nv), C.byref(nf), C.byref(ns)), self._handle)
+        recs = (L.AblationVariant * max(nv.value, 1))()
+        L.check(lib.vb200_coalition_ablation_layout(self._handle, *args, recs, C.byref(nv), C.byref(nf), C.byref(ns)), self._handle)
+        return [(r.message, r.kind, r.unit, r.samples, r.offset, r.length) for r in recs[:nv.value]], nf.value
+
+    @staticmethod
+    def _coalition_structs(msgs, units, bitmaps):
+        """``_lib.CoalitionMessage`` array for engine messages ``msgs`` with their units and uint64 bitmaps; the arrays the structs
+        point at are returned with it and must outlive every call that reads it."""
+        keep, out = [], []
+        for m, us, bm in zip(msgs, units, bitmaps):
+            po = np.cumsum([0] + [len(p) for p, _ in us]).astype(np.int32)
+            bo = np.cumsum([0] + [len(b) for _, b in us]).astype(np.int32)
+            ps = np.array([x for p, _ in us for x in p] or [0], dtype=np.int32)
+            bs = np.array([x for _, b in us for x in b] or [0], dtype=np.int32)
+            bm = np.ascontiguousarray(bm, dtype=np.uint64)
+            keep += [po, bo, ps, bs, bm]
+            out.append(L.CoalitionMessage(*m, len(us), po.ctypes.data, ps.ctypes.data, bo.ctypes.data, bs.ctypes.data, bm.shape[0],
+                                          bm.ctypes.data if bm.shape[0] else None))
+        return (L.CoalitionMessage * len(out))(*out), keep
+
+    def _coalition_run(self, name, question, segment_ids, task_tokens, box_features, boxes, image_wh, n_tokens, n_boxes, messages, units,
+                       coalitions, mask_token, max_tokens, max_boxes, slot, return_logits):
+        """What ``coalition_ablation`` and ``shapley`` share: the messages checked, the layout split along its records into calls of
+        at most 1024 samples, and per message its full input's score and its coalitions' probabilities and top-1s as device tensors."""
+        nt, nb = _host_ints(n_tokens), _host_ints(n_boxes)
+        B = len(nt)
+        if len(nb) != B or B < 1:
+            raise ValueError(f"{name}: n_tokens and n_boxes must have the same, positive length")
+        if not messages:
+            raise ValueError(f"{name}: no messages")
+        msgs = coalition_messages(messages, B)
+        if len(units) != len(msgs) or len(coalitions) != len(msgs):
+            raise ValueError(f"{name}: units and coalitions need one entry per message ({len(msgs)})")
+        us = [coalition_units(u, nt[ib], sum(nb[ib:ib + k]), i) for i, (u, (_, ib, k, _)) in enumerate(zip(units, msgs))]
+        bms = [coalition_bitmaps(c, len(u)) for c, u in zip(coalitions, us)]
+        device = self._engine_device()
+        F = self._dims["v_feature_size"]
+        q = _to_device(question, torch.int64, device).reshape(-1)
+        seg = _to_device(segment_ids if segment_ids is not None else torch.zeros_like(q), torch.int64, device).reshape(-1)
+        tk = _task_rows(task_tokens if task_tokens is not None else torch.zeros(B, 1, dtype=torch.int64), B, device)
+        bf = _to_device(box_features, torch.float32, device).reshape(-1, F)
+        bx = _to_device(boxes, torch.float32, device).reshape(-1, 4)
+        wh = _to_device(image_wh, torch.float32, device)
+        if q.numel() != sum(nt) or seg.numel() != sum(nt) or bf.shape[0] != sum(nb) or bx.shape[0] != sum(nb) or tuple(wh.shape) != (B, 2):
+            raise ValueError(f"{name}: question / segment_ids need sum(n_tokens) entries, box_features / boxes sum(n_boxes) rows, "
+                             "image_wh [B, 2]")
+        arr, keep = self._coalition_structs(msgs, us, bms)
+        recs, _ = self._coalition_layout(nt, nb, arr)
+        inp = L.PackedRegionInputs(B, int(max_tokens), int(max_boxes), _int32s(nt), _int32s(nb), q.data_ptr(), seg.data_ptr(),
+                                   tk.data_ptr(), bf.data_ptr(), bx.data_ptr(), wh.data_ptr(), None)
+        res = [dict(units=u, prob_d=[], top1_d=[], logits=[], samples=0) for u in us]
+        for call in coalition_calls([r[:4] for r in recs]):
+            carr, ckeep = self._coalition_structs([msgs[m] for m, _ in call], [us[m] for m, _ in call],
+                                                  [bms[m][c0:c1] for m, (c0, c1) in call])
+            crecs, n_floats = self._coalition_layout(nt, nb, carr)
+            logits = torch.empty(n_floats, dtype=torch.float32, device=device)
+            scores = torch.empty(len(crecs), 4, dtype=torch.int32, device=device)       # vb200_ablation_score
+            self._call("vb200_coalition_ablation", C.byref(inp), carr, len(carr), int(mask_token), logits.data_ptr(), scores.data_ptr(),
+                       int(slot))
+            prob, top1 = scores[:, 1].view(torch.float32), scores[:, 2]
+            at = 0
+            for j, (m, (c0, c1)) in enumerate(call):
+                r = res[m]
+                n = c1 - c0
+                if "answer" not in r:
+                    sc = scores[at].cpu()
+                    r.update(answer=int(sc[0]), prob=float(sc[1:2].view(torch.float32)), top1=int(sc[2]),
+                             top1_prob=float(sc[3:4].view(torch.float32)))
+                    if return_logits:
+                        r["logits"].append(logits[crecs[at][4]:crecs[at][4] + crecs[at][5]])
+                r["prob_d"].append(prob[at + 1:at + 1 + n])
+                r["top1_d"].append(top1[at + 1:at + 1 + n])
+                if return_logits:
+                    r["logits"] += [logits[o:o + k] for *_, o, k in crecs[at + 1:at + 1 + n]]
+                r["samples"] += sum(c[3] for c in crecs[at:at + 1 + n])
+                at += 1 + n
+            del carr, ckeep
+        del arr, keep
+        for r in res:
+            r["prob_d"] = torch.cat(r["prob_d"])
+            r["top1_d"] = torch.cat(r["top1_d"])
+        return res
+
+    @torch.no_grad()
+    def coalition_ablation(self, question, segment_ids, task_tokens, box_features, boxes, image_wh, n_tokens, n_boxes, messages, units,
+                           coalitions, mask_token: int = 103, max_tokens: int = 0, max_boxes: int = 0, slot: int = 0,
+                           return_logits: bool = False):
+        """The answer with any set of units removed at once (vb200_coalition_ablation): the packed detector-output batch of
+        ``message_ablation``, ``messages`` ``(family or task id, image_begin, n_images, answer=None)`` of every family but grounding,
+        per message its ``units`` (None: the defaults of ``coalition_units``; else ``(positions, boxes)`` groups, boxes numbered across
+        the message's images) and its ``coalitions``, a bool [n_coalitions, n_units] array (True: the unit is present).  An absent
+        unit's positions are replaced by ``mask_token`` in every image and its boxes dropped from their images.  Calls above the
+        engine's 1024 forward samples are split along its layout records (``coalition_calls``), each piece with its full input.
+        Returns per message ``answer`` / ``prob`` / ``top1`` / ``top1_prob`` of the full input, ``units``, ``coalition_prob`` (the
+        attributed answer's probability, v(S)) and ``coalition_top1`` as CPU tensors, ``samples`` (the forward samples run); with
+        ``return_logits`` the segments (device tensors), the full input's first, then the coalitions' in order."""
+        res = self._coalition_run("coalition_ablation", question, segment_ids, task_tokens, box_features, boxes, image_wh, n_tokens,
+                                  n_boxes, messages, units, coalitions, mask_token, max_tokens, max_boxes, slot, return_logits)
+        for r in res:
+            r["coalition_prob"] = r.pop("prob_d").cpu()
+            r["coalition_top1"] = r.pop("top1_d").cpu().to(torch.int64)
+            logits = r.pop("logits")
+            if return_logits:
+                r["logits"] = logits
+        return res
+
+    @torch.no_grad()
+    def shapley(self, question, segment_ids, task_tokens, box_features, boxes, image_wh, n_tokens, n_boxes, messages, units=None,
+                permutations: int = 8, seed: int = 0, antithetic: bool = True, mask_token: int = 103, max_tokens: int = 0,
+                max_boxes: int = 0, slot: int = 0):
+        """Permutation-sampled Shapley values of each message's units for its answer (``coalition_ablation``, then
+        vb200_shapley_values on the device).  ``messages`` as for ``coalition_ablation``; ``units`` None (the defaults of
+        ``coalition_units`` for every message) or one entry per message (None or ``(positions, boxes)`` groups).  ``permutations`` P
+        rows per message are drawn message by message from one CPU ``torch.Generator`` seeded with ``seed``; with ``antithetic`` row
+        2i + 1 reverses row 2i and the standard error is taken over the P / 2 pair means.  v(empty) and v(all) are evaluated once per
+        message and the P (n - 1) interior chain coalitions after them.  Returns per message ``answer``, ``prob`` (v(all)),
+        ``empty_prob`` (v(empty)), ``units``, ``phi`` and ``stderr`` (float32 CPU tensors [n_units]), ``perm`` and ``samples`` (the
+        forward samples run)."""
+        msgs = coalition_messages(messages, len(_host_ints(n_tokens)))
+        units = [None] * len(msgs) if units is None else list(units)
+        if len(units) != len(msgs):
+            raise ValueError(f"shapley: units need one entry per message ({len(msgs)})")
+        nt, nb = _host_ints(n_tokens), _host_ints(n_boxes)
+        if len(nb) != len(nt):
+            raise ValueError("shapley: n_tokens and n_boxes must have the same, positive length")
+        units = [coalition_units(u, nt[ib], sum(nb[ib:ib + k]), i) for i, (u, (_, ib, k, _)) in enumerate(zip(units, msgs))]
+        gen = torch.Generator().manual_seed(int(seed))
+        perms = [shapley_permutations(len(u), permutations, gen, antithetic) for u in units]
+        res = self._coalition_run("shapley", question, segment_ids, task_tokens, box_features, boxes, image_wh, nt, nb,
+                                  [m for m in msgs], units, [shapley_chain(p) for p in perms], mask_token, max_tokens, max_boxes, slot,
+                                  False)
+        device = self._engine_device()
+        g = 2 if antithetic else 1
+        values, descs, at_v, at_p, at_o = [], [], 0, 0, 0
+        for r, p in zip(res, perms):
+            P, n = p.shape
+            full = torch.tensor([r["prob"]], dtype=torch.float32, device=device)
+            values.append(torch.cat([r["prob_d"][:1], full, r["prob_d"][1:]]))
+            descs.append(L.ShapleyMessage(n, P, g, at_p, at_v, at_o))
+            at_v, at_p, at_o = at_v + 2 + P * (n - 1), at_p + P * n, at_o + n
+        vals = torch.cat(values).contiguous()
+        perm_d = torch.cat([p.reshape(-1) for p in perms]).to(device=device, dtype=torch.int32)
+        phi = torch.empty(at_o, dtype=torch.float32, device=device)
+        se = torch.empty(at_o, dtype=torch.float32, device=device)
+        arr = (L.ShapleyMessage * len(descs))(*descs)
+        self._call("vb200_shapley_values", arr, len(descs), perm_d.data_ptr(), vals.data_ptr(), phi.data_ptr(), se.data_ptr())
+        phi, se = phi.cpu(), se.cpu()
+        out = []
+        for r, p, d in zip(res, perms, descs):
+            o, n = d.out_offset, d.n_units
+            out.append(dict(answer=r["answer"], prob=r["prob"], empty_prob=float(r["prob_d"][0]), units=r["units"],
+                            phi=phi[o:o + n], stderr=se[o:o + n], perm=p, samples=r["samples"]))
+        return out
 
     # ------------------------------------------------------------------ answer decode (worker.py:295-386)
     def decode_answers(self, out, messages, spatials=None):

@@ -601,6 +601,41 @@ def custom_head_ablation_packed(requests, max_boxes: int = 100, *, entries=None)
     return answers
 
 
+def custom_shapley_packed(requests, max_boxes: int = 100, *, units=None, permutations: int = 8, seed: int = 0, antithetic: bool = True):
+    """Shapley values of each answer's question tokens and detector boxes: `custom_prediction_packed` (decode="device") for
+    `custom_prediction` argument tuples `(query, task, features, infos, task_id)`, plus `model.shapley` over the images the answer
+    reads, as `custom_ablation_packed` chooses them.  `units`: None for the defaults (one unit per position 1 .. Tin - 2 and per box),
+    or `(positions, boxes)` groups applied to every request.  Returns per request `{"answer": <custom_prediction_packed's answer>,
+    "shapley": <shapley's dict>}` -- with `box_pixels`, per unit the [x1, y1, x2, y2] of its boxes from `infos` -- or the exception of
+    a request that fails validation.  Grounding requests get a ValueError: their answer is a box, which a coalition would renumber."""
+    p = pack_region_requests(requests, max_boxes=max_boxes)
+    answers = p["answers"]
+    if not p["spans"]:
+        return answers
+    args = (p["question"], p["segment_ids"], p["task_tokens"], p["box_features"], p["boxes"], p["image_wh"], p["n_tokens"], p["n_boxes"])
+    msgs = {i: m[:4] for i, m in ablation_messages(requests, p["spans"]).items() if requests[i][4] not in GROUNDING_TASKS}
+    mask = (tokenizer.vocab.get("[MASK]", 103) if tokenizer is not None and hasattr(tokenizer, "vocab") else 103)
+    with model_lock:
+        out, spatials = model.forward_regions_packed(*args, select=p["select"], max_tokens=p["max_tokens"], max_boxes=p["max_boxes"])
+        sh = model.shapley(*args, list(msgs.values()), units=None if units is None else [units] * len(msgs), permutations=permutations,
+                           seed=seed, antithetic=antithetic, mask_token=mask, max_tokens=p["max_tokens"],
+                           max_boxes=p["max_boxes"]) if msgs else []
+    answers = _answer_regions(answers, requests, out, spatials, p["spans"], p["n_tokens"], p["n_boxes"], "device")
+    for i in p["spans"]:
+        if i not in msgs:
+            answers[i] = ValueError("custom_shapley_packed: a grounding answer is a box, which a coalition would renumber")
+    for i, s in zip(msgs, sh):
+        infos, lo = requests[i][3], p["spans"][i][0]
+        first = list(accumulate([p["n_boxes"][lo + k] for k in range(len(infos))], initial=0))     # each image's first box
+
+        def pixels(b):
+            k = max(k for k in range(len(infos)) if first[k] <= b)
+            return _pixel_box(infos[k], b - first[k] + 1)
+        s["box_pixels"] = [[pixels(b) for b in bs] for _, bs in s["units"]]
+        answers[i] = {"answer": answers[i], "shapley": s}
+    return answers
+
+
 def _per_image(x, counts):
     """A per-image sequence as given, or one tensor over all images' rows split by `counts` (the reference's `.split`)."""
     if torch.is_tensor(x) or isinstance(x, np.ndarray):
