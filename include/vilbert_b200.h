@@ -570,7 +570,8 @@ int vb200_decode_answers_host(vb200_handle h, const vb200_decode_msg* msgs /* HO
  * VB200_ERR_INVALID, with nothing enqueued, no output written and a message naming the sample, for: split_fp32 and pre-training
  * engines; an excluded or unknown family; a range outside [0, Tin_i] / [0, n_boxes_i] or reversed; box ablation on an image with
  * fewer than 2 boxes; mask_token outside [0, vocab); answer outside [-1, width); more than VB200_ABLATION_MAX_VARIANTS variants;
- * NULL required pointers; box_features not 16-byte aligned; and every length rule of vb200_forward_regions_packed.
+ * NULL required pointers; box_features not 16-byte aligned; variant_logits or scores not 4-byte aligned; and every length rule of
+ * vb200_forward_regions_packed.
  * Asynchronous on cuda_stream: the variant descriptors reach the device through engine-owned pinned staging and the variants' ids
  * live in an engine-owned workspace, both stream-ordered, so back-to-back calls need no synchronisation. */
 #define VB200_ABLATION_MAX_VARIANTS 1024

@@ -284,6 +284,7 @@ def test_rejections(tiny, tiny_oracle):
         (dict(msgs=[(width, 0, 0, 0, 0), (-1, 0, 0, 0, 0)]), "sample 0 has answer"),
         (dict(msgs=[(-2, 0, 0, 0, 0), (-1, 0, 0, 0, 0)]), "sample 0 has answer"),
         (dict(lg=None), "NULL"),
+        (dict(lg=logits.view(-1).view(torch.uint8)[2:]), "variant_logits is not 4-byte aligned"),
         (dict(bf=a[3].data_ptr() + 4), "16-byte aligned"),
         (dict(nt=[6, 0]), "n_tokens 0"),
         (dict(nb=[3, 0]), "n_boxes 0"),

@@ -2117,8 +2117,9 @@ struct vb200_engine {
                                                   reinterpret_cast<const vb::RelevanceSample*>(dst + eb), batch, max_cols, relevance, st));
         rel_ws.release(st);
     }
-    // ---- answer and message ablation.  Both entry points check their inputs, describe every variant as a message ablation layout
-    // (AblLayout) and run it through run_ablation: one packed forward of every variant's samples, one segment gather, one scoring.
+    // ---- answer, message, head and coalition ablation.  Every entry point converts its messages to AblMsgs, ablation_layout
+    // describes every variant (AblLayout) and run_ablation runs them: one packed forward of every variant's samples, one segment
+    // gather, one scoring.
     // The rejections every ablation call shares: the batch's pointers, mask_token, slot and the length rules of
     // vb200_forward_regions_packed on the samples (every variant is no longer than its samples).  Returns the region capacity.
     int check_ablation_inputs(const char* api, const vb200_packed_region_inputs* in, int64_t mask_token, int slot) const {
@@ -2155,6 +2156,33 @@ struct vb200_engine {
         bool grounding = false;
         bool gated = false;            // head ablation: the samples run the gated plan
     };
+    // One message of any ablation kind: its family, images and answer; the positions [token_begin, token_end) and boxes [box_begin,
+    // box_end) it masks and drops one at a time (answer and message ablation); the attention entries [entry_begin, entry_end) whose
+    // heads it gates one at a time (head ablation); and its units and coalitions (coalition ablation, else null).
+    struct AblMsg {
+        int family, image_begin, n_images, answer;
+        int token_begin, token_end, box_begin, box_end;
+        int entry_begin, entry_end;
+        const vb200_coalition_message* coal;
+    };
+    static AblMsg abl_msg(int family, int sample, const vb200_ablation_msg& a) {
+        return {family, sample, 1, a.answer, a.token_begin, a.token_end, a.box_begin, a.box_end, 0, 0, nullptr};
+    }
+    static AblMsg abl_msg(const vb200_ablation_message& m) {
+        return {m.family, m.image_begin, m.n_images, m.answer, m.token_begin, m.token_end, m.box_begin, m.box_end, 0, 0, nullptr};
+    }
+    static AblMsg abl_msg(const vb200_head_ablation_message& m) {
+        return {m.family, m.image_begin, m.n_images, m.answer, 0, 0, 0, 0, m.entry_begin, m.entry_end, nullptr};
+    }
+    static AblMsg abl_msg(const vb200_coalition_message& m) { return {m.family, m.image_begin, m.n_images, m.answer, 0, 0, 0, 0, 0, 0, &m}; }
+    template <typename M>
+    static std::vector<AblMsg> abl_msgs(const char* api, const M* msgs, int n_msgs) {
+        if (msgs == nullptr) fail(VB200_ERR_INVALID, "%s: msgs is NULL", api);
+        if (n_msgs < 1) fail(VB200_ERR_INVALID, "%s: n_msgs must be positive (n_msgs = %d)", api, n_msgs);
+        std::vector<AblMsg> m;
+        for (int i = 0; i < n_msgs; ++i) m.push_back(abl_msg(msgs[i]));
+        return m;
+    }
     // Coalition message i's units and coalitions checked against its question length T and box count nb; pos_unit / box_unit get
     // each position's and box's unit (-1: in none).
     static void check_coalitions(const char* api, int i, const vb200_coalition_message& c, int T, int nb, std::vector<int>& pos_unit,
@@ -2199,17 +2227,16 @@ struct vb200_engine {
             if (c.coalitions[s * W + W - 1] & past)
                 fail(VB200_ERR_INVALID, "%s: message %d coalition %d sets a bit at or past n_units %d", api, i, s, c.n_units);
     }
-    // The messages checked against the batch's lengths and laid out; no sample cap (run_ablation applies it).  entries (head
-    // ablation, one [begin, end) per message): after its token and box variants, each message gets one variant per head of every
-    // entry in the range (kind 3, unit entry * gate_heads + head): the message's samples, unablated, with that one gate at 0.
-    // coal (coalition ablation, one per message, whose token and box ranges are empty): after the full input, one variant per
-    // coalition (kind 4, unit = its index): every sample of the message with the coalition's absent units removed.
-    AblLayout ablation_layout(const char* api, int batch, const int32_t* n_tokens, const int32_t* n_boxes, const vb200_ablation_message* msgs,
-                              int n_msgs, const std::vector<std::array<int, 2>>* entries = nullptr,
-                              const vb200_coalition_message* coal = nullptr) const {
-        if (n_tokens == nullptr || n_boxes == nullptr || msgs == nullptr) fail(VB200_ERR_INVALID, "%s: n_tokens / n_boxes / msgs is NULL", api);
+    // The messages checked against the batch's lengths and laid out; no sample cap (run_ablation applies it).  After its token and
+    // box variants, each message gets one variant per head of every entry in its entry range (kind 3, unit entry * gate_heads +
+    // head): the message's samples, unablated, with that one gate at 0.  A coalition message (token and box ranges empty) gets after
+    // the full input one variant per coalition (kind 4, unit = its index): every sample of the message with the coalition's absent
+    // units removed.  gated: the samples run the gated plan (head ablation).
+    AblLayout ablation_layout(const char* api, int batch, const int32_t* n_tokens, const int32_t* n_boxes, const std::vector<AblMsg>& msgs,
+                              bool gated) const {
+        if (n_tokens == nullptr || n_boxes == nullptr) fail(VB200_ERR_INVALID, "%s: n_tokens / n_boxes is NULL", api);
         if (batch < 1) fail(VB200_ERR_INVALID, "%s: batch must be positive (batch = %d)", api, batch);
-        if (n_msgs < 1) fail(VB200_ERR_INVALID, "%s: n_msgs must be positive (n_msgs = %d)", api, n_msgs);
+        const int n_msgs = static_cast<int>(msgs.size());
         std::vector<int> tok0(batch + 1, 0), box0(batch + 1, 0);
         for (int i = 0; i < batch; ++i) {
             if (n_tokens[i] < 1 || n_boxes[i] < 1)
@@ -2220,16 +2247,14 @@ struct vb200_engine {
             box0[i + 1] = box0[i] + n_boxes[i];
         }
         AblLayout L;
+        L.gated = gated;
         std::vector<std::vector<AblVariant>> per(n_msgs);
         std::vector<int> entry_heads;
-        if (entries != nullptr) {
-            L.gated = true;
-            for (int kind : attention_kinds(schedule)) entry_heads.push_back(kind == 0 ? cfg.heads : kind == 1 ? cfg.v_heads : cfg.bi_heads);
-        }
-        std::vector<std::vector<int>> pos_unit(coal ? n_msgs : 0), box_unit(coal ? n_msgs : 0);   // owning unit, -1: none
+        for (int kind : attention_kinds(schedule)) entry_heads.push_back(kind == 0 ? cfg.heads : kind == 1 ? cfg.v_heads : cfg.bi_heads);
+        std::vector<std::vector<int>> pos_unit(n_msgs), box_unit(n_msgs);   // a coalition message's owning units, -1: none
         // one sample: message m's question with the positions of bitmap run `masked` replaced (-1: none), image `image` with the
         // nbox boxes of kept-list run `kept` (-1: all its boxes)
-        auto sample = [&](const vb200_ablation_message& m, int masked, int image, int kept = -1, int nbox = -1, int gate = -1) {
+        auto sample = [&](const AblMsg& m, int masked, int image, int kept = -1, int nbox = -1, int gate = -1) {
             L.gate.push_back(gate);
             L.text.push_back({tok0[m.image_begin], n_tokens[m.image_begin], masked, m.image_begin});
             L.img.push_back({image, box0[image], kept});
@@ -2244,13 +2269,13 @@ struct vb200_engine {
             for (int p : pos) L.mask[at + p / 32] |= 1u << (p % 32);
             return at;
         };
-        auto reduced = [&](const vb200_ablation_message& m, int masked, int image, const std::vector<int32_t>& rows) {   // `rows` kept
+        auto reduced = [&](const AblMsg& m, int masked, int image, const std::vector<int32_t>& rows) {   // `rows` kept
             if (static_cast<int>(rows.size()) == n_boxes[image]) return sample(m, masked, image);
             const int at = static_cast<int>(L.kept.size());
             L.kept.insert(L.kept.end(), rows.begin(), rows.end());
             return sample(m, masked, image, at, static_cast<int>(rows.size()));
         };
-        auto without = [&](const vb200_ablation_message& m, int image, int skip) {   // image without box `skip`
+        auto without = [&](const AblMsg& m, int image, int skip) {   // image without box `skip`
             std::vector<int32_t> rows;
             for (int r = 0; r < n_boxes[image]; ++r)
                 if (r != skip) rows.push_back(r);
@@ -2258,7 +2283,7 @@ struct vb200_engine {
         };
         for (int pass = 0; pass < 2; ++pass)
             for (int i = 0; i < n_msgs; ++i) {
-                const vb200_ablation_message& m = msgs[i];
+                const AblMsg& m = msgs[i];
                 const int f = m.family, K = m.n_images, ib = m.image_begin;
                 int head = 0, width = 0, images = 1;
                 switch (f) {
@@ -2292,13 +2317,10 @@ struct vb200_engine {
                         if (n_boxes[ib + k] < 2 && m.box_begin < box0[ib + k + 1] - box0[ib] && m.box_end > box0[ib + k] - box0[ib])
                             fail(VB200_ERR_INVALID, "%s: message %d drops a box of its image %d, which has %d box (box ablation needs >= 2)",
                                  api, i, k, n_boxes[ib + k]);
-                    if (entries != nullptr) {
-                        const auto& r = (*entries)[i];
-                        if (r[0] < 0 || r[0] > r[1] || r[1] > static_cast<int>(entry_heads.size()))
-                            fail(VB200_ERR_INVALID, "%s: message %d has the entry range [%d, %d), reversed or outside [0, %d]", api, i, r[0],
-                                 r[1], static_cast<int>(entry_heads.size()));
-                    }
-                    if (coal != nullptr) check_coalitions(api, i, coal[i], T, nb, pos_unit[i], box_unit[i]);
+                    if (m.entry_begin < 0 || m.entry_begin > m.entry_end || m.entry_end > static_cast<int>(entry_heads.size()))
+                        fail(VB200_ERR_INVALID, "%s: message %d has the entry range [%d, %d), reversed or outside [0, %d]", api, i,
+                             m.entry_begin, m.entry_end, static_cast<int>(entry_heads.size()));
+                    if (m.coal != nullptr) check_coalitions(api, i, *m.coal, T, nb, pos_unit[i], box_unit[i]);
                 }
                 if ((f == VB200_DECODE_NLVR2) != (pass == 0)) continue;
                 std::vector<AblVariant>& out = per[i];
@@ -2340,14 +2362,13 @@ struct vb200_engine {
                         variant(2, u, 1, seg(first), f == VB200_DECODE_GROUNDING ? j + 1 : -1);
                     }
                 }
-                if (entries != nullptr)
-                    for (int e = (*entries)[i][0]; e < (*entries)[i][1]; ++e)
-                        for (int h = 0; h < entry_heads[e]; ++h) {
-                            const int unit = e * gate_heads() + h;
-                            variant(3, unit, K, seg(all_images(-1, unit)), -1);
-                        }
-                if (coal != nullptr) {
-                    const vb200_coalition_message& c = coal[i];
+                for (int e = m.entry_begin; e < m.entry_end; ++e)
+                    for (int h = 0; h < entry_heads[e]; ++h) {
+                        const int unit = e * gate_heads() + h;
+                        variant(3, unit, K, seg(all_images(-1, unit)), -1);
+                    }
+                if (m.coal != nullptr) {
+                    const vb200_coalition_message& c = *m.coal;
                     const size_t W = (static_cast<size_t>(c.n_units) + 63) / 64;
                     for (int s = 0; s < c.n_coalitions; ++s) {
                         const uint64_t* bits = c.coalitions + s * W;
@@ -2466,142 +2487,103 @@ struct vb200_engine {
             dec_ws.release(st);
         }
     }
-    // vb200_answer_ablation: one single-image message of `family` per sample, checked in the samples' terms first
-    void answer_ablation(const vb200_packed_region_inputs* in, const vb200_ablation_msg* msgs, int family, int64_t mask_token,
-                         float* variant_logits, vb200_ablation_score* scores, int slot, cudaStream_t st) {
-        const char* api = "vb200_answer_ablation";
-        if (in == nullptr || msgs == nullptr || variant_logits == nullptr) fail(VB200_ERR_INVALID, "%s: in / msgs / variant_logits is NULL", api);
-        if (x3) fail(VB200_ERR_INVALID, "%s: packed batches are not supported in split_fp32 (fp32x) mode", api);
-        if (pretraining) fail(VB200_ERR_INVALID, "%s: a pre-training engine has no task head to attribute an answer of", api);
-        int width = 0;
-        switch (family) {
-            case VB200_DECODE_VQA: width = num_labels; break;
-            case VB200_DECODE_GQA: width = gqa_labels; break;
-            case VB200_DECODE_SNLI_VE: width = 3; break;
-            case VB200_DECODE_NLVR2: fail(VB200_ERR_INVALID, "%s: family NLVR2 is not supported (an answer reads two images)", api);
-            case VB200_DECODE_RETRIEVAL: fail(VB200_ERR_INVALID, "%s: family retrieval is not supported (an answer ranks many images)", api);
-            case VB200_DECODE_GROUNDING:
-                fail(VB200_ERR_INVALID, "%s: family grounding is not supported (the answer is a box a variant may remove)", api);
-            default: fail(VB200_ERR_INVALID, "%s: unknown family %d", api, family);
-        }
-        if (width < 1) fail(VB200_ERR_INVALID, "%s: family %d's head has no columns on this engine", api, family);
-        const int max_regions = check_ablation_inputs(api, in, mask_token, slot);
-        std::vector<vb200_ablation_message> m(in->batch);
-        int64_t count = 0;
-        for (int i = 0; i < in->batch; ++i) {
-            const vb200_ablation_msg& a = msgs[i];
-            const int T = in->n_tokens[i], nb = in->n_boxes[i];
-            if (a.answer < -1 || a.answer >= width)
-                fail(VB200_ERR_INVALID, "%s: sample %d has answer %d outside [-1, %d)", api, i, a.answer, width);
-            if (a.token_begin < 0 || a.token_begin > a.token_end || a.token_end > T)
-                fail(VB200_ERR_INVALID, "%s: sample %d has the token range [%d, %d), reversed or outside [0, %d]", api, i, a.token_begin,
-                     a.token_end, T);
-            if (a.box_begin < 0 || a.box_begin > a.box_end || a.box_end > nb)
-                fail(VB200_ERR_INVALID, "%s: sample %d has the box range [%d, %d), reversed or outside [0, %d]", api, i, a.box_begin, a.box_end,
-                     nb);
-            if (a.box_end > a.box_begin && nb < 2)
-                fail(VB200_ERR_INVALID, "%s: sample %d drops a box of an image with %d box (box ablation needs >= 2)", api, i, nb);
-            count += 1 + (a.token_end - a.token_begin) + (a.box_end - a.box_begin);
-            if (count > VB200_ABLATION_MAX_VARIANTS)
-                fail(VB200_ERR_INVALID, "%s: the variants of samples 0..%d number %lld, above %d (split the ranges across calls)", api, i,
-                     static_cast<long long>(count), VB200_ABLATION_MAX_VARIANTS);
-            m[i] = {family, i, 1, a.answer, a.token_begin, a.token_end, a.box_begin, a.box_end};
-        }
-        run_ablation(api, in, ablation_layout(api, in->batch, in->n_tokens, in->n_boxes, m.data(), in->batch), max_regions, mask_token,
-                     variant_logits, scores, slot, st);
-    }
-    void message_ablation(const vb200_packed_region_inputs* in, const vb200_ablation_message* msgs, int n_msgs, int64_t mask_token,
-                          float* variant_logits, vb200_ablation_score* scores, int slot, cudaStream_t st) {
-        const char* api = "vb200_message_ablation";
+    // The four run entry points: the rejections they share, then the call's messages (messages(), which checks them in the entry
+    // point's own terms where it has any), laid out and run.
+    template <typename Messages>
+    void ablate(const char* api, const vb200_packed_region_inputs* in, const void* msgs, bool gated, int64_t mask_token, float* variant_logits,
+                vb200_ablation_score* scores, int slot, cudaStream_t st, Messages messages) {
         if (in == nullptr || msgs == nullptr || variant_logits == nullptr) fail(VB200_ERR_INVALID, "%s: in / msgs / variant_logits is NULL", api);
         if (x3) fail(VB200_ERR_INVALID, "%s: packed batches are not supported in split_fp32 (fp32x) mode", api);
         if (pretraining) fail(VB200_ERR_INVALID, "%s: a pre-training engine has no task head to attribute an answer of", api);
         if (reinterpret_cast<uintptr_t>(variant_logits) & 3) fail(VB200_ERR_INVALID, "%s: variant_logits is not 4-byte aligned", api);
         if (reinterpret_cast<uintptr_t>(scores) & 3) fail(VB200_ERR_INVALID, "%s: scores is not 4-byte aligned", api);
         const int max_regions = check_ablation_inputs(api, in, mask_token, slot);
-        run_ablation(api, in, ablation_layout(api, in->batch, in->n_tokens, in->n_boxes, msgs, n_msgs), max_regions, mask_token,
+        run_ablation(api, in, ablation_layout(api, in->batch, in->n_tokens, in->n_boxes, messages(), gated), max_regions, mask_token,
                      variant_logits, scores, slot, st);
     }
-    // vb200_head_ablation[_layout]: each head message as a message with no token or box range, plus its entry range
-    static std::vector<vb200_ablation_message> head_messages(const vb200_head_ablation_message* msgs, int n,
-                                                             std::vector<std::array<int, 2>>& entries) {
-        std::vector<vb200_ablation_message> m;
-        for (int i = 0; i < n; ++i) {
-            m.push_back({msgs[i].family, msgs[i].image_begin, msgs[i].n_images, msgs[i].answer, 0, 0, 0, 0});
-            entries.push_back({msgs[i].entry_begin, msgs[i].entry_end});
-        }
-        return m;
-    }
-    void head_ablation(const vb200_packed_region_inputs* in, const vb200_head_ablation_message* msgs, int n_msgs, float* variant_logits,
-                       vb200_ablation_score* scores, int slot, cudaStream_t st) {
-        const char* api = "vb200_head_ablation";
-        if (in == nullptr || msgs == nullptr || variant_logits == nullptr) fail(VB200_ERR_INVALID, "%s: in / msgs / variant_logits is NULL", api);
-        if (x3) fail(VB200_ERR_INVALID, "%s: packed batches are not supported in split_fp32 (fp32x) mode", api);
-        if (pretraining) fail(VB200_ERR_INVALID, "%s: a pre-training engine has no task head to attribute an answer of", api);
-        if (reinterpret_cast<uintptr_t>(variant_logits) & 3) fail(VB200_ERR_INVALID, "%s: variant_logits is not 4-byte aligned", api);
-        if (reinterpret_cast<uintptr_t>(scores) & 3) fail(VB200_ERR_INVALID, "%s: scores is not 4-byte aligned", api);
-        if (n_msgs < 1) fail(VB200_ERR_INVALID, "%s: n_msgs must be positive (n_msgs = %d)", api, n_msgs);
-        const int max_regions = check_ablation_inputs(api, in, 0, slot);     // no position is masked: any valid token id
-        std::vector<std::array<int, 2>> entries;
-        const std::vector<vb200_ablation_message> m = head_messages(msgs, n_msgs, entries);
-        run_ablation(api, in, ablation_layout(api, in->batch, in->n_tokens, in->n_boxes, m.data(), n_msgs, &entries), max_regions, 0,
-                     variant_logits, scores, slot, st);
-    }
-    void head_ablation_layout(int batch, const int32_t* n_tokens, const int32_t* n_boxes, const vb200_head_ablation_message* msgs, int n_msgs,
-                              vb200_ablation_variant* variants, int64_t* n_variants, int64_t* n_floats, int64_t* n_samples) const {
-        const char* api = "vb200_head_ablation_layout";
+    // The three layout entry points: the layout's records (variants NULL: none) and totals.
+    template <typename M>
+    void layout(const char* api, int batch, const int32_t* n_tokens, const int32_t* n_boxes, const M* msgs, int n_msgs, bool gated,
+                vb200_ablation_variant* variants, int64_t* n_variants, int64_t* n_floats, int64_t* n_samples) const {
         if (n_variants == nullptr || n_floats == nullptr || n_samples == nullptr)
             fail(VB200_ERR_INVALID, "%s: n_variants / n_floats / n_samples is NULL", api);
         if (pretraining) fail(VB200_ERR_INVALID, "%s: a pre-training engine has no task head to attribute an answer of", api);
-        if (msgs == nullptr) fail(VB200_ERR_INVALID, "%s: msgs is NULL", api);
-        if (n_msgs < 1) fail(VB200_ERR_INVALID, "%s: n_msgs must be positive (n_msgs = %d)", api, n_msgs);
-        std::vector<std::array<int, 2>> entries;
-        const std::vector<vb200_ablation_message> m = head_messages(msgs, n_msgs, entries);
-        put_layout(ablation_layout(api, batch, n_tokens, n_boxes, m.data(), n_msgs, &entries), variants, n_variants, n_floats, n_samples);
-    }
-    static void put_layout(const AblLayout& L, vb200_ablation_variant* variants, int64_t* n_variants, int64_t* n_floats, int64_t* n_samples) {
+        const AblLayout L = ablation_layout(api, batch, n_tokens, n_boxes, abl_msgs(api, msgs, n_msgs), gated);
         if (variants != nullptr)
             for (size_t k = 0; k < L.v.size(); ++k) variants[k] = L.v[k].rec;
         *n_variants = static_cast<int64_t>(L.v.size());
         *n_floats = L.n_floats;
         *n_samples = static_cast<int64_t>(L.text.size());
     }
+    // vb200_answer_ablation: one single-image message of `family` per sample, checked in the samples' terms first
+    void answer_ablation(const vb200_packed_region_inputs* in, const vb200_ablation_msg* msgs, int family, int64_t mask_token,
+                         float* variant_logits, vb200_ablation_score* scores, int slot, cudaStream_t st) {
+        const char* api = "vb200_answer_ablation";
+        ablate(api, in, msgs, false, mask_token, variant_logits, scores, slot, st, [&] {
+            int width = 0;
+            switch (family) {
+                case VB200_DECODE_VQA: width = num_labels; break;
+                case VB200_DECODE_GQA: width = gqa_labels; break;
+                case VB200_DECODE_SNLI_VE: width = 3; break;
+                case VB200_DECODE_NLVR2: fail(VB200_ERR_INVALID, "%s: family NLVR2 is not supported (an answer reads two images)", api);
+                case VB200_DECODE_RETRIEVAL:
+                    fail(VB200_ERR_INVALID, "%s: family retrieval is not supported (an answer ranks many images)", api);
+                case VB200_DECODE_GROUNDING:
+                    fail(VB200_ERR_INVALID, "%s: family grounding is not supported (the answer is a box a variant may remove)", api);
+                default: fail(VB200_ERR_INVALID, "%s: unknown family %d", api, family);
+            }
+            if (width < 1) fail(VB200_ERR_INVALID, "%s: family %d's head has no columns on this engine", api, family);
+            std::vector<AblMsg> m;
+            int64_t count = 0;
+            for (int i = 0; i < in->batch; ++i) {
+                const vb200_ablation_msg& a = msgs[i];
+                const int T = in->n_tokens[i], nb = in->n_boxes[i];
+                if (a.answer < -1 || a.answer >= width)
+                    fail(VB200_ERR_INVALID, "%s: sample %d has answer %d outside [-1, %d)", api, i, a.answer, width);
+                if (a.token_begin < 0 || a.token_begin > a.token_end || a.token_end > T)
+                    fail(VB200_ERR_INVALID, "%s: sample %d has the token range [%d, %d), reversed or outside [0, %d]", api, i,
+                         a.token_begin, a.token_end, T);
+                if (a.box_begin < 0 || a.box_begin > a.box_end || a.box_end > nb)
+                    fail(VB200_ERR_INVALID, "%s: sample %d has the box range [%d, %d), reversed or outside [0, %d]", api, i, a.box_begin,
+                         a.box_end, nb);
+                if (a.box_end > a.box_begin && nb < 2)
+                    fail(VB200_ERR_INVALID, "%s: sample %d drops a box of an image with %d box (box ablation needs >= 2)", api, i, nb);
+                count += 1 + (a.token_end - a.token_begin) + (a.box_end - a.box_begin);
+                if (count > VB200_ABLATION_MAX_VARIANTS)
+                    fail(VB200_ERR_INVALID, "%s: the variants of samples 0..%d number %lld, above %d (split the ranges across calls)", api,
+                         i, static_cast<long long>(count), VB200_ABLATION_MAX_VARIANTS);
+                m.push_back(abl_msg(family, i, a));
+            }
+            return m;
+        });
+    }
+    void message_ablation(const vb200_packed_region_inputs* in, const vb200_ablation_message* msgs, int n_msgs, int64_t mask_token,
+                          float* variant_logits, vb200_ablation_score* scores, int slot, cudaStream_t st) {
+        const char* api = "vb200_message_ablation";
+        ablate(api, in, msgs, false, mask_token, variant_logits, scores, slot, st, [&] { return abl_msgs(api, msgs, n_msgs); });
+    }
     void message_ablation_layout(int batch, const int32_t* n_tokens, const int32_t* n_boxes, const vb200_ablation_message* msgs, int n_msgs,
                                  vb200_ablation_variant* variants, int64_t* n_variants, int64_t* n_floats, int64_t* n_samples) const {
-        const char* api = "vb200_message_ablation_layout";
-        if (n_variants == nullptr || n_floats == nullptr || n_samples == nullptr)
-            fail(VB200_ERR_INVALID, "%s: n_variants / n_floats / n_samples is NULL", api);
-        if (pretraining) fail(VB200_ERR_INVALID, "%s: a pre-training engine has no task head to attribute an answer of", api);
-        put_layout(ablation_layout(api, batch, n_tokens, n_boxes, msgs, n_msgs), variants, n_variants, n_floats, n_samples);
+        layout("vb200_message_ablation_layout", batch, n_tokens, n_boxes, msgs, n_msgs, false, variants, n_variants, n_floats, n_samples);
     }
-    // vb200_coalition_ablation[_layout]: each coalition message as a message with no token or box range, plus its units and coalitions
-    AblLayout coalition_layout(const char* api, int batch, const int32_t* n_tokens, const int32_t* n_boxes, const vb200_coalition_message* msgs,
-                               int n_msgs) const {
-        if (msgs == nullptr) fail(VB200_ERR_INVALID, "%s: msgs is NULL", api);
-        if (n_msgs < 1) fail(VB200_ERR_INVALID, "%s: n_msgs must be positive (n_msgs = %d)", api, n_msgs);
-        std::vector<vb200_ablation_message> m;
-        for (int i = 0; i < n_msgs; ++i) m.push_back({msgs[i].family, msgs[i].image_begin, msgs[i].n_images, msgs[i].answer, 0, 0, 0, 0});
-        return ablation_layout(api, batch, n_tokens, n_boxes, m.data(), n_msgs, nullptr, msgs);
+    // head ablation masks no position: mask_token 0 is any valid token id
+    void head_ablation(const vb200_packed_region_inputs* in, const vb200_head_ablation_message* msgs, int n_msgs, float* variant_logits,
+                       vb200_ablation_score* scores, int slot, cudaStream_t st) {
+        const char* api = "vb200_head_ablation";
+        ablate(api, in, msgs, true, 0, variant_logits, scores, slot, st, [&] { return abl_msgs(api, msgs, n_msgs); });
     }
-    void coalition_ablation_layout(int batch, const int32_t* n_tokens, const int32_t* n_boxes, const vb200_coalition_message* msgs, int n_msgs,
-                                   vb200_ablation_variant* variants, int64_t* n_variants, int64_t* n_floats, int64_t* n_samples) const {
-        const char* api = "vb200_coalition_ablation_layout";
-        if (n_variants == nullptr || n_floats == nullptr || n_samples == nullptr)
-            fail(VB200_ERR_INVALID, "%s: n_variants / n_floats / n_samples is NULL", api);
-        if (pretraining) fail(VB200_ERR_INVALID, "%s: a pre-training engine has no task head to attribute an answer of", api);
-        put_layout(coalition_layout(api, batch, n_tokens, n_boxes, msgs, n_msgs), variants, n_variants, n_floats, n_samples);
+    void head_ablation_layout(int batch, const int32_t* n_tokens, const int32_t* n_boxes, const vb200_head_ablation_message* msgs, int n_msgs,
+                              vb200_ablation_variant* variants, int64_t* n_variants, int64_t* n_floats, int64_t* n_samples) const {
+        layout("vb200_head_ablation_layout", batch, n_tokens, n_boxes, msgs, n_msgs, true, variants, n_variants, n_floats, n_samples);
     }
     void coalition_ablation(const vb200_packed_region_inputs* in, const vb200_coalition_message* msgs, int n_msgs, int64_t mask_token,
                             float* variant_logits, vb200_ablation_score* scores, int slot, cudaStream_t st) {
         const char* api = "vb200_coalition_ablation";
-        if (in == nullptr || msgs == nullptr || variant_logits == nullptr) fail(VB200_ERR_INVALID, "%s: in / msgs / variant_logits is NULL", api);
-        if (x3) fail(VB200_ERR_INVALID, "%s: packed batches are not supported in split_fp32 (fp32x) mode", api);
-        if (pretraining) fail(VB200_ERR_INVALID, "%s: a pre-training engine has no task head to attribute an answer of", api);
-        if (reinterpret_cast<uintptr_t>(variant_logits) & 3) fail(VB200_ERR_INVALID, "%s: variant_logits is not 4-byte aligned", api);
-        if (reinterpret_cast<uintptr_t>(scores) & 3) fail(VB200_ERR_INVALID, "%s: scores is not 4-byte aligned", api);
-        const int max_regions = check_ablation_inputs(api, in, mask_token, slot);
-        run_ablation(api, in, coalition_layout(api, in->batch, in->n_tokens, in->n_boxes, msgs, n_msgs), max_regions, mask_token,
-                     variant_logits, scores, slot, st);
+        ablate(api, in, msgs, false, mask_token, variant_logits, scores, slot, st, [&] { return abl_msgs(api, msgs, n_msgs); });
+    }
+    void coalition_ablation_layout(int batch, const int32_t* n_tokens, const int32_t* n_boxes, const vb200_coalition_message* msgs, int n_msgs,
+                                   vb200_ablation_variant* variants, int64_t* n_variants, int64_t* n_floats, int64_t* n_samples) const {
+        layout("vb200_coalition_ablation_layout", batch, n_tokens, n_boxes, msgs, n_msgs, false, variants, n_variants, n_floats, n_samples);
     }
     // vb200_shapley_values: every descriptor is checked before anything is enqueued
     void shapley_values(const vb200_shapley_message* msgs, int n_msgs, const int32_t* perm, const float* values, float* phi, float* se,

@@ -98,6 +98,52 @@ def packed_offsets(lengths, extra: int = 0):
     return offs
 
 
+class PackedRegionBatch:
+    """A packed detector-output batch, ``forward_regions_packed``'s inputs, checked and staged on the engine's ``device`` once.
+    ``name`` (the calling method) starts every error message.  ``inputs`` is the batch's vb200_packed_region_inputs, valid while the
+    batch lives; ``subset`` the batch of some of its samples, their rows packed back to back."""
+
+    @staticmethod
+    def lengths(name, n_tokens, n_boxes):
+        """``n_tokens`` / ``n_boxes`` as host int lists of the same, positive length."""
+        nt, nb = _host_ints(n_tokens), _host_ints(n_boxes)
+        if len(nb) != len(nt) or not nt:
+            raise ValueError(f"{name}: n_tokens and n_boxes must have the same, positive length")
+        return nt, nb
+
+    def __init__(self, name, device, feature_size, question, segment_ids, task_tokens, box_features, boxes, image_wh, n_tokens, n_boxes):
+        nt, nb = self.lengths(name, n_tokens, n_boxes)
+        B = len(nt)
+        q = _to_device(question, torch.int64, device).reshape(-1)
+        seg = _to_device(segment_ids if segment_ids is not None else torch.zeros_like(q), torch.int64, device).reshape(-1)
+        tk = _task_rows(task_tokens if task_tokens is not None else torch.zeros(B, 1, dtype=torch.int64), B, device)
+        bf = _to_device(box_features, torch.float32, device).reshape(-1, feature_size)
+        bx = _to_device(boxes, torch.float32, device).reshape(-1, 4)
+        wh = _to_device(image_wh, torch.float32, device)
+        if q.numel() != sum(nt) or seg.numel() != sum(nt) or bf.shape[0] != sum(nb) or bx.shape[0] != sum(nb) or tuple(wh.shape) != (B, 2):
+            raise ValueError(f"{name}: question / segment_ids need sum(n_tokens) entries, box_features / boxes sum(n_boxes) rows, "
+                             "image_wh [B, 2]")
+        self.name, self.device, self.feature_size = name, device, feature_size
+        self.nt, self.nb, self.tensors = nt, nb, (q, seg, tk, bf, bx, wh)
+
+    def subset(self, samples):
+        t_off, b_off = packed_offsets(self.nt), packed_offsets(self.nb)
+        tcat = lambda t: torch.cat([t[t_off[i]:t_off[i + 1]] for i in samples])
+        bcat = lambda t: torch.cat([t[b_off[i]:b_off[i + 1]] for i in samples])
+        q, seg, tk, bf, bx, wh = self.tensors
+        return PackedRegionBatch(self.name, self.device, self.feature_size, tcat(q), tcat(seg), tk[samples], bcat(bf), bcat(bx),
+                                 wh[samples], [self.nt[i] for i in samples], [self.nb[i] for i in samples])
+
+    def inputs(self, max_tokens: int = 0, max_boxes: int = 0, spatials=None):
+        return L.PackedRegionInputs(len(self.nt), int(max_tokens), int(max_boxes), _int32s(self.nt), _int32s(self.nb),
+                                    *[t.data_ptr() for t in self.tensors], spatials)
+
+
+def _structs(cls, rows):
+    """A ctypes array of ``cls``, one per tuple of field values in ``rows``."""
+    return (cls * len(rows))(*[cls(*r) for r in rows])
+
+
 # the families whose answer is one row of one image (vb200_answer_ablation)
 ABLATION_FAMILIES = {"vqa": L.DECODE_VQA, "gqa": L.DECODE_GQA, "snli_ve": L.DECODE_SNLI_VE}
 
@@ -136,25 +182,8 @@ def ablation_calls(ranges, cap: int = L.ABLATION_MAX_VARIANTS):
     """The engine calls for these per-sample ranges: each call a list of (sample, (token_begin, token_end, box_begin, box_end))
     pieces whose variants (1 + tokens + boxes each) number at most ``cap``.  A batch is split at sample boundaries; a sample with more
     than ``cap`` variants is split into pieces of its units (tokens first, then boxes), each with its own unablated variant."""
-    pieces = []
-    for i, (tb, te, bb, be) in enumerate(ranges):
-        units = [("t", p) for p in range(tb, te)] + [("b", j) for j in range(bb, be)]
-        for c in range(0, max(len(units), 1), cap - 1):
-            chunk = units[c:c + cap - 1]
-            toks = [p for k, p in chunk if k == "t"]
-            bxs = [j for k, j in chunk if k == "b"]
-            r = (toks[0], toks[-1] + 1) if toks else (0, 0)
-            r += (bxs[0], bxs[-1] + 1) if bxs else (0, 0)
-            pieces.append((i, r))
-    calls, size = [], cap
-    for i, r in pieces:
-        k = 1 + (r[1] - r[0]) + (r[3] - r[2])
-        if size + k > cap:
-            calls.append([])
-            size = 0
-        calls[-1].append((i, r))
-        size += k
-    return calls
+    return message_calls([r for i, (tb, te, bb, be) in enumerate(ranges)
+                          for r in [(i, 0, -1, 1)] + [(i, 1, p, 1) for p in range(tb, te)] + [(i, 2, j, 1) for j in range(bb, be)]], cap)
 
 
 def ablation_variants(call):
@@ -185,29 +214,36 @@ def message_family(family):
     return f
 
 
+def _message_head(name, i, family, image_begin, n_images, answer, batch: int, top1: str = "the unablated top-1"):
+    """``(family, image_begin, n_images, answer)`` of message i of an ablation call checked against a batch of ``batch`` images:
+    the family by name, task id or value; the images it reads (``n_images`` right for the family, all inside the batch); the
+    answer an index >= 0, or None / -1 (``top1``).  ``name`` starts every error message."""
+    f = message_family(family)
+    ib, k = int(image_begin), int(n_images)
+    want = _FAMILY_IMAGES.get(f)
+    if (k != want) if want else k < 1:
+        raise ValueError(f"{name}: message {i} has n_images {k} (the family reads {want or '>= 1'})")
+    if ib < 0 or ib + k > batch:
+        raise ValueError(f"{name}: message {i} has images [{ib}, {ib + k}) outside the batch of {batch}")
+    a = -1 if answer is None else int(answer)
+    if a < -1:
+        raise ValueError(f"{name}: message {i} has answer {a} (an index >= 0, or None / -1: {top1})")
+    return f, ib, k, a
+
+
 def message_pieces(messages, n_tokens, n_boxes):
     """The engine messages (``_lib.AblationMessage`` fields as tuples) for ``message_ablation``'s ``messages`` and the batch's
     lengths, and for each the index of the message it belongs to.  A message is ``(family, image_begin, n_images, answer=None,
     tokens=None, boxes=None)``; by default positions 1 .. Tin - 2 of image_begin's question are masked and every box of the
     message's images with at least two boxes is dropped (boxes numbered across the message's images).  The default boxes of a
     message with a one-box image between others run as separate pieces, each with its own unablated variant."""
-    B = len(n_tokens)
     out = []
     for i, m in enumerate(messages):
         m = tuple(m) + (None,) * (6 - len(m))
         if len(m) != 6:
             raise ValueError(f"message_ablation: message {i} has {len(m)} fields (family, image_begin, n_images, answer, tokens, boxes)")
-        fam, ib, k, answer, tokens, boxes = m
-        f = message_family(fam)
-        ib, k = int(ib), int(k)
-        want = _FAMILY_IMAGES.get(f)
-        if (k != want) if want else k < 1:
-            raise ValueError(f"message_ablation: message {i} has n_images {k} (the family reads {want or '>= 1'})")
-        if ib < 0 or ib + k > B:
-            raise ValueError(f"message_ablation: message {i} has images [{ib}, {ib + k}) outside the batch of {B}")
-        a = -1 if answer is None else int(answer)
-        if a < -1:
-            raise ValueError(f"message_ablation: message {i} has answer {a} (an index >= 0, or None / -1: the unablated top-1)")
+        f, ib, k, a = _message_head("message_ablation", i, *m[:4], len(n_tokens))
+        tokens, boxes = m[4:]
         tin, nb = int(n_tokens[ib]), [int(n) for n in n_boxes[ib:ib + k]]
         first = [sum(nb[:j]) for j in range(k + 1)]            # each image's first box in the message's numbering
         tb, te = (1, max(1, tin - 1)) if tokens is None else (int(tokens[0]), int(tokens[1]))
@@ -236,40 +272,56 @@ def message_pieces(messages, n_tokens, n_boxes):
     return out
 
 
-def message_calls(variants, cap: int = L.ABLATION_MAX_VARIANTS):
-    """The engine calls for a message ablation layout: ``variants`` are its records ``(message, kind, unit, samples)`` in layout order
-    (``vb200_message_ablation_layout``).  Each call is a list of pieces ``(message, (token_begin, token_end, box_begin, box_end))``
-    whose variants run at most ``cap`` forward samples.  Messages are kept whole where they fit; a message above ``cap`` is split
-    into pieces of its units (positions first, then boxes), each with its own unablated variant."""
-    groups = []
+def _span(units):
+    """``(first, last + 1)`` of consecutive units, ``(0, 0)`` for none."""
+    return (units[0], units[-1] + 1) if units else (0, 0)
+
+
+def _layout_calls(variants, cap, name, per):
+    """The engine calls of an ablation layout, split greedily: ``variants`` are its records ``(message, kind, unit, samples)`` in
+    layout order, each message's first (kind 0) its unablated variant.  Consecutive records of one ``(kind, unit)`` are one atom,
+    which stays in one call.  Each message is cut into pieces of consecutive atoms of at most ``cap`` forward samples, each piece
+    with the message's unablated variant, and the pieces are packed into calls in order.  Each call is a list of pieces
+    ``(message, atoms)``, an atom ``[kind, unit, samples]``; ``name`` and ``per`` word the error of a message that cannot fit."""
+    groups, last = [], None
     for m, kind, unit, samples in variants:
         if kind == 0:
-            groups.append((m, samples, []))
+            groups.append((m, samples, atoms := []))
+            last = None
+        elif last is not None and last[1] == unit and last[0] == kind:
+            last[2] += samples
         else:
-            groups[-1][2].append((kind, unit, samples))
+            atoms.append(last := [kind, unit, samples])
     pieces = []
-    for m, base, units in groups:
-        if base + max([s for _, _, s in units], default=0) > cap:
-            raise ValueError(f"message_ablation: message {m} runs {base} samples per unablated variant, too many for {cap} per call")
+    for m, base, atoms in groups:
+        if base + max([a[2] for a in atoms], default=0) > cap:
+            raise ValueError(f"{name}: message {m} runs {base} samples per {per}, too many for {cap} per call")
         chunk, size = [], base
-        for u in units:
-            if size + u[2] > cap:
+        for a in atoms:
+            n = a[2]
+            if size + n > cap:
                 pieces.append((m, chunk, size))
                 chunk, size = [], base
-            chunk.append(u)
-            size += u[2]
+            chunk.append(a)
+            size += n
         pieces.append((m, chunk, size))
     calls, size = [], cap + 1
     for m, chunk, n in pieces:
         if size + n > cap:
             calls.append([])
             size = 0
-        toks = [u for k, u, _ in chunk if k == 1]
-        bxs = [u for k, u, _ in chunk if k == 2]
-        r = ((toks[0], toks[-1] + 1) if toks else (0, 0)) + ((bxs[0], bxs[-1] + 1) if bxs else (0, 0))
-        calls[-1].append((m, r))
+        calls[-1].append((m, chunk))
         size += n
     return calls
+
+
+def message_calls(variants, cap: int = L.ABLATION_MAX_VARIANTS):
+    """The engine calls for a message ablation layout: ``variants`` are its records ``(message, kind, unit, samples)`` in layout order
+    (``vb200_message_ablation_layout``).  Each call is a list of pieces ``(message, (token_begin, token_end, box_begin, box_end))``
+    whose variants run at most ``cap`` forward samples.  Messages are kept whole where they fit; a message above ``cap`` is split
+    into pieces of its units (positions first, then boxes), each with its own unablated variant."""
+    calls = _layout_calls(variants, cap, "message_ablation", "unablated variant")
+    return [[(m, _span([u for k, u, _ in a if k == 1]) + _span([u for k, u, _ in a if k == 2])) for m, a in call] for call in calls]
 
 
 def head_messages(messages, batch: int, n_entries: int):
@@ -281,17 +333,9 @@ def head_messages(messages, batch: int, n_entries: int):
         m = tuple(m)
         if not 3 <= len(m) <= 5:
             raise ValueError(f"head_ablation: message {i} has {len(m)} fields (family, image_begin, n_images, answer, entries)")
-        fam, ib, k, answer, entries = m + (None,) * (5 - len(m))
-        f = message_family(fam)
-        ib, k = int(ib), int(k)
-        want = _FAMILY_IMAGES.get(f)
-        if (k != want) if want else k < 1:
-            raise ValueError(f"head_ablation: message {i} has n_images {k} (the family reads {want or '>= 1'})")
-        if ib < 0 or ib + k > batch:
-            raise ValueError(f"head_ablation: message {i} has images [{ib}, {ib + k}) outside the batch of {batch}")
-        a = -1 if answer is None else int(answer)
-        if a < -1:
-            raise ValueError(f"head_ablation: message {i} has answer {a} (an index >= 0, or None / -1: the unablated top-1)")
+        m += (None,) * (5 - len(m))
+        f, ib, k, a = _message_head("head_ablation", i, *m[:4], batch)
+        entries = m[4]
         eb, ee = (0, n_entries) if entries is None else (int(entries[0]), int(entries[1]))
         if not 0 <= eb <= ee <= n_entries:
             raise ValueError(f"head_ablation: message {i} has the entry range [{eb}, {ee}), reversed or outside [0, {n_entries}]")
@@ -304,33 +348,8 @@ def head_calls(variants, max_heads: int, cap: int = L.ABLATION_MAX_VARIANTS):
     (``vb200_head_ablation_layout``).  Each call is a list of pieces ``(message, (entry_begin, entry_end))`` whose variants run at
     most ``cap`` forward samples.  Messages are kept whole where they fit; a message above ``cap`` is split at entry boundaries, each
     piece with its own unablated variant."""
-    groups = []
-    for m, kind, unit, samples in variants:
-        if kind == 0:
-            groups.append((m, samples, {}))
-        else:
-            e = unit // max_heads
-            groups[-1][2][e] = groups[-1][2].get(e, 0) + samples
-    pieces = []
-    for m, base, entries in groups:
-        if base + max(entries.values(), default=0) > cap:
-            raise ValueError(f"head_ablation: message {m} runs {base} samples per variant, too many for {cap} per call")
-        chunk, size = [], base
-        for e, n in sorted(entries.items()):
-            if size + n > cap:
-                pieces.append((m, chunk, size))
-                chunk, size = [], base
-            chunk.append(e)
-            size += n
-        pieces.append((m, chunk, size))
-    calls, size = [], cap + 1
-    for m, chunk, n in pieces:
-        if size + n > cap:
-            calls.append([])
-            size = 0
-        calls[-1].append((m, (chunk[0], chunk[-1] + 1) if chunk else (0, 0)))
-        size += n
-    return calls
+    calls = _layout_calls([(m, kind, unit // max_heads, n) for m, kind, unit, n in variants], cap, "head_ablation", "variant")
+    return [[(m, _span([e for _, e, _ in a])) for m, a in call] for call in calls]
 
 
 # the families a coalition can attribute (grounding's answer is a box, which a coalition would renumber)
@@ -345,21 +364,10 @@ def coalition_messages(messages, batch: int):
         m = tuple(m)
         if not 3 <= len(m) <= 4:
             raise ValueError(f"coalition_ablation: message {i} has {len(m)} fields (family, image_begin, n_images, answer)")
-        fam, ib, k, answer = m + (None,) * (4 - len(m))
-        f = message_family(fam)
-        if f not in COALITION_FAMILIES:
+        if message_family(m[0]) not in COALITION_FAMILIES:
             raise ValueError(f"coalition_ablation: message {i} is a grounding message (its answer is a box, which a coalition would "
                              "renumber)")
-        ib, k = int(ib), int(k)
-        want = _FAMILY_IMAGES.get(f)
-        if (k != want) if want else k < 1:
-            raise ValueError(f"coalition_ablation: message {i} has n_images {k} (the family reads {want or '>= 1'})")
-        if ib < 0 or ib + k > batch:
-            raise ValueError(f"coalition_ablation: message {i} has images [{ib}, {ib + k}) outside the batch of {batch}")
-        a = -1 if answer is None else int(answer)
-        if a < -1:
-            raise ValueError(f"coalition_ablation: message {i} has answer {a} (an index >= 0, or None / -1: the full input's top-1)")
-        out.append((f, ib, k, a))
+        out.append(_message_head("coalition_ablation", i, *m + (None,) * (4 - len(m)), batch, "the full input's top-1"))
     return out
 
 
@@ -409,27 +417,8 @@ def coalition_calls(variants, cap: int = L.ABLATION_MAX_VARIANTS):
     order (``vb200_coalition_ablation_layout``).  Each call is a list of pieces ``(message, (coalition_begin, coalition_end))``
     whose variants run at most ``cap`` forward samples; a message above that is split into runs of its coalitions, each piece with
     its own full-input variant."""
-    groups = []
-    for m, kind, unit, samples in variants:
-        if kind == 0:
-            groups.append((m, samples, 0))
-        else:
-            groups[-1] = groups[-1][:2] + (groups[-1][2] + 1,)
-    pieces = []
-    for m, base, n in groups:
-        if base * (2 if n else 1) > cap:
-            raise ValueError(f"coalition_ablation: message {m} runs {base} samples per variant, too many for {cap} per call")
-        per = max(1, (cap - base) // base)                 # coalitions beside the full input in one piece
-        for c in range(0, max(n, 1), per):
-            pieces.append((m, (c, min(n, c + per)), base * (1 + min(n, c + per) - c)))
-    calls, size = [], cap + 1
-    for m, r, n in pieces:
-        if size + n > cap:
-            calls.append([])
-            size = 0
-        calls[-1].append((m, r))
-        size += n
-    return calls
+    calls = _layout_calls(variants, cap, "coalition_ablation", "variant")
+    return [[(m, _span([c for _, c, _ in a])) for m, a in call] for call in calls]
 
 
 def shapley_permutations(n_units: int, permutations: int, generator, antithetic: bool = True):
@@ -1173,23 +1162,12 @@ class VILBertForVLTasks(object):
         ``self.return_attention``, else ``[]``.  ``output_layer_states`` returns ``(result, states)`` and ``head_mask`` gates the
         heads as in ``forward_packed`` (vb200_forward_regions_packed_gated)."""
         device = self._engine_device()
-        nt, nb = _host_ints(n_tokens), _host_ints(n_boxes)
+        batch = PackedRegionBatch("forward_regions_packed", device, self._dims["v_feature_size"], question, segment_ids, task_tokens,
+                                  box_features, boxes, image_wh, n_tokens, n_boxes)
+        nt, nb = batch.nt, batch.nb
         B = len(nt)
-        if len(nb) != B or B < 1:
-            raise ValueError("forward_regions_packed: n_tokens and n_boxes must have the same, positive length")
-        F = self._dims["v_feature_size"]
-        q = _to_device(question, torch.int64, device).reshape(-1)
-        seg = _to_device(segment_ids if segment_ids is not None else torch.zeros_like(q), torch.int64, device).reshape(-1)
-        tk = _task_rows(task_tokens if task_tokens is not None else torch.zeros(B, 1, dtype=torch.int64), B, device)
-        bf = _to_device(box_features, torch.float32, device).reshape(-1, F)
-        bx = _to_device(boxes, torch.float32, device).reshape(-1, 4)
-        wh = _to_device(image_wh, torch.float32, device)
-        sum_tin, sum_n = sum(nt), sum(nb)
-        if q.numel() != sum_tin or seg.numel() != sum_tin or bf.shape[0] != sum_n or bx.shape[0] != sum_n or tuple(wh.shape) != (B, 2):
-            raise ValueError("forward_regions_packed: question / segment_ids need sum(n_tokens) entries, box_features / boxes "
-                             "sum(n_boxes) rows, image_wh [B, 2]")
-        rows_t = sum_tin + (B if self._dims["task_specific_tokens"] else 0)
-        rows_v = sum_n + B
+        rows_t = sum(nt) + (B if self._dims["task_specific_tokens"] else 0)
+        rows_v = sum(nb) + B
         sp = torch.empty(rows_v, 5, dtype=torch.float32, device=device) if return_spatials else None
         outs, o = self._alloc_packed_outputs(B, rows_t, rows_v, select, debug_taps, device)
         want_attn = bool(output_all_attention_masks and self.return_attention)
@@ -1197,8 +1175,7 @@ class VILBertForVLTasks(object):
             select, maps = self._packed_attention(nt, [n + 1 for n in nb], select, o, device)
         if output_layer_states:
             select, states = self._packed_states(nt, [n + 1 for n in nb], select, o, device)
-        inp = L.PackedRegionInputs(B, int(max_tokens), int(max_boxes), _int32s(nt), _int32s(nb), q.data_ptr(), seg.data_ptr(),
-                                   tk.data_ptr(), bf.data_ptr(), bx.data_ptr(), wh.data_ptr(), sp.data_ptr() if sp is not None else None)
+        inp = batch.inputs(max_tokens, max_boxes, sp.data_ptr() if sp is not None else None)
         if head_mask is None:
             self._call("vb200_forward_regions_packed", C.byref(inp), C.byref(o), select, slot)
         else:
@@ -1240,10 +1217,8 @@ class VILBertForVLTasks(object):
         ``tokens`` / ``boxes`` (the ablated positions and boxes) with ``token_prob`` / ``box_prob`` (the answer's probability without
         that unit) and ``token_top1`` / ``box_top1`` (the variant's own top-1), CPU tensors; with ``return_logits`` also ``logits``,
         a device tensor [1 + tokens + boxes, width] in that variant order."""
-        nt, nb = _host_ints(n_tokens), _host_ints(n_boxes)
+        nt, nb = PackedRegionBatch.lengths("answer_ablation", n_tokens, n_boxes)
         B = len(nt)
-        if len(nb) != B or B < 1:
-            raise ValueError("answer_ablation: n_tokens and n_boxes must have the same, positive length")
         fam = ABLATION_FAMILIES.get(family, 0) if isinstance(family, str) else int(family)
         if fam not in ABLATION_FAMILIES.values():
             raise ValueError(f"answer_ablation: family {family!r} is not one of {sorted(ABLATION_FAMILIES)} (NLVR2, retrieval and "
@@ -1257,42 +1232,19 @@ class VILBertForVLTasks(object):
         if any(a < -1 for a in answers):
             raise ValueError("answer_ablation: an answer column must be >= 0 (or None / -1: the unablated top-1)")
         calls = ablation_calls(ablation_ranges(nt, nb, tokens, boxes_range))
-        device = self._engine_device()
+        batch = PackedRegionBatch("answer_ablation", self._engine_device(), self._dims["v_feature_size"], question, segment_ids,
+                                  task_tokens, box_features, boxes, image_wh, nt, nb)
         d = self._dims
         width = {L.DECODE_VQA: d["num_labels"], L.DECODE_GQA: d["gqa_labels"], L.DECODE_SNLI_VE: 3}[fam]
-        F = d["v_feature_size"]
-        q = _to_device(question, torch.int64, device).reshape(-1)
-        seg = _to_device(segment_ids if segment_ids is not None else torch.zeros_like(q), torch.int64, device).reshape(-1)
-        tk = _task_rows(task_tokens if task_tokens is not None else torch.zeros(B, 1, dtype=torch.int64), B, device)
-        bf = _to_device(box_features, torch.float32, device).reshape(-1, F)
-        bx = _to_device(boxes, torch.float32, device).reshape(-1, 4)
-        wh = _to_device(image_wh, torch.float32, device)
-        t_off, b_off = packed_offsets(nt), packed_offsets(nb)
-        if q.numel() != t_off[-1] or seg.numel() != t_off[-1] or bf.shape[0] != b_off[-1] or bx.shape[0] != b_off[-1] \
-                or tuple(wh.shape) != (B, 2):
-            raise ValueError("answer_ablation: question / segment_ids need sum(n_tokens) entries, box_features / boxes sum(n_boxes) "
-                             "rows, image_wh [B, 2]")
         res = [dict(tokens=[], token_prob=[], token_top1=[], boxes=[], box_prob=[], box_top1=[], logits=[]) for _ in range(B)]
         for call in calls:
-            samples = [i for i, _ in call]
-            if len(calls) == 1:
-                cq, cseg, ctk, cbf, cbx, cwh = q, seg, tk, bf, bx, wh
-            else:                            # this call's samples (or pieces of one), packed back to back
-                tcat = lambda t: torch.cat([t[t_off[i]:t_off[i + 1]] for i in samples])
-                bcat = lambda t: torch.cat([t[b_off[i]:b_off[i + 1]] for i in samples])
-                cq, cseg, cbf, cbx = tcat(q), tcat(seg), bcat(bf), bcat(bx)
-                ctk, cwh = tk[samples].contiguous(), wh[samples].contiguous()
-            msgs = (L.AblationMsg * len(call))(*[L.AblationMsg(answers[i], *r) for i, r in call])
+            sub = batch if len(calls) == 1 else batch.subset([i for i, _ in call])   # this call's samples (or pieces of one)
+            msgs = _structs(L.AblationMsg, [(answers[i],) + r for i, r in call])
             variants = ablation_variants(call)
-            logits = torch.empty(len(variants), width, dtype=torch.float32, device=device)
-            scores = torch.empty(len(variants), 4, dtype=torch.int32, device=device)       # vb200_ablation_score
-            inp = L.PackedRegionInputs(len(call), int(max_tokens), int(max_boxes), _int32s([nt[i] for i in samples]),
-                                       _int32s([nb[i] for i in samples]), cq.data_ptr(), cseg.data_ptr(), ctk.data_ptr(), cbf.data_ptr(),
-                                       cbx.data_ptr(), cwh.data_ptr(), None)
-            self._call("vb200_answer_ablation", C.byref(inp), msgs, fam, int(mask_token), logits.data_ptr(), scores.data_ptr(), int(slot))
-            sc = scores.cpu()
-            col, top1 = sc[:, 0].tolist(), sc[:, 2].tolist()
-            prob, top1_prob = sc[:, 1].view(torch.float32).tolist(), sc[:, 3].view(torch.float32).tolist()
+            logits, col, prob, top1, top1_prob = self._ablation_run("vb200_answer_ablation", sub.inputs(max_tokens, max_boxes),
+                                                                    (msgs, fam, int(mask_token)), len(variants) * width,
+                                                                    len(variants), slot)
+            logits = logits.view(len(variants), width)
             for k, (i, kind, unit) in enumerate(variants):
                 r = res[i]
                 if kind == "base":
@@ -1314,25 +1266,41 @@ class VILBertForVLTasks(object):
                 r["logits"] = torch.cat(logits)
         return res
 
-    def _message_layout(self, n_tokens, n_boxes, msgs):
-        """vb200_message_ablation_layout: the records ``(message, kind, unit, samples, offset, length)`` and the floats they need."""
-        arr = (L.AblationMessage * len(msgs))(*[L.AblationMessage(*m) for m in msgs])
+    def _ablation_layout(self, fn, n_tokens, n_boxes, arr):
+        """``fn`` (vb200_message / head / coalition_ablation_layout) for the engine messages ``arr``: the records ``(message, kind,
+        unit, samples, offset, length)`` and the floats they need."""
         lib, nv, nf, ns = L.load(), C.c_int64(), C.c_int64(), C.c_int64()
-        args = (len(n_tokens), _int32s(n_tokens), _int32s(n_boxes), arr, len(msgs))
-        L.check(lib.vb200_message_ablation_layout(self._handle, *args, None, C.byref(nv), C.byref(nf), C.byref(ns)), self._handle)
+        args = (len(n_tokens), _int32s(n_tokens), _int32s(n_boxes), arr, len(arr))
+        L.check(getattr(lib, fn)(self._handle, *args, None, C.byref(nv), C.byref(nf), C.byref(ns)), self._handle)
         recs = (L.AblationVariant * max(nv.value, 1))()
-        L.check(lib.vb200_message_ablation_layout(self._handle, *args, recs, C.byref(nv), C.byref(nf), C.byref(ns)), self._handle)
-        return [(r.message, r.kind, r.unit, r.samples, r.offset, r.length) for r in recs[:nv.value]], nf.value, arr
+        L.check(getattr(lib, fn)(self._handle, *args, recs, C.byref(nv), C.byref(nf), C.byref(ns)), self._handle)
+        return [(r.message, r.kind, r.unit, r.samples, r.offset, r.length) for r in recs[:nv.value]], nf.value
+
+    def _message_layout(self, n_tokens, n_boxes, msgs):
+        """vb200_message_ablation_layout of messages given as ``_lib.AblationMessage`` field tuples: the records, the floats they
+        need and the struct array."""
+        arr = _structs(L.AblationMessage, msgs)
+        return (*self._ablation_layout("vb200_message_ablation_layout", n_tokens, n_boxes, arr), arr)
 
     def _head_layout(self, n_tokens, n_boxes, msgs):
-        """vb200_head_ablation_layout: the records ``(message, kind, unit, samples, offset, length)`` and the floats they need."""
-        arr = (L.HeadAblationMessage * len(msgs))(*[L.HeadAblationMessage(*m) for m in msgs])
-        lib, nv, nf, ns = L.load(), C.c_int64(), C.c_int64(), C.c_int64()
-        args = (len(n_tokens), _int32s(n_tokens), _int32s(n_boxes), arr, len(msgs))
-        L.check(lib.vb200_head_ablation_layout(self._handle, *args, None, C.byref(nv), C.byref(nf), C.byref(ns)), self._handle)
-        recs = (L.AblationVariant * max(nv.value, 1))()
-        L.check(lib.vb200_head_ablation_layout(self._handle, *args, recs, C.byref(nv), C.byref(nf), C.byref(ns)), self._handle)
-        return [(r.message, r.kind, r.unit, r.samples, r.offset, r.length) for r in recs[:nv.value]], nf.value, arr
+        """vb200_head_ablation_layout of messages given as ``_lib.HeadAblationMessage`` field tuples: the records, the floats they
+        need and the struct array."""
+        arr = _structs(L.HeadAblationMessage, msgs)
+        return (*self._ablation_layout("vb200_head_ablation_layout", n_tokens, n_boxes, arr), arr)
+
+    def _coalition_layout(self, n_tokens, n_boxes, arr):
+        """vb200_coalition_ablation_layout of a ``_lib.CoalitionMessage`` array: the records and the floats they need."""
+        return self._ablation_layout("vb200_coalition_ablation_layout", n_tokens, n_boxes, arr)
+
+    def _ablation_run(self, fn, inp, args, n_floats, n_variants, slot):
+        """One ablation call: ``fn`` on the batch ``inp`` with its message arguments ``args``.  Returns the variants' segments, a
+        device tensor of ``n_floats``, and their scores (vb200_ablation_score) as lists: answer, prob, top1, top1_prob."""
+        device = self._engine_device()
+        logits = torch.empty(n_floats, dtype=torch.float32, device=device)
+        scores = torch.empty(n_variants, 4, dtype=torch.int32, device=device)       # vb200_ablation_score
+        self._call(fn, C.byref(inp), *args, logits.data_ptr(), scores.data_ptr(), int(slot))
+        sc = scores.cpu()
+        return logits, sc[:, 0].tolist(), sc[:, 1].view(torch.float32).tolist(), sc[:, 2].tolist(), sc[:, 3].view(torch.float32).tolist()
 
     @torch.no_grad()
     def head_ablation(self, question, segment_ids, task_tokens, box_features, boxes, image_wh, n_tokens, n_boxes, messages,
@@ -1345,39 +1313,21 @@ class VILBertForVLTasks(object):
         ``head_prob`` (the attributed answer's probability with that head removed) and ``head_top1`` (the variant's top-1), NaN / -1
         where no variant ran (an entry outside the range, or a slot past the entry's head count); with ``return_logits`` the segments
         in layout order."""
-        nt, nb = _host_ints(n_tokens), _host_ints(n_boxes)
-        B = len(nt)
-        if len(nb) != B or B < 1:
-            raise ValueError("head_ablation: n_tokens and n_boxes must have the same, positive length")
+        nt, nb = PackedRegionBatch.lengths("head_ablation", n_tokens, n_boxes)
         if not messages:
             raise ValueError("head_ablation: no messages")
         E, H = head_mask_shape(self.config)
-        msgs = head_messages(messages, B, E)
-        device = self._engine_device()
-        F = self._dims["v_feature_size"]
-        q = _to_device(question, torch.int64, device).reshape(-1)
-        seg = _to_device(segment_ids if segment_ids is not None else torch.zeros_like(q), torch.int64, device).reshape(-1)
-        tk = _task_rows(task_tokens if task_tokens is not None else torch.zeros(B, 1, dtype=torch.int64), B, device)
-        bf = _to_device(box_features, torch.float32, device).reshape(-1, F)
-        bx = _to_device(boxes, torch.float32, device).reshape(-1, 4)
-        wh = _to_device(image_wh, torch.float32, device)
-        if q.numel() != sum(nt) or seg.numel() != sum(nt) or bf.shape[0] != sum(nb) or bx.shape[0] != sum(nb) or tuple(wh.shape) != (B, 2):
-            raise ValueError("head_ablation: question / segment_ids need sum(n_tokens) entries, box_features / boxes sum(n_boxes) "
-                             "rows, image_wh [B, 2]")
+        msgs = head_messages(messages, len(nt), E)
+        batch = PackedRegionBatch("head_ablation", self._engine_device(), self._dims["v_feature_size"], question, segment_ids,
+                                  task_tokens, box_features, boxes, image_wh, nt, nb)
+        inp = batch.inputs(max_tokens, max_boxes)
         recs, _, _ = self._head_layout(nt, nb, msgs)
-        inp = L.PackedRegionInputs(B, int(max_tokens), int(max_boxes), _int32s(nt), _int32s(nb), q.data_ptr(), seg.data_ptr(),
-                                   tk.data_ptr(), bf.data_ptr(), bx.data_ptr(), wh.data_ptr(), None)
         res = [dict(head_prob=torch.full((E, H), float("nan")), head_top1=torch.full((E, H), -1, dtype=torch.int64), logits=[])
                for _ in msgs]
         for call in head_calls([r[:4] for r in recs], H):
-            cmsgs = [msgs[p][:4] + r for p, r in call]
-            crecs, n_floats, arr = self._head_layout(nt, nb, cmsgs)
-            logits = torch.empty(n_floats, dtype=torch.float32, device=device)
-            scores = torch.empty(len(crecs), 4, dtype=torch.int32, device=device)       # vb200_ablation_score
-            self._call("vb200_head_ablation", C.byref(inp), arr, len(cmsgs), logits.data_ptr(), scores.data_ptr(), int(slot))
-            sc = scores.cpu()
-            col, top1 = sc[:, 0].tolist(), sc[:, 2].tolist()
-            prob, top1_prob = sc[:, 1].view(torch.float32).tolist(), sc[:, 3].view(torch.float32).tolist()
+            crecs, n_floats, arr = self._head_layout(nt, nb, [msgs[p][:4] + r for p, r in call])
+            logits, col, prob, top1, top1_prob = self._ablation_run("vb200_head_ablation", inp, (arr, len(arr)), n_floats, len(crecs),
+                                                                    slot)
             for k, (m, kind, unit, _, off, n) in enumerate(crecs):
                 r = res[call[m][0]]
                 if kind == 0:
@@ -1407,39 +1357,20 @@ class VILBertForVLTasks(object):
         ``token_prob`` / ``token_top1``; ``boxes`` as ``(image of the message, box)`` pairs with ``box_prob`` / ``box_top1`` (CPU
         tensors; grounding reports rows in the unablated image's numbering, answer -1 / prob 0 where the attributed box is dropped);
         with ``return_logits`` also ``logits``, the variants' segments (device tensors) in that order."""
-        nt, nb = _host_ints(n_tokens), _host_ints(n_boxes)
-        B = len(nt)
-        if len(nb) != B or B < 1:
-            raise ValueError("message_ablation: n_tokens and n_boxes must have the same, positive length")
+        nt, nb = PackedRegionBatch.lengths("message_ablation", n_tokens, n_boxes)
         if not messages:
             raise ValueError("message_ablation: no messages")
         pieces = message_pieces(messages, nt, nb)
-        device = self._engine_device()
-        F = self._dims["v_feature_size"]
-        q = _to_device(question, torch.int64, device).reshape(-1)
-        seg = _to_device(segment_ids if segment_ids is not None else torch.zeros_like(q), torch.int64, device).reshape(-1)
-        tk = _task_rows(task_tokens if task_tokens is not None else torch.zeros(B, 1, dtype=torch.int64), B, device)
-        bf = _to_device(box_features, torch.float32, device).reshape(-1, F)
-        bx = _to_device(boxes, torch.float32, device).reshape(-1, 4)
-        wh = _to_device(image_wh, torch.float32, device)
-        if q.numel() != sum(nt) or seg.numel() != sum(nt) or bf.shape[0] != sum(nb) or bx.shape[0] != sum(nb) or tuple(wh.shape) != (B, 2):
-            raise ValueError("message_ablation: question / segment_ids need sum(n_tokens) entries, box_features / boxes sum(n_boxes) "
-                             "rows, image_wh [B, 2]")
+        batch = PackedRegionBatch("message_ablation", self._engine_device(), self._dims["v_feature_size"], question, segment_ids,
+                                  task_tokens, box_features, boxes, image_wh, nt, nb)
+        inp = batch.inputs(max_tokens, max_boxes)
         msgs = [p for p, _ in pieces]
         recs, _, _ = self._message_layout(nt, nb, msgs)
-        inp = L.PackedRegionInputs(B, int(max_tokens), int(max_boxes), _int32s(nt), _int32s(nb), q.data_ptr(), seg.data_ptr(),
-                                   tk.data_ptr(), bf.data_ptr(), bx.data_ptr(), wh.data_ptr(), None)
         res = [dict(tokens=[], token_prob=[], token_top1=[], boxes=[], box_prob=[], box_top1=[], logits=[]) for _ in messages]
         for call in message_calls([r[:4] for r in recs]):
-            cmsgs = [msgs[p][:4] + r for p, r in call]
-            crecs, n_floats, arr = self._message_layout(nt, nb, cmsgs)
-            logits = torch.empty(n_floats, dtype=torch.float32, device=device)
-            scores = torch.empty(len(crecs), 4, dtype=torch.int32, device=device)       # vb200_ablation_score
-            self._call("vb200_message_ablation", C.byref(inp), arr, len(cmsgs), int(mask_token), logits.data_ptr(), scores.data_ptr(),
-                       int(slot))
-            sc = scores.cpu()
-            col, top1 = sc[:, 0].tolist(), sc[:, 2].tolist()
-            prob, top1_prob = sc[:, 1].view(torch.float32).tolist(), sc[:, 3].view(torch.float32).tolist()
+            crecs, n_floats, arr = self._message_layout(nt, nb, [msgs[p][:4] + r for p, r in call])
+            logits, col, prob, top1, top1_prob = self._ablation_run("vb200_message_ablation", inp, (arr, len(arr), int(mask_token)),
+                                                                    n_floats, len(crecs), slot)
             for k, (m, kind, unit, _, off, n) in enumerate(crecs):
                 p = call[m][0]
                 r = res[pieces[p][1]]
@@ -1472,15 +1403,6 @@ class VILBertForVLTasks(object):
         return res
 
     # ------------------------------------------------------------------ coalition ablation and Shapley values
-    def _coalition_layout(self, n_tokens, n_boxes, arr):
-        """vb200_coalition_ablation_layout: the records ``(message, kind, unit, samples, offset, length)`` and the floats they need."""
-        lib, nv, nf, ns = L.load(), C.c_int64(), C.c_int64(), C.c_int64()
-        args = (len(n_tokens), _int32s(n_tokens), _int32s(n_boxes), arr, len(arr))
-        L.check(lib.vb200_coalition_ablation_layout(self._handle, *args, None, C.byref(nv), C.byref(nf), C.byref(ns)), self._handle)
-        recs = (L.AblationVariant * max(nv.value, 1))()
-        L.check(lib.vb200_coalition_ablation_layout(self._handle, *args, recs, C.byref(nv), C.byref(nf), C.byref(ns)), self._handle)
-        return [(r.message, r.kind, r.unit, r.samples, r.offset, r.length) for r in recs[:nv.value]], nf.value
-
     @staticmethod
     def _coalition_structs(msgs, units, bitmaps):
         """``_lib.CoalitionMessage`` array for engine messages ``msgs`` with their units and uint64 bitmaps; the arrays the structs
@@ -1500,64 +1422,43 @@ class VILBertForVLTasks(object):
     def _coalition_run(self, name, question, segment_ids, task_tokens, box_features, boxes, image_wh, n_tokens, n_boxes, messages, units,
                        coalitions, mask_token, max_tokens, max_boxes, slot, return_logits):
         """What ``coalition_ablation`` and ``shapley`` share: the messages checked, the layout split along its records into calls of
-        at most 1024 samples, and per message its full input's score and its coalitions' probabilities and top-1s as device tensors."""
-        nt, nb = _host_ints(n_tokens), _host_ints(n_boxes)
-        B = len(nt)
-        if len(nb) != B or B < 1:
-            raise ValueError(f"{name}: n_tokens and n_boxes must have the same, positive length")
+        at most 1024 samples, and per message its full input's score and its coalitions' probabilities and top-1s as lists."""
+        nt, nb = PackedRegionBatch.lengths(name, n_tokens, n_boxes)
         if not messages:
             raise ValueError(f"{name}: no messages")
-        msgs = coalition_messages(messages, B)
+        msgs = coalition_messages(messages, len(nt))
         if len(units) != len(msgs) or len(coalitions) != len(msgs):
             raise ValueError(f"{name}: units and coalitions need one entry per message ({len(msgs)})")
         us = [coalition_units(u, nt[ib], sum(nb[ib:ib + k]), i) for i, (u, (_, ib, k, _)) in enumerate(zip(units, msgs))]
         bms = [coalition_bitmaps(c, len(u)) for c, u in zip(coalitions, us)]
-        device = self._engine_device()
-        F = self._dims["v_feature_size"]
-        q = _to_device(question, torch.int64, device).reshape(-1)
-        seg = _to_device(segment_ids if segment_ids is not None else torch.zeros_like(q), torch.int64, device).reshape(-1)
-        tk = _task_rows(task_tokens if task_tokens is not None else torch.zeros(B, 1, dtype=torch.int64), B, device)
-        bf = _to_device(box_features, torch.float32, device).reshape(-1, F)
-        bx = _to_device(boxes, torch.float32, device).reshape(-1, 4)
-        wh = _to_device(image_wh, torch.float32, device)
-        if q.numel() != sum(nt) or seg.numel() != sum(nt) or bf.shape[0] != sum(nb) or bx.shape[0] != sum(nb) or tuple(wh.shape) != (B, 2):
-            raise ValueError(f"{name}: question / segment_ids need sum(n_tokens) entries, box_features / boxes sum(n_boxes) rows, "
-                             "image_wh [B, 2]")
+        batch = PackedRegionBatch(name, self._engine_device(), self._dims["v_feature_size"], question, segment_ids, task_tokens,
+                                  box_features, boxes, image_wh, nt, nb)
+        inp = batch.inputs(max_tokens, max_boxes)
         arr, keep = self._coalition_structs(msgs, us, bms)
         recs, _ = self._coalition_layout(nt, nb, arr)
-        inp = L.PackedRegionInputs(B, int(max_tokens), int(max_boxes), _int32s(nt), _int32s(nb), q.data_ptr(), seg.data_ptr(),
-                                   tk.data_ptr(), bf.data_ptr(), bx.data_ptr(), wh.data_ptr(), None)
         res = [dict(units=u, prob_d=[], top1_d=[], logits=[], samples=0) for u in us]
         for call in coalition_calls([r[:4] for r in recs]):
             carr, ckeep = self._coalition_structs([msgs[m] for m, _ in call], [us[m] for m, _ in call],
                                                   [bms[m][c0:c1] for m, (c0, c1) in call])
             crecs, n_floats = self._coalition_layout(nt, nb, carr)
-            logits = torch.empty(n_floats, dtype=torch.float32, device=device)
-            scores = torch.empty(len(crecs), 4, dtype=torch.int32, device=device)       # vb200_ablation_score
-            self._call("vb200_coalition_ablation", C.byref(inp), carr, len(carr), int(mask_token), logits.data_ptr(), scores.data_ptr(),
-                       int(slot))
-            prob, top1 = scores[:, 1].view(torch.float32), scores[:, 2]
+            logits, col, prob, top1, top1_prob = self._ablation_run("vb200_coalition_ablation", inp, (carr, len(carr), int(mask_token)),
+                                                                    n_floats, len(crecs), slot)
             at = 0
-            for j, (m, (c0, c1)) in enumerate(call):
+            for m, (c0, c1) in call:
                 r = res[m]
                 n = c1 - c0
                 if "answer" not in r:
-                    sc = scores[at].cpu()
-                    r.update(answer=int(sc[0]), prob=float(sc[1:2].view(torch.float32)), top1=int(sc[2]),
-                             top1_prob=float(sc[3:4].view(torch.float32)))
+                    r.update(answer=col[at], prob=prob[at], top1=top1[at], top1_prob=top1_prob[at])
                     if return_logits:
                         r["logits"].append(logits[crecs[at][4]:crecs[at][4] + crecs[at][5]])
-                r["prob_d"].append(prob[at + 1:at + 1 + n])
-                r["top1_d"].append(top1[at + 1:at + 1 + n])
+                r["prob_d"] += prob[at + 1:at + 1 + n]
+                r["top1_d"] += top1[at + 1:at + 1 + n]
                 if return_logits:
                     r["logits"] += [logits[o:o + k] for *_, o, k in crecs[at + 1:at + 1 + n]]
                 r["samples"] += sum(c[3] for c in crecs[at:at + 1 + n])
                 at += 1 + n
             del carr, ckeep
         del arr, keep
-        for r in res:
-            r["prob_d"] = torch.cat(r["prob_d"])
-            r["top1_d"] = torch.cat(r["top1_d"])
         return res
 
     @torch.no_grad()
@@ -1576,8 +1477,8 @@ class VILBertForVLTasks(object):
         res = self._coalition_run("coalition_ablation", question, segment_ids, task_tokens, box_features, boxes, image_wh, n_tokens,
                                   n_boxes, messages, units, coalitions, mask_token, max_tokens, max_boxes, slot, return_logits)
         for r in res:
-            r["coalition_prob"] = r.pop("prob_d").cpu()
-            r["coalition_top1"] = r.pop("top1_d").cpu().to(torch.int64)
+            r["coalition_prob"] = torch.tensor(r.pop("prob_d"), dtype=torch.float32)
+            r["coalition_top1"] = torch.tensor(r.pop("top1_d"), dtype=torch.int64)
             logits = r.pop("logits")
             if return_logits:
                 r["logits"] = logits
@@ -1595,13 +1496,11 @@ class VILBertForVLTasks(object):
         message and the P (n - 1) interior chain coalitions after them.  Returns per message ``answer``, ``prob`` (v(all)),
         ``empty_prob`` (v(empty)), ``units``, ``phi`` and ``stderr`` (float32 CPU tensors [n_units]), ``perm`` and ``samples`` (the
         forward samples run)."""
-        msgs = coalition_messages(messages, len(_host_ints(n_tokens)))
+        nt, nb = PackedRegionBatch.lengths("shapley", n_tokens, n_boxes)
+        msgs = coalition_messages(messages, len(nt))
         units = [None] * len(msgs) if units is None else list(units)
         if len(units) != len(msgs):
             raise ValueError(f"shapley: units need one entry per message ({len(msgs)})")
-        nt, nb = _host_ints(n_tokens), _host_ints(n_boxes)
-        if len(nb) != len(nt):
-            raise ValueError("shapley: n_tokens and n_boxes must have the same, positive length")
         units = [coalition_units(u, nt[ib], sum(nb[ib:ib + k]), i) for i, (u, (_, ib, k, _)) in enumerate(zip(units, msgs))]
         gen = torch.Generator().manual_seed(int(seed))
         perms = [shapley_permutations(len(u), permutations, gen, antithetic) for u in units]
@@ -1613,11 +1512,10 @@ class VILBertForVLTasks(object):
         values, descs, at_v, at_p, at_o = [], [], 0, 0, 0
         for r, p in zip(res, perms):
             P, n = p.shape
-            full = torch.tensor([r["prob"]], dtype=torch.float32, device=device)
-            values.append(torch.cat([r["prob_d"][:1], full, r["prob_d"][1:]]))
+            values += r["prob_d"][:1] + [r["prob"]] + r["prob_d"][1:]
             descs.append(L.ShapleyMessage(n, P, g, at_p, at_v, at_o))
             at_v, at_p, at_o = at_v + 2 + P * (n - 1), at_p + P * n, at_o + n
-        vals = torch.cat(values).contiguous()
+        vals = torch.tensor(values, dtype=torch.float32, device=device)
         perm_d = torch.cat([p.reshape(-1) for p in perms]).to(device=device, dtype=torch.int32)
         phi = torch.empty(at_o, dtype=torch.float32, device=device)
         se = torch.empty(at_o, dtype=torch.float32, device=device)

@@ -551,6 +551,26 @@ def _pixel_box(info, row):
     return [float(v) for v in np.asarray(info["bbox"], dtype=np.float32)[row - 1, :4]]
 
 
+def _explain_packed(requests, max_boxes, messages, explain):
+    """What the `custom_*_packed` explainers share: the requests packed by `pack_region_requests`, then under `model_lock` their
+    answers (`custom_prediction_packed`, decode="device") and `explain(args, msgs, mask, kw)` on the same batch: `args` the
+    batch's arguments of `model.forward_regions_packed`, `msgs` the list of `messages(spans)` ({request: message}), `mask` the
+    tokenizer's [MASK] id and `kw` the plan capacities.  Returns (answers, the packed batch `p`, the message dict, explain's
+    results); with no request that passes validation, or no message, nothing is explained."""
+    p = pack_region_requests(requests, max_boxes=max_boxes)
+    if not p["spans"]:
+        return p["answers"], p, {}, []
+    args = (p["question"], p["segment_ids"], p["task_tokens"], p["box_features"], p["boxes"], p["image_wh"], p["n_tokens"], p["n_boxes"])
+    msgs = messages(p["spans"])
+    mask = (tokenizer.vocab.get("[MASK]", 103) if tokenizer is not None and hasattr(tokenizer, "vocab") else 103)
+    kw = dict(max_tokens=p["max_tokens"], max_boxes=p["max_boxes"])
+    with model_lock:
+        out, spatials = model.forward_regions_packed(*args, select=p["select"], **kw)
+        res = explain(args, list(msgs.values()), mask, kw) if msgs else []
+    answers = _answer_regions(p["answers"], requests, out, spatials, p["spans"], p["n_tokens"], p["n_boxes"], "device")
+    return answers, p, msgs, res
+
+
 def custom_ablation_packed(requests, max_boxes: int = 100, *, tokens=None, boxes=None):
     """Why each answer: `custom_prediction_packed` (decode="device") for `custom_prediction` argument tuples
     `(query, task, features, infos, task_id)`, plus the answer's ablation over its question tokens and detector boxes
@@ -560,17 +580,8 @@ def custom_ablation_packed(requests, max_boxes: int = 100, *, tokens=None, boxes
     Returns per request `{"answer": <custom_prediction_packed's answer>, "ablation": <message_ablation's dict>}` -- whose `boxes` are
     `(image, box)` pairs, with `box_pixels` their [x1, y1, x2, y2] from `infos`, and for grounding `answer_box` the pixel box of the
     attributed row -- or the exception of a request that fails validation."""
-    p = pack_region_requests(requests, max_boxes=max_boxes)
-    answers = p["answers"]
-    if not p["spans"]:
-        return answers
-    args = (p["question"], p["segment_ids"], p["task_tokens"], p["box_features"], p["boxes"], p["image_wh"], p["n_tokens"], p["n_boxes"])
-    msgs = ablation_messages(requests, p["spans"], tokens, boxes)
-    mask = (tokenizer.vocab.get("[MASK]", 103) if tokenizer is not None and hasattr(tokenizer, "vocab") else 103)
-    with model_lock:
-        out, spatials = model.forward_regions_packed(*args, select=p["select"], max_tokens=p["max_tokens"], max_boxes=p["max_boxes"])
-        ab = model.message_ablation(*args, list(msgs.values()), mask_token=mask, max_tokens=p["max_tokens"], max_boxes=p["max_boxes"])
-    answers = _answer_regions(answers, requests, out, spatials, p["spans"], p["n_tokens"], p["n_boxes"], "device")
+    answers, _, msgs, ab = _explain_packed(requests, max_boxes, lambda spans: ablation_messages(requests, spans, tokens, boxes),
+                                           lambda args, m, mask, kw: model.message_ablation(*args, m, mask_token=mask, **kw))
     for i, a in zip(msgs, ab):
         infos = requests[i][3]
         a["box_pixels"] = [_pixel_box(infos[img], b + 1) for img, b in a["boxes"]]
@@ -586,16 +597,9 @@ def custom_head_ablation_packed(requests, max_boxes: int = 100, *, entries=None)
     answer reads, as `custom_ablation_packed` chooses them.  `entries`: one (begin, end) range of attention entries for every
     request, or None for all.  Returns per request `{"answer": <custom_prediction_packed's answer>, "ablation": <head_ablation's
     dict>}`, or the exception of a request that fails validation."""
-    p = pack_region_requests(requests, max_boxes=max_boxes)
-    answers = p["answers"]
-    if not p["spans"]:
-        return answers
-    args = (p["question"], p["segment_ids"], p["task_tokens"], p["box_features"], p["boxes"], p["image_wh"], p["n_tokens"], p["n_boxes"])
-    msgs = {i: m[:4] + (entries,) for i, m in ablation_messages(requests, p["spans"]).items()}
-    with model_lock:
-        out, spatials = model.forward_regions_packed(*args, select=p["select"], max_tokens=p["max_tokens"], max_boxes=p["max_boxes"])
-        ab = model.head_ablation(*args, list(msgs.values()), max_tokens=p["max_tokens"], max_boxes=p["max_boxes"])
-    answers = _answer_regions(answers, requests, out, spatials, p["spans"], p["n_tokens"], p["n_boxes"], "device")
+    answers, _, msgs, ab = _explain_packed(
+        requests, max_boxes, lambda spans: {i: m[:4] + (entries,) for i, m in ablation_messages(requests, spans).items()},
+        lambda args, m, mask, kw: model.head_ablation(*args, m, **kw))
     for i, a in zip(msgs, ab):
         answers[i] = {"answer": answers[i], "ablation": a}
     return answers
@@ -608,19 +612,11 @@ def custom_shapley_packed(requests, max_boxes: int = 100, *, units=None, permuta
     or `(positions, boxes)` groups applied to every request.  Returns per request `{"answer": <custom_prediction_packed's answer>,
     "shapley": <shapley's dict>}` -- with `box_pixels`, per unit the [x1, y1, x2, y2] of its boxes from `infos` -- or the exception of
     a request that fails validation.  Grounding requests get a ValueError: their answer is a box, which a coalition would renumber."""
-    p = pack_region_requests(requests, max_boxes=max_boxes)
-    answers = p["answers"]
-    if not p["spans"]:
-        return answers
-    args = (p["question"], p["segment_ids"], p["task_tokens"], p["box_features"], p["boxes"], p["image_wh"], p["n_tokens"], p["n_boxes"])
-    msgs = {i: m[:4] for i, m in ablation_messages(requests, p["spans"]).items() if requests[i][4] not in GROUNDING_TASKS}
-    mask = (tokenizer.vocab.get("[MASK]", 103) if tokenizer is not None and hasattr(tokenizer, "vocab") else 103)
-    with model_lock:
-        out, spatials = model.forward_regions_packed(*args, select=p["select"], max_tokens=p["max_tokens"], max_boxes=p["max_boxes"])
-        sh = model.shapley(*args, list(msgs.values()), units=None if units is None else [units] * len(msgs), permutations=permutations,
-                           seed=seed, antithetic=antithetic, mask_token=mask, max_tokens=p["max_tokens"],
-                           max_boxes=p["max_boxes"]) if msgs else []
-    answers = _answer_regions(answers, requests, out, spatials, p["spans"], p["n_tokens"], p["n_boxes"], "device")
+    answers, p, msgs, sh = _explain_packed(
+        requests, max_boxes,
+        lambda spans: {i: m[:4] for i, m in ablation_messages(requests, spans).items() if requests[i][4] not in GROUNDING_TASKS},
+        lambda args, m, mask, kw: model.shapley(*args, m, units=None if units is None else [units] * len(m), permutations=permutations,
+                                                seed=seed, antithetic=antithetic, mask_token=mask, **kw))
     for i in p["spans"]:
         if i not in msgs:
             answers[i] = ValueError("custom_shapley_packed: a grounding answer is a box, which a coalition would renumber")
