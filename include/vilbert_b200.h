@@ -747,6 +747,41 @@ typedef struct {
 int vb200_shapley_values(vb200_handle h, const vb200_shapley_message* msgs /* HOST [n_msgs] */, int32_t n_msgs, const int32_t* perm,
                          const float* values, float* phi, float* stderr_out, void* cuda_stream);
 
+/* ---- Shapley-Taylor interaction indices of order 2 (Sundararajan, Dhamdhere & Agarwal 2020) from the same permutation chains, on
+ * the device (float64 throughout): which pairs of units an answer needs together (> 0) or either of (< 0).  For a pair {a, b} the
+ * index is the mean over permutations of v(S + {a, b}) - v(S + {a}) - v(S + {b}) + v(S), S the units before the first of a and b.
+ * Message i has n = n_units >= 2 units, P = n_perm permutations in groups of g = group (as vb200_shapley_values) and Q = n_pairs
+ * pairs (a, b), a != b, both in [0, n).  perm + perm_offset as vb200_shapley_values.  values + value_offset: DEVICE fp32
+ * [2 + P (n - 1) + 2 P Q]: the 2 + P (n - 1) values vb200_shapley_values reads (so the same value_offset serves both calls), then for
+ * p = 0 .. P-1 and q = 0 .. Q-1 the pair x1[p][q] at 2 + P (n - 1) + 2 (p Q + q) and x2[p][q] right after it.  With r the smaller of
+ * pair q's two ranks in row p (rank: the unit's position in the row), S the first r units of row p and "second" whichever of a, b has
+ * the larger rank: x1[p][q] = v(S + {second}), x2[p][q] = v(S + {a, b}).  With c[p][j] as in vb200_shapley_values and every value
+ * widened to double:
+ *   d[p][q] = ((x2[p][q] - c[p][r + 1]) - x1[p][q]) + c[p][r];
+ *   s = 0; for p = 0 .. P-1: s = s + d[p][q];              I_q = s / P;
+ *   G = P / g; for k = 0 .. G-1: m = 0; for i = 0 .. g-1: m = m + d[k g + i][q];  m = m / g;  t = m - I_q;  ss = ss + t * t
+ *     (ss from 0);
+ *   stderr_q = sqrt((ss / (G - 1)) / G), NaN when G < 2.
+ * Each step is one correctly rounded float64 operation in that order (no fused multiply-add), so a numpy restatement in float64
+ * reproduces it bit for bit; (a, b) and (b, a) give the same bits, since r and "second" follow the ranks.  inter + out_offset and
+ * stderr + out_offset: DEVICE fp32 [Q], the float64 results rounded to nearest.  A permutation row that is not a permutation gives
+ * NaN in both outputs for every pair of its message.  Pair q's first and second differences come from four values:
+ * c[p][r] = v(S), c[p][r + 1] = v(S + {first}) from the chain, x1 and x2 from two more coalitions per permutation and pair.
+ * VB200_ERR_INVALID, with nothing enqueued and a message naming the message or pair, for every rejection of vb200_shapley_values,
+ * n_units < 2, n_pairs < 1, more than VB200_INTERACTION_MAX_PAIRS pairs over all messages, NULL pairs, and a pair with a == b or an
+ * index outside [0, n).  The pairs are staged with the descriptors; asynchronous on cuda_stream. */
+#define VB200_INTERACTION_MAX_PAIRS 65536     /* pairs per call, all messages together */
+typedef struct {
+    int32_t n_units, n_perm, group, n_pairs;
+    int64_t perm_offset;              /* int32 elements of perm where the message's [n_perm, n_units] table starts */
+    int64_t value_offset;             /* floats of values where its 2 + P (n - 1) + 2 P Q values start (layout above) */
+    int64_t out_offset;               /* floats of inter and of stderr_out where its n_pairs outputs start */
+    const int32_t* pairs;             /* HOST [n_pairs, 2] unit indices (a, b) */
+} vb200_interaction_message;
+
+int vb200_interaction_values(vb200_handle h, const vb200_interaction_message* msgs /* HOST [n_msgs] */, int32_t n_msgs,
+                             const int32_t* perm, const float* values, float* inter, float* stderr_out, void* cuda_stream);
+
 /* ---- Detector-region selection: the feature extraction step of the reference worker (worker.py:123-176) on the detector's raw heads,
  * for every image of a batch in one call, written straight into the packed box_features / boxes that vb200_forward_regions_packed reads.
  * For image i with n_i proposals, C score columns (column 0 is background) and features [n_i, F]:

@@ -164,6 +164,16 @@ class ShapleyMessage(C.Structure):
                 ("value_offset", C.c_int64), ("out_offset", C.c_int64)]
 
 
+INTERACTION_MAX_PAIRS = 65536
+
+
+class InteractionMessage(C.Structure):
+    """vb200_interaction_message: units, permutations, group size and pair count of one message, where its permutation table,
+    values and outputs start in the call's device arrays, and its HOST int32 [n_pairs, 2] pairs."""
+    _fields_ = [("n_units", C.c_int32), ("n_perm", C.c_int32), ("group", C.c_int32), ("n_pairs", C.c_int32),
+                ("perm_offset", C.c_int64), ("value_offset", C.c_int64), ("out_offset", C.c_int64), ("pairs", C.c_void_p)]
+
+
 class Detections(C.Structure):
     """vb200_detections: one image's raw detector heads (device pointers) and its first output row."""
     _fields_ = [("n_proposals", C.c_int32), ("dst_row", C.c_int32), ("im_scale", C.c_double), ("proposals", C.c_void_p),
@@ -223,7 +233,7 @@ EXPORTS = ["vb200_abi_version", "vb200_create", "vb200_destroy", "vb200_last_err
            "vb200_pretraining_heads", "vb200_create_pretraining", "vb200_pretraining_objectives", "vb200_answer_ablation",
            "vb200_message_ablation_layout", "vb200_message_ablation", "vb200_forward_packed_gated", "vb200_forward_regions_packed_gated",
            "vb200_head_ablation_layout", "vb200_head_ablation", "vb200_coalition_ablation_layout", "vb200_coalition_ablation",
-           "vb200_shapley_values"]
+           "vb200_shapley_values", "vb200_interaction_values"]
 
 _lib = None
 
@@ -320,6 +330,7 @@ def load():
                                                     C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     lib.vb200_coalition_ablation.argtypes = [vp, C.POINTER(PackedRegionInputs), C.POINTER(CoalitionMessage), i32, i64, vp, vp, i32, vp]
     lib.vb200_shapley_values.argtypes = [vp, C.POINTER(ShapleyMessage), i32, vp, vp, vp, vp, vp]
+    lib.vb200_interaction_values.argtypes = [vp, C.POINTER(InteractionMessage), i32, vp, vp, vp, vp, vp]
     for name in EXPORTS:
         if name not in ("vb200_last_error",):
             getattr(lib, name).restype = C.c_int

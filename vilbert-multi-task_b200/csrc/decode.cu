@@ -206,4 +206,71 @@ cudaError_t launch_shapley_values(const ShapleyDesc* descs, int n, cudaStream_t 
     return launch_ex(shapley_values_kernel, dim3(n), dim3(kShapleyMaxUnits), 0, 0, st, descs);
 }
 
+// Shapley-Taylor pair indices: CTA (m, k) takes pairs [k * 1024, k * 1024 + 1024) of message m, thread t owns pair k * 1024 + t.
+// For each permutation p the CTA inverts row p into shared memory as shapley_values_kernel does; each thread then reads its pair's
+// two ranks, the chain values c[p][r] and c[p][r + 1] and its x1, x2, and forms the second difference in float64.  Pass 1 sums the
+// differences over p in order; pass 2 recomputes them group by group for the two-pass standard error.  Each thread's sums are
+// serial in p, so numpy's sequential float64 arithmetic gives the same bits.  Thread t < n also checks that unit t has a position in
+// row p; every CTA of a message checks every row in full, so a row that is not a permutation gives NaN for every pair of the message.
+__global__ void __launch_bounds__(kInteractionPairs)
+interaction_values_kernel(const InteractionDesc* __restrict__ descs) {
+    __shared__ int inv[kShapleyMaxUnits];
+    const InteractionDesc d = descs[blockIdx.x];
+    const int q = blockIdx.y * kInteractionPairs + threadIdx.x;
+    if (blockIdx.y * kInteractionPairs >= d.n_pairs) return;         // the whole CTA: this message has fewer pairs
+    const int n = d.n_units, P = d.n_perm, g = d.group, Q = d.n_pairs, t = threadIdx.x;
+    const bool on = q < Q;
+    const int a = on ? d.pairs[2 * q] : 0, b = on ? d.pairs[2 * q + 1] : 0;
+    const float* __restrict__ v = d.values;
+    const float* __restrict__ x = v + 2 + static_cast<int64_t>(P) * (n - 1);    // x1, x2 of (p, q) at 2 (p Q + q)
+    auto chain = [&](int p, int j) -> double {                 // c[p][j]: v(empty) at 0, the chain in between (j < n here)
+        return static_cast<double>(j == 0 ? v[0] : v[2 + static_cast<int64_t>(p) * (n - 1) + (j - 1)]);
+    };
+    bool bad = false;
+    auto delta = [&](int p) -> double {                        // the pair's second difference in permutation p (every thread calls)
+        const int32_t* __restrict__ row = d.perm + static_cast<int64_t>(p) * n;
+        __syncthreads();                                       // the previous permutation's reads of inv are done
+        if (t < n) inv[t] = -1;
+        __syncthreads();
+        if (t < n) {
+            const int w = row[t];
+            if (w >= 0 && w < n) inv[w] = t;
+        }
+        __syncthreads();
+        if (t < n && inv[t] < 0) bad = true;                   // unit t has no position: row p is not a permutation
+        if (!on) return 0.0;
+        const int ra = inv[a], rb = inv[b];
+        if (ra < 0 || rb < 0) return 0.0;                      // flagged by the threads of units a and b
+        const int r = min(ra, rb);
+        const int64_t at = 2 * (static_cast<int64_t>(p) * Q + q);
+        const double x1 = static_cast<double>(x[at]), x2 = static_cast<double>(x[at + 1]);
+        return __dadd_rn(__dsub_rn(__dsub_rn(x2, chain(p, r + 1)), x1), chain(p, r));
+    };
+    double sum = 0.0;
+    for (int p = 0; p < P; ++p) sum = __dadd_rn(sum, delta(p));
+    const double inter = __ddiv_rn(sum, static_cast<double>(P));
+    const int G = P / g;
+    double ss = 0.0;
+    for (int k = 0; k < G; ++k) {
+        double m = 0.0;
+        for (int i = 0; i < g; ++i) m = __dadd_rn(m, delta(k * g + i));
+        m = __ddiv_rn(m, static_cast<double>(g));
+        const double dm = __dsub_rn(m, inter);
+        ss = __dadd_rn(ss, __dmul_rn(dm, dm));
+    }
+    bad = __syncthreads_or(bad) != 0;
+    if (!on) return;
+    const double nan = __longlong_as_double(0x7ff8000000000000ll);
+    const double se = G < 2 ? nan : __dsqrt_rn(__ddiv_rn(__ddiv_rn(ss, static_cast<double>(G - 1)), static_cast<double>(G)));
+    d.inter[q] = static_cast<float>(bad ? nan : inter);
+    d.stderr_out[q] = static_cast<float>(bad ? nan : se);
+}
+
+// messages along x (any count), pair blocks along y (at most VB200_INTERACTION_MAX_PAIRS / 1024 = 64)
+cudaError_t launch_interaction_values(const InteractionDesc* descs, int n, int max_pairs, cudaStream_t st) {
+    if (n < 1 || max_pairs < 1) return cudaErrorInvalidValue;
+    const dim3 grid(n, (max_pairs + kInteractionPairs - 1) / kInteractionPairs);
+    return launch_ex(interaction_values_kernel, grid, dim3(kInteractionPairs), 0, 0, st, descs);
+}
+
 }  // namespace vb

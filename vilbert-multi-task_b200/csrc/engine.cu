@@ -2611,6 +2611,61 @@ struct vb200_engine {
         CUDA_CHECK(vb::launch_shapley_values(stage_decode(d, st), n_msgs, st));
         dec_ws.release(st);
     }
+    // vb200_interaction_values: every descriptor and pair is checked before anything is enqueued; the pairs follow the descriptors in
+    // one staged copy
+    void interaction_values(const vb200_interaction_message* msgs, int n_msgs, const int32_t* perm, const float* values, float* inter,
+                            float* se, cudaStream_t st) {
+        const char* api = "vb200_interaction_values";
+        if (msgs == nullptr || perm == nullptr || values == nullptr || inter == nullptr || se == nullptr)
+            fail(VB200_ERR_INVALID, "%s: msgs / perm / values / inter / stderr is NULL", api);
+        if (n_msgs < 1) fail(VB200_ERR_INVALID, "%s: n_msgs must be positive (n_msgs = %d)", api, n_msgs);
+        if ((reinterpret_cast<uintptr_t>(perm) | reinterpret_cast<uintptr_t>(values) | reinterpret_cast<uintptr_t>(inter) |
+             reinterpret_cast<uintptr_t>(se)) & 3)
+            fail(VB200_ERR_INVALID, "%s: perm / values / inter / stderr is not 4-byte aligned", api);
+        std::vector<vb::InteractionDesc> d(n_msgs);
+        int64_t total = 0;
+        int max_pairs = 0;
+        for (int i = 0; i < n_msgs; ++i) {
+            const vb200_interaction_message& m = msgs[i];
+            if (m.n_units < 2 || m.n_units > VB200_COALITION_MAX_UNITS)
+                fail(VB200_ERR_INVALID, "%s: message %d has n_units %d outside [2, %d]", api, i, m.n_units, VB200_COALITION_MAX_UNITS);
+            if (m.n_perm < 1) fail(VB200_ERR_INVALID, "%s: message %d has n_perm %d (must be >= 1)", api, i, m.n_perm);
+            if (m.group != 1 && m.group != 2) fail(VB200_ERR_INVALID, "%s: message %d has group %d (1 or 2)", api, i, m.group);
+            if (m.n_perm % m.group) fail(VB200_ERR_INVALID, "%s: message %d has n_perm %d, not a multiple of group %d", api, i, m.n_perm, m.group);
+            if (m.perm_offset < 0 || m.value_offset < 0 || m.out_offset < 0)
+                fail(VB200_ERR_INVALID, "%s: message %d has a negative offset", api, i);
+            if (m.n_pairs < 1) fail(VB200_ERR_INVALID, "%s: message %d has n_pairs %d (must be >= 1)", api, i, m.n_pairs);
+            if (m.pairs == nullptr) fail(VB200_ERR_INVALID, "%s: message %d has NULL pairs", api, i);
+            total += m.n_pairs;
+            if (total > VB200_INTERACTION_MAX_PAIRS)
+                fail(VB200_ERR_INVALID, "%s: the pairs of messages 0..%d number %lld, above %d (split the messages across calls)", api, i,
+                     static_cast<long long>(total), VB200_INTERACTION_MAX_PAIRS);
+            for (int q = 0; q < m.n_pairs; ++q) {
+                const int a = m.pairs[2 * q], b = m.pairs[2 * q + 1];
+                if (a < 0 || a >= m.n_units || b < 0 || b >= m.n_units)
+                    fail(VB200_ERR_INVALID, "%s: message %d pair %d (%d, %d) has a unit outside [0, %d)", api, i, q, a, b, m.n_units);
+                if (a == b) fail(VB200_ERR_INVALID, "%s: message %d pair %d pairs unit %d with itself", api, i, q, a);
+            }
+            max_pairs = std::max(max_pairs, static_cast<int>(m.n_pairs));
+            d[i] = {perm + m.perm_offset, values + m.value_offset, nullptr, inter + m.out_offset, se + m.out_offset, m.n_units, m.n_perm,
+                    m.group, m.n_pairs};
+        }
+        CUDA_CHECK(cudaSetDevice(opt.device));
+        const size_t desc_bytes = d.size() * sizeof(vb::InteractionDesc), bytes = desc_bytes + static_cast<size_t>(total) * 8;
+        char* dst = dec_ws.acquire(bytes, st);
+        dec_in.stage(bytes, st, [&](char* h, const auto& put) {
+            size_t at = desc_bytes;
+            for (int i = 0; i < n_msgs; ++i) {
+                d[i].pairs = reinterpret_cast<const int32_t*>(dst + at);
+                memcpy(h + at, msgs[i].pairs, static_cast<size_t>(msgs[i].n_pairs) * 8);
+                at += static_cast<size_t>(msgs[i].n_pairs) * 8;
+            }
+            memcpy(h, d.data(), desc_bytes);
+            put(dst, 0, bytes);
+        });
+        CUDA_CHECK(vb::launch_interaction_values(reinterpret_cast<const vb::InteractionDesc*>(dst), n_msgs, max_pairs, st));
+        dec_ws.release(st);
+    }
     // ---- region selection: every descriptor is checked before anything is enqueued
     void select_regions(const vb200_detections* imgs, int n, const vb200_select_params* p, const vb200_selected* out, cudaStream_t st) {
         const char* api = "vb200_select_regions";
@@ -3338,6 +3393,12 @@ int vb200_shapley_values(vb200_handle h, const vb200_shapley_message* msgs, int3
                          float* phi, float* stderr_out, void* cuda_stream) {
     if (h == nullptr) return VB200_ERR_INVALID;
     return guard(h, [&] { h->shapley_values(msgs, n_msgs, perm, values, phi, stderr_out, static_cast<cudaStream_t>(cuda_stream)); });
+}
+
+int vb200_interaction_values(vb200_handle h, const vb200_interaction_message* msgs, int32_t n_msgs, const int32_t* perm,
+                             const float* values, float* inter, float* stderr_out, void* cuda_stream) {
+    if (h == nullptr) return VB200_ERR_INVALID;
+    return guard(h, [&] { h->interaction_values(msgs, n_msgs, perm, values, inter, stderr_out, static_cast<cudaStream_t>(cuda_stream)); });
 }
 
 int vb200_head_ablation(vb200_handle h, const vb200_packed_region_inputs* in, const vb200_head_ablation_message* msgs, int32_t n_msgs,

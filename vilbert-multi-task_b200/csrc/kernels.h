@@ -230,6 +230,14 @@ cudaError_t launch_segment_gather(const SegmentDesc* descs, int n, const Segment
 struct ShapleyDesc { const int32_t* perm; const float* values; float* phi; float* stderr_out; int32_t n_units, n_perm, group; };
 constexpr int kShapleyMaxUnits = 1024;
 cudaError_t launch_shapley_values(const ShapleyDesc* descs, int n, cudaStream_t st);
+// Shapley-Taylor pair indices (decode.cu, vb200_interaction_values): the arithmetic documented at vb200_interaction_values.  CTA
+// (m, k) takes pairs [k * kInteractionPairs, (k + 1) * kInteractionPairs) of message m, one thread per pair; max_pairs is the
+// largest n_pairs of the call.  pairs: [n_pairs, 2] int32 on the device, values: 2 + P (n - 1) + 2 P Q floats, inter / stderr: Q.
+struct InteractionDesc {
+    const int32_t* perm; const float* values; const int32_t* pairs; float* inter; float* stderr_out; int32_t n_units, n_perm, group, n_pairs;
+};
+constexpr int kInteractionPairs = 1024;
+cudaError_t launch_interaction_values(const InteractionDesc* descs, int n, int max_pairs, cudaStream_t st);
 // Attention relevance (relevance.cu, vb200_attention_relevance): per sample b (one CTA) the rollout rows of the text CLS row and the
 // image global row, [2, T_b + V_b] at relevance + out.  Entry e of the maps starts at float `offset` and holds sample b's
 // [heads, Lq_b, Lk_b] block at heads * prefix[k] (k 0 text layers, 1 image layers, 2 both directions of a connection layer); kinds

@@ -480,6 +480,105 @@ def shapley_reference(values, perm, group: int, dtype=np.float32):
     return phi.astype(dtype), se.astype(dtype)
 
 
+def cross_pairs(units):
+    """Every (word unit, box unit) pair of one message's ``units`` (``(positions, boxes)`` tuples) in unit order: a word unit has
+    positions only, a box unit boxes only; units with both are in no pair."""
+    words = [u for u, (ps, bs) in enumerate(units) if ps and not bs]
+    boxes = [u for u, (ps, bs) in enumerate(units) if bs and not ps]
+    return [(w, b) for w in words for b in boxes]
+
+
+def interaction_pairs(pairs, units):
+    """``shapley_interactions``' ``pairs`` checked against each message's ``units``: per message ``"cross"`` (``cross_pairs``) or a
+    list of ``(a, b)`` unit indices, a != b.  Returns int32 numpy arrays [Q, 2], at least one pair per message and at most
+    ``_lib.INTERACTION_MAX_PAIRS`` over all messages."""
+    pairs = list(pairs)
+    if len(pairs) != len(units):
+        raise ValueError(f"shapley_interactions: pairs need one entry per message ({len(units)})")
+    out, total = [], 0
+    for i, (p, us) in enumerate(zip(pairs, units)):
+        n = len(us)
+        if n < 2:
+            raise ValueError(f"shapley_interactions: message {i} has {n} unit; a pair needs two")
+        if isinstance(p, str):
+            if p != "cross":
+                raise ValueError(f"shapley_interactions: message {i} pairs {p!r}: a list of (a, b) or \"cross\"")
+            p = cross_pairs(us)
+        a = np.asarray([tuple(int(x) for x in ab) for ab in p], dtype=np.int64).reshape(-1, 2)
+        if len(a) == 0:
+            raise ValueError(f"shapley_interactions: message {i} has no pairs")
+        for q, (x, y) in enumerate(a.tolist()):
+            if not (0 <= x < n and 0 <= y < n):
+                raise ValueError(f"shapley_interactions: message {i} pair {q} ({x}, {y}) has a unit outside [0, {n})")
+            if x == y:
+                raise ValueError(f"shapley_interactions: message {i} pair {q} pairs unit {x} with itself")
+        total += len(a)
+        if total > L.INTERACTION_MAX_PAIRS:
+            raise ValueError(f"shapley_interactions: messages 0..{i} have {total} pairs, above {L.INTERACTION_MAX_PAIRS}")
+        out.append(a.astype(np.int32))
+    return out
+
+
+def _ranks(perm):
+    """rank[p, u]: the position of unit u in row p of ``perm`` (int64 [P, n])."""
+    P, n = perm.shape
+    rank = torch.empty_like(perm)
+    rank.scatter_(1, perm, torch.arange(n).expand(P, n).contiguous())
+    return rank
+
+
+def interaction_coalitions(perm, pairs):
+    """The coalitions the Shapley-Taylor pair indices add to ``shapley_chain(perm)``: for each row p of ``perm`` and pair q = (a, b)
+    of ``pairs`` [Q, 2], with S the units ranked before the first of a and b in row p, S + {second} then S + {a, b}.
+    bool [2 P Q, n], True: present."""
+    perm = torch.as_tensor(perm, dtype=torch.int64)
+    pairs = torch.as_tensor(np.asarray(pairs), dtype=torch.int64).reshape(-1, 2)
+    P, n = perm.shape
+    Q = pairs.shape[0]
+    rank = _ranks(perm)
+    ra, rb = rank[:, pairs[:, 0]], rank[:, pairs[:, 1]]                        # [P, Q]
+    a, b = pairs[:, 0].expand(P, Q), pairs[:, 1].expand(P, Q)
+    first, second = torch.where(ra < rb, a, b), torch.where(ra < rb, b, a)
+    x1 = rank.view(P, 1, n) < torch.minimum(ra, rb).view(P, Q, 1)              # S
+    x1.scatter_(2, second.unsqueeze(2), True)
+    x2 = x1.clone()
+    x2.scatter_(2, first.unsqueeze(2), True)
+    return torch.stack([x1, x2], 2).reshape(2 * P * Q, n)
+
+
+def interaction_reference(values, perm, pairs, group: int, dtype=np.float32):
+    """numpy float64 restatement of vb200_interaction_values for one message: ``values`` [2 + P (n - 1) + 2 P Q] (v(empty), v(all),
+    the chains, then x1, x2 per permutation and pair), ``perm`` [P, n], ``pairs`` [Q, 2].  Returns (interaction, stderr) [Q], each
+    step the header's, in its order, rounded to ``dtype`` (float32: the device's outputs; float64: before that rounding)."""
+    v = np.asarray(values, dtype=np.float32).astype(np.float64)
+    perm = np.asarray(perm, dtype=np.int64)
+    pairs = np.asarray(pairs, dtype=np.int64).reshape(-1, 2)
+    P, n = perm.shape
+    Q = len(pairs)
+    c = np.empty((P, n + 1), dtype=np.float64)
+    c[:, 0], c[:, n] = v[0], v[1]
+    c[:, 1:n] = v[2:2 + P * (n - 1)].reshape(P, n - 1)
+    x = v[2 + P * (n - 1):].reshape(P, Q, 2)
+    rank = _ranks(torch.from_numpy(perm)).numpy()
+    r = np.minimum(rank[:, pairs[:, 0]], rank[:, pairs[:, 1]])                  # [P, Q]
+    rows = np.arange(P)[:, None]
+    d = ((x[:, :, 1] - c[rows, r + 1]) - x[:, :, 0]) + c[rows, r]             # elementwise: one rounding per step
+    s = np.zeros(Q)
+    for p in range(P):
+        s = s + d[p]
+    inter = s / P
+    G = P // group
+    ss = np.zeros(Q)
+    for k in range(G):
+        m = np.zeros(Q)
+        for i in range(group):
+            m = m + d[k * group + i]
+        t = m / group - inter
+        ss = ss + t * t
+    se = np.sqrt(ss / (G - 1) / G) if G >= 2 else np.full(Q, np.nan)
+    return inter.astype(dtype), se.astype(dtype)
+
+
 def attention_list(kinds, layout_entry, entries):
     """The reference's attn_data_list from the maps of the selected entries: ``kinds`` / ``layout_entry`` are the full entry list's
     kinds and each entry's index in ``entries`` (-1: not selected) as ``attention_selection`` returns them.  One position per layer in
@@ -1526,6 +1625,60 @@ class VILBertForVLTasks(object):
         for r, p, d in zip(res, perms, descs):
             o, n = d.out_offset, d.n_units
             out.append(dict(answer=r["answer"], prob=r["prob"], empty_prob=float(r["prob_d"][0]), units=r["units"],
+                            phi=phi[o:o + n], stderr=se[o:o + n], perm=p, samples=r["samples"]))
+        return out
+
+    @torch.no_grad()
+    def shapley_interactions(self, question, segment_ids, task_tokens, box_features, boxes, image_wh, n_tokens, n_boxes, messages,
+                             pairs, units=None, permutations: int = 8, seed: int = 0, antithetic: bool = True, mask_token: int = 103,
+                             max_tokens: int = 0, max_boxes: int = 0, slot: int = 0):
+        """Shapley-Taylor interaction indices of order 2 for chosen pairs of each message's units (Sundararajan et al. 2020): for a
+        pair {a, b}, the mean over permutations of v(S + {a, b}) - v(S + {a}) - v(S + {b}) + v(S), S the units before the first
+        of a and b -- positive when the answer needs both units, negative when either is enough.  ``messages``, ``units``,
+        ``permutations``, ``seed`` and ``antithetic`` as for ``shapley``, whose permutations and chains this call draws and
+        evaluates in the same way, so its ``phi`` and ``stderr`` are ``shapley``'s bits.  ``pairs``: per message ``"cross"`` (every
+        word unit with every box unit, ``cross_pairs``) or a list of ``(a, b)`` unit indices.  Beyond the chains each permutation
+        and pair adds the two coalitions of ``interaction_coalitions``; everything runs in one ``coalition_ablation`` pass (split at
+        the engine's 1024 samples per call), then vb200_shapley_values and vb200_interaction_values on the device.
+        Cost per message: (2 + P (n - 1) + 2 P Q) x its samples per variant (1, 2 for NLVR2, K for retrieval) forward samples,
+        plus the full input once more for every engine call past the first.
+        Returns per message ``answer``, ``prob`` (v(all)), ``empty_prob`` (v(empty)), ``units``, ``pairs`` (int64 [Q, 2]),
+        ``interaction`` and ``interaction_stderr`` (float32 CPU tensors [Q]), ``phi`` and ``stderr`` ([n_units]), ``perm`` and
+        ``samples`` (the forward samples run)."""
+        nt, nb = PackedRegionBatch.lengths("shapley_interactions", n_tokens, n_boxes)
+        msgs = coalition_messages(messages, len(nt))
+        units = [None] * len(msgs) if units is None else list(units)
+        if len(units) != len(msgs):
+            raise ValueError(f"shapley_interactions: units need one entry per message ({len(msgs)})")
+        units = [coalition_units(u, nt[ib], sum(nb[ib:ib + k]), i) for i, (u, (_, ib, k, _)) in enumerate(zip(units, msgs))]
+        prs = interaction_pairs(pairs, units)
+        gen = torch.Generator().manual_seed(int(seed))
+        perms = [shapley_permutations(len(u), permutations, gen, antithetic) for u in units]
+        coal = [torch.cat([shapley_chain(p), interaction_coalitions(p, q)]) for p, q in zip(perms, prs)]
+        res = self._coalition_run("shapley_interactions", question, segment_ids, task_tokens, box_features, boxes, image_wh, nt, nb,
+                                  msgs, units, coal, mask_token, max_tokens, max_boxes, slot, False)
+        device = self._engine_device()
+        g = 2 if antithetic else 1
+        values, sdesc, idesc, at_v, at_p, at_o, at_q = [], [], [], 0, 0, 0, 0
+        for r, p, q in zip(res, perms, prs):
+            P, n = p.shape
+            values += r["prob_d"][:1] + [r["prob"]] + r["prob_d"][1:]
+            sdesc.append(L.ShapleyMessage(n, P, g, at_p, at_v, at_o))
+            idesc.append(L.InteractionMessage(n, P, g, len(q), at_p, at_v, at_q, q.ctypes.data))
+            at_v, at_p, at_o, at_q = at_v + 2 + P * (n - 1) + 2 * P * len(q), at_p + P * n, at_o + n, at_q + len(q)
+        vals = torch.tensor(values, dtype=torch.float32, device=device)
+        perm_d = torch.cat([p.reshape(-1) for p in perms]).to(device=device, dtype=torch.int32)
+        phi, se = (torch.empty(at_o, dtype=torch.float32, device=device) for _ in range(2))
+        inter, ise = (torch.empty(at_q, dtype=torch.float32, device=device) for _ in range(2))
+        sarr, iarr = (L.ShapleyMessage * len(sdesc))(*sdesc), (L.InteractionMessage * len(idesc))(*idesc)
+        self._call("vb200_shapley_values", sarr, len(sdesc), perm_d.data_ptr(), vals.data_ptr(), phi.data_ptr(), se.data_ptr())
+        self._call("vb200_interaction_values", iarr, len(idesc), perm_d.data_ptr(), vals.data_ptr(), inter.data_ptr(), ise.data_ptr())
+        phi, se, inter, ise = phi.cpu(), se.cpu(), inter.cpu(), ise.cpu()
+        out = []
+        for r, p, q, sd, idd in zip(res, perms, prs, sdesc, idesc):
+            o, n, oq, k = sd.out_offset, sd.n_units, idd.out_offset, idd.n_pairs
+            out.append(dict(answer=r["answer"], prob=r["prob"], empty_prob=float(r["prob_d"][0]), units=r["units"],
+                            pairs=torch.from_numpy(q.astype(np.int64)), interaction=inter[oq:oq + k], interaction_stderr=ise[oq:oq + k],
                             phi=phi[o:o + n], stderr=se[o:o + n], perm=p, samples=r["samples"]))
         return out
 

@@ -612,14 +612,37 @@ def custom_shapley_packed(requests, max_boxes: int = 100, *, units=None, permuta
     or `(positions, boxes)` groups applied to every request.  Returns per request `{"answer": <custom_prediction_packed's answer>,
     "shapley": <shapley's dict>}` -- with `box_pixels`, per unit the [x1, y1, x2, y2] of its boxes from `infos` -- or the exception of
     a request that fails validation.  Grounding requests get a ValueError: their answer is a box, which a coalition would renumber."""
+    return _coalition_packed(requests, max_boxes, "custom_shapley_packed", "shapley",
+                             lambda args, m, mask, kw: model.shapley(*args, m, units=None if units is None else [units] * len(m),
+                                                                     permutations=permutations, seed=seed, antithetic=antithetic,
+                                                                     mask_token=mask, **kw))
+
+
+def custom_interactions_packed(requests, max_boxes: int = 100, *, pairs="cross", units=None, permutations: int = 8, seed: int = 0,
+                               antithetic: bool = True):
+    """Which words work together with which boxes for each answer: `custom_prediction_packed` (decode="device") for
+    `custom_prediction` argument tuples `(query, task, features, infos, task_id)`, plus `model.shapley_interactions` over the images
+    the answer reads, as `custom_ablation_packed` chooses them.  `pairs`: "cross" (every word unit with every box unit) or a list of
+    `(a, b)` unit indices, applied to every request; `units` as for `custom_shapley_packed`.  Returns per request
+    `{"answer": <custom_prediction_packed's answer>, "interactions": <shapley_interactions' dict>}` -- with `box_pixels`, per unit
+    the [x1, y1, x2, y2] of its boxes from `infos` -- or the exception of a request that fails validation.  Grounding requests get
+    the ValueError `custom_shapley_packed` gives them."""
+    return _coalition_packed(requests, max_boxes, "custom_interactions_packed", "interactions",
+                             lambda args, m, mask, kw: model.shapley_interactions(
+                                 *args, m, [pairs] * len(m), units=None if units is None else [units] * len(m),
+                                 permutations=permutations, seed=seed, antithetic=antithetic, mask_token=mask, **kw))
+
+
+def _coalition_packed(requests, max_boxes, name, key, explain):
+    """What the coalition explainers share: `_explain_packed` with every request but grounding as a message, `explain(args, msgs,
+    mask, kw)` the model call, and per answered request `{"answer": ..., key: <its dict with box_pixels per unit>}`."""
     answers, p, msgs, sh = _explain_packed(
         requests, max_boxes,
         lambda spans: {i: m[:4] for i, m in ablation_messages(requests, spans).items() if requests[i][4] not in GROUNDING_TASKS},
-        lambda args, m, mask, kw: model.shapley(*args, m, units=None if units is None else [units] * len(m), permutations=permutations,
-                                                seed=seed, antithetic=antithetic, mask_token=mask, **kw))
+        explain)
     for i in p["spans"]:
         if i not in msgs:
-            answers[i] = ValueError("custom_shapley_packed: a grounding answer is a box, which a coalition would renumber")
+            answers[i] = ValueError(f"{name}: a grounding answer is a box, which a coalition would renumber")
     for i, s in zip(msgs, sh):
         infos, lo = requests[i][3], p["spans"][i][0]
         first = list(accumulate([p["n_boxes"][lo + k] for k in range(len(infos))], initial=0))     # each image's first box
@@ -628,7 +651,7 @@ def custom_shapley_packed(requests, max_boxes: int = 100, *, units=None, permuta
             k = max(k for k in range(len(infos)) if first[k] <= b)
             return _pixel_box(infos[k], b - first[k] + 1)
         s["box_pixels"] = [[pixels(b) for b in bs] for _, bs in s["units"]]
-        answers[i] = {"answer": answers[i], "shapley": s}
+        answers[i] = {"answer": answers[i], key: s}
     return answers
 
 
