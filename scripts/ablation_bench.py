@@ -22,6 +22,8 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+import harness  # noqa: E402
+
 TIN, BOXES = 37, 100
 
 
@@ -31,8 +33,7 @@ def messages(n, seed, F, vocab):
     g = torch.Generator().manual_seed(seed)
     out = []
     for _ in range(n):
-        xy = torch.rand(BOXES, 2, generator=g) * torch.tensor([448.0, 336.0])
-        bx = torch.cat([xy, torch.minimum(xy + 40 + 120 * torch.rand(BOXES, 2, generator=g), torch.tensor([640.0, 480.0]))], 1)
+        bx = harness.pixel_boxes(g, BOXES)
         out.append((torch.randint(1000, vocab, (TIN,), generator=g), torch.relu(torch.randn(BOXES, F, generator=g)) * 1.5, bx,
                     (640.0, 480.0)))
     return out
@@ -48,14 +49,10 @@ def main():
 
     import torch
     import vilbert_b200 as vb
-    from vilbert_b200 import synthetic as S
-    from bench import ClockSampler
 
-    if not torch.cuda.is_available():
-        raise SystemExit("ablation_bench.py needs an H100: there is no CPU path")
+    harness.require_gpu("ablation_bench.py")
     cfg = vb.BertConfig(task_specific_tokens=True, visualization=True)
-    model = vb.VILBertForVLTasks.from_pretrained(S.synthetic_state_dict(cfg, seed=42), config=cfg, num_labels=3129,
-                                                 compute_dtype="bf16").eval().cuda(0)
+    model = harness.synthetic_model(cfg, "bf16")
     dev = torch.device("cuda", 0)
     mask_token = 103
     tokens, boxes_range = (1, TIN - 1), (0, BOXES)
@@ -107,49 +104,22 @@ def main():
         p = probs.view(B, per_msg, -1).gather(2, ans.view(B, 1, 1).expand(B, per_msg, 1)).cpu()
         return logits, p, vq.numel() * 8 + vf.numel() * 4 + vb_.numel() * 4
 
-    def timed(fn, x, steps):
-        for _ in range(args.warmup):
-            fn(x)
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        torch.cuda.synchronize()
-        e0.record()
-        for _ in range(steps):
-            fn(x)
-        e1.record()
-        e1.synchronize()
-        return e0.elapsed_time(e1) / steps
-
     results = {}
-    clock = ClockSampler(0)
-    clock.start()
-    for n_msg in (1, 8):
-        x = inputs(messages(n_msg, args.seed + n_msg, cfg.v_feature_size, cfg.vocab_size))
-        a_logits, _ = device_call(x)
-        b_logits, _, built = torch_call(x)
-        torch.cuda.synchronize()
-        ms = {"device": [], "torch": []}
-        for _ in range(args.rounds):
-            ms["device"].append(timed(device_call, x, args.steps))
-            ms["torch"].append(timed(torch_call, x, args.steps))
-        results[f"{n_msg}_messages"] = {
-            "variants": n_msg * per_msg, "engine_calls": -(-n_msg * per_msg // 1024),
-            "device_ms_per_message": statistics.median(ms["device"]) / n_msg,
-            "torch_ms_per_message": statistics.median(ms["torch"]) / n_msg,
-            "windows_ms": ms, "torch_bytes_built_per_message": built // n_msg,
-            "logits_bitwise_equal": bool(torch.equal(a_logits, b_logits))}
-    clock.stop_flag = True
-    clock.join()
-
-    try:
-        import pynvml as nv_
-        nv_.nvmlInit()
-        h = nv_.nvmlDeviceGetHandleByIndex(0)
-        name = nv_.nvmlDeviceGetName(h)
-        card = {"name": name.decode() if isinstance(name, bytes) else name,
-                "power_limit_w": nv_.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0}
-    except Exception as e:          # NVML missing: report it
-        card = {"name": torch.cuda.get_device_name(0), "nvml_error": repr(e)}
-    card.update(clock.result())
+    with harness.sampled_clock() as clock:
+        for n_msg in (1, 8):
+            x = inputs(messages(n_msg, args.seed + n_msg, cfg.v_feature_size, cfg.vocab_size))
+            a_logits, _ = device_call(x)
+            b_logits, _, built = torch_call(x)
+            torch.cuda.synchronize()
+            ms = harness.alternate({"device": lambda: device_call(x), "torch": lambda: torch_call(x)}, args.rounds, args.steps,
+                                   args.warmup)
+            results[f"{n_msg}_messages"] = {
+                "variants": n_msg * per_msg, "engine_calls": -(-n_msg * per_msg // 1024),
+                "device_ms_per_message": statistics.median(ms["device"]) / n_msg,
+                "torch_ms_per_message": statistics.median(ms["torch"]) / n_msg,
+                "windows_ms": ms, "torch_bytes_built_per_message": built // n_msg,
+                "logits_bitwise_equal": bool(torch.equal(a_logits, b_logits))}
+    card = harness.card(clock)
     print(json.dumps({"workload": f"full synthetic model, bf16, VQA, messages of {TIN} tokens and {BOXES} boxes, positions "
                                   f"{tokens[0]}..{tokens[1] - 1} masked and every box dropped ({per_msg} variants per message), seed {args.seed}",
                       **results, "steps": args.steps, "rounds": args.rounds, "card": card}), flush=True)

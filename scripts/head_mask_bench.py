@@ -21,6 +21,8 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+import harness  # noqa: E402
+
 B, TIN, V = 64, 30, 36
 
 
@@ -35,15 +37,11 @@ def main():
 
     import torch
     import vilbert_b200 as vb
-    from vilbert_b200 import synthetic as S
     from vilbert_b200.model import head_mask_shape
-    from bench import ClockSampler
 
-    if not torch.cuda.is_available():
-        raise SystemExit("head_mask_bench.py needs an H100: there is no CPU path")
+    harness.require_gpu("head_mask_bench.py")
     cfg = vb.BertConfig(task_specific_tokens=True)
-    model = vb.VILBertForVLTasks.from_pretrained(S.synthetic_state_dict(cfg, seed=42), config=cfg, num_labels=3129,
-                                                 compute_dtype="bf16").eval().cuda(0)
+    model = harness.synthetic_model(cfg, "bf16")
     dev = torch.device("cuda", 0)
     g = torch.Generator().manual_seed(args.seed)
     q = torch.randint(1000, cfg.vocab_size, (B * TIN,), generator=g).to(dev)
@@ -55,29 +53,11 @@ def main():
     paths = {"ungated": lambda: model.forward_packed(*x, select=vb.OUT_VIL_PREDICTION)[0],
              "gated_ones": lambda: model.forward_packed(*x, select=vb.OUT_VIL_PREDICTION, head_mask=ones)[0]}
 
-    def timed(fn, steps):
-        for _ in range(args.warmup):
-            fn()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        torch.cuda.synchronize()
-        e0.record()
-        for _ in range(steps):
-            fn()
-        e1.record()
-        e1.synchronize()
-        return e0.elapsed_time(e1) / steps
-
     out = {k: fn().clone() for k, fn in paths.items()}
     torch.cuda.synchronize()
     diff = float((out["ungated"] - out["gated_ones"]).abs().max())
-    ms = {k: [] for k in paths}
-    clock = ClockSampler(0)
-    clock.start()
-    for _ in range(args.rounds):
-        for k, fn in paths.items():
-            ms[k].append(timed(fn, args.steps))
-    clock.stop_flag = True
-    clock.join()
+    with harness.sampled_clock() as clock:
+        ms = harness.alternate(paths, args.rounds, args.steps, args.warmup)
 
     # device time per call in a separate profiled pass: the kernels' summed time and the copies', per path
     from torch.profiler import ProfilerActivity, profile
@@ -96,16 +76,7 @@ def main():
                      "copy_us_per_call": sum(e.device_time for e in copy) / args.profile_calls,
                      "copies_per_call": len(copy) / args.profile_calls}
 
-    try:
-        import pynvml as nv_
-        nv_.nvmlInit()
-        h = nv_.nvmlDeviceGetHandleByIndex(0)
-        name = nv_.nvmlDeviceGetName(h)
-        card = {"name": name.decode() if isinstance(name, bytes) else name,
-                "power_limit_w": nv_.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0}
-    except Exception as e:          # NVML missing: report it
-        card = {"name": torch.cuda.get_device_name(0), "nvml_error": repr(e)}
-    card.update(clock.result())
+    card = harness.card(clock)
     print(json.dumps({"workload": f"full synthetic model, bf16, packed VQA forward, batch {B}, {TIN} tokens, {V} regions, seed {args.seed}",
                       **{f"{k}_ms": statistics.median(v) for k, v in ms.items()}, "windows_ms": ms, "device": device, "max_abs_diff": diff,
                       "steps": args.steps, "rounds": args.rounds, "card": card}), flush=True)

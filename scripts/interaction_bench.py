@@ -24,6 +24,8 @@ import time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+import harness  # noqa: E402
+
 TIN, BOXES, P = 37, 100, 8
 WORDS, BOX_UNITS = 8, 16
 
@@ -42,18 +44,13 @@ def main():
     import vilbert_b200 as vb
     from vilbert_b200 import _lib as L
     from vilbert_b200 import model as M
-    from vilbert_b200 import synthetic as S
-    from bench import ClockSampler
 
-    if not torch.cuda.is_available():
-        raise SystemExit("interaction_bench.py needs an H100: there is no CPU path")
+    harness.require_gpu("interaction_bench.py")
     cfg = vb.BertConfig(task_specific_tokens=True)
-    model = vb.VILBertForVLTasks.from_pretrained(S.synthetic_state_dict(cfg, seed=42), config=cfg, num_labels=3129,
-                                                 compute_dtype="bf16").eval().cuda(0)
+    model = harness.synthetic_model(cfg, "bf16")
     dev = torch.device("cuda", 0)
     g = torch.Generator().manual_seed(args.seed)
-    xy = torch.rand(BOXES, 2, generator=g) * torch.tensor([448.0, 336.0])
-    bx = torch.cat([xy, torch.minimum(xy + 40 + 120 * torch.rand(BOXES, 2, generator=g), torch.tensor([640.0, 480.0]))], 1)
+    bx = harness.pixel_boxes(g, BOXES)
     feats = torch.relu(torch.randn(BOXES, cfg.v_feature_size, generator=g)) * 1.5
     q = torch.randint(1000, cfg.vocab_size, (TIN,), generator=g)
     x = (q.to(dev), torch.zeros(TIN, dtype=torch.long, device=dev), torch.tensor([[1]], device=dev), feats.to(dev), bx.to(dev),
@@ -72,29 +69,12 @@ def main():
     def interactions():
         return model.shapley_interactions(*x, msgs, [pairs], permutations=P, seed=args.seed)
 
-    def timed(fn):
-        for _ in range(args.warmup):
-            fn()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        torch.cuda.synchronize()
-        e0.record()
-        for _ in range(args.steps):
-            fn()
-        e1.record()
-        e1.synchronize()
-        return e0.elapsed_time(e1) / args.steps / len(msgs)
-
     a, b = shapley()[0], interactions()[0]
     torch.cuda.synchronize()
     assert torch.equal(a["phi"], b["phi"]), "shapley_interactions' phi differs from shapley's"
-    ms = {"shapley": [], "shapley_interactions": []}
-    clock = ClockSampler(0)
-    clock.start()
-    for _ in range(args.rounds):
-        ms["shapley"].append(timed(shapley))
-        ms["shapley_interactions"].append(timed(interactions))
-    clock.stop_flag = True
-    clock.join()
+    with harness.sampled_clock() as clock:
+        ms = harness.alternate({"shapley": shapley, "shapley_interactions": interactions}, args.rounds, args.steps, args.warmup)
+    ms = {k: [t / len(msgs) for t in v] for k, v in ms.items()}
 
     # the estimator alone: the call's permutations and pairs, values of the call's size (its time does not depend on them)
     perm = b["perm"].numpy()
@@ -108,16 +88,7 @@ def main():
     def kernel():
         model._call("vb200_interaction_values", arr, 1, perm_d.data_ptr(), vals_d.data_ptr(), inter.data_ptr(), se.data_ptr())
 
-    for _ in range(10):
-        kernel()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    torch.cuda.synchronize()
-    e0.record()
-    for _ in range(args.kernel_iters):
-        kernel()
-    e1.record()
-    e1.synchronize()
-    kernel_us = e0.elapsed_time(e1) / args.kernel_iters * 1000.0
+    kernel_us = harness.timed(kernel, args.kernel_iters, 10) * 1000.0
     want = M.interaction_reference(vals, perm, pr, 2)
     assert np.array_equal(inter.cpu().numpy(), want[0]) and np.array_equal(se.cpu().numpy(), want[1])
     t0 = time.perf_counter()
@@ -126,16 +97,7 @@ def main():
         M.interaction_reference(vals, perm, pr, 2)
     numpy_us = (time.perf_counter() - t0) / reps * 1e6
 
-    try:
-        import pynvml as nv_
-        nv_.nvmlInit()
-        h = nv_.nvmlDeviceGetHandleByIndex(0)
-        name = nv_.nvmlDeviceGetName(h)
-        card = {"name": name.decode() if isinstance(name, bytes) else name,
-                "power_limit_w": nv_.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0}
-    except Exception as e:          # NVML missing: report it
-        card = {"name": torch.cuda.get_device_name(0), "nvml_error": repr(e)}
-    card.update(clock.result())
+    card = harness.card(clock)
     chain = 2 + P * (n - 1)
     print(json.dumps({"workload": f"full synthetic model, bf16, one VQA message, {TIN} tokens and {BOXES} boxes, default units (n = {n}), "
                                   f"P = {P} antithetic, Q = {Q} pairs ({WORDS} word units x {BOX_UNITS} box units), seed {args.seed}",

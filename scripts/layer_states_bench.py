@@ -24,6 +24,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "scripts"))
 
+import harness  # noqa: E402
+
 T_CAP, BOX_CAP = 37, 100
 
 
@@ -39,15 +41,11 @@ def main():
 
     import torch
     import vilbert_b200 as vb
-    from vilbert_b200 import synthetic as S
-    from bench import ClockSampler
     from packed_attention_bench import detector_rows
 
-    if not torch.cuda.is_available():
-        raise SystemExit("layer_states_bench.py needs an H100: there is no CPU path")
+    harness.require_gpu("layer_states_bench.py")
     cfg = vb.BertConfig(task_specific_tokens=True, visualization=True)
-    model = vb.VILBertForVLTasks.from_pretrained(S.synthetic_state_dict(cfg, seed=42), config=cfg, num_labels=3129,
-                                                 compute_dtype=args.dtype).eval().cuda(0)
+    model = harness.synthetic_model(cfg, args.dtype)
     rows = detector_rows(args.batch, args.seed, cfg.v_feature_size, cfg.vocab_size)
     B = len(rows)
     tin, nb = [len(r[0]) for r in rows], [r[1].shape[0] for r in rows]
@@ -85,25 +83,13 @@ def main():
 
     def timed(name):
         select(name)
-        for _ in range(args.warmup):
-            call(name)
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        torch.cuda.synchronize()
-        e0.record()
-        for _ in range(args.steps):
-            call(name)
-        e1.record()
-        e1.synchronize()
-        return e0.elapsed_time(e1) / args.steps
+        return harness.timed(lambda: call(name), args.steps, args.warmup)
 
-    clock = ClockSampler(0)
-    clock.start()
-    ms = {k: [] for k in variants}
-    for _ in range(args.rounds):
-        for k in variants:
-            ms[k].append(timed(k))
-    clock.stop_flag = True
-    clock.join()
+    with harness.sampled_clock() as clock:
+        ms = {k: [] for k in variants}
+        for _ in range(args.rounds):
+            for k in variants:
+                ms[k].append(timed(k))
 
     from torch.profiler import ProfilerActivity, profile
 
@@ -125,16 +111,7 @@ def main():
         return t / n / 1e3
     kernel_ms = {k: state_kernel_ms(k) for k in variants}
 
-    try:
-        import pynvml as nv_
-        nv_.nvmlInit()
-        h = nv_.nvmlDeviceGetHandleByIndex(0)
-        name = nv_.nvmlDeviceGetName(h)
-        card = {"name": name.decode() if isinstance(name, bytes) else name,
-                "power_limit_w": nv_.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0}
-    except Exception as e:          # NVML missing: report it
-        card = {"name": torch.cuda.get_device_name(0), "nvml_error": repr(e)}
-    card.update(clock.result())
+    card = harness.card(clock)
     result = {k: {"ms_per_call": statistics.median(v), "windows_ms": [min(v), max(v)], "state_floats_per_call": floats[k],
                   "device_ms_per_call_state_kernels": kernel_ms[k]} for k, v in ms.items()}
     print(json.dumps({"workload": f"batch {B} VQA rows, U{{5..20}} tokens, U{{10..100}} boxes, seed {args.seed}, {args.dtype}, "

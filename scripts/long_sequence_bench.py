@@ -20,6 +20,8 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+import harness  # noqa: E402
+
 
 def main():
     ap = argparse.ArgumentParser()
@@ -30,7 +32,6 @@ def main():
     import torch
     import vilbert_b200 as vb
     from vilbert_b200 import _lib as L
-    from bench import ClockSampler
     from oracle import vilbert_ref as R
 
     lib = L.load()
@@ -47,60 +48,49 @@ def main():
         torch.cuda.synchronize()
         return a.elapsed_time(b) / args.iters
 
-    clock = ClockSampler(0)
-    clock.start()
-    ops = []
-    B = 64
-    for d, heads in ((64, 12), (128, 8)):
-        H = heads * d
-        for L_ in (31, 36, 101, 256, 512, 1024):
-            qkv = torch.randn(B * L_, 3 * H, device="cuda").half()
-            mask = torch.zeros(B * L_, device="cuda")
-            ctx = torch.empty(B * L_, H, device="cuda").half()
-            ct, ci = torch.empty_like(ctx), torch.empty_like(ctx)
-            row = {"D": d, "heads": heads, "B": B, "L": L_, "self_flops": 4.0 * B * heads * L_ * L_ * d,
-                   "co_flops": 8.0 * B * heads * L_ * L_ * d}
+    with harness.sampled_clock() as clock:
+        ops = []
+        B = 64
+        for d, heads in ((64, 12), (128, 8)):
+            H = heads * d
+            for L_ in (31, 36, 101, 256, 512, 1024):
+                qkv = torch.randn(B * L_, 3 * H, device="cuda").half()
+                mask = torch.zeros(B * L_, device="cuda")
+                ctx = torch.empty(B * L_, H, device="cuda").half()
+                ct, ci = torch.empty_like(ctx), torch.empty_like(ctx)
+                row = {"D": d, "heads": heads, "B": B, "L": L_, "self_flops": 4.0 * B * heads * L_ * L_ * d,
+                       "co_flops": 8.0 * B * heads * L_ * L_ * d}
 
-            def self_(name, offs=()):
-                return lambda: L.check(getattr(lib, name)(qkv.data_ptr(), 3 * H, H, mask.data_ptr(), ctx.data_ptr(), H, B, L_, heads,
-                                                          d, 1, *offs, st()))
+                def self_(name, offs=()):
+                    return lambda: L.check(getattr(lib, name)(qkv.data_ptr(), 3 * H, H, mask.data_ptr(), ctx.data_ptr(), H, B, L_,
+                                                              heads, d, 1, *offs, st()))
 
-            def co_(name, offs=()):
-                return lambda: L.check(getattr(lib, name)(qkv.data_ptr(), 3 * H, qkv.data_ptr(), 3 * H, H, mask.data_ptr(),
-                                                          mask.data_ptr(), ct.data_ptr(), H, ci.data_ptr(), H, B, L_, L_, heads, d, 1,
-                                                          *offs, st()))
-            row["stream_self_ms"] = timed(self_("vb200_self_attention_stream", (None,)))
-            row["stream_co_ms"] = timed(co_("vb200_co_attention_stream", (None, None)))
-            if L_ <= 256:
-                row["staged_self_ms"] = timed(self_("vb200_self_attention"))
-                row["staged_co_ms"] = timed(co_("vb200_co_attention"))
-            ops.append(row)
-            del qkv, mask, ctx, ct, ci
+                def co_(name, offs=()):
+                    return lambda: L.check(getattr(lib, name)(qkv.data_ptr(), 3 * H, qkv.data_ptr(), 3 * H, H, mask.data_ptr(),
+                                                              mask.data_ptr(), ct.data_ptr(), H, ci.data_ptr(), H, B, L_, L_, heads,
+                                                              d, 1, *offs, st()))
+                row["stream_self_ms"] = timed(self_("vb200_self_attention_stream", (None,)))
+                row["stream_co_ms"] = timed(co_("vb200_co_attention_stream", (None, None)))
+                if L_ <= 256:
+                    row["staged_self_ms"] = timed(self_("vb200_self_attention"))
+                    row["staged_co_ms"] = timed(co_("vb200_co_attention"))
+                ops.append(row)
+                del qkv, mask, ctx, ct, ci
 
-    oracle = R.build(seed=42)
-    cfg = vb.BertConfig.from_dict(oracle.config.to_dict())
-    model = vb.VILBertForVLTasks.from_pretrained(oracle.state_dict(), config=cfg, num_labels=oracle.num_labels, compute_dtype="bf16",
-                                                 max_rows_per_sample=1024).eval().cuda(0)
-    del oracle
-    shapes = []
-    for tin, v in ((30, 36), (511, 36), (30, 1000), (511, 1000)):
-        inp = [t.cuda() for t in R.make_inputs(args.batch, tin, v, seed=1, full_masks=True)]
-        ms = timed(lambda: model(*inp))
-        n, fl = model.plan_info(args.batch, tin, v)
-        shapes.append({"Tin": tin, "V": v, "batch": args.batch, "ms": ms, "pairs_per_s": args.batch / ms * 1e3, "launches": n,
-                       "flops": fl})
-    model.close()
-    clock.stop_flag = True
-    clock.join()
-    try:
-        import pynvml as nv
-        nv.nvmlInit()
-        h = nv.nvmlDeviceGetHandleByIndex(0)
-        name = nv.nvmlDeviceGetName(h)
-        card = {"name": name.decode() if isinstance(name, bytes) else name, "power_limit_w": nv.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0}
-    except Exception as e:      # noqa: BLE001
-        card = {"name": torch.cuda.get_device_name(0), "nvml_error": repr(e)}
-    card.update(clock.result())
+        oracle = R.build(seed=42)
+        cfg = vb.BertConfig.from_dict(oracle.config.to_dict())
+        model = vb.VILBertForVLTasks.from_pretrained(oracle.state_dict(), config=cfg, num_labels=oracle.num_labels,
+                                                     compute_dtype="bf16", max_rows_per_sample=1024).eval().cuda(0)
+        del oracle
+        shapes = []
+        for tin, v in ((30, 36), (511, 36), (30, 1000), (511, 1000)):
+            inp = [t.cuda() for t in R.make_inputs(args.batch, tin, v, seed=1, full_masks=True)]
+            ms = timed(lambda: model(*inp))
+            n, fl = model.plan_info(args.batch, tin, v)
+            shapes.append({"Tin": tin, "V": v, "batch": args.batch, "ms": ms, "pairs_per_s": args.batch / ms * 1e3, "launches": n,
+                           "flops": fl})
+        model.close()
+    card = harness.card(clock)
     print(json.dumps({"card": card, "ops": ops, "model": shapes}))
 
 

@@ -23,6 +23,8 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+import harness  # noqa: E402
+
 TIN, BOXES, CAP = 37, 100, 1024
 NLVR2, RET, GRD = 3, 5, 6
 FAMILIES = [("grounding", GRD, 1, True), ("nlvr2", NLVR2, 2, True), ("retrieval_k4", RET, 4, True), ("retrieval_k10", RET, 10, False)]
@@ -38,14 +40,10 @@ def main():
 
     import torch
     import vilbert_b200 as vb
-    from vilbert_b200 import synthetic as S
-    from bench import ClockSampler
 
-    if not torch.cuda.is_available():
-        raise SystemExit("message_ablation_bench.py needs an H100: there is no CPU path")
+    harness.require_gpu("message_ablation_bench.py")
     cfg = vb.BertConfig(task_specific_tokens=True, visualization=True)
-    model = vb.VILBertForVLTasks.from_pretrained(S.synthetic_state_dict(cfg, seed=42), config=cfg, num_labels=3129,
-                                                 compute_dtype="bf16").eval().cuda(0)
+    model = harness.synthetic_model(cfg, "bf16")
     dev = torch.device("cuda", 0)
     mask_token, tokens = 103, (1, TIN - 1)
     pooled = vb.OUT_VIL_PREDICTION | vb.OUT_VIL_PREDICTION_GQA | vb.OUT_VIL_LOGIT | vb.OUT_VIL_BINARY_PREDICTION | vb.OUT_VIL_TRI_PREDICTION
@@ -53,8 +51,7 @@ def main():
     def message(K, seed):
         """K images sharing one question: token ids [TIN], box features [K * BOXES, F], pixel boxes, image sizes."""
         g = torch.Generator().manual_seed(seed)
-        xy = torch.rand(K * BOXES, 2, generator=g) * torch.tensor([448.0, 336.0])
-        bx = torch.cat([xy, torch.minimum(xy + 40 + 120 * torch.rand(K * BOXES, 2, generator=g), torch.tensor([640.0, 480.0]))], 1)
+        bx = harness.pixel_boxes(g, K * BOXES)
         q = torch.randint(1000, cfg.vocab_size, (TIN,), generator=g)
         f = torch.relu(torch.randn(K * BOXES, cfg.v_feature_size, generator=g)) * 1.5
         return (q.repeat(K).to(dev), torch.zeros(K * TIN, dtype=torch.long, device=dev), torch.ones(K, 1, dtype=torch.long, device=dev),
@@ -116,54 +113,30 @@ def main():
         p = torch.stack([pr[0] for pr in probs]).cpu()
         return torch.cat(segs), p, built, sum(len(v) for v in var)
 
-    def timed(fn, steps):
-        for _ in range(args.warmup):
-            fn()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        torch.cuda.synchronize()
-        e0.record()
-        for _ in range(steps):
-            fn()
-        e1.record()
-        e1.synchronize()
-        return e0.elapsed_time(e1) / steps
-
     results = {}
-    clock = ClockSampler(0)
-    clock.start()
-    for name, fam, K, time_torch in FAMILIES:
-        x = message(K, args.seed + K)
-        a, _ = device_call(x, fam, K)
-        b, _, built, torch_samples = torch_call(x, fam, K)
-        torch.cuda.synchronize()
-        nt, nb = x[6], x[7]
-        recs, _, _ = model._message_layout(nt, nb, [vb.model.message_pieces([(fam, 0, K, None, tokens, None)], nt, nb)[0][0]])
-        r = {"device_samples": sum(rc[3] for rc in recs), "torch_samples": torch_samples,
-             "max_abs_diff": float((a - b).abs().max()) if a.shape == b.shape else None}
-        del b
-        ms = {"device": [], "torch": []}
-        for _ in range(args.rounds):
-            ms["device"].append(timed(lambda: device_call(x, fam, K), args.steps))
+    with harness.sampled_clock() as clock:
+        for name, fam, K, time_torch in FAMILIES:
+            x = message(K, args.seed + K)
+            a, _ = device_call(x, fam, K)
+            b, _, built, torch_samples = torch_call(x, fam, K)
+            torch.cuda.synchronize()
+            nt, nb = x[6], x[7]
+            recs, _, _ = model._message_layout(nt, nb, [vb.model.message_pieces([(fam, 0, K, None, tokens, None)], nt, nb)[0][0]])
+            r = {"device_samples": sum(rc[3] for rc in recs), "torch_samples": torch_samples,
+                 "max_abs_diff": float((a - b).abs().max()) if a.shape == b.shape else None}
+            del b
+            paths = {"device": lambda: device_call(x, fam, K)}
             if time_torch:
-                ms["torch"].append(timed(lambda: torch_call(x, fam, K), args.steps))
-        r["device_ms_per_message"] = statistics.median(ms["device"])
-        r["torch_ms_per_message"] = statistics.median(ms["torch"]) if time_torch else None
-        r["torch_bytes_built_per_message"] = built
-        r["windows_ms"] = ms
-        results[name] = r
-    clock.stop_flag = True
-    clock.join()
+                paths["torch"] = lambda: torch_call(x, fam, K)
+            # "torch" stays [] where (b) is not timed
+            ms = {"device": [], "torch": [], **harness.alternate(paths, args.rounds, args.steps, args.warmup)}
+            r["device_ms_per_message"] = statistics.median(ms["device"])
+            r["torch_ms_per_message"] = statistics.median(ms["torch"]) if time_torch else None
+            r["torch_bytes_built_per_message"] = built
+            r["windows_ms"] = ms
+            results[name] = r
 
-    try:
-        import pynvml as nv_
-        nv_.nvmlInit()
-        h = nv_.nvmlDeviceGetHandleByIndex(0)
-        name = nv_.nvmlDeviceGetName(h)
-        card = {"name": name.decode() if isinstance(name, bytes) else name,
-                "power_limit_w": nv_.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0}
-    except Exception as e:          # NVML missing: report it
-        card = {"name": torch.cuda.get_device_name(0), "nvml_error": repr(e)}
-    card.update(clock.result())
+    card = harness.card(clock)
     print(json.dumps({"workload": f"full synthetic model, bf16, one message per family of {TIN} tokens and {BOXES} boxes per image, "
                                   f"positions {tokens[0]}..{tokens[1] - 1} masked and every box dropped, seed {args.seed}",
                       **results, "steps": args.steps, "rounds": args.rounds, "card": card}), flush=True)

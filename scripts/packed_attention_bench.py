@@ -25,6 +25,8 @@ import time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+import harness  # noqa: E402
+
 T_CAP, BOX_CAP = 37, 100
 
 
@@ -59,14 +61,10 @@ def main():
 
     import torch
     import vilbert_b200 as vb
-    from vilbert_b200 import synthetic as S
-    from bench import ClockSampler
 
-    if not torch.cuda.is_available():
-        raise SystemExit("packed_attention_bench.py needs an H100: there is no CPU path")
+    harness.require_gpu("packed_attention_bench.py")
     cfg = vb.BertConfig(task_specific_tokens=True, visualization=True)
-    model = vb.VILBertForVLTasks.from_pretrained(S.synthetic_state_dict(cfg, seed=42), config=cfg, num_labels=3129,
-                                                 compute_dtype=args.dtype, return_attention=True).eval().cuda(0)
+    model = harness.synthetic_model(cfg, args.dtype, return_attention=True)
     sel = vb.OUT_VIL_PREDICTION
     rows = detector_rows(args.batch, args.seed, cfg.v_feature_size, cfg.vocab_size)
     B, F = len(rows), cfg.v_feature_size
@@ -100,26 +98,8 @@ def main():
     if not torch.equal(logits["packed"], logits["packed_maps"]):
         raise SystemExit("VQA logits differ with and without the packed maps")
 
-    def timed(fn):
-        for _ in range(args.warmup):
-            fn()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        torch.cuda.synchronize()
-        e0.record()
-        for _ in range(args.steps):
-            fn()
-        e1.record()
-        e1.synchronize()
-        return e0.elapsed_time(e1) / args.steps
-
-    clock = ClockSampler(0)
-    clock.start()
-    ms = {k: [] for k in arms}
-    for _ in range(args.rounds):
-        for k, fn in arms.items():
-            ms[k].append(timed(fn))
-    clock.stop_flag = True
-    clock.join()
+    with harness.sampled_clock() as clock:
+        ms = harness.alternate(arms, args.rounds, args.steps, args.warmup)
 
     from torch.profiler import ProfilerActivity, profile
 
@@ -151,17 +131,7 @@ def main():
         split_packed_attention(flat, layout, t_rows, v_rows)
     split_ms = (time.perf_counter() - t0) / 20 * 1e3
 
-    card = {}
-    try:
-        import pynvml as nv_
-        nv_.nvmlInit()
-        h = nv_.nvmlDeviceGetHandleByIndex(0)
-        name = nv_.nvmlDeviceGetName(h)
-        card = {"name": name.decode() if isinstance(name, bytes) else name,
-                "power_limit_w": nv_.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0}
-    except Exception as e:          # NVML missing: report it
-        card = {"name": torch.cuda.get_device_name(0), "nvml_error": repr(e)}
-    card.update(clock.result())
+    card = harness.card(clock)
     result = {k: {"ms_per_call": statistics.median(v), "windows_ms": v, "map_floats_per_call": floats[k],
                   "device_ms_per_call_all_activity": dev_ms[k][0], "device_ms_per_call_map_kernels": dev_ms[k][1]}
               for k, v in ms.items()}

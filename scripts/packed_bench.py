@@ -21,6 +21,8 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+import harness  # noqa: E402
+
 
 def workload(batch, seed, F, vocab):
     import torch
@@ -54,14 +56,10 @@ def main():
     import statistics
     import torch
     import vilbert_b200 as vb
-    from vilbert_b200 import synthetic as S
-    from bench import ClockSampler
 
-    if not torch.cuda.is_available():
-        raise SystemExit("packed_bench.py needs an H100: there is no CPU path")
+    harness.require_gpu("packed_bench.py")
     cfg = vb.BertConfig(task_specific_tokens=True, visualization=True)
-    model = vb.VILBertForVLTasks.from_pretrained(S.synthetic_state_dict(cfg, seed=42), config=cfg, num_labels=3129,
-                                                 compute_dtype=args.dtype).eval().cuda(0)
+    model = harness.synthetic_model(cfg, args.dtype)
     B, T_PAD, V_CAP = args.batch, 37, 101
     sel = vb.OUT_VIL_PREDICTION
     samples = workload(B, args.seed, cfg.v_feature_size, cfg.vocab_size)
@@ -98,38 +96,10 @@ def main():
     if not parity <= 1e-5:
         raise SystemExit(f"packed VQA logits differ from dense: {parity}")
 
-    def timed(fn):
-        for _ in range(args.warmup):
-            fn()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        torch.cuda.synchronize()
-        e0.record()
-        for _ in range(args.steps):
-            fn()
-        e1.record()
-        e1.synchronize()
-        return e0.elapsed_time(e1) / 1e3
-
-    clock = ClockSampler(0)
-    clock.start()
-    secs = {"dense": [], "packed": []}
-    for _ in range(args.rounds):
-        secs["dense"].append(timed(run_dense))
-        secs["packed"].append(timed(run_packed))
-    clock.stop_flag = True
-    clock.join()
-
-    card = {}
-    try:
-        import pynvml as nv_
-        nv_.nvmlInit()
-        h = nv_.nvmlDeviceGetHandleByIndex(0)
-        name = nv_.nvmlDeviceGetName(h)
-        card = {"name": name.decode() if isinstance(name, bytes) else name,
-                "power_limit_w": nv_.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0}
-    except Exception as e:          # NVML missing: report it
-        card = {"name": torch.cuda.get_device_name(0), "nvml_error": repr(e)}
-    card.update(clock.result())
+    with harness.sampled_clock() as clock:
+        ms = harness.alternate({"dense": run_dense, "packed": run_packed}, args.rounds, args.steps, args.warmup)
+    secs = {k: [t * args.steps / 1e3 for t in v] for k, v in ms.items()}          # whole windows, in seconds
+    card = harness.card(clock)
 
     def path(name, issued):
         t = statistics.median(secs[name])

@@ -22,6 +22,8 @@ import time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+import harness  # noqa: E402
+
 B, TIN, V = 64, 36, 37
 
 
@@ -38,10 +40,8 @@ def main():
     import vilbert_b200 as vb
     from vilbert_b200 import _lib as L
     from vilbert_b200 import synthetic as S
-    from bench import ClockSampler
 
-    if not torch.cuda.is_available():
-        raise SystemExit("pretraining_objectives_bench.py needs an H100: there is no CPU path")
+    harness.require_gpu("pretraining_objectives_bench.py")
     cfg = vb.BertConfig(task_specific_tokens=False)
     model = vb.BertForMultiModalPreTraining.from_pretrained(S.synthetic_pretraining_state_dict(cfg, seed=42), config=cfg,
                                                             compute_dtype=args.dtype).eval().cuda(0)
@@ -81,17 +81,14 @@ def main():
         torch.cuda.synchronize()
         return (time.perf_counter() - t0) * 1e3 / args.reps
 
-    clock = ClockSampler(0)
-    clock.start()
-    for _ in range(2):                                   # warm-up windows
-        window(path_a)
-        window(path_b)
-    ms = {"a": [], "b": []}
-    for _ in range(args.rounds):
-        ms["a"].append(window(path_a))
-        ms["b"].append(window(path_b))
-    clock.stop_flag = True
-    clock.join()
+    with harness.sampled_clock() as clock:
+        for _ in range(2):                               # warm-up windows
+            window(path_a)
+            window(path_b)
+        ms = {"a": [], "b": []}
+        for _ in range(args.rounds):
+            ms["a"].append(window(path_a))
+            ms["b"].append(window(path_b))
 
     H, Hv, Hb = cfg.hidden_size, cfg.v_hidden_size, cfg.bi_hidden_size
     taps_bytes = 4 * (B * TIN * H + B * V * Hv + B * Hb)
@@ -100,16 +97,7 @@ def main():
 
     def summary(xs):
         return {"median_ms": round(statistics.median(xs), 3), "min_ms": round(min(xs), 3), "max_ms": round(max(xs), 3)}
-    try:
-        import pynvml as nv_
-        nv_.nvmlInit()
-        h = nv_.nvmlDeviceGetHandleByIndex(0)
-        name = nv_.nvmlDeviceGetName(h)
-        card = {"name": name.decode() if isinstance(name, bytes) else name,
-                "power_limit_w": nv_.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0}
-    except Exception as e:          # NVML missing: report it
-        card = {"name": torch.cuda.get_device_name(0), "nvml_error": repr(e)}
-    card.update(clock.result())
+    card = harness.card(clock)
     print(json.dumps({
         "workload": f"batch {B}, {TIN} tokens, V {V}, {args.dtype}; {n_t} masked tokens, {n_v} masked regions, {n_p} labelled pairs",
         "a_full_rows_torch": {**summary(ms["a"]), "bytes_written": bytes_a},

@@ -22,6 +22,8 @@ import time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+import harness  # noqa: E402
+
 B, TIN, V = 64, 37, 101
 SHARE = 0.15
 TOP_K = 5
@@ -43,13 +45,10 @@ def main():
     import vilbert_b200 as vb
     from vilbert_b200 import _lib as L
     from vilbert_b200 import synthetic as S
-    from bench import ClockSampler
 
-    if not torch.cuda.is_available():
-        raise SystemExit("pretraining_rows_bench.py needs an H100: there is no CPU path")
+    harness.require_gpu("pretraining_rows_bench.py")
     cfg = vb.BertConfig(task_specific_tokens=True, visualization=True)
-    model = vb.VILBertForVLTasks.from_pretrained(S.synthetic_state_dict(cfg, seed=42), config=cfg, num_labels=3129,
-                                                 compute_dtype=args.dtype).eval().cuda(0)
+    model = harness.synthetic_model(cfg, args.dtype)
     inp = [t.cuda() for t in S.synthetic_request(B, TIN, V, seed=args.seed)]
     T = TIN + 1
     H, Hv, Hb, vocab, vt = cfg.hidden_size, cfg.v_hidden_size, cfg.bi_hidden_size, cfg.vocab_size, cfg.v_target_size
@@ -79,17 +78,14 @@ def main():
         torch.cuda.synchronize()
         return (time.perf_counter() - t0) * 1e3 / args.reps
 
-    clock = ClockSampler(0)
-    clock.start()
-    for _ in range(2):                                   # warm-up windows
-        window(path_a)
-        window(path_b)
-    ms = {"a": [], "b": []}
-    for _ in range(args.rounds):
-        ms["a"].append(window(path_a))
-        ms["b"].append(window(path_b))
-    clock.stop_flag = True
-    clock.join()
+    with harness.sampled_clock() as clock:
+        for _ in range(2):                               # warm-up windows
+            window(path_a)
+            window(path_b)
+        ms = {"a": [], "b": []}
+        for _ in range(args.rounds):
+            ms["a"].append(window(path_a))
+            ms["b"].append(window(path_b))
 
     _, flops_a = model.plan_info(B, TIN, V, L.OUT_ALL)
     _, flops_task = model.plan_info(B, TIN, V, L.OUT_TASK_HEADS)
@@ -102,16 +98,7 @@ def main():
 
     def summary(xs):
         return {"median_ms": round(statistics.median(xs), 3), "min_ms": round(min(xs), 3), "max_ms": round(max(xs), 3)}
-    try:
-        import pynvml as nv_
-        nv_.nvmlInit()
-        h = nv_.nvmlDeviceGetHandleByIndex(0)
-        name = nv_.nvmlDeviceGetName(h)
-        card = {"name": name.decode() if isinstance(name, bytes) else name,
-                "power_limit_w": nv_.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0}
-    except Exception as e:          # NVML missing: report it
-        card = {"name": torch.cuda.get_device_name(0), "nvml_error": repr(e)}
-    card.update(clock.result())
+    card = harness.card(clock)
     print(json.dumps({
         "workload": f"batch {B}, Tin {TIN} (T {T}), V {V}, {args.dtype}; (b) {n_t} text rows and {n_v} region rows, top_k {TOP_K}",
         "a_all_rows": {**summary(ms["a"]), "bytes_written": bytes_a, "issued_gflop": round(flops_a / 1e9, 1),

@@ -23,6 +23,8 @@ import time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+import harness  # noqa: E402
+
 
 def _events_ms(fn, reps):
     import torch
@@ -142,32 +144,15 @@ def main():
     ap.add_argument("--seed", type=int, default=0)
     args = ap.parse_args()
 
-    import torch
     import vilbert_b200 as vb
-    from vilbert_b200 import synthetic as S
-    from bench import ClockSampler
 
-    if not torch.cuda.is_available():
-        raise SystemExit("region_select_bench.py needs an H100: there is no CPU path")
+    harness.require_gpu("region_select_bench.py")
     cfg = vb.BertConfig(task_specific_tokens=True, visualization=True)
-    model = vb.VILBertForVLTasks.from_pretrained(S.synthetic_state_dict(cfg, seed=42), config=cfg, num_labels=3129,
-                                                 compute_dtype=args.dtype).eval().cuda(0)
-    clock = ClockSampler(0)
-    clock.start()
-    result = {"a_device_selection": device_selection(model, args), "b_reference_loop": reference_loop(args),
-              "c_worker_64_vqa": worker_window(model, args)}
-    clock.stop_flag = True
-    clock.join()
-    try:
-        import pynvml as nv_
-        nv_.nvmlInit()
-        h = nv_.nvmlDeviceGetHandleByIndex(0)
-        name = nv_.nvmlDeviceGetName(h)
-        card = {"name": name.decode() if isinstance(name, bytes) else name,
-                "power_limit_w": nv_.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0}
-    except Exception as e:          # NVML missing: report it
-        card = {"name": torch.cuda.get_device_name(0), "nvml_error": repr(e)}
-    card.update(clock.result())
+    model = harness.synthetic_model(cfg, args.dtype)
+    with harness.sampled_clock() as clock:
+        result = {"a_device_selection": device_selection(model, args), "b_reference_loop": reference_loop(args),
+                  "c_worker_64_vqa": worker_window(model, args)}
+    card = harness.card(clock)
     print(json.dumps({"workload": f"1000 proposals x 1601 classes x 2048 features per image, seed {args.seed}, {args.dtype}",
                       **result, "rounds": args.rounds, "reps": args.reps, "card": card}), flush=True)
     model.close()

@@ -28,6 +28,8 @@ import time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+import harness  # noqa: E402
+
 T_PAD, BOX_CAP = 37, 100
 
 
@@ -83,22 +85,8 @@ def compare_paths(model, rows, sel, args):
     if parity != parity:
         raise SystemExit("packed VQA logits are NaN")
 
-    def timed(fn):
-        for _ in range(args.warmup):
-            fn()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        torch.cuda.synchronize()
-        e0.record()
-        for _ in range(args.steps):
-            fn()
-        e1.record()
-        e1.synchronize()
-        return e0.elapsed_time(e1) / 1e3
-
-    secs = {"dense": [], "packed": []}
-    for _ in range(args.rounds):
-        secs["dense"].append(timed(run_dense))
-        secs["packed"].append(timed(run_packed))
+    ms = harness.alternate({"dense": run_dense, "packed": run_packed}, args.rounds, args.steps, args.warmup)
+    secs = {k: [t * args.steps / 1e3 for t in v] for k, v in ms.items()}          # whole windows, in seconds
 
     def path(name, issued):
         t = statistics.median(secs[name])
@@ -166,38 +154,19 @@ def main():
     ap.add_argument("--seed", type=int, default=0)
     args = ap.parse_args()
 
-    import torch
     import vilbert_b200 as vb
-    from vilbert_b200 import synthetic as S
-    from bench import ClockSampler
 
-    if not torch.cuda.is_available():
-        raise SystemExit("regions_packed_bench.py needs an H100: there is no CPU path")
+    harness.require_gpu("regions_packed_bench.py")
     cfg = vb.BertConfig(task_specific_tokens=True, visualization=True)
-    model = vb.VILBertForVLTasks.from_pretrained(S.synthetic_state_dict(cfg, seed=42), config=cfg, num_labels=3129,
-                                                 compute_dtype=args.dtype).eval().cuda(0)
+    model = harness.synthetic_model(cfg, args.dtype)
     sel = vb.OUT_VIL_PREDICTION
-    clock = ClockSampler(0)
-    clock.start()
-    result = {}
-    for key, boxes in (("a_100_boxes", "100"), ("b_10_100_boxes", "10..100")):
-        rows = detector_rows(args.batch, args.seed, cfg.v_feature_size, cfg.vocab_size, boxes)
-        result[key] = compare_paths(model, rows, sel, args)
-    result["worker_64_messages_100_boxes"] = compare_workers(model, args.batch, args.seed + 1, cfg.v_feature_size, args)
-    clock.stop_flag = True
-    clock.join()
-
-    card = {}
-    try:
-        import pynvml as nv_
-        nv_.nvmlInit()
-        h = nv_.nvmlDeviceGetHandleByIndex(0)
-        name = nv_.nvmlDeviceGetName(h)
-        card = {"name": name.decode() if isinstance(name, bytes) else name,
-                "power_limit_w": nv_.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0}
-    except Exception as e:          # NVML missing: report it
-        card = {"name": torch.cuda.get_device_name(0), "nvml_error": repr(e)}
-    card.update(clock.result())
+    with harness.sampled_clock() as clock:
+        result = {}
+        for key, boxes in (("a_100_boxes", "100"), ("b_10_100_boxes", "10..100")):
+            rows = detector_rows(args.batch, args.seed, cfg.v_feature_size, cfg.vocab_size, boxes)
+            result[key] = compare_paths(model, rows, sel, args)
+        result["worker_64_messages_100_boxes"] = compare_workers(model, args.batch, args.seed + 1, cfg.v_feature_size, args)
+    card = harness.card(clock)
     print(json.dumps({"workload": f"batch {args.batch} VQA rows, text padded to {T_PAD} (U{{5..28}} words + 2), detector boxes "
                                   f"(a) 100 / (b) U{{10..100}} per image, seed {args.seed}, {args.dtype}",
                       **result, "steps": args.steps, "rounds": args.rounds, "card": card}), flush=True)

@@ -20,6 +20,8 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+import harness  # noqa: E402
+
 T_CAP, BOX_CAP = 37, 100
 
 
@@ -31,8 +33,7 @@ def rows(batch, seed, F, vocab):
     for _ in range(batch):
         t = int(torch.randint(5, T_CAP + 1, (1,), generator=g))
         n = int(torch.randint(10, BOX_CAP + 1, (1,), generator=g))
-        xy = torch.rand(n, 2, generator=g) * torch.tensor([448.0, 336.0])
-        bx = torch.cat([xy, torch.minimum(xy + 40 + 120 * torch.rand(n, 2, generator=g), torch.tensor([640.0, 480.0]))], 1)
+        bx = harness.pixel_boxes(g, n)
         out.append((torch.randint(1000, vocab, (t,), generator=g), torch.relu(torch.randn(n, F, generator=g)) * 1.5, bx,
                     (640.0, 480.0)))
     return out
@@ -79,14 +80,10 @@ def main():
 
     import torch
     import vilbert_b200 as vb
-    from vilbert_b200 import synthetic as S
-    from bench import ClockSampler
 
-    if not torch.cuda.is_available():
-        raise SystemExit("relevance_bench.py needs an H100: there is no CPU path")
+    harness.require_gpu("relevance_bench.py")
     cfg = vb.BertConfig(task_specific_tokens=True, visualization=True)
-    model = vb.VILBertForVLTasks.from_pretrained(S.synthetic_state_dict(cfg, seed=42), config=cfg, num_labels=3129, compute_dtype="bf16",
-                                                 return_attention=True, attention_heads="mean").eval().cuda(0)
+    model = harness.synthetic_model(cfg, "bf16", return_attention=True, attention_heads="mean")
     rs = rows(args.batch, args.seed, cfg.v_feature_size, cfg.vocab_size)
     B = len(rs)
     tin, nb = [len(r[0]) for r in rs], [r[1].shape[0] for r in rs]
@@ -106,28 +103,13 @@ def main():
     torch.cuda.synchronize()
     max_diff = max(float((x - y).abs().max()) for x, y in zip(a, b))
 
-    def timed(fn, steps):
-        for _ in range(args.warmup):
-            fn()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        torch.cuda.synchronize()
-        e0.record()
-        for _ in range(steps):
-            fn()
-        e1.record()
-        e1.synchronize()
-        return e0.elapsed_time(e1) / steps
-
-    clock = ClockSampler(0)
-    clock.start()
-    ms = {k: [] for k in variants}
-    call_ms = []
-    for _ in range(args.rounds):
-        for k, fn in variants.items():
-            ms[k].append(timed(fn, args.steps))
-        call_ms.append(timed(lambda: model.attention_relevance(attn), 10 * args.steps))
-    clock.stop_flag = True
-    clock.join()
+    with harness.sampled_clock() as clock:
+        ms = {k: [] for k in variants}
+        call_ms = []
+        for _ in range(args.rounds):
+            for k, fn in variants.items():
+                ms[k].append(harness.timed(fn, args.steps, args.warmup))
+            call_ms.append(harness.timed(lambda: model.attention_relevance(attn), 10 * args.steps, args.warmup))
 
     from torch.profiler import ProfilerActivity, profile
     n = 20
@@ -143,16 +125,7 @@ def main():
             kernel_us += d
     kernel_us /= n
 
-    try:
-        import pynvml as nv_
-        nv_.nvmlInit()
-        h = nv_.nvmlDeviceGetHandleByIndex(0)
-        name = nv_.nvmlDeviceGetName(h)
-        card = {"name": name.decode() if isinstance(name, bytes) else name,
-                "power_limit_w": nv_.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0}
-    except Exception as e:          # NVML missing: report it
-        card = {"name": torch.cuda.get_device_name(0), "nvml_error": repr(e)}
-    card.update(clock.result())
+    card = harness.card(clock)
     print(json.dumps({"workload": f"batch {B} VQA rows, U{{5..{T_CAP}}} tokens, U{{10..{BOX_CAP}}} boxes, seed {args.seed}, bf16, "
                                   f"head-mean maps, forward_regions_packed at capacities {T_CAP} / {BOX_CAP}",
                       "forward_plus_device_ms": statistics.median(ms["device"]), "forward_plus_torch_loop_ms": statistics.median(ms["torch_loop"]),

@@ -23,6 +23,8 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+import harness  # noqa: E402
+
 
 def suffix_flops(cfg, T, V):
     """Algorithmic FLOPs of one pair's suffix (connection layers, the text / image layers scheduled after the first connection
@@ -51,15 +53,11 @@ def main():
     import torch
     import vilbert_b200 as vb
     from vilbert_b200 import parallel as P
-    from vilbert_b200 import synthetic as S
     from oracle import vilbert_ref as R
-    from bench import ClockSampler
 
-    if not torch.cuda.is_available():
-        raise SystemExit("retrieval_packed_bench.py needs an H100: there is no CPU path")
+    harness.require_gpu("retrieval_packed_bench.py")
     cfg = vb.BertConfig(task_specific_tokens=True, visualization=True)
-    model = vb.VILBertForVLTasks.from_pretrained(S.synthetic_state_dict(cfg, seed=42), config=cfg, num_labels=3129,
-                                                 compute_dtype=args.dtype).eval().cuda(0)
+    model = harness.synthetic_model(cfg, args.dtype)
     dev = torch.device("cuda", 0)
     n_cap, n_img, T_PAD = args.captions, args.images, 30
     q, _, _, seg, im, _, _, _ = R.make_inputs(n_cap, T_PAD, 1, seed=args.seed, vocab_size=cfg.vocab_size)
@@ -75,58 +73,35 @@ def main():
             vm = (torch.arange(V)[None, :] < v_lens[:, None]).to(torch.uint8)
         return tuple(t.to(dev) for t in (f, s, vm)), vm.sum(dim=1).tolist(), V
 
-    def timed(fn):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        torch.cuda.synchronize()
-        e0.record()
-        out = fn()
-        e1.record()
-        e1.synchronize()
-        return e0.elapsed_time(e1) / 1e3, out
-
     pairs = n_cap * n_img
     padded_pairs = -(-pairs // args.pair_batch) * args.pair_batch
-    clock = ClockSampler(0)
-    clock.start()
     results = {}
-    for kind in ("fixed", "detector"):
-        imgs, v_lens, V_PAD = images(kind)
-        run = {"dense": lambda: P.retrieval_scores_cached(model, captions, imgs, pair_batch=args.pair_batch),
-               "packed": lambda: P.retrieval_scores_packed(model, captions, imgs, pair_batch=args.pair_batch)}
-        scores = {k: fn() for k, fn in run.items()}                  # warm-up: every plan either path uses
-        torch.cuda.synchronize()
-        secs = {"dense": [], "packed": []}
-        for _ in range(args.rounds):
-            for k in ("dense", "packed"):
-                t, scores[k] = timed(run[k])
-                secs[k].append(t)
-        diff = float((scores["packed"] - scores["dense"]).abs().max())
-        useful = sum(suffix_flops(cfg, t + 1, v) for t in t_lens for v in v_lens)
-        dense_issued = padded_pairs * suffix_flops(cfg, T_PAD + 1, V_PAD)
-        packed_issued = useful + (padded_pairs - pairs) * suffix_flops(cfg, t_lens[0] + 1, v_lens[0])
-        path = lambda k, issued: {"pairs_per_s": pairs / statistics.median(secs[k]), "s_per_block": statistics.median(secs[k]),
-                                  "runs_s": secs[k], "flops_useful": useful, "flops_issued": issued}
-        results[kind] = {"regions": "36" if kind == "fixed" else f"U{{10..101}} padded to {V_PAD}",
-                         "mean_regions": sum(v_lens) / n_img, "mean_tokens": sum(t_lens) / n_cap,
-                         "dense": path("dense", dense_issued), "packed": path("packed", packed_issued),
-                         "speedup": statistics.median(secs["dense"]) / statistics.median(secs["packed"]),
-                         "issued_flops_ratio_packed_vs_dense": packed_issued / dense_issued, "max_abs_score_diff": diff}
-        del imgs, scores
-        torch.cuda.empty_cache()
-    clock.stop_flag = True
-    clock.join()
+    with harness.sampled_clock() as clock:
+        for kind in ("fixed", "detector"):
+            imgs, v_lens, V_PAD = images(kind)
+            run = {"dense": lambda: P.retrieval_scores_cached(model, captions, imgs, pair_batch=args.pair_batch),
+                   "packed": lambda: P.retrieval_scores_packed(model, captions, imgs, pair_batch=args.pair_batch)}
+            scores = {k: fn() for k, fn in run.items()}              # warm-up: every plan either path uses
+            torch.cuda.synchronize()
+            secs = {"dense": [], "packed": []}
+            for _ in range(args.rounds):
+                for k in ("dense", "packed"):
+                    secs[k].append(harness.timed(lambda: scores.update({k: run[k]()}), 1, 0) / 1e3)
+            diff = float((scores["packed"] - scores["dense"]).abs().max())
+            useful = sum(suffix_flops(cfg, t + 1, v) for t in t_lens for v in v_lens)
+            dense_issued = padded_pairs * suffix_flops(cfg, T_PAD + 1, V_PAD)
+            packed_issued = useful + (padded_pairs - pairs) * suffix_flops(cfg, t_lens[0] + 1, v_lens[0])
+            path = lambda k, issued: {"pairs_per_s": pairs / statistics.median(secs[k]), "s_per_block": statistics.median(secs[k]),
+                                      "runs_s": secs[k], "flops_useful": useful, "flops_issued": issued}
+            results[kind] = {"regions": "36" if kind == "fixed" else f"U{{10..101}} padded to {V_PAD}",
+                             "mean_regions": sum(v_lens) / n_img, "mean_tokens": sum(t_lens) / n_cap,
+                             "dense": path("dense", dense_issued), "packed": path("packed", packed_issued),
+                             "speedup": statistics.median(secs["dense"]) / statistics.median(secs["packed"]),
+                             "issued_flops_ratio_packed_vs_dense": packed_issued / dense_issued, "max_abs_score_diff": diff}
+            del imgs, scores
+            torch.cuda.empty_cache()
 
-    card = {}
-    try:
-        import pynvml as nv_
-        nv_.nvmlInit()
-        h = nv_.nvmlDeviceGetHandleByIndex(0)
-        name = nv_.nvmlDeviceGetName(h)
-        card = {"name": name.decode() if isinstance(name, bytes) else name,
-                "power_limit_w": nv_.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0}
-    except Exception as e:          # NVML missing: report it
-        card = {"name": torch.cuda.get_device_name(0), "nvml_error": repr(e)}
-    card.update(clock.result())
+    card = harness.card(clock)
     print(json.dumps({"workload": f"{n_cap} captions x {n_img} images (make_inputs captions, 7..30 tokens padded to {T_PAD}), "
                                   f"pair batch {args.pair_batch}, seed {args.seed}, {args.dtype}",
                       "results": results, "rounds": args.rounds, "card": card}), flush=True)

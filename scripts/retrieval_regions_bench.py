@@ -27,6 +27,8 @@ import time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+import harness  # noqa: E402
+
 IMAGE_W, IMAGE_H = 1333.0, 800.0                  # the synthetic heads' original image (proposals are at im_scale times it)
 
 
@@ -80,13 +82,10 @@ def main():
     from vilbert_b200 import synthetic as S
     from vilbert_b200 import worker_api as W
     from oracle import vilbert_ref as R
-    from bench import ClockSampler
 
-    if not torch.cuda.is_available():
-        raise SystemExit("retrieval_regions_bench.py needs an H100: there is no CPU path")
+    harness.require_gpu("retrieval_regions_bench.py")
     cfg = vb.BertConfig(task_specific_tokens=True, visualization=True)
-    model = vb.VILBertForVLTasks.from_pretrained(S.synthetic_state_dict(cfg, seed=42), config=cfg, num_labels=3129,
-                                                 compute_dtype=args.dtype).eval().cuda(0)
+    model = harness.synthetic_model(cfg, args.dtype)
     W.model = model
     dev = torch.device("cuda", 0)
     n_cap, n_img, K = args.captions, args.images, args.max_boxes
@@ -110,54 +109,36 @@ def main():
                                                                        ii[s0:s0 + args.pair_batch])[2].view(-1)
         return out[:total].view(n_cap, n_img)
 
-    clock = ClockSampler(0)
-    clock.start()
-    states = {k: fn() for k, fn in encode.items()}                    # warm-up: every plan either path uses
-    scores = {k: score(v) for k, v in states.items()}
-    torch.cuda.synchronize()
-    enc_s, pair_s = {k: [] for k in encode}, {k: [] for k in encode}
-    for _ in range(args.rounds):
-        for k in encode:
-            del states[k]
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            states[k] = encode[k]()
-            torch.cuda.synchronize()
-            enc_s[k].append(time.perf_counter() - t0)
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            scores[k] = score(states[k])
-            e1.record()
-            e1.synchronize()
-            pair_s[k].append(e0.elapsed_time(e1) / 1e3)
-    diff = float((scores["host"] - scores["device"]).abs().max())
+    with harness.sampled_clock() as clock:
+        states = {k: fn() for k, fn in encode.items()}                # warm-up: every plan either path uses
+        scores = {k: score(v) for k, v in states.items()}
+        torch.cuda.synchronize()
+        enc_s, pair_s = {k: [] for k in encode}, {k: [] for k in encode}
+        for _ in range(args.rounds):
+            for k in encode:
+                del states[k]
+                torch.cuda.synchronize()
+                t0 = time.perf_counter()
+                states[k] = encode[k]()
+                torch.cuda.synchronize()
+                enc_s[k].append(time.perf_counter() - t0)
+                pair_s[k].append(harness.timed(lambda: scores.update({k: score(states[k])}), 1, 0) / 1e3)
+        diff = float((scores["host"] - scores["device"]).abs().max())
 
-    # (b) against the worker's forward of the same pairs: one selection of the sampled images, then forward_regions_packed
-    g = torch.Generator().manual_seed(args.seed + 3)
-    pc = torch.randint(0, n_cap, (args.sample,), generator=g).tolist()
-    pi = torch.randint(0, n_img, (args.sample,), generator=g).tolist()
-    r = model.select_regions([heads[i] for i in pi], K)
-    t_offs = [0] + list(torch.cumsum(torch.tensor(t_lens), 0).tolist())
-    rows = lambda x: torch.cat([x[t_offs[c]:t_offs[c + 1]] for c in pc])
-    fwd, _ = model.forward_regions_packed(rows(q_rows), rows(seg_rows), torch.full((args.sample, 1), 7, dtype=torch.long, device=dev),
-                                          r["box_features"], r["boxes"], image_wh[pi], [t_lens[c] for c in pc], r["n_boxes"],
-                                          select=vb.OUT_VIL_LOGIT, return_spatials=False)
-    torch.cuda.synchronize()
-    fwd_diff = float((fwd[2].view(-1) - scores["device"][pc, pi]).abs().max())
-    clock.stop_flag = True
-    clock.join()
+        # (b) against the worker's forward of the same pairs: one selection of the sampled images, then forward_regions_packed
+        g = torch.Generator().manual_seed(args.seed + 3)
+        pc = torch.randint(0, n_cap, (args.sample,), generator=g).tolist()
+        pi = torch.randint(0, n_img, (args.sample,), generator=g).tolist()
+        r = model.select_regions([heads[i] for i in pi], K)
+        t_offs = [0] + list(torch.cumsum(torch.tensor(t_lens), 0).tolist())
+        rows = lambda x: torch.cat([x[t_offs[c]:t_offs[c + 1]] for c in pc])
+        fwd, _ = model.forward_regions_packed(rows(q_rows), rows(seg_rows), torch.full((args.sample, 1), 7, dtype=torch.long, device=dev),
+                                              r["box_features"], r["boxes"], image_wh[pi], [t_lens[c] for c in pc], r["n_boxes"],
+                                              select=vb.OUT_VIL_LOGIT, return_spatials=False)
+        torch.cuda.synchronize()
+        fwd_diff = float((fwd[2].view(-1) - scores["device"][pc, pi]).abs().max())
 
-    card = {}
-    try:
-        import pynvml as nv_
-        nv_.nvmlInit()
-        h = nv_.nvmlDeviceGetHandleByIndex(0)
-        name = nv_.nvmlDeviceGetName(h)
-        card = {"name": name.decode() if isinstance(name, bytes) else name,
-                "power_limit_w": nv_.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0}
-    except Exception as e:          # NVML missing: report it
-        card = {"name": torch.cuda.get_device_name(0), "nvml_error": repr(e)}
-    card.update(clock.result())
+    card = harness.card(clock)
     med = lambda xs: statistics.median(xs)
     print(json.dumps({
         "workload": f"{n_cap} captions x {n_img} images, heads {args.proposals} x 1601 x 2048 ({len(pool)} distinct), top {K} boxes, "

@@ -25,6 +25,8 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+import harness  # noqa: E402
+
 TIN, BOXES, P = 37, 100, 8
 CHUNK = 1024
 
@@ -40,20 +42,15 @@ def main():
     import torch
     import vilbert_b200 as vb
     from vilbert_b200 import model as M
-    from vilbert_b200 import synthetic as S
-    from bench import ClockSampler
 
-    if not torch.cuda.is_available():
-        raise SystemExit("shapley_bench.py needs an H100: there is no CPU path")
+    harness.require_gpu("shapley_bench.py")
     cfg = vb.BertConfig(task_specific_tokens=True)
-    model = vb.VILBertForVLTasks.from_pretrained(S.synthetic_state_dict(cfg, seed=42), config=cfg, num_labels=3129,
-                                                 compute_dtype="bf16").eval().cuda(0)
+    model = harness.synthetic_model(cfg, "bf16")
     dev = torch.device("cuda", 0)
     g = torch.Generator().manual_seed(args.seed)
 
     def image():
-        xy = torch.rand(BOXES, 2, generator=g) * torch.tensor([448.0, 336.0])
-        bx = torch.cat([xy, torch.minimum(xy + 40 + 120 * torch.rand(BOXES, 2, generator=g), torch.tensor([640.0, 480.0]))], 1)
+        bx = harness.pixel_boxes(g, BOXES)
         return (torch.relu(torch.randn(BOXES, cfg.v_feature_size, generator=g)) * 1.5).to(dev), bx.to(dev)
 
     q = [torch.randint(1000, cfg.vocab_size, (TIN,), generator=g).to(dev) for _ in range(2)]
@@ -118,39 +115,13 @@ def main():
             out.append(dict(phi=(s / P).float().cpu(), samples=C * K))
         return out
 
-    def timed(fn):
-        for _ in range(args.warmup):
-            fn()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        torch.cuda.synchronize()
-        e0.record()
-        for _ in range(args.steps):
-            fn()
-        e1.record()
-        e1.synchronize()
-        return e0.elapsed_time(e1) / args.steps / len(msgs)
-
     a, b = device_call(), torch_call()
     torch.cuda.synchronize()
     diff = max(float((ra["phi"] - rb["phi"]).abs().max()) for ra, rb in zip(a, b))
-    ms = {"device": [], "torch": []}
-    clock = ClockSampler(0)
-    clock.start()
-    for _ in range(args.rounds):
-        ms["device"].append(timed(device_call))
-        ms["torch"].append(timed(torch_call))
-    clock.stop_flag = True
-    clock.join()
-    try:
-        import pynvml as nv_
-        nv_.nvmlInit()
-        h = nv_.nvmlDeviceGetHandleByIndex(0)
-        name = nv_.nvmlDeviceGetName(h)
-        card = {"name": name.decode() if isinstance(name, bytes) else name,
-                "power_limit_w": nv_.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0}
-    except Exception as e:          # NVML missing: report it
-        card = {"name": torch.cuda.get_device_name(0), "nvml_error": repr(e)}
-    card.update(clock.result())
+    with harness.sampled_clock() as clock:
+        ms = harness.alternate({"device": device_call, "torch": torch_call}, args.rounds, args.steps, args.warmup)
+    ms = {k: [t / len(msgs) for t in v] for k, v in ms.items()}
+    card = harness.card(clock)
     print(json.dumps({"workload": f"full synthetic model, bf16, one VQA and one NLVR2 message, {TIN} tokens and {BOXES} boxes per image, "
                                   f"default units, P = {P} antithetic, seed {args.seed}",
                       "device_samples": [r["samples"] for r in a], "torch_samples": [r["samples"] for r in b],

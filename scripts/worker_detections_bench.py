@@ -23,6 +23,8 @@ import time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+import harness  # noqa: E402
+
 N_MSGS = 64
 
 
@@ -71,17 +73,12 @@ def main():
     ap.add_argument("--seed", type=int, default=0)
     args = ap.parse_args()
 
-    import torch
     import vilbert_b200 as vb
-    from vilbert_b200 import synthetic as S
     from vilbert_b200 import worker_api as W
-    from bench import ClockSampler
 
-    if not torch.cuda.is_available():
-        raise SystemExit("worker_detections_bench.py needs an H100: there is no CPU path")
+    harness.require_gpu("worker_detections_bench.py")
     cfg = vb.BertConfig(task_specific_tokens=True, visualization=True)
-    model = vb.VILBertForVLTasks.from_pretrained(S.synthetic_state_dict(cfg, seed=42), config=cfg, num_labels=3129,
-                                                 compute_dtype=args.dtype).eval().cuda(0)
+    model = harness.synthetic_model(cfg, args.dtype)
     msgs = messages(model, args.seed)
     paths = {}
     for decode in ("host", "device"):
@@ -96,18 +93,15 @@ def main():
         res = fn(W, worker, msgs)
         return time.perf_counter() - t0, res
 
-    clock = ClockSampler(0)
-    clock.start()
-    answers = {}
-    for name in paths:
-        for _ in range(2):
-            _, answers[name] = window(name)
-    secs = {name: [] for name in paths}
-    for _ in range(args.rounds):
+    with harness.sampled_clock() as clock:
+        answers = {}
         for name in paths:
-            secs[name].append(window(name)[0])
-    clock.stop_flag = True
-    clock.join()
+            for _ in range(2):
+                _, answers[name] = window(name)
+        secs = {name: [] for name in paths}
+        for _ in range(args.rounds):
+            for name in paths:
+                secs[name].append(window(name)[0])
     for _, worker in paths.values():
         worker.close()
     result = {name: {"messages_per_s": N_MSGS / statistics.median(s), "windows_s": s} for name, s in secs.items()}
@@ -116,16 +110,7 @@ def main():
         result[f"answers_equal_{decode}"] = f"{sum(x == y for x, y in zip(a, b))}/{N_MSGS}"
         result[f"speedup_{decode}"] = result[f"b_device_selected_{decode}"]["messages_per_s"] / \
             result[f"a_host_selected_{decode}"]["messages_per_s"]
-    try:
-        import pynvml as nv_
-        nv_.nvmlInit()
-        h = nv_.nvmlDeviceGetHandleByIndex(0)
-        name = nv_.nvmlDeviceGetName(h)
-        card = {"name": name.decode() if isinstance(name, bytes) else name,
-                "power_limit_w": nv_.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0}
-    except Exception as e:          # NVML missing: report it
-        card = {"name": torch.cuda.get_device_name(0), "nvml_error": repr(e)}
-    card.update(clock.result())
+    card = harness.card(clock)
     print(json.dumps({"workload": f"{N_MSGS} single-image VQA messages, device heads of 1000 proposals x 1601 classes x 2048 "
                                   f"features, submitted at once; seed {args.seed}, {args.dtype}",
                       **result, "rounds": args.rounds, "card": card}), flush=True)
