@@ -163,7 +163,9 @@ int vb200_abi_version(void);
 
 /* from_pretrained + cuda(device): parse the BertConfig JSON, audit the state_dict against the upstream key list,
  * repack weights to device (16-bit GEMM operands in the format vb200_options::act_fp16 selects -- fp16 by default, bf16, or the
- * fp16 hi/lo pairs of split_fp32 -- and fp32 LayerNorm / bias / embedding tables). */
+ * fp16 hi/lo pairs of split_fp32 -- and fp32 LayerNorm / bias / embedding tables).  VB200_ERR_CONFIG, naming the field and the
+ * entry, for a t_biattention_id / v_biattention_id entry outside [0, num_hidden_layers] / [0, v_num_hidden_layers] or below the
+ * entry before it (equal entries are connection layers back to back; empty lists are a model without connection layers). */
 int vb200_create(const char* config_json, int64_t n_tensors, const vb200_tensor* tensors, const vb200_options* opt,
                  vb200_handle* out);
 /* BertForMultiModalPreTraining.from_pretrained + cuda(device): the same arguments, options and audit rules as vb200_create (`module.`

@@ -87,6 +87,39 @@ def tiny_cfg(**kw):
     return vb.BertConfig(**d)
 
 
+# Configurations the engine accepts beyond the two model shapes the other suites build (tiny_config and the 268 M model share one
+# layer schedule, head sizes 64 / 128 / 128, bi_hidden == v_hidden, widths of 1, 2 or a multiple of 2 column tiles of 128 and task
+# tokens on).  Each entry overrides oracle.vilbert_ref.tiny_config; CONFIG_LABELS is the number of answer labels of every entry (a
+# ragged N).  tests/test_config_matrix.py pins each entry's schedule and the property it exists for; tests/test_gpu_configs.py runs
+# them on the engine.
+CONFIG_LABELS = 129
+CONFIGS = {
+    # connection heads (8 x 64) outnumber the stream heads (text 2 x 128, image 4 x 64); bi_hidden_size != v_hidden_size
+    "heads_swapped": dict(hidden_size=256, num_attention_heads=2, v_hidden_size=256, v_num_attention_heads=4, bi_hidden_size=512,
+                          bi_num_attention_heads=8),
+    # widths of 3 and 5 column tiles; image-embedding K = 200 + 64 = 264
+    "odd_widths": dict(hidden_size=384, num_attention_heads=6, intermediate_size=640, v_hidden_size=640, v_num_attention_heads=5,
+                       v_intermediate_size=384, bi_hidden_size=384, bi_num_attention_heads=3, v_feature_size=200, v_target_size=37),
+    # an image layer ahead of C0, connection layers back to back, both streams ending in a connection layer
+    "back_to_back": dict(num_hidden_layers=6, v_num_hidden_layers=4, t_biattention_id=[1, 3, 3, 6], v_biattention_id=[1, 1, 1, 4]),
+    # the text stream ends in a connection layer (its tail cannot be pruned), the image stream in an image layer
+    "text_ends_in_c": dict(num_hidden_layers=4, v_num_hidden_layers=3, t_biattention_id=[2, 4], v_biattention_id=[0, 1]),
+    # no connection layer: the retrieval suffix is the heads alone
+    "no_coattention": dict(num_hidden_layers=3, v_num_hidden_layers=2, t_biattention_id=[], v_biattention_id=[]),
+    # the multi-task heads without the task row
+    "no_task_tokens": dict(task_specific_tokens=False),
+    # the text embedding at its 1024-wide limit, 8 x 128 text heads
+    "wide_text": dict(hidden_size=1024, num_attention_heads=8, intermediate_size=1024, num_hidden_layers=2, v_num_hidden_layers=2,
+                      t_biattention_id=[1], v_biattention_id=[1]),
+}
+
+
+def config_oracle(name):
+    """The fp32 oracle of CONFIGS[name] with seeded synthetic weights (seed 7, CONFIG_LABELS answer labels)."""
+    from oracle import vilbert_ref as R
+    return R.build(R.tiny_config(**CONFIGS[name]), seed=7, num_labels=CONFIG_LABELS)
+
+
 def free_port():
     """A free TCP port on 127.0.0.1 for a gloo process group."""
     s = socket.socket()

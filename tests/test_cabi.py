@@ -175,6 +175,13 @@ def test_checkpoint_legacy_names_accepted():
     (dict(num_attention_heads=4), "head size"),
     (dict(hidden_size=100, num_attention_heads=1), "head size"),
     (dict(fusion_method="sum"), "fusion_method"),
+    # connection-layer ids outside the layer counts, negative or decreasing
+    (dict(num_hidden_layers=4), "t_biattention_id[0] = 6 is outside [0, num_hidden_layers = 4]"),
+    (dict(v_num_hidden_layers=2), "v_biattention_id[3] = 3 is outside [0, v_num_hidden_layers = 2]"),
+    (dict(t_biattention_id=[6, 7, 8, 9, 10, 13]), "t_biattention_id[5] = 13 is outside [0, num_hidden_layers = 12]"),
+    (dict(v_biattention_id=[-1, 1, 2, 3, 4, 5]), "v_biattention_id[0] = -1 is outside"),
+    (dict(t_biattention_id=[6, 7, 8, 10, 9, 11]), "t_biattention_id[4] = 9 is below t_biattention_id[3] = 10"),
+    (dict(v_biattention_id=[0, 1, 2, 3, 5, 4]), "v_biattention_id[5] = 4 is below v_biattention_id[4] = 5"),
 ])
 def test_config_rejections(kw, needle):
     cfg = support.tiny_cfg(**kw)

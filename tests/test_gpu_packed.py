@@ -41,7 +41,7 @@ def _check_bitwise(model, samples, packed):
     import vilbert_b200 as vb
     (out, taps) = packed
     B = len(samples)
-    t_rows = [len(s[0]) + 1 for s in samples]
+    t_rows = [len(s[0]) + model._dims["task_specific_tokens"] for s in samples]
     v_rows = [s[2].shape[0] for s in samples]
     for i, smp in enumerate(samples):
         ref, rtaps = support.dense_alone(model, smp, select=vb.OUT_ALL, debug_taps=True)

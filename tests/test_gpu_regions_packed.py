@@ -49,7 +49,7 @@ def _check_bitwise(model, imgs, packed):
     import vilbert_b200 as vb
     (out, taps), sp = packed
     B = len(imgs)
-    t_rows = [len(im[0]) + 1 for im in imgs]
+    t_rows = [len(im[0]) + model._dims["task_specific_tokens"] for im in imgs]
     v_rows = [im[2].shape[0] + 1 for im in imgs]
     for i, im in enumerate(imgs):
         (ref, rtaps), rsp = support.regions_alone(model, im, vb.OUT_ALL, debug_taps=True)

@@ -83,7 +83,7 @@ def run_dense(model, oracle, mode, inp, every=1):
                                 output_layer_states=True)
     torch.cuda.synchronize()
     ref = S.StepRef(oracle, mode, device="cuda")
-    tm, vm = (m.cuda() for m in S.key_masks(inp[4], inp[5]))
+    tm, vm = (m.cuda() for m in S.key_masks(inp[4], inp[5], oracle.config.task_specific_tokens))
     sl = slice(None, None, every)
     maps = [tuple(x[sl] for x in m) if isinstance(m, tuple) else m[sl] for m in res[9]]
     out = S.teacher_forced(ref, [s[sl] for s in states], ref.text_embed(inp[0][sl], inp[3][sl], inp[7][sl]),

@@ -35,8 +35,8 @@ def _oracle_run(oracle64, inp):
     return states, out[9], collect["final"], out[:9]
 
 
-def _masks(inp):
-    return S.key_masks(inp[4], inp[5])
+def _masks(inp, task_tokens=True):
+    return S.key_masks(inp[4], inp[5], task_tokens)
 
 
 # ------------------------------------------------------------------------------------------------------------ restatement
@@ -44,7 +44,7 @@ def _check_restatement(oracle, inp, tag):
     o64 = X.fp64(oracle)
     states, maps, final, outs = _oracle_run(o64, inp)
     ref = S.StepRef(oracle)
-    tm, vm = _masks(inp)
+    tm, vm = _masks(inp, oracle.config.task_specific_tokens)
     emb_t = ref.text_embed(inp[0], inp[3], inp[7])
     emb_v = ref.image_embed(inp[1], inp[2])
     res = S.teacher_forced(ref, states, emb_t, emb_v, tm, vm, maps)

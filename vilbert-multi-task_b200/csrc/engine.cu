@@ -209,6 +209,20 @@ Config parse_config(const char* json) {
     if (c.hidden_act != "gelu" || c.v_hidden_act != "gelu") fail(VB200_ERR_CONFIG, "only hidden_act = gelu is supported");
     if (c.fusion != "mul") fail(VB200_ERR_CONFIG, "only fusion_method = mul is supported");
     if (c.v_bi_id.size() != c.t_bi_id.size()) fail(VB200_ERR_CONFIG, "v_biattention_id / t_biattention_id length mismatch");
+    // Connection layer i runs after the stream layers below ids[i]: every id must lie in [0, the stream's layer count] and no id
+    // may be below the one before it (equal neighbours are back-to-back connection layers).  Anything else would index past the
+    // layer lists when a plan is built, or leave checkpoint layers that never run.
+    auto ids_ok = [](const char* field, const std::vector<int>& ids, int n_layers, const char* n_field) {
+        for (size_t i = 0; i < ids.size(); ++i) {
+            if (ids[i] < 0 || ids[i] > n_layers)
+                fail(VB200_ERR_CONFIG, "%s[%zu] = %d is outside [0, %s = %d]", field, i, ids[i], n_field, n_layers);
+            if (i > 0 && ids[i] < ids[i - 1])
+                fail(VB200_ERR_CONFIG, "%s[%zu] = %d is below %s[%zu] = %d: the ids must not decrease", field, i, ids[i], field, i - 1,
+                     ids[i - 1]);
+        }
+    };
+    ids_ok("t_biattention_id", c.t_bi_id, c.layers, "num_hidden_layers");
+    ids_ok("v_biattention_id", c.v_bi_id, c.v_layers, "v_num_hidden_layers");
     auto head_ok = [](int hid, int heads) { return heads > 0 && hid % heads == 0 && (hid / heads == 64 || hid / heads == 128); };
     if (!head_ok(c.hidden, c.heads) || !head_ok(c.v_hidden, c.v_heads) || !head_ok(c.bi_hidden, c.bi_heads))
         fail(VB200_ERR_CONFIG, "attention head size must be 64 or 128");
