@@ -154,6 +154,24 @@ def test_model_rejects_fused_layernorm():
         vb.VILBertForVLTasks.from_pretrained(sd, config=cfg, num_labels=40, fused_layernorm=True)
 
 
+@pytest.mark.parametrize("kw,want", [
+    ({}, dict(use_cuda_graph=1, use_pdl=0, strict=1, act_fp16=1, split_fp32=0, max_plans=0)),
+    (dict(use_cuda_graph=False, use_pdl=False, strict=False), dict(use_cuda_graph=-1, use_pdl=-1, strict=-1)),
+    (dict(use_pdl=True, max_plans=3), dict(use_pdl=1, max_plans=3)),
+    (dict(compute_dtype="bf16"), dict(act_fp16=-1, split_fp32=0)),
+    (dict(compute_dtype="fp32x", use_cuda_graph=True), dict(use_cuda_graph=1, act_fp16=1, split_fp32=1)),
+])
+def test_model_options_reach_the_engine(kw, want):
+    """The model's keywords become vb200_options in the tri-state convention (1 on, -1 off, 0 the engine default): use_pdl=None
+    leaves the engine's default, False is -1 and not 0; the reserved fields stay 0."""
+    cfg = support.tiny_cfg()
+    sd = S.synthetic_state_dict(cfg, num_labels=40, gqa_labels=24, seed=1)
+    o = vb.VILBertForVLTasks.from_pretrained(sd, config=cfg, num_labels=40, **kw)._options(2)
+    assert (o.device, o.num_labels, o.fused_layernorm, o.ln_fold) == (2, 40, 0, 0)
+    for field, value in want.items():
+        assert getattr(o, field) == value, (field, getattr(o, field), value)
+
+
 def test_checkpoint_legacy_names_accepted():
     """`module.` prefixes (DataParallel) and gamma/beta LayerNorm names ([UPSTREAM] from_pretrained fix-ups)."""
     cfg = support.tiny_cfg()

@@ -1605,6 +1605,10 @@ struct vb200_engine {
         std::unique_ptr<Plan> up(new Plan());
         Plan& pl = *up;
         const Config& c = cfg;
+        // The build's stream: the zero fills below and the validation pass.  A plain cudaMemset would go to the legacy default
+        // stream, which a non-blocking stream (this one, and a caller's) does not wait for, so the validation pass could read what an
+        // evicted plan left in the same memory.  The build synchronises it before the plan is used on any other stream.
+        const Stream ws = make_stream();
         if (B < 1 || Tin < 1 || V < 1) fail(VB200_ERR_INVALID, "batch, n_tokens and n_regions must be positive");
         if (Tin > c.max_pos && !packed) fail(VB200_ERR_INVALID, "n_tokens %d exceeds max_position_embeddings %d", Tin, c.max_pos);
         pl.B = B; pl.Tin = Tin; pl.T = T; pl.V = V;
@@ -1616,7 +1620,7 @@ struct vb200_engine {
                                    mode == PACKED_SUFFIX, want_states ? static_cast<size_t>(selected_states()) : 0};
             const size_t n_meta = pl.layout.size();
             pl.d_meta = pl.mem.alloc_n<int>(n_meta);
-            CUDA_CHECK(cudaMemset(pl.d_meta, 0, n_meta * sizeof(int)));
+            CUDA_CHECK(cudaMemsetAsync(pl.d_meta, 0, n_meta * sizeof(int), ws.get()));
             pl.meta.copied = make_event();
             pl.meta.reserve(n_meta * sizeof(int));
         }
@@ -1648,8 +1652,8 @@ struct vb200_engine {
         if (mode == PACKED_SUFFIX) {
             // the attention kernels read the additive key masks in packed plans too, and every packed row is real: all zero, for good
             // (no embedding kernel of a packed suffix writes them)
-            CUDA_CHECK(cudaMemset(pl.mask_t, 0, static_cast<size_t>(Mt) * sizeof(float)));
-            CUDA_CHECK(cudaMemset(pl.mask_v, 0, static_cast<size_t>(Mv) * sizeof(float)));
+            CUDA_CHECK(cudaMemsetAsync(pl.mask_t, 0, static_cast<size_t>(Mt) * sizeof(float), ws.get()));
+            CUDA_CHECK(cudaMemsetAsync(pl.mask_v, 0, static_cast<size_t>(Mv) * sizeof(float), ws.get()));
         }
         for (int i = 0; i < 2; ++i) {
             pl.t_f32[i] = b.buf32(Mt, H);
@@ -1709,15 +1713,12 @@ struct vb200_engine {
         if (do_s) b.heads(select);
         for (const Op& op : pl.ops) pl.flops += op.flops;
 
-        if (timeline) attach_timeline(pl);
+        if (timeline) attach_timeline(pl, ws.get());
         // One eager pass first: opts kernels into their shared-memory sizes and surfaces launch-configuration
         // errors with a real message (errors inside a capture only invalidate the capture).
-        if (!pl.ops.empty()) {
-            const Stream ws = make_stream();
-            run_ops(pl, ws.get());
-            CUDA_CHECK(cudaStreamSynchronize(ws.get()));
-            if (opt.use_cuda_graph) capture(pl);
-        }
+        if (!pl.ops.empty()) run_ops(pl, ws.get());
+        CUDA_CHECK(cudaStreamSynchronize(ws.get()));
+        if (!pl.ops.empty() && opt.use_cuda_graph) capture(pl);
         Plan* raw = up.get();
         raw->last_use = ++use_clock;
         plans[key] = std::move(up);
@@ -1729,12 +1730,12 @@ struct vb200_engine {
     // clock64 at setup done, first k-block landed, last MMA committed, epilogue done) into a plan-owned buffer; a replay overwrites the
     // previous one, so after a run the buffer holds the LAST forward of this plan (scripts/step_timeline.py reads two slots' worth).
     static constexpr int kTimelineCtas = 304;
-    void attach_timeline(Plan& pl) {
+    void attach_timeline(Plan& pl, cudaStream_t st) {
         size_t n = 0;
         for (const Op& op : pl.ops) n += std::holds_alternative<GemmCall>(op.args);
         if (n == 0) return;
         pl.timeline = pl.mem.alloc_n<long long>(n * kTimelineCtas * 16);
-        CUDA_CHECK(cudaMemset(pl.timeline, 0, n * kTimelineCtas * 16 * sizeof(long long)));
+        CUDA_CHECK(cudaMemsetAsync(pl.timeline, 0, n * kTimelineCtas * 16 * sizeof(long long), st));
         size_t i = 0;
         for (Op& op : pl.ops)
             if (GemmCall* g = std::get_if<GemmCall>(&op.args)) g->ep.timing = pl.timeline + (i++) * kTimelineCtas * 16;

@@ -826,16 +826,7 @@ class VILBertForVLTasks(object):
             t.shape[1] = v.shape[1] if v.dim() == 2 else 0
             t.data = v.data_ptr()
             keep.append(v)
-        opt = L.Options()
-        opt.device = device
-        opt.num_labels = int(self.num_labels or 0)
-        opt.use_cuda_graph = 1 if self._opts["use_cuda_graph"] else -1
-        # None: engine default (programmatic dependent launch on every kernel); True: the same, forced; False: none
-        opt.use_pdl = 0 if self._opts["use_pdl"] is None else (1 if self._opts["use_pdl"] else -1)
-        opt.strict = 1 if self._opts["strict"] else -1
-        opt.act_fp16 = -1 if self._opts["compute_dtype"] == "bf16" else 1
-        opt.split_fp32 = 1 if self._opts["compute_dtype"] == "fp32x" else 0
-        opt.max_plans = self._opts["max_plans"]
+        opt = self._options(device)
         h = C.c_void_p()
         with torch.cuda.device(device):
             rc = getattr(lib, self._create_fn)(self._config_json(), len(self._sd), arr, C.byref(opt), C.byref(h))
@@ -851,6 +842,20 @@ class VILBertForVLTasks(object):
             v = C.c_int64()
             L.check(lib.vb200_model_dim(h, key.encode(), C.byref(v)), h)
             self._dims[key] = v.value
+
+    def _options(self, device: int):
+        """The vb200_options of this model's constructor arguments (tri-state flags: 1 on, -1 off, 0 the engine default)."""
+        opt = L.Options()
+        opt.device = device
+        opt.num_labels = int(self.num_labels or 0)
+        opt.use_cuda_graph = 1 if self._opts["use_cuda_graph"] else -1
+        # None: engine default (programmatic dependent launch on every kernel); True: the same, forced; False: none
+        opt.use_pdl = 0 if self._opts["use_pdl"] is None else (1 if self._opts["use_pdl"] else -1)
+        opt.strict = 1 if self._opts["strict"] else -1
+        opt.act_fp16 = -1 if self._opts["compute_dtype"] == "bf16" else 1
+        opt.split_fp32 = 1 if self._opts["compute_dtype"] == "fp32x" else 0
+        opt.max_plans = self._opts["max_plans"]
+        return opt
 
     def close(self):
         if self._handle is not None:
